@@ -57,6 +57,74 @@ __device__ __forceinline__ uint32_t ld32u_ro(const uint8_t* p) {  // read-only d
   return __funnelshift_r(lo, hi, sh);
 }
 
+// ---- the n bytes at p (1 <= n <= 16) as two little-endian 8-byte values: lo = bytes 0..7, hi = bytes 8..15 (bytes
+// past n are unspecified).  Reads only the aligned 8-byte words that contain a byte of [p, p+n) — one, two or three
+// of them — so it cannot cross an allocation edge that the span itself does not cross.  RO selects the read-only data
+// path (__ldg), which is right only for memory that no thread writes while the kernel runs.
+template <bool RO>
+__device__ __forceinline__ void ld_span16(const uint8_t* p, int n, uint64_t& lo, uint64_t& hi) {
+  const int b = (int)(reinterpret_cast<uintptr_t>(p) & 7u);  // position of byte 0 in the first word
+  // (p - b, not an integer cast: the compiler keeps p's address space and emits global loads)
+  const uint64_t* w = reinterpret_cast<const uint64_t*>(p - b);
+  const uint64_t w0 = RO ? __ldg(w) : w[0];
+  const uint64_t w1 = b + n > 8 ? (RO ? __ldg(w + 1) : w[1]) : 0ull;
+  const uint64_t w2 = b + n > 16 ? (RO ? __ldg(w + 2) : w[2]) : 0ull;
+  const unsigned s = 8u * (unsigned)b;
+  lo = (w0 >> s) | ((w1 << 1) << (63u - s));  // (x << 1) << (63 - s): no shift by 64 when s == 0
+  hi = (w1 >> s) | ((w2 << 1) << (63u - s));
+}
+// ---- stores bytes 0..n-1 (0 <= n <= 16) of (lo, hi) as ld_span16 returns them at p, with naturally aligned 1, 2, 4
+// and 8-byte stores (at most seven; each writes only bytes of [p, p+n))
+__device__ __forceinline__ void st_span16(uint8_t* p, int n, uint64_t lo, uint64_t hi) {
+  // head: up to 8-byte alignment, while the bytes last
+  if ((reinterpret_cast<uintptr_t>(p) & 1u) && n >= 1) {
+    *p = (uint8_t)lo;
+    lo = (lo >> 8) | (hi << 56);
+    hi >>= 8;
+    p += 1;
+    n -= 1;
+  }
+  if ((reinterpret_cast<uintptr_t>(p) & 2u) && n >= 2) {
+    *reinterpret_cast<uint16_t*>(p) = (uint16_t)lo;
+    lo = (lo >> 16) | (hi << 48);
+    hi >>= 16;
+    p += 2;
+    n -= 2;
+  }
+  if ((reinterpret_cast<uintptr_t>(p) & 4u) && n >= 4) {
+    *reinterpret_cast<uint32_t*>(p) = (uint32_t)lo;
+    lo = (lo >> 32) | (hi << 32);
+    hi >>= 32;
+    p += 4;
+    n -= 4;
+  }
+  // body and tail: sizes only shrink from here, so every store stays naturally aligned
+  if (n >= 8) {
+    *reinterpret_cast<uint64_t*>(p) = lo;
+    lo = hi;
+    p += 8;
+    n -= 8;
+  }
+  if (n >= 8) {
+    *reinterpret_cast<uint64_t*>(p) = lo;
+    p += 8;
+    n -= 8;
+  }
+  if (n >= 4) {
+    *reinterpret_cast<uint32_t*>(p) = (uint32_t)lo;
+    lo >>= 32;
+    p += 4;
+    n -= 4;
+  }
+  if (n >= 2) {
+    *reinterpret_cast<uint16_t*>(p) = (uint16_t)lo;
+    lo >>= 16;
+    p += 2;
+    n -= 2;
+  }
+  if (n >= 1) *p = (uint8_t)lo;
+}
+
 // ---- cooperative byte copy by a group of G lanes (lane in [0,G)), arbitrary alignment.
 // Fast path moves 16 bytes per lane per step with aligned 128-bit stores; source words are re-aligned with
 // funnel shifts so the loads stay aligned too.

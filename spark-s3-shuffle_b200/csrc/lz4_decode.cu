@@ -300,8 +300,10 @@ __global__ void __launch_bounds__(kCopyThreads) lz4_copy_kernel(const BlockDesc*
     base_op += __shfl_sync(FULL, inc, 31);
 
     // ---- literals: independent of everything, all lanes at once; long runs go through the whole warp
-    if (lit <= 16) {
-      for (int j = 0; j < lit; j++) out[op + j] = __ldg(in + lip + j);
+    if (lit > 0 && lit <= 16) {  // aligned 8-byte words of the compressed block (read-only: __ldg)
+      uint64_t lo, hi;
+      ld_span16<true>(in + lip, lit, lo, hi);
+      st_span16(out + op, lit, lo, hi);
     }
     unsigned biglit = __ballot_sync(FULL, lit > 16);
     while (biglit) {
@@ -315,7 +317,7 @@ __global__ void __launch_bounds__(kCopyThreads) lz4_copy_kernel(const BlockDesc*
     __syncwarp();
 
     // ---- matches, in dependency rounds (lz_batch.cuh)
-    lz_execute_matches(out, op + lit, ml, off, lane);
+    lz_execute_matches<true>(out, op + lit, ml, off, lane);
   }
 }
 

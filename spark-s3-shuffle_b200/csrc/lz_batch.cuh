@@ -17,7 +17,14 @@
 namespace b2s {
 
 // (Tried: moving a short match in groups of four bytes — four independent loads, then four stores — when the group's
-// source cannot be its own output: the read pass got slower.)
+// source cannot be its own output: the read pass got slower.  Those were still byte loads; see WIDE below.)
+//
+// WIDE: a short match (ml <= 16) whose source is apart from its output (off >= ml) reads that source as one to three
+// aligned 8-byte words (ld_span16) instead of ml byte loads.  The 32 lanes' sources lie in up to 32 different places,
+// so every warp-wide load instruction touches up to 32 sectors; fewer, wider loads cut those instructions (and their
+// round trips) by the match length.  The Zstandard executor passes WIDE = false and keeps the byte loop: inlined into
+// its larger kernel, the wide copy raised the register count from 64 to 80 and its execute stage measured slower.
+template <bool WIDE>
 __device__ __forceinline__ void lz_execute_matches(uint8_t* out, int mdst, int ml, int off, int lane) {
   constexpr unsigned FULL = 0xffffffffu;
   const int msrc = mdst - off;
@@ -44,8 +51,14 @@ __device__ __forceinline__ void lz_execute_matches(uint8_t* out, int mdst, int m
   while (done != FULL) {
     const bool ready = pending && (need & ~done) == 0;
     if (ready && ml <= 16) {
-      // sequential byte copy: also right for an overlapping match (off < ml)
-      for (int j = 0; j < ml; j++) out[mdst + j] = out[msrc + j];
+      if (WIDE && off >= ml) {  // the source is complete and apart from the output: read it in aligned 8-byte words
+        uint64_t lo, hi;
+        ld_span16<false>(out + msrc, ml, lo, hi);  // plain loads: `out` is written by this warp
+        st_span16(out + mdst, ml, lo, hi);
+      } else {
+        // overlapping match (off < ml): sequential byte copy, later bytes are read from bytes it has just written
+        for (int j = 0; j < ml; j++) out[mdst + j] = out[msrc + j];
+      }
     }
     unsigned longmask = __ballot_sync(FULL, ready && ml > 16);
     while (longmask) {

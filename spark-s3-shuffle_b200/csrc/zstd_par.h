@@ -538,7 +538,7 @@ B2S_HD inline int64_t execute_stream(const BlockInfo* blocks, uint32_t nb, const
           for (uint32_t q = lane; q < n_l; q += 32) ob[o_l + q] = lit[p_l + q];
         }
         __syncwarp();
-        lz_execute_matches(ob, (int)(o + ll), (int)ml, (int)off, lane);
+        lz_execute_matches<false>(ob, (int)(o + ll), (int)ml, (int)off, lane);
         produced += sum;
         lpos += lsum;
       }
