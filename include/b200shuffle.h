@@ -116,6 +116,44 @@ int b2s_compress_packed(uint32_t codec, int32_t level, uint32_t codec_block_size
                         uint64_t dst_cap, uint64_t* dst_off, uint64_t* dst_len, uint64_t* dst_total,
                         uint64_t* checksum_out, int32_t* status);
 
+/* ---- write side, serialized shuffle: partition + compress in one call ----
+ * Replaces what ShuffleExternalSorter / UnsafeShuffleWriter (serialized shuffle, spark.shuffle.sort) and the Bypass
+ * writer do on the CPU before S3ShuffleMapOutputWriter sees a byte: split the map task's serialized records by reduce
+ * id, then compress + checksum each partition.  With a relocatable serializer a partition's stream is the
+ * concatenation of its records in insertion order, so the caller hands over the records back to back plus one
+ * partition id per record and gets the finished .data arena, partitionLengths and .checksum values back.
+ *
+ * Records: record i is rec_len[i] bytes of rec_base, back to back (sum rec_len == rec_bytes), reduce id rec_part[i].
+ * Output, per partition p of num_partitions (empty ones included): dst_off[p], dst_len[p], checksum_out[p] (may be
+ * NULL), status[p].  Partitions come in ascending id; the records of a partition keep their input order (a stable
+ * partition, as Spark's writers produce).  A partition with no bytes has dst_len 0, takes no room in the arena (its
+ * dst_off is where the next partition starts) and has the checksum of a zero-length slice; every other partition is a
+ * complete, self-terminated stream in the codec's JVM wire format, byte for byte what b2s_compress_packed makes of it.
+ * codec B2S_CODEC_NONE partitions and checksums only: the arena holds the partitioned records
+ * (spark.shuffle.compress=false).  *dst_total = arena bytes.
+ * Errors: num_partitions outside [1, 2^24] (PackedRecordPointer's 24-bit partition id), an id >= num_partitions or
+ * sum rec_len != rec_bytes -> B2S_E_ARG, nothing reported as written, b2s_last_error() names the first offending
+ * record.  dst_cap below the arena -> B2S_E_DST_TOO_SMALL, status[p] = B2S_E_DST_TOO_SMALL for the partitions that do
+ * not fit and *dst_total = the bytes needed.  Device memory for the records, their partitioned copy and the codec
+ * workspace that cannot be had -> B2S_E_NOMEM.  n_records = 0 is valid: every partition is empty.
+ * Runs on the calling thread's device, on its write lane (like b2s_compress_*), and fills b2s_last_timing. */
+/* worst-case .data bytes for rec_bytes of records spread over num_partitions partitions, any distribution */
+uint64_t b2s_partition_compress_bound(uint32_t codec, uint32_t codec_block_size, uint32_t num_partitions,
+                                      uint64_t rec_bytes);
+/* host records (ideally b2s_host_alloc memory): one upload, the partition step, compression, one download */
+int b2s_partition_compress_packed(uint32_t codec, int32_t level, uint32_t codec_block_size, uint32_t checksum_alg,
+                                  uint32_t num_partitions, uint64_t n_records, const uint8_t* rec_base,
+                                  uint64_t rec_bytes, const uint32_t* rec_len, const uint32_t* rec_part,
+                                  uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_off, uint64_t* dst_len,
+                                  uint64_t* dst_total, uint64_t* checksum_out, int32_t* status);
+/* same, with rec_base / rec_len / rec_part / dst_base in device memory of dev_index (they are data-sized); the
+ * per-partition outputs stay host arrays, as in the other _dev calls */
+int b2s_partition_compress_dev(uint32_t dev_index, uint32_t codec, int32_t level, uint32_t codec_block_size,
+                               uint32_t checksum_alg, uint32_t num_partitions, uint64_t n_records,
+                               const uint8_t* rec_base, uint64_t rec_bytes, const uint32_t* rec_len,
+                               const uint32_t* rec_part, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_off,
+                               uint64_t* dst_len, uint64_t* dst_total, uint64_t* checksum_out, int32_t* status);
+
 /* ---- read side ---- */
 /* n compressed blocks as produced by S3BufferedPrefetchIterator.next() (storage/S3BufferedPrefetchIterator.scala:196-212).
  * Block i covers n_slices[i] consecutive reduce partitions (1 for ShuffleBlockId, >1 for ShuffleBlockBatchId,

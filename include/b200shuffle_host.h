@@ -10,6 +10,8 @@
  *   S3ShuffleHelper            helper/S3ShuffleHelper.scala:44-59 (.index/.checksum), :67-92 (cached readers), :94-103 (algorithms)
  *   S3ShuffleMapOutputWriter   shuffle/S3ShuffleMapOutputWriter.scala:67-83 (getPartitionWriter), :91-118 (commitAllPartitions),
  *                              :168-202 (partition stream), + the GPU "compress on commit" mode of SURVEY.md §3.2 option B
+ *   S3SerializedShuffleWriter  UnsafeShuffleWriter + ShuffleExternalSorter.insertRecord [U] for a SerializedShuffleHandle:
+ *                              records + reduce ids -> GPU partition + compress -> commitAllPartitions' output path
  *   S3MeasureOutputStream      shuffle/S3MeasureOutputStream.scala:8-65 (timing + byte counters of the .data stream)
  *   S3SingleSpillShuffleMapOutputWriter  shuffle/S3SingleSpillShuffleMapOutputWriter.scala:24-64 (+ GPU checksum verification)
  *   S3ShuffleReader            storage/S3ShuffleReader.scala:77-110 (block list -> prefetch -> verify -> decompress),
@@ -93,6 +95,22 @@ int b2sh_writer_abort(b2sh_writer* w);
  * write/flush/close, and the reference's log line ("Statistics: Stage .. -- Writing shuffle_0_1_0.data N took T ms (B MiB/s)"). */
 int b2sh_writer_statistics(b2sh_writer* w, uint64_t* bytes, uint64_t* nanos, char* line, uint32_t cap);
 void b2sh_writer_destroy(b2sh_writer* w);
+
+/* ---- GPU serialized writer: UnsafeShuffleWriter / ShuffleExternalSorter for a SerializedShuffleHandle (relocatable
+ * serializer, no map-side aggregation; INTEGRATION.md §3d).  insert() = ShuffleExternalSorter.insertRecord(record,
+ * partitionId), in any partition order; commit() partitions, compresses and checksums every partition in ONE
+ * b2s_partition_compress_packed call and writes .data/.index/.checksum like b2sh_writer_commit_all_partitions — the
+ * files are byte-identical to that writer's when it is fed the same records partition by partition, every partition
+ * opened in ascending order.  partition_lengths_out receives num_partitions values.  Needs
+ * spark.shuffle.s3.gpu.enabled; codec "none" partitions and checksums only. ---- */
+typedef struct b2sh_serialized_writer b2sh_serialized_writer;
+int b2sh_serialized_writer_create(b2sh_dispatcher* d, int32_t shuffle_id, int64_t map_id, int32_t num_partitions,
+                                  b2sh_serialized_writer** out);
+int b2sh_serialized_writer_insert(b2sh_serialized_writer* w, int32_t partition_id, const uint8_t* bytes, uint64_t len);
+int b2sh_serialized_writer_commit(b2sh_serialized_writer* w, int64_t* partition_lengths_out);
+int b2sh_serialized_writer_statistics(b2sh_serialized_writer* w, uint64_t* bytes, uint64_t* nanos, char* line,
+                                      uint32_t cap);
+void b2sh_serialized_writer_destroy(b2sh_serialized_writer* w);
 
 /* ---- single-spill writer (shuffle/S3SingleSpillShuffleMapOutputWriter.scala:24-64): moves an already compressed +
  * checksummed spill file to the .data object, then writes .checksum and .index.  verify_on_transfer != 0 recomputes the

@@ -5,6 +5,8 @@
  * org.apache.spark.shuffle.gpu.B200Codec (INTEGRATION.md §2).  Call sites on the reference side:
  *   init / shutdown / bindThreadToDevice   shuffle/S3ShuffleDataIO.scala:30-32 (initializeExecutor), task threads
  *   compressPacked                         shuffle/S3ShuffleMapOutputWriter.scala:91-118 (commitAllPartitions)
+ *   partitionCompressPacked                the GPU serialized writer (INTEGRATION.md §3d): records + reduce ids of a
+ *                                          map task in, .data arena + partitionLengths + checksums out
  *   decompressPacked / decompressedSize    storage/S3ShuffleReader.scala:98-110 (the codec seam, batched drain of
  *                                          storage/S3BufferedPrefetchIterator.scala:196-212)
  *   checksumPacked                         shuffle/S3SingleSpillShuffleMapOutputWriter.scala:54-63,
@@ -20,6 +22,7 @@
  */
 #include <jni.h>
 #include <stdint.h>
+#include <stdlib.h>
 
 #include "b200shuffle.h"
 
@@ -119,6 +122,48 @@ JNIEXPORT jint JNICALL J(compressPacked)(JNIEnv* e, jclass c, jint codec, jint l
   crit_put(e, dstOff, dO, 0);
   crit_put(e, len, l, JNI_ABORT); /* inputs: nothing to copy back */
   crit_put(e, off, o, JNI_ABORT);
+  return rc;
+}
+
+/* ---- write side, serialized shuffle (ShuffleExternalSorter.insertRecord's records + partition ids): partition by
+ *      reduce id and compress every partition in one call.  records / recLen (u32) / recPart (u32) / dst are direct
+ *      buffer addresses (data-sized); dstOff/dstLen/checksums: long[numPartitions], status: int[numPartitions],
+ *      meta: long[1] = {dst_total}.  The per-partition results are collected in native memory during the blocking
+ *      call and copied out with Set<Type>ArrayRegion afterwards: no Java array is held in a critical region while the
+ *      GPU works. ---- */
+JNIEXPORT jint JNICALL J(partitionCompressPacked)(JNIEnv* e, jclass c, jint codec, jint level, jint blockSize, jint alg,
+                                                  jint numPartitions, jlong nRecords, jlong records, jlong recBytes,
+                                                  jlong recLen, jlong recPart, jlong dst, jlong dstCap,
+                                                  jlongArray dstOff, jlongArray dstLen, jlongArray meta,
+                                                  jlongArray checksums, jintArray status) {
+  (void)c;
+  if (numPartitions < 1 || !dstOff || !dstLen || !meta || !status || (*e)->GetArrayLength(e, dstOff) < numPartitions ||
+      (*e)->GetArrayLength(e, dstLen) < numPartitions || (*e)->GetArrayLength(e, status) < numPartitions ||
+      (*e)->GetArrayLength(e, meta) < 1 || (checksums && (*e)->GetArrayLength(e, checksums) < numPartitions))
+    return B2S_E_ARG;
+  const size_t R = (size_t)numPartitions;
+  uint64_t* buf = (uint64_t*)malloc(R * 3 * sizeof(uint64_t));
+  int32_t* st = (int32_t*)malloc(R * sizeof(int32_t));
+  if (!buf || !st) {
+    free(buf);
+    free(st);
+    return B2S_E_NOMEM;
+  }
+  uint64_t total = 0;
+  const int rc = b2s_partition_compress_packed(
+      (uint32_t)codec, (int32_t)level, (uint32_t)blockSize, (uint32_t)alg, (uint32_t)numPartitions, (uint64_t)nRecords,
+      PTR(const uint8_t, records), (uint64_t)recBytes, PTR(const uint32_t, recLen), PTR(const uint32_t, recPart),
+      PTR(uint8_t, dst), (uint64_t)dstCap, buf, buf + R, &total, buf + 2 * R, st);
+  if (rc == 0 || rc == B2S_E_DST_TOO_SMALL) {
+    (*e)->SetLongArrayRegion(e, dstOff, 0, numPartitions, (const jlong*)buf);
+    (*e)->SetLongArrayRegion(e, dstLen, 0, numPartitions, (const jlong*)(buf + R));
+    if (checksums) (*e)->SetLongArrayRegion(e, checksums, 0, numPartitions, (const jlong*)(buf + 2 * R));
+    (*e)->SetIntArrayRegion(e, status, 0, numPartitions, (const jint*)st);
+  }
+  const jlong m = (jlong)total;
+  (*e)->SetLongArrayRegion(e, meta, 0, 1, &m);
+  free(st);
+  free(buf);
   return rc;
 }
 

@@ -36,5 +36,7 @@ struct JNINativeInterface_ {
   void (*ReleasePrimitiveArrayCritical)(JNIEnv* env, jarray array, void* carray, jint mode);
   jsize (*GetArrayLength)(JNIEnv* env, jarray array);
   jstring (*NewStringUTF)(JNIEnv* env, const char* utf);
+  void (*SetLongArrayRegion)(JNIEnv* env, jlongArray array, jsize start, jsize len, const jlong* buf);
+  void (*SetIntArrayRegion)(JNIEnv* env, jintArray array, jsize start, jsize len, const jint* buf);
 };
 #endif

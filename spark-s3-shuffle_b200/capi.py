@@ -54,6 +54,11 @@ PROTOTYPES = [
     ("b2s_compress_batch", C.c_int, [_u32, _i32, _u32, _u32, _u32, _vp, _u64p, _vp, _u64p, _u64p, _u64p, _i32p]),
     ("b2s_compress_packed", C.c_int,
      [_u32, _i32, _u32, _u32, _u32, _u8p, _u64p, _u64p, _u8p, _u64, _u64p, _u64p, _u64p, _u64p, _i32p]),
+    ("b2s_partition_compress_bound", _u64, [_u32, _u32, _u32, _u64]),
+    ("b2s_partition_compress_packed", C.c_int,
+     [_u32, _i32, _u32, _u32, _u32, _u64, _u8p, _u64, _u32p, _u32p, _u8p, _u64, _u64p, _u64p, _u64p, _u64p, _i32p]),
+    ("b2s_partition_compress_dev", C.c_int,
+     [_u32, _u32, _i32, _u32, _u32, _u32, _u64, _vp, _u64, _u32p, _u32p, _vp, _u64, _u64p, _u64p, _u64p, _u64p, _i32p]),
     ("b2s_decompress_batch", C.c_int,
      [_u32, _u32, _u32, _vp, _u64p, _u32p, _vp, _vp, _vp, _u64p, _u64p, _i32p, _i32p]),
     ("b2s_decompress_packed", C.c_int,
@@ -238,6 +243,31 @@ def compress_packed(codec, src, off, length, dst, block_size=0, checksum_alg=CHE
     return dict(dst_off=dst_off[:n], dst_len=dst_len[:n], total=total.value, checksums=cks[:n], status=st[:n])
 
 
+def partition_compress_bound(codec, block_size, num_partitions, rec_bytes):
+    return load().b2s_partition_compress_bound(codec, block_size, num_partitions, rec_bytes)
+
+
+def _partition_out(num_partitions):
+    return (np.zeros(num_partitions, dtype=np.uint64), np.zeros(num_partitions, dtype=np.uint64),
+            np.zeros(num_partitions, dtype=np.uint64), np.zeros(num_partitions, dtype=np.int32))
+
+
+def partition_compress_packed(codec, records, rec_len, rec_part, num_partitions, dst, block_size=0,
+                              checksum_alg=CHECKSUM_NONE, level=0):
+    """records: the serialized records back to back (uint8 array, ideally HostBuffer.array); rec_len / rec_part: one
+    length and one reduce id per record.  -> dict(dst_off, dst_len, total, checksums, status), one entry per partition"""
+    records, dst = _as_u8(records), _as_u8(dst)
+    rec_len = np.ascontiguousarray(rec_len, dtype=np.uint32)
+    rec_part = np.ascontiguousarray(rec_part, dtype=np.uint32)
+    dst_off, dst_len, cks, st = _partition_out(num_partitions)
+    total = _u64(0)
+    _check(load().b2s_partition_compress_packed(codec, level, block_size, checksum_alg, num_partitions, rec_len.size,
+                                                _ptr(records), records.size, _ptr(rec_len), _ptr(rec_part), _ptr(dst),
+                                                dst.size, _ptr(dst_off), _ptr(dst_len), C.addressof(total), _ptr(cks),
+                                                _ptr(st)), "b2s_partition_compress_packed")
+    return dict(dst_off=dst_off, dst_len=dst_len, total=total.value, checksums=cks, status=st)
+
+
 def decompressed_size_batch(codec, blocks):
     arrs = [_as_u8(b) for b in blocks]
     n = len(arrs)
@@ -368,3 +398,15 @@ def decompress_dev(codec, d_src, off, length, d_dst, dst_cap, checksum_alg=CHECK
                                      _ptr(sc), d_dst, dst_cap, _ptr(dst_off), _ptr(dst_len), C.addressof(total),
                                      _ptr(st), _ptr(bad)), "b2s_decompress_dev")
     return dict(dst_off=dst_off[:n], dst_len=dst_len[:n], total=total.value, status=st[:n], bad_slice=bad[:n])
+
+
+def partition_compress_dev(codec, d_records, rec_bytes, d_rec_len, d_rec_part, n_records, num_partitions, d_dst,
+                           dst_cap, block_size=0, checksum_alg=CHECKSUM_NONE, level=0, dev=0):
+    """d_*: device addresses (records, u32 lengths, u32 reduce ids, destination arena)"""
+    dst_off, dst_len, cks, st = _partition_out(num_partitions)
+    total = _u64(0)
+    _check(load().b2s_partition_compress_dev(dev, codec, level, block_size, checksum_alg, num_partitions, n_records,
+                                             d_records, rec_bytes, d_rec_len, d_rec_part, d_dst, dst_cap,
+                                             _ptr(dst_off), _ptr(dst_len), C.addressof(total), _ptr(cks), _ptr(st)),
+           "b2s_partition_compress_dev")
+    return dict(dst_off=dst_off, dst_len=dst_len, total=total.value, checksums=cks, status=st)

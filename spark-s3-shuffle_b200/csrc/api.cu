@@ -229,7 +229,9 @@ struct Slot {
   cudaEvent_t ev_k0 = nullptr, ev_k1 = nullptr;            // kernel region
   cudaEvent_t ev_t0 = nullptr, ev_t1 = nullptr;            // dominant kernel
   cudaEvent_t ev_h0 = nullptr, ev_h1 = nullptr, ev_d0 = nullptr, ev_d1 = nullptr;  // copies
+  cudaEvent_t ev_p0 = nullptr, ev_p1 = nullptr;            // partition step (b2s_partition_compress_*)
   DevBuf meta, scratch, desc, src, dst, zmeta;
+  DevBuf pws, parena;  // partition workspace (sort keys, offsets) and the partitioned arena in front of compression
   PinBuf hmeta;
   // per-launch event pairs around the dominant kernel of a call (grow-only pool; `used` pairs are valid)
   std::vector<cudaEvent_t> ev_dom;
@@ -326,14 +328,20 @@ struct CompressJob {
   uint8_t *h_up = nullptr, *h_down = nullptr;
 };
 
-// lays out pinned + device meta for a compress chunk; returns 0 or error
-int compress_prepare(Slot& S, uint32_t codec, uint32_t bs, uint32_t n, const uint64_t* src_len, CompressJob& J) {
+// codec and codec block size a compress job accepts
+int check_codec_block(uint32_t codec, uint32_t bs) {
   if (codec != B2S_CODEC_LZ4BLOCK && codec != B2S_CODEC_SNAPPY_XERIAL && codec != B2S_CODEC_ZSTD)
     return fail(B2S_E_UNSUPPORTED, "codec %s not supported by this build", "");
   if (codec != B2S_CODEC_SNAPPY_XERIAL && (bs < 64 || bs > 65536))
     return fail(B2S_E_UNSUPPORTED, "lz4 / zstd block size must be in [64, 65536]%s");
   if (codec == B2S_CODEC_SNAPPY_XERIAL && (bs < 64 || bs > 32768))
     return fail(B2S_E_UNSUPPORTED, "snappy block size must be in [64, 32768]%s");
+  return 0;
+}
+
+// lays out pinned + device meta for a compress chunk; returns 0 or error
+int compress_prepare(Slot& S, uint32_t codec, uint32_t bs, uint32_t n, const uint64_t* src_len, CompressJob& J) {
+  if (int rc = check_codec_block(codec, bs)) return rc;
   J.n = n;
   J.codec = codec;
   uint64_t nb = 0;
@@ -935,7 +943,8 @@ int b2s_init(uint32_t gpu_mask, uint64_t pinned_bytes_per_gpu, uint32_t streams_
         CU(cudaStreamCreateWithPriority(&S.st2, cudaStreamNonBlocking, prio));
         cudaEvent_t* evs2[] = {&S.ev_fork, &S.ev_match[0], &S.ev_match[1], &S.ev_free[0], &S.ev_free[1]};
         for (auto p : evs2) CU(cudaEventCreateWithFlags(p, cudaEventDisableTiming));
-        cudaEvent_t* evs[] = {&S.ev_a, &S.ev_b, &S.ev_k0, &S.ev_k1, &S.ev_t0, &S.ev_t1, &S.ev_h0, &S.ev_h1, &S.ev_d0, &S.ev_d1};
+        cudaEvent_t* evs[] = {&S.ev_a, &S.ev_b, &S.ev_k0, &S.ev_k1, &S.ev_t0, &S.ev_t1, &S.ev_h0, &S.ev_h1, &S.ev_d0, &S.ev_d1,
+                              &S.ev_p0, &S.ev_p1};
         for (auto p : evs) CU(cudaEventCreate(p));
         // pinned_bytes_per_gpu: the library's own pinned descriptor blocks are sized up front (split over the slots)
         // instead of growing on first use; 0 = grow on demand.  Payload staging is the caller's (b2s_host_alloc).
@@ -975,8 +984,11 @@ void b2s_shutdown(void) {
       S.zmeta.release();
       S.src.release();
       S.dst.release();
+      S.pws.release();
+      S.parena.release();
       S.hmeta.release();
-      cudaEvent_t evs[] = {S.ev_a, S.ev_b, S.ev_k0, S.ev_k1, S.ev_t0, S.ev_t1, S.ev_h0, S.ev_h1, S.ev_d0, S.ev_d1};
+      cudaEvent_t evs[] = {S.ev_a, S.ev_b, S.ev_k0, S.ev_k1, S.ev_t0, S.ev_t1, S.ev_h0, S.ev_h1, S.ev_d0, S.ev_d1,
+                           S.ev_p0, S.ev_p1};
       for (auto ev : evs)
         if (ev) cudaEventDestroy(ev);
       for (auto ev : S.ev_dom) cudaEventDestroy(ev);
@@ -1465,6 +1477,330 @@ int b2s_compress_packed(uint32_t codec, int32_t level, uint32_t codec_block_size
   for (uint32_t i = 0; i < n; i++) ptr[i] = src_base + src_off[i];
   return compress_host(codec, level, codec_block_size, checksum_alg, n, ptr.data(), src_len, dst_base, dst_cap, nullptr,
                        nullptr, dst_off, dst_len, dst_total, checksum_out, status);
+}
+
+// ------------------------------------------------------------------------------------------------------------
+// write side, serialized shuffle: partition records by reduce id, then compress every partition
+// ------------------------------------------------------------------------------------------------------------
+uint64_t b2s_partition_compress_bound(uint32_t codec, uint32_t codec_block_size, uint32_t num_partitions,
+                                      uint64_t rec_bytes) {
+  if (codec == B2S_CODEC_NONE) return rec_bytes;
+  // k non-empty partitions of L_p bytes: sum ceil(L_p / bs) <= (rec_bytes + k (bs - 1)) / bs, and every bound below
+  // grows with k, which is at most min(num_partitions, rec_bytes)
+  const uint64_t bs = block_size_or_default(codec, codec_block_size);
+  const uint64_t k = std::min<uint64_t>(num_partitions, rec_bytes);
+  const uint64_t nb = (rec_bytes + k * (bs - 1)) / bs;
+  switch (codec) {
+    case B2S_CODEC_LZ4BLOCK: return rec_bytes + (nb + k) * 21;
+    case B2S_CODEC_SNAPPY_XERIAL: return 16 * k + nb * 37 + rec_bytes + rec_bytes / 6;
+    case B2S_CODEC_ZSTD: return rec_bytes + nb * 3 + 9 * k;
+    default: return rec_bytes;
+  }
+}
+
+// checksum of a zero-length slice (what b2s_checksum_* returns for it): Adler-32 starts at 1, the CRCs at 0
+static uint64_t empty_checksum(uint32_t alg) { return alg == B2S_CHECKSUM_ADLER32 ? 1 : 0; }
+
+// first record whose bytes reach past rec_bytes, by bisection over the device record offsets (error path only)
+static uint64_t first_record_past(const uint64_t* d_off, const uint32_t* d_len, uint64_t n, uint64_t rec_bytes) {
+  uint64_t lo = 0, hi = n;  // answer in [lo, hi)
+  while (lo + 1 < hi) {
+    const uint64_t mid = lo + (hi - lo) / 2;
+    uint64_t o = 0;
+    if (cudaMemcpy(&o, d_off + mid, 8, cudaMemcpyDeviceToHost) != cudaSuccess) break;
+    if (o > rec_bytes) hi = mid;  // record mid starts past the end: the first offender is earlier
+    else lo = mid;
+  }
+  for (uint64_t i = lo; i < hi; i++) {  // lo is the last record starting within rec_bytes
+    uint64_t o = 0;
+    uint32_t l = 0;
+    if (cudaMemcpy(&o, d_off + i, 8, cudaMemcpyDeviceToHost) != cudaSuccess ||
+        cudaMemcpy(&l, d_len + i, 4, cudaMemcpyDeviceToHost) != cudaSuccess)
+      break;
+    if (o + l > rec_bytes) return i;
+  }
+  return lo;
+}
+
+// The partition step and the compression of the non-empty partitions, on device-resident records.  d_dst receives the
+// .data arena (dst_cap bytes); *arena_bytes the bytes it needs.  Returns B2S_E_DST_TOO_SMALL (status[] set for the
+// partitions that do not fit) when dst_cap is short.
+static int partition_compress_run(Device* D, Slot& S, uint32_t codec, int32_t level, uint32_t bs, uint32_t alg,
+                                  uint32_t R, uint64_t n, const uint8_t* d_rec, uint64_t rec_bytes,
+                                  const uint32_t* d_len, const uint32_t* d_part, uint8_t* d_dst, uint64_t dst_cap,
+                                  uint64_t* dst_off, uint64_t* dst_len, uint64_t* checksum_out, int32_t* status,
+                                  uint64_t* arena_bytes, uint64_t* launches) {
+  cudaStream_t st = S.st;
+  std::vector<uint64_t> pstart(R), plen(R);
+  CU(cudaEventRecord(S.ev_p0, st));
+  CU(cudaEventRecord(S.ev_k0, st));
+  PartitionPlan P;
+  if (n) {
+    int rc = S.pws.ensure(partition_ws_bytes(n, R));
+    if (rc) return rc;
+    launch_partition(d_len, d_part, n, R, (uint8_t*)S.pws.p, &P, st, launches);
+    // the one readback between the partition step and compression: [bad id, byte total, partition offsets]
+    rc = S.hmeta.ensure(P.readback_bytes);
+    if (rc) return rc;
+    const uint64_t* rb = (const uint64_t*)S.hmeta.p;
+    CU(cudaMemcpyAsync(S.hmeta.p, P.readback, P.readback_bytes, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    CU(cudaGetLastError());
+    char msg[256];
+    if (rb[0] != ~0ull) {
+      uint32_t id = 0;
+      CU(cudaMemcpy(&id, d_part + rb[0], 4, cudaMemcpyDeviceToHost));
+      snprintf(msg, sizeof msg, "record %llu has partition id %u, num_partitions is %u", (unsigned long long)rb[0], id, R);
+      return fail(B2S_E_ARG, "%s", msg);
+    }
+    if (rb[1] != rec_bytes) {
+      if (rb[1] > rec_bytes)
+        snprintf(msg, sizeof msg, "rec_len sums to %llu bytes, rec_bytes is %llu: record %llu ends past rec_bytes",
+                 (unsigned long long)rb[1], (unsigned long long)rec_bytes,
+                 (unsigned long long)first_record_past(P.src_off, d_len, n, rec_bytes));
+      else
+        snprintf(msg, sizeof msg, "rec_len sums to %llu bytes, rec_bytes is %llu", (unsigned long long)rb[1],
+                 (unsigned long long)rec_bytes);
+      return fail(B2S_E_ARG, "%s", msg);
+    }
+    uint64_t next = rec_bytes;
+    for (uint32_t p = R; p-- > 0;) {
+      const uint64_t s = rb[2 + p];
+      pstart[p] = s == ~0ull ? next : s;
+      plen[p] = next - pstart[p];
+      next = pstart[p];
+    }
+  } else if (rec_bytes) {
+    return fail(B2S_E_ARG, "rec_len sums to 0 bytes, rec_bytes is %s", std::to_string(rec_bytes).c_str());
+  }
+
+  if (codec == B2S_CODEC_NONE) {
+    *arena_bytes = rec_bytes;
+    memcpy(dst_off, pstart.data(), (size_t)R * 8);
+    memcpy(dst_len, plen.data(), (size_t)R * 8);
+    if (rec_bytes > dst_cap) {
+      for (uint32_t p = 0; p < R; p++) status[p] = pstart[p] + plen[p] > dst_cap ? B2S_E_DST_TOO_SMALL : B2S_OK;
+      return fail(B2S_E_DST_TOO_SMALL, "dst_cap is below the %s bytes of records", std::to_string(rec_bytes).c_str());
+    }
+    launch_partition_gather(d_rec, d_len, n, P, d_dst, st, launches);
+    CU(cudaEventRecord(S.ev_p1, st));
+    CU(cudaEventRecord(S.ev_t0, st));
+    CU(cudaEventRecord(S.ev_t1, st));
+    if (alg && rec_bytes) {  // over every partition, empty ones included
+      size_t ws_elems = checksum_ws_elems(R) + 4;
+      int rc = S.meta.ensure(align_up((size_t)R * 8, 16) * 3 + align_up(((size_t)R + 1) * 8, 16) + ws_elems * 8 + 128);
+      if (rc) return rc;
+      rc = S.hmeta.ensure(align_up((size_t)R * 8, 16) * 3 + 64);
+      if (rc) return rc;
+      Carver hc(S.hmeta.p), dc(S.meta.p);
+      uint64_t* h_off = hc.take<uint64_t>(R);
+      uint64_t* h_len = hc.take<uint64_t>(R);
+      uint64_t* h_out = hc.take<uint64_t>(R);
+      uint64_t* d_off = dc.take<uint64_t>(R);
+      uint64_t* d_slen = dc.take<uint64_t>(R);
+      uint64_t* d_out = dc.take<uint64_t>(R);
+      uint64_t* d_work = dc.take<uint64_t>((size_t)R + 1);
+      uint64_t* d_ws = dc.take<uint64_t>(ws_elems);
+      memcpy(h_off, pstart.data(), (size_t)R * 8);
+      memcpy(h_len, plen.data(), (size_t)R * 8);
+      CU(cudaMemcpyAsync(d_off, h_off, (size_t)R * 8, cudaMemcpyHostToDevice, st));
+      CU(cudaMemcpyAsync(d_slen, h_len, (size_t)R * 8, cudaMemcpyHostToDevice, st));
+      launch_checksum(D->tabs, alg, d_dst, d_off, d_slen, R, pick_tile_shift(rec_bytes), d_work, d_ws, d_out, st,
+                      launches);
+      CU(cudaEventRecord(S.ev_k1, st));
+      CU(cudaMemcpyAsync(h_out, d_out, (size_t)R * 8, cudaMemcpyDeviceToHost, st));
+      CU(cudaStreamSynchronize(st));
+      memcpy(checksum_out, h_out, (size_t)R * 8);
+    } else {
+      CU(cudaEventRecord(S.ev_k1, st));
+      CU(cudaStreamSynchronize(st));
+      for (uint32_t p = 0; p < R; p++) checksum_out[p] = alg ? empty_checksum(alg) : 0;
+    }
+    CU(cudaGetLastError());
+    for (uint32_t p = 0; p < R; p++) status[p] = B2S_OK;
+    return 0;
+  }
+
+  // compress the non-empty partitions of the partitioned arena with the pipeline behind b2s_compress_dev
+  std::vector<uint32_t> ne;
+  for (uint32_t p = 0; p < R; p++)
+    if (plen[p]) ne.push_back(p);
+  const uint32_t m = (uint32_t)ne.size();
+  std::vector<uint64_t> ne_len(m);
+  for (uint32_t k = 0; k < m; k++) ne_len[k] = plen[ne[k]];
+  CompressJob J;
+  uint64_t total = 0;
+  if (m) {
+    int rc = S.parena.ensure(rec_bytes + 64);
+    if (rc) return rc;
+    launch_partition_gather(d_rec, d_len, n, P, (uint8_t*)S.parena.p, st, launches);
+    CU(cudaEventRecord(S.ev_p1, st));
+    rc = compress_prepare(S, codec, bs, m, ne_len.data(), J);
+    if (rc) return rc;
+    for (uint32_t k = 0; k < m; k++) {
+      J.h_src_off[k] = pstart[ne[k]];
+      J.h_src_len[k] = ne_len[k];
+    }
+    CompressDevMeta M;
+    rc = compress_enqueue(g_ctx, S, D->tabs, bs, alg, J, (const uint8_t*)S.parena.p, d_dst, dst_cap, M, launches, level);
+    if (rc) return rc;
+    CU(cudaEventSynchronize(S.ev_a));
+    CU(cudaGetLastError());
+    total = J.h_total[0] + stream_overhead(codec) * m;
+  } else {
+    CU(cudaEventRecord(S.ev_p1, st));
+    CU(cudaEventRecord(S.ev_k0, st));
+    CU(cudaEventRecord(S.ev_t0, st));
+    CU(cudaEventRecord(S.ev_t1, st));
+    CU(cudaEventRecord(S.ev_k1, st));
+    CU(cudaStreamSynchronize(st));
+  }
+  *arena_bytes = total;
+  bool short_dst = false;
+  uint64_t at = 0;  // an empty partition sits where the next non-empty one starts
+  for (uint32_t p = 0, k = 0; p < R; p++) {
+    if (k < m && ne[k] == p) {
+      dst_off[p] = J.h_dst_off[k];
+      dst_len[p] = J.h_dst_len[k];
+      checksum_out[p] = alg ? J.h_cks[k] : 0;
+      status[p] = J.h_status[k];
+      if (dst_off[p] + dst_len[p] > dst_cap) status[p] = B2S_E_DST_TOO_SMALL;
+      short_dst |= status[p] == B2S_E_DST_TOO_SMALL;
+      at = dst_off[p] + dst_len[p];
+      k++;
+    } else {
+      dst_off[p] = at;
+      dst_len[p] = 0;
+      checksum_out[p] = alg ? empty_checksum(alg) : 0;
+      status[p] = B2S_OK;
+    }
+  }
+  if (short_dst) return fail(B2S_E_DST_TOO_SMALL, "dst_cap is below the %s bytes of the .data arena",
+                             std::to_string(total).c_str());
+  return 0;
+}
+
+static int partition_args(uint32_t codec, uint32_t bs, uint32_t alg, uint32_t R, uint64_t n, const void* rec_base,
+                          uint64_t rec_bytes, const uint32_t* rec_len, const uint32_t* rec_part, const void* dst_base,
+                          const uint64_t* dst_off, const uint64_t* dst_len, const int32_t* status) {
+  if (alg > B2S_CHECKSUM_CRC32C) return fail(B2S_E_UNSUPPORTED, "Unsupported shuffle checksum algorithm%s");
+  if (codec != B2S_CODEC_NONE)
+    if (int rc = check_codec_block(codec, bs)) return rc;
+  if (R < 1 || R > (1u << 24)) return fail(B2S_E_ARG, "num_partitions must be in [1, 2^24]%s");
+  if (n > 0xffffffffull) return fail(B2S_E_ARG, "more than 2^32 - 1 records in one call%s");
+  if ((n && (!rec_len || !rec_part)) || (rec_bytes && !rec_base) || !dst_off || !dst_len || !status)
+    return fail(B2S_E_ARG, "null argument%s");
+  if (rec_bytes && !dst_base) return fail(B2S_E_ARG, "null argument%s");
+  return 0;
+}
+
+static void partition_timing(Slot& S, uint32_t codec, uint64_t n_launches, uint64_t rec_bytes, uint64_t arena) {
+  add_timing(S, false);
+  // kernel_ms: partition step + compression; top_kernel_ms: the codec step, or the partition step for codec NONE
+  t_timing.kernel_ms = ms_between(S.ev_p0, S.ev_k1);
+  if (codec == B2S_CODEC_NONE) t_timing.top_kernel_ms = ms_between(S.ev_p0, S.ev_p1);
+  t_timing.kernel_launches = n_launches;
+  t_timing.src_bytes = rec_bytes;
+  t_timing.dst_bytes = arena;
+  g_ctx->launches += n_launches;
+}
+
+int b2s_partition_compress_dev(uint32_t dev_index, uint32_t codec, int32_t level, uint32_t codec_block_size,
+                               uint32_t checksum_alg, uint32_t num_partitions, uint64_t n_records,
+                               const uint8_t* rec_base, uint64_t rec_bytes, const uint32_t* rec_len,
+                               const uint32_t* rec_part, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_off,
+                               uint64_t* dst_len, uint64_t* dst_total, uint64_t* checksum_out, int32_t* status) {
+  WallTimer wt;
+  t_timing = b2s_timing{};
+  if (dst_total) *dst_total = 0;
+  const uint32_t bs = block_size_or_default(codec, codec_block_size);
+  int rc = partition_args(codec, bs, checksum_alg, num_partitions, n_records, rec_base, rec_bytes, rec_len, rec_part,
+                          dst_base, dst_off, dst_len, status);
+  if (rc) return rc;
+  Device* D;
+  rc = get_device(dev_index, &D);
+  if (rc) return rc;
+  Lane& Ln = D->lane[kLaneWrite];
+  std::lock_guard<std::mutex> lk(Ln.mtx);
+  Slot& S = Ln.slot[0];
+  std::vector<uint64_t> cks(num_partitions);
+  uint64_t launches = 0, arena = 0;
+  rc = partition_compress_run(D, S, codec, level, bs, checksum_alg, num_partitions, n_records, rec_base, rec_bytes,
+                              rec_len, rec_part, dst_base, dst_cap, dst_off, dst_len, cks.data(), status, &arena,
+                              &launches);
+  if (rc && rc != B2S_E_DST_TOO_SMALL) return rc;
+  if (checksum_out) memcpy(checksum_out, cks.data(), (size_t)num_partitions * 8);
+  if (dst_total) *dst_total = arena;
+  partition_timing(S, codec, launches, rec_bytes, arena);
+  t_timing.total_ms = wt.ms();
+  return rc;
+}
+
+int b2s_partition_compress_packed(uint32_t codec, int32_t level, uint32_t codec_block_size, uint32_t checksum_alg,
+                                  uint32_t num_partitions, uint64_t n_records, const uint8_t* rec_base,
+                                  uint64_t rec_bytes, const uint32_t* rec_len, const uint32_t* rec_part,
+                                  uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_off, uint64_t* dst_len,
+                                  uint64_t* dst_total, uint64_t* checksum_out, int32_t* status) {
+  WallTimer wt;
+  t_timing = b2s_timing{};
+  if (dst_total) *dst_total = 0;
+  const uint32_t bs = block_size_or_default(codec, codec_block_size);
+  int rc = partition_args(codec, bs, checksum_alg, num_partitions, n_records, rec_base, rec_bytes, rec_len, rec_part,
+                          dst_base, dst_off, dst_len, status);
+  if (rc) return rc;
+  Device* D;
+  rc = get_device(t_device, &D);
+  if (rc) return rc;
+  Lane& Ln = D->lane[kLaneWrite];
+  std::lock_guard<std::mutex> lk(Ln.mtx);
+  Slot& S = Ln.slot[0];
+  // one upload of [records | rec_len | rec_part]; the whole map output is partitioned at once, so there is no chunking
+  const size_t rec_sz = align_up(rec_bytes, 16), len_sz = align_up(n_records * 4, 16);
+  rc = S.src.ensure(rec_sz + 2 * len_sz + 64);
+  if (rc) return rc;
+  const uint64_t bound = b2s_partition_compress_bound(codec, bs, num_partitions, rec_bytes);
+  rc = S.dst.ensure(bound + 64);
+  if (rc) return rc;
+  uint8_t* d_rec = (uint8_t*)S.src.p;
+  uint32_t* d_len = (uint32_t*)(d_rec + rec_sz);
+  uint32_t* d_part = (uint32_t*)(d_rec + rec_sz + len_sz);
+  cudaStream_t st = S.st;
+  CU(cudaEventRecord(S.ev_h0, st));
+  if (rec_bytes) CU(copy_async(d_rec, rec_base, rec_bytes, cudaMemcpyHostToDevice, st));
+  if (n_records) {
+    CU(cudaMemcpyAsync(d_len, rec_len, n_records * 4, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(d_part, rec_part, n_records * 4, cudaMemcpyHostToDevice, st));
+  }
+  CU(cudaEventRecord(S.ev_h1, st));
+  std::vector<uint64_t> cks(num_partitions);
+  uint64_t launches = 0, arena = 0;
+  rc = partition_compress_run(D, S, codec, level, bs, checksum_alg, num_partitions, n_records, d_rec, rec_bytes, d_len,
+                              d_part, (uint8_t*)S.dst.p, S.dst.cap, dst_off, dst_len, cks.data(), status, &arena,
+                              &launches);
+  if (rc) return rc;
+  // the device arena is sized by the bound, so a short caller arena shows up here: copy what fits, flag the rest
+  int result = 0;
+  uint64_t fit = arena;
+  if (arena > dst_cap) {
+    fit = dst_cap;
+    for (uint32_t p = 0; p < num_partitions; p++)
+      if (dst_len[p] && dst_off[p] + dst_len[p] > dst_cap) status[p] = B2S_E_DST_TOO_SMALL;
+    result = fail(B2S_E_DST_TOO_SMALL, "dst_cap is below the %s bytes of the .data arena", std::to_string(arena).c_str());
+  }
+  CU(cudaEventRecord(S.ev_d0, st));
+  if (fit) CU(copy_async(dst_base, S.dst.p, fit, cudaMemcpyDeviceToHost, st));
+  CU(cudaEventRecord(S.ev_d1, st));
+  CU(cudaStreamSynchronize(st));
+  CU(cudaGetLastError());
+  if (checksum_out) memcpy(checksum_out, cks.data(), (size_t)num_partitions * 8);
+  if (dst_total) *dst_total = arena;
+  partition_timing(S, codec, launches, rec_bytes, arena);
+  t_timing.h2d_ms = ms_between(S.ev_h0, S.ev_h1);
+  t_timing.d2h_ms = ms_between(S.ev_d0, S.ev_d1);
+  t_timing.h2d_bytes = rec_bytes + n_records * 8;
+  t_timing.d2h_bytes = fit;
+  t_timing.total_ms = wt.ms();
+  return result;
 }
 
 // ------------------------------------------------------------------------------------------------------------

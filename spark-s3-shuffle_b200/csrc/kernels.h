@@ -154,6 +154,28 @@ void launch_zstd_stream_meta(const uint32_t* d_blk_base, uint32_t n_streams, uin
                              const uint64_t* d_scan_total, uint8_t* dst_base, uint64_t dst_cap, uint64_t* d_dst_off,
                              uint64_t* d_dst_len, int32_t* d_status, cudaStream_t st, uint64_t* launches);
 
+// ---------------- partition.cu (stable partition of serialized records by reduce id) ----------------
+// Record i is rec_base[src_off[i] .. + rec_len[i]) with id rec_part[i]; n < 2^32.  After launch_partition the records
+// of partition p, in input order, belong at part_start[p] .. (the arena offsets of the records in sorted order are in
+// sdst; idx = sorted record indices, nullptr = identity).  readback = [first record with an id >= num_partitions
+// (~0 = none), sum of rec_len, part_start[num_partitions] (~0 = no records)], readback_bytes long.
+struct PartitionPlan {
+  uint64_t* src_off = nullptr;
+  uint64_t* sdst = nullptr;
+  const uint32_t* idx = nullptr;
+  uint64_t* readback = nullptr;
+  size_t readback_bytes = 0;
+};
+uint32_t partition_radix_passes(uint32_t num_partitions);
+size_t partition_ws_bytes(uint64_t n, uint32_t num_partitions);  // d_ws of launch_partition
+void launch_partition(const uint32_t* d_rec_len, const uint32_t* d_rec_part, uint64_t n, uint32_t num_partitions,
+                      uint8_t* d_ws, PartitionPlan* plan, cudaStream_t st,
+                      uint64_t* launches);
+// copies the records into d_dst in sorted order (only once the readback has shown every id valid and the lengths sum
+// to the arena size)
+void launch_partition_gather(const uint8_t* rec_base, const uint32_t* d_rec_len, uint64_t n, const PartitionPlan& plan,
+                             uint8_t* d_dst, cudaStream_t st, uint64_t* launches);
+
 // ---------------- gen.cu (bench utility) ----------------
 void launch_gen_terasort(uint8_t* d_dst, uint64_t first_record, uint64_t n_records, uint64_t seed, cudaStream_t st);
 

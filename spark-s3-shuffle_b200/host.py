@@ -63,6 +63,11 @@ PROTOTYPES = [
      [_vp, _u32, C.POINTER(_i64), C.POINTER(_i32), C.POINTER(_i32), C.POINTER(_vp), C.POINTER(_u64)]),
     ("b2sh_reader_remote_bytes_read", _u64, [_vp]),
     ("b2sh_reader_destroy", None, [_vp]),
+    ("b2sh_serialized_writer_create", C.c_int, [_vp, _i32, _i64, _i32, C.POINTER(_vp)]),
+    ("b2sh_serialized_writer_insert", C.c_int, [_vp, _i32, _vp, _u64]),
+    ("b2sh_serialized_writer_commit", C.c_int, [_vp, _vp]),
+    ("b2sh_serialized_writer_statistics", C.c_int, [_vp, C.POINTER(_u64), C.POINTER(_u64), C.c_char_p, _u32]),
+    ("b2sh_serialized_writer_destroy", None, [_vp]),
     ("b2sh_writer_statistics", C.c_int, [_vp, C.POINTER(_u64), C.POINTER(_u64), C.c_char_p, _u32]),
     ("b2sh_reader_open", C.c_int, [_vp]),
     ("b2sh_reader_next_batch", C.c_int, [_vp, _u32, C.POINTER(_u32)]),
@@ -253,6 +258,37 @@ class S3ShuffleMapOutputWriter:
     def close(self):
         if self._h:
             load().b2sh_writer_destroy(self._h)
+            self._h = None
+
+
+class S3SerializedShuffleWriter:
+    """The GPU serialized writer (UnsafeShuffleWriter + ShuffleExternalSorter for a SerializedShuffleHandle):
+    insertRecord(partitionId, record) in any partition order; commit() partitions, compresses and checksums on the GPU
+    in one call and writes .data/.index/.checksum as S3ShuffleMapOutputWriter.commitAllPartitions does."""
+
+    def __init__(self, dispatcher, shuffleId, mapId, numPartitions):
+        self._h = _vp()
+        self.numPartitions = numPartitions
+        _check(load().b2sh_serialized_writer_create(dispatcher._h, shuffleId, mapId, numPartitions, C.byref(self._h)))
+
+    def insertRecord(self, partitionId, record):
+        a = np.frombuffer(record, dtype=np.uint8) if not isinstance(record, np.ndarray) else np.ascontiguousarray(record)
+        _check(load().b2sh_serialized_writer_insert(self._h, partitionId, a.ctypes.data if a.size else None, a.size))
+
+    def commit(self):
+        """-> partitionLengths (MapOutputCommitMessage)"""
+        out = np.zeros(self.numPartitions, dtype=np.int64)
+        _check(load().b2sh_serialized_writer_commit(self._h, out.ctypes.data))
+        return out
+
+    def statistics(self):
+        b, ns, line = _u64(), _u64(), C.create_string_buffer(512)
+        _check(load().b2sh_serialized_writer_statistics(self._h, C.byref(b), C.byref(ns), line, 512))
+        return b.value, ns.value, line.value.decode()
+
+    def close(self):
+        if self._h:
+            load().b2sh_serialized_writer_destroy(self._h)
             self._h = None
 
 

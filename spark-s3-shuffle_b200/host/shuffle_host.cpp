@@ -321,6 +321,33 @@ static void submit_or_throw(CoalescingQueue& q, CodecRequest& r, const char* wha
   if (rc != 0) throw CodecException(std::string(what) + ": " + b2s_strerror(rc) + ": " + r.error);
 }
 
+// The output half of commitAllPartitions (shuffle/S3ShuffleMapOutputWriter.scala:91-118): the .data object from
+// `segments` (its bytes in order, data_len in all; created when createData), then .index and .checksum.
+static void writeMapOutput(S3ShuffleDispatcher& d, int32_t shuffleId, int64_t mapId, bool createData,
+                           const std::vector<std::pair<const uint8_t*, uint64_t>>& segments, uint64_t data_len,
+                           const std::vector<int64_t>& partitionLengths, const std::vector<int64_t>& checksums,
+                           std::unique_ptr<S3MeasureOutputStream>& measure) {
+  int64_t sum = 0;
+  for (int64_t v : partitionLengths) sum += v;
+  if ((int64_t)data_len != sum)
+    throw RuntimeException("S3ShuffleMapOutputWriter: Unexpected output length " + std::to_string(data_len) +
+                           ", expected: " + std::to_string(sum) + ".");
+  if (createData) {
+    std::string path = d.getPath(BlockId{BlockId::Data, shuffleId, mapId, 0, 0});
+    mkdirs(path.substr(0, path.rfind('/')));
+    // initStream (:43-49): BufferedOutputStream(S3MeasureOutputStream(createBlock(shuffleBlock), name), bufferSize)
+    measure.reset(new S3MeasureOutputStream(path, BlockId{BlockId::Data, shuffleId, mapId, 0, 0}.name(),
+                                            (size_t)d.bufferSize));
+    for (auto& sg : segments) measure->write(sg.first, sg.second);
+    measure->flush();  // :102-107
+    measure->close();
+  }
+  if (sum > 0 || d.alwaysCreateIndex) {  // :111
+    S3ShuffleHelper::writePartitionLengths(d, shuffleId, mapId, partitionLengths);
+    if (d.checksumEnabled) S3ShuffleHelper::writeChecksum(d, shuffleId, mapId, checksums);
+  }
+}
+
 // ---- S3ShuffleMapOutputWriter (shuffle/S3ShuffleMapOutputWriter.scala) --------------------------------------
 class S3ShuffleMapOutputWriter {
  public:
@@ -431,25 +458,9 @@ class S3ShuffleMapOutputWriter {
     } else if (checksums_in) {
       for (int32_t p = 0; p < numPartitions_; p++) checksums[(size_t)p] = checksums_in[p];
     }
-    int64_t sum = 0;
-    for (int64_t v : partitionLengths_) sum += v;
-    if ((int64_t)data_len != sum)
-      throw RuntimeException("S3ShuffleMapOutputWriter: Unexpected output length " + std::to_string(data_len) +
-                             ", expected: " + std::to_string(sum) + ".");
-    if (lastPartitionWriterId_ >= 0) {  // the .data object exists as soon as a stream was opened (:43-49)
-      std::string path = d_.getPath(BlockId{BlockId::Data, shuffleId_, mapId_, 0, 0});
-      mkdirs(path.substr(0, path.rfind('/')));
-      // initStream (:43-49): BufferedOutputStream(S3MeasureOutputStream(createBlock(shuffleBlock), name), bufferSize)
-      measure_.reset(new S3MeasureOutputStream(path, BlockId{BlockId::Data, shuffleId_, mapId_, 0, 0}.name(),
-                                               (size_t)d_.bufferSize));
-      for (auto& sg : segments) measure_->write(sg.first, sg.second);
-      measure_->flush();  // :102-107
-      measure_->close();
-    }
-    if (sum > 0 || d_.alwaysCreateIndex) {  // :111
-      S3ShuffleHelper::writePartitionLengths(d_, shuffleId_, mapId_, partitionLengths_);
-      if (d_.checksumEnabled) S3ShuffleHelper::writeChecksum(d_, shuffleId_, mapId_, checksums);
-    }
+    // the .data object exists as soon as a stream was opened (:43-49)
+    writeMapOutput(d_, shuffleId_, mapId_, lastPartitionWriterId_ >= 0, segments, data_len, partitionLengths_,
+                   checksums, measure_);
     return partitionLengths_;
   }
   void abort() {  // :120-134
@@ -468,6 +479,63 @@ class S3ShuffleMapOutputWriter {
   int32_t lastPartitionWriterId_ = -1, current_ = -1;
   bool streamOpen_ = false, gpu_ = true;
   PinnedArena buf_, out_;
+  std::unique_ptr<S3MeasureOutputStream> measure_;
+};
+
+// ---- GPU serialized writer: what UnsafeShuffleWriter + ShuffleExternalSorter do for a SerializedShuffleHandle -----
+// insertRecord(record, partitionId) collects the serialized records back to back with their reduce ids, in any
+// partition order (ShuffleExternalSorter.insertRecord).  commit() hands them to ONE b2s_partition_compress_packed call
+// (stable partition by reduce id, then compress + checksum every partition on the GPU) and writes .data / .index /
+// .checksum through the same code as S3ShuffleMapOutputWriter.commitAllPartitions.  The files are byte for byte what
+// that writer produces when every partition is opened in order and fed its records in insertion order.
+class S3SerializedShuffleWriter {
+ public:
+  S3SerializedShuffleWriter(S3ShuffleDispatcher& d, int32_t shuffleId, int64_t mapId, int32_t numPartitions)
+      : d_(d), shuffleId_(shuffleId), mapId_(mapId), numPartitions_(numPartitions) {
+    if (numPartitions < 1 || numPartitions > (1 << 24))  // PackedRecordPointer's 24-bit partition id
+      throw RuntimeException("Precondition: numPartitions must be in [1, 2^24].");
+    if (!d.gpuEnabled) throw UnsupportedOperationException("the serialized GPU writer needs spark.shuffle.s3.gpu.enabled");
+  }
+  void insertRecord(int32_t partitionId, const uint8_t* b, uint64_t n) {
+    if (partitionId < 0 || partitionId >= numPartitions_) throw RuntimeException("Precondition: Invalid partition id.");
+    if (n > 0xffffffffull) throw RuntimeException("Precondition: record longer than 4 GiB.");
+    records_.append(b, n);
+    recLen_.push_back((uint32_t)n);
+    recPart_.push_back((uint32_t)partitionId);
+  }
+  std::vector<int64_t> commit() {
+    ensure_codec_runtime();
+    const uint32_t R = (uint32_t)numPartitions_;
+    const uint32_t codec = (uint32_t)d_.codecId();
+    const uint32_t alg = d_.checksumEnabled ? S3ShuffleHelper::createChecksumAlgorithm(d_.checksumAlgorithm) : 0;
+    const uint64_t bound = b2s_partition_compress_bound(codec, d_.lz4BlockSize, R, records_.size());
+    out_.resize(bound ? bound : 1);
+    std::vector<uint64_t> doff(R), dlen(R), cks(R);
+    std::vector<int32_t> status(R);
+    uint64_t total = 0;
+    int rc = b2s_partition_compress_packed(codec, d_.zstdLevel, d_.lz4BlockSize, alg, R, recLen_.size(), records_.data(),
+                                           records_.size(), recLen_.data(), recPart_.data(), out_.data(), bound,
+                                           doff.data(), dlen.data(), &total, cks.data(), status.data());
+    if (rc != 0)
+      throw CodecException(std::string("b2s_partition_compress_packed: ") + b2s_strerror(rc) + ": " + b2s_last_error());
+    std::vector<int64_t> lengths(R), checksums(R);
+    for (uint32_t p = 0; p < R; p++) {
+      if (status[p] != 0) throw IOException(std::string("compress failed: ") + b2s_strerror(status[p]));
+      lengths[p] = (int64_t)dlen[p];
+      checksums[p] = (int64_t)cks[p];
+    }
+    writeMapOutput(d_, shuffleId_, mapId_, true, {{out_.data(), total}}, total, lengths, checksums, measure_);
+    return lengths;
+  }
+  const S3MeasureOutputStream* measure() const { return measure_.get(); }
+
+ private:
+  S3ShuffleDispatcher& d_;
+  int32_t shuffleId_;
+  int64_t mapId_;
+  int32_t numPartitions_;
+  PinnedArena records_, out_;
+  std::vector<uint32_t> recLen_, recPart_;
   std::unique_ptr<S3MeasureOutputStream> measure_;
 };
 
@@ -773,6 +841,7 @@ using namespace b2s::host;
 static thread_local std::string t_err;
 struct b2sh_dispatcher { std::unique_ptr<S3ShuffleDispatcher> d; };
 struct b2sh_writer { std::unique_ptr<S3ShuffleMapOutputWriter> w; int32_t n; };
+struct b2sh_serialized_writer { std::unique_ptr<S3SerializedShuffleWriter> w; };
 struct b2sh_reader { std::unique_ptr<S3ShuffleReader> r; };
 struct b2sh_prefetch { std::unique_ptr<PrefetchHandle> p; };
 struct b2sh_codec { std::unique_ptr<B200CompressionCodec> c; };
@@ -850,6 +919,23 @@ int b2sh_writer_commit_all_partitions(b2sh_writer* w, const int64_t* checksums_i
 int b2sh_writer_abort(b2sh_writer* w) { return guarded([&] { w->w->abort(); }); }
 void b2sh_writer_destroy(b2sh_writer* w) { delete w; }
 
+int b2sh_serialized_writer_create(b2sh_dispatcher* d, int32_t shuffle_id, int64_t map_id, int32_t num_partitions,
+                                  b2sh_serialized_writer** out) {
+  return guarded([&] {
+    *out = new b2sh_serialized_writer{std::make_unique<S3SerializedShuffleWriter>(*d->d, shuffle_id, map_id, num_partitions)};
+  });
+}
+int b2sh_serialized_writer_insert(b2sh_serialized_writer* w, int32_t partition_id, const uint8_t* bytes, uint64_t len) {
+  return guarded([&] { w->w->insertRecord(partition_id, bytes, len); });
+}
+int b2sh_serialized_writer_commit(b2sh_serialized_writer* w, int64_t* partition_lengths_out) {
+  return guarded([&] {
+    std::vector<int64_t> l = w->w->commit();
+    memcpy(partition_lengths_out, l.data(), l.size() * 8);
+  });
+}
+void b2sh_serialized_writer_destroy(b2sh_serialized_writer* w) { delete w; }
+
 int b2sh_single_spill_transfer(b2sh_dispatcher* d, int32_t shuffle_id, int64_t map_id, const char* spill_file,
                                const int64_t* partition_lengths, const int64_t* checksums, uint32_t num_partitions,
                                int verify_on_transfer) {
@@ -911,6 +997,17 @@ static void fill_prefetch_stats(const S3BufferedPrefetchIterator::Statistics& s,
 }
 
 int b2sh_writer_statistics(b2sh_writer* w, uint64_t* bytes, uint64_t* nanos, char* line, uint32_t cap) {
+  return guarded([&] {
+    const S3MeasureOutputStream* m = w->w->measure();
+    if (!m) throw RuntimeException("no .data object was written");
+    if (bytes) *bytes = (uint64_t)m->bytes();
+    if (nanos) *nanos = (uint64_t)m->timings();
+    copy_line(m->statistics(), line, cap);
+  });
+}
+
+int b2sh_serialized_writer_statistics(b2sh_serialized_writer* w, uint64_t* bytes, uint64_t* nanos, char* line,
+                                      uint32_t cap) {
   return guarded([&] {
     const S3MeasureOutputStream* m = w->w->measure();
     if (!m) throw RuntimeException("no .data object was written");
