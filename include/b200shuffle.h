@@ -172,6 +172,40 @@ int b2s_decompress_packed(uint32_t codec, uint32_t checksum_alg, uint32_t n, con
                           uint64_t dst_cap, uint64_t* dst_off, uint64_t* dst_len, uint64_t* dst_total,
                           int32_t* status, int32_t* bad_slice);
 
+/* ---- read side, key-sorted: verify + decompress + sort a reduce task's records in one call ----
+ * Replaces, for a shuffle with a key ordering and no aggregator (sortByKey, repartitionAndSortWithinPartitions,
+ * TeraSort), the ExternalSorter that storage/S3ShuffleReader.scala:141-149 feeds with the decoded records.  The n blocks
+ * are the task's fetched blocks, with the slice and checksum arguments of b2s_decompress_packed; slices are verified
+ * before decoding.  Every decoded record is record_bytes long (a fixed-size serialized record, e.g. TeraSort's Kryo
+ * record: 104 bytes, key at 2, 10 bytes), and its key is bytes [key_off, key_off + key_len), compared as unsigned bytes,
+ * lexicographically, ascending.
+ * Output: the arena holds every record of every block exactly once, sorted by key; the sort is stable (equal keys keep
+ * block order, then their order within the block), so with a relocatable serializer the arena is again a valid
+ * serialized stream.  *dst_total = sum of the decoded lengths, *n_records = record count.  codec B2S_CODEC_NONE
+ * verifies and sorts only (spark.shuffle.compress=false).
+ * Per block: a corrupt stream, or a decoded length that is not a multiple of record_bytes (b2s_last_error() names the
+ * block), sets status[i] = B2S_E_CORRUPT; a checksum mismatch sets B2S_E_CHECKSUM and bad_slice[i] (may be NULL).  When
+ * a block fails, nothing is sorted, *n_records = 0 and the call returns 0; blocks whose slices fail verification are
+ * not decoded.
+ * Errors: key_len outside [1, 16], key_off + key_len > record_bytes, record_bytes == 0 or more than 2^32 - 1 records ->
+ * B2S_E_ARG; dst_cap below the decoded bytes -> B2S_E_DST_TOO_SMALL with *dst_total = the bytes needed; device memory
+ * for the whole task (compressed blocks, decoded records, sorted copy, sort workspace) that cannot be had -> B2S_E_NOMEM,
+ * and the caller keeps its CPU sorter.  Runs on the read lane without chunking — the whole task is resident at once —
+ * and fills b2s_last_timing (top_kernel_ms = the sort step).  The device buffers of the task stay allocated for the
+ * next call up to 1 GiB each; larger ones are freed when the call returns. */
+int b2s_decompress_sort_packed(uint32_t codec, uint32_t checksum_alg, uint32_t n, const uint8_t* src_base,
+                               const uint64_t* src_off, const uint64_t* src_len, const uint32_t* slice_base,
+                               const uint64_t* slice_len, const uint64_t* slice_checksum, uint32_t record_bytes,
+                               uint32_t key_off, uint32_t key_len, uint8_t* dst_base, uint64_t dst_cap,
+                               uint64_t* dst_total, uint64_t* n_records, int32_t* status, int32_t* bad_slice);
+/* same, with src_base / dst_base in device memory of dev_index; the descriptor arrays stay host arrays */
+int b2s_decompress_sort_dev(uint32_t dev_index, uint32_t codec, uint32_t checksum_alg, uint32_t n,
+                            const uint8_t* src_base, const uint64_t* src_off, const uint64_t* src_len,
+                            const uint32_t* slice_base, const uint64_t* slice_len, const uint64_t* slice_checksum,
+                            uint32_t record_bytes, uint32_t key_off, uint32_t key_len, uint8_t* dst_base,
+                            uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records, int32_t* status,
+                            int32_t* bad_slice);
+
 /* ---- device-resident variants (data pointers are device memory on device `dev_index` of the b2s_init selection;
  *      descriptor arrays are host memory).  Synchronous; timings retrievable with b2s_last_timing. ---- */
 int b2s_checksum_dev(uint32_t dev_index, uint32_t alg, uint32_t n, const void* d_base, const uint64_t* off,

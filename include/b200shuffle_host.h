@@ -128,6 +128,15 @@ int b2sh_reader_create(b2sh_dispatcher* d, int32_t shuffle_id, const int64_t* ma
  * block k's decoded stream is at data + off[k].  A checksum mismatch returns B2SH_E_SPARK with the reference's message,
  * a malformed stream B2SH_E_IO. */
 int b2sh_reader_read(b2sh_reader* r, uint32_t* n_blocks);
+/* read_sorted(): read() for a shuffle with a key ordering, no aggregator and fixed-size records (INTEGRATION.md §3e,
+ * spark.shuffle.s3.gpu.sortKey).  Resolves and fetches the task's non-empty blocks as read() does, then makes ONE
+ * b2s_decompress_sort_packed call: *data / *len / *n_records receive every record of the task sorted by the unsigned
+ * bytes [key_off, key_off + key_len) of each record_bytes-long record (stable: equal keys in map, then reduce-id
+ * order).  The buffer stays valid until the reader's next read or its destruction.  A checksum mismatch returns
+ * B2SH_E_SPARK with the reference's message, a malformed stream (or one that does not hold whole records) B2SH_E_IO.
+ * Codec "none" is verified and sorted only. */
+int b2sh_reader_read_sorted(b2sh_reader* r, uint32_t record_bytes, uint32_t key_off, uint32_t key_len,
+                            const uint8_t** data, uint64_t* len, uint64_t* n_records);
 int b2sh_reader_block(b2sh_reader* r, uint32_t k, int64_t* map_id, int32_t* start_reduce, int32_t* end_reduce,
                       const uint8_t** data, uint64_t* len);
 uint64_t b2sh_reader_remote_bytes_read(b2sh_reader* r); /* metric parity with storage/S3ShuffleReader.scala:94-95 */

@@ -201,6 +201,67 @@ JNIEXPORT jint JNICALL J(decompressPacked)(JNIEnv* e, jclass c, jint codec, jint
   return rc;
 }
 
+/* ---- read side, key-sorted (S3ShuffleReader.read with a key ordering, INTEGRATION.md §3e): verify, decode and sort
+ *      the task's fixed-size records by key in one call.  src / dst are direct buffer addresses (data-sized); off/len:
+ *      long[n], sliceBase: int[n+1], sliceLen/sliceChecksum: long[slices] (inputs, copied in with Get<Type>ArrayRegion);
+ *      meta: long[2] = {dst_total, n_records}; status, badSlice: int[n].  All arrays go through native copies, so no
+ *      Java array is held in a critical region while the GPU works. ---- */
+JNIEXPORT jint JNICALL J(decompressSortPacked)(JNIEnv* e, jclass c, jint codec, jint alg, jint n, jlong src,
+                                               jlongArray off, jlongArray len, jintArray sliceBase, jlongArray sliceLen,
+                                               jlongArray sliceChecksum, jint recordBytes, jint keyOff, jint keyLen,
+                                               jlong dst, jlong dstCap, jlongArray meta, jintArray status,
+                                               jintArray badSlice) {
+  (void)c;
+  if (n < 0 || !meta || (*e)->GetArrayLength(e, meta) < 2) return B2S_E_ARG;
+  if (n > 0 && (!off || !len || !status || (*e)->GetArrayLength(e, off) < n || (*e)->GetArrayLength(e, len) < n ||
+                (*e)->GetArrayLength(e, status) < n || (badSlice && (*e)->GetArrayLength(e, badSlice) < n)))
+    return B2S_E_ARG;
+  const int with_slices = alg != 0 && n > 0;
+  if (with_slices && (!sliceBase || !sliceLen || !sliceChecksum || (*e)->GetArrayLength(e, sliceBase) < n + 1))
+    return B2S_E_ARG;
+  const size_t N = (size_t)n;
+  uint64_t* blk = (uint64_t*)malloc((N * 2 + 1) * sizeof(uint64_t));
+  int32_t* st = (int32_t*)malloc((N * 2 + 1) * sizeof(int32_t));
+  uint32_t* sb = (uint32_t*)malloc((N + 1) * sizeof(uint32_t));
+  uint64_t* sl = 0;
+  int rc = blk && st && sb ? 0 : B2S_E_NOMEM;
+  if (rc == 0 && n > 0) {
+    (*e)->GetLongArrayRegion(e, off, 0, n, (jlong*)blk);
+    (*e)->GetLongArrayRegion(e, len, 0, n, (jlong*)(blk + N));
+  }
+  if (rc == 0 && with_slices) {
+    (*e)->GetIntArrayRegion(e, sliceBase, 0, n + 1, (jint*)sb);
+    const jsize ns = (jsize)sb[n];
+    if (ns < 0 || (*e)->GetArrayLength(e, sliceLen) < ns || (*e)->GetArrayLength(e, sliceChecksum) < ns) {
+      rc = B2S_E_ARG;
+    } else if (!(sl = (uint64_t*)malloc(((size_t)ns * 2 + 1) * sizeof(uint64_t)))) {
+      rc = B2S_E_NOMEM;
+    } else {
+      (*e)->GetLongArrayRegion(e, sliceLen, 0, ns, (jlong*)sl);
+      (*e)->GetLongArrayRegion(e, sliceChecksum, 0, ns, (jlong*)(sl + ns));
+    }
+  }
+  uint64_t total = 0, nrec = 0;
+  if (rc == 0) {
+    const size_t ns = with_slices ? (size_t)sb[n] : 0;
+    rc = b2s_decompress_sort_packed((uint32_t)codec, (uint32_t)alg, (uint32_t)n, PTR(const uint8_t, src), blk,
+                                    blk + N, with_slices ? sb : 0, with_slices ? sl : 0, with_slices ? sl + ns : 0,
+                                    (uint32_t)recordBytes, (uint32_t)keyOff, (uint32_t)keyLen, PTR(uint8_t, dst),
+                                    (uint64_t)dstCap, &total, &nrec, st, st + N);
+    if ((rc == 0 || rc == B2S_E_DST_TOO_SMALL) && n > 0) {
+      (*e)->SetIntArrayRegion(e, status, 0, n, (const jint*)st);
+      if (badSlice) (*e)->SetIntArrayRegion(e, badSlice, 0, n, (const jint*)(st + N));
+    }
+    const jlong m[2] = {(jlong)total, (jlong)nrec};
+    (*e)->SetLongArrayRegion(e, meta, 0, 2, m);
+  }
+  free(sl);
+  free(sb);
+  free(st);
+  free(blk);
+  return rc;
+}
+
 /* decoded size of each of n compressed streams laid out in one arena (sizes the destination of decompressPacked) */
 JNIEXPORT jint JNICALL J(decompressedSizePacked)(JNIEnv* e, jclass c, jint codec, jint n, jlong src, jlongArray off,
                                                  jlongArray len, jlongArray outLen, jintArray status) {

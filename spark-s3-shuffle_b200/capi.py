@@ -63,6 +63,12 @@ PROTOTYPES = [
      [_u32, _u32, _u32, _vp, _u64p, _u32p, _vp, _vp, _vp, _u64p, _u64p, _i32p, _i32p]),
     ("b2s_decompress_packed", C.c_int,
      [_u32, _u32, _u32, _u8p, _u64p, _u64p, _u32p, _u64p, _u64p, _u8p, _u64, _u64p, _u64p, _u64p, _i32p, _i32p]),
+    ("b2s_decompress_sort_packed", C.c_int,
+     [_u32, _u32, _u32, _u8p, _u64p, _u64p, _u32p, _u64p, _u64p, _u32, _u32, _u32, _u8p, _u64, _u64p, _u64p, _i32p,
+      _i32p]),
+    ("b2s_decompress_sort_dev", C.c_int,
+     [_u32, _u32, _u32, _u32, _vp, _u64p, _u64p, _u32p, _u64p, _u64p, _u32, _u32, _u32, _vp, _u64, _u64p, _u64p, _i32p,
+      _i32p]),
     ("b2s_checksum_dev", C.c_int, [_u32, _u32, _u32, _vp, _u64p, _u64p, _u64p]),
     ("b2s_compress_dev", C.c_int,
      [_u32, _u32, _i32, _u32, _u32, _u32, _vp, _u64p, _u64p, _vp, _u64, _u64p, _u64p, _u64p, _u64p, _i32p]),
@@ -334,6 +340,32 @@ def decompress_packed(codec, src, off, length, dst, checksum_alg=CHECKSUM_NONE, 
     return dict(dst_off=dst_off[:n], dst_len=dst_len[:n], total=total.value, status=st[:n], bad_slice=bad[:n])
 
 
+def _sort_slices(checksum_alg, slice_base, slice_len, slice_checksum):
+    if checksum_alg == CHECKSUM_NONE:
+        return None, None, None
+    return (np.ascontiguousarray(slice_base, dtype=np.uint32), np.ascontiguousarray(slice_len, dtype=np.uint64),
+            np.ascontiguousarray(slice_checksum, dtype=np.uint64))
+
+
+def decompress_sort_packed(codec, src, off, length, dst, record_bytes, key_off, key_len, checksum_alg=CHECKSUM_NONE,
+                           slice_base=None, slice_len=None, slice_checksum=None):
+    """Verifies and decodes a reduce task's blocks and sorts their fixed-size records by the unsigned bytes
+    [key_off, key_off + key_len) into dst (stable).  -> dict(total, n_records, status, bad_slice)"""
+    src, dst = _as_u8(src), _as_u8(dst)
+    off = np.ascontiguousarray(off, dtype=np.uint64)
+    length = np.ascontiguousarray(length, dtype=np.uint64)
+    n = off.size
+    sb, sl, sc = _sort_slices(checksum_alg, slice_base, slice_len, slice_checksum)
+    st = np.zeros(max(n, 1), dtype=np.int32)
+    bad = np.zeros(max(n, 1), dtype=np.int32)
+    total, nrec = _u64(0), _u64(0)
+    _check(load().b2s_decompress_sort_packed(codec, checksum_alg, n, _ptr(src), _ptr(off), _ptr(length), _ptr(sb),
+                                             _ptr(sl), _ptr(sc), record_bytes, key_off, key_len, _ptr(dst), dst.size,
+                                             C.addressof(total), C.addressof(nrec), _ptr(st), _ptr(bad)),
+           "b2s_decompress_sort_packed")
+    return dict(total=total.value, n_records=nrec.value, status=st[:n], bad_slice=bad[:n])
+
+
 # ---------------------------------------------------------------------------------------------------------------
 # device-resident API (bench.py roofline leg); d_* are raw device addresses (ints)
 # ---------------------------------------------------------------------------------------------------------------
@@ -398,6 +430,23 @@ def decompress_dev(codec, d_src, off, length, d_dst, dst_cap, checksum_alg=CHECK
                                      _ptr(sc), d_dst, dst_cap, _ptr(dst_off), _ptr(dst_len), C.addressof(total),
                                      _ptr(st), _ptr(bad)), "b2s_decompress_dev")
     return dict(dst_off=dst_off[:n], dst_len=dst_len[:n], total=total.value, status=st[:n], bad_slice=bad[:n])
+
+
+def decompress_sort_dev(codec, d_src, off, length, d_dst, dst_cap, record_bytes, key_off, key_len,
+                        checksum_alg=CHECKSUM_NONE, slice_base=None, slice_len=None, slice_checksum=None, dev=0):
+    """decompress_sort_packed on device-resident blocks (d_src) into a device arena (d_dst)"""
+    off = np.ascontiguousarray(off, dtype=np.uint64)
+    length = np.ascontiguousarray(length, dtype=np.uint64)
+    n = off.size
+    sb, sl, sc = _sort_slices(checksum_alg, slice_base, slice_len, slice_checksum)
+    st = np.zeros(max(n, 1), dtype=np.int32)
+    bad = np.zeros(max(n, 1), dtype=np.int32)
+    total, nrec = _u64(0), _u64(0)
+    _check(load().b2s_decompress_sort_dev(dev, codec, checksum_alg, n, d_src, _ptr(off), _ptr(length), _ptr(sb),
+                                          _ptr(sl), _ptr(sc), record_bytes, key_off, key_len, d_dst, dst_cap,
+                                          C.addressof(total), C.addressof(nrec), _ptr(st), _ptr(bad)),
+           "b2s_decompress_sort_dev")
+    return dict(total=total.value, n_records=nrec.value, status=st[:n], bad_slice=bad[:n])
 
 
 def partition_compress_dev(codec, d_records, rec_bytes, d_rec_len, d_rec_part, n_records, num_partitions, d_dst,

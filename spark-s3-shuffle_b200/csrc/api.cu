@@ -166,10 +166,12 @@ struct DevBuf {
     size_t want = align_up(bytes + bytes / 8, 1 << 20);
     cudaError_t e = cudaMalloc(&p, want);
     if (e != cudaSuccess) {
+      (void)cudaGetLastError();  // an allocation failure is reported as B2S_E_NOMEM, not left for a later CU() check
       e = cudaMalloc(&p, bytes);
       want = bytes;
     }
     if (e != cudaSuccess) {
+      (void)cudaGetLastError();
       p = nullptr;
       return fail(B2S_E_NOMEM, "cudaMalloc: %s", cudaGetErrorString(e));
     }
@@ -194,6 +196,7 @@ struct PinBuf {
     numa::PreferNode near(t_numa_node);
     cudaError_t e = cudaHostAlloc(&p, want, cudaHostAllocDefault);
     if (e != cudaSuccess) {
+      (void)cudaGetLastError();  // reported as B2S_E_NOMEM, not left for a later CU() check
       p = nullptr;
       return fail(B2S_E_NOMEM, "cudaHostAlloc: %s", cudaGetErrorString(e));
     }
@@ -522,8 +525,12 @@ struct DecompressJob {
   bool size_only = false;
 };
 
-int decompress_prepare(Slot& S, uint32_t codec, uint32_t alg, uint32_t n, uint32_t n_slices, DecompressJob& J) {
-  if (codec != B2S_CODEC_LZ4BLOCK && codec != B2S_CODEC_SNAPPY_XERIAL && codec != B2S_CODEC_ZSTD)
+// allow_none: codec NONE verifies the slices only and reports the stored lengths as decoded lengths in phase A (the
+// key sort of uncompressed blocks); phase B is not run for it
+int decompress_prepare(Slot& S, uint32_t codec, uint32_t alg, uint32_t n, uint32_t n_slices, DecompressJob& J,
+                       bool allow_none = false) {
+  if (codec != B2S_CODEC_LZ4BLOCK && codec != B2S_CODEC_SNAPPY_XERIAL && codec != B2S_CODEC_ZSTD &&
+      !(allow_none && codec == B2S_CODEC_NONE))
     return fail(B2S_E_UNSUPPORTED, "codec %s not supported by this build", "");
   J.n = n;
   J.codec = codec;
@@ -629,7 +636,10 @@ int decompress_enqueue_a(Slot& S, const ChecksumTables& tabs, uint32_t alg, Deco
     CU(cudaMemsetAsync(J.nblk, 0, (size_t)n * 8, st));
   } else if (J.codec == B2S_CODEC_SNAPPY_XERIAL)
     launch_xerial_count(d_src, J.src_off, J.src_len, n, J.nblk, J.olen, J.totals + 2, J.status, st, launches);
-  else
+  else if (J.codec == B2S_CODEC_NONE) {  // stored bytes: decoded length = block length, no codec blocks
+    CU(cudaMemcpyAsync(J.olen, J.src_len, (size_t)n * 8, cudaMemcpyDeviceToDevice, st));
+    CU(cudaMemsetAsync(J.nblk, 0, (size_t)n * 8, st));
+  } else
     launch_lz4block_count(d_src, J.src_off, J.src_len, n, J.nblk, J.olen, J.totals + 2, J.status, st, launches);
   // dst_off = exclusive scan(olen) ; blk_base = exclusive scan(nblk) (in place)
   CU(cudaMemcpyAsync(J.dst_off, J.olen, (size_t)n * 8, cudaMemcpyDeviceToDevice, st));
@@ -2160,6 +2170,264 @@ int b2s_decompress_packed(uint32_t codec, uint32_t checksum_alg, uint32_t n, con
   for (uint32_t i = 0; i < n; i++) ptr[i] = src_base + src_off[i];
   return decompress_host(codec, checksum_alg, n, ptr.data(), src_len, slice_base, slice_len, slice_checksum, dst_base,
                          dst_cap, nullptr, nullptr, dst_off, dst_len, dst_total, status, bad_slice, false);
+}
+
+// ------------------------------------------------------------------------------------------------------------
+// read side, key-sorted: verify + decode a reduce task's blocks, then sort its fixed-size records by key
+// ------------------------------------------------------------------------------------------------------------
+static int sort_args(uint32_t codec, uint32_t alg, uint32_t n, const uint64_t* src_off, const uint64_t* src_len,
+                     const uint32_t* slice_base, const uint64_t* slice_len, const uint64_t* slice_checksum,
+                     uint32_t record_bytes, uint32_t key_off, uint32_t key_len, const void* src_base,
+                     const void* dst_base, uint64_t dst_cap, const uint64_t* dst_total, const uint64_t* n_records,
+                     const int32_t* status) {
+  if (alg > B2S_CHECKSUM_CRC32C) return fail(B2S_E_UNSUPPORTED, "Unsupported shuffle checksum algorithm%s");
+  if (codec > B2S_CODEC_ZSTD) return fail(B2S_E_UNSUPPORTED, "codec %s not supported by this build", "");
+  if (record_bytes == 0) return fail(B2S_E_ARG, "record_bytes must be at least 1%s");
+  if (key_len < 1 || key_len > 16) return fail(B2S_E_ARG, "key_len must be in [1, 16]%s");
+  if ((uint64_t)key_off + key_len > record_bytes) return fail(B2S_E_ARG, "key_off + key_len exceeds record_bytes%s");
+  if (!dst_total || !n_records) return fail(B2S_E_ARG, "null argument%s");
+  if (n && (!src_base || !src_off || !src_len || !status)) return fail(B2S_E_ARG, "null argument%s");
+  if (dst_cap && !dst_base) return fail(B2S_E_ARG, "null argument%s");
+  if (alg && n && (!slice_base || !slice_len || !slice_checksum)) return fail(B2S_E_ARG, "slice arrays required%s");
+  if (alg && n) return check_slices(n, src_len, slice_base, slice_len);
+  return 0;
+}
+
+// without a usable device the sort calls report B2S_E_CUDA (b2s_init has failed for that reason), otherwise as get_device
+static int sort_device(uint32_t dev_index, Device** out) {
+  if (!g_ctx) {
+    int count = 0;
+    const cudaError_t e = cudaGetDeviceCount(&count);
+    if (e != cudaSuccess || count <= 0)
+      return fail(B2S_E_CUDA, "no CUDA device: %s", e != cudaSuccess ? cudaGetErrorString(e) : "device count is 0");
+  }
+  return get_device(dev_index, out);
+}
+
+// The whole-task buffers of a sort call (read-lane slot 0: compressed blocks, decoded arena, sorted copy, sort
+// workspace) only grow while they are in use.  When a call ends — whatever its result — every one of them above
+// kSortKeepBytes is freed, so one oversized task does not keep several times its size of device memory for the rest
+// of the process; buffers up to that size stay for the next call (a TeraSort reducer of 200 over 10 GiB needs ~55 MB).
+constexpr size_t kSortKeepBytes = 1ull << 30;
+struct SortBufferTrim {
+  Slot& S;
+  ~SortBufferTrim() {
+    for (DevBuf* b : {&S.src, &S.dst, &S.parena, &S.pws})
+      if (b->cap > kSortKeepBytes) b->release();
+  }
+};
+
+// The whole reduce task on the device: compressed blocks at d_src + src_dev_off[i] (src_contiguous: back to back from
+// d_src in block order, no gaps).  Phase A verifies the slices and sizes every block; a failed block, or a decoded
+// length that is not a multiple of record_bytes, ends the call with status[] set and *n_rec = 0 (nothing decoded or
+// sorted).  Then the blocks are decoded into S.dst (codec NONE: used in place, or copied there), their records sorted
+// into *d_sorted (nullptr: into S.parena, returned there).
+static int decompress_sort_run(Device* D, Slot& S, uint32_t codec, uint32_t alg, uint32_t n, const uint8_t* d_src,
+                               const uint64_t* src_dev_off, const uint64_t* src_len, bool src_contiguous,
+                               const uint32_t* slice_base, const uint64_t* slice_len, const uint64_t* slice_sum,
+                               uint32_t record_bytes, uint32_t key_off, uint32_t key_len, uint8_t** d_sorted,
+                               uint64_t out_cap, uint64_t* total, uint64_t* n_rec, int32_t* status, int32_t* bad_slice,
+                               uint64_t* launches) {
+  cudaStream_t st = S.st;
+  DecompressJob J;
+  const uint32_t ns = alg ? slice_base[n] : 0;
+  int rc = decompress_prepare(S, codec, alg, n, ns, J, true);
+  if (rc) return rc;
+  memcpy(J.h_src_off, src_dev_off, (size_t)n * 8);
+  memcpy(J.h_src_len, src_len, (size_t)n * 8);
+  fill_slices(J, 0, n, src_dev_off, src_len, slice_base, slice_len, slice_sum);
+  uint64_t srcb = 0;
+  for (uint32_t i = 0; i < n; i++) srcb += src_len[i];
+  rc = decompress_enqueue_a(S, D->tabs, alg, J, d_src, srcb, launches);
+  if (rc) return rc;
+  // the phase-A verdicts (checksums, stream headers) and decoded lengths, before anything is decoded
+  CU(cudaMemcpyAsync(J.h_down, J.d_down, J.down_bytes, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  CU(cudaGetLastError());
+  *total = J.h_totals[1];
+  *n_rec = 0;
+  bool failed = false;
+  char msg[256];
+  for (uint32_t i = 0; i < n; i++) {
+    if (J.h_status[i] == B2S_OK && J.h_dst_len[i] % record_bytes) {
+      J.h_status[i] = B2S_E_CORRUPT;
+      if (!failed) {
+        snprintf(msg, sizeof msg, "block %u decodes to %llu bytes, not a multiple of record_bytes %u", i,
+                 (unsigned long long)J.h_dst_len[i], record_bytes);
+        fail(B2S_E_CORRUPT, "%s", msg);
+      }
+    }
+    failed |= J.h_status[i] != B2S_OK;
+  }
+  auto report = [&]() {
+    memcpy(status, J.h_status, (size_t)n * 4);
+    if (bad_slice) memcpy(bad_slice, J.h_bad, (size_t)n * 4);
+  };
+  auto skip_events = [&](bool decode, bool sort) -> int {  // stand-ins for the steps a call does not run
+    if (decode) {
+      CU(cudaEventRecord(S.ev_t0, st));
+      CU(cudaEventRecord(S.ev_t1, st));
+      CU(cudaEventRecord(S.ev_k1, st));
+    }
+    if (sort) {
+      CU(cudaEventRecord(S.ev_p0, st));
+      CU(cudaEventRecord(S.ev_p1, st));
+    }
+    CU(cudaStreamSynchronize(st));
+    return 0;
+  };
+  if (failed) {
+    report();
+    return skip_events(true, true);
+  }
+  const uint64_t records = *total / record_bytes;
+  if (records > 0xffffffffull)
+    return fail(B2S_E_ARG, "more than 2^32 - 1 records in one call (%s bytes)", std::to_string(*total).c_str());
+  if (*total > out_cap) {
+    report();
+    return fail(B2S_E_DST_TOO_SMALL, "dst_cap is below the %s decoded bytes", std::to_string(*total).c_str());
+  }
+
+  // the decoded arena: every block's records back to back in block order
+  const uint8_t* arena = d_src;
+  if (codec == B2S_CODEC_NONE) {
+    if (!src_contiguous && *total) {
+      if ((rc = S.dst.ensure(*total + 64))) return rc;
+      for (uint32_t i = 0; i < n; i++)
+        if (src_len[i])
+          CU(cudaMemcpyAsync((uint8_t*)S.dst.p + J.h_dst_off[i], d_src + src_dev_off[i], src_len[i],
+                             cudaMemcpyDeviceToDevice, st));
+      arena = (const uint8_t*)S.dst.p;
+    }
+    if ((rc = skip_events(true, false))) return rc;
+  } else {
+    if ((rc = S.dst.ensure(*total + 64))) return rc;
+    rc = decompress_enqueue_b(S, J, d_src, (uint8_t*)S.dst.p, S.dst.cap, launches);
+    if (rc) return rc;
+    CU(cudaEventSynchronize(S.ev_b));
+    CU(cudaGetLastError());
+    for (uint32_t i = 0; i < n; i++) failed |= J.h_status[i] != B2S_OK;
+    if (failed) {
+      report();
+      return skip_events(false, true);
+    }
+    arena = (const uint8_t*)S.dst.p;
+  }
+  report();
+
+  if (!*d_sorted) {
+    if ((rc = S.parena.ensure(*total + 64))) return rc;
+    *d_sorted = (uint8_t*)S.parena.p;
+  }
+  if (records && (rc = S.pws.ensure(key_sort_ws_bytes(records, key_len)))) return rc;
+  CU(cudaEventRecord(S.ev_p0, st));
+  launch_key_sort(arena, records, record_bytes, key_off, key_len, (uint8_t*)S.pws.p, *d_sorted, st, launches);
+  CU(cudaEventRecord(S.ev_p1, st));
+  CU(cudaStreamSynchronize(st));
+  CU(cudaGetLastError());
+  *n_rec = records;
+  return 0;
+}
+
+// kernel_ms: verification + decode + sort; top_kernel_ms: the sort step
+static void sort_timing(Slot& S, uint64_t n_launches, uint64_t src_bytes, uint64_t total) {
+  add_timing(S, false);
+  t_timing.kernel_ms = ms_between(S.ev_k0, S.ev_p1);
+  t_timing.top_kernel_ms = ms_between(S.ev_p0, S.ev_p1);
+  t_timing.kernel_launches = n_launches;
+  t_timing.src_bytes = src_bytes;
+  t_timing.dst_bytes = total;
+  g_ctx->launches += n_launches;
+}
+
+int b2s_decompress_sort_dev(uint32_t dev_index, uint32_t codec, uint32_t checksum_alg, uint32_t n,
+                            const uint8_t* src_base, const uint64_t* src_off, const uint64_t* src_len,
+                            const uint32_t* slice_base, const uint64_t* slice_len, const uint64_t* slice_checksum,
+                            uint32_t record_bytes, uint32_t key_off, uint32_t key_len, uint8_t* dst_base,
+                            uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records, int32_t* status,
+                            int32_t* bad_slice) {
+  WallTimer wt;
+  t_timing = b2s_timing{};
+  if (dst_total) *dst_total = 0;
+  if (n_records) *n_records = 0;
+  Device* D;
+  int rc = sort_device(dev_index, &D);
+  if (rc) return rc;
+  rc = sort_args(codec, checksum_alg, n, src_off, src_len, slice_base, slice_len, slice_checksum, record_bytes, key_off,
+                 key_len, src_base, dst_base, dst_cap, dst_total, n_records, status);
+  if (rc || !n) return rc;
+  Lane& Ln = D->lane[kLaneRead];
+  std::lock_guard<std::mutex> lk(Ln.mtx);
+  Slot& S = Ln.slot[0];
+  SortBufferTrim trim{S};
+  uint64_t launches = 0, srcb = 0;
+  for (uint32_t i = 0; i < n; i++) srcb += src_len[i];
+  uint8_t* out = dst_base;
+  rc = decompress_sort_run(D, S, codec, checksum_alg, n, src_base, src_off, src_len, false, slice_base, slice_len,
+                           slice_checksum, record_bytes, key_off, key_len, &out, dst_cap, dst_total, n_records, status,
+                           bad_slice, &launches);
+  if (rc) return rc;
+  sort_timing(S, launches, srcb, *dst_total);
+  t_timing.total_ms = wt.ms();
+  return 0;
+}
+
+int b2s_decompress_sort_packed(uint32_t codec, uint32_t checksum_alg, uint32_t n, const uint8_t* src_base,
+                               const uint64_t* src_off, const uint64_t* src_len, const uint32_t* slice_base,
+                               const uint64_t* slice_len, const uint64_t* slice_checksum, uint32_t record_bytes,
+                               uint32_t key_off, uint32_t key_len, uint8_t* dst_base, uint64_t dst_cap,
+                               uint64_t* dst_total, uint64_t* n_records, int32_t* status, int32_t* bad_slice) {
+  WallTimer wt;
+  t_timing = b2s_timing{};
+  if (dst_total) *dst_total = 0;
+  if (n_records) *n_records = 0;
+  Device* D;
+  int rc = sort_device(t_device, &D);
+  if (rc) return rc;
+  rc = sort_args(codec, checksum_alg, n, src_off, src_len, slice_base, slice_len, slice_checksum, record_bytes, key_off,
+                 key_len, src_base, dst_base, dst_cap, dst_total, n_records, status);
+  if (rc || !n) return rc;
+  Lane& Ln = D->lane[kLaneRead];
+  std::lock_guard<std::mutex> lk(Ln.mtx);
+  Slot& S = Ln.slot[0];
+  SortBufferTrim trim{S};
+  // one upload of every block, back to back (the whole task is resident at once: no chunking)
+  std::vector<uint64_t> dev_off(n);
+  uint64_t srcb = 0;
+  for (uint32_t i = 0; i < n; i++) {
+    dev_off[i] = srcb;
+    srcb += src_len[i];
+  }
+  if ((rc = S.src.ensure(srcb + 64))) return rc;
+  cudaStream_t st = S.st;
+  CU(cudaEventRecord(S.ev_h0, st));
+  for (uint32_t i = 0; i < n;) {  // blocks adjacent in host memory go up in one copy
+    uint32_t j = i + 1;
+    while (j < n && src_off[j] == src_off[j - 1] + src_len[j - 1]) j++;
+    const uint64_t bytes = dev_off[j - 1] + src_len[j - 1] - dev_off[i];
+    if (bytes) CU(copy_async((uint8_t*)S.src.p + dev_off[i], src_base + src_off[i], bytes, cudaMemcpyHostToDevice, st));
+    i = j;
+  }
+  CU(cudaEventRecord(S.ev_h1, st));
+  uint64_t launches = 0;
+  uint8_t* sorted = nullptr;
+  rc = decompress_sort_run(D, S, codec, checksum_alg, n, (const uint8_t*)S.src.p, dev_off.data(), src_len, true,
+                           slice_base, slice_len, slice_checksum, record_bytes, key_off, key_len, &sorted, dst_cap,
+                           dst_total, n_records, status, bad_slice, &launches);
+  if (rc) return rc;
+  const uint64_t down = *n_records ? *dst_total : 0;
+  CU(cudaEventRecord(S.ev_d0, st));
+  if (down) CU(copy_async(dst_base, sorted, down, cudaMemcpyDeviceToHost, st));
+  CU(cudaEventRecord(S.ev_d1, st));
+  CU(cudaStreamSynchronize(st));
+  CU(cudaGetLastError());
+  sort_timing(S, launches, srcb, *dst_total);
+  t_timing.h2d_ms = ms_between(S.ev_h0, S.ev_h1);
+  t_timing.d2h_ms = ms_between(S.ev_d0, S.ev_d1);
+  t_timing.h2d_bytes = srcb;
+  t_timing.d2h_bytes = down;
+  t_timing.total_ms = wt.ms();
+  return 0;
 }
 
 int b2s_decompressed_size_batch(uint32_t codec, uint32_t n, const uint8_t* const* src, const uint64_t* src_len,

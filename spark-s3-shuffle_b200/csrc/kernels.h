@@ -166,6 +166,14 @@ struct PartitionPlan {
   uint64_t* readback = nullptr;
   size_t readback_bytes = 0;
 };
+// One stable LSD radix pass over n (key, record index) pairs (n < 2^32), digit (key >> shift) & (nd - 1), nd a power of
+// two <= 256: a per-tile histogram, one scan over the digit-major histogram, a stable scatter.  idx_in == nullptr: the
+// index is the position.  hist: radix_hist_elems(n) u64, hist_total: one u64, scan_ws: scan_ws_elems(that) u64.
+// Shared by the partition step and the key sort (sort.cu).
+size_t radix_hist_elems(uint64_t n);
+void launch_radix_pass(const uint32_t* keys_in, const uint32_t* idx_in, uint32_t n, int shift, uint32_t nd,
+                       uint64_t* hist, uint64_t* hist_total, uint64_t* scan_ws, uint32_t* keys_out, uint32_t* idx_out,
+                       cudaStream_t st, uint64_t* launches);
 uint32_t partition_radix_passes(uint32_t num_partitions);
 size_t partition_ws_bytes(uint64_t n, uint32_t num_partitions);  // d_ws of launch_partition
 void launch_partition(const uint32_t* d_rec_len, const uint32_t* d_rec_part, uint64_t n, uint32_t num_partitions,
@@ -175,6 +183,14 @@ void launch_partition(const uint32_t* d_rec_len, const uint32_t* d_rec_part, uin
 // to the arena size)
 void launch_partition_gather(const uint8_t* rec_base, const uint32_t* d_rec_len, uint64_t n, const PartitionPlan& plan,
                              uint8_t* d_dst, cudaStream_t st, uint64_t* launches);
+
+// ---------------- sort.cu (stable sort of fixed-size records by an unsigned byte key) ----------------
+// n records of record_bytes each, back to back at d_rec (n < 2^32); the key of a record is its bytes
+// [key_off, key_off + key_len), 1 <= key_len <= 16, compared as unsigned bytes, lexicographically.  Writes the records
+// to d_dst in ascending key order, equal keys in input order.  d_ws: key_sort_ws_bytes(n, key_len).
+size_t key_sort_ws_bytes(uint64_t n, uint32_t key_len);
+void launch_key_sort(const uint8_t* d_rec, uint64_t n, uint32_t record_bytes, uint32_t key_off, uint32_t key_len,
+                     uint8_t* d_ws, uint8_t* d_dst, cudaStream_t st, uint64_t* launches);
 
 // ---------------- gen.cu (bench utility) ----------------
 void launch_gen_terasort(uint8_t* d_dst, uint64_t first_record, uint64_t n_records, uint64_t seed, cudaStream_t st);

@@ -226,9 +226,23 @@ uint32_t partition_radix_passes(uint32_t num_partitions) {
   return (bits + 7) / 8;
 }
 
-size_t partition_ws_bytes(uint64_t n, uint32_t num_partitions) {
+size_t radix_hist_elems(uint64_t n) {
   const uint64_t ntiles = (n + kPartTile - 1) / kPartTile;
-  const size_t hist = (size_t)256 * (ntiles ? ntiles : 1);
+  return (size_t)256 * (ntiles ? ntiles : 1);
+}
+
+void launch_radix_pass(const uint32_t* keys_in, const uint32_t* idx_in, uint32_t n, int shift, uint32_t nd,
+                       uint64_t* hist, uint64_t* hist_total, uint64_t* scan_ws, uint32_t* keys_out, uint32_t* idx_out,
+                       cudaStream_t st, uint64_t* launches) {
+  const uint32_t ntiles = (uint32_t)(((uint64_t)n + kPartTile - 1) / kPartTile);
+  part_hist_kernel<<<ntiles, kPartThreads, 0, st>>>(keys_in, n, shift, nd, ntiles, hist);
+  launch_exclusive_scan_u64(hist, (size_t)nd * ntiles, hist_total, scan_ws, st, launches);
+  part_scatter_kernel<<<ntiles, kPartThreads, 0, st>>>(keys_in, idx_in, n, shift, nd, ntiles, hist, keys_out, idx_out);
+  if (launches) *launches += 2;
+}
+
+size_t partition_ws_bytes(uint64_t n, uint32_t num_partitions) {
+  const size_t hist = radix_hist_elems(n);
   auto a = [](size_t b) { return (b + 255) / 256 * 256; };
   return a((n + 1) * 8) * 2 + a(n * 4) * 4 + a(hist * 8) + a(scan_ws_elems(std::max<size_t>(hist, n + 1)) * 8) +
          256 + a(((size_t)num_partitions + 2) * 8) + 1024;
@@ -238,8 +252,7 @@ void launch_partition(const uint32_t* d_rec_len, const uint32_t* d_rec_part, uin
                       uint8_t* d_ws, PartitionPlan* plan, cudaStream_t st,
                       uint64_t* launches) {
   auto a = [](size_t b) { return (b + 255) / 256 * 256; };
-  const uint64_t ntiles = (n + kPartTile - 1) / kPartTile;
-  const size_t hist_elems = (size_t)256 * (ntiles ? ntiles : 1);
+  const size_t hist_elems = radix_hist_elems(n);
   uint8_t* p = d_ws;
   plan->src_off = (uint64_t*)p;  p += a((n + 1) * 8);
   plan->sdst = (uint64_t*)p;     p += a((n + 1) * 8);
@@ -274,14 +287,10 @@ void launch_partition(const uint32_t* d_rec_len, const uint32_t* d_rec_part, uin
     const uint32_t* kin = keys ? keys : d_rec_part;
     uint32_t* kout = (k & 1) ? kB : kA;
     uint32_t* iout = (k & 1) ? iB : iA;
-    part_hist_kernel<<<(unsigned)ntiles, kPartThreads, 0, st>>>(kin, (uint32_t)n, shift, nd, (uint32_t)ntiles, hist);
-    launch_exclusive_scan_u64(hist, (size_t)nd * ntiles, unused_total, ws, st, launches);
-    part_scatter_kernel<<<(unsigned)ntiles, kPartThreads, 0, st>>>(kin, idx, (uint32_t)n, shift, nd, (uint32_t)ntiles,
-                                                                   hist, kout, iout);
+    launch_radix_pass(kin, idx, (uint32_t)n, shift, nd, hist, unused_total, ws, kout, iout, st, launches);
     keys = kout;
     idx = iout;
     shift += (int)pb;
-    if (launches) *launches += 2;
   }
   plan->idx = idx;
   part_sorted_len_kernel<<<grid_for(n), kPartThreads, 0, st>>>(idx, d_rec_len, n, plan->sdst);

@@ -59,6 +59,8 @@ PROTOTYPES = [
     ("b2sh_single_spill_transfer", C.c_int, [_vp, _i32, _i64, C.c_char_p, _vp, _vp, _u32, C.c_int]),
     ("b2sh_reader_create", C.c_int, [_vp, _i32, _vp, _u32, _i32, _i32, C.c_int, C.POINTER(_vp)]),
     ("b2sh_reader_read", C.c_int, [_vp, C.POINTER(_u32)]),
+    ("b2sh_reader_read_sorted", C.c_int,
+     [_vp, _u32, _u32, _u32, C.POINTER(_vp), C.POINTER(_u64), C.POINTER(_u64)]),
     ("b2sh_reader_block", C.c_int,
      [_vp, _u32, C.POINTER(_i64), C.POINTER(_i32), C.POINTER(_i32), C.POINTER(_vp), C.POINTER(_u64)]),
     ("b2sh_reader_remote_bytes_read", _u64, [_vp]),
@@ -319,6 +321,14 @@ class S3ShuffleReader:
         n = _u32(0)
         _check(load().b2sh_reader_read(self._h, C.byref(n)))
         return self._blocks(n.value)
+
+    def readSorted(self, recordBytes, keyOffset, keyLength):
+        """read() with a key ordering (spark.shuffle.s3.gpu.sortKey=recordBytes,keyOffset,keyLength): every record
+        of the task in ascending unsigned-byte key order, stable.  -> (bytes, number of records)"""
+        p, ln, nrec = _vp(), _u64(), _u64()
+        _check(load().b2sh_reader_read_sorted(self._h, recordBytes, keyOffset, keyLength, C.byref(p), C.byref(ln),
+                                              C.byref(nrec)))
+        return (C.string_at(p.value, ln.value) if ln.value else b""), nrec.value
 
     def _blocks(self, n):
         out = []

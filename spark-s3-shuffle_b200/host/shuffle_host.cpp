@@ -682,14 +682,94 @@ class S3ShuffleReader {
     decoded_ = std::move(bufs);
   }
 
-  void open() {
+  void open() { start(false); }
+
+  // read() for a shuffle with a key ordering whose records are recordBytes long and order by the unsigned bytes
+  // [keyOff, keyOff + keyLen) (INTEGRATION.md §3e): every non-empty block is fetched and staged, then ONE
+  // b2s_decompress_sort_packed call verifies, decodes and key-sorts all of the task's records.  The blocks go in
+  // computeShuffleBlocks order (map, then reduce id), so records with equal keys come out in that order whatever the
+  // order the fetches completed in.  Codec NONE (spark.shuffle.compress=false) is verified and sorted only.
+  void readSorted(uint32_t recordBytes, uint32_t keyOff, uint32_t keyLen) {
+    start(true);
+    std::vector<std::pair<uint64_t, std::vector<uint8_t>>> fetched;  // (tag, compressed bytes)
+    while (iter_->hasNext()) {
+      for (auto& f : iter_->nextBatch(0)) {
+        auto& st = *f.stream;
+        // the whole block through the adaptor, from its first byte: the buffered head, then (a block larger than the
+        // task's budget) the tail straight from the block stream
+        std::vector<uint8_t> b((size_t)st.totalBytes());
+        int64_t at = 0, r;
+        while (at < st.totalBytes() && (r = st.read(b.data() + at, st.totalBytes() - at)) > 0) at += r;
+        b.resize((size_t)at);
+        fetched.emplace_back(f.tag, std::move(b));
+        st.close();  // the budget goes back to the prefetcher before the next fetches are waited for
+      }
+      batches_++;
+    }
+    stats_ = iter_->statistics();
+    std::sort(fetched.begin(), fetched.end(), [](const auto& a, const auto& b) { return a.first < b.first; });
+    const uint32_t n = (uint32_t)fetched.size();
+    const bool verify = d_.checksumEnabled;
+    const uint32_t alg = verify ? S3ShuffleHelper::createChecksumAlgorithm(d_.checksumAlgorithm) : 0;
+    std::vector<uint64_t> off(n), len(n), tags(n), sliceLen, sliceSum;
+    std::vector<uint32_t> sliceBase(n + 1, 0);
+    uint64_t bytes = 0;
+    for (uint32_t k = 0; k < n; k++) {
+      tags[k] = fetched[k].first;
+      off[k] = bytes;
+      len[k] = fetched[k].second.size();
+      bytes += len[k];
+      const ShuffleBlockInfo& bi = info_[fetched[k].first];
+      sliceLen.insert(sliceLen.end(), bi.sliceLen.begin(), bi.sliceLen.end());
+      sliceSum.insert(sliceSum.end(), bi.sliceSum.begin(), bi.sliceSum.end());
+      sliceBase[k + 1] = (uint32_t)sliceLen.size();
+    }
+    PinnedArena src;
+    src.resize(bytes ? bytes : 1);
+    for (uint32_t k = 0; k < n; k++) memcpy(src.data() + off[k], fetched[k].second.data(), (size_t)len[k]);
+    fetched.clear();
+    ensure_codec_runtime();
+    const uint32_t codec = (uint32_t)d_.codecId();
+    // Output size: codec NONE decodes to the stored bytes.  For a codec, a first guess of 4x the compressed bytes (the
+    // pages of the untouched tail are never faulted in); a call it is too small for ends after verification with the
+    // bytes needed in `total`, and the one retry uses exactly that.
+    uint64_t cap = codec == B2S_CODEC_NONE ? bytes : bytes * 4;
+    std::vector<int32_t> status(n), bad(n);
+    uint64_t total = 0, records = 0;
+    int rc = B2S_E_DST_TOO_SMALL;
+    for (int attempt = 0; attempt < 2 && rc == B2S_E_DST_TOO_SMALL; attempt++) {
+      if (attempt) cap = total;
+      sorted_.reset(new uint8_t[(size_t)(cap ? cap : 1)]);
+      rc = b2s_decompress_sort_packed(codec, alg, n, src.data(), off.data(), len.data(), verify ? sliceBase.data() : nullptr,
+                                      verify ? sliceLen.data() : nullptr, verify ? sliceSum.data() : nullptr, recordBytes,
+                                      keyOff, keyLen, sorted_.get(), cap, &total, &records, status.data(), bad.data());
+    }
+    if (rc != 0)
+      throw CodecException(std::string("b2s_decompress_sort_packed: ") + b2s_strerror(rc) + ": " + b2s_last_error());
+    for (uint32_t k = 0; k < n; k++) {
+      const BlockId& id = info_[tags[k]].id;
+      if (status[k] == B2S_E_CHECKSUM)  // storage/S3ChecksumValidationStream.scala:72-74
+        throw SparkException("Invalid checksum detected for " + id.name());
+      if (status[k] == B2S_E_CORRUPT) throw IOException("Stream is corrupted");
+      if (status[k] != 0) throw IOException(std::string("decompress failed: ") + b2s_strerror(status[k]));
+    }
+    sortedLen_ = total;
+    sortedRecords_ = records;
+  }
+  const uint8_t* sortedData() const { return sorted_.get(); }
+  uint64_t sortedLen() const { return sortedLen_; }
+  uint64_t sortedRecords() const { return sortedRecords_; }
+
+  void start(bool allowNone) {
     iter_.reset();
     info_.clear();
     blocks_.clear();
     decoded_.clear();
+    sorted_.reset();
+    sortedLen_ = sortedRecords_ = 0;
     remoteBytesRead_ = remoteBlocksFetched_ = 0;
     batches_ = 0;
-    if (d_.codecId() == B2S_CODEC_NONE)
+    if (!allowNone && d_.codecId() == B2S_CODEC_NONE)
       throw UnsupportedOperationException("spark.shuffle.compress=false is served by the stock reader path");
     auto src = computeShuffleBlockStreams(d_, shuffleId_, mapIds_, start_, end_, batch_, info_, remoteBytesRead_,
                                           remoteBlocksFetched_);
@@ -806,6 +886,8 @@ class S3ShuffleReader {
   std::unique_ptr<S3BufferedPrefetchIterator> iter_;
   std::vector<Block> blocks_;
   std::vector<std::unique_ptr<uint8_t[]>> decoded_;
+  std::unique_ptr<uint8_t[]> sorted_;  // readSorted(): the task's records in key order
+  uint64_t sortedLen_ = 0, sortedRecords_ = 0;
   uint64_t remoteBytesRead_ = 0, remoteBlocksFetched_ = 0, batches_ = 0;
   S3BufferedPrefetchIterator::Statistics stats_;
 };
@@ -959,6 +1041,15 @@ int b2sh_reader_read(b2sh_reader* r, uint32_t* n_blocks) {
   return guarded([&] {
     r->r->read();
     *n_blocks = (uint32_t)r->r->blocks().size();
+  });
+}
+int b2sh_reader_read_sorted(b2sh_reader* r, uint32_t record_bytes, uint32_t key_off, uint32_t key_len,
+                            const uint8_t** data, uint64_t* len, uint64_t* n_records) {
+  return guarded([&] {
+    r->r->readSorted(record_bytes, key_off, key_len);
+    *data = r->r->sortedData();
+    *len = r->r->sortedLen();
+    *n_records = r->r->sortedRecords();
   });
 }
 int b2sh_reader_block(b2sh_reader* r, uint32_t k, int64_t* map_id, int32_t* start_reduce, int32_t* end_reduce,
