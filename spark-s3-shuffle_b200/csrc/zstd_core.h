@@ -3,10 +3,13 @@
 // Replaces, for spark.io.compression.codec=zstd, com.github.luben.zstd.ZstdInputStreamNoFinalizer [U] (zstd-jni 1.5.5-x ->
 // libzstd ZSTD_decompressStream) under serializerManager.wrapStream at storage/S3ShuffleReader.scala:107-109.
 // The same functions are compiled by nvcc into the kernels of zstd.cu (the product) and by the host compiler into the
-// unit test tests/test_zstd_core.py, which checks them against libzstd.so.1 on frames produced by libzstd itself
-// (levels 1..3, streaming mode without content size as zstd-jni writes them, raw/RLE/compressed blocks, Huffman
-// 1- and 4-stream literals, treeless literals, predefined/RLE/FSE/repeat sequence tables, repeat offsets,
-// concatenated and skippable frames).  Nothing here is a CPU fallback: the C ABI only ever launches the device build.
+// unit tests tests/test_zstd_core.py and tests/test_zstd_levels.py, which check them against libzstd.so.1 on frames
+// produced by libzstd itself (levels -5 to 22 — every strategy — in streaming mode without content size as zstd-jni
+// writes them, with content checksum, with 2 workers, with long distance matching and a 2^27 window; raw/RLE/compressed
+// blocks, raw literals inside compressed blocks, Huffman 1- and 4-stream literals, treeless literals,
+// predefined/RLE/FSE/repeat sequence tables, all six repeat-offset forms, concatenated and skippable frames).
+// tests/test_gpu_zstd_levels.py sends the same frames through the kernels.  Nothing here is a CPU fallback: the C ABI
+// only ever launches the device build.
 //
 // Scope: frames without dictionary; window <= the decoded size the caller provides room for; Content_Checksum is
 // skipped, not verified (Spark's ZStdCompressionCodec leaves it off).

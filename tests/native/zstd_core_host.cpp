@@ -59,6 +59,64 @@ extern "C" long long zc_decode_par(const unsigned char* src, unsigned long long 
   return execute_stream(blocks.data(), (uint32_t)t.nblk, src, lit.data(), ll.data(), ml.data(), ofv.data(), dst, cap);
 }
 
+// Coverage probes: what a frame really contains, read with the same walk and entropy stages.
+// zc_frame_sequences: every sequence of every block as (literal length, match length, offset VALUE) — repeat codes stay
+// 1..3, new offsets are offset + 3.  Returns the sequence count (cap too small: the count, nothing beyond cap written)
+// or a negative error.
+extern "C" long long zc_frame_sequences(const unsigned char* src, unsigned long long n, unsigned* ll_out,
+                                        unsigned* ml_out, unsigned* ofv_out, unsigned long long cap) {
+  using namespace b2s::zstd;
+  StreamTotals t{0, 0, 0};
+  int rc = walk_stream(src, n, nullptr, 0, 0, 0, 0, 0, &t);
+  if (rc < 0) return rc;
+  std::vector<BlockInfo> blocks(t.nblk ? t.nblk : 1);
+  rc = walk_stream(src, n, blocks.data(), 0, 0, 0, 0, 0, &t);
+  if (rc < 0) return rc;
+  std::vector<unsigned char> lit(t.lit + 64);
+  std::vector<uint32_t> ll(t.nseq + 1), ml(t.nseq + 1), ofv(t.nseq + 1);
+  Workspace* w = (Workspace*)malloc(sizeof(Workspace));
+  w->lit = nullptr;
+  for (uint32_t b = 0; b < t.nblk; b++) {
+    const long long r = entropy_block(w, blocks.data(), b, src, lit.data(), ll.data(), ml.data(), ofv.data(), false);
+    if (r < 0) {
+      free(w);
+      return r;
+    }
+  }
+  free(w);
+  for (uint64_t i = 0; i < t.nseq && i < cap; i++) {
+    ll_out[i] = ll[i];
+    ml_out[i] = ml[i];
+    ofv_out[i] = ofv[i];
+  }
+  return (long long)t.nseq;
+}
+
+// zc_frame_blocks: six ints per block — block type (0 raw, 1 RLE, 2 compressed), literals type (0 raw, 1 RLE,
+// 2 Huffman, 3 treeless), Huffman stream count (1 / 4), the Symbol_Compression_Modes byte, the Huffman weights' form
+// (1 FSE-compressed, 0 direct, -1 no tree in this block) and the sequence count.  Returns the block count (at most cap
+// blocks written) or a negative error.
+extern "C" long long zc_frame_blocks(const unsigned char* src, unsigned long long n, int* out, unsigned long long cap) {
+  using namespace b2s::zstd;
+  StreamTotals t{0, 0, 0};
+  int rc = walk_stream(src, n, nullptr, 0, 0, 0, 0, 0, &t);
+  if (rc < 0) return rc;
+  std::vector<BlockInfo> blocks(t.nblk ? t.nblk : 1);
+  rc = walk_stream(src, n, blocks.data(), 0, 0, 0, 0, 0, &t);
+  if (rc < 0) return rc;
+  for (uint64_t k = 0; k < t.nblk && k < cap; k++) {
+    const BlockInfo& b = blocks[k];
+    int* o = out + 6 * k;
+    o[0] = b.type;
+    o[1] = b.type == 2 ? b.ltype : -1;
+    o[2] = b.type == 2 ? b.lstreams : 0;
+    o[3] = b.modes;
+    o[4] = (b.type == 2 && b.ltype == 2) ? (src[b.src + b.lit_hdr] < 128 ? 1 : 0) : -1;  // Huffman header byte
+    o[5] = (int)b.nseq;
+  }
+  return (long long)t.nblk;
+}
+
 // ------------------------------------------------------------------------------------------------------------------
 // CPU model of the GPU Zstandard ENCODER (zstd_enc.cu): the shared window match finder + greedy parse (the same
 // specification as orc_lz4_compress_block_win in oracle/), then the encoder core of zstd_enc_core.h.

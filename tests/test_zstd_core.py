@@ -1,5 +1,7 @@
 """The Zstandard decoder core (spark-s3-shuffle_b200/csrc/zstd_core.h — the functions the CUDA kernels call) compiled
-for the host and pinned on libzstd.so.1: frames produced by the real library, in the shapes zstd-jni writes them."""
+for the host and pinned on libzstd.so.1: frames produced by the real library at levels 1..3, in the shapes zstd-jni
+writes them, plus the encoder model.  Levels -5 to 22, frame options, long distance matching and every repeat-offset
+form are pinned in tests/test_zstd_levels.py."""
 import ctypes as C
 import os
 import subprocess
