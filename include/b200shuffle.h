@@ -58,6 +58,7 @@ extern "C" {
 #define B2S_E_CUDA (-6)          /* no device / CUDA failure; b2s_last_error() has the text                  */
 #define B2S_E_NOT_INIT (-7)
 #define B2S_E_NOMEM (-8)
+#define B2S_E_NOT_CACHED (-9) /* an exchange-cache source is not resident (evicted, removed, other device): fetch it */
 
 /* ---- lifecycle: call once per executor, beside S3ShuffleDataIO.initializeExecutor (shuffle/S3ShuffleDataIO.scala:30-32) ---- */
 /* gpu_mask: bit i selects CUDA device i (0 = all visible devices).  The per-stream-pointer calls (b2s_*_batch) shard
@@ -205,6 +206,70 @@ int b2s_decompress_sort_dev(uint32_t dev_index, uint32_t codec, uint32_t checksu
                             uint32_t record_bytes, uint32_t key_off, uint32_t key_len, uint8_t* dst_base,
                             uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records, int32_t* status,
                             int32_t* bad_slice);
+
+/* ---- exchange cache: map outputs kept resident in HBM for reducers on the same device ----
+ * (docs/f4_gpu_resident_exchange.md steps 2 and 3, local half.)  The serialized writer's partition step already leaves
+ * a map task's records partitioned by reduce id in HBM; the cached store keeps that arena, keyed by (shuffle_id,
+ * map_id), on the calling thread's device, and a reducer on the same device reads its partitions of it with one gather
+ * instead of fetching, verifying and decoding the .data ranges.  The object store stays the source of truth: an entry is
+ * never the only copy, and a miss is served by the usual fetch.  An entry on another device of the process is a miss.
+ *
+ * Budget: per device, in bytes of cached records; 0 (the default) turns the cache off.  Stores evict least recently used
+ * entries that no read is using until the new entry fits; a read counts as a use.  Lowering a budget evicts down to it.
+ * Device memory: when one of the library's own workspaces cannot grow, unreferenced entries of that device are evicted
+ * and the allocation is retried once, so a generous budget does not make another call fail with B2S_E_NOMEM.
+ * Concurrency: every read references the entries it uses from its lookup until its stream has synchronised; eviction
+ * and removal unlink an entry at once and free its memory when its last reader is done.
+ * Without a usable device every call returns B2S_E_CUDA; before b2s_init, B2S_E_NOT_INIT. */
+int b2s_exchange_set_budget(uint32_t dev_index, uint64_t bytes);
+/* b2s_partition_compress_packed, byte for byte (outputs, status and return value), that also keeps the partitioned
+ * records and their partition offsets as the entry (shuffle_id, map_id), replacing an existing entry of that key.  The
+ * records are copied device to device into an exact-size allocation.  *cached = 1 when the entry was stored, 0 when it
+ * does not fit (the budget is 0 or below its size, or the rest of the cache is in use) or the call did not succeed. */
+int b2s_partition_compress_cached_packed(int32_t shuffle_id, int64_t map_id, uint32_t codec, int32_t level,
+                                         uint32_t codec_block_size, uint32_t checksum_alg, uint32_t num_partitions,
+                                         uint64_t n_records, const uint8_t* rec_base, uint64_t rec_bytes,
+                                         const uint32_t* rec_len, const uint32_t* rec_part, uint8_t* dst_base,
+                                         uint64_t dst_cap, uint64_t* dst_off, uint64_t* dst_len, uint64_t* dst_total,
+                                         uint64_t* checksum_out, int32_t* status, int32_t* cached);
+/* len[i] = bytes of partitions [start_reduce, end_reduce) of map_ids[i] when that map output is resident on the calling
+ * thread's device, UINT64_MAX otherwise.  Returns the number of hits.  Nothing is referenced: a later read can still
+ * find an entry gone.  start_reduce < 0, end_reduce < start_reduce, NULL arrays, or a resident entry with fewer than
+ * end_reduce partitions -> B2S_E_ARG. */
+int b2s_exchange_lookup(int32_t shuffle_id, int32_t start_reduce, int32_t end_reduce, uint32_t n_maps,
+                        const int64_t* map_ids, uint64_t* len);
+/* the partitions [start_reduce, end_reduce) of each map output, back to back in map_ids order, copied to host memory:
+ * dst_off[i] / dst_len[i], status[i] = B2S_OK or B2S_E_NOT_CACHED (dst_len 0).  For shuffles without a key ordering.
+ * dst_cap below the bytes -> B2S_E_DST_TOO_SMALL with *dst_total = the bytes needed.  Runs on the read lane. */
+int b2s_exchange_read_packed(int32_t shuffle_id, int32_t start_reduce, int32_t end_reduce, uint32_t n_maps,
+                             const int64_t* map_ids, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_off,
+                             uint64_t* dst_len, uint64_t* dst_total, int32_t* status);
+/* b2s_decompress_sort_packed over n sources of which some are served from the cache.  Source i is the cached range
+ * [start_reduce, end_reduce) of map_ids[i] when cached[i] != 0 (its src_off / src_len and slices are ignored; its slice
+ * range may be empty), fetched block i otherwise.  The contract is decompress_sort's with source order as block order:
+ * the sort is stable, fetched blocks are verified and decoded as there, and when any source fails nothing is sorted,
+ * *n_records = 0 and the call returns 0.  A cached source that is not resident sets status[i] = B2S_E_NOT_CACHED; one
+ * that is not a whole number of records, B2S_E_CORRUPT.  Cached sources are not checksum-verified (they never left the
+ * device).  Decoded blocks are written straight to their place among the cached ranges; one gather moves the cached
+ * ranges.  kernel_ms covers gather, verification, decode and sort; top_kernel_ms the sort. */
+int b2s_exchange_read_sort_packed(int32_t shuffle_id, int32_t start_reduce, int32_t end_reduce, const int64_t* map_ids,
+                                  const uint8_t* cached, uint32_t codec, uint32_t checksum_alg, uint32_t n,
+                                  const uint8_t* src_base, const uint64_t* src_off, const uint64_t* src_len,
+                                  const uint32_t* slice_base, const uint64_t* slice_len,
+                                  const uint64_t* slice_checksum, uint32_t record_bytes, uint32_t key_off,
+                                  uint32_t key_len, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_total,
+                                  uint64_t* n_records, int32_t* status, int32_t* bad_slice);
+/* same, with src_base / dst_base in device memory of dev_index (and the cache entries of that device) */
+int b2s_exchange_read_sort_dev(uint32_t dev_index, int32_t shuffle_id, int32_t start_reduce, int32_t end_reduce,
+                               const int64_t* map_ids, const uint8_t* cached, uint32_t codec, uint32_t checksum_alg,
+                               uint32_t n, const uint8_t* src_base, const uint64_t* src_off, const uint64_t* src_len,
+                               const uint32_t* slice_base, const uint64_t* slice_len, const uint64_t* slice_checksum,
+                               uint32_t record_bytes, uint32_t key_off, uint32_t key_len, uint8_t* dst_base,
+                               uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records, int32_t* status,
+                               int32_t* bad_slice);
+/* removes the entry (shuffle_id, map_id) — map_id -1: every map output of the shuffle — on every device (the hook for
+ * removeShuffle).  Returns the number of entries removed. */
+int b2s_exchange_remove(int32_t shuffle_id, int64_t map_id);
 
 /* ---- device-resident variants (data pointers are device memory on device `dev_index` of the b2s_init selection;
  *      descriptor arrays are host memory).  Synchronous; timings retrievable with b2s_last_timing. ---- */

@@ -45,7 +45,10 @@ const char* b2sh_last_error(void);
 
 /* ---- dispatcher: conf is "key=value\n" lines using the reference's keys (spark.shuffle.s3.rootDir, .bufferSize,
  * .folderPrefixes, .alwaysCreateIndex, .cleanup, spark.shuffle.checksum.enabled/.algorithm, spark.io.compression.codec,
- * spark.io.compression.lz4.blockSize, spark.app.id) plus the additive spark.shuffle.s3.gpu.enabled (default true). ---- */
+ * spark.io.compression.lz4.blockSize, spark.app.id) plus the additive spark.shuffle.s3.gpu.enabled (default true) and
+ * spark.shuffle.s3.gpu.exchangeCacheBytes (default 0 = off; INTEGRATION.md §3f): the per-device budget of the exchange
+ * cache, which keeps the serialized writer's partitioned map outputs in HBM for reducers on the same device.
+ * remove_shuffle also removes the shuffle's cached map outputs. ---- */
 typedef struct b2sh_dispatcher b2sh_dispatcher;
 int b2sh_dispatcher_create(const char* conf, b2sh_dispatcher** out);
 void b2sh_dispatcher_destroy(b2sh_dispatcher* d);
@@ -102,7 +105,8 @@ void b2sh_writer_destroy(b2sh_writer* w);
  * b2s_partition_compress_packed call and writes .data/.index/.checksum like b2sh_writer_commit_all_partitions — the
  * files are byte-identical to that writer's when it is fed the same records partition by partition, every partition
  * opened in ascending order.  partition_lengths_out receives num_partitions values.  Needs
- * spark.shuffle.s3.gpu.enabled; codec "none" partitions and checksums only. ---- */
+ * spark.shuffle.s3.gpu.enabled; codec "none" partitions and checksums only.  With the exchange cache on the call is
+ * b2s_partition_compress_cached_packed: the same files, and the partitioned records stay in HBM. ---- */
 typedef struct b2sh_serialized_writer b2sh_serialized_writer;
 int b2sh_serialized_writer_create(b2sh_dispatcher* d, int32_t shuffle_id, int64_t map_id, int32_t num_partitions,
                                   b2sh_serialized_writer** out);
@@ -126,7 +130,9 @@ int b2sh_reader_create(b2sh_dispatcher* d, int32_t shuffle_id, const int64_t* ma
 /* read(): resolves block ranges from .index, drops empty blocks, fetches the remaining ones, verifies every
  * partition slice against .checksum and decompresses — all blocks of the task in one C-ABI batch.  Afterwards
  * block k's decoded stream is at data + off[k].  A checksum mismatch returns B2SH_E_SPARK with the reference's message,
- * a malformed stream B2SH_E_IO. */
+ * a malformed stream B2SH_E_IO.  With the exchange cache on, the maps resident on the calling thread's device are read
+ * from it first (one block per map covering [start_partition, end_partition)); only the others are fetched, and only
+ * their bytes count in remote_bytes_read. */
 int b2sh_reader_read(b2sh_reader* r, uint32_t* n_blocks);
 /* read_sorted(): read() for a shuffle with a key ordering, no aggregator and fixed-size records (INTEGRATION.md §3e,
  * spark.shuffle.s3.gpu.sortKey).  Resolves and fetches the task's non-empty blocks as read() does, then makes ONE
@@ -134,7 +140,9 @@ int b2sh_reader_read(b2sh_reader* r, uint32_t* n_blocks);
  * bytes [key_off, key_off + key_len) of each record_bytes-long record (stable: equal keys in map, then reduce-id
  * order).  The buffer stays valid until the reader's next read or its destruction.  A checksum mismatch returns
  * B2SH_E_SPARK with the reference's message, a malformed stream (or one that does not hold whole records) B2SH_E_IO.
- * Codec "none" is verified and sorted only. */
+ * Codec "none" is verified and sorted only.  With the exchange cache on, a map resident on the calling thread's device
+ * is one cached source in that order (b2s_exchange_read_sort_packed) instead of its fetched blocks; maps evicted before
+ * the call are fetched and the call is repeated. */
 int b2sh_reader_read_sorted(b2sh_reader* r, uint32_t record_bytes, uint32_t key_off, uint32_t key_len,
                             const uint8_t** data, uint64_t* len, uint64_t* n_records);
 int b2sh_reader_block(b2sh_reader* r, uint32_t k, int64_t* map_id, int32_t* start_reduce, int32_t* end_reduce,

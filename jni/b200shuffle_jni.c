@@ -131,13 +131,12 @@ JNIEXPORT jint JNICALL J(compressPacked)(JNIEnv* e, jclass c, jint codec, jint l
  *      meta: long[1] = {dst_total}.  The per-partition results are collected in native memory during the blocking
  *      call and copied out with Set<Type>ArrayRegion afterwards: no Java array is held in a critical region while the
  *      GPU works. ---- */
-JNIEXPORT jint JNICALL J(partitionCompressPacked)(JNIEnv* e, jclass c, jint codec, jint level, jint blockSize, jint alg,
-                                                  jint numPartitions, jlong nRecords, jlong records, jlong recBytes,
-                                                  jlong recLen, jlong recPart, jlong dst, jlong dstCap,
-                                                  jlongArray dstOff, jlongArray dstLen, jlongArray meta,
-                                                  jlongArray checksums, jintArray status) {
-  (void)c;
-  if (numPartitions < 1 || !dstOff || !dstLen || !meta || !status || (*e)->GetArrayLength(e, dstOff) < numPartitions ||
+/* cached (may be NULL): int[1], the cached store's flag; then (shuffleId, mapId) keys the exchange-cache entry */
+static jint partition_compress(JNIEnv* e, jint shuffleId, jlong mapId, jintArray cached, jint codec, jint level,
+                               jint blockSize, jint alg, jint numPartitions, jlong nRecords, jlong records,
+                               jlong recBytes, jlong recLen, jlong recPart, jlong dst, jlong dstCap, jlongArray dstOff,
+                               jlongArray dstLen, jlongArray meta, jlongArray checksums, jintArray status) {
+  if ((cached && (*e)->GetArrayLength(e, cached) < 1) || numPartitions < 1 || !dstOff || !dstLen || !meta || !status || (*e)->GetArrayLength(e, dstOff) < numPartitions ||
       (*e)->GetArrayLength(e, dstLen) < numPartitions || (*e)->GetArrayLength(e, status) < numPartitions ||
       (*e)->GetArrayLength(e, meta) < 1 || (checksums && (*e)->GetArrayLength(e, checksums) < numPartitions))
     return B2S_E_ARG;
@@ -150,10 +149,19 @@ JNIEXPORT jint JNICALL J(partitionCompressPacked)(JNIEnv* e, jclass c, jint code
     return B2S_E_NOMEM;
   }
   uint64_t total = 0;
-  const int rc = b2s_partition_compress_packed(
-      (uint32_t)codec, (int32_t)level, (uint32_t)blockSize, (uint32_t)alg, (uint32_t)numPartitions, (uint64_t)nRecords,
-      PTR(const uint8_t, records), (uint64_t)recBytes, PTR(const uint32_t, recLen), PTR(const uint32_t, recPart),
-      PTR(uint8_t, dst), (uint64_t)dstCap, buf, buf + R, &total, buf + 2 * R, st);
+  int32_t stored = 0;
+  const int rc =
+      cached ? b2s_partition_compress_cached_packed(
+                   (int32_t)shuffleId, (int64_t)mapId, (uint32_t)codec, (int32_t)level, (uint32_t)blockSize,
+                   (uint32_t)alg, (uint32_t)numPartitions, (uint64_t)nRecords, PTR(const uint8_t, records),
+                   (uint64_t)recBytes, PTR(const uint32_t, recLen), PTR(const uint32_t, recPart), PTR(uint8_t, dst),
+                   (uint64_t)dstCap, buf, buf + R, &total, buf + 2 * R, st, &stored)
+             : b2s_partition_compress_packed(
+                   (uint32_t)codec, (int32_t)level, (uint32_t)blockSize, (uint32_t)alg, (uint32_t)numPartitions,
+                   (uint64_t)nRecords, PTR(const uint8_t, records), (uint64_t)recBytes, PTR(const uint32_t, recLen),
+                   PTR(const uint32_t, recPart), PTR(uint8_t, dst), (uint64_t)dstCap, buf, buf + R, &total,
+                   buf + 2 * R, st);
+  if (cached) (*e)->SetIntArrayRegion(e, cached, 0, 1, (const jint*)&stored);
   if (rc == 0 || rc == B2S_E_DST_TOO_SMALL) {
     (*e)->SetLongArrayRegion(e, dstOff, 0, numPartitions, (const jlong*)buf);
     (*e)->SetLongArrayRegion(e, dstLen, 0, numPartitions, (const jlong*)(buf + R));
@@ -165,6 +173,27 @@ JNIEXPORT jint JNICALL J(partitionCompressPacked)(JNIEnv* e, jclass c, jint code
   free(st);
   free(buf);
   return rc;
+}
+JNIEXPORT jint JNICALL J(partitionCompressPacked)(JNIEnv* e, jclass c, jint codec, jint level, jint blockSize, jint alg,
+                                                  jint numPartitions, jlong nRecords, jlong records, jlong recBytes,
+                                                  jlong recLen, jlong recPart, jlong dst, jlong dstCap,
+                                                  jlongArray dstOff, jlongArray dstLen, jlongArray meta,
+                                                  jlongArray checksums, jintArray status) {
+  (void)c;
+  return partition_compress(e, 0, 0, 0, codec, level, blockSize, alg, numPartitions, nRecords, records, recBytes, recLen,
+                            recPart, dst, dstCap, dstOff, dstLen, meta, checksums, status);
+}
+/* the same, keeping the partitioned records in the exchange cache as (shuffleId, mapId); cached: int[1] = stored */
+JNIEXPORT jint JNICALL J(partitionCompressCachedPacked)(JNIEnv* e, jclass c, jint shuffleId, jlong mapId, jint codec,
+                                                        jint level, jint blockSize, jint alg, jint numPartitions,
+                                                        jlong nRecords, jlong records, jlong recBytes, jlong recLen,
+                                                        jlong recPart, jlong dst, jlong dstCap, jlongArray dstOff,
+                                                        jlongArray dstLen, jlongArray meta, jlongArray checksums,
+                                                        jintArray status, jintArray cached) {
+  (void)c;
+  if (!cached) return B2S_E_ARG;
+  return partition_compress(e, shuffleId, mapId, cached, codec, level, blockSize, alg, numPartitions, nRecords, records,
+                            recBytes, recLen, recPart, dst, dstCap, dstOff, dstLen, meta, checksums, status);
 }
 
 /* ---- read side: n prefetched blocks; block i owns slices [sliceBase[i], sliceBase[i+1]) of sliceLen/sliceChecksum
@@ -206,13 +235,16 @@ JNIEXPORT jint JNICALL J(decompressPacked)(JNIEnv* e, jclass c, jint codec, jint
  *      long[n], sliceBase: int[n+1], sliceLen/sliceChecksum: long[slices] (inputs, copied in with Get<Type>ArrayRegion);
  *      meta: long[2] = {dst_total, n_records}; status, badSlice: int[n].  All arrays go through native copies, so no
  *      Java array is held in a critical region while the GPU works. ---- */
-JNIEXPORT jint JNICALL J(decompressSortPacked)(JNIEnv* e, jclass c, jint codec, jint alg, jint n, jlong src,
-                                               jlongArray off, jlongArray len, jintArray sliceBase, jlongArray sliceLen,
-                                               jlongArray sliceChecksum, jint recordBytes, jint keyOff, jint keyLen,
-                                               jlong dst, jlong dstCap, jlongArray meta, jintArray status,
-                                               jintArray badSlice) {
-  (void)c;
+/* mapIds (NULL: a plain decompressSortPacked): long[n] and cached: int[n] make it an exchange-cache read of the
+ * partitions [startReduce, endReduce) of shuffleId */
+static jint sort_packed(JNIEnv* e, jint shuffleId, jint startReduce, jint endReduce, jlongArray mapIds,
+                        jintArray cached, jint codec, jint alg, jint n, jlong src, jlongArray off, jlongArray len,
+                        jintArray sliceBase, jlongArray sliceLen, jlongArray sliceChecksum, jint recordBytes,
+                        jint keyOff, jint keyLen, jlong dst, jlong dstCap, jlongArray meta, jintArray status,
+                        jintArray badSlice) {
   if (n < 0 || !meta || (*e)->GetArrayLength(e, meta) < 2) return B2S_E_ARG;
+  if (mapIds && n > 0 && (!cached || (*e)->GetArrayLength(e, mapIds) < n || (*e)->GetArrayLength(e, cached) < n))
+    return B2S_E_ARG;
   if (n > 0 && (!off || !len || !status || (*e)->GetArrayLength(e, off) < n || (*e)->GetArrayLength(e, len) < n ||
                 (*e)->GetArrayLength(e, status) < n || (badSlice && (*e)->GetArrayLength(e, badSlice) < n)))
     return B2S_E_ARG;
@@ -223,11 +255,18 @@ JNIEXPORT jint JNICALL J(decompressSortPacked)(JNIEnv* e, jclass c, jint codec, 
   uint64_t* blk = (uint64_t*)malloc((N * 2 + 1) * sizeof(uint64_t));
   int32_t* st = (int32_t*)malloc((N * 2 + 1) * sizeof(int32_t));
   uint32_t* sb = (uint32_t*)malloc((N + 1) * sizeof(uint32_t));
+  int64_t* ids = (int64_t*)malloc((N + 1) * sizeof(int64_t));
+  uint8_t* hit = (uint8_t*)malloc(N + 1);
   uint64_t* sl = 0;
-  int rc = blk && st && sb ? 0 : B2S_E_NOMEM;
+  int rc = blk && st && sb && ids && hit ? 0 : B2S_E_NOMEM;
   if (rc == 0 && n > 0) {
     (*e)->GetLongArrayRegion(e, off, 0, n, (jlong*)blk);
     (*e)->GetLongArrayRegion(e, len, 0, n, (jlong*)(blk + N));
+    if (mapIds) {
+      (*e)->GetLongArrayRegion(e, mapIds, 0, n, (jlong*)ids);
+      (*e)->GetIntArrayRegion(e, cached, 0, n, (jint*)st); /* st is scratch until the call */
+      for (size_t i = 0; i < N; i++) hit[i] = st[i] != 0;
+    }
   }
   if (rc == 0 && with_slices) {
     (*e)->GetIntArrayRegion(e, sliceBase, 0, n + 1, (jint*)sb);
@@ -244,10 +283,18 @@ JNIEXPORT jint JNICALL J(decompressSortPacked)(JNIEnv* e, jclass c, jint codec, 
   uint64_t total = 0, nrec = 0;
   if (rc == 0) {
     const size_t ns = with_slices ? (size_t)sb[n] : 0;
-    rc = b2s_decompress_sort_packed((uint32_t)codec, (uint32_t)alg, (uint32_t)n, PTR(const uint8_t, src), blk,
-                                    blk + N, with_slices ? sb : 0, with_slices ? sl : 0, with_slices ? sl + ns : 0,
-                                    (uint32_t)recordBytes, (uint32_t)keyOff, (uint32_t)keyLen, PTR(uint8_t, dst),
-                                    (uint64_t)dstCap, &total, &nrec, st, st + N);
+    if (mapIds)
+      rc = b2s_exchange_read_sort_packed((int32_t)shuffleId, (int32_t)startReduce, (int32_t)endReduce, ids, hit,
+                                         (uint32_t)codec, (uint32_t)alg, (uint32_t)n, PTR(const uint8_t, src), blk,
+                                         blk + N, with_slices ? sb : 0, with_slices ? sl : 0,
+                                         with_slices ? sl + ns : 0, (uint32_t)recordBytes, (uint32_t)keyOff,
+                                         (uint32_t)keyLen, PTR(uint8_t, dst), (uint64_t)dstCap, &total, &nrec, st,
+                                         st + N);
+    else
+      rc = b2s_decompress_sort_packed((uint32_t)codec, (uint32_t)alg, (uint32_t)n, PTR(const uint8_t, src), blk,
+                                      blk + N, with_slices ? sb : 0, with_slices ? sl : 0, with_slices ? sl + ns : 0,
+                                      (uint32_t)recordBytes, (uint32_t)keyOff, (uint32_t)keyLen, PTR(uint8_t, dst),
+                                      (uint64_t)dstCap, &total, &nrec, st, st + N);
     if ((rc == 0 || rc == B2S_E_DST_TOO_SMALL) && n > 0) {
       (*e)->SetIntArrayRegion(e, status, 0, n, (const jint*)st);
       if (badSlice) (*e)->SetIntArrayRegion(e, badSlice, 0, n, (const jint*)(st + N));
@@ -255,11 +302,96 @@ JNIEXPORT jint JNICALL J(decompressSortPacked)(JNIEnv* e, jclass c, jint codec, 
     const jlong m[2] = {(jlong)total, (jlong)nrec};
     (*e)->SetLongArrayRegion(e, meta, 0, 2, m);
   }
+  free(hit);
+  free(ids);
   free(sl);
   free(sb);
   free(st);
   free(blk);
   return rc;
+}
+JNIEXPORT jint JNICALL J(decompressSortPacked)(JNIEnv* e, jclass c, jint codec, jint alg, jint n, jlong src,
+                                               jlongArray off, jlongArray len, jintArray sliceBase, jlongArray sliceLen,
+                                               jlongArray sliceChecksum, jint recordBytes, jint keyOff, jint keyLen,
+                                               jlong dst, jlong dstCap, jlongArray meta, jintArray status,
+                                               jintArray badSlice) {
+  (void)c;
+  return sort_packed(e, 0, 0, 0, 0, 0, codec, alg, n, src, off, len, sliceBase, sliceLen, sliceChecksum, recordBytes,
+                     keyOff, keyLen, dst, dstCap, meta, status, badSlice);
+}
+
+/* ---- exchange cache (INTEGRATION.md §3f): map outputs kept in HBM for reducers on the same device ---- */
+JNIEXPORT jint JNICALL J(exchangeSetBudget)(JNIEnv* e, jclass c, jint dev, jlong bytes) {
+  (void)e; (void)c;
+  return b2s_exchange_set_budget((uint32_t)dev, (uint64_t)bytes);
+}
+JNIEXPORT jint JNICALL J(exchangeRemove)(JNIEnv* e, jclass c, jint shuffleId, jlong mapId) {
+  (void)e; (void)c;
+  return b2s_exchange_remove((int32_t)shuffleId, (int64_t)mapId);
+}
+/* len: long[n] = bytes of [startReduce, endReduce) of each resident map, -1 (UINT64_MAX) otherwise; returns the hits */
+JNIEXPORT jint JNICALL J(exchangeLookup)(JNIEnv* e, jclass c, jint shuffleId, jint startReduce, jint endReduce, jint n,
+                                         jlongArray mapIds, jlongArray len) {
+  (void)c;
+  if (n < 0 || (n > 0 && (!mapIds || !len || (*e)->GetArrayLength(e, mapIds) < n || (*e)->GetArrayLength(e, len) < n)))
+    return B2S_E_ARG;
+  const size_t N = (size_t)n;
+  uint64_t* buf = (uint64_t*)malloc((N * 2 + 1) * sizeof(uint64_t));
+  if (!buf) return B2S_E_NOMEM;
+  if (n > 0) (*e)->GetLongArrayRegion(e, mapIds, 0, n, (jlong*)buf);
+  const int rc = b2s_exchange_lookup((int32_t)shuffleId, (int32_t)startReduce, (int32_t)endReduce, (uint32_t)n,
+                                     (const int64_t*)buf, buf + N);
+  if (rc >= 0 && n > 0) (*e)->SetLongArrayRegion(e, len, 0, n, (const jlong*)(buf + N));
+  free(buf);
+  return rc;
+}
+/* the cached ranges back to back into dst (a direct buffer address); dstOff/dstLen: long[n], status: int[n],
+ * meta: long[1] = {dst_total} */
+JNIEXPORT jint JNICALL J(exchangeReadPacked)(JNIEnv* e, jclass c, jint shuffleId, jint startReduce, jint endReduce,
+                                             jint n, jlongArray mapIds, jlong dst, jlong dstCap, jlongArray dstOff,
+                                             jlongArray dstLen, jlongArray meta, jintArray status) {
+  (void)c;
+  if (n < 0 || !meta || (*e)->GetArrayLength(e, meta) < 1) return B2S_E_ARG;
+  if (n > 0 && (!mapIds || !dstOff || !dstLen || !status || (*e)->GetArrayLength(e, mapIds) < n ||
+                (*e)->GetArrayLength(e, dstOff) < n || (*e)->GetArrayLength(e, dstLen) < n ||
+                (*e)->GetArrayLength(e, status) < n))
+    return B2S_E_ARG;
+  const size_t N = (size_t)n;
+  uint64_t* buf = (uint64_t*)malloc((N * 3 + 1) * sizeof(uint64_t));
+  int32_t* st = (int32_t*)malloc((N + 1) * sizeof(int32_t));
+  if (!buf || !st) {
+    free(buf);
+    free(st);
+    return B2S_E_NOMEM;
+  }
+  if (n > 0) (*e)->GetLongArrayRegion(e, mapIds, 0, n, (jlong*)buf);
+  uint64_t total = 0;
+  const int rc = b2s_exchange_read_packed((int32_t)shuffleId, (int32_t)startReduce, (int32_t)endReduce, (uint32_t)n,
+                                          (const int64_t*)buf, PTR(uint8_t, dst), (uint64_t)dstCap, buf + N,
+                                          buf + 2 * N, &total, st);
+  if (rc == 0 && n > 0) {
+    (*e)->SetLongArrayRegion(e, dstOff, 0, n, (const jlong*)(buf + N));
+    (*e)->SetLongArrayRegion(e, dstLen, 0, n, (const jlong*)(buf + 2 * N));
+    (*e)->SetIntArrayRegion(e, status, 0, n, (const jint*)st);
+  }
+  const jlong m = (jlong)total;
+  (*e)->SetLongArrayRegion(e, meta, 0, 1, &m);
+  free(st);
+  free(buf);
+  return rc;
+}
+/* decompressSortPacked over sources of which those with cached[i] != 0 are the cached range of mapIds[i]
+ * (mapIds: long[n], cached: int[n]); the other arguments as decompressSortPacked */
+JNIEXPORT jint JNICALL J(exchangeReadSortPacked)(JNIEnv* e, jclass c, jint shuffleId, jint startReduce, jint endReduce,
+                                                 jlongArray mapIds, jintArray cached, jint codec, jint alg, jint n,
+                                                 jlong src, jlongArray off, jlongArray len, jintArray sliceBase,
+                                                 jlongArray sliceLen, jlongArray sliceChecksum, jint recordBytes,
+                                                 jint keyOff, jint keyLen, jlong dst, jlong dstCap, jlongArray meta,
+                                                 jintArray status, jintArray badSlice) {
+  (void)c;
+  if (!mapIds) return B2S_E_ARG;
+  return sort_packed(e, shuffleId, startReduce, endReduce, mapIds, cached, codec, alg, n, src, off, len, sliceBase,
+                     sliceLen, sliceChecksum, recordBytes, keyOff, keyLen, dst, dstCap, meta, status, badSlice);
 }
 
 /* decoded size of each of n compressed streams laid out in one arena (sizes the destination of decompressPacked) */

@@ -12,8 +12,9 @@ from . import _build
 # ---- constants mirrored from b200shuffle.h ----
 CODEC_NONE, CODEC_LZ4BLOCK, CODEC_SNAPPY_XERIAL, CODEC_ZSTD = 0, 1, 2, 3
 CHECKSUM_NONE, CHECKSUM_ADLER32, CHECKSUM_CRC32, CHECKSUM_CRC32C = 0, 1, 2, 3
-OK, E_CORRUPT, E_CHECKSUM, E_DST_TOO_SMALL, E_UNSUPPORTED, E_ARG, E_CUDA, E_NOT_INIT, E_NOMEM = (
-    0, -1, -2, -3, -4, -5, -6, -7, -8)
+OK, E_CORRUPT, E_CHECKSUM, E_DST_TOO_SMALL, E_UNSUPPORTED, E_ARG, E_CUDA, E_NOT_INIT, E_NOMEM, E_NOT_CACHED = (
+    0, -1, -2, -3, -4, -5, -6, -7, -8, -9)
+NOT_RESIDENT = 2**64 - 1  # b2s_exchange_lookup's length of a map output that is not resident
 CODEC_BY_NAME = {"lz4": CODEC_LZ4BLOCK, "snappy": CODEC_SNAPPY_XERIAL, "zstd": CODEC_ZSTD}
 CHECKSUM_BY_NAME = {"ADLER32": CHECKSUM_ADLER32, "CRC32": CHECKSUM_CRC32, "CRC32C": CHECKSUM_CRC32C}
 
@@ -69,6 +70,19 @@ PROTOTYPES = [
     ("b2s_decompress_sort_dev", C.c_int,
      [_u32, _u32, _u32, _u32, _vp, _u64p, _u64p, _u32p, _u64p, _u64p, _u32, _u32, _u32, _vp, _u64, _u64p, _u64p, _i32p,
       _i32p]),
+    ("b2s_exchange_set_budget", C.c_int, [_u32, _u64]),
+    ("b2s_partition_compress_cached_packed", C.c_int,
+     [_i32, C.c_int64, _u32, _i32, _u32, _u32, _u32, _u64, _u8p, _u64, _u32p, _u32p, _u8p, _u64, _u64p, _u64p, _u64p,
+      _u64p, _i32p, _i32p]),
+    ("b2s_exchange_lookup", C.c_int, [_i32, _i32, _i32, _u32, _vp, _u64p]),
+    ("b2s_exchange_read_packed", C.c_int, [_i32, _i32, _i32, _u32, _vp, _u8p, _u64, _u64p, _u64p, _u64p, _i32p]),
+    ("b2s_exchange_read_sort_packed", C.c_int,
+     [_i32, _i32, _i32, _vp, _vp, _u32, _u32, _u32, _u8p, _u64p, _u64p, _u32p, _u64p, _u64p, _u32, _u32, _u32, _u8p,
+      _u64, _u64p, _u64p, _i32p, _i32p]),
+    ("b2s_exchange_read_sort_dev", C.c_int,
+     [_u32, _i32, _i32, _i32, _vp, _vp, _u32, _u32, _u32, _vp, _u64p, _u64p, _u32p, _u64p, _u64p, _u32, _u32, _u32,
+      _vp, _u64, _u64p, _u64p, _i32p, _i32p]),
+    ("b2s_exchange_remove", C.c_int, [_i32, C.c_int64]),
     ("b2s_checksum_dev", C.c_int, [_u32, _u32, _u32, _vp, _u64p, _u64p, _u64p]),
     ("b2s_compress_dev", C.c_int,
      [_u32, _u32, _i32, _u32, _u32, _u32, _vp, _u64p, _u64p, _vp, _u64, _u64p, _u64p, _u64p, _u64p, _i32p]),
@@ -459,3 +473,107 @@ def partition_compress_dev(codec, d_records, rec_bytes, d_rec_len, d_rec_part, n
                                              _ptr(dst_off), _ptr(dst_len), C.addressof(total), _ptr(cks), _ptr(st)),
            "b2s_partition_compress_dev")
     return dict(dst_off=dst_off, dst_len=dst_len, total=total.value, checksums=cks, status=st)
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# exchange cache: map outputs kept resident in HBM for reducers on the same device
+# ---------------------------------------------------------------------------------------------------------------
+def exchange_set_budget(nbytes, dev=0):
+    """per-device budget in bytes of cached records; 0 (the default) turns the cache off"""
+    _check(load().b2s_exchange_set_budget(dev, nbytes), "b2s_exchange_set_budget")
+
+
+def partition_compress_cached_packed(shuffle_id, map_id, codec, records, rec_len, rec_part, num_partitions, dst,
+                                     block_size=0, checksum_alg=CHECKSUM_NONE, level=0):
+    """partition_compress_packed that also keeps the partitioned records as the cache entry (shuffle_id, map_id).
+    -> dict(dst_off, dst_len, total, checksums, status, cached)"""
+    records, dst = _as_u8(records), _as_u8(dst)
+    rec_len = np.ascontiguousarray(rec_len, dtype=np.uint32)
+    rec_part = np.ascontiguousarray(rec_part, dtype=np.uint32)
+    dst_off, dst_len, cks, st = _partition_out(num_partitions)
+    total, cached = _u64(0), _i32(0)
+    _check(load().b2s_partition_compress_cached_packed(
+        shuffle_id, map_id, codec, level, block_size, checksum_alg, num_partitions, rec_len.size, _ptr(records),
+        records.size, _ptr(rec_len), _ptr(rec_part), _ptr(dst), dst.size, _ptr(dst_off), _ptr(dst_len),
+        C.addressof(total), _ptr(cks), _ptr(st), C.addressof(cached)), "b2s_partition_compress_cached_packed")
+    return dict(dst_off=dst_off, dst_len=dst_len, total=total.value, checksums=cks, status=st, cached=cached.value)
+
+
+def exchange_lookup(shuffle_id, start_reduce, end_reduce, map_ids):
+    """-> (hits, lengths): lengths[i] = bytes of the range of map_ids[i], NOT_RESIDENT when it is not resident"""
+    ids = np.ascontiguousarray(map_ids, dtype=np.int64)
+    ln = np.zeros(max(ids.size, 1), dtype=np.uint64)
+    rc = load().b2s_exchange_lookup(shuffle_id, start_reduce, end_reduce, ids.size, _ptr(ids), _ptr(ln))
+    if rc < 0:
+        raise B2SError(rc, "b2s_exchange_lookup")
+    return rc, ln[: ids.size]
+
+
+def exchange_read_packed(shuffle_id, start_reduce, end_reduce, map_ids, dst):
+    """the cached ranges back to back into dst.  -> dict(dst_off, dst_len, total, status)"""
+    ids = np.ascontiguousarray(map_ids, dtype=np.int64)
+    dst = _as_u8(dst)
+    n = ids.size
+    dst_off = np.zeros(max(n, 1), dtype=np.uint64)
+    dst_len = np.zeros(max(n, 1), dtype=np.uint64)
+    st = np.zeros(max(n, 1), dtype=np.int32)
+    total = _u64(0)
+    _check(load().b2s_exchange_read_packed(shuffle_id, start_reduce, end_reduce, n, _ptr(ids), _ptr(dst), dst.size,
+                                           _ptr(dst_off), _ptr(dst_len), C.addressof(total), _ptr(st)),
+           "b2s_exchange_read_packed")
+    return dict(dst_off=dst_off[:n], dst_len=dst_len[:n], total=total.value, status=st[:n])
+
+
+def _exchange_sources(map_ids, cached):
+    return (np.ascontiguousarray(map_ids, dtype=np.int64),
+            np.ascontiguousarray(np.asarray(cached, dtype=bool), dtype=np.uint8))
+
+
+def exchange_read_sort_packed(shuffle_id, start_reduce, end_reduce, map_ids, cached, codec, src, off, length, dst,
+                              record_bytes, key_off, key_len, checksum_alg=CHECKSUM_NONE, slice_base=None,
+                              slice_len=None, slice_checksum=None):
+    """decompress_sort_packed over sources of which those with cached[i] set are the cached range of map_ids[i].
+    -> dict(total, n_records, status, bad_slice)"""
+    ids, cm = _exchange_sources(map_ids, cached)
+    src, dst = _as_u8(src), _as_u8(dst)
+    off = np.ascontiguousarray(off, dtype=np.uint64)
+    length = np.ascontiguousarray(length, dtype=np.uint64)
+    n = ids.size
+    sb, sl, sc = _sort_slices(checksum_alg, slice_base, slice_len, slice_checksum)
+    st = np.zeros(max(n, 1), dtype=np.int32)
+    bad = np.zeros(max(n, 1), dtype=np.int32)
+    total, nrec = _u64(0), _u64(0)
+    _check(load().b2s_exchange_read_sort_packed(shuffle_id, start_reduce, end_reduce, _ptr(ids), _ptr(cm), codec,
+                                                checksum_alg, n, _ptr(src), _ptr(off), _ptr(length), _ptr(sb),
+                                                _ptr(sl), _ptr(sc), record_bytes, key_off, key_len, _ptr(dst),
+                                                dst.size, C.addressof(total), C.addressof(nrec), _ptr(st), _ptr(bad)),
+           "b2s_exchange_read_sort_packed")
+    return dict(total=total.value, n_records=nrec.value, status=st[:n], bad_slice=bad[:n])
+
+
+def exchange_read_sort_dev(shuffle_id, start_reduce, end_reduce, map_ids, cached, codec, d_src, off, length, d_dst,
+                           dst_cap, record_bytes, key_off, key_len, checksum_alg=CHECKSUM_NONE, slice_base=None,
+                           slice_len=None, slice_checksum=None, dev=0):
+    """exchange_read_sort_packed with the fetched blocks (d_src) and the output (d_dst) in device memory"""
+    ids, cm = _exchange_sources(map_ids, cached)
+    off = np.ascontiguousarray(off, dtype=np.uint64)
+    length = np.ascontiguousarray(length, dtype=np.uint64)
+    n = ids.size
+    sb, sl, sc = _sort_slices(checksum_alg, slice_base, slice_len, slice_checksum)
+    st = np.zeros(max(n, 1), dtype=np.int32)
+    bad = np.zeros(max(n, 1), dtype=np.int32)
+    total, nrec = _u64(0), _u64(0)
+    _check(load().b2s_exchange_read_sort_dev(dev, shuffle_id, start_reduce, end_reduce, _ptr(ids), _ptr(cm), codec,
+                                             checksum_alg, n, d_src, _ptr(off), _ptr(length), _ptr(sb), _ptr(sl),
+                                             _ptr(sc), record_bytes, key_off, key_len, d_dst, dst_cap,
+                                             C.addressof(total), C.addressof(nrec), _ptr(st), _ptr(bad)),
+           "b2s_exchange_read_sort_dev")
+    return dict(total=total.value, n_records=nrec.value, status=st[:n], bad_slice=bad[:n])
+
+
+def exchange_remove(shuffle_id, map_id=-1):
+    """removes (shuffle_id, map_id), or every map output of the shuffle (map_id -1), on every device -> count"""
+    rc = load().b2s_exchange_remove(shuffle_id, map_id)
+    if rc < 0:
+        raise B2SError(rc, "b2s_exchange_remove")
+    return rc

@@ -13,6 +13,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <map>
 #include <mutex>
 #include <string>
 #include <thread>
@@ -155,6 +156,8 @@ struct PreferNode {
 }  // namespace numa
 thread_local int t_numa_node = -1;  // node of the device this thread's pinned allocations should sit next to
 
+bool exchange_shed_current_device();  // exchange cache (below): frees the current device's unreferenced entries
+
 struct DevBuf {
   void* p = nullptr;
   size_t cap = 0;
@@ -169,6 +172,11 @@ struct DevBuf {
       (void)cudaGetLastError();  // an allocation failure is reported as B2S_E_NOMEM, not left for a later CU() check
       e = cudaMalloc(&p, bytes);
       want = bytes;
+    }
+    // a workspace never fails for want of memory the exchange cache holds: it gives back what no read uses, once
+    if (e != cudaSuccess && exchange_shed_current_device()) {
+      (void)cudaGetLastError();
+      e = cudaMalloc(&p, bytes);
     }
     if (e != cudaSuccess) {
       (void)cudaGetLastError();
@@ -235,6 +243,7 @@ struct Slot {
   cudaEvent_t ev_p0 = nullptr, ev_p1 = nullptr;            // partition step (b2s_partition_compress_*)
   DevBuf meta, scratch, desc, src, dst, zmeta;
   DevBuf pws, parena;  // partition workspace (sort keys, offsets) and the partitioned arena in front of compression
+  DevBuf xpieces;      // the copy pieces of an exchange-cache read (exchange.cu)
   PinBuf hmeta;
   // per-launch event pairs around the dominant kernel of a call (grow-only pool; `used` pairs are valid)
   std::vector<cudaEvent_t> ev_dom;
@@ -872,6 +881,194 @@ int shard_over_devices(uint32_t n, F&& run_subset) {
 }
 bool want_sharding(uint32_t n) { return g_ctx && g_ctx->devs.size() > 1 && n >= 2 * g_ctx->devs.size(); }
 
+// --------------------------------------------------------------------------------------------------------------
+// exchange cache (docs/f4_gpu_resident_exchange.md steps 2-3): partitioned map outputs kept in HBM, per CUDA device,
+// under a byte budget, least recently used out first.  An entry is linked in `by_key` while it can be found; a read
+// references the entries it uses until its stream has synchronised, and an entry unlinked (evicted, removed, replaced)
+// while referenced is freed by its last reader.  `used` counts the bytes of linked entries.  The lock is never held
+// across a CUDA call: device memory is allocated and freed outside it.
+// --------------------------------------------------------------------------------------------------------------
+constexpr int kMaxOrdinals = 32;  // b2s_init selects devices 0..31
+struct ExEntry {
+  int32_t shuffle = 0;
+  int64_t map = 0;
+  int ordinal = 0;  // CUDA device holding buf
+  uint8_t* buf = nullptr;
+  uint64_t bytes = 0;
+  std::vector<uint64_t> part_start;  // R + 1 offsets of the partitions in buf
+  uint32_t refs = 0;
+  uint64_t last_use = 0;
+  bool linked = true;
+};
+struct ExCache {
+  std::mutex mtx;
+  std::map<std::pair<int32_t, int64_t>, ExEntry*> by_key;
+  uint64_t budget[kMaxOrdinals] = {}, used[kMaxOrdinals] = {};
+  uint64_t tick = 0;
+};
+ExCache g_ex;
+
+// unlinks e (caller holds g_ex.mtx); an unreferenced entry goes to `dead`, for the caller to free outside the lock
+void ex_unlink(ExEntry* e, std::vector<ExEntry*>& dead) {
+  g_ex.by_key.erase({e->shuffle, e->map});
+  g_ex.used[e->ordinal] -= e->bytes;
+  e->linked = false;
+  if (!e->refs) dead.push_back(e);
+}
+
+void ex_free(const std::vector<ExEntry*>& dead) {
+  if (dead.empty()) return;
+  int cur = 0;
+  cudaGetDevice(&cur);
+  for (ExEntry* e : dead) {
+    if (e->buf) {
+      cudaSetDevice(e->ordinal);
+      cudaFree(e->buf);
+    }
+    delete e;
+  }
+  cudaSetDevice(cur);
+  (void)cudaGetLastError();
+}
+
+// unlinks least recently used unreferenced entries of `ordinal` until `bytes` more fit under its budget (caller holds
+// the lock).  When they cannot be made to fit it returns false, having evicted nothing unless `partial` (a lowered
+// budget: evict what can go, the referenced rest goes when it is released and evicted later).
+bool ex_make_room(int ordinal, uint64_t bytes, std::vector<ExEntry*>& dead, bool partial = false) {
+  const uint64_t budget = g_ex.budget[ordinal];
+  uint64_t idle = 0;
+  for (auto& kv : g_ex.by_key)
+    if (kv.second->ordinal == ordinal && !kv.second->refs) idle += kv.second->bytes;
+  const bool fits = bytes <= budget && g_ex.used[ordinal] - idle <= budget - bytes;
+  if (!fits && !partial) return false;
+  while (g_ex.used[ordinal] + bytes > budget) {
+    ExEntry* victim = nullptr;
+    for (auto& kv : g_ex.by_key) {
+      ExEntry* e = kv.second;
+      if (e->ordinal == ordinal && !e->refs && (!victim || e->last_use < victim->last_use)) victim = e;
+    }
+    if (!victim) break;
+    ex_unlink(victim, dead);
+  }
+  return fits;
+}
+
+bool exchange_shed_current_device() {
+  int ordinal = 0;
+  if (cudaGetDevice(&ordinal) != cudaSuccess || ordinal < 0 || ordinal >= kMaxOrdinals) return false;
+  std::vector<ExEntry*> dead;
+  {
+    std::lock_guard<std::mutex> lk(g_ex.mtx);
+    std::vector<ExEntry*> idle;
+    for (auto& kv : g_ex.by_key)
+      if (kv.second->ordinal == ordinal && !kv.second->refs) idle.push_back(kv.second);
+    for (ExEntry* e : idle) ex_unlink(e, dead);
+  }
+  ex_free(dead);
+  return !dead.empty();
+}
+
+// The entries a read uses, referenced from its lookup until the read's stream has synchronised.  entry[i]: the
+// resident entry of map_ids[i] on `ordinal` (nullptr: not resident, or want[i] == 0); each use counts for the LRU order.
+struct ExRefs {
+  std::vector<ExEntry*> entry;
+  ExRefs(int ordinal, int32_t shuffle, uint32_t n, const int64_t* map_ids, const uint8_t* want) : entry(n, nullptr) {
+    std::lock_guard<std::mutex> lk(g_ex.mtx);
+    for (uint32_t i = 0; i < n; i++) {
+      if (want && !want[i]) continue;
+      auto it = g_ex.by_key.find({shuffle, map_ids[i]});
+      if (it == g_ex.by_key.end() || it->second->ordinal != ordinal) continue;
+      entry[i] = it->second;
+      entry[i]->refs++;
+      entry[i]->last_use = ++g_ex.tick;
+    }
+  }
+  ~ExRefs() {
+    std::vector<ExEntry*> dead;
+    {
+      std::lock_guard<std::mutex> lk(g_ex.mtx);
+      for (ExEntry* e : entry)
+        if (e && --e->refs == 0 && !e->linked) dead.push_back(e);
+    }
+    ex_free(dead);
+  }
+  // B2S_E_ARG when a resident entry has fewer than end_reduce partitions
+  int check_range(int32_t end_reduce) const {
+    for (const ExEntry* e : entry)
+      if (e && (uint64_t)end_reduce + 1 > e->part_start.size())
+        return fail(B2S_E_ARG, "end_reduce exceeds the partitions of a cached map output%s");
+    return 0;
+  }
+  // the bytes of partitions [start, end) of source i inside its entry
+  const uint8_t* range(uint32_t i, int32_t start, int32_t end, uint64_t* len) const {
+    const ExEntry* e = entry[i];
+    *len = e->part_start[(size_t)end] - e->part_start[(size_t)start];
+    return e->buf + e->part_start[(size_t)start];
+  }
+};
+
+// Keeps `bytes` of partitioned records at d_rec (device memory of the current device `ordinal`, stream st) as the
+// entry (shuffle, map): exact-size allocation, device-to-device copy.  Returns 1 when stored, 0 when it does not fit.
+int ex_store(int ordinal, cudaStream_t st, int32_t shuffle, int64_t map, const uint8_t* d_rec, uint64_t bytes,
+             std::vector<uint64_t>&& part_start) {
+  std::vector<ExEntry*> dead;
+  bool fits;
+  {
+    std::lock_guard<std::mutex> lk(g_ex.mtx);
+    auto it = g_ex.by_key.find({shuffle, map});
+    if (it != g_ex.by_key.end()) ex_unlink(it->second, dead);  // a stale output of this map is never served again
+    fits = g_ex.budget[ordinal] > 0 && ex_make_room(ordinal, bytes, dead);
+    if (fits) g_ex.used[ordinal] += bytes;  // reserved until the entry is linked
+  }
+  ex_free(dead);
+  dead.clear();
+  if (!fits) return 0;
+  ExEntry* e = new ExEntry();
+  e->shuffle = shuffle;
+  e->map = map;
+  e->ordinal = ordinal;
+  e->bytes = bytes;
+  e->part_start = std::move(part_start);
+  bool ok = true;
+  if (bytes) {
+    ok = cudaMalloc(&e->buf, bytes) == cudaSuccess &&
+         cudaMemcpyAsync(e->buf, d_rec, bytes, cudaMemcpyDeviceToDevice, st) == cudaSuccess &&
+         cudaStreamSynchronize(st) == cudaSuccess;
+    if (!ok) (void)cudaGetLastError();  // not stored; the call's own outputs are unaffected
+  }
+  {
+    std::lock_guard<std::mutex> lk(g_ex.mtx);
+    g_ex.used[ordinal] -= bytes;
+    if (!ok) {
+      dead.push_back(e);
+    } else {
+      auto it = g_ex.by_key.find({shuffle, map});
+      if (it != g_ex.by_key.end()) ex_unlink(it->second, dead);  // stored by another thread meanwhile
+      g_ex.used[ordinal] += bytes;
+      e->last_use = ++g_ex.tick;
+      g_ex.by_key[{shuffle, map}] = e;
+    }
+  }
+  ex_free(dead);
+  return ok ? 1 : 0;
+}
+
+// without a usable device the exchange calls report B2S_E_CUDA (b2s_init has failed for that reason)
+int exchange_ready() {
+  if (g_ctx) return 0;
+  int count = 0;
+  const cudaError_t e = cudaGetDeviceCount(&count);
+  if (e != cudaSuccess || count <= 0)
+    return fail(B2S_E_CUDA, "no CUDA device: %s", e != cudaSuccess ? cudaGetErrorString(e) : "device count is 0");
+  return fail(B2S_E_NOT_INIT, "b2s_init has not been called%s");
+}
+
+int reduce_range_args(int32_t start_reduce, int32_t end_reduce) {
+  if (start_reduce < 0 || end_reduce < start_reduce || end_reduce > (1 << 24))
+    return fail(B2S_E_ARG, "reduce range must satisfy 0 <= start_reduce <= end_reduce <= 2^24%s");
+  return 0;
+}
+
 }  // namespace
 
 // ==============================================================================================================
@@ -892,6 +1089,7 @@ const char* b2s_strerror(int32_t code) {
     case B2S_E_CUDA: return "CUDA failure or no usable device";
     case B2S_E_NOT_INIT: return "b2s_init has not been called";
     case B2S_E_NOMEM: return "out of memory";
+    case B2S_E_NOT_CACHED: return "not resident in the exchange cache";
     default: return "unknown error";
   }
 }
@@ -982,6 +1180,13 @@ int b2s_init(uint32_t gpu_mask, uint64_t pinned_bytes_per_gpu, uint32_t streams_
 void b2s_shutdown(void) {
   std::lock_guard<std::mutex> lk(g_init_mtx);
   if (!g_ctx) return;
+  std::vector<ExEntry*> dead;
+  {
+    std::lock_guard<std::mutex> lx(g_ex.mtx);
+    while (!g_ex.by_key.empty()) ex_unlink(g_ex.by_key.begin()->second, dead);
+    for (int d = 0; d < kMaxOrdinals; d++) g_ex.budget[d] = 0;
+  }
+  ex_free(dead);
   for (Device* D : g_ctx->devs) {
     cudaSetDevice(D->ordinal);
     cudaDeviceSynchronize();
@@ -996,6 +1201,7 @@ void b2s_shutdown(void) {
       S.dst.release();
       S.pws.release();
       S.parena.release();
+      S.xpieces.release();
       S.hmeta.release();
       cudaEvent_t evs[] = {S.ev_a, S.ev_b, S.ev_k0, S.ev_k1, S.ev_t0, S.ev_t1, S.ev_h0, S.ev_h1, S.ev_d0, S.ev_d1,
                            S.ev_p0, S.ev_p1};
@@ -1534,12 +1740,14 @@ static uint64_t first_record_past(const uint64_t* d_off, const uint32_t* d_len, 
 
 // The partition step and the compression of the non-empty partitions, on device-resident records.  d_dst receives the
 // .data arena (dst_cap bytes); *arena_bytes the bytes it needs.  Returns B2S_E_DST_TOO_SMALL (status[] set for the
-// partitions that do not fit) when dst_cap is short.
+// partitions that do not fit) when dst_cap is short.  part_start (optional) receives the R + 1 partition offsets of the
+// partitioned records, which are in d_dst (codec NONE) or S.parena.
 static int partition_compress_run(Device* D, Slot& S, uint32_t codec, int32_t level, uint32_t bs, uint32_t alg,
                                   uint32_t R, uint64_t n, const uint8_t* d_rec, uint64_t rec_bytes,
                                   const uint32_t* d_len, const uint32_t* d_part, uint8_t* d_dst, uint64_t dst_cap,
                                   uint64_t* dst_off, uint64_t* dst_len, uint64_t* checksum_out, int32_t* status,
-                                  uint64_t* arena_bytes, uint64_t* launches) {
+                                  uint64_t* arena_bytes, uint64_t* launches,
+                                  std::vector<uint64_t>* part_start = nullptr) {
   cudaStream_t st = S.st;
   std::vector<uint64_t> pstart(R), plen(R);
   CU(cudaEventRecord(S.ev_p0, st));
@@ -1582,6 +1790,10 @@ static int partition_compress_run(Device* D, Slot& S, uint32_t codec, int32_t le
     }
   } else if (rec_bytes) {
     return fail(B2S_E_ARG, "rec_len sums to 0 bytes, rec_bytes is %s", std::to_string(rec_bytes).c_str());
+  }
+  if (part_start) {
+    part_start->assign(pstart.begin(), pstart.end());
+    part_start->push_back(rec_bytes);
   }
 
   if (codec == B2S_CODEC_NONE) {
@@ -1746,11 +1958,19 @@ int b2s_partition_compress_dev(uint32_t dev_index, uint32_t codec, int32_t level
   return rc;
 }
 
-int b2s_partition_compress_packed(uint32_t codec, int32_t level, uint32_t codec_block_size, uint32_t checksum_alg,
-                                  uint32_t num_partitions, uint64_t n_records, const uint8_t* rec_base,
-                                  uint64_t rec_bytes, const uint32_t* rec_len, const uint32_t* rec_part,
-                                  uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_off, uint64_t* dst_len,
-                                  uint64_t* dst_total, uint64_t* checksum_out, int32_t* status) {
+// what a cached store keeps: the exchange-cache key and where to report whether it was stored
+struct ExStore {
+  int32_t shuffle;
+  int64_t map;
+  int32_t* cached;
+};
+
+static int partition_compress_packed(uint32_t codec, int32_t level, uint32_t codec_block_size, uint32_t checksum_alg,
+                                     uint32_t num_partitions, uint64_t n_records, const uint8_t* rec_base,
+                                     uint64_t rec_bytes, const uint32_t* rec_len, const uint32_t* rec_part,
+                                     uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_off, uint64_t* dst_len,
+                                     uint64_t* dst_total, uint64_t* checksum_out, int32_t* status,
+                                     const ExStore* store) {
   WallTimer wt;
   t_timing = b2s_timing{};
   if (dst_total) *dst_total = 0;
@@ -1782,11 +2002,11 @@ int b2s_partition_compress_packed(uint32_t codec, int32_t level, uint32_t codec_
     CU(cudaMemcpyAsync(d_part, rec_part, n_records * 4, cudaMemcpyHostToDevice, st));
   }
   CU(cudaEventRecord(S.ev_h1, st));
-  std::vector<uint64_t> cks(num_partitions);
+  std::vector<uint64_t> cks(num_partitions), part_start;
   uint64_t launches = 0, arena = 0;
   rc = partition_compress_run(D, S, codec, level, bs, checksum_alg, num_partitions, n_records, d_rec, rec_bytes, d_len,
                               d_part, (uint8_t*)S.dst.p, S.dst.cap, dst_off, dst_len, cks.data(), status, &arena,
-                              &launches);
+                              &launches, store ? &part_start : nullptr);
   if (rc) return rc;
   // the device arena is sized by the bound, so a short caller arena shows up here: copy what fits, flag the rest
   int result = 0;
@@ -1809,8 +2029,39 @@ int b2s_partition_compress_packed(uint32_t codec, int32_t level, uint32_t codec_
   t_timing.d2h_ms = ms_between(S.ev_d0, S.ev_d1);
   t_timing.h2d_bytes = rec_bytes + n_records * 8;
   t_timing.d2h_bytes = fit;
+  if (store && !result) {
+    // the partitioned records are still in this slot (the write lane is held): in front of compression, or the arena
+    // itself for codec NONE
+    const uint8_t* parts = (const uint8_t*)(codec == B2S_CODEC_NONE ? S.dst.p : S.parena.p);
+    *store->cached = ex_store(D->ordinal, st, store->shuffle, store->map, parts, rec_bytes, std::move(part_start));
+  }
   t_timing.total_ms = wt.ms();
   return result;
+}
+
+int b2s_partition_compress_packed(uint32_t codec, int32_t level, uint32_t codec_block_size, uint32_t checksum_alg,
+                                  uint32_t num_partitions, uint64_t n_records, const uint8_t* rec_base,
+                                  uint64_t rec_bytes, const uint32_t* rec_len, const uint32_t* rec_part,
+                                  uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_off, uint64_t* dst_len,
+                                  uint64_t* dst_total, uint64_t* checksum_out, int32_t* status) {
+  return partition_compress_packed(codec, level, codec_block_size, checksum_alg, num_partitions, n_records, rec_base,
+                                   rec_bytes, rec_len, rec_part, dst_base, dst_cap, dst_off, dst_len, dst_total,
+                                   checksum_out, status, nullptr);
+}
+
+int b2s_partition_compress_cached_packed(int32_t shuffle_id, int64_t map_id, uint32_t codec, int32_t level,
+                                         uint32_t codec_block_size, uint32_t checksum_alg, uint32_t num_partitions,
+                                         uint64_t n_records, const uint8_t* rec_base, uint64_t rec_bytes,
+                                         const uint32_t* rec_len, const uint32_t* rec_part, uint8_t* dst_base,
+                                         uint64_t dst_cap, uint64_t* dst_off, uint64_t* dst_len, uint64_t* dst_total,
+                                         uint64_t* checksum_out, int32_t* status, int32_t* cached) {
+  if (!cached) return fail(B2S_E_ARG, "null argument%s");
+  *cached = 0;
+  if (int rc = exchange_ready()) return rc;
+  const ExStore store{shuffle_id, map_id, cached};
+  return partition_compress_packed(codec, level, codec_block_size, checksum_alg, num_partitions, n_records, rec_base,
+                                   rec_bytes, rec_len, rec_part, dst_base, dst_cap, dst_off, dst_len, dst_total,
+                                   checksum_out, status, &store);
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -2217,51 +2468,84 @@ struct SortBufferTrim {
   }
 };
 
+// A source of an exchange-cache sorted read (b2s_exchange_read_sort_*): a cached range (records on the device, held by
+// a reference for the call; status B2S_E_NOT_CACHED when it is not resident) or fetched block `block`.
+struct SortSource {
+  bool cached = false;
+  int32_t status = B2S_OK;
+  const uint8_t* src = nullptr;
+  uint64_t len = 0;
+  uint32_t block = 0;
+};
+
 // The whole reduce task on the device: compressed blocks at d_src + src_dev_off[i] (src_contiguous: back to back from
 // d_src in block order, no gaps).  Phase A verifies the slices and sizes every block; a failed block, or a decoded
 // length that is not a multiple of record_bytes, ends the call with status[] set and *n_rec = 0 (nothing decoded or
 // sorted).  Then the blocks are decoded into S.dst (codec NONE: used in place, or copied there), their records sorted
 // into *d_sorted (nullptr: into S.parena, returned there).
+// mix (exchange-cache reads): the call's sources in order, the n blocks being its fetched ones; status[] / bad_slice[]
+// are per source.  Every source's records land at their source-order place in S.dst: phase A's decoded offsets are
+// shifted past the cached bytes in front of each block before phase B decodes, and one gather moves the cached ranges
+// (codec NONE: and the fetched blocks) around them.
 static int decompress_sort_run(Device* D, Slot& S, uint32_t codec, uint32_t alg, uint32_t n, const uint8_t* d_src,
                                const uint64_t* src_dev_off, const uint64_t* src_len, bool src_contiguous,
                                const uint32_t* slice_base, const uint64_t* slice_len, const uint64_t* slice_sum,
                                uint32_t record_bytes, uint32_t key_off, uint32_t key_len, uint8_t** d_sorted,
                                uint64_t out_cap, uint64_t* total, uint64_t* n_rec, int32_t* status, int32_t* bad_slice,
-                               uint64_t* launches) {
+                               uint64_t* launches, const std::vector<SortSource>* mix = nullptr) {
   cudaStream_t st = S.st;
   DecompressJob J;
-  const uint32_t ns = alg ? slice_base[n] : 0;
-  int rc = decompress_prepare(S, codec, alg, n, ns, J, true);
-  if (rc) return rc;
-  memcpy(J.h_src_off, src_dev_off, (size_t)n * 8);
-  memcpy(J.h_src_len, src_len, (size_t)n * 8);
-  fill_slices(J, 0, n, src_dev_off, src_len, slice_base, slice_len, slice_sum);
-  uint64_t srcb = 0;
-  for (uint32_t i = 0; i < n; i++) srcb += src_len[i];
-  rc = decompress_enqueue_a(S, D->tabs, alg, J, d_src, srcb, launches);
-  if (rc) return rc;
-  // the phase-A verdicts (checksums, stream headers) and decoded lengths, before anything is decoded
-  CU(cudaMemcpyAsync(J.h_down, J.d_down, J.down_bytes, cudaMemcpyDeviceToHost, st));
-  CU(cudaStreamSynchronize(st));
-  CU(cudaGetLastError());
-  *total = J.h_totals[1];
+  int rc;
+  if (n) {
+    const uint32_t ns = alg ? slice_base[n] : 0;
+    rc = decompress_prepare(S, codec, alg, n, ns, J, true);
+    if (rc) return rc;
+    memcpy(J.h_src_off, src_dev_off, (size_t)n * 8);
+    memcpy(J.h_src_len, src_len, (size_t)n * 8);
+    fill_slices(J, 0, n, src_dev_off, src_len, slice_base, slice_len, slice_sum);
+    uint64_t srcb = 0;
+    for (uint32_t i = 0; i < n; i++) srcb += src_len[i];
+    rc = decompress_enqueue_a(S, D->tabs, alg, J, d_src, srcb, launches);
+    if (rc) return rc;
+    // the phase-A verdicts (checksums, stream headers) and decoded lengths, before anything is decoded
+    CU(cudaMemcpyAsync(J.h_down, J.d_down, J.down_bytes, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    CU(cudaGetLastError());
+  } else {  // every source is cached
+    CU(cudaEventRecord(S.ev_k0, st));
+  }
+  const uint32_t n_src = mix ? (uint32_t)mix->size() : n;
+  auto cached = [&](uint32_t i) { return mix && (*mix)[i].cached; };
+  auto block = [&](uint32_t i) { return mix ? (*mix)[i].block : i; };
+  std::vector<int32_t> cached_status(n_src, B2S_OK);
+  std::vector<uint64_t> place(n_src);  // each source's offset in the decoded arena
+  uint64_t at = 0;
   *n_rec = 0;
   bool failed = false;
   char msg[256];
-  for (uint32_t i = 0; i < n; i++) {
-    if (J.h_status[i] == B2S_OK && J.h_dst_len[i] % record_bytes) {
-      J.h_status[i] = B2S_E_CORRUPT;
+  for (uint32_t i = 0; i < n_src; i++) {
+    const bool c = cached(i);
+    int32_t& s = c ? cached_status[i] : J.h_status[block(i)];
+    const uint64_t len = c ? (*mix)[i].len : J.h_dst_len[block(i)];
+    if (c) s = (*mix)[i].status;
+    if (s == B2S_OK && len % record_bytes) {
+      s = B2S_E_CORRUPT;
       if (!failed) {
-        snprintf(msg, sizeof msg, "block %u decodes to %llu bytes, not a multiple of record_bytes %u", i,
-                 (unsigned long long)J.h_dst_len[i], record_bytes);
+        snprintf(msg, sizeof msg, "%s %u %s %llu bytes, not a multiple of record_bytes %u", c ? "cached source" : "block",
+                 i, c ? "holds" : "decodes to", (unsigned long long)len, record_bytes);
         fail(B2S_E_CORRUPT, "%s", msg);
       }
     }
-    failed |= J.h_status[i] != B2S_OK;
+    failed |= s != B2S_OK;
+    place[i] = at;
+    at += len;
   }
+  *total = mix ? at : J.h_totals[1];
   auto report = [&]() {
-    memcpy(status, J.h_status, (size_t)n * 4);
-    if (bad_slice) memcpy(bad_slice, J.h_bad, (size_t)n * 4);
+    for (uint32_t i = 0; i < n_src; i++) {
+      status[i] = cached(i) ? cached_status[i] : J.h_status[block(i)];
+      if (bad_slice) bad_slice[i] = cached(i) ? -1 : J.h_bad[block(i)];
+    }
   };
   auto skip_events = [&](bool decode, bool sort) -> int {  // stand-ins for the steps a call does not run
     if (decode) {
@@ -2290,8 +2574,31 @@ static int decompress_sort_run(Device* D, Slot& S, uint32_t codec, uint32_t alg,
 
   // the decoded arena: every block's records back to back in block order
   const uint8_t* arena = d_src;
-  if (codec == B2S_CODEC_NONE) {
-    if (!src_contiguous && *total) {
+  if (mix) {
+    if ((rc = S.dst.ensure(*total + 64))) return rc;
+    arena = (const uint8_t*)S.dst.p;
+    std::vector<ExchangePiece> pieces;
+    for (uint32_t i = 0; i < n_src; i++) {
+      const SortSource& s = (*mix)[i];
+      if (s.cached)
+        exchange_add_pieces(pieces, s.src, place[i], s.len);
+      else if (codec == B2S_CODEC_NONE)
+        exchange_add_pieces(pieces, d_src + src_dev_off[s.block], place[i], src_len[s.block]);
+      else
+        J.h_dst_off[s.block] = place[i];
+    }
+    if (n && codec != B2S_CODEC_NONE)  // phase B decodes every block straight to its place among the cached ranges
+      CU(cudaMemcpyAsync(J.dst_off, J.h_dst_off, (size_t)n * 8, cudaMemcpyHostToDevice, st));
+    if (!pieces.empty()) {
+      if ((rc = S.xpieces.ensure(pieces.size() * sizeof(ExchangePiece)))) return rc;
+      CU(cudaMemcpyAsync(S.xpieces.p, pieces.data(), pieces.size() * sizeof(ExchangePiece), cudaMemcpyHostToDevice,
+                         st));
+      launch_exchange_gather((const ExchangePiece*)S.xpieces.p, (uint32_t)pieces.size(), (uint8_t*)S.dst.p, st,
+                             launches);
+    }
+  }
+  if (codec == B2S_CODEC_NONE || !n) {
+    if (!mix && !src_contiguous && *total) {
       if ((rc = S.dst.ensure(*total + 64))) return rc;
       for (uint32_t i = 0; i < n; i++)
         if (src_len[i])
@@ -2301,7 +2608,7 @@ static int decompress_sort_run(Device* D, Slot& S, uint32_t codec, uint32_t alg,
     }
     if ((rc = skip_events(true, false))) return rc;
   } else {
-    if ((rc = S.dst.ensure(*total + 64))) return rc;
+    if (!mix && (rc = S.dst.ensure(*total + 64))) return rc;
     rc = decompress_enqueue_b(S, J, d_src, (uint8_t*)S.dst.p, S.dst.cap, launches);
     if (rc) return rc;
     CU(cudaEventSynchronize(S.ev_b));
@@ -2340,6 +2647,80 @@ static void sort_timing(Slot& S, uint64_t n_launches, uint64_t src_bytes, uint64
   g_ctx->launches += n_launches;
 }
 
+// decompress_sort on the read lane of D over device-resident blocks, sorted into dst_base (device memory)
+static int sort_dev_run(Device* D, uint32_t codec, uint32_t alg, uint32_t n, const uint8_t* src_base,
+                        const uint64_t* src_off, const uint64_t* src_len, const uint32_t* slice_base,
+                        const uint64_t* slice_len, const uint64_t* slice_checksum, uint32_t record_bytes,
+                        uint32_t key_off, uint32_t key_len, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_total,
+                        uint64_t* n_records, int32_t* status, int32_t* bad_slice, const WallTimer& wt,
+                        const std::vector<SortSource>* mix = nullptr) {
+  Lane& Ln = D->lane[kLaneRead];
+  std::lock_guard<std::mutex> lk(Ln.mtx);
+  Slot& S = Ln.slot[0];
+  SortBufferTrim trim{S};
+  uint64_t launches = 0, srcb = 0;
+  for (uint32_t i = 0; i < n; i++) srcb += src_len[i];
+  uint8_t* out = dst_base;
+  int rc = decompress_sort_run(D, S, codec, alg, n, src_base, src_off, src_len, false, slice_base, slice_len,
+                               slice_checksum, record_bytes, key_off, key_len, &out, dst_cap, dst_total, n_records,
+                               status, bad_slice, &launches, mix);
+  if (rc) return rc;
+  sort_timing(S, launches, srcb, *dst_total);
+  t_timing.total_ms = wt.ms();
+  return 0;
+}
+
+// decompress_sort on the read lane of D over host blocks: one upload, the sort, one download into dst_base
+static int sort_packed_run(Device* D, uint32_t codec, uint32_t alg, uint32_t n, const uint8_t* src_base,
+                           const uint64_t* src_off, const uint64_t* src_len, const uint32_t* slice_base,
+                           const uint64_t* slice_len, const uint64_t* slice_checksum, uint32_t record_bytes,
+                           uint32_t key_off, uint32_t key_len, uint8_t* dst_base, uint64_t dst_cap,
+                           uint64_t* dst_total, uint64_t* n_records, int32_t* status, int32_t* bad_slice,
+                           const WallTimer& wt, const std::vector<SortSource>* mix = nullptr) {
+  Lane& Ln = D->lane[kLaneRead];
+  std::lock_guard<std::mutex> lk(Ln.mtx);
+  Slot& S = Ln.slot[0];
+  SortBufferTrim trim{S};
+  // one upload of every block, back to back (the whole task is resident at once: no chunking)
+  std::vector<uint64_t> dev_off(n);
+  uint64_t srcb = 0;
+  for (uint32_t i = 0; i < n; i++) {
+    dev_off[i] = srcb;
+    srcb += src_len[i];
+  }
+  int rc;
+  if ((rc = S.src.ensure(srcb + 64))) return rc;
+  cudaStream_t st = S.st;
+  CU(cudaEventRecord(S.ev_h0, st));
+  for (uint32_t i = 0; i < n;) {  // blocks adjacent in host memory go up in one copy
+    uint32_t j = i + 1;
+    while (j < n && src_off[j] == src_off[j - 1] + src_len[j - 1]) j++;
+    const uint64_t bytes = dev_off[j - 1] + src_len[j - 1] - dev_off[i];
+    if (bytes) CU(copy_async((uint8_t*)S.src.p + dev_off[i], src_base + src_off[i], bytes, cudaMemcpyHostToDevice, st));
+    i = j;
+  }
+  CU(cudaEventRecord(S.ev_h1, st));
+  uint64_t launches = 0;
+  uint8_t* sorted = nullptr;
+  rc = decompress_sort_run(D, S, codec, alg, n, (const uint8_t*)S.src.p, dev_off.data(), src_len, true, slice_base,
+                           slice_len, slice_checksum, record_bytes, key_off, key_len, &sorted, dst_cap, dst_total,
+                           n_records, status, bad_slice, &launches, mix);
+  if (rc) return rc;
+  const uint64_t down = *n_records ? *dst_total : 0;
+  CU(cudaEventRecord(S.ev_d0, st));
+  if (down) CU(copy_async(dst_base, sorted, down, cudaMemcpyDeviceToHost, st));
+  CU(cudaEventRecord(S.ev_d1, st));
+  CU(cudaStreamSynchronize(st));
+  CU(cudaGetLastError());
+  sort_timing(S, launches, srcb, *dst_total);
+  t_timing.h2d_ms = ms_between(S.ev_h0, S.ev_h1);
+  t_timing.d2h_ms = ms_between(S.ev_d0, S.ev_d1);
+  t_timing.h2d_bytes = srcb;
+  t_timing.d2h_bytes = down;
+  t_timing.total_ms = wt.ms();
+  return 0;
+}
+
 int b2s_decompress_sort_dev(uint32_t dev_index, uint32_t codec, uint32_t checksum_alg, uint32_t n,
                             const uint8_t* src_base, const uint64_t* src_off, const uint64_t* src_len,
                             const uint32_t* slice_base, const uint64_t* slice_len, const uint64_t* slice_checksum,
@@ -2356,20 +2737,8 @@ int b2s_decompress_sort_dev(uint32_t dev_index, uint32_t codec, uint32_t checksu
   rc = sort_args(codec, checksum_alg, n, src_off, src_len, slice_base, slice_len, slice_checksum, record_bytes, key_off,
                  key_len, src_base, dst_base, dst_cap, dst_total, n_records, status);
   if (rc || !n) return rc;
-  Lane& Ln = D->lane[kLaneRead];
-  std::lock_guard<std::mutex> lk(Ln.mtx);
-  Slot& S = Ln.slot[0];
-  SortBufferTrim trim{S};
-  uint64_t launches = 0, srcb = 0;
-  for (uint32_t i = 0; i < n; i++) srcb += src_len[i];
-  uint8_t* out = dst_base;
-  rc = decompress_sort_run(D, S, codec, checksum_alg, n, src_base, src_off, src_len, false, slice_base, slice_len,
-                           slice_checksum, record_bytes, key_off, key_len, &out, dst_cap, dst_total, n_records, status,
-                           bad_slice, &launches);
-  if (rc) return rc;
-  sort_timing(S, launches, srcb, *dst_total);
-  t_timing.total_ms = wt.ms();
-  return 0;
+  return sort_dev_run(D, codec, checksum_alg, n, src_base, src_off, src_len, slice_base, slice_len, slice_checksum,
+                      record_bytes, key_off, key_len, dst_base, dst_cap, dst_total, n_records, status, bad_slice, wt);
 }
 
 int b2s_decompress_sort_packed(uint32_t codec, uint32_t checksum_alg, uint32_t n, const uint8_t* src_base,
@@ -2387,47 +2756,243 @@ int b2s_decompress_sort_packed(uint32_t codec, uint32_t checksum_alg, uint32_t n
   rc = sort_args(codec, checksum_alg, n, src_off, src_len, slice_base, slice_len, slice_checksum, record_bytes, key_off,
                  key_len, src_base, dst_base, dst_cap, dst_total, n_records, status);
   if (rc || !n) return rc;
+  return sort_packed_run(D, codec, checksum_alg, n, src_base, src_off, src_len, slice_base, slice_len, slice_checksum,
+                         record_bytes, key_off, key_len, dst_base, dst_cap, dst_total, n_records, status, bad_slice,
+                         wt);
+}
+
+// ------------------------------------------------------------------------------------------------------------
+// exchange cache calls
+// ------------------------------------------------------------------------------------------------------------
+int b2s_exchange_set_budget(uint32_t dev_index, uint64_t bytes) {
+  int rc = exchange_ready();
+  if (rc) return rc;
+  Device* D;
+  if ((rc = get_device(dev_index, &D))) return rc;
+  std::vector<ExEntry*> dead;
+  {
+    std::lock_guard<std::mutex> lk(g_ex.mtx);
+    g_ex.budget[D->ordinal] = bytes;
+    ex_make_room(D->ordinal, 0, dead, true);
+    if (!bytes)  // off: every entry goes, a referenced one when its reader is done
+      for (auto it = g_ex.by_key.begin(); it != g_ex.by_key.end();) {
+        ExEntry* e = (it++)->second;
+        if (e->ordinal == D->ordinal) ex_unlink(e, dead);
+      }
+  }
+  ex_free(dead);
+  return 0;
+}
+
+int b2s_exchange_remove(int32_t shuffle_id, int64_t map_id) {
+  int rc = exchange_ready();
+  if (rc) return rc;
+  std::vector<ExEntry*> dead;
+  int removed = 0;
+  {
+    std::lock_guard<std::mutex> lk(g_ex.mtx);
+    for (auto it = g_ex.by_key.begin(); it != g_ex.by_key.end();) {
+      ExEntry* e = (it++)->second;
+      if (e->shuffle == shuffle_id && (map_id == -1 || e->map == map_id)) {
+        ex_unlink(e, dead);  // a referenced entry is freed by its last reader
+        removed++;
+      }
+    }
+  }
+  ex_free(dead);
+  return removed;
+}
+
+int b2s_exchange_lookup(int32_t shuffle_id, int32_t start_reduce, int32_t end_reduce, uint32_t n_maps,
+                        const int64_t* map_ids, uint64_t* len) {
+  int rc = reduce_range_args(start_reduce, end_reduce);
+  if (rc) return rc;
+  if (n_maps && (!map_ids || !len)) return fail(B2S_E_ARG, "null argument%s");
+  if ((rc = exchange_ready())) return rc;
+  Device* D;
+  if ((rc = get_device(t_device, &D))) return rc;
+  std::lock_guard<std::mutex> lk(g_ex.mtx);
+  int hits = 0;
+  for (uint32_t i = 0; i < n_maps; i++) {
+    len[i] = UINT64_MAX;
+    auto it = g_ex.by_key.find({shuffle_id, map_ids[i]});
+    if (it == g_ex.by_key.end() || it->second->ordinal != D->ordinal) continue;
+    const std::vector<uint64_t>& ps = it->second->part_start;
+    if ((uint64_t)end_reduce + 1 > ps.size())
+      return fail(B2S_E_ARG, "end_reduce exceeds the partitions of a cached map output%s");
+    len[i] = ps[(size_t)end_reduce] - ps[(size_t)start_reduce];
+    hits++;
+  }
+  return hits;
+}
+
+int b2s_exchange_read_packed(int32_t shuffle_id, int32_t start_reduce, int32_t end_reduce, uint32_t n_maps,
+                             const int64_t* map_ids, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_off,
+                             uint64_t* dst_len, uint64_t* dst_total, int32_t* status) {
+  WallTimer wt;
+  t_timing = b2s_timing{};
+  if (dst_total) *dst_total = 0;
+  int rc = reduce_range_args(start_reduce, end_reduce);
+  if (rc) return rc;
+  if (!dst_total || (n_maps && (!map_ids || !dst_off || !dst_len || !status)) || (dst_cap && !dst_base))
+    return fail(B2S_E_ARG, "null argument%s");
+  if ((rc = exchange_ready())) return rc;
+  Device* D;
+  if ((rc = get_device(t_device, &D))) return rc;
+  ExRefs refs(D->ordinal, shuffle_id, n_maps, map_ids, nullptr);
+  if ((rc = refs.check_range(end_reduce))) return rc;
+  std::vector<ExchangePiece> pieces;
+  uint64_t total = 0;
+  for (uint32_t i = 0; i < n_maps; i++) {
+    uint64_t len = 0;
+    if (refs.entry[i]) {
+      const uint8_t* src = refs.range(i, start_reduce, end_reduce, &len);
+      exchange_add_pieces(pieces, src, total, len);
+    }
+    status[i] = refs.entry[i] ? B2S_OK : B2S_E_NOT_CACHED;
+    dst_off[i] = total;
+    dst_len[i] = len;
+    total += len;
+  }
+  *dst_total = total;
+  if (total > dst_cap) return fail(B2S_E_DST_TOO_SMALL, "dst_cap is below the %s cached bytes", std::to_string(total).c_str());
   Lane& Ln = D->lane[kLaneRead];
   std::lock_guard<std::mutex> lk(Ln.mtx);
   Slot& S = Ln.slot[0];
   SortBufferTrim trim{S};
-  // one upload of every block, back to back (the whole task is resident at once: no chunking)
-  std::vector<uint64_t> dev_off(n);
-  uint64_t srcb = 0;
-  for (uint32_t i = 0; i < n; i++) {
-    dev_off[i] = srcb;
-    srcb += src_len[i];
-  }
-  if ((rc = S.src.ensure(srcb + 64))) return rc;
   cudaStream_t st = S.st;
-  CU(cudaEventRecord(S.ev_h0, st));
-  for (uint32_t i = 0; i < n;) {  // blocks adjacent in host memory go up in one copy
-    uint32_t j = i + 1;
-    while (j < n && src_off[j] == src_off[j - 1] + src_len[j - 1]) j++;
-    const uint64_t bytes = dev_off[j - 1] + src_len[j - 1] - dev_off[i];
-    if (bytes) CU(copy_async((uint8_t*)S.src.p + dev_off[i], src_base + src_off[i], bytes, cudaMemcpyHostToDevice, st));
-    i = j;
-  }
-  CU(cudaEventRecord(S.ev_h1, st));
   uint64_t launches = 0;
-  uint8_t* sorted = nullptr;
-  rc = decompress_sort_run(D, S, codec, checksum_alg, n, (const uint8_t*)S.src.p, dev_off.data(), src_len, true,
-                           slice_base, slice_len, slice_checksum, record_bytes, key_off, key_len, &sorted, dst_cap,
-                           dst_total, n_records, status, bad_slice, &launches);
-  if (rc) return rc;
-  const uint64_t down = *n_records ? *dst_total : 0;
+  if ((rc = S.dst.ensure(total + 64)) || (rc = S.xpieces.ensure(pieces.size() * sizeof(ExchangePiece) + 64)))
+    return rc;
+  CU(cudaEventRecord(S.ev_k0, st));
+  CU(cudaEventRecord(S.ev_t0, st));
+  if (!pieces.empty()) {
+    CU(cudaMemcpyAsync(S.xpieces.p, pieces.data(), pieces.size() * sizeof(ExchangePiece), cudaMemcpyHostToDevice, st));
+    launch_exchange_gather((const ExchangePiece*)S.xpieces.p, (uint32_t)pieces.size(), (uint8_t*)S.dst.p, st,
+                           &launches);
+  }
+  CU(cudaEventRecord(S.ev_t1, st));
+  CU(cudaEventRecord(S.ev_k1, st));
   CU(cudaEventRecord(S.ev_d0, st));
-  if (down) CU(copy_async(dst_base, sorted, down, cudaMemcpyDeviceToHost, st));
+  if (total) CU(copy_async(dst_base, S.dst.p, total, cudaMemcpyDeviceToHost, st));
   CU(cudaEventRecord(S.ev_d1, st));
   CU(cudaStreamSynchronize(st));
   CU(cudaGetLastError());
-  sort_timing(S, launches, srcb, *dst_total);
-  t_timing.h2d_ms = ms_between(S.ev_h0, S.ev_h1);
+  add_timing(S, false);
   t_timing.d2h_ms = ms_between(S.ev_d0, S.ev_d1);
-  t_timing.h2d_bytes = srcb;
-  t_timing.d2h_bytes = down;
+  t_timing.d2h_bytes = total;
+  t_timing.kernel_launches = launches;
+  t_timing.src_bytes = total;
+  t_timing.dst_bytes = total;
   t_timing.total_ms = wt.ms();
+  g_ctx->launches += launches;
   return 0;
+}
+
+// The sources of an exchange sorted read: the fetched ones compacted in source order with their slices (what
+// decompress_sort_run takes as its blocks), and every source in order.
+struct MixedSources {
+  std::vector<SortSource> src;
+  std::vector<uint64_t> off, len, slice_len, slice_sum;
+  std::vector<uint32_t> slice_base{0};
+};
+
+static int exchange_sort_args(int32_t start_reduce, int32_t end_reduce, const int64_t* map_ids, const uint8_t* cached,
+                              uint32_t codec, uint32_t alg, uint32_t n, const uint8_t* src_base,
+                              const uint64_t* src_off, const uint64_t* src_len, const uint32_t* slice_base,
+                              const uint64_t* slice_len, const uint64_t* slice_checksum, uint32_t record_bytes,
+                              uint32_t key_off, uint32_t key_len, const void* dst_base, uint64_t dst_cap,
+                              const uint64_t* dst_total, const uint64_t* n_records, const int32_t* status,
+                              MixedSources& M) {
+  int rc = reduce_range_args(start_reduce, end_reduce);
+  if (rc) return rc;
+  if (n && (!map_ids || !cached || !status)) return fail(B2S_E_ARG, "null argument%s");
+  M.src.resize(n);
+  for (uint32_t i = 0; i < n; i++) {
+    M.src[i].cached = cached[i] != 0;
+    if (M.src[i].cached) continue;
+    if (!src_off || !src_len) return fail(B2S_E_ARG, "null argument%s");
+    if (alg && (!slice_base || !slice_len || !slice_checksum)) return fail(B2S_E_ARG, "slice arrays required%s");
+    M.src[i].block = (uint32_t)M.off.size();
+    M.off.push_back(src_off[i]);
+    M.len.push_back(src_len[i]);
+    if (alg) {
+      if (slice_base[i + 1] < slice_base[i]) return fail(B2S_E_ARG, "slice_base must be non-decreasing%s");
+      M.slice_len.insert(M.slice_len.end(), slice_len + slice_base[i], slice_len + slice_base[i + 1]);
+      M.slice_sum.insert(M.slice_sum.end(), slice_checksum + slice_base[i], slice_checksum + slice_base[i + 1]);
+      M.slice_base.push_back((uint32_t)M.slice_len.size());
+    }
+  }
+  const uint32_t m = (uint32_t)M.off.size();
+  return sort_args(codec, alg, m, M.off.data(), M.len.data(), M.slice_base.data(), M.slice_len.data(),
+                   M.slice_sum.data(), record_bytes, key_off, key_len, src_base, dst_base, dst_cap, dst_total,
+                   n_records, status);
+}
+
+// references the cached sources of M on device D and describes them; B2S_E_ARG when a range exceeds an entry
+static int exchange_sort_sources(const ExRefs& refs, int32_t start_reduce, int32_t end_reduce, MixedSources& M) {
+  if (int rc = refs.check_range(end_reduce)) return rc;
+  for (uint32_t i = 0; i < (uint32_t)M.src.size(); i++) {
+    SortSource& s = M.src[i];
+    if (!s.cached) continue;
+    if (refs.entry[i]) s.src = refs.range(i, start_reduce, end_reduce, &s.len);
+    else s.status = B2S_E_NOT_CACHED;
+  }
+  return 0;
+}
+
+int b2s_exchange_read_sort_packed(int32_t shuffle_id, int32_t start_reduce, int32_t end_reduce, const int64_t* map_ids,
+                                  const uint8_t* cached, uint32_t codec, uint32_t checksum_alg, uint32_t n,
+                                  const uint8_t* src_base, const uint64_t* src_off, const uint64_t* src_len,
+                                  const uint32_t* slice_base, const uint64_t* slice_len,
+                                  const uint64_t* slice_checksum, uint32_t record_bytes, uint32_t key_off,
+                                  uint32_t key_len, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_total,
+                                  uint64_t* n_records, int32_t* status, int32_t* bad_slice) {
+  WallTimer wt;
+  t_timing = b2s_timing{};
+  if (dst_total) *dst_total = 0;
+  if (n_records) *n_records = 0;
+  MixedSources M;
+  int rc = exchange_sort_args(start_reduce, end_reduce, map_ids, cached, codec, checksum_alg, n, src_base, src_off,
+                              src_len, slice_base, slice_len, slice_checksum, record_bytes, key_off, key_len, dst_base,
+                              dst_cap, dst_total, n_records, status, M);
+  if (rc) return rc;
+  if ((rc = exchange_ready())) return rc;
+  Device* D;
+  if ((rc = get_device(t_device, &D)) || !n) return rc;
+  ExRefs refs(D->ordinal, shuffle_id, n, map_ids, cached);
+  if ((rc = exchange_sort_sources(refs, start_reduce, end_reduce, M))) return rc;
+  const uint32_t m = (uint32_t)M.off.size();
+  return sort_packed_run(D, codec, checksum_alg, m, src_base, M.off.data(), M.len.data(), M.slice_base.data(),
+                         M.slice_len.data(), M.slice_sum.data(), record_bytes, key_off, key_len, dst_base, dst_cap,
+                         dst_total, n_records, status, bad_slice, wt, &M.src);
+}
+
+int b2s_exchange_read_sort_dev(uint32_t dev_index, int32_t shuffle_id, int32_t start_reduce, int32_t end_reduce,
+                               const int64_t* map_ids, const uint8_t* cached, uint32_t codec, uint32_t checksum_alg,
+                               uint32_t n, const uint8_t* src_base, const uint64_t* src_off, const uint64_t* src_len,
+                               const uint32_t* slice_base, const uint64_t* slice_len, const uint64_t* slice_checksum,
+                               uint32_t record_bytes, uint32_t key_off, uint32_t key_len, uint8_t* dst_base,
+                               uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records, int32_t* status,
+                               int32_t* bad_slice) {
+  WallTimer wt;
+  t_timing = b2s_timing{};
+  if (dst_total) *dst_total = 0;
+  if (n_records) *n_records = 0;
+  MixedSources M;
+  int rc = exchange_sort_args(start_reduce, end_reduce, map_ids, cached, codec, checksum_alg, n, src_base, src_off,
+                              src_len, slice_base, slice_len, slice_checksum, record_bytes, key_off, key_len, dst_base,
+                              dst_cap, dst_total, n_records, status, M);
+  if (rc) return rc;
+  if ((rc = exchange_ready())) return rc;
+  Device* D;
+  if ((rc = get_device(dev_index, &D)) || !n) return rc;
+  ExRefs refs(D->ordinal, shuffle_id, n, map_ids, cached);
+  if ((rc = exchange_sort_sources(refs, start_reduce, end_reduce, M))) return rc;
+  const uint32_t m = (uint32_t)M.off.size();
+  return sort_dev_run(D, codec, checksum_alg, m, src_base, M.off.data(), M.len.data(), M.slice_base.data(),
+                      M.slice_len.data(), M.slice_sum.data(), record_bytes, key_off, key_len, dst_base, dst_cap,
+                      dst_total, n_records, status, bad_slice, wt, &M.src);
 }
 
 int b2s_decompressed_size_batch(uint32_t codec, uint32_t n, const uint8_t* const* src, const uint64_t* src_len,

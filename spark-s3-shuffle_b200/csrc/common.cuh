@@ -125,6 +125,30 @@ __device__ __forceinline__ void st_span16(uint8_t* p, int n, uint64_t lo, uint64
   if (n >= 1) *p = (uint8_t)lo;
 }
 
+// ---- the whole warp copies n bytes (any alignment): aligned 16-byte destination pieces, one per lane per step, sources
+// read with ld_span16 (read-only path: s must not be written while the kernel runs)
+__device__ __forceinline__ void warp_copy(uint8_t* d, const uint8_t* s, uint64_t n, uint32_t lane) {
+  uint64_t lo, hi;
+  uint32_t head = (uint32_t)((16u - (reinterpret_cast<uintptr_t>(d) & 15u)) & 15u);
+  if (head > n) head = (uint32_t)n;
+  if (lane == 0 && head) {
+    ld_span16<true>(s, (int)head, lo, hi);
+    st_span16(d, (int)head, lo, hi);
+  }
+  d += head;
+  s += head;
+  n -= head;
+  const uint64_t body = n & ~uint64_t(15);
+  for (uint64_t q = (uint64_t)lane * 16; q < body; q += 32 * 16) {
+    ld_span16<true>(s + q, 16, lo, hi);
+    *reinterpret_cast<ulonglong2*>(d + q) = make_ulonglong2(lo, hi);
+  }
+  if (lane == 0 && n > body) {
+    ld_span16<true>(s + body, (int)(n - body), lo, hi);
+    st_span16(d + body, (int)(n - body), lo, hi);
+  }
+}
+
 // ---- cooperative byte copy by a group of G lanes (lane in [0,G)), arbitrary alignment.
 // Fast path moves 16 bytes per lane per step with aligned 128-bit stores; source words are re-aligned with
 // funnel shifts so the loads stay aligned too.

@@ -3,6 +3,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <vector>
+
 #include "common.cuh"
 
 namespace b2s {
@@ -191,6 +193,20 @@ void launch_partition_gather(const uint8_t* rec_base, const uint32_t* d_rec_len,
 size_t key_sort_ws_bytes(uint64_t n, uint32_t key_len);
 void launch_key_sort(const uint8_t* d_rec, uint64_t n, uint32_t record_bytes, uint32_t key_off, uint32_t key_len,
                      uint8_t* d_ws, uint8_t* d_dst, cudaStream_t st, uint64_t* launches);
+
+// ---------------- exchange.cu (exchange-cache reads: ranges of device memory gathered into one arena) ----------------
+// piece: len bytes at src (device pointer, any alignment) go to d_dst + dst
+struct ExchangePiece {
+  const uint8_t* src;
+  uint64_t dst;
+  uint64_t len;
+};
+constexpr uint64_t kExchangePieceBytes = 32 << 10;
+// appends the range [src, src + len) -> dst, cut into pieces of at most kExchangePieceBytes
+void exchange_add_pieces(std::vector<ExchangePiece>& pieces, const uint8_t* src, uint64_t dst, uint64_t len);
+// one launch copies every piece (d_pieces: device copy of the pieces)
+void launch_exchange_gather(const ExchangePiece* d_pieces, uint32_t n, uint8_t* d_dst, cudaStream_t st,
+                            uint64_t* launches);
 
 // ---------------- gen.cu (bench utility) ----------------
 void launch_gen_terasort(uint8_t* d_dst, uint64_t first_record, uint64_t n_records, uint64_t seed, cudaStream_t st);

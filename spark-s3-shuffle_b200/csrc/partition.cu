@@ -157,29 +157,6 @@ __device__ __forceinline__ void lane_copy(uint8_t* __restrict__ d, const uint8_t
   }
 }
 
-// the whole warp copies n bytes: aligned 16-byte destination pieces, one per lane per step
-__device__ __forceinline__ void warp_copy(uint8_t* d, const uint8_t* s, uint64_t n, uint32_t lane) {
-  uint64_t lo, hi;
-  uint32_t head = (uint32_t)((16u - (reinterpret_cast<uintptr_t>(d) & 15u)) & 15u);
-  if (head > n) head = (uint32_t)n;
-  if (lane == 0 && head) {
-    ld_span16<true>(s, (int)head, lo, hi);
-    st_span16(d, (int)head, lo, hi);
-  }
-  d += head;
-  s += head;
-  n -= head;
-  const uint64_t body = n & ~uint64_t(15);
-  for (uint64_t q = (uint64_t)lane * 16; q < body; q += 32 * 16) {
-    ld_span16<true>(s + q, 16, lo, hi);
-    *reinterpret_cast<ulonglong2*>(d + q) = make_ulonglong2(lo, hi);
-  }
-  if (lane == 0 && n > body) {
-    ld_span16<true>(s + body, (int)(n - body), lo, hi);
-    st_span16(d + body, (int)(n - body), lo, hi);
-  }
-}
-
 // A warp takes 32 consecutive sorted records, so its stores land in one contiguous stretch of the arena.  Records up to
 // kLaneCopyMax bytes are copied by their own lane; longer ones afterwards by the whole warp, one at a time.
 __global__ void __launch_bounds__(kPartThreads) part_gather_kernel(const uint8_t* __restrict__ src,

@@ -152,6 +152,8 @@ class S3ShuffleDispatcher {
     gpuCodecBufferSize = (uint64_t)getSize("spark.shuffle.s3.gpu.codecBufferSize", 64L * 1024 * 1024);  // additive
     gpuReadBatchBlocks = getInt("spark.shuffle.s3.gpu.readBatchBlocks", 0);  // additive; 0 = all completed blocks
     gpuCoalesce = getBool("spark.shuffle.s3.gpu.coalesce", false);  // additive: group-commit the calls of concurrent task threads
+    // additive: per-device bytes of map outputs kept in HBM for reducers on the same device (INTEGRATION.md §3f); 0 = off
+    gpuExchangeCacheBytes = (uint64_t)std::max(0L, getSize("spark.shuffle.s3.gpu.exchangeCacheBytes", 0));
     if (!rootIsLocal && rootDir.find("://") != std::string::npos)
       throw UnsupportedOperationException("only file:// roots are implemented by the host mirror: " + rootDir);
   }
@@ -183,6 +185,17 @@ class S3ShuffleDispatcher {
       fs::remove_all(fs::path(shuffleDir(i, shuffleId)), ec);  // like the reference: failures are only logged
     }
   }
+  // the exchange-cache budget on every device, once the codec runtime is up (the writer stores, the reader looks up)
+  void applyExchangeBudget() {
+    std::call_once(exchangeBudgetSet_, [&] {
+      const int n = b2s_device_count();
+      for (int i = 0; i < n; i++) {
+        const int rc = b2s_exchange_set_budget((uint32_t)i, gpuExchangeCacheBytes);
+        if (rc != 0)
+          throw CodecException(std::string("b2s_exchange_set_budget: ") + b2s_strerror(rc) + ": " + b2s_last_error());
+      }
+    });
+  }
   int codecId() const {
     if (!shuffleCompress) return B2S_CODEC_NONE;
     if (codecName == "lz4" || codecName == "org.apache.spark.io.LZ4CompressionCodec") return B2S_CODEC_LZ4BLOCK;
@@ -201,6 +214,7 @@ class S3ShuffleDispatcher {
   uint64_t gpuCodecBufferSize = 64ull << 20;
   int gpuReadBatchBlocks = 0;
   bool gpuCoalesce = false;
+  uint64_t gpuExchangeCacheBytes = 0;
   CoalescingQueue queue;  // one per dispatcher = one per executor JVM (helper/S3ShuffleDispatcher.scala:240-254)
 
   // caches of S3ShuffleHelper (helper/S3ShuffleHelper.scala:15-16) live with the dispatcher instance here
@@ -230,6 +244,7 @@ class S3ShuffleDispatcher {
     return it == conf_.end() ? d : (it->second == "true" || it->second == "1");
   }
   std::map<std::string, std::string> conf_;
+  std::once_flag exchangeBudgetSet_;
 };
 
 // ---- S3ShuffleHelper (helper/S3ShuffleHelper.scala) ---------------------------------------------------------
@@ -513,9 +528,19 @@ class S3SerializedShuffleWriter {
     std::vector<uint64_t> doff(R), dlen(R), cks(R);
     std::vector<int32_t> status(R);
     uint64_t total = 0;
-    int rc = b2s_partition_compress_packed(codec, d_.zstdLevel, d_.lz4BlockSize, alg, R, recLen_.size(), records_.data(),
-                                           records_.size(), recLen_.data(), recPart_.data(), out_.data(), bound,
-                                           doff.data(), dlen.data(), &total, cks.data(), status.data());
+    int rc;
+    if (d_.gpuExchangeCacheBytes) {  // the same outputs, and the partitioned records stay in HBM for local reducers
+      d_.applyExchangeBudget();
+      int32_t cached = 0;
+      rc = b2s_partition_compress_cached_packed(shuffleId_, mapId_, codec, d_.zstdLevel, d_.lz4BlockSize, alg, R,
+                                                recLen_.size(), records_.data(), records_.size(), recLen_.data(),
+                                                recPart_.data(), out_.data(), bound, doff.data(), dlen.data(), &total,
+                                                cks.data(), status.data(), &cached);
+    } else {
+      rc = b2s_partition_compress_packed(codec, d_.zstdLevel, d_.lz4BlockSize, alg, R, recLen_.size(), records_.data(),
+                                         records_.size(), recLen_.data(), recPart_.data(), out_.data(), bound,
+                                         doff.data(), dlen.data(), &total, cks.data(), status.data());
+    }
     if (rc != 0)
       throw CodecException(std::string("b2s_partition_compress_packed: ") + b2s_strerror(rc) + ": " + b2s_last_error());
     std::vector<int64_t> lengths(R), checksums(R);
@@ -609,17 +634,22 @@ class S3SingleSpillShuffleMapOutputWriter {
 // call that decodes the block: verify first, then decompress, the reference's order (:99-110).
 struct ShuffleBlockInfo {
   BlockId id;
+  uint32_t mapPos = 0;  // index of the block's map in the reader's map list
   std::vector<uint64_t> sliceLen, sliceSum;
 };
 
 // computeShuffleBlocks (storage/S3ShuffleReader.scala:160-197, file-listing variant) + S3ShuffleBlockIterator
-// (storage/S3ShuffleBlockIterator.scala:36-43) + filterNot(maxBytes == 0) and the read metrics (:89-97)
+// (storage/S3ShuffleBlockIterator.scala:36-43) + filterNot(maxBytes == 0) and the read metrics (:89-97).  want (may be
+// nullptr = every map): the maps to fetch; the others are served from the exchange cache.
 static std::deque<S3BufferedPrefetchIterator::Source> computeShuffleBlockStreams(
     S3ShuffleDispatcher& d, int32_t shuffleId, const std::vector<int64_t>& mapIds, int32_t start, int32_t end,
-    bool batch, std::vector<ShuffleBlockInfo>& info, uint64_t& remoteBytesRead, uint64_t& remoteBlocksFetched) {
+    bool batch, std::vector<ShuffleBlockInfo>& info, uint64_t& remoteBytesRead, uint64_t& remoteBlocksFetched,
+    const std::vector<uint8_t>* want = nullptr) {
   std::deque<S3BufferedPrefetchIterator::Source> out;
   const bool verify = d.checksumEnabled;
-  for (int64_t mapId : mapIds) {
+  for (uint32_t pos = 0; pos < (uint32_t)mapIds.size(); pos++) {
+    if (want && !(*want)[pos]) continue;
+    const int64_t mapId = mapIds[pos];
     std::vector<int64_t> acc = S3ShuffleHelper::getPartitionLengths(d, shuffleId, mapId);
     if ((int)acc.size() < end + 1)
       throw SparkException("index of map " + std::to_string(mapId) + " has too few partitions");
@@ -635,6 +665,7 @@ static std::deque<S3BufferedPrefetchIterator::Source> computeShuffleBlockStreams
       remoteBytesRead += (uint64_t)(b - a);    // incRemoteBytesRead (:94)
       remoteBlocksFetched += 1;                // incRemoteBlocksFetched (:95)
       ShuffleBlockInfo bi;
+      bi.mapPos = pos;
       bi.id = (re - rs > 1) ? BlockId{BlockId::ShuffleBatch, shuffleId, mapId, rs, re}
                             : BlockId{BlockId::Shuffle, shuffleId, mapId, rs, re};
       if (verify && sums.size() < (size_t)re)  // a short or stale .checksum object (the reference: ArrayIndexOutOfBounds)
@@ -668,11 +699,15 @@ class S3ShuffleReader {
         batch_(doBatchFetch || d.forceBatchFetch) {}
   ~S3ShuffleReader() { iter_.reset(); }
 
-  // read(): storage/S3ShuffleReader.scala:77-110 — everything the task reads, drained batch by batch
+  // read(): storage/S3ShuffleReader.scala:77-110 — everything the task reads, drained batch by batch.  With the exchange
+  // cache on (INTEGRATION.md §3f) the maps resident on this thread's device come from it first, one block per map
+  // covering [start, end); only the others are fetched, and only their bytes count as remote bytes read.
   void read() {
-    open();
+    std::vector<uint8_t> fetch = cacheMisses();
     std::vector<Block> all;
     std::vector<std::unique_ptr<uint8_t[]>> bufs;
+    if (d_.codecId() != B2S_CODEC_NONE) readCached(fetch, all, bufs);  // codec "none" is refused by start() below
+    start(false, &fetch);
     while (nextBatch((size_t)d_.gpuReadBatchBlocks)) {
       all.insert(all.end(), blocks_.begin(), blocks_.end());
       for (auto& p : decoded_) bufs.push_back(std::move(p));
@@ -688,10 +723,137 @@ class S3ShuffleReader {
   // [keyOff, keyOff + keyLen) (INTEGRATION.md §3e): every non-empty block is fetched and staged, then ONE
   // b2s_decompress_sort_packed call verifies, decodes and key-sorts all of the task's records.  The blocks go in
   // computeShuffleBlocks order (map, then reduce id), so records with equal keys come out in that order whatever the
-  // order the fetches completed in.  Codec NONE (spark.shuffle.compress=false) is verified and sorted only.
+  // order the fetches completed in.  Codec NONE (spark.shuffle.compress=false) is verified and sorted only.  With the
+  // exchange cache on, a map resident on this thread's device is one cached source in that order instead of its blocks
+  // (b2s_exchange_read_sort_packed); maps the cache no longer holds when the call runs are fetched and the call repeated.
   void readSorted(uint32_t recordBytes, uint32_t keyOff, uint32_t keyLen) {
-    start(true);
+    std::vector<uint8_t> fetch = cacheMisses();
+    start(true, &fetch);
     std::vector<std::pair<uint64_t, std::vector<uint8_t>>> fetched;  // (tag, compressed bytes)
+    drainWhole(fetched);
+    const uint32_t M = (uint32_t)mapIds_.size();
+    const bool verify = d_.checksumEnabled;
+    const uint32_t alg = verify ? S3ShuffleHelper::createChecksumAlgorithm(d_.checksumAlgorithm) : 0;
+    ensure_codec_runtime();
+    const uint32_t codec = (uint32_t)d_.codecId();
+    while (true) {
+      std::sort(fetched.begin(), fetched.end(), [](const auto& a, const auto& b) { return a.first < b.first; });
+      std::vector<std::vector<uint32_t>> ofMap(M);  // the fetched blocks of each map, in reduce-id order
+      for (uint32_t k = 0; k < (uint32_t)fetched.size(); k++) ofMap[info_[fetched[k].first].mapPos].push_back(k);
+      std::vector<int64_t> ids;
+      std::vector<uint8_t> cached;
+      std::vector<uint64_t> off, len, tags, sliceLen, sliceSum;
+      std::vector<uint32_t> sliceBase(1, 0), mapOf, from;  // from: the source's entry of `fetched`
+      uint64_t bytes = 0;
+      for (uint32_t m = 0; m < M; m++) {
+        if (!fetch[m]) {
+          ids.push_back(mapIds_[m]);
+          cached.push_back(1);
+          off.push_back(bytes);
+          len.push_back(0);
+          tags.push_back(~0ull);
+          from.push_back(0);
+          mapOf.push_back(m);
+          sliceBase.push_back((uint32_t)sliceLen.size());
+          continue;
+        }
+        for (uint32_t k : ofMap[m]) {
+          const ShuffleBlockInfo& bi = info_[fetched[k].first];
+          ids.push_back(mapIds_[m]);
+          cached.push_back(0);
+          off.push_back(bytes);
+          len.push_back(fetched[k].second.size());
+          tags.push_back(fetched[k].first);
+          from.push_back(k);
+          mapOf.push_back(m);
+          bytes += len.back();
+          sliceLen.insert(sliceLen.end(), bi.sliceLen.begin(), bi.sliceLen.end());
+          sliceSum.insert(sliceSum.end(), bi.sliceSum.begin(), bi.sliceSum.end());
+          sliceBase.push_back((uint32_t)sliceLen.size());
+        }
+      }
+      const uint32_t n = (uint32_t)ids.size();
+      PinnedArena src;
+      src.resize(bytes ? bytes : 1);
+      for (uint32_t k = 0; k < n; k++)
+        if (!cached[k]) memcpy(src.data() + off[k], fetched[from[k]].second.data(), (size_t)len[k]);
+      uint64_t cachedBytes = 0;
+      if (std::find(cached.begin(), cached.end(), 1) != cached.end()) {
+        std::vector<uint64_t> hitLen(n);
+        const int rc = b2s_exchange_lookup(shuffleId_, start_, end_, n, ids.data(), hitLen.data());
+        if (rc < 0) throw CodecException(std::string("b2s_exchange_lookup: ") + b2s_strerror(rc) + ": " + b2s_last_error());
+        for (uint32_t k = 0; k < n; k++)
+          if (cached[k] && hitLen[k] != UINT64_MAX) cachedBytes += hitLen[k];
+      }
+      // Output size: codec NONE decodes to the stored bytes.  For a codec, a first guess of 4x the compressed bytes (the
+      // pages of the untouched tail are never faulted in); a call it is too small for ends after verification with the
+      // bytes needed in `total`, and the one retry uses exactly that.
+      uint64_t cap = (codec == B2S_CODEC_NONE ? bytes : bytes * 4) + cachedBytes;
+      std::vector<int32_t> status(n), bad(n);
+      uint64_t total = 0, records = 0;
+      int rc = B2S_E_DST_TOO_SMALL;
+      for (int attempt = 0; attempt < 2 && rc == B2S_E_DST_TOO_SMALL; attempt++) {
+        if (attempt) cap = total;
+        sorted_.reset(new uint8_t[(size_t)(cap ? cap : 1)]);
+        if (fetch == std::vector<uint8_t>(M, 1))
+          rc = b2s_decompress_sort_packed(codec, alg, n, src.data(), off.data(), len.data(),
+                                          verify ? sliceBase.data() : nullptr, verify ? sliceLen.data() : nullptr,
+                                          verify ? sliceSum.data() : nullptr, recordBytes, keyOff, keyLen, sorted_.get(),
+                                          cap, &total, &records, status.data(), bad.data());
+        else
+          rc = b2s_exchange_read_sort_packed(shuffleId_, start_, end_, ids.data(), cached.data(), codec, alg, n,
+                                             src.data(), off.data(), len.data(), verify ? sliceBase.data() : nullptr,
+                                             verify ? sliceLen.data() : nullptr, verify ? sliceSum.data() : nullptr,
+                                             recordBytes, keyOff, keyLen, sorted_.get(), cap, &total, &records,
+                                             status.data(), bad.data());
+      }
+      if (rc != 0)
+        throw CodecException(std::string("b2s_decompress_sort_packed: ") + b2s_strerror(rc) + ": " + b2s_last_error());
+      std::vector<uint8_t> late(M, 0);  // maps evicted between the lookup and the call: fetch them, then sort again
+      for (uint32_t k = 0; k < n; k++)
+        if (status[k] == B2S_E_NOT_CACHED) late[mapOf[k]] = fetch[mapOf[k]] = 1;
+      if (std::find(late.begin(), late.end(), 1) != late.end()) {
+        auto more = computeShuffleBlockStreams(d_, shuffleId_, mapIds_, start_, end_, batch_, info_, remoteBytesRead_,
+                                               remoteBlocksFetched_, &late);
+        iter_.reset(new S3BufferedPrefetchIterator(std::move(more), d_.maxBufferSizeTask, d_.maxConcurrencyTask));
+        drainWhole(fetched);
+        continue;
+      }
+      for (uint32_t k = 0; k < n; k++) {
+        const BlockId id = cached[k] ? cachedBlockId(ids[k]) : info_[tags[k]].id;
+        if (status[k] == B2S_E_CHECKSUM)  // storage/S3ChecksumValidationStream.scala:72-74
+          throw SparkException("Invalid checksum detected for " + id.name());
+        if (status[k] == B2S_E_CORRUPT) throw IOException("Stream is corrupted");
+        if (status[k] != 0) throw IOException(std::string("decompress failed: ") + b2s_strerror(status[k]));
+      }
+      sortedLen_ = total;
+      sortedRecords_ = records;
+      return;
+    }
+  }
+  const uint8_t* sortedData() const { return sorted_.get(); }
+  uint64_t sortedLen() const { return sortedLen_; }
+  uint64_t sortedRecords() const { return sortedRecords_; }
+
+  // want (nullptr = every map): the maps whose blocks are fetched
+  void start(bool allowNone, const std::vector<uint8_t>* want = nullptr) {
+    iter_.reset();
+    info_.clear();
+    blocks_.clear();
+    decoded_.clear();
+    sorted_.reset();
+    sortedLen_ = sortedRecords_ = 0;
+    remoteBytesRead_ = remoteBlocksFetched_ = 0;
+    batches_ = 0;
+    if (!allowNone && d_.codecId() == B2S_CODEC_NONE)
+      throw UnsupportedOperationException("spark.shuffle.compress=false is served by the stock reader path");
+    auto src = computeShuffleBlockStreams(d_, shuffleId_, mapIds_, start_, end_, batch_, info_, remoteBytesRead_,
+                                          remoteBlocksFetched_, want);
+    iter_.reset(new S3BufferedPrefetchIterator(std::move(src), d_.maxBufferSizeTask, d_.maxConcurrencyTask));
+  }
+
+  // every block the prefetcher delivers, whole, appended to `fetched` as (tag, bytes)
+  void drainWhole(std::vector<std::pair<uint64_t, std::vector<uint8_t>>>& fetched) {
     while (iter_->hasNext()) {
       for (auto& f : iter_->nextBatch(0)) {
         auto& st = *f.stream;
@@ -707,73 +869,65 @@ class S3ShuffleReader {
       batches_++;
     }
     stats_ = iter_->statistics();
-    std::sort(fetched.begin(), fetched.end(), [](const auto& a, const auto& b) { return a.first < b.first; });
-    const uint32_t n = (uint32_t)fetched.size();
-    const bool verify = d_.checksumEnabled;
-    const uint32_t alg = verify ? S3ShuffleHelper::createChecksumAlgorithm(d_.checksumAlgorithm) : 0;
-    std::vector<uint64_t> off(n), len(n), tags(n), sliceLen, sliceSum;
-    std::vector<uint32_t> sliceBase(n + 1, 0);
-    uint64_t bytes = 0;
-    for (uint32_t k = 0; k < n; k++) {
-      tags[k] = fetched[k].first;
-      off[k] = bytes;
-      len[k] = fetched[k].second.size();
-      bytes += len[k];
-      const ShuffleBlockInfo& bi = info_[fetched[k].first];
-      sliceLen.insert(sliceLen.end(), bi.sliceLen.begin(), bi.sliceLen.end());
-      sliceSum.insert(sliceSum.end(), bi.sliceSum.begin(), bi.sliceSum.end());
-      sliceBase[k + 1] = (uint32_t)sliceLen.size();
-    }
-    PinnedArena src;
-    src.resize(bytes ? bytes : 1);
-    for (uint32_t k = 0; k < n; k++) memcpy(src.data() + off[k], fetched[k].second.data(), (size_t)len[k]);
-    fetched.clear();
+  }
+
+  // 1 for each map to fetch: every map, or, with the exchange cache on, those not resident on this thread's device
+  std::vector<uint8_t> cacheMisses() {
+    std::vector<uint8_t> fetch(mapIds_.size(), 1);
+    if (!d_.gpuExchangeCacheBytes || mapIds_.empty()) return fetch;
     ensure_codec_runtime();
-    const uint32_t codec = (uint32_t)d_.codecId();
-    // Output size: codec NONE decodes to the stored bytes.  For a codec, a first guess of 4x the compressed bytes (the
-    // pages of the untouched tail are never faulted in); a call it is too small for ends after verification with the
-    // bytes needed in `total`, and the one retry uses exactly that.
-    uint64_t cap = codec == B2S_CODEC_NONE ? bytes : bytes * 4;
-    std::vector<int32_t> status(n), bad(n);
-    uint64_t total = 0, records = 0;
-    int rc = B2S_E_DST_TOO_SMALL;
-    for (int attempt = 0; attempt < 2 && rc == B2S_E_DST_TOO_SMALL; attempt++) {
+    std::vector<uint64_t> len(mapIds_.size());
+    const int rc = b2s_exchange_lookup(shuffleId_, start_, end_, (uint32_t)mapIds_.size(), mapIds_.data(), len.data());
+    if (rc < 0) throw CodecException(std::string("b2s_exchange_lookup: ") + b2s_strerror(rc) + ": " + b2s_last_error());
+    for (size_t m = 0; m < len.size(); m++) fetch[m] = len[m] == UINT64_MAX;
+    return fetch;
+  }
+  BlockId cachedBlockId(int64_t mapId) const {
+    return end_ - start_ > 1 ? BlockId{BlockId::ShuffleBatch, shuffleId_, mapId, start_, end_}
+                             : BlockId{BlockId::Shuffle, shuffleId_, mapId, start_, start_ + 1};
+  }
+
+  // the maps not in `fetch`, from the exchange cache in one b2s_exchange_read_packed call: one block per map covering
+  // [start, end) (empty ones dropped, as the fetch path drops empty blocks).  Maps it no longer holds go back to `fetch`.
+  void readCached(std::vector<uint8_t>& fetch, std::vector<Block>& all, std::vector<std::unique_ptr<uint8_t[]>>& bufs) {
+    std::vector<int64_t> ids;
+    std::vector<uint32_t> pos;
+    for (uint32_t m = 0; m < (uint32_t)mapIds_.size(); m++)
+      if (!fetch[m]) {
+        ids.push_back(mapIds_[m]);
+        pos.push_back(m);
+      }
+    if (ids.empty()) return;
+    const uint32_t n = (uint32_t)ids.size();
+    std::vector<uint64_t> off(n), len(n);
+    std::vector<int32_t> status(n);
+    int rc = b2s_exchange_lookup(shuffleId_, start_, end_, n, ids.data(), len.data());
+    if (rc < 0) throw CodecException(std::string("b2s_exchange_lookup: ") + b2s_strerror(rc) + ": " + b2s_last_error());
+    uint64_t cap = 0, total = 0;
+    for (uint64_t l : len) cap += l == UINT64_MAX ? 0 : l;
+    std::unique_ptr<uint8_t[]> buf;
+    rc = B2S_E_DST_TOO_SMALL;
+    for (int attempt = 0; attempt < 2 && rc == B2S_E_DST_TOO_SMALL; attempt++) {  // an entry stored again may have grown
       if (attempt) cap = total;
-      sorted_.reset(new uint8_t[(size_t)(cap ? cap : 1)]);
-      rc = b2s_decompress_sort_packed(codec, alg, n, src.data(), off.data(), len.data(), verify ? sliceBase.data() : nullptr,
-                                      verify ? sliceLen.data() : nullptr, verify ? sliceSum.data() : nullptr, recordBytes,
-                                      keyOff, keyLen, sorted_.get(), cap, &total, &records, status.data(), bad.data());
+      buf.reset(new uint8_t[(size_t)(cap ? cap : 1)]);
+      rc = b2s_exchange_read_packed(shuffleId_, start_, end_, n, ids.data(), buf.get(), cap, off.data(), len.data(),
+                                    &total, status.data());
     }
     if (rc != 0)
-      throw CodecException(std::string("b2s_decompress_sort_packed: ") + b2s_strerror(rc) + ": " + b2s_last_error());
+      throw CodecException(std::string("b2s_exchange_read_packed: ") + b2s_strerror(rc) + ": " + b2s_last_error());
     for (uint32_t k = 0; k < n; k++) {
-      const BlockId& id = info_[tags[k]].id;
-      if (status[k] == B2S_E_CHECKSUM)  // storage/S3ChecksumValidationStream.scala:72-74
-        throw SparkException("Invalid checksum detected for " + id.name());
-      if (status[k] == B2S_E_CORRUPT) throw IOException("Stream is corrupted");
-      if (status[k] != 0) throw IOException(std::string("decompress failed: ") + b2s_strerror(status[k]));
+      if (status[k] != B2S_OK) {
+        fetch[pos[k]] = 1;
+        continue;
+      }
+      if (!len[k]) continue;
+      Block blk;
+      blk.id = cachedBlockId(ids[k]);
+      blk.data = buf.get() + off[k];
+      blk.len = len[k];
+      all.push_back(blk);
     }
-    sortedLen_ = total;
-    sortedRecords_ = records;
-  }
-  const uint8_t* sortedData() const { return sorted_.get(); }
-  uint64_t sortedLen() const { return sortedLen_; }
-  uint64_t sortedRecords() const { return sortedRecords_; }
-
-  void start(bool allowNone) {
-    iter_.reset();
-    info_.clear();
-    blocks_.clear();
-    decoded_.clear();
-    sorted_.reset();
-    sortedLen_ = sortedRecords_ = 0;
-    remoteBytesRead_ = remoteBlocksFetched_ = 0;
-    batches_ = 0;
-    if (!allowNone && d_.codecId() == B2S_CODEC_NONE)
-      throw UnsupportedOperationException("spark.shuffle.compress=false is served by the stock reader path");
-    auto src = computeShuffleBlockStreams(d_, shuffleId_, mapIds_, start_, end_, batch_, info_, remoteBytesRead_,
-                                          remoteBlocksFetched_);
-    iter_.reset(new S3BufferedPrefetchIterator(std::move(src), d_.maxBufferSizeTask, d_.maxConcurrencyTask));
+    bufs.push_back(std::move(buf));
   }
 
   // SURVEY.md §8(f)-2: drain the blocks the prefetcher has completed, verify + decode them in ONE C-ABI batch, give
@@ -964,6 +1118,8 @@ int b2sh_dispatcher_remove_shuffle(b2sh_dispatcher* d, int32_t shuffle_id) {
   return guarded([&] {
     d->d->removeShuffle(shuffle_id);
     S3ShuffleHelper::purgeCachedDataForShuffle(*d->d, shuffle_id);
+    // the map outputs kept in HBM go too (without a device or before b2s_init nothing was cached: nothing to do)
+    if (d->d->gpuExchangeCacheBytes) (void)b2s_exchange_remove(shuffle_id, -1);
   });
 }
 int b2sh_helper_checksum_algorithm(const char* name) {
