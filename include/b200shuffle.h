@@ -161,7 +161,9 @@ int b2s_partition_compress_dev(uint32_t dev_index, uint32_t codec, int32_t level
  * storage/S3ChecksumValidationStream.scala:22-27); slice_len[i][k] / slice_checksum[i][k] are the .index differences and
  * .checksum values of those partitions.  With checksum_alg != 0 every slice is verified over the compressed bytes
  * before decoding; a mismatch yields status[i] = B2S_E_CHECKSUM and bad_slice[i] = k (may be NULL).
- * n_slices / slice_* may be NULL when checksum_alg == 0. */
+ * n_slices / slice_* may be NULL when checksum_alg == 0.
+ * A block whose status is not B2S_OK leaves the bytes of its own output range unspecified (the decoder may have
+ * written part of it before it met the corruption); the output ranges of the other blocks are never touched by it. */
 int b2s_decompress_batch(uint32_t codec, uint32_t checksum_alg, uint32_t n, const uint8_t* const* src,
                          const uint64_t* src_len, const uint32_t* n_slices, const uint64_t* const* slice_len,
                          const uint64_t* const* slice_checksum, uint8_t* const* dst, const uint64_t* dst_cap,

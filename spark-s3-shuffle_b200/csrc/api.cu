@@ -56,7 +56,7 @@ uint64_t g_host_chunk_bytes = 256ull << 20;  // host-pointer calls: bytes per pi
 constexpr uint32_t kChunkStreams = 1u << 18;
 constexpr uint32_t kXxhSeed = 0x9747b28cu;
 uint32_t g_lz4_chunk_blocks = 32768;  // codec blocks per match/parse/emit (or tokens/copy) pass: bounds the workspace; B2S_LZ4_CHUNK_BLOCKS
-uint32_t g_lz4d_chunk_blocks = 65536;  // decode side: the token walk is latency bound, more blocks per launch = more loads in flight; B2S_LZ4D_CHUNK_BLOCKS
+uint32_t g_lz4d_chunk_blocks = 65536;  // Snappy decode only (LZ4 decodes in one launch): codec blocks per token walk + copy pair; the walk is latency bound, more blocks per launch = more loads in flight; B2S_LZ4D_CHUNK_BLOCKS
 int g_lz4d_legacy = 0;
 int g_trace = 0;  // B2S_TRACE=1: per-chunk timeline of the compress pipeline on stderr  // B2S_LZ4D_LEGACY=1: single-kernel tile decoder for every block size (A/B comparisons)
 
@@ -694,13 +694,20 @@ int decompress_enqueue_b(Slot& S, DecompressJob& J, const uint8_t* d_src, uint8_
   const bool small_blocks = max_olen <= 65536 && max_clen < 65536;
   if (J.codec == B2S_CODEC_SNAPPY_XERIAL && !small_blocks)
     return fail(B2S_E_UNSUPPORTED, "snappy chunks larger than 64 KiB are not supported%s");
-  if (J.nb && small_blocks && (J.codec == B2S_CODEC_SNAPPY_XERIAL || !g_lz4d_legacy)) {
+  if (J.nb && small_blocks && J.codec == B2S_CODEC_LZ4BLOCK && !g_lz4d_legacy) {
+    // one launch over every codec block: warp per block, parse and copies together (lz4_decode.cu)
+    cudaEvent_t e0 = nullptr, e1 = nullptr;
+    S.dom_pair(&e0, &e1);
+    CU(cudaEventRecord(e0, st));
+    launch_lz4_decode_warp(desc, (uint32_t)J.nb, d_src, d_dst, J.status, J.counter, st, launches);
+    CU(cudaEventRecord(e1, st));
+  } else if (J.nb && small_blocks && J.codec == B2S_CODEC_SNAPPY_XERIAL) {
     // tokens (thread per block) + copy (lane per sequence), in chunks that bound the record workspace
     const uint32_t nb = (uint32_t)J.nb;
-    const uint32_t rec_stride = lz4_decode_rec_stride(J.codec, (uint32_t)max_olen, (uint32_t)max_clen);
+    const uint32_t rec_stride = snappy_decode_rec_stride((uint32_t)max_clen);
     const uint32_t chunk = std::min<uint32_t>(nb, g_lz4d_chunk_blocks);
     const size_t nrec_bytes = align_up((size_t)nb * 4, 256);
-    const size_t ws_bytes = align_up(lz4_decode_ws_bytes(chunk, rec_stride), 256);
+    const size_t ws_bytes = align_up(snappy_decode_ws_bytes(chunk, rec_stride), 256);
     rc = S.scratch.ensure(nrec_bytes + ws_bytes * (nb > chunk ? 2 : 1));
     if (rc) return rc;
     uint32_t* nrec = (uint32_t*)S.scratch.p;
@@ -719,7 +726,8 @@ int decompress_enqueue_b(Slot& S, DecompressJob& J, const uint8_t* d_src, uint8_
         cudaEventCreate(&q1);
         CU(cudaEventRecord(q0, S.st2));
       }
-      launch_lz4_tokens(J.codec, desc, b0, m, rec_stride, d_src, ws, nrec, J.status, S.st2, launches);
+      launch_snappy_tokens(desc, b0, m, d_src, reinterpret_cast<uint2*>(ws), rec_stride, nrec, J.status, S.st2,
+                           launches);
       if (q1) CU(cudaEventRecord(q1, S.st2));
       CU(cudaEventRecord(S.ev_match[par], S.st2));
       CU(cudaStreamWaitEvent(st, S.ev_match[par], 0));
@@ -1116,7 +1124,6 @@ int b2s_init(uint32_t gpu_mask, uint64_t pinned_bytes_per_gpu, uint32_t streams_
   g_lz4_hlog = env_int("B2S_LZ4_HLOG", g_lz4_hlog);
   g_lz4d_tile = env_int("B2S_LZ4D_TILE", g_lz4d_tile);
   g_lz4_pipe = env_int("B2S_LZ4_PIPE", g_lz4_pipe);
-  g_lz4d_tokens = env_int("B2S_LZ4D_TOKENS", g_lz4d_tokens);
   g_lz4_chunk_blocks = (uint32_t)std::max(1, env_int("B2S_LZ4_CHUNK_BLOCKS", (int)g_lz4_chunk_blocks));
   g_lz4d_legacy = env_int("B2S_LZ4D_LEGACY", 0);
   g_trace = env_int("B2S_TRACE", 0);

@@ -44,7 +44,7 @@ void launch_xxh32_verify(const BlockDesc* d_desc, uint32_t n_blocks, const uint8
                          uint32_t mask, int32_t* d_status, cudaStream_t st, uint64_t* launches);
 
 // ---------------- lz4_compress.cu (K3: match / parse / emit + write-side LZ4Block framing) ----------------
-extern int g_lz4_hlog, g_lz4d_tile, g_lz4_pipe, g_lz4d_tokens;
+extern int g_lz4_hlog, g_lz4d_tile, g_lz4_pipe;
 // bytes of workspace for one pass over `chunk_blocks` codec blocks (off u16 + ml8 u8 per position, 8-byte records)
 size_t lz4_compress_ws_bytes(uint32_t chunk_blocks, uint32_t block_size, uint32_t codec);
 // Codec blocks [b0, b0+m) of the batch, in two halves that may run on different streams (d_ws is handed from one to
@@ -82,18 +82,20 @@ void launch_lz4block_fill(const uint8_t* src_base, const uint64_t* d_src_off, co
 void launch_lz4_decompress(const BlockDesc* d_desc, uint32_t n_blocks, const uint8_t* src_base, uint8_t* dst_base,
                            int32_t* d_status, unsigned int* d_counter, cudaStream_t st, uint64_t* launches);
 
-// ---------------- lz4_decode.cu (K4: tokens + copy; codec blocks <= 64 KiB; the copy kernel also serves Snappy) ------
-uint32_t lz4_decode_rec_stride(uint32_t codec, uint32_t max_olen, uint32_t max_clen);
-size_t lz4_decode_ws_bytes(uint32_t chunk_blocks, uint32_t rec_stride);
-// codec blocks [b0, b0+m): launch_lz4_tokens writes per-sequence records into d_ws (LZ4 or Snappy element grammar;
-// malformed blocks set status[stream] = B2S_E_CORRUPT), launch_lz4_copy performs the byte copies from them.  d_nrec is
-// indexed by global block id.  Two calls so that the token walk of chunk k+1 can run beside the copies of chunk k.
-void launch_lz4_tokens(uint32_t codec, const BlockDesc* d_desc, uint32_t b0, uint32_t m, uint32_t rec_stride,
-                       const uint8_t* src_base, uint8_t* d_ws, uint32_t* d_nrec, int32_t* d_status, cudaStream_t st,
-                       uint64_t* launches);
+// ---------------- lz4_decode.cu (K4: LZ4 codec blocks <= 64 KiB; the copy kernel of the Snappy decoder) ------
+// Snappy record workspace: records per codec block, and bytes for chunk_blocks codec blocks
+uint32_t snappy_decode_rec_stride(uint32_t max_clen);
+size_t snappy_decode_ws_bytes(uint32_t chunk_blocks, uint32_t rec_stride);
+// codec blocks [b0, b0+m): the byte copies from the per-sequence records of launch_snappy_tokens in d_ws (d_nrec is
+// indexed by global block id).  A separate launch so that the token walk of chunk k+1 can run beside the copies of
+// chunk k.
 void launch_lz4_copy(const BlockDesc* d_desc, uint32_t b0, uint32_t m, uint32_t rec_stride, const uint8_t* src_base,
                      uint8_t* dst_base, const uint8_t* d_ws, const uint32_t* d_nrec, cudaStream_t st,
                      uint64_t* launches);
+// LZ4 codec blocks [0, nb) in one launch, a warp per block (parse + copies; malformed blocks set status[stream] =
+// B2S_E_CORRUPT).  d_counter: one device word of scratch.
+void launch_lz4_decode_warp(const BlockDesc* d_desc, uint32_t nb, const uint8_t* src_base, uint8_t* dst_base,
+                            int32_t* d_status, unsigned int* d_counter, cudaStream_t st, uint64_t* launches);
 
 // ---------------- snappy.cu (K5: xerial framing, Snappy emit / tokens; match, parse and copy kernels are shared) ------
 void launch_snappy_emit(const uint8_t* src_base, const uint64_t* d_src_off, const uint64_t* d_src_len,

@@ -1,264 +1,45 @@
-// lz4_decode.cu — K4: LZ4 block decompression as two kernels (LZ4_decompress_fast semantics: driven by originalLen,
-// must consume exactly compressedLen; oracle: orc_lz4_decompress_block).
+// lz4_decode.cu — K4: LZ4 block decompression (LZ4_decompress_fast semantics: driven by originalLen, must consume
+// exactly compressedLen; oracle: orc_lz4_decompress_block), and the copy kernel of the Snappy decoder.
 //
 // Replaces liblz4's LZ4_decompress_fast as driven by lz4-java's LZ4BlockInputStream [U] under
 // serializerManager.wrapStream at storage/S3ShuffleReader.scala:107-109.
 //
-// Same split as the compressor (lz4_compress.cu): the token chain of a block is inherently serial, the byte copies
-// are not.  The first, single-kernel decoder (kept below in lz4.cu as the path for codec blocks > 64 KiB) carried the
-// serial chain on 8-lane tiles and spent several warp-instructions per output byte.
-//
-//   P1 lz4_tokens_kernel  THREAD per codec block: walks tokens / length bytes / offsets, validates every bound the
-//                         JVM reader would trip over, and writes one 8-byte record per sequence
-//                         (literal count, match length, offset, literal source position).
-//   P2 lz4_copy_kernel    warp per codec block, LANE per sequence: output positions by a warp scan, all literals of a
-//                         batch of 32 sequences copied at once, then the matches in dependency rounds — a match is
-//                         ready when its source lies entirely below the output of the earliest unfinished match;
-//                         short matches are copied by their lanes, long ones by the whole warp.
+//   lz4_decode_warp_kernel  WARP per LZ4 codec block (<= 64 KiB), persistent grid: the token chain is resolved 32
+//                           sequences at a time by pointer doubling over speculative headers in a 128-byte window,
+//                           then the batch's literals and matches are copied as in the copy kernel.  Nothing goes
+//                           through HBM between parse and copy.  (The first, single-kernel decoder in lz4.cu carried
+//                           the serial chain on 8-lane tiles; it stays the path for codec blocks > 64 KiB.)
+//   lz4_copy_kernel         Snappy: warp per codec block, LANE per sequence, from the records of snappy_tokens_kernel
+//                           (snappy.cu): output positions by a warp scan, all literals of a batch of 32 sequences at
+//                           once, then the matches in dependency rounds (lz_batch.cuh).
 #include "kernels.h"
 #include "lz_batch.cuh"
-#include "tma_ring.cuh"
 
 namespace b2s {
 
 constexpr int kMinMatch = 4, kMFLimit = 12, kLastLiterals = 5;
-int g_lz4d_tokens = 1;  // B2S_LZ4D_TOKENS: 1 = global loads + L1 prefetch, 2 = TMA ring (tma_ring.cuh)
 
-// record: x = literal count | match length << 16 (0 = final sequence) ; y = offset | literal source position << 16
-__global__ void __launch_bounds__(64) lz4_tokens_kernel(const BlockDesc* __restrict__ desc, uint32_t b0, uint32_t m,
-                                                        const uint8_t* __restrict__ src_base, uint2* __restrict__ rec,
-                                                        uint32_t rec_stride, uint32_t* __restrict__ nrec,
-                                                        int32_t* __restrict__ status) {
-  const uint32_t bl = blockIdx.x * blockDim.x + threadIdx.x;
-  if (bl >= m) return;
-  const uint32_t b = b0 + bl;
-  const BlockDesc d = desc[b];
-  if (d.olen == 0 || (d.stream & 0x80000000u)) {  // no-op descriptor or stored RAW (copied by P2)
-    nrec[b] = 0;
-    return;
+// The literals of a batch of up to 32 sequences (lane l: lit bytes from in + lip to out + op; lit == 0: none): all
+// lanes at once, runs longer than 16 bytes by the whole warp.  Ends with __syncwarp, so the literals are visible to the
+// match copies that follow.
+__device__ __forceinline__ void lz_copy_literals(const uint8_t* __restrict__ in, uint8_t* out, int lip, int lit, int op,
+                                                 int lane) {
+  constexpr unsigned FULL = 0xffffffffu;
+  if (lit > 0 && lit <= 16) {  // aligned 8-byte words of the compressed block (read-only: __ldg)
+    uint64_t lo, hi;
+    ld_span16<true>(in + lip, lit, lo, hi);
+    st_span16(out + op, lit, lo, hi);
   }
-  const uint8_t* __restrict__ in = src_base + d.src;
-  const int clen = (int)d.clen, olen = (int)d.olen;
-  uint2* __restrict__ r = rec + (size_t)bl * rec_stride;
-  int ip = 0, op = 0;
-  uint32_t ns = 0;
-  bool err = false;
-  int pf_sector = -1;
-  for (int k = 64; k < 512 && k < clen; k += 64) asm volatile("prefetch.global.L1 [%0];" ::"l"(in + k));
-  // The token chain is what bounds this kernel (one dependent L1 round trip per field).  Every sequence therefore
-  // starts with ONE 8-byte window read at ip — three independent aligned word loads — which holds the token, and for
-  // the common short sequence (literals <= 5) also the offset: one round trip instead of two or three.
-  const uintptr_t a0 = reinterpret_cast<uintptr_t>(in);
-  while (true) {
-    if (ip >= clen) {
-      err = true;
-      break;
-    }
-    if ((ip >> 5) != pf_sector) {  // entering a new 32-byte sector: pull the sector 16 ahead towards L1/L2 now
-      pf_sector = ip >> 5;
-      if (ip + 512 < clen) asm volatile("prefetch.global.L1 [%0];" ::"l"(in + ip + 512));
-    }
-    // window: bytes ip .. ip+7 (only aligned words that contain bytes of the block are read: ip + 7 may pass the end
-    // of the block by < 8 bytes, inside the same or the next aligned word of the arena's 256-byte granule)
-    const uintptr_t wa = a0 + (uintptr_t)ip;
-    const uint32_t* wp = reinterpret_cast<const uint32_t*>(wa & ~uintptr_t(3));
-    const unsigned wsh = (wa & 3u) * 8u;
-    const int avail = clen - ip;  // >= 1
-    const uint32_t x0 = __ldg(wp);
-    const uint32_t x1 = ((int)(wa & 3u) + avail > 4) ? __ldg(wp + 1) : 0u;
-    const uint32_t x2 = ((int)(wa & 3u) + avail > 8) ? __ldg(wp + 2) : 0u;
-    const uint32_t lo = __funnelshift_r(x0, x1, wsh), hi = __funnelshift_r(x1, x2, wsh);
-    const int token = (int)(lo & 0xffu);
-    ip++;
-    int ll = token >> 4;
-    if (ll == 15) {
-      int bb;
-      do {
-        if (ip >= clen) {
-          err = true;
-          break;
-        }
-        bb = __ldg(in + ip++);
-        ll += bb;
-      } while (bb == 255);
-      if (err) break;
-    }
-    if (ll > olen - op || ll > clen - ip) {
-      err = true;
-      break;
-    }
-    const int lit_ip = ip;
-    ip += ll;
-    op += ll;
-    if (olen - op < kMFLimit) {  // last sequence: literals only; a match may not start < 12 bytes before the end
-      if (op != olen || ip != clen) err = true;
-      else r[ns++] = make_uint2((uint32_t)ll, (uint32_t)lit_ip << 16);
-      break;
-    }
-    if (ip + 2 > clen) {
-      err = true;
-      break;
-    }
-    int off;
-    if (ll <= 5 && (token >> 4) != 15) {  // offset bytes sit at window bytes 1+ll, 2+ll (<= 7)
-      const unsigned sb = 8u * (unsigned)(1 + ll);
-      const uint32_t w = sb < 32 ? __funnelshift_r(lo, hi, sb) : hi >> (sb - 32);
-      off = (int)(w & 0xffffu);
-    } else {
-      off = __ldg(in + ip) | (__ldg(in + ip + 1) << 8);
-    }
-    ip += 2;
-    int ml = token & 15;
-    if (ml == 15) {
-      int bb;
-      do {
-        if (ip >= clen) {
-          err = true;
-          break;
-        }
-        bb = __ldg(in + ip++);
-        ml += bb;
-      } while (bb == 255);
-      if (err) break;
-    }
-    ml += kMinMatch;
-    if (ml > olen - op || off == 0 || off > op) {
-      err = true;
-      break;
-    }
-    r[ns++] = make_uint2((uint32_t)ll | ((uint32_t)ml << 16), (uint32_t)off | ((uint32_t)lit_ip << 16));
-    op += ml;
-    if (olen - op < kLastLiterals) {  // the last 5 bytes of a block are literals
-      err = true;
-      break;
-    }
+  unsigned biglit = __ballot_sync(FULL, lit > 16);
+  while (biglit) {
+    const int l = __ffs(biglit) - 1;
+    biglit &= biglit - 1;
+    const int n_l = __shfl_sync(FULL, lit, l), op_l = __shfl_sync(FULL, op, l), ip_l = __shfl_sync(FULL, lip, l);
+    if (n_l >= 96) group_copy<32>(out + op_l, in + ip_l, (uint32_t)n_l, lane);
+    else
+      for (int j = lane; j < n_l; j += 32) out[op_l + j] = __ldg(in + ip_l + j);
   }
-  if (err) {
-    set_status(status, d.stream & 0x7fffffffu, B2S_E_CORRUPT);
-    ns = 0;
-  }
-  nrec[b] = ns;
-}
-
-// The same walk with the compressed stream arriving through the TMA ring of tma_ring.cuh (B2S_LZ4D_TOKENS=2): the
-// stream is requested in 64-byte bulk copies four pieces ahead of the cursor and read from shared memory — no global
-// load instruction in the token chain, no prefetch bookkeeping.  Literal bytes are skipped over, not read; pieces the
-// walk jumps across are still fetched (the ring is strictly sequential) but never waited for longer than they take.
-constexpr int kTokThreads = 64;
-__global__ void __launch_bounds__(kTokThreads) lz4_tokens_tma_kernel(const BlockDesc* __restrict__ desc, uint32_t b0,
-                                                                     uint32_t m, const uint8_t* __restrict__ src_base,
-                                                                     uint2* __restrict__ rec, uint32_t rec_stride,
-                                                                     uint32_t* __restrict__ nrec,
-                                                                     int32_t* __restrict__ status) {
-  __shared__ __align__(128) uint8_t s_ring[kTokThreads * kRingBytes];
-  __shared__ __align__(8) uint64_t s_bars[kTokThreads * kRingStages];
-  const uint32_t bl = blockIdx.x * blockDim.x + threadIdx.x;
-  if (bl >= m) return;
-  const uint32_t b = b0 + bl;
-  const BlockDesc d = desc[b];
-  if (d.olen == 0 || (d.stream & 0x80000000u)) {  // no-op descriptor or stored RAW (copied by P2)
-    nrec[b] = 0;
-    return;
-  }
-  const uint8_t* __restrict__ in = src_base + d.src;
-  const int clen = (int)d.clen, olen = (int)d.olen;
-  uint2* __restrict__ r = rec + (size_t)bl * rec_stride;
-  TmaRing R;
-  R.init(s_ring + threadIdx.x * kRingBytes, s_bars + threadIdx.x * kRingStages, in, clen);
-  const int sh0 = (int)(reinterpret_cast<uintptr_t>(in) & 15u);  // stream position of block byte 0
-  int ip = 0, op = 0;
-  uint32_t ns = 0;
-  bool err = false;
-  while (true) {
-    if (ip >= clen) {
-      err = true;
-      break;
-    }
-    // window: bytes ip .. ip+7 from three aligned words of the ring (bytes past the block's end are never used)
-    const int u = sh0 + ip;
-    R.consume_to(u);
-    R.ensure(u + 11);
-    const int w = u & ~3;
-    const unsigned wsh = (unsigned)(u & 3) * 8u;
-    const uint32_t x0 = R.word(w), x1 = R.word(w + 4), x2 = R.word(w + 8);
-    const uint32_t lo = __funnelshift_r(x0, x1, wsh), hi = __funnelshift_r(x1, x2, wsh);
-    const int token = (int)(lo & 0xffu);
-    ip++;
-    int ll = token >> 4;
-    if (ll == 15) {
-      int bb;
-      do {
-        if (ip >= clen) {
-          err = true;
-          break;
-        }
-        R.ensure(sh0 + ip);
-        bb = (int)R.byte(sh0 + ip);
-        ip++;
-        ll += bb;
-      } while (bb == 255);
-      if (err) break;
-    }
-    if (ll > olen - op || ll > clen - ip) {
-      err = true;
-      break;
-    }
-    const int lit_ip = ip;
-    ip += ll;
-    op += ll;
-    if (olen - op < kMFLimit) {  // last sequence: literals only; a match may not start < 12 bytes before the end
-      if (op != olen || ip != clen) err = true;
-      else r[ns++] = make_uint2((uint32_t)ll, (uint32_t)lit_ip << 16);
-      break;
-    }
-    if (ip + 2 > clen) {
-      err = true;
-      break;
-    }
-    int off;
-    if (ll <= 5 && (token >> 4) != 15) {  // offset bytes sit at window bytes 1+ll, 2+ll (<= 7)
-      const unsigned sb = 8u * (unsigned)(1 + ll);
-      const uint32_t wv = sb < 32 ? __funnelshift_r(lo, hi, sb) : hi >> (sb - 32);
-      off = (int)(wv & 0xffffu);
-    } else {
-      R.consume_to(sh0 + ip);
-      R.ensure(sh0 + ip + 1);
-      off = (int)(R.byte(sh0 + ip) | (R.byte(sh0 + ip + 1) << 8));
-    }
-    ip += 2;
-    int ml = token & 15;
-    if (ml == 15) {
-      int bb;
-      do {
-        if (ip >= clen) {
-          err = true;
-          break;
-        }
-        R.ensure(sh0 + ip);
-        bb = (int)R.byte(sh0 + ip);
-        ip++;
-        ml += bb;
-      } while (bb == 255);
-      if (err) break;
-    }
-    ml += kMinMatch;
-    if (ml > olen - op || off == 0 || off > op) {
-      err = true;
-      break;
-    }
-    r[ns++] = make_uint2((uint32_t)ll | ((uint32_t)ml << 16), (uint32_t)off | ((uint32_t)lit_ip << 16));
-    op += ml;
-    if (olen - op < kLastLiterals) {  // the last 5 bytes of a block are literals
-      err = true;
-      break;
-    }
-  }
-  R.drain();
-  if (err) {
-    set_status(status, d.stream & 0x7fffffffu, B2S_E_CORRUPT);
-    ns = 0;
-  }
-  nrec[b] = ns;
+  __syncwarp();
 }
 
 constexpr int kCopyThreads = 256;
@@ -300,56 +81,257 @@ __global__ void __launch_bounds__(kCopyThreads) lz4_copy_kernel(const BlockDesc*
     base_op += __shfl_sync(FULL, inc, 31);
 
     // ---- literals: independent of everything, all lanes at once; long runs go through the whole warp
-    if (lit > 0 && lit <= 16) {  // aligned 8-byte words of the compressed block (read-only: __ldg)
-      uint64_t lo, hi;
-      ld_span16<true>(in + lip, lit, lo, hi);
-      st_span16(out + op, lit, lo, hi);
-    }
-    unsigned biglit = __ballot_sync(FULL, lit > 16);
-    while (biglit) {
-      const int l = __ffs(biglit) - 1;
-      biglit &= biglit - 1;
-      const int n_l = __shfl_sync(FULL, lit, l), op_l = __shfl_sync(FULL, op, l), ip_l = __shfl_sync(FULL, lip, l);
-      if (n_l >= 96) group_copy<32>(out + op_l, in + ip_l, (uint32_t)n_l, lane);
-      else
-        for (int j = lane; j < n_l; j += 32) out[op_l + j] = __ldg(in + ip_l + j);
-    }
-    __syncwarp();
+    lz_copy_literals(in, out, lip, lit, op, lane);
 
     // ---- matches, in dependency rounds (lz_batch.cuh)
     lz_execute_matches<true>(out, op + lit, ml, off, lane);
   }
 }
 
-// records per codec block: an LZ4 sequence takes >= 3 compressed bytes and (all but the last) >= 4 output bytes; a
-// Snappy element takes >= 2 compressed bytes and may produce a single byte
-uint32_t lz4_decode_rec_stride(uint32_t codec, uint32_t max_olen, uint32_t max_clen) {
-  if (codec == B2S_CODEC_SNAPPY_XERIAL) return max_clen / 2 + 2;
-  const uint32_t a = max_olen / 4 + 2, b = max_clen / 3 + 2;
-  return a < b ? a : b;
+// ---- lz4_decode_warp_kernel: WARP per LZ4 codec block, token parse and copies in one pass, no per-sequence records.
+//
+// Each step loads the 128 compressed bytes from the cursor ip into shared memory (aligned words that hold block bytes
+// only).  Lane l owns window positions 4l..4l+3 and computes the header a token at each of them would have — ll with
+// at most one extension byte, the offset, ml with at most one extension byte — and next(p), the position of the token
+// after it.  A header that needs a byte at or past the window's end (or the block's), or a second extension byte, is
+// "unresolved".  Pointer doubling over next (four rounds of shuffles on four byte-packed tables J_k = next^(2^k)) then
+// gives lane s the s-th token of the chain from ip in five more shuffles.  The resolved prefix of the chain, up to 32
+// tokens, is one batch; an unresolved token after it (a long length, a header across the window end, the final
+// literals-only sequence) is decoded by its lane alone from global memory with every check of the serial walk.
+//
+// Every sequence of the batch is validated against the same bounds as LZ4_decompress_fast's safe reader before any of
+// its bytes is written; the batch is cut at the first bad sequence, so a corrupt block writes nothing outside its own
+// output range (what lies inside it is unspecified).  Speculative headers at literal bytes are never validated, copied
+// or read past the window.
+constexpr int kWarpDecWarps = 8, kWin = 128;
+constexpr uint32_t kUnresolved = 0xffu;
+
+// one token at ip, serially, with the checks of the JVM reader; false = corrupt.  last = literals-only final sequence.
+__device__ __noinline__ bool lz4_token_serial(const uint8_t* __restrict__ in, int clen, int olen, int op, int& ip,
+                                             int& ll, int& lip, int& off, int& ml, bool& last) {
+  last = false;
+  off = 0;
+  ml = 0;
+  if (ip >= clen) return false;
+  const int token = __ldg(in + ip++);
+  ll = token >> 4;
+  if (ll == 15) {
+    int bb;
+    do {
+      if (ip >= clen) return false;
+      bb = __ldg(in + ip++);
+      ll += bb;
+    } while (bb == 255);
+  }
+  if (ll > olen - op || ll > clen - ip) return false;
+  lip = ip;
+  ip += ll;
+  const int opl = op + ll;
+  if (olen - opl < kMFLimit) {  // last sequence: literals only; a match may not start < 12 bytes before the end
+    last = true;
+    return opl == olen && ip == clen;
+  }
+  if (ip + 2 > clen) return false;
+  off = __ldg(in + ip) | (__ldg(in + ip + 1) << 8);
+  ip += 2;
+  ml = token & 15;
+  if (ml == 15) {
+    int bb;
+    do {
+      if (ip >= clen) return false;
+      bb = __ldg(in + ip++);
+      ml += bb;
+    } while (bb == 255);
+  }
+  ml += kMinMatch;
+  if (ml > olen - opl || off == 0 || off > opl) return false;
+  return olen - (opl + ml) >= kLastLiterals;  // the last 5 bytes of a block are literals
 }
-size_t lz4_decode_ws_bytes(uint32_t chunk_blocks, uint32_t rec_stride) {
+
+// J_{k+1} = J_k o J_k on the four positions this lane owns (byte b of a table = entry of position 4*lane + b; entries
+// >= kWin — the window's end or kUnresolved — map to themselves)
+__device__ __forceinline__ uint32_t lz4_compose(uint32_t jt) {
+  uint32_t r = 0;
+#pragma unroll
+  for (int b = 0; b < 4; b++) {
+    const uint32_t q = (jt >> (8 * b)) & 0xffu;
+    const uint32_t v = __shfl_sync(0xffffffffu, jt, (int)(q >> 2) & 31);
+    const uint32_t e = q < (uint32_t)kWin ? (v >> (8 * (q & 3u))) & 0xffu : q;
+    r |= e << (8 * b);
+  }
+  return r;
+}
+__device__ __forceinline__ uint32_t lz4_lookup(uint32_t jt, uint32_t p) {
+  const uint32_t v = __shfl_sync(0xffffffffu, jt, (int)(p >> 2) & 31);
+  return p < (uint32_t)kWin ? (v >> (8 * (p & 3u))) & 0xffu : p;
+}
+
+__global__ void __launch_bounds__(kWarpDecWarps * 32, 4)
+    lz4_decode_warp_kernel(const BlockDesc* __restrict__ desc, uint32_t nb, const uint8_t* __restrict__ src_base,
+                           uint8_t* dst_base, int32_t* __restrict__ status, unsigned int* __restrict__ work_counter) {
+  constexpr unsigned FULL = 0xffffffffu;
+  __shared__ __align__(16) uint32_t s_win_all[kWarpDecWarps][kWin / 4];
+  __shared__ __align__(16) uint2 s_hdr_all[kWarpDecWarps][kWin];
+  const int lane = threadIdx.x & 31;
+  uint32_t* s_win = s_win_all[threadIdx.x >> 5];
+  const uint8_t* s_wb = reinterpret_cast<const uint8_t*>(s_win);
+  uint2* s_hdr = s_hdr_all[threadIdx.x >> 5];
+
+  for (;;) {
+    uint32_t b = 0;
+    if (lane == 0) b = atomicAdd(work_counter, 1u);
+    b = __shfl_sync(FULL, b, 0);
+    if (b >= nb) break;
+    const BlockDesc d = desc[b];
+    if (d.olen == 0) continue;  // no-op descriptor
+    const uint8_t* __restrict__ in = src_base + d.src;
+    uint8_t* out = dst_base + d.dst;
+    if (d.stream & 0x80000000u) {  // stored RAW
+      group_copy<32>(out, in, d.olen, lane);
+      continue;
+    }
+    const int clen = (int)d.clen, olen = (int)d.olen;
+    int ip = 0, base_op = 0;
+    bool err = false;
+    for (;;) {
+      if (ip >= clen) {  // a token must start here
+        err = true;
+        break;
+      }
+      // ---- window: bytes ip .. ip + lim - 1 of the block, from the aligned words that contain them
+      const int lim = min(clen - ip, kWin);
+      const uintptr_t wa = reinterpret_cast<uintptr_t>(in) + (uintptr_t)ip;
+      const uint32_t* wp = reinterpret_cast<const uint32_t*>(wa & ~uintptr_t(3));
+      const int a = (int)(wa & 3u);
+      const unsigned wsh = 8u * (unsigned)a;
+      const uint32_t w = 4 * lane < a + lim ? __ldg(wp + lane) : 0u;
+      const uint32_t w32 = (lane == 31 && kWin < a + lim) ? __ldg(wp + 32) : 0u;
+      uint32_t wn = __shfl_down_sync(FULL, w, 1);
+      if (lane == 31) wn = w32;
+      const uint32_t mine = __funnelshift_r(w, wn, wsh);  // window bytes 4*lane .. 4*lane + 3
+      s_win[lane] = mine;
+      __syncwarp();
+
+      // ---- speculative header at each of my four positions
+      uint32_t j0 = 0;
+#pragma unroll
+      for (int k = 0; k < 4; k++) {
+        const int p = 4 * lane + k;
+        const int token = (int)((mine >> (8 * k)) & 0xffu);
+        int q = p + 1;
+        int ll = token >> 4;
+        bool ok = p < lim;
+        if (ll == 15) {
+          const int e = s_wb[q & (kWin - 1)];
+          ok = ok && q < lim && e != 255;
+          ll += e;
+          q++;
+        }
+        const int lit = q;
+        q += ll;
+        ok = ok && q + 1 < lim;
+        const int off = s_wb[q & (kWin - 1)] | (s_wb[(q + 1) & (kWin - 1)] << 8);
+        q += 2;
+        int ml = token & 15;
+        if (ml == 15) {
+          const int e = s_wb[q & (kWin - 1)];
+          ok = ok && q < lim && e != 255;
+          ml += e;
+          q++;
+        }
+        ml += kMinMatch;
+        if (ok) s_hdr[p] = make_uint2((uint32_t)ll | ((uint32_t)ml << 16), (uint32_t)off | ((uint32_t)lit << 16));
+        j0 |= (ok ? (uint32_t)q : kUnresolved) << (8 * k);
+      }
+      __syncwarp();
+
+      // ---- chain from position 0: lane s gets its s-th token (>= kWin: past the chain's resolved part)
+      const uint32_t j1 = lz4_compose(j0), j2 = lz4_compose(j1), j3 = lz4_compose(j2), j4 = lz4_compose(j3);
+      uint32_t c = 0, t;
+      t = lz4_lookup(j0, c); if (lane & 1) c = t;
+      t = lz4_lookup(j1, c); if (lane & 2) c = t;
+      t = lz4_lookup(j2, c); if (lane & 4) c = t;
+      t = lz4_lookup(j3, c); if (lane & 8) c = t;
+      t = lz4_lookup(j4, c); if (lane & 16) c = t;
+      const uint32_t nxt = lz4_lookup(j0, c);
+      const bool resolved = c < (uint32_t)kWin && nxt != kUnresolved;
+      const unsigned resmask = __ballot_sync(FULL, resolved);
+      const int nres = __popc(resmask);  // the chain is monotone: the resolved lanes are 0 .. nres-1
+      const bool serial = nres < 32 && __shfl_sync(FULL, c, nres & 31) < (uint32_t)kWin;  // unresolved token at lane nres
+
+      int ll = 0, ml = 0, off = 0, lip = 0;
+      if (resolved) {
+        const uint2 h = s_hdr[c];
+        ll = (int)(h.x & 0xffffu);
+        ml = (int)(h.x >> 16);
+        off = (int)(h.y & 0xffffu);
+        lip = ip + (int)(h.y >> 16);
+      }
+      // output positions: inclusive scan of ll + ml over the resolved lanes
+      int inc = ll + ml;
+#pragma unroll
+      for (int s = 1; s < 32; s <<= 1) {
+        const int u = __shfl_up_sync(FULL, inc, s);
+        if (lane >= s) inc += u;
+      }
+      bool bad = false, last = false;
+      int nip = ip + (nres == 32 ? (int)__shfl_sync(FULL, nxt, 31) : kWin);  // cursor after the batch
+      if (serial && lane == nres) {
+        const int op0 = base_op + inc;  // inc = sum over the resolved lanes here
+        int tip = ip + (int)c;
+        bad = !lz4_token_serial(in, clen, olen, op0, tip, ll, lip, off, ml, last);
+        inc += ll + ml;
+        nip = tip;
+      }
+      const int nbatch = nres + (serial ? 1 : 0);
+      if (serial) nip = __shfl_sync(FULL, nip, nres);
+      const int op = base_op + inc - (ll + ml);
+      if (resolved) {  // the serial lane has checked itself; a resolved token is never the final one
+        const int opl = op + ll;
+        bad = ll > olen - op || olen - opl < kMFLimit || ml > olen - opl || off == 0 || off > opl ||
+              olen - (opl + ml) < kLastLiterals;
+      }
+      const unsigned badmask = __ballot_sync(FULL, bad) & (nbatch == 32 ? FULL : (1u << nbatch) - 1u);
+      const int nok = badmask ? __ffs(badmask) - 1 : nbatch;
+      if (lane >= nok) ll = ml = 0;
+      const int total = __shfl_sync(FULL, inc, nbatch - 1);  // only used when the batch is copied whole
+
+      lz_copy_literals(in, out, lip, ll, op, lane);
+      lz_execute_matches<true>(out, op + ll, ml, off, lane);
+      if (badmask) {
+        err = true;
+        break;
+      }
+      if (__shfl_sync(FULL, last ? 1 : 0, nbatch - 1)) break;  // the final sequence is done
+      base_op += total;
+      ip = nip;
+      __syncwarp();  // the next window overwrites s_win / s_hdr
+    }
+    if (err && lane == 0) set_status(status, d.stream & 0x7fffffffu, B2S_E_CORRUPT);
+  }
+}
+
+void launch_lz4_decode_warp(const BlockDesc* d_desc, uint32_t nb, const uint8_t* src_base, uint8_t* dst_base,
+                            int32_t* d_status, unsigned int* d_counter, cudaStream_t st, uint64_t* launches) {
+  if (!nb) return;
+  cudaMemsetAsync(d_counter, 0, sizeof(unsigned int), st);
+  int per_sm = 0;
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, lz4_decode_warp_kernel, kWarpDecWarps * 32, 0);
+  if (per_sm < 1) per_sm = 1;
+  const uint64_t want = ((uint64_t)nb + kWarpDecWarps - 1) / kWarpDecWarps;
+  uint64_t grid = (uint64_t)kSMs * per_sm;  // persistent: one wave, warps pull blocks from the counter
+  if (grid > want) grid = want;
+  lz4_decode_warp_kernel<<<(unsigned)grid, kWarpDecWarps * 32, 0, st>>>(d_desc, nb, src_base, dst_base, d_status,
+                                                                         d_counter);
+  *launches += 1;
+}
+
+// records per codec block: a Snappy element takes >= 2 compressed bytes and may produce a single byte
+uint32_t snappy_decode_rec_stride(uint32_t max_clen) { return max_clen / 2 + 2; }
+size_t snappy_decode_ws_bytes(uint32_t chunk_blocks, uint32_t rec_stride) {
   return (size_t)chunk_blocks * rec_stride * 8 + 256;
 }
 
-// tokens and copy are launched separately so the runtime can put the (latency-bound) token walk of chunk k+1 on a side
-// stream beside the (issue-bound) copies of chunk k
-void launch_lz4_tokens(uint32_t codec, const BlockDesc* d_desc, uint32_t b0, uint32_t m, uint32_t rec_stride,
-                       const uint8_t* src_base, uint8_t* d_ws, uint32_t* d_nrec, int32_t* d_status, cudaStream_t st,
-                       uint64_t* launches) {
-  if (!m) return;
-  uint2* rec = reinterpret_cast<uint2*>(d_ws);
-  if (codec == B2S_CODEC_SNAPPY_XERIAL) {
-    launch_snappy_tokens(d_desc, b0, m, src_base, rec, rec_stride, d_nrec, d_status, st, launches);
-  } else if (g_lz4d_tokens == 2) {
-    lz4_tokens_tma_kernel<<<(m + kTokThreads - 1) / kTokThreads, kTokThreads, 0, st>>>(d_desc, b0, m, src_base, rec,
-                                                                                     rec_stride, d_nrec, d_status);
-    *launches += 1;
-  } else {
-    lz4_tokens_kernel<<<(m + 63) / 64, 64, 0, st>>>(d_desc, b0, m, src_base, rec, rec_stride, d_nrec, d_status);
-    *launches += 1;
-  }
-}
 void launch_lz4_copy(const BlockDesc* d_desc, uint32_t b0, uint32_t m, uint32_t rec_stride, const uint8_t* src_base,
                      uint8_t* dst_base, const uint8_t* d_ws, const uint32_t* d_nrec, cudaStream_t st,
                      uint64_t* launches) {

@@ -4,16 +4,18 @@ LZ4Block 32 KiB + CRC32C, one GPU, device-resident), split by kernel.
 
 The wave is built as bench.py builds it (gen_terasort_dev, seed 42, then compress_dev); the read call
 (decompress_dev) is then timed over --calls calls after --warmup untimed ones.  Per call, from last_timing():
-  copy_ms    dominant_ms: the lz4_copy_kernel launches (CUDA events around each launch, summed)
-  decode_ms  top_kernel_ms: token walk + copy, first token launch to last copy launch
+  copy_ms    dominant_ms: the decode launches (CUDA events around each launch, summed): lz4_decode_warp_kernel for
+             LZ4, the lz4_copy_kernel launches for Snappy
+  decode_ms  top_kernel_ms: the whole decode (Snappy: first token launch to last copy launch)
   read_ms    kernel_ms: the whole read pass (CRC32C verify, descriptors, decode, XXH32 verify)
-A child process, run first, repeats one read call with B2S_TRACE=1 and reports the per-chunk timeline: the token walk
-of a chunk runs on the side stream while the previous chunk's copies run on the main one.  The card's name and power
+A child process, run first, repeats one read call with B2S_TRACE=1 and reports the per-chunk timeline of the Snappy
+decoder: the token walk of a chunk runs on the side stream while the previous chunk's copies run on the main one (LZ4
+decodes in one launch and has no such rows).  The card's name and power
 limit are read in the same run.
 
     python tools/decode_split.py [--calls 7] [--warmup 3] [--codec lz4|snappy] [--blocks N] [--chunk-blocks N]
 
-Prints one JSON document.  --chunk-blocks sets B2S_LZ4D_CHUNK_BLOCKS (codec blocks per token/copy launch pair).
+Prints one JSON document.  --chunk-blocks sets B2S_LZ4D_CHUNK_BLOCKS (Snappy: codec blocks per token/copy launch pair).
 """
 import argparse
 import json
