@@ -253,30 +253,18 @@ static void win_find_offsets(const uint8_t* src, int n, int hash_log, uint16_t* 
 }
 
 /* The greedy walk shared by the CPU models of the three GPU encoders: from cursor *p, the next match the parse takes
- * (its position in *p, its length in *mlen), or 0 when the block holds no further match.  sub > 0: the sub-chunk rule
- * of the warp-parallel parse (see orc_lz4_compress_block_win_sub). */
-static int win_next_match(const uint8_t* src, const uint16_t* off, int n, int sub, int* p, int* mlen) {
+ * (its position in *p, its length in *mlen), or 0 when the block holds no further match. */
+static int win_next_match(const uint8_t* src, const uint16_t* off, int n, int* p, int* mlen) {
   const int mflimit = n - LZ4_MFLIMIT, matchlimit = n - LZ4_LASTLITERALS;
   int q = *p;
   while (q <= mflimit) {
-    int chunk_hi = n;
-    if (sub > 0) {
-      chunk_hi = (q / sub + 1) * sub;
-      if (chunk_hi > n) chunk_hi = n;
-    }
-    const int plim = mflimit < chunk_hi - 4 ? mflimit : chunk_hi - 4;
-    const int elim = matchlimit < chunk_hi ? matchlimit : chunk_hi;
-    if (q > plim) { /* nothing can start in the rest of this sub-chunk */
-      q = chunk_hi;
-      continue;
-    }
     if (!off[q]) {
       q++;
       continue;
     }
     const int c = q - off[q];
     int l = LZ4_MINMATCH;
-    while (q + l < elim && src[q + l] == src[c + l]) l++;
+    while (q + l < matchlimit && src[q + l] == src[c + l]) l++;
     *p = q;
     *mlen = l;
     return 1;
@@ -284,24 +272,14 @@ static int win_next_match(const uint8_t* src, const uint16_t* off, int n, int su
   return 0;
 }
 
-/* Sub-chunk size the GPU parse uses for codec blocks of `block_size` bytes: 1/32 of the (32-rounded) block, itself
- * rounded up to a multiple of 32 — one sub-chunk per lane of the warp that parses the block (lz4_parse4_kernel). */
-int orc_lz4_subchunk(uint32_t block_size) {
-  const uint32_t stride = (block_size + 31u) & ~31u;
-  return (int)(((stride >> 5) + 31u) & ~31u);
-}
-
-/* sub > 0: the greedy parse restarts at every multiple of `sub` — a match neither starts in the last three positions of
- * a sub-chunk nor extends past its end (the 32 lanes of a warp parse the 32 sub-chunks of a block independently).
- * sub == 0: one parse over the whole block (the round-1 kernels, still used for Snappy and Zstandard). */
-int orc_lz4_compress_block_win_sub(const uint8_t* src, int n, uint8_t* dst, int cap, int hash_log, int sub) {
+int orc_lz4_compress_block_win(const uint8_t* src, int n, uint8_t* dst, int cap, int hash_log) {
   if (n > 65536 || hash_log > 16 || hash_log < 4) return 0;
   uint16_t* off = (uint16_t*)calloc((size_t)(n > 0 ? n : 1), sizeof(uint16_t));
   int op = 0, anchor = 0;
   if (n >= LZ4_MFLIMIT + 1) {
     win_find_offsets(src, n, hash_log, off); /* phase A */
     int p = 0, mlen = 0;                      /* phase B + C */
-    while (win_next_match(src, off, n, sub, &p, &mlen)) {
+    while (win_next_match(src, off, n, &p, &mlen)) {
       op = lz4_emit_seq(src, anchor, p - anchor, off[p], mlen, dst, op, cap);
       if (op < 0) {
         free(off);
@@ -314,9 +292,6 @@ int orc_lz4_compress_block_win_sub(const uint8_t* src, int n, uint8_t* dst, int 
   op = lz4_emit_seq(src, anchor, n - anchor, 0, 0, dst, op, cap);
   free(off);
   return op < 0 ? 0 : op;
-}
-int orc_lz4_compress_block_win(const uint8_t* src, int n, uint8_t* dst, int cap, int hash_log) {
-  return orc_lz4_compress_block_win_sub(src, n, dst, cap, hash_log, 0);
 }
 
 /* LZ4_decompress_fast semantics (lz4 1.9.4 LZ4_decompress_unsafe_generic), plus input bounds checks */
@@ -400,7 +375,7 @@ uint64_t orc_lz4block_bound(uint64_t n, uint32_t block_size) {
 
 static int64_t lz4block_compress_impl(const uint8_t* src, uint64_t n, uint32_t block_size, uint8_t* dst, uint64_t cap,
                                       int compressor, orc_lz4_compress_fn ext) {
-  if (block_size < 64 || block_size > (1u << 25)) return -3;
+  if (block_size < 64 || block_size > (1u << 25) || compressor < 0 || compressor > 1) return -3;
   const int level = lz4b_level(block_size);
   uint64_t op = 0;
   uint8_t* tmp = (uint8_t*)malloc(block_size + block_size / 255 + 32);
@@ -415,10 +390,8 @@ static int64_t lz4block_compress_impl(const uint8_t* src, uint64_t n, uint32_t b
     int tcap = (int)(block_size + block_size / 255 + 32);
     if (ext)
       clen = ext((const char*)(src + off), (char*)tmp, (int)o, tcap);
-    else if (compressor == 1) /* the default GPU pipeline: single-cursor greedy parse */
-      clen = (o <= 65536) ? orc_lz4_compress_block_win_sub(src + off, (int)o, tmp, (int)o - 1, 12, 0) : 0;
-    else if (compressor == 2) /* B2S_LZ4_PIPE=4: sub-chunk parallel parse */
-      clen = (o <= 65536) ? orc_lz4_compress_block_win_sub(src + off, (int)o, tmp, (int)o - 1, 12, orc_lz4_subchunk(block_size)) : 0;
+    else if (compressor == 1) /* the GPU pipeline: single-cursor greedy parse */
+      clen = (o <= 65536) ? orc_lz4_compress_block_win(src + off, (int)o, tmp, (int)o - 1, 12) : 0;
     else
       clen = orc_lz4_compress_block(src + off, (int)o, tmp, tcap);
     int method = LZ4B_LZ4;
@@ -576,8 +549,7 @@ int64_t orc_snappy_compress_raw(const uint8_t* src, uint64_t n, uint8_t* dst, ui
 /* CPU model of the GPU Snappy compressor: the same match finding and greedy parse as orc_lz4_compress_block_win
  * (including its end-of-block margins: no match starts in the last 12 bytes or covers the last 5 — legal, merely
  * conservative, for Snappy), emitted in the Snappy element grammar.  One chunk <= 32 KiB (the xerial block size). */
-int64_t orc_snappy_compress_raw_win_sub(const uint8_t* src, uint64_t n64, uint8_t* dst, uint64_t cap, int hash_log,
-                                        int sub) {
+int64_t orc_snappy_compress_raw_win(const uint8_t* src, uint64_t n64, uint8_t* dst, uint64_t cap, int hash_log) {
   if (n64 > 32768 || cap < orc_snappy_max_compressed(n64)) return -2;
   const int n = (int)n64;
   uint64_t op = 0;
@@ -592,7 +564,7 @@ int64_t orc_snappy_compress_raw_win_sub(const uint8_t* src, uint64_t n64, uint8_
     uint16_t* off = (uint16_t*)calloc((size_t)n, sizeof(uint16_t));
     win_find_offsets(src, n, hash_log, off);
     int p = 0, mlen = 0;
-    while (win_next_match(src, off, n, sub, &p, &mlen)) {
+    while (win_next_match(src, off, n, &p, &mlen)) {
       if (p > anchor) op = snappy_emit_literal(dst, op, src + anchor, (uint64_t)(p - anchor));
       op = snappy_emit_copy(dst, op, off[p], (uint32_t)mlen);
       p += mlen;
@@ -602,9 +574,6 @@ int64_t orc_snappy_compress_raw_win_sub(const uint8_t* src, uint64_t n64, uint8_
   }
   if (anchor < n) op = snappy_emit_literal(dst, op, src + anchor, (uint64_t)(n - anchor));
   return (int64_t)op;
-}
-int64_t orc_snappy_compress_raw_win(const uint8_t* src, uint64_t n64, uint8_t* dst, uint64_t cap, int hash_log) {
-  return orc_snappy_compress_raw_win_sub(src, n64, dst, cap, hash_log, 0);
 }
 
 int64_t orc_snappy_uncompressed_length(const uint8_t* src, uint64_t n) {
@@ -686,14 +655,14 @@ uint64_t orc_xerial_bound(uint64_t n, uint32_t block_size) {
 }
 static int64_t xerial_compress_impl(const uint8_t* src, uint64_t n, uint32_t block_size, uint8_t* dst, uint64_t cap,
                                     int compressor) {
+  if (compressor < 0 || compressor > 1) return -3;
   if (cap < ORC_XERIAL_HEADER) return -2;
   memcpy(dst, XERIAL_HEADER, 16);
   uint64_t op = 16;
   for (uint64_t off = 0; off < n; off += block_size) {
     uint64_t o = n - off < block_size ? n - off : block_size;
     if (op + 4 + orc_snappy_max_compressed(o) > cap) return -2;
-    int64_t c = compressor >= 1 ? orc_snappy_compress_raw_win_sub(src + off, o, dst + op + 4, cap - op - 4, 12,
-                                                                  compressor == 2 ? orc_lz4_subchunk(block_size) : 0)
+    int64_t c = compressor == 1 ? orc_snappy_compress_raw_win(src + off, o, dst + op + 4, cap - op - 4, 12)
                                 : orc_snappy_compress_raw(src + off, o, dst + op + 4, cap - op - 4);
     if (c < 0) return c;
     wr_be32(dst + op, (uint32_t)c);
@@ -704,8 +673,8 @@ static int64_t xerial_compress_impl(const uint8_t* src, uint64_t n, uint32_t blo
 int64_t orc_xerial_compress(const uint8_t* src, uint64_t n, uint32_t block_size, uint8_t* dst, uint64_t cap) {
   return xerial_compress_impl(src, n, block_size, dst, cap, 0);
 }
-/* compressor: 0 = restated snappy-style greedy, 1 = GPU window model (hash_log 12, block_size <= 32 KiB),
- * 2 = the same with the sub-chunk parallel parse (B2S_LZ4_PIPE=4) */
+/* compressor: 0 = restated snappy-style greedy, 1 = GPU window model (hash_log 12, block_size <= 32 KiB);
+ * any other value returns -3 */
 int64_t orc_xerial_compress2(const uint8_t* src, uint64_t n, uint32_t block_size, uint8_t* dst, uint64_t cap,
                              int compressor) {
   return xerial_compress_impl(src, n, block_size, dst, cap, compressor);

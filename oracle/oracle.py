@@ -48,10 +48,6 @@ def lib():
         L.orc_lz4_compress_block.argtypes = [u8p, C.c_int, u8p, C.c_int]
         L.orc_lz4_compress_block_win.restype = C.c_int
         L.orc_lz4_compress_block_win.argtypes = [u8p, C.c_int, u8p, C.c_int, C.c_int]
-        L.orc_lz4_compress_block_win_sub.restype = C.c_int
-        L.orc_lz4_compress_block_win_sub.argtypes = [u8p, C.c_int, u8p, C.c_int, C.c_int, C.c_int]
-        L.orc_lz4_subchunk.restype = C.c_int
-        L.orc_lz4_subchunk.argtypes = [C.c_uint32]
         L.orc_lz4_decompress_block.restype = C.c_int
         L.orc_lz4_decompress_block.argtypes = [u8p, C.c_int, u8p, C.c_int]
         L.orc_lz4block_bound.restype = C.c_uint64
@@ -136,18 +132,13 @@ def xxh32(b, seed=0x9747B28C):
 
 
 # ---- raw LZ4 block ----
-def lz4_subchunk(block_size):
-    """positions per lane of the GPU's sub-chunk parallel parse for codec blocks of block_size bytes"""
-    return lib().orc_lz4_subchunk(block_size)
-
-
-def lz4_compress_block(b, win=False, hash_log=12, cap=None, sub=0):
-    """win=True: the CPU model of the GPU compressor; sub > 0: with the parse restarted every `sub` positions"""
+def lz4_compress_block(b, win=False, hash_log=12, cap=None):
+    """win=True: the CPU model of the GPU compressor"""
     a = _u8(b)
     cap = cap if cap is not None else a.size + a.size // 255 + 32
     out = np.empty(max(cap, 1), dtype=np.uint8)
     if win:
-        n = lib().orc_lz4_compress_block_win_sub(_p(a), a.size, out.ctypes.data, cap, hash_log, sub)
+        n = lib().orc_lz4_compress_block_win(_p(a), a.size, out.ctypes.data, cap, hash_log)
     else:
         n = lib().orc_lz4_compress_block(_p(a), a.size, out.ctypes.data, cap)
     return out[:n].tobytes() if n > 0 else None

@@ -57,25 +57,10 @@ constexpr uint32_t kChunkStreams = 1u << 18;
 constexpr uint32_t kXxhSeed = 0x9747b28cu;
 uint32_t g_lz4_chunk_blocks = 32768;  // codec blocks per match/parse/emit (or tokens/copy) pass: bounds the workspace; B2S_LZ4_CHUNK_BLOCKS
 uint32_t g_lz4d_chunk_blocks = 65536;  // Snappy decode only (LZ4 decodes in one launch): codec blocks per token walk + copy pair; the walk is latency bound, more blocks per launch = more loads in flight; B2S_LZ4D_CHUNK_BLOCKS
-int g_lz4d_legacy = 0;
-int g_trace = 0;  // B2S_TRACE=1: per-chunk timeline of the compress pipeline on stderr  // B2S_LZ4D_LEGACY=1: single-kernel tile decoder for every block size (A/B comparisons)
 
 inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
-int g_read_priority = 1;       // B2S_READ_PRIORITY=0: both lanes at the default stream priority
 int g_read_lag = 1;            // B2S_READ_LAG: chunks between the stages of the read pipeline (upload+sizes | decode | download)
-int g_overlap = 1;             // B2S_OVERLAP=0: match / token kernels on the main stream (no two-stream overlap); A/B runs
-uint64_t g_copy_piece = 0;     // B2S_COPY_PIECE_MB: host<->device payload copies are issued in pieces of this size so the
-                               // copy engines interleave the two lanes' transfers instead of draining one lane's queue
-cudaError_t copy_async(void* dst, const void* src, size_t bytes, cudaMemcpyKind kind, cudaStream_t st) {
-  if (!g_copy_piece || bytes <= g_copy_piece) return cudaMemcpyAsync(dst, src, bytes, kind, st);
-  for (size_t at = 0; at < bytes; at += g_copy_piece) {
-    const size_t k = std::min<size_t>(g_copy_piece, bytes - at);
-    cudaError_t e = cudaMemcpyAsync((uint8_t*)dst + at, (const uint8_t*)src + at, k, kind, st);
-    if (e != cudaSuccess) return e;
-  }
-  return cudaSuccess;
-}
 
 // --------------------------------------------------------------------------------------------------------------
 // NUMA placement of pinned staging (SURVEY.md §8e: "NUMA-pin staging buffers to the GPU's socket").  On the 8-GPU boxes
@@ -247,7 +232,6 @@ struct Slot {
   PinBuf hmeta;
   // per-launch event pairs around the dominant kernel of a call (grow-only pool; `used` pairs are valid)
   std::vector<cudaEvent_t> ev_dom;
-  std::vector<cudaEvent_t> trace;  // B2S_TRACE=1: (match0, match1, tail0, tail1) per compress chunk, printed by add_timing
   size_t dom_used = 0;
   int dom_pair(cudaEvent_t* a, cudaEvent_t* b) {
     if (dom_used * 2 + 2 > ev_dom.size()) {
@@ -454,9 +438,8 @@ int compress_enqueue(Context* C, Slot& S, const ChecksumTables& tabs, uint32_t b
   // side stream while parse (latency bound, one thread per block), scan and emit of chunk k run on the main stream;
   // the two workspaces alternate.  The side stream forks BEFORE the per-block XXH32 pass (LZ4Block headers; only the
   // emit kernel needs it), so that pass runs beside the first chunk's match kernel instead of in front of it.
-  cudaStream_t side = g_overlap ? S.st2 : st;
   CU(cudaEventRecord(S.ev_fork, st));
-  CU(cudaStreamWaitEvent(side, S.ev_fork, 0));
+  CU(cudaStreamWaitEvent(S.st2, S.ev_fork, 0));
   if (codec == B2S_CODEC_LZ4BLOCK)
     launch_xxh32_encode(d_src, M.src_off, M.src_len, M.blk_base, n, nb, bs, kXxhSeed, M.hash, st, launches);
   CU(cudaMemsetAsync(M.total, 0, 16, st));
@@ -467,22 +450,13 @@ int compress_enqueue(Context* C, Slot& S, const ChecksumTables& tabs, uint32_t b
     uint8_t* ws = (uint8_t*)S.scratch.p + (size_t)par * ws_bytes;
     cudaEvent_t e0 = nullptr, e1 = nullptr;
     S.dom_pair(&e0, &e1);
-    if (k >= 2) CU(cudaStreamWaitEvent(side, S.ev_free[par], 0));  // emit of chunk k-2 has released this workspace
-    launch_lz4_match(d_src, M.src_off, M.src_len, M.blk_base, n, b0, m, bs, codec, ws, M.counter + par, side, launches,
+    if (k >= 2) CU(cudaStreamWaitEvent(S.st2, S.ev_free[par], 0));  // emit of chunk k-2 has released this workspace
+    launch_lz4_match(d_src, M.src_off, M.src_len, M.blk_base, n, b0, m, bs, codec, ws, M.counter + par, S.st2, launches,
                      e0, e1, hlog_for_level(codec, level));
-    CU(cudaEventRecord(S.ev_match[par], side));
+    CU(cudaEventRecord(S.ev_match[par], S.st2));
     CU(cudaStreamWaitEvent(st, S.ev_match[par], 0));
-    cudaEvent_t t0 = nullptr, t1 = nullptr, tp = nullptr;
-    if (g_trace && S.trace.size() < 4096) {
-      cudaEventCreate(&t0);
-      cudaEventCreate(&t1);
-      cudaEventCreate(&tp);
-      S.trace.push_back(e0); S.trace.push_back(e1); S.trace.push_back(t0); S.trace.push_back(t1); S.trace.push_back(tp);
-      CU(cudaEventRecord(t0, st));
-    }
     launch_lz4_parse_emit(d_src, M.src_off, M.src_len, M.blk_base, n, b0, m, bs, codec, ws, M.nseq, M.csize, M.hash,
-                          M.sizes, M.total, M.ws, d_dst, dst_cap, st, launches, tp);
-    if (t1) CU(cudaEventRecord(t1, st));
+                          M.sizes, M.total, M.ws, d_dst, dst_cap, st, launches);
     CU(cudaEventRecord(S.ev_free[par], st));
   }
   CU(cudaEventRecord(S.ev_t1, st));
@@ -694,7 +668,7 @@ int decompress_enqueue_b(Slot& S, DecompressJob& J, const uint8_t* d_src, uint8_
   const bool small_blocks = max_olen <= 65536 && max_clen < 65536;
   if (J.codec == B2S_CODEC_SNAPPY_XERIAL && !small_blocks)
     return fail(B2S_E_UNSUPPORTED, "snappy chunks larger than 64 KiB are not supported%s");
-  if (J.nb && small_blocks && J.codec == B2S_CODEC_LZ4BLOCK && !g_lz4d_legacy) {
+  if (J.nb && small_blocks && J.codec == B2S_CODEC_LZ4BLOCK) {
     // one launch over every codec block: warp per block, parse and copies together (lz4_decode.cu)
     cudaEvent_t e0 = nullptr, e1 = nullptr;
     S.dom_pair(&e0, &e1);
@@ -720,15 +694,8 @@ int decompress_enqueue_b(Slot& S, DecompressJob& J, const uint8_t* d_src, uint8_
       const int par = (int)(k & 1);
       uint8_t* ws = (uint8_t*)S.scratch.p + nrec_bytes + (size_t)par * ws_bytes;
       if (k >= 2) CU(cudaStreamWaitEvent(S.st2, S.ev_free[par], 0));
-      cudaEvent_t q0 = nullptr, q1 = nullptr;
-      if (g_trace && S.trace.size() < 4096) {
-        cudaEventCreate(&q0);
-        cudaEventCreate(&q1);
-        CU(cudaEventRecord(q0, S.st2));
-      }
       launch_snappy_tokens(desc, b0, m, d_src, reinterpret_cast<uint2*>(ws), rec_stride, nrec, J.status, S.st2,
                            launches);
-      if (q1) CU(cudaEventRecord(q1, S.st2));
       CU(cudaEventRecord(S.ev_match[par], S.st2));
       CU(cudaStreamWaitEvent(st, S.ev_match[par], 0));
       cudaEvent_t e0 = nullptr, e1 = nullptr;
@@ -736,18 +703,10 @@ int decompress_enqueue_b(Slot& S, DecompressJob& J, const uint8_t* d_src, uint8_
       CU(cudaEventRecord(e0, st));
       launch_lz4_copy(desc, b0, m, rec_stride, d_src, d_dst, ws, nrec, st, launches);
       CU(cudaEventRecord(e1, st));
-      if (q0) {  // trace rows: (tokens0, tokens1, copy0, copy1, copy1)
-        S.trace.push_back(q0); S.trace.push_back(q1);
-        cudaEvent_t c0 = nullptr, c1 = nullptr, c2 = nullptr;
-        cudaEventCreate(&c0); cudaEventCreate(&c1); cudaEventCreate(&c2);
-        // e0/e1 belong to the dom pool; re-record private copies right here (same stream position as e1)
-        CU(cudaEventRecord(c1, st)); CU(cudaEventRecord(c2, st));
-        S.trace.push_back(e0); S.trace.push_back(c1); S.trace.push_back(c2);
-        cudaEventDestroy(c0);
-      }
       CU(cudaEventRecord(S.ev_free[par], st));
     }
   } else if (J.nb) {
+    // LZ4Block with a codec block over 64 KiB (lz4-java allows up to 32 MiB): the tile decoder takes the whole batch
     launch_lz4_decompress(desc, (uint32_t)J.nb, d_src, d_dst, J.status, J.counter, st, launches);
   }
   CU(cudaEventRecord(S.ev_t1, st));
@@ -778,18 +737,6 @@ void add_timing(Slot& S, bool copies) {
   for (size_t k = 0; k < S.dom_used; k++) {
     t_timing.dominant_ms += ms_between(S.ev_dom[2 * k], S.ev_dom[2 * k + 1]);
     t_timing.dominant_launches++;
-  }
-  if (g_trace && !S.trace.empty()) {
-    cudaEvent_t base = S.trace[0];
-    for (size_t k = 0; k + 4 < S.trace.size(); k += 5) {
-      fprintf(stderr, "chunk %2zu: A(match|tokens) %7.3f..%7.3f  B(parse|copy) %7.3f..%7.3f  end %7.3f ms\n", k / 5,
-              ms_between(base, S.trace[k]), ms_between(base, S.trace[k + 1]), ms_between(base, S.trace[k + 2]),
-              ms_between(base, S.trace[k + 4]), ms_between(base, S.trace[k + 3]));
-      // (events at k, k+1 [compress] / k+2 [decode] belong to the dominant-kernel pool or are leaked: tracing only)
-      cudaEventDestroy(S.trace[k + 3]);
-      cudaEventDestroy(S.trace[k + 4]);
-    }
-    S.trace.clear();
   }
   S.dom_used = 0;
   if (copies) t_timing.h2d_ms += ms_between(S.ev_h0, S.ev_h1);  // d2h is added once the payload copy has run
@@ -1122,16 +1069,9 @@ int b2s_init(uint32_t gpu_mask, uint64_t pinned_bytes_per_gpu, uint32_t streams_
   if (e != cudaSuccess || count <= 0)
     return fail(B2S_E_CUDA, "no CUDA device: %s", e != cudaSuccess ? cudaGetErrorString(e) : "device count is 0");
   g_lz4_hlog = env_int("B2S_LZ4_HLOG", g_lz4_hlog);
-  g_lz4d_tile = env_int("B2S_LZ4D_TILE", g_lz4d_tile);
-  g_lz4_pipe = env_int("B2S_LZ4_PIPE", g_lz4_pipe);
   g_lz4_chunk_blocks = (uint32_t)std::max(1, env_int("B2S_LZ4_CHUNK_BLOCKS", (int)g_lz4_chunk_blocks));
-  g_lz4d_legacy = env_int("B2S_LZ4D_LEGACY", 0);
-  g_trace = env_int("B2S_TRACE", 0);
   g_numa = env_int("B2S_NUMA", 1);
-  g_overlap = env_int("B2S_OVERLAP", g_overlap);
-  g_read_priority = env_int("B2S_READ_PRIORITY", g_read_priority);
   g_read_lag = std::max(1, env_int("B2S_READ_LAG", g_read_lag));
-  g_copy_piece = (uint64_t)std::max(0, env_int("B2S_COPY_PIECE_MB", 0)) << 20;
   g_lz4d_chunk_blocks = (uint32_t)std::max(1, env_int("B2S_LZ4D_CHUNK_BLOCKS", (int)g_lz4d_chunk_blocks));
   g_host_chunk_bytes = (uint64_t)std::max(1, env_int("B2S_HOST_CHUNK_MB", (int)(g_host_chunk_bytes >> 20))) << 20;
   // streams_per_gpu: pipeline slots (stream pairs + staging) per lane, 0 = default; B2S_SLOTS overrides
@@ -1153,7 +1093,7 @@ int b2s_init(uint32_t gpu_mask, uint64_t pinned_bytes_per_gpu, uint32_t streams_
         // trips per chunk): they get the higher stream priority so they are not queued behind the write lane's grids
         int prio_lo = 0, prio_hi = 0;
         cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi);
-        const int prio = (l == kLaneRead && g_read_priority) ? prio_hi : prio_lo;
+        const int prio = l == kLaneRead ? prio_hi : prio_lo;
         CU(cudaStreamCreateWithPriority(&S.st, cudaStreamNonBlocking, prio));
         CU(cudaStreamCreateWithPriority(&S.st2, cudaStreamNonBlocking, prio));
         cudaEvent_t* evs2[] = {&S.ev_fork, &S.ev_match[0], &S.ev_match[1], &S.ev_free[0], &S.ev_free[1]};
@@ -1445,7 +1385,7 @@ static int checksum_host(uint32_t alg, uint32_t n, const uint8_t* const* ptr, co
     if (rc) return rc;
     CU(cudaEventRecord(S.ev_h0, S.st));
     for (const Run& r : runs)
-      CU(copy_async((uint8_t*)S.src.p + r.dev_off, r.host, r.bytes, cudaMemcpyHostToDevice, S.st));
+      CU(cudaMemcpyAsync((uint8_t*)S.src.p + r.dev_off, r.host, r.bytes, cudaMemcpyHostToDevice, S.st));
     CU(cudaEventRecord(S.ev_h1, S.st));
     rc = checksum_chunk_dev(D, S, alg, cnt, (const uint8_t*)S.src.p, dev_off.data(), len + i0, out + i0, bytes,
                             &launches);
@@ -1583,12 +1523,12 @@ static int compress_host(uint32_t codec, int32_t level, uint32_t codec_block_siz
         }
         // copy what fits so that earlier streams of the chunk stay valid
         uint64_t fit = packed_cap > run_off ? packed_cap - run_off : 0;
-        if (fit) CU(copy_async(packed_dst + run_off, S.dst.p, fit, cudaMemcpyDeviceToHost, S.st));
+        if (fit) CU(cudaMemcpyAsync(packed_dst + run_off, S.dst.p, fit, cudaMemcpyDeviceToHost, S.st));
         t_timing.d2h_bytes += fit;
       } else {
         for (uint32_t k = 0; k < J.n; k++) dst_off[i0 + k] = run_off + J.h_dst_off[k];
         if (chunk_total)
-          CU(copy_async(packed_dst + run_off, S.dst.p, chunk_total, cudaMemcpyDeviceToHost, S.st));
+          CU(cudaMemcpyAsync(packed_dst + run_off, S.dst.p, chunk_total, cudaMemcpyDeviceToHost, S.st));
         t_timing.d2h_bytes += chunk_total;
       }
       run_off += chunk_total;
@@ -1632,7 +1572,7 @@ static int compress_host(uint32_t codec, int32_t level, uint32_t codec_block_siz
     if (rc) return rc;
     CU(cudaEventRecord(S.ev_h0, S.st));
     for (const Run& r : runs[c % g_nslot])
-      CU(copy_async((uint8_t*)S.src.p + r.dev_off, r.host, r.bytes, cudaMemcpyHostToDevice, S.st));
+      CU(cudaMemcpyAsync((uint8_t*)S.src.p + r.dev_off, r.host, r.bytes, cudaMemcpyHostToDevice, S.st));
     CU(cudaEventRecord(S.ev_h1, S.st));
     t_timing.h2d_bytes += bytes;
     t_timing.src_bytes += bytes;
@@ -2003,7 +1943,7 @@ static int partition_compress_packed(uint32_t codec, int32_t level, uint32_t cod
   uint32_t* d_part = (uint32_t*)(d_rec + rec_sz + len_sz);
   cudaStream_t st = S.st;
   CU(cudaEventRecord(S.ev_h0, st));
-  if (rec_bytes) CU(copy_async(d_rec, rec_base, rec_bytes, cudaMemcpyHostToDevice, st));
+  if (rec_bytes) CU(cudaMemcpyAsync(d_rec, rec_base, rec_bytes, cudaMemcpyHostToDevice, st));
   if (n_records) {
     CU(cudaMemcpyAsync(d_len, rec_len, n_records * 4, cudaMemcpyHostToDevice, st));
     CU(cudaMemcpyAsync(d_part, rec_part, n_records * 4, cudaMemcpyHostToDevice, st));
@@ -2025,7 +1965,7 @@ static int partition_compress_packed(uint32_t codec, int32_t level, uint32_t cod
     result = fail(B2S_E_DST_TOO_SMALL, "dst_cap is below the %s bytes of the .data arena", std::to_string(arena).c_str());
   }
   CU(cudaEventRecord(S.ev_d0, st));
-  if (fit) CU(copy_async(dst_base, S.dst.p, fit, cudaMemcpyDeviceToHost, st));
+  if (fit) CU(cudaMemcpyAsync(dst_base, S.dst.p, fit, cudaMemcpyDeviceToHost, st));
   CU(cudaEventRecord(S.ev_d1, st));
   CU(cudaStreamSynchronize(st));
   CU(cudaGetLastError());
@@ -2265,7 +2205,7 @@ static int decompress_host(uint32_t codec, uint32_t alg, uint32_t n, const uint8
     if (r) return r;
     CU(cudaEventRecord(S.ev_h0, S.st));
     for (const Run& q : runs[c % g_nslot])
-      CU(copy_async((uint8_t*)S.src.p + q.dev_off, q.host, q.bytes, cudaMemcpyHostToDevice, S.st));
+      CU(cudaMemcpyAsync((uint8_t*)S.src.p + q.dev_off, q.host, q.bytes, cudaMemcpyHostToDevice, S.st));
     CU(cudaEventRecord(S.ev_h1, S.st));
     t_timing.h2d_bytes += bytes;
     t_timing.src_bytes += bytes;
@@ -2309,7 +2249,7 @@ static int decompress_host(uint32_t codec, uint32_t alg, uint32_t n, const uint8
           if (status[i0 + k] == 0 && run_off + J.h_dst_off[k] + J.h_dst_len[k] > packed_cap)
             status[i0 + k] = B2S_E_DST_TOO_SMALL;
       }
-      if (fit) CU(copy_async(packed_dst + run_off, S.dst.p, fit, cudaMemcpyDeviceToHost, S.st));
+      if (fit) CU(cudaMemcpyAsync(packed_dst + run_off, S.dst.p, fit, cudaMemcpyDeviceToHost, S.st));
       t_timing.d2h_bytes += fit;
     } else {
       for (uint32_t k = 0; k < J.n; k++) {
@@ -2703,7 +2643,7 @@ static int sort_packed_run(Device* D, uint32_t codec, uint32_t alg, uint32_t n, 
     uint32_t j = i + 1;
     while (j < n && src_off[j] == src_off[j - 1] + src_len[j - 1]) j++;
     const uint64_t bytes = dev_off[j - 1] + src_len[j - 1] - dev_off[i];
-    if (bytes) CU(copy_async((uint8_t*)S.src.p + dev_off[i], src_base + src_off[i], bytes, cudaMemcpyHostToDevice, st));
+    if (bytes) CU(cudaMemcpyAsync((uint8_t*)S.src.p + dev_off[i], src_base + src_off[i], bytes, cudaMemcpyHostToDevice, st));
     i = j;
   }
   CU(cudaEventRecord(S.ev_h1, st));
@@ -2715,7 +2655,7 @@ static int sort_packed_run(Device* D, uint32_t codec, uint32_t alg, uint32_t n, 
   if (rc) return rc;
   const uint64_t down = *n_records ? *dst_total : 0;
   CU(cudaEventRecord(S.ev_d0, st));
-  if (down) CU(copy_async(dst_base, sorted, down, cudaMemcpyDeviceToHost, st));
+  if (down) CU(cudaMemcpyAsync(dst_base, sorted, down, cudaMemcpyDeviceToHost, st));
   CU(cudaEventRecord(S.ev_d1, st));
   CU(cudaStreamSynchronize(st));
   CU(cudaGetLastError());
@@ -2881,7 +2821,7 @@ int b2s_exchange_read_packed(int32_t shuffle_id, int32_t start_reduce, int32_t e
   CU(cudaEventRecord(S.ev_t1, st));
   CU(cudaEventRecord(S.ev_k1, st));
   CU(cudaEventRecord(S.ev_d0, st));
-  if (total) CU(copy_async(dst_base, S.dst.p, total, cudaMemcpyDeviceToHost, st));
+  if (total) CU(cudaMemcpyAsync(dst_base, S.dst.p, total, cudaMemcpyDeviceToHost, st));
   CU(cudaEventRecord(S.ev_d1, st));
   CU(cudaStreamSynchronize(st));
   CU(cudaGetLastError());

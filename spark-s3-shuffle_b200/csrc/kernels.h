@@ -44,7 +44,7 @@ void launch_xxh32_verify(const BlockDesc* d_desc, uint32_t n_blocks, const uint8
                          uint32_t mask, int32_t* d_status, cudaStream_t st, uint64_t* launches);
 
 // ---------------- lz4_compress.cu (K3: match / parse / emit + write-side LZ4Block framing) ----------------
-extern int g_lz4_hlog, g_lz4d_tile, g_lz4_pipe;
+extern int g_lz4_hlog;
 // bytes of workspace for one pass over `chunk_blocks` codec blocks (off u16 + ml8 u8 per position, 8-byte records)
 size_t lz4_compress_ws_bytes(uint32_t chunk_blocks, uint32_t block_size, uint32_t codec);
 // Codec blocks [b0, b0+m) of the batch, in two halves that may run on different streams (d_ws is handed from one to
@@ -61,8 +61,7 @@ void launch_lz4_parse_emit(const uint8_t* src_base, const uint64_t* d_src_off, c
                            const uint32_t* d_blk_base, uint32_t n_streams, uint32_t b0, uint32_t m,
                            uint32_t block_size, uint32_t codec, uint8_t* d_ws, uint32_t* d_nseq, uint32_t* d_csize,
                            const uint32_t* d_hash, uint64_t* d_sizes, uint64_t* d_running_total, uint64_t* d_scan_ws,
-                           uint8_t* dst_base, uint64_t dst_cap, cudaStream_t st, uint64_t* launches,
-                           cudaEvent_t ev_parsed = nullptr);
+                           uint8_t* dst_base, uint64_t dst_cap, cudaStream_t st, uint64_t* launches);
 // per stream: dst_off/dst_len, end mark, B2S_E_DST_TOO_SMALL (d_scan = packed block offsets, d_scan_total = their sum)
 void launch_lz4block_stream_meta(const uint32_t* d_blk_base, uint32_t n_streams, uint32_t n_blocks, uint32_t block_size,
                                  const uint64_t* d_scan, const uint64_t* d_scan_total, uint8_t* dst_base,

@@ -12,8 +12,9 @@
 // Parallelism: every codec block (<= 64 KiB here) is independent.
 //  compress : one warp per block, window-batched greedy parse (see K3 below).  Deterministic; the CPU model
 //             orc_lz4_compress_block_win() in oracle/ produces identical bytes.
-//  decompress: a tile of TILE lanes (4/8/16/32) per block; the token chain is serial, the tile parses uniformly and
-//             copies literals / (overlapping) matches TILE bytes per step.
+//  decompress: blocks up to 64 KiB take one warp each (lz4_decode_warp_kernel, lz4_decode.cu); a batch with a larger
+//             block takes a tile of 8 lanes per block here: the token chain is serial, the tile parses uniformly and
+//             copies literals / (overlapping) matches 8 bytes per step.
 // This is latency/issue-bound byte-stream work (no tensor cores, HBM far from saturated by one block per tile), so
 // the levers are blocks in flight per SM (small per-tile state: 4-8 KiB hash table, no staged copy of the block)
 // and instructions per sequence.
@@ -23,7 +24,6 @@ namespace b2s {
 
 constexpr int kLz4Threads = 128;
 constexpr int kMinMatch = 4, kMFLimit = 12, kLastLiterals = 5;
-int g_lz4d_tile = 8;  // B2S_LZ4D_TILE (api.cu reads it once at init)
 
 // ------------------------------------------------------------------------------------------------------------
 // LZ4Block framing, read side: header walk (LZ4BlockInputStream.refill [U])
@@ -321,12 +321,7 @@ void launch_lz4_decompress(const BlockDesc* d_desc, uint32_t n_blocks, const uin
                            int32_t* d_status, unsigned int* d_counter, cudaStream_t st, uint64_t* launches) {
   if (!n_blocks) return;
   cudaMemsetAsync(d_counter, 0, sizeof(unsigned int), st);
-  switch (g_lz4d_tile) {
-    case 4: launch_lz4_decompress_t<4>(d_desc, n_blocks, src_base, dst_base, d_status, d_counter, st); break;
-    case 16: launch_lz4_decompress_t<16>(d_desc, n_blocks, src_base, dst_base, d_status, d_counter, st); break;
-    case 32: launch_lz4_decompress_t<32>(d_desc, n_blocks, src_base, dst_base, d_status, d_counter, st); break;
-    default: launch_lz4_decompress_t<8>(d_desc, n_blocks, src_base, dst_base, d_status, d_counter, st); break;
-  }
+  launch_lz4_decompress_t<8>(d_desc, n_blocks, src_base, dst_base, d_status, d_counter, st);
   *launches += 1;
 }
 

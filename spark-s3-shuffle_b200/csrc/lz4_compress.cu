@@ -25,7 +25,6 @@
 // pass so the workspace stays bounded.  Algorithmic bytes stay (1 + r) per input byte; the extra traffic is the off/ml
 // intermediate.
 #include "kernels.h"
-#include "lz4_parse_core.h"
 
 namespace b2s {
 
@@ -408,357 +407,6 @@ __global__ void __launch_bounds__(64) lz4_parse_kernel(
 }
 
 // ------------------------------------------------------------------------------------------------------------
-// A2 / B4: the alternative generation (B2S_LZ4_PIPE=4): match without lengths, sub-chunk parallel parse
-// ------------------------------------------------------------------------------------------------------------
-// The first generation's match kernel is issue bound at 152 warp-instructions per
-// window, and about half of them compute FULL match lengths for all 32 positions (8-byte compares = a third candidate
-// word and a third source word per lane, segment ballots, the cooperative extension loop, the carry) although the
-// greedy parse consults only ~4 positions per window.
-//
-//   A2 lz4_match2_kernel  verifies FOUR bytes and stores off[p] only (2 B per position instead of 4) + one 32-bit
-//                         match mask per window.  The candidate and source word pairs already hold the fifth byte, so
-//                         for codec blocks <= 32 KiB (offsets < 2^15) bit 15 of off[p] says "the match is exactly 4
-//                         long" — the common case on record-shaped data (12 of 14 sequences per terasort record).
-//                         71 (81 with the masks) instead of 152 warp-instructions per window, DRAM traffic 2.2x instead
-//                         of 3.7x algorithmic.
-//   B4 lz4_parse4_kernel  one WARP per block, lane per sub-chunk, lengths measured for the matches the parse takes.
-// Measured end to end this generation is NOT faster than the first (what the match kernel saves, measuring lengths per
-// taken match costs again in scattered 32-byte-sector traffic) — it is kept for its lower latency on task-sized batches.
-struct Pending2 {
-  uint32_t c0, c1, v, b4, d;  // candidate words, the 4 source bytes, source word holding byte p+4 (pre-shifted), offset (0 = dead)
-  unsigned csh;
-};
-
-template <int HLOG>
-__global__ void __launch_bounds__(kMatchWarps * 32, 3) lz4_match2_kernel(
-    const uint8_t* __restrict__ src_base, const uint64_t* __restrict__ src_off, const uint64_t* __restrict__ src_len,
-    const uint32_t* __restrict__ blk_base, uint32_t n_streams, uint32_t b0, uint32_t m, uint32_t block_size,
-    uint32_t stride, uint16_t* __restrict__ offarr, uint32_t* __restrict__ maskarr,
-    unsigned int* __restrict__ work_counter) {
-  extern __shared__ __align__(16) uint16_t smem_tables[];
-  constexpr unsigned FULL = 0xffffffffu;
-  const int lane = threadIdx.x & 31;
-  uint16_t* table = smem_tables + (size_t)(threadIdx.x >> 5) * (1 << HLOG);
-  const int r_me = 31 - lane;  // lane l owns window position 31 - l (see lz4_match_kernel)
-  const bool flag4 = stride <= 32768u;
-
-  for (;;) {
-    uint32_t bl = 0;
-    if (lane == 0) bl = atomicAdd(work_counter, 1u);
-    bl = __shfl_sync(FULL, bl, 0);
-    if (bl >= m) break;
-    const BlockSpan B = block_span(src_base, src_off, src_len, blk_base, n_streams, b0 + bl, block_size);
-    const uint8_t* __restrict__ s = B.s;
-    const int n = B.n;
-    uint16_t* oq = offarr + (size_t)bl * stride + r_me;
-    uint32_t* mq = maskarr + (size_t)bl * (stride >> 5);  // one word per window: bit r = position r matched
-    {
-      uint4* t4 = reinterpret_cast<uint4*>(table);
-      for (int j = lane; j < (1 << HLOG) / 8; j += 32) t4[j] = make_uint4(0, 0, 0, 0);
-    }
-    __syncwarp();
-    if (n < kMFLimit + 1) continue;
-    const int mflimit = n - kMFLimit;
-
-    auto finish = [&](const Pending2& W) {
-      const bool ok = __funnelshift_r(W.c0, W.c1, W.csh) == W.v;
-      uint32_t off = ok ? W.d : 0u;
-      // fifth byte: byte (cand & 3) of c1 against byte (p & 3) of the second source word (b4 is pre-shifted)
-      if (flag4 && off && (((W.c1 >> W.csh) ^ W.b4) & 0xffu)) off |= 0x8000u;
-      __stcs(oq, (uint16_t)off);
-      oq += 32;
-      const unsigned mb = __ballot_sync(FULL, off != 0u);
-      if (lane == 0) *mq = __brev(mb);
-      mq++;
-    };
-
-    const uintptr_t a0 = reinterpret_cast<uintptr_t>(s + (r_me <= mflimit ? r_me : mflimit));
-    const uint32_t* wp = reinterpret_cast<const uint32_t*>(a0 & ~uintptr_t(3));
-    const unsigned sh = (reinterpret_cast<uintptr_t>(s + r_me) & 3u) * 8u;
-    uint32_t w0 = __ldg(wp), w1 = __ldg(wp + 1);
-    uint32_t carry_v = 0;
-    auto step = [&](int pos, Pending2& N, const Pending2& F, bool have_prev) {
-      const bool full = pos + 31 <= mflimit;  // uniform
-      const int p = pos + r_me;
-      const bool valid = p <= mflimit;
-      const int pc = valid ? p : mflimit;
-      uint32_t v, b4;
-      if (full) {
-        v = __funnelshift_r(w0, w1, sh);
-        b4 = w1 >> sh;
-        if (pos + 63 <= mflimit) {  // the next window is full as well: request its words now
-          wp += 8;
-          w0 = __ldg(wp);
-          w1 = __ldg(wp + 1);
-        }
-      } else {  // last, partial window: clamped positions, plain loads (pc + 4 <= n - 8)
-        v = ld32u_ro(s + pc);
-        b4 = __ldg(s + pc + 4);
-      }
-      const uint32_t vprev = __shfl_down_sync(FULL, v, 1);
-      bool rle = vprev == v;
-      if (lane == 31) rle = pos > 0 && carry_v == v;
-      carry_v = __shfl_sync(FULL, v, 0);
-      const uint32_t h = (v * 2654435761u) >> (32 - HLOG);
-      int cand = table[h];
-      if (rle) cand = pc - 1;
-      const bool older = cand < pc;
-      if (!older) cand = 0;  // keep the loads in bounds; the result is discarded
-      {
-        const uintptr_t ca = reinterpret_cast<uintptr_t>(s + cand);
-        const uint32_t* cw = reinterpret_cast<const uint32_t*>(ca & ~uintptr_t(3));
-        N.csh = (ca & 3u) * 8u;
-        N.c0 = __ldg(cw);
-        N.c1 = __ldg(cw + 1);  // covers cand + 4: cand + 7 < p + 7 <= n - 5
-      }
-      N.v = v;
-      N.b4 = b4;
-      N.d = (valid && older) ? (uint32_t)(pc - cand) : 0u;
-
-      if (have_prev) finish(F);
-
-      __syncwarp();
-      if (valid) table[h] = (uint16_t)p;
-      __syncwarp();
-      for (;;) {
-        const bool lost = valid && table[h] < (uint16_t)p;
-        if (!__ballot_sync(FULL, lost)) break;
-        if (lost) table[h] = (uint16_t)p;
-        __syncwarp();
-      }
-    };
-
-    Pending2 PA, PB;
-    PA.c0 = PA.c1 = PA.v = PA.b4 = PA.d = 0;
-    PA.csh = 0;
-    PB = PA;
-    bool last_is_a = true;
-    for (int pos = 0; pos <= mflimit; pos += 64) {
-      step(pos, PA, PB, pos > 0);
-      last_is_a = true;
-      if (pos + 32 > mflimit) break;
-      step(pos + 32, PB, PA, true);
-      last_is_a = false;
-    }
-    if (last_is_a) finish(PA); else finish(PB);
-    __syncwarp();
-  }
-}
-
-struct ParseMemDev {
-  const uint32_t* __restrict__ mk;  // the block's window masks
-  __device__ __forceinline__ uint32_t mask(int w) const { return __ldg(mk + w); }
-};
-
-// B4: sub-chunk parallel parse — one WARP per codec block, lane k parses sub-chunk k (lz4_parse_core.h, walk_subchunk),
-// then the warp stitches the 32 staged record lists into the dense record array the emit kernels read:
-//   1. anchors: the first sequence of a sub-chunk owns the literals since the last match of any earlier sub-chunk
-//      (inclusive max-scan of the lanes' last match ends);
-//   2. sizes: size of that first sequence + the lane's remaining sequences -> exclusive scan = the lane's output offset
-//      inside the block (Zstandard: literal bytes instead of output bytes);
-//   3. compaction in place: lane k staged its records at slot k * (S/4 + 1); dense index <= staged index, so batches of
-//      32 records are read, patched (anchor / literal count of a first record, offsets made absolute) and written back
-//      in increasing order without ever overwriting an unread record;
-//   4. the block's final literal run, its record count and sizes (RAW decision for LZ4Block).
-constexpr int kParse4Warps = 4;
-__host__ __device__ inline uint32_t parse4_sub(uint32_t stride) { return ((stride >> 5) + 31u) & ~31u; }
-
-template <int CODEC>
-__global__ void __launch_bounds__(kParse4Warps * 32) lz4_parse4_kernel(
-    const uint8_t* __restrict__ src_base, const uint64_t* __restrict__ src_off, const uint64_t* __restrict__ src_len,
-    const uint32_t* __restrict__ blk_base, uint32_t n_streams, uint32_t b0, uint32_t m, uint32_t block_size,
-    uint32_t stride, uint32_t max_seq, const uint16_t* __restrict__ offarr, const uint32_t* __restrict__ maskarr,
-    uint2* seqarr, uint32_t* __restrict__ nseq, uint32_t* __restrict__ csize, uint64_t* __restrict__ sizes) {
-  constexpr unsigned FULL = 0xffffffffu;
-  constexpr bool SNAPPY = CODEC == 1, ZSTD = CODEC == 2;
-  const int lane = threadIdx.x & 31;
-  const uint32_t bl = blockIdx.x * kParse4Warps + (threadIdx.x >> 5);
-  if (bl >= m) return;  // warp-uniform
-  const uint32_t b = b0 + bl;
-  const BlockSpan B = block_span(src_base, src_off, src_len, blk_base, n_streams, b, block_size);
-  const int n = B.n;
-  const int S = (int)parse4_sub(stride);
-  const int slot = S / 4 + 1;
-  uint2* seq = seqarr + (size_t)bl * max_seq;
-  ParseMemDev mem;
-  mem.mk = maskarr + (size_t)bl * (stride >> 5);
-
-  const int lo = lane * S;
-  lzparse::SubResult R;
-  R.nrec = 0;
-  R.rest = 0;
-  R.pm0 = R.len0 = R.d0 = 0;
-  R.last_end = -1;
-  if (n >= kMFLimit + 1) {
-    // The walk of lzparse::walk_subchunk (the lane-local statement of this loop, tested on the CPU), restructured so
-    // that the 32 lanes advance one SEQUENCE per trip in lock step and matches that need measuring are measured by the
-    // whole warp: 32 consecutive bytes of the match against 32 consecutive bytes of its source per round — two
-    // coalesced loads instead of a per-lane gather of six words per eight bytes (ncu of the per-lane version: 11.5 GB
-    // of DRAM reads per GiB of input, 80 bytes per sequence, almost all of it extension traffic).
-    const uint8_t* __restrict__ s = B.s;
-    const bool flag4 = stride <= 32768u;
-    const uint32_t omask = flag4 ? 0x7fffu : 0xffffu;
-    const int mflimit = n - kMFLimit, matchlimit = n - kLastLiterals;
-    const int hi = lo + S < n ? lo + S : n;
-    const int plim = mflimit < hi - 4 ? mflimit : hi - 4;
-    const int elim = matchlimit < hi ? matchlimit : hi;
-    const int last_w = plim >> 5;
-    const uint16_t* __restrict__ offrow = offarr + (size_t)bl * stride;
-    bool done = lo >= n || lo > plim;
-    int wi = lo >> 5;
-    uint32_t mw = done ? 0u : mem.mask(wi);
-    int anchor = lo, rel = 0;
-    uint2* sp = seq + (size_t)lane * slot;
-    uint2* const sp0 = sp;
-    while (!__all_sync(FULL, done)) {
-      // A: next match at or after my cursor
-      int pm = -1, ed = 0, len = 4;
-      bool x4 = true;
-      while (!done && pm < 0) {
-        if (mw == 0u) {
-          wi++;
-          if (wi > last_w) done = true;
-          else mw = mem.mask(wi);
-        } else {
-          const int q = (wi << 5) + __ffs(mw) - 1;
-          if (q > plim) {
-            done = true;
-          } else {
-            pm = q;
-            const uint32_t o16 = offrow[q];
-            ed = (int)(o16 & omask);
-            x4 = (flag4 && (o16 & 0x8000u)) || q + 4 >= elim;
-          }
-        }
-      }
-      // B: measure the matches that are not flagged "exactly 4", one after the other, with all lanes
-      unsigned need = __ballot_sync(FULL, pm >= 0 && !x4);
-      while (need) {
-        const int l = __ffs(need) - 1;
-        need &= need - 1;
-        const int pm_l = __shfl_sync(FULL, pm, l), d_l = __shfl_sync(FULL, ed, l), elim_l = __shfl_sync(FULL, elim, l);
-        int len_l = elim_l - pm_l;
-        for (int pos = pm_l + 4 + lane;; pos += 32) {
-          const bool stop = pos >= elim_l || __ldg(s + pos) != __ldg(s + pos - d_l);
-          const unsigned bm = __ballot_sync(FULL, stop);
-          if (bm) {
-            const int e = pos - lane + __ffs(bm) - 1;
-            len_l = (e < elim_l ? e : elim_l) - pm_l;
-            break;
-          }
-        }
-        if (lane == l) len = len_l;
-      }
-      // C: one sequence per lane
-      if (pm >= 0) {
-        if (sp == sp0) {
-          R.pm0 = pm;
-          R.len0 = len;
-          R.d0 = ed;
-          *sp++ = make_uint2((uint32_t)pm, (uint32_t)len);
-        } else {
-          const int lit = pm - anchor;
-          *sp++ = make_uint2((uint32_t)anchor | ((uint32_t)lit << 16), (uint32_t)len | ((uint32_t)rel << 16));
-          rel += lzparse::seq_size<CODEC>(lit, len, ed);
-        }
-        const int p = pm + len;
-        anchor = p;
-        const int nw = p >> 5;
-        if (nw != wi) {
-          wi = nw;
-          if (wi > last_w) {
-            done = true;
-            mw = 0u;
-          } else {
-            mw = mem.mask(wi);
-          }
-        }
-        mw &= ~0u << (p & 31);
-      }
-    }
-    R.nrec = (int)(sp - sp0);
-    R.rest = rel;
-    R.last_end = R.nrec ? anchor : -1;
-  }
-  __syncwarp();  // staged records are visible to the other lanes
-
-  // 1. anchor of my first sequence = the last match end of any earlier lane (0 if none)
-  int amax = R.last_end;
-#pragma unroll
-  for (int d = 1; d < 32; d <<= 1) {
-    const int t = __shfl_up_sync(FULL, amax, d);
-    if (lane >= d && t > amax) amax = t;
-  }
-  int anchor_in = __shfl_up_sync(FULL, amax, 1);
-  if (lane == 0 || anchor_in < 0) anchor_in = 0;
-  const int anchor_f = __shfl_sync(FULL, amax, 31) < 0 ? 0 : __shfl_sync(FULL, amax, 31);
-  // 2. sizes and counts
-  const int size0 = R.nrec ? lzparse::seq_size<CODEC>(R.pm0 - anchor_in, R.len0, R.d0) : 0;
-  int inc = size0 + R.rest, cnt = R.nrec;
-#pragma unroll
-  for (int d = 1; d < 32; d <<= 1) {
-    const int t = __shfl_up_sync(FULL, inc, d), u = __shfl_up_sync(FULL, cnt, d);
-    if (lane >= d) {
-      inc += t;
-      cnt += u;
-    }
-  }
-  const int op0 = SNAPPY ? (n < 128 ? 1 : n < 16384 ? 2 : 3) : 0;  // Snappy: varint(n) comes first
-  const int base = op0 + inc - (size0 + R.rest);                  // my first record's output offset
-  const int N = __shfl_sync(FULL, cnt, 31);
-  int total = op0 + __shfl_sync(FULL, inc, 31);
-  // 3. compaction
-  for (int t = 0; t < N; t += 32) {
-    const int i = t + lane;
-    const int ic = i < N ? i : N - 1;  // every lane takes part in the shuffles; the surplus lanes are masked at the end
-    int k = 0;                         // owner: first lane whose inclusive record count exceeds ic
-#pragma unroll
-    for (int step = 16; step >= 1; step >>= 1) {
-      const int c = __shfl_sync(FULL, cnt, k + step - 1);
-      if (c <= ic) k += step;
-    }
-    const int j = ic - (__shfl_sync(FULL, cnt, k) - __shfl_sync(FULL, R.nrec, k));
-    const int base_k = __shfl_sync(FULL, base, k), size0_k = __shfl_sync(FULL, size0, k),
-              anc_k = __shfl_sync(FULL, anchor_in, k);
-    uint2 r = seq[(size_t)k * slot + j];
-    if (j == 0) {
-      const int pm = (int)r.x, len = (int)r.y;
-      r.x = (uint32_t)anc_k | ((uint32_t)(pm - anc_k) << 16);
-      r.y = (uint32_t)len | ((uint32_t)base_k << 16);
-    } else {
-      r.y += (uint32_t)(base_k + size0_k) << 16;
-    }
-    __syncwarp();
-    if (i < N) seq[i] = r;
-    __syncwarp();
-  }
-  // 4. final literals, counts, sizes
-  if (lane == 0) {
-    uint32_t ns = (uint32_t)N;
-    const int lit = n - anchor_f;
-    if (ZSTD) {
-      seq[ns++] = make_uint2((uint32_t)anchor_f | ((uint32_t)lit << 16), (uint32_t)total << 16);
-      nseq[b] = ns;
-    } else if (SNAPPY) {
-      if (lit) {
-        seq[ns++] = make_uint2((uint32_t)anchor_f | ((uint32_t)lit << 16), (uint32_t)total << 16);
-        total += lit + (lit - 1 < 60 ? 1 : lit - 1 < 256 ? 2 : 3);
-      }
-      nseq[b] = ns;
-      csize[b] = (uint32_t)total;
-      sizes[b] = 4u + (uint64_t)total;
-    } else {
-      seq[ns++] = make_uint2((uint32_t)anchor_f | ((uint32_t)lit << 16), (uint32_t)total << 16);
-      total += 1 + lit + (lit >= 15 ? (lit - 15) / 255 + 1 : 0);
-      const bool fail = total > n - 1;  // LZ4BlockOutputStream stores RAW when compressedLength >= originalLength
-      nseq[b] = ns;
-      csize[b] = fail ? ((uint32_t)n | 0x80000000u) : (uint32_t)total;
-      sizes[b] = 21u + (uint64_t)(fail ? n : total);
-    }
-  }
-}
-
-// ------------------------------------------------------------------------------------------------------------
 // C: emission, one lane per sequence, into the block's final packed position; also writes the LZ4Block header
 // ------------------------------------------------------------------------------------------------------------
 __device__ __forceinline__ int lz4b_level(uint32_t block_size) {
@@ -895,19 +543,6 @@ __global__ void __launch_bounds__(kEmitThreads) lz4_emit_kernel(
 // launchers
 // ------------------------------------------------------------------------------------------------------------
 int g_lz4_hlog = 12;  // B2S_LZ4_HLOG (api.cu reads it once at init); 12 is the specified default
-// B2S_LZ4_PIPE selects the match / parse generation (read once at b2s_init):
-//   1 (default)  lz4_match_kernel (offsets + full match lengths) -> lz4_parse_kernel (thread per block, no source access)
-//   4            lz4_match2_kernel (offsets only, 71 instead of 152 warp-instructions per window) -> lz4_parse4_kernel
-//                (warp per block, lane per sub-chunk).  A different — sub-chunked — parse, i.e. slightly different
-//                bytes (specification: compressor 2 in oracle/); lower latency for task-sized batches, but measured
-//                slower at scale: what the match kernel saves, measuring matches lane by lane costs again in scattered
-//                32-byte-sector traffic
-//   (2 / 3, match2 -> thread-per-block parses with in-parse extension, were measured slower still and removed)
-int g_lz4_pipe = 1;
-static int pipe_for(uint32_t codec) {
-  (void)codec;
-  return g_lz4_pipe;
-}
 
 template <int HLOG>
 static void launch_match_t(const uint8_t* src_base, const uint64_t* d_src_off, const uint64_t* d_src_len,
@@ -927,58 +562,33 @@ static void launch_match_t(const uint8_t* src_base, const uint64_t* d_src_off, c
       d_counter);
 }
 
-template <int HLOG>
-static void launch_match2_t(const uint8_t* src_base, const uint64_t* d_src_off, const uint64_t* d_src_len,
-                            const uint32_t* d_blk_base, uint32_t n_streams, uint32_t b0, uint32_t m,
-                            uint32_t block_size, uint32_t stride, uint16_t* d_off, uint32_t* d_mask,
-                            unsigned int* d_counter, cudaStream_t st) {
-  const size_t smem = (size_t)kMatchWarps * (2u << HLOG);
-  cudaFuncSetAttribute(lz4_match2_kernel<HLOG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  int per_sm = 0;
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, lz4_match2_kernel<HLOG>, kMatchWarps * 32, smem);
-  if (per_sm < 1) per_sm = 1;
-  uint64_t want = ((uint64_t)m + kMatchWarps - 1) / kMatchWarps;
-  uint64_t grid = (uint64_t)kSMs * per_sm;  // persistent: one wave, warps pull blocks from the counter
-  if (grid > want) grid = want;
-  lz4_match2_kernel<HLOG><<<(unsigned)grid, kMatchWarps * 32, smem, st>>>(
-      src_base, d_src_off, d_src_len, d_blk_base, n_streams, b0, m, block_size, stride, d_off, d_mask, d_counter);
-}
-
-// Workspace of one pass over `m` codec blocks, by pipeline generation and codec:
-//   off   u16 per position                                     (all)
-//   aux   generation 1: ml u16 per position; generation >= 2: one 32-bit match mask per window
-//   seq   8-byte records, max_seq per block                     (all)
+// Workspace of one pass over `m` codec blocks:
+//   off   u16 per position
+//   ml    u16 per position
+//   seq   8-byte records, max_seq per block
 //   bits  zstd_bits_stride(): sequence-section header + bitstream (Zstandard only)
 struct Lz4Ws {
   uint32_t stride, max_seq;
   uint16_t *off, *ml;
-  uint32_t* mask;
   uint2* seq;
   uint8_t* bits;
 };
-static size_t ws_aux_bytes(size_t stride, int pipe) { return pipe == 1 ? stride * 2 : stride / 8; }
-static size_t ws_max_seq(size_t stride, int pipe) {
-  // generation 4 stages 32 lists of up to S/4 records at slots of S/4 + 1 before compacting them in place
-  return pipe == 4 ? 32 * (parse4_sub((uint32_t)stride) / 4 + 1) + 2 : stride / 4 + 2;
-}
+static size_t ws_max_seq(size_t stride) { return stride / 4 + 2; }
 size_t lz4_compress_ws_bytes(uint32_t chunk_blocks, uint32_t block_size, uint32_t codec) {
   const size_t stride = (block_size + 31u) & ~31u;
-  const int pipe = pipe_for(codec);
-  const size_t per_block = stride * 2 + ws_aux_bytes(stride, pipe) + ws_max_seq(stride, pipe) * 8 +
+  const size_t per_block = stride * 2 + stride * 2 + ws_max_seq(stride) * 8 +
                            (codec == B2S_CODEC_ZSTD ? zstd_bits_stride(stride) : 0);
   return (size_t)chunk_blocks * per_block + 1024;
 }
-static Lz4Ws carve_ws(uint8_t* d_ws, uint32_t m, uint32_t block_size, uint32_t codec) {
+static Lz4Ws carve_ws(uint8_t* d_ws, uint32_t m, uint32_t block_size) {
   Lz4Ws w;
-  const int pipe = pipe_for(codec);
   w.stride = (block_size + 31u) & ~31u;
-  w.max_seq = (uint32_t)ws_max_seq(w.stride, pipe);
+  w.max_seq = (uint32_t)ws_max_seq(w.stride);
   size_t at = 0;
   w.off = reinterpret_cast<uint16_t*>(d_ws);
   at += (size_t)m * w.stride * 2;
   w.ml = reinterpret_cast<uint16_t*>(d_ws + at);
-  w.mask = reinterpret_cast<uint32_t*>(d_ws + at);
-  at += (size_t)m * ws_aux_bytes(w.stride, pipe);
+  at += (size_t)m * w.stride * 2;
   at = (at + 15) & ~size_t(15);
   w.seq = reinterpret_cast<uint2*>(d_ws + at);
   at += (size_t)m * w.max_seq * 8;
@@ -987,18 +597,11 @@ static Lz4Ws carve_ws(uint8_t* d_ws, uint32_t m, uint32_t block_size, uint32_t c
 }
 
 template <int CODEC>
-static void launch_parse_t(const uint8_t* src_base, const uint64_t* d_src_off, const uint64_t* d_src_len,
-                           const uint32_t* d_blk_base, uint32_t n_streams, uint32_t b0, uint32_t m,
-                           uint32_t block_size, const Lz4Ws& w, uint32_t* d_nseq, uint32_t* d_csize, uint64_t* d_sizes,
-                           cudaStream_t st) {
-  const int pipe = pipe_for(CODEC == 0 ? B2S_CODEC_LZ4BLOCK : CODEC == 1 ? B2S_CODEC_SNAPPY_XERIAL : B2S_CODEC_ZSTD);
-  if (pipe == 4)
-    lz4_parse4_kernel<CODEC><<<(m + kParse4Warps - 1) / kParse4Warps, kParse4Warps * 32, 0, st>>>(
-        src_base, d_src_off, d_src_len, d_blk_base, n_streams, b0, m, block_size, w.stride, w.max_seq, w.off, w.mask,
-        w.seq, d_nseq, d_csize, d_sizes);
-  else
-    lz4_parse_kernel<CODEC><<<(m + 63) / 64, 64, 0, st>>>(d_src_len, d_blk_base, n_streams, b0, m, block_size, w.stride,
-                                                          w.max_seq, w.ml, w.seq, d_nseq, d_csize, d_sizes);
+static void launch_parse_t(const uint64_t* d_src_len, const uint32_t* d_blk_base, uint32_t n_streams, uint32_t b0,
+                           uint32_t m, uint32_t block_size, const Lz4Ws& w, uint32_t* d_nseq, uint32_t* d_csize,
+                           uint64_t* d_sizes, cudaStream_t st) {
+  lz4_parse_kernel<CODEC><<<(m + 63) / 64, 64, 0, st>>>(d_src_len, d_blk_base, n_streams, b0, m, block_size, w.stride,
+                                                        w.max_seq, w.ml, w.seq, d_nseq, d_csize, d_sizes);
 }
 
 void launch_lz4_match(const uint8_t* src_base, const uint64_t* d_src_off, const uint64_t* d_src_len,
@@ -1007,15 +610,12 @@ void launch_lz4_match(const uint8_t* src_base, const uint64_t* d_src_off, const 
                       cudaEvent_t ev0, cudaEvent_t ev1, int hlog) {
   if (!m) return;
   const uint32_t near_limit = codec == B2S_CODEC_SNAPPY_XERIAL ? 2048u : 0u;
-  const Lz4Ws w = carve_ws(d_ws, m, block_size, codec);
+  const Lz4Ws w = carve_ws(d_ws, m, block_size);
   cudaMemsetAsync(d_counter, 0, sizeof(unsigned int), st);
   if (ev0) cudaEventRecord(ev0, st);
-#define B2S_LZ4M(H)                                                                                                    \
-  (pipe_for(codec) == 1                                                                                                \
-       ? launch_match_t<H>(src_base, d_src_off, d_src_len, d_blk_base, n_streams, b0, m, block_size, w.stride,         \
-                           near_limit, w.off, w.ml, d_counter, st)                                                     \
-       : launch_match2_t<H>(src_base, d_src_off, d_src_len, d_blk_base, n_streams, b0, m, block_size, w.stride, w.off, \
-                            w.mask, d_counter, st))
+#define B2S_LZ4M(H)                                                                                        \
+  launch_match_t<H>(src_base, d_src_off, d_src_len, d_blk_base, n_streams, b0, m, block_size, w.stride, near_limit, \
+                    w.off, w.ml, d_counter, st)
   switch (hlog > 0 ? hlog : g_lz4_hlog) {
     case 10: B2S_LZ4M(10); break;
     case 11: B2S_LZ4M(11); break;
@@ -1031,12 +631,11 @@ void launch_lz4_parse_emit(const uint8_t* src_base, const uint64_t* d_src_off, c
                            const uint32_t* d_blk_base, uint32_t n_streams, uint32_t b0, uint32_t m,
                            uint32_t block_size, uint32_t codec, uint8_t* d_ws, uint32_t* d_nseq, uint32_t* d_csize,
                            const uint32_t* d_hash, uint64_t* d_sizes, uint64_t* d_running_total, uint64_t* d_scan_ws,
-                           uint8_t* dst_base, uint64_t dst_cap, cudaStream_t st, uint64_t* launches,
-                           cudaEvent_t ev_parsed) {
+                           uint8_t* dst_base, uint64_t dst_cap, cudaStream_t st, uint64_t* launches) {
   if (!m) return;
-  const Lz4Ws w = carve_ws(d_ws, m, block_size, codec);
+  const Lz4Ws w = carve_ws(d_ws, m, block_size);
   if (codec == B2S_CODEC_ZSTD) {
-    launch_parse_t<2>(src_base, d_src_off, d_src_len, d_blk_base, n_streams, b0, m, block_size, w, d_nseq, d_csize, d_sizes, st);
+    launch_parse_t<2>(d_src_len, d_blk_base, n_streams, b0, m, block_size, w, d_nseq, d_csize, d_sizes, st);
     uint8_t* d_bits = w.bits;
     // d_hash is unused by this codec and carries the bitstream sizes from the entropy stage to the emit kernel
     launch_zstd_seqenc(src_base, d_src_off, d_src_len, d_blk_base, n_streams, b0, m, block_size, w.stride, w.max_seq,
@@ -1048,15 +647,14 @@ void launch_lz4_parse_emit(const uint8_t* src_base, const uint64_t* d_src_off, c
     return;
   }
   if (codec == B2S_CODEC_SNAPPY_XERIAL) {
-    launch_parse_t<1>(src_base, d_src_off, d_src_len, d_blk_base, n_streams, b0, m, block_size, w, d_nseq, d_csize, d_sizes, st);
+    launch_parse_t<1>(d_src_len, d_blk_base, n_streams, b0, m, block_size, w, d_nseq, d_csize, d_sizes, st);
     launch_exclusive_scan_u64(d_sizes + b0, m, d_running_total, d_scan_ws, st, launches, d_running_total);
     launch_snappy_emit(src_base, d_src_off, d_src_len, d_blk_base, n_streams, b0, m, block_size, w.stride, w.max_seq,
                        w.off, w.seq, d_nseq, d_csize, d_sizes, dst_base, dst_cap, st, launches);
     *launches += 1;
     return;
   }
-  launch_parse_t<0>(src_base, d_src_off, d_src_len, d_blk_base, n_streams, b0, m, block_size, w, d_nseq, d_csize, d_sizes, st);
-  if (ev_parsed) cudaEventRecord(ev_parsed, st);  // B2S_TRACE timeline
+  launch_parse_t<0>(d_src_len, d_blk_base, n_streams, b0, m, block_size, w, d_nseq, d_csize, d_sizes, st);
   // packed offsets of this chunk's blocks, chained onto the running total of the chunks before it
   launch_exclusive_scan_u64(d_sizes + b0, m, d_running_total, d_scan_ws, st, launches, d_running_total);
   lz4_emit_kernel<<<(m + kEmitThreads / 32 - 1) / (kEmitThreads / 32), kEmitThreads, 0, st>>>(

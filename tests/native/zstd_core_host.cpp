@@ -156,8 +156,6 @@ extern "C" long long zc_compress_model(const unsigned char* src, unsigned long l
                                        unsigned char* dst, unsigned long long cap) {
   return zc_compress_model_hlog(src, n, block_size, dst, cap, 12);
 }
-static int g_model_subchunk = 0;  // 1: the sub-chunk parallel parse of B2S_LZ4_PIPE=4
-extern "C" void zc_model_subchunk(int on) { g_model_subchunk = on; }
 // hash_log: 12 = unspecified level / level 2; level 1 -> 11, level >= 3 -> 13 (hlog_for_level in csrc/api.cu)
 extern "C" long long zc_compress_model_hlog(const unsigned char* src, unsigned long long n, unsigned block_size,
                                             unsigned char* dst, unsigned long long cap, int hash_log) {
@@ -183,27 +181,15 @@ extern "C" long long zc_compress_model_hlog(const unsigned char* src, unsigned l
       std::vector<uint16_t> off((size_t)bn, 0);
       win_find_offsets(s, bn, hash_log, off);
       const int mflimit = bn - 12, matchlimit = bn - 5;
-      // the warp-parallel parse restarts in every sub-chunk of 1/32 block (rounded up to 32 positions); a match neither
-      // starts in a sub-chunk's last three positions nor extends past its end (oracle: orc_lz4_compress_block_win_sub)
-      const int stride = (int)((block_size + 31u) & ~31u);
-      const int sub = g_model_subchunk ? ((stride >> 5) + 31) & ~31 : bn + 1;  // bn + 1: one cursor over the block
       int p = 0;
       while (p <= mflimit) {
-        int chunk_hi = (p / sub + 1) * sub;
-        if (chunk_hi > bn) chunk_hi = bn;
-        const int plim = mflimit < chunk_hi - 4 ? mflimit : chunk_hi - 4;
-        const int elim = matchlimit < chunk_hi ? matchlimit : chunk_hi;
-        if (p > plim) {
-          p = chunk_hi;
-          continue;
-        }
         if (!off[p]) {
           p++;
           continue;
         }
         const int c = p - off[p];
         int ml = 4;
-        while (p + ml < elim && s[p + ml] == s[c + ml]) ml++;
+        while (p + ml < matchlimit && s[p + ml] == s[c + ml]) ml++;
         seqs.push_back(Seq{(uint32_t)(p - anchor), (uint32_t)ml, off[p]});
         lits.insert(lits.end(), s + anchor, s + p);
         p += ml;

@@ -1,5 +1,7 @@
 """The warp-per-block LZ4 decoder (lz4_decode_warp_kernel): token boundaries found in 128-byte windows, length
-extensions, decoy literal bytes, match forms, every corruption rule, RAW blocks and empty streams.
+extensions, decoy literal bytes, match forms, every corruption rule, RAW blocks and empty streams.  A batch with a
+codec block over 64 KiB (lz4-java allows up to 32 MiB) goes to the tile decoder (lz4_decompress_kernel) as a whole:
+blocks of 128 KiB to 32 MiB, a batch mixing large and small blocks, and every corruption rule inside a large block.
 
 The streams are LZ4Block (lz4-java framing) assembled sequence by sequence, so that token starts, offsets and
 extension bytes land at known window positions.  Every good stream is checked against the oracle's decoder first, then
@@ -225,18 +227,29 @@ def test_match_forms(capi, oracle):
     check_good(capi, oracle, streams, expected)
 
 
-@pytest.mark.parametrize("size", [13, 100, 1000, 4096, 32768, 65536])
+@pytest.mark.parametrize("size", [13, 100, 1000, 4096, 32768, 65536, 131072, 1 << 20])
 def test_compressed_blocks_of_every_size(capi, oracle, size):
-    """blocks of 13 bytes to 64 KiB from the oracle's compressor and from liblz4"""
+    """blocks of 13 bytes to 1 MiB from the oracle's compressor and from liblz4"""
     streams, expected = [], []
-    # (random bytes in 64 KiB blocks would expand past 64 KiB, which is the tile decoder's case)
-    for kind in ("terasort", "text", "runs", "period") + (("random",) if size < 65536 else ()):
+    # (random bytes in 64 KiB blocks reach 64 KiB compressed, which would move this batch to the tile decoder)
+    for kind in ("terasort", "text", "runs", "period") + (("random",) if size != 65536 else ()):
         data = corpus(oracle, kind, size * 3 + 7, seed=size)
         streams.append(oracle_stream(oracle, data, size))
         expected.append(data)
         streams.append(liblz4_stream(oracle, data, size))
         expected.append(data)
     check_good(capi, oracle, streams, expected)
+
+
+def test_largest_blocks_and_mixed_block_sizes(capi, oracle):
+    """one 32 MiB codec block (lz4-java's largest), and a batch in which one stream of 128 KiB blocks sends 32 KiB-block
+    streams to the tile decoder with it"""
+    big = corpus(oracle, "terasort", 32 << 20, seed=7)
+    check_good(capi, oracle, [liblz4_stream(oracle, big, 32 << 20)], [big])
+    data = [corpus(oracle, kind, 300000, seed=8) for kind in ("terasort", "text", "random", "runs")]
+    streams = [oracle_stream(oracle, data[0], 32768), liblz4_stream(oracle, data[1], 131072),
+               liblz4_stream(oracle, data[2], 32768), oracle.lz4block_compress(data[3])]
+    check_good(capi, oracle, streams, data)
 
 
 def test_raw_blocks_and_empty_streams(capi, oracle):
@@ -305,5 +318,24 @@ def test_one_corrupt_stream_among_good_ones(capi, oracle, rule):
             outs, st, dst, r = decode(capi, streams, dev)
             assert st == [0, capi.E_CORRUPT, 0], (rule, n, dev)
             assert outs[0] == data and outs[2] == data, (rule, n, dev)
+            end = int(r["dst_off"][2]) + int(r["dst_len"][2])
+            assert (dst[end:] == 0xA5).all()
+
+
+def test_corrupt_large_block_among_good_ones(capi, oracle):
+    """the bad sequence after 27000 good ones, in a block that claims over 128 KiB, so the tile decoder takes the
+    batch: the bad stream alone is CORRUPT (an offset cannot reach past 135000 output bytes, hence no
+    offset_past_output)"""
+    data = [corpus(oracle, kind, 100000, seed=9) for kind in ("terasort", "text")]
+    good = [liblz4_stream(oracle, data[0], 131072), oracle.lz4block_compress(data[1])]
+    for rule in [r for r in RULES if r != "offset_past_output"]:
+        payload, olen = corrupt_case(rule, 27000)
+        bad = frame(oracle, payload, olen) + END_MARK
+        with pytest.raises(IOError):
+            oracle.lz4block_decompress(bad)
+        for dev in (False, True):
+            outs, st, dst, r = decode(capi, [good[0], bad, good[1]], dev)
+            assert st == [0, capi.E_CORRUPT, 0], (rule, dev)
+            assert outs[0] == data[0] and outs[2] == data[1], (rule, dev)
             end = int(r["dst_off"][2]) + int(r["dst_len"][2])
             assert (dst[end:] == 0xA5).all()

@@ -8,10 +8,7 @@ The wave is built as bench.py builds it (gen_terasort_dev, seed 42, then compres
              LZ4, the lz4_copy_kernel launches for Snappy
   decode_ms  top_kernel_ms: the whole decode (Snappy: first token launch to last copy launch)
   read_ms    kernel_ms: the whole read pass (CRC32C verify, descriptors, decode, XXH32 verify)
-A child process, run first, repeats one read call with B2S_TRACE=1 and reports the per-chunk timeline of the Snappy
-decoder: the token walk of a chunk runs on the side stream while the previous chunk's copies run on the main one (LZ4
-decodes in one launch and has no such rows).  The card's name and power
-limit are read in the same run.
+The card's name and power limit are read in the same run.
 
     python tools/decode_split.py [--calls 7] [--warmup 3] [--codec lz4|snappy] [--blocks N] [--chunk-blocks N]
 
@@ -20,7 +17,6 @@ Prints one JSON document.  --chunk-blocks sets B2S_LZ4D_CHUNK_BLOCKS (Snappy: co
 import argparse
 import json
 import os
-import re
 import statistics
 import subprocess
 import sys
@@ -33,8 +29,6 @@ sys.path.insert(0, ROOT)
 RECORD = 104
 LZ4_BLOCK = 32768
 RECORDS_PER_BLOCK = 6453  # bench.py config 2: 671,112-byte shuffle blocks
-TRACE_ROW = re.compile(r"chunk +(\d+): A\(match\|tokens\) +([\d.]+)\.\. *([\d.]+) +B\(parse\|copy\) +([\d.]+)\.\. *"
-                       r"([\d.]+) +end +([\d.]+) ms")
 
 
 def card():
@@ -69,23 +63,6 @@ def read_call(c, codec, wave):
     return c.last_timing()
 
 
-def traced_timeline(args):
-    """per-chunk timeline of one read call, from a child process run with B2S_TRACE=1"""
-    env = dict(os.environ, B2S_TRACE="1")
-    cmd = [sys.executable, os.path.abspath(__file__), "--trace-only", "--codec", args.codec,
-           "--blocks", str(args.blocks)]
-    p = subprocess.run(cmd, env=env, capture_output=True, text=True)
-    if p.returncode != 0:
-        raise SystemExit("traced run failed:\n" + p.stderr)
-    timeline = []
-    for line in p.stderr.split("--- read call ---", 1)[-1].splitlines():
-        m = TRACE_ROW.search(line)
-        if m:
-            k, t0, t1, c0, c1, end = m.groups()
-            timeline.append({"chunk": int(k), "tokens_ms": [float(t0), float(t1)], "copy_ms": [float(c0), float(end)]})
-    return timeline
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--calls", type=int, default=7)
@@ -93,15 +70,11 @@ def main():
     ap.add_argument("--codec", default="lz4", choices=["lz4", "snappy"])
     ap.add_argument("--blocks", type=int, default=16000, help="shuffle blocks in the wave (bench.py config 2: 16,000)")
     ap.add_argument("--chunk-blocks", type=int, default=0, help="B2S_LZ4D_CHUNK_BLOCKS (0 = the library default)")
-    ap.add_argument("--trace-only", action="store_true", help=argparse.SUPPRESS)  # the B2S_TRACE=1 child
     args = ap.parse_args()
     if args.calls < 5:
         raise SystemExit("--calls must be >= 5")
     if args.chunk_blocks:
         os.environ["B2S_LZ4D_CHUNK_BLOCKS"] = str(args.chunk_blocks)
-
-    if not args.trace_only:  # first, while this process holds no device memory: both waves do not fit at once
-        timeline = traced_timeline(args)
 
     import spark_s3_shuffle_b200 as pkg
 
@@ -109,12 +82,6 @@ def main():
     c.init(1)
     codec = {"lz4": c.CODEC_LZ4BLOCK, "snappy": c.CODEC_SNAPPY_XERIAL}[args.codec]
     wave = make_wave(c, codec, args.blocks)
-    if args.trace_only:  # one traced read call; the timeline rows go to stderr, after this marker
-        read_call(c, codec, wave)
-        sys.stderr.flush()
-        os.write(2, b"--- read call ---\n")
-        read_call(c, codec, wave)
-        return 0
 
     for _ in range(args.warmup):
         read_call(c, codec, wave)
@@ -138,7 +105,6 @@ def main():
         "read_ms": summary(read),
         "copy_share_of_decode": round(statistics.median(copy) / statistics.median(decode), 3),
         "copy_share_of_read": round(statistics.median(copy) / statistics.median(read), 3),
-        "timeline_ms": timeline,
     }
     print(json.dumps(doc, indent=1))
     return 0

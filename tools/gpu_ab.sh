@@ -1,7 +1,6 @@
 # A/B harness for the GPU box (one `gpurun -- 'bash tools/gpu_ab.sh <spec-file>'` call = many variants on the same box).
 # The spec file holds one variant per line:   <name> [ENV=VALUE ...] [-- bench.py args]
-# e.g.   p1        B2S_LZ4_PIPE=1
-#        p4_serial B2S_LZ4_PIPE=4 B2S_OVERLAP=0
+# e.g.   hlog11    B2S_LZ4_HLOG=11
 # Every variant runs `bench.py --no-e2e --no-cpu --steps 4 --warmup 3` (device-resident) unless args are given; results
 # land in gpurun_out/ab_<name>.json and a one-line summary is printed.  This is how the round-2 tables in
 # profiles/r2_compress_generations.md / r2_tma_tokens.md were produced (env switches: csrc/api.cu, b2s_init).
