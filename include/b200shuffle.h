@@ -48,6 +48,11 @@ extern "C" {
 #define B2S_CHECKSUM_CRC32 2
 #define B2S_CHECKSUM_CRC32C 3 /* north-star addition; the Scala shim adds the "CRC32C" case */
 
+/* key types of the row sort (b2s_decompress_sort_rows_*) */
+#define B2S_KEY_BYTES 0 /* key_len (1..16) bytes, unsigned, lexicographic */
+#define B2S_KEY_INT32 1 /* 4 bytes, little-endian two's complement: UnsafeRow's IntegerType / DateType slot */
+#define B2S_KEY_INT64 2 /* 8 bytes, little-endian two's complement: LongType, TimestampType, Decimal(p <= 18) */
+
 /* per-block status / call errors.  The Scala shim maps them to the reference's exception types:            */
 #define B2S_OK 0
 #define B2S_E_CORRUPT (-1)       /* IOException("Stream is corrupted")  (LZ4BlockInputStream et al. [U])   */
@@ -208,6 +213,46 @@ int b2s_decompress_sort_dev(uint32_t dev_index, uint32_t codec, uint32_t checksu
                             uint32_t record_bytes, uint32_t key_off, uint32_t key_len, uint8_t* dst_base,
                             uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records, int32_t* status,
                             int32_t* bad_slice);
+
+/* ---- read side, row-sorted: verify + decompress + sort a reduce task's UnsafeRow records by one typed key ----
+ * The Spark SQL counterpart of b2s_decompress_sort_*: the SortExec that a sort-merge join runs on every reducer right
+ * after the shuffle read.  Blocks, slices and checksums are those of b2s_decompress_sort_packed.  A decoded block is a
+ * sequence of records as UnsafeRowSerializer writes them: [s: int32 big-endian][s bytes of row], s >= 0, no end
+ * marker (the last record ends exactly at the block's decoded end).  A block of several concatenated streams
+ * (ShuffleBlockBatchId) is still a whole number of records; an empty block holds none.
+ * Key (offsets count from the start of the row, after the 4-byte size):
+ *   B2S_KEY_BYTES: key_len (1..16) bytes at key_off, unsigned, lexicographic (the fixed-size call's meaning)
+ *   B2S_KEY_INT32: 4 bytes at key_off (key_len 4), little-endian two's complement, ordered as signed
+ *   B2S_KEY_INT64: the same with 8 bytes (key_len 8)
+ * Nulls: null_field = -1 means the key has no null bit.  With null_field >= 0 a record is null when bit
+ * (null_field & 63) of the little-endian u64 at row offset 8 * (null_field >> 6) is set (UnsafeRow's null bitset);
+ * null records sort before every other record (ASC NULLS FIRST) and their key bytes are ignored.
+ * Output: every record, size prefix included, back to back in ascending key order — again a valid UnsafeRowSerializer
+ * stream.  The sort is stable: equal keys, and nulls among themselves, keep block order, then their order within the
+ * block.  *dst_total = decoded bytes, *n_records = record count.
+ * Per block, B2S_E_CORRUPT (b2s_last_error() names the block and the byte offset of its first bad record) when a size is
+ * negative, a record runs past the block end, the block ends inside a size prefix, a row is shorter than key_off +
+ * key_len, or (null_field >= 0) a row does not hold the null-bit word.  Checksums, B2S_E_DST_TOO_SMALL, B2S_E_NOMEM,
+ * "nothing is sorted when a block fails", codec NONE, the read lane and the 1 GiB buffer trim are as in
+ * b2s_decompress_sort_*.
+ * Errors -> B2S_E_ARG: an unknown key_type; key_len outside [1, 16] for BYTES, other than 4 / 8 for INT32 / INT64;
+ * null_field < -1; more than 2^32 - 1 records.
+ * Timing (b2s_last_timing): kernel_ms = verification + decode + framing + sort; top_kernel_ms = framing + sort (from
+ * the end of decoding, including the one readback that sizes the sort: the record count and the per-block framing
+ * verdicts); dominant_ms / dominant_launches = the framing step alone. */
+int b2s_decompress_sort_rows_packed(uint32_t codec, uint32_t checksum_alg, uint32_t n, const uint8_t* src_base,
+                                    const uint64_t* src_off, const uint64_t* src_len, const uint32_t* slice_base,
+                                    const uint64_t* slice_len, const uint64_t* slice_checksum, uint32_t key_type,
+                                    uint32_t key_off, uint32_t key_len, int32_t null_field, uint8_t* dst_base,
+                                    uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records, int32_t* status,
+                                    int32_t* bad_slice);
+/* same, with src_base / dst_base in device memory of dev_index; the descriptor arrays stay host arrays */
+int b2s_decompress_sort_rows_dev(uint32_t dev_index, uint32_t codec, uint32_t checksum_alg, uint32_t n,
+                                 const uint8_t* src_base, const uint64_t* src_off, const uint64_t* src_len,
+                                 const uint32_t* slice_base, const uint64_t* slice_len, const uint64_t* slice_checksum,
+                                 uint32_t key_type, uint32_t key_off, uint32_t key_len, int32_t null_field,
+                                 uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records,
+                                 int32_t* status, int32_t* bad_slice);
 
 /* ---- exchange cache: map outputs kept resident in HBM for reducers on the same device ----
  * (docs/f4_gpu_resident_exchange.md steps 2 and 3, local half.)  The serialized writer's partition step already leaves

@@ -145,6 +145,16 @@ int b2sh_reader_read(b2sh_reader* r, uint32_t* n_blocks);
  * the call are fetched and the call is repeated. */
 int b2sh_reader_read_sorted(b2sh_reader* r, uint32_t record_bytes, uint32_t key_off, uint32_t key_len,
                             const uint8_t** data, uint64_t* len, uint64_t* n_records);
+/* read_sorted_rows(): read() for a Spark SQL exchange whose reducer sorts the rows by one typed key (INTEGRATION.md
+ * §3g, spark.shuffle.s3.gpu.sortRows).  Fetches the task's non-empty blocks as read_sorted() does, then makes ONE
+ * b2s_decompress_sort_rows_packed call: *data / *len / *n_records receive every UnsafeRowSerializer record of the task
+ * ([int32 big-endian size][row]) sorted by the key key_type (B2S_KEY_*) at row offset key_off, nulls first (null_field:
+ * the key's null bit, -1 = none), stable in map, then reduce-id order.  The buffer stays valid until the reader's next
+ * read or its destruction.  A checksum mismatch returns B2SH_E_SPARK with the reference's message, a malformed row
+ * stream B2SH_E_IO.  Codec "none" is verified and sorted only.  The exchange cache is not consulted: every block is
+ * fetched. */
+int b2sh_reader_read_sorted_rows(b2sh_reader* r, uint32_t key_type, uint32_t key_off, uint32_t key_len,
+                                 int32_t null_field, const uint8_t** data, uint64_t* len, uint64_t* n_records);
 int b2sh_reader_block(b2sh_reader* r, uint32_t k, int64_t* map_id, int32_t* start_reduce, int32_t* end_reduce,
                       const uint8_t** data, uint64_t* len);
 uint64_t b2sh_reader_remote_bytes_read(b2sh_reader* r); /* metric parity with storage/S3ShuffleReader.scala:94-95 */

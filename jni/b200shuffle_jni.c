@@ -236,12 +236,13 @@ JNIEXPORT jint JNICALL J(decompressPacked)(JNIEnv* e, jclass c, jint codec, jint
  *      meta: long[2] = {dst_total, n_records}; status, badSlice: int[n].  All arrays go through native copies, so no
  *      Java array is held in a critical region while the GPU works. ---- */
 /* mapIds (NULL: a plain decompressSortPacked): long[n] and cached: int[n] make it an exchange-cache read of the
- * partitions [startReduce, endReduce) of shuffleId */
+ * partitions [startReduce, endReduce) of shuffleId.  rows: a row sort (decompressSortRowsPacked) of UnsafeRow records
+ * by the key keyType at keyOff (recordBytes unused, mapIds NULL) */
 static jint sort_packed(JNIEnv* e, jint shuffleId, jint startReduce, jint endReduce, jlongArray mapIds,
                         jintArray cached, jint codec, jint alg, jint n, jlong src, jlongArray off, jlongArray len,
                         jintArray sliceBase, jlongArray sliceLen, jlongArray sliceChecksum, jint recordBytes,
-                        jint keyOff, jint keyLen, jlong dst, jlong dstCap, jlongArray meta, jintArray status,
-                        jintArray badSlice) {
+                        int rows, jint keyType, jint keyOff, jint keyLen, jint nullField, jlong dst, jlong dstCap,
+                        jlongArray meta, jintArray status, jintArray badSlice) {
   if (n < 0 || !meta || (*e)->GetArrayLength(e, meta) < 2) return B2S_E_ARG;
   if (mapIds && n > 0 && (!cached || (*e)->GetArrayLength(e, mapIds) < n || (*e)->GetArrayLength(e, cached) < n))
     return B2S_E_ARG;
@@ -283,7 +284,13 @@ static jint sort_packed(JNIEnv* e, jint shuffleId, jint startReduce, jint endRed
   uint64_t total = 0, nrec = 0;
   if (rc == 0) {
     const size_t ns = with_slices ? (size_t)sb[n] : 0;
-    if (mapIds)
+    if (rows)
+      rc = b2s_decompress_sort_rows_packed((uint32_t)codec, (uint32_t)alg, (uint32_t)n, PTR(const uint8_t, src), blk,
+                                           blk + N, with_slices ? sb : 0, with_slices ? sl : 0,
+                                           with_slices ? sl + ns : 0, (uint32_t)keyType, (uint32_t)keyOff,
+                                           (uint32_t)keyLen, (int32_t)nullField, PTR(uint8_t, dst), (uint64_t)dstCap,
+                                           &total, &nrec, st, st + N);
+    else if (mapIds)
       rc = b2s_exchange_read_sort_packed((int32_t)shuffleId, (int32_t)startReduce, (int32_t)endReduce, ids, hit,
                                          (uint32_t)codec, (uint32_t)alg, (uint32_t)n, PTR(const uint8_t, src), blk,
                                          blk + N, with_slices ? sb : 0, with_slices ? sl : 0,
@@ -317,7 +324,20 @@ JNIEXPORT jint JNICALL J(decompressSortPacked)(JNIEnv* e, jclass c, jint codec, 
                                                jintArray badSlice) {
   (void)c;
   return sort_packed(e, 0, 0, 0, 0, 0, codec, alg, n, src, off, len, sliceBase, sliceLen, sliceChecksum, recordBytes,
-                     keyOff, keyLen, dst, dstCap, meta, status, badSlice);
+                     0, 0, keyOff, keyLen, -1, dst, dstCap, meta, status, badSlice);
+}
+
+/* ---- read side, row-sorted (a Spark SQL exchange read followed by a SortExec, INTEGRATION.md §3g): verify, decode and
+ *      sort the task's length-prefixed UnsafeRow records by one typed key (keyType B2S_KEY_*, keyOff in the row,
+ *      nullField -1 or the key's null bit).  Arrays as decompressSortPacked. ---- */
+JNIEXPORT jint JNICALL J(decompressSortRowsPacked)(JNIEnv* e, jclass c, jint codec, jint alg, jint n, jlong src,
+                                                   jlongArray off, jlongArray len, jintArray sliceBase,
+                                                   jlongArray sliceLen, jlongArray sliceChecksum, jint keyType,
+                                                   jint keyOff, jint keyLen, jint nullField, jlong dst, jlong dstCap,
+                                                   jlongArray meta, jintArray status, jintArray badSlice) {
+  (void)c;
+  return sort_packed(e, 0, 0, 0, 0, 0, codec, alg, n, src, off, len, sliceBase, sliceLen, sliceChecksum, 0, 1, keyType,
+                     keyOff, keyLen, nullField, dst, dstCap, meta, status, badSlice);
 }
 
 /* ---- exchange cache (INTEGRATION.md §3f): map outputs kept in HBM for reducers on the same device ---- */
@@ -391,7 +411,8 @@ JNIEXPORT jint JNICALL J(exchangeReadSortPacked)(JNIEnv* e, jclass c, jint shuff
   (void)c;
   if (!mapIds) return B2S_E_ARG;
   return sort_packed(e, shuffleId, startReduce, endReduce, mapIds, cached, codec, alg, n, src, off, len, sliceBase,
-                     sliceLen, sliceChecksum, recordBytes, keyOff, keyLen, dst, dstCap, meta, status, badSlice);
+                     sliceLen, sliceChecksum, recordBytes, 0, 0, keyOff, keyLen, -1, dst, dstCap, meta, status,
+                     badSlice);
 }
 
 /* decoded size of each of n compressed streams laid out in one arena (sizes the destination of decompressPacked) */

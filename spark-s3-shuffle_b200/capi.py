@@ -12,6 +12,7 @@ from . import _build
 # ---- constants mirrored from b200shuffle.h ----
 CODEC_NONE, CODEC_LZ4BLOCK, CODEC_SNAPPY_XERIAL, CODEC_ZSTD = 0, 1, 2, 3
 CHECKSUM_NONE, CHECKSUM_ADLER32, CHECKSUM_CRC32, CHECKSUM_CRC32C = 0, 1, 2, 3
+KEY_BYTES, KEY_INT32, KEY_INT64 = 0, 1, 2  # key types of the row sort (decompress_sort_rows_*)
 OK, E_CORRUPT, E_CHECKSUM, E_DST_TOO_SMALL, E_UNSUPPORTED, E_ARG, E_CUDA, E_NOT_INIT, E_NOMEM, E_NOT_CACHED = (
     0, -1, -2, -3, -4, -5, -6, -7, -8, -9)
 NOT_RESIDENT = 2**64 - 1  # b2s_exchange_lookup's length of a map output that is not resident
@@ -70,6 +71,12 @@ PROTOTYPES = [
     ("b2s_decompress_sort_dev", C.c_int,
      [_u32, _u32, _u32, _u32, _vp, _u64p, _u64p, _u32p, _u64p, _u64p, _u32, _u32, _u32, _vp, _u64, _u64p, _u64p, _i32p,
       _i32p]),
+    ("b2s_decompress_sort_rows_packed", C.c_int,
+     [_u32, _u32, _u32, _u8p, _u64p, _u64p, _u32p, _u64p, _u64p, _u32, _u32, _u32, _i32, _u8p, _u64, _u64p, _u64p,
+      _i32p, _i32p]),
+    ("b2s_decompress_sort_rows_dev", C.c_int,
+     [_u32, _u32, _u32, _u32, _vp, _u64p, _u64p, _u32p, _u64p, _u64p, _u32, _u32, _u32, _i32, _vp, _u64, _u64p, _u64p,
+      _i32p, _i32p]),
     ("b2s_exchange_set_budget", C.c_int, [_u32, _u64]),
     ("b2s_partition_compress_cached_packed", C.c_int,
      [_i32, C.c_int64, _u32, _i32, _u32, _u32, _u32, _u64, _u8p, _u64, _u32p, _u32p, _u8p, _u64, _u64p, _u64p, _u64p,
@@ -380,6 +387,26 @@ def decompress_sort_packed(codec, src, off, length, dst, record_bytes, key_off, 
     return dict(total=total.value, n_records=nrec.value, status=st[:n], bad_slice=bad[:n])
 
 
+def decompress_sort_rows_packed(codec, src, off, length, dst, key_type, key_off, key_len, null_field=-1,
+                                checksum_alg=CHECKSUM_NONE, slice_base=None, slice_len=None, slice_checksum=None):
+    """Verifies and decodes a reduce task's blocks of length-prefixed UnsafeRow records ([int32 big-endian size][row])
+    and sorts the records by the typed key at row offset key_off (KEY_BYTES / KEY_INT32 / KEY_INT64; nulls first when
+    null_field >= 0) into dst (stable).  -> dict(total, n_records, status, bad_slice)"""
+    src, dst = _as_u8(src), _as_u8(dst)
+    off = np.ascontiguousarray(off, dtype=np.uint64)
+    length = np.ascontiguousarray(length, dtype=np.uint64)
+    n = off.size
+    sb, sl, sc = _sort_slices(checksum_alg, slice_base, slice_len, slice_checksum)
+    st = np.zeros(max(n, 1), dtype=np.int32)
+    bad = np.zeros(max(n, 1), dtype=np.int32)
+    total, nrec = _u64(0), _u64(0)
+    _check(load().b2s_decompress_sort_rows_packed(codec, checksum_alg, n, _ptr(src), _ptr(off), _ptr(length), _ptr(sb),
+                                                  _ptr(sl), _ptr(sc), key_type, key_off, key_len, null_field,
+                                                  _ptr(dst), dst.size, C.addressof(total), C.addressof(nrec), _ptr(st),
+                                                  _ptr(bad)), "b2s_decompress_sort_rows_packed")
+    return dict(total=total.value, n_records=nrec.value, status=st[:n], bad_slice=bad[:n])
+
+
 # ---------------------------------------------------------------------------------------------------------------
 # device-resident API (bench.py roofline leg); d_* are raw device addresses (ints)
 # ---------------------------------------------------------------------------------------------------------------
@@ -460,6 +487,23 @@ def decompress_sort_dev(codec, d_src, off, length, d_dst, dst_cap, record_bytes,
                                           _ptr(sl), _ptr(sc), record_bytes, key_off, key_len, d_dst, dst_cap,
                                           C.addressof(total), C.addressof(nrec), _ptr(st), _ptr(bad)),
            "b2s_decompress_sort_dev")
+    return dict(total=total.value, n_records=nrec.value, status=st[:n], bad_slice=bad[:n])
+
+
+def decompress_sort_rows_dev(codec, d_src, off, length, d_dst, dst_cap, key_type, key_off, key_len, null_field=-1,
+                             checksum_alg=CHECKSUM_NONE, slice_base=None, slice_len=None, slice_checksum=None, dev=0):
+    """decompress_sort_rows_packed on device-resident blocks (d_src) into a device arena (d_dst)"""
+    off = np.ascontiguousarray(off, dtype=np.uint64)
+    length = np.ascontiguousarray(length, dtype=np.uint64)
+    n = off.size
+    sb, sl, sc = _sort_slices(checksum_alg, slice_base, slice_len, slice_checksum)
+    st = np.zeros(max(n, 1), dtype=np.int32)
+    bad = np.zeros(max(n, 1), dtype=np.int32)
+    total, nrec = _u64(0), _u64(0)
+    _check(load().b2s_decompress_sort_rows_dev(dev, codec, checksum_alg, n, d_src, _ptr(off), _ptr(length), _ptr(sb),
+                                               _ptr(sl), _ptr(sc), key_type, key_off, key_len, null_field, d_dst,
+                                               dst_cap, C.addressof(total), C.addressof(nrec), _ptr(st), _ptr(bad)),
+           "b2s_decompress_sort_rows_dev")
     return dict(total=total.value, n_records=nrec.value, status=st[:n], bad_slice=bad[:n])
 
 

@@ -226,9 +226,11 @@ struct Slot {
   cudaEvent_t ev_t0 = nullptr, ev_t1 = nullptr;            // dominant kernel
   cudaEvent_t ev_h0 = nullptr, ev_h1 = nullptr, ev_d0 = nullptr, ev_d1 = nullptr;  // copies
   cudaEvent_t ev_p0 = nullptr, ev_p1 = nullptr;            // partition step (b2s_partition_compress_*)
+  cudaEvent_t ev_f[4] = {nullptr, nullptr, nullptr, nullptr};  // row framing: walk + count, emit (sort_rows)
   DevBuf meta, scratch, desc, src, dst, zmeta;
   DevBuf pws, parena;  // partition workspace (sort keys, offsets) and the partitioned arena in front of compression
   DevBuf xpieces;      // the copy pieces of an exchange-cache read (exchange.cu)
+  DevBuf fws;          // row framing workspace: bitmap over the decoded arena, tile counts, verdicts (rows.cu)
   PinBuf hmeta;
   // per-launch event pairs around the dominant kernel of a call (grow-only pool; `used` pairs are valid)
   std::vector<cudaEvent_t> ev_dom;
@@ -1099,7 +1101,7 @@ int b2s_init(uint32_t gpu_mask, uint64_t pinned_bytes_per_gpu, uint32_t streams_
         cudaEvent_t* evs2[] = {&S.ev_fork, &S.ev_match[0], &S.ev_match[1], &S.ev_free[0], &S.ev_free[1]};
         for (auto p : evs2) CU(cudaEventCreateWithFlags(p, cudaEventDisableTiming));
         cudaEvent_t* evs[] = {&S.ev_a, &S.ev_b, &S.ev_k0, &S.ev_k1, &S.ev_t0, &S.ev_t1, &S.ev_h0, &S.ev_h1, &S.ev_d0, &S.ev_d1,
-                              &S.ev_p0, &S.ev_p1};
+                              &S.ev_p0, &S.ev_p1, &S.ev_f[0], &S.ev_f[1], &S.ev_f[2], &S.ev_f[3]};
         for (auto p : evs) CU(cudaEventCreate(p));
         // pinned_bytes_per_gpu: the library's own pinned descriptor blocks are sized up front (split over the slots)
         // instead of growing on first use; 0 = grow on demand.  Payload staging is the caller's (b2s_host_alloc).
@@ -1149,9 +1151,10 @@ void b2s_shutdown(void) {
       S.pws.release();
       S.parena.release();
       S.xpieces.release();
+      S.fws.release();
       S.hmeta.release();
       cudaEvent_t evs[] = {S.ev_a, S.ev_b, S.ev_k0, S.ev_k1, S.ev_t0, S.ev_t1, S.ev_h0, S.ev_h1, S.ev_d0, S.ev_d1,
-                           S.ev_p0, S.ev_p1};
+                           S.ev_p0, S.ev_p1, S.ev_f[0], S.ev_f[1], S.ev_f[2], S.ev_f[3]};
       for (auto ev : evs)
         if (ev) cudaEventDestroy(ev);
       for (auto ev : S.ev_dom) cudaEventDestroy(ev);
@@ -2371,18 +2374,46 @@ int b2s_decompress_packed(uint32_t codec, uint32_t checksum_alg, uint32_t n, con
 }
 
 // ------------------------------------------------------------------------------------------------------------
-// read side, key-sorted: verify + decode a reduce task's blocks, then sort its fixed-size records by key
+// read side, key-sorted: verify + decode a reduce task's blocks, then sort its records by key
 // ------------------------------------------------------------------------------------------------------------
+// What the records of a sort call are: fixed-size (record_bytes long, an unsigned byte key) or length-prefixed UnsafeRow
+// records (rows: [size: int32 big-endian][row], a typed key at key_off in the row, null bit null_field)
+struct RecordSpec {
+  bool is_rows = false;
+  uint32_t record_bytes = 0;
+  uint32_t key_type = B2S_KEY_BYTES;
+  uint32_t key_off = 0, key_len = 0;
+  int32_t null_field = -1;
+  bool rows() const { return is_rows; }
+};
+static RecordSpec fixed_spec(uint32_t record_bytes, uint32_t key_off, uint32_t key_len) {
+  RecordSpec r;
+  r.record_bytes = record_bytes;
+  r.key_off = key_off;
+  r.key_len = key_len;
+  return r;
+}
+
 static int sort_args(uint32_t codec, uint32_t alg, uint32_t n, const uint64_t* src_off, const uint64_t* src_len,
                      const uint32_t* slice_base, const uint64_t* slice_len, const uint64_t* slice_checksum,
-                     uint32_t record_bytes, uint32_t key_off, uint32_t key_len, const void* src_base,
-                     const void* dst_base, uint64_t dst_cap, const uint64_t* dst_total, const uint64_t* n_records,
-                     const int32_t* status) {
+                     const RecordSpec& spec, const void* src_base, const void* dst_base, uint64_t dst_cap,
+                     const uint64_t* dst_total, const uint64_t* n_records, const int32_t* status) {
   if (alg > B2S_CHECKSUM_CRC32C) return fail(B2S_E_UNSUPPORTED, "Unsupported shuffle checksum algorithm%s");
   if (codec > B2S_CODEC_ZSTD) return fail(B2S_E_UNSUPPORTED, "codec %s not supported by this build", "");
-  if (record_bytes == 0) return fail(B2S_E_ARG, "record_bytes must be at least 1%s");
-  if (key_len < 1 || key_len > 16) return fail(B2S_E_ARG, "key_len must be in [1, 16]%s");
-  if ((uint64_t)key_off + key_len > record_bytes) return fail(B2S_E_ARG, "key_off + key_len exceeds record_bytes%s");
+  const uint32_t key_len = spec.key_len;
+  if (spec.rows()) {
+    if (spec.key_type > B2S_KEY_INT64) return fail(B2S_E_ARG, "unknown key_type%s");
+    if (spec.key_type == B2S_KEY_BYTES && (key_len < 1 || key_len > 16))
+      return fail(B2S_E_ARG, "key_len must be in [1, 16]%s");
+    if (spec.key_type == B2S_KEY_INT32 && key_len != 4) return fail(B2S_E_ARG, "key_len of an INT32 key must be 4%s");
+    if (spec.key_type == B2S_KEY_INT64 && key_len != 8) return fail(B2S_E_ARG, "key_len of an INT64 key must be 8%s");
+    if (spec.null_field < -1) return fail(B2S_E_ARG, "null_field must be -1 or a field ordinal%s");
+  } else {
+    if (spec.record_bytes == 0) return fail(B2S_E_ARG, "record_bytes must be at least 1%s");
+    if (key_len < 1 || key_len > 16) return fail(B2S_E_ARG, "key_len must be in [1, 16]%s");
+    if ((uint64_t)spec.key_off + key_len > spec.record_bytes)
+      return fail(B2S_E_ARG, "key_off + key_len exceeds record_bytes%s");
+  }
   if (!dst_total || !n_records) return fail(B2S_E_ARG, "null argument%s");
   if (n && (!src_base || !src_off || !src_len || !status)) return fail(B2S_E_ARG, "null argument%s");
   if (dst_cap && !dst_base) return fail(B2S_E_ARG, "null argument%s");
@@ -2410,7 +2441,7 @@ constexpr size_t kSortKeepBytes = 1ull << 30;
 struct SortBufferTrim {
   Slot& S;
   ~SortBufferTrim() {
-    for (DevBuf* b : {&S.src, &S.dst, &S.parena, &S.pws})
+    for (DevBuf* b : {&S.src, &S.dst, &S.parena, &S.pws, &S.fws})
       if (b->cap > kSortKeepBytes) b->release();
   }
 };
@@ -2426,10 +2457,12 @@ struct SortSource {
 };
 
 // The whole reduce task on the device: compressed blocks at d_src + src_dev_off[i] (src_contiguous: back to back from
-// d_src in block order, no gaps).  Phase A verifies the slices and sizes every block; a failed block, or a decoded
-// length that is not a multiple of record_bytes, ends the call with status[] set and *n_rec = 0 (nothing decoded or
-// sorted).  Then the blocks are decoded into S.dst (codec NONE: used in place, or copied there), their records sorted
-// into *d_sorted (nullptr: into S.parena, returned there).
+// d_src in block order, no gaps).  Phase A verifies the slices and sizes every block; a failed block, or (fixed-size
+// records) a decoded length that is not a multiple of record_bytes, ends the call with status[] set and *n_rec = 0
+// (nothing decoded or sorted).  Then the blocks are decoded into S.dst (codec NONE: used in place, or copied there) and
+// their records sorted into *d_sorted (nullptr: into S.parena, returned there).  Rows are framed first, over each
+// source's range of the decoded arena; the record count and the per-source verdicts come back in one readback, which
+// sizes the sort workspace, and a source that is not whole records fails the call as above.
 // mix (exchange-cache reads): the call's sources in order, the n blocks being its fetched ones; status[] / bad_slice[]
 // are per source.  Every source's records land at their source-order place in S.dst: phase A's decoded offsets are
 // shifted past the cached bytes in front of each block before phase B decodes, and one gather moves the cached ranges
@@ -2437,9 +2470,9 @@ struct SortSource {
 static int decompress_sort_run(Device* D, Slot& S, uint32_t codec, uint32_t alg, uint32_t n, const uint8_t* d_src,
                                const uint64_t* src_dev_off, const uint64_t* src_len, bool src_contiguous,
                                const uint32_t* slice_base, const uint64_t* slice_len, const uint64_t* slice_sum,
-                               uint32_t record_bytes, uint32_t key_off, uint32_t key_len, uint8_t** d_sorted,
-                               uint64_t out_cap, uint64_t* total, uint64_t* n_rec, int32_t* status, int32_t* bad_slice,
-                               uint64_t* launches, const std::vector<SortSource>* mix = nullptr) {
+                               const RecordSpec& spec, uint8_t** d_sorted, uint64_t out_cap, uint64_t* total,
+                               uint64_t* n_rec, int32_t* status, int32_t* bad_slice, uint64_t* launches,
+                               const std::vector<SortSource>* mix = nullptr) {
   cudaStream_t st = S.st;
   DecompressJob J;
   int rc;
@@ -2465,7 +2498,7 @@ static int decompress_sort_run(Device* D, Slot& S, uint32_t codec, uint32_t alg,
   auto cached = [&](uint32_t i) { return mix && (*mix)[i].cached; };
   auto block = [&](uint32_t i) { return mix ? (*mix)[i].block : i; };
   std::vector<int32_t> cached_status(n_src, B2S_OK);
-  std::vector<uint64_t> place(n_src);  // each source's offset in the decoded arena
+  std::vector<uint64_t> place(n_src), length(n_src);  // each source's range of the decoded arena
   uint64_t at = 0;
   *n_rec = 0;
   bool failed = false;
@@ -2475,16 +2508,17 @@ static int decompress_sort_run(Device* D, Slot& S, uint32_t codec, uint32_t alg,
     int32_t& s = c ? cached_status[i] : J.h_status[block(i)];
     const uint64_t len = c ? (*mix)[i].len : J.h_dst_len[block(i)];
     if (c) s = (*mix)[i].status;
-    if (s == B2S_OK && len % record_bytes) {
+    if (s == B2S_OK && !spec.rows() && len % spec.record_bytes) {
       s = B2S_E_CORRUPT;
       if (!failed) {
         snprintf(msg, sizeof msg, "%s %u %s %llu bytes, not a multiple of record_bytes %u", c ? "cached source" : "block",
-                 i, c ? "holds" : "decodes to", (unsigned long long)len, record_bytes);
+                 i, c ? "holds" : "decodes to", (unsigned long long)len, spec.record_bytes);
         fail(B2S_E_CORRUPT, "%s", msg);
       }
     }
     failed |= s != B2S_OK;
     place[i] = at;
+    length[i] = len;
     at += len;
   }
   *total = mix ? at : J.h_totals[1];
@@ -2504,6 +2538,8 @@ static int decompress_sort_run(Device* D, Slot& S, uint32_t codec, uint32_t alg,
       CU(cudaEventRecord(S.ev_p0, st));
       CU(cudaEventRecord(S.ev_p1, st));
     }
+    if (sort && spec.rows())
+      for (cudaEvent_t e : S.ev_f) CU(cudaEventRecord(e, st));
     CU(cudaStreamSynchronize(st));
     return 0;
   };
@@ -2511,8 +2547,7 @@ static int decompress_sort_run(Device* D, Slot& S, uint32_t codec, uint32_t alg,
     report();
     return skip_events(true, true);
   }
-  const uint64_t records = *total / record_bytes;
-  if (records > 0xffffffffull)
+  if (!spec.rows() && *total / spec.record_bytes > 0xffffffffull)
     return fail(B2S_E_ARG, "more than 2^32 - 1 records in one call (%s bytes)", std::to_string(*total).c_str());
   if (*total > out_cap) {
     report();
@@ -2573,17 +2608,79 @@ static int decompress_sort_run(Device* D, Slot& S, uint32_t codec, uint32_t alg,
     if ((rc = S.parena.ensure(*total + 64))) return rc;
     *d_sorted = (uint8_t*)S.parena.p;
   }
-  if (records && (rc = S.pws.ensure(key_sort_ws_bytes(records, key_len)))) return rc;
+  if (!spec.rows()) {
+    const uint64_t records = *total / spec.record_bytes;
+    if (records && (rc = S.pws.ensure(key_sort_ws_bytes(records, spec.key_len)))) return rc;
+    CU(cudaEventRecord(S.ev_p0, st));
+    launch_key_sort(arena, records, spec.record_bytes, spec.key_off, spec.key_len, (uint8_t*)S.pws.p, *d_sorted, st,
+                    launches);
+    CU(cudaEventRecord(S.ev_p1, st));
+    CU(cudaStreamSynchronize(st));
+    CU(cudaGetLastError());
+    *n_rec = records;
+    return 0;
+  }
+
+  // rows: frame every source's range, then one readback of the record count and the verdicts
+  const uint64_t min_key = (uint64_t)spec.key_off + spec.key_len;
+  const uint64_t min_null = spec.null_field >= 0 ? 8ull * (uint32_t)(spec.null_field >> 6) + 8 : 0;
+  if ((rc = S.fws.ensure(rows_frame_ws_bytes(*total, n_src)))) return rc;
+  uint8_t* fws = (uint8_t*)S.fws.p;
+  uint64_t frame_launches = *launches;
   CU(cudaEventRecord(S.ev_p0, st));
-  launch_key_sort(arena, records, record_bytes, key_off, key_len, (uint8_t*)S.pws.p, *d_sorted, st, launches);
+  CU(cudaEventRecord(S.ev_f[0], st));
+  launch_rows_frame(arena, *total, place.data(), length.data(), n_src, min_key, min_null, fws, st, launches);
+  CU(cudaEventRecord(S.ev_f[1], st));
+  std::vector<uint64_t> rb(n_src + 1);
+  CU(cudaMemcpyAsync(rb.data(), rows_frame_readback(fws, *total, n_src), rows_frame_readback_bytes(n_src),
+                     cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  CU(cudaGetLastError());
+  for (uint32_t i = 0; i < n_src; i++) {
+    const uint64_t v = rb[1 + i];
+    if (v == ~0ull) continue;
+    (cached(i) ? cached_status[i] : J.h_status[block(i)]) = B2S_E_CORRUPT;
+    if (!failed) {
+      static const char* const why[] = {"", "the block ends inside a size prefix", "the size is negative",
+                                        "the record runs past the block end", "the row is shorter than key_off + key_len",
+                                        "the row does not hold the null-bit word"};
+      snprintf(msg, sizeof msg, "%s %u: bad row record at byte %llu: %s", cached(i) ? "cached source" : "block", i,
+               (unsigned long long)(v & ((1ull << 61) - 1)), why[v >> 61]);
+      fail(B2S_E_CORRUPT, "%s", msg);
+    }
+    failed = true;
+  }
+  if (failed) {
+    report();
+    CU(cudaEventRecord(S.ev_f[2], st));
+    CU(cudaEventRecord(S.ev_f[3], st));
+    CU(cudaEventRecord(S.ev_p1, st));
+    CU(cudaStreamSynchronize(st));
+    return 0;
+  }
+  const uint64_t records = rb[0];
+  if (records > 0xffffffffull)
+    return fail(B2S_E_ARG, "more than 2^32 - 1 records in one call (%s records)", std::to_string(records).c_str());
+  const uint32_t key_bytes = rows_key_bytes(spec.key_len, spec.null_field);
+  if (records && (rc = S.pws.ensure(rows_sort_ws_bytes(records, key_bytes)))) return rc;
+  CU(cudaEventRecord(S.ev_f[2], st));
+  launch_rows_emit(arena, *total, n_src, fws, records, key_bytes, (uint8_t*)S.pws.p, st, launches);
+  CU(cudaEventRecord(S.ev_f[3], st));
+  frame_launches = *launches - frame_launches;
+  launch_rows_sort(arena, records, spec.key_type, spec.key_off, spec.key_len, spec.null_field, (uint8_t*)S.pws.p,
+                   *d_sorted, st, launches);
   CU(cudaEventRecord(S.ev_p1, st));
   CU(cudaStreamSynchronize(st));
   CU(cudaGetLastError());
+  // the dominant step of a row sort is the framing (walk + count, emit), not the decoder's kernel
+  S.dom_used = 0;
+  t_timing.dominant_ms = ms_between(S.ev_f[0], S.ev_f[1]) + ms_between(S.ev_f[2], S.ev_f[3]);
+  t_timing.dominant_launches = frame_launches;
   *n_rec = records;
   return 0;
 }
 
-// kernel_ms: verification + decode + sort; top_kernel_ms: the sort step
+// kernel_ms: verification + decode + sort; top_kernel_ms: the sort step (rows: framing + sort)
 static void sort_timing(Slot& S, uint64_t n_launches, uint64_t src_bytes, uint64_t total) {
   add_timing(S, false);
   t_timing.kernel_ms = ms_between(S.ev_k0, S.ev_p1);
@@ -2597,9 +2694,9 @@ static void sort_timing(Slot& S, uint64_t n_launches, uint64_t src_bytes, uint64
 // decompress_sort on the read lane of D over device-resident blocks, sorted into dst_base (device memory)
 static int sort_dev_run(Device* D, uint32_t codec, uint32_t alg, uint32_t n, const uint8_t* src_base,
                         const uint64_t* src_off, const uint64_t* src_len, const uint32_t* slice_base,
-                        const uint64_t* slice_len, const uint64_t* slice_checksum, uint32_t record_bytes,
-                        uint32_t key_off, uint32_t key_len, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_total,
-                        uint64_t* n_records, int32_t* status, int32_t* bad_slice, const WallTimer& wt,
+                        const uint64_t* slice_len, const uint64_t* slice_checksum, const RecordSpec& spec,
+                        uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records,
+                        int32_t* status, int32_t* bad_slice, const WallTimer& wt,
                         const std::vector<SortSource>* mix = nullptr) {
   Lane& Ln = D->lane[kLaneRead];
   std::lock_guard<std::mutex> lk(Ln.mtx);
@@ -2609,8 +2706,8 @@ static int sort_dev_run(Device* D, uint32_t codec, uint32_t alg, uint32_t n, con
   for (uint32_t i = 0; i < n; i++) srcb += src_len[i];
   uint8_t* out = dst_base;
   int rc = decompress_sort_run(D, S, codec, alg, n, src_base, src_off, src_len, false, slice_base, slice_len,
-                               slice_checksum, record_bytes, key_off, key_len, &out, dst_cap, dst_total, n_records,
-                               status, bad_slice, &launches, mix);
+                               slice_checksum, spec, &out, dst_cap, dst_total, n_records, status, bad_slice,
+                               &launches, mix);
   if (rc) return rc;
   sort_timing(S, launches, srcb, *dst_total);
   t_timing.total_ms = wt.ms();
@@ -2620,10 +2717,10 @@ static int sort_dev_run(Device* D, uint32_t codec, uint32_t alg, uint32_t n, con
 // decompress_sort on the read lane of D over host blocks: one upload, the sort, one download into dst_base
 static int sort_packed_run(Device* D, uint32_t codec, uint32_t alg, uint32_t n, const uint8_t* src_base,
                            const uint64_t* src_off, const uint64_t* src_len, const uint32_t* slice_base,
-                           const uint64_t* slice_len, const uint64_t* slice_checksum, uint32_t record_bytes,
-                           uint32_t key_off, uint32_t key_len, uint8_t* dst_base, uint64_t dst_cap,
-                           uint64_t* dst_total, uint64_t* n_records, int32_t* status, int32_t* bad_slice,
-                           const WallTimer& wt, const std::vector<SortSource>* mix = nullptr) {
+                           const uint64_t* slice_len, const uint64_t* slice_checksum, const RecordSpec& spec,
+                           uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records,
+                           int32_t* status, int32_t* bad_slice, const WallTimer& wt,
+                           const std::vector<SortSource>* mix = nullptr) {
   Lane& Ln = D->lane[kLaneRead];
   std::lock_guard<std::mutex> lk(Ln.mtx);
   Slot& S = Ln.slot[0];
@@ -2650,8 +2747,8 @@ static int sort_packed_run(Device* D, uint32_t codec, uint32_t alg, uint32_t n, 
   uint64_t launches = 0;
   uint8_t* sorted = nullptr;
   rc = decompress_sort_run(D, S, codec, alg, n, (const uint8_t*)S.src.p, dev_off.data(), src_len, true, slice_base,
-                           slice_len, slice_checksum, record_bytes, key_off, key_len, &sorted, dst_cap, dst_total,
-                           n_records, status, bad_slice, &launches, mix);
+                           slice_len, slice_checksum, spec, &sorted, dst_cap, dst_total, n_records, status, bad_slice,
+                           &launches, mix);
   if (rc) return rc;
   const uint64_t down = *n_records ? *dst_total : 0;
   CU(cudaEventRecord(S.ev_d0, st));
@@ -2681,11 +2778,12 @@ int b2s_decompress_sort_dev(uint32_t dev_index, uint32_t codec, uint32_t checksu
   Device* D;
   int rc = sort_device(dev_index, &D);
   if (rc) return rc;
-  rc = sort_args(codec, checksum_alg, n, src_off, src_len, slice_base, slice_len, slice_checksum, record_bytes, key_off,
-                 key_len, src_base, dst_base, dst_cap, dst_total, n_records, status);
+  const RecordSpec spec = fixed_spec(record_bytes, key_off, key_len);
+  rc = sort_args(codec, checksum_alg, n, src_off, src_len, slice_base, slice_len, slice_checksum, spec, src_base,
+                 dst_base, dst_cap, dst_total, n_records, status);
   if (rc || !n) return rc;
   return sort_dev_run(D, codec, checksum_alg, n, src_base, src_off, src_len, slice_base, slice_len, slice_checksum,
-                      record_bytes, key_off, key_len, dst_base, dst_cap, dst_total, n_records, status, bad_slice, wt);
+                      spec, dst_base, dst_cap, dst_total, n_records, status, bad_slice, wt);
 }
 
 int b2s_decompress_sort_packed(uint32_t codec, uint32_t checksum_alg, uint32_t n, const uint8_t* src_base,
@@ -2700,12 +2798,64 @@ int b2s_decompress_sort_packed(uint32_t codec, uint32_t checksum_alg, uint32_t n
   Device* D;
   int rc = sort_device(t_device, &D);
   if (rc) return rc;
-  rc = sort_args(codec, checksum_alg, n, src_off, src_len, slice_base, slice_len, slice_checksum, record_bytes, key_off,
-                 key_len, src_base, dst_base, dst_cap, dst_total, n_records, status);
+  const RecordSpec spec = fixed_spec(record_bytes, key_off, key_len);
+  rc = sort_args(codec, checksum_alg, n, src_off, src_len, slice_base, slice_len, slice_checksum, spec, src_base,
+                 dst_base, dst_cap, dst_total, n_records, status);
   if (rc || !n) return rc;
   return sort_packed_run(D, codec, checksum_alg, n, src_base, src_off, src_len, slice_base, slice_len, slice_checksum,
-                         record_bytes, key_off, key_len, dst_base, dst_cap, dst_total, n_records, status, bad_slice,
-                         wt);
+                         spec, dst_base, dst_cap, dst_total, n_records, status, bad_slice, wt);
+}
+
+static RecordSpec rows_spec(uint32_t key_type, uint32_t key_off, uint32_t key_len, int32_t null_field) {
+  RecordSpec r;
+  r.is_rows = true;
+  r.key_type = key_type;
+  r.key_off = key_off;
+  r.key_len = key_len;
+  r.null_field = null_field;
+  return r;
+}
+
+int b2s_decompress_sort_rows_dev(uint32_t dev_index, uint32_t codec, uint32_t checksum_alg, uint32_t n,
+                                 const uint8_t* src_base, const uint64_t* src_off, const uint64_t* src_len,
+                                 const uint32_t* slice_base, const uint64_t* slice_len, const uint64_t* slice_checksum,
+                                 uint32_t key_type, uint32_t key_off, uint32_t key_len, int32_t null_field,
+                                 uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records,
+                                 int32_t* status, int32_t* bad_slice) {
+  WallTimer wt;
+  t_timing = b2s_timing{};
+  if (dst_total) *dst_total = 0;
+  if (n_records) *n_records = 0;
+  Device* D;
+  int rc = sort_device(dev_index, &D);
+  if (rc) return rc;
+  const RecordSpec spec = rows_spec(key_type, key_off, key_len, null_field);
+  rc = sort_args(codec, checksum_alg, n, src_off, src_len, slice_base, slice_len, slice_checksum, spec, src_base,
+                 dst_base, dst_cap, dst_total, n_records, status);
+  if (rc || !n) return rc;
+  return sort_dev_run(D, codec, checksum_alg, n, src_base, src_off, src_len, slice_base, slice_len, slice_checksum,
+                      spec, dst_base, dst_cap, dst_total, n_records, status, bad_slice, wt);
+}
+
+int b2s_decompress_sort_rows_packed(uint32_t codec, uint32_t checksum_alg, uint32_t n, const uint8_t* src_base,
+                                    const uint64_t* src_off, const uint64_t* src_len, const uint32_t* slice_base,
+                                    const uint64_t* slice_len, const uint64_t* slice_checksum, uint32_t key_type,
+                                    uint32_t key_off, uint32_t key_len, int32_t null_field, uint8_t* dst_base,
+                                    uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records, int32_t* status,
+                                    int32_t* bad_slice) {
+  WallTimer wt;
+  t_timing = b2s_timing{};
+  if (dst_total) *dst_total = 0;
+  if (n_records) *n_records = 0;
+  Device* D;
+  int rc = sort_device(t_device, &D);
+  if (rc) return rc;
+  const RecordSpec spec = rows_spec(key_type, key_off, key_len, null_field);
+  rc = sort_args(codec, checksum_alg, n, src_off, src_len, slice_base, slice_len, slice_checksum, spec, src_base,
+                 dst_base, dst_cap, dst_total, n_records, status);
+  if (rc || !n) return rc;
+  return sort_packed_run(D, codec, checksum_alg, n, src_base, src_off, src_len, slice_base, slice_len, slice_checksum,
+                         spec, dst_base, dst_cap, dst_total, n_records, status, bad_slice, wt);
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -2872,8 +3022,8 @@ static int exchange_sort_args(int32_t start_reduce, int32_t end_reduce, const in
   }
   const uint32_t m = (uint32_t)M.off.size();
   return sort_args(codec, alg, m, M.off.data(), M.len.data(), M.slice_base.data(), M.slice_len.data(),
-                   M.slice_sum.data(), record_bytes, key_off, key_len, src_base, dst_base, dst_cap, dst_total,
-                   n_records, status);
+                   M.slice_sum.data(), fixed_spec(record_bytes, key_off, key_len), src_base, dst_base, dst_cap,
+                   dst_total, n_records, status);
 }
 
 // references the cached sources of M on device D and describes them; B2S_E_ARG when a range exceeds an entry
@@ -2911,8 +3061,8 @@ int b2s_exchange_read_sort_packed(int32_t shuffle_id, int32_t start_reduce, int3
   if ((rc = exchange_sort_sources(refs, start_reduce, end_reduce, M))) return rc;
   const uint32_t m = (uint32_t)M.off.size();
   return sort_packed_run(D, codec, checksum_alg, m, src_base, M.off.data(), M.len.data(), M.slice_base.data(),
-                         M.slice_len.data(), M.slice_sum.data(), record_bytes, key_off, key_len, dst_base, dst_cap,
-                         dst_total, n_records, status, bad_slice, wt, &M.src);
+                         M.slice_len.data(), M.slice_sum.data(), fixed_spec(record_bytes, key_off, key_len), dst_base,
+                         dst_cap, dst_total, n_records, status, bad_slice, wt, &M.src);
 }
 
 int b2s_exchange_read_sort_dev(uint32_t dev_index, int32_t shuffle_id, int32_t start_reduce, int32_t end_reduce,
@@ -2938,8 +3088,8 @@ int b2s_exchange_read_sort_dev(uint32_t dev_index, int32_t shuffle_id, int32_t s
   if ((rc = exchange_sort_sources(refs, start_reduce, end_reduce, M))) return rc;
   const uint32_t m = (uint32_t)M.off.size();
   return sort_dev_run(D, codec, checksum_alg, m, src_base, M.off.data(), M.len.data(), M.slice_base.data(),
-                      M.slice_len.data(), M.slice_sum.data(), record_bytes, key_off, key_len, dst_base, dst_cap,
-                      dst_total, n_records, status, bad_slice, wt, &M.src);
+                      M.slice_len.data(), M.slice_sum.data(), fixed_spec(record_bytes, key_off, key_len), dst_base,
+                      dst_cap, dst_total, n_records, status, bad_slice, wt, &M.src);
 }
 
 int b2s_decompressed_size_batch(uint32_t codec, uint32_t n, const uint8_t* const* src, const uint64_t* src_len,

@@ -186,14 +186,61 @@ void launch_partition(const uint32_t* d_rec_len, const uint32_t* d_rec_part, uin
 // to the arena size)
 void launch_partition_gather(const uint8_t* rec_base, const uint32_t* d_rec_len, uint64_t n, const PartitionPlan& plan,
                              uint8_t* d_dst, cudaStream_t st, uint64_t* launches);
+// sdst[j] = arena offset of the j-th record in the order idx (nullptr = identity): rec_len[idx[j]] scanned.
+// total: one u64 (the grand total); scan_ws: scan_ws_elems(n) u64
+void launch_sorted_offsets(const uint32_t* idx, const uint32_t* d_rec_len, uint64_t n, uint64_t* sdst, uint64_t* total,
+                           uint64_t* scan_ws, cudaStream_t st, uint64_t* launches);
 
 // ---------------- sort.cu (stable sort of fixed-size records by an unsigned byte key) ----------------
 // n records of record_bytes each, back to back at d_rec (n < 2^32); the key of a record is its bytes
 // [key_off, key_off + key_len), 1 <= key_len <= 16, compared as unsigned bytes, lexicographically.  Writes the records
 // to d_dst in ascending key order, equal keys in input order.  d_ws: key_sort_ws_bytes(n, key_len).
-size_t key_sort_ws_bytes(uint64_t n, uint32_t key_len);
+size_t key_sort_ws_bytes(uint64_t n, uint32_t key_bytes);
 void launch_key_sort(const uint8_t* d_rec, uint64_t n, uint32_t record_bytes, uint32_t key_off, uint32_t key_len,
                      uint8_t* d_ws, uint8_t* d_dst, cudaStream_t st, uint64_t* launches);
+// The per-record arrays of a key sort of n records with key_bytes key bytes, carved from key_sort_ws_bytes(n, key_bytes)
+// bytes: the key as ceil(key_bytes / 4) big-endian u32 words, word-major (words[k * n + i], zero-padded on the right);
+// radix buffers; the gather's per-record length, source and destination offsets; histogram and its scan workspace.
+struct KeySortWs {
+  uint32_t* words;
+  uint32_t* K[2];
+  uint32_t* I[2];
+  uint32_t* len;
+  uint64_t* src_off;
+  uint64_t* sdst;
+  uint64_t* hist;
+  uint64_t* scan_ws;
+  uint64_t* total;
+};
+KeySortWs carve_key_sort_ws(uint8_t* d_ws, uint64_t n, uint32_t key_bytes);
+// LSD radix sort of the key words (one 8-bit pass per key byte, least significant first), stable; returns the sorted
+// record indices (nullptr when n < 2: input order)
+const uint32_t* launch_key_radix(const KeySortWs& w, uint64_t n, uint32_t key_bytes, cudaStream_t st,
+                                 uint64_t* launches);
+
+// ---------------- rows.cu (stable sort of length-prefixed UnsafeRow records by a typed key) ----------------
+// Framing: the n_ranges decoded blocks [off[i], off[i] + len[i]) of the arena (arena_bytes long, 64 bytes of slack
+// after it) are walked as [size: int32 big-endian][size bytes] records.  d_fws: rows_frame_ws_bytes(arena_bytes,
+// n_ranges).  Afterwards rows_frame_readback(d_fws) holds rows_frame_readback_bytes(n_ranges) bytes: [record count,
+// verdict of range 0, 1, ...]; a verdict is ~0 when the range is whole records, else kRowsBad* << 61 | the offset of the
+// range's first bad record.  A record is bad when its prefix is cut by the range end, its size is negative, it runs past
+// the range end, its row is shorter than min_key bytes, or shorter than min_null bytes.
+constexpr uint64_t kRowsBadPrefix = 1, kRowsBadNegative = 2, kRowsBadPastEnd = 3, kRowsBadKey = 4, kRowsBadNull = 5;
+size_t rows_frame_ws_bytes(uint64_t arena_bytes, uint32_t n_ranges);
+inline size_t rows_frame_readback_bytes(uint32_t n_ranges) { return ((size_t)n_ranges + 1) * 8; }
+uint64_t* rows_frame_readback(uint8_t* d_fws, uint64_t arena_bytes, uint32_t n_ranges);
+void launch_rows_frame(const uint8_t* arena, uint64_t arena_bytes, const uint64_t* h_off, const uint64_t* h_len,
+                       uint32_t n_ranges, uint64_t min_key, uint64_t min_null, uint8_t* d_fws, cudaStream_t st,
+                       uint64_t* launches);
+// key bytes of the sort: key_len, plus the leading null byte of a nullable key
+inline uint32_t rows_key_bytes(uint32_t key_len, int32_t null_field) { return key_len + (null_field >= 0 ? 1 : 0); }
+size_t rows_sort_ws_bytes(uint64_t n, uint32_t key_bytes);
+// the framed records (n = the read-back count) as dense offsets and lengths in arena order, into the sort workspace
+void launch_rows_emit(const uint8_t* arena, uint64_t arena_bytes, uint32_t n_ranges, uint8_t* d_fws, uint64_t n,
+                      uint32_t key_bytes, uint8_t* d_ws, cudaStream_t st, uint64_t* launches);
+// the emitted records to d_dst, ascending by key (nulls first), stable.  key_type B2S_KEY_*
+void launch_rows_sort(const uint8_t* arena, uint64_t n, uint32_t key_type, uint32_t key_off, uint32_t key_len,
+                      int32_t null_field, uint8_t* d_ws, uint8_t* d_dst, cudaStream_t st, uint64_t* launches);
 
 // ---------------- exchange.cu (exchange-cache reads: ranges of device memory gathered into one arena) ----------------
 // piece: len bytes at src (device pointer, any alignment) go to d_dst + dst

@@ -270,10 +270,16 @@ void launch_partition(const uint32_t* d_rec_len, const uint32_t* d_rec_part, uin
     shift += (int)pb;
   }
   plan->idx = idx;
-  part_sorted_len_kernel<<<grid_for(n), kPartThreads, 0, st>>>(idx, d_rec_len, n, plan->sdst);
-  launch_exclusive_scan_u64(plan->sdst, n, unused_total, ws, st, launches);
+  launch_sorted_offsets(idx, d_rec_len, n, plan->sdst, unused_total, ws, st, launches);
   part_bounds_kernel<<<grid_for(n), kPartThreads, 0, st>>>(keys, d_rec_part, n, num_partitions, plan->sdst, part_start);
-  if (launches) *launches += 3;
+  if (launches) *launches += 2;
+}
+
+void launch_sorted_offsets(const uint32_t* idx, const uint32_t* d_rec_len, uint64_t n, uint64_t* sdst, uint64_t* total,
+                           uint64_t* scan_ws, cudaStream_t st, uint64_t* launches) {
+  part_sorted_len_kernel<<<grid_for(n), kPartThreads, 0, st>>>(idx, d_rec_len, n, sdst);
+  launch_exclusive_scan_u64(sdst, n, total, scan_ws, st, launches);
+  if (launches) *launches += 1;
 }
 
 void launch_partition_gather(const uint8_t* rec_base, const uint32_t* d_rec_len, uint64_t n, const PartitionPlan& plan,

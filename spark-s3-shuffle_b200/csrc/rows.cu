@@ -1,0 +1,345 @@
+// rows.cu — stable sort of length-prefixed UnsafeRow records by one typed key (the reduce side of a Spark SQL exchange:
+// the SortExec a sort-merge join runs right after the shuffle read).  A decoded block is a sequence of
+// [size: int32 big-endian][size bytes of row] records, as UnsafeRowSerializer writes them.  Steps, all on the device:
+//   frame  : a warp per block (persistent grid, blocks taken from a counter) walks the size chain.  The walk only moves
+//            forward, so the block is staged through a per-warp shared-memory ring of windows with cp.async, several
+//            windows ahead of the walk; each hop is a shared-memory load.  A record longer than a window restarts the
+//            staging at the next record.  Every record is validated; its start sets one bit of a bitmap over the decoded
+//            arena (1 bit per byte), and a block's first bad record goes to its verdict
+//   count  : set bits per 64 KiB tile of the arena, scanned: the record count, read back with the verdicts
+//   emit   : the bitmap compacted into dense record offsets (u64) and lengths (u32, prefix included), arena order
+//   keys   : one thread per record: the typed key as big-endian u32 words (int32 / int64: byte-swapped, sign bit
+//            flipped; a nullable key gets a leading byte 0 = null, 1 = non-null, and a null record's key bytes are 0)
+//   radix / gather : the fixed-size sort's radix passes (launch_key_radix), sorted lengths -> scan -> destination
+//            offsets (launch_sorted_offsets), the partition step's gather
+#include <algorithm>
+
+#include "kernels.h"
+
+namespace b2s {
+
+namespace {
+
+constexpr unsigned FULL = 0xffffffffu;
+constexpr int kFrameWarps = 4;
+constexpr uint32_t kFrameWin = 1024;                     // bytes per staged window
+constexpr uint32_t kFrameRing = 8;                       // windows per warp: the walk's two and six in flight
+constexpr uint32_t kFrameRingBytes = kFrameWin * kFrameRing;
+constexpr uint32_t kFrameChunks = kFrameWin / (16 * 32);  // 16-byte copies per lane per window
+constexpr int kRowThreads = 256;
+constexpr uint32_t kTileWords = kRowThreads * 8;          // bitmap words per count / emit tile (64 KiB of arena)
+
+inline size_t a256(size_t b) { return (b + 255) / 256 * 256; }
+
+inline unsigned grid_for(uint64_t n) {
+  const uint64_t want = (n + kRowThreads - 1) / kRowThreads;
+  return (unsigned)(want < (uint64_t)kSMs * 16 ? (want ? want : 1) : (uint64_t)kSMs * 16);
+}
+
+__device__ __forceinline__ void cp_async16(uint32_t saddr, const void* g) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(saddr), "l"(g) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void cp_async_wait() {
+  asm volatile("cp.async.wait_group %0;\n" ::"n"(N) : "memory");
+}
+
+// Block b = arena bytes [r_off[b], r_off[b] + r_len[b]).  Window k of a block is arena bytes [A + k W, A + (k + 1) W)
+// with A the block start rounded down to 16; it is staged in ring slot k mod R.  While the walk is in window k, windows
+// k .. k + R - 1 have been issued (one cp.async group each, in order), so waiting until at most R - 2 groups are pending
+// makes windows k and k + 1 resident: every size prefix that starts in window k lies in them.  A slot is refilled only
+// once its window has landed and been walked (a pending copy into it could otherwise land after the new one).  16-byte
+// pieces are copied while they start before the block end; the last may reach 15 bytes past it, into the arena's slack.
+__global__ void __launch_bounds__(kFrameWarps * 32) rows_frame_kernel(
+    const uint8_t* __restrict__ arena, const uint64_t* __restrict__ r_off, const uint64_t* __restrict__ r_len,
+    uint32_t n, uint64_t min_key, uint64_t min_null, uint32_t* __restrict__ bitmap, uint64_t* __restrict__ verdict,
+    unsigned int* __restrict__ counter) {
+  __shared__ __align__(16) uint32_t s_ring[kFrameWarps][kFrameRingBytes / 4];
+  const uint32_t lane = threadIdx.x & 31;
+  const uint32_t* ring = s_ring[threadIdx.x >> 5];
+  const uint32_t ring_s = (uint32_t)__cvta_generic_to_shared(ring);
+  for (;;) {
+    uint32_t b = 0;
+    if (lane == 0) b = atomicAdd(counter, 1u);
+    b = __shfl_sync(FULL, b, 0);
+    if (b >= n) break;
+    const uint64_t start = r_off[b], end = start + r_len[b];
+    const uint64_t A = start & ~15ull;
+    auto issue = [&](uint64_t k) {
+      const uint64_t w0 = A + k * kFrameWin;
+      const uint32_t slot = (uint32_t)(k % kFrameRing) * kFrameWin;
+#pragma unroll
+      for (uint32_t c = 0; c < kFrameChunks; c++) {
+        const uint32_t o = (c * 32 + lane) * 16;
+        if (w0 + o < end) cp_async16(ring_s + slot + o, arena + w0 + o);
+      }
+      cp_async_commit();
+    };
+    for (uint32_t j = 0; j < kFrameRing; j++) issue(j);
+    uint64_t k = 0, p = start, bad = ~0ull;
+    while (p < end) {
+      const uint64_t kp = (p - A) / kFrameWin;
+      if (kp != k) {
+        if (kp == k + 1) {  // window k is resident and walked: its slot takes window k + R
+          issue(k + kFrameRing);
+        } else {  // a record longer than a window: let what is in flight land, restage from the next record
+          cp_async_wait<0>();
+          __syncwarp();
+          for (uint32_t j = 0; j < kFrameRing; j++) issue(kp + j);
+        }
+        k = kp;
+      }
+      cp_async_wait<kFrameRing - 2>();
+      __syncwarp();
+      if (lane == 0) {  // the records that start in window k
+        const uint64_t wend = A + (k + 1) * kFrameWin;
+        uint64_t q = p, cw = q >> 5;
+        uint32_t acc = 0;
+        while (q < wend && q < end) {
+          uint64_t why = 0;
+          int32_t s = 0;
+          if (q + 4 > end) {
+            why = kRowsBadPrefix;
+          } else {
+            const uint32_t o = (uint32_t)(q - A) & (kFrameRingBytes - 1);
+            const uint32_t lo = ring[o >> 2], hi = ring[((o >> 2) + 1) & (kFrameRingBytes / 4 - 1)];
+            s = (int32_t)__byte_perm(__funnelshift_r(lo, hi, (o & 3) * 8), 0, 0x0123);
+            if (s < 0) why = kRowsBadNegative;
+            else if (q + 4 + (uint32_t)s > end) why = kRowsBadPastEnd;
+            else if ((uint64_t)s < min_key) why = kRowsBadKey;
+            else if ((uint64_t)s < min_null) why = kRowsBadNull;
+          }
+          if (why) {
+            bad = (why << 61) | (q - start);
+            break;
+          }
+          if ((q >> 5) != cw) {
+            if (acc) atomicOr(bitmap + cw, acc);
+            cw = q >> 5;
+            acc = 0;
+          }
+          acc |= 1u << (q & 31);
+          q += 4 + (uint32_t)s;
+        }
+        if (acc) atomicOr(bitmap + cw, acc);
+        p = q;
+      }
+      p = __shfl_sync(FULL, p, 0);
+      bad = __shfl_sync(FULL, bad, 0);
+      __syncwarp();  // lane 0's ring reads are done before the next refill overwrites a slot
+      if (bad != ~0ull) break;
+    }
+    cp_async_wait<0>();  // nothing in flight into the ring when the next block starts
+    __syncwarp();
+    if (lane == 0) verdict[b] = bad;
+  }
+}
+
+// exclusive scan of one u32 per thread over the CTA (kRowThreads threads)
+__device__ __forceinline__ uint32_t cta_exclusive_scan(uint32_t v) {
+  __shared__ uint32_t warp_sums[kRowThreads / 32];
+  const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  uint32_t inc = v;
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const uint32_t t = __shfl_up_sync(FULL, inc, d);
+    if (lane >= (uint32_t)d) inc += t;
+  }
+  if (lane == 31) warp_sums[wid] = inc;
+  __syncthreads();
+  uint32_t before = 0;
+  for (uint32_t w = 0; w < wid; w++) before += warp_sums[w];
+  return before + inc - v;
+}
+
+// cnt[tile] = records starting in the tile's 64 KiB of arena; a thread takes 8 consecutive bitmap words
+__global__ void __launch_bounds__(kRowThreads) rows_count_kernel(const uint32_t* __restrict__ bitmap,
+                                                                 uint64_t* __restrict__ cnt) {
+  __shared__ uint32_t warp_sums[kRowThreads / 32];
+  const uint4* w = reinterpret_cast<const uint4*>(bitmap + (size_t)blockIdx.x * kTileWords) + threadIdx.x * 2;
+  const uint4 a = w[0], b = w[1];
+  uint32_t c = __popc(a.x) + __popc(a.y) + __popc(a.z) + __popc(a.w) + __popc(b.x) + __popc(b.y) + __popc(b.z) +
+               __popc(b.w);
+#pragma unroll
+  for (int d = 16; d; d >>= 1) c += __shfl_xor_sync(FULL, c, d);
+  if ((threadIdx.x & 31) == 0) warp_sums[threadIdx.x >> 5] = c;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    uint32_t t = 0;
+    for (int k = 0; k < kRowThreads / 32; k++) t += warp_sums[k];
+    cnt[blockIdx.x] = t;
+  }
+}
+
+// record j of the arena (tile_base: the scanned tile counts): rec_off[j] = its offset, rec_len[j] = 4 + its size
+__global__ void __launch_bounds__(kRowThreads) rows_emit_kernel(const uint8_t* __restrict__ arena,
+                                                                const uint32_t* __restrict__ bitmap,
+                                                                const uint64_t* __restrict__ tile_base,
+                                                                uint64_t* __restrict__ rec_off,
+                                                                uint32_t* __restrict__ rec_len) {
+  const uint64_t w0 = (uint64_t)blockIdx.x * kTileWords + threadIdx.x * 8;
+  const uint4* w = reinterpret_cast<const uint4*>(bitmap + w0);
+  const uint4 a = w[0], b = w[1];
+  const uint32_t words[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+  uint32_t c = 0;
+#pragma unroll
+  for (int k = 0; k < 8; k++) c += __popc(words[k]);
+  uint64_t j = tile_base[blockIdx.x] + cta_exclusive_scan(c);
+#pragma unroll
+  for (int k = 0; k < 8; k++) {
+    uint32_t m = words[k];
+    while (m) {
+      const uint64_t off = (w0 + k) * 32 + (uint32_t)(__ffs(m) - 1);
+      m &= m - 1;
+      rec_off[j] = off;
+      rec_len[j] = 4 + __byte_perm(ld32u_ro(arena + off), 0, 0x0123);
+      j++;
+    }
+  }
+}
+
+// words[k * n + i] = key word k of record i (see the file comment), k < W
+__global__ void __launch_bounds__(kRowThreads) rows_keys_kernel(const uint8_t* __restrict__ arena,
+                                                                const uint64_t* __restrict__ rec_off, uint64_t n,
+                                                                uint32_t key_type, uint32_t key_off, uint32_t key_len,
+                                                                int32_t null_field, uint32_t W,
+                                                                uint32_t* __restrict__ words) {
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+    const uint8_t* row = arena + rec_off[i] + 4;
+    uint64_t lo, hi;
+    ld_span16<true>(row + key_off, (int)key_len, lo, hi);
+    uint64_t top, bot;  // the key bytes as one 128-bit big-endian value, left-aligned
+    if (key_type == B2S_KEY_INT32) {
+      top = (uint64_t)((uint32_t)lo ^ 0x80000000u) << 32;
+      bot = 0;
+    } else if (key_type == B2S_KEY_INT64) {
+      top = lo ^ (1ull << 63);
+      bot = 0;
+    } else {
+      if (key_len < 8) {
+        lo &= (1ull << (8 * key_len)) - 1;
+        hi = 0;
+      } else if (key_len < 16) {
+        hi &= (1ull << (8 * (key_len - 8))) - 1;
+      }
+      top = __byte_perm((uint32_t)lo, 0, 0x0123);
+      top = (top << 32) | __byte_perm((uint32_t)(lo >> 32), 0, 0x0123);
+      bot = __byte_perm((uint32_t)hi, 0, 0x0123);
+      bot = (bot << 32) | __byte_perm((uint32_t)(hi >> 32), 0, 0x0123);
+    }
+    uint32_t spill = 0;
+    if (null_field >= 0) {
+      uint64_t nw, unused;
+      ld_span16<true>(row + 8 * (uint32_t)(null_field >> 6), 8, nw, unused);
+      const bool is_null = (nw >> (null_field & 63)) & 1;
+      if (is_null) top = bot = 0;
+      spill = (uint32_t)(bot & 0xff) << 24;
+      bot = (bot >> 8) | (top << 56);
+      top = (top >> 8) | ((uint64_t)(is_null ? 0 : 1) << 56);
+    }
+    const uint32_t kw[5] = {(uint32_t)(top >> 32), (uint32_t)top, (uint32_t)(bot >> 32), (uint32_t)bot, spill};
+#pragma unroll
+    for (uint32_t k = 0; k < 5; k++)
+      if (k < W) words[(size_t)k * n + i] = kw[k];
+  }
+}
+
+// the framing workspace: bitmap (whole tiles), tile counts, their scan workspace, readback, ranges, work counter
+struct FrameWs {
+  uint32_t* bitmap;
+  uint64_t* tile_cnt;
+  uint64_t* scan_ws;
+  uint64_t* readback;
+  uint64_t* r_off;
+  uint64_t* r_len;
+  unsigned int* counter;
+  uint64_t tiles;
+};
+
+inline uint64_t frame_tiles(uint64_t arena_bytes) {
+  const uint64_t words = (arena_bytes + 31) / 32;
+  return std::max<uint64_t>((words + kTileWords - 1) / kTileWords, 1);
+}
+
+FrameWs carve_frame_ws(uint8_t* d_fws, uint64_t arena_bytes, uint32_t n_ranges) {
+  FrameWs f;
+  f.tiles = frame_tiles(arena_bytes);
+  uint8_t* p = d_fws;
+  f.bitmap = (uint32_t*)p;   p += a256(f.tiles * kTileWords * 4);
+  f.tile_cnt = (uint64_t*)p; p += a256(f.tiles * 8);
+  f.scan_ws = (uint64_t*)p;  p += a256(scan_ws_elems(f.tiles) * 8);
+  f.readback = (uint64_t*)p; p += a256(rows_frame_readback_bytes(n_ranges));
+  f.r_off = (uint64_t*)p;    p += a256((size_t)n_ranges * 8);
+  f.r_len = (uint64_t*)p;    p += a256((size_t)n_ranges * 8);
+  f.counter = (unsigned int*)p;
+  return f;
+}
+
+}  // namespace
+
+size_t rows_frame_ws_bytes(uint64_t arena_bytes, uint32_t n_ranges) {
+  const uint64_t tiles = frame_tiles(arena_bytes);
+  return a256(tiles * kTileWords * 4) + a256(tiles * 8) + a256(scan_ws_elems(tiles) * 8) +
+         a256(rows_frame_readback_bytes(n_ranges)) + 2 * a256((size_t)n_ranges * 8) + 256;
+}
+
+uint64_t* rows_frame_readback(uint8_t* d_fws, uint64_t arena_bytes, uint32_t n_ranges) {
+  return carve_frame_ws(d_fws, arena_bytes, n_ranges).readback;
+}
+
+void launch_rows_frame(const uint8_t* arena, uint64_t arena_bytes, const uint64_t* h_off, const uint64_t* h_len,
+                       uint32_t n_ranges, uint64_t min_key, uint64_t min_null, uint8_t* d_fws, cudaStream_t st,
+                       uint64_t* launches) {
+  const FrameWs f = carve_frame_ws(d_fws, arena_bytes, n_ranges);
+  cudaMemsetAsync(f.bitmap, 0, f.tiles * kTileWords * 4, st);
+  cudaMemsetAsync(f.readback, 0xff, rows_frame_readback_bytes(n_ranges), st);
+  cudaMemsetAsync(f.counter, 0, sizeof(unsigned int), st);
+  if (n_ranges) {
+    cudaMemcpyAsync(f.r_off, h_off, (size_t)n_ranges * 8, cudaMemcpyHostToDevice, st);
+    cudaMemcpyAsync(f.r_len, h_len, (size_t)n_ranges * 8, cudaMemcpyHostToDevice, st);
+    int per_sm = 0;
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, rows_frame_kernel, kFrameWarps * 32, 0);
+    if (per_sm < 1) per_sm = 1;
+    const uint64_t want = ((uint64_t)n_ranges + kFrameWarps - 1) / kFrameWarps;
+    const uint64_t grid = std::min<uint64_t>((uint64_t)kSMs * per_sm, want);  // persistent: one wave
+    rows_frame_kernel<<<(unsigned)grid, kFrameWarps * 32, 0, st>>>(arena, f.r_off, f.r_len, n_ranges, min_key,
+                                                                    min_null, f.bitmap, f.readback + 1, f.counter);
+    if (launches) *launches += 1;
+  }
+  rows_count_kernel<<<(unsigned)f.tiles, kRowThreads, 0, st>>>(f.bitmap, f.tile_cnt);
+  launch_exclusive_scan_u64(f.tile_cnt, f.tiles, f.readback, f.scan_ws, st, launches);
+  if (launches) *launches += 1;
+}
+
+size_t rows_sort_ws_bytes(uint64_t n, uint32_t key_bytes) {
+  return key_sort_ws_bytes(n, key_bytes) + a256(scan_ws_elems(n) * 8);
+}
+
+void launch_rows_emit(const uint8_t* arena, uint64_t arena_bytes, uint32_t n_ranges, uint8_t* d_fws, uint64_t n,
+                      uint32_t key_bytes, uint8_t* d_ws, cudaStream_t st, uint64_t* launches) {
+  if (!n) return;
+  const FrameWs f = carve_frame_ws(d_fws, arena_bytes, n_ranges);
+  const KeySortWs w = carve_key_sort_ws(d_ws, n, key_bytes);
+  rows_emit_kernel<<<(unsigned)f.tiles, kRowThreads, 0, st>>>(arena, f.bitmap, f.tile_cnt, w.src_off, w.len);
+  if (launches) *launches += 1;
+}
+
+void launch_rows_sort(const uint8_t* arena, uint64_t n, uint32_t key_type, uint32_t key_off, uint32_t key_len,
+                      int32_t null_field, uint8_t* d_ws, uint8_t* d_dst, cudaStream_t st, uint64_t* launches) {
+  if (!n) return;
+  const uint32_t key_bytes = rows_key_bytes(key_len, null_field);
+  const KeySortWs w = carve_key_sort_ws(d_ws, n, key_bytes);
+  uint64_t* offsets_scan_ws = (uint64_t*)(d_ws + key_sort_ws_bytes(n, key_bytes));
+  rows_keys_kernel<<<grid_for(n), kRowThreads, 0, st>>>(arena, w.src_off, n, key_type, key_off, key_len, null_field,
+                                                        (key_bytes + 3) / 4, w.words);
+  if (launches) *launches += 1;
+  PartitionPlan plan;
+  plan.src_off = w.src_off;
+  plan.sdst = w.sdst;
+  plan.idx = launch_key_radix(w, n, key_bytes, st, launches);
+  launch_sorted_offsets(plan.idx, w.len, n, w.sdst, w.total, offsets_scan_ws, st, launches);
+  launch_partition_gather(arena, w.len, n, plan, d_dst, st, launches);
+}
+
+}  // namespace b2s

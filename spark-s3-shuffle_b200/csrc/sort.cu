@@ -70,63 +70,71 @@ inline size_t a256(size_t b) { return (b + 255) / 256 * 256; }
 
 }  // namespace
 
-size_t key_sort_ws_bytes(uint64_t n, uint32_t key_len) {
-  const size_t W = (key_len + 3) / 4, hist = radix_hist_elems(n);
+size_t key_sort_ws_bytes(uint64_t n, uint32_t key_bytes) {
+  const size_t W = (key_bytes + 3) / 4, hist = radix_hist_elems(n);
   return a256(n * 4 * W) + a256(n * 4) * 5 + a256(n * 8) * 2 + a256(hist * 8) + a256(scan_ws_elems(hist) * 8) + 256;
+}
+
+KeySortWs carve_key_sort_ws(uint8_t* d_ws, uint64_t n, uint32_t key_bytes) {
+  const uint32_t W = (key_bytes + 3) / 4;
+  const size_t hist_elems = radix_hist_elems(n);
+  KeySortWs w;
+  uint8_t* p = d_ws;
+  w.words = (uint32_t*)p;   p += a256(n * 4 * W);  // W arrays of n words: word k at words + k * n
+  w.K[0] = (uint32_t*)p;    p += a256(n * 4);
+  w.K[1] = (uint32_t*)p;    p += a256(n * 4);
+  w.I[0] = (uint32_t*)p;    p += a256(n * 4);
+  w.I[1] = (uint32_t*)p;    p += a256(n * 4);
+  w.len = (uint32_t*)p;     p += a256(n * 4);
+  w.src_off = (uint64_t*)p; p += a256(n * 8);
+  w.sdst = (uint64_t*)p;    p += a256(n * 8);
+  w.hist = (uint64_t*)p;    p += a256(hist_elems * 8);
+  w.scan_ws = (uint64_t*)p; p += a256(scan_ws_elems(hist_elems) * 8);
+  w.total = (uint64_t*)p;  // grand totals of the histogram scans
+  return w;
+}
+
+const uint32_t* launch_key_radix(const KeySortWs& w, uint64_t n, uint32_t key_bytes, cudaStream_t st,
+                                 uint64_t* launches) {
+  if (n < 2) return nullptr;
+  const uint32_t W = (key_bytes + 3) / 4;
+  const uint32_t* idx = nullptr;  // current order; nullptr = input order
+  uint32_t pass = 0;
+  for (int k = (int)W - 1; k >= 0; k--) {
+    const uint32_t* kin = w.words + (size_t)k * n;
+    if (idx) {  // the current keys' buffer is free again: put this word there, in the current order
+      uint32_t* kg = w.K[(pass - 1) & 1];
+      sort_word_gather_kernel<<<grid_for(n), kSortThreads, 0, st>>>(kin, idx, n, kg);
+      if (launches) *launches += 1;
+      kin = kg;
+    }
+    // the last word holds key_bytes - 4 (W - 1) real bytes in its high end; the others hold four
+    const uint32_t real = k == (int)W - 1 ? key_bytes - 4 * (W - 1) : 4;
+    for (uint32_t shift = 32 - 8 * real; shift < 32; shift += 8, pass++) {
+      launch_radix_pass(kin, idx, (uint32_t)n, (int)shift, 256, w.hist, w.total, w.scan_ws, w.K[pass & 1],
+                        w.I[pass & 1], st, launches);
+      kin = w.K[pass & 1];
+      idx = w.I[pass & 1];
+    }
+  }
+  return idx;
 }
 
 void launch_key_sort(const uint8_t* d_rec, uint64_t n, uint32_t record_bytes, uint32_t key_off, uint32_t key_len,
                      uint8_t* d_ws, uint8_t* d_dst, cudaStream_t st, uint64_t* launches) {
   if (!n) return;
-  const uint32_t W = (key_len + 3) / 4;
-  const size_t hist_elems = radix_hist_elems(n);
-  uint8_t* p = d_ws;
-  uint32_t* words = (uint32_t*)p;  p += a256(n * 4 * W);  // W arrays of n words: word w at words + w * n
-  uint32_t* K[2];
-  uint32_t* I[2];
-  K[0] = (uint32_t*)p;  p += a256(n * 4);
-  K[1] = (uint32_t*)p;  p += a256(n * 4);
-  I[0] = (uint32_t*)p;  p += a256(n * 4);
-  I[1] = (uint32_t*)p;  p += a256(n * 4);
-  uint32_t* len = (uint32_t*)p;     p += a256(n * 4);
-  uint64_t* src_off = (uint64_t*)p; p += a256(n * 8);
-  uint64_t* sdst = (uint64_t*)p;    p += a256(n * 8);
-  uint64_t* hist = (uint64_t*)p;    p += a256(hist_elems * 8);
-  uint64_t* ws = (uint64_t*)p;      p += a256(scan_ws_elems(hist_elems) * 8);
-  uint64_t* unused_total = (uint64_t*)p;  // grand totals of the histogram scans
-
-  sort_keys_kernel<<<grid_for(n), kSortThreads, 0, st>>>(d_rec, n, record_bytes, key_off, key_len, words);
+  const KeySortWs w = carve_key_sort_ws(d_ws, n, key_len);
+  sort_keys_kernel<<<grid_for(n), kSortThreads, 0, st>>>(d_rec, n, record_bytes, key_off, key_len, w.words);
   if (launches) *launches += 1;
+  const uint32_t* idx = launch_key_radix(w, n, key_len, st, launches);
 
-  const uint32_t* idx = nullptr;  // current order; nullptr = input order
-  if (n > 1) {
-    uint32_t pass = 0;
-    for (int w = (int)W - 1; w >= 0; w--) {
-      const uint32_t* kin = words + (size_t)w * n;
-      if (idx) {  // the current keys' buffer is free again: put this word there, in the current order
-        uint32_t* kg = K[(pass - 1) & 1];
-        sort_word_gather_kernel<<<grid_for(n), kSortThreads, 0, st>>>(kin, idx, n, kg);
-        if (launches) *launches += 1;
-        kin = kg;
-      }
-      // the last word holds key_len - 4 (W - 1) real bytes in its high end; the others hold four
-      const uint32_t real = w == (int)W - 1 ? key_len - 4 * (W - 1) : 4;
-      for (uint32_t shift = 32 - 8 * real; shift < 32; shift += 8, pass++) {
-        launch_radix_pass(kin, idx, (uint32_t)n, (int)shift, 256, hist, unused_total, ws, K[pass & 1], I[pass & 1],
-                          st, launches);
-        kin = K[pass & 1];
-        idx = I[pass & 1];
-      }
-    }
-  }
-
-  sort_fixed_offsets_kernel<<<grid_for(n), kSortThreads, 0, st>>>(n, record_bytes, src_off, sdst, len);
+  sort_fixed_offsets_kernel<<<grid_for(n), kSortThreads, 0, st>>>(n, record_bytes, w.src_off, w.sdst, w.len);
   if (launches) *launches += 1;
   PartitionPlan plan;
-  plan.src_off = src_off;
-  plan.sdst = sdst;
+  plan.src_off = w.src_off;
+  plan.sdst = w.sdst;
   plan.idx = idx;
-  launch_partition_gather(d_rec, len, n, plan, d_dst, st, launches);
+  launch_partition_gather(d_rec, w.len, n, plan, d_dst, st, launches);
 }
 
 }  // namespace b2s

@@ -61,6 +61,8 @@ PROTOTYPES = [
     ("b2sh_reader_read", C.c_int, [_vp, C.POINTER(_u32)]),
     ("b2sh_reader_read_sorted", C.c_int,
      [_vp, _u32, _u32, _u32, C.POINTER(_vp), C.POINTER(_u64), C.POINTER(_u64)]),
+    ("b2sh_reader_read_sorted_rows", C.c_int,
+     [_vp, _u32, _u32, _u32, _i32, C.POINTER(_vp), C.POINTER(_u64), C.POINTER(_u64)]),
     ("b2sh_reader_block", C.c_int,
      [_vp, _u32, C.POINTER(_i64), C.POINTER(_i32), C.POINTER(_i32), C.POINTER(_vp), C.POINTER(_u64)]),
     ("b2sh_reader_remote_bytes_read", _u64, [_vp]),
@@ -328,6 +330,15 @@ class S3ShuffleReader:
         p, ln, nrec = _vp(), _u64(), _u64()
         _check(load().b2sh_reader_read_sorted(self._h, recordBytes, keyOffset, keyLength, C.byref(p), C.byref(ln),
                                               C.byref(nrec)))
+        return (C.string_at(p.value, ln.value) if ln.value else b""), nrec.value
+
+    def readSortedRows(self, keyType, keyOffset, keyLength, nullField=-1):
+        """read() of a SQL exchange sorted by one typed key (spark.shuffle.s3.gpu.sortRows): every UnsafeRowSerializer
+        record of the task in ascending key order, nulls first, stable.  Fetched blocks only (no exchange cache).
+        -> (bytes, number of records)"""
+        p, ln, nrec = _vp(), _u64(), _u64()
+        _check(load().b2sh_reader_read_sorted_rows(self._h, keyType, keyOffset, keyLength, nullField, C.byref(p),
+                                                   C.byref(ln), C.byref(nrec)))
         return (C.string_at(p.value, ln.value) if ln.value else b""), nrec.value
 
     def _blocks(self, n):

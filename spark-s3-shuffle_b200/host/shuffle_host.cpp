@@ -831,6 +831,62 @@ class S3ShuffleReader {
       return;
     }
   }
+  // read() for a Spark SQL exchange whose rows the reducer sorts by one typed key (INTEGRATION.md §3g): every non-empty
+  // block is fetched and staged, then ONE b2s_decompress_sort_rows_packed call verifies, decodes and sorts the task's
+  // UnsafeRowSerializer records ([int32 big-endian size][row]) by the key keyType at row offset keyOff, nulls first
+  // (nullField: the key's null bit, -1 = none).  Blocks go in computeShuffleBlocks order, so equal keys come out in map,
+  // then reduce-id order.  Codec NONE is verified and sorted only.  It reads fetched blocks only: the exchange cache is
+  // not consulted.
+  void readSortedRows(uint32_t keyType, uint32_t keyOff, uint32_t keyLen, int32_t nullField) {
+    start(true);
+    std::vector<std::pair<uint64_t, std::vector<uint8_t>>> fetched;  // (tag, compressed bytes)
+    drainWhole(fetched);
+    std::sort(fetched.begin(), fetched.end(), [](const auto& a, const auto& b) { return a.first < b.first; });
+    const bool verify = d_.checksumEnabled;
+    const uint32_t alg = verify ? S3ShuffleHelper::createChecksumAlgorithm(d_.checksumAlgorithm) : 0;
+    ensure_codec_runtime();
+    const uint32_t codec = (uint32_t)d_.codecId();
+    const uint32_t n = (uint32_t)fetched.size();
+    std::vector<uint64_t> off, len, sliceLen, sliceSum;
+    std::vector<uint32_t> sliceBase(1, 0);
+    uint64_t bytes = 0;
+    for (const auto& f : fetched) {
+      const ShuffleBlockInfo& bi = info_[f.first];
+      off.push_back(bytes);
+      len.push_back(f.second.size());
+      bytes += f.second.size();
+      sliceLen.insert(sliceLen.end(), bi.sliceLen.begin(), bi.sliceLen.end());
+      sliceSum.insert(sliceSum.end(), bi.sliceSum.begin(), bi.sliceSum.end());
+      sliceBase.push_back((uint32_t)sliceLen.size());
+    }
+    PinnedArena src;
+    src.resize(bytes ? bytes : 1);
+    for (uint32_t k = 0; k < n; k++) memcpy(src.data() + off[k], fetched[k].second.data(), (size_t)len[k]);
+    // output size as in readSorted: a first guess, then one retry with the bytes needed
+    uint64_t cap = codec == B2S_CODEC_NONE ? bytes : bytes * 4;
+    std::vector<int32_t> status(n), bad(n);
+    uint64_t total = 0, records = 0;
+    int rc = B2S_E_DST_TOO_SMALL;
+    for (int attempt = 0; attempt < 2 && rc == B2S_E_DST_TOO_SMALL; attempt++) {
+      if (attempt) cap = total;
+      sorted_.reset(new uint8_t[(size_t)(cap ? cap : 1)]);
+      rc = b2s_decompress_sort_rows_packed(codec, alg, n, src.data(), off.data(), len.data(),
+                                           verify ? sliceBase.data() : nullptr, verify ? sliceLen.data() : nullptr,
+                                           verify ? sliceSum.data() : nullptr, keyType, keyOff, keyLen, nullField,
+                                           sorted_.get(), cap, &total, &records, status.data(), bad.data());
+    }
+    if (rc != 0)
+      throw CodecException(std::string("b2s_decompress_sort_rows_packed: ") + b2s_strerror(rc) + ": " +
+                           b2s_last_error());
+    for (uint32_t k = 0; k < n; k++) {
+      if (status[k] == B2S_E_CHECKSUM)  // storage/S3ChecksumValidationStream.scala:72-74
+        throw SparkException("Invalid checksum detected for " + info_[fetched[k].first].id.name());
+      if (status[k] == B2S_E_CORRUPT) throw IOException("Stream is corrupted");
+      if (status[k] != 0) throw IOException(std::string("decompress failed: ") + b2s_strerror(status[k]));
+    }
+    sortedLen_ = total;
+    sortedRecords_ = records;
+  }
   const uint8_t* sortedData() const { return sorted_.get(); }
   uint64_t sortedLen() const { return sortedLen_; }
   uint64_t sortedRecords() const { return sortedRecords_; }
@@ -1203,6 +1259,15 @@ int b2sh_reader_read_sorted(b2sh_reader* r, uint32_t record_bytes, uint32_t key_
                             const uint8_t** data, uint64_t* len, uint64_t* n_records) {
   return guarded([&] {
     r->r->readSorted(record_bytes, key_off, key_len);
+    *data = r->r->sortedData();
+    *len = r->r->sortedLen();
+    *n_records = r->r->sortedRecords();
+  });
+}
+int b2sh_reader_read_sorted_rows(b2sh_reader* r, uint32_t key_type, uint32_t key_off, uint32_t key_len,
+                                 int32_t null_field, const uint8_t** data, uint64_t* len, uint64_t* n_records) {
+  return guarded([&] {
+    r->r->readSortedRows(key_type, key_off, key_len, null_field);
     *data = r->r->sortedData();
     *len = r->r->sortedLen();
     *n_records = r->r->sortedRecords();
