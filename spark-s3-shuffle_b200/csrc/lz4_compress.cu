@@ -9,11 +9,17 @@
 // serial piece is isolated and given one THREAD per codec block, and the abundant HBM bandwidth carries small
 // intermediates between the phases:
 //
-//   A  lz4_match_kernel   warp per block, all lanes busy, no parse dependency: for every position p of a FIXED window
-//                         of 32 positions look the 4 bytes up in a per-warp u16 hash table in shared memory (state
-//                         before the window; byte runs use the offset-1 candidate), verify the candidate, measure
-//                         the match locally up to 8 bytes  ->  off[p] (u16, 0 = none), ml8[p] (u8);
+//   A  lz4_match_kernel   CTA per block, its W warps on W contiguous segments of the block: for every position p of a
+//                         FIXED window of 32 positions look the 4 bytes up in a per-warp u16 hash table in shared
+//                         memory (state before the window; byte runs use the offset-1 candidate), verify the
+//                         candidate, measure the match  ->  off[p] (u16, 0 = none), ml[p] (u16);
 //                         then insert the 32 positions (highest position wins a slot, deterministic).
+//                         The block is staged in shared memory once (cp.async.bulk), so no source read goes to
+//                         global memory.  Each warp starts from the exact table the sequential walk holds at its
+//                         segment's first window: a slot holds the highest earlier position hashing to it, a per-slot
+//                         maximum, so it is the exclusive prefix max of the tables of the segments before.
+//                         HLOG 13 (Zstandard level >= 3) runs lz4_match_warp_kernel instead: warp per block, words
+//                         from global memory.
 //   B  lz4_parse_kernel   THREAD per block: greedy walk over ml8[] (8 positions per 64-bit load), long matches
 //                         extended on the source; emits one 8-byte record per sequence with its output offset
 //                         (running sum — no scan needed later), decides RAW (compressedLength >= originalLength).
@@ -29,7 +35,8 @@
 namespace b2s {
 
 constexpr int kMinMatch = 4, kMFLimit = 12, kLastLiterals = 5;
-constexpr int kMatchWarps = 9;  // 9 warps x 8 KiB tables = 72 KiB per CTA, 3 CTAs per SM = 27 warps
+constexpr int kMatchMaxWarps = 16;  // per CTA; the launcher picks W from the shared-memory budget
+constexpr int kMatchWarps = 9;  // warp-per-block kernel (HLOG 13): 9 warps x 16 KiB tables = 144 KiB, 1 CTA per SM
 
 __device__ __forceinline__ uint32_t find_stream_of_block(const uint32_t* __restrict__ blk_base, uint32_t n_streams,
                                                          uint32_t b) {
@@ -62,6 +69,242 @@ __device__ __forceinline__ BlockSpan block_span(const uint8_t* __restrict__ src_
 // ------------------------------------------------------------------------------------------------------------
 // A: match finding
 // ------------------------------------------------------------------------------------------------------------
+// Shared memory of one CTA: the staged block (stage_bytes), then W hash tables of 2^HLOG u16 slots.  Stage byte i holds
+// the source byte at (block start rounded down to 16) + i, so the aligned interior of the block arrives with one bulk
+// copy whatever the block's offset; the head and tail bytes outside that interior are plain loads, and no read goes
+// past the block's last byte.  stage_bytes >= block_size + 31 covers the offset (<= 15) and the 12-byte reads at the
+// block's end.
+__device__ __forceinline__ uint32_t smem_addr(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+
+// bytes i..i+3 of the staged block (little-endian)
+__device__ __forceinline__ uint32_t stage_rd32(const uint32_t* st32, int i) {
+  return __funnelshift_r(st32[i >> 2], st32[(i >> 2) + 1], (i & 3) * 8);
+}
+
+template <int HLOG>
+__global__ void __launch_bounds__(kMatchMaxWarps * 32, 2) lz4_match_kernel(
+    const uint8_t* __restrict__ src_base, const uint64_t* __restrict__ src_off, const uint64_t* __restrict__ src_len,
+    const uint32_t* __restrict__ blk_base, uint32_t n_streams, uint32_t b0, uint32_t m, uint32_t block_size,
+    uint32_t stride, uint32_t near_limit, uint16_t* __restrict__ offarr, uint16_t* __restrict__ mlarr,
+    unsigned int* __restrict__ work_counter, uint32_t stage_bytes) {
+  extern __shared__ __align__(16) uint8_t smem[];
+  __shared__ __align__(8) uint64_t bar;  // completion of the bulk copy
+  __shared__ const uint8_t* blk_src;     // source address of stage byte 0
+  __shared__ uint32_t blk_id;
+  __shared__ int blk_n, blk_a, blk_bulk;
+  constexpr unsigned FULL = 0xffffffffu;
+  const int W = blockDim.x >> 5, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const uint32_t* st32 = reinterpret_cast<const uint32_t*>(smem);
+  uint16_t* tables = reinterpret_cast<uint16_t*>(smem + stage_bytes);
+  uint16_t* table = tables + (size_t)warp * (1 << HLOG);
+  // Lane l owns window position r = 31 - l: same-address shared stores resolve in favour of the lowest lane on this
+  // part, so a contested hash slot receives the highest position on the first store and the read-back that
+  // guarantees determinism almost never iterates.
+  const int r_me = 31 - lane;
+  const uint32_t bar_a = smem_addr(&bar);
+  if (threadIdx.x == 0) {
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar_a) : "memory");
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  uint32_t phase = 0;
+
+  for (;;) {
+    __syncthreads();  // the previous block's staged bytes and tables are no longer read
+    if (threadIdx.x == 0) {
+      const uint32_t bl = atomicAdd(work_counter, 1u);
+      blk_id = bl;
+      if (bl < m) {
+        const BlockSpan B = block_span(src_base, src_off, src_len, blk_base, n_streams, b0 + bl, block_size);
+        const int a = (int)(reinterpret_cast<uintptr_t>(B.s) & 15u);
+        const int lo = (a + 15) & ~15, hi = (a + B.n) & ~15;
+        blk_src = B.s - a;
+        blk_n = B.n;
+        blk_a = a;
+        blk_bulk = hi > lo;
+        if (hi > lo) {
+          // order the generic-proxy reads of the previous block before the async-proxy writes of this one
+          asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+          asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar_a), "r"(hi - lo) : "memory");
+          asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                       ::"r"(smem_addr(smem + lo)), "l"(B.s - a + lo), "r"(hi - lo), "r"(bar_a) : "memory");
+        }
+      }
+    }
+    __syncthreads();
+    const uint32_t bl = blk_id;
+    if (bl >= m) break;
+    const int n = blk_n, a = blk_a;
+    {
+      const uint8_t* g = blk_src;
+      const int lo = (a + 15) & ~15, hi = (a + n) & ~15;
+      const int head_end = lo < a + n ? lo : a + n, tail_beg = hi > lo ? hi : lo;
+      for (int i = a + threadIdx.x; i < head_end; i += blockDim.x) smem[i] = __ldg(g + i);
+      for (int i = tail_beg + threadIdx.x; i < a + n; i += blockDim.x) smem[i] = __ldg(g + i);
+    }
+    if (blk_bulk) {
+      uint32_t done;
+      do {
+        asm volatile(
+            "{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2; selp.u32 %0, 1, 0, p; }"
+            : "=r"(done)
+            : "r"(bar_a), "r"(phase)
+            : "memory");
+      } while (!done);
+      phase ^= 1u;
+    }
+    __syncthreads();  // head and tail bytes visible
+    if (n < kMFLimit + 1) continue;
+    const int mflimit = n - kMFLimit;
+    const int matchlimit = n - kLastLiterals;
+    // warp j walks windows [wb, we): contiguous segments, in block order
+    const int nw = mflimit / 32 + 1, per = (nw + W - 1) / W;
+    const int wb = warp * per < nw ? warp * per : nw;
+    const int we = wb + per < nw ? wb + per : nw;
+
+    // pass 1: the table of the warp's own segment alone (the last segment's is never needed)
+    if (warp < W - 1) {
+      uint4* t4 = reinterpret_cast<uint4*>(table);
+      for (int j = lane; j < (1 << HLOG) / 8; j += 32) t4[j] = make_uint4(0, 0, 0, 0);
+      __syncwarp();
+      for (int k = wb; k < we; k++) {
+        const int p = 32 * k + r_me;
+        const bool valid = p <= mflimit;
+        const uint32_t h = (stage_rd32(st32, a + (valid ? p : mflimit)) * 2654435761u) >> (32 - HLOG);
+        if (valid) table[h] = (uint16_t)p;
+        __syncwarp();
+        for (;;) {
+          const bool lost = valid && table[h] < (uint16_t)p;
+          if (!__ballot_sync(FULL, lost)) break;
+          if (lost) table[h] = (uint16_t)p;
+          __syncwarp();
+        }
+      }
+    }
+    __syncthreads();
+    // exclusive prefix max over the W tables, two slots per word: table j becomes the state before segment j
+    {
+      uint32_t* t32 = reinterpret_cast<uint32_t*>(tables);
+      constexpr int TW = (1 << HLOG) / 2;
+      for (int k = threadIdx.x; k < TW; k += blockDim.x) {
+        uint32_t run = 0;
+        for (int j = 0; j < W; j++) {
+          const uint32_t t = t32[j * TW + k];
+          t32[j * TW + k] = run;
+          run = __vmaxu2(run, t);
+        }
+      }
+    }
+    __syncthreads();
+
+    // pass 2: the sequential window walk over the segment.
+    // Full match lengths come without touching the source almost always: if positions p and p+1 both matched with the
+    // same offset, then L[p] = L[p+1] + 1 (same alignment of the comparison).  So inside a window every run of equal
+    // offsets takes its lengths from the run's last position q: L[p] = L[q] + (q - p), and L[q] is the local length
+    // unless q is itself "long" (8 local bytes equal, room to grow) — only those run ends are measured, cooperatively,
+    // 32 bytes per ballot round (past the segment's end if need be: the whole block is staged).  A run that fills the
+    // whole window and continues the previous window's run takes the length of its last position from the carry
+    // instead; carry_off = 0 disables that at the segment's first window, which only costs a measurement.
+    uint32_t carry_off = 0;
+    int carry_L = 0;
+    uint32_t carry_v = wb > 0 ? stage_rd32(st32, a + 32 * wb - 1) : 0u;  // the 4 bytes at the window start - 1
+    uint16_t* oq = offarr + (size_t)bl * stride + 32 * wb + r_me;  // position < stride always
+    uint16_t* mq = mlarr + (size_t)bl * stride + 32 * wb + r_me;
+    for (int k = wb; k < we; k++) {
+      const int pos = 32 * k;
+      const int p = pos + r_me;
+      const bool valid = p <= mflimit;
+      const int pc = valid ? p : mflimit;
+      const int i = a + pc;
+      const unsigned sh = (i & 3) * 8;
+      const uint32_t w1 = st32[(i >> 2) + 1];
+      const uint32_t v = __funnelshift_r(st32[i >> 2], w1, sh);
+      const uint32_t v2 = __funnelshift_r(w1, st32[(i >> 2) + 2], sh);
+      // byte run: the 4 bytes at p-1 equal those at p, i.e. v(p-1) == v(p) — the neighbour lane's value
+      const uint32_t vprev = __shfl_down_sync(FULL, v, 1);
+      bool rle = vprev == v;
+      if (lane == 31) rle = pos > 0 && carry_v == v;
+      carry_v = __shfl_sync(FULL, v, 0);
+      const uint32_t h = (v * 2654435761u) >> (32 - HLOG);
+      int cand = table[h];
+      if (rle) cand = pc - 1;
+      const bool older = cand < pc;
+      if (!older) cand = 0;
+      // verify, local match length (<= 8)
+      const int ci = a + cand;  // cand + 11 < p + 11 <= n - 1
+      const unsigned csh = (ci & 3) * 8;
+      const uint32_t c1 = st32[(ci >> 2) + 1];
+      const bool ok = valid && older && __funnelshift_r(st32[ci >> 2], c1, csh) == v;
+      const uint32_t x = __funnelshift_r(c1, st32[(ci >> 2) + 2], csh) ^ v2;
+      int ml = x ? 4 + ((__ffs(x) - 1) >> 3) : 8;
+      const int lim = matchlimit - pc;
+      ml = ml < lim ? ml : lim;
+      const bool lng = ok && x == 0 && lim > 8;
+      const uint32_t off = ok ? (uint32_t)(pc - cand) : 0u;
+      int L = ok ? ml : 0;
+      const unsigned lngmask = __brev(__ballot_sync(FULL, lng));  // bit r <-> window position r
+      if (lngmask) {
+        const uint32_t next_off = __shfl_up_sync(FULL, off, 1);   // position r+1 lives in lane-1
+        const bool brk = lane == 0 || off == 0 || off != next_off;
+        const unsigned brkmask = __brev(__ballot_sync(FULL, brk));  // run ends; bit 31 always set
+        unsigned extmask = brkmask & lngmask;
+        const uint32_t off0 = __shfl_sync(FULL, off, 31);  // position 0
+        if ((extmask >> 31) && (brkmask & 0x7fffffffu) == 0 && off0 == carry_off) {
+          extmask &= 0x7fffffffu;  // one run through the whole window, continuing the carried one
+          if (lane == 0) L = carry_L - 32;
+        }
+        while (extmask) {
+          const int q = __ffs(extmask) - 1;
+          extmask &= extmask - 1;
+          const int oq_ = (int)__shfl_sync(FULL, off, 31 - q);
+          const int mpos = pos + q;
+          const int maxl = matchlimit - mpos;
+          const uint8_t* sa = smem + a + mpos + lane;
+          const uint8_t* sc = sa - oq_;
+          int Lq = maxl;
+          for (int base = 8;; base += 32) {
+            const int kk = base + lane;
+            const bool stop = kk >= maxl || sa[base] != sc[base];
+            const unsigned bm = __ballot_sync(FULL, stop);
+            if (bm) {
+              const int e = base + __ffs(bm) - 1;
+              Lq = e < maxl ? e : maxl;
+              break;
+            }
+          }
+          if (r_me == q) L = Lq;
+        }
+        // lengths inside runs from their ends
+        const int d = __ffs(brkmask >> r_me) - 1;  // distance to my run's last position
+        const int Lend = __shfl_sync(FULL, L, lane - d);
+        if (off) L = Lend + d;
+      }
+      carry_off = __shfl_sync(FULL, off, 0);
+      carry_L = __shfl_sync(FULL, L, 0);
+      __stcs(oq, (uint16_t)off);
+      // Snappy (near_limit = 2048, blocks <= 32 KiB so L < 2^15): bit 15 tells the parse kernel that the offset fits
+      // the 2-byte copy element, sparing it a dependent load of off[]
+      __stcs(mq, (uint16_t)(L | ((off != 0u && off < near_limit) ? 0x8000 : 0)));
+      oq += 32;
+      mq += 32;
+
+      // insert the window; a read-back settles slots hit twice so that the highest position wins
+      __syncwarp();
+      if (valid) table[h] = (uint16_t)p;
+      __syncwarp();
+      for (;;) {
+        const bool lost = valid && table[h] < (uint16_t)p;
+        if (!__ballot_sync(FULL, lost)) break;
+        if (lost) table[h] = (uint16_t)p;
+        __syncwarp();
+      }
+    }
+  }
+}
+
+// A, warp per block: the kernel for HLOG 13 (Zstandard level >= 3).  Its 16 KiB tables leave room for few warps per
+// SM in the CTA-per-block kernel, whose per-block table work (zeroing, pass 1, prefix max) doubles with the table, and
+// that kernel measured slower there (bench.py --config 5, DESIGN §5).  Source and candidate words come from global
+// memory.
 // Candidate words of one window, requested in iteration k and consumed in iteration k+1 so that their latency is
 // covered by a whole iteration of table work (the hash-table chain window -> insert -> next lookup never waits on
 // a global load).
@@ -73,7 +316,7 @@ struct PendingWindow {
 };
 
 template <int HLOG>
-__global__ void __launch_bounds__(kMatchWarps * 32, 3) lz4_match_kernel(
+__global__ void __launch_bounds__(kMatchWarps * 32, 3) lz4_match_warp_kernel(
     const uint8_t* __restrict__ src_base, const uint64_t* __restrict__ src_off, const uint64_t* __restrict__ src_len,
     const uint32_t* __restrict__ blk_base, uint32_t n_streams, uint32_t b0, uint32_t m, uint32_t block_size,
     uint32_t stride, uint32_t near_limit, uint16_t* __restrict__ offarr, uint16_t* __restrict__ mlarr,
@@ -549,15 +792,57 @@ static void launch_match_t(const uint8_t* src_base, const uint64_t* d_src_off, c
                            const uint32_t* d_blk_base, uint32_t n_streams, uint32_t b0, uint32_t m,
                            uint32_t block_size, uint32_t stride, uint32_t near_limit, uint16_t* d_off,
                            uint16_t* d_ml, unsigned int* d_counter, cudaStream_t st) {
-  const size_t smem = (size_t)kMatchWarps * (2u << HLOG);
+  // W warps per CTA and CTAs per SM from the shared-memory budget: the staged block plus W tables per CTA.  The most
+  // warps per SM wins, two CTAs on a tie (one CTA stages its next block while the other computes).  The budget leaves
+  // 64 KiB of the SM's shared memory to L1 (a 164 KiB carve-out instead of 228 on H100): the parse kernel of the
+  // previous chunk runs beside this one, one thread per block streaming ml[] through L1 prefetches, and it slows down
+  // by up to 2.5x when L1 is smaller than what its co-resident threads prefetch.  Measured on the config-2 and config-3
+  // write passes (DESIGN §5).  HLOG 12 with 32 KiB blocks: 1 CTA x 16 warps; HLOG 11: 2 x 12;
+  // 64 KiB blocks at HLOG 12: 1 x 12.
+  int dev = 0, sm_smem = 0, reserved = 0;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&sm_smem, cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev);
+  cudaDeviceGetAttribute(&reserved, cudaDevAttrReservedSharedMemoryPerBlock, dev);
+  sm_smem -= 64 << 10;
+  cudaFuncAttributes fa;
+  cudaFuncGetAttributes(&fa, lz4_match_kernel<HLOG>);
+  const uint32_t stage = (block_size + 31u + 15u) & ~15u;
+  const long table = 2l << HLOG;
+  int warps = 0, ctas = 0;
+  for (int c = 2; c >= 1; c--) {
+    const long room = (long)sm_smem / c - reserved - (long)fa.sharedSizeBytes - stage;
+    const int w = room < table ? 0 : (int)(room / table < kMatchMaxWarps ? room / table : kMatchMaxWarps);
+    if (w * c > warps * ctas) {
+      warps = w;
+      ctas = c;
+    }
+  }
+  const size_t smem = stage + (size_t)warps * table;
   cudaFuncSetAttribute(lz4_match_kernel<HLOG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);  // per device and cheap: set on every launch
   int per_sm = 0;
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, lz4_match_kernel<HLOG>, kMatchWarps * 32, smem);
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, lz4_match_kernel<HLOG>, warps * 32, smem);
+  if (per_sm > ctas) per_sm = ctas;
+  if (per_sm < 1) per_sm = 1;
+  uint64_t grid = (uint64_t)kSMs * per_sm;  // persistent: one wave, CTAs pull blocks from the counter
+  if (grid > m) grid = m;
+  lz4_match_kernel<HLOG><<<(unsigned)grid, warps * 32, smem, st>>>(
+      src_base, d_src_off, d_src_len, d_blk_base, n_streams, b0, m, block_size, stride, near_limit, d_off, d_ml,
+      d_counter, stage);
+}
+
+static void launch_match_warp_13(const uint8_t* src_base, const uint64_t* d_src_off, const uint64_t* d_src_len,
+                                 const uint32_t* d_blk_base, uint32_t n_streams, uint32_t b0, uint32_t m,
+                                 uint32_t block_size, uint32_t stride, uint32_t near_limit, uint16_t* d_off,
+                                 uint16_t* d_ml, unsigned int* d_counter, cudaStream_t st) {
+  const size_t smem = (size_t)kMatchWarps * (2u << 13);
+  cudaFuncSetAttribute(lz4_match_warp_kernel<13>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);  // per device and cheap: set on every launch
+  int per_sm = 0;
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, lz4_match_warp_kernel<13>, kMatchWarps * 32, smem);
   if (per_sm < 1) per_sm = 1;
   uint64_t want = ((uint64_t)m + kMatchWarps - 1) / kMatchWarps;
   uint64_t grid = (uint64_t)kSMs * per_sm;  // persistent: one wave, warps pull blocks from the counter
   if (grid > want) grid = want;
-  lz4_match_kernel<HLOG><<<(unsigned)grid, kMatchWarps * 32, smem, st>>>(
+  lz4_match_warp_kernel<13><<<(unsigned)grid, kMatchWarps * 32, smem, st>>>(
       src_base, d_src_off, d_src_len, d_blk_base, n_streams, b0, m, block_size, stride, near_limit, d_off, d_ml,
       d_counter);
 }
@@ -619,7 +904,10 @@ void launch_lz4_match(const uint8_t* src_base, const uint64_t* d_src_off, const 
   switch (hlog > 0 ? hlog : g_lz4_hlog) {
     case 10: B2S_LZ4M(10); break;
     case 11: B2S_LZ4M(11); break;
-    case 13: B2S_LZ4M(13); break;
+    case 13:  // Zstandard level >= 3
+      launch_match_warp_13(src_base, d_src_off, d_src_len, d_blk_base, n_streams, b0, m, block_size, w.stride,
+                           near_limit, w.off, w.ml, d_counter, st);
+      break;
     default: B2S_LZ4M(12); break;
   }
 #undef B2S_LZ4M
