@@ -307,6 +307,7 @@ int orc_lz4_decompress_block(const uint8_t* src, int src_len, uint8_t* dst, int 
         if (ip >= src_len) return -1;
         b = src[ip++];
         ll += b;
+        if (ll > orig_len) return -1; /* cannot be valid, and a long run of 0xFF bytes must not wrap the counter */
       } while (b == 255);
     }
     if (ll > orig_len - op || ll > src_len - ip) return -1;
@@ -327,6 +328,7 @@ int orc_lz4_decompress_block(const uint8_t* src, int src_len, uint8_t* dst, int 
         if (ip >= src_len) return -1;
         b = src[ip++];
         ml += b;
+        if (ml > orig_len) return -1;
       } while (b == 255);
     }
     ml += LZ4_MINMATCH;

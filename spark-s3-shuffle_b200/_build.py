@@ -14,7 +14,7 @@ OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libb200shuffle.so")
 HOST_LIB = os.path.join(HERE, "libb200shuffle_host.so")
 HOST_SRC = os.path.join(HERE, "host", "shuffle_host.cpp")
-SOURCES = ["api.cu", "scan.cu", "partition.cu", "sort.cu", "rows.cu", "exchange.cu", "checksum.cu", "xxh32.cu", "lz4.cu", "lz4_compress.cu", "lz4_decode.cu", "snappy.cu", "zstd.cu", "zstd_enc.cu", "gen.cu"]
+SOURCES = ["api.cu", "scan.cu", "partition.cu", "sort.cu", "rows.cu", "exchange.cu", "checksum.cu", "xxh32.cu", "lz4_compress.cu", "lz4_decode.cu", "snappy.cu", "zstd.cu", "zstd_enc.cu", "gen.cu"]
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = GENCODE + [
     "-O3", "-lineinfo", "-std=c++17",

@@ -492,7 +492,7 @@ struct DecompressJob {
   uint64_t *h_src_off = nullptr, *h_src_len = nullptr;
   uint64_t *h_slice_off = nullptr, *h_slice_len = nullptr, *h_slice_sum = nullptr;
   uint32_t *h_slice_owner = nullptr, *h_slice_base = nullptr;
-  uint64_t* h_totals = nullptr;  // [nb_total, olen_total]
+  uint64_t* h_totals = nullptr;  // [nb_total, olen_total, Snappy: largest chunk olen, clen]
   uint64_t *h_dst_off = nullptr, *h_dst_len = nullptr;
   int32_t *h_status = nullptr, *h_bad = nullptr;
   size_t up_bytes = 0, down_bytes = 0;
@@ -625,7 +625,7 @@ int decompress_enqueue_a(Slot& S, const ChecksumTables& tabs, uint32_t alg, Deco
     CU(cudaMemcpyAsync(J.olen, J.src_len, (size_t)n * 8, cudaMemcpyDeviceToDevice, st));
     CU(cudaMemsetAsync(J.nblk, 0, (size_t)n * 8, st));
   } else
-    launch_lz4block_count(d_src, J.src_off, J.src_len, n, J.nblk, J.olen, J.totals + 2, J.status, st, launches);
+    launch_lz4block_count(d_src, J.src_off, J.src_len, n, J.nblk, J.olen, J.status, st, launches);
   // dst_off = exclusive scan(olen) ; blk_base = exclusive scan(nblk) (in place)
   CU(cudaMemcpyAsync(J.dst_off, J.olen, (size_t)n * 8, cudaMemcpyDeviceToDevice, st));
   launch_exclusive_scan_u64(J.dst_off, n, J.totals + 1, J.ws, st, launches);
@@ -666,18 +666,17 @@ int decompress_enqueue_b(Slot& S, DecompressJob& J, const uint8_t* d_src, uint8_
     launch_lz4block_fill(d_src, J.src_off, J.src_len, J.n, J.nblk, J.dst_off, J.olen, dst_cap, J.status, desc, st,
                          launches);
   CU(cudaEventRecord(S.ev_t0, st));
-  const uint64_t max_olen = J.h_totals[2], max_clen = J.h_totals[3];
-  const bool small_blocks = max_olen <= 65536 && max_clen < 65536;
-  if (J.codec == B2S_CODEC_SNAPPY_XERIAL && !small_blocks)
-    return fail(B2S_E_UNSUPPORTED, "snappy chunks larger than 64 KiB are not supported%s");
-  if (J.nb && small_blocks && J.codec == B2S_CODEC_LZ4BLOCK) {
+  if (J.nb && J.codec == B2S_CODEC_LZ4BLOCK) {
     // one launch over every codec block: warp per block, parse and copies together (lz4_decode.cu)
     cudaEvent_t e0 = nullptr, e1 = nullptr;
     S.dom_pair(&e0, &e1);
     CU(cudaEventRecord(e0, st));
     launch_lz4_decode_warp(desc, (uint32_t)J.nb, d_src, d_dst, J.status, J.counter, st, launches);
     CU(cudaEventRecord(e1, st));
-  } else if (J.nb && small_blocks && J.codec == B2S_CODEC_SNAPPY_XERIAL) {
+  } else if (J.nb && J.codec == B2S_CODEC_SNAPPY_XERIAL) {
+    const uint64_t max_olen = J.h_totals[2], max_clen = J.h_totals[3];
+    if (max_olen > 65536 || max_clen >= 65536)
+      return fail(B2S_E_UNSUPPORTED, "snappy chunks larger than 64 KiB are not supported%s");
     // tokens (thread per block) + copy (lane per sequence), in chunks that bound the record workspace
     const uint32_t nb = (uint32_t)J.nb;
     const uint32_t rec_stride = snappy_decode_rec_stride((uint32_t)max_clen);
@@ -703,13 +702,10 @@ int decompress_enqueue_b(Slot& S, DecompressJob& J, const uint8_t* d_src, uint8_
       cudaEvent_t e0 = nullptr, e1 = nullptr;
       S.dom_pair(&e0, &e1);
       CU(cudaEventRecord(e0, st));
-      launch_lz4_copy(desc, b0, m, rec_stride, d_src, d_dst, ws, nrec, st, launches);
+      launch_snappy_copy(desc, b0, m, rec_stride, d_src, d_dst, ws, nrec, st, launches);
       CU(cudaEventRecord(e1, st));
       CU(cudaEventRecord(S.ev_free[par], st));
     }
-  } else if (J.nb) {
-    // LZ4Block with a codec block over 64 KiB (lz4-java allows up to 32 MiB): the tile decoder takes the whole batch
-    launch_lz4_decompress(desc, (uint32_t)J.nb, d_src, d_dst, J.status, J.counter, st, launches);
   }
   CU(cudaEventRecord(S.ev_t1, st));
   // One XXH32 pass over all decoded blocks after the last chunk.  Queueing it chunk by chunk on the side stream (beside

@@ -9,35 +9,6 @@ namespace b2s {
 
 constexpr int kSMs = 132;  // H100 SXM; grids are sized in multiples of this
 
-// ---- sub-warp tiles: TILE consecutive lanes cooperate on one codec block ----
-template <int TILE>
-__device__ __forceinline__ unsigned tile_mask() {
-  if constexpr (TILE == 32) {
-    return 0xffffffffu;
-  } else {
-    const unsigned lane = threadIdx.x & 31;
-    return ((1u << TILE) - 1u) << (lane & ~(TILE - 1));
-  }
-}
-template <int TILE>
-__device__ __forceinline__ unsigned tile_ballot(bool pred) {
-  const unsigned m = tile_mask<TILE>();
-  unsigned b = __ballot_sync(m, pred);
-  if constexpr (TILE == 32) {
-    return b;
-  } else {
-    return (b >> ((threadIdx.x & 31) & ~(TILE - 1))) & ((1u << TILE) - 1u);
-  }
-}
-template <int TILE, typename T>
-__device__ __forceinline__ T tile_shfl(T v, int src_lane_in_tile) {
-  return __shfl_sync(tile_mask<TILE>(), v, src_lane_in_tile, TILE);
-}
-template <int TILE>
-__device__ __forceinline__ void tile_sync() {
-  __syncwarp(tile_mask<TILE>());
-}
-
 // ---- unaligned little-endian 32-bit load from global memory: two aligned words + funnel shift.
 // Only ever touches the aligned words that contain bytes p..p+3 (safe at allocation edges).
 __device__ __forceinline__ uint32_t ld32u(const uint8_t* p) {

@@ -68,35 +68,20 @@ void launch_lz4block_stream_meta(const uint32_t* d_blk_base, uint32_t n_streams,
                                  uint64_t dst_cap, uint64_t* d_dst_off, uint64_t* d_dst_len, int32_t* d_status,
                                  cudaStream_t st, uint64_t* launches);
 
-// ---------------- lz4.cu (K4 + read-side LZ4Block framing) ----------------
+// ---------------- lz4_decode.cu (read-side LZ4Block framing + K4) ----------------
 // header walk pass 1: per stream block count + decoded bytes; malformed -> status CORRUPT (streams already failed are skipped)
-// d_maxima[0..1] (pre-zeroed) receive the largest originalLen / compressedLen of any codec block of the batch
 void launch_lz4block_count(const uint8_t* src_base, const uint64_t* d_src_off, const uint64_t* d_src_len, uint32_t n,
-                           uint64_t* d_nblk, uint64_t* d_olen, uint64_t* d_maxima, int32_t* d_status, cudaStream_t st,
-                           uint64_t* launches);
+                           uint64_t* d_nblk, uint64_t* d_olen, int32_t* d_status, cudaStream_t st, uint64_t* launches);
 // header walk pass 2: descriptors at d_blk_base[i]+k; streams that overflow dst_cap get status DST_TOO_SMALL + no-op descriptors
 void launch_lz4block_fill(const uint8_t* src_base, const uint64_t* d_src_off, const uint64_t* d_src_len, uint32_t n,
                           const uint64_t* d_blk_base, const uint64_t* d_dst_off, uint64_t* d_olen, uint64_t dst_cap,
                           int32_t* d_status, BlockDesc* d_desc, cudaStream_t st, uint64_t* launches);
-void launch_lz4_decompress(const BlockDesc* d_desc, uint32_t n_blocks, const uint8_t* src_base, uint8_t* dst_base,
-                           int32_t* d_status, unsigned int* d_counter, cudaStream_t st, uint64_t* launches);
-
-// ---------------- lz4_decode.cu (K4: LZ4 codec blocks <= 64 KiB; the copy kernel of the Snappy decoder) ------
-// Snappy record workspace: records per codec block, and bytes for chunk_blocks codec blocks
-uint32_t snappy_decode_rec_stride(uint32_t max_clen);
-size_t snappy_decode_ws_bytes(uint32_t chunk_blocks, uint32_t rec_stride);
-// codec blocks [b0, b0+m): the byte copies from the per-sequence records of launch_snappy_tokens in d_ws (d_nrec is
-// indexed by global block id).  A separate launch so that the token walk of chunk k+1 can run beside the copies of
-// chunk k.
-void launch_lz4_copy(const BlockDesc* d_desc, uint32_t b0, uint32_t m, uint32_t rec_stride, const uint8_t* src_base,
-                     uint8_t* dst_base, const uint8_t* d_ws, const uint32_t* d_nrec, cudaStream_t st,
-                     uint64_t* launches);
 // LZ4 codec blocks [0, nb) in one launch, a warp per block (parse + copies; malformed blocks set status[stream] =
 // B2S_E_CORRUPT).  d_counter: one device word of scratch.
 void launch_lz4_decode_warp(const BlockDesc* d_desc, uint32_t nb, const uint8_t* src_base, uint8_t* dst_base,
                             int32_t* d_status, unsigned int* d_counter, cudaStream_t st, uint64_t* launches);
 
-// ---------------- snappy.cu (K5: xerial framing, Snappy emit / tokens; match, parse and copy kernels are shared) ------
+// ---------------- snappy.cu (K5: xerial framing, Snappy emit / tokens / copy; match and parse kernels are shared) ------
 void launch_snappy_emit(const uint8_t* src_base, const uint64_t* d_src_off, const uint64_t* d_src_len,
                         const uint32_t* d_blk_base, uint32_t n_streams, uint32_t b0, uint32_t m, uint32_t block_size,
                         uint32_t stride, uint32_t max_seq, const uint16_t* d_off, const uint2* d_seq,
@@ -105,6 +90,8 @@ void launch_snappy_emit(const uint8_t* src_base, const uint64_t* d_src_off, cons
 void launch_xerial_stream_meta(const uint32_t* d_blk_base, uint32_t n_streams, uint32_t n_blocks, const uint64_t* d_scan,
                                const uint64_t* d_scan_total, uint8_t* dst_base, uint64_t dst_cap, uint64_t* d_dst_off,
                                uint64_t* d_dst_len, int32_t* d_status, cudaStream_t st, uint64_t* launches);
+// d_maxima[0..1] (pre-zeroed) receive the largest uncompressed / compressed length of any chunk of the batch (the
+// decoder takes chunks up to 64 KiB and sizes its records by the largest)
 void launch_xerial_count(const uint8_t* src_base, const uint64_t* d_src_off, const uint64_t* d_src_len, uint32_t n,
                          uint64_t* d_nblk, uint64_t* d_olen, uint64_t* d_maxima, int32_t* d_status, cudaStream_t st,
                          uint64_t* launches);
@@ -114,6 +101,15 @@ void launch_xerial_fill(const uint8_t* src_base, const uint64_t* d_src_off, cons
 void launch_snappy_tokens(const BlockDesc* d_desc, uint32_t b0, uint32_t m, const uint8_t* src_base, uint2* d_rec,
                           uint32_t rec_stride, uint32_t* d_nrec, int32_t* d_status, cudaStream_t st,
                           uint64_t* launches);
+// Snappy record workspace: records per codec block, and bytes for chunk_blocks codec blocks
+uint32_t snappy_decode_rec_stride(uint32_t max_clen);
+size_t snappy_decode_ws_bytes(uint32_t chunk_blocks, uint32_t rec_stride);
+// codec blocks [b0, b0+m): the byte copies from the per-sequence records of launch_snappy_tokens in d_ws (d_nrec is
+// indexed by global block id).  A separate launch so that the token walk of chunk k+1 can run beside the copies of
+// chunk k.
+void launch_snappy_copy(const BlockDesc* d_desc, uint32_t b0, uint32_t m, uint32_t rec_stride, const uint8_t* src_base,
+                        uint8_t* dst_base, const uint8_t* d_ws, const uint32_t* d_nrec, cudaStream_t st,
+                        uint64_t* launches);
 
 // ---------------- zstd.cu (K6: Zstandard frame decoding, block-parallel; core in zstd_core.h + zstd_par.h) ----------------
 // d_cnt / d_base: three arrays of n u64 each (blocks, sequences, literal-workspace bytes per stream); d_base holds their

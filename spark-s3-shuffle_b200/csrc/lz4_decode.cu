@@ -1,17 +1,19 @@
-// lz4_decode.cu — K4: LZ4 block decompression (LZ4_decompress_fast semantics: driven by originalLen, must consume
-// exactly compressedLen; oracle: orc_lz4_decompress_block), and the copy kernel of the Snappy decoder.
+// lz4_decode.cu — the read side of LZ4Block: the lz4-java stream framing and K4, LZ4 block decompression
+// (LZ4_decompress_fast semantics: driven by originalLen, must consume exactly compressedLen; oracle:
+// orc_lz4_decompress_block).  K3, the compressor, and the write-side framing live in lz4_compress.cu.
 //
 // Replaces liblz4's LZ4_decompress_fast as driven by lz4-java's LZ4BlockInputStream [U] under
 // serializerManager.wrapStream at storage/S3ShuffleReader.scala:107-109.
+// Wire format (oracle/b2s_oracle.c restates it): per <= blockSize bytes of input a 21-byte header
+//   "LZ4Block" | token = method(0x10 RAW, 0x20 LZ4) | level | compressedLen LE32 | originalLen LE32 | XXH32&0x0FFFFFFF LE32
+// then the payload; a stream ends with a header whose three ints are zero.
 //
-//   lz4_decode_warp_kernel  WARP per LZ4 codec block (<= 64 KiB), persistent grid: the token chain is resolved 32
-//                           sequences at a time by pointer doubling over speculative headers in a 128-byte window,
-//                           then the batch's literals and matches are copied as in the copy kernel.  Nothing goes
-//                           through HBM between parse and copy.  (The first, single-kernel decoder in lz4.cu carried
-//                           the serial chain on 8-lane tiles; it stays the path for codec blocks > 64 KiB.)
-//   lz4_copy_kernel         Snappy: warp per codec block, LANE per sequence, from the records of snappy_tokens_kernel
-//                           (snappy.cu): output positions by a warp scan, all literals of a batch of 32 sequences at
-//                           once, then the matches in dependency rounds (lz_batch.cuh).
+//   lz4block_walk_kernel    THREAD per stream: header walk, run twice (count codec blocks and decoded bytes, then write
+//                           one descriptor per codec block).
+//   lz4_decode_warp_kernel  WARP per LZ4 codec block of any size lz4-java writes (up to 32 MiB), persistent grid: the
+//                           token chain is resolved 32 sequences at a time by pointer doubling over speculative headers
+//                           in a 128-byte window, then the batch's literals and matches are copied (lz_batch.cuh).
+//                           Nothing goes through HBM between parse and copy.
 #include "kernels.h"
 #include "lz_batch.cuh"
 
@@ -19,73 +21,121 @@ namespace b2s {
 
 constexpr int kMinMatch = 4, kMFLimit = 12, kLastLiterals = 5;
 
-// The literals of a batch of up to 32 sequences (lane l: lit bytes from in + lip to out + op; lit == 0: none): all
-// lanes at once, runs longer than 16 bytes by the whole warp.  Ends with __syncwarp, so the literals are visible to the
-// match copies that follow.
-__device__ __forceinline__ void lz_copy_literals(const uint8_t* __restrict__ in, uint8_t* out, int lip, int lit, int op,
-                                                 int lane) {
-  constexpr unsigned FULL = 0xffffffffu;
-  if (lit > 0 && lit <= 16) {  // aligned 8-byte words of the compressed block (read-only: __ldg)
-    uint64_t lo, hi;
-    ld_span16<true>(in + lip, lit, lo, hi);
-    st_span16(out + op, lit, lo, hi);
-  }
-  unsigned biglit = __ballot_sync(FULL, lit > 16);
-  while (biglit) {
-    const int l = __ffs(biglit) - 1;
-    biglit &= biglit - 1;
-    const int n_l = __shfl_sync(FULL, lit, l), op_l = __shfl_sync(FULL, op, l), ip_l = __shfl_sync(FULL, lip, l);
-    if (n_l >= 96) group_copy<32>(out + op_l, in + ip_l, (uint32_t)n_l, lane);
-    else
-      for (int j = lane; j < n_l; j += 32) out[op_l + j] = __ldg(in + ip_l + j);
-  }
-  __syncwarp();
+// ------------------------------------------------------------------------------------------------------------
+// LZ4Block framing, read side: header walk (LZ4BlockInputStream.refill [U])
+// ------------------------------------------------------------------------------------------------------------
+struct Lz4bHeader {
+  int method;
+  int level;
+  int32_t clen, olen;
+  uint32_t check;
+  bool magic_ok;
+};
+__device__ __forceinline__ Lz4bHeader lz4b_read_header(const uint8_t* p) {
+  Lz4bHeader h;
+  h.magic_ok = ld32u_ro(p) == 0x42345A4Cu && ld32u_ro(p + 4) == 0x6B636F6Cu;
+  const int token = p[8];
+  h.method = token & 0xF0;
+  h.level = 10 + (token & 0x0F);
+  h.clen = (int32_t)ld32u_ro(p + 9);
+  h.olen = (int32_t)ld32u_ro(p + 13);
+  h.check = ld32u_ro(p + 17);
+  return h;
+}
+__device__ __forceinline__ bool lz4b_header_valid(const Lz4bHeader& h) {
+  if (!h.magic_ok) return false;
+  if (h.method != 0x10 && h.method != 0x20) return false;
+  if (h.olen > (1 << h.level) || h.olen < 0 || h.clen < 0 || (h.olen == 0 && h.clen != 0) ||
+      (h.olen != 0 && h.clen == 0) || (h.method == 0x10 && h.olen != h.clen))
+    return false;
+  return true;
 }
 
-constexpr int kCopyThreads = 256;
-__global__ void __launch_bounds__(kCopyThreads) lz4_copy_kernel(const BlockDesc* __restrict__ desc, uint32_t b0,
-                                                                uint32_t m, const uint8_t* __restrict__ src_base,
-                                                                uint8_t* dst_base, const uint2* __restrict__ rec,
-                                                                uint32_t rec_stride,
-                                                                const uint32_t* __restrict__ nrec) {
-  constexpr unsigned FULL = 0xffffffffu;
-  const int lane = threadIdx.x & 31;
-  const uint32_t bl = blockIdx.x * (kCopyThreads / 32) + (threadIdx.x >> 5);
-  if (bl >= m) return;
-  const uint32_t b = b0 + bl;
-  const BlockDesc d = desc[b];
-  if (d.olen == 0) return;
-  const uint8_t* __restrict__ in = src_base + d.src;
-  uint8_t* out = dst_base + d.dst;
-  if (d.stream & 0x80000000u) {
-    group_copy<32>(out, in, d.olen, lane);
+// FILL=false: count blocks/bytes per stream.  FILL=true: write descriptors.
+template <bool FILL>
+__global__ void lz4block_walk_kernel(const uint8_t* __restrict__ src_base, const uint64_t* __restrict__ src_off,
+                                     const uint64_t* __restrict__ src_len, uint32_t n, uint64_t* __restrict__ nblk,
+                                     uint64_t* __restrict__ olen_total, const uint64_t* __restrict__ blk_base,
+                                     const uint64_t* __restrict__ dst_off, uint64_t dst_cap,
+                                     int32_t* __restrict__ status, BlockDesc* __restrict__ desc) {
+  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  if (FILL && status[i] != 0 && status[i] != B2S_E_DST_TOO_SMALL) return;
+  if (!FILL && status[i] != 0) {  // failed checksum verification: nothing of this block is decoded
+    nblk[i] = 0;
+    olen_total[i] = 0;
     return;
   }
-  const uint32_t n = nrec[b];
-  const uint2* __restrict__ r = rec + (size_t)bl * rec_stride;
-  int base_op = 0;
-  for (uint32_t i0 = 0; i0 < n; i0 += 32) {
-    const uint32_t i = i0 + lane;
-    uint2 q = make_uint2(0, 0);
-    if (i < n) q = r[i];
-    const int lit = (int)(q.x & 0xffffu), ml = (int)(q.x >> 16);
-    const int off = (int)(q.y & 0xffffu), lip = (int)(q.y >> 16);
-    // output position of every sequence of the batch: exclusive scan of lit + ml
-    int inc = lit + ml;
-#pragma unroll
-    for (int s = 1; s < 32; s <<= 1) {
-      const int t = __shfl_up_sync(FULL, inc, s);
-      if (lane >= s) inc += t;
+  const uint8_t* p = src_base + src_off[i];
+  const uint64_t len = src_len[i];
+  uint64_t ip = 0, cnt = 0, total = 0;
+  bool bad = false;
+  bool too_small = false;
+  if (FILL) too_small = (dst_off[i] + olen_total[i] > dst_cap);
+  while (ip < len) {
+    if (len - ip < 21) {
+      bad = true;
+      break;
     }
-    const int op = base_op + inc - (lit + ml);
-    base_op += __shfl_sync(FULL, inc, 31);
-
-    // ---- literals: independent of everything, all lanes at once; long runs go through the whole warp
-    lz_copy_literals(in, out, lip, lit, op, lane);
-
-    // ---- matches, in dependency rounds (lz_batch.cuh)
-    lz_execute_matches<true>(out, op + lit, ml, off, lane);
+    const Lz4bHeader h = lz4b_read_header(p + ip);
+    if (!lz4b_header_valid(h)) {
+      bad = true;
+      break;
+    }
+    ip += 21;
+    if (h.olen == 0 && h.clen == 0) {
+      if (h.check != 0) {
+        bad = true;
+        break;
+      }
+      continue;  // end mark; stopOnEmptyBlock=false: a concatenated stream may follow
+    }
+    if ((uint64_t)h.clen > len - ip) {
+      bad = true;
+      break;
+    }
+    if (FILL) {
+      BlockDesc d;
+      d.src = src_off[i] + ip;
+      d.dst = dst_off[i] + total;
+      d.clen = too_small ? 0u : (uint32_t)h.clen;
+      d.olen = too_small ? 0u : (uint32_t)h.olen;
+      d.check = h.check;
+      d.stream = i | (h.method == 0x10 ? 0x80000000u : 0u);
+      desc[blk_base[i] + cnt] = d;
+    }
+    cnt++;
+    total += (uint64_t)h.olen;
+    ip += (uint64_t)h.clen;
   }
+  if (!FILL) {
+    if (bad) {
+      status[i] = B2S_E_CORRUPT;
+      cnt = 0;
+      total = 0;
+    }
+    nblk[i] = cnt;
+    olen_total[i] = total;
+  } else if (too_small) {
+    status[i] = B2S_E_DST_TOO_SMALL;
+  }
+}
+
+void launch_lz4block_count(const uint8_t* src_base, const uint64_t* d_src_off, const uint64_t* d_src_len, uint32_t n,
+                           uint64_t* d_nblk, uint64_t* d_olen, int32_t* d_status, cudaStream_t st, uint64_t* launches) {
+  if (!n) return;
+  lz4block_walk_kernel<false><<<(n + 127) / 128, 128, 0, st>>>(src_base, d_src_off, d_src_len, n, d_nblk, d_olen,
+                                                              nullptr, nullptr, 0, d_status, nullptr);
+  *launches += 1;
+}
+
+void launch_lz4block_fill(const uint8_t* src_base, const uint64_t* d_src_off, const uint64_t* d_src_len, uint32_t n,
+                          const uint64_t* d_blk_base, const uint64_t* d_dst_off, uint64_t* d_olen, uint64_t dst_cap,
+                          int32_t* d_status, BlockDesc* d_desc, cudaStream_t st, uint64_t* launches) {
+  if (!n) return;
+  lz4block_walk_kernel<true><<<(n + 127) / 128, 128, 0, st>>>(src_base, d_src_off, d_src_len, n, nullptr, d_olen,
+                                                             d_blk_base, d_dst_off, dst_cap, d_status, d_desc);
+  *launches += 1;
 }
 
 // ---- lz4_decode_warp_kernel: WARP per LZ4 codec block, token parse and copies in one pass, no per-sequence records.
@@ -121,6 +171,7 @@ __device__ __noinline__ bool lz4_token_serial(const uint8_t* __restrict__ in, in
       if (ip >= clen) return false;
       bb = __ldg(in + ip++);
       ll += bb;
+      if (ll > olen) return false;  // cannot be valid, and a long run of 0xFF bytes must not wrap the counter
     } while (bb == 255);
   }
   if (ll > olen - op || ll > clen - ip) return false;
@@ -141,6 +192,7 @@ __device__ __noinline__ bool lz4_token_serial(const uint8_t* __restrict__ in, in
       if (ip >= clen) return false;
       bb = __ldg(in + ip++);
       ml += bb;
+      if (ml > olen) return false;
     } while (bb == 255);
   }
   ml += kMinMatch;
@@ -323,21 +375,6 @@ void launch_lz4_decode_warp(const BlockDesc* d_desc, uint32_t nb, const uint8_t*
   if (grid > want) grid = want;
   lz4_decode_warp_kernel<<<(unsigned)grid, kWarpDecWarps * 32, 0, st>>>(d_desc, nb, src_base, dst_base, d_status,
                                                                          d_counter);
-  *launches += 1;
-}
-
-// records per codec block: a Snappy element takes >= 2 compressed bytes and may produce a single byte
-uint32_t snappy_decode_rec_stride(uint32_t max_clen) { return max_clen / 2 + 2; }
-size_t snappy_decode_ws_bytes(uint32_t chunk_blocks, uint32_t rec_stride) {
-  return (size_t)chunk_blocks * rec_stride * 8 + 256;
-}
-
-void launch_lz4_copy(const BlockDesc* d_desc, uint32_t b0, uint32_t m, uint32_t rec_stride, const uint8_t* src_base,
-                     uint8_t* dst_base, const uint8_t* d_ws, const uint32_t* d_nrec, cudaStream_t st,
-                     uint64_t* launches) {
-  if (!m) return;
-  lz4_copy_kernel<<<(m + kCopyThreads / 32 - 1) / (kCopyThreads / 32), kCopyThreads, 0, st>>>(
-      d_desc, b0, m, src_base, dst_base, reinterpret_cast<const uint2*>(d_ws), rec_stride, d_nrec);
   *launches += 1;
 }
 

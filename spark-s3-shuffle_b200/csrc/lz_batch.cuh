@@ -1,11 +1,12 @@
-// lz_batch.cuh — executes the MATCH copies of a batch of up to 32 LZ sequences, one lane per sequence (device only).
-// Shared by lz4_copy_kernel (LZ4 + Snappy, lz4_decode.cu) and the Zstandard warp decoder (zstd_core.h under
+// lz_batch.cuh — copies the LITERALS and executes the MATCH copies of a batch of up to 32 LZ sequences, one lane per
+// sequence (device only).  The literal copy is shared by the two LZ decoders, lz4_decode_warp_kernel (lz4_decode.cu)
+// and snappy_copy_kernel (snappy.cu); the match copy by those and the Zstandard warp decoder (zstd_core.h under
 // B2S_ZSTD_WARP).
 //
-// Preconditions: the literals of the whole batch are already in place (and made visible with __syncwarp); positions
-// are relative to `out`; lane l's match writes [mdst, mdst+ml) and reads [mdst-off, mdst-off+ml) (ml == 0: no match);
-// mdst is non-decreasing with the lane index and the output intervals are disjoint; everything below the batch's first
-// output byte is final.
+// Match preconditions: the literals of the whole batch are already in place (and made visible with __syncwarp);
+// positions are relative to `out`; lane l's match writes [mdst, mdst+ml) and reads [mdst-off, mdst-off+ml) (ml == 0:
+// no match); mdst is non-decreasing with the lane index and the output intervals are disjoint; everything below the
+// batch's first output byte is final.
 //
 // The matches a lane depends on — those whose output intersects its source [msrc, min(msrc+ml, mdst)) (the part of
 // the source that is its OWN output is produced by the sequential copy itself) — form a contiguous lane range
@@ -15,6 +16,29 @@
 #include "common.cuh"
 
 namespace b2s {
+
+// The literals of a batch of up to 32 sequences (lane l: lit bytes from in + lip to out + op; lit == 0: none): all
+// lanes at once, runs longer than 16 bytes by the whole warp.  Ends with __syncwarp, so the literals are visible to the
+// match copies that follow.
+__device__ __forceinline__ void lz_copy_literals(const uint8_t* __restrict__ in, uint8_t* out, int lip, int lit, int op,
+                                                 int lane) {
+  constexpr unsigned FULL = 0xffffffffu;
+  if (lit > 0 && lit <= 16) {  // aligned 8-byte words of the compressed block (read-only: __ldg)
+    uint64_t lo, hi;
+    ld_span16<true>(in + lip, lit, lo, hi);
+    st_span16(out + op, lit, lo, hi);
+  }
+  unsigned biglit = __ballot_sync(FULL, lit > 16);
+  while (biglit) {
+    const int l = __ffs(biglit) - 1;
+    biglit &= biglit - 1;
+    const int n_l = __shfl_sync(FULL, lit, l), op_l = __shfl_sync(FULL, op, l), ip_l = __shfl_sync(FULL, lip, l);
+    if (n_l >= 96) group_copy<32>(out + op_l, in + ip_l, (uint32_t)n_l, lane);
+    else
+      for (int j = lane; j < n_l; j += 32) out[op_l + j] = __ldg(in + ip_l + j);
+  }
+  __syncwarp();
+}
 
 // (Tried: moving a short match in groups of four bytes — four independent loads, then four stores — when the group's
 // source cannot be its own output: the read pass got slower.  Those were still byte loads; see WIDE below.)

@@ -9,9 +9,11 @@
 //
 // write: lz4_match_kernel (shared, lz4_compress.cu) -> lz4_parse_kernel<SNAPPY> (shared, element sizes differ)
 //        -> snappy_emit_kernel (lane per sequence, Snappy element grammar) ; specification: orc_snappy_compress_raw_win
-// read : xerial_walk_kernel (chunk descriptors) -> snappy_tokens_kernel (thread per chunk: elements -> the same 8-byte
-//        records as LZ4) -> lz4_copy_kernel (shared, lz4_decode.cu)
+// read : xerial_walk_kernel (chunk descriptors) -> snappy_tokens_kernel (thread per chunk: elements -> 8-byte records)
+//        -> snappy_copy_kernel (warp per chunk, lane per record; literal and match copies shared with the LZ4 decoder,
+//        lz_batch.cuh)
 #include "kernels.h"
+#include "lz_batch.cuh"
 
 namespace b2s {
 
@@ -318,7 +320,7 @@ void launch_xerial_fill(const uint8_t* src_base, const uint64_t* d_src_off, cons
 
 // ------------------------------------------------------------------------------------------------------------
 // read side: elements -> records (thread per chunk).  A literal element followed by a copy element becomes one
-// record; the copy kernel (lz4_copy_kernel) does not care which codec produced them.
+// record for the copy kernel (snappy_copy_kernel).
 // record: x = literal count | match length << 16 ; y = offset | literal source position << 16
 // ------------------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(64) snappy_tokens_kernel(const BlockDesc* __restrict__ desc, uint32_t b0, uint32_t m,
@@ -426,6 +428,71 @@ void launch_snappy_tokens(const BlockDesc* d_desc, uint32_t b0, uint32_t m, cons
                           uint64_t* launches) {
   if (!m) return;
   snappy_tokens_kernel<<<(m + 63) / 64, 64, 0, st>>>(d_desc, b0, m, src_base, d_rec, rec_stride, d_nrec, d_status);
+  *launches += 1;
+}
+
+// ------------------------------------------------------------------------------------------------------------
+// read side: records -> bytes.  Warp per codec block, LANE per sequence: output positions by a warp scan, all literals
+// of a batch of 32 sequences at once, then the matches in dependency rounds (lz_batch.cuh).
+// ------------------------------------------------------------------------------------------------------------
+constexpr int kCopyThreads = 256;
+__global__ void __launch_bounds__(kCopyThreads) snappy_copy_kernel(const BlockDesc* __restrict__ desc, uint32_t b0,
+                                                                   uint32_t m, const uint8_t* __restrict__ src_base,
+                                                                   uint8_t* dst_base, const uint2* __restrict__ rec,
+                                                                   uint32_t rec_stride,
+                                                                   const uint32_t* __restrict__ nrec) {
+  constexpr unsigned FULL = 0xffffffffu;
+  const int lane = threadIdx.x & 31;
+  const uint32_t bl = blockIdx.x * (kCopyThreads / 32) + (threadIdx.x >> 5);
+  if (bl >= m) return;
+  const uint32_t b = b0 + bl;
+  const BlockDesc d = desc[b];
+  if (d.olen == 0) return;
+  const uint8_t* __restrict__ in = src_base + d.src;
+  uint8_t* out = dst_base + d.dst;
+  if (d.stream & 0x80000000u) {
+    group_copy<32>(out, in, d.olen, lane);
+    return;
+  }
+  const uint32_t n = nrec[b];
+  const uint2* __restrict__ r = rec + (size_t)bl * rec_stride;
+  int base_op = 0;
+  for (uint32_t i0 = 0; i0 < n; i0 += 32) {
+    const uint32_t i = i0 + lane;
+    uint2 q = make_uint2(0, 0);
+    if (i < n) q = r[i];
+    const int lit = (int)(q.x & 0xffffu), ml = (int)(q.x >> 16);
+    const int off = (int)(q.y & 0xffffu), lip = (int)(q.y >> 16);
+    // output position of every sequence of the batch: exclusive scan of lit + ml
+    int inc = lit + ml;
+#pragma unroll
+    for (int s = 1; s < 32; s <<= 1) {
+      const int t = __shfl_up_sync(FULL, inc, s);
+      if (lane >= s) inc += t;
+    }
+    const int op = base_op + inc - (lit + ml);
+    base_op += __shfl_sync(FULL, inc, 31);
+
+    // ---- literals: independent of everything, all lanes at once; long runs go through the whole warp
+    lz_copy_literals(in, out, lip, lit, op, lane);
+
+    // ---- matches, in dependency rounds (lz_batch.cuh)
+    lz_execute_matches<true>(out, op + lit, ml, off, lane);
+  }
+}
+
+// records per codec block: a Snappy element takes >= 2 compressed bytes and may produce a single byte
+uint32_t snappy_decode_rec_stride(uint32_t max_clen) { return max_clen / 2 + 2; }
+size_t snappy_decode_ws_bytes(uint32_t chunk_blocks, uint32_t rec_stride) {
+  return (size_t)chunk_blocks * rec_stride * 8 + 256;
+}
+
+void launch_snappy_copy(const BlockDesc* d_desc, uint32_t b0, uint32_t m, uint32_t rec_stride, const uint8_t* src_base,
+                        uint8_t* dst_base, const uint8_t* d_ws, const uint32_t* d_nrec, cudaStream_t st,
+                        uint64_t* launches) {
+  if (!m) return;
+  snappy_copy_kernel<<<(m + kCopyThreads / 32 - 1) / (kCopyThreads / 32), kCopyThreads, 0, st>>>(
+      d_desc, b0, m, src_base, dst_base, reinterpret_cast<const uint2*>(d_ws), rec_stride, d_nrec);
   *launches += 1;
 }
 

@@ -1,4 +1,5 @@
-"""The byte movement of the LZ4 / Snappy copy kernel (lz4_copy_kernel + lz_execute_matches), case by case.
+"""The byte movement the LZ4 and Snappy decoders share (lz_copy_literals + lz_execute_matches, lz_batch.cuh, run by
+lz4_decode_warp_kernel and snappy_copy_kernel), case by case.
 
 Short literals and short non-overlapping matches are read as aligned 8-byte words and re-aligned in registers,
 overlapping matches are copied byte by byte, long literals and matches by the whole warp.  The blocks here are

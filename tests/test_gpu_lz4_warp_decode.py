@@ -1,7 +1,7 @@
 """The warp-per-block LZ4 decoder (lz4_decode_warp_kernel): token boundaries found in 128-byte windows, length
-extensions, decoy literal bytes, match forms, every corruption rule, RAW blocks and empty streams.  A batch with a
-codec block over 64 KiB (lz4-java allows up to 32 MiB) goes to the tile decoder (lz4_decompress_kernel) as a whole:
-blocks of 128 KiB to 32 MiB, a batch mixing large and small blocks, and every corruption rule inside a large block.
+extensions, decoy literal bytes, match forms, every corruption rule, RAW blocks and empty streams.  It decodes codec
+blocks of every size lz4-java writes (up to 32 MiB): blocks of 128 KiB to 32 MiB, a batch mixing large and small
+blocks, every corruption rule inside a large block, and length-extension runs long enough to overflow a 32-bit length.
 
 The streams are LZ4Block (lz4-java framing) assembled sequence by sequence, so that token starts, offsets and
 extension bytes land at known window positions.  Every good stream is checked against the oracle's decoder first, then
@@ -231,8 +231,7 @@ def test_match_forms(capi, oracle):
 def test_compressed_blocks_of_every_size(capi, oracle, size):
     """blocks of 13 bytes to 1 MiB from the oracle's compressor and from liblz4"""
     streams, expected = [], []
-    # (random bytes in 64 KiB blocks reach 64 KiB compressed, which would move this batch to the tile decoder)
-    for kind in ("terasort", "text", "runs", "period") + (("random",) if size != 65536 else ()):
+    for kind in ("terasort", "text", "runs", "period", "random"):
         data = corpus(oracle, kind, size * 3 + 7, seed=size)
         streams.append(oracle_stream(oracle, data, size))
         expected.append(data)
@@ -242,8 +241,8 @@ def test_compressed_blocks_of_every_size(capi, oracle, size):
 
 
 def test_largest_blocks_and_mixed_block_sizes(capi, oracle):
-    """one 32 MiB codec block (lz4-java's largest), and a batch in which one stream of 128 KiB blocks sends 32 KiB-block
-    streams to the tile decoder with it"""
+    """one 32 MiB codec block (lz4-java's largest), and a batch in which one stream of 128 KiB blocks sits among
+    streams of 32 KiB blocks"""
     big = corpus(oracle, "terasort", 32 << 20, seed=7)
     check_good(capi, oracle, [liblz4_stream(oracle, big, 32 << 20)], [big])
     data = [corpus(oracle, kind, 300000, seed=8) for kind in ("terasort", "text", "random", "runs")]
@@ -323,9 +322,8 @@ def test_one_corrupt_stream_among_good_ones(capi, oracle, rule):
 
 
 def test_corrupt_large_block_among_good_ones(capi, oracle):
-    """the bad sequence after 27000 good ones, in a block that claims over 128 KiB, so the tile decoder takes the
-    batch: the bad stream alone is CORRUPT (an offset cannot reach past 135000 output bytes, hence no
-    offset_past_output)"""
+    """the bad sequence after 27000 good ones, in a block that claims over 128 KiB: the bad stream alone is CORRUPT
+    (an offset cannot reach past 135000 output bytes, hence no offset_past_output)"""
     data = [corpus(oracle, kind, 100000, seed=9) for kind in ("terasort", "text")]
     good = [liblz4_stream(oracle, data[0], 131072), oracle.lz4block_compress(data[1])]
     for rule in [r for r in RULES if r != "offset_past_output"]:
@@ -339,3 +337,27 @@ def test_corrupt_large_block_among_good_ones(capi, oracle):
             assert outs[0] == data[0] and outs[2] == data[1], (rule, dev)
             end = int(r["dst_off"][2]) + int(r["dst_len"][2])
             assert (dst[end:] == 0xA5).all()
+
+
+@pytest.mark.parametrize("which", ["ll", "ml"])
+def test_length_run_past_olen_among_good_ones(capi, oracle, which):
+    """a codec block claiming 32 MiB whose literal length (first sequence) or match length (second sequence) carries
+    9 MiB of 0xFF extension bytes, enough to wrap a 32-bit length: the bad stream alone is CORRUPT and nothing is
+    written past the arena"""
+    run = b"\xff" * (9 << 20) + b"\x00"
+    lit = bytes(range(64))
+    if which == "ll":
+        payload = b"\xf0" + run + lit
+    else:
+        payload = enc_seq(b"abcdefgh", 1, 4) + bytes([0x0F]) + (1).to_bytes(2, "little") + run + enc_last(lit)
+    bad = frame(oracle, payload, 32 << 20) + END_MARK
+    with pytest.raises(IOError):
+        oracle.lz4block_decompress(bad)
+    data = [corpus(oracle, kind, 100000, seed=10) for kind in ("terasort", "text")]
+    good = [liblz4_stream(oracle, data[0], 131072), oracle.lz4block_compress(data[1])]
+    for dev in (False, True):
+        outs, st, dst, r = decode(capi, [good[0], bad, good[1]], dev)
+        assert st == [0, capi.E_CORRUPT, 0], dev
+        assert outs[0] == data[0] and outs[2] == data[1], dev
+        end = int(r["dst_off"][2]) + int(r["dst_len"][2])
+        assert (dst[end:] == 0xA5).all()

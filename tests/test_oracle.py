@@ -124,6 +124,22 @@ def test_lz4_decoder_enforces_end_of_block_rules(oracle):
     assert oracle.lz4_decompress_block(bytes([0x10, 1, 9, 0]) + bytes(20), 40)[0] is None
 
 
+def test_lz4_decoder_bounds_long_length_runs(oracle):
+    """A literal or match length extended by 9 MiB of 0xFF bytes would pass 2^31: the block is rejected, not decoded
+    with a wrapped length (a codec block claiming 32 MiB, lz4-java's largest)."""
+    run = b"\xff" * (9 << 20) + b"\x00"
+    lit = bytes(range(64))
+    olen = 32 << 20
+    payloads = [b"\xf0" + run + lit,  # literal length of the first sequence
+                bytes([0x40]) + b"abcd" + b"\x01\x00" + bytes([0x0F]) + b"\x01\x00" + run + bytes([0xF0, 49]) + lit]
+    for payload in payloads:
+        assert oracle.lz4_decompress_block(payload, olen)[0] is None
+        frame = (b"LZ4Block" + bytes([0x2F]) + len(payload).to_bytes(4, "little") + olen.to_bytes(4, "little")
+                 + (oracle.xxh32(b"") & 0x0FFFFFFF).to_bytes(4, "little") + payload)
+        with pytest.raises(IOError):
+            oracle.lz4block_decompress(frame + b"LZ4Block" + bytes([0x15]) + bytes(12))
+
+
 def test_lz4block_reader_rejections(oracle):
     data = corpus(oracle, "terasort", 50000, seed=5)
     good = oracle.lz4block_compress(data)
