@@ -1,13 +1,15 @@
 // api.cu — runtime + C ABI of libb200shuffle.so (see include/b200shuffle.h for the contract and the reference
 // interfaces each entry point replaces).
 //
-// Structure: a process-wide context with one Device per selected GPU.  A Device owns NSLOT pipeline slots; a slot is
-// a CUDA stream plus grow-only device buffers (staged source/destination arenas, descriptor "meta" block, codec
-// scratch) and a pinned host block for descriptor traffic.  Host-pointer entry points cut a batch into chunks of
-// ~64 MiB, and run H2D -> kernels -> (size readback) -> D2H per chunk on rotating slots so copies of one chunk
-// overlap kernels of another.  "_dev" entry points run the same kernel sequence on caller-owned device arenas.
+// Structure: a process-wide context with one Device per selected GPU.  A Device runs two lanes (write side, read side),
+// each with up to NSLOT pipeline slots; a slot is a pair of CUDA streams plus grow-only device buffers (staged
+// source/destination arenas, descriptor "meta" block, codec scratch) and a pinned host block for descriptor traffic.
+// Host-pointer entry points cut a batch into chunks of ~256 MiB, and run H2D -> kernels -> (size readback) -> D2H per
+// chunk on rotating slots so copies of one chunk overlap kernels of another.  "_dev" entry points run the same
+// kernel sequence on caller-owned device arenas.
 // There is no CPU fallback anywhere in this file: without a device every compute entry point fails with B2S_E_CUDA.
 #include <algorithm>
+#include <array>
 #include <atomic>
 #include <chrono>
 #include <cstdio>
@@ -15,6 +17,7 @@
 #include <cstring>
 #include <map>
 #include <mutex>
+#include <optional>
 #include <string>
 #include <thread>
 #include <vector>
@@ -247,6 +250,32 @@ struct Slot {
     dom_used++;
     return 0;
   }
+  // the fixed events, created by create() and destroyed by release(); the first kUntimed only order the two streams
+  static constexpr int kUntimed = 5;
+  std::array<cudaEvent_t*, 21> events() {
+    return {&ev_fork, &ev_match[0], &ev_match[1], &ev_free[0], &ev_free[1], &ev_a,    &ev_b,
+            &ev_k0,   &ev_k1,       &ev_t0,       &ev_t1,      &ev_h0,      &ev_h1,   &ev_d0,
+            &ev_d1,   &ev_p0,       &ev_p1,       &ev_f[0],    &ev_f[1],    &ev_f[2], &ev_f[3]};
+  }
+  int create(int prio) {
+    CU(cudaStreamCreateWithPriority(&st, cudaStreamNonBlocking, prio));
+    CU(cudaStreamCreateWithPriority(&st2, cudaStreamNonBlocking, prio));
+    const auto evs = events();
+    for (int k = 0; k < (int)evs.size(); k++)
+      CU(k < kUntimed ? cudaEventCreateWithFlags(evs[k], cudaEventDisableTiming) : cudaEventCreate(evs[k]));
+    return 0;
+  }
+  // frees whatever the slot holds (buffers, events, streams); a slot that was never created holds nothing
+  void release() {
+    for (DevBuf* b : {&meta, &scratch, &desc, &src, &dst, &zmeta, &pws, &parena, &xpieces, &fws}) b->release();
+    hmeta.release();
+    for (cudaEvent_t* e : events())
+      if (*e) cudaEventDestroy(*e);
+    for (cudaEvent_t e : ev_dom) cudaEventDestroy(e);
+    ev_dom.clear();
+    if (st2) cudaStreamDestroy(st2);
+    if (st) cudaStreamDestroy(st);
+  }
 };
 
 // A device runs two independent LANES: write-side calls (compress) take lane 0, read-side calls (decompress,
@@ -279,9 +308,16 @@ int env_int(const char* name, int dflt) {
   return v && *v ? atoi(v) : dflt;
 }
 
-uint32_t block_size_or_default(uint32_t codec, uint32_t bs) {
-  (void)codec;
-  return bs ? bs : 32768u;
+uint32_t block_size_or_default(uint32_t bs) { return bs ? bs : 32768u; }
+
+// B2S_E_CUDA (and the reason) when the process sees no CUDA device; otherwise 0 and, when asked, the device count
+int no_device(int* count_out = nullptr) {
+  int count = 0;
+  const cudaError_t e = cudaGetDeviceCount(&count);
+  if (e != cudaSuccess || count <= 0)
+    return fail(B2S_E_CUDA, "no CUDA device: %s", e != cudaSuccess ? cudaGetErrorString(e) : "device count is 0");
+  if (count_out) *count_out = count;
+  return 0;
 }
 
 // pick the checksum work-item size: enough items to fill the machine, big enough to amortise the combine
@@ -314,16 +350,54 @@ inline uint64_t stream_overhead(uint32_t codec) {
   return codec == B2S_CODEC_SNAPPY_XERIAL ? 16ull : codec == B2S_CODEC_ZSTD ? 9ull : 21ull;  // + zstd: frame header 6 + end block 3
 }
 
-struct CompressJob {
-  uint32_t n = 0, nb = 0, codec = 0;
-  // pinned host mirror
-  uint64_t *h_src_off = nullptr, *h_src_len = nullptr;
-  uint32_t* h_blk_base = nullptr;
-  uint64_t *h_dst_off = nullptr, *h_dst_len = nullptr, *h_cks = nullptr, *h_total = nullptr;
-  int32_t* h_status = nullptr;
+// A compress chunk's descriptor block: the upload region (copied host -> device in one piece), the download region
+// (device -> host in one piece), then, on the device only, the work arrays.  The pinned block and the device "meta"
+// block are both carved by compress_layout, so the two copies move the same arrays.
+struct CompressLayout {
+  uint8_t *up = nullptr, *down = nullptr;
   size_t up_bytes = 0, down_bytes = 0;
-  uint8_t *d_up = nullptr, *d_down = nullptr;
-  uint8_t *h_up = nullptr, *h_down = nullptr;
+  uint64_t *src_off = nullptr, *src_len = nullptr;  // upload
+  uint32_t* blk_base = nullptr;
+  uint64_t *dst_off = nullptr, *dst_len = nullptr, *cks = nullptr, *total = nullptr;  // download
+  int32_t* status = nullptr;
+  uint32_t *csize = nullptr, *hash = nullptr, *nseq = nullptr;  // device only
+  uint64_t *sizes = nullptr, *work_base = nullptr, *ws = nullptr;
+  unsigned int* counter = nullptr;
+};
+// ws_elems < 0: the pinned block, which ends after the download region
+CompressLayout compress_layout(void* base, uint32_t n, uint32_t nb, ptrdiff_t ws_elems) {
+  CompressLayout L;
+  Carver c(base);
+  L.up = (uint8_t*)c.take<uint64_t>(0);
+  L.src_off = c.take<uint64_t>(n);
+  L.src_len = c.take<uint64_t>(n);
+  L.blk_base = c.take<uint32_t>(n + 1);
+  c.off = align_up(c.off, 16);
+  L.up_bytes = c.off;
+  L.down = (uint8_t*)c.take<uint64_t>(0);
+  L.dst_off = c.take<uint64_t>(n);
+  L.dst_len = c.take<uint64_t>(n);
+  L.cks = c.take<uint64_t>(n);
+  L.total = c.take<uint64_t>(2);
+  L.status = c.take<int32_t>(n);
+  c.off = align_up(c.off, 16);
+  L.down_bytes = c.off - L.up_bytes;
+  if (ws_elems < 0) return L;
+  L.csize = c.take<uint32_t>(nb);
+  L.hash = c.take<uint32_t>(nb);
+  L.nseq = c.take<uint32_t>(nb);
+  L.sizes = c.take<uint64_t>((size_t)nb + 1);
+  L.work_base = c.take<uint64_t>((size_t)n + 1);
+  L.ws = c.take<uint64_t>((size_t)ws_elems);
+  L.counter = c.take<unsigned int>(4);
+  return L;
+}
+
+// a compress chunk: h is the pinned block (the host reads dst_off, dst_len, cks, total and status there after ev_a),
+// d the device meta block
+struct CompressJob {
+  uint32_t n = 0, nb = 0;
+  CompressLayout h, d;
 };
 
 // codec and codec block size a compress job accepts
@@ -337,49 +411,6 @@ int check_codec_block(uint32_t codec, uint32_t bs) {
   return 0;
 }
 
-// lays out pinned + device meta for a compress chunk; returns 0 or error
-int compress_prepare(Slot& S, uint32_t codec, uint32_t bs, uint32_t n, const uint64_t* src_len, CompressJob& J) {
-  if (int rc = check_codec_block(codec, bs)) return rc;
-  J.n = n;
-  J.codec = codec;
-  uint64_t nb = 0;
-  for (uint32_t i = 0; i < n; i++) nb += (src_len[i] + bs - 1) / bs;
-  if (nb >= 0x7fffffffull) return fail(B2S_E_ARG, "too many codec blocks in one chunk%s");
-  J.nb = (uint32_t)nb;
-  // pinned: upload [src_off | src_len | blk_base], download [dst_off | dst_len | cks | total | status]
-  size_t up = align_up(n * 8, 16) * 2 + align_up((n + 1) * 4, 16);
-  size_t down = align_up(n * 8, 16) * 3 + 16 + align_up(n * 4, 16);
-  int rc = S.hmeta.ensure(up + down + 64);
-  if (rc) return rc;
-  Carver hc(S.hmeta.p);
-  J.h_up = (uint8_t*)hc.take<uint64_t>(0);
-  J.h_src_off = hc.take<uint64_t>(n);
-  J.h_src_len = hc.take<uint64_t>(n);
-  J.h_blk_base = hc.take<uint32_t>(n + 1);
-  hc.off = align_up(hc.off, 16);
-  J.up_bytes = hc.off;
-  J.h_down = (uint8_t*)hc.take<uint64_t>(0);
-  size_t d0 = hc.off;
-  J.h_dst_off = hc.take<uint64_t>(n);
-  J.h_dst_len = hc.take<uint64_t>(n);
-  J.h_cks = hc.take<uint64_t>(n);
-  J.h_total = hc.take<uint64_t>(2);
-  J.h_status = hc.take<int32_t>(n);
-  hc.off = align_up(hc.off, 16);
-  J.down_bytes = hc.off - d0;
-  return 0;
-}
-
-struct CompressDevMeta {
-  uint64_t *src_off, *src_len;
-  uint32_t* blk_base;
-  uint64_t *dst_off, *dst_len, *cks, *total;
-  int32_t* status;
-  uint32_t *csize, *hash, *nseq;
-  uint64_t *sizes, *work_base, *ws;
-  unsigned int* counter;
-};
-
 // Compression level.  LZ4Block and Snappy have none in the reference either (lz4-java's fast compressor, snappy-java);
 // for Zstandard (spark.io.compression.zstd.level, codec chosen at storage/S3ShuffleReader.scala:57-60) the level sets the
 // match finder's hash-table size: 1 -> 2^11 entries per block (fastest), 2 / unspecified -> 2^12, >= 3 -> 2^13 (more
@@ -389,52 +420,47 @@ int hlog_for_level(uint32_t codec, int32_t level) {
   return level == 1 ? 11 : level == 2 ? 12 : 13;
 }
 
-int compress_enqueue(Context* C, Slot& S, const ChecksumTables& tabs, uint32_t bs, uint32_t alg, CompressJob& J,
-                     const uint8_t* d_src, uint8_t* d_dst, uint64_t dst_cap, CompressDevMeta& M, uint64_t* launches,
-                     int32_t level) {
-  const uint32_t n = J.n, nb = J.nb;
-  const uint32_t chunk = std::min<uint32_t>(nb ? nb : 1, g_lz4_chunk_blocks);
-  size_t ws_elems = std::max(scan_ws_elems(nb + 1), checksum_ws_elems(n)) + 4;
-  size_t need = J.up_bytes + J.down_bytes + align_up((size_t)nb * 4, 16) * 3 + align_up(((size_t)nb + 1) * 8, 16) +
-                align_up(((size_t)n + 1) * 8, 16) + ws_elems * 8 + 256;
-  int rc = S.meta.ensure(need);
+// Enqueues the compression of n streams at d_src + src_off[i] (src_len[i] bytes) into d_dst on S.st.  The results
+// are in J.h once ev_a has completed.
+int compress_chunk(Slot& S, const ChecksumTables& tabs, uint32_t codec, int32_t level, uint32_t bs, uint32_t alg,
+                   uint32_t n, const uint64_t* src_off, const uint64_t* src_len, const uint8_t* d_src, uint8_t* d_dst,
+                   uint64_t dst_cap, CompressJob& J, uint64_t* launches) {
+  if (int rc = check_codec_block(codec, bs)) return rc;
+  uint64_t nb64 = 0;
+  for (uint32_t i = 0; i < n; i++) nb64 += (src_len[i] + bs - 1) / bs;
+  if (nb64 >= 0x7fffffffull) return fail(B2S_E_ARG, "too many codec blocks in one chunk%s");
+  const uint32_t nb = (uint32_t)nb64;
+  J.n = n;
+  J.nb = nb;
+  size_t up = align_up(n * 8, 16) * 2 + align_up((n + 1) * 4, 16);
+  size_t down = align_up(n * 8, 16) * 3 + 16 + align_up(n * 4, 16);
+  int rc = S.hmeta.ensure(up + down + 64);
   if (rc) return rc;
-  const size_t ws_bytes = align_up(lz4_compress_ws_bytes(chunk, bs, J.codec), 256);
-  rc = S.scratch.ensure(ws_bytes * (nb > chunk ? 2 : 1));
-  if (rc) return rc;
-  Carver dc(S.meta.p);
-  J.d_up = (uint8_t*)dc.take<uint64_t>(0);
-  M.src_off = dc.take<uint64_t>(n);
-  M.src_len = dc.take<uint64_t>(n);
-  M.blk_base = dc.take<uint32_t>(n + 1);
-  dc.off = align_up(dc.off, 16);
-  J.d_down = (uint8_t*)dc.take<uint64_t>(0);
-  M.dst_off = dc.take<uint64_t>(n);
-  M.dst_len = dc.take<uint64_t>(n);
-  M.cks = dc.take<uint64_t>(n);
-  M.total = dc.take<uint64_t>(2);
-  M.status = dc.take<int32_t>(n);
-  M.csize = dc.take<uint32_t>(nb);
-  M.hash = dc.take<uint32_t>(nb);
-  M.nseq = dc.take<uint32_t>(nb);
-  M.sizes = dc.take<uint64_t>((size_t)nb + 1);
-  M.work_base = dc.take<uint64_t>((size_t)n + 1);
-  M.ws = dc.take<uint64_t>(ws_elems);
-  M.counter = dc.take<unsigned int>(4);
-
-  // blk_base prefix on the host
+  J.h = compress_layout(S.hmeta.p, n, nb, -1);
+  memcpy(J.h.src_off, src_off, (size_t)n * 8);
+  memcpy(J.h.src_len, src_len, (size_t)n * 8);
   uint64_t acc = 0;
   for (uint32_t i = 0; i < n; i++) {
-    J.h_blk_base[i] = (uint32_t)acc;
-    acc += (J.h_src_len[i] + bs - 1) / bs;
+    J.h.blk_base[i] = (uint32_t)acc;
+    acc += (src_len[i] + bs - 1) / bs;
   }
-  J.h_blk_base[n] = (uint32_t)acc;
+  J.h.blk_base[n] = (uint32_t)acc;
+
+  const uint32_t chunk = std::min<uint32_t>(nb ? nb : 1, g_lz4_chunk_blocks);
+  size_t ws_elems = std::max(scan_ws_elems(nb + 1), checksum_ws_elems(n)) + 4;
+  size_t need = J.h.up_bytes + J.h.down_bytes + align_up((size_t)nb * 4, 16) * 3 + align_up(((size_t)nb + 1) * 8, 16) +
+                align_up(((size_t)n + 1) * 8, 16) + ws_elems * 8 + 256;
+  rc = S.meta.ensure(need);
+  if (rc) return rc;
+  const size_t ws_bytes = align_up(lz4_compress_ws_bytes(chunk, bs, codec), 256);
+  rc = S.scratch.ensure(ws_bytes * (nb > chunk ? 2 : 1));
+  if (rc) return rc;
+  const CompressLayout M = J.d = compress_layout(S.meta.p, n, nb, (ptrdiff_t)ws_elems);
 
   cudaStream_t st = S.st;
-  CU(cudaMemcpyAsync(J.d_up, J.h_up, J.up_bytes, cudaMemcpyHostToDevice, st));
-  CU(cudaMemsetAsync(J.d_down, 0, J.down_bytes, st));
+  CU(cudaMemcpyAsync(M.up, J.h.up, M.up_bytes, cudaMemcpyHostToDevice, st));
+  CU(cudaMemsetAsync(M.down, 0, M.down_bytes, st));
   CU(cudaEventRecord(S.ev_k0, st));
-  const uint32_t codec = J.codec;
   CU(cudaEventRecord(S.ev_t0, st));
   // Chunks of `chunk` codec blocks.  The match kernel (issue bound, shared-memory limited) of chunk k+1 runs on the
   // side stream while parse (latency bound, one thread per block), scan and emit of chunk k run on the main stream;
@@ -476,34 +502,65 @@ int compress_enqueue(Context* C, Slot& S, const ChecksumTables& tabs, uint32_t b
     launch_checksum(tabs, alg, d_dst, M.dst_off, M.dst_len, n, shift, M.work_base, M.ws, M.cks, st, launches);
   }
   CU(cudaEventRecord(S.ev_k1, st));
-  CU(cudaMemcpyAsync(J.h_down, J.d_down, J.down_bytes, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(J.h.down, M.down, M.down_bytes, cudaMemcpyDeviceToHost, st));
   CU(cudaEventRecord(S.ev_a, st));
   CU(cudaGetLastError());
-  (void)C;
   return 0;
 }
 
 // --------------------------------------------------------------------------------------------------------------
 // decompress job
 // --------------------------------------------------------------------------------------------------------------
+// A decompress chunk's descriptor block, carved like a compress chunk's (compress_layout): upload region, download
+// region, device-only work arrays.  dst_len is the decoded length of every stream.
+struct DecompressLayout {
+  uint8_t *up = nullptr, *down = nullptr;
+  size_t up_bytes = 0, down_bytes = 0;
+  uint64_t *src_off = nullptr, *src_len = nullptr, *slice_off = nullptr, *slice_len = nullptr, *slice_sum = nullptr;
+  uint32_t *slice_owner = nullptr, *slice_base = nullptr;  // upload
+  uint64_t* totals = nullptr;  // download: [nb_total, olen_total, Snappy: largest chunk olen, clen]
+  uint64_t *dst_off = nullptr, *dst_len = nullptr;
+  int32_t *status = nullptr, *bad = nullptr;
+  uint64_t *nblk = nullptr, *cks_got = nullptr, *work_base = nullptr, *ws = nullptr;  // device only
+  unsigned int* counter = nullptr;
+};
+// ws_elems < 0: the pinned block, which ends after the download region
+DecompressLayout decompress_layout(void* base, uint32_t n, uint32_t s, ptrdiff_t ws_elems) {
+  DecompressLayout L;
+  Carver c(base);
+  L.up = (uint8_t*)c.take<uint64_t>(0);
+  L.src_off = c.take<uint64_t>(n);
+  L.src_len = c.take<uint64_t>(n);
+  L.slice_off = c.take<uint64_t>(s);
+  L.slice_len = c.take<uint64_t>(s);
+  L.slice_sum = c.take<uint64_t>(s);
+  L.slice_owner = c.take<uint32_t>(s);
+  L.slice_base = c.take<uint32_t>((size_t)n + 1);
+  c.off = align_up(c.off, 16);
+  L.up_bytes = c.off;
+  L.down = (uint8_t*)c.take<uint64_t>(0);
+  L.totals = c.take<uint64_t>(4);
+  L.dst_off = c.take<uint64_t>(n);
+  L.dst_len = c.take<uint64_t>(n);
+  L.status = c.take<int32_t>(n);
+  L.bad = c.take<int32_t>(n);
+  c.off = align_up(c.off, 16);
+  L.down_bytes = c.off - L.up_bytes;
+  if (ws_elems < 0) return L;
+  L.nblk = c.take<uint64_t>(n);
+  L.cks_got = c.take<uint64_t>(s);
+  L.work_base = c.take<uint64_t>((size_t)s + 1);
+  L.ws = c.take<uint64_t>((size_t)ws_elems);
+  L.counter = c.take<unsigned int>(4);
+  return L;
+}
+
+// a decompress chunk: h is the pinned block (the host reads totals after ev_a, the rest after ev_b), d the device
+// meta block
 struct DecompressJob {
   uint32_t n = 0, n_slices = 0, codec = 0;
   uint64_t nb = 0, total_out = 0;
-  uint64_t *h_src_off = nullptr, *h_src_len = nullptr;
-  uint64_t *h_slice_off = nullptr, *h_slice_len = nullptr, *h_slice_sum = nullptr;
-  uint32_t *h_slice_owner = nullptr, *h_slice_base = nullptr;
-  uint64_t* h_totals = nullptr;  // [nb_total, olen_total, Snappy: largest chunk olen, clen]
-  uint64_t *h_dst_off = nullptr, *h_dst_len = nullptr;
-  int32_t *h_status = nullptr, *h_bad = nullptr;
-  size_t up_bytes = 0, down_bytes = 0;
-  uint8_t *h_up = nullptr, *h_down = nullptr, *d_up = nullptr, *d_down = nullptr;
-  // device
-  uint64_t *src_off = nullptr, *src_len = nullptr, *slice_off = nullptr, *slice_len = nullptr, *slice_sum = nullptr;
-  uint32_t *slice_owner = nullptr, *slice_base = nullptr;
-  uint64_t *nblk = nullptr, *olen = nullptr, *dst_off = nullptr, *totals = nullptr, *cks_got = nullptr,
-           *work_base = nullptr, *ws = nullptr;
-  int32_t *status = nullptr, *bad = nullptr;
-  unsigned int* counter = nullptr;
+  DecompressLayout h, d;
   // zstd: per-stream counts / bases (blocks, sequences, literal bytes) and their totals
   uint64_t *zcnt = nullptr, *zbase = nullptr;
   uint64_t znb = 0, znseq = 0, zlit = 0;
@@ -512,11 +569,21 @@ struct DecompressJob {
 
 // allow_none: codec NONE verifies the slices only and reports the stored lengths as decoded lengths in phase A (the
 // key sort of uncompressed blocks); phase B is not run for it
-int decompress_prepare(Slot& S, uint32_t codec, uint32_t alg, uint32_t n, uint32_t n_slices, DecompressJob& J,
-                       bool allow_none = false) {
+int check_decode_codec(uint32_t codec, bool allow_none) {
   if (codec != B2S_CODEC_LZ4BLOCK && codec != B2S_CODEC_SNAPPY_XERIAL && codec != B2S_CODEC_ZSTD &&
       !(allow_none && codec == B2S_CODEC_NONE))
     return fail(B2S_E_UNSUPPORTED, "codec %s not supported by this build", "");
+  return 0;
+}
+
+// Phase A of decoding n streams at d_src + src_off[i] (src_len[i] bytes; src_bytes in all), enqueued on S.st: checksum
+// verify of their n_slices slices (slice_base[0..n], indices into slice_len / slice_sum), header count, scans, and
+// the readback of J.h.totals, there once ev_a has completed.
+int decompress_phase_a(Slot& S, const ChecksumTables& tabs, uint32_t codec, uint32_t alg, uint32_t n,
+                       const uint64_t* src_off, const uint64_t* src_len, uint32_t n_slices, const uint32_t* slice_base,
+                       const uint64_t* slice_len, const uint64_t* slice_sum, const uint8_t* d_src, uint64_t src_bytes,
+                       DecompressJob& J, uint64_t* launches, bool allow_none = false) {
+  if (int rc = check_decode_codec(codec, allow_none)) return rc;
   J.n = n;
   J.codec = codec;
   J.n_slices = alg ? n_slices : 0;
@@ -526,71 +593,42 @@ int decompress_prepare(Slot& S, uint32_t codec, uint32_t alg, uint32_t n, uint32
   size_t down = 32 + align_up(n * 8, 16) * 2 + align_up(n * 4, 16) * 2;
   int rc = S.hmeta.ensure(up + down + 128);
   if (rc) return rc;
-  Carver hc(S.hmeta.p);
-  J.h_up = (uint8_t*)hc.take<uint64_t>(0);
-  J.h_src_off = hc.take<uint64_t>(n);
-  J.h_src_len = hc.take<uint64_t>(n);
-  J.h_slice_off = hc.take<uint64_t>(s);
-  J.h_slice_len = hc.take<uint64_t>(s);
-  J.h_slice_sum = hc.take<uint64_t>(s);
-  J.h_slice_owner = hc.take<uint32_t>(s);
-  J.h_slice_base = hc.take<uint32_t>((size_t)n + 1);
-  hc.off = align_up(hc.off, 16);
-  J.up_bytes = hc.off;
-  J.h_down = (uint8_t*)hc.take<uint64_t>(0);
-  size_t d0 = hc.off;
-  J.h_totals = hc.take<uint64_t>(4);
-  J.h_dst_off = hc.take<uint64_t>(n);
-  J.h_dst_len = hc.take<uint64_t>(n);
-  J.h_status = hc.take<int32_t>(n);
-  J.h_bad = hc.take<int32_t>(n);
-  hc.off = align_up(hc.off, 16);
-  J.down_bytes = hc.off - d0;
-  return 0;
-}
+  const DecompressLayout H = J.h = decompress_layout(S.hmeta.p, n, s, -1);
+  memcpy(H.src_off, src_off, (size_t)n * 8);
+  memcpy(H.src_len, src_len, (size_t)n * 8);
+  uint32_t q0 = 0;  // the slices of stream k are checked where the stream sits on the device
+  for (uint32_t k = 0; k < n; k++) {
+    H.slice_base[k] = q0;
+    if (!s) continue;
+    uint64_t o = src_off[k];
+    for (uint32_t q = slice_base[k]; q < slice_base[k + 1]; q++, q0++) {
+      H.slice_off[q0] = o;
+      H.slice_len[q0] = slice_len[q];
+      H.slice_sum[q0] = slice_sum[q];
+      H.slice_owner[q0] = k;
+      o += slice_len[q];
+    }
+  }
+  H.slice_base[n] = q0;
 
-// phase A: checksum verify + header count + scans + totals readback
-int decompress_enqueue_a(Slot& S, const ChecksumTables& tabs, uint32_t alg, DecompressJob& J, const uint8_t* d_src,
-                         uint64_t src_bytes, uint64_t* launches) {
-  const uint32_t n = J.n, s = J.n_slices;
   size_t ws_elems = std::max(scan_ws_elems((size_t)n + 1), checksum_ws_elems(s)) + 4;
-  size_t need = J.up_bytes + J.down_bytes + align_up((size_t)n * 8, 16) * 1 + align_up((size_t)s * 8, 16) +
+  size_t need = H.up_bytes + H.down_bytes + align_up((size_t)n * 8, 16) * 1 + align_up((size_t)s * 8, 16) +
                 align_up(((size_t)s + 1) * 8, 16) + ws_elems * 8 + 256;
-  int rc = S.meta.ensure(need);
+  rc = S.meta.ensure(need);
   if (rc) return rc;
-  Carver dc(S.meta.p);
-  J.d_up = (uint8_t*)dc.take<uint64_t>(0);
-  J.src_off = dc.take<uint64_t>(n);
-  J.src_len = dc.take<uint64_t>(n);
-  J.slice_off = dc.take<uint64_t>(s);
-  J.slice_len = dc.take<uint64_t>(s);
-  J.slice_sum = dc.take<uint64_t>(s);
-  J.slice_owner = dc.take<uint32_t>(s);
-  J.slice_base = dc.take<uint32_t>((size_t)n + 1);
-  dc.off = align_up(dc.off, 16);
-  J.d_down = (uint8_t*)dc.take<uint64_t>(0);
-  J.totals = dc.take<uint64_t>(4);
-  J.dst_off = dc.take<uint64_t>(n);
-  J.olen = dc.take<uint64_t>(n);
-  J.status = dc.take<int32_t>(n);
-  J.bad = dc.take<int32_t>(n);
-  J.nblk = dc.take<uint64_t>(n);
-  J.cks_got = dc.take<uint64_t>(s);
-  J.work_base = dc.take<uint64_t>((size_t)s + 1);
-  J.ws = dc.take<uint64_t>(ws_elems);
-  J.counter = dc.take<unsigned int>(4);
+  const DecompressLayout M = J.d = decompress_layout(S.meta.p, n, s, (ptrdiff_t)ws_elems);
 
   cudaStream_t st = S.st;
-  CU(cudaMemcpyAsync(J.d_up, J.h_up, J.up_bytes, cudaMemcpyHostToDevice, st));
-  CU(cudaMemsetAsync(J.d_down, 0, J.down_bytes, st));
-  CU(cudaMemsetAsync(J.bad, 0xff, (size_t)n * 4, st));
+  CU(cudaMemcpyAsync(M.up, H.up, M.up_bytes, cudaMemcpyHostToDevice, st));
+  CU(cudaMemsetAsync(M.down, 0, M.down_bytes, st));
+  CU(cudaMemsetAsync(M.bad, 0xff, (size_t)n * 4, st));
   CU(cudaEventRecord(S.ev_k0, st));
   if (alg != B2S_CHECKSUM_NONE && s) {
-    launch_checksum(tabs, alg, d_src, J.slice_off, J.slice_len, s, pick_tile_shift(src_bytes), J.work_base, J.ws,
-                    J.cks_got, st, launches);
-    launch_checksum_compare(J.cks_got, J.slice_sum, J.slice_owner, J.slice_base, s, J.status, J.bad, st, launches);
+    launch_checksum(tabs, alg, d_src, M.slice_off, M.slice_len, s, pick_tile_shift(src_bytes), M.work_base, M.ws,
+                    M.cks_got, st, launches);
+    launch_checksum_compare(M.cks_got, M.slice_sum, M.slice_owner, M.slice_base, s, M.status, M.bad, st, launches);
   }
-  if (J.codec == B2S_CODEC_ZSTD) {
+  if (codec == B2S_CODEC_ZSTD) {
     // walk (count) -> totals to the host -> walk (fill) -> entropy decode of every block in parallel -> stream sizes.
     // The one blocking readback sizes the descriptor array and the literal / sequence workspace (zstd_par.h).
     rc = S.zmeta.ensure(((size_t)n * 6 + 8) * 8);
@@ -598,9 +636,9 @@ int decompress_enqueue_a(Slot& S, const ChecksumTables& tabs, uint32_t alg, Deco
     J.zcnt = (uint64_t*)S.zmeta.p;
     J.zbase = J.zcnt + (size_t)n * 3;
     uint64_t* ztot = J.zbase + (size_t)n * 3;
-    launch_zstd_count(d_src, J.src_off, J.src_len, n, J.zcnt, J.status, st, launches);
+    launch_zstd_count(d_src, M.src_off, M.src_len, n, J.zcnt, M.status, st, launches);
     CU(cudaMemcpyAsync(J.zbase, J.zcnt, (size_t)n * 24, cudaMemcpyDeviceToDevice, st));
-    for (int k = 0; k < 3; k++) launch_exclusive_scan_u64(J.zbase + (size_t)n * k, n, ztot + k, J.ws, st, launches);
+    for (int k = 0; k < 3; k++) launch_exclusive_scan_u64(J.zbase + (size_t)n * k, n, ztot + k, M.ws, st, launches);
     uint64_t h[3] = {0, 0, 0};
     CU(cudaMemcpyAsync(h, ztot, 24, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
@@ -614,23 +652,23 @@ int decompress_enqueue_a(Slot& S, const ChecksumTables& tabs, uint32_t alg, Deco
       rc = S.scratch.ensure(zstd_ws_bytes(J.zlit, J.znseq));
       if (rc) return rc;
     }
-    launch_zstd_fill(d_src, J.src_off, J.src_len, n, J.zcnt, J.zbase, S.desc.p, J.status, st, launches);
-    launch_zstd_entropy(J.size_only, d_src, S.desc.p, J.znb, (uint8_t*)S.scratch.p, J.zlit, J.znseq, J.status, st,
+    launch_zstd_fill(d_src, M.src_off, M.src_len, n, J.zcnt, J.zbase, S.desc.p, M.status, st, launches);
+    launch_zstd_entropy(J.size_only, d_src, S.desc.p, J.znb, (uint8_t*)S.scratch.p, J.zlit, J.znseq, M.status, st,
                         launches);
-    launch_zstd_sum(S.desc.p, J.zcnt, J.zbase, n, J.olen, J.status, st, launches);
-    CU(cudaMemsetAsync(J.nblk, 0, (size_t)n * 8, st));
-  } else if (J.codec == B2S_CODEC_SNAPPY_XERIAL)
-    launch_xerial_count(d_src, J.src_off, J.src_len, n, J.nblk, J.olen, J.totals + 2, J.status, st, launches);
-  else if (J.codec == B2S_CODEC_NONE) {  // stored bytes: decoded length = block length, no codec blocks
-    CU(cudaMemcpyAsync(J.olen, J.src_len, (size_t)n * 8, cudaMemcpyDeviceToDevice, st));
-    CU(cudaMemsetAsync(J.nblk, 0, (size_t)n * 8, st));
+    launch_zstd_sum(S.desc.p, J.zcnt, J.zbase, n, M.dst_len, M.status, st, launches);
+    CU(cudaMemsetAsync(M.nblk, 0, (size_t)n * 8, st));
+  } else if (codec == B2S_CODEC_SNAPPY_XERIAL)
+    launch_xerial_count(d_src, M.src_off, M.src_len, n, M.nblk, M.dst_len, M.totals + 2, M.status, st, launches);
+  else if (codec == B2S_CODEC_NONE) {  // stored bytes: decoded length = block length, no codec blocks
+    CU(cudaMemcpyAsync(M.dst_len, M.src_len, (size_t)n * 8, cudaMemcpyDeviceToDevice, st));
+    CU(cudaMemsetAsync(M.nblk, 0, (size_t)n * 8, st));
   } else
-    launch_lz4block_count(d_src, J.src_off, J.src_len, n, J.nblk, J.olen, J.status, st, launches);
-  // dst_off = exclusive scan(olen) ; blk_base = exclusive scan(nblk) (in place)
-  CU(cudaMemcpyAsync(J.dst_off, J.olen, (size_t)n * 8, cudaMemcpyDeviceToDevice, st));
-  launch_exclusive_scan_u64(J.dst_off, n, J.totals + 1, J.ws, st, launches);
-  launch_exclusive_scan_u64(J.nblk, n, J.totals + 0, J.ws, st, launches);
-  CU(cudaMemcpyAsync(J.h_totals, J.totals, 32, cudaMemcpyDeviceToHost, st));
+    launch_lz4block_count(d_src, M.src_off, M.src_len, n, M.nblk, M.dst_len, M.status, st, launches);
+  // dst_off = exclusive scan(dst_len) ; blk_base = exclusive scan(nblk) (in place)
+  CU(cudaMemcpyAsync(M.dst_off, M.dst_len, (size_t)n * 8, cudaMemcpyDeviceToDevice, st));
+  launch_exclusive_scan_u64(M.dst_off, n, M.totals + 1, M.ws, st, launches);
+  launch_exclusive_scan_u64(M.nblk, n, M.totals + 0, M.ws, st, launches);
+  CU(cudaMemcpyAsync(H.totals, M.totals, 32, cudaMemcpyDeviceToHost, st));
   CU(cudaEventRecord(S.ev_a, st));
   CU(cudaGetLastError());
   return 0;
@@ -639,16 +677,16 @@ int decompress_enqueue_a(Slot& S, const ChecksumTables& tabs, uint32_t alg, Deco
 // phase B (after ev_a): descriptors, decode, XXH32 verify, meta readback
 int decompress_enqueue_b(Slot& S, DecompressJob& J, const uint8_t* d_src, uint8_t* d_dst, uint64_t dst_cap,
                          uint64_t* launches) {
-  J.nb = J.h_totals[0];
-  J.total_out = J.h_totals[1];
+  J.nb = J.h.totals[0];
+  J.total_out = J.h.totals[1];
   if (J.codec == B2S_CODEC_ZSTD) {
     cudaStream_t zst = S.st;
     CU(cudaEventRecord(S.ev_t0, zst));
-    launch_zstd_execute(d_src, S.desc.p, J.zcnt, J.zbase, J.n, (const uint8_t*)S.scratch.p, J.zlit, J.znseq, J.olen,
-                        d_dst, J.dst_off, dst_cap, J.status, zst, launches);
+    launch_zstd_execute(d_src, S.desc.p, J.zcnt, J.zbase, J.n, (const uint8_t*)S.scratch.p, J.zlit, J.znseq, J.d.dst_len,
+                        d_dst, J.d.dst_off, dst_cap, J.d.status, zst, launches);
     CU(cudaEventRecord(S.ev_t1, zst));
     CU(cudaEventRecord(S.ev_k1, zst));
-    CU(cudaMemcpyAsync(J.h_down, J.d_down, J.down_bytes, cudaMemcpyDeviceToHost, zst));
+    CU(cudaMemcpyAsync(J.h.down, J.d.down, J.d.down_bytes, cudaMemcpyDeviceToHost, zst));
     CU(cudaEventRecord(S.ev_b, zst));
     CU(cudaGetLastError());
     return 0;
@@ -660,10 +698,10 @@ int decompress_enqueue_b(Slot& S, DecompressJob& J, const uint8_t* d_src, uint8_
   BlockDesc* desc = (BlockDesc*)S.desc.p;
   CU(cudaMemsetAsync(desc, 0, (size_t)J.nb * sizeof(BlockDesc), st));
   if (J.codec == B2S_CODEC_SNAPPY_XERIAL)
-    launch_xerial_fill(d_src, J.src_off, J.src_len, J.n, J.nblk, J.dst_off, J.olen, dst_cap, J.status, desc, st,
+    launch_xerial_fill(d_src, J.d.src_off, J.d.src_len, J.n, J.d.nblk, J.d.dst_off, J.d.dst_len, dst_cap, J.d.status, desc, st,
                        launches);
   else
-    launch_lz4block_fill(d_src, J.src_off, J.src_len, J.n, J.nblk, J.dst_off, J.olen, dst_cap, J.status, desc, st,
+    launch_lz4block_fill(d_src, J.d.src_off, J.d.src_len, J.n, J.d.nblk, J.d.dst_off, J.d.dst_len, dst_cap, J.d.status, desc, st,
                          launches);
   CU(cudaEventRecord(S.ev_t0, st));
   if (J.nb && J.codec == B2S_CODEC_LZ4BLOCK) {
@@ -671,10 +709,10 @@ int decompress_enqueue_b(Slot& S, DecompressJob& J, const uint8_t* d_src, uint8_
     cudaEvent_t e0 = nullptr, e1 = nullptr;
     S.dom_pair(&e0, &e1);
     CU(cudaEventRecord(e0, st));
-    launch_lz4_decode_warp(desc, (uint32_t)J.nb, d_src, d_dst, J.status, J.counter, st, launches);
+    launch_lz4_decode_warp(desc, (uint32_t)J.nb, d_src, d_dst, J.d.status, J.d.counter, st, launches);
     CU(cudaEventRecord(e1, st));
   } else if (J.nb && J.codec == B2S_CODEC_SNAPPY_XERIAL) {
-    const uint64_t max_olen = J.h_totals[2], max_clen = J.h_totals[3];
+    const uint64_t max_olen = J.h.totals[2], max_clen = J.h.totals[3];
     if (max_olen > 65536 || max_clen >= 65536)
       return fail(B2S_E_UNSUPPORTED, "snappy chunks larger than 64 KiB are not supported%s");
     // tokens (thread per block) + copy (lane per sequence), in chunks that bound the record workspace
@@ -695,7 +733,7 @@ int decompress_enqueue_b(Slot& S, DecompressJob& J, const uint8_t* d_src, uint8_
       const int par = (int)(k & 1);
       uint8_t* ws = (uint8_t*)S.scratch.p + nrec_bytes + (size_t)par * ws_bytes;
       if (k >= 2) CU(cudaStreamWaitEvent(S.st2, S.ev_free[par], 0));
-      launch_snappy_tokens(desc, b0, m, d_src, reinterpret_cast<uint2*>(ws), rec_stride, nrec, J.status, S.st2,
+      launch_snappy_tokens(desc, b0, m, d_src, reinterpret_cast<uint2*>(ws), rec_stride, nrec, J.d.status, S.st2,
                            launches);
       CU(cudaEventRecord(S.ev_match[par], S.st2));
       CU(cudaStreamWaitEvent(st, S.ev_match[par], 0));
@@ -712,9 +750,9 @@ int decompress_enqueue_b(Slot& S, DecompressJob& J, const uint8_t* d_src, uint8_
   // the next chunk's copy kernel) was measured slower: both kernels are
   // memory-latency bound and take each other's L2 / DRAM queue slots.
   if (J.codec == B2S_CODEC_LZ4BLOCK)
-    launch_xxh32_verify(desc, (uint32_t)J.nb, d_dst, kXxhSeed, 0x0FFFFFFFu, J.status, st, launches);
+    launch_xxh32_verify(desc, (uint32_t)J.nb, d_dst, kXxhSeed, 0x0FFFFFFFu, J.d.status, st, launches);
   CU(cudaEventRecord(S.ev_k1, st));
-  CU(cudaMemcpyAsync(J.h_down, J.d_down, J.down_bytes, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(J.h.down, J.d.down, J.d.down_bytes, cudaMemcpyDeviceToHost, st));
   CU(cudaEventRecord(S.ev_b, st));
   CU(cudaGetLastError());
   return 0;
@@ -738,6 +776,30 @@ void add_timing(Slot& S, bool copies) {
   }
   S.dom_used = 0;
   if (copies) t_timing.h2d_ms += ms_between(S.ev_h0, S.ev_h1);  // d2h is added once the payload copy has run
+}
+
+// what a call moved: bytes into and out of its kernels, and over PCIe
+struct CallBytes {
+  uint64_t src = 0, dst = 0, h2d = 0, d2h = 0;
+};
+constexpr int kH2D = 1, kD2H = 2;
+
+// Ends a successful call's b2s_last_timing: its bytes, its launches (also counted for the process) and its wall time.
+// S: the one slot the call ran on, whose kernel events are read, and its copy events where the call recorded them
+// (copies: kH2D | kD2H); nullptr for a call pipelined over slots, whose chunks added their own times (add_timing).
+void end_timing(const WallTimer& wt, uint64_t launches, const CallBytes& b, Slot* S = nullptr, int copies = 0) {
+  if (S) {
+    add_timing(*S, false);
+    if (copies & kH2D) t_timing.h2d_ms = ms_between(S->ev_h0, S->ev_h1);
+    if (copies & kD2H) t_timing.d2h_ms = ms_between(S->ev_d0, S->ev_d1);
+  }
+  t_timing.src_bytes += b.src;
+  t_timing.dst_bytes += b.dst;
+  t_timing.h2d_bytes += b.h2d;
+  t_timing.d2h_bytes += b.d2h;
+  t_timing.kernel_launches = launches;
+  g_ctx->launches += launches;
+  t_timing.total_ms = wt.ms();
 }
 
 // groups streams [i0, i1) into chunks of ~g_host_chunk_bytes
@@ -784,6 +846,53 @@ uint64_t plan_runs(uint32_t cnt, const uint8_t* const* ptr, const uint64_t* len,
     cur = dev_off[i] + len[i];
   }
   return cur;
+}
+
+// Stages the cnt sources of a chunk in S.src: dev_off[i] receives where source i sits, the return value the arena's
+// bytes (what the chunk uploads).  The copies run between ev_h0 and ev_h1.
+int upload_chunk(Slot& S, uint32_t cnt, const uint8_t* const* ptr, const uint64_t* len, uint64_t* dev_off,
+                 std::vector<Run>& runs, uint64_t* bytes) {
+  *bytes = plan_runs(cnt, ptr, len, dev_off, runs);
+  if (int rc = S.src.ensure(*bytes + 64)) return rc;
+  CU(cudaEventRecord(S.ev_h0, S.st));
+  for (const Run& r : runs)
+    CU(cudaMemcpyAsync((uint8_t*)S.src.p + r.dev_off, r.host, r.bytes, cudaMemcpyHostToDevice, S.st));
+  CU(cudaEventRecord(S.ev_h1, S.st));
+  return 0;
+}
+
+// Copies a finished chunk of n streams (stream k: len[k] bytes at off[k] of S.dst, chunk_total bytes in all) to the
+// host between ev_d0 and ev_d1, and adds what it copied to d2h_bytes.  packed_dst: the whole chunk at run_off of that
+// arena, as much of it as fits in packed_cap, and every stream still OK that does not fit entirely gets
+// B2S_E_DST_TOO_SMALL.  dst: stream k of an OK status to dst[k], or B2S_E_DST_TOO_SMALL when it exceeds dst_cap[k].
+// Neither: nothing is copied.
+int download_chunk(Slot& S, uint32_t n, const uint64_t* off, const uint64_t* len, uint64_t chunk_total,
+                   uint8_t* packed_dst, uint64_t packed_cap, uint64_t run_off, uint8_t* const* dst,
+                   const uint64_t* dst_cap, int32_t* status) {
+  CU(cudaEventRecord(S.ev_d0, S.st));
+  if (packed_dst) {
+    uint64_t fit = chunk_total;
+    if (run_off + chunk_total > packed_cap) {
+      fit = packed_cap > run_off ? packed_cap - run_off : 0;
+      for (uint32_t k = 0; k < n; k++)
+        if (status[k] == B2S_OK && run_off + off[k] + len[k] > packed_cap) status[k] = B2S_E_DST_TOO_SMALL;
+    }
+    // what fits is copied, so that the streams in front of the first one that does not stay valid
+    if (fit) CU(cudaMemcpyAsync(packed_dst + run_off, S.dst.p, fit, cudaMemcpyDeviceToHost, S.st));
+    t_timing.d2h_bytes += fit;
+  } else if (dst) {
+    for (uint32_t k = 0; k < n; k++) {
+      if (status[k] != B2S_OK || len[k] == 0) continue;
+      if (len[k] > dst_cap[k]) {
+        status[k] = B2S_E_DST_TOO_SMALL;
+        continue;
+      }
+      CU(cudaMemcpyAsync(dst[k], (uint8_t*)S.dst.p + off[k], len[k], cudaMemcpyDeviceToHost, S.st));
+      t_timing.d2h_bytes += len[k];
+    }
+  }
+  CU(cudaEventRecord(S.ev_d1, S.st));
+  return 0;
 }
 
 
@@ -1009,10 +1118,7 @@ int ex_store(int ordinal, cudaStream_t st, int32_t shuffle, int64_t map, const u
 // without a usable device the exchange calls report B2S_E_CUDA (b2s_init has failed for that reason)
 int exchange_ready() {
   if (g_ctx) return 0;
-  int count = 0;
-  const cudaError_t e = cudaGetDeviceCount(&count);
-  if (e != cudaSuccess || count <= 0)
-    return fail(B2S_E_CUDA, "no CUDA device: %s", e != cudaSuccess ? cudaGetErrorString(e) : "device count is 0");
+  if (int rc = no_device()) return rc;
   return fail(B2S_E_NOT_INIT, "b2s_init has not been called%s");
 }
 
@@ -1020,6 +1126,55 @@ int reduce_range_args(int32_t start_reduce, int32_t end_reduce) {
   if (start_reduce < 0 || end_reduce < start_reduce || end_reduce > (1 << 24))
     return fail(B2S_E_ARG, "reduce range must satisfy 0 <= start_reduce <= end_reduce <= 2^24%s");
   return 0;
+}
+
+// creates the streams, events and tables of CUDA device d for D (b2s_init); on failure destroy_device frees what it made
+int create_device(Device& D, int d, uint64_t pinned_bytes_per_gpu) {
+  D.ordinal = d;
+  CU(cudaSetDevice(d));
+  char busid[32] = {0};
+  if (g_numa && cudaDeviceGetPCIBusId(busid, sizeof busid, d) == cudaSuccess) D.numa_node = numa::node_of_pci(busid);
+  (void)cudaGetLastError();
+  t_numa_node = D.numa_node;
+  for (int l = 0; l < kLanes; l++)
+    for (int k = 0; k < g_nslot; k++) {
+      Slot& S = D.lane[l].slot[k];
+      // the read lane's kernels are short and latency bound (token walks, per-stream header walks, two host round
+      // trips per chunk): they get the higher stream priority so they are not queued behind the write lane's grids
+      int prio_lo = 0, prio_hi = 0;
+      cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi);
+      if (int rc = S.create(l == kLaneRead ? prio_hi : prio_lo)) return rc;
+      // pinned_bytes_per_gpu: the library's own pinned descriptor blocks are sized up front (split over the slots)
+      // instead of growing on first use; 0 = grow on demand.  Payload staging is the caller's (b2s_host_alloc).
+      if (pinned_bytes_per_gpu) {
+        const uint64_t per = std::min<uint64_t>(pinned_bytes_per_gpu / (uint64_t)(kLanes * g_nslot), 64ull << 20);
+        if (per >= 4096 && S.hmeta.ensure(per)) return B2S_E_NOMEM;
+      }
+    }
+  if (checksum_tables_create(&D.tabs)) return fail(B2S_E_CUDA, "checksum table upload failed%s");
+  if (zstd_ctables_create(&D.zstd_ctables)) return fail(B2S_E_CUDA, "zstd table upload failed%s");
+  zstd_set_ctables(d, D.zstd_ctables);
+  CU(cudaEventCreate(&D.ev_mark[0]));
+  CU(cudaEventCreate(&D.ev_mark[1]));
+  return 0;
+}
+
+void destroy_device(Device* D) {
+  cudaSetDevice(D->ordinal);
+  cudaDeviceSynchronize();
+  for (Lane& Ln : D->lane)
+    for (Slot& S : Ln.slot) S.release();
+  checksum_tables_destroy(&D->tabs);
+  zstd_set_ctables(D->ordinal, nullptr);
+  zstd_ctables_destroy(D->zstd_ctables);
+  for (auto ev : D->ev_mark)
+    if (ev) cudaEventDestroy(ev);
+  delete D;
+}
+
+void destroy_context(Context* C) {
+  for (Device* D : C->devs) destroy_device(D);
+  delete C;
 }
 
 }  // namespace
@@ -1063,9 +1218,7 @@ int b2s_init(uint32_t gpu_mask, uint64_t pinned_bytes_per_gpu, uint32_t streams_
     setenv("CUDA_DEVICE_MAX_CONNECTIONS", v, 0);
   }
   int count = 0;
-  cudaError_t e = cudaGetDeviceCount(&count);
-  if (e != cudaSuccess || count <= 0)
-    return fail(B2S_E_CUDA, "no CUDA device: %s", e != cudaSuccess ? cudaGetErrorString(e) : "device count is 0");
+  if (int rc = no_device(&count)) return rc;
   g_lz4_hlog = env_int("B2S_LZ4_HLOG", g_lz4_hlog);
   g_lz4_chunk_blocks = (uint32_t)std::max(1, env_int("B2S_LZ4_CHUNK_BLOCKS", (int)g_lz4_chunk_blocks));
   g_numa = env_int("B2S_NUMA", 1);
@@ -1077,41 +1230,12 @@ int b2s_init(uint32_t gpu_mask, uint64_t pinned_bytes_per_gpu, uint32_t streams_
   Context* C = new Context();
   for (int d = 0; d < count && d < 32; d++) {
     if (gpu_mask && !(gpu_mask & (1u << d))) continue;
-    CU(cudaSetDevice(d));
     Device* D = new Device();
-    D->ordinal = d;
-    char busid[32] = {0};
-    if (g_numa && cudaDeviceGetPCIBusId(busid, sizeof busid, d) == cudaSuccess) D->numa_node = numa::node_of_pci(busid);
-    (void)cudaGetLastError();
-    t_numa_node = D->numa_node;
-    for (int l = 0; l < kLanes; l++)
-      for (int k = 0; k < g_nslot; k++) {
-        Slot& S = D->lane[l].slot[k];
-        // the read lane's kernels are short and latency bound (token walks, per-stream header walks, two host round
-        // trips per chunk): they get the higher stream priority so they are not queued behind the write lane's grids
-        int prio_lo = 0, prio_hi = 0;
-        cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi);
-        const int prio = l == kLaneRead ? prio_hi : prio_lo;
-        CU(cudaStreamCreateWithPriority(&S.st, cudaStreamNonBlocking, prio));
-        CU(cudaStreamCreateWithPriority(&S.st2, cudaStreamNonBlocking, prio));
-        cudaEvent_t* evs2[] = {&S.ev_fork, &S.ev_match[0], &S.ev_match[1], &S.ev_free[0], &S.ev_free[1]};
-        for (auto p : evs2) CU(cudaEventCreateWithFlags(p, cudaEventDisableTiming));
-        cudaEvent_t* evs[] = {&S.ev_a, &S.ev_b, &S.ev_k0, &S.ev_k1, &S.ev_t0, &S.ev_t1, &S.ev_h0, &S.ev_h1, &S.ev_d0, &S.ev_d1,
-                              &S.ev_p0, &S.ev_p1, &S.ev_f[0], &S.ev_f[1], &S.ev_f[2], &S.ev_f[3]};
-        for (auto p : evs) CU(cudaEventCreate(p));
-        // pinned_bytes_per_gpu: the library's own pinned descriptor blocks are sized up front (split over the slots)
-        // instead of growing on first use; 0 = grow on demand.  Payload staging is the caller's (b2s_host_alloc).
-        if (pinned_bytes_per_gpu) {
-          const uint64_t per = std::min<uint64_t>(pinned_bytes_per_gpu / (uint64_t)(kLanes * g_nslot), 64ull << 20);
-          if (per >= 4096 && S.hmeta.ensure(per)) return B2S_E_NOMEM;
-        }
-      }
-    if (checksum_tables_create(&D->tabs)) return fail(B2S_E_CUDA, "checksum table upload failed%s");
-    if (zstd_ctables_create(&D->zstd_ctables)) return fail(B2S_E_CUDA, "zstd table upload failed%s");
-    zstd_set_ctables(d, D->zstd_ctables);
-    CU(cudaEventCreate(&D->ev_mark[0]));
-    CU(cudaEventCreate(&D->ev_mark[1]));
     C->devs.push_back(D);
+    if (int rc = create_device(*D, d, pinned_bytes_per_gpu)) {
+      destroy_context(C);
+      return rc;
+    }
   }
   if (C->devs.empty()) {
     delete C;
@@ -1132,42 +1256,7 @@ void b2s_shutdown(void) {
     for (int d = 0; d < kMaxOrdinals; d++) g_ex.budget[d] = 0;
   }
   ex_free(dead);
-  for (Device* D : g_ctx->devs) {
-    cudaSetDevice(D->ordinal);
-    cudaDeviceSynchronize();
-    for (int l = 0; l < kLanes; l++)
-    for (int k = 0; k < NSLOT; k++) {
-      Slot& S = D->lane[l].slot[k];
-      S.meta.release();
-      S.scratch.release();
-      S.desc.release();
-      S.zmeta.release();
-      S.src.release();
-      S.dst.release();
-      S.pws.release();
-      S.parena.release();
-      S.xpieces.release();
-      S.fws.release();
-      S.hmeta.release();
-      cudaEvent_t evs[] = {S.ev_a, S.ev_b, S.ev_k0, S.ev_k1, S.ev_t0, S.ev_t1, S.ev_h0, S.ev_h1, S.ev_d0, S.ev_d1,
-                           S.ev_p0, S.ev_p1, S.ev_f[0], S.ev_f[1], S.ev_f[2], S.ev_f[3]};
-      for (auto ev : evs)
-        if (ev) cudaEventDestroy(ev);
-      for (auto ev : S.ev_dom) cudaEventDestroy(ev);
-      S.ev_dom.clear();
-      cudaEvent_t evs2[] = {S.ev_fork, S.ev_match[0], S.ev_match[1], S.ev_free[0], S.ev_free[1]};
-      for (auto ev : evs2)
-        if (ev) cudaEventDestroy(ev);
-      if (S.st2) cudaStreamDestroy(S.st2);
-      if (S.st) cudaStreamDestroy(S.st);
-    }
-    checksum_tables_destroy(&D->tabs);
-    zstd_ctables_destroy(D->zstd_ctables);
-    for (auto ev : D->ev_mark)
-      if (ev) cudaEventDestroy(ev);
-    delete D;
-  }
-  delete g_ctx;
+  destroy_context(g_ctx);
   g_ctx = nullptr;
 }
 
@@ -1223,7 +1312,7 @@ int b2s_host_unregister(void* p) {
 }
 
 uint64_t b2s_compress_bound(uint32_t codec, uint32_t codec_block_size, uint64_t src_len) {
-  const uint64_t bs = block_size_or_default(codec, codec_block_size);
+  const uint64_t bs = block_size_or_default(codec_block_size);
   const uint64_t nb = (src_len + bs - 1) / bs;
   switch (codec) {
     case B2S_CODEC_LZ4BLOCK: return src_len + (nb + 1) * 21;  // RAW fallback bounds every block by its input
@@ -1353,11 +1442,7 @@ int b2s_checksum_dev(uint32_t dev_index, uint32_t alg, uint32_t n, const void* d
   for (uint32_t i = 0; i < n; i++) total += len[i];
   rc = checksum_chunk_dev(D, Ln.slot[0], alg, n, (const uint8_t*)d_base, off, len, out, total, &launches);
   if (rc) return rc;
-  add_timing(Ln.slot[0], false);
-  t_timing.kernel_launches = launches;
-  t_timing.src_bytes = total;
-  t_timing.total_ms = wt.ms();
-  g_ctx->launches += launches;
+  end_timing(wt, launches, CallBytes{total, 0, 0, 0}, &Ln.slot[0]);
   return 0;
 }
 
@@ -1379,25 +1464,17 @@ static int checksum_host(uint32_t alg, uint32_t n, const uint8_t* const* ptr, co
     Slot& S = Ln.slot[0];
     const uint32_t i0 = starts[c], cnt = starts[c + 1] - starts[c];
     dev_off.resize(cnt);
-    uint64_t bytes = plan_runs(cnt, ptr + i0, len + i0, dev_off.data(), runs);
-    rc = S.src.ensure(bytes + 64);
-    if (rc) return rc;
-    CU(cudaEventRecord(S.ev_h0, S.st));
-    for (const Run& r : runs)
-      CU(cudaMemcpyAsync((uint8_t*)S.src.p + r.dev_off, r.host, r.bytes, cudaMemcpyHostToDevice, S.st));
-    CU(cudaEventRecord(S.ev_h1, S.st));
+    uint64_t bytes = 0;
+    if ((rc = upload_chunk(S, cnt, ptr + i0, len + i0, dev_off.data(), runs, &bytes))) return rc;
     rc = checksum_chunk_dev(D, S, alg, cnt, (const uint8_t*)S.src.p, dev_off.data(), len + i0, out + i0, bytes,
                             &launches);
     if (rc) return rc;
-    add_timing(S, false);
-    t_timing.h2d_ms += ms_between(S.ev_h0, S.ev_h1);
+    add_timing(S, true);
     t_timing.h2d_bytes += bytes;
     t_timing.d2h_bytes += (uint64_t)cnt * 8;
     t_timing.src_bytes += bytes;
   }
-  t_timing.kernel_launches = launches;
-  t_timing.total_ms = wt.ms();
-  g_ctx->launches += launches;
+  end_timing(wt, launches, CallBytes{});
   return 0;
 }
 
@@ -1446,35 +1523,24 @@ int b2s_compress_dev(uint32_t dev_index, uint32_t codec, int32_t level, uint32_t
   Lane& Ln = D->lane[kLaneWrite];
   std::lock_guard<std::mutex> lk(Ln.mtx);
   Slot& S = Ln.slot[0];
-  const uint32_t bs = block_size_or_default(codec, codec_block_size);
   CompressJob J;
-  rc = compress_prepare(S, codec, bs, n, src_len, J);
-  if (rc) return rc;
-  memcpy(J.h_src_off, src_off, (size_t)n * 8);
-  memcpy(J.h_src_len, src_len, (size_t)n * 8);
-  CompressDevMeta M;
   uint64_t launches = 0;
-  rc = compress_enqueue(g_ctx, S, D->tabs, bs, checksum_alg, J, (const uint8_t*)d_src_base, (uint8_t*)d_dst_base,
-                        dst_cap, M, &launches, level);
+  rc = compress_chunk(S, D->tabs, codec, level, block_size_or_default(codec_block_size), checksum_alg, n, src_off,
+                      src_len, (const uint8_t*)d_src_base, (uint8_t*)d_dst_base, dst_cap, J, &launches);
   if (rc) return rc;
   CU(cudaEventSynchronize(S.ev_a));
   CU(cudaGetLastError());
-  memcpy(dst_off, J.h_dst_off, (size_t)n * 8);
-  memcpy(dst_len, J.h_dst_len, (size_t)n * 8);
-  memcpy(status, J.h_status, (size_t)n * 4);
+  memcpy(dst_off, J.h.dst_off, (size_t)n * 8);
+  memcpy(dst_len, J.h.dst_len, (size_t)n * 8);
+  memcpy(status, J.h.status, (size_t)n * 4);
   if (checksum_out) {
-    if (checksum_alg) memcpy(checksum_out, J.h_cks, (size_t)n * 8);
+    if (checksum_alg) memcpy(checksum_out, J.h.cks, (size_t)n * 8);
     else memset(checksum_out, 0, (size_t)n * 8);
   }
-  uint64_t total = J.h_total[0] + stream_overhead(codec) * n, srcb = 0;
+  uint64_t total = J.h.total[0] + stream_overhead(codec) * n, srcb = 0;
   for (uint32_t i = 0; i < n; i++) srcb += src_len[i];
   if (dst_total) *dst_total = total;
-  add_timing(S, false);
-  t_timing.kernel_launches = launches;
-  t_timing.src_bytes = srcb;
-  t_timing.dst_bytes = total;
-  t_timing.total_ms = wt.ms();
-  g_ctx->launches += launches;
+  end_timing(wt, launches, CallBytes{srcb, total, 0, 0}, &S);
   return 0;
 }
 
@@ -1493,60 +1559,35 @@ static int compress_host(uint32_t codec, int32_t level, uint32_t codec_block_siz
   if (!n) return 0;
   Lane& Ln = D->lane[kLaneWrite];
   std::lock_guard<std::mutex> lk(Ln.mtx);
-  const uint32_t bs = block_size_or_default(codec, codec_block_size);
+  const uint32_t bs = block_size_or_default(codec_block_size);
+  if ((rc = check_codec_block(codec, bs))) return rc;  // before anything is staged
   std::vector<uint32_t> starts;
   make_chunks(n, src_len, starts);
   const size_t nchunks = starts.size() - 1;
   std::vector<CompressJob> jobs(nchunks);
-  std::vector<std::vector<Run>> runs(g_nslot);
+  std::vector<Run> runs;
+  std::vector<uint64_t> dev_off;
   uint64_t launches = 0, run_off = 0;
 
   auto finish = [&](size_t c) -> int {
     Slot& S = Ln.slot[c % g_nslot];
-    CompressJob& J = jobs[c];
-    const uint32_t i0 = starts[c];
+    const CompressLayout& H = jobs[c].h;
+    const uint32_t i0 = starts[c], cnt = jobs[c].n;
     CU(cudaEventSynchronize(S.ev_a));
     add_timing(S, true);
-    const uint64_t chunk_total = J.h_total[0] + stream_overhead(codec) * J.n;
-    for (uint32_t k = 0; k < J.n; k++) {
-      status[i0 + k] = J.h_status[k];
-      dst_len[i0 + k] = J.h_dst_len[k];
-      if (checksum_out) checksum_out[i0 + k] = alg ? J.h_cks[k] : 0;
+    const uint64_t chunk_total = H.total[0] + stream_overhead(codec) * cnt;
+    for (uint32_t k = 0; k < cnt; k++) {
+      status[i0 + k] = H.status[k];
+      dst_len[i0 + k] = H.dst_len[k];
+      dst_off[i0 + k] = run_off + H.dst_off[k];
+      if (checksum_out) checksum_out[i0 + k] = alg ? H.cks[k] : 0;
     }
-    CU(cudaEventRecord(S.ev_d0, S.st));
-    if (packed_dst) {
-      if (run_off + chunk_total > packed_cap) {
-        for (uint32_t k = 0; k < J.n; k++) {
-          dst_off[i0 + k] = run_off + J.h_dst_off[k];
-          if (run_off + J.h_dst_off[k] + J.h_dst_len[k] > packed_cap) status[i0 + k] = B2S_E_DST_TOO_SMALL;
-        }
-        // copy what fits so that earlier streams of the chunk stay valid
-        uint64_t fit = packed_cap > run_off ? packed_cap - run_off : 0;
-        if (fit) CU(cudaMemcpyAsync(packed_dst + run_off, S.dst.p, fit, cudaMemcpyDeviceToHost, S.st));
-        t_timing.d2h_bytes += fit;
-      } else {
-        for (uint32_t k = 0; k < J.n; k++) dst_off[i0 + k] = run_off + J.h_dst_off[k];
-        if (chunk_total)
-          CU(cudaMemcpyAsync(packed_dst + run_off, S.dst.p, chunk_total, cudaMemcpyDeviceToHost, S.st));
-        t_timing.d2h_bytes += chunk_total;
-      }
-      run_off += chunk_total;
-    } else {
-      for (uint32_t k = 0; k < J.n; k++) {
-        const uint32_t i = i0 + k;
-        if (status[i] != 0) continue;
-        if (J.h_dst_len[k] > dst_cap[i]) {
-          status[i] = B2S_E_DST_TOO_SMALL;
-          continue;
-        }
-        CU(cudaMemcpyAsync(dst[i], (uint8_t*)S.dst.p + J.h_dst_off[k], J.h_dst_len[k], cudaMemcpyDeviceToHost, S.st));
-        t_timing.d2h_bytes += J.h_dst_len[k];
-      }
-      run_off += chunk_total;
-    }
-    CU(cudaEventRecord(S.ev_d1, S.st));
+    // a stream has at least its framing bytes, and no status but B2S_E_DST_TOO_SMALL
+    const int r = download_chunk(S, cnt, H.dst_off, H.dst_len, chunk_total, packed_dst, packed_cap, run_off,
+                                 dst ? dst + i0 : nullptr, dst_cap ? dst_cap + i0 : nullptr, status + i0);
+    run_off += chunk_total;
     t_timing.dst_bytes += chunk_total;
-    return 0;
+    return r;
   };
 
   for (size_t c = 0; c < nchunks; c++) {
@@ -1558,26 +1599,15 @@ static int compress_host(uint32_t codec, int32_t level, uint32_t codec_block_siz
       t_timing.d2h_ms += ms_between(S.ev_d0, S.ev_d1);
     }
     const uint32_t i0 = starts[c], cnt = starts[c + 1] - starts[c];
-    CompressJob& J = jobs[c];
-    rc = compress_prepare(S, codec, bs, cnt, src_len + i0, J);
-    if (rc) return rc;
-    memcpy(J.h_src_len, src_len + i0, (size_t)cnt * 8);
-    uint64_t bytes = plan_runs(cnt, src + i0, src_len + i0, J.h_src_off, runs[c % g_nslot]);
-    rc = S.src.ensure(bytes + 64);
-    if (rc) return rc;
-    uint64_t bound = 0;
+    uint64_t bound = 0, bytes = 0;
     for (uint32_t k = 0; k < cnt; k++) bound += b2s_compress_bound(codec, bs, src_len[i0 + k]);
-    rc = S.dst.ensure(bound + 64);
-    if (rc) return rc;
-    CU(cudaEventRecord(S.ev_h0, S.st));
-    for (const Run& r : runs[c % g_nslot])
-      CU(cudaMemcpyAsync((uint8_t*)S.src.p + r.dev_off, r.host, r.bytes, cudaMemcpyHostToDevice, S.st));
-    CU(cudaEventRecord(S.ev_h1, S.st));
+    if ((rc = S.dst.ensure(bound + 64))) return rc;
+    dev_off.resize(cnt);
+    if ((rc = upload_chunk(S, cnt, src + i0, src_len + i0, dev_off.data(), runs, &bytes))) return rc;
     t_timing.h2d_bytes += bytes;
     t_timing.src_bytes += bytes;
-    CompressDevMeta M;
-    rc = compress_enqueue(g_ctx, S, D->tabs, bs, alg, J, (const uint8_t*)S.src.p, (uint8_t*)S.dst.p, S.dst.cap, M,
-                          &launches, level);
+    rc = compress_chunk(S, D->tabs, codec, level, bs, alg, cnt, dev_off.data(), src_len + i0, (const uint8_t*)S.src.p,
+                        (uint8_t*)S.dst.p, S.dst.cap, jobs[c], &launches);
     if (rc) return rc;
   }
   for (size_t c = nchunks > (size_t)g_nslot ? nchunks - g_nslot : 0; c < nchunks; c++) {
@@ -1590,9 +1620,7 @@ static int compress_host(uint32_t codec, int32_t level, uint32_t codec_block_siz
   }
   CU(cudaGetLastError());
   if (dst_total) *dst_total = run_off;
-  t_timing.kernel_launches = launches;
-  t_timing.total_ms = wt.ms();
-  g_ctx->launches += launches;
+  end_timing(wt, launches, CallBytes{});
   return 0;
 }
 
@@ -1649,7 +1677,7 @@ uint64_t b2s_partition_compress_bound(uint32_t codec, uint32_t codec_block_size,
   if (codec == B2S_CODEC_NONE) return rec_bytes;
   // k non-empty partitions of L_p bytes: sum ceil(L_p / bs) <= (rec_bytes + k (bs - 1)) / bs, and every bound below
   // grows with k, which is at most min(num_partitions, rec_bytes)
-  const uint64_t bs = block_size_or_default(codec, codec_block_size);
+  const uint64_t bs = block_size_or_default(codec_block_size);
   const uint64_t k = std::min<uint64_t>(num_partitions, rec_bytes);
   const uint64_t nb = (rec_bytes + k * (bs - 1)) / bs;
   switch (codec) {
@@ -1752,33 +1780,9 @@ static int partition_compress_run(Device* D, Slot& S, uint32_t codec, int32_t le
     }
     launch_partition_gather(d_rec, d_len, n, P, d_dst, st, launches);
     CU(cudaEventRecord(S.ev_p1, st));
-    CU(cudaEventRecord(S.ev_t0, st));
-    CU(cudaEventRecord(S.ev_t1, st));
     if (alg && rec_bytes) {  // over every partition, empty ones included
-      size_t ws_elems = checksum_ws_elems(R) + 4;
-      int rc = S.meta.ensure(align_up((size_t)R * 8, 16) * 3 + align_up(((size_t)R + 1) * 8, 16) + ws_elems * 8 + 128);
+      int rc = checksum_chunk_dev(D, S, alg, R, d_dst, pstart.data(), plen.data(), checksum_out, rec_bytes, launches);
       if (rc) return rc;
-      rc = S.hmeta.ensure(align_up((size_t)R * 8, 16) * 3 + 64);
-      if (rc) return rc;
-      Carver hc(S.hmeta.p), dc(S.meta.p);
-      uint64_t* h_off = hc.take<uint64_t>(R);
-      uint64_t* h_len = hc.take<uint64_t>(R);
-      uint64_t* h_out = hc.take<uint64_t>(R);
-      uint64_t* d_off = dc.take<uint64_t>(R);
-      uint64_t* d_slen = dc.take<uint64_t>(R);
-      uint64_t* d_out = dc.take<uint64_t>(R);
-      uint64_t* d_work = dc.take<uint64_t>((size_t)R + 1);
-      uint64_t* d_ws = dc.take<uint64_t>(ws_elems);
-      memcpy(h_off, pstart.data(), (size_t)R * 8);
-      memcpy(h_len, plen.data(), (size_t)R * 8);
-      CU(cudaMemcpyAsync(d_off, h_off, (size_t)R * 8, cudaMemcpyHostToDevice, st));
-      CU(cudaMemcpyAsync(d_slen, h_len, (size_t)R * 8, cudaMemcpyHostToDevice, st));
-      launch_checksum(D->tabs, alg, d_dst, d_off, d_slen, R, pick_tile_shift(rec_bytes), d_work, d_ws, d_out, st,
-                      launches);
-      CU(cudaEventRecord(S.ev_k1, st));
-      CU(cudaMemcpyAsync(h_out, d_out, (size_t)R * 8, cudaMemcpyDeviceToHost, st));
-      CU(cudaStreamSynchronize(st));
-      memcpy(checksum_out, h_out, (size_t)R * 8);
     } else {
       CU(cudaEventRecord(S.ev_k1, st));
       CU(cudaStreamSynchronize(st));
@@ -1794,8 +1798,11 @@ static int partition_compress_run(Device* D, Slot& S, uint32_t codec, int32_t le
   for (uint32_t p = 0; p < R; p++)
     if (plen[p]) ne.push_back(p);
   const uint32_t m = (uint32_t)ne.size();
-  std::vector<uint64_t> ne_len(m);
-  for (uint32_t k = 0; k < m; k++) ne_len[k] = plen[ne[k]];
+  std::vector<uint64_t> ne_off(m), ne_len(m);
+  for (uint32_t k = 0; k < m; k++) {
+    ne_off[k] = pstart[ne[k]];
+    ne_len[k] = plen[ne[k]];
+  }
   CompressJob J;
   uint64_t total = 0;
   if (m) {
@@ -1803,18 +1810,12 @@ static int partition_compress_run(Device* D, Slot& S, uint32_t codec, int32_t le
     if (rc) return rc;
     launch_partition_gather(d_rec, d_len, n, P, (uint8_t*)S.parena.p, st, launches);
     CU(cudaEventRecord(S.ev_p1, st));
-    rc = compress_prepare(S, codec, bs, m, ne_len.data(), J);
-    if (rc) return rc;
-    for (uint32_t k = 0; k < m; k++) {
-      J.h_src_off[k] = pstart[ne[k]];
-      J.h_src_len[k] = ne_len[k];
-    }
-    CompressDevMeta M;
-    rc = compress_enqueue(g_ctx, S, D->tabs, bs, alg, J, (const uint8_t*)S.parena.p, d_dst, dst_cap, M, launches, level);
+    rc = compress_chunk(S, D->tabs, codec, level, bs, alg, m, ne_off.data(), ne_len.data(),
+                        (const uint8_t*)S.parena.p, d_dst, dst_cap, J, launches);
     if (rc) return rc;
     CU(cudaEventSynchronize(S.ev_a));
     CU(cudaGetLastError());
-    total = J.h_total[0] + stream_overhead(codec) * m;
+    total = J.h.total[0] + stream_overhead(codec) * m;
   } else {
     CU(cudaEventRecord(S.ev_p1, st));
     CU(cudaEventRecord(S.ev_k0, st));
@@ -1828,10 +1829,10 @@ static int partition_compress_run(Device* D, Slot& S, uint32_t codec, int32_t le
   uint64_t at = 0;  // an empty partition sits where the next non-empty one starts
   for (uint32_t p = 0, k = 0; p < R; p++) {
     if (k < m && ne[k] == p) {
-      dst_off[p] = J.h_dst_off[k];
-      dst_len[p] = J.h_dst_len[k];
-      checksum_out[p] = alg ? J.h_cks[k] : 0;
-      status[p] = J.h_status[k];
+      dst_off[p] = J.h.dst_off[k];
+      dst_len[p] = J.h.dst_len[k];
+      checksum_out[p] = alg ? J.h.cks[k] : 0;
+      status[p] = J.h.status[k];
       if (dst_off[p] + dst_len[p] > dst_cap) status[p] = B2S_E_DST_TOO_SMALL;
       short_dst |= status[p] == B2S_E_DST_TOO_SMALL;
       at = dst_off[p] + dst_len[p];
@@ -1862,15 +1863,10 @@ static int partition_args(uint32_t codec, uint32_t bs, uint32_t alg, uint32_t R,
   return 0;
 }
 
-static void partition_timing(Slot& S, uint32_t codec, uint64_t n_launches, uint64_t rec_bytes, uint64_t arena) {
-  add_timing(S, false);
-  // kernel_ms: partition step + compression; top_kernel_ms: the codec step, or the partition step for codec NONE
+// kernel_ms: partition step + compression; top_kernel_ms: the codec step, or the partition step for codec NONE
+static void partition_kernel_times(Slot& S, uint32_t codec) {
   t_timing.kernel_ms = ms_between(S.ev_p0, S.ev_k1);
   if (codec == B2S_CODEC_NONE) t_timing.top_kernel_ms = ms_between(S.ev_p0, S.ev_p1);
-  t_timing.kernel_launches = n_launches;
-  t_timing.src_bytes = rec_bytes;
-  t_timing.dst_bytes = arena;
-  g_ctx->launches += n_launches;
 }
 
 int b2s_partition_compress_dev(uint32_t dev_index, uint32_t codec, int32_t level, uint32_t codec_block_size,
@@ -1881,7 +1877,7 @@ int b2s_partition_compress_dev(uint32_t dev_index, uint32_t codec, int32_t level
   WallTimer wt;
   t_timing = b2s_timing{};
   if (dst_total) *dst_total = 0;
-  const uint32_t bs = block_size_or_default(codec, codec_block_size);
+  const uint32_t bs = block_size_or_default(codec_block_size);
   int rc = partition_args(codec, bs, checksum_alg, num_partitions, n_records, rec_base, rec_bytes, rec_len, rec_part,
                           dst_base, dst_off, dst_len, status);
   if (rc) return rc;
@@ -1899,8 +1895,8 @@ int b2s_partition_compress_dev(uint32_t dev_index, uint32_t codec, int32_t level
   if (rc && rc != B2S_E_DST_TOO_SMALL) return rc;
   if (checksum_out) memcpy(checksum_out, cks.data(), (size_t)num_partitions * 8);
   if (dst_total) *dst_total = arena;
-  partition_timing(S, codec, launches, rec_bytes, arena);
-  t_timing.total_ms = wt.ms();
+  end_timing(wt, launches, CallBytes{rec_bytes, arena, 0, 0}, &S);
+  partition_kernel_times(S, codec);
   return rc;
 }
 
@@ -1920,7 +1916,7 @@ static int partition_compress_packed(uint32_t codec, int32_t level, uint32_t cod
   WallTimer wt;
   t_timing = b2s_timing{};
   if (dst_total) *dst_total = 0;
-  const uint32_t bs = block_size_or_default(codec, codec_block_size);
+  const uint32_t bs = block_size_or_default(codec_block_size);
   int rc = partition_args(codec, bs, checksum_alg, num_partitions, n_records, rec_base, rec_bytes, rec_len, rec_part,
                           dst_base, dst_off, dst_len, status);
   if (rc) return rc;
@@ -1970,18 +1966,14 @@ static int partition_compress_packed(uint32_t codec, int32_t level, uint32_t cod
   CU(cudaGetLastError());
   if (checksum_out) memcpy(checksum_out, cks.data(), (size_t)num_partitions * 8);
   if (dst_total) *dst_total = arena;
-  partition_timing(S, codec, launches, rec_bytes, arena);
-  t_timing.h2d_ms = ms_between(S.ev_h0, S.ev_h1);
-  t_timing.d2h_ms = ms_between(S.ev_d0, S.ev_d1);
-  t_timing.h2d_bytes = rec_bytes + n_records * 8;
-  t_timing.d2h_bytes = fit;
   if (store && !result) {
     // the partitioned records are still in this slot (the write lane is held): in front of compression, or the arena
     // itself for codec NONE
     const uint8_t* parts = (const uint8_t*)(codec == B2S_CODEC_NONE ? S.dst.p : S.parena.p);
     *store->cached = ex_store(D->ordinal, st, store->shuffle, store->map, parts, rec_bytes, std::move(part_start));
   }
-  t_timing.total_ms = wt.ms();
+  end_timing(wt, launches, CallBytes{rec_bytes, arena, rec_bytes + n_records * 8, fit}, &S, kH2D | kD2H);
+  partition_kernel_times(S, codec);
   return result;
 }
 
@@ -2013,27 +2005,6 @@ int b2s_partition_compress_cached_packed(int32_t shuffle_id, int64_t map_id, uin
 // ------------------------------------------------------------------------------------------------------------
 // read side
 // ------------------------------------------------------------------------------------------------------------
-// fills the slice arrays of a job for blocks [i0, i0+cnt); dev_off = device offsets of the blocks
-static void fill_slices(DecompressJob& J, uint32_t i0, uint32_t cnt, const uint64_t* dev_off, const uint64_t* src_len,
-                        const uint32_t* slice_base, const uint64_t* slice_len, const uint64_t* slice_sum) {
-  uint32_t s = 0;
-  for (uint32_t k = 0; k < cnt; k++) {
-    J.h_slice_base[k] = s;
-    if (!J.n_slices) continue;
-    uint64_t o = dev_off[k];
-    for (uint32_t q = slice_base[i0 + k]; q < slice_base[i0 + k + 1]; q++) {
-      J.h_slice_off[s] = o;
-      J.h_slice_len[s] = slice_len[q];
-      J.h_slice_sum[s] = slice_sum[q];
-      J.h_slice_owner[s] = k;
-      o += slice_len[q];
-      s++;
-    }
-    (void)src_len;
-  }
-  J.h_slice_base[cnt] = s;
-}
-
 // slices of a block must tile it exactly (S3ChecksumValidationStream walks .index differences over the block)
 static int check_slices(uint32_t n, const uint64_t* src_len, const uint32_t* slice_base, const uint64_t* slice_len) {
   for (uint32_t i = 0; i < n; i++) {
@@ -2065,32 +2036,22 @@ int b2s_decompress_dev(uint32_t dev_index, uint32_t codec, uint32_t checksum_alg
   std::lock_guard<std::mutex> lk(Ln.mtx);
   Slot& S = Ln.slot[0];
   DecompressJob J;
-  const uint32_t ns = checksum_alg ? slice_base[n] : 0;
-  rc = decompress_prepare(S, codec, checksum_alg, n, ns, J);
-  if (rc) return rc;
-  memcpy(J.h_src_off, src_off, (size_t)n * 8);
-  memcpy(J.h_src_len, src_len, (size_t)n * 8);
-  fill_slices(J, 0, n, src_off, src_len, slice_base, slice_len, slice_checksum);
   uint64_t srcb = 0, launches = 0;
   for (uint32_t i = 0; i < n; i++) srcb += src_len[i];
-  rc = decompress_enqueue_a(S, D->tabs, checksum_alg, J, (const uint8_t*)d_src_base, srcb, &launches);
+  rc = decompress_phase_a(S, D->tabs, codec, checksum_alg, n, src_off, src_len, checksum_alg ? slice_base[n] : 0,
+                          slice_base, slice_len, slice_checksum, (const uint8_t*)d_src_base, srcb, J, &launches);
   if (rc) return rc;
   CU(cudaEventSynchronize(S.ev_a));
   rc = decompress_enqueue_b(S, J, (const uint8_t*)d_src_base, (uint8_t*)d_dst_base, dst_cap, &launches);
   if (rc) return rc;
   CU(cudaEventSynchronize(S.ev_b));
   CU(cudaGetLastError());
-  memcpy(dst_off, J.h_dst_off, (size_t)n * 8);
-  memcpy(dst_len, J.h_dst_len, (size_t)n * 8);
-  memcpy(status, J.h_status, (size_t)n * 4);
-  if (bad_slice) memcpy(bad_slice, J.h_bad, (size_t)n * 4);
+  memcpy(dst_off, J.h.dst_off, (size_t)n * 8);
+  memcpy(dst_len, J.h.dst_len, (size_t)n * 8);
+  memcpy(status, J.h.status, (size_t)n * 4);
+  if (bad_slice) memcpy(bad_slice, J.h.bad, (size_t)n * 4);
   if (dst_total) *dst_total = J.total_out;
-  add_timing(S, false);
-  t_timing.kernel_launches = launches;
-  t_timing.src_bytes = srcb;
-  t_timing.dst_bytes = J.total_out;
-  t_timing.total_ms = wt.ms();
-  g_ctx->launches += launches;
+  end_timing(wt, launches, CallBytes{srcb, J.total_out, 0, 0}, &S);
   return 0;
 }
 
@@ -2176,12 +2137,13 @@ static int decompress_host(uint32_t codec, uint32_t alg, uint32_t n, const uint8
   }
   Lane& Ln = D->lane[kLaneRead];
   std::lock_guard<std::mutex> lk(Ln.mtx);
+  if ((rc = check_decode_codec(codec, false))) return rc;  // before anything is staged
   std::vector<uint32_t> starts;
   make_chunks(n, src_len, starts);
   const size_t nchunks = starts.size() - 1;
   std::vector<DecompressJob> jobs(nchunks);
-  std::vector<uint64_t> chunk_src_bytes(nchunks);
-  std::vector<std::vector<Run>> runs(g_nslot);
+  std::vector<Run> runs;
+  std::vector<uint64_t> dev_off;
   uint64_t launches = 0, run_off = 0;
 
   auto stage_a = [&](size_t c) -> int {
@@ -2192,80 +2154,50 @@ static int decompress_host(uint32_t codec, uint32_t alg, uint32_t n, const uint8
     }
     const uint32_t i0 = starts[c], cnt = starts[c + 1] - starts[c];
     DecompressJob& J = jobs[c];
-    const uint32_t ns = alg ? slice_base[i0 + cnt] - slice_base[i0] : 0;
-    int r = decompress_prepare(S, codec, alg, cnt, ns, J);
-    if (r) return r;
     J.size_only = size_only;
-    memcpy(J.h_src_len, src_len + i0, (size_t)cnt * 8);
-    uint64_t bytes = plan_runs(cnt, src + i0, src_len + i0, J.h_src_off, runs[c % g_nslot]);
-    chunk_src_bytes[c] = bytes;
-    fill_slices(J, i0, cnt, J.h_src_off, src_len, slice_base, slice_len, slice_sum);
-    r = S.src.ensure(bytes + 64);
-    if (r) return r;
-    CU(cudaEventRecord(S.ev_h0, S.st));
-    for (const Run& q : runs[c % g_nslot])
-      CU(cudaMemcpyAsync((uint8_t*)S.src.p + q.dev_off, q.host, q.bytes, cudaMemcpyHostToDevice, S.st));
-    CU(cudaEventRecord(S.ev_h1, S.st));
+    dev_off.resize(cnt);
+    uint64_t bytes = 0;
+    if (int r = upload_chunk(S, cnt, src + i0, src_len + i0, dev_off.data(), runs, &bytes)) return r;
     t_timing.h2d_bytes += bytes;
     t_timing.src_bytes += bytes;
-    return decompress_enqueue_a(S, D->tabs, alg, J, (const uint8_t*)S.src.p, bytes, &launches);
+    const uint32_t ns = alg ? slice_base[i0 + cnt] - slice_base[i0] : 0;
+    return decompress_phase_a(S, D->tabs, codec, alg, cnt, dev_off.data(), src_len + i0, ns,
+                              alg ? slice_base + i0 : nullptr, slice_len, slice_sum, (const uint8_t*)S.src.p, bytes,
+                              J, &launches);
   };
   auto stage_b = [&](size_t c) -> int {
     Slot& S = Ln.slot[c % g_nslot];
     DecompressJob& J = jobs[c];
     CU(cudaEventSynchronize(S.ev_a));
     if (size_only) {
-      J.total_out = J.h_totals[1];
-      CU(cudaMemcpyAsync(J.h_down, J.d_down, J.down_bytes, cudaMemcpyDeviceToHost, S.st));
+      J.total_out = J.h.totals[1];
+      CU(cudaMemcpyAsync(J.h.down, J.d.down, J.d.down_bytes, cudaMemcpyDeviceToHost, S.st));
       CU(cudaEventRecord(S.ev_b, S.st));
       return 0;
     }
-    int r = S.dst.ensure(J.h_totals[1] + 64);
+    int r = S.dst.ensure(J.h.totals[1] + 64);
     if (r) return r;
     return decompress_enqueue_b(S, J, (const uint8_t*)S.src.p, (uint8_t*)S.dst.p, S.dst.cap, &launches);
   };
   auto stage_c = [&](size_t c) -> int {
     Slot& S = Ln.slot[c % g_nslot];
-    DecompressJob& J = jobs[c];
+    const DecompressJob& J = jobs[c];
     const uint32_t i0 = starts[c];
     CU(cudaEventSynchronize(S.ev_b));
     if (!size_only) add_timing(S, true);
-    CU(cudaEventRecord(S.ev_d0, S.st));
     for (uint32_t k = 0; k < J.n; k++) {
       const uint32_t i = i0 + k;
-      status[i] = J.h_status[k];
-      dst_len[i] = size_only ? J.h_dst_len[k] : J.h_dst_len[k];
-      if (bad_slice) bad_slice[i] = J.h_bad[k];
-      if (dst_off) dst_off[i] = run_off + J.h_dst_off[k];
+      status[i] = J.h.status[k];
+      dst_len[i] = J.h.dst_len[k];  // size_only: the decoded lengths of phase A
+      if (bad_slice) bad_slice[i] = J.h.bad[k];
+      if (dst_off) dst_off[i] = run_off + J.h.dst_off[k];
     }
-    if (size_only) {
-      // h_dst_len holds olen from phase A
-    } else if (packed_dst) {
-      uint64_t fit = J.total_out;
-      if (run_off + J.total_out > packed_cap) {
-        fit = packed_cap > run_off ? packed_cap - run_off : 0;
-        for (uint32_t k = 0; k < J.n; k++)
-          if (status[i0 + k] == 0 && run_off + J.h_dst_off[k] + J.h_dst_len[k] > packed_cap)
-            status[i0 + k] = B2S_E_DST_TOO_SMALL;
-      }
-      if (fit) CU(cudaMemcpyAsync(packed_dst + run_off, S.dst.p, fit, cudaMemcpyDeviceToHost, S.st));
-      t_timing.d2h_bytes += fit;
-    } else {
-      for (uint32_t k = 0; k < J.n; k++) {
-        const uint32_t i = i0 + k;
-        if (status[i] != 0 || J.h_dst_len[k] == 0) continue;
-        if (J.h_dst_len[k] > dst_cap[i]) {
-          status[i] = B2S_E_DST_TOO_SMALL;
-          continue;
-        }
-        CU(cudaMemcpyAsync(dst[i], (uint8_t*)S.dst.p + J.h_dst_off[k], J.h_dst_len[k], cudaMemcpyDeviceToHost, S.st));
-        t_timing.d2h_bytes += J.h_dst_len[k];
-      }
-    }
-    CU(cudaEventRecord(S.ev_d1, S.st));
+    // a size_only call has no destination: nothing is copied
+    const int r = download_chunk(S, J.n, J.h.dst_off, J.h.dst_len, J.total_out, packed_dst, packed_cap, run_off,
+                                 dst ? dst + i0 : nullptr, dst_cap ? dst_cap + i0 : nullptr, status + i0);
     run_off += J.total_out;
     t_timing.dst_bytes += J.total_out;
-    return 0;
+    return r;
   };
 
   // software pipeline over the chunks: enqueue chunk c's upload + phase A first (never blocks on younger work), then
@@ -2285,16 +2217,14 @@ static int decompress_host(uint32_t codec, uint32_t alg, uint32_t n, const uint8
   }
   CU(cudaGetLastError());
   if (dst_total) *dst_total = run_off;
-  t_timing.kernel_launches = launches;
-  t_timing.total_ms = wt.ms();
-  g_ctx->launches += launches;
+  end_timing(wt, launches, CallBytes{});
   return 0;
 }
 
 // builds the flattened slice arrays used by the engine from the per-block pointer form
-static int flatten_slices(uint32_t n, const uint32_t* n_slices, const uint64_t* const* slice_len,
-                          const uint64_t* const* slice_checksum, std::vector<uint32_t>& base,
-                          std::vector<uint64_t>& len, std::vector<uint64_t>& sum) {
+static void flatten_slices(uint32_t n, const uint32_t* n_slices, const uint64_t* const* slice_len,
+                           const uint64_t* const* slice_checksum, std::vector<uint32_t>& base,
+                           std::vector<uint64_t>& len, std::vector<uint64_t>& sum) {
   base.assign((size_t)n + 1, 0);
   for (uint32_t i = 0; i < n; i++) base[i + 1] = base[i] + n_slices[i];
   len.resize(base[n]);
@@ -2304,7 +2234,6 @@ static int flatten_slices(uint32_t n, const uint32_t* n_slices, const uint64_t* 
       len[base[i] + k] = slice_len[i][k];
       sum[base[i] + k] = slice_checksum[i][k];
     }
-  return 0;
 }
 
 int b2s_decompress_batch(uint32_t codec, uint32_t checksum_alg, uint32_t n, const uint8_t* const* src,
@@ -2389,6 +2318,15 @@ static RecordSpec fixed_spec(uint32_t record_bytes, uint32_t key_off, uint32_t k
   r.key_len = key_len;
   return r;
 }
+static RecordSpec rows_spec(uint32_t key_type, uint32_t key_off, uint32_t key_len, int32_t null_field) {
+  RecordSpec r;
+  r.is_rows = true;
+  r.key_type = key_type;
+  r.key_off = key_off;
+  r.key_len = key_len;
+  r.null_field = null_field;
+  return r;
+}
 
 static int sort_args(uint32_t codec, uint32_t alg, uint32_t n, const uint64_t* src_off, const uint64_t* src_len,
                      const uint32_t* slice_base, const uint64_t* slice_len, const uint64_t* slice_checksum,
@@ -2420,12 +2358,8 @@ static int sort_args(uint32_t codec, uint32_t alg, uint32_t n, const uint64_t* s
 
 // without a usable device the sort calls report B2S_E_CUDA (b2s_init has failed for that reason), otherwise as get_device
 static int sort_device(uint32_t dev_index, Device** out) {
-  if (!g_ctx) {
-    int count = 0;
-    const cudaError_t e = cudaGetDeviceCount(&count);
-    if (e != cudaSuccess || count <= 0)
-      return fail(B2S_E_CUDA, "no CUDA device: %s", e != cudaSuccess ? cudaGetErrorString(e) : "device count is 0");
-  }
+  if (!g_ctx)
+    if (int rc = no_device()) return rc;
   return get_device(dev_index, out);
 }
 
@@ -2473,18 +2407,13 @@ static int decompress_sort_run(Device* D, Slot& S, uint32_t codec, uint32_t alg,
   DecompressJob J;
   int rc;
   if (n) {
-    const uint32_t ns = alg ? slice_base[n] : 0;
-    rc = decompress_prepare(S, codec, alg, n, ns, J, true);
-    if (rc) return rc;
-    memcpy(J.h_src_off, src_dev_off, (size_t)n * 8);
-    memcpy(J.h_src_len, src_len, (size_t)n * 8);
-    fill_slices(J, 0, n, src_dev_off, src_len, slice_base, slice_len, slice_sum);
     uint64_t srcb = 0;
     for (uint32_t i = 0; i < n; i++) srcb += src_len[i];
-    rc = decompress_enqueue_a(S, D->tabs, alg, J, d_src, srcb, launches);
+    rc = decompress_phase_a(S, D->tabs, codec, alg, n, src_dev_off, src_len, alg ? slice_base[n] : 0, slice_base,
+                            slice_len, slice_sum, d_src, srcb, J, launches, true);
     if (rc) return rc;
     // the phase-A verdicts (checksums, stream headers) and decoded lengths, before anything is decoded
-    CU(cudaMemcpyAsync(J.h_down, J.d_down, J.down_bytes, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(J.h.down, J.d.down, J.d.down_bytes, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
     CU(cudaGetLastError());
   } else {  // every source is cached
@@ -2501,8 +2430,8 @@ static int decompress_sort_run(Device* D, Slot& S, uint32_t codec, uint32_t alg,
   char msg[256];
   for (uint32_t i = 0; i < n_src; i++) {
     const bool c = cached(i);
-    int32_t& s = c ? cached_status[i] : J.h_status[block(i)];
-    const uint64_t len = c ? (*mix)[i].len : J.h_dst_len[block(i)];
+    int32_t& s = c ? cached_status[i] : J.h.status[block(i)];
+    const uint64_t len = c ? (*mix)[i].len : J.h.dst_len[block(i)];
     if (c) s = (*mix)[i].status;
     if (s == B2S_OK && !spec.rows() && len % spec.record_bytes) {
       s = B2S_E_CORRUPT;
@@ -2517,11 +2446,11 @@ static int decompress_sort_run(Device* D, Slot& S, uint32_t codec, uint32_t alg,
     length[i] = len;
     at += len;
   }
-  *total = mix ? at : J.h_totals[1];
+  *total = mix ? at : J.h.totals[1];
   auto report = [&]() {
     for (uint32_t i = 0; i < n_src; i++) {
-      status[i] = cached(i) ? cached_status[i] : J.h_status[block(i)];
-      if (bad_slice) bad_slice[i] = cached(i) ? -1 : J.h_bad[block(i)];
+      status[i] = cached(i) ? cached_status[i] : J.h.status[block(i)];
+      if (bad_slice) bad_slice[i] = cached(i) ? -1 : J.h.bad[block(i)];
     }
   };
   auto skip_events = [&](bool decode, bool sort) -> int {  // stand-ins for the steps a call does not run
@@ -2563,10 +2492,10 @@ static int decompress_sort_run(Device* D, Slot& S, uint32_t codec, uint32_t alg,
       else if (codec == B2S_CODEC_NONE)
         exchange_add_pieces(pieces, d_src + src_dev_off[s.block], place[i], src_len[s.block]);
       else
-        J.h_dst_off[s.block] = place[i];
+        J.h.dst_off[s.block] = place[i];
     }
     if (n && codec != B2S_CODEC_NONE)  // phase B decodes every block straight to its place among the cached ranges
-      CU(cudaMemcpyAsync(J.dst_off, J.h_dst_off, (size_t)n * 8, cudaMemcpyHostToDevice, st));
+      CU(cudaMemcpyAsync(J.d.dst_off, J.h.dst_off, (size_t)n * 8, cudaMemcpyHostToDevice, st));
     if (!pieces.empty()) {
       if ((rc = S.xpieces.ensure(pieces.size() * sizeof(ExchangePiece)))) return rc;
       CU(cudaMemcpyAsync(S.xpieces.p, pieces.data(), pieces.size() * sizeof(ExchangePiece), cudaMemcpyHostToDevice,
@@ -2580,7 +2509,7 @@ static int decompress_sort_run(Device* D, Slot& S, uint32_t codec, uint32_t alg,
       if ((rc = S.dst.ensure(*total + 64))) return rc;
       for (uint32_t i = 0; i < n; i++)
         if (src_len[i])
-          CU(cudaMemcpyAsync((uint8_t*)S.dst.p + J.h_dst_off[i], d_src + src_dev_off[i], src_len[i],
+          CU(cudaMemcpyAsync((uint8_t*)S.dst.p + J.h.dst_off[i], d_src + src_dev_off[i], src_len[i],
                              cudaMemcpyDeviceToDevice, st));
       arena = (const uint8_t*)S.dst.p;
     }
@@ -2591,7 +2520,7 @@ static int decompress_sort_run(Device* D, Slot& S, uint32_t codec, uint32_t alg,
     if (rc) return rc;
     CU(cudaEventSynchronize(S.ev_b));
     CU(cudaGetLastError());
-    for (uint32_t i = 0; i < n; i++) failed |= J.h_status[i] != B2S_OK;
+    for (uint32_t i = 0; i < n; i++) failed |= J.h.status[i] != B2S_OK;
     if (failed) {
       report();
       return skip_events(false, true);
@@ -2635,7 +2564,7 @@ static int decompress_sort_run(Device* D, Slot& S, uint32_t codec, uint32_t alg,
   for (uint32_t i = 0; i < n_src; i++) {
     const uint64_t v = rb[1 + i];
     if (v == ~0ull) continue;
-    (cached(i) ? cached_status[i] : J.h_status[block(i)]) = B2S_E_CORRUPT;
+    (cached(i) ? cached_status[i] : J.h.status[block(i)]) = B2S_E_CORRUPT;
     if (!failed) {
       static const char* const why[] = {"", "the block ends inside a size prefix", "the size is negative",
                                         "the record runs past the block end", "the row is shorter than key_off + key_len",
@@ -2677,14 +2606,9 @@ static int decompress_sort_run(Device* D, Slot& S, uint32_t codec, uint32_t alg,
 }
 
 // kernel_ms: verification + decode + sort; top_kernel_ms: the sort step (rows: framing + sort)
-static void sort_timing(Slot& S, uint64_t n_launches, uint64_t src_bytes, uint64_t total) {
-  add_timing(S, false);
+static void sort_kernel_times(Slot& S) {
   t_timing.kernel_ms = ms_between(S.ev_k0, S.ev_p1);
   t_timing.top_kernel_ms = ms_between(S.ev_p0, S.ev_p1);
-  t_timing.kernel_launches = n_launches;
-  t_timing.src_bytes = src_bytes;
-  t_timing.dst_bytes = total;
-  g_ctx->launches += n_launches;
 }
 
 // decompress_sort on the read lane of D over device-resident blocks, sorted into dst_base (device memory)
@@ -2693,7 +2617,7 @@ static int sort_dev_run(Device* D, uint32_t codec, uint32_t alg, uint32_t n, con
                         const uint64_t* slice_len, const uint64_t* slice_checksum, const RecordSpec& spec,
                         uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records,
                         int32_t* status, int32_t* bad_slice, const WallTimer& wt,
-                        const std::vector<SortSource>* mix = nullptr) {
+                        const std::vector<SortSource>* mix) {
   Lane& Ln = D->lane[kLaneRead];
   std::lock_guard<std::mutex> lk(Ln.mtx);
   Slot& S = Ln.slot[0];
@@ -2705,8 +2629,8 @@ static int sort_dev_run(Device* D, uint32_t codec, uint32_t alg, uint32_t n, con
                                slice_checksum, spec, &out, dst_cap, dst_total, n_records, status, bad_slice,
                                &launches, mix);
   if (rc) return rc;
-  sort_timing(S, launches, srcb, *dst_total);
-  t_timing.total_ms = wt.ms();
+  end_timing(wt, launches, CallBytes{srcb, *dst_total, 0, 0}, &S);
+  sort_kernel_times(S);
   return 0;
 }
 
@@ -2716,7 +2640,7 @@ static int sort_packed_run(Device* D, uint32_t codec, uint32_t alg, uint32_t n, 
                            const uint64_t* slice_len, const uint64_t* slice_checksum, const RecordSpec& spec,
                            uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records,
                            int32_t* status, int32_t* bad_slice, const WallTimer& wt,
-                           const std::vector<SortSource>* mix = nullptr) {
+                           const std::vector<SortSource>* mix) {
   Lane& Ln = D->lane[kLaneRead];
   std::lock_guard<std::mutex> lk(Ln.mtx);
   Slot& S = Ln.slot[0];
@@ -2752,13 +2676,114 @@ static int sort_packed_run(Device* D, uint32_t codec, uint32_t alg, uint32_t n, 
   CU(cudaEventRecord(S.ev_d1, st));
   CU(cudaStreamSynchronize(st));
   CU(cudaGetLastError());
-  sort_timing(S, launches, srcb, *dst_total);
-  t_timing.h2d_ms = ms_between(S.ev_h0, S.ev_h1);
-  t_timing.d2h_ms = ms_between(S.ev_d0, S.ev_d1);
-  t_timing.h2d_bytes = srcb;
-  t_timing.d2h_bytes = down;
-  t_timing.total_ms = wt.ms();
+  end_timing(wt, launches, CallBytes{srcb, *dst_total, srcb, down}, &S, kH2D | kD2H);
+  sort_kernel_times(S);
   return 0;
+}
+
+// The sources of an exchange sorted read: the fetched ones compacted in source order with their slices (what
+// decompress_sort_run takes as its blocks), and every source in order.
+struct MixedSources {
+  std::vector<SortSource> src;
+  std::vector<uint64_t> off, len, slice_len, slice_sum;
+  std::vector<uint32_t> slice_base{0};
+};
+
+static int exchange_sort_args(int32_t start_reduce, int32_t end_reduce, const int64_t* map_ids, const uint8_t* cached,
+                              uint32_t codec, uint32_t alg, uint32_t n, const uint8_t* src_base,
+                              const uint64_t* src_off, const uint64_t* src_len, const uint32_t* slice_base,
+                              const uint64_t* slice_len, const uint64_t* slice_checksum, const RecordSpec& spec,
+                              const void* dst_base, uint64_t dst_cap,
+                              const uint64_t* dst_total, const uint64_t* n_records, const int32_t* status,
+                              MixedSources& M) {
+  int rc = reduce_range_args(start_reduce, end_reduce);
+  if (rc) return rc;
+  if (n && (!map_ids || !cached || !status)) return fail(B2S_E_ARG, "null argument%s");
+  M.src.resize(n);
+  for (uint32_t i = 0; i < n; i++) {
+    M.src[i].cached = cached[i] != 0;
+    if (M.src[i].cached) continue;
+    if (!src_off || !src_len) return fail(B2S_E_ARG, "null argument%s");
+    if (alg && (!slice_base || !slice_len || !slice_checksum)) return fail(B2S_E_ARG, "slice arrays required%s");
+    M.src[i].block = (uint32_t)M.off.size();
+    M.off.push_back(src_off[i]);
+    M.len.push_back(src_len[i]);
+    if (alg) {
+      if (slice_base[i + 1] < slice_base[i]) return fail(B2S_E_ARG, "slice_base must be non-decreasing%s");
+      M.slice_len.insert(M.slice_len.end(), slice_len + slice_base[i], slice_len + slice_base[i + 1]);
+      M.slice_sum.insert(M.slice_sum.end(), slice_checksum + slice_base[i], slice_checksum + slice_base[i + 1]);
+      M.slice_base.push_back((uint32_t)M.slice_len.size());
+    }
+  }
+  const uint32_t m = (uint32_t)M.off.size();
+  return sort_args(codec, alg, m, M.off.data(), M.len.data(), M.slice_base.data(), M.slice_len.data(),
+                   M.slice_sum.data(), spec, src_base, dst_base, dst_cap, dst_total, n_records, status);
+}
+
+// references the cached sources of M on device D and describes them; B2S_E_ARG when a range exceeds an entry
+static int exchange_sort_sources(const ExRefs& refs, int32_t start_reduce, int32_t end_reduce, MixedSources& M) {
+  if (int rc = refs.check_range(end_reduce)) return rc;
+  for (uint32_t i = 0; i < (uint32_t)M.src.size(); i++) {
+    SortSource& s = M.src[i];
+    if (!s.cached) continue;
+    if (refs.entry[i]) s.src = refs.range(i, start_reduce, end_reduce, &s.len);
+    else s.status = B2S_E_NOT_CACHED;
+  }
+  return 0;
+}
+
+// the exchange-cache key of a sorted read whose sources may be resident (b2s_exchange_read_sort_*)
+struct ExchangeRead {
+  int32_t shuffle, start_reduce, end_reduce;
+  const int64_t* map_ids;
+  const uint8_t* cached;
+};
+
+// The body of the sort calls: zero the outputs, check the arguments and take the device, then run on the read lane
+// over device-resident blocks into device memory, or (packed) over host blocks into host memory.  x: an exchange read,
+// whose sources are cached ranges or fetched blocks.  A plain sort checks the device before its arguments; an
+// exchange read checks its arguments, then that the exchange cache can be used, then the device.
+static int sort_call(uint32_t dev_index, bool packed, const ExchangeRead* x, uint32_t codec, uint32_t alg, uint32_t n,
+                     const uint8_t* src_base, const uint64_t* src_off, const uint64_t* src_len,
+                     const uint32_t* slice_base, const uint64_t* slice_len, const uint64_t* slice_checksum,
+                     const RecordSpec& spec, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_total,
+                     uint64_t* n_records, int32_t* status, int32_t* bad_slice) {
+  WallTimer wt;
+  t_timing = b2s_timing{};
+  if (dst_total) *dst_total = 0;
+  if (n_records) *n_records = 0;
+  Device* D;
+  MixedSources M;
+  int rc;
+  if (!x) {
+    if ((rc = sort_device(dev_index, &D))) return rc;
+    rc = sort_args(codec, alg, n, src_off, src_len, slice_base, slice_len, slice_checksum, spec, src_base, dst_base,
+                   dst_cap, dst_total, n_records, status);
+  } else if ((rc = exchange_sort_args(x->start_reduce, x->end_reduce, x->map_ids, x->cached, codec, alg, n, src_base,
+                                      src_off, src_len, slice_base, slice_len, slice_checksum, spec, dst_base, dst_cap,
+                                      dst_total, n_records, status, M)) ||
+             (rc = exchange_ready())) {
+    return rc;
+  } else {
+    rc = sort_device(dev_index, &D);
+  }
+  if (rc || !n) return rc;
+  std::optional<ExRefs> refs;
+  const std::vector<SortSource>* mix = nullptr;
+  if (x) {
+    refs.emplace(D->ordinal, x->shuffle, n, x->map_ids, x->cached);
+    if ((rc = exchange_sort_sources(*refs, x->start_reduce, x->end_reduce, M))) return rc;
+    n = (uint32_t)M.off.size();
+    src_off = M.off.data();
+    src_len = M.len.data();
+    slice_base = M.slice_base.data();
+    slice_len = M.slice_len.data();
+    slice_checksum = M.slice_sum.data();
+    mix = &M.src;
+  }
+  return (packed ? sort_packed_run : sort_dev_run)(D, codec, alg, n, src_base, src_off, src_len, slice_base, slice_len,
+                                                   slice_checksum, spec, dst_base, dst_cap, dst_total, n_records,
+                                                   status, bad_slice, wt, mix);
 }
 
 int b2s_decompress_sort_dev(uint32_t dev_index, uint32_t codec, uint32_t checksum_alg, uint32_t n,
@@ -2767,19 +2792,9 @@ int b2s_decompress_sort_dev(uint32_t dev_index, uint32_t codec, uint32_t checksu
                             uint32_t record_bytes, uint32_t key_off, uint32_t key_len, uint8_t* dst_base,
                             uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records, int32_t* status,
                             int32_t* bad_slice) {
-  WallTimer wt;
-  t_timing = b2s_timing{};
-  if (dst_total) *dst_total = 0;
-  if (n_records) *n_records = 0;
-  Device* D;
-  int rc = sort_device(dev_index, &D);
-  if (rc) return rc;
-  const RecordSpec spec = fixed_spec(record_bytes, key_off, key_len);
-  rc = sort_args(codec, checksum_alg, n, src_off, src_len, slice_base, slice_len, slice_checksum, spec, src_base,
-                 dst_base, dst_cap, dst_total, n_records, status);
-  if (rc || !n) return rc;
-  return sort_dev_run(D, codec, checksum_alg, n, src_base, src_off, src_len, slice_base, slice_len, slice_checksum,
-                      spec, dst_base, dst_cap, dst_total, n_records, status, bad_slice, wt);
+  return sort_call(dev_index, false, nullptr, codec, checksum_alg, n, src_base, src_off, src_len, slice_base, slice_len,
+                   slice_checksum, fixed_spec(record_bytes, key_off, key_len), dst_base, dst_cap, dst_total, n_records,
+                   status, bad_slice);
 }
 
 int b2s_decompress_sort_packed(uint32_t codec, uint32_t checksum_alg, uint32_t n, const uint8_t* src_base,
@@ -2787,29 +2802,9 @@ int b2s_decompress_sort_packed(uint32_t codec, uint32_t checksum_alg, uint32_t n
                                const uint64_t* slice_len, const uint64_t* slice_checksum, uint32_t record_bytes,
                                uint32_t key_off, uint32_t key_len, uint8_t* dst_base, uint64_t dst_cap,
                                uint64_t* dst_total, uint64_t* n_records, int32_t* status, int32_t* bad_slice) {
-  WallTimer wt;
-  t_timing = b2s_timing{};
-  if (dst_total) *dst_total = 0;
-  if (n_records) *n_records = 0;
-  Device* D;
-  int rc = sort_device(t_device, &D);
-  if (rc) return rc;
-  const RecordSpec spec = fixed_spec(record_bytes, key_off, key_len);
-  rc = sort_args(codec, checksum_alg, n, src_off, src_len, slice_base, slice_len, slice_checksum, spec, src_base,
-                 dst_base, dst_cap, dst_total, n_records, status);
-  if (rc || !n) return rc;
-  return sort_packed_run(D, codec, checksum_alg, n, src_base, src_off, src_len, slice_base, slice_len, slice_checksum,
-                         spec, dst_base, dst_cap, dst_total, n_records, status, bad_slice, wt);
-}
-
-static RecordSpec rows_spec(uint32_t key_type, uint32_t key_off, uint32_t key_len, int32_t null_field) {
-  RecordSpec r;
-  r.is_rows = true;
-  r.key_type = key_type;
-  r.key_off = key_off;
-  r.key_len = key_len;
-  r.null_field = null_field;
-  return r;
+  return sort_call(t_device, true, nullptr, codec, checksum_alg, n, src_base, src_off, src_len, slice_base, slice_len,
+                   slice_checksum, fixed_spec(record_bytes, key_off, key_len), dst_base, dst_cap, dst_total, n_records,
+                   status, bad_slice);
 }
 
 int b2s_decompress_sort_rows_dev(uint32_t dev_index, uint32_t codec, uint32_t checksum_alg, uint32_t n,
@@ -2818,19 +2813,9 @@ int b2s_decompress_sort_rows_dev(uint32_t dev_index, uint32_t codec, uint32_t ch
                                  uint32_t key_type, uint32_t key_off, uint32_t key_len, int32_t null_field,
                                  uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records,
                                  int32_t* status, int32_t* bad_slice) {
-  WallTimer wt;
-  t_timing = b2s_timing{};
-  if (dst_total) *dst_total = 0;
-  if (n_records) *n_records = 0;
-  Device* D;
-  int rc = sort_device(dev_index, &D);
-  if (rc) return rc;
-  const RecordSpec spec = rows_spec(key_type, key_off, key_len, null_field);
-  rc = sort_args(codec, checksum_alg, n, src_off, src_len, slice_base, slice_len, slice_checksum, spec, src_base,
-                 dst_base, dst_cap, dst_total, n_records, status);
-  if (rc || !n) return rc;
-  return sort_dev_run(D, codec, checksum_alg, n, src_base, src_off, src_len, slice_base, slice_len, slice_checksum,
-                      spec, dst_base, dst_cap, dst_total, n_records, status, bad_slice, wt);
+  return sort_call(dev_index, false, nullptr, codec, checksum_alg, n, src_base, src_off, src_len, slice_base, slice_len,
+                   slice_checksum, rows_spec(key_type, key_off, key_len, null_field), dst_base, dst_cap, dst_total,
+                   n_records, status, bad_slice);
 }
 
 int b2s_decompress_sort_rows_packed(uint32_t codec, uint32_t checksum_alg, uint32_t n, const uint8_t* src_base,
@@ -2839,19 +2824,9 @@ int b2s_decompress_sort_rows_packed(uint32_t codec, uint32_t checksum_alg, uint3
                                     uint32_t key_off, uint32_t key_len, int32_t null_field, uint8_t* dst_base,
                                     uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records, int32_t* status,
                                     int32_t* bad_slice) {
-  WallTimer wt;
-  t_timing = b2s_timing{};
-  if (dst_total) *dst_total = 0;
-  if (n_records) *n_records = 0;
-  Device* D;
-  int rc = sort_device(t_device, &D);
-  if (rc) return rc;
-  const RecordSpec spec = rows_spec(key_type, key_off, key_len, null_field);
-  rc = sort_args(codec, checksum_alg, n, src_off, src_len, slice_base, slice_len, slice_checksum, spec, src_base,
-                 dst_base, dst_cap, dst_total, n_records, status);
-  if (rc || !n) return rc;
-  return sort_packed_run(D, codec, checksum_alg, n, src_base, src_off, src_len, slice_base, slice_len, slice_checksum,
-                         spec, dst_base, dst_cap, dst_total, n_records, status, bad_slice, wt);
+  return sort_call(t_device, true, nullptr, codec, checksum_alg, n, src_base, src_off, src_len, slice_base, slice_len,
+                   slice_checksum, rows_spec(key_type, key_off, key_len, null_field), dst_base, dst_cap, dst_total,
+                   n_records, status, bad_slice);
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -2982,58 +2957,6 @@ int b2s_exchange_read_packed(int32_t shuffle_id, int32_t start_reduce, int32_t e
   return 0;
 }
 
-// The sources of an exchange sorted read: the fetched ones compacted in source order with their slices (what
-// decompress_sort_run takes as its blocks), and every source in order.
-struct MixedSources {
-  std::vector<SortSource> src;
-  std::vector<uint64_t> off, len, slice_len, slice_sum;
-  std::vector<uint32_t> slice_base{0};
-};
-
-static int exchange_sort_args(int32_t start_reduce, int32_t end_reduce, const int64_t* map_ids, const uint8_t* cached,
-                              uint32_t codec, uint32_t alg, uint32_t n, const uint8_t* src_base,
-                              const uint64_t* src_off, const uint64_t* src_len, const uint32_t* slice_base,
-                              const uint64_t* slice_len, const uint64_t* slice_checksum, uint32_t record_bytes,
-                              uint32_t key_off, uint32_t key_len, const void* dst_base, uint64_t dst_cap,
-                              const uint64_t* dst_total, const uint64_t* n_records, const int32_t* status,
-                              MixedSources& M) {
-  int rc = reduce_range_args(start_reduce, end_reduce);
-  if (rc) return rc;
-  if (n && (!map_ids || !cached || !status)) return fail(B2S_E_ARG, "null argument%s");
-  M.src.resize(n);
-  for (uint32_t i = 0; i < n; i++) {
-    M.src[i].cached = cached[i] != 0;
-    if (M.src[i].cached) continue;
-    if (!src_off || !src_len) return fail(B2S_E_ARG, "null argument%s");
-    if (alg && (!slice_base || !slice_len || !slice_checksum)) return fail(B2S_E_ARG, "slice arrays required%s");
-    M.src[i].block = (uint32_t)M.off.size();
-    M.off.push_back(src_off[i]);
-    M.len.push_back(src_len[i]);
-    if (alg) {
-      if (slice_base[i + 1] < slice_base[i]) return fail(B2S_E_ARG, "slice_base must be non-decreasing%s");
-      M.slice_len.insert(M.slice_len.end(), slice_len + slice_base[i], slice_len + slice_base[i + 1]);
-      M.slice_sum.insert(M.slice_sum.end(), slice_checksum + slice_base[i], slice_checksum + slice_base[i + 1]);
-      M.slice_base.push_back((uint32_t)M.slice_len.size());
-    }
-  }
-  const uint32_t m = (uint32_t)M.off.size();
-  return sort_args(codec, alg, m, M.off.data(), M.len.data(), M.slice_base.data(), M.slice_len.data(),
-                   M.slice_sum.data(), fixed_spec(record_bytes, key_off, key_len), src_base, dst_base, dst_cap,
-                   dst_total, n_records, status);
-}
-
-// references the cached sources of M on device D and describes them; B2S_E_ARG when a range exceeds an entry
-static int exchange_sort_sources(const ExRefs& refs, int32_t start_reduce, int32_t end_reduce, MixedSources& M) {
-  if (int rc = refs.check_range(end_reduce)) return rc;
-  for (uint32_t i = 0; i < (uint32_t)M.src.size(); i++) {
-    SortSource& s = M.src[i];
-    if (!s.cached) continue;
-    if (refs.entry[i]) s.src = refs.range(i, start_reduce, end_reduce, &s.len);
-    else s.status = B2S_E_NOT_CACHED;
-  }
-  return 0;
-}
-
 int b2s_exchange_read_sort_packed(int32_t shuffle_id, int32_t start_reduce, int32_t end_reduce, const int64_t* map_ids,
                                   const uint8_t* cached, uint32_t codec, uint32_t checksum_alg, uint32_t n,
                                   const uint8_t* src_base, const uint64_t* src_off, const uint64_t* src_len,
@@ -3041,24 +2964,10 @@ int b2s_exchange_read_sort_packed(int32_t shuffle_id, int32_t start_reduce, int3
                                   const uint64_t* slice_checksum, uint32_t record_bytes, uint32_t key_off,
                                   uint32_t key_len, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_total,
                                   uint64_t* n_records, int32_t* status, int32_t* bad_slice) {
-  WallTimer wt;
-  t_timing = b2s_timing{};
-  if (dst_total) *dst_total = 0;
-  if (n_records) *n_records = 0;
-  MixedSources M;
-  int rc = exchange_sort_args(start_reduce, end_reduce, map_ids, cached, codec, checksum_alg, n, src_base, src_off,
-                              src_len, slice_base, slice_len, slice_checksum, record_bytes, key_off, key_len, dst_base,
-                              dst_cap, dst_total, n_records, status, M);
-  if (rc) return rc;
-  if ((rc = exchange_ready())) return rc;
-  Device* D;
-  if ((rc = get_device(t_device, &D)) || !n) return rc;
-  ExRefs refs(D->ordinal, shuffle_id, n, map_ids, cached);
-  if ((rc = exchange_sort_sources(refs, start_reduce, end_reduce, M))) return rc;
-  const uint32_t m = (uint32_t)M.off.size();
-  return sort_packed_run(D, codec, checksum_alg, m, src_base, M.off.data(), M.len.data(), M.slice_base.data(),
-                         M.slice_len.data(), M.slice_sum.data(), fixed_spec(record_bytes, key_off, key_len), dst_base,
-                         dst_cap, dst_total, n_records, status, bad_slice, wt, &M.src);
+  const ExchangeRead x{shuffle_id, start_reduce, end_reduce, map_ids, cached};
+  return sort_call(t_device, true, &x, codec, checksum_alg, n, src_base, src_off, src_len, slice_base, slice_len,
+                   slice_checksum, fixed_spec(record_bytes, key_off, key_len), dst_base, dst_cap, dst_total, n_records,
+                   status, bad_slice);
 }
 
 int b2s_exchange_read_sort_dev(uint32_t dev_index, int32_t shuffle_id, int32_t start_reduce, int32_t end_reduce,
@@ -3068,24 +2977,10 @@ int b2s_exchange_read_sort_dev(uint32_t dev_index, int32_t shuffle_id, int32_t s
                                uint32_t record_bytes, uint32_t key_off, uint32_t key_len, uint8_t* dst_base,
                                uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records, int32_t* status,
                                int32_t* bad_slice) {
-  WallTimer wt;
-  t_timing = b2s_timing{};
-  if (dst_total) *dst_total = 0;
-  if (n_records) *n_records = 0;
-  MixedSources M;
-  int rc = exchange_sort_args(start_reduce, end_reduce, map_ids, cached, codec, checksum_alg, n, src_base, src_off,
-                              src_len, slice_base, slice_len, slice_checksum, record_bytes, key_off, key_len, dst_base,
-                              dst_cap, dst_total, n_records, status, M);
-  if (rc) return rc;
-  if ((rc = exchange_ready())) return rc;
-  Device* D;
-  if ((rc = get_device(dev_index, &D)) || !n) return rc;
-  ExRefs refs(D->ordinal, shuffle_id, n, map_ids, cached);
-  if ((rc = exchange_sort_sources(refs, start_reduce, end_reduce, M))) return rc;
-  const uint32_t m = (uint32_t)M.off.size();
-  return sort_dev_run(D, codec, checksum_alg, m, src_base, M.off.data(), M.len.data(), M.slice_base.data(),
-                      M.slice_len.data(), M.slice_sum.data(), fixed_spec(record_bytes, key_off, key_len), dst_base,
-                      dst_cap, dst_total, n_records, status, bad_slice, wt, &M.src);
+  const ExchangeRead x{shuffle_id, start_reduce, end_reduce, map_ids, cached};
+  return sort_call(dev_index, false, &x, codec, checksum_alg, n, src_base, src_off, src_len, slice_base, slice_len,
+                   slice_checksum, fixed_spec(record_bytes, key_off, key_len), dst_base, dst_cap, dst_total, n_records,
+                   status, bad_slice);
 }
 
 int b2s_decompressed_size_batch(uint32_t codec, uint32_t n, const uint8_t* const* src, const uint64_t* src_len,
