@@ -53,6 +53,16 @@ extern "C" {
 #define B2S_KEY_INT32 1 /* 4 bytes, little-endian two's complement: UnsafeRow's IntegerType / DateType slot */
 #define B2S_KEY_INT64 2 /* 8 bytes, little-endian two's complement: LongType, TimestampType, Decimal(p <= 18) */
 
+/* aggregate ops of the row aggregation (b2s_decompress_aggregate_rows_*), each over an 8-byte slot of the row */
+#define B2S_AGG_SUM_INT64 0   /* wrapping two's-complement sum: Sum(long), Count, Average's count */
+#define B2S_AGG_SUM_FLOAT64 1 /* IEEE double sum: Sum(double), Average's sum */
+#define B2S_AGG_MIN_INT32 2
+#define B2S_AGG_MAX_INT32 3
+#define B2S_AGG_MIN_INT64 4
+#define B2S_AGG_MAX_INT64 5
+#define B2S_AGG_MIN_FLOAT64 6
+#define B2S_AGG_MAX_FLOAT64 7
+
 /* per-block status / call errors.  The Scala shim maps them to the reference's exception types:            */
 #define B2S_OK 0
 #define B2S_E_CORRUPT (-1)       /* IOException("Stream is corrupted")  (LZ4BlockInputStream et al. [U])   */
@@ -253,6 +263,56 @@ int b2s_decompress_sort_rows_dev(uint32_t dev_index, uint32_t codec, uint32_t ch
                                  uint32_t key_type, uint32_t key_off, uint32_t key_len, int32_t null_field,
                                  uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records,
                                  int32_t* status, int32_t* bad_slice);
+
+/* ---- read side, aggregated: verify + decompress + group a reduce task's UnsafeRow records by key and merge ----
+ * The HashAggregateExec(Final) that a grouped aggregation runs on every reducer right after the shuffle read: the rows
+ * are the partial aggregates of the map side, one per map per key, and the call merges them into one row per key.
+ * Blocks, slices, checksums, key_type, key_off, key_len and null_field mean exactly what they mean in
+ * b2s_decompress_sort_rows_packed.  A group is a maximal set of records with equal keys; all null keys form one group.
+ * Aggregates: n_aggs (0..16) of them; aggregate a reads the 8-byte little-endian slot at row offset agg_off[a] with
+ * op agg_op[a] and null bit agg_null_field[a] (-1: never null; else as null_field).  An aggregate is taken over the
+ * group's non-null inputs, in stable order (block order, then order within the block), as one HashAggregateExec
+ * buffer merges them:
+ *   B2S_AGG_SUM_INT64   : 64-bit wrapping sum (non-ANSI Add)
+ *   B2S_AGG_SUM_FLOAT64 : ((0.0 + x1) + x2) + ... in double, left to right, no reassociation, no FMA — bit for bit
+ *                         coalesce(coalesce(sum.left, 0) + sum.right, sum.left); a lone -0.0 gives +0.0
+ *   B2S_AGG_MIN/MAX_INT32   : signed, on the low 4 bytes of the slot; written with the high 4 bytes zero
+ *   B2S_AGG_MIN/MAX_INT64   : signed
+ *   B2S_AGG_MIN/MAX_FLOAT64 : Spark SQL's double order: -0.0 == 0.0, NaN == NaN and above every other value; among
+ *                             equal values the first in stable order is kept with its exact bits (Least / Greatest)
+ * A group with no non-null input for aggregate a gets its null bit set and an all-zero slot (UnsafeRow.setNullAt);
+ * otherwise the null bit is cleared and the slot holds the result.  n_aggs = 0 keeps the first row of every key.
+ * Output: one record per group, back to back, groups in the row sort's order (ascending, nulls first) — again a valid
+ * UnsafeRowSerializer stream.  A group's record is its first record in stable order, byte for byte (size prefix and
+ * variable-length region included) except each aggregate's slot and null bit.  *dst_total = output bytes, *n_records =
+ * input records, *n_groups = output records.  The output is never longer than the decoded input, so a dst_cap of at
+ * least the decoded bytes never gets B2S_E_DST_TOO_SMALL.
+ * Per block, B2S_E_CORRUPT for every framing rule of b2s_decompress_sort_rows_packed and when a row is shorter than an
+ * aggregate slot (agg_off[a] + 8) or an aggregate's null word.  Checksums, "nothing is written when a block fails"
+ * (*n_records = *n_groups = 0, the call returns 0), B2S_E_NOMEM, codec NONE, the read lane and the 1 GiB buffer trim
+ * are as in b2s_decompress_sort_*.  dst_cap below the output bytes -> B2S_E_DST_TOO_SMALL with *dst_total = the bytes
+ * needed.
+ * Errors -> B2S_E_ARG: those of b2s_decompress_sort_rows_packed; n_aggs > 16; an unknown op; agg_null_field[a] < -1;
+ * NULL agg arrays with n_aggs > 0; an aggregate slot that overlaps another slot, the key bytes, or an 8-byte null word
+ * that the key or an aggregate uses.
+ * Timing (b2s_last_timing): kernel_ms = the whole call; top_kernel_ms = framing + keys + radix + aggregation;
+ * dominant_ms / dominant_launches = the aggregation step alone, from the sorted indices to the written output. */
+int b2s_decompress_aggregate_rows_packed(uint32_t codec, uint32_t checksum_alg, uint32_t n, const uint8_t* src_base,
+                                         const uint64_t* src_off, const uint64_t* src_len, const uint32_t* slice_base,
+                                         const uint64_t* slice_len, const uint64_t* slice_checksum, uint32_t key_type,
+                                         uint32_t key_off, uint32_t key_len, int32_t null_field, uint32_t n_aggs,
+                                         const uint32_t* agg_op, const uint32_t* agg_off, const int32_t* agg_null_field,
+                                         uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records,
+                                         uint64_t* n_groups, int32_t* status, int32_t* bad_slice);
+/* same, with src_base / dst_base in device memory of dev_index; the descriptor and aggregate arrays stay host arrays */
+int b2s_decompress_aggregate_rows_dev(uint32_t dev_index, uint32_t codec, uint32_t checksum_alg, uint32_t n,
+                                      const uint8_t* src_base, const uint64_t* src_off, const uint64_t* src_len,
+                                      const uint32_t* slice_base, const uint64_t* slice_len,
+                                      const uint64_t* slice_checksum, uint32_t key_type, uint32_t key_off,
+                                      uint32_t key_len, int32_t null_field, uint32_t n_aggs, const uint32_t* agg_op,
+                                      const uint32_t* agg_off, const int32_t* agg_null_field, uint8_t* dst_base,
+                                      uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records, uint64_t* n_groups,
+                                      int32_t* status, int32_t* bad_slice);
 
 /* ---- exchange cache: map outputs kept resident in HBM for reducers on the same device ----
  * (docs/f4_gpu_resident_exchange.md steps 2 and 3, local half.)  The serialized writer's partition step already leaves

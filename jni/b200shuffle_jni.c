@@ -237,13 +237,20 @@ JNIEXPORT jint JNICALL J(decompressPacked)(JNIEnv* e, jclass c, jint codec, jint
  *      Java array is held in a critical region while the GPU works. ---- */
 /* mapIds (NULL: a plain decompressSortPacked): long[n] and cached: int[n] make it an exchange-cache read of the
  * partitions [startReduce, endReduce) of shuffleId.  rows: a row sort (decompressSortRowsPacked) of UnsafeRow records
- * by the key keyType at keyOff (recordBytes unused, mapIds NULL) */
+ * by the key keyType at keyOff (recordBytes unused, mapIds NULL).  aggOp (rows only; NULL otherwise): a row
+ * aggregation (decompressAggregateRowsPacked) with int[nAggs] aggOp / aggOff / aggNullField, and meta long[3] =
+ * {dst_total, n_records, n_groups} */
 static jint sort_packed(JNIEnv* e, jint shuffleId, jint startReduce, jint endReduce, jlongArray mapIds,
                         jintArray cached, jint codec, jint alg, jint n, jlong src, jlongArray off, jlongArray len,
                         jintArray sliceBase, jlongArray sliceLen, jlongArray sliceChecksum, jint recordBytes,
-                        int rows, jint keyType, jint keyOff, jint keyLen, jint nullField, jlong dst, jlong dstCap,
-                        jlongArray meta, jintArray status, jintArray badSlice) {
-  if (n < 0 || !meta || (*e)->GetArrayLength(e, meta) < 2) return B2S_E_ARG;
+                        int rows, jint keyType, jint keyOff, jint keyLen, jint nullField, jint nAggs, jintArray aggOp,
+                        jintArray aggOff, jintArray aggNullField, jlong dst, jlong dstCap, jlongArray meta,
+                        jintArray status, jintArray badSlice) {
+  const jsize n_meta = aggOp ? 3 : 2;
+  if (n < 0 || !meta || (*e)->GetArrayLength(e, meta) < n_meta) return B2S_E_ARG;
+  if (aggOp && (nAggs < 0 || nAggs > 16 || !aggOff || !aggNullField || (*e)->GetArrayLength(e, aggOp) < nAggs ||
+                (*e)->GetArrayLength(e, aggOff) < nAggs || (*e)->GetArrayLength(e, aggNullField) < nAggs))
+    return B2S_E_ARG;
   if (mapIds && n > 0 && (!cached || (*e)->GetArrayLength(e, mapIds) < n || (*e)->GetArrayLength(e, cached) < n))
     return B2S_E_ARG;
   if (n > 0 && (!off || !len || !status || (*e)->GetArrayLength(e, off) < n || (*e)->GetArrayLength(e, len) < n ||
@@ -281,10 +288,23 @@ static jint sort_packed(JNIEnv* e, jint shuffleId, jint startReduce, jint endRed
       (*e)->GetLongArrayRegion(e, sliceChecksum, 0, ns, (jlong*)(sl + ns));
     }
   }
-  uint64_t total = 0, nrec = 0;
+  uint64_t total = 0, nrec = 0, ngrp = 0;
   if (rc == 0) {
     const size_t ns = with_slices ? (size_t)sb[n] : 0;
-    if (rows)
+    if (aggOp) {
+      uint32_t aop[16], aoff[16];
+      int32_t anf[16];
+      if (nAggs > 0) {
+        (*e)->GetIntArrayRegion(e, aggOp, 0, nAggs, (jint*)aop);
+        (*e)->GetIntArrayRegion(e, aggOff, 0, nAggs, (jint*)aoff);
+        (*e)->GetIntArrayRegion(e, aggNullField, 0, nAggs, (jint*)anf);
+      }
+      rc = b2s_decompress_aggregate_rows_packed((uint32_t)codec, (uint32_t)alg, (uint32_t)n, PTR(const uint8_t, src),
+                                                blk, blk + N, with_slices ? sb : 0, with_slices ? sl : 0,
+                                                with_slices ? sl + ns : 0, (uint32_t)keyType, (uint32_t)keyOff,
+                                                (uint32_t)keyLen, (int32_t)nullField, (uint32_t)nAggs, aop, aoff, anf,
+                                                PTR(uint8_t, dst), (uint64_t)dstCap, &total, &nrec, &ngrp, st, st + N);
+    } else if (rows)
       rc = b2s_decompress_sort_rows_packed((uint32_t)codec, (uint32_t)alg, (uint32_t)n, PTR(const uint8_t, src), blk,
                                            blk + N, with_slices ? sb : 0, with_slices ? sl : 0,
                                            with_slices ? sl + ns : 0, (uint32_t)keyType, (uint32_t)keyOff,
@@ -306,8 +326,8 @@ static jint sort_packed(JNIEnv* e, jint shuffleId, jint startReduce, jint endRed
       (*e)->SetIntArrayRegion(e, status, 0, n, (const jint*)st);
       if (badSlice) (*e)->SetIntArrayRegion(e, badSlice, 0, n, (const jint*)(st + N));
     }
-    const jlong m[2] = {(jlong)total, (jlong)nrec};
-    (*e)->SetLongArrayRegion(e, meta, 0, 2, m);
+    const jlong m[3] = {(jlong)total, (jlong)nrec, (jlong)ngrp};
+    (*e)->SetLongArrayRegion(e, meta, 0, n_meta, m);
   }
   free(hit);
   free(ids);
@@ -324,7 +344,7 @@ JNIEXPORT jint JNICALL J(decompressSortPacked)(JNIEnv* e, jclass c, jint codec, 
                                                jintArray badSlice) {
   (void)c;
   return sort_packed(e, 0, 0, 0, 0, 0, codec, alg, n, src, off, len, sliceBase, sliceLen, sliceChecksum, recordBytes,
-                     0, 0, keyOff, keyLen, -1, dst, dstCap, meta, status, badSlice);
+                     0, 0, keyOff, keyLen, -1, 0, 0, 0, 0, dst, dstCap, meta, status, badSlice);
 }
 
 /* ---- read side, row-sorted (a Spark SQL exchange read followed by a SortExec, INTEGRATION.md §3g): verify, decode and
@@ -337,7 +357,25 @@ JNIEXPORT jint JNICALL J(decompressSortRowsPacked)(JNIEnv* e, jclass c, jint cod
                                                    jlongArray meta, jintArray status, jintArray badSlice) {
   (void)c;
   return sort_packed(e, 0, 0, 0, 0, 0, codec, alg, n, src, off, len, sliceBase, sliceLen, sliceChecksum, 0, 1, keyType,
-                     keyOff, keyLen, nullField, dst, dstCap, meta, status, badSlice);
+                     keyOff, keyLen, nullField, 0, 0, 0, 0, dst, dstCap, meta, status, badSlice);
+}
+
+/* ---- read side, aggregated (a Spark SQL exchange read followed by a HashAggregateExec(Final), INTEGRATION.md §3h):
+ *      verify, decode, group the task's UnsafeRow records by one typed key and merge nAggs aggregates (aggOp /
+ *      aggOff / aggNullField: int[nAggs], B2S_AGG_* ops).  meta: long[3] = {dst_total, n_records, n_groups}; other
+ *      arrays as decompressSortRowsPacked. ---- */
+JNIEXPORT jint JNICALL J(decompressAggregateRowsPacked)(JNIEnv* e, jclass c, jint codec, jint alg, jint n, jlong src,
+                                                        jlongArray off, jlongArray len, jintArray sliceBase,
+                                                        jlongArray sliceLen, jlongArray sliceChecksum, jint keyType,
+                                                        jint keyOff, jint keyLen, jint nullField, jint nAggs,
+                                                        jintArray aggOp, jintArray aggOff, jintArray aggNullField,
+                                                        jlong dst, jlong dstCap, jlongArray meta, jintArray status,
+                                                        jintArray badSlice) {
+  (void)c;
+  if (!aggOp) return B2S_E_ARG;
+  return sort_packed(e, 0, 0, 0, 0, 0, codec, alg, n, src, off, len, sliceBase, sliceLen, sliceChecksum, 0, 1, keyType,
+                     keyOff, keyLen, nullField, nAggs, aggOp, aggOff, aggNullField, dst, dstCap, meta, status,
+                     badSlice);
 }
 
 /* ---- exchange cache (INTEGRATION.md §3f): map outputs kept in HBM for reducers on the same device ---- */
@@ -411,8 +449,8 @@ JNIEXPORT jint JNICALL J(exchangeReadSortPacked)(JNIEnv* e, jclass c, jint shuff
   (void)c;
   if (!mapIds) return B2S_E_ARG;
   return sort_packed(e, shuffleId, startReduce, endReduce, mapIds, cached, codec, alg, n, src, off, len, sliceBase,
-                     sliceLen, sliceChecksum, recordBytes, 0, 0, keyOff, keyLen, -1, dst, dstCap, meta, status,
-                     badSlice);
+                     sliceLen, sliceChecksum, recordBytes, 0, 0, keyOff, keyLen, -1, 0, 0, 0, 0, dst, dstCap, meta,
+                     status, badSlice);
 }
 
 /* decoded size of each of n compressed streams laid out in one arena (sizes the destination of decompressPacked) */

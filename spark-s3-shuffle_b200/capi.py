@@ -13,6 +13,9 @@ from . import _build
 CODEC_NONE, CODEC_LZ4BLOCK, CODEC_SNAPPY_XERIAL, CODEC_ZSTD = 0, 1, 2, 3
 CHECKSUM_NONE, CHECKSUM_ADLER32, CHECKSUM_CRC32, CHECKSUM_CRC32C = 0, 1, 2, 3
 KEY_BYTES, KEY_INT32, KEY_INT64 = 0, 1, 2  # key types of the row sort (decompress_sort_rows_*)
+# aggregate ops of the row aggregation (decompress_aggregate_rows_*)
+(AGG_SUM_INT64, AGG_SUM_FLOAT64, AGG_MIN_INT32, AGG_MAX_INT32, AGG_MIN_INT64, AGG_MAX_INT64, AGG_MIN_FLOAT64,
+ AGG_MAX_FLOAT64) = range(8)
 OK, E_CORRUPT, E_CHECKSUM, E_DST_TOO_SMALL, E_UNSUPPORTED, E_ARG, E_CUDA, E_NOT_INIT, E_NOMEM, E_NOT_CACHED = (
     0, -1, -2, -3, -4, -5, -6, -7, -8, -9)
 NOT_RESIDENT = 2**64 - 1  # b2s_exchange_lookup's length of a map output that is not resident
@@ -77,6 +80,12 @@ PROTOTYPES = [
     ("b2s_decompress_sort_rows_dev", C.c_int,
      [_u32, _u32, _u32, _u32, _vp, _u64p, _u64p, _u32p, _u64p, _u64p, _u32, _u32, _u32, _i32, _vp, _u64, _u64p, _u64p,
       _i32p, _i32p]),
+    ("b2s_decompress_aggregate_rows_packed", C.c_int,
+     [_u32, _u32, _u32, _u8p, _u64p, _u64p, _u32p, _u64p, _u64p, _u32, _u32, _u32, _i32, _u32, _u32p, _u32p, _i32p,
+      _u8p, _u64, _u64p, _u64p, _u64p, _i32p, _i32p]),
+    ("b2s_decompress_aggregate_rows_dev", C.c_int,
+     [_u32, _u32, _u32, _u32, _vp, _u64p, _u64p, _u32p, _u64p, _u64p, _u32, _u32, _u32, _i32, _u32, _u32p, _u32p, _i32p,
+      _vp, _u64, _u64p, _u64p, _u64p, _i32p, _i32p]),
     ("b2s_exchange_set_budget", C.c_int, [_u32, _u64]),
     ("b2s_partition_compress_cached_packed", C.c_int,
      [_i32, C.c_int64, _u32, _i32, _u32, _u32, _u32, _u64, _u8p, _u64, _u32p, _u32p, _u8p, _u64, _u64p, _u64p, _u64p,
@@ -407,6 +416,39 @@ def decompress_sort_rows_packed(codec, src, off, length, dst, key_type, key_off,
     return dict(total=total.value, n_records=nrec.value, status=st[:n], bad_slice=bad[:n])
 
 
+def _agg_arrays(aggs):
+    """aggs = [(op, off, null_field), ...] -> (n, op, off, null_field) arrays"""
+    aggs = list(aggs)
+    op = np.array([a[0] for a in aggs] or [0], dtype=np.uint32)
+    off = np.array([a[1] for a in aggs] or [0], dtype=np.uint32)
+    nf = np.array([a[2] for a in aggs] or [0], dtype=np.int32)
+    return len(aggs), op, off, nf
+
+
+def decompress_aggregate_rows_packed(codec, src, off, length, dst, key_type, key_off, key_len, null_field=-1, aggs=(),
+                                     checksum_alg=CHECKSUM_NONE, slice_base=None, slice_len=None, slice_checksum=None):
+    """Verifies and decodes a reduce task's blocks of UnsafeRow records, groups them by the typed key (as
+    decompress_sort_rows_packed orders them) and merges every aggregate (op AGG_*, 8-byte slot at row offset off,
+    null bit null_field or -1) over each group into one row per group in dst.
+    -> dict(total, n_records, n_groups, status, bad_slice)"""
+    src, dst = _as_u8(src), _as_u8(dst)
+    off = np.ascontiguousarray(off, dtype=np.uint64)
+    length = np.ascontiguousarray(length, dtype=np.uint64)
+    n = off.size
+    sb, sl, sc = _sort_slices(checksum_alg, slice_base, slice_len, slice_checksum)
+    na, aop, aoff, anf = _agg_arrays(aggs)
+    st = np.zeros(max(n, 1), dtype=np.int32)
+    bad = np.zeros(max(n, 1), dtype=np.int32)
+    total, nrec, ngrp = _u64(0), _u64(0), _u64(0)
+    _check(load().b2s_decompress_aggregate_rows_packed(codec, checksum_alg, n, _ptr(src), _ptr(off), _ptr(length),
+                                                       _ptr(sb), _ptr(sl), _ptr(sc), key_type, key_off, key_len,
+                                                       null_field, na, _ptr(aop), _ptr(aoff), _ptr(anf), _ptr(dst),
+                                                       dst.size, C.addressof(total), C.addressof(nrec),
+                                                       C.addressof(ngrp), _ptr(st), _ptr(bad)),
+           "b2s_decompress_aggregate_rows_packed")
+    return dict(total=total.value, n_records=nrec.value, n_groups=ngrp.value, status=st[:n], bad_slice=bad[:n])
+
+
 # ---------------------------------------------------------------------------------------------------------------
 # device-resident API (bench.py roofline leg); d_* are raw device addresses (ints)
 # ---------------------------------------------------------------------------------------------------------------
@@ -505,6 +547,26 @@ def decompress_sort_rows_dev(codec, d_src, off, length, d_dst, dst_cap, key_type
                                                dst_cap, C.addressof(total), C.addressof(nrec), _ptr(st), _ptr(bad)),
            "b2s_decompress_sort_rows_dev")
     return dict(total=total.value, n_records=nrec.value, status=st[:n], bad_slice=bad[:n])
+
+
+def decompress_aggregate_rows_dev(codec, d_src, off, length, d_dst, dst_cap, key_type, key_off, key_len,
+                                  null_field=-1, aggs=(), checksum_alg=CHECKSUM_NONE, slice_base=None, slice_len=None,
+                                  slice_checksum=None, dev=0):
+    """decompress_aggregate_rows_packed on device-resident blocks (d_src) into a device arena (d_dst)"""
+    off = np.ascontiguousarray(off, dtype=np.uint64)
+    length = np.ascontiguousarray(length, dtype=np.uint64)
+    n = off.size
+    sb, sl, sc = _sort_slices(checksum_alg, slice_base, slice_len, slice_checksum)
+    na, aop, aoff, anf = _agg_arrays(aggs)
+    st = np.zeros(max(n, 1), dtype=np.int32)
+    bad = np.zeros(max(n, 1), dtype=np.int32)
+    total, nrec, ngrp = _u64(0), _u64(0), _u64(0)
+    _check(load().b2s_decompress_aggregate_rows_dev(dev, codec, checksum_alg, n, d_src, _ptr(off), _ptr(length),
+                                                    _ptr(sb), _ptr(sl), _ptr(sc), key_type, key_off, key_len,
+                                                    null_field, na, _ptr(aop), _ptr(aoff), _ptr(anf), d_dst, dst_cap,
+                                                    C.addressof(total), C.addressof(nrec), C.addressof(ngrp), _ptr(st),
+                                                    _ptr(bad)), "b2s_decompress_aggregate_rows_dev")
+    return dict(total=total.value, n_records=nrec.value, n_groups=ngrp.value, status=st[:n], bad_slice=bad[:n])
 
 
 def partition_compress_dev(codec, d_records, rec_bytes, d_rec_len, d_rec_part, n_records, num_partitions, d_dst,

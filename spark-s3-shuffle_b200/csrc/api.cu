@@ -230,6 +230,7 @@ struct Slot {
   cudaEvent_t ev_h0 = nullptr, ev_h1 = nullptr, ev_d0 = nullptr, ev_d1 = nullptr;  // copies
   cudaEvent_t ev_p0 = nullptr, ev_p1 = nullptr;            // partition step (b2s_partition_compress_*)
   cudaEvent_t ev_f[4] = {nullptr, nullptr, nullptr, nullptr};  // row framing: walk + count, emit (sort_rows)
+  cudaEvent_t ev_g[2] = {nullptr, nullptr};                    // grouping + merge (aggregate_rows)
   DevBuf meta, scratch, desc, src, dst, zmeta;
   DevBuf pws, parena;  // partition workspace (sort keys, offsets) and the partitioned arena in front of compression
   DevBuf xpieces;      // the copy pieces of an exchange-cache read (exchange.cu)
@@ -252,10 +253,10 @@ struct Slot {
   }
   // the fixed events, created by create() and destroyed by release(); the first kUntimed only order the two streams
   static constexpr int kUntimed = 5;
-  std::array<cudaEvent_t*, 21> events() {
-    return {&ev_fork, &ev_match[0], &ev_match[1], &ev_free[0], &ev_free[1], &ev_a,    &ev_b,
-            &ev_k0,   &ev_k1,       &ev_t0,       &ev_t1,      &ev_h0,      &ev_h1,   &ev_d0,
-            &ev_d1,   &ev_p0,       &ev_p1,       &ev_f[0],    &ev_f[1],    &ev_f[2], &ev_f[3]};
+  std::array<cudaEvent_t*, 23> events() {
+    return {&ev_fork, &ev_match[0], &ev_match[1], &ev_free[0], &ev_free[1], &ev_a,    &ev_b,    &ev_k0,
+            &ev_k1,   &ev_t0,       &ev_t1,       &ev_h0,      &ev_h1,      &ev_d0,   &ev_d1,   &ev_p0,
+            &ev_p1,   &ev_f[0],     &ev_f[1],     &ev_f[2],    &ev_f[3],    &ev_g[0], &ev_g[1]};
   }
   int create(int prio) {
     CU(cudaStreamCreateWithPriority(&st, cudaStreamNonBlocking, prio));
@@ -2302,13 +2303,19 @@ int b2s_decompress_packed(uint32_t codec, uint32_t checksum_alg, uint32_t n, con
 // read side, key-sorted: verify + decode a reduce task's blocks, then sort its records by key
 // ------------------------------------------------------------------------------------------------------------
 // What the records of a sort call are: fixed-size (record_bytes long, an unsigned byte key) or length-prefixed UnsafeRow
-// records (rows: [size: int32 big-endian][row], a typed key at key_off in the row, null bit null_field)
+// records (rows: [size: int32 big-endian][row], a typed key at key_off in the row, null bit null_field).  aggregate:
+// rows grouped by the key and merged (b2s_decompress_aggregate_rows_*: the caller's n_aggs aggregates), not sorted.
 struct RecordSpec {
   bool is_rows = false;
   uint32_t record_bytes = 0;
   uint32_t key_type = B2S_KEY_BYTES;
   uint32_t key_off = 0, key_len = 0;
   int32_t null_field = -1;
+  bool aggregate = false;
+  uint32_t n_aggs = 0;
+  const uint32_t* agg_op = nullptr;
+  const uint32_t* agg_off = nullptr;
+  const int32_t* agg_null_field = nullptr;
   bool rows() const { return is_rows; }
 };
 static RecordSpec fixed_spec(uint32_t record_bytes, uint32_t key_off, uint32_t key_len) {
@@ -2328,6 +2335,57 @@ static RecordSpec rows_spec(uint32_t key_type, uint32_t key_off, uint32_t key_le
   return r;
 }
 
+static bool overlaps(uint64_t a0, uint64_t a1, uint64_t b0, uint64_t b1) { return a0 < b1 && b0 < a1; }
+// the row offset of field f's 8-byte null word
+static uint64_t null_word(int32_t f) { return 8ull * (uint32_t)(f >> 6); }
+
+static RecordSpec aggregate_spec(uint32_t key_type, uint32_t key_off, uint32_t key_len, int32_t null_field,
+                                 uint32_t n_aggs, const uint32_t* op, const uint32_t* off, const int32_t* agg_null) {
+  RecordSpec r = rows_spec(key_type, key_off, key_len, null_field);
+  r.aggregate = true;
+  r.n_aggs = n_aggs;
+  r.agg_op = op;
+  r.agg_off = off;
+  r.agg_null_field = agg_null;
+  return r;
+}
+
+// each aggregate is a known op on 8 bytes that touch no other slot, the key, or a null word in use
+static int agg_args(const RecordSpec& spec) {
+  const uint32_t n = spec.n_aggs;
+  if (n > kMaxAggs) return fail(B2S_E_ARG, "n_aggs must be at most 16%s");
+  if (n && (!spec.agg_op || !spec.agg_off || !spec.agg_null_field)) return fail(B2S_E_ARG, "null argument%s");
+  std::vector<std::pair<uint64_t, uint64_t>> words;  // the null words the key and the aggregates use
+  if (spec.null_field >= 0) words.push_back({null_word(spec.null_field), null_word(spec.null_field) + 8});
+  for (uint32_t k = 0; k < n; k++) {
+    if (spec.agg_op[k] > B2S_AGG_MAX_FLOAT64) return fail(B2S_E_ARG, "unknown aggregate op%s");
+    const int32_t f = spec.agg_null_field[k];
+    if (f < -1) return fail(B2S_E_ARG, "agg_null_field must be -1 or a field ordinal%s");
+    if (f >= 0) words.push_back({null_word(f), null_word(f) + 8});
+  }
+  for (uint32_t k = 0; k < n; k++) {
+    const uint64_t s0 = spec.agg_off[k], s1 = s0 + 8;
+    if (overlaps(s0, s1, spec.key_off, (uint64_t)spec.key_off + spec.key_len))
+      return fail(B2S_E_ARG, "an aggregate slot overlaps the key%s");
+    for (uint32_t m = 0; m < k; m++)
+      if (overlaps(s0, s1, spec.agg_off[m], (uint64_t)spec.agg_off[m] + 8))
+        return fail(B2S_E_ARG, "aggregate slots overlap%s");
+    for (const auto& w : words)
+      if (overlaps(s0, s1, w.first, w.second)) return fail(B2S_E_ARG, "an aggregate slot overlaps a null word%s");
+  }
+  return 0;
+}
+
+// the bytes a row must hold for the aggregates: every slot and every aggregate null word (0 without aggregates)
+static uint64_t agg_min_row(const RecordSpec& spec) {
+  uint64_t m = 0;
+  for (uint32_t k = 0; k < spec.n_aggs; k++) {
+    m = std::max<uint64_t>(m, (uint64_t)spec.agg_off[k] + 8);
+    if (spec.agg_null_field[k] >= 0) m = std::max<uint64_t>(m, null_word(spec.agg_null_field[k]) + 8);
+  }
+  return m;
+}
+
 static int sort_args(uint32_t codec, uint32_t alg, uint32_t n, const uint64_t* src_off, const uint64_t* src_len,
                      const uint32_t* slice_base, const uint64_t* slice_len, const uint64_t* slice_checksum,
                      const RecordSpec& spec, const void* src_base, const void* dst_base, uint64_t dst_cap,
@@ -2342,6 +2400,8 @@ static int sort_args(uint32_t codec, uint32_t alg, uint32_t n, const uint64_t* s
     if (spec.key_type == B2S_KEY_INT32 && key_len != 4) return fail(B2S_E_ARG, "key_len of an INT32 key must be 4%s");
     if (spec.key_type == B2S_KEY_INT64 && key_len != 8) return fail(B2S_E_ARG, "key_len of an INT64 key must be 8%s");
     if (spec.null_field < -1) return fail(B2S_E_ARG, "null_field must be -1 or a field ordinal%s");
+    if (spec.aggregate)
+      if (int rc = agg_args(spec)) return rc;
   } else {
     if (spec.record_bytes == 0) return fail(B2S_E_ARG, "record_bytes must be at least 1%s");
     if (key_len < 1 || key_len > 16) return fail(B2S_E_ARG, "key_len must be in [1, 16]%s");
@@ -2386,6 +2446,46 @@ struct SortSource {
   uint32_t block = 0;
 };
 
+// The end of an aggregation (b2s_decompress_aggregate_rows_*), from the sorted indices idx of the records: grouping,
+// one readback of the group count and output bytes (which checks out_cap), the heads' gather and the merge into
+// d_out.  *total = output bytes.  The dominant step is this one.
+static int aggregate_rows_tail(Slot& S, const RecordSpec& spec, const uint8_t* arena, uint64_t records,
+                               const uint32_t* idx, uint8_t* ws, uint8_t* aws, uint8_t* d_out, uint64_t out_cap,
+                               uint64_t* total, uint64_t* n_rec, uint64_t* n_groups, uint64_t* launches) {
+  cudaStream_t st = S.st;
+  const uint32_t key_bytes = rows_key_bytes(spec.key_len, spec.null_field);
+  AggSpec agg;
+  agg.n = spec.n_aggs;
+  for (uint32_t k = 0; k < agg.n; k++) {
+    agg.op[k] = spec.agg_op[k];
+    agg.off[k] = spec.agg_off[k];
+    agg.null_field[k] = spec.agg_null_field[k];
+  }
+  const uint64_t agg_launches = *launches;
+  uint64_t rb[2] = {0, 0};  // groups, output bytes
+  CU(cudaEventRecord(S.ev_g[0], st));
+  if (records) {
+    launch_rows_group(arena, records, idx, key_bytes, agg, ws, aws, st, launches);
+    CU(cudaMemcpyAsync(rb, rows_aggregate_readback(aws, records, agg.n), sizeof rb, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    CU(cudaGetLastError());
+  }
+  *total = rb[1];
+  if (rb[1] > out_cap)
+    return fail(B2S_E_DST_TOO_SMALL, "dst_cap is below the %s output bytes", std::to_string(rb[1]).c_str());
+  launch_rows_aggregate(arena, records, rb[0], key_bytes, agg.n, ws, aws, d_out, st, launches);
+  CU(cudaEventRecord(S.ev_g[1], st));
+  CU(cudaEventRecord(S.ev_p1, st));
+  CU(cudaStreamSynchronize(st));
+  CU(cudaGetLastError());
+  S.dom_used = 0;
+  t_timing.dominant_ms = ms_between(S.ev_g[0], S.ev_g[1]);
+  t_timing.dominant_launches = *launches - agg_launches;
+  *n_rec = records;
+  if (n_groups) *n_groups = rb[0];
+  return 0;
+}
+
 // The whole reduce task on the device: compressed blocks at d_src + src_dev_off[i] (src_contiguous: back to back from
 // d_src in block order, no gaps).  Phase A verifies the slices and sizes every block; a failed block, or (fixed-size
 // records) a decoded length that is not a multiple of record_bytes, ends the call with status[] set and *n_rec = 0
@@ -2401,8 +2501,8 @@ static int decompress_sort_run(Device* D, Slot& S, uint32_t codec, uint32_t alg,
                                const uint64_t* src_dev_off, const uint64_t* src_len, bool src_contiguous,
                                const uint32_t* slice_base, const uint64_t* slice_len, const uint64_t* slice_sum,
                                const RecordSpec& spec, uint8_t** d_sorted, uint64_t out_cap, uint64_t* total,
-                               uint64_t* n_rec, int32_t* status, int32_t* bad_slice, uint64_t* launches,
-                               const std::vector<SortSource>* mix = nullptr) {
+                               uint64_t* n_rec, uint64_t* n_groups, int32_t* status, int32_t* bad_slice,
+                               uint64_t* launches, const std::vector<SortSource>* mix = nullptr) {
   cudaStream_t st = S.st;
   DecompressJob J;
   int rc;
@@ -2474,7 +2574,7 @@ static int decompress_sort_run(Device* D, Slot& S, uint32_t codec, uint32_t alg,
   }
   if (!spec.rows() && *total / spec.record_bytes > 0xffffffffull)
     return fail(B2S_E_ARG, "more than 2^32 - 1 records in one call (%s bytes)", std::to_string(*total).c_str());
-  if (*total > out_cap) {
+  if (!spec.aggregate && *total > out_cap) {  // an aggregation's output is sized once the groups are known
     report();
     return fail(B2S_E_DST_TOO_SMALL, "dst_cap is below the %s decoded bytes", std::to_string(*total).c_str());
   }
@@ -2554,7 +2654,8 @@ static int decompress_sort_run(Device* D, Slot& S, uint32_t codec, uint32_t alg,
   uint64_t frame_launches = *launches;
   CU(cudaEventRecord(S.ev_p0, st));
   CU(cudaEventRecord(S.ev_f[0], st));
-  launch_rows_frame(arena, *total, place.data(), length.data(), n_src, min_key, min_null, fws, st, launches);
+  launch_rows_frame(arena, *total, place.data(), length.data(), n_src, min_key, min_null, agg_min_row(spec), fws, st,
+                    launches);
   CU(cudaEventRecord(S.ev_f[1], st));
   std::vector<uint64_t> rb(n_src + 1);
   CU(cudaMemcpyAsync(rb.data(), rows_frame_readback(fws, *total, n_src), rows_frame_readback_bytes(n_src),
@@ -2568,7 +2669,8 @@ static int decompress_sort_run(Device* D, Slot& S, uint32_t codec, uint32_t alg,
     if (!failed) {
       static const char* const why[] = {"", "the block ends inside a size prefix", "the size is negative",
                                         "the record runs past the block end", "the row is shorter than key_off + key_len",
-                                        "the row does not hold the null-bit word"};
+                                        "the row does not hold the null-bit word",
+                                        "the row is shorter than an aggregate slot"};
       snprintf(msg, sizeof msg, "%s %u: bad row record at byte %llu: %s", cached(i) ? "cached source" : "block", i,
                (unsigned long long)(v & ((1ull << 61) - 1)), why[v >> 61]);
       fail(B2S_E_CORRUPT, "%s", msg);
@@ -2587,13 +2689,19 @@ static int decompress_sort_run(Device* D, Slot& S, uint32_t codec, uint32_t alg,
   if (records > 0xffffffffull)
     return fail(B2S_E_ARG, "more than 2^32 - 1 records in one call (%s records)", std::to_string(records).c_str());
   const uint32_t key_bytes = rows_key_bytes(spec.key_len, spec.null_field);
-  if (records && (rc = S.pws.ensure(rows_sort_ws_bytes(records, key_bytes)))) return rc;
+  const size_t sort_ws = rows_sort_ws_bytes(records, key_bytes);
+  const size_t agg_ws = spec.aggregate ? rows_aggregate_ws_bytes(records, spec.n_aggs) : 0;
+  if (records && (rc = S.pws.ensure(sort_ws + agg_ws))) return rc;
+  uint8_t* ws = (uint8_t*)S.pws.p;
   CU(cudaEventRecord(S.ev_f[2], st));
-  launch_rows_emit(arena, *total, n_src, fws, records, key_bytes, (uint8_t*)S.pws.p, st, launches);
+  launch_rows_emit(arena, *total, n_src, fws, records, key_bytes, ws, st, launches);
   CU(cudaEventRecord(S.ev_f[3], st));
   frame_launches = *launches - frame_launches;
-  launch_rows_sort(arena, records, spec.key_type, spec.key_off, spec.key_len, spec.null_field, (uint8_t*)S.pws.p,
-                   *d_sorted, st, launches);
+  const uint32_t* idx = launch_rows_order(arena, records, spec.key_type, spec.key_off, spec.key_len, spec.null_field,
+                                          ws, st, launches);
+  if (spec.aggregate) return aggregate_rows_tail(S, spec, arena, records, idx, ws, ws + sort_ws, *d_sorted, out_cap,
+                                                 total, n_rec, n_groups, launches);
+  launch_rows_gather(arena, records, key_bytes, idx, ws, *d_sorted, st, launches);
   CU(cudaEventRecord(S.ev_p1, st));
   CU(cudaStreamSynchronize(st));
   CU(cudaGetLastError());
@@ -2616,7 +2724,7 @@ static int sort_dev_run(Device* D, uint32_t codec, uint32_t alg, uint32_t n, con
                         const uint64_t* src_off, const uint64_t* src_len, const uint32_t* slice_base,
                         const uint64_t* slice_len, const uint64_t* slice_checksum, const RecordSpec& spec,
                         uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records,
-                        int32_t* status, int32_t* bad_slice, const WallTimer& wt,
+                        uint64_t* n_groups, int32_t* status, int32_t* bad_slice, const WallTimer& wt,
                         const std::vector<SortSource>* mix) {
   Lane& Ln = D->lane[kLaneRead];
   std::lock_guard<std::mutex> lk(Ln.mtx);
@@ -2626,8 +2734,8 @@ static int sort_dev_run(Device* D, uint32_t codec, uint32_t alg, uint32_t n, con
   for (uint32_t i = 0; i < n; i++) srcb += src_len[i];
   uint8_t* out = dst_base;
   int rc = decompress_sort_run(D, S, codec, alg, n, src_base, src_off, src_len, false, slice_base, slice_len,
-                               slice_checksum, spec, &out, dst_cap, dst_total, n_records, status, bad_slice,
-                               &launches, mix);
+                               slice_checksum, spec, &out, dst_cap, dst_total, n_records, n_groups, status,
+                               bad_slice, &launches, mix);
   if (rc) return rc;
   end_timing(wt, launches, CallBytes{srcb, *dst_total, 0, 0}, &S);
   sort_kernel_times(S);
@@ -2639,7 +2747,7 @@ static int sort_packed_run(Device* D, uint32_t codec, uint32_t alg, uint32_t n, 
                            const uint64_t* src_off, const uint64_t* src_len, const uint32_t* slice_base,
                            const uint64_t* slice_len, const uint64_t* slice_checksum, const RecordSpec& spec,
                            uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records,
-                           int32_t* status, int32_t* bad_slice, const WallTimer& wt,
+                           uint64_t* n_groups, int32_t* status, int32_t* bad_slice, const WallTimer& wt,
                            const std::vector<SortSource>* mix) {
   Lane& Ln = D->lane[kLaneRead];
   std::lock_guard<std::mutex> lk(Ln.mtx);
@@ -2667,8 +2775,8 @@ static int sort_packed_run(Device* D, uint32_t codec, uint32_t alg, uint32_t n, 
   uint64_t launches = 0;
   uint8_t* sorted = nullptr;
   rc = decompress_sort_run(D, S, codec, alg, n, (const uint8_t*)S.src.p, dev_off.data(), src_len, true, slice_base,
-                           slice_len, slice_checksum, spec, &sorted, dst_cap, dst_total, n_records, status, bad_slice,
-                           &launches, mix);
+                           slice_len, slice_checksum, spec, &sorted, dst_cap, dst_total, n_records, n_groups, status,
+                           bad_slice, &launches, mix);
   if (rc) return rc;
   const uint64_t down = *n_records ? *dst_total : 0;
   CU(cudaEventRecord(S.ev_d0, st));
@@ -2747,11 +2855,12 @@ static int sort_call(uint32_t dev_index, bool packed, const ExchangeRead* x, uin
                      const uint8_t* src_base, const uint64_t* src_off, const uint64_t* src_len,
                      const uint32_t* slice_base, const uint64_t* slice_len, const uint64_t* slice_checksum,
                      const RecordSpec& spec, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_total,
-                     uint64_t* n_records, int32_t* status, int32_t* bad_slice) {
+                     uint64_t* n_records, int32_t* status, int32_t* bad_slice, uint64_t* n_groups = nullptr) {
   WallTimer wt;
   t_timing = b2s_timing{};
   if (dst_total) *dst_total = 0;
   if (n_records) *n_records = 0;
+  if (n_groups) *n_groups = 0;
   Device* D;
   MixedSources M;
   int rc;
@@ -2783,7 +2892,7 @@ static int sort_call(uint32_t dev_index, bool packed, const ExchangeRead* x, uin
   }
   return (packed ? sort_packed_run : sort_dev_run)(D, codec, alg, n, src_base, src_off, src_len, slice_base, slice_len,
                                                    slice_checksum, spec, dst_base, dst_cap, dst_total, n_records,
-                                                   status, bad_slice, wt, mix);
+                                                   n_groups, status, bad_slice, wt, mix);
 }
 
 int b2s_decompress_sort_dev(uint32_t dev_index, uint32_t codec, uint32_t checksum_alg, uint32_t n,
@@ -2827,6 +2936,51 @@ int b2s_decompress_sort_rows_packed(uint32_t codec, uint32_t checksum_alg, uint3
   return sort_call(t_device, true, nullptr, codec, checksum_alg, n, src_base, src_off, src_len, slice_base, slice_len,
                    slice_checksum, rows_spec(key_type, key_off, key_len, null_field), dst_base, dst_cap, dst_total,
                    n_records, status, bad_slice);
+}
+
+// the row sort's call with the aggregates; *dst_total is 0 when a block failed (nothing is written)
+static int aggregate_call(uint32_t dev_index, bool packed, uint32_t codec, uint32_t alg, uint32_t n,
+                          const uint8_t* src_base, const uint64_t* src_off, const uint64_t* src_len,
+                          const uint32_t* slice_base, const uint64_t* slice_len, const uint64_t* slice_checksum,
+                          const RecordSpec& spec, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_total,
+                          uint64_t* n_records, uint64_t* n_groups, int32_t* status, int32_t* bad_slice) {
+  if (!n_groups) {
+    if (dst_total) *dst_total = 0;
+    if (n_records) *n_records = 0;
+    return fail(B2S_E_ARG, "null argument%s");
+  }
+  const int rc = sort_call(dev_index, packed, nullptr, codec, alg, n, src_base, src_off, src_len, slice_base,
+                           slice_len, slice_checksum, spec, dst_base, dst_cap, dst_total, n_records, status, bad_slice,
+                           n_groups);
+  if (!rc && !*n_records) *dst_total = 0;
+  return rc;
+}
+
+int b2s_decompress_aggregate_rows_packed(uint32_t codec, uint32_t checksum_alg, uint32_t n, const uint8_t* src_base,
+                                         const uint64_t* src_off, const uint64_t* src_len, const uint32_t* slice_base,
+                                         const uint64_t* slice_len, const uint64_t* slice_checksum, uint32_t key_type,
+                                         uint32_t key_off, uint32_t key_len, int32_t null_field, uint32_t n_aggs,
+                                         const uint32_t* agg_op, const uint32_t* agg_off, const int32_t* agg_null_field,
+                                         uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records,
+                                         uint64_t* n_groups, int32_t* status, int32_t* bad_slice) {
+  return aggregate_call(t_device, true, codec, checksum_alg, n, src_base, src_off, src_len, slice_base, slice_len,
+                        slice_checksum,
+                        aggregate_spec(key_type, key_off, key_len, null_field, n_aggs, agg_op, agg_off, agg_null_field),
+                        dst_base, dst_cap, dst_total, n_records, n_groups, status, bad_slice);
+}
+
+int b2s_decompress_aggregate_rows_dev(uint32_t dev_index, uint32_t codec, uint32_t checksum_alg, uint32_t n,
+                                      const uint8_t* src_base, const uint64_t* src_off, const uint64_t* src_len,
+                                      const uint32_t* slice_base, const uint64_t* slice_len,
+                                      const uint64_t* slice_checksum, uint32_t key_type, uint32_t key_off,
+                                      uint32_t key_len, int32_t null_field, uint32_t n_aggs, const uint32_t* agg_op,
+                                      const uint32_t* agg_off, const int32_t* agg_null_field, uint8_t* dst_base,
+                                      uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records, uint64_t* n_groups,
+                                      int32_t* status, int32_t* bad_slice) {
+  return aggregate_call(dev_index, false, codec, checksum_alg, n, src_base, src_off, src_len, slice_base, slice_len,
+                        slice_checksum,
+                        aggregate_spec(key_type, key_off, key_len, null_field, n_aggs, agg_op, agg_off, agg_null_field),
+                        dst_base, dst_cap, dst_total, n_records, n_groups, status, bad_slice);
 }
 
 // ------------------------------------------------------------------------------------------------------------

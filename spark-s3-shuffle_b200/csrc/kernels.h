@@ -220,23 +220,51 @@ const uint32_t* launch_key_radix(const KeySortWs& w, uint64_t n, uint32_t key_by
 // n_ranges).  Afterwards rows_frame_readback(d_fws) holds rows_frame_readback_bytes(n_ranges) bytes: [record count,
 // verdict of range 0, 1, ...]; a verdict is ~0 when the range is whole records, else kRowsBad* << 61 | the offset of the
 // range's first bad record.  A record is bad when its prefix is cut by the range end, its size is negative, it runs past
-// the range end, its row is shorter than min_key bytes, or shorter than min_null bytes.
-constexpr uint64_t kRowsBadPrefix = 1, kRowsBadNegative = 2, kRowsBadPastEnd = 3, kRowsBadKey = 4, kRowsBadNull = 5;
+// the range end, its row is shorter than min_key bytes, shorter than min_null bytes, or shorter than min_agg bytes.
+constexpr uint64_t kRowsBadPrefix = 1, kRowsBadNegative = 2, kRowsBadPastEnd = 3, kRowsBadKey = 4, kRowsBadNull = 5,
+                   kRowsBadAgg = 6;
 size_t rows_frame_ws_bytes(uint64_t arena_bytes, uint32_t n_ranges);
 inline size_t rows_frame_readback_bytes(uint32_t n_ranges) { return ((size_t)n_ranges + 1) * 8; }
 uint64_t* rows_frame_readback(uint8_t* d_fws, uint64_t arena_bytes, uint32_t n_ranges);
 void launch_rows_frame(const uint8_t* arena, uint64_t arena_bytes, const uint64_t* h_off, const uint64_t* h_len,
-                       uint32_t n_ranges, uint64_t min_key, uint64_t min_null, uint8_t* d_fws, cudaStream_t st,
-                       uint64_t* launches);
+                       uint32_t n_ranges, uint64_t min_key, uint64_t min_null, uint64_t min_agg, uint8_t* d_fws,
+                       cudaStream_t st, uint64_t* launches);
 // key bytes of the sort: key_len, plus the leading null byte of a nullable key
 inline uint32_t rows_key_bytes(uint32_t key_len, int32_t null_field) { return key_len + (null_field >= 0 ? 1 : 0); }
 size_t rows_sort_ws_bytes(uint64_t n, uint32_t key_bytes);
 // the framed records (n = the read-back count) as dense offsets and lengths in arena order, into the sort workspace
 void launch_rows_emit(const uint8_t* arena, uint64_t arena_bytes, uint32_t n_ranges, uint8_t* d_fws, uint64_t n,
                       uint32_t key_bytes, uint8_t* d_ws, cudaStream_t st, uint64_t* launches);
-// the emitted records to d_dst, ascending by key (nulls first), stable.  key_type B2S_KEY_*
-void launch_rows_sort(const uint8_t* arena, uint64_t n, uint32_t key_type, uint32_t key_off, uint32_t key_len,
-                      int32_t null_field, uint8_t* d_ws, uint8_t* d_dst, cudaStream_t st, uint64_t* launches);
+// keys + radix: the emitted records' order, ascending by key (nulls first), stable, as sorted record indices (nullptr
+// when n < 2: arena order).  The key words stay in the workspace in record order.  key_type B2S_KEY_*
+const uint32_t* launch_rows_order(const uint8_t* arena, uint64_t n, uint32_t key_type, uint32_t key_off,
+                                  uint32_t key_len, int32_t null_field, uint8_t* d_ws, cudaStream_t st,
+                                  uint64_t* launches);
+// the emitted records to d_dst in the order idx
+void launch_rows_gather(const uint8_t* arena, uint64_t n, uint32_t key_bytes, const uint32_t* idx, uint8_t* d_ws,
+                        uint8_t* d_dst, cudaStream_t st, uint64_t* launches);
+
+// ---------------- aggregate.cu (group key-sorted rows and merge their aggregate buffers) ----------------
+// Aggregate a: op[a] (B2S_AGG_*) over the 8-byte slot at row offset off[a], null bit null_field[a] (-1: never null).
+constexpr uint32_t kMaxAggs = 16;
+struct AggSpec {
+  uint32_t n = 0;
+  uint32_t op[kMaxAggs] = {};
+  uint32_t off[kMaxAggs] = {};
+  int32_t null_field[kMaxAggs] = {};
+};
+// d_aws: rows_aggregate_ws_bytes(n, n_aggs), beside the sort workspace d_ws of the same n records
+size_t rows_aggregate_ws_bytes(uint64_t n, uint32_t n_aggs);
+// after launch_rows_group: [group count, output bytes] (device)
+uint64_t* rows_aggregate_readback(uint8_t* d_aws, uint64_t n, uint32_t n_aggs);
+// the groups of the records in the order idx (launch_rows_order): heads, group starts, the heads' output offsets and
+// the readback.  Also stages every aggregate's inputs in sorted order.
+void launch_rows_group(const uint8_t* arena, uint64_t n, const uint32_t* idx, uint32_t key_bytes, const AggSpec& spec,
+                       uint8_t* d_ws, uint8_t* d_aws, cudaStream_t st, uint64_t* launches);
+// the groups (count read back) to d_dst: the first record of each, whole, with the aggregates' slots and null bits
+// replaced by the merged values
+void launch_rows_aggregate(const uint8_t* arena, uint64_t n, uint64_t groups, uint32_t key_bytes, uint32_t n_aggs,
+                           uint8_t* d_ws, uint8_t* d_aws, uint8_t* d_dst, cudaStream_t st, uint64_t* launches);
 
 // ---------------- exchange.cu (exchange-cache reads: ranges of device memory gathered into one arena) ----------------
 // piece: len bytes at src (device pointer, any alignment) go to d_dst + dst

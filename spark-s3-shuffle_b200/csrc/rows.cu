@@ -10,8 +10,9 @@
 //   emit   : the bitmap compacted into dense record offsets (u64) and lengths (u32, prefix included), arena order
 //   keys   : one thread per record: the typed key as big-endian u32 words (int32 / int64: byte-swapped, sign bit
 //            flipped; a nullable key gets a leading byte 0 = null, 1 = non-null, and a null record's key bytes are 0)
-//   radix / gather : the fixed-size sort's radix passes (launch_key_radix), sorted lengths -> scan -> destination
-//            offsets (launch_sorted_offsets), the partition step's gather
+//   radix  : the fixed-size sort's radix passes (launch_key_radix): the sorted record indices
+//   gather : sorted lengths -> scan -> destination offsets (launch_sorted_offsets), the partition step's gather (a row
+//            sort; a grouped aggregation gathers only each group's first record, aggregate.cu)
 #include <algorithm>
 
 #include "kernels.h"
@@ -53,7 +54,8 @@ __device__ __forceinline__ void cp_async_wait() {
 // pieces are copied while they start before the block end; the last may reach 15 bytes past it, into the arena's slack.
 __global__ void __launch_bounds__(kFrameWarps * 32) rows_frame_kernel(
     const uint8_t* __restrict__ arena, const uint64_t* __restrict__ r_off, const uint64_t* __restrict__ r_len,
-    uint32_t n, uint64_t min_key, uint64_t min_null, uint32_t* __restrict__ bitmap, uint64_t* __restrict__ verdict,
+    uint32_t n, uint64_t min_key, uint64_t min_null, uint64_t min_agg, uint32_t* __restrict__ bitmap,
+    uint64_t* __restrict__ verdict,
     unsigned int* __restrict__ counter) {
   __shared__ __align__(16) uint32_t s_ring[kFrameWarps][kFrameRingBytes / 4];
   const uint32_t lane = threadIdx.x & 31;
@@ -109,6 +111,7 @@ __global__ void __launch_bounds__(kFrameWarps * 32) rows_frame_kernel(
             else if (q + 4 + (uint32_t)s > end) why = kRowsBadPastEnd;
             else if ((uint64_t)s < min_key) why = kRowsBadKey;
             else if ((uint64_t)s < min_null) why = kRowsBadNull;
+            else if ((uint64_t)s < min_agg) why = kRowsBadAgg;
           }
           if (why) {
             bad = (why << 61) | (q - start);
@@ -289,8 +292,8 @@ uint64_t* rows_frame_readback(uint8_t* d_fws, uint64_t arena_bytes, uint32_t n_r
 }
 
 void launch_rows_frame(const uint8_t* arena, uint64_t arena_bytes, const uint64_t* h_off, const uint64_t* h_len,
-                       uint32_t n_ranges, uint64_t min_key, uint64_t min_null, uint8_t* d_fws, cudaStream_t st,
-                       uint64_t* launches) {
+                       uint32_t n_ranges, uint64_t min_key, uint64_t min_null, uint64_t min_agg, uint8_t* d_fws,
+                       cudaStream_t st, uint64_t* launches) {
   const FrameWs f = carve_frame_ws(d_fws, arena_bytes, n_ranges);
   cudaMemsetAsync(f.bitmap, 0, f.tiles * kTileWords * 4, st);
   cudaMemsetAsync(f.readback, 0xff, rows_frame_readback_bytes(n_ranges), st);
@@ -304,7 +307,8 @@ void launch_rows_frame(const uint8_t* arena, uint64_t arena_bytes, const uint64_
     const uint64_t want = ((uint64_t)n_ranges + kFrameWarps - 1) / kFrameWarps;
     const uint64_t grid = std::min<uint64_t>((uint64_t)kSMs * per_sm, want);  // persistent: one wave
     rows_frame_kernel<<<(unsigned)grid, kFrameWarps * 32, 0, st>>>(arena, f.r_off, f.r_len, n_ranges, min_key,
-                                                                    min_null, f.bitmap, f.readback + 1, f.counter);
+                                                                    min_null, min_agg, f.bitmap, f.readback + 1,
+                                                                    f.counter);
     if (launches) *launches += 1;
   }
   rows_count_kernel<<<(unsigned)f.tiles, kRowThreads, 0, st>>>(f.bitmap, f.tile_cnt);
@@ -325,19 +329,27 @@ void launch_rows_emit(const uint8_t* arena, uint64_t arena_bytes, uint32_t n_ran
   if (launches) *launches += 1;
 }
 
-void launch_rows_sort(const uint8_t* arena, uint64_t n, uint32_t key_type, uint32_t key_off, uint32_t key_len,
-                      int32_t null_field, uint8_t* d_ws, uint8_t* d_dst, cudaStream_t st, uint64_t* launches) {
-  if (!n) return;
+const uint32_t* launch_rows_order(const uint8_t* arena, uint64_t n, uint32_t key_type, uint32_t key_off,
+                                  uint32_t key_len, int32_t null_field, uint8_t* d_ws, cudaStream_t st,
+                                  uint64_t* launches) {
+  if (!n) return nullptr;
   const uint32_t key_bytes = rows_key_bytes(key_len, null_field);
   const KeySortWs w = carve_key_sort_ws(d_ws, n, key_bytes);
-  uint64_t* offsets_scan_ws = (uint64_t*)(d_ws + key_sort_ws_bytes(n, key_bytes));
   rows_keys_kernel<<<grid_for(n), kRowThreads, 0, st>>>(arena, w.src_off, n, key_type, key_off, key_len, null_field,
                                                         (key_bytes + 3) / 4, w.words);
   if (launches) *launches += 1;
+  return launch_key_radix(w, n, key_bytes, st, launches);
+}
+
+void launch_rows_gather(const uint8_t* arena, uint64_t n, uint32_t key_bytes, const uint32_t* idx, uint8_t* d_ws,
+                        uint8_t* d_dst, cudaStream_t st, uint64_t* launches) {
+  if (!n) return;
+  const KeySortWs w = carve_key_sort_ws(d_ws, n, key_bytes);
+  uint64_t* offsets_scan_ws = (uint64_t*)(d_ws + key_sort_ws_bytes(n, key_bytes));
   PartitionPlan plan;
   plan.src_off = w.src_off;
   plan.sdst = w.sdst;
-  plan.idx = launch_key_radix(w, n, key_bytes, st, launches);
+  plan.idx = idx;
   launch_sorted_offsets(plan.idx, w.len, n, w.sdst, w.total, offsets_scan_ws, st, launches);
   launch_partition_gather(arena, w.len, n, plan, d_dst, st, launches);
 }

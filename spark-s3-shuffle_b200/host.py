@@ -63,6 +63,9 @@ PROTOTYPES = [
      [_vp, _u32, _u32, _u32, C.POINTER(_vp), C.POINTER(_u64), C.POINTER(_u64)]),
     ("b2sh_reader_read_sorted_rows", C.c_int,
      [_vp, _u32, _u32, _u32, _i32, C.POINTER(_vp), C.POINTER(_u64), C.POINTER(_u64)]),
+    ("b2sh_reader_read_aggregated_rows", C.c_int,
+     [_vp, _u32, _u32, _u32, _i32, _u32, _vp, _vp, _vp, C.POINTER(_vp), C.POINTER(_u64), C.POINTER(_u64),
+      C.POINTER(_u64)]),
     ("b2sh_reader_block", C.c_int,
      [_vp, _u32, C.POINTER(_i64), C.POINTER(_i32), C.POINTER(_i32), C.POINTER(_vp), C.POINTER(_u64)]),
     ("b2sh_reader_remote_bytes_read", _u64, [_vp]),
@@ -340,6 +343,21 @@ class S3ShuffleReader:
         _check(load().b2sh_reader_read_sorted_rows(self._h, keyType, keyOffset, keyLength, nullField, C.byref(p),
                                                    C.byref(ln), C.byref(nrec)))
         return (C.string_at(p.value, ln.value) if ln.value else b""), nrec.value
+
+    def readAggregatedRows(self, keyType, keyOffset, keyLength, nullField=-1, aggs=()):
+        """read() of a SQL exchange whose partial aggregates are merged by one typed key
+        (spark.shuffle.s3.gpu.aggregateRows): one UnsafeRowSerializer record per key, in the row sort's order, with
+        each aggregate (op, offset, null field) merged over the key's records.  Fetched blocks only (no exchange cache).
+        -> (bytes, number of input records, number of groups)"""
+        aggs = list(aggs)
+        op = np.array([a[0] for a in aggs] or [0], dtype=np.uint32)
+        off = np.array([a[1] for a in aggs] or [0], dtype=np.uint32)
+        nf = np.array([a[2] for a in aggs] or [0], dtype=np.int32)
+        p, ln, nrec, ngrp = _vp(), _u64(), _u64(), _u64()
+        _check(load().b2sh_reader_read_aggregated_rows(self._h, keyType, keyOffset, keyLength, nullField, len(aggs),
+                                                       op.ctypes.data, off.ctypes.data, nf.ctypes.data, C.byref(p),
+                                                       C.byref(ln), C.byref(nrec), C.byref(ngrp)))
+        return (C.string_at(p.value, ln.value) if ln.value else b""), nrec.value, ngrp.value
 
     def _blocks(self, n):
         out = []

@@ -838,6 +838,32 @@ class S3ShuffleReader {
   // then reduce-id order.  Codec NONE is verified and sorted only.  It reads fetched blocks only: the exchange cache is
   // not consulted.
   void readSortedRows(uint32_t keyType, uint32_t keyOff, uint32_t keyLen, int32_t nullField) {
+    readRows(keyType, keyOff, keyLen, nullField, nullptr);
+  }
+  // The aggregates of readAggregatedRows: aggregate k is op[k] (B2S_AGG_*) over the 8-byte slot at row offset off[k],
+  // null bit nullField[k] (-1 = never null).
+  struct RowAggregates {
+    uint32_t n;
+    const uint32_t* op;
+    const uint32_t* off;
+    const int32_t* nullField;
+  };
+  // read() for a Spark SQL exchange whose reducer merges partial aggregates by one typed key (INTEGRATION.md §3h): the
+  // blocks are fetched and staged as readSortedRows does, then ONE b2s_decompress_aggregate_rows_packed call verifies,
+  // decodes, groups and merges them into one row per key, in the row sort's order.  The exchange cache is not
+  // consulted.
+  void readAggregatedRows(uint32_t keyType, uint32_t keyOff, uint32_t keyLen, int32_t nullField,
+                          const RowAggregates& aggs) {
+    readRows(keyType, keyOff, keyLen, nullField, &aggs);
+  }
+  const uint8_t* sortedData() const { return sorted_.get(); }
+  uint64_t sortedLen() const { return sortedLen_; }
+  uint64_t sortedRecords() const { return sortedRecords_; }
+  uint64_t sortedGroups() const { return sortedGroups_; }
+
+ private:
+  // the body of readSortedRows (aggs == nullptr) and readAggregatedRows
+  void readRows(uint32_t keyType, uint32_t keyOff, uint32_t keyLen, int32_t nullField, const RowAggregates* aggs) {
     start(true);
     std::vector<std::pair<uint64_t, std::vector<uint8_t>>> fetched;  // (tag, compressed bytes)
     drainWhole(fetched);
@@ -865,19 +891,27 @@ class S3ShuffleReader {
     // output size as in readSorted: a first guess, then one retry with the bytes needed
     uint64_t cap = codec == B2S_CODEC_NONE ? bytes : bytes * 4;
     std::vector<int32_t> status(n), bad(n);
-    uint64_t total = 0, records = 0;
+    uint64_t total = 0, records = 0, groups = 0;
     int rc = B2S_E_DST_TOO_SMALL;
     for (int attempt = 0; attempt < 2 && rc == B2S_E_DST_TOO_SMALL; attempt++) {
       if (attempt) cap = total;
       sorted_.reset(new uint8_t[(size_t)(cap ? cap : 1)]);
-      rc = b2s_decompress_sort_rows_packed(codec, alg, n, src.data(), off.data(), len.data(),
-                                           verify ? sliceBase.data() : nullptr, verify ? sliceLen.data() : nullptr,
-                                           verify ? sliceSum.data() : nullptr, keyType, keyOff, keyLen, nullField,
-                                           sorted_.get(), cap, &total, &records, status.data(), bad.data());
+      if (aggs)
+        rc = b2s_decompress_aggregate_rows_packed(
+            codec, alg, n, src.data(), off.data(), len.data(), verify ? sliceBase.data() : nullptr,
+            verify ? sliceLen.data() : nullptr, verify ? sliceSum.data() : nullptr, keyType, keyOff, keyLen, nullField,
+            aggs->n, aggs->op, aggs->off, aggs->nullField, sorted_.get(), cap, &total, &records, &groups,
+            status.data(), bad.data());
+      else
+        rc = b2s_decompress_sort_rows_packed(codec, alg, n, src.data(), off.data(), len.data(),
+                                             verify ? sliceBase.data() : nullptr, verify ? sliceLen.data() : nullptr,
+                                             verify ? sliceSum.data() : nullptr, keyType, keyOff, keyLen, nullField,
+                                             sorted_.get(), cap, &total, &records, status.data(), bad.data());
     }
     if (rc != 0)
-      throw CodecException(std::string("b2s_decompress_sort_rows_packed: ") + b2s_strerror(rc) + ": " +
-                           b2s_last_error());
+      throw CodecException(std::string(aggs ? "b2s_decompress_aggregate_rows_packed: "
+                                            : "b2s_decompress_sort_rows_packed: ") +
+                           b2s_strerror(rc) + ": " + b2s_last_error());
     for (uint32_t k = 0; k < n; k++) {
       if (status[k] == B2S_E_CHECKSUM)  // storage/S3ChecksumValidationStream.scala:72-74
         throw SparkException("Invalid checksum detected for " + info_[fetched[k].first].id.name());
@@ -886,11 +920,10 @@ class S3ShuffleReader {
     }
     sortedLen_ = total;
     sortedRecords_ = records;
+    sortedGroups_ = groups;
   }
-  const uint8_t* sortedData() const { return sorted_.get(); }
-  uint64_t sortedLen() const { return sortedLen_; }
-  uint64_t sortedRecords() const { return sortedRecords_; }
 
+ public:
   // want (nullptr = every map): the maps whose blocks are fetched
   void start(bool allowNone, const std::vector<uint8_t>* want = nullptr) {
     iter_.reset();
@@ -898,7 +931,7 @@ class S3ShuffleReader {
     blocks_.clear();
     decoded_.clear();
     sorted_.reset();
-    sortedLen_ = sortedRecords_ = 0;
+    sortedLen_ = sortedRecords_ = sortedGroups_ = 0;
     remoteBytesRead_ = remoteBlocksFetched_ = 0;
     batches_ = 0;
     if (!allowNone && d_.codecId() == B2S_CODEC_NONE)
@@ -1097,7 +1130,7 @@ class S3ShuffleReader {
   std::vector<Block> blocks_;
   std::vector<std::unique_ptr<uint8_t[]>> decoded_;
   std::unique_ptr<uint8_t[]> sorted_;  // readSorted(): the task's records in key order
-  uint64_t sortedLen_ = 0, sortedRecords_ = 0;
+  uint64_t sortedLen_ = 0, sortedRecords_ = 0, sortedGroups_ = 0;
   uint64_t remoteBytesRead_ = 0, remoteBlocksFetched_ = 0, batches_ = 0;
   S3BufferedPrefetchIterator::Statistics stats_;
 };
@@ -1271,6 +1304,19 @@ int b2sh_reader_read_sorted_rows(b2sh_reader* r, uint32_t key_type, uint32_t key
     *data = r->r->sortedData();
     *len = r->r->sortedLen();
     *n_records = r->r->sortedRecords();
+  });
+}
+int b2sh_reader_read_aggregated_rows(b2sh_reader* r, uint32_t key_type, uint32_t key_off, uint32_t key_len,
+                                     int32_t null_field, uint32_t n_aggs, const uint32_t* agg_op,
+                                     const uint32_t* agg_off, const int32_t* agg_null_field, const uint8_t** data,
+                                     uint64_t* len, uint64_t* n_records, uint64_t* n_groups) {
+  return guarded([&] {
+    r->r->readAggregatedRows(key_type, key_off, key_len, null_field,
+                             S3ShuffleReader::RowAggregates{n_aggs, agg_op, agg_off, agg_null_field});
+    *data = r->r->sortedData();
+    *len = r->r->sortedLen();
+    *n_records = r->r->sortedRecords();
+    *n_groups = r->r->sortedGroups();
   });
 }
 int b2sh_reader_block(b2sh_reader* r, uint32_t k, int64_t* map_id, int32_t* start_reduce, int32_t* end_reduce,
