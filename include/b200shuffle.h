@@ -52,6 +52,10 @@ extern "C" {
 #define B2S_KEY_BYTES 0 /* key_len (1..16) bytes, unsigned, lexicographic */
 #define B2S_KEY_INT32 1 /* 4 bytes, little-endian two's complement: UnsafeRow's IntegerType / DateType slot */
 #define B2S_KEY_INT64 2 /* 8 bytes, little-endian two's complement: LongType, TimestampType, Decimal(p <= 18) */
+/* the composite-key calls (b2s_decompress_*_rows_keys_*) also take: an 8-byte UnsafeRow slot (offset << 32) | size
+ * naming the size bytes at row offset offset, unsigned lexicographic, a proper prefix first (StringType under
+ * UTF8_BINARY, BinaryType) */
+#define B2S_STRING_KEY 3
 
 /* aggregate ops of the row aggregation (b2s_decompress_aggregate_rows_*), each over an 8-byte slot of the row */
 #define B2S_AGG_SUM_INT64 0   /* wrapping two's-complement sum: Sum(long), Count, Average's count */
@@ -313,6 +317,66 @@ int b2s_decompress_aggregate_rows_dev(uint32_t dev_index, uint32_t codec, uint32
                                       const uint32_t* agg_off, const int32_t* agg_null_field, uint8_t* dst_base,
                                       uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records, uint64_t* n_groups,
                                       int32_t* status, int32_t* bad_slice);
+
+/* ---- read side, composite key: the row sort and the row aggregation by several key columns, strings included ----
+ * b2s_decompress_sort_rows_* and b2s_decompress_aggregate_rows_* with a key of n_keys (1..16) columns, given as
+ * parallel arrays: column c is key_type[c] at row offset key_off[c], key_len[c] bytes, null bit key_null_field[c].
+ * Columns compare left to right; each is read exactly as the single-key calls read their key (B2S_KEY_BYTES,
+ * B2S_KEY_INT32, B2S_KEY_INT64: the same key_len rules), and a null sorts first within its column (-1: never null).
+ * B2S_STRING_KEY (these calls only): key_len 8, the slot of a variable-length value; a null string and an empty string
+ * are different keys.  Two columns may share a slot or a null word.
+ * Sort: every record, stably sorted by the composite key (ascending, nulls first per column).  Aggregate: a group is a
+ * maximal run of records whose every column is equal (both null, or both non-null with equal values; strings: equal
+ * length and bytes); aggregates, output rows, group order and *n_groups are as in b2s_decompress_aggregate_rows_*.
+ * With n_keys == 1 and a fixed-width column the output is byte for byte that of the single-key call.
+ * Per block, B2S_E_CORRUPT for every framing rule of the single-key calls, applied with the largest key_off + key_len
+ * and null word of all columns, and when a non-null string's offset + size runs past the end of its row
+ * (b2s_last_error() names the block and the byte offset of its first bad record).  When a block fails nothing is
+ * written: *n_records (= *n_groups) = 0 and the call returns 0.
+ * Errors -> B2S_E_ARG: n_keys outside [1, 16]; NULL key arrays; an unknown key_type; a key_len its type does not allow;
+ * key_null_field[c] < -1; the aggregate checks of b2s_decompress_aggregate_rows_* against every column (no aggregate
+ * slot overlaps any key slot or a null word any column uses).  Checksums, codec NONE, B2S_E_DST_TOO_SMALL,
+ * B2S_E_NOMEM, the read lane, the 1 GiB buffer trim and b2s_last_timing are as in the single-key calls.
+ * The key is sorted by its first 20 encoded bytes (a column takes its bytes, plus one for its null bit; a string 9 per
+ * started 8 bytes of value, at least 9).  A key longer than that — any string column, or fixed-width columns of more
+ * than 20 bytes — is refined in rounds of 16 more bytes over the records still tied, and each round makes one small
+ * blocking readback (the count of tied records; the first round also brings the string checks' verdicts). */
+int b2s_decompress_sort_rows_keys_packed(uint32_t codec, uint32_t checksum_alg, uint32_t n, const uint8_t* src_base,
+                                         const uint64_t* src_off, const uint64_t* src_len, const uint32_t* slice_base,
+                                         const uint64_t* slice_len, const uint64_t* slice_checksum, uint32_t n_keys,
+                                         const uint32_t* key_type, const uint32_t* key_off, const uint32_t* key_len,
+                                         const int32_t* key_null_field, uint8_t* dst_base, uint64_t dst_cap,
+                                         uint64_t* dst_total, uint64_t* n_records, int32_t* status,
+                                         int32_t* bad_slice);
+/* same, with src_base / dst_base in device memory of dev_index; the descriptor and key arrays stay host arrays */
+int b2s_decompress_sort_rows_keys_dev(uint32_t dev_index, uint32_t codec, uint32_t checksum_alg, uint32_t n,
+                                      const uint8_t* src_base, const uint64_t* src_off, const uint64_t* src_len,
+                                      const uint32_t* slice_base, const uint64_t* slice_len,
+                                      const uint64_t* slice_checksum, uint32_t n_keys, const uint32_t* key_type,
+                                      const uint32_t* key_off, const uint32_t* key_len, const int32_t* key_null_field,
+                                      uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records,
+                                      int32_t* status, int32_t* bad_slice);
+int b2s_decompress_aggregate_rows_keys_packed(uint32_t codec, uint32_t checksum_alg, uint32_t n,
+                                              const uint8_t* src_base, const uint64_t* src_off,
+                                              const uint64_t* src_len, const uint32_t* slice_base,
+                                              const uint64_t* slice_len, const uint64_t* slice_checksum,
+                                              uint32_t n_keys, const uint32_t* key_type, const uint32_t* key_off,
+                                              const uint32_t* key_len, const int32_t* key_null_field, uint32_t n_aggs,
+                                              const uint32_t* agg_op, const uint32_t* agg_off,
+                                              const int32_t* agg_null_field, uint8_t* dst_base, uint64_t dst_cap,
+                                              uint64_t* dst_total, uint64_t* n_records, uint64_t* n_groups,
+                                              int32_t* status, int32_t* bad_slice);
+/* same, with src_base / dst_base in device memory of dev_index; the descriptor, key and aggregate arrays stay host
+ * arrays */
+int b2s_decompress_aggregate_rows_keys_dev(uint32_t dev_index, uint32_t codec, uint32_t checksum_alg, uint32_t n,
+                                           const uint8_t* src_base, const uint64_t* src_off, const uint64_t* src_len,
+                                           const uint32_t* slice_base, const uint64_t* slice_len,
+                                           const uint64_t* slice_checksum, uint32_t n_keys, const uint32_t* key_type,
+                                           const uint32_t* key_off, const uint32_t* key_len,
+                                           const int32_t* key_null_field, uint32_t n_aggs, const uint32_t* agg_op,
+                                           const uint32_t* agg_off, const int32_t* agg_null_field, uint8_t* dst_base,
+                                           uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records,
+                                           uint64_t* n_groups, int32_t* status, int32_t* bad_slice);
 
 /* ---- exchange cache: map outputs kept resident in HBM for reducers on the same device ----
  * (docs/f4_gpu_resident_exchange.md steps 2 and 3, local half.)  The serialized writer's partition step already leaves

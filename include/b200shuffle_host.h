@@ -166,6 +166,19 @@ int b2sh_reader_read_aggregated_rows(b2sh_reader* r, uint32_t key_type, uint32_t
                                      int32_t null_field, uint32_t n_aggs, const uint32_t* agg_op,
                                      const uint32_t* agg_off, const int32_t* agg_null_field, const uint8_t** data,
                                      uint64_t* len, uint64_t* n_records, uint64_t* n_groups);
+/* read_sorted_rows_keys() / read_aggregated_rows_keys(): read_sorted_rows() / read_aggregated_rows() by a composite
+ * key of n_keys (1..16) columns, strings included (key_type / key_off / key_len / key_null_field as in
+ * b2s_decompress_sort_rows_keys_packed): ONE b2s_decompress_sort_rows_keys_packed or
+ * b2s_decompress_aggregate_rows_keys_packed call, with the same buffer lifetime and error mapping. */
+int b2sh_reader_read_sorted_rows_keys(b2sh_reader* r, uint32_t n_keys, const uint32_t* key_type,
+                                      const uint32_t* key_off, const uint32_t* key_len, const int32_t* key_null_field,
+                                      const uint8_t** data, uint64_t* len, uint64_t* n_records);
+int b2sh_reader_read_aggregated_rows_keys(b2sh_reader* r, uint32_t n_keys, const uint32_t* key_type,
+                                          const uint32_t* key_off, const uint32_t* key_len,
+                                          const int32_t* key_null_field, uint32_t n_aggs, const uint32_t* agg_op,
+                                          const uint32_t* agg_off, const int32_t* agg_null_field,
+                                          const uint8_t** data, uint64_t* len, uint64_t* n_records,
+                                          uint64_t* n_groups);
 int b2sh_reader_block(b2sh_reader* r, uint32_t k, int64_t* map_id, int32_t* start_reduce, int32_t* end_reduce,
                       const uint8_t** data, uint64_t* len);
 uint64_t b2sh_reader_remote_bytes_read(b2sh_reader* r); /* metric parity with storage/S3ShuffleReader.scala:94-95 */

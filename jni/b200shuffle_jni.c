@@ -239,15 +239,24 @@ JNIEXPORT jint JNICALL J(decompressPacked)(JNIEnv* e, jclass c, jint codec, jint
  * partitions [startReduce, endReduce) of shuffleId.  rows: a row sort (decompressSortRowsPacked) of UnsafeRow records
  * by the key keyType at keyOff (recordBytes unused, mapIds NULL).  aggOp (rows only; NULL otherwise): a row
  * aggregation (decompressAggregateRowsPacked) with int[nAggs] aggOp / aggOff / aggNullField, and meta long[3] =
- * {dst_total, n_records, n_groups} */
+ * {dst_total, n_records, n_groups}.  keys (rows only; NULL: the one key keyType / keyOff / keyLen / nullField): a
+ * composite key (decompressSortRowsKeysPacked / decompressAggregateRowsKeysPacked) */
+typedef struct {
+  jint n; /* 1..16 columns */
+  jintArray type, off, len, nullField;
+} composite_key;
 static jint sort_packed(JNIEnv* e, jint shuffleId, jint startReduce, jint endReduce, jlongArray mapIds,
                         jintArray cached, jint codec, jint alg, jint n, jlong src, jlongArray off, jlongArray len,
                         jintArray sliceBase, jlongArray sliceLen, jlongArray sliceChecksum, jint recordBytes,
-                        int rows, jint keyType, jint keyOff, jint keyLen, jint nullField, jint nAggs, jintArray aggOp,
-                        jintArray aggOff, jintArray aggNullField, jlong dst, jlong dstCap, jlongArray meta,
-                        jintArray status, jintArray badSlice) {
+                        int rows, jint keyType, jint keyOff, jint keyLen, jint nullField, const composite_key* keys,
+                        jint nAggs, jintArray aggOp, jintArray aggOff, jintArray aggNullField, jlong dst, jlong dstCap,
+                        jlongArray meta, jintArray status, jintArray badSlice) {
   const jsize n_meta = aggOp ? 3 : 2;
   if (n < 0 || !meta || (*e)->GetArrayLength(e, meta) < n_meta) return B2S_E_ARG;
+  if (keys && (keys->n < 1 || keys->n > 16 || !keys->type || !keys->off || !keys->len || !keys->nullField ||
+               (*e)->GetArrayLength(e, keys->type) < keys->n || (*e)->GetArrayLength(e, keys->off) < keys->n ||
+               (*e)->GetArrayLength(e, keys->len) < keys->n || (*e)->GetArrayLength(e, keys->nullField) < keys->n))
+    return B2S_E_ARG;
   if (aggOp && (nAggs < 0 || nAggs > 16 || !aggOff || !aggNullField || (*e)->GetArrayLength(e, aggOp) < nAggs ||
                 (*e)->GetArrayLength(e, aggOff) < nAggs || (*e)->GetArrayLength(e, aggNullField) < nAggs))
     return B2S_E_ARG;
@@ -291,6 +300,14 @@ static jint sort_packed(JNIEnv* e, jint shuffleId, jint startReduce, jint endRed
   uint64_t total = 0, nrec = 0, ngrp = 0;
   if (rc == 0) {
     const size_t ns = with_slices ? (size_t)sb[n] : 0;
+    uint32_t kt[16], ko[16], kl[16];
+    int32_t knf[16];
+    if (keys) {
+      (*e)->GetIntArrayRegion(e, keys->type, 0, keys->n, (jint*)kt);
+      (*e)->GetIntArrayRegion(e, keys->off, 0, keys->n, (jint*)ko);
+      (*e)->GetIntArrayRegion(e, keys->len, 0, keys->n, (jint*)kl);
+      (*e)->GetIntArrayRegion(e, keys->nullField, 0, keys->n, (jint*)knf);
+    }
     if (aggOp) {
       uint32_t aop[16], aoff[16];
       int32_t anf[16];
@@ -299,12 +316,23 @@ static jint sort_packed(JNIEnv* e, jint shuffleId, jint startReduce, jint endRed
         (*e)->GetIntArrayRegion(e, aggOff, 0, nAggs, (jint*)aoff);
         (*e)->GetIntArrayRegion(e, aggNullField, 0, nAggs, (jint*)anf);
       }
-      rc = b2s_decompress_aggregate_rows_packed((uint32_t)codec, (uint32_t)alg, (uint32_t)n, PTR(const uint8_t, src),
+      if (keys)
+        rc = b2s_decompress_aggregate_rows_keys_packed(
+            (uint32_t)codec, (uint32_t)alg, (uint32_t)n, PTR(const uint8_t, src), blk, blk + N, with_slices ? sb : 0,
+            with_slices ? sl : 0, with_slices ? sl + ns : 0, (uint32_t)keys->n, kt, ko, kl, knf, (uint32_t)nAggs, aop,
+            aoff, anf, PTR(uint8_t, dst), (uint64_t)dstCap, &total, &nrec, &ngrp, st, st + N);
+      else
+        rc = b2s_decompress_aggregate_rows_packed(
+            (uint32_t)codec, (uint32_t)alg, (uint32_t)n, PTR(const uint8_t, src), blk, blk + N, with_slices ? sb : 0,
+            with_slices ? sl : 0, with_slices ? sl + ns : 0, (uint32_t)keyType, (uint32_t)keyOff, (uint32_t)keyLen,
+            (int32_t)nullField, (uint32_t)nAggs, aop, aoff, anf, PTR(uint8_t, dst), (uint64_t)dstCap, &total, &nrec,
+            &ngrp, st, st + N);
+    } else if (keys)
+      rc = b2s_decompress_sort_rows_keys_packed((uint32_t)codec, (uint32_t)alg, (uint32_t)n, PTR(const uint8_t, src),
                                                 blk, blk + N, with_slices ? sb : 0, with_slices ? sl : 0,
-                                                with_slices ? sl + ns : 0, (uint32_t)keyType, (uint32_t)keyOff,
-                                                (uint32_t)keyLen, (int32_t)nullField, (uint32_t)nAggs, aop, aoff, anf,
-                                                PTR(uint8_t, dst), (uint64_t)dstCap, &total, &nrec, &ngrp, st, st + N);
-    } else if (rows)
+                                                with_slices ? sl + ns : 0, (uint32_t)keys->n, kt, ko, kl, knf,
+                                                PTR(uint8_t, dst), (uint64_t)dstCap, &total, &nrec, st, st + N);
+    else if (rows)
       rc = b2s_decompress_sort_rows_packed((uint32_t)codec, (uint32_t)alg, (uint32_t)n, PTR(const uint8_t, src), blk,
                                            blk + N, with_slices ? sb : 0, with_slices ? sl : 0,
                                            with_slices ? sl + ns : 0, (uint32_t)keyType, (uint32_t)keyOff,
@@ -344,7 +372,7 @@ JNIEXPORT jint JNICALL J(decompressSortPacked)(JNIEnv* e, jclass c, jint codec, 
                                                jintArray badSlice) {
   (void)c;
   return sort_packed(e, 0, 0, 0, 0, 0, codec, alg, n, src, off, len, sliceBase, sliceLen, sliceChecksum, recordBytes,
-                     0, 0, keyOff, keyLen, -1, 0, 0, 0, 0, dst, dstCap, meta, status, badSlice);
+                     0, 0, keyOff, keyLen, -1, 0, 0, 0, 0, 0, dst, dstCap, meta, status, badSlice);
 }
 
 /* ---- read side, row-sorted (a Spark SQL exchange read followed by a SortExec, INTEGRATION.md §3g): verify, decode and
@@ -357,7 +385,7 @@ JNIEXPORT jint JNICALL J(decompressSortRowsPacked)(JNIEnv* e, jclass c, jint cod
                                                    jlongArray meta, jintArray status, jintArray badSlice) {
   (void)c;
   return sort_packed(e, 0, 0, 0, 0, 0, codec, alg, n, src, off, len, sliceBase, sliceLen, sliceChecksum, 0, 1, keyType,
-                     keyOff, keyLen, nullField, 0, 0, 0, 0, dst, dstCap, meta, status, badSlice);
+                     keyOff, keyLen, nullField, 0, 0, 0, 0, 0, dst, dstCap, meta, status, badSlice);
 }
 
 /* ---- read side, aggregated (a Spark SQL exchange read followed by a HashAggregateExec(Final), INTEGRATION.md §3h):
@@ -374,8 +402,38 @@ JNIEXPORT jint JNICALL J(decompressAggregateRowsPacked)(JNIEnv* e, jclass c, jin
   (void)c;
   if (!aggOp) return B2S_E_ARG;
   return sort_packed(e, 0, 0, 0, 0, 0, codec, alg, n, src, off, len, sliceBase, sliceLen, sliceChecksum, 0, 1, keyType,
-                     keyOff, keyLen, nullField, nAggs, aggOp, aggOff, aggNullField, dst, dstCap, meta, status,
+                     keyOff, keyLen, nullField, 0, nAggs, aggOp, aggOff, aggNullField, dst, dstCap, meta, status,
                      badSlice);
+}
+
+/* ---- read side, composite key (INTEGRATION.md §3g / §3h): the row sort and the row aggregation by nKeys (1..16)
+ *      columns, strings included: keyType (B2S_KEY_* or B2S_STRING_KEY) / keyOff / keyLen / keyNullField are
+ *      int[nKeys]; other arrays and meta as decompressSortRowsPacked / decompressAggregateRowsPacked. ---- */
+JNIEXPORT jint JNICALL J(decompressSortRowsKeysPacked)(JNIEnv* e, jclass c, jint codec, jint alg, jint n, jlong src,
+                                                       jlongArray off, jlongArray len, jintArray sliceBase,
+                                                       jlongArray sliceLen, jlongArray sliceChecksum, jint nKeys,
+                                                       jintArray keyType, jintArray keyOff, jintArray keyLen,
+                                                       jintArray keyNullField, jlong dst, jlong dstCap,
+                                                       jlongArray meta, jintArray status, jintArray badSlice) {
+  (void)c;
+  const composite_key k = {nKeys, keyType, keyOff, keyLen, keyNullField};
+  return sort_packed(e, 0, 0, 0, 0, 0, codec, alg, n, src, off, len, sliceBase, sliceLen, sliceChecksum, 0, 1, 0, 0, 0,
+                     -1, &k, 0, 0, 0, 0, dst, dstCap, meta, status, badSlice);
+}
+JNIEXPORT jint JNICALL J(decompressAggregateRowsKeysPacked)(JNIEnv* e, jclass c, jint codec, jint alg, jint n,
+                                                            jlong src, jlongArray off, jlongArray len,
+                                                            jintArray sliceBase, jlongArray sliceLen,
+                                                            jlongArray sliceChecksum, jint nKeys, jintArray keyType,
+                                                            jintArray keyOff, jintArray keyLen,
+                                                            jintArray keyNullField, jint nAggs, jintArray aggOp,
+                                                            jintArray aggOff, jintArray aggNullField, jlong dst,
+                                                            jlong dstCap, jlongArray meta, jintArray status,
+                                                            jintArray badSlice) {
+  (void)c;
+  if (!aggOp) return B2S_E_ARG;
+  const composite_key k = {nKeys, keyType, keyOff, keyLen, keyNullField};
+  return sort_packed(e, 0, 0, 0, 0, 0, codec, alg, n, src, off, len, sliceBase, sliceLen, sliceChecksum, 0, 1, 0, 0, 0,
+                     -1, &k, nAggs, aggOp, aggOff, aggNullField, dst, dstCap, meta, status, badSlice);
 }
 
 /* ---- exchange cache (INTEGRATION.md §3f): map outputs kept in HBM for reducers on the same device ---- */
@@ -449,8 +507,8 @@ JNIEXPORT jint JNICALL J(exchangeReadSortPacked)(JNIEnv* e, jclass c, jint shuff
   (void)c;
   if (!mapIds) return B2S_E_ARG;
   return sort_packed(e, shuffleId, startReduce, endReduce, mapIds, cached, codec, alg, n, src, off, len, sliceBase,
-                     sliceLen, sliceChecksum, recordBytes, 0, 0, keyOff, keyLen, -1, 0, 0, 0, 0, dst, dstCap, meta,
-                     status, badSlice);
+                     sliceLen, sliceChecksum, recordBytes, 0, 0, keyOff, keyLen, -1, 0, 0, 0, 0, 0, dst, dstCap,
+                     meta, status, badSlice);
 }
 
 /* decoded size of each of n compressed streams laid out in one arena (sizes the destination of decompressPacked) */

@@ -13,6 +13,7 @@ from . import _build
 CODEC_NONE, CODEC_LZ4BLOCK, CODEC_SNAPPY_XERIAL, CODEC_ZSTD = 0, 1, 2, 3
 CHECKSUM_NONE, CHECKSUM_ADLER32, CHECKSUM_CRC32, CHECKSUM_CRC32C = 0, 1, 2, 3
 KEY_BYTES, KEY_INT32, KEY_INT64 = 0, 1, 2  # key types of the row sort (decompress_sort_rows_*)
+STRING_KEY = 3  # the composite-key calls' variable-length key column (decompress_*_rows_keys_*)
 # aggregate ops of the row aggregation (decompress_aggregate_rows_*)
 (AGG_SUM_INT64, AGG_SUM_FLOAT64, AGG_MIN_INT32, AGG_MAX_INT32, AGG_MIN_INT64, AGG_MAX_INT64, AGG_MIN_FLOAT64,
  AGG_MAX_FLOAT64) = range(8)
@@ -86,6 +87,18 @@ PROTOTYPES = [
     ("b2s_decompress_aggregate_rows_dev", C.c_int,
      [_u32, _u32, _u32, _u32, _vp, _u64p, _u64p, _u32p, _u64p, _u64p, _u32, _u32, _u32, _i32, _u32, _u32p, _u32p, _i32p,
       _vp, _u64, _u64p, _u64p, _u64p, _i32p, _i32p]),
+    ("b2s_decompress_sort_rows_keys_packed", C.c_int,
+     [_u32, _u32, _u32, _u8p, _u64p, _u64p, _u32p, _u64p, _u64p, _u32, _u32p, _u32p, _u32p, _i32p, _u8p, _u64, _u64p,
+      _u64p, _i32p, _i32p]),
+    ("b2s_decompress_sort_rows_keys_dev", C.c_int,
+     [_u32, _u32, _u32, _u32, _vp, _u64p, _u64p, _u32p, _u64p, _u64p, _u32, _u32p, _u32p, _u32p, _i32p, _vp, _u64,
+      _u64p, _u64p, _i32p, _i32p]),
+    ("b2s_decompress_aggregate_rows_keys_packed", C.c_int,
+     [_u32, _u32, _u32, _u8p, _u64p, _u64p, _u32p, _u64p, _u64p, _u32, _u32p, _u32p, _u32p, _i32p, _u32, _u32p, _u32p,
+      _i32p, _u8p, _u64, _u64p, _u64p, _u64p, _i32p, _i32p]),
+    ("b2s_decompress_aggregate_rows_keys_dev", C.c_int,
+     [_u32, _u32, _u32, _u32, _vp, _u64p, _u64p, _u32p, _u64p, _u64p, _u32, _u32p, _u32p, _u32p, _i32p, _u32, _u32p,
+      _u32p, _i32p, _vp, _u64, _u64p, _u64p, _u64p, _i32p, _i32p]),
     ("b2s_exchange_set_budget", C.c_int, [_u32, _u64]),
     ("b2s_partition_compress_cached_packed", C.c_int,
      [_i32, C.c_int64, _u32, _i32, _u32, _u32, _u32, _u64, _u8p, _u64, _u32p, _u32p, _u8p, _u64, _u64p, _u64p, _u64p,
@@ -449,6 +462,60 @@ def decompress_aggregate_rows_packed(codec, src, off, length, dst, key_type, key
     return dict(total=total.value, n_records=nrec.value, n_groups=ngrp.value, status=st[:n], bad_slice=bad[:n])
 
 
+def _key_arrays(keys):
+    """keys = [(key_type, key_off, key_len, null_field), ...] -> (n, type, off, len, null_field) arrays"""
+    keys = list(keys)
+    kt = np.array([k[0] for k in keys] or [0], dtype=np.uint32)
+    ko = np.array([k[1] for k in keys] or [0], dtype=np.uint32)
+    kl = np.array([k[2] for k in keys] or [0], dtype=np.uint32)
+    kn = np.array([k[3] for k in keys] or [0], dtype=np.int32)
+    return len(keys), kt, ko, kl, kn
+
+
+def decompress_sort_rows_keys_packed(codec, src, off, length, dst, keys, checksum_alg=CHECKSUM_NONE, slice_base=None,
+                                     slice_len=None, slice_checksum=None):
+    """decompress_sort_rows_packed by a composite key: keys = [(KEY_* or STRING_KEY, row offset, length, null field
+    or -1), ...], compared left to right.  -> dict(total, n_records, status, bad_slice)"""
+    src, dst = _as_u8(src), _as_u8(dst)
+    off = np.ascontiguousarray(off, dtype=np.uint64)
+    length = np.ascontiguousarray(length, dtype=np.uint64)
+    n = off.size
+    sb, sl, sc = _sort_slices(checksum_alg, slice_base, slice_len, slice_checksum)
+    nk, kt, ko, kl, kn = _key_arrays(keys)
+    st = np.zeros(max(n, 1), dtype=np.int32)
+    bad = np.zeros(max(n, 1), dtype=np.int32)
+    total, nrec = _u64(0), _u64(0)
+    _check(load().b2s_decompress_sort_rows_keys_packed(codec, checksum_alg, n, _ptr(src), _ptr(off), _ptr(length),
+                                                       _ptr(sb), _ptr(sl), _ptr(sc), nk, _ptr(kt), _ptr(ko), _ptr(kl),
+                                                       _ptr(kn), _ptr(dst), dst.size, C.addressof(total),
+                                                       C.addressof(nrec), _ptr(st), _ptr(bad)),
+           "b2s_decompress_sort_rows_keys_packed")
+    return dict(total=total.value, n_records=nrec.value, status=st[:n], bad_slice=bad[:n])
+
+
+def decompress_aggregate_rows_keys_packed(codec, src, off, length, dst, keys, aggs=(), checksum_alg=CHECKSUM_NONE,
+                                          slice_base=None, slice_len=None, slice_checksum=None):
+    """decompress_aggregate_rows_packed grouped by a composite key (keys as in decompress_sort_rows_keys_packed).
+    -> dict(total, n_records, n_groups, status, bad_slice)"""
+    src, dst = _as_u8(src), _as_u8(dst)
+    off = np.ascontiguousarray(off, dtype=np.uint64)
+    length = np.ascontiguousarray(length, dtype=np.uint64)
+    n = off.size
+    sb, sl, sc = _sort_slices(checksum_alg, slice_base, slice_len, slice_checksum)
+    nk, kt, ko, kl, kn = _key_arrays(keys)
+    na, aop, aoff, anf = _agg_arrays(aggs)
+    st = np.zeros(max(n, 1), dtype=np.int32)
+    bad = np.zeros(max(n, 1), dtype=np.int32)
+    total, nrec, ngrp = _u64(0), _u64(0), _u64(0)
+    _check(load().b2s_decompress_aggregate_rows_keys_packed(codec, checksum_alg, n, _ptr(src), _ptr(off), _ptr(length),
+                                                            _ptr(sb), _ptr(sl), _ptr(sc), nk, _ptr(kt), _ptr(ko),
+                                                            _ptr(kl), _ptr(kn), na, _ptr(aop), _ptr(aoff), _ptr(anf),
+                                                            _ptr(dst), dst.size, C.addressof(total), C.addressof(nrec),
+                                                            C.addressof(ngrp), _ptr(st), _ptr(bad)),
+           "b2s_decompress_aggregate_rows_keys_packed")
+    return dict(total=total.value, n_records=nrec.value, n_groups=ngrp.value, status=st[:n], bad_slice=bad[:n])
+
+
 # ---------------------------------------------------------------------------------------------------------------
 # device-resident API (bench.py roofline leg); d_* are raw device addresses (ints)
 # ---------------------------------------------------------------------------------------------------------------
@@ -566,6 +633,46 @@ def decompress_aggregate_rows_dev(codec, d_src, off, length, d_dst, dst_cap, key
                                                     null_field, na, _ptr(aop), _ptr(aoff), _ptr(anf), d_dst, dst_cap,
                                                     C.addressof(total), C.addressof(nrec), C.addressof(ngrp), _ptr(st),
                                                     _ptr(bad)), "b2s_decompress_aggregate_rows_dev")
+    return dict(total=total.value, n_records=nrec.value, n_groups=ngrp.value, status=st[:n], bad_slice=bad[:n])
+
+
+def decompress_sort_rows_keys_dev(codec, d_src, off, length, d_dst, dst_cap, keys, checksum_alg=CHECKSUM_NONE,
+                                  slice_base=None, slice_len=None, slice_checksum=None, dev=0):
+    """decompress_sort_rows_keys_packed on device-resident blocks (d_src) into a device arena (d_dst)"""
+    off = np.ascontiguousarray(off, dtype=np.uint64)
+    length = np.ascontiguousarray(length, dtype=np.uint64)
+    n = off.size
+    sb, sl, sc = _sort_slices(checksum_alg, slice_base, slice_len, slice_checksum)
+    nk, kt, ko, kl, kn = _key_arrays(keys)
+    st = np.zeros(max(n, 1), dtype=np.int32)
+    bad = np.zeros(max(n, 1), dtype=np.int32)
+    total, nrec = _u64(0), _u64(0)
+    _check(load().b2s_decompress_sort_rows_keys_dev(dev, codec, checksum_alg, n, d_src, _ptr(off), _ptr(length),
+                                                    _ptr(sb), _ptr(sl), _ptr(sc), nk, _ptr(kt), _ptr(ko), _ptr(kl),
+                                                    _ptr(kn), d_dst, dst_cap, C.addressof(total), C.addressof(nrec),
+                                                    _ptr(st), _ptr(bad)), "b2s_decompress_sort_rows_keys_dev")
+    return dict(total=total.value, n_records=nrec.value, status=st[:n], bad_slice=bad[:n])
+
+
+def decompress_aggregate_rows_keys_dev(codec, d_src, off, length, d_dst, dst_cap, keys, aggs=(),
+                                       checksum_alg=CHECKSUM_NONE, slice_base=None, slice_len=None,
+                                       slice_checksum=None, dev=0):
+    """decompress_aggregate_rows_keys_packed on device-resident blocks (d_src) into a device arena (d_dst)"""
+    off = np.ascontiguousarray(off, dtype=np.uint64)
+    length = np.ascontiguousarray(length, dtype=np.uint64)
+    n = off.size
+    sb, sl, sc = _sort_slices(checksum_alg, slice_base, slice_len, slice_checksum)
+    nk, kt, ko, kl, kn = _key_arrays(keys)
+    na, aop, aoff, anf = _agg_arrays(aggs)
+    st = np.zeros(max(n, 1), dtype=np.int32)
+    bad = np.zeros(max(n, 1), dtype=np.int32)
+    total, nrec, ngrp = _u64(0), _u64(0), _u64(0)
+    _check(load().b2s_decompress_aggregate_rows_keys_dev(dev, codec, checksum_alg, n, d_src, _ptr(off), _ptr(length),
+                                                         _ptr(sb), _ptr(sl), _ptr(sc), nk, _ptr(kt), _ptr(ko),
+                                                         _ptr(kl), _ptr(kn), na, _ptr(aop), _ptr(aoff), _ptr(anf),
+                                                         d_dst, dst_cap, C.addressof(total), C.addressof(nrec),
+                                                         C.addressof(ngrp), _ptr(st), _ptr(bad)),
+           "b2s_decompress_aggregate_rows_keys_dev")
     return dict(total=total.value, n_records=nrec.value, n_groups=ngrp.value, status=st[:n], bad_slice=bad[:n])
 
 

@@ -71,6 +71,7 @@ __global__ void __launch_bounds__(kAggThreads) agg_heads_kernel(const uint8_t* _
                                                                 const uint64_t* __restrict__ rec_off,
                                                                 const uint32_t* __restrict__ idx, uint64_t n,
                                                                 const uint32_t* __restrict__ words, uint32_t W,
+                                                                const uint32_t* __restrict__ heads,
                                                                 const AggSpec* __restrict__ spec,
                                                                 uint64_t* __restrict__ head, uint32_t* __restrict__ nulls,
                                                                 uint64_t* __restrict__ vals) {
@@ -78,7 +79,9 @@ __global__ void __launch_bounds__(kAggThreads) agg_heads_kernel(const uint8_t* _
   for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (uint64_t)gridDim.x * blockDim.x) {
     const uint32_t i = idx ? idx[j] : (uint32_t)j;
     bool h = j == 0;
-    if (!h) {
+    if (heads) {
+      h = heads[j] != 0;
+    } else if (!h) {
       const uint32_t p = idx ? idx[j - 1] : (uint32_t)(j - 1);
 #pragma unroll
       for (uint32_t k = 0; k < 5; k++)
@@ -335,8 +338,9 @@ uint64_t* rows_aggregate_readback(uint8_t* d_aws, uint64_t n, uint32_t n_aggs) {
   return carve_agg_ws(d_aws, n, n_aggs).readback;
 }
 
-void launch_rows_group(const uint8_t* arena, uint64_t n, const uint32_t* idx, uint32_t key_bytes, const AggSpec& spec,
-                       uint8_t* d_ws, uint8_t* d_aws, cudaStream_t st, uint64_t* launches) {
+void launch_rows_group(const uint8_t* arena, uint64_t n, const uint32_t* idx, const uint32_t* heads,
+                       uint32_t key_bytes, const AggSpec& spec, uint8_t* d_ws, uint8_t* d_aws, cudaStream_t st,
+                       uint64_t* launches) {
   const AggWs a = carve_agg_ws(d_aws, n, spec.n);
   if (!n) {
     cudaMemsetAsync(a.readback, 0, 16, st);
@@ -345,8 +349,8 @@ void launch_rows_group(const uint8_t* arena, uint64_t n, const uint32_t* idx, ui
   const KeySortWs w = carve_key_sort_ws(d_ws, n, key_bytes);
   uint64_t* scan_ws = (uint64_t*)(d_ws + key_sort_ws_bytes(n, key_bytes));
   cudaMemcpyAsync(a.spec, &spec, sizeof(AggSpec), cudaMemcpyHostToDevice, st);
-  agg_heads_kernel<<<grid_for(n), kAggThreads, 0, st>>>(arena, w.src_off, idx, n, w.words, (key_bytes + 3) / 4, a.spec,
-                                                        a.head, a.nulls, a.vals);
+  agg_heads_kernel<<<grid_for(n), kAggThreads, 0, st>>>(arena, w.src_off, idx, n, w.words, (key_bytes + 3) / 4, heads,
+                                                        a.spec, a.head, a.nulls, a.vals);
   launch_exclusive_scan_u64(a.head, n, a.readback, scan_ws, st, launches);
   agg_compact_kernel<<<grid_for(n), kAggThreads, 0, st>>>(a.head, a.readback, idx, w.len, n, a.hidx, a.gpos, a.glen);
   // the group lengths are already in group order: no index

@@ -2303,14 +2303,15 @@ int b2s_decompress_packed(uint32_t codec, uint32_t checksum_alg, uint32_t n, con
 // read side, key-sorted: verify + decode a reduce task's blocks, then sort its records by key
 // ------------------------------------------------------------------------------------------------------------
 // What the records of a sort call are: fixed-size (record_bytes long, an unsigned byte key) or length-prefixed UnsafeRow
-// records (rows: [size: int32 big-endian][row], a typed key at key_off in the row, null bit null_field).  aggregate:
-// rows grouped by the key and merged (b2s_decompress_aggregate_rows_*: the caller's n_aggs aggregates), not sorted.
+// records (rows: [size: int32 big-endian][row], key columns in the row, each with its null bit).  aggregate: rows
+// grouped by the key and merged (b2s_decompress_aggregate_rows_*: the caller's n_aggs aggregates), not sorted.
 struct RecordSpec {
   bool is_rows = false;
   uint32_t record_bytes = 0;
-  uint32_t key_type = B2S_KEY_BYTES;
-  uint32_t key_off = 0, key_len = 0;
-  int32_t null_field = -1;
+  KeySpec keys;             // rows: the key columns; fixed-size records: one B2S_KEY_BYTES column
+  uint32_t n_keys = 1;      // as the caller passed it; keys holds the columns when it is in [1, 16]
+  bool key_arrays = true;   // the caller's key arrays are not NULL
+  bool strings = false;     // B2S_STRING_KEY columns accepted (the *_keys calls)
   bool aggregate = false;
   uint32_t n_aggs = 0;
   const uint32_t* agg_op = nullptr;
@@ -2321,17 +2322,36 @@ struct RecordSpec {
 static RecordSpec fixed_spec(uint32_t record_bytes, uint32_t key_off, uint32_t key_len) {
   RecordSpec r;
   r.record_bytes = record_bytes;
-  r.key_off = key_off;
-  r.key_len = key_len;
+  r.keys.n = 1;
+  r.keys.off[0] = key_off;
+  r.keys.len[0] = key_len;
+  r.keys.null_field[0] = -1;
   return r;
 }
 static RecordSpec rows_spec(uint32_t key_type, uint32_t key_off, uint32_t key_len, int32_t null_field) {
+  RecordSpec r = fixed_spec(0, key_off, key_len);
+  r.is_rows = true;
+  r.keys.type[0] = key_type;
+  r.keys.null_field[0] = null_field;
+  return r;
+}
+// the *_keys calls: n_keys parallel columns; checked by sort_args, after the device
+static RecordSpec keys_spec(uint32_t n_keys, const uint32_t* type, const uint32_t* off, const uint32_t* len,
+                            const int32_t* null_field) {
   RecordSpec r;
   r.is_rows = true;
-  r.key_type = key_type;
-  r.key_off = key_off;
-  r.key_len = key_len;
-  r.null_field = null_field;
+  r.strings = true;
+  r.n_keys = n_keys;
+  r.key_arrays = type && off && len && null_field;
+  if (r.key_arrays && n_keys >= 1 && n_keys <= kMaxKeys) {
+    r.keys.n = n_keys;
+    for (uint32_t c = 0; c < n_keys; c++) {
+      r.keys.type[c] = type[c];
+      r.keys.off[c] = off[c];
+      r.keys.len[c] = len[c];
+      r.keys.null_field[c] = null_field[c];
+    }
+  }
   return r;
 }
 
@@ -2339,9 +2359,8 @@ static bool overlaps(uint64_t a0, uint64_t a1, uint64_t b0, uint64_t b1) { retur
 // the row offset of field f's 8-byte null word
 static uint64_t null_word(int32_t f) { return 8ull * (uint32_t)(f >> 6); }
 
-static RecordSpec aggregate_spec(uint32_t key_type, uint32_t key_off, uint32_t key_len, int32_t null_field,
-                                 uint32_t n_aggs, const uint32_t* op, const uint32_t* off, const int32_t* agg_null) {
-  RecordSpec r = rows_spec(key_type, key_off, key_len, null_field);
+static RecordSpec with_aggregates(RecordSpec r, uint32_t n_aggs, const uint32_t* op, const uint32_t* off,
+                                  const int32_t* agg_null) {
   r.aggregate = true;
   r.n_aggs = n_aggs;
   r.agg_op = op;
@@ -2349,14 +2368,20 @@ static RecordSpec aggregate_spec(uint32_t key_type, uint32_t key_off, uint32_t k
   r.agg_null_field = agg_null;
   return r;
 }
+static RecordSpec aggregate_spec(uint32_t key_type, uint32_t key_off, uint32_t key_len, int32_t null_field,
+                                 uint32_t n_aggs, const uint32_t* op, const uint32_t* off, const int32_t* agg_null) {
+  return with_aggregates(rows_spec(key_type, key_off, key_len, null_field), n_aggs, op, off, agg_null);
+}
 
-// each aggregate is a known op on 8 bytes that touch no other slot, the key, or a null word in use
+// each aggregate is a known op on 8 bytes that touch no other slot, a key column, or a null word in use
 static int agg_args(const RecordSpec& spec) {
   const uint32_t n = spec.n_aggs;
+  const KeySpec& ks = spec.keys;
   if (n > kMaxAggs) return fail(B2S_E_ARG, "n_aggs must be at most 16%s");
   if (n && (!spec.agg_op || !spec.agg_off || !spec.agg_null_field)) return fail(B2S_E_ARG, "null argument%s");
   std::vector<std::pair<uint64_t, uint64_t>> words;  // the null words the key and the aggregates use
-  if (spec.null_field >= 0) words.push_back({null_word(spec.null_field), null_word(spec.null_field) + 8});
+  for (uint32_t c = 0; c < ks.n; c++)
+    if (ks.null_field[c] >= 0) words.push_back({null_word(ks.null_field[c]), null_word(ks.null_field[c]) + 8});
   for (uint32_t k = 0; k < n; k++) {
     if (spec.agg_op[k] > B2S_AGG_MAX_FLOAT64) return fail(B2S_E_ARG, "unknown aggregate op%s");
     const int32_t f = spec.agg_null_field[k];
@@ -2365,8 +2390,9 @@ static int agg_args(const RecordSpec& spec) {
   }
   for (uint32_t k = 0; k < n; k++) {
     const uint64_t s0 = spec.agg_off[k], s1 = s0 + 8;
-    if (overlaps(s0, s1, spec.key_off, (uint64_t)spec.key_off + spec.key_len))
-      return fail(B2S_E_ARG, "an aggregate slot overlaps the key%s");
+    for (uint32_t c = 0; c < ks.n; c++)
+      if (overlaps(s0, s1, ks.off[c], (uint64_t)ks.off[c] + ks.len[c]))
+        return fail(B2S_E_ARG, "an aggregate slot overlaps the key%s");
     for (uint32_t m = 0; m < k; m++)
       if (overlaps(s0, s1, spec.agg_off[m], (uint64_t)spec.agg_off[m] + 8))
         return fail(B2S_E_ARG, "aggregate slots overlap%s");
@@ -2392,20 +2418,27 @@ static int sort_args(uint32_t codec, uint32_t alg, uint32_t n, const uint64_t* s
                      const uint64_t* dst_total, const uint64_t* n_records, const int32_t* status) {
   if (alg > B2S_CHECKSUM_CRC32C) return fail(B2S_E_UNSUPPORTED, "Unsupported shuffle checksum algorithm%s");
   if (codec > B2S_CODEC_ZSTD) return fail(B2S_E_UNSUPPORTED, "codec %s not supported by this build", "");
-  const uint32_t key_len = spec.key_len;
+  const KeySpec& ks = spec.keys;
   if (spec.rows()) {
-    if (spec.key_type > B2S_KEY_INT64) return fail(B2S_E_ARG, "unknown key_type%s");
-    if (spec.key_type == B2S_KEY_BYTES && (key_len < 1 || key_len > 16))
-      return fail(B2S_E_ARG, "key_len must be in [1, 16]%s");
-    if (spec.key_type == B2S_KEY_INT32 && key_len != 4) return fail(B2S_E_ARG, "key_len of an INT32 key must be 4%s");
-    if (spec.key_type == B2S_KEY_INT64 && key_len != 8) return fail(B2S_E_ARG, "key_len of an INT64 key must be 8%s");
-    if (spec.null_field < -1) return fail(B2S_E_ARG, "null_field must be -1 or a field ordinal%s");
+    if (spec.n_keys < 1 || spec.n_keys > kMaxKeys) return fail(B2S_E_ARG, "n_keys must be in [1, 16]%s");
+    if (!spec.key_arrays) return fail(B2S_E_ARG, "null argument%s");
+    for (uint32_t c = 0; c < ks.n; c++) {
+      const uint32_t type = ks.type[c], key_len = ks.len[c];
+      if (type > B2S_KEY_INT64 && !(spec.strings && type == kStringKey)) return fail(B2S_E_ARG, "unknown key_type%s");
+      if (type == B2S_KEY_BYTES && (key_len < 1 || key_len > 16))
+        return fail(B2S_E_ARG, "key_len must be in [1, 16]%s");
+      if (type == B2S_KEY_INT32 && key_len != 4) return fail(B2S_E_ARG, "key_len of an INT32 key must be 4%s");
+      if (type == B2S_KEY_INT64 && key_len != 8) return fail(B2S_E_ARG, "key_len of an INT64 key must be 8%s");
+      if (type == kStringKey && key_len != 8) return fail(B2S_E_ARG, "key_len of a string key must be 8%s");
+      if (ks.null_field[c] < -1) return fail(B2S_E_ARG, "null_field must be -1 or a field ordinal%s");
+    }
     if (spec.aggregate)
       if (int rc = agg_args(spec)) return rc;
   } else {
+    const uint32_t key_len = ks.len[0];
     if (spec.record_bytes == 0) return fail(B2S_E_ARG, "record_bytes must be at least 1%s");
     if (key_len < 1 || key_len > 16) return fail(B2S_E_ARG, "key_len must be in [1, 16]%s");
-    if ((uint64_t)spec.key_off + key_len > spec.record_bytes)
+    if ((uint64_t)ks.off[0] + key_len > spec.record_bytes)
       return fail(B2S_E_ARG, "key_off + key_len exceeds record_bytes%s");
   }
   if (!dst_total || !n_records) return fail(B2S_E_ARG, "null argument%s");
@@ -2450,10 +2483,11 @@ struct SortSource {
 // one readback of the group count and output bytes (which checks out_cap), the heads' gather and the merge into
 // d_out.  *total = output bytes.  The dominant step is this one.
 static int aggregate_rows_tail(Slot& S, const RecordSpec& spec, const uint8_t* arena, uint64_t records,
-                               const uint32_t* idx, uint8_t* ws, uint8_t* aws, uint8_t* d_out, uint64_t out_cap,
-                               uint64_t* total, uint64_t* n_rec, uint64_t* n_groups, uint64_t* launches) {
+                               const uint32_t* idx, const uint32_t* heads, uint8_t* ws, uint8_t* aws, uint8_t* d_out,
+                               uint64_t out_cap, uint64_t* total, uint64_t* n_rec, uint64_t* n_groups,
+                               uint64_t* launches) {
   cudaStream_t st = S.st;
-  const uint32_t key_bytes = rows_key_bytes(spec.key_len, spec.null_field);
+  const uint32_t key_bytes = rows_key_bytes(spec.keys);
   AggSpec agg;
   agg.n = spec.n_aggs;
   for (uint32_t k = 0; k < agg.n; k++) {
@@ -2465,7 +2499,7 @@ static int aggregate_rows_tail(Slot& S, const RecordSpec& spec, const uint8_t* a
   uint64_t rb[2] = {0, 0};  // groups, output bytes
   CU(cudaEventRecord(S.ev_g[0], st));
   if (records) {
-    launch_rows_group(arena, records, idx, key_bytes, agg, ws, aws, st, launches);
+    launch_rows_group(arena, records, idx, heads, key_bytes, agg, ws, aws, st, launches);
     CU(cudaMemcpyAsync(rb, rows_aggregate_readback(aws, records, agg.n), sizeof rb, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
     CU(cudaGetLastError());
@@ -2635,10 +2669,10 @@ static int decompress_sort_run(Device* D, Slot& S, uint32_t codec, uint32_t alg,
   }
   if (!spec.rows()) {
     const uint64_t records = *total / spec.record_bytes;
-    if (records && (rc = S.pws.ensure(key_sort_ws_bytes(records, spec.key_len)))) return rc;
+    if (records && (rc = S.pws.ensure(key_sort_ws_bytes(records, spec.keys.len[0])))) return rc;
     CU(cudaEventRecord(S.ev_p0, st));
-    launch_key_sort(arena, records, spec.record_bytes, spec.key_off, spec.key_len, (uint8_t*)S.pws.p, *d_sorted, st,
-                    launches);
+    launch_key_sort(arena, records, spec.record_bytes, spec.keys.off[0], spec.keys.len[0], (uint8_t*)S.pws.p,
+                    *d_sorted, st, launches);
     CU(cudaEventRecord(S.ev_p1, st));
     CU(cudaStreamSynchronize(st));
     CU(cudaGetLastError());
@@ -2647,8 +2681,12 @@ static int decompress_sort_run(Device* D, Slot& S, uint32_t codec, uint32_t alg,
   }
 
   // rows: frame every source's range, then one readback of the record count and the verdicts
-  const uint64_t min_key = (uint64_t)spec.key_off + spec.key_len;
-  const uint64_t min_null = spec.null_field >= 0 ? 8ull * (uint32_t)(spec.null_field >> 6) + 8 : 0;
+  const KeySpec& ks = spec.keys;
+  uint64_t min_key = 0, min_null = 0;
+  for (uint32_t c = 0; c < ks.n; c++) {
+    min_key = std::max<uint64_t>(min_key, (uint64_t)ks.off[c] + ks.len[c]);
+    if (ks.null_field[c] >= 0) min_null = std::max<uint64_t>(min_null, null_word(ks.null_field[c]) + 8);
+  }
   if ((rc = S.fws.ensure(rows_frame_ws_bytes(*total, n_src)))) return rc;
   uint8_t* fws = (uint8_t*)S.fws.p;
   uint64_t frame_launches = *launches;
@@ -2662,45 +2700,75 @@ static int decompress_sort_run(Device* D, Slot& S, uint32_t codec, uint32_t alg,
                      cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
   CU(cudaGetLastError());
-  for (uint32_t i = 0; i < n_src; i++) {
-    const uint64_t v = rb[1 + i];
-    if (v == ~0ull) continue;
-    (cached(i) ? cached_status[i] : J.h.status[block(i)]) = B2S_E_CORRUPT;
-    if (!failed) {
-      static const char* const why[] = {"", "the block ends inside a size prefix", "the size is negative",
-                                        "the record runs past the block end", "the row is shorter than key_off + key_len",
-                                        "the row does not hold the null-bit word",
-                                        "the row is shorter than an aggregate slot"};
-      snprintf(msg, sizeof msg, "%s %u: bad row record at byte %llu: %s", cached(i) ? "cached source" : "block", i,
-               (unsigned long long)(v & ((1ull << 61) - 1)), why[v >> 61]);
-      fail(B2S_E_CORRUPT, "%s", msg);
+  // a source whose verdict (framing, or the key pass's string check) is not ~0 fails, the first one named
+  auto take_verdicts = [&](const uint64_t* v) {
+    for (uint32_t i = 0; i < n_src; i++) {
+      if (v[i] == ~0ull) continue;
+      (cached(i) ? cached_status[i] : J.h.status[block(i)]) = B2S_E_CORRUPT;
+      if (!failed) {
+        static const char* const why[] = {"", "the block ends inside a size prefix", "the size is negative",
+                                          "the record runs past the block end",
+                                          "the row is shorter than key_off + key_len",
+                                          "the row does not hold the null-bit word",
+                                          "the row is shorter than an aggregate slot",
+                                          "a string key runs past the end of its row"};
+        snprintf(msg, sizeof msg, "%s %u: bad row record at byte %llu: %s", cached(i) ? "cached source" : "block", i,
+                 (unsigned long long)(v[i] & ((1ull << 61) - 1)), why[v[i] >> 61]);
+        fail(B2S_E_CORRUPT, "%s", msg);
+      }
+      failed = true;
     }
-    failed = true;
-  }
-  if (failed) {
+  };
+  auto failed_rows = [&]() -> int {  // nothing is sorted or written
     report();
     CU(cudaEventRecord(S.ev_f[2], st));
     CU(cudaEventRecord(S.ev_f[3], st));
     CU(cudaEventRecord(S.ev_p1, st));
     CU(cudaStreamSynchronize(st));
     return 0;
-  }
+  };
+  take_verdicts(rb.data() + 1);
+  if (failed) return failed_rows();
   const uint64_t records = rb[0];
   if (records > 0xffffffffull)
     return fail(B2S_E_ARG, "more than 2^32 - 1 records in one call (%s records)", std::to_string(records).c_str());
-  const uint32_t key_bytes = rows_key_bytes(spec.key_len, spec.null_field);
+  const uint32_t key_bytes = rows_key_bytes(ks);
+  const bool refine = rows_key_refines(ks);
   const size_t sort_ws = rows_sort_ws_bytes(records, key_bytes);
   const size_t agg_ws = spec.aggregate ? rows_aggregate_ws_bytes(records, spec.n_aggs) : 0;
-  if (records && (rc = S.pws.ensure(sort_ws + agg_ws))) return rc;
+  const size_t refine_ws = refine ? rows_refine_ws_bytes(records, n_src) : 0;
+  if (records && (rc = S.pws.ensure(sort_ws + agg_ws + refine_ws))) return rc;
   uint8_t* ws = (uint8_t*)S.pws.p;
+  uint8_t* rws = refine ? ws + sort_ws + agg_ws : nullptr;
   CU(cudaEventRecord(S.ev_f[2], st));
   launch_rows_emit(arena, *total, n_src, fws, records, key_bytes, ws, st, launches);
   CU(cudaEventRecord(S.ev_f[3], st));
   frame_launches = *launches - frame_launches;
-  const uint32_t* idx = launch_rows_order(arena, records, spec.key_type, spec.key_off, spec.key_len, spec.null_field,
-                                          ws, st, launches);
-  if (spec.aggregate) return aggregate_rows_tail(S, spec, arena, records, idx, ws, ws + sort_ws, *d_sorted, out_cap,
-                                                 total, n_rec, n_groups, launches);
+  const uint32_t* idx = launch_rows_order(arena, records, ks, rows_frame_ranges(fws, *total, n_src), n_src, ws, rws,
+                                          st, launches);
+  const uint32_t* heads = nullptr;
+  if (refine && records) {
+    // one readback per round: the tied records and their runs (the first also brings the string verdicts)
+    std::vector<uint64_t> rrb(n_src + 1);
+    for (uint32_t d = kKeyPrefixBytes, round = 0;; d += kKeyChunkBytes, round++) {
+      launch_rows_refine_mark(records, d, rws, n_src, st, launches);
+      CU(cudaMemcpyAsync(rrb.data(), rows_refine_readback(rws, records, n_src), (round ? 1 : rrb.size()) * 8,
+                         cudaMemcpyDeviceToHost, st));
+      CU(cudaStreamSynchronize(st));
+      CU(cudaGetLastError());
+      if (!round) {
+        take_verdicts(rrb.data() + 1);
+        if (failed) return failed_rows();
+      }
+      const uint64_t tied = rrb[0] & 0xffffffffull, runs = rrb[0] >> 32;
+      if (!tied) break;
+      launch_rows_refine_round(arena, records, ks, tied, runs, d, ws, rws, n_src, st, launches);
+    }
+    idx = rows_refine_order(rws, records, n_src);
+    heads = rows_refine_heads(rws, records, n_src);
+  }
+  if (spec.aggregate) return aggregate_rows_tail(S, spec, arena, records, idx, heads, ws, ws + sort_ws, *d_sorted,
+                                                 out_cap, total, n_rec, n_groups, launches);
   launch_rows_gather(arena, records, key_bytes, idx, ws, *d_sorted, st, launches);
   CU(cudaEventRecord(S.ev_p1, st));
   CU(cudaStreamSynchronize(st));
@@ -2980,6 +3048,63 @@ int b2s_decompress_aggregate_rows_dev(uint32_t dev_index, uint32_t codec, uint32
   return aggregate_call(dev_index, false, codec, checksum_alg, n, src_base, src_off, src_len, slice_base, slice_len,
                         slice_checksum,
                         aggregate_spec(key_type, key_off, key_len, null_field, n_aggs, agg_op, agg_off, agg_null_field),
+                        dst_base, dst_cap, dst_total, n_records, n_groups, status, bad_slice);
+}
+
+int b2s_decompress_sort_rows_keys_packed(uint32_t codec, uint32_t checksum_alg, uint32_t n, const uint8_t* src_base,
+                                         const uint64_t* src_off, const uint64_t* src_len, const uint32_t* slice_base,
+                                         const uint64_t* slice_len, const uint64_t* slice_checksum, uint32_t n_keys,
+                                         const uint32_t* key_type, const uint32_t* key_off, const uint32_t* key_len,
+                                         const int32_t* key_null_field, uint8_t* dst_base, uint64_t dst_cap,
+                                         uint64_t* dst_total, uint64_t* n_records, int32_t* status,
+                                         int32_t* bad_slice) {
+  return sort_call(t_device, true, nullptr, codec, checksum_alg, n, src_base, src_off, src_len, slice_base, slice_len,
+                   slice_checksum, keys_spec(n_keys, key_type, key_off, key_len, key_null_field), dst_base, dst_cap,
+                   dst_total, n_records, status, bad_slice);
+}
+
+int b2s_decompress_sort_rows_keys_dev(uint32_t dev_index, uint32_t codec, uint32_t checksum_alg, uint32_t n,
+                                      const uint8_t* src_base, const uint64_t* src_off, const uint64_t* src_len,
+                                      const uint32_t* slice_base, const uint64_t* slice_len,
+                                      const uint64_t* slice_checksum, uint32_t n_keys, const uint32_t* key_type,
+                                      const uint32_t* key_off, const uint32_t* key_len, const int32_t* key_null_field,
+                                      uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records,
+                                      int32_t* status, int32_t* bad_slice) {
+  return sort_call(dev_index, false, nullptr, codec, checksum_alg, n, src_base, src_off, src_len, slice_base, slice_len,
+                   slice_checksum, keys_spec(n_keys, key_type, key_off, key_len, key_null_field), dst_base, dst_cap,
+                   dst_total, n_records, status, bad_slice);
+}
+
+int b2s_decompress_aggregate_rows_keys_packed(uint32_t codec, uint32_t checksum_alg, uint32_t n,
+                                              const uint8_t* src_base, const uint64_t* src_off,
+                                              const uint64_t* src_len, const uint32_t* slice_base,
+                                              const uint64_t* slice_len, const uint64_t* slice_checksum,
+                                              uint32_t n_keys, const uint32_t* key_type, const uint32_t* key_off,
+                                              const uint32_t* key_len, const int32_t* key_null_field, uint32_t n_aggs,
+                                              const uint32_t* agg_op, const uint32_t* agg_off,
+                                              const int32_t* agg_null_field, uint8_t* dst_base, uint64_t dst_cap,
+                                              uint64_t* dst_total, uint64_t* n_records, uint64_t* n_groups,
+                                              int32_t* status, int32_t* bad_slice) {
+  return aggregate_call(t_device, true, codec, checksum_alg, n, src_base, src_off, src_len, slice_base, slice_len,
+                        slice_checksum,
+                        with_aggregates(keys_spec(n_keys, key_type, key_off, key_len, key_null_field), n_aggs, agg_op,
+                                        agg_off, agg_null_field),
+                        dst_base, dst_cap, dst_total, n_records, n_groups, status, bad_slice);
+}
+
+int b2s_decompress_aggregate_rows_keys_dev(uint32_t dev_index, uint32_t codec, uint32_t checksum_alg, uint32_t n,
+                                           const uint8_t* src_base, const uint64_t* src_off, const uint64_t* src_len,
+                                           const uint32_t* slice_base, const uint64_t* slice_len,
+                                           const uint64_t* slice_checksum, uint32_t n_keys, const uint32_t* key_type,
+                                           const uint32_t* key_off, const uint32_t* key_len,
+                                           const int32_t* key_null_field, uint32_t n_aggs, const uint32_t* agg_op,
+                                           const uint32_t* agg_off, const int32_t* agg_null_field, uint8_t* dst_base,
+                                           uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records,
+                                           uint64_t* n_groups, int32_t* status, int32_t* bad_slice) {
+  return aggregate_call(dev_index, false, codec, checksum_alg, n, src_base, src_off, src_len, slice_base, slice_len,
+                        slice_checksum,
+                        with_aggregates(keys_spec(n_keys, key_type, key_off, key_len, key_null_field), n_aggs, agg_op,
+                                        agg_off, agg_null_field),
                         dst_base, dst_cap, dst_total, n_records, n_groups, status, bad_slice);
 }
 

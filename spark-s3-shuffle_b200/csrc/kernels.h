@@ -210,9 +210,10 @@ struct KeySortWs {
 };
 KeySortWs carve_key_sort_ws(uint8_t* d_ws, uint64_t n, uint32_t key_bytes);
 // LSD radix sort of the key words (one 8-bit pass per key byte, least significant first), stable; returns the sorted
-// record indices (nullptr when n < 2: input order)
+// record indices (nullptr when n < 2: input order).  lead_bytes (a key of more than one word): only the low lead_bytes
+// bytes of word 0 can be non-zero, so only they take passes.
 const uint32_t* launch_key_radix(const KeySortWs& w, uint64_t n, uint32_t key_bytes, cudaStream_t st,
-                                 uint64_t* launches);
+                                 uint64_t* launches, uint32_t lead_bytes = 4);
 
 // ---------------- rows.cu (stable sort of length-prefixed UnsafeRow records by a typed key) ----------------
 // Framing: the n_ranges decoded blocks [off[i], off[i] + len[i]) of the arena (arena_bytes long, 64 bytes of slack
@@ -221,25 +222,78 @@ const uint32_t* launch_key_radix(const KeySortWs& w, uint64_t n, uint32_t key_by
 // verdict of range 0, 1, ...]; a verdict is ~0 when the range is whole records, else kRowsBad* << 61 | the offset of the
 // range's first bad record.  A record is bad when its prefix is cut by the range end, its size is negative, it runs past
 // the range end, its row is shorter than min_key bytes, shorter than min_null bytes, or shorter than min_agg bytes.
+// kRowsBadString is the key pass's verdict (launch_rows_order): a non-null string key runs past its row.
 constexpr uint64_t kRowsBadPrefix = 1, kRowsBadNegative = 2, kRowsBadPastEnd = 3, kRowsBadKey = 4, kRowsBadNull = 5,
-                   kRowsBadAgg = 6;
+                   kRowsBadAgg = 6, kRowsBadString = 7;
 size_t rows_frame_ws_bytes(uint64_t arena_bytes, uint32_t n_ranges);
 inline size_t rows_frame_readback_bytes(uint32_t n_ranges) { return ((size_t)n_ranges + 1) * 8; }
 uint64_t* rows_frame_readback(uint8_t* d_fws, uint64_t arena_bytes, uint32_t n_ranges);
+// the ranges' arena offsets on the device (ascending), as launch_rows_frame uploaded them
+const uint64_t* rows_frame_ranges(uint8_t* d_fws, uint64_t arena_bytes, uint32_t n_ranges);
 void launch_rows_frame(const uint8_t* arena, uint64_t arena_bytes, const uint64_t* h_off, const uint64_t* h_len,
                        uint32_t n_ranges, uint64_t min_key, uint64_t min_null, uint64_t min_agg, uint8_t* d_fws,
                        cudaStream_t st, uint64_t* launches);
-// key bytes of the sort: key_len, plus the leading null byte of a nullable key
-inline uint32_t rows_key_bytes(uint32_t key_len, int32_t null_field) { return key_len + (null_field >= 0 ? 1 : 0); }
+// The sort key of a row: n columns compared left to right.  Column c: type[c] B2S_KEY_* or B2S_STRING_KEY at row offset
+// off[c], len[c] bytes (a string: its 8-byte slot, (offset << 32) | size), null bit null_field[c] (-1: never null).
+// It is encoded as one byte string compared by memcmp, prefix-free, column after column: a nullable column's null byte
+// (0 null, 1 not), then a fixed-width value big-endian with the sign bit of an int flipped (zero when null), or a
+// non-null string as groups of 8 bytes zero-padded, each followed by a marker: 9 when more bytes follow, else the number
+// of real bytes in the group (0..8); an empty string is one group of zeros with marker 0, a null string nothing.
+constexpr uint32_t kMaxKeys = 16;
+constexpr uint32_t kStringKey = B2S_STRING_KEY;
+struct KeySpec {
+  uint32_t n = 0;
+  uint32_t type[kMaxKeys] = {};
+  uint32_t off[kMaxKeys] = {};
+  uint32_t len[kMaxKeys] = {};
+  int32_t null_field[kMaxKeys] = {};
+};
+// The first pass radix-sorts the first kKeyPrefixBytes bytes of every encoded key (fewer when every key is shorter);
+// keys longer than that are refined in rounds of kKeyChunkBytes more bytes over the records still tied.
+constexpr uint32_t kKeyPrefixBytes = 20, kKeyChunkBytes = 16;
+// the encoded key's length when it is the same for every row (no string column), else ~0u
+inline uint32_t rows_key_encoded_bytes(const KeySpec& ks) {
+  uint32_t b = 0;
+  for (uint32_t c = 0; c < ks.n; c++) {
+    if (ks.type[c] == kStringKey) return ~0u;
+    b += ks.len[c] + (ks.null_field[c] >= 0 ? 1 : 0);
+  }
+  return b;
+}
+// key bytes of the first pass; a single column: key_len, plus the leading null byte of a nullable key
+inline uint32_t rows_key_bytes(const KeySpec& ks) {
+  const uint32_t b = rows_key_encoded_bytes(ks);
+  return b < kKeyPrefixBytes ? b : kKeyPrefixBytes;
+}
+inline bool rows_key_refines(const KeySpec& ks) { return rows_key_encoded_bytes(ks) > kKeyPrefixBytes; }
 size_t rows_sort_ws_bytes(uint64_t n, uint32_t key_bytes);
 // the framed records (n = the read-back count) as dense offsets and lengths in arena order, into the sort workspace
 void launch_rows_emit(const uint8_t* arena, uint64_t arena_bytes, uint32_t n_ranges, uint8_t* d_fws, uint64_t n,
                       uint32_t key_bytes, uint8_t* d_ws, cudaStream_t st, uint64_t* launches);
-// keys + radix: the emitted records' order, ascending by key (nulls first), stable, as sorted record indices (nullptr
-// when n < 2: arena order).  The key words stay in the workspace in record order.  key_type B2S_KEY_*
-const uint32_t* launch_rows_order(const uint8_t* arena, uint64_t n, uint32_t key_type, uint32_t key_off,
-                                  uint32_t key_len, int32_t null_field, uint8_t* d_ws, cudaStream_t st,
+// The refinement workspace (keys that refine): per record the encoded key length, per position the current order and
+// its group-head flags, the compaction's scan and maps, and the readback [tied records | segments << 32, string verdict
+// of range 0, 1, ...] (a verdict as rows_frame_readback's: ~0 or kRowsBadString << 61 | offset).
+size_t rows_refine_ws_bytes(uint64_t n, uint32_t n_ranges);
+uint64_t* rows_refine_readback(uint8_t* d_rws, uint64_t n, uint32_t n_ranges);
+// keys + radix: the emitted records' order by their first key_bytes encoded bytes, stable, as sorted record indices
+// (nullptr when n < 2: arena order).  The key words stay in the workspace in record order.  With d_rws (keys that
+// refine): also every key's encoded length and the string verdicts (ranges: rows_frame_ranges), and the order and
+// head flags that launch_rows_refine_* start from.
+const uint32_t* launch_rows_order(const uint8_t* arena, uint64_t n, const KeySpec& ks, const uint64_t* ranges,
+                                  uint32_t n_ranges, uint8_t* d_ws, uint8_t* d_rws, cudaStream_t st,
                                   uint64_t* launches);
+// Refinement round at encoded byte d (kKeyPrefixBytes, then + kKeyChunkBytes per round).  mark: the tied records (a
+// run of equal first-d-byte keys of two or more whose keys go on past d) counted into the readback.  round (m tied
+// records in segs runs, as read back): their next kKeyChunkBytes bytes extracted, the m records sorted stably by (run,
+// bytes) and put back into their runs' positions, the head flags split where the bytes differ.
+void launch_rows_refine_mark(uint64_t n, uint32_t d, uint8_t* d_rws, uint32_t n_ranges, cudaStream_t st,
+                             uint64_t* launches);
+void launch_rows_refine_round(const uint8_t* arena, uint64_t n, const KeySpec& ks, uint64_t m, uint64_t segs,
+                              uint32_t d, uint8_t* d_ws, uint8_t* d_rws, uint32_t n_ranges, cudaStream_t st,
+                              uint64_t* launches);
+// after the last round (no tied record): the sorted record indices, and per position 1 where a new key starts
+const uint32_t* rows_refine_order(uint8_t* d_rws, uint64_t n, uint32_t n_ranges);
+const uint32_t* rows_refine_heads(uint8_t* d_rws, uint64_t n, uint32_t n_ranges);
 // the emitted records to d_dst in the order idx
 void launch_rows_gather(const uint8_t* arena, uint64_t n, uint32_t key_bytes, const uint32_t* idx, uint8_t* d_ws,
                         uint8_t* d_dst, cudaStream_t st, uint64_t* launches);
@@ -258,9 +312,11 @@ size_t rows_aggregate_ws_bytes(uint64_t n, uint32_t n_aggs);
 // after launch_rows_group: [group count, output bytes] (device)
 uint64_t* rows_aggregate_readback(uint8_t* d_aws, uint64_t n, uint32_t n_aggs);
 // the groups of the records in the order idx (launch_rows_order): heads, group starts, the heads' output offsets and
-// the readback.  Also stages every aggregate's inputs in sorted order.
-void launch_rows_group(const uint8_t* arena, uint64_t n, const uint32_t* idx, uint32_t key_bytes, const AggSpec& spec,
-                       uint8_t* d_ws, uint8_t* d_aws, cudaStream_t st, uint64_t* launches);
+// the readback.  Also stages every aggregate's inputs in sorted order.  heads (keys that refine: rows_refine_heads)
+// flags where a new key starts; nullptr: where the key words differ.
+void launch_rows_group(const uint8_t* arena, uint64_t n, const uint32_t* idx, const uint32_t* heads,
+                       uint32_t key_bytes, const AggSpec& spec, uint8_t* d_ws, uint8_t* d_aws, cudaStream_t st,
+                       uint64_t* launches);
 // the groups (count read back) to d_dst: the first record of each, whole, with the aggregates' slots and null bits
 // replaced by the merged values
 void launch_rows_aggregate(const uint8_t* arena, uint64_t n, uint64_t groups, uint32_t key_bytes, uint32_t n_aggs,

@@ -8,9 +8,13 @@
 //            arena (1 bit per byte), and a block's first bad record goes to its verdict
 //   count  : set bits per 64 KiB tile of the arena, scanned: the record count, read back with the verdicts
 //   emit   : the bitmap compacted into dense record offsets (u64) and lengths (u32, prefix included), arena order
-//   keys   : one thread per record: the typed key as big-endian u32 words (int32 / int64: byte-swapped, sign bit
-//            flipped; a nullable key gets a leading byte 0 = null, 1 = non-null, and a null record's key bytes are 0)
+//   keys   : one thread per record: the first bytes (at most kKeyPrefixBytes) of the encoded key (kernels.h, KeySpec)
+//            as big-endian u32 words (one column: int32 / int64 byte-swapped, sign bit flipped; a nullable key gets a
+//            leading byte 0 = null, 1 = non-null, and a null record's key bytes are 0)
 //   radix  : the fixed-size sort's radix passes (launch_key_radix): the sorted record indices
+//   refine : only for keys longer than the first pass: rounds over the records still tied (runs of equal first bytes
+//            whose keys go on): compacted in order, their next kKeyChunkBytes bytes extracted behind their run number,
+//            radix-sorted stably and put back into their runs' positions, until no run is tied
 //   gather : sorted lengths -> scan -> destination offsets (launch_sorted_offsets), the partition step's gather (a row
 //            sort; a grouped aggregation gathers only each group's first record, aggregate.cu)
 #include <algorithm>
@@ -202,50 +206,218 @@ __global__ void __launch_bounds__(kRowThreads) rows_emit_kernel(const uint8_t* _
   }
 }
 
-// words[k * n + i] = key word k of record i (see the file comment), k < W
-__global__ void __launch_bounds__(kRowThreads) rows_keys_kernel(const uint8_t* __restrict__ arena,
-                                                                const uint64_t* __restrict__ rec_off, uint64_t n,
-                                                                uint32_t key_type, uint32_t key_off, uint32_t key_len,
-                                                                int32_t null_field, uint32_t W,
-                                                                uint32_t* __restrict__ words) {
-  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
-    const uint8_t* row = arena + rec_off[i] + 4;
-    uint64_t lo, hi;
-    ld_span16<true>(row + key_off, (int)key_len, lo, hi);
-    uint64_t top, bot;  // the key bytes as one 128-bit big-endian value, left-aligned
-    if (key_type == B2S_KEY_INT32) {
-      top = (uint64_t)((uint32_t)lo ^ 0x80000000u) << 32;
-      bot = 0;
-    } else if (key_type == B2S_KEY_INT64) {
-      top = lo ^ (1ull << 63);
-      bot = 0;
-    } else {
-      if (key_len < 8) {
-        lo &= (1ull << (8 * key_len)) - 1;
-        hi = 0;
-      } else if (key_len < 16) {
-        hi &= (1ull << (8 * (key_len - 8))) - 1;
-      }
-      top = __byte_perm((uint32_t)lo, 0, 0x0123);
-      top = (top << 32) | __byte_perm((uint32_t)(lo >> 32), 0, 0x0123);
-      bot = __byte_perm((uint32_t)hi, 0, 0x0123);
-      bot = (bot << 32) | __byte_perm((uint32_t)(hi >> 32), 0, 0x0123);
-    }
-    uint32_t spill = 0;
-    if (null_field >= 0) {
+// Bytes [d, d + nb) (nb <= 20) of one record's encoded key (kernels.h, KeySpec), as five big-endian u32 words.  Named
+// words, not an array: an array indexed by the byte position would live in local memory.
+struct KeyWindow {
+  uint32_t w0, w1, w2, w3, w4;
+  uint32_t d, nb;
+  __device__ __forceinline__ void put(uint32_t p, uint32_t v) {
+    const uint32_t q = p - d;
+    if (q >= nb) return;
+    const uint32_t x = v << (8 * (3 - (q & 3))), k = q >> 2;
+    w0 |= k == 0 ? x : 0u;
+    w1 |= k == 1 ? x : 0u;
+    w2 |= k == 2 ? x : 0u;
+    w3 |= k == 3 ? x : 0u;
+    w4 |= k == 4 ? x : 0u;
+  }
+  __device__ __forceinline__ uint32_t word(uint32_t k) const {
+    return k == 0 ? w0 : k == 1 ? w1 : k == 2 ? w2 : k == 3 ? w3 : w4;
+  }
+};
+
+// The window kw of the encoded key of a row of row_size bytes.  whole: every column is walked and the return value is
+// the key's encoded length (else the walk stops at the window's end).  *bad: a non-null string slot runs past the row;
+// its bytes are then clamped to the row, so no load leaves it.
+__device__ __forceinline__ uint32_t encode_key(const uint8_t* row, uint32_t row_size, const KeySpec& ks, KeyWindow& kw,
+                                               bool whole, bool* bad) {
+  const uint32_t wend = kw.d + kw.nb;
+  uint32_t p = 0;
+  for (uint32_t c = 0; c < ks.n; c++) {
+    if (!whole && p >= wend) break;
+    const uint32_t ty = ks.type[c], off = ks.off[c], len = ks.len[c];
+    const int32_t nf = ks.null_field[c];
+    bool is_null = false;
+    if (nf >= 0) {
       uint64_t nw, unused;
-      ld_span16<true>(row + 8 * (uint32_t)(null_field >> 6), 8, nw, unused);
-      const bool is_null = (nw >> (null_field & 63)) & 1;
-      if (is_null) top = bot = 0;
-      spill = (uint32_t)(bot & 0xff) << 24;
-      bot = (bot >> 8) | (top << 56);
-      top = (top >> 8) | ((uint64_t)(is_null ? 0 : 1) << 56);
+      ld_span16<true>(row + 8 * (uint32_t)(nf >> 6), 8, nw, unused);
+      is_null = (nw >> (nf & 63)) & 1;
+      kw.put(p++, is_null ? 0 : 1);
     }
-    const uint32_t kw[5] = {(uint32_t)(top >> 32), (uint32_t)top, (uint32_t)(bot >> 32), (uint32_t)bot, spill};
+    if (ty == kStringKey) {
+      if (is_null) continue;
+      uint64_t slot, unused;
+      ld_span16<true>(row + off, 8, slot, unused);
+      uint32_t so = (uint32_t)(slot >> 32), sz = (uint32_t)slot;
+      if ((uint64_t)so + sz > row_size) {
+        *bad = true;
+        so = min(so, row_size);
+        sz = min(sz, row_size - so);
+      }
+      const uint32_t groups = sz ? (sz + 7) / 8 : 1;
+      for (uint32_t g = kw.d > p ? (kw.d - p) / 9 : 0; g < groups && p + 9 * g < wend; g++) {
+        const uint32_t base = p + 9 * g, real = min(8u, sz - 8 * g);
+        uint64_t v = 0, unused2;
+        if (real) {
+          ld_span16<true>(row + so + 8 * g, (int)real, v, unused2);
+          if (real < 8) v &= (1ull << (8 * real)) - 1;
+        }
+        for (uint32_t b = 0; b < 8; b++) kw.put(base + b, (uint32_t)(v >> (8 * b)) & 0xff);
+        kw.put(base + 8, g + 1 < groups ? 9 : real);
+      }
+      p += 9 * groups;
+    } else {
+      if (!is_null && p < wend && p + len > kw.d) {  // a null's bytes stay zero
+        uint64_t lo, hi;
+        ld_span16<true>(row + off, (int)len, lo, hi);
+        for (uint32_t b = 0; b < len; b++) {
+          uint32_t v;
+          if (ty == B2S_KEY_BYTES) {
+            v = (uint32_t)(b < 8 ? lo >> (8 * b) : hi >> (8 * (b - 8))) & 0xff;
+          } else {  // little-endian two's complement: most significant byte first, sign bit flipped
+            v = (uint32_t)(lo >> (8 * (len - 1 - b))) & 0xff;
+            if (b == 0) v ^= 0x80;
+          }
+          kw.put(p + b, v);
+        }
+      }
+      p += len;
+    }
+  }
+  return p;
+}
+
+// The first pass: words[k * n + i] = word k of record i's encoded key, k < ceil(key_bytes / 4).  klen (keys that
+// refine): klen[i] = the encoded length, and a record whose string runs past its row lowers its range's verdict
+// (verdict[r], ranges: the ranges' arena offsets, ascending) to its offset in the range.
+__global__ void __launch_bounds__(kRowThreads) rows_keys_kernel(
+    const uint8_t* __restrict__ arena, const uint64_t* __restrict__ rec_off, const uint32_t* __restrict__ rec_len,
+    uint64_t n, const __grid_constant__ KeySpec ks, uint32_t key_bytes, uint32_t* __restrict__ words,
+    uint32_t* __restrict__ klen, const uint64_t* __restrict__ ranges, uint32_t n_ranges, uint64_t* __restrict__ verdict) {
+  const uint32_t W = (key_bytes + 3) / 4;
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+    const uint64_t ro = rec_off[i];
+    KeyWindow kw{0, 0, 0, 0, 0, 0, key_bytes};
+    bool bad = false;
+    const uint32_t len = encode_key(arena + ro + 4, rec_len[i] - 4, ks, kw, klen != nullptr, &bad);
 #pragma unroll
     for (uint32_t k = 0; k < 5; k++)
-      if (k < W) words[(size_t)k * n + i] = kw[k];
+      if (k < W) words[(size_t)k * n + i] = kw.word(k);
+    if (klen) klen[i] = len;
+    if (bad) {  // the range holding the record: the last that starts at or before it
+      uint32_t lo = 0, hi = n_ranges;
+      while (hi - lo > 1) {
+        const uint32_t mid = (lo + hi) / 2;
+        if (ranges[mid] <= ro) lo = mid;
+        else hi = mid;
+      }
+      atomicMin((unsigned long long*)(verdict + lo), (unsigned long long)((kRowsBadString << 61) | (ro - ranges[lo])));
+    }
   }
+}
+
+// ---- refinement (keys longer than the first pass: kernels.h, launch_rows_refine_*) ----
+// ord[j] = the record at position j of the current order, head[j] = 1 where a new key (so far) starts
+__global__ void __launch_bounds__(kRowThreads) refine_init_kernel(const uint32_t* __restrict__ idx, uint64_t n,
+                                                                  const uint32_t* __restrict__ words, uint32_t W,
+                                                                  uint32_t* __restrict__ ord,
+                                                                  uint32_t* __restrict__ head) {
+  for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (uint64_t)gridDim.x * blockDim.x) {
+    const uint32_t i = idx ? idx[j] : (uint32_t)j;
+    ord[j] = i;
+    bool h = j == 0;
+    if (!h) {
+      const uint32_t p = idx ? idx[j - 1] : (uint32_t)(j - 1);
+#pragma unroll
+      for (uint32_t k = 0; k < 5; k++)
+        if (k < W) h |= words[(size_t)k * n + i] != words[(size_t)k * n + p];
+    }
+    head[j] = h;
+  }
+}
+
+// Position j is tied at byte d: its run of equal keys so far has two or more records, and its key goes on past d.
+// Keys equal over [0, d) end together or both go on (the encoding is prefix-free), so a run is tied as a whole.
+__device__ __forceinline__ bool tied(uint64_t j, uint64_t n, uint32_t d, const uint32_t* __restrict__ ord,
+                                     const uint32_t* __restrict__ head, const uint32_t* __restrict__ klen) {
+  return klen[ord[j]] > d && (!head[j] || (j + 1 < n && !head[j + 1]));
+}
+
+// scan[j] = head[j] << 32 | 1 for a tied position, else 0: its exclusive scan numbers the tied records and their runs
+__global__ void __launch_bounds__(kRowThreads) refine_mark_kernel(const uint32_t* __restrict__ ord,
+                                                                  const uint32_t* __restrict__ head,
+                                                                  const uint32_t* __restrict__ klen, uint64_t n,
+                                                                  uint32_t d, uint64_t* __restrict__ scan) {
+  for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (uint64_t)gridDim.x * blockDim.x)
+    scan[j] = tied(j, n, d, ord, head, klen) ? ((uint64_t)head[j] << 32) | 1 : 0;
+}
+
+// tied position j, the k-th tied record, of run s: cpos[k] = j, cidx[k] = its record; its sort key (stride m) = s,
+// then its encoded key bytes [d, d + kKeyChunkBytes)
+__global__ void __launch_bounds__(kRowThreads) refine_extract_kernel(
+    const uint8_t* __restrict__ arena, const uint64_t* __restrict__ rec_off, const uint32_t* __restrict__ rec_len,
+    uint64_t n, const __grid_constant__ KeySpec ks, const uint32_t* __restrict__ ord, const uint32_t* __restrict__ head,
+    const uint32_t* __restrict__ klen, const uint64_t* __restrict__ scan, uint64_t m, uint32_t d,
+    uint32_t* __restrict__ cpos, uint32_t* __restrict__ cidx, uint32_t* __restrict__ words) {
+  for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (uint64_t)gridDim.x * blockDim.x) {
+    if (!tied(j, n, d, ord, head, klen)) continue;
+    const uint32_t k = (uint32_t)scan[j], s = (uint32_t)(scan[j] >> 32) + head[j] - 1;
+    const uint32_t i = ord[j];
+    cpos[k] = (uint32_t)j;
+    cidx[k] = i;
+    KeyWindow kw{0, 0, 0, 0, 0, d, kKeyChunkBytes};
+    bool bad = false;
+    encode_key(arena + rec_off[i] + 4, rec_len[i] - 4, ks, kw, false, &bad);
+    words[k] = s;
+#pragma unroll
+    for (uint32_t q = 0; q < 4; q++) words[(size_t)(q + 1) * m + k] = kw.word(q);
+  }
+}
+
+// the k-th of the sorted tied records (sidx) to the k-th tied position; a new key starts where (run, bytes) changes
+__global__ void __launch_bounds__(kRowThreads) refine_scatter_kernel(const uint32_t* __restrict__ sidx, uint64_t m,
+                                                                     const uint32_t* __restrict__ words,
+                                                                     const uint32_t* __restrict__ cpos,
+                                                                     const uint32_t* __restrict__ cidx,
+                                                                     uint32_t* __restrict__ ord,
+                                                                     uint32_t* __restrict__ head) {
+  for (uint64_t k = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; k < m; k += (uint64_t)gridDim.x * blockDim.x) {
+    const uint32_t r = sidx ? sidx[k] : (uint32_t)k, j = cpos[k];
+    ord[j] = cidx[r];
+    bool h = k == 0;
+    if (!h) {
+      const uint32_t p = sidx ? sidx[k - 1] : (uint32_t)(k - 1);
+#pragma unroll
+      for (uint32_t q = 0; q < 5; q++) h |= words[(size_t)q * m + r] != words[(size_t)q * m + p];
+    }
+    head[j] = h;
+  }
+}
+
+// the refinement workspace (kernels.h, rows_refine_ws_bytes)
+struct RefineWs {
+  uint32_t* ord;
+  uint32_t* head;
+  uint32_t* klen;
+  uint32_t* cpos;
+  uint32_t* cidx;
+  uint64_t* scan;
+  uint64_t* scan_ws;
+  uint64_t* readback;
+};
+
+RefineWs carve_refine_ws(uint8_t* d_rws, uint64_t n) {
+  RefineWs r;
+  uint8_t* p = d_rws;
+  r.ord = (uint32_t*)p;     p += a256(n * 4);
+  r.head = (uint32_t*)p;    p += a256(n * 4);
+  r.klen = (uint32_t*)p;    p += a256(n * 4);
+  r.cpos = (uint32_t*)p;    p += a256(n * 4);
+  r.cidx = (uint32_t*)p;    p += a256(n * 4);
+  r.scan = (uint64_t*)p;    p += a256(n * 8);
+  r.scan_ws = (uint64_t*)p; p += a256(scan_ws_elems(n) * 8);
+  r.readback = (uint64_t*)p;
+  return r;
 }
 
 // the framing workspace: bitmap (whole tiles), tile counts, their scan workspace, readback, ranges, work counter
@@ -329,16 +501,60 @@ void launch_rows_emit(const uint8_t* arena, uint64_t arena_bytes, uint32_t n_ran
   if (launches) *launches += 1;
 }
 
-const uint32_t* launch_rows_order(const uint8_t* arena, uint64_t n, uint32_t key_type, uint32_t key_off,
-                                  uint32_t key_len, int32_t null_field, uint8_t* d_ws, cudaStream_t st,
+const uint64_t* rows_frame_ranges(uint8_t* d_fws, uint64_t arena_bytes, uint32_t n_ranges) {
+  return carve_frame_ws(d_fws, arena_bytes, n_ranges).r_off;
+}
+
+size_t rows_refine_ws_bytes(uint64_t n, uint32_t n_ranges) {
+  return 5 * a256(n * 4) + a256(n * 8) + a256(scan_ws_elems(n) * 8) + a256(((size_t)n_ranges + 1) * 8);
+}
+
+uint64_t* rows_refine_readback(uint8_t* d_rws, uint64_t n, uint32_t) { return carve_refine_ws(d_rws, n).readback; }
+const uint32_t* rows_refine_order(uint8_t* d_rws, uint64_t n, uint32_t) { return carve_refine_ws(d_rws, n).ord; }
+const uint32_t* rows_refine_heads(uint8_t* d_rws, uint64_t n, uint32_t) { return carve_refine_ws(d_rws, n).head; }
+
+const uint32_t* launch_rows_order(const uint8_t* arena, uint64_t n, const KeySpec& ks, const uint64_t* ranges,
+                                  uint32_t n_ranges, uint8_t* d_ws, uint8_t* d_rws, cudaStream_t st,
                                   uint64_t* launches) {
   if (!n) return nullptr;
-  const uint32_t key_bytes = rows_key_bytes(key_len, null_field);
+  const uint32_t key_bytes = rows_key_bytes(ks);
   const KeySortWs w = carve_key_sort_ws(d_ws, n, key_bytes);
-  rows_keys_kernel<<<grid_for(n), kRowThreads, 0, st>>>(arena, w.src_off, n, key_type, key_off, key_len, null_field,
-                                                        (key_bytes + 3) / 4, w.words);
+  RefineWs r{};
+  if (d_rws) {
+    r = carve_refine_ws(d_rws, n);
+    cudaMemsetAsync(r.readback + 1, 0xff, (size_t)n_ranges * 8, st);
+  }
+  rows_keys_kernel<<<grid_for(n), kRowThreads, 0, st>>>(arena, w.src_off, w.len, n, ks, key_bytes, w.words, r.klen,
+                                                        ranges, n_ranges, d_rws ? r.readback + 1 : nullptr);
   if (launches) *launches += 1;
-  return launch_key_radix(w, n, key_bytes, st, launches);
+  const uint32_t* idx = launch_key_radix(w, n, key_bytes, st, launches);
+  if (d_rws) {
+    refine_init_kernel<<<grid_for(n), kRowThreads, 0, st>>>(idx, n, w.words, (key_bytes + 3) / 4, r.ord, r.head);
+    if (launches) *launches += 1;
+  }
+  return idx;
+}
+
+void launch_rows_refine_mark(uint64_t n, uint32_t d, uint8_t* d_rws, uint32_t, cudaStream_t st, uint64_t* launches) {
+  const RefineWs r = carve_refine_ws(d_rws, n);
+  refine_mark_kernel<<<grid_for(n), kRowThreads, 0, st>>>(r.ord, r.head, r.klen, n, d, r.scan);
+  launch_exclusive_scan_u64(r.scan, n, r.readback, r.scan_ws, st, launches);
+  if (launches) *launches += 1;
+}
+
+void launch_rows_refine_round(const uint8_t* arena, uint64_t n, const KeySpec& ks, uint64_t m, uint64_t segs,
+                              uint32_t d, uint8_t* d_ws, uint8_t* d_rws, uint32_t, cudaStream_t st,
+                              uint64_t* launches) {
+  // the first pass's workspace, its key words no longer needed: the m tied records' keys at stride m
+  const KeySortWs w = carve_key_sort_ws(d_ws, n, kKeyPrefixBytes);
+  const RefineWs r = carve_refine_ws(d_rws, n);
+  refine_extract_kernel<<<grid_for(n), kRowThreads, 0, st>>>(arena, w.src_off, w.len, n, ks, r.ord, r.head, r.klen,
+                                                             r.scan, m, d, r.cpos, r.cidx, w.words);
+  // the run number takes as many passes as it has bytes (none for a single run)
+  const uint32_t lead = segs <= 1 ? 0 : segs <= 256 ? 1 : segs <= 65536 ? 2 : segs <= (1u << 24) ? 3 : 4;
+  const uint32_t* sidx = launch_key_radix(w, m, 4 + kKeyChunkBytes, st, launches, lead);
+  refine_scatter_kernel<<<grid_for(m), kRowThreads, 0, st>>>(sidx, m, w.words, r.cpos, r.cidx, r.ord, r.head);
+  if (launches) *launches += 2;
 }
 
 void launch_rows_gather(const uint8_t* arena, uint64_t n, uint32_t key_bytes, const uint32_t* idx, uint8_t* d_ws,

@@ -95,12 +95,17 @@ KeySortWs carve_key_sort_ws(uint8_t* d_ws, uint64_t n, uint32_t key_bytes) {
 }
 
 const uint32_t* launch_key_radix(const KeySortWs& w, uint64_t n, uint32_t key_bytes, cudaStream_t st,
-                                 uint64_t* launches) {
+                                 uint64_t* launches, uint32_t lead_bytes) {
   if (n < 2) return nullptr;
   const uint32_t W = (key_bytes + 3) / 4;
   const uint32_t* idx = nullptr;  // current order; nullptr = input order
   uint32_t pass = 0;
   for (int k = (int)W - 1; k >= 0; k--) {
+    // the last word holds key_bytes - 4 (W - 1) real bytes in its high end; word 0 of several, lead_bytes in its low
+    // end; the others hold four
+    const uint32_t real = k == (int)W - 1 ? key_bytes - 4 * (W - 1) : 4;
+    const uint32_t end = k == 0 && W > 1 ? 8 * lead_bytes : 32;
+    if (32 - 8 * real >= end) continue;
     const uint32_t* kin = w.words + (size_t)k * n;
     if (idx) {  // the current keys' buffer is free again: put this word there, in the current order
       uint32_t* kg = w.K[(pass - 1) & 1];
@@ -108,9 +113,7 @@ const uint32_t* launch_key_radix(const KeySortWs& w, uint64_t n, uint32_t key_by
       if (launches) *launches += 1;
       kin = kg;
     }
-    // the last word holds key_bytes - 4 (W - 1) real bytes in its high end; the others hold four
-    const uint32_t real = k == (int)W - 1 ? key_bytes - 4 * (W - 1) : 4;
-    for (uint32_t shift = 32 - 8 * real; shift < 32; shift += 8, pass++) {
+    for (uint32_t shift = 32 - 8 * real; shift < end; shift += 8, pass++) {
       launch_radix_pass(kin, idx, (uint32_t)n, (int)shift, 256, w.hist, w.total, w.scan_ws, w.K[pass & 1],
                         w.I[pass & 1], st, launches);
       kin = w.K[pass & 1];

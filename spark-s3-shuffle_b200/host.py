@@ -11,6 +11,13 @@ from . import _build
 OK, E_RUNTIME, E_IO, E_SPARK, E_UNSUPPORTED, E_CODEC = 0, -101, -102, -103, -104, -105
 
 
+
+def _key_columns(keys):
+    """[(type, offset, length, null field), ...] -> the four parallel arrays of the composite-key reads"""
+    keys = list(keys)
+    col = [np.array([k[c] for k in keys] or [0], dtype=np.uint32 if c < 3 else np.int32) for c in range(4)]
+    return tuple(col)
+
 class RuntimeException(RuntimeError):
     """java.lang.RuntimeException (preconditions, length mismatch: shuffle/S3ShuffleMapOutputWriter.scala:68-73,96-100)"""
 
@@ -65,6 +72,11 @@ PROTOTYPES = [
      [_vp, _u32, _u32, _u32, _i32, C.POINTER(_vp), C.POINTER(_u64), C.POINTER(_u64)]),
     ("b2sh_reader_read_aggregated_rows", C.c_int,
      [_vp, _u32, _u32, _u32, _i32, _u32, _vp, _vp, _vp, C.POINTER(_vp), C.POINTER(_u64), C.POINTER(_u64),
+      C.POINTER(_u64)]),
+    ("b2sh_reader_read_sorted_rows_keys", C.c_int,
+     [_vp, _u32, _vp, _vp, _vp, _vp, C.POINTER(_vp), C.POINTER(_u64), C.POINTER(_u64)]),
+    ("b2sh_reader_read_aggregated_rows_keys", C.c_int,
+     [_vp, _u32, _vp, _vp, _vp, _vp, _u32, _vp, _vp, _vp, C.POINTER(_vp), C.POINTER(_u64), C.POINTER(_u64),
       C.POINTER(_u64)]),
     ("b2sh_reader_block", C.c_int,
      [_vp, _u32, C.POINTER(_i64), C.POINTER(_i32), C.POINTER(_i32), C.POINTER(_vp), C.POINTER(_u64)]),
@@ -357,6 +369,31 @@ class S3ShuffleReader:
         _check(load().b2sh_reader_read_aggregated_rows(self._h, keyType, keyOffset, keyLength, nullField, len(aggs),
                                                        op.ctypes.data, off.ctypes.data, nf.ctypes.data, C.byref(p),
                                                        C.byref(ln), C.byref(nrec), C.byref(ngrp)))
+        return (C.string_at(p.value, ln.value) if ln.value else b""), nrec.value, ngrp.value
+
+    def readSortedRowsKeys(self, keys):
+        """readSortedRows by a composite key: keys = [(keyType or STRING_KEY, keyOffset, keyLength, nullField), ...],
+        compared left to right.  -> (bytes, number of records)"""
+        kt, ko, kl, kn = _key_columns(keys)
+        p, ln, nrec = _vp(), _u64(), _u64()
+        _check(load().b2sh_reader_read_sorted_rows_keys(self._h, len(keys), kt.ctypes.data, ko.ctypes.data,
+                                                        kl.ctypes.data, kn.ctypes.data, C.byref(p), C.byref(ln),
+                                                        C.byref(nrec)))
+        return (C.string_at(p.value, ln.value) if ln.value else b""), nrec.value
+
+    def readAggregatedRowsKeys(self, keys, aggs=()):
+        """readAggregatedRows grouped by a composite key (keys as in readSortedRowsKeys).
+        -> (bytes, number of input records, number of groups)"""
+        kt, ko, kl, kn = _key_columns(keys)
+        aggs = list(aggs)
+        op = np.array([a[0] for a in aggs] or [0], dtype=np.uint32)
+        off = np.array([a[1] for a in aggs] or [0], dtype=np.uint32)
+        nf = np.array([a[2] for a in aggs] or [0], dtype=np.int32)
+        p, ln, nrec, ngrp = _vp(), _u64(), _u64(), _u64()
+        _check(load().b2sh_reader_read_aggregated_rows_keys(self._h, len(keys), kt.ctypes.data, ko.ctypes.data,
+                                                            kl.ctypes.data, kn.ctypes.data, len(aggs), op.ctypes.data,
+                                                            off.ctypes.data, nf.ctypes.data, C.byref(p), C.byref(ln),
+                                                            C.byref(nrec), C.byref(ngrp)))
         return (C.string_at(p.value, ln.value) if ln.value else b""), nrec.value, ngrp.value
 
     def _blocks(self, n):

@@ -838,8 +838,21 @@ class S3ShuffleReader {
   // then reduce-id order.  Codec NONE is verified and sorted only.  It reads fetched blocks only: the exchange cache is
   // not consulted.
   void readSortedRows(uint32_t keyType, uint32_t keyOff, uint32_t keyLen, int32_t nullField) {
-    readRows(keyType, keyOff, keyLen, nullField, nullptr);
+    readRows(RowKeys{1, &keyType, &keyOff, &keyLen, &nullField, false}, nullptr);
   }
+  // The key columns of readSortedRowsKeys / readAggregatedRowsKeys: column c is type[c] (B2S_KEY_* or B2S_STRING_KEY)
+  // at row offset off[c], len[c] bytes, null bit nullField[c].  composite: the *_rows_keys_* calls, else the one-key ones.
+  struct RowKeys {
+    uint32_t n;
+    const uint32_t* type;
+    const uint32_t* off;
+    const uint32_t* len;
+    const int32_t* nullField;
+    bool composite;
+  };
+  // readSortedRows by a composite key of up to 16 columns, strings included: ONE b2s_decompress_sort_rows_keys_packed
+  // call.  The exchange cache is not consulted.
+  void readSortedRowsKeys(const RowKeys& keys) { readRows(keys, nullptr); }
   // The aggregates of readAggregatedRows: aggregate k is op[k] (B2S_AGG_*) over the 8-byte slot at row offset off[k],
   // null bit nullField[k] (-1 = never null).
   struct RowAggregates {
@@ -854,16 +867,19 @@ class S3ShuffleReader {
   // consulted.
   void readAggregatedRows(uint32_t keyType, uint32_t keyOff, uint32_t keyLen, int32_t nullField,
                           const RowAggregates& aggs) {
-    readRows(keyType, keyOff, keyLen, nullField, &aggs);
+    readRows(RowKeys{1, &keyType, &keyOff, &keyLen, &nullField, false}, &aggs);
   }
+  // readAggregatedRows grouped by a composite key (readSortedRowsKeys): ONE b2s_decompress_aggregate_rows_keys_packed
+  // call.  The exchange cache is not consulted.
+  void readAggregatedRowsKeys(const RowKeys& keys, const RowAggregates& aggs) { readRows(keys, &aggs); }
   const uint8_t* sortedData() const { return sorted_.get(); }
   uint64_t sortedLen() const { return sortedLen_; }
   uint64_t sortedRecords() const { return sortedRecords_; }
   uint64_t sortedGroups() const { return sortedGroups_; }
 
  private:
-  // the body of readSortedRows (aggs == nullptr) and readAggregatedRows
-  void readRows(uint32_t keyType, uint32_t keyOff, uint32_t keyLen, int32_t nullField, const RowAggregates* aggs) {
+  // the body of the row reads: sorted (aggs == nullptr) or aggregated, by one key or a composite one
+  void readRows(const RowKeys& keys, const RowAggregates* aggs) {
     start(true);
     std::vector<std::pair<uint64_t, std::vector<uint8_t>>> fetched;  // (tag, compressed bytes)
     drainWhole(fetched);
@@ -896,21 +912,33 @@ class S3ShuffleReader {
     for (int attempt = 0; attempt < 2 && rc == B2S_E_DST_TOO_SMALL; attempt++) {
       if (attempt) cap = total;
       sorted_.reset(new uint8_t[(size_t)(cap ? cap : 1)]);
-      if (aggs)
-        rc = b2s_decompress_aggregate_rows_packed(
-            codec, alg, n, src.data(), off.data(), len.data(), verify ? sliceBase.data() : nullptr,
-            verify ? sliceLen.data() : nullptr, verify ? sliceSum.data() : nullptr, keyType, keyOff, keyLen, nullField,
-            aggs->n, aggs->op, aggs->off, aggs->nullField, sorted_.get(), cap, &total, &records, &groups,
-            status.data(), bad.data());
+      const uint32_t* sb = verify ? sliceBase.data() : nullptr;
+      const uint64_t* sl = verify ? sliceLen.data() : nullptr;
+      const uint64_t* sc = verify ? sliceSum.data() : nullptr;
+      if (aggs && keys.composite)
+        rc = b2s_decompress_aggregate_rows_keys_packed(codec, alg, n, src.data(), off.data(), len.data(), sb, sl, sc,
+                                                       keys.n, keys.type, keys.off, keys.len, keys.nullField, aggs->n,
+                                                       aggs->op, aggs->off, aggs->nullField, sorted_.get(), cap,
+                                                       &total, &records, &groups, status.data(), bad.data());
+      else if (aggs)
+        rc = b2s_decompress_aggregate_rows_packed(codec, alg, n, src.data(), off.data(), len.data(), sb, sl, sc,
+                                                  keys.type[0], keys.off[0], keys.len[0], keys.nullField[0], aggs->n,
+                                                  aggs->op, aggs->off, aggs->nullField, sorted_.get(), cap, &total,
+                                                  &records, &groups, status.data(), bad.data());
+      else if (keys.composite)
+        rc = b2s_decompress_sort_rows_keys_packed(codec, alg, n, src.data(), off.data(), len.data(), sb, sl, sc, keys.n,
+                                                  keys.type, keys.off, keys.len, keys.nullField, sorted_.get(), cap,
+                                                  &total, &records, status.data(), bad.data());
       else
-        rc = b2s_decompress_sort_rows_packed(codec, alg, n, src.data(), off.data(), len.data(),
-                                             verify ? sliceBase.data() : nullptr, verify ? sliceLen.data() : nullptr,
-                                             verify ? sliceSum.data() : nullptr, keyType, keyOff, keyLen, nullField,
-                                             sorted_.get(), cap, &total, &records, status.data(), bad.data());
+        rc = b2s_decompress_sort_rows_packed(codec, alg, n, src.data(), off.data(), len.data(), sb, sl, sc,
+                                             keys.type[0], keys.off[0], keys.len[0], keys.nullField[0], sorted_.get(),
+                                             cap, &total, &records, status.data(), bad.data());
     }
     if (rc != 0)
-      throw CodecException(std::string(aggs ? "b2s_decompress_aggregate_rows_packed: "
-                                            : "b2s_decompress_sort_rows_packed: ") +
+      throw CodecException(std::string(aggs ? (keys.composite ? "b2s_decompress_aggregate_rows_keys_packed: "
+                                                              : "b2s_decompress_aggregate_rows_packed: ")
+                                            : (keys.composite ? "b2s_decompress_sort_rows_keys_packed: "
+                                                              : "b2s_decompress_sort_rows_packed: ")) +
                            b2s_strerror(rc) + ": " + b2s_last_error());
     for (uint32_t k = 0; k < n; k++) {
       if (status[k] == B2S_E_CHECKSUM)  // storage/S3ChecksumValidationStream.scala:72-74
@@ -1313,6 +1341,31 @@ int b2sh_reader_read_aggregated_rows(b2sh_reader* r, uint32_t key_type, uint32_t
   return guarded([&] {
     r->r->readAggregatedRows(key_type, key_off, key_len, null_field,
                              S3ShuffleReader::RowAggregates{n_aggs, agg_op, agg_off, agg_null_field});
+    *data = r->r->sortedData();
+    *len = r->r->sortedLen();
+    *n_records = r->r->sortedRecords();
+    *n_groups = r->r->sortedGroups();
+  });
+}
+int b2sh_reader_read_sorted_rows_keys(b2sh_reader* r, uint32_t n_keys, const uint32_t* key_type,
+                                      const uint32_t* key_off, const uint32_t* key_len, const int32_t* key_null_field,
+                                      const uint8_t** data, uint64_t* len, uint64_t* n_records) {
+  return guarded([&] {
+    r->r->readSortedRowsKeys(S3ShuffleReader::RowKeys{n_keys, key_type, key_off, key_len, key_null_field, true});
+    *data = r->r->sortedData();
+    *len = r->r->sortedLen();
+    *n_records = r->r->sortedRecords();
+  });
+}
+int b2sh_reader_read_aggregated_rows_keys(b2sh_reader* r, uint32_t n_keys, const uint32_t* key_type,
+                                          const uint32_t* key_off, const uint32_t* key_len,
+                                          const int32_t* key_null_field, uint32_t n_aggs, const uint32_t* agg_op,
+                                          const uint32_t* agg_off, const int32_t* agg_null_field,
+                                          const uint8_t** data, uint64_t* len, uint64_t* n_records,
+                                          uint64_t* n_groups) {
+  return guarded([&] {
+    r->r->readAggregatedRowsKeys(S3ShuffleReader::RowKeys{n_keys, key_type, key_off, key_len, key_null_field, true},
+                                 S3ShuffleReader::RowAggregates{n_aggs, agg_op, agg_off, agg_null_field});
     *data = r->r->sortedData();
     *len = r->r->sortedLen();
     *n_records = r->r->sortedRecords();
