@@ -361,17 +361,20 @@ def decompress_batch(codec, blocks, checksum_alg=CHECKSUM_NONE, slices=None, dst
     return res, [int(v) for v in st[:n]], [int(v) for v in bad[:n]]
 
 
+def _slice_arrays(checksum_alg, slice_base, slice_len, slice_checksum):
+    if checksum_alg == CHECKSUM_NONE:
+        return None, None, None
+    return (np.ascontiguousarray(slice_base, dtype=np.uint32), np.ascontiguousarray(slice_len, dtype=np.uint64),
+            np.ascontiguousarray(slice_checksum, dtype=np.uint64))
+
+
 def decompress_packed(codec, src, off, length, dst, checksum_alg=CHECKSUM_NONE, slice_base=None, slice_len=None,
                       slice_checksum=None):
     src, dst = _as_u8(src), _as_u8(dst)
     off = np.ascontiguousarray(off, dtype=np.uint64)
     length = np.ascontiguousarray(length, dtype=np.uint64)
     n = off.size
-    sb = sl = sc = None
-    if checksum_alg != CHECKSUM_NONE:
-        sb = np.ascontiguousarray(slice_base, dtype=np.uint32)
-        sl = np.ascontiguousarray(slice_len, dtype=np.uint64)
-        sc = np.ascontiguousarray(slice_checksum, dtype=np.uint64)
+    sb, sl, sc = _slice_arrays(checksum_alg, slice_base, slice_len, slice_checksum)
     dst_off = np.zeros(max(n, 1), dtype=np.uint64)
     dst_len = np.zeros(max(n, 1), dtype=np.uint64)
     st = np.zeros(max(n, 1), dtype=np.int32)
@@ -383,52 +386,6 @@ def decompress_packed(codec, src, off, length, dst, checksum_alg=CHECKSUM_NONE, 
     return dict(dst_off=dst_off[:n], dst_len=dst_len[:n], total=total.value, status=st[:n], bad_slice=bad[:n])
 
 
-def _sort_slices(checksum_alg, slice_base, slice_len, slice_checksum):
-    if checksum_alg == CHECKSUM_NONE:
-        return None, None, None
-    return (np.ascontiguousarray(slice_base, dtype=np.uint32), np.ascontiguousarray(slice_len, dtype=np.uint64),
-            np.ascontiguousarray(slice_checksum, dtype=np.uint64))
-
-
-def decompress_sort_packed(codec, src, off, length, dst, record_bytes, key_off, key_len, checksum_alg=CHECKSUM_NONE,
-                           slice_base=None, slice_len=None, slice_checksum=None):
-    """Verifies and decodes a reduce task's blocks and sorts their fixed-size records by the unsigned bytes
-    [key_off, key_off + key_len) into dst (stable).  -> dict(total, n_records, status, bad_slice)"""
-    src, dst = _as_u8(src), _as_u8(dst)
-    off = np.ascontiguousarray(off, dtype=np.uint64)
-    length = np.ascontiguousarray(length, dtype=np.uint64)
-    n = off.size
-    sb, sl, sc = _sort_slices(checksum_alg, slice_base, slice_len, slice_checksum)
-    st = np.zeros(max(n, 1), dtype=np.int32)
-    bad = np.zeros(max(n, 1), dtype=np.int32)
-    total, nrec = _u64(0), _u64(0)
-    _check(load().b2s_decompress_sort_packed(codec, checksum_alg, n, _ptr(src), _ptr(off), _ptr(length), _ptr(sb),
-                                             _ptr(sl), _ptr(sc), record_bytes, key_off, key_len, _ptr(dst), dst.size,
-                                             C.addressof(total), C.addressof(nrec), _ptr(st), _ptr(bad)),
-           "b2s_decompress_sort_packed")
-    return dict(total=total.value, n_records=nrec.value, status=st[:n], bad_slice=bad[:n])
-
-
-def decompress_sort_rows_packed(codec, src, off, length, dst, key_type, key_off, key_len, null_field=-1,
-                                checksum_alg=CHECKSUM_NONE, slice_base=None, slice_len=None, slice_checksum=None):
-    """Verifies and decodes a reduce task's blocks of length-prefixed UnsafeRow records ([int32 big-endian size][row])
-    and sorts the records by the typed key at row offset key_off (KEY_BYTES / KEY_INT32 / KEY_INT64; nulls first when
-    null_field >= 0) into dst (stable).  -> dict(total, n_records, status, bad_slice)"""
-    src, dst = _as_u8(src), _as_u8(dst)
-    off = np.ascontiguousarray(off, dtype=np.uint64)
-    length = np.ascontiguousarray(length, dtype=np.uint64)
-    n = off.size
-    sb, sl, sc = _sort_slices(checksum_alg, slice_base, slice_len, slice_checksum)
-    st = np.zeros(max(n, 1), dtype=np.int32)
-    bad = np.zeros(max(n, 1), dtype=np.int32)
-    total, nrec = _u64(0), _u64(0)
-    _check(load().b2s_decompress_sort_rows_packed(codec, checksum_alg, n, _ptr(src), _ptr(off), _ptr(length), _ptr(sb),
-                                                  _ptr(sl), _ptr(sc), key_type, key_off, key_len, null_field,
-                                                  _ptr(dst), dst.size, C.addressof(total), C.addressof(nrec), _ptr(st),
-                                                  _ptr(bad)), "b2s_decompress_sort_rows_packed")
-    return dict(total=total.value, n_records=nrec.value, status=st[:n], bad_slice=bad[:n])
-
-
 def _agg_arrays(aggs):
     """aggs = [(op, off, null_field), ...] -> (n, op, off, null_field) arrays"""
     aggs = list(aggs)
@@ -436,30 +393,6 @@ def _agg_arrays(aggs):
     off = np.array([a[1] for a in aggs] or [0], dtype=np.uint32)
     nf = np.array([a[2] for a in aggs] or [0], dtype=np.int32)
     return len(aggs), op, off, nf
-
-
-def decompress_aggregate_rows_packed(codec, src, off, length, dst, key_type, key_off, key_len, null_field=-1, aggs=(),
-                                     checksum_alg=CHECKSUM_NONE, slice_base=None, slice_len=None, slice_checksum=None):
-    """Verifies and decodes a reduce task's blocks of UnsafeRow records, groups them by the typed key (as
-    decompress_sort_rows_packed orders them) and merges every aggregate (op AGG_*, 8-byte slot at row offset off,
-    null bit null_field or -1) over each group into one row per group in dst.
-    -> dict(total, n_records, n_groups, status, bad_slice)"""
-    src, dst = _as_u8(src), _as_u8(dst)
-    off = np.ascontiguousarray(off, dtype=np.uint64)
-    length = np.ascontiguousarray(length, dtype=np.uint64)
-    n = off.size
-    sb, sl, sc = _sort_slices(checksum_alg, slice_base, slice_len, slice_checksum)
-    na, aop, aoff, anf = _agg_arrays(aggs)
-    st = np.zeros(max(n, 1), dtype=np.int32)
-    bad = np.zeros(max(n, 1), dtype=np.int32)
-    total, nrec, ngrp = _u64(0), _u64(0), _u64(0)
-    _check(load().b2s_decompress_aggregate_rows_packed(codec, checksum_alg, n, _ptr(src), _ptr(off), _ptr(length),
-                                                       _ptr(sb), _ptr(sl), _ptr(sc), key_type, key_off, key_len,
-                                                       null_field, na, _ptr(aop), _ptr(aoff), _ptr(anf), _ptr(dst),
-                                                       dst.size, C.addressof(total), C.addressof(nrec),
-                                                       C.addressof(ngrp), _ptr(st), _ptr(bad)),
-           "b2s_decompress_aggregate_rows_packed")
-    return dict(total=total.value, n_records=nrec.value, n_groups=ngrp.value, status=st[:n], bad_slice=bad[:n])
 
 
 def _key_arrays(keys):
@@ -472,48 +405,77 @@ def _key_arrays(keys):
     return len(keys), kt, ko, kl, kn
 
 
+def _arg(a):
+    return _ptr(a) if isinstance(a, np.ndarray) else a
+
+
+def _sort_call(symbol, codec, src, off, length, dst, dst_cap, mid, checksum_alg, slices, dev=None, lead=(), n=None):
+    """One call of the sort family, whose arguments are [dev,] *lead, codec, checksum_alg, n, src, off, length, the
+    three slice arrays, *mid, dst, dst_cap, total, n_records, [n_groups,] status, bad_slice.  dev None: the packed form,
+    src and dst host arrays (dst_cap is dst's size); else src and dst are device addresses.  lead and mid are the
+    call's own arguments, numpy arrays among them passed as pointers; n defaults to the number of blocks in off.
+    -> dict(total, n_records, status, bad_slice), with n_groups after n_records for the aggregate calls"""
+    if dev is None:
+        src, dst = _as_u8(src), _as_u8(dst)
+        dst_cap = dst.size
+    off = np.ascontiguousarray(off, dtype=np.uint64)
+    length = np.ascontiguousarray(length, dtype=np.uint64)
+    n = off.size if n is None else n
+    sb, sl, sc = _slice_arrays(checksum_alg, *slices)
+    st = np.zeros(max(n, 1), dtype=np.int32)
+    bad = np.zeros(max(n, 1), dtype=np.int32)
+    groups = "_aggregate_" in symbol
+    counts = [_u64(0) for _ in range(3 if groups else 2)]
+    args = ([] if dev is None else [dev]) + [*lead, codec, checksum_alg, n, src, off, length, sb, sl, sc, *mid, dst,
+                                             dst_cap]
+    _check(getattr(load(), symbol)(*map(_arg, args), *map(C.addressof, counts), _ptr(st), _ptr(bad)), symbol)
+    r = dict(zip(("total", "n_records", "n_groups"), (c.value for c in counts)))
+    r.update(status=st[:n], bad_slice=bad[:n])
+    return r
+
+
+def decompress_sort_packed(codec, src, off, length, dst, record_bytes, key_off, key_len, checksum_alg=CHECKSUM_NONE,
+                           slice_base=None, slice_len=None, slice_checksum=None):
+    """Verifies and decodes a reduce task's blocks and sorts their fixed-size records by the unsigned bytes
+    [key_off, key_off + key_len) into dst (stable).  -> dict(total, n_records, status, bad_slice)"""
+    return _sort_call("b2s_decompress_sort_packed", codec, src, off, length, dst, None,
+                      (record_bytes, key_off, key_len), checksum_alg, (slice_base, slice_len, slice_checksum))
+
+
+def decompress_sort_rows_packed(codec, src, off, length, dst, key_type, key_off, key_len, null_field=-1,
+                                checksum_alg=CHECKSUM_NONE, slice_base=None, slice_len=None, slice_checksum=None):
+    """Verifies and decodes a reduce task's blocks of length-prefixed UnsafeRow records ([int32 big-endian size][row])
+    and sorts the records by the typed key at row offset key_off (KEY_BYTES / KEY_INT32 / KEY_INT64; nulls first when
+    null_field >= 0) into dst (stable).  -> dict(total, n_records, status, bad_slice)"""
+    return _sort_call("b2s_decompress_sort_rows_packed", codec, src, off, length, dst, None,
+                      (key_type, key_off, key_len, null_field), checksum_alg, (slice_base, slice_len, slice_checksum))
+
+
+def decompress_aggregate_rows_packed(codec, src, off, length, dst, key_type, key_off, key_len, null_field=-1, aggs=(),
+                                     checksum_alg=CHECKSUM_NONE, slice_base=None, slice_len=None, slice_checksum=None):
+    """Verifies and decodes a reduce task's blocks of UnsafeRow records, groups them by the typed key (as
+    decompress_sort_rows_packed orders them) and merges every aggregate (op AGG_*, 8-byte slot at row offset off,
+    null bit null_field or -1) over each group into one row per group in dst.
+    -> dict(total, n_records, n_groups, status, bad_slice)"""
+    return _sort_call("b2s_decompress_aggregate_rows_packed", codec, src, off, length, dst, None,
+                      (key_type, key_off, key_len, null_field, *_agg_arrays(aggs)), checksum_alg,
+                      (slice_base, slice_len, slice_checksum))
+
+
 def decompress_sort_rows_keys_packed(codec, src, off, length, dst, keys, checksum_alg=CHECKSUM_NONE, slice_base=None,
                                      slice_len=None, slice_checksum=None):
     """decompress_sort_rows_packed by a composite key: keys = [(KEY_* or STRING_KEY, row offset, length, null field
     or -1), ...], compared left to right.  -> dict(total, n_records, status, bad_slice)"""
-    src, dst = _as_u8(src), _as_u8(dst)
-    off = np.ascontiguousarray(off, dtype=np.uint64)
-    length = np.ascontiguousarray(length, dtype=np.uint64)
-    n = off.size
-    sb, sl, sc = _sort_slices(checksum_alg, slice_base, slice_len, slice_checksum)
-    nk, kt, ko, kl, kn = _key_arrays(keys)
-    st = np.zeros(max(n, 1), dtype=np.int32)
-    bad = np.zeros(max(n, 1), dtype=np.int32)
-    total, nrec = _u64(0), _u64(0)
-    _check(load().b2s_decompress_sort_rows_keys_packed(codec, checksum_alg, n, _ptr(src), _ptr(off), _ptr(length),
-                                                       _ptr(sb), _ptr(sl), _ptr(sc), nk, _ptr(kt), _ptr(ko), _ptr(kl),
-                                                       _ptr(kn), _ptr(dst), dst.size, C.addressof(total),
-                                                       C.addressof(nrec), _ptr(st), _ptr(bad)),
-           "b2s_decompress_sort_rows_keys_packed")
-    return dict(total=total.value, n_records=nrec.value, status=st[:n], bad_slice=bad[:n])
+    return _sort_call("b2s_decompress_sort_rows_keys_packed", codec, src, off, length, dst, None, _key_arrays(keys),
+                      checksum_alg, (slice_base, slice_len, slice_checksum))
 
 
 def decompress_aggregate_rows_keys_packed(codec, src, off, length, dst, keys, aggs=(), checksum_alg=CHECKSUM_NONE,
                                           slice_base=None, slice_len=None, slice_checksum=None):
     """decompress_aggregate_rows_packed grouped by a composite key (keys as in decompress_sort_rows_keys_packed).
     -> dict(total, n_records, n_groups, status, bad_slice)"""
-    src, dst = _as_u8(src), _as_u8(dst)
-    off = np.ascontiguousarray(off, dtype=np.uint64)
-    length = np.ascontiguousarray(length, dtype=np.uint64)
-    n = off.size
-    sb, sl, sc = _sort_slices(checksum_alg, slice_base, slice_len, slice_checksum)
-    nk, kt, ko, kl, kn = _key_arrays(keys)
-    na, aop, aoff, anf = _agg_arrays(aggs)
-    st = np.zeros(max(n, 1), dtype=np.int32)
-    bad = np.zeros(max(n, 1), dtype=np.int32)
-    total, nrec, ngrp = _u64(0), _u64(0), _u64(0)
-    _check(load().b2s_decompress_aggregate_rows_keys_packed(codec, checksum_alg, n, _ptr(src), _ptr(off), _ptr(length),
-                                                            _ptr(sb), _ptr(sl), _ptr(sc), nk, _ptr(kt), _ptr(ko),
-                                                            _ptr(kl), _ptr(kn), na, _ptr(aop), _ptr(aoff), _ptr(anf),
-                                                            _ptr(dst), dst.size, C.addressof(total), C.addressof(nrec),
-                                                            C.addressof(ngrp), _ptr(st), _ptr(bad)),
-           "b2s_decompress_aggregate_rows_keys_packed")
-    return dict(total=total.value, n_records=nrec.value, n_groups=ngrp.value, status=st[:n], bad_slice=bad[:n])
+    return _sort_call("b2s_decompress_aggregate_rows_keys_packed", codec, src, off, length, dst, None,
+                      (*_key_arrays(keys), *_agg_arrays(aggs)), checksum_alg, (slice_base, slice_len, slice_checksum))
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -566,11 +528,7 @@ def decompress_dev(codec, d_src, off, length, d_dst, dst_cap, checksum_alg=CHECK
     off = np.ascontiguousarray(off, dtype=np.uint64)
     length = np.ascontiguousarray(length, dtype=np.uint64)
     n = off.size
-    sb = sl = sc = None
-    if checksum_alg != CHECKSUM_NONE:
-        sb = np.ascontiguousarray(slice_base, dtype=np.uint32)
-        sl = np.ascontiguousarray(slice_len, dtype=np.uint64)
-        sc = np.ascontiguousarray(slice_checksum, dtype=np.uint64)
+    sb, sl, sc = _slice_arrays(checksum_alg, slice_base, slice_len, slice_checksum)
     dst_off = np.zeros(max(n, 1), dtype=np.uint64)
     dst_len = np.zeros(max(n, 1), dtype=np.uint64)
     st = np.zeros(max(n, 1), dtype=np.int32)
@@ -585,95 +543,41 @@ def decompress_dev(codec, d_src, off, length, d_dst, dst_cap, checksum_alg=CHECK
 def decompress_sort_dev(codec, d_src, off, length, d_dst, dst_cap, record_bytes, key_off, key_len,
                         checksum_alg=CHECKSUM_NONE, slice_base=None, slice_len=None, slice_checksum=None, dev=0):
     """decompress_sort_packed on device-resident blocks (d_src) into a device arena (d_dst)"""
-    off = np.ascontiguousarray(off, dtype=np.uint64)
-    length = np.ascontiguousarray(length, dtype=np.uint64)
-    n = off.size
-    sb, sl, sc = _sort_slices(checksum_alg, slice_base, slice_len, slice_checksum)
-    st = np.zeros(max(n, 1), dtype=np.int32)
-    bad = np.zeros(max(n, 1), dtype=np.int32)
-    total, nrec = _u64(0), _u64(0)
-    _check(load().b2s_decompress_sort_dev(dev, codec, checksum_alg, n, d_src, _ptr(off), _ptr(length), _ptr(sb),
-                                          _ptr(sl), _ptr(sc), record_bytes, key_off, key_len, d_dst, dst_cap,
-                                          C.addressof(total), C.addressof(nrec), _ptr(st), _ptr(bad)),
-           "b2s_decompress_sort_dev")
-    return dict(total=total.value, n_records=nrec.value, status=st[:n], bad_slice=bad[:n])
+    return _sort_call("b2s_decompress_sort_dev", codec, d_src, off, length, d_dst, dst_cap,
+                      (record_bytes, key_off, key_len), checksum_alg, (slice_base, slice_len, slice_checksum), dev)
 
 
 def decompress_sort_rows_dev(codec, d_src, off, length, d_dst, dst_cap, key_type, key_off, key_len, null_field=-1,
                              checksum_alg=CHECKSUM_NONE, slice_base=None, slice_len=None, slice_checksum=None, dev=0):
     """decompress_sort_rows_packed on device-resident blocks (d_src) into a device arena (d_dst)"""
-    off = np.ascontiguousarray(off, dtype=np.uint64)
-    length = np.ascontiguousarray(length, dtype=np.uint64)
-    n = off.size
-    sb, sl, sc = _sort_slices(checksum_alg, slice_base, slice_len, slice_checksum)
-    st = np.zeros(max(n, 1), dtype=np.int32)
-    bad = np.zeros(max(n, 1), dtype=np.int32)
-    total, nrec = _u64(0), _u64(0)
-    _check(load().b2s_decompress_sort_rows_dev(dev, codec, checksum_alg, n, d_src, _ptr(off), _ptr(length), _ptr(sb),
-                                               _ptr(sl), _ptr(sc), key_type, key_off, key_len, null_field, d_dst,
-                                               dst_cap, C.addressof(total), C.addressof(nrec), _ptr(st), _ptr(bad)),
-           "b2s_decompress_sort_rows_dev")
-    return dict(total=total.value, n_records=nrec.value, status=st[:n], bad_slice=bad[:n])
+    return _sort_call("b2s_decompress_sort_rows_dev", codec, d_src, off, length, d_dst, dst_cap,
+                      (key_type, key_off, key_len, null_field), checksum_alg, (slice_base, slice_len, slice_checksum),
+                      dev)
 
 
 def decompress_aggregate_rows_dev(codec, d_src, off, length, d_dst, dst_cap, key_type, key_off, key_len,
                                   null_field=-1, aggs=(), checksum_alg=CHECKSUM_NONE, slice_base=None, slice_len=None,
                                   slice_checksum=None, dev=0):
     """decompress_aggregate_rows_packed on device-resident blocks (d_src) into a device arena (d_dst)"""
-    off = np.ascontiguousarray(off, dtype=np.uint64)
-    length = np.ascontiguousarray(length, dtype=np.uint64)
-    n = off.size
-    sb, sl, sc = _sort_slices(checksum_alg, slice_base, slice_len, slice_checksum)
-    na, aop, aoff, anf = _agg_arrays(aggs)
-    st = np.zeros(max(n, 1), dtype=np.int32)
-    bad = np.zeros(max(n, 1), dtype=np.int32)
-    total, nrec, ngrp = _u64(0), _u64(0), _u64(0)
-    _check(load().b2s_decompress_aggregate_rows_dev(dev, codec, checksum_alg, n, d_src, _ptr(off), _ptr(length),
-                                                    _ptr(sb), _ptr(sl), _ptr(sc), key_type, key_off, key_len,
-                                                    null_field, na, _ptr(aop), _ptr(aoff), _ptr(anf), d_dst, dst_cap,
-                                                    C.addressof(total), C.addressof(nrec), C.addressof(ngrp), _ptr(st),
-                                                    _ptr(bad)), "b2s_decompress_aggregate_rows_dev")
-    return dict(total=total.value, n_records=nrec.value, n_groups=ngrp.value, status=st[:n], bad_slice=bad[:n])
+    return _sort_call("b2s_decompress_aggregate_rows_dev", codec, d_src, off, length, d_dst, dst_cap,
+                      (key_type, key_off, key_len, null_field, *_agg_arrays(aggs)), checksum_alg,
+                      (slice_base, slice_len, slice_checksum), dev)
 
 
 def decompress_sort_rows_keys_dev(codec, d_src, off, length, d_dst, dst_cap, keys, checksum_alg=CHECKSUM_NONE,
                                   slice_base=None, slice_len=None, slice_checksum=None, dev=0):
     """decompress_sort_rows_keys_packed on device-resident blocks (d_src) into a device arena (d_dst)"""
-    off = np.ascontiguousarray(off, dtype=np.uint64)
-    length = np.ascontiguousarray(length, dtype=np.uint64)
-    n = off.size
-    sb, sl, sc = _sort_slices(checksum_alg, slice_base, slice_len, slice_checksum)
-    nk, kt, ko, kl, kn = _key_arrays(keys)
-    st = np.zeros(max(n, 1), dtype=np.int32)
-    bad = np.zeros(max(n, 1), dtype=np.int32)
-    total, nrec = _u64(0), _u64(0)
-    _check(load().b2s_decompress_sort_rows_keys_dev(dev, codec, checksum_alg, n, d_src, _ptr(off), _ptr(length),
-                                                    _ptr(sb), _ptr(sl), _ptr(sc), nk, _ptr(kt), _ptr(ko), _ptr(kl),
-                                                    _ptr(kn), d_dst, dst_cap, C.addressof(total), C.addressof(nrec),
-                                                    _ptr(st), _ptr(bad)), "b2s_decompress_sort_rows_keys_dev")
-    return dict(total=total.value, n_records=nrec.value, status=st[:n], bad_slice=bad[:n])
+    return _sort_call("b2s_decompress_sort_rows_keys_dev", codec, d_src, off, length, d_dst, dst_cap,
+                      _key_arrays(keys), checksum_alg, (slice_base, slice_len, slice_checksum), dev)
 
 
 def decompress_aggregate_rows_keys_dev(codec, d_src, off, length, d_dst, dst_cap, keys, aggs=(),
                                        checksum_alg=CHECKSUM_NONE, slice_base=None, slice_len=None,
                                        slice_checksum=None, dev=0):
     """decompress_aggregate_rows_keys_packed on device-resident blocks (d_src) into a device arena (d_dst)"""
-    off = np.ascontiguousarray(off, dtype=np.uint64)
-    length = np.ascontiguousarray(length, dtype=np.uint64)
-    n = off.size
-    sb, sl, sc = _sort_slices(checksum_alg, slice_base, slice_len, slice_checksum)
-    nk, kt, ko, kl, kn = _key_arrays(keys)
-    na, aop, aoff, anf = _agg_arrays(aggs)
-    st = np.zeros(max(n, 1), dtype=np.int32)
-    bad = np.zeros(max(n, 1), dtype=np.int32)
-    total, nrec, ngrp = _u64(0), _u64(0), _u64(0)
-    _check(load().b2s_decompress_aggregate_rows_keys_dev(dev, codec, checksum_alg, n, d_src, _ptr(off), _ptr(length),
-                                                         _ptr(sb), _ptr(sl), _ptr(sc), nk, _ptr(kt), _ptr(ko),
-                                                         _ptr(kl), _ptr(kn), na, _ptr(aop), _ptr(aoff), _ptr(anf),
-                                                         d_dst, dst_cap, C.addressof(total), C.addressof(nrec),
-                                                         C.addressof(ngrp), _ptr(st), _ptr(bad)),
-           "b2s_decompress_aggregate_rows_keys_dev")
-    return dict(total=total.value, n_records=nrec.value, n_groups=ngrp.value, status=st[:n], bad_slice=bad[:n])
+    return _sort_call("b2s_decompress_aggregate_rows_keys_dev", codec, d_src, off, length, d_dst, dst_cap,
+                      (*_key_arrays(keys), *_agg_arrays(aggs)), checksum_alg, (slice_base, slice_len, slice_checksum),
+                      dev)
 
 
 def partition_compress_dev(codec, d_records, rec_bytes, d_rec_len, d_rec_part, n_records, num_partitions, d_dst,
@@ -748,20 +652,9 @@ def exchange_read_sort_packed(shuffle_id, start_reduce, end_reduce, map_ids, cac
     """decompress_sort_packed over sources of which those with cached[i] set are the cached range of map_ids[i].
     -> dict(total, n_records, status, bad_slice)"""
     ids, cm = _exchange_sources(map_ids, cached)
-    src, dst = _as_u8(src), _as_u8(dst)
-    off = np.ascontiguousarray(off, dtype=np.uint64)
-    length = np.ascontiguousarray(length, dtype=np.uint64)
-    n = ids.size
-    sb, sl, sc = _sort_slices(checksum_alg, slice_base, slice_len, slice_checksum)
-    st = np.zeros(max(n, 1), dtype=np.int32)
-    bad = np.zeros(max(n, 1), dtype=np.int32)
-    total, nrec = _u64(0), _u64(0)
-    _check(load().b2s_exchange_read_sort_packed(shuffle_id, start_reduce, end_reduce, _ptr(ids), _ptr(cm), codec,
-                                                checksum_alg, n, _ptr(src), _ptr(off), _ptr(length), _ptr(sb),
-                                                _ptr(sl), _ptr(sc), record_bytes, key_off, key_len, _ptr(dst),
-                                                dst.size, C.addressof(total), C.addressof(nrec), _ptr(st), _ptr(bad)),
-           "b2s_exchange_read_sort_packed")
-    return dict(total=total.value, n_records=nrec.value, status=st[:n], bad_slice=bad[:n])
+    return _sort_call("b2s_exchange_read_sort_packed", codec, src, off, length, dst, None,
+                      (record_bytes, key_off, key_len), checksum_alg, (slice_base, slice_len, slice_checksum),
+                      lead=(shuffle_id, start_reduce, end_reduce, ids, cm), n=ids.size)
 
 
 def exchange_read_sort_dev(shuffle_id, start_reduce, end_reduce, map_ids, cached, codec, d_src, off, length, d_dst,
@@ -769,19 +662,9 @@ def exchange_read_sort_dev(shuffle_id, start_reduce, end_reduce, map_ids, cached
                            slice_len=None, slice_checksum=None, dev=0):
     """exchange_read_sort_packed with the fetched blocks (d_src) and the output (d_dst) in device memory"""
     ids, cm = _exchange_sources(map_ids, cached)
-    off = np.ascontiguousarray(off, dtype=np.uint64)
-    length = np.ascontiguousarray(length, dtype=np.uint64)
-    n = ids.size
-    sb, sl, sc = _sort_slices(checksum_alg, slice_base, slice_len, slice_checksum)
-    st = np.zeros(max(n, 1), dtype=np.int32)
-    bad = np.zeros(max(n, 1), dtype=np.int32)
-    total, nrec = _u64(0), _u64(0)
-    _check(load().b2s_exchange_read_sort_dev(dev, shuffle_id, start_reduce, end_reduce, _ptr(ids), _ptr(cm), codec,
-                                             checksum_alg, n, d_src, _ptr(off), _ptr(length), _ptr(sb), _ptr(sl),
-                                             _ptr(sc), record_bytes, key_off, key_len, d_dst, dst_cap,
-                                             C.addressof(total), C.addressof(nrec), _ptr(st), _ptr(bad)),
-           "b2s_exchange_read_sort_dev")
-    return dict(total=total.value, n_records=nrec.value, status=st[:n], bad_slice=bad[:n])
+    return _sort_call("b2s_exchange_read_sort_dev", codec, d_src, off, length, d_dst, dst_cap,
+                      (record_bytes, key_off, key_len), checksum_alg, (slice_base, slice_len, slice_checksum), dev,
+                      lead=(shuffle_id, start_reduce, end_reduce, ids, cm), n=ids.size)
 
 
 def exchange_remove(shuffle_id, map_id=-1):

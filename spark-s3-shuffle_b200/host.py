@@ -7,16 +7,10 @@ import ctypes as C
 import numpy as np
 
 from . import _build
+from .capi import _agg_arrays, _arg, _key_arrays
 
 OK, E_RUNTIME, E_IO, E_SPARK, E_UNSUPPORTED, E_CODEC = 0, -101, -102, -103, -104, -105
 
-
-
-def _key_columns(keys):
-    """[(type, offset, length, null field), ...] -> the four parallel arrays of the composite-key reads"""
-    keys = list(keys)
-    col = [np.array([k[c] for k in keys] or [0], dtype=np.uint32 if c < 3 else np.int32) for c in range(4)]
-    return tuple(col)
 
 class RuntimeException(RuntimeError):
     """java.lang.RuntimeException (preconditions, length mismatch: shuffle/S3ShuffleMapOutputWriter.scala:68-73,96-100)"""
@@ -325,6 +319,15 @@ class S3SingleSpillShuffleMapOutputWriter:
                                                  pl.ctypes.data, ck.ctypes.data, pl.size, int(verifyOnTransfer)))
 
 
+def _read_sorted(h, fn, *args, groups=False):
+    """fn(h, *args, &data, &len, &records[, &groups]): one of the reader's sorted reads, numpy arrays in args passed as
+    pointers.  -> (bytes, number of records[, number of groups])"""
+    p, ln, nrec, ngrp = _vp(), _u64(), _u64(), _u64()
+    counts = (nrec, ngrp) if groups else (nrec,)
+    _check(fn(h, *map(_arg, args), C.byref(p), C.byref(ln), *map(C.byref, counts)))
+    return ((C.string_at(p.value, ln.value) if ln.value else b""),) + tuple(c.value for c in counts)
+
+
 class S3ShuffleReader:
     """storage/S3ShuffleReader.scala — read() yields (blockName-parts, decoded bytes) per non-empty block."""
 
@@ -342,59 +345,32 @@ class S3ShuffleReader:
     def readSorted(self, recordBytes, keyOffset, keyLength):
         """read() with a key ordering (spark.shuffle.s3.gpu.sortKey=recordBytes,keyOffset,keyLength): every record
         of the task in ascending unsigned-byte key order, stable.  -> (bytes, number of records)"""
-        p, ln, nrec = _vp(), _u64(), _u64()
-        _check(load().b2sh_reader_read_sorted(self._h, recordBytes, keyOffset, keyLength, C.byref(p), C.byref(ln),
-                                              C.byref(nrec)))
-        return (C.string_at(p.value, ln.value) if ln.value else b""), nrec.value
+        return _read_sorted(self._h, load().b2sh_reader_read_sorted, recordBytes, keyOffset, keyLength)
 
     def readSortedRows(self, keyType, keyOffset, keyLength, nullField=-1):
         """read() of a SQL exchange sorted by one typed key (spark.shuffle.s3.gpu.sortRows): every UnsafeRowSerializer
         record of the task in ascending key order, nulls first, stable.  Fetched blocks only (no exchange cache).
         -> (bytes, number of records)"""
-        p, ln, nrec = _vp(), _u64(), _u64()
-        _check(load().b2sh_reader_read_sorted_rows(self._h, keyType, keyOffset, keyLength, nullField, C.byref(p),
-                                                   C.byref(ln), C.byref(nrec)))
-        return (C.string_at(p.value, ln.value) if ln.value else b""), nrec.value
+        return _read_sorted(self._h, load().b2sh_reader_read_sorted_rows, keyType, keyOffset, keyLength, nullField)
 
     def readAggregatedRows(self, keyType, keyOffset, keyLength, nullField=-1, aggs=()):
         """read() of a SQL exchange whose partial aggregates are merged by one typed key
         (spark.shuffle.s3.gpu.aggregateRows): one UnsafeRowSerializer record per key, in the row sort's order, with
         each aggregate (op, offset, null field) merged over the key's records.  Fetched blocks only (no exchange cache).
         -> (bytes, number of input records, number of groups)"""
-        aggs = list(aggs)
-        op = np.array([a[0] for a in aggs] or [0], dtype=np.uint32)
-        off = np.array([a[1] for a in aggs] or [0], dtype=np.uint32)
-        nf = np.array([a[2] for a in aggs] or [0], dtype=np.int32)
-        p, ln, nrec, ngrp = _vp(), _u64(), _u64(), _u64()
-        _check(load().b2sh_reader_read_aggregated_rows(self._h, keyType, keyOffset, keyLength, nullField, len(aggs),
-                                                       op.ctypes.data, off.ctypes.data, nf.ctypes.data, C.byref(p),
-                                                       C.byref(ln), C.byref(nrec), C.byref(ngrp)))
-        return (C.string_at(p.value, ln.value) if ln.value else b""), nrec.value, ngrp.value
+        return _read_sorted(self._h, load().b2sh_reader_read_aggregated_rows, keyType, keyOffset, keyLength,
+                            nullField, *_agg_arrays(aggs), groups=True)
 
     def readSortedRowsKeys(self, keys):
         """readSortedRows by a composite key: keys = [(keyType or STRING_KEY, keyOffset, keyLength, nullField), ...],
         compared left to right.  -> (bytes, number of records)"""
-        kt, ko, kl, kn = _key_columns(keys)
-        p, ln, nrec = _vp(), _u64(), _u64()
-        _check(load().b2sh_reader_read_sorted_rows_keys(self._h, len(keys), kt.ctypes.data, ko.ctypes.data,
-                                                        kl.ctypes.data, kn.ctypes.data, C.byref(p), C.byref(ln),
-                                                        C.byref(nrec)))
-        return (C.string_at(p.value, ln.value) if ln.value else b""), nrec.value
+        return _read_sorted(self._h, load().b2sh_reader_read_sorted_rows_keys, *_key_arrays(keys))
 
     def readAggregatedRowsKeys(self, keys, aggs=()):
         """readAggregatedRows grouped by a composite key (keys as in readSortedRowsKeys).
         -> (bytes, number of input records, number of groups)"""
-        kt, ko, kl, kn = _key_columns(keys)
-        aggs = list(aggs)
-        op = np.array([a[0] for a in aggs] or [0], dtype=np.uint32)
-        off = np.array([a[1] for a in aggs] or [0], dtype=np.uint32)
-        nf = np.array([a[2] for a in aggs] or [0], dtype=np.int32)
-        p, ln, nrec, ngrp = _vp(), _u64(), _u64(), _u64()
-        _check(load().b2sh_reader_read_aggregated_rows_keys(self._h, len(keys), kt.ctypes.data, ko.ctypes.data,
-                                                            kl.ctypes.data, kn.ctypes.data, len(aggs), op.ctypes.data,
-                                                            off.ctypes.data, nf.ctypes.data, C.byref(p), C.byref(ln),
-                                                            C.byref(nrec), C.byref(ngrp)))
-        return (C.string_at(p.value, ln.value) if ln.value else b""), nrec.value, ngrp.value
+        return _read_sorted(self._h, load().b2sh_reader_read_aggregated_rows_keys, *_key_arrays(keys),
+                            *_agg_arrays(aggs), groups=True)
 
     def _blocks(self, n):
         out = []

@@ -686,6 +686,56 @@ static std::deque<S3BufferedPrefetchIterator::Source> computeShuffleBlockStreams
   return out;
 }
 
+// A block as a sorted read drains it from the prefetcher: (its tag, the whole compressed block).
+using FetchedBlock = std::pair<uint64_t, std::vector<uint8_t>>;
+
+// The sources of one sorted-read call, staged in the order given: their bytes back to back in one pinned arena, each
+// source's offset and length there, and its checksum slices (source k's are [sliceBase[k], sliceBase[k + 1])).  A null
+// source, the place of a map the exchange cache serves, stages as no bytes and no slices.
+struct StagedBlocks {
+  StagedBlocks(const std::vector<ShuffleBlockInfo>& info, const std::vector<const FetchedBlock*>& sources) {
+    for (const FetchedBlock* f : sources) {
+      off.push_back(bytes);
+      len.push_back(f ? f->second.size() : 0);
+      bytes += len.back();
+      if (f) {
+        const ShuffleBlockInfo& bi = info[f->first];
+        sliceLen.insert(sliceLen.end(), bi.sliceLen.begin(), bi.sliceLen.end());
+        sliceSum.insert(sliceSum.end(), bi.sliceSum.begin(), bi.sliceSum.end());
+      }
+      sliceBase.push_back((uint32_t)sliceLen.size());
+    }
+    src.resize(bytes ? bytes : 1);
+    for (size_t k = 0; k < sources.size(); k++)
+      if (sources[k]) memcpy(src.data() + off[k], sources[k]->second.data(), (size_t)len[k]);
+  }
+  PinnedArena src;
+  uint64_t bytes = 0;
+  std::vector<uint64_t> off, len, sliceLen, sliceSum;
+  std::vector<uint32_t> sliceBase{0};
+};
+
+// A block's status from a decode call, thrown as the reference reports it.
+static void throwBlockStatus(int32_t status, const BlockId& id) {
+  if (status == B2S_E_CHECKSUM)  // storage/S3ChecksumValidationStream.scala:72-74
+    throw SparkException("Invalid checksum detected for " + id.name());
+  if (status == B2S_E_CORRUPT) throw IOException("Stream is corrupted");
+  if (status != 0) throw IOException(std::string("decompress failed: ") + b2s_strerror(status));
+}
+
+// Runs call(cap) with `out` reset to cap bytes.  A call that finds cap too small ends with the bytes it needs in
+// `total`; it then runs once more with exactly that.
+template <typename Call>
+static int callWithRetry(std::unique_ptr<uint8_t[]>& out, uint64_t cap, const uint64_t& total, Call&& call) {
+  int rc = B2S_E_DST_TOO_SMALL;
+  for (int attempt = 0; attempt < 2 && rc == B2S_E_DST_TOO_SMALL; attempt++) {
+    if (attempt) cap = total;
+    out.reset(new uint8_t[(size_t)(cap ? cap : 1)]);
+    rc = call(cap);
+  }
+  return rc;
+}
+
 class S3ShuffleReader {
  public:
   struct Block {
@@ -729,7 +779,7 @@ class S3ShuffleReader {
   void readSorted(uint32_t recordBytes, uint32_t keyOff, uint32_t keyLen) {
     std::vector<uint8_t> fetch = cacheMisses();
     start(true, &fetch);
-    std::vector<std::pair<uint64_t, std::vector<uint8_t>>> fetched;  // (tag, compressed bytes)
+    std::vector<FetchedBlock> fetched;
     drainWhole(fetched);
     const uint32_t M = (uint32_t)mapIds_.size();
     const bool verify = d_.checksumEnabled;
@@ -742,71 +792,46 @@ class S3ShuffleReader {
       for (uint32_t k = 0; k < (uint32_t)fetched.size(); k++) ofMap[info_[fetched[k].first].mapPos].push_back(k);
       std::vector<int64_t> ids;
       std::vector<uint8_t> cached;
-      std::vector<uint64_t> off, len, tags, sliceLen, sliceSum;
-      std::vector<uint32_t> sliceBase(1, 0), mapOf, from;  // from: the source's entry of `fetched`
-      uint64_t bytes = 0;
+      std::vector<uint32_t> mapOf;
+      std::vector<const FetchedBlock*> from;  // the source's entry of `fetched`, null for a cached source
+      auto add = [&](uint32_t m, const FetchedBlock* f) {
+        ids.push_back(mapIds_[m]);
+        cached.push_back(f ? 0 : 1);
+        from.push_back(f);
+        mapOf.push_back(m);
+      };
       for (uint32_t m = 0; m < M; m++) {
-        if (!fetch[m]) {
-          ids.push_back(mapIds_[m]);
-          cached.push_back(1);
-          off.push_back(bytes);
-          len.push_back(0);
-          tags.push_back(~0ull);
-          from.push_back(0);
-          mapOf.push_back(m);
-          sliceBase.push_back((uint32_t)sliceLen.size());
-          continue;
-        }
-        for (uint32_t k : ofMap[m]) {
-          const ShuffleBlockInfo& bi = info_[fetched[k].first];
-          ids.push_back(mapIds_[m]);
-          cached.push_back(0);
-          off.push_back(bytes);
-          len.push_back(fetched[k].second.size());
-          tags.push_back(fetched[k].first);
-          from.push_back(k);
-          mapOf.push_back(m);
-          bytes += len.back();
-          sliceLen.insert(sliceLen.end(), bi.sliceLen.begin(), bi.sliceLen.end());
-          sliceSum.insert(sliceSum.end(), bi.sliceSum.begin(), bi.sliceSum.end());
-          sliceBase.push_back((uint32_t)sliceLen.size());
-        }
+        if (!fetch[m]) add(m, nullptr);
+        else for (uint32_t k : ofMap[m]) add(m, &fetched[k]);
       }
       const uint32_t n = (uint32_t)ids.size();
-      PinnedArena src;
-      src.resize(bytes ? bytes : 1);
-      for (uint32_t k = 0; k < n; k++)
-        if (!cached[k]) memcpy(src.data() + off[k], fetched[from[k]].second.data(), (size_t)len[k]);
+      StagedBlocks src(info_, from);
       uint64_t cachedBytes = 0;
       if (std::find(cached.begin(), cached.end(), 1) != cached.end()) {
         std::vector<uint64_t> hitLen(n);
-        const int rc = b2s_exchange_lookup(shuffleId_, start_, end_, n, ids.data(), hitLen.data());
-        if (rc < 0) throw CodecException(std::string("b2s_exchange_lookup: ") + b2s_strerror(rc) + ": " + b2s_last_error());
+        lookup(n, ids.data(), hitLen.data());
         for (uint32_t k = 0; k < n; k++)
           if (cached[k] && hitLen[k] != UINT64_MAX) cachedBytes += hitLen[k];
       }
+      const uint32_t* sb = verify ? src.sliceBase.data() : nullptr;
+      const uint64_t* sl = verify ? src.sliceLen.data() : nullptr;
+      const uint64_t* sc = verify ? src.sliceSum.data() : nullptr;
+      std::vector<int32_t> status(n), bad(n);
+      uint64_t total = 0, records = 0;
       // Output size: codec NONE decodes to the stored bytes.  For a codec, a first guess of 4x the compressed bytes (the
       // pages of the untouched tail are never faulted in); a call it is too small for ends after verification with the
       // bytes needed in `total`, and the one retry uses exactly that.
-      uint64_t cap = (codec == B2S_CODEC_NONE ? bytes : bytes * 4) + cachedBytes;
-      std::vector<int32_t> status(n), bad(n);
-      uint64_t total = 0, records = 0;
-      int rc = B2S_E_DST_TOO_SMALL;
-      for (int attempt = 0; attempt < 2 && rc == B2S_E_DST_TOO_SMALL; attempt++) {
-        if (attempt) cap = total;
-        sorted_.reset(new uint8_t[(size_t)(cap ? cap : 1)]);
+      const uint64_t guess = (codec == B2S_CODEC_NONE ? src.bytes : src.bytes * 4) + cachedBytes;
+      const int rc = callWithRetry(sorted_, guess, total, [&](uint64_t cap) {
         if (fetch == std::vector<uint8_t>(M, 1))
-          rc = b2s_decompress_sort_packed(codec, alg, n, src.data(), off.data(), len.data(),
-                                          verify ? sliceBase.data() : nullptr, verify ? sliceLen.data() : nullptr,
-                                          verify ? sliceSum.data() : nullptr, recordBytes, keyOff, keyLen, sorted_.get(),
-                                          cap, &total, &records, status.data(), bad.data());
-        else
-          rc = b2s_exchange_read_sort_packed(shuffleId_, start_, end_, ids.data(), cached.data(), codec, alg, n,
-                                             src.data(), off.data(), len.data(), verify ? sliceBase.data() : nullptr,
-                                             verify ? sliceLen.data() : nullptr, verify ? sliceSum.data() : nullptr,
-                                             recordBytes, keyOff, keyLen, sorted_.get(), cap, &total, &records,
-                                             status.data(), bad.data());
-      }
+          return b2s_decompress_sort_packed(codec, alg, n, src.src.data(), src.off.data(), src.len.data(), sb, sl, sc,
+                                            recordBytes, keyOff, keyLen, sorted_.get(), cap, &total, &records,
+                                            status.data(), bad.data());
+        return b2s_exchange_read_sort_packed(shuffleId_, start_, end_, ids.data(), cached.data(), codec, alg, n,
+                                             src.src.data(), src.off.data(), src.len.data(), sb, sl, sc, recordBytes,
+                                             keyOff, keyLen, sorted_.get(), cap, &total, &records, status.data(),
+                                             bad.data());
+      });
       if (rc != 0)
         throw CodecException(std::string("b2s_decompress_sort_packed: ") + b2s_strerror(rc) + ": " + b2s_last_error());
       std::vector<uint8_t> late(M, 0);  // maps evicted between the lookup and the call: fetch them, then sort again
@@ -819,29 +844,16 @@ class S3ShuffleReader {
         drainWhole(fetched);
         continue;
       }
-      for (uint32_t k = 0; k < n; k++) {
-        const BlockId id = cached[k] ? cachedBlockId(ids[k]) : info_[tags[k]].id;
-        if (status[k] == B2S_E_CHECKSUM)  // storage/S3ChecksumValidationStream.scala:72-74
-          throw SparkException("Invalid checksum detected for " + id.name());
-        if (status[k] == B2S_E_CORRUPT) throw IOException("Stream is corrupted");
-        if (status[k] != 0) throw IOException(std::string("decompress failed: ") + b2s_strerror(status[k]));
-      }
+      for (uint32_t k = 0; k < n; k++)
+        throwBlockStatus(status[k], cached[k] ? cachedBlockId(ids[k]) : info_[from[k]->first].id);
       sortedLen_ = total;
       sortedRecords_ = records;
       return;
     }
   }
-  // read() for a Spark SQL exchange whose rows the reducer sorts by one typed key (INTEGRATION.md §3g): every non-empty
-  // block is fetched and staged, then ONE b2s_decompress_sort_rows_packed call verifies, decodes and sorts the task's
-  // UnsafeRowSerializer records ([int32 big-endian size][row]) by the key keyType at row offset keyOff, nulls first
-  // (nullField: the key's null bit, -1 = none).  Blocks go in computeShuffleBlocks order, so equal keys come out in map,
-  // then reduce-id order.  Codec NONE is verified and sorted only.  It reads fetched blocks only: the exchange cache is
-  // not consulted.
-  void readSortedRows(uint32_t keyType, uint32_t keyOff, uint32_t keyLen, int32_t nullField) {
-    readRows(RowKeys{1, &keyType, &keyOff, &keyLen, &nullField, false}, nullptr);
-  }
-  // The key columns of readSortedRowsKeys / readAggregatedRowsKeys: column c is type[c] (B2S_KEY_* or B2S_STRING_KEY)
-  // at row offset off[c], len[c] bytes, null bit nullField[c].  composite: the *_rows_keys_* calls, else the one-key ones.
+  // The key columns of readRows: column c is type[c] (B2S_KEY_* or B2S_STRING_KEY) at row offset off[c], len[c] bytes,
+  // null bit nullField[c].  composite: the *_rows_keys_* calls (up to 16 columns, strings included), else the one-key
+  // ones.
   struct RowKeys {
     uint32_t n;
     const uint32_t* type;
@@ -850,38 +862,24 @@ class S3ShuffleReader {
     const int32_t* nullField;
     bool composite;
   };
-  // readSortedRows by a composite key of up to 16 columns, strings included: ONE b2s_decompress_sort_rows_keys_packed
-  // call.  The exchange cache is not consulted.
-  void readSortedRowsKeys(const RowKeys& keys) { readRows(keys, nullptr); }
-  // The aggregates of readAggregatedRows: aggregate k is op[k] (B2S_AGG_*) over the 8-byte slot at row offset off[k],
-  // null bit nullField[k] (-1 = never null).
+  // The aggregates of readRows: aggregate k is op[k] (B2S_AGG_*) over the 8-byte slot at row offset off[k], null bit
+  // nullField[k] (-1 = never null).
   struct RowAggregates {
     uint32_t n;
     const uint32_t* op;
     const uint32_t* off;
     const int32_t* nullField;
   };
-  // read() for a Spark SQL exchange whose reducer merges partial aggregates by one typed key (INTEGRATION.md §3h): the
-  // blocks are fetched and staged as readSortedRows does, then ONE b2s_decompress_aggregate_rows_packed call verifies,
-  // decodes, groups and merges them into one row per key, in the row sort's order.  The exchange cache is not
-  // consulted.
-  void readAggregatedRows(uint32_t keyType, uint32_t keyOff, uint32_t keyLen, int32_t nullField,
-                          const RowAggregates& aggs) {
-    readRows(RowKeys{1, &keyType, &keyOff, &keyLen, &nullField, false}, &aggs);
-  }
-  // readAggregatedRows grouped by a composite key (readSortedRowsKeys): ONE b2s_decompress_aggregate_rows_keys_packed
-  // call.  The exchange cache is not consulted.
-  void readAggregatedRowsKeys(const RowKeys& keys, const RowAggregates& aggs) { readRows(keys, &aggs); }
-  const uint8_t* sortedData() const { return sorted_.get(); }
-  uint64_t sortedLen() const { return sortedLen_; }
-  uint64_t sortedRecords() const { return sortedRecords_; }
-  uint64_t sortedGroups() const { return sortedGroups_; }
-
- private:
-  // the body of the row reads: sorted (aggs == nullptr) or aggregated, by one key or a composite one
+  // read() for a Spark SQL exchange whose rows the reducer sorts (aggs == nullptr, INTEGRATION.md §3g) or whose partial
+  // aggregates it merges (INTEGRATION.md §3h) by one typed key or a composite one: every non-empty block is fetched and
+  // staged, then ONE b2s_decompress_{sort,aggregate}_rows[_keys]_packed call verifies, decodes and sorts the task's
+  // UnsafeRowSerializer records ([int32 big-endian size][row]) by the key, nulls first, or groups them and merges each
+  // group into one row per key in that order.  Blocks go in computeShuffleBlocks order, so equal keys come out in map,
+  // then reduce-id order.  Codec NONE is verified and sorted only.  It reads fetched blocks only: the exchange cache is
+  // not consulted.
   void readRows(const RowKeys& keys, const RowAggregates* aggs) {
     start(true);
-    std::vector<std::pair<uint64_t, std::vector<uint8_t>>> fetched;  // (tag, compressed bytes)
+    std::vector<FetchedBlock> fetched;
     drainWhole(fetched);
     std::sort(fetched.begin(), fetched.end(), [](const auto& a, const auto& b) { return a.first < b.first; });
     const bool verify = d_.checksumEnabled;
@@ -889,69 +887,52 @@ class S3ShuffleReader {
     ensure_codec_runtime();
     const uint32_t codec = (uint32_t)d_.codecId();
     const uint32_t n = (uint32_t)fetched.size();
-    std::vector<uint64_t> off, len, sliceLen, sliceSum;
-    std::vector<uint32_t> sliceBase(1, 0);
-    uint64_t bytes = 0;
-    for (const auto& f : fetched) {
-      const ShuffleBlockInfo& bi = info_[f.first];
-      off.push_back(bytes);
-      len.push_back(f.second.size());
-      bytes += f.second.size();
-      sliceLen.insert(sliceLen.end(), bi.sliceLen.begin(), bi.sliceLen.end());
-      sliceSum.insert(sliceSum.end(), bi.sliceSum.begin(), bi.sliceSum.end());
-      sliceBase.push_back((uint32_t)sliceLen.size());
-    }
-    PinnedArena src;
-    src.resize(bytes ? bytes : 1);
-    for (uint32_t k = 0; k < n; k++) memcpy(src.data() + off[k], fetched[k].second.data(), (size_t)len[k]);
-    // output size as in readSorted: a first guess, then one retry with the bytes needed
-    uint64_t cap = codec == B2S_CODEC_NONE ? bytes : bytes * 4;
+    std::vector<const FetchedBlock*> blocks;
+    for (const auto& f : fetched) blocks.push_back(&f);
+    StagedBlocks src(info_, blocks);
+    const uint32_t* sb = verify ? src.sliceBase.data() : nullptr;
+    const uint64_t* sl = verify ? src.sliceLen.data() : nullptr;
+    const uint64_t* sc = verify ? src.sliceSum.data() : nullptr;
     std::vector<int32_t> status(n), bad(n);
     uint64_t total = 0, records = 0, groups = 0;
-    int rc = B2S_E_DST_TOO_SMALL;
-    for (int attempt = 0; attempt < 2 && rc == B2S_E_DST_TOO_SMALL; attempt++) {
-      if (attempt) cap = total;
-      sorted_.reset(new uint8_t[(size_t)(cap ? cap : 1)]);
-      const uint32_t* sb = verify ? sliceBase.data() : nullptr;
-      const uint64_t* sl = verify ? sliceLen.data() : nullptr;
-      const uint64_t* sc = verify ? sliceSum.data() : nullptr;
+    // output size as in readSorted: a first guess, then one retry with the bytes needed
+    const uint64_t guess = codec == B2S_CODEC_NONE ? src.bytes : src.bytes * 4;
+    const int rc = callWithRetry(sorted_, guess, total, [&](uint64_t cap) {
       if (aggs && keys.composite)
-        rc = b2s_decompress_aggregate_rows_keys_packed(codec, alg, n, src.data(), off.data(), len.data(), sb, sl, sc,
-                                                       keys.n, keys.type, keys.off, keys.len, keys.nullField, aggs->n,
-                                                       aggs->op, aggs->off, aggs->nullField, sorted_.get(), cap,
-                                                       &total, &records, &groups, status.data(), bad.data());
-      else if (aggs)
-        rc = b2s_decompress_aggregate_rows_packed(codec, alg, n, src.data(), off.data(), len.data(), sb, sl, sc,
-                                                  keys.type[0], keys.off[0], keys.len[0], keys.nullField[0], aggs->n,
-                                                  aggs->op, aggs->off, aggs->nullField, sorted_.get(), cap, &total,
-                                                  &records, &groups, status.data(), bad.data());
-      else if (keys.composite)
-        rc = b2s_decompress_sort_rows_keys_packed(codec, alg, n, src.data(), off.data(), len.data(), sb, sl, sc, keys.n,
-                                                  keys.type, keys.off, keys.len, keys.nullField, sorted_.get(), cap,
-                                                  &total, &records, status.data(), bad.data());
-      else
-        rc = b2s_decompress_sort_rows_packed(codec, alg, n, src.data(), off.data(), len.data(), sb, sl, sc,
+        return b2s_decompress_aggregate_rows_keys_packed(codec, alg, n, src.src.data(), src.off.data(), src.len.data(),
+                                                         sb, sl, sc, keys.n, keys.type, keys.off, keys.len,
+                                                         keys.nullField, aggs->n, aggs->op, aggs->off, aggs->nullField,
+                                                         sorted_.get(), cap, &total, &records, &groups, status.data(),
+                                                         bad.data());
+      if (aggs)
+        return b2s_decompress_aggregate_rows_packed(codec, alg, n, src.src.data(), src.off.data(), src.len.data(), sb,
+                                                    sl, sc, keys.type[0], keys.off[0], keys.len[0], keys.nullField[0],
+                                                    aggs->n, aggs->op, aggs->off, aggs->nullField, sorted_.get(), cap,
+                                                    &total, &records, &groups, status.data(), bad.data());
+      if (keys.composite)
+        return b2s_decompress_sort_rows_keys_packed(codec, alg, n, src.src.data(), src.off.data(), src.len.data(), sb,
+                                                    sl, sc, keys.n, keys.type, keys.off, keys.len, keys.nullField,
+                                                    sorted_.get(), cap, &total, &records, status.data(), bad.data());
+      return b2s_decompress_sort_rows_packed(codec, alg, n, src.src.data(), src.off.data(), src.len.data(), sb, sl, sc,
                                              keys.type[0], keys.off[0], keys.len[0], keys.nullField[0], sorted_.get(),
                                              cap, &total, &records, status.data(), bad.data());
-    }
+    });
     if (rc != 0)
       throw CodecException(std::string(aggs ? (keys.composite ? "b2s_decompress_aggregate_rows_keys_packed: "
                                                               : "b2s_decompress_aggregate_rows_packed: ")
                                             : (keys.composite ? "b2s_decompress_sort_rows_keys_packed: "
                                                               : "b2s_decompress_sort_rows_packed: ")) +
                            b2s_strerror(rc) + ": " + b2s_last_error());
-    for (uint32_t k = 0; k < n; k++) {
-      if (status[k] == B2S_E_CHECKSUM)  // storage/S3ChecksumValidationStream.scala:72-74
-        throw SparkException("Invalid checksum detected for " + info_[fetched[k].first].id.name());
-      if (status[k] == B2S_E_CORRUPT) throw IOException("Stream is corrupted");
-      if (status[k] != 0) throw IOException(std::string("decompress failed: ") + b2s_strerror(status[k]));
-    }
+    for (uint32_t k = 0; k < n; k++) throwBlockStatus(status[k], info_[fetched[k].first].id);
     sortedLen_ = total;
     sortedRecords_ = records;
     sortedGroups_ = groups;
   }
+  const uint8_t* sortedData() const { return sorted_.get(); }
+  uint64_t sortedLen() const { return sortedLen_; }
+  uint64_t sortedRecords() const { return sortedRecords_; }
+  uint64_t sortedGroups() const { return sortedGroups_; }
 
- public:
   // want (nullptr = every map): the maps whose blocks are fetched
   void start(bool allowNone, const std::vector<uint8_t>* want = nullptr) {
     iter_.reset();
@@ -970,7 +951,7 @@ class S3ShuffleReader {
   }
 
   // every block the prefetcher delivers, whole, appended to `fetched` as (tag, bytes)
-  void drainWhole(std::vector<std::pair<uint64_t, std::vector<uint8_t>>>& fetched) {
+  void drainWhole(std::vector<FetchedBlock>& fetched) {
     while (iter_->hasNext()) {
       for (auto& f : iter_->nextBatch(0)) {
         auto& st = *f.stream;
@@ -994,10 +975,14 @@ class S3ShuffleReader {
     if (!d_.gpuExchangeCacheBytes || mapIds_.empty()) return fetch;
     ensure_codec_runtime();
     std::vector<uint64_t> len(mapIds_.size());
-    const int rc = b2s_exchange_lookup(shuffleId_, start_, end_, (uint32_t)mapIds_.size(), mapIds_.data(), len.data());
-    if (rc < 0) throw CodecException(std::string("b2s_exchange_lookup: ") + b2s_strerror(rc) + ": " + b2s_last_error());
+    lookup((uint32_t)mapIds_.size(), mapIds_.data(), len.data());
     for (size_t m = 0; m < len.size(); m++) fetch[m] = len[m] == UINT64_MAX;
     return fetch;
+  }
+  // b2s_exchange_lookup of the reader's range for n maps: len[k] is UINT64_MAX when ids[k] is not resident
+  void lookup(uint32_t n, const int64_t* ids, uint64_t* len) {
+    const int rc = b2s_exchange_lookup(shuffleId_, start_, end_, n, ids, len);
+    if (rc < 0) throw CodecException(std::string("b2s_exchange_lookup: ") + b2s_strerror(rc) + ": " + b2s_last_error());
   }
   BlockId cachedBlockId(int64_t mapId) const {
     return end_ - start_ > 1 ? BlockId{BlockId::ShuffleBatch, shuffleId_, mapId, start_, end_}
@@ -1018,18 +1003,14 @@ class S3ShuffleReader {
     const uint32_t n = (uint32_t)ids.size();
     std::vector<uint64_t> off(n), len(n);
     std::vector<int32_t> status(n);
-    int rc = b2s_exchange_lookup(shuffleId_, start_, end_, n, ids.data(), len.data());
-    if (rc < 0) throw CodecException(std::string("b2s_exchange_lookup: ") + b2s_strerror(rc) + ": " + b2s_last_error());
-    uint64_t cap = 0, total = 0;
-    for (uint64_t l : len) cap += l == UINT64_MAX ? 0 : l;
+    lookup(n, ids.data(), len.data());
+    uint64_t guess = 0, total = 0;
+    for (uint64_t l : len) guess += l == UINT64_MAX ? 0 : l;
     std::unique_ptr<uint8_t[]> buf;
-    rc = B2S_E_DST_TOO_SMALL;
-    for (int attempt = 0; attempt < 2 && rc == B2S_E_DST_TOO_SMALL; attempt++) {  // an entry stored again may have grown
-      if (attempt) cap = total;
-      buf.reset(new uint8_t[(size_t)(cap ? cap : 1)]);
-      rc = b2s_exchange_read_packed(shuffleId_, start_, end_, n, ids.data(), buf.get(), cap, off.data(), len.data(),
-                                    &total, status.data());
-    }
+    const int rc = callWithRetry(buf, guess, total, [&](uint64_t cap) {  // an entry stored again may have grown
+      return b2s_exchange_read_packed(shuffleId_, start_, end_, n, ids.data(), buf.get(), cap, off.data(), len.data(),
+                                      &total, status.data());
+    });
     if (rc != 0)
       throw CodecException(std::string("b2s_exchange_read_packed: ") + b2s_strerror(rc) + ": " + b2s_last_error());
     for (uint32_t k = 0; k < n; k++) {
@@ -1127,10 +1108,7 @@ class S3ShuffleReader {
     if (rc != 0) throw CodecException(std::string("b2s_decompress_batch: ") + b2s_strerror(rc) + ": " + rcText);
     for (uint32_t k = 0; k < n; k++) {
       const BlockId& id = info_[got[k].tag].id;
-      if (status[k] == B2S_E_CHECKSUM)  // storage/S3ChecksumValidationStream.scala:72-74
-        throw SparkException("Invalid checksum detected for " + id.name());
-      if (status[k] == B2S_E_CORRUPT) throw IOException("Stream is corrupted");
-      if (status[k] != 0) throw IOException(std::string("decompress failed: ") + b2s_strerror(status[k]));
+      throwBlockStatus(status[k], id);
       Block blk;
       blk.id = id;
       blk.data = dst[k];
@@ -1316,22 +1294,26 @@ int b2sh_reader_read(b2sh_reader* r, uint32_t* n_blocks) {
     *n_blocks = (uint32_t)r->r->blocks().size();
   });
 }
+// a sorted read's result: its bytes, their length, the records read and (the aggregated reads) the groups
+static void sorted_result(const S3ShuffleReader& r, const uint8_t** data, uint64_t* len, uint64_t* n_records,
+                          uint64_t* n_groups = nullptr) {
+  *data = r.sortedData();
+  *len = r.sortedLen();
+  *n_records = r.sortedRecords();
+  if (n_groups) *n_groups = r.sortedGroups();
+}
 int b2sh_reader_read_sorted(b2sh_reader* r, uint32_t record_bytes, uint32_t key_off, uint32_t key_len,
                             const uint8_t** data, uint64_t* len, uint64_t* n_records) {
   return guarded([&] {
     r->r->readSorted(record_bytes, key_off, key_len);
-    *data = r->r->sortedData();
-    *len = r->r->sortedLen();
-    *n_records = r->r->sortedRecords();
+    sorted_result(*r->r, data, len, n_records);
   });
 }
 int b2sh_reader_read_sorted_rows(b2sh_reader* r, uint32_t key_type, uint32_t key_off, uint32_t key_len,
                                  int32_t null_field, const uint8_t** data, uint64_t* len, uint64_t* n_records) {
   return guarded([&] {
-    r->r->readSortedRows(key_type, key_off, key_len, null_field);
-    *data = r->r->sortedData();
-    *len = r->r->sortedLen();
-    *n_records = r->r->sortedRecords();
+    r->r->readRows(S3ShuffleReader::RowKeys{1, &key_type, &key_off, &key_len, &null_field, false}, nullptr);
+    sorted_result(*r->r, data, len, n_records);
   });
 }
 int b2sh_reader_read_aggregated_rows(b2sh_reader* r, uint32_t key_type, uint32_t key_off, uint32_t key_len,
@@ -1339,22 +1321,17 @@ int b2sh_reader_read_aggregated_rows(b2sh_reader* r, uint32_t key_type, uint32_t
                                      const uint32_t* agg_off, const int32_t* agg_null_field, const uint8_t** data,
                                      uint64_t* len, uint64_t* n_records, uint64_t* n_groups) {
   return guarded([&] {
-    r->r->readAggregatedRows(key_type, key_off, key_len, null_field,
-                             S3ShuffleReader::RowAggregates{n_aggs, agg_op, agg_off, agg_null_field});
-    *data = r->r->sortedData();
-    *len = r->r->sortedLen();
-    *n_records = r->r->sortedRecords();
-    *n_groups = r->r->sortedGroups();
+    const S3ShuffleReader::RowAggregates aggs{n_aggs, agg_op, agg_off, agg_null_field};
+    r->r->readRows(S3ShuffleReader::RowKeys{1, &key_type, &key_off, &key_len, &null_field, false}, &aggs);
+    sorted_result(*r->r, data, len, n_records, n_groups);
   });
 }
 int b2sh_reader_read_sorted_rows_keys(b2sh_reader* r, uint32_t n_keys, const uint32_t* key_type,
                                       const uint32_t* key_off, const uint32_t* key_len, const int32_t* key_null_field,
                                       const uint8_t** data, uint64_t* len, uint64_t* n_records) {
   return guarded([&] {
-    r->r->readSortedRowsKeys(S3ShuffleReader::RowKeys{n_keys, key_type, key_off, key_len, key_null_field, true});
-    *data = r->r->sortedData();
-    *len = r->r->sortedLen();
-    *n_records = r->r->sortedRecords();
+    r->r->readRows(S3ShuffleReader::RowKeys{n_keys, key_type, key_off, key_len, key_null_field, true}, nullptr);
+    sorted_result(*r->r, data, len, n_records);
   });
 }
 int b2sh_reader_read_aggregated_rows_keys(b2sh_reader* r, uint32_t n_keys, const uint32_t* key_type,
@@ -1364,12 +1341,9 @@ int b2sh_reader_read_aggregated_rows_keys(b2sh_reader* r, uint32_t n_keys, const
                                           const uint8_t** data, uint64_t* len, uint64_t* n_records,
                                           uint64_t* n_groups) {
   return guarded([&] {
-    r->r->readAggregatedRowsKeys(S3ShuffleReader::RowKeys{n_keys, key_type, key_off, key_len, key_null_field, true},
-                                 S3ShuffleReader::RowAggregates{n_aggs, agg_op, agg_off, agg_null_field});
-    *data = r->r->sortedData();
-    *len = r->r->sortedLen();
-    *n_records = r->r->sortedRecords();
-    *n_groups = r->r->sortedGroups();
+    const S3ShuffleReader::RowAggregates aggs{n_aggs, agg_op, agg_off, agg_null_field};
+    r->r->readRows(S3ShuffleReader::RowKeys{n_keys, key_type, key_off, key_len, key_null_field, true}, &aggs);
+    sorted_result(*r->r, data, len, n_records, n_groups);
   });
 }
 int b2sh_reader_block(b2sh_reader* r, uint32_t k, int64_t* map_id, int32_t* start_reduce, int32_t* end_reduce,

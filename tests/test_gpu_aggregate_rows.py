@@ -3,97 +3,19 @@ aggregate rows in, one row per key out.  The model parses the decoded streams in
 sorted order (the row sort's order), and merges every aggregate over each group in that order — the double sum
 sequentially — into a copy of the group's first record.  The call must be byte for byte that model."""
 import ctypes as C
-import math
 import struct
-import uuid
 
 import numpy as np
 import pytest
 
 import spark_s3_shuffle_b200 as pkg
-from test_gpu_sort_rows import CHECKSUMS, CODECS, KEY_BYTES, KEY_INT32, KEY_INT64, blocks_of, build_blocks, parse, \
-    sort_key, stream
+from rows_model import CHECKSUMS, CODECS, KEY_BYTES, KEY_INT32, KEY_INT64, MAX_F64, MAX_I32, MAX_I64, MIN_F64, \
+    MIN_I32, MIN_I64, SUM_F64, SUM_I64, blocks_of, build_blocks, mirror, model_aggregate, parse, run, stream, write_maps
 
 pytestmark = pytest.mark.gpu
 
-SUM_I64, SUM_F64, MIN_I32, MAX_I32, MIN_I64, MAX_I64, MIN_F64, MAX_F64 = range(8)
 ALL_OPS = list(range(8))
 KEY_LEN = {KEY_INT32: 4, KEY_INT64: 8, KEY_BYTES: 6}
-
-
-# ---------------------------------------------------------------------------------------------------------------
-# model
-# ---------------------------------------------------------------------------------------------------------------
-def is_null(row, f):
-    return f >= 0 and (int.from_bytes(row[8 * (f >> 6):8 * (f >> 6) + 8], "little") >> (f & 63)) & 1
-
-
-def f64(b):
-    return struct.unpack("<d", b)[0]
-
-
-def dkey(b):
-    """Spark SQL's double order: -0.0 == 0.0, NaN == NaN above everything"""
-    x = f64(b)
-    if math.isnan(x):
-        return (1, 0.0)
-    return (0, x + 0.0)
-
-
-def merge(op, vals):
-    """vals: the non-null 8-byte slots of a group in stable order -> the result slot"""
-    if op == SUM_I64:
-        return (sum(int.from_bytes(v, "little") for v in vals) % 2**64).to_bytes(8, "little")
-    if op == SUM_F64:
-        s = 0.0
-        for v in vals:
-            s = s + f64(v)
-        return struct.pack("<d", s)
-    if op in (MIN_I32, MAX_I32):
-        key = [int.from_bytes(v[:4], "little", signed=True) for v in vals]
-    elif op in (MIN_I64, MAX_I64):
-        key = [int.from_bytes(v, "little", signed=True) for v in vals]
-    else:
-        key = [dkey(v) for v in vals]
-    best = 0
-    for k in range(1, len(vals)):
-        if (key[k] > key[best]) if op in (MAX_I32, MAX_I64, MAX_F64) else (key[k] < key[best]):
-            best = k
-    return vals[best][:4] + bytes(4) if op in (MIN_I32, MAX_I32) else vals[best]
-
-
-def model_aggregate(plain, kt, ko, kl, nf, aggs):
-    buf = b"".join(plain)
-    recs = parse(buf)
-    keys = [sort_key(buf, o, kt, ko, kl, nf) for o, _ in recs]
-    order = sorted(range(len(recs)), key=lambda i: keys[i])
-    out, groups, j = [], 0, 0
-    while j < len(order):
-        e = j
-        while e < len(order) and keys[order[e]] == keys[order[j]]:
-            e += 1
-        o, ln = recs[order[j]]
-        rec = bytearray(buf[o:o + ln])
-        row = memoryview(rec)[4:]
-        nulls = []
-        for op, off, anf in aggs:
-            vals = []
-            for i in order[j:e]:
-                r = buf[recs[i][0] + 4:recs[i][0] + recs[i][1]]
-                if not is_null(r, anf):
-                    vals.append(bytes(r[off:off + 8]))
-            row[off:off + 8] = merge(op, vals) if vals else bytes(8)
-            nulls.append((anf, not vals))
-        for anf, null in nulls:
-            if anf >= 0:
-                w = 8 * (anf >> 6)
-                v = int.from_bytes(row[w:w + 8], "little")
-                v = v | (1 << (anf & 63)) if null else v & ~(1 << (anf & 63))
-                row[w:w + 8] = v.to_bytes(8, "little")
-        out.append(bytes(rec))
-        groups += 1
-        j = e
-    return b"".join(out), len(recs), groups
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -169,36 +91,12 @@ def make_rows(rng, n, kt, keys, ops, nw=1, key_null=-1, key_null_frac=0.0, agg_n
     return rows, aggs
 
 
-def agg_packed(capi, codec, alg, blocks, kt, ko, kl, nf, aggs, cap):
-    arena, off, ln, sb, sl, sc = blocks
-    dst = np.zeros(max(cap, 1), np.uint8)
-    r = capi.decompress_aggregate_rows_packed(codec, arena, off, ln, dst[:cap], kt, ko, kl, nf, aggs, alg, sb, sl, sc)
-    return dst[: r["total"]].tobytes(), r
-
-
-def agg_dev(capi, codec, alg, blocks, kt, ko, kl, nf, aggs, cap):
-    arena, off, ln, sb, sl, sc = blocks
-    d_src = capi.dev_alloc(max(arena.size, 1))
-    d_dst = capi.dev_alloc(max(cap, 1))
-    try:
-        capi.dev_memcpy(d_src, arena.ctypes.data, arena.size, 1)
-        r = capi.decompress_aggregate_rows_dev(codec, d_src, off, ln, d_dst, cap, kt, ko, kl, nf, aggs, alg, sb, sl,
-                                               sc)
-        out = np.zeros(max(r["total"], 1), np.uint8)
-        if r["total"]:
-            capi.dev_memcpy(out.ctypes.data, d_dst, r["total"], 2)
-        return out[: r["total"]].tobytes(), r
-    finally:
-        capi.dev_free(d_src)
-        capi.dev_free(d_dst)
-
-
 def check(capi, codec, level, alg, plain, kt, ko, kl, nf, aggs, dev=False, blocks=None):
     blocks = blocks or build_blocks(capi, codec, level, alg, plain)
     total = sum(len(b) for b in plain)
-    got, r = (agg_dev if dev else agg_packed)(capi, codec, alg, blocks, kt, ko, kl, nf, aggs, total)
+    got, r = run(capi, "decompress_aggregate_rows", codec, alg, blocks, (kt, ko, kl, nf, aggs), total, dev)
     assert (r["status"] == 0).all(), r["status"]
-    want, n, g = model_aggregate(plain, kt, ko, kl, nf, aggs)
+    want, n, g = model_aggregate(plain, [(kt, ko, kl, nf)], aggs)
     assert (r["n_records"], r["n_groups"], r["total"]) == (n, g, len(want))
     assert got == want
     return got, r
@@ -351,7 +249,7 @@ def test_one_group_of_more_than_a_million_records(capi):
     rec[:, 44:52] = iv.view(np.uint8).reshape(n, 8)
     aggs = [(SUM_F64, 16, 1), (SUM_I64, 24, -1), (MAX_F64, 32, -1), (MIN_I64, 40, -1)]
     blocks = build_blocks(capi, 1, 0, 3, [rec.tobytes()])
-    got, r = agg_packed(capi, 1, 3, blocks, KEY_INT64, 8, 8, -1, aggs, rec.size)
+    got, r = run(capi, "decompress_aggregate_rows", 1, 3, blocks, (KEY_INT64, 8, 8, -1, aggs), rec.size)
     assert (r["status"] == 0).all() and r["n_records"] == n and r["n_groups"] == 1
     want = bytearray(rec[0].tobytes())
     want[4:12] = bytes(8)
@@ -395,8 +293,8 @@ def test_each_framing_rule_fails_its_block(capi, rule):
     for codec in (0, 1):
         blocks = build_blocks(capi, codec, 1, 3, plain)
         for dev in (False, True):
-            got, r = (agg_dev if dev else agg_packed)(capi, codec, 3, blocks, KEY_INT64, 8, 8, nf, aggs,
-                                                      sum(map(len, plain)))
+            got, r = run(capi, "decompress_aggregate_rows", codec, 3, blocks, (KEY_INT64, 8, 8, nf, aggs),
+                         sum(map(len, plain)), dev)
             assert list(r["status"]) == [0, capi.E_CORRUPT, 0, 0]
             assert r["n_records"] == 0 and r["n_groups"] == 0 and r["total"] == 0 and got == b""
             err = capi.load().b2s_last_error()
@@ -412,8 +310,8 @@ def test_bad_checksum_in_one_block(capi):
         blocks[5] = blocks[5].copy()
         blocks[5][1] ^= 0x10
         for dev in (False, True):
-            got, r = (agg_dev if dev else agg_packed)(capi, codec, 2, tuple(blocks), KEY_INT64, 8, 8, -1, AGG1,
-                                                      sum(map(len, plain)))
+            got, r = run(capi, "decompress_aggregate_rows", codec, 2, tuple(blocks), (KEY_INT64, 8, 8, -1, AGG1),
+                         sum(map(len, plain)), dev)
             assert list(r["status"]) == [0, capi.E_CHECKSUM, 0] and r["bad_slice"][1] == 0
             assert r["n_groups"] == 0 and got == b""
 
@@ -421,11 +319,11 @@ def test_bad_checksum_in_one_block(capi):
 def test_short_destination_reports_the_output_bytes(capi):
     rng = np.random.default_rng(62)
     plain = [stream(good_rows(rng)) for _ in range(2)]
-    want, _, _ = model_aggregate(plain, KEY_INT64, 8, 8, -1, AGG1)
+    want, _, _ = model_aggregate(plain, [(KEY_INT64, 8, 8, -1)], AGG1)
     blocks = build_blocks(capi, 1, 0, 0, plain)
-    for fn in (agg_packed, agg_dev):
+    for dev in (False, True):
         with pytest.raises(capi.B2SError) as e:
-            fn(capi, 1, 0, blocks, KEY_INT64, 8, 8, -1, AGG1, len(want) - 1)
+            run(capi, "decompress_aggregate_rows", 1, 0, blocks, (KEY_INT64, 8, 8, -1, AGG1), len(want) - 1, dev)
         assert e.value.code == capi.E_DST_TOO_SMALL
     arena, off, ln, _, _, _ = blocks
     dst = np.zeros(len(want), np.uint8)
@@ -437,7 +335,7 @@ def test_short_destination_reports_the_output_bytes(capi):
         op.ctypes.data, ao.ctypes.data, an.ctypes.data, dst.ctypes.data, len(want) - 1, C.byref(total), C.byref(nrec),
         C.byref(ngrp), st.ctypes.data, bad.ctypes.data)
     assert rc == capi.E_DST_TOO_SMALL and total.value == len(want) and ngrp.value == 0
-    got, r = agg_packed(capi, 1, 0, blocks, KEY_INT64, 8, 8, -1, AGG1, len(want))
+    got, r = run(capi, "decompress_aggregate_rows", 1, 0, blocks, (KEY_INT64, 8, 8, -1, AGG1), len(want))
     assert got == want
 
 
@@ -454,7 +352,7 @@ def test_bad_aggregate_arguments(capi, aggs, nf):
     rng = np.random.default_rng(63)
     blocks = build_blocks(capi, 1, 0, 0, [stream(good_rows(rng))])
     with pytest.raises(capi.B2SError) as e:
-        agg_packed(capi, 1, 0, blocks, KEY_INT64, 8, 8, nf, aggs, 1 << 16)
+        run(capi, "decompress_aggregate_rows", 1, 0, blocks, (KEY_INT64, 8, 8, nf, aggs), 1 << 16)
     assert e.value.code == capi.E_ARG
 
 
@@ -471,7 +369,8 @@ def test_null_aggregate_arrays_and_row_sort_argument_errors(capi):
     assert rc == capi.E_ARG
     for kt, kl in ((3, 8), (KEY_INT64, 4)):
         with pytest.raises(capi.B2SError) as e:
-            agg_packed(capi, 1, 0, (arena, off, ln, None, None, None), kt, 8, kl, -1, AGG1, 1 << 16)
+            run(capi, "decompress_aggregate_rows", 1, 0, (arena, off, ln, None, None, None), (kt, 8, kl, -1, AGG1),
+                1 << 16)
         assert e.value.code == capi.E_ARG
 
 
@@ -510,26 +409,6 @@ def test_partition_then_aggregate_end_to_end(capi, name, codec, level):
 # ---------------------------------------------------------------------------------------------------------------
 # 5. the host mirror: b2sh_reader_read_aggregated_rows over the serialized writer's files
 # ---------------------------------------------------------------------------------------------------------------
-def mirror(tmp_path, codec):
-    return pkg.host.S3ShuffleDispatcher({
-        "spark.app.id": "app-" + uuid.uuid4().hex[:12],
-        "spark.shuffle.s3.rootDir": "file://" + str(tmp_path) + "/spark-s3-shuffle",
-        "spark.shuffle.checksum.enabled": True,
-        "spark.shuffle.checksum.algorithm": "CRC32C",
-        "spark.io.compression.codec": "lz4",
-        "spark.shuffle.compress": codec != "none",
-    })
-
-
-def write_maps(host, d, maps, R):
-    for m, (rows, ids) in enumerate(maps):
-        w = host.S3SerializedShuffleWriter(d, 0, m, R)
-        for row, p in zip(rows, ids):
-            w.insertRecord(int(p), len(row).to_bytes(4, "big") + row)
-        w.commit()
-        w.close()
-
-
 @pytest.mark.parametrize("codec", ["lz4", "none"])
 def test_host_mirror_reads_rows_aggregated(tmp_path, codec):
     host = pkg.host
@@ -547,7 +426,7 @@ def test_host_mirror_reads_rows_aggregated(tmp_path, codec):
         data, n, g = rd.readAggregatedRows(KEY_INT32, 8, 4, 0, aggs)
         rd.close()
         want, wn, wg = model_aggregate([stream([r for r, p in zip(rows, ids) if p == red]) for rows, ids in maps],
-                                       KEY_INT32, 8, 4, 0, aggs)
+                                       [(KEY_INT32, 8, 4, 0)], aggs)
         assert (n, g) == (wn, wg) and data == want
     d.close()
 

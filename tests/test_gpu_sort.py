@@ -8,12 +8,11 @@ import numpy as np
 import pytest
 
 import spark_s3_shuffle_b200 as pkg
+from rows_model import CHECKSUMS, CODECS, build_blocks, mirror, run
 
 pytestmark = pytest.mark.gpu
 
 REC, KEY_OFF, KEY_LEN = 104, 2, 10  # a Kryo-serialized TeraSort record: 0x01 0x0B, 10-byte key, 0x01 0x5B, 90 bytes
-CODECS = [("none", 0, 0), ("lz4", 1, 0), ("snappy", 2, 0), ("zstd1", 3, 1), ("zstd3", 3, 3)]
-CHECKSUMS = [0, 1, 2, 3]  # none, ADLER32, CRC32, CRC32C
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -47,51 +46,10 @@ def split_blocks(recs, sizes):
     return out
 
 
-def build_blocks(capi, codec, level, alg, plain):
-    """one compressed stream per block, one slice per block -> (arena, off, len, slice_base, slice_len, slice_ck)"""
-    n = len(plain)
-    lens = np.array([len(b) for b in plain], dtype=np.uint64)
-    offs = np.concatenate([[0], np.cumsum(lens)[:-1]]).astype(np.uint64) if n else np.zeros(0, np.uint64)
-    src = np.frombuffer(b"".join(plain), np.uint8) if lens.sum() else np.zeros(1, np.uint8)
-    if codec == 0:
-        arena, off, ln = src, offs, lens
-    else:
-        bound = sum(capi.compress_bound(codec, 0, int(l)) for l in lens) + 64
-        dst = np.zeros(bound, np.uint8)
-        r = capi.compress_packed(codec, src, offs, lens, dst, 0, 0, level)
-        assert (r["status"] == 0).all()
-        arena, off, ln = dst[: max(r["total"], 1)], r["dst_off"], r["dst_len"]
-    ck = capi.checksum_packed(alg, arena, off, ln) if alg and n else np.zeros(n, np.uint64)
-    return arena, off, ln, np.arange(n + 1, dtype=np.uint32), np.array(ln, dtype=np.uint64), ck
-
-
-def sort_packed(capi, codec, alg, blocks, rb, ko, kl, cap):
-    arena, off, ln, sb, sl, sc = blocks
-    dst = np.zeros(max(cap, 1), np.uint8)
-    r = capi.decompress_sort_packed(codec, arena, off, ln, dst[:cap], rb, ko, kl, alg, sb, sl, sc)
-    return dst[: r["total"]].tobytes() if r["n_records"] else b"", r
-
-
-def sort_dev(capi, codec, alg, blocks, rb, ko, kl, cap):
-    arena, off, ln, sb, sl, sc = blocks
-    d_src = capi.dev_alloc(max(arena.size, 1))
-    d_dst = capi.dev_alloc(max(cap, 1))
-    try:
-        capi.dev_memcpy(d_src, arena.ctypes.data, arena.size, 1)
-        r = capi.decompress_sort_dev(codec, d_src, off, ln, d_dst, cap, rb, ko, kl, alg, sb, sl, sc)
-        out = np.zeros(max(r["total"], 1), np.uint8)
-        if r["n_records"] and r["total"]:
-            capi.dev_memcpy(out.ctypes.data, d_dst, r["total"], 2)
-        return out[: r["total"]].tobytes() if r["n_records"] else b"", r
-    finally:
-        capi.dev_free(d_src)
-        capi.dev_free(d_dst)
-
-
 def check(capi, codec, level, alg, plain, rb, ko, kl, dev=False):
     blocks = build_blocks(capi, codec, level, alg, plain)
     total = sum(len(b) for b in plain)
-    got, r = (sort_dev if dev else sort_packed)(capi, codec, alg, blocks, rb, ko, kl, total)
+    got, r = run(capi, "decompress_sort", codec, alg, blocks, (rb, ko, kl), total, dev)
     assert (r["status"] == 0).all(), r["status"]
     assert r["total"] == total and r["n_records"] == total // rb
     assert got == model_sort(plain, rb, ko, kl)
@@ -133,11 +91,11 @@ def test_blocks_with_several_slices(capi, oracle):
     off = np.array([a_off[0], a_off[2]], np.uint64)
     ln = np.array([a_ln[0] + a_ln[1], a_ln[2] + a_ln[3]], np.uint64)
     blocks = (a_arena, off, ln, np.array([0, 2, 4], np.uint32), np.array(a_ln, np.uint64), np.array(a_ck, np.uint64))
-    got, r = sort_packed(capi, 1, 3, blocks, REC, KEY_OFF, KEY_LEN, recs.size)
+    got, r = run(capi, "decompress_sort", 1, 3, blocks, (REC, KEY_OFF, KEY_LEN), recs.size)
     assert (r["status"] == 0).all() and got == model_sort(parts, REC, KEY_OFF, KEY_LEN)
     bad_ck = blocks[5].copy()
     bad_ck[3] ^= 1  # second slice of the second block
-    got, r = sort_packed(capi, 1, 3, blocks[:5] + (bad_ck,), REC, KEY_OFF, KEY_LEN, recs.size)
+    got, r = run(capi, "decompress_sort", 1, 3, blocks[:5] + (bad_ck,), (REC, KEY_OFF, KEY_LEN), recs.size)
     assert list(r["status"]) == [0, capi.E_CHECKSUM] and r["bad_slice"][1] == 1 and r["n_records"] == 0
 
 
@@ -209,7 +167,7 @@ def test_more_than_2_pow_24_records_and_2_gib(capi):
     plain = split_blocks(recs, sizes)
     blocks = build_blocks(capi, 1, 0, 3, plain)
     del plain
-    got, r = sort_packed(capi, 1, 3, blocks, rb, ko, kl, recs.size)
+    got, r = run(capi, "decompress_sort", 1, 3, blocks, (rb, ko, kl), recs.size)
     assert (r["status"] == 0).all() and r["n_records"] == n and r["total"] == recs.size
     key = recs[:, ko:ko + kl].copy().view(">u8").ravel()
     order = np.argsort(key, kind="stable")
@@ -225,10 +183,10 @@ def test_bad_arguments(capi, oracle):
     blocks = build_blocks(capi, 1, 0, 0, [terasort_records(oracle, 100).tobytes()])
     for rb, ko, kl in [(REC, 2, 0), (REC, 2, 17), (REC, REC - 9, 10), (0, 0, 1), (10, 0, 11)]:
         with pytest.raises(capi.B2SError) as e:
-            sort_packed(capi, 1, 0, blocks, rb, ko, kl, 100 * REC)
+            run(capi, "decompress_sort", 1, 0, blocks, (rb, ko, kl), 100 * REC)
         assert e.value.code == capi.E_ARG
     with pytest.raises(capi.B2SError) as e:
-        sort_packed(capi, 1, 7, blocks, REC, 2, 10, 100 * REC)
+        run(capi, "decompress_sort", 1, 7, blocks, (REC, 2, 10), 100 * REC)
     assert e.value.code == capi.E_UNSUPPORTED
 
 
@@ -240,7 +198,7 @@ def test_bad_checksum_in_one_slice(capi, oracle):
         blocks[5] = blocks[5].copy()
         blocks[5][1] ^= 0x10
         for dev in (False, True):
-            got, r = (sort_dev if dev else sort_packed)(capi, codec, 2, tuple(blocks), REC, 2, 10, recs.size)
+            got, r = run(capi, "decompress_sort", codec, 2, tuple(blocks), (REC, 2, 10), recs.size, dev)
             assert list(r["status"]) == [0, capi.E_CHECKSUM, 0] and r["bad_slice"][1] == 0
             assert r["n_records"] == 0 and got == b""
 
@@ -250,7 +208,7 @@ def test_block_that_is_not_whole_records(capi, oracle):
     plain = [recs[:100 * REC], recs[100 * REC:200 * REC - 1], recs[200 * REC - 1:]]
     for codec in (0, 1):
         blocks = build_blocks(capi, codec, 0, 3, plain)
-        got, r = sort_packed(capi, codec, 3, blocks, REC, 2, 10, len(recs))
+        got, r = run(capi, "decompress_sort", codec, 3, blocks, (REC, 2, 10), len(recs))
         assert list(r["status"]) == [0, capi.E_CORRUPT, capi.E_CORRUPT] and r["n_records"] == 0 and got == b""
         assert b"block 1 " in capi.load().b2s_last_error()
 
@@ -262,7 +220,7 @@ def test_corrupt_stream(capi, oracle):
         arena, off, ln, sb, sl, sc = build_blocks(capi, codec, 1, 0, plain)
         arena = arena.copy()
         arena[int(off[2]):int(off[2] + ln[2])] = 0xA5  # every byte of the third stream
-        got, r = sort_packed(capi, codec, 0, (arena, off, ln, sb, sl, sc), REC, 2, 10, recs.size)
+        got, r = run(capi, "decompress_sort", codec, 0, (arena, off, ln, sb, sl, sc), (REC, 2, 10), recs.size)
         assert r["status"][2] == capi.E_CORRUPT and r["n_records"] == 0 and got == b""
 
 
@@ -298,7 +256,7 @@ def test_beside_a_concurrent_compress(capi, oracle):
     recs = terasort_records(oracle, 200_000, seed=9)
     plain = split_blocks(recs, [50_000] * 4)
     blocks = build_blocks(capi, 1, 0, 3, plain)
-    want_sorted, _ = sort_packed(capi, 1, 3, blocks, REC, 2, 10, recs.size)
+    want_sorted, _ = run(capi, "decompress_sort", 1, 3, blocks, (REC, 2, 10), recs.size)
     src = recs.ravel()
     offs = np.arange(0, src.size, 1 << 20, dtype=np.uint64)
     lens = np.minimum(np.uint64(1 << 20), np.uint64(src.size) - offs).astype(np.uint64)
@@ -308,7 +266,7 @@ def test_beside_a_concurrent_compress(capi, oracle):
     out = {}
 
     def sorter():
-        out["sort"] = [sort_packed(capi, 1, 3, blocks, REC, 2, 10, recs.size)[0] for _ in range(3)]
+        out["sort"] = [run(capi, "decompress_sort", 1, 3, blocks, (REC, 2, 10), recs.size)[0] for _ in range(3)]
 
     def compressor():
         res = []
@@ -356,8 +314,8 @@ def test_terasort_end_to_end(capi, oracle, name, codec, level):
         off = np.concatenate([[0], np.cumsum(lens)[:-1]]).astype(np.uint64)
         ck = np.array([outs[m][1]["checksums"][red] for m in range(M)], np.uint64)
         decoded = sum(int(np.sum(key_range_ids(maps[m], R) == red)) for m in range(M)) * REC
-        got, r = sort_packed(capi, codec, 3, (arena, off, lens, np.arange(M + 1, dtype=np.uint32), lens, ck), REC, 2,
-                             10, decoded)
+        got, r = run(capi, "decompress_sort", codec, 3, (arena, off, lens, np.arange(M + 1, dtype=np.uint32), lens, ck),
+                     (REC, 2, 10), decoded)
         assert (r["status"] == 0).all() and r["total"] == decoded
         sorted_all.append(got)
     out = np.frombuffer(b"".join(sorted_all), np.uint8).reshape(-1, REC)
@@ -367,25 +325,11 @@ def test_terasort_end_to_end(capi, oracle, name, codec, level):
     assert out.tobytes() == model_sort([m.tobytes() for m in maps], REC, 2, 10)  # a permutation, stable by map order
 
 
-def mirror_conf(tmp_path, codec, **extra):
-    import uuid
-    conf = {
-        "spark.app.id": "app-" + uuid.uuid4().hex[:12],
-        "spark.shuffle.s3.rootDir": "file://" + str(tmp_path) + "/spark-s3-shuffle",
-        "spark.shuffle.checksum.enabled": True,
-        "spark.shuffle.checksum.algorithm": "CRC32C",
-        "spark.io.compression.codec": "lz4",
-        "spark.shuffle.compress": codec != "none",
-    }
-    conf.update(extra)
-    return conf
-
-
 @pytest.mark.parametrize("codec", ["lz4", "none"])
 def test_terasort_through_the_host_mirror(tmp_path, oracle, codec):
     """serialized-writer files of M maps, read back per reducer with b2sh_reader_read_sorted"""
     host = pkg.host
-    d = host.S3ShuffleDispatcher(mirror_conf(tmp_path, codec))
+    d = mirror(tmp_path, codec)
     M, R, per_map = 3, 8, 5000
     maps = [terasort_records(oracle, per_map, seed=40 + m) for m in range(M)]
     for m in range(M):
@@ -411,7 +355,7 @@ def test_host_mirror_blocks_larger_than_the_task_budget(tmp_path, oracle, codec,
     head plus a tail read through from the block stream, and must be staged whole.  The compressible records (zero
     payload) decode to more than 4x their compressed size, past the first output guess of read_sorted."""
     host = pkg.host
-    d = host.S3ShuffleDispatcher(mirror_conf(tmp_path, codec, **{"spark.shuffle.s3.maxBufferSizeTask": 20_000}))
+    d = mirror(tmp_path, codec, **{"spark.shuffle.s3.maxBufferSizeTask": 20_000})
     M, R, per_map = 2, 2, 4000
     maps = [terasort_records(oracle, per_map, seed=60 + m).copy() for m in range(M)]
     if shape == "compressible":

@@ -3,18 +3,16 @@ records ([int32 big-endian size][row]) in, every record out, sorted by one typed
 little-endian int32 / int64), nulls first, stable.  The model parses the decoded streams in Python and sorts the
 records stably by (non-null flag, key); the call must be byte for byte that model."""
 import ctypes as C
-import uuid
 
 import numpy as np
 import pytest
 
 import spark_s3_shuffle_b200 as pkg
+from rows_model import CHECKSUMS, CODECS, KEY_BYTES, KEY_INT32, KEY_INT64, blocks_of, build_blocks, mirror, \
+    model_sort, run, stream, write_maps
 
 pytestmark = pytest.mark.gpu
 
-CODECS = [("none", 0, 0), ("lz4", 1, 0), ("snappy", 2, 0), ("zstd1", 3, 1), ("zstd3", 3, 3)]
-CHECKSUMS = [0, 1, 2, 3]  # none, ADLER32, CRC32, CRC32C
-KEY_BYTES, KEY_INT32, KEY_INT64 = 0, 1, 2
 KEY_LEN = {KEY_INT32: 4, KEY_INT64: 8}
 INT_EDGES = {KEY_INT32: [-2**31, 2**31 - 1, 0, -1, 1], KEY_INT64: [-2**63, 2**63 - 1, 0, -1, 1, -2**31 - 1, 2**31]}
 
@@ -22,37 +20,6 @@ INT_EDGES = {KEY_INT32: [-2**31, 2**31 - 1, 0, -1, 1], KEY_INT64: [-2**63, 2**63
 # ---------------------------------------------------------------------------------------------------------------
 # model and helpers
 # ---------------------------------------------------------------------------------------------------------------
-def stream(rows):
-    """UnsafeRowSerializer framing of the rows"""
-    return b"".join(len(r).to_bytes(4, "big") + bytes(r) for r in rows)
-
-
-def parse(buf):
-    """decoded stream -> [(offset, record length)]"""
-    out, p = [], 0
-    while p < len(buf):
-        s = int.from_bytes(buf[p:p + 4], "big")
-        out.append((p, 4 + s))
-        p += 4 + s
-    assert p == len(buf)
-    return out
-
-
-def sort_key(buf, o, kt, ko, kl, nf):
-    row = o + 4
-    if nf >= 0 and (int.from_bytes(buf[row + 8 * (nf >> 6):row + 8 * (nf >> 6) + 8], "little") >> (nf & 63)) & 1:
-        return (0, b"" if kt == KEY_BYTES else 0)
-    k = buf[row + ko:row + ko + kl]
-    return (1, k if kt == KEY_BYTES else int.from_bytes(k, "little", signed=True))
-
-
-def model_sort(plain, kt, ko, kl, nf=-1):
-    buf = b"".join(plain)
-    recs = parse(buf)
-    order = sorted(range(len(recs)), key=lambda i: sort_key(buf, recs[i][0], kt, ko, kl, nf))  # stable
-    return b"".join(buf[recs[i][0]:recs[i][0] + recs[i][1]] for i in order), len(recs)
-
-
 def make_rows(rng, n, kt, ko, kl, nf=-1, lens=None, keys=None, null_frac=0.0, tag_at=None):
     """n random rows of lens[i] bytes (default 56) with the key at ko and, when nf >= 0, the null bit set with
     probability null_frac.  keys: the key values (ints, or bytes); tag_at: the row's index as 4 bytes there."""
@@ -86,65 +53,15 @@ def int_keys(rng, n, kt, ties=False):
     return k
 
 
-def build_blocks(capi, codec, level, alg, plain):
-    """one compressed stream per block, one slice per block -> (arena, off, len, slice_base, slice_len, slice_ck)"""
-    n = len(plain)
-    lens = np.array([len(b) for b in plain], dtype=np.uint64)
-    offs = np.concatenate([[0], np.cumsum(lens)[:-1]]).astype(np.uint64) if n else np.zeros(0, np.uint64)
-    src = np.frombuffer(b"".join(plain), np.uint8) if lens.sum() else np.zeros(1, np.uint8)
-    if codec == 0:
-        arena, off, ln = src, offs, lens
-    else:
-        bound = sum(capi.compress_bound(codec, 0, int(l)) for l in lens) + 64
-        dst = np.zeros(bound, np.uint8)
-        r = capi.compress_packed(codec, src, offs, lens, dst, 0, 0, level)
-        assert (r["status"] == 0).all()
-        arena, off, ln = dst[: max(r["total"], 1)], r["dst_off"], r["dst_len"]
-    ck = capi.checksum_packed(alg, arena, off, ln) if alg and n else np.zeros(n, np.uint64)
-    return arena, off, ln, np.arange(n + 1, dtype=np.uint32), np.array(ln, dtype=np.uint64), ck
-
-
-def sort_packed(capi, codec, alg, blocks, kt, ko, kl, nf, cap):
-    arena, off, ln, sb, sl, sc = blocks
-    dst = np.zeros(max(cap, 1), np.uint8)
-    r = capi.decompress_sort_rows_packed(codec, arena, off, ln, dst[:cap], kt, ko, kl, nf, alg, sb, sl, sc)
-    return dst[: r["total"]].tobytes() if r["n_records"] else b"", r
-
-
-def sort_dev(capi, codec, alg, blocks, kt, ko, kl, nf, cap):
-    arena, off, ln, sb, sl, sc = blocks
-    d_src = capi.dev_alloc(max(arena.size, 1))
-    d_dst = capi.dev_alloc(max(cap, 1))
-    try:
-        capi.dev_memcpy(d_src, arena.ctypes.data, arena.size, 1)
-        r = capi.decompress_sort_rows_dev(codec, d_src, off, ln, d_dst, cap, kt, ko, kl, nf, alg, sb, sl, sc)
-        out = np.zeros(max(r["total"], 1), np.uint8)
-        if r["n_records"] and r["total"]:
-            capi.dev_memcpy(out.ctypes.data, d_dst, r["total"], 2)
-        return out[: r["total"]].tobytes() if r["n_records"] else b"", r
-    finally:
-        capi.dev_free(d_src)
-        capi.dev_free(d_dst)
-
-
 def check(capi, codec, level, alg, plain, kt, ko, kl, nf=-1, dev=False, blocks=None):
     blocks = blocks or build_blocks(capi, codec, level, alg, plain)
     total = sum(len(b) for b in plain)
-    got, r = (sort_dev if dev else sort_packed)(capi, codec, alg, blocks, kt, ko, kl, nf, total)
+    got, r = run(capi, "decompress_sort_rows", codec, alg, blocks, (kt, ko, kl, nf), total, dev)
     assert (r["status"] == 0).all(), r["status"]
-    want, n = model_sort(plain, kt, ko, kl, nf)
+    want, n = model_sort(plain, [(kt, ko, kl, nf)])
     assert r["total"] == total and r["n_records"] == n
     assert got == want
     return got
-
-
-def blocks_of(rows, sizes):
-    out, at = [], 0
-    for s in sizes:
-        out.append(stream(rows[at:at + s]))
-        at += s
-    assert at == len(rows)
-    return out
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -298,7 +215,7 @@ def test_one_block_of_a_million_records(capi):
     rec[:, 12:20] = keys.view(np.uint8).reshape(n, 8)
     for codec in (1, 0):
         blocks = build_blocks(capi, codec, 0, 3, [rec.tobytes()])
-        got, r = sort_packed(capi, codec, 3, blocks, KEY_INT64, 8, 8, 0, rec.size)
+        got, r = run(capi, "decompress_sort_rows", codec, 3, blocks, (KEY_INT64, 8, 8, 0), rec.size)
         assert (r["status"] == 0).all() and r["n_records"] == n
         order = np.lexsort((np.where(nulls, 0, keys), ~nulls))  # stable: non-null flag, then key
         assert got == rec[order].tobytes()
@@ -340,8 +257,8 @@ def test_each_corruption_rule_fails_its_block(capi, rule):
     for codec in (0, 1, 3):
         blocks = build_blocks(capi, codec, 1, 3, plain)
         for dev in (False, True):
-            got, r = (sort_dev if dev else sort_packed)(capi, codec, 3, blocks, KEY_INT64, 8, 8, nf,
-                                                         sum(map(len, plain)))
+            got, r = run(capi, "decompress_sort_rows", codec, 3, blocks, (KEY_INT64, 8, 8, nf), sum(map(len, plain)),
+                         dev)
             assert list(r["status"]) == [0, capi.E_CORRUPT, 0, 0] and r["n_records"] == 0 and got == b""
             err = capi.load().b2s_last_error()
             assert b"block 1: " in err and (b"at byte %d:" % len(head)) in err, err
@@ -355,8 +272,8 @@ def test_bad_checksum_in_one_block(capi):
         blocks[5] = blocks[5].copy()
         blocks[5][1] ^= 0x10
         for dev in (False, True):
-            got, r = (sort_dev if dev else sort_packed)(capi, codec, 2, tuple(blocks), KEY_INT64, 8, 8, -1,
-                                                         sum(map(len, plain)))
+            got, r = run(capi, "decompress_sort_rows", codec, 2, tuple(blocks), (KEY_INT64, 8, 8, -1),
+                         sum(map(len, plain)), dev)
             assert list(r["status"]) == [0, capi.E_CHECKSUM, 0] and r["bad_slice"][1] == 0
             assert r["n_records"] == 0 and got == b""
 
@@ -382,7 +299,7 @@ def test_bad_arguments(capi, kt, ko, kl, nf):
     rng = np.random.default_rng(63)
     blocks = build_blocks(capi, 1, 0, 0, [stream(good_rows(rng))])
     with pytest.raises(capi.B2SError) as e:
-        sort_packed(capi, 1, 0, blocks, kt, ko, kl, nf, 1 << 16)
+        run(capi, "decompress_sort_rows", 1, 0, blocks, (kt, ko, kl, nf), 1 << 16)
     assert e.value.code == capi.E_ARG
 
 
@@ -419,27 +336,6 @@ def test_sql_exchange_end_to_end(capi, name, codec, level):
 # ---------------------------------------------------------------------------------------------------------------
 # 7. the host mirror: b2sh_reader_read_sorted_rows over the serialized writer's files
 # ---------------------------------------------------------------------------------------------------------------
-def mirror(tmp_path, codec):
-    host = pkg.host
-    return host.S3ShuffleDispatcher({
-        "spark.app.id": "app-" + uuid.uuid4().hex[:12],
-        "spark.shuffle.s3.rootDir": "file://" + str(tmp_path) + "/spark-s3-shuffle",
-        "spark.shuffle.checksum.enabled": True,
-        "spark.shuffle.checksum.algorithm": "CRC32C",
-        "spark.io.compression.codec": "lz4",
-        "spark.shuffle.compress": codec != "none",
-    })
-
-
-def write_maps(host, d, maps, R):
-    for m, (rows, ids) in enumerate(maps):
-        w = host.S3SerializedShuffleWriter(d, 0, m, R)
-        for row, p in zip(rows, ids):
-            w.insertRecord(int(p), len(row).to_bytes(4, "big") + row)
-        w.commit()
-        w.close()
-
-
 @pytest.mark.parametrize("codec", ["lz4", "none"])
 def test_host_mirror_reads_rows_sorted(tmp_path, codec):
     host = pkg.host
@@ -457,7 +353,7 @@ def test_host_mirror_reads_rows_sorted(tmp_path, codec):
         data, n = rd.readSortedRows(KEY_INT32, 8, 4, 0)
         rd.close()
         want, wn = model_sort([stream([r for r, p in zip(rows, ids) if p == red]) for rows, ids in maps],
-                              KEY_INT32, 8, 4, 0)
+                              [(KEY_INT32, 8, 4, 0)])
         assert n == wn and data == want
     d.close()
 

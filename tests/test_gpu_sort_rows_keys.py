@@ -7,70 +7,12 @@ import numpy as np
 import pytest
 
 import spark_s3_shuffle_b200 as pkg
-from test_gpu_aggregate_rows import is_null, merge, mirror, write_maps
-from test_gpu_sort_rows import CHECKSUMS, CODECS, KEY_BYTES, KEY_INT32, KEY_INT64, blocks_of, build_blocks, parse, \
-    stream
+from rows_model import CHECKSUMS, CODECS, KEY_BYTES, KEY_INT32, KEY_INT64, MAX_I64, MIN_I32, MIN_I64, STRING, SUM_I64, \
+    blocks_of, build_blocks, mirror, model_aggregate, model_sort, run, stream, write_maps
 
 pytestmark = pytest.mark.gpu
 
-STRING = 3
-SUM_I64, SUM_F64, MIN_I32, MAX_I32, MIN_I64, MAX_I64, MIN_F64, MAX_F64 = range(8)
 P, CHUNK = 20, 16  # the first pass's key bytes and a refinement round's
-
-
-# ---------------------------------------------------------------------------------------------------------------
-# model
-# ---------------------------------------------------------------------------------------------------------------
-def col_value(row, col):
-    kt, ko, kl, nf = col
-    if nf >= 0 and is_null(row, nf):
-        return (0, b"" if kt in (KEY_BYTES, STRING) else 0)
-    if kt == STRING:
-        slot = int.from_bytes(row[ko:ko + 8], "little")
-        o, s = slot >> 32, slot & 0xFFFFFFFF
-        return (1, bytes(row[o:o + s]))
-    k = bytes(row[ko:ko + kl])
-    return (1, k if kt == KEY_BYTES else int.from_bytes(k, "little", signed=True))
-
-
-def model_keys(plain, keys):
-    buf = b"".join(plain)
-    recs = parse(buf)
-    kv = [tuple(col_value(buf[o + 4:o + ln], c) for c in keys) for o, ln in recs]
-    order = sorted(range(len(recs)), key=lambda i: kv[i])  # stable
-    return buf, recs, kv, order
-
-
-def model_sort(plain, keys):
-    buf, recs, _, order = model_keys(plain, keys)
-    return b"".join(buf[recs[i][0]:recs[i][0] + recs[i][1]] for i in order), len(recs)
-
-
-def model_aggregate(plain, keys, aggs):
-    buf, recs, kv, order = model_keys(plain, keys)
-    out, j = [], 0
-    while j < len(order):
-        e = j
-        while e < len(order) and kv[order[e]] == kv[order[j]]:
-            e += 1
-        o, ln = recs[order[j]]
-        rec = bytearray(buf[o:o + ln])
-        row = memoryview(rec)[4:]
-        nulls = []
-        for op, off, anf in aggs:
-            vals = [bytes(buf[recs[i][0] + 4 + off:recs[i][0] + 4 + off + 8]) for i in order[j:e]
-                    if not is_null(buf[recs[i][0] + 4:recs[i][0] + recs[i][1]], anf)]
-            row[off:off + 8] = merge(op, vals) if vals else bytes(8)
-            nulls.append((anf, not vals))
-        for anf, null in nulls:
-            if anf >= 0:
-                w = 8 * (anf >> 6)
-                v = int.from_bytes(row[w:w + 8], "little")
-                v = v | (1 << (anf & 63)) if null else v & ~(1 << (anf & 63))
-                row[w:w + 8] = v.to_bytes(8, "little")
-        out.append(bytes(rec))
-        j = e
-    return b"".join(out), len(recs), len(out)
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -141,48 +83,10 @@ def rand_rows(rng, n, keys, null_frac=0.15, aggs=(), tail=True):
     return rows
 
 
-def run_sort(capi, codec, alg, blocks, keys, cap, dev=False):
-    arena, off, ln, sb, sl, sc = blocks
-    if not dev:
-        dst = np.zeros(max(cap, 1), np.uint8)
-        r = capi.decompress_sort_rows_keys_packed(codec, arena, off, ln, dst[:cap], keys, alg, sb, sl, sc)
-        return dst[: r["total"]].tobytes() if r["n_records"] else b"", r
-    d_src, d_dst = capi.dev_alloc(max(arena.size, 1)), capi.dev_alloc(max(cap, 1))
-    try:
-        capi.dev_memcpy(d_src, arena.ctypes.data, arena.size, 1)
-        r = capi.decompress_sort_rows_keys_dev(codec, d_src, off, ln, d_dst, cap, keys, alg, sb, sl, sc)
-        out = np.zeros(max(r["total"], 1), np.uint8)
-        if r["n_records"] and r["total"]:
-            capi.dev_memcpy(out.ctypes.data, d_dst, r["total"], 2)
-        return out[: r["total"]].tobytes() if r["n_records"] else b"", r
-    finally:
-        capi.dev_free(d_src)
-        capi.dev_free(d_dst)
-
-
-def run_agg(capi, codec, alg, blocks, keys, aggs, cap, dev=False):
-    arena, off, ln, sb, sl, sc = blocks
-    if not dev:
-        dst = np.zeros(max(cap, 1), np.uint8)
-        r = capi.decompress_aggregate_rows_keys_packed(codec, arena, off, ln, dst[:cap], keys, aggs, alg, sb, sl, sc)
-        return dst[: r["total"]].tobytes(), r
-    d_src, d_dst = capi.dev_alloc(max(arena.size, 1)), capi.dev_alloc(max(cap, 1))
-    try:
-        capi.dev_memcpy(d_src, arena.ctypes.data, arena.size, 1)
-        r = capi.decompress_aggregate_rows_keys_dev(codec, d_src, off, ln, d_dst, cap, keys, aggs, alg, sb, sl, sc)
-        out = np.zeros(max(r["total"], 1), np.uint8)
-        if r["total"]:
-            capi.dev_memcpy(out.ctypes.data, d_dst, r["total"], 2)
-        return out[: r["total"]].tobytes(), r
-    finally:
-        capi.dev_free(d_src)
-        capi.dev_free(d_dst)
-
-
 def check_sort(capi, plain, keys, codec=1, level=0, alg=0, dev=False, blocks=None):
     blocks = blocks or build_blocks(capi, codec, level, alg, plain)
     total = sum(len(b) for b in plain)
-    got, r = run_sort(capi, codec, alg, blocks, keys, total, dev)
+    got, r = run(capi, "decompress_sort_rows_keys", codec, alg, blocks, (keys,), total, dev)
     assert (r["status"] == 0).all(), r["status"]
     want, n = model_sort(plain, keys)
     assert (r["total"], r["n_records"]) == (total, n)
@@ -193,7 +97,7 @@ def check_sort(capi, plain, keys, codec=1, level=0, alg=0, dev=False, blocks=Non
 def check_agg(capi, plain, keys, aggs, codec=1, level=0, alg=0, dev=False, blocks=None):
     blocks = blocks or build_blocks(capi, codec, level, alg, plain)
     total = sum(len(b) for b in plain)
-    got, r = run_agg(capi, codec, alg, blocks, keys, aggs, total, dev)
+    got, r = run(capi, "decompress_aggregate_rows_keys", codec, alg, blocks, (keys, aggs), total, dev)
     assert (r["status"] == 0).all(), r["status"]
     want, n, g = model_aggregate(plain, keys, aggs)
     assert (r["n_records"], r["n_groups"], r["total"]) == (n, g, len(want))
@@ -368,11 +272,11 @@ def test_one_column_is_the_single_key_call(capi, kt, kl, nf):
     total = sum(len(b) for b in plain)
     want = np.zeros(total, np.uint8)
     r1 = capi.decompress_sort_rows_packed(1, arena, off, ln, want, kt, 8, kl, nf, 3, sb, sl, sc)
-    got, r2 = run_sort(capi, 1, 3, blocks, keys, total)
+    got, r2 = run(capi, "decompress_sort_rows_keys", 1, 3, blocks, (keys,), total)
     assert got == want.tobytes() and r1["n_records"] == r2["n_records"] == 4000
     want = np.zeros(total, np.uint8)
     a1 = capi.decompress_aggregate_rows_packed(1, arena, off, ln, want, kt, 8, kl, nf, aggs, 3, sb, sl, sc)
-    got, a2 = run_agg(capi, 1, 3, blocks, keys, aggs, total)
+    got, a2 = run(capi, "decompress_aggregate_rows_keys", 1, 3, blocks, (keys, aggs), total)
     assert got == want[: a1["total"]].tobytes()
     assert (a1["n_records"], a1["n_groups"], a1["total"]) == (a2["n_records"], a2["n_groups"], a2["total"])
 
@@ -393,8 +297,8 @@ def test_string_past_its_row_fails_the_block(capi):
     for aggregate in (False, True):
         blocks = build_blocks(capi, 2, 0, 0, plain)
         total = sum(len(b) for b in plain)
-        got, r = (run_agg(capi, 2, 0, blocks, keys, [], total) if aggregate
-                  else run_sort(capi, 2, 0, blocks, keys, total))
+        got, r = (run(capi, "decompress_aggregate_rows_keys", 2, 0, blocks, (keys, []), total) if aggregate
+                  else run(capi, "decompress_sort_rows_keys", 2, 0, blocks, (keys,), total))
         assert list(r["status"]) == [0, capi.E_CORRUPT]
         assert r["n_records"] == 0 and got == b""
         err = capi.load().b2s_last_error().decode()
@@ -419,10 +323,11 @@ def test_bad_checksum_in_one_block(capi):
     arena, off, ln, sb, sl, sc = build_blocks(capi, 1, 0, 3, plain)
     sc = sc.copy()
     sc[1] ^= 1
+    blocks = (arena, off, ln, sb, sl, sc)
     total = sum(len(b) for b in plain)
     for aggregate in (False, True):
-        got, r = (run_agg(capi, 1, 3, (arena, off, ln, sb, sl, sc), keys, [], total) if aggregate
-                  else run_sort(capi, 1, 3, (arena, off, ln, sb, sl, sc), keys, total))
+        got, r = (run(capi, "decompress_aggregate_rows_keys", 1, 3, blocks, (keys, []), total) if aggregate
+                  else run(capi, "decompress_sort_rows_keys", 1, 3, blocks, (keys,), total))
         assert list(r["status"]) == [0, capi.E_CHECKSUM, 0] and r["n_records"] == 0
 
 
@@ -434,11 +339,11 @@ def test_short_destination_reports_the_bytes_needed(capi):
     blocks = build_blocks(capi, 0, 0, 0, plain)
     total = sum(len(b) for b in plain)
     with pytest.raises(capi.B2SError) as e:
-        run_sort(capi, 0, 0, blocks, keys, total - 1)
+        run(capi, "decompress_sort_rows_keys", 0, 0, blocks, (keys,), total - 1)
     assert e.value.code == capi.E_DST_TOO_SMALL
     want, _, _ = model_aggregate(plain, keys, [])
     with pytest.raises(capi.B2SError) as e:
-        run_agg(capi, 0, 0, blocks, keys, [], len(want) - 1)
+        run(capi, "decompress_aggregate_rows_keys", 0, 0, blocks, (keys, []), len(want) - 1)
     assert e.value.code == capi.E_DST_TOO_SMALL
     assert str(len(want)) in capi.load().b2s_last_error().decode()
 
@@ -466,9 +371,9 @@ def test_bad_arguments(capi, keys, aggs):
     for aggregate in ([True] if aggs else [False, True]):
         with pytest.raises(capi.B2SError) as e:
             if aggregate:
-                run_agg(capi, 0, 0, blocks, keys, aggs, 4096)
+                run(capi, "decompress_aggregate_rows_keys", 0, 0, blocks, (keys, aggs), 4096)
             else:
-                run_sort(capi, 0, 0, blocks, keys, 4096)
+                run(capi, "decompress_sort_rows_keys", 0, 0, blocks, (keys,), 4096)
         assert e.value.code == capi.E_ARG
 
 
@@ -527,7 +432,7 @@ def test_host_mirror_reads_rows_by_a_composite_key(capi, tmp_path, codec):
         want, wn = model_sort(plain, keys)
         assert n == wn and data == want
         blocks = build_blocks(capi, 0, 0, 0, plain)
-        assert data == run_sort(capi, 0, 0, blocks, keys, sum(len(b) for b in plain))[0]
+        assert data == run(capi, "decompress_sort_rows_keys", 0, 0, blocks, (keys,), sum(len(b) for b in plain))[0]
         data, n, g = rd.readAggregatedRowsKeys(keys, aggs)
         rd.close()
         want, wn, wg = model_aggregate(plain, keys, aggs)
