@@ -56,6 +56,19 @@ extern "C" {
  * naming the size bytes at row offset offset, unsigned lexicographic, a proper prefix first (StringType under
  * UTF8_BINARY, BinaryType) */
 #define B2S_STRING_KEY 3
+/* ... and these column types (4 is unassigned); BooleanType needs none: it is B2S_KEY_BYTES with key_len 1 (0 / 1) */
+#define B2S_KEY_INT16 (5)   /* 2 bytes, little-endian two's complement: ShortType */
+#define B2S_KEY_INT8 (6)    /* 1 byte, signed: ByteType */
+#define B2S_KEY_FLOAT32 (7) /* 4 bytes, IEEE float, Spark SQL's order: -0.0 == 0.0, NaN == NaN above +inf: FloatType */
+#define B2S_KEY_FLOAT64 (8) /* 8 bytes, IEEE double, the same order: DoubleType */
+/* an 8-byte UnsafeRow slot (offset << 32) | size naming size (1..16) bytes at row offset offset: the unscaled value of
+ * a Decimal(p > 18), big-endian two's complement (BigInteger.toByteArray), ordered as a signed integer */
+#define B2S_DECIMAL_KEY (9)
+/* order flags, OR-ed into a composite-key column's key_type: its non-null values sort in reverse; its nulls sort after
+ * its non-null values (Spark's SortOrder direction and null ordering; NULLS_LAST on a column without a null bit is
+ * accepted and changes nothing) */
+#define B2S_KEY_DESCENDING (1u << 8)
+#define B2S_KEY_NULLS_LAST (1u << 9)
 
 /* aggregate ops of the row aggregation (b2s_decompress_aggregate_rows_*), each over an 8-byte slot of the row */
 #define B2S_AGG_SUM_INT64 0   /* wrapping two's-complement sum: Sum(long), Count, Average's count */
@@ -323,24 +336,41 @@ int b2s_decompress_aggregate_rows_dev(uint32_t dev_index, uint32_t codec, uint32
  * parallel arrays: column c is key_type[c] at row offset key_off[c], key_len[c] bytes, null bit key_null_field[c].
  * Columns compare left to right; each is read exactly as the single-key calls read their key (B2S_KEY_BYTES,
  * B2S_KEY_INT32, B2S_KEY_INT64: the same key_len rules), and a null sorts first within its column (-1: never null).
- * B2S_STRING_KEY (these calls only): key_len 8, the slot of a variable-length value; a null string and an empty string
- * are different keys.  Two columns may share a slot or a null word.
- * Sort: every record, stably sorted by the composite key (ascending, nulls first per column).  Aggregate: a group is a
- * maximal run of records whose every column is equal (both null, or both non-null with equal values; strings: equal
- * length and bytes); aggregates, output rows, group order and *n_groups are as in b2s_decompress_aggregate_rows_*.
- * With n_keys == 1 and a fixed-width column the output is byte for byte that of the single-key call.
+ * These calls only:
+ *   B2S_STRING_KEY: key_len 8, the slot of a variable-length value; a null string and an empty string are different
+ *   B2S_KEY_INT16 / B2S_KEY_INT8: key_len 2 / 1, signed; BooleanType is B2S_KEY_BYTES with key_len 1
+ *   B2S_KEY_FLOAT32 / B2S_KEY_FLOAT64: key_len 4 / 8, Spark SQL's order (SQLOrderingUtil.compareDoubles): -0.0 == 0.0,
+ *     every NaN equals every other NaN and sorts above +inf
+ *   B2S_DECIMAL_KEY: key_len 8, the slot of a Decimal(p > 18): size (1..16) bytes of the unscaled value, big-endian
+ *     two's complement, compared as signed integers (one column has one scale, so this is value order); a null
+ *     decimal's slot is not read
+ *   order flags OR-ed into key_type[c]: B2S_KEY_DESCENDING reverses the order of the column's non-null values;
+ *     B2S_KEY_NULLS_LAST puts its nulls after them (no effect with key_null_field[c] == -1).  Independent, as Spark's
+ *     SortOrder direction and null ordering.
+ * Two columns may share a slot or a null word.
+ * Sort: every record, stably sorted by the composite key (per column: ascending, nulls first, unless flagged).
+ * Aggregate: a group is a maximal run of records whose every column is equal (both null, or both non-null with equal
+ * values; strings: equal length and bytes; floats: as compared, so 0.0 and -0.0 form one group and all NaNs one);
+ * aggregates, output rows (each group's first record, its key bytes as they were), group order (the sort's) and
+ * *n_groups are as in b2s_decompress_aggregate_rows_*.
+ * With n_keys == 1, a fixed-width column of a single-key type and no flag the output is byte for byte that of the
+ * single-key call.
  * Per block, B2S_E_CORRUPT for every framing rule of the single-key calls, applied with the largest key_off + key_len
- * and null word of all columns, and when a non-null string's offset + size runs past the end of its row
- * (b2s_last_error() names the block and the byte offset of its first bad record).  When a block fails nothing is
- * written: *n_records (= *n_groups) = 0 and the call returns 0.
- * Errors -> B2S_E_ARG: n_keys outside [1, 16]; NULL key arrays; an unknown key_type; a key_len its type does not allow;
- * key_null_field[c] < -1; the aggregate checks of b2s_decompress_aggregate_rows_* against every column (no aggregate
- * slot overlaps any key slot or a null word any column uses).  Checksums, codec NONE, B2S_E_DST_TOO_SMALL,
+ * and null word of all columns, when a non-null string's offset + size runs past the end of its row, and when a
+ * non-null decimal's size is 0 or above 16 or its offset + size runs past the end of its row (b2s_last_error() names
+ * the block and the byte offset of its first bad record).  When a block fails nothing is written: *n_records
+ * (= *n_groups) = 0 and the call returns 0.
+ * Errors -> B2S_E_ARG: n_keys outside [1, 16]; NULL key arrays; an unknown key_type or a key_type bit above the low 8
+ * other than the two flags; a key_len its type does not allow; key_null_field[c] < -1; the aggregate checks of
+ * b2s_decompress_aggregate_rows_* against every column (no aggregate slot overlaps any key slot, a string's or
+ * decimal's 8-byte slot included, or a null word any column uses).  Checksums, codec NONE, B2S_E_DST_TOO_SMALL,
  * B2S_E_NOMEM, the read lane, the 1 GiB buffer trim and b2s_last_timing are as in the single-key calls.
- * The key is sorted by its first 20 encoded bytes (a column takes its bytes, plus one for its null bit; a string 9 per
- * started 8 bytes of value, at least 9).  A key longer than that — any string column, or fixed-width columns of more
- * than 20 bytes — is refined in rounds of 16 more bytes over the records still tied, and each round makes one small
- * blocking readback (the count of tied records; the first round also brings the string checks' verdicts). */
+ * The key is sorted by its first 20 encoded bytes (a column takes its value bytes — a decimal 16 — plus one for its
+ * null bit; a string 9 per started 8 bytes of value, at least 9).  A key longer than that — any string column, or
+ * fixed-width columns of more than 20 bytes — is refined in rounds of 16 more bytes over the records still tied, and
+ * each round makes one small blocking readback (the count of tied records; the first round also brings the string and
+ * decimal checks' verdicts).  A key with a decimal column always takes that first round, for its verdicts, even when
+ * it fits in 20 bytes.  DESCENDING and NULLS_LAST change no widths: a flagged key costs what the unflagged one does. */
 int b2s_decompress_sort_rows_keys_packed(uint32_t codec, uint32_t checksum_alg, uint32_t n, const uint8_t* src_base,
                                          const uint64_t* src_off, const uint64_t* src_len, const uint32_t* slice_base,
                                          const uint64_t* slice_len, const uint64_t* slice_checksum, uint32_t n_keys,

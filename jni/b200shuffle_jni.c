@@ -407,8 +407,10 @@ JNIEXPORT jint JNICALL J(decompressAggregateRowsPacked)(JNIEnv* e, jclass c, jin
 }
 
 /* ---- read side, composite key (INTEGRATION.md §3g / §3h): the row sort and the row aggregation by nKeys (1..16)
- *      columns, strings included: keyType (B2S_KEY_* or B2S_STRING_KEY) / keyOff / keyLen / keyNullField are
- *      int[nKeys]; other arrays and meta as decompressSortRowsPacked / decompressAggregateRowsPacked. ---- */
+ *      columns, strings included: keyType (B2S_KEY_*, B2S_STRING_KEY or B2S_DECIMAL_KEY, OR-ed with the order flags
+ *      B2S_KEY_DESCENDING / B2S_KEY_NULLS_LAST; as a Java int the flags are plain bits 8 and 9) / keyOff / keyLen /
+ *      keyNullField are int[nKeys], passed through unchanged; other arrays and meta as decompressSortRowsPacked /
+ *      decompressAggregateRowsPacked. ---- */
 JNIEXPORT jint JNICALL J(decompressSortRowsKeysPacked)(JNIEnv* e, jclass c, jint codec, jint alg, jint n, jlong src,
                                                        jlongArray off, jlongArray len, jintArray sliceBase,
                                                        jlongArray sliceLen, jlongArray sliceChecksum, jint nKeys,

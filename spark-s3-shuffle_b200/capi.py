@@ -14,6 +14,9 @@ CODEC_NONE, CODEC_LZ4BLOCK, CODEC_SNAPPY_XERIAL, CODEC_ZSTD = 0, 1, 2, 3
 CHECKSUM_NONE, CHECKSUM_ADLER32, CHECKSUM_CRC32, CHECKSUM_CRC32C = 0, 1, 2, 3
 KEY_BYTES, KEY_INT32, KEY_INT64 = 0, 1, 2  # key types of the row sort (decompress_sort_rows_*)
 STRING_KEY = 3  # the composite-key calls' variable-length key column (decompress_*_rows_keys_*)
+# the composite-key calls' other column types (BooleanType is KEY_BYTES with length 1) and order flags
+KEY_INT16, KEY_INT8, KEY_FLOAT32, KEY_FLOAT64, DECIMAL_KEY = 5, 6, 7, 8, 9
+KEY_DESCENDING, KEY_NULLS_LAST = 1 << 8, 1 << 9
 # aggregate ops of the row aggregation (decompress_aggregate_rows_*)
 (AGG_SUM_INT64, AGG_SUM_FLOAT64, AGG_MIN_INT32, AGG_MAX_INT32, AGG_MIN_INT64, AGG_MAX_INT64, AGG_MIN_FLOAT64,
  AGG_MAX_FLOAT64) = range(8)
@@ -464,15 +467,20 @@ def decompress_aggregate_rows_packed(codec, src, off, length, dst, key_type, key
 
 def decompress_sort_rows_keys_packed(codec, src, off, length, dst, keys, checksum_alg=CHECKSUM_NONE, slice_base=None,
                                      slice_len=None, slice_checksum=None):
-    """decompress_sort_rows_packed by a composite key: keys = [(KEY_* or STRING_KEY, row offset, length, null field
-    or -1), ...], compared left to right.  -> dict(total, n_records, status, bad_slice)"""
+    """decompress_sort_rows_packed by a composite key: keys = [(key type, row offset, length, null field or -1), ...],
+    compared left to right.  A key type is KEY_BYTES (1..16 bytes), KEY_INT8 / INT16 / INT32 / INT64 (1 / 2 / 4 / 8),
+    KEY_FLOAT32 / FLOAT64 (4 / 8, Spark SQL's order: -0.0 == 0.0, NaN above +inf), STRING_KEY or DECIMAL_KEY (the
+    8-byte (offset << 32) | size slot of a string, or of a Decimal(p > 18)'s 1..16 big-endian bytes), OR-ed with
+    KEY_DESCENDING (the column's values in reverse) and / or KEY_NULLS_LAST (its nulls after its values); without
+    flags a column is ascending, nulls first.  -> dict(total, n_records, status, bad_slice)"""
     return _sort_call("b2s_decompress_sort_rows_keys_packed", codec, src, off, length, dst, None, _key_arrays(keys),
                       checksum_alg, (slice_base, slice_len, slice_checksum))
 
 
 def decompress_aggregate_rows_keys_packed(codec, src, off, length, dst, keys, aggs=(), checksum_alg=CHECKSUM_NONE,
                                           slice_base=None, slice_len=None, slice_checksum=None):
-    """decompress_aggregate_rows_packed grouped by a composite key (keys as in decompress_sort_rows_keys_packed).
+    """decompress_aggregate_rows_packed grouped by a composite key (keys as in decompress_sort_rows_keys_packed; the
+    groups come out in that order, and float keys group by Spark SQL's equality: 0.0 with -0.0, every NaN together).
     -> dict(total, n_records, n_groups, status, bad_slice)"""
     return _sort_call("b2s_decompress_aggregate_rows_keys_packed", codec, src, off, length, dst, None,
                       (*_key_arrays(keys), *_agg_arrays(aggs)), checksum_alg, (slice_base, slice_len, slice_checksum))

@@ -2311,7 +2311,7 @@ struct RecordSpec {
   KeySpec keys;             // rows: the key columns; fixed-size records: one B2S_KEY_BYTES column
   uint32_t n_keys = 1;      // as the caller passed it; keys holds the columns when it is in [1, 16]
   bool key_arrays = true;   // the caller's key arrays are not NULL
-  bool strings = false;     // B2S_STRING_KEY columns accepted (the *_keys calls)
+  bool composite = false;   // the *_keys calls: string, decimal, 16 / 8-bit and float columns and order flags accepted
   bool aggregate = false;
   uint32_t n_aggs = 0;
   const uint32_t* agg_op = nullptr;
@@ -2340,7 +2340,7 @@ static RecordSpec keys_spec(uint32_t n_keys, const uint32_t* type, const uint32_
                             const int32_t* null_field) {
   RecordSpec r;
   r.is_rows = true;
-  r.strings = true;
+  r.composite = true;
   r.n_keys = n_keys;
   r.key_arrays = type && off && len && null_field;
   if (r.key_arrays && n_keys >= 1 && n_keys <= kMaxKeys) {
@@ -2423,13 +2423,17 @@ static int sort_args(uint32_t codec, uint32_t alg, uint32_t n, const uint64_t* s
     if (spec.n_keys < 1 || spec.n_keys > kMaxKeys) return fail(B2S_E_ARG, "n_keys must be in [1, 16]%s");
     if (!spec.key_arrays) return fail(B2S_E_ARG, "null argument%s");
     for (uint32_t c = 0; c < ks.n; c++) {
-      const uint32_t type = ks.type[c], key_len = ks.len[c];
-      if (type > B2S_KEY_INT64 && !(spec.strings && type == kStringKey)) return fail(B2S_E_ARG, "unknown key_type%s");
+      const uint32_t type = ks.type[c] & kKeyTypeMask, flags = ks.type[c] & ~kKeyTypeMask, key_len = ks.len[c];
+      const bool composite_type = type == kStringKey || (type >= B2S_KEY_INT16 && type <= kDecimalKey);
+      if (type > B2S_KEY_INT64 && !(spec.composite && composite_type)) return fail(B2S_E_ARG, "unknown key_type%s");
+      if (flags && (!spec.composite || (flags & ~(B2S_KEY_DESCENDING | B2S_KEY_NULLS_LAST))))
+        return fail(B2S_E_ARG, "unknown key_type flag%s");
       if (type == B2S_KEY_BYTES && (key_len < 1 || key_len > 16))
         return fail(B2S_E_ARG, "key_len must be in [1, 16]%s");
-      if (type == B2S_KEY_INT32 && key_len != 4) return fail(B2S_E_ARG, "key_len of an INT32 key must be 4%s");
-      if (type == B2S_KEY_INT64 && key_len != 8) return fail(B2S_E_ARG, "key_len of an INT64 key must be 8%s");
-      if (type == kStringKey && key_len != 8) return fail(B2S_E_ARG, "key_len of a string key must be 8%s");
+      // the fixed key_len of every other type: the value's bytes, or a string's or decimal's 8-byte slot
+      static const uint32_t fixed_len[] = {0, 4, 8, 8, 0, 2, 1, 4, 8, 8};
+      if (type != B2S_KEY_BYTES && key_len != fixed_len[type])
+        return fail(B2S_E_ARG, "key_len does not match the key_type (INT8 1, INT16 2, INT32 / FLOAT32 4, else 8)%s");
       if (ks.null_field[c] < -1) return fail(B2S_E_ARG, "null_field must be -1 or a field ordinal%s");
     }
     if (spec.aggregate)
@@ -2711,7 +2715,8 @@ static int decompress_sort_run(Device* D, Slot& S, uint32_t codec, uint32_t alg,
                                           "the row is shorter than key_off + key_len",
                                           "the row does not hold the null-bit word",
                                           "the row is shorter than an aggregate slot",
-                                          "a string key runs past the end of its row"};
+                                          "a string key runs past the end of its row, or a decimal key's size "
+                                          "is not in [1, 16] or its bytes run past the end of its row"};
         snprintf(msg, sizeof msg, "%s %u: bad row record at byte %llu: %s", cached(i) ? "cached source" : "block", i,
                  (unsigned long long)(v[i] & ((1ull << 61) - 1)), why[v[i] >> 61]);
         fail(B2S_E_CORRUPT, "%s", msg);

@@ -222,7 +222,8 @@ const uint32_t* launch_key_radix(const KeySortWs& w, uint64_t n, uint32_t key_by
 // verdict of range 0, 1, ...]; a verdict is ~0 when the range is whole records, else kRowsBad* << 61 | the offset of the
 // range's first bad record.  A record is bad when its prefix is cut by the range end, its size is negative, it runs past
 // the range end, its row is shorter than min_key bytes, shorter than min_null bytes, or shorter than min_agg bytes.
-// kRowsBadString is the key pass's verdict (launch_rows_order): a non-null string key runs past its row.
+// kRowsBadString is the key pass's verdict (launch_rows_order): a non-null string key runs past its row, or a non-null
+// decimal's slot does not name 1..16 bytes inside its row.
 constexpr uint64_t kRowsBadPrefix = 1, kRowsBadNegative = 2, kRowsBadPastEnd = 3, kRowsBadKey = 4, kRowsBadNull = 5,
                    kRowsBadAgg = 6, kRowsBadString = 7;
 size_t rows_frame_ws_bytes(uint64_t arena_bytes, uint32_t n_ranges);
@@ -233,14 +234,22 @@ const uint64_t* rows_frame_ranges(uint8_t* d_fws, uint64_t arena_bytes, uint32_t
 void launch_rows_frame(const uint8_t* arena, uint64_t arena_bytes, const uint64_t* h_off, const uint64_t* h_len,
                        uint32_t n_ranges, uint64_t min_key, uint64_t min_null, uint64_t min_agg, uint8_t* d_fws,
                        cudaStream_t st, uint64_t* launches);
-// The sort key of a row: n columns compared left to right.  Column c: type[c] B2S_KEY_* or B2S_STRING_KEY at row offset
-// off[c], len[c] bytes (a string: its 8-byte slot, (offset << 32) | size), null bit null_field[c] (-1: never null).
+// The sort key of a row: n columns compared left to right.  Column c: type[c] (low 8 bits: B2S_KEY_*, B2S_STRING_KEY or
+// B2S_DECIMAL_KEY; above them the order flags B2S_KEY_DESCENDING / B2S_KEY_NULLS_LAST) at row offset off[c], len[c]
+// bytes (a string or a decimal: its 8-byte slot, (offset << 32) | size), null bit null_field[c] (-1: never null).
 // It is encoded as one byte string compared by memcmp, prefix-free, column after column: a nullable column's null byte
-// (0 null, 1 not), then a fixed-width value big-endian with the sign bit of an int flipped (zero when null), or a
-// non-null string as groups of 8 bytes zero-padded, each followed by a marker: 9 when more bytes follow, else the number
-// of real bytes in the group (0..8); an empty string is one group of zeros with marker 0, a null string nothing.
+// (0 null, 1 not; NULLS_LAST: 1 null, 0 not), then the value (all zero when null): BYTES as they are; an int big-endian
+// with its sign bit flipped; a float with -0.0 made +0.0 and every NaN the canonical NaN, then every bit flipped when
+// negative, else the sign bit, big-endian; a decimal's 1..16 bytes sign-extended to 16, sign bit flipped; a non-null
+// string as groups of 8 bytes zero-padded, each followed by a marker: 9 when more bytes follow, else the number of real
+// bytes in the group (0..8) (an empty string is one group of zeros with marker 0, a null string nothing).  DESCENDING
+// complements every value byte of the column (a string's markers included): the column's code stays prefix-free and
+// its order reverses.
 constexpr uint32_t kMaxKeys = 16;
-constexpr uint32_t kStringKey = B2S_STRING_KEY;
+constexpr uint32_t kStringKey = B2S_STRING_KEY, kDecimalKey = B2S_DECIMAL_KEY;
+constexpr uint32_t kKeyTypeMask = 0xff;
+// the encoded value bytes of a fixed-width column of type ty (low 8 bits) and key_len len: a decimal's 16, else len
+__host__ __device__ inline uint32_t key_value_bytes(uint32_t ty, uint32_t len) { return ty == kDecimalKey ? 16 : len; }
 struct KeySpec {
   uint32_t n = 0;
   uint32_t type[kMaxKeys] = {};
@@ -255,8 +264,9 @@ constexpr uint32_t kKeyPrefixBytes = 20, kKeyChunkBytes = 16;
 inline uint32_t rows_key_encoded_bytes(const KeySpec& ks) {
   uint32_t b = 0;
   for (uint32_t c = 0; c < ks.n; c++) {
-    if (ks.type[c] == kStringKey) return ~0u;
-    b += ks.len[c] + (ks.null_field[c] >= 0 ? 1 : 0);
+    const uint32_t ty = ks.type[c] & kKeyTypeMask;
+    if (ty == kStringKey) return ~0u;
+    b += key_value_bytes(ty, ks.len[c]) + (ks.null_field[c] >= 0 ? 1 : 0);
   }
   return b;
 }
@@ -265,7 +275,14 @@ inline uint32_t rows_key_bytes(const KeySpec& ks) {
   const uint32_t b = rows_key_encoded_bytes(ks);
   return b < kKeyPrefixBytes ? b : kKeyPrefixBytes;
 }
-inline bool rows_key_refines(const KeySpec& ks) { return rows_key_encoded_bytes(ks) > kKeyPrefixBytes; }
+// The key takes the refinement path: it is longer than the first pass, or it has a decimal column, whose slots are
+// checked there (the first round's readback brings the verdicts; when the key fits the first pass no record is tied).
+inline bool rows_key_refines(const KeySpec& ks) {
+  if (rows_key_encoded_bytes(ks) > kKeyPrefixBytes) return true;
+  for (uint32_t c = 0; c < ks.n; c++)
+    if ((ks.type[c] & kKeyTypeMask) == kDecimalKey) return true;
+  return false;
+}
 size_t rows_sort_ws_bytes(uint64_t n, uint32_t key_bytes);
 // the framed records (n = the read-back count) as dense offsets and lengths in arena order, into the sort workspace
 void launch_rows_emit(const uint8_t* arena, uint64_t arena_bytes, uint32_t n_ranges, uint8_t* d_fws, uint64_t n,

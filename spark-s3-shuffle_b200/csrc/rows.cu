@@ -10,7 +10,8 @@
 //   emit   : the bitmap compacted into dense record offsets (u64) and lengths (u32, prefix included), arena order
 //   keys   : one thread per record: the first bytes (at most kKeyPrefixBytes) of the encoded key (kernels.h, KeySpec)
 //            as big-endian u32 words (one column: int32 / int64 byte-swapped, sign bit flipped; a nullable key gets a
-//            leading byte 0 = null, 1 = non-null, and a null record's key bytes are 0)
+//            leading byte 0 = null, 1 = non-null, and a null record's key bytes are 0; the composite calls' types and
+//            order flags are further column encodings of the same function, encode_key)
 //   radix  : the fixed-size sort's radix passes (launch_key_radix): the sorted record indices
 //   refine : only for keys longer than the first pass: rounds over the records still tied (runs of equal first bytes
 //            whose keys go on): compacted in order, their next kKeyChunkBytes bytes extracted behind their run number,
@@ -226,23 +227,71 @@ struct KeyWindow {
   }
 };
 
+__device__ __forceinline__ uint64_t bswap64(uint64_t x) {
+  return ((uint64_t)__byte_perm((uint32_t)x, 0, 0x0123) << 32) | __byte_perm((uint32_t)(x >> 32), 0, 0x0123);
+}
+
+// A fixed-width number's len (1..8) bytes v (little-endian; bytes past len unspecified) as an unsigned number of len
+// bytes whose order is the column's: an int with its sign bit flipped; a float (Spark SQL's order) with -0.0 made +0.0
+// and every NaN the canonical quiet NaN, then every bit flipped when negative, else the sign bit.
+__device__ __forceinline__ uint64_t ordered_bits(uint32_t ty, uint32_t len, uint64_t v) {
+  const uint64_t sign = 1ull << (8 * len - 1), mag = v & (sign - 1);
+  if (ty != B2S_KEY_FLOAT32 && ty != B2S_KEY_FLOAT64) return v ^ sign;
+  const bool f32 = ty == B2S_KEY_FLOAT32;
+  if (mag == 0) return sign;                                                   // +-0.0
+  if (mag > (f32 ? 0x7f800000ull : 0x7ff0000000000000ull))                     // NaN
+    return (f32 ? 0x7fc00000ull : 0x7ff8000000000000ull) | sign;
+  return (v & sign) ? ~v & (sign | (sign - 1)) : v ^ sign;
+}
+
+// A decimal's slot (offset << 32) | size -> (hi, lo): its size bytes of the row, big-endian two's complement,
+// sign-extended to 128 bits with the sign bit flipped.  *bad: the size is not 1..16 or the bytes run past the row; they
+// are then clamped to 16 and to the row, so no load leaves it.
+__device__ __forceinline__ void decimal_bits(const uint8_t* row, uint32_t row_size, uint64_t slot, uint64_t& hi,
+                                             uint64_t& lo, bool* bad) {
+  uint32_t so = (uint32_t)(slot >> 32), sz = (uint32_t)slot;
+  if (sz - 1 >= 16u || (uint64_t)so + sz > row_size) {
+    *bad = true;
+    so = min(so, row_size);
+    sz = min(min(sz, 16u), row_size - so);
+  }
+  hi = lo = 0;
+  if (sz) {
+    uint64_t a, b;
+    ld_span16<true>(row + so, (int)sz, a, b);
+    hi = bswap64(a);  // the 16 bytes from the value's first as a big-endian number: the value is its top sz bytes
+    lo = bswap64(b);
+    const uint32_t s = 8 * (16 - sz);  // an arithmetic shift right by s sign-extends it
+    if (s >= 64) {
+      lo = (uint64_t)((int64_t)hi >> (s - 64));
+      hi = (uint64_t)((int64_t)hi >> 63);
+    } else if (s) {
+      lo = (lo >> s) | (hi << (64 - s));
+      hi = (uint64_t)((int64_t)hi >> s);
+    }
+  }
+  hi ^= 1ull << 63;
+}
+
 // The window kw of the encoded key of a row of row_size bytes.  whole: every column is walked and the return value is
-// the key's encoded length (else the walk stops at the window's end).  *bad: a non-null string slot runs past the row;
-// its bytes are then clamped to the row, so no load leaves it.
+// the key's encoded length (else the walk stops at the window's end); every non-null decimal slot is then checked.
+// *bad: a non-null string slot runs past the row, or a decimal slot is bad (decimal_bits); the bytes read are then
+// clamped to the row, so no load leaves it.
 __device__ __forceinline__ uint32_t encode_key(const uint8_t* row, uint32_t row_size, const KeySpec& ks, KeyWindow& kw,
                                                bool whole, bool* bad) {
   const uint32_t wend = kw.d + kw.nb;
   uint32_t p = 0;
   for (uint32_t c = 0; c < ks.n; c++) {
     if (!whole && p >= wend) break;
-    const uint32_t ty = ks.type[c], off = ks.off[c], len = ks.len[c];
+    const uint32_t ty = ks.type[c] & kKeyTypeMask, off = ks.off[c], len = ks.len[c];
+    const uint32_t flip = ks.type[c] & B2S_KEY_DESCENDING ? 0xff : 0;  // DESC: every value byte complemented
     const int32_t nf = ks.null_field[c];
     bool is_null = false;
     if (nf >= 0) {
       uint64_t nw, unused;
       ld_span16<true>(row + 8 * (uint32_t)(nf >> 6), 8, nw, unused);
       is_null = (nw >> (nf & 63)) & 1;
-      kw.put(p++, is_null ? 0 : 1);
+      kw.put(p++, is_null == ((ks.type[c] & B2S_KEY_NULLS_LAST) != 0) ? 1 : 0);
     }
     if (ty == kStringKey) {
       if (is_null) continue;
@@ -262,26 +311,25 @@ __device__ __forceinline__ uint32_t encode_key(const uint8_t* row, uint32_t row_
           ld_span16<true>(row + so + 8 * g, (int)real, v, unused2);
           if (real < 8) v &= (1ull << (8 * real)) - 1;
         }
-        for (uint32_t b = 0; b < 8; b++) kw.put(base + b, (uint32_t)(v >> (8 * b)) & 0xff);
-        kw.put(base + 8, g + 1 < groups ? 9 : real);
+        for (uint32_t b = 0; b < 8; b++) kw.put(base + b, ((uint32_t)(v >> (8 * b)) & 0xff) ^ flip);
+        kw.put(base + 8, (g + 1 < groups ? 9 : real) ^ flip);
       }
       p += 9 * groups;
     } else {
-      if (!is_null && p < wend && p + len > kw.d) {  // a null's bytes stay zero
+      const uint32_t w = key_value_bytes(ty, len);
+      const bool in_window = p < wend && p + w > kw.d;
+      if (!is_null && (in_window || (whole && ty == kDecimalKey))) {  // a null's bytes stay zero
         uint64_t lo, hi;
         ld_span16<true>(row + off, (int)len, lo, hi);
-        for (uint32_t b = 0; b < len; b++) {
-          uint32_t v;
-          if (ty == B2S_KEY_BYTES) {
-            v = (uint32_t)(b < 8 ? lo >> (8 * b) : hi >> (8 * (b - 8))) & 0xff;
-          } else {  // little-endian two's complement: most significant byte first, sign bit flipped
-            v = (uint32_t)(lo >> (8 * (len - 1 - b))) & 0xff;
-            if (b == 0) v ^= 0x80;
-          }
-          kw.put(p + b, v);
+        if (ty == kDecimalKey) decimal_bits(row, row_size, /* the slot */ lo, hi, lo, bad);
+        else if (ty != B2S_KEY_BYTES) lo = ordered_bits(ty, len, lo);
+        // BYTES in memory order; a number (lo, or hi:lo for a decimal) most significant byte first
+        for (uint32_t b = 0; in_window && b < w; b++) {
+          const uint32_t s = ty == B2S_KEY_BYTES ? b : w - 1 - b;
+          kw.put(p + b, ((uint32_t)(s < 8 ? lo >> (8 * s) : hi >> (8 * (s - 8))) & 0xff) ^ flip);
         }
       }
-      p += len;
+      p += w;
     }
   }
   return p;
@@ -289,8 +337,9 @@ __device__ __forceinline__ uint32_t encode_key(const uint8_t* row, uint32_t row_
 
 // The first pass: words[k * n + i] = word k of record i's encoded key, k < ceil(key_bytes / 4).  klen (keys that
 // refine): klen[i] = the encoded length, and a record whose string runs past its row lowers its range's verdict
-// (verdict[r], ranges: the ranges' arena offsets, ascending) to its offset in the range.
-__global__ void __launch_bounds__(kRowThreads) rows_keys_kernel(
+// (verdict[r], ranges: the ranges' arena offsets, ascending) to its offset in the range.  Eight CTAs per SM: the key
+// pass of every row sort keeps full occupancy (32 registers, no spills with the wider encodings' branches).
+__global__ void __launch_bounds__(kRowThreads, 8) rows_keys_kernel(
     const uint8_t* __restrict__ arena, const uint64_t* __restrict__ rec_off, const uint32_t* __restrict__ rec_len,
     uint64_t n, const __grid_constant__ KeySpec ks, uint32_t key_bytes, uint32_t* __restrict__ words,
     uint32_t* __restrict__ klen, const uint64_t* __restrict__ ranges, uint32_t n_ranges, uint64_t* __restrict__ verdict) {

@@ -362,12 +362,14 @@ class S3ShuffleReader:
                             nullField, *_agg_arrays(aggs), groups=True)
 
     def readSortedRowsKeys(self, keys):
-        """readSortedRows by a composite key: keys = [(keyType or STRING_KEY, keyOffset, keyLength, nullField), ...],
-        compared left to right.  -> (bytes, number of records)"""
+        """readSortedRows by a composite key: keys = [(keyType, keyOffset, keyLength, nullField), ...], compared left
+        to right.  keyType: KEY_* or STRING_KEY / DECIMAL_KEY, OR-ed with KEY_DESCENDING and / or KEY_NULLS_LAST
+        (capi.decompress_sort_rows_keys_packed).  -> (bytes, number of records)"""
         return _read_sorted(self._h, load().b2sh_reader_read_sorted_rows_keys, *_key_arrays(keys))
 
     def readAggregatedRowsKeys(self, keys, aggs=()):
-        """readAggregatedRows grouped by a composite key (keys as in readSortedRowsKeys).
+        """readAggregatedRows grouped by a composite key (keys as in readSortedRowsKeys, flags included: groups come
+        out in that order; floats group by Spark SQL's equality, 0.0 with -0.0 and NaN with NaN).
         -> (bytes, number of input records, number of groups)"""
         return _read_sorted(self._h, load().b2sh_reader_read_aggregated_rows_keys, *_key_arrays(keys),
                             *_agg_arrays(aggs), groups=True)

@@ -851,8 +851,9 @@ class S3ShuffleReader {
       return;
     }
   }
-  // The key columns of readRows: column c is type[c] (B2S_KEY_* or B2S_STRING_KEY) at row offset off[c], len[c] bytes,
-  // null bit nullField[c].  composite: the *_rows_keys_* calls (up to 16 columns, strings included), else the one-key
+  // The key columns of readRows: column c is type[c] (B2S_KEY_*, B2S_STRING_KEY or B2S_DECIMAL_KEY, with the order
+  // flags B2S_KEY_DESCENDING / B2S_KEY_NULLS_LAST) at row offset off[c], len[c] bytes, null bit nullField[c].
+  // composite: the *_rows_keys_* calls (up to 16 columns, strings, decimals and flags included), else the one-key
   // ones.
   struct RowKeys {
     uint32_t n;

@@ -10,6 +10,9 @@ one block: --codec, default snappy, + CRC32C), the reducer a hash of the key:
          ints, then a count and a sum buffer (longs).  --groups distinct keys, so a key has about rows / groups rows.
   join : the build side of a sort-merge join on (string id, int): a 16-40 byte id with a shared 12-byte prefix, an int,
          and two longs (the second used for the two-INT64 comparison below).
+  window: q67's window input, rank() over (partition by i_category order by sumsales desc): i_category (one of ten
+         names, or null) and sumsales, a nullable decimal(28,2) (out of line, 1..16 bytes), plus a long.  The exchange
+         hashes i_category, so only the reducers holding a category have rows, and only they are timed.
 Strings sit in a 56-byte area per column after the fixed fields (rows are fixed-length, slots hold the real sizes).
 Per reducer, after --warmup untimed calls, CUDA-event times (b2s_last_timing.kernel_ms: the whole call on the device):
   decode   : decompress_dev alone (verify + decode)
@@ -17,6 +20,9 @@ Per reducer, after --warmup untimed calls, CUDA-event times (b2s_last_timing.ker
   first    : the same rows sorted by one INT32 column (resolved by the first pass: no refinement)
   agg      : q67 only, the composite-key aggregation; its aggregation step is dominant_ms
   i64x2    : join only, the two-INT64 composite beside the single-INT64 row sort on the same rows
+  window   : window only, the sort by (i_category ASC NULLS FIRST, sumsales DESC NULLS LAST), as the WindowExec's
+             SortExec asks; asc: the same columns ASC NULLS FIRST; i64: a one-INT64 row sort of the same rows.  Every
+             output is checked against a Python sort of the reducer's rows.
 Refinement rounds and the records tied in each are counted by a CPU model of the key encoding (20 bytes first, then 16
 per round), which also validates every output byte against a Python sort (and the aggregation's groups and sums).
 The card's name and power limit are read in the same run.
@@ -26,6 +32,7 @@ The card's name and power limit are read in the same run.
 Prints one JSON document.
 """
 import argparse
+import functools
 import json
 import os
 import statistics
@@ -37,7 +44,10 @@ import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-STRING, KEY_INT32, KEY_INT64 = 3, 1, 2
+STRING, KEY_INT32, KEY_INT64, DECIMAL = 3, 1, 2, 9
+DESC, NULLS_LAST = 1 << 8, 1 << 9
+CATEGORIES = [b"Books", b"Children", b"Electronics", b"Home", b"Jewelry", b"Men", b"Music", b"Shoes", b"Sports",
+              b"Women"]
 SLOT = 56  # bytes of string area per string column
 
 
@@ -114,6 +124,34 @@ def make_rows(rng, shape, n, groups):
     return rows, keys, aggs, g
 
 
+def window_rows(rng, n):
+    """-> (rows uint8 [n, 64], category id per row (len(CATEGORIES): null), sumsales per row (None: null))
+    row: null word (bit 1 i_category, bit 2 sumsales), i_category slot, sumsales slot, a long, then 16 bytes of string
+    and 16 of decimal"""
+    cat = rng.integers(0, len(CATEGORIES) + 1, n)
+    cents = rng.integers(0, 10**9, n) * rng.choice(np.array([1, 1, 1, 10**9]), n)  # a few wider than 8 bytes
+    null_sales = rng.random(n) < 0.01
+    rows = np.zeros((n, 64), np.uint8)
+    rows[:, 24:32] = rng.integers(-2**62, 2**62, n).view(np.uint8).reshape(n, 8)
+    word = np.where(cat == len(CATEGORIES), 2, 0) | np.where(null_sales, 4, 0)
+    rows[:, 0:8] = word.astype(np.uint64).view(np.uint8).reshape(n, 8)
+    sales = []
+    for i in range(n):
+        if cat[i] < len(CATEGORIES):
+            b = CATEGORIES[cat[i]]
+            rows[i, 32:32 + len(b)] = np.frombuffer(b, np.uint8)
+            rows[i, 8:16] = np.frombuffer(((32 << 32) | len(b)).to_bytes(8, "little"), np.uint8)
+        if null_sales[i]:
+            sales.append(None)
+            continue
+        v = int(cents[i]) * (1 if i % 7 else -1)
+        b = v.to_bytes((v if v >= 0 else ~v).bit_length() // 8 + 1, "big", signed=True)  # BigInteger.toByteArray
+        rows[i, 48:48 + len(b)] = np.frombuffer(b, np.uint8)
+        rows[i, 16:24] = np.frombuffer(((48 << 32) | len(b)).to_bytes(8, "little"), np.uint8)
+        sales.append(v)
+    return rows, cat, sales
+
+
 def col_value(row, c):
     kt, ko, kl, _ = c
     if kt == STRING:
@@ -157,6 +195,76 @@ def rounds(enc_sorted):
         d += 16
 
 
+def stage(c, codec, alg, plain):
+    """one reducer's blocks (plain: one stream per map) compressed, checksummed and put on the device -> (the _dev
+    calls' leading arguments, their slice keywords, decoded bytes, d_src, d_dst)"""
+    lens = np.array([len(b) for b in plain], np.uint64)
+    offs = np.concatenate([[0], np.cumsum(lens)[:-1]]).astype(np.uint64)
+    src = np.frombuffer(b"".join(plain), np.uint8)
+    if codec:
+        dst = np.zeros(sum(c.compress_bound(codec, 0, int(x)) for x in lens) + 64, np.uint8)
+        cr = c.compress_packed(codec, src, offs, lens, dst, 0, 0)
+        arena, off, ln = dst[:max(cr["total"], 1)], cr["dst_off"], cr["dst_len"]
+    else:
+        arena, off, ln = src, offs, lens
+    ck = c.checksum_packed(alg, arena, off, ln)
+    sb, sl = np.arange(len(plain) + 1, dtype=np.uint32), np.array(ln, np.uint64)
+    total = int(lens.sum())
+    d_src, d_dst = c.dev_alloc(max(arena.size, 1)), c.dev_alloc(max(total, 1))
+    c.dev_memcpy(d_src, arena.ctypes.data, arena.size, 1)
+    sk = dict(checksum_alg=alg, slice_base=sb, slice_len=sl, slice_checksum=ck)
+    return (codec, d_src, off, ln, d_dst, total), sk, total, d_src, d_dst
+
+
+def timed_call(c, warmup, f, *a, **k):
+    for _ in range(warmup):
+        f(*a, **k)
+    res = f(*a, **k)
+    return res, c.last_timing()
+
+
+def window(c, args, rng, codec, alg):
+    """the window shape (module docstring): per non-empty reducer the flagged sort, the ASC one and one INT64"""
+    rows, cat, sales = window_rows(rng, args.rows)
+    L = rows.shape[1]
+    red = (cat * 2654435761 % 2**32) % args.partitions
+    mp = rng.integers(0, args.maps, args.rows)
+    order = np.lexsort((mp, red))
+    prefix = L.to_bytes(4, "big")
+    sorts = {"window": [(STRING, 8, 8, 1), (DECIMAL | DESC | NULLS_LAST, 16, 8, 2)],
+             "asc": [(STRING, 8, 8, 1), (DECIMAL, 16, 8, 2)]}
+    stats, ok, sizes = {k: [] for k in ("decode", "window", "asc", "i64")}, True, []
+    for r in sorted(set(red.tolist())):
+        idx = order[red[order] == r]
+        maps_of = mp[idx]
+        plain = [b"".join(prefix + rows[i].tobytes() for i in idx[maps_of == m]) for m in range(args.maps)]
+        ins = [i for m in range(args.maps) for i in idx[maps_of == m]]  # block order
+        a, sk, total, d_src, d_dst = stage(c, codec, alg, plain)
+        _, t = timed_call(c, args.warmup, c.decompress_dev, *a, **sk)
+        stats["decode"].append(t["kernel_ms"])
+        got = np.zeros(max(total, 1), np.uint8)
+        models = {  # Python sort keys: category ASC NULLS FIRST, then sumsales DESC NULLS LAST / ASC NULLS FIRST
+            "window": lambda i: (cat[i] != len(CATEGORIES), CATEGORIES[cat[i]] if cat[i] < len(CATEGORIES) else b"",
+                                 sales[i] is None, -(sales[i] or 0)),
+            "asc": lambda i: (cat[i] != len(CATEGORIES), CATEGORIES[cat[i]] if cat[i] < len(CATEGORIES) else b"",
+                              sales[i] is not None, sales[i] or 0),
+            "i64": lambda i: int(rows[i, 24:32].view(np.int64)[0])}
+        for name, model in models.items():
+            if name == "i64":
+                res, t = timed_call(c, args.warmup, c.decompress_sort_rows_dev, *a, KEY_INT64, 24, 8, -1, **sk)
+            else:
+                res, t = timed_call(c, args.warmup, c.decompress_sort_rows_keys_dev, *a, sorts[name], **sk)
+            stats[name].append(t["kernel_ms"])
+            c.dev_memcpy(got.ctypes.data, d_dst, total, 2)
+            want = b"".join(prefix + rows[i].tobytes() for i in sorted(ins, key=model))  # stable
+            ok &= got[:total].tobytes() == want and res["n_records"] == len(ins)
+        sizes.append(len(ins))
+        c.dev_free(d_src)
+        c.dev_free(d_dst)
+    return {"reducers": len(sizes), "rows_per_reducer": spread(sizes), "validated": bool(ok),
+            "ms_per_reducer": {k: spread(v) for k, v in stats.items()}}
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--rows", type=int, default=1_000_000)
@@ -167,6 +275,7 @@ def main():
     ap.add_argument("--warmup", type=int, default=2)
     ap.add_argument("--seed", type=int, default=42)
     ap.add_argument("--reducers", type=int, default=0, help="reducers timed (0: all)")
+    ap.add_argument("--shapes", default="q67,join,window")
     args = ap.parse_args()
     import spark_s3_shuffle_b200 as pkg
     c = pkg.capi
@@ -175,7 +284,8 @@ def main():
     alg = c.CHECKSUM_CRC32C
     out = {"card": card(), "rows": args.rows, "maps": args.maps, "partitions": args.partitions, "codec": args.codec}
     rng = np.random.default_rng(args.seed)
-    for shape in ("q67", "join"):
+    timed = functools.partial(timed_call, c, args.warmup)
+    for shape in [x for x in args.shapes.split(",") if x in ("q67", "join")]:
         rows, keys, aggs, g = make_rows(rng, shape, args.rows, args.groups)
         L = rows.shape[1]
         red = (g * 2654435761 % 2**32) % args.partitions
@@ -194,29 +304,8 @@ def main():
                 sel = rows[idx[maps_of == m]]
                 recs = np.concatenate([np.tile(np.frombuffer(prefix, np.uint8), (sel.shape[0], 1)), sel], 1)
                 plain.append(recs.tobytes())
-            lens = np.array([len(b) for b in plain], np.uint64)
-            offs = np.concatenate([[0], np.cumsum(lens)[:-1]]).astype(np.uint64)
-            src = np.frombuffer(b"".join(plain), np.uint8)
-            if codec:
-                dst = np.zeros(sum(c.compress_bound(codec, 0, int(x)) for x in lens) + 64, np.uint8)
-                cr = c.compress_packed(codec, src, offs, lens, dst, 0, 0)
-                arena, off, ln = dst[:max(cr["total"], 1)], cr["dst_off"], cr["dst_len"]
-            else:
-                arena, off, ln = src, offs, lens
-            ck = c.checksum_packed(alg, arena, off, ln)
-            sb, sl = np.arange(len(plain) + 1, dtype=np.uint32), np.array(ln, np.uint64)
-            total = int(lens.sum())
-            d_src, d_dst = c.dev_alloc(max(arena.size, 1)), c.dev_alloc(max(total, 1))
-            c.dev_memcpy(d_src, arena.ctypes.data, arena.size, 1)
-
-            def timed(f, *a, **k):
-                for _ in range(args.warmup):
-                    f(*a, **k)
-                res = f(*a, **k)
-                return res, c.last_timing()
-            a = (codec, d_src, off, ln, d_dst, total)
-            sk = dict(checksum_alg=alg, slice_base=sb, slice_len=sl, slice_checksum=ck)
-            _, t = timed(c.decompress_dev, codec, d_src, off, ln, d_dst, total, **sk)
+            a, sk, total, d_src, d_dst = stage(c, codec, alg, plain)
+            _, t = timed(c.decompress_dev, *a, **sk)
             stats["decode"].append(t["kernel_ms"])
             _, t = timed(c.decompress_sort_rows_dev, *a, KEY_INT32, ik[1], 4, -1, **sk)
             stats["first"].append(t["kernel_ms"])
@@ -259,6 +348,8 @@ def main():
             "refinement_rounds": spread(n_rounds),
             "tied_records_per_round_median_reducer": round_counts[sorted(range(R), key=lambda i: n_rounds[i])[R // 2]],
         }
+    if "window" in args.shapes.split(","):
+        out["window"] = window(c, args, rng, codec, alg)
     c.shutdown()
     print(json.dumps(out, indent=1))
 
