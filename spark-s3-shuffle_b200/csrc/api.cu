@@ -2202,15 +2202,23 @@ static int decompress_host(uint32_t codec, uint32_t alg, uint32_t n, const uint8
   };
 
   // software pipeline over the chunks: enqueue chunk c's upload + phase A first (never blocks on younger work), then
-  // phase B of chunk c-1 (waits for its sizes), then the download of chunk c-2 (waits for its decode)
-  // (lag chunks between the stages, so that lag uploads / decodes are queued on the device while the host waits for one
-  // chunk's sizes — the write lane keeps g_nslot chunks in flight and would otherwise own the copy queues; needs
-  // 2 * lag + 1 <= g_nslot slots)
+  // phase B of chunk c-lag (waits for its sizes), then the download of chunk c-2*lag (waits for its decode).  lag
+  // chunks between the stages keep lag uploads / decodes queued on the device while the host waits for one chunk's
+  // sizes (the write lane keeps g_nslot chunks in flight and would otherwise own the copy queues).
+  // Invariant: stage_a(c) restages slot c % g_nslot (its source arena and the pinned block that holds the statuses,
+  // lengths and offsets stage_c reads), so chunk c - g_nslot, the slot's previous chunk, has been through stage_c
+  // before it.  With 2 * lag + 1 <= g_nslot (every slot count from 3) the loop order already guarantees that; with 2
+  // slots (lag 1) the download of chunk c-2 moves in front of stage_a(c), and one chunk is decoded while the next is
+  // sized.
   const size_t lag = (size_t)std::max(1, std::min(g_read_lag, (g_nslot - 1) / 2));
+  size_t done = 0;  // chunks through stage_c, in order
   for (size_t c = 0; c < nchunks + 2 * lag; c++) {
+    for (; done + g_nslot <= c && done < nchunks; done++)
+      if ((rc = stage_c(done))) return rc;
     if (c < nchunks && (rc = stage_a(c))) return rc;
     if (c >= lag && c - lag < nchunks && (rc = stage_b(c - lag))) return rc;
-    if (c >= 2 * lag && c - 2 * lag < nchunks && (rc = stage_c(c - 2 * lag))) return rc;
+    for (; done + 2 * lag <= c && done < nchunks; done++)
+      if ((rc = stage_c(done))) return rc;
   }
   for (int k = 0; k < g_nslot; k++) {
     CU(cudaStreamSynchronize(Ln.slot[k].st));

@@ -282,7 +282,8 @@ def test_decompress_dst_too_small(capi, oracle):
 
 # ------------------------------------------------------------------ many blocks, multiple chunks, device API
 def test_many_small_blocks_config3_shape(capi, oracle):
-    """Config-3 shape: thousands of ~64 KiB shuffle blocks in one call (exercises batching + chunk pipeline)."""
+    """Config-3 shape: thousands of ~64 KiB shuffle blocks in one call (~197 MB: many streams in one host chunk; the
+    pipelines over several chunks and slots are tested in test_gpu_chunk_pipelines.py)."""
     n, per = 3000, 65520
     raw = oracle.gen_terasort(0, n * per // 104 + 1).tobytes()
     blocks = [raw[i * per:(i + 1) * per] for i in range(n)]
