@@ -13,83 +13,24 @@
 //        into the slice accumulator.  init/xorout are applied algebraically at the end.
 //   Adler32: two dp4a per 32-bit word, 64-bit weighted sums, same work-item combine.
 // Algorithmic traffic: 1 byte read per input byte, nothing written but 8 bytes per slice.
+#include "crc_gf.h"
 #include "kernels.h"
 
 namespace b2s {
 
 constexpr int kCkThreads = 256;  // 8 warps per CTA
-constexpr uint32_t kOne = 0x80000000u;  // x^0 in the reflected representation
 
-// ---------------- GF(2) helpers (host + device) ----------------
-__host__ __device__ __forceinline__ uint32_t gf_mul(uint32_t a, uint32_t b, uint32_t poly) {
-  uint32_t p = 0;
-#pragma unroll 8
-  for (int i = 0; i < 32; i++) {
-    p ^= (uint32_t)((int32_t)a >> 31) & b;
-    a <<= 1;
-    b = (b >> 1) ^ ((0u - (b & 1u)) & poly);
-  }
-  return p;
-}
-// x^(8*e) mod P for |e| bytes; tab = x^(+-2^k)
-__host__ __device__ inline uint32_t gf_xpow8(uint64_t e, const uint32_t* tab, uint32_t poly) {
-  uint32_t p = kOne;
-  unsigned k = 3;
-  while (e) {
-    if (e & 1) p = gf_mul(tab[k & 31], p, poly);
-    e >>= 1;
-    k++;
-  }
-  return p;
-}
-
-// ---------------- table construction (host, once per device) ----------------
-static void build_tables(uint32_t poly, uint32_t* rows /*16*256*/, uint32_t* misc /*97*/) {
-  uint32_t t0[256];
-  for (uint32_t i = 0; i < 256; i++) {
-    uint32_t c = i;
-    for (int k = 0; k < 8; k++) c = (c & 1) ? (c >> 1) ^ poly : (c >> 1);
-    t0[i] = c;
-  }
-  // Z_j[b] = register after byte b followed by j zero bytes
-  uint32_t z[256];
-  for (int b = 0; b < 256; b++) z[b] = t0[b];
-  for (int j = 0; j <= 511; j++) {
-    if (j >= 496) {
-      int k = 511 - j;  // R[k] = Z_{511-k}
-      for (int b = 0; b < 256; b++) rows[k * 256 + b] = z[b];
-    }
-    for (int b = 0; b < 256; b++) z[b] = (z[b] >> 8) ^ t0[z[b] & 0xff];
-  }
-  uint32_t* x2n = misc;
-  uint32_t* xinv2n = misc + 32;
-  uint32_t* lane_const = misc + 64;
-  uint32_t p = 1u << 30;  // x^1
-  x2n[0] = p;
-  for (int k = 1; k < 32; k++) {
-    p = gf_mul(p, p, poly);
-    x2n[k] = p;
-  }
-  p = (((kOne ^ poly) << 1) | 1u);  // x^-1
-  xinv2n[0] = p;
-  for (int k = 1; k < 32; k++) {
-    p = gf_mul(p, p, poly);
-    xinv2n[k] = p;
-  }
-  for (int l = 0; l < 32; l++) lane_const[l] = gf_xpow8((uint64_t)16 * (31 - l), x2n, poly);
-  misc[96] = poly;
-}
-
+// ---------------- table construction (host, once per device; crc_gf.h) ----------------
 int checksum_tables_create(ChecksumTables* t) {
   static const uint32_t polys[2] = {0xEDB88320u, 0x82F63B78u};
   for (int w = 0; w < 2; w++) {
     uint32_t* rows = new uint32_t[16 * 256];
-    uint32_t misc[97];
-    build_tables(polys[w], rows, misc);
+    uint32_t misc[kMiscWords];
+    build_crc_tables(polys[w], rows, misc);
     if (cudaMalloc(&t->d_crc_rows[w], 16 * 256 * 4) != cudaSuccess) return -1;
-    if (cudaMalloc(&t->d_crc_misc[w], 97 * 4) != cudaSuccess) return -1;
+    if (cudaMalloc(&t->d_crc_misc[w], kMiscWords * 4) != cudaSuccess) return -1;
     cudaMemcpy(t->d_crc_rows[w], rows, 16 * 256 * 4, cudaMemcpyHostToDevice);
-    cudaMemcpy(t->d_crc_misc[w], misc, 97 * 4, cudaMemcpyHostToDevice);
+    cudaMemcpy(t->d_crc_misc[w], misc, kMiscWords * 4, cudaMemcpyHostToDevice);
     delete[] rows;
   }
   return 0;
@@ -185,11 +126,11 @@ __global__ void __launch_bounds__(kCkThreads) crc_items_kernel(const uint8_t* __
                                                                const uint32_t* __restrict__ g_misc,
                                                                uint32_t* __restrict__ acc) {
   __shared__ uint32_t R[16][256];
-  __shared__ uint32_t misc[97];
+  __shared__ uint32_t misc[kMiscWords];
   for (int i = threadIdx.x; i < 16 * 256; i += kCkThreads) (&R[0][0])[i] = g_rows[i];
-  for (int i = threadIdx.x; i < 97; i += kCkThreads) misc[i] = g_misc[i];
+  for (int i = threadIdx.x; i < kMiscWords; i += kCkThreads) misc[i] = g_misc[i];
   __syncthreads();
-  const uint32_t poly = misc[96];
+  const uint32_t poly = misc[kMiscPoly];
   const int lane = threadIdx.x & 31;
   const uint64_t total = work_base[n];
   const uint64_t wstride = (uint64_t)gridDim.x * (kCkThreads / 32);
@@ -229,15 +170,15 @@ __global__ void __launch_bounds__(kCkThreads) crc_items_kernel(const uint8_t* __
       s = crc_row(R, s, w);
     }
     // fold lanes: lane l is over-advanced by 16*l bytes relative to lane 31's frame -> bring all to "row end + 496"
-    uint32_t v = gf_mul(s, misc[64 + lane], poly);
+    uint32_t v = gf_mul(s, misc[kMiscLane + lane], poly);
 #pragma unroll
     for (int d = 16; d; d >>= 1) v ^= __shfl_xor_sync(0xffffffffu, v, d);
     // shift to the item's place in the slice: x^(8*(after - zpad - 496)), built lane-parallel from bit factors
     int64_t e = (int64_t)after - (int64_t)zpad - 496;
-    const uint32_t* tab = e >= 0 ? misc : misc + 32;
+    const uint32_t* tab = misc + (e >= 0 ? kMiscXPow : kMiscXInv);
     uint64_t ue = (uint64_t)(e >= 0 ? e : -e);
-    uint32_t f = ((ue >> lane) & 1) ? tab[(lane + 3) & 31] : kOne;
-    if ((ue >> (lane + 32)) & 1) f = gf_mul(f, tab[(lane + 35) & 31], poly);
+    uint32_t f = ((ue >> lane) & 1) ? tab[lane + 3] : kGfOne;
+    if ((ue >> (lane + 32)) & 1) f = gf_mul(f, tab[lane + 35], poly);
 #pragma unroll
     for (int d = 16; d; d >>= 1) {
       uint32_t o = __shfl_xor_sync(0xffffffffu, f, d);
@@ -251,9 +192,9 @@ __global__ void crc_finalize_kernel(const uint32_t* __restrict__ acc, const uint
                                     const uint32_t* __restrict__ g_misc, uint64_t* __restrict__ out) {
   uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  const uint32_t poly = g_misc[96];
+  const uint32_t poly = g_misc[kMiscPoly];
   // crc(M) = raw0(M) ^ 0xFFFFFFFF * x^(8|M|) ^ 0xFFFFFFFF
-  uint32_t init = gf_mul(gf_xpow8(len[i], g_misc, poly), 0xffffffffu, poly);
+  uint32_t init = gf_mul(gf_xpow8(len[i], g_misc + kMiscXPow, poly), 0xffffffffu, poly);
   out[i] = (uint64_t)(acc[i] ^ init ^ 0xffffffffu);
 }
 

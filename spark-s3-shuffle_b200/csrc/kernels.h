@@ -21,7 +21,7 @@ void launch_exclusive_scan_u64(uint64_t* d_v, size_t n, uint64_t* d_total, uint6
 // ---------------- checksum.cu (K1) ----------------
 struct ChecksumTables {
   uint32_t* d_crc_rows[2];  // [crc32, crc32c] : 16 x 256 row-advance tables (Z_496..Z_511)
-  uint32_t* d_crc_misc[2];  // x2n[32] | xinv2n[32] | lane_const[32] | poly
+  uint32_t* d_crc_misc[2];  // x2n[67] | xinv2n[67] | lane_const[32] | poly (crc_gf.h: kMisc*)
 };
 int checksum_tables_create(ChecksumTables* t);  // on the current device
 void checksum_tables_destroy(ChecksumTables* t);
