@@ -26,6 +26,7 @@
 #include <sys/syscall.h>
 #include <unistd.h>
 
+#include "chunk_schedule.h"
 #include "kernels.h"
 
 using namespace b2s;
@@ -421,6 +422,27 @@ int hlog_for_level(uint32_t codec, int32_t level) {
   return level == 1 ? 11 : level == 2 ? 12 : 13;
 }
 
+// Runs codec blocks [0, nb) in groups of `group`, group k in workspace par = k & 1 (ws_bytes at ws0): first(b0, m, ws,
+// par, e0, e1) enqueues its first pass on S.st2, second(...) its second pass on S.st, beside the first pass of group
+// k+1.  e0 / e1 (S.dom_pair) time whichever pass the caller counts as dominant.  The caller has forked S.st2 from S.st.
+template <class First, class Second>
+int run_block_groups(Slot& S, uint32_t nb, uint32_t group, uint8_t* ws0, size_t ws_bytes, First first, Second second) {
+  for (uint32_t b0 = 0, k = 0; b0 < nb; b0 += group, k++) {
+    const uint32_t m = std::min<uint32_t>(group, nb - b0);
+    const int par = (int)(k & 1);
+    uint8_t* ws = ws0 + (size_t)par * ws_bytes;
+    cudaEvent_t e0 = nullptr, e1 = nullptr;
+    S.dom_pair(&e0, &e1);
+    if (k >= 2) CU(cudaStreamWaitEvent(S.st2, S.ev_free[par], 0));  // group k-2's second pass has released ws
+    if (int rc = first(b0, m, ws, par, e0, e1)) return rc;
+    CU(cudaEventRecord(S.ev_match[par], S.st2));
+    CU(cudaStreamWaitEvent(S.st, S.ev_match[par], 0));
+    if (int rc = second(b0, m, ws, par, e0, e1)) return rc;
+    CU(cudaEventRecord(S.ev_free[par], S.st));
+  }
+  return 0;
+}
+
 // Enqueues the compression of n streams at d_src + src_off[i] (src_len[i] bytes) into d_dst on S.st.  The results
 // are in J.h once ev_a has completed.
 int compress_chunk(Slot& S, const ChecksumTables& tabs, uint32_t codec, int32_t level, uint32_t bs, uint32_t alg,
@@ -463,31 +485,25 @@ int compress_chunk(Slot& S, const ChecksumTables& tabs, uint32_t codec, int32_t 
   CU(cudaMemsetAsync(M.down, 0, M.down_bytes, st));
   CU(cudaEventRecord(S.ev_k0, st));
   CU(cudaEventRecord(S.ev_t0, st));
-  // Chunks of `chunk` codec blocks.  The match kernel (issue bound, shared-memory limited) of chunk k+1 runs on the
-  // side stream while parse (latency bound, one thread per block), scan and emit of chunk k run on the main stream;
-  // the two workspaces alternate.  The side stream forks BEFORE the per-block XXH32 pass (LZ4Block headers; only the
-  // emit kernel needs it), so that pass runs beside the first chunk's match kernel instead of in front of it.
+  // Match kernels (issue bound, shared-memory limited) on the side stream, parse (latency bound), scan and emit on st.
+  // The side stream forks BEFORE the per-block XXH32 pass (LZ4Block headers; only the emit kernel needs it), so that
+  // pass runs beside the first group's match kernel instead of in front of it.
   CU(cudaEventRecord(S.ev_fork, st));
   CU(cudaStreamWaitEvent(S.st2, S.ev_fork, 0));
   if (codec == B2S_CODEC_LZ4BLOCK)
     launch_xxh32_encode(d_src, M.src_off, M.src_len, M.blk_base, n, nb, bs, kXxhSeed, M.hash, st, launches);
   CU(cudaMemsetAsync(M.total, 0, 16, st));
-  uint32_t k = 0;
-  for (uint32_t b0 = 0; b0 < nb; b0 += chunk, k++) {
-    const uint32_t m = std::min<uint32_t>(chunk, nb - b0);
-    const int par = (int)(k & 1);
-    uint8_t* ws = (uint8_t*)S.scratch.p + (size_t)par * ws_bytes;
-    cudaEvent_t e0 = nullptr, e1 = nullptr;
-    S.dom_pair(&e0, &e1);
-    if (k >= 2) CU(cudaStreamWaitEvent(S.st2, S.ev_free[par], 0));  // emit of chunk k-2 has released this workspace
+  auto match = [&](uint32_t b0, uint32_t m, uint8_t* ws, int par, cudaEvent_t e0, cudaEvent_t e1) {
     launch_lz4_match(d_src, M.src_off, M.src_len, M.blk_base, n, b0, m, bs, codec, ws, M.counter + par, S.st2, launches,
                      e0, e1, hlog_for_level(codec, level));
-    CU(cudaEventRecord(S.ev_match[par], S.st2));
-    CU(cudaStreamWaitEvent(st, S.ev_match[par], 0));
+    return 0;
+  };
+  auto parse_emit = [&](uint32_t b0, uint32_t m, uint8_t* ws, int, cudaEvent_t, cudaEvent_t) {
     launch_lz4_parse_emit(d_src, M.src_off, M.src_len, M.blk_base, n, b0, m, bs, codec, ws, M.nseq, M.csize, M.hash,
                           M.sizes, M.total, M.ws, d_dst, dst_cap, st, launches);
-    CU(cudaEventRecord(S.ev_free[par], st));
-  }
+    return 0;
+  };
+  if (int r = run_block_groups(S, nb, chunk, (uint8_t*)S.scratch.p, ws_bytes, match, parse_emit)) return r;
   CU(cudaEventRecord(S.ev_t1, st));
   if (codec == B2S_CODEC_ZSTD)
     launch_zstd_stream_meta(M.blk_base, n, nb, M.sizes, M.total, d_dst, dst_cap, M.dst_off, M.dst_len, M.status, st,
@@ -725,26 +741,21 @@ int decompress_enqueue_b(Slot& S, DecompressJob& J, const uint8_t* d_src, uint8_
     rc = S.scratch.ensure(nrec_bytes + ws_bytes * (nb > chunk ? 2 : 1));
     if (rc) return rc;
     uint32_t* nrec = (uint32_t*)S.scratch.p;
-    // token walk (thread per block, latency bound) of chunk k+1 on the side stream, copies of chunk k on the main one
+    // token walk (thread per block, latency bound) of group k+1 on the side stream, copies of group k on the main one
     CU(cudaEventRecord(S.ev_fork, st));
     CU(cudaStreamWaitEvent(S.st2, S.ev_fork, 0));
-    uint32_t k = 0;
-    for (uint32_t b0 = 0; b0 < nb; b0 += chunk, k++) {
-      const uint32_t m = std::min<uint32_t>(chunk, nb - b0);
-      const int par = (int)(k & 1);
-      uint8_t* ws = (uint8_t*)S.scratch.p + nrec_bytes + (size_t)par * ws_bytes;
-      if (k >= 2) CU(cudaStreamWaitEvent(S.st2, S.ev_free[par], 0));
+    auto tokens = [&](uint32_t b0, uint32_t m, uint8_t* ws, int, cudaEvent_t, cudaEvent_t) {
       launch_snappy_tokens(desc, b0, m, d_src, reinterpret_cast<uint2*>(ws), rec_stride, nrec, J.d.status, S.st2,
                            launches);
-      CU(cudaEventRecord(S.ev_match[par], S.st2));
-      CU(cudaStreamWaitEvent(st, S.ev_match[par], 0));
-      cudaEvent_t e0 = nullptr, e1 = nullptr;
-      S.dom_pair(&e0, &e1);
+      return 0;
+    };
+    auto copy = [&](uint32_t b0, uint32_t m, uint8_t* ws, int, cudaEvent_t e0, cudaEvent_t e1) -> int {
       CU(cudaEventRecord(e0, st));
       launch_snappy_copy(desc, b0, m, rec_stride, d_src, d_dst, ws, nrec, st, launches);
       CU(cudaEventRecord(e1, st));
-      CU(cudaEventRecord(S.ev_free[par], st));
-    }
+      return 0;
+    };
+    if (int r = run_block_groups(S, nb, chunk, (uint8_t*)S.scratch.p + nrec_bytes, ws_bytes, tokens, copy)) return r;
   }
   CU(cudaEventRecord(S.ev_t1, st));
   // One XXH32 pass over all decoded blocks after the last chunk.  Queueing it chunk by chunk on the side stream (beside
@@ -803,21 +814,11 @@ void end_timing(const WallTimer& wt, uint64_t launches, const CallBytes& b, Slot
   t_timing.total_ms = wt.ms();
 }
 
-// groups streams [i0, i1) into chunks of ~g_host_chunk_bytes
-void make_chunks(uint32_t n, const uint64_t* len, std::vector<uint32_t>& starts) {
-  starts.clear();
-  uint32_t i = 0;
-  while (i < n) {
-    starts.push_back(i);
-    uint64_t bytes = 0;
-    uint32_t cnt = 0;
-    while (i < n && cnt < kChunkStreams && (cnt == 0 || bytes + len[i] <= g_host_chunk_bytes)) {
-      bytes += len[i];
-      i++;
-      cnt++;
-    }
-  }
-  starts.push_back(n);
+// run_chunks' retire: the slot's stream has drained, the payload download of its last chunk included
+int retire_slot(Slot& S, bool used) {
+  CU(cudaStreamSynchronize(S.st));
+  if (used) t_timing.d2h_ms += ms_between(S.ev_d0, S.ev_d1);
+  return 0;
 }
 
 // device layout of a chunk's sources: runs that are contiguous in host memory stay contiguous (one memcpy each)
@@ -1456,8 +1457,7 @@ static int checksum_host(uint32_t alg, uint32_t n, const uint8_t* const* ptr, co
   if (!n) return 0;
   Lane& Ln = D->lane[kLaneRead];
   std::lock_guard<std::mutex> lk(Ln.mtx);
-  std::vector<uint32_t> starts;
-  make_chunks(n, len, starts);
+  const std::vector<uint32_t> starts = chunk_starts(n, len, kChunkStreams, g_host_chunk_bytes);
   std::vector<uint64_t> dev_off;
   std::vector<Run> runs;
   uint64_t launches = 0;
@@ -1562,18 +1562,25 @@ static int compress_host(uint32_t codec, int32_t level, uint32_t codec_block_siz
   std::lock_guard<std::mutex> lk(Ln.mtx);
   const uint32_t bs = block_size_or_default(codec_block_size);
   if ((rc = check_codec_block(codec, bs))) return rc;  // before anything is staged
-  std::vector<uint32_t> starts;
-  make_chunks(n, src_len, starts);
-  const size_t nchunks = starts.size() - 1;
-  std::vector<CompressJob> jobs(nchunks);
+  const std::vector<uint32_t> starts = chunk_starts(n, src_len, kChunkStreams, g_host_chunk_bytes);
+  std::vector<CompressJob> jobs(starts.size() - 1);
   std::vector<Run> runs;
   std::vector<uint64_t> dev_off;
   uint64_t launches = 0, run_off = 0;
 
-  auto finish = [&](size_t c) -> int {
-    Slot& S = Ln.slot[c % g_nslot];
+  auto enqueue = [&](Slot& S, size_t c, uint32_t i0, uint32_t cnt) -> int {
+    uint64_t bound = 0, bytes = 0;
+    for (uint32_t k = 0; k < cnt; k++) bound += b2s_compress_bound(codec, bs, src_len[i0 + k]);
+    if (int r = S.dst.ensure(bound + 64)) return r;
+    dev_off.resize(cnt);
+    if (int r = upload_chunk(S, cnt, src + i0, src_len + i0, dev_off.data(), runs, &bytes)) return r;
+    t_timing.h2d_bytes += bytes;
+    t_timing.src_bytes += bytes;
+    return compress_chunk(S, D->tabs, codec, level, bs, alg, cnt, dev_off.data(), src_len + i0,
+                          (const uint8_t*)S.src.p, (uint8_t*)S.dst.p, S.dst.cap, jobs[c], &launches);
+  };
+  auto finish = [&](Slot& S, size_t c, uint32_t i0, uint32_t cnt) -> int {
     const CompressLayout& H = jobs[c].h;
-    const uint32_t i0 = starts[c], cnt = jobs[c].n;
     CU(cudaEventSynchronize(S.ev_a));
     add_timing(S, true);
     const uint64_t chunk_total = H.total[0] + stream_overhead(codec) * cnt;
@@ -1591,34 +1598,8 @@ static int compress_host(uint32_t codec, int32_t level, uint32_t codec_block_siz
     return r;
   };
 
-  for (size_t c = 0; c < nchunks; c++) {
-    Slot& S = Ln.slot[c % g_nslot];
-    if (c >= (size_t)g_nslot) {
-      rc = finish(c - g_nslot);
-      if (rc) return rc;
-      CU(cudaStreamSynchronize(S.st));  // payload of the slot's previous chunk has left the device
-      t_timing.d2h_ms += ms_between(S.ev_d0, S.ev_d1);
-    }
-    const uint32_t i0 = starts[c], cnt = starts[c + 1] - starts[c];
-    uint64_t bound = 0, bytes = 0;
-    for (uint32_t k = 0; k < cnt; k++) bound += b2s_compress_bound(codec, bs, src_len[i0 + k]);
-    if ((rc = S.dst.ensure(bound + 64))) return rc;
-    dev_off.resize(cnt);
-    if ((rc = upload_chunk(S, cnt, src + i0, src_len + i0, dev_off.data(), runs, &bytes))) return rc;
-    t_timing.h2d_bytes += bytes;
-    t_timing.src_bytes += bytes;
-    rc = compress_chunk(S, D->tabs, codec, level, bs, alg, cnt, dev_off.data(), src_len + i0, (const uint8_t*)S.src.p,
-                        (uint8_t*)S.dst.p, S.dst.cap, jobs[c], &launches);
-    if (rc) return rc;
-  }
-  for (size_t c = nchunks > (size_t)g_nslot ? nchunks - g_nslot : 0; c < nchunks; c++) {
-    rc = finish(c);
-    if (rc) return rc;
-  }
-  for (int k = 0; k < g_nslot; k++) {
-    CU(cudaStreamSynchronize(Ln.slot[k].st));
-    if ((size_t)k < nchunks) t_timing.d2h_ms += ms_between(Ln.slot[k].ev_d0, Ln.slot[k].ev_d1);
-  }
+  if (int r = run_chunks(Ln.slot, g_nslot, starts, {{0, enqueue}, {(size_t)g_nslot, finish}}, retire_slot))
+    return r;
   CU(cudaGetLastError());
   if (dst_total) *dst_total = run_off;
   end_timing(wt, launches, CallBytes{});
@@ -2139,21 +2120,13 @@ static int decompress_host(uint32_t codec, uint32_t alg, uint32_t n, const uint8
   Lane& Ln = D->lane[kLaneRead];
   std::lock_guard<std::mutex> lk(Ln.mtx);
   if ((rc = check_decode_codec(codec, false))) return rc;  // before anything is staged
-  std::vector<uint32_t> starts;
-  make_chunks(n, src_len, starts);
-  const size_t nchunks = starts.size() - 1;
-  std::vector<DecompressJob> jobs(nchunks);
+  const std::vector<uint32_t> starts = chunk_starts(n, src_len, kChunkStreams, g_host_chunk_bytes);
+  std::vector<DecompressJob> jobs(starts.size() - 1);
   std::vector<Run> runs;
   std::vector<uint64_t> dev_off;
   uint64_t launches = 0, run_off = 0;
 
-  auto stage_a = [&](size_t c) -> int {
-    Slot& S = Ln.slot[c % g_nslot];
-    if (c >= (size_t)g_nslot) {
-      CU(cudaStreamSynchronize(S.st));
-      t_timing.d2h_ms += ms_between(S.ev_d0, S.ev_d1);
-    }
-    const uint32_t i0 = starts[c], cnt = starts[c + 1] - starts[c];
+  auto stage_a = [&](Slot& S, size_t c, uint32_t i0, uint32_t cnt) -> int {
     DecompressJob& J = jobs[c];
     J.size_only = size_only;
     dev_off.resize(cnt);
@@ -2166,8 +2139,7 @@ static int decompress_host(uint32_t codec, uint32_t alg, uint32_t n, const uint8
                               alg ? slice_base + i0 : nullptr, slice_len, slice_sum, (const uint8_t*)S.src.p, bytes,
                               J, &launches);
   };
-  auto stage_b = [&](size_t c) -> int {
-    Slot& S = Ln.slot[c % g_nslot];
+  auto stage_b = [&](Slot& S, size_t c, uint32_t, uint32_t) -> int {
     DecompressJob& J = jobs[c];
     CU(cudaEventSynchronize(S.ev_a));
     if (size_only) {
@@ -2180,10 +2152,8 @@ static int decompress_host(uint32_t codec, uint32_t alg, uint32_t n, const uint8
     if (r) return r;
     return decompress_enqueue_b(S, J, (const uint8_t*)S.src.p, (uint8_t*)S.dst.p, S.dst.cap, &launches);
   };
-  auto stage_c = [&](size_t c) -> int {
-    Slot& S = Ln.slot[c % g_nslot];
+  auto stage_c = [&](Slot& S, size_t c, uint32_t i0, uint32_t) -> int {
     const DecompressJob& J = jobs[c];
-    const uint32_t i0 = starts[c];
     CU(cudaEventSynchronize(S.ev_b));
     if (!size_only) add_timing(S, true);
     for (uint32_t k = 0; k < J.n; k++) {
@@ -2201,29 +2171,11 @@ static int decompress_host(uint32_t codec, uint32_t alg, uint32_t n, const uint8
     return r;
   };
 
-  // software pipeline over the chunks: enqueue chunk c's upload + phase A first (never blocks on younger work), then
-  // phase B of chunk c-lag (waits for its sizes), then the download of chunk c-2*lag (waits for its decode).  lag
-  // chunks between the stages keep lag uploads / decodes queued on the device while the host waits for one chunk's
+  // lag chunks between the stages keep lag uploads / decodes queued on the device while the host waits for one chunk's
   // sizes (the write lane keeps g_nslot chunks in flight and would otherwise own the copy queues).
-  // Invariant: stage_a(c) restages slot c % g_nslot (its source arena and the pinned block that holds the statuses,
-  // lengths and offsets stage_c reads), so chunk c - g_nslot, the slot's previous chunk, has been through stage_c
-  // before it.  With 2 * lag + 1 <= g_nslot (every slot count from 3) the loop order already guarantees that; with 2
-  // slots (lag 1) the download of chunk c-2 moves in front of stage_a(c), and one chunk is decoded while the next is
-  // sized.
   const size_t lag = (size_t)std::max(1, std::min(g_read_lag, (g_nslot - 1) / 2));
-  size_t done = 0;  // chunks through stage_c, in order
-  for (size_t c = 0; c < nchunks + 2 * lag; c++) {
-    for (; done + g_nslot <= c && done < nchunks; done++)
-      if ((rc = stage_c(done))) return rc;
-    if (c < nchunks && (rc = stage_a(c))) return rc;
-    if (c >= lag && c - lag < nchunks && (rc = stage_b(c - lag))) return rc;
-    for (; done + 2 * lag <= c && done < nchunks; done++)
-      if ((rc = stage_c(done))) return rc;
-  }
-  for (int k = 0; k < g_nslot; k++) {
-    CU(cudaStreamSynchronize(Ln.slot[k].st));
-    if ((size_t)k < nchunks) t_timing.d2h_ms += ms_between(Ln.slot[k].ev_d0, Ln.slot[k].ev_d1);
-  }
+  if (int r = run_chunks(Ln.slot, g_nslot, starts, {{0, stage_a}, {lag, stage_b}, {2 * lag, stage_c}}, retire_slot))
+    return r;
   CU(cudaGetLastError());
   if (dst_total) *dst_total = run_off;
   end_timing(wt, launches, CallBytes{});
@@ -3238,14 +3190,7 @@ int b2s_exchange_read_packed(int32_t shuffle_id, int32_t start_reduce, int32_t e
   CU(cudaEventRecord(S.ev_d1, st));
   CU(cudaStreamSynchronize(st));
   CU(cudaGetLastError());
-  add_timing(S, false);
-  t_timing.d2h_ms = ms_between(S.ev_d0, S.ev_d1);
-  t_timing.d2h_bytes = total;
-  t_timing.kernel_launches = launches;
-  t_timing.src_bytes = total;
-  t_timing.dst_bytes = total;
-  t_timing.total_ms = wt.ms();
-  g_ctx->launches += launches;
+  end_timing(wt, launches, CallBytes{total, total, 0, total}, &S, kD2H);
   return 0;
 }
 

@@ -5,7 +5,7 @@ The chunk size, the slot count, the read pipeline's lag and the codec-block grou
 B2S_HOST_CHUNK_MB / B2S_SLOTS / B2S_READ_LAG / B2S_LZ4_CHUNK_BLOCKS / B2S_LZ4D_CHUNK_BLOCKS, so
 tests/test_gpu_chunk_pipelines.py starts this worker once per configuration with the environment set.  It prints one
 JSON line: each check's name with "ok" or its failure, and what the calls reached (chunks, slot reuses, block groups),
-computed on the host from the same chunking rule as api.cu's make_chunks.
+computed on the host from the same chunking rule as chunk_schedule.h's chunk_starts.
 
     python tests/chunk_pipeline_worker.py <config name> <libzc.so: the Zstd encoder's CPU model>
 """
@@ -64,7 +64,7 @@ def check(name, fn, *args):
 # the chunking rule of the host-pointer calls, and what a call reached
 # ---------------------------------------------------------------------------------------------------------------------
 def make_chunks(lens):
-    """api.cu make_chunks: a chunk takes streams while it has fewer than 2^18 and its bytes stay within the chunk size
+    """chunk_schedule.h chunk_starts: a chunk takes streams while it has fewer than 2^18 and its bytes stay within the chunk size
     (its first stream always) -> chunk start indices followed by len(lens)"""
     starts, i, n = [], 0, len(lens)
     while i < n:
