@@ -187,6 +187,43 @@ int b2s_partition_compress_dev(uint32_t dev_index, uint32_t codec, int32_t level
                                const uint32_t* rec_part, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_off,
                                uint64_t* dst_len, uint64_t* dst_total, uint64_t* checksum_out, int32_t* status);
 
+/* ---- write side, hash-partitioned rows: Spark's HashPartitioning ids computed on the GPU ----
+ * b2s_partition_compress_* for a HashPartitioning exchange of UnsafeRows: the reduce id of every record is Spark's
+ * pmod(Murmur3Hash(key columns, 42), num_partitions), bit for bit, so the caller passes no rec_part.  Record i is
+ * rec_len[i] bytes as UnsafeRowSerializer writes a row: [size s: int32 big-endian][s bytes of row], rec_len[i] = 4 + s.
+ * The key columns are given as to the composite-key calls (b2s_decompress_*_rows_keys_*, below): n_keys (1..16),
+ * key_type[c] at row offset key_off[c], key_len[c] bytes, null bit key_null_field[c] (-1: never null).  Starting from
+ * h = 42, each column left to right sets h = its hash with seed h; a null column leaves h as it is (all null: 42).
+ *   B2S_KEY_BYTES, key_len 1 (BooleanType): hashInt(byte != 0 ? 1 : 0)
+ *   B2S_KEY_INT8 / B2S_KEY_INT16 / B2S_KEY_INT32 (ByteType, ShortType, IntegerType, DateType): hashInt of the value
+ *   B2S_KEY_INT64 (LongType, TimestampType, Decimal(p <= 18)): hashLong
+ *   B2S_KEY_FLOAT32 / B2S_KEY_FLOAT64: hashInt(floatToIntBits) / hashLong(doubleToLongBits), -0.0 as 0.0 and every NaN
+ *     as the canonical NaN (Spark >= 3.2)
+ *   B2S_STRING_KEY (StringType, BinaryType) / B2S_DECIMAL_KEY (Decimal(p > 18), 1..16 bytes): hashUnsafeBytes of the
+ *     slot's bytes, with Spark's tail (every byte after the last whole 4-byte word mixed on its own, sign-extended)
+ * Outputs: byte for byte what b2s_partition_compress_packed / _dev return for the same records and those ids.
+ * Errors, B2S_E_ARG: what b2s_partition_compress_* rejects; n_keys outside 1..16, a type not listed, a key_len that does
+ * not match its type, an order flag, key_null_field < -1.  A bad record -> B2S_E_ARG, nothing reported as written, and
+ * b2s_last_error() names the lowest bad record and why: rec_len < 4, a size prefix other than rec_len - 4, a row that
+ * does not hold a key slot or a key's null word, a non-null string past the row, a non-null decimal whose size is not
+ * 1..16 or that runs past the row.  No usable device -> B2S_E_CUDA.  b2s_last_timing as for the partition calls, plus
+ * dominant_ms / dominant_launches = the hash step alone.  No exchange-cache form. */
+int b2s_partition_compress_rows_hash_packed(uint32_t codec, int32_t level, uint32_t codec_block_size,
+                                            uint32_t checksum_alg, uint32_t num_partitions, uint64_t n_records,
+                                            const uint8_t* rec_base, uint64_t rec_bytes, const uint32_t* rec_len,
+                                            uint32_t n_keys, const uint32_t* key_type, const uint32_t* key_off,
+                                            const uint32_t* key_len, const int32_t* key_null_field, uint8_t* dst_base,
+                                            uint64_t dst_cap, uint64_t* dst_off, uint64_t* dst_len,
+                                            uint64_t* dst_total, uint64_t* checksum_out, int32_t* status);
+/* same, with rec_base / rec_len / dst_base in device memory of dev_index */
+int b2s_partition_compress_rows_hash_dev(uint32_t dev_index, uint32_t codec, int32_t level, uint32_t codec_block_size,
+                                         uint32_t checksum_alg, uint32_t num_partitions, uint64_t n_records,
+                                         const uint8_t* rec_base, uint64_t rec_bytes, const uint32_t* rec_len,
+                                         uint32_t n_keys, const uint32_t* key_type, const uint32_t* key_off,
+                                         const uint32_t* key_len, const int32_t* key_null_field, uint8_t* dst_base,
+                                         uint64_t dst_cap, uint64_t* dst_off, uint64_t* dst_len, uint64_t* dst_total,
+                                         uint64_t* checksum_out, int32_t* status);
+
 /* ---- read side ---- */
 /* n compressed blocks as produced by S3BufferedPrefetchIterator.next() (storage/S3BufferedPrefetchIterator.scala:196-212).
  * Block i covers n_slices[i] consecutive reduce partitions (1 for ShuffleBlockId, >1 for ShuffleBlockBatchId,

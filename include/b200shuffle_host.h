@@ -110,6 +110,13 @@ void b2sh_writer_destroy(b2sh_writer* w);
 typedef struct b2sh_serialized_writer b2sh_serialized_writer;
 int b2sh_serialized_writer_create(b2sh_dispatcher* d, int32_t shuffle_id, int64_t map_id, int32_t num_partitions,
                                   b2sh_serialized_writer** out);
+/* HashPartitioning of UnsafeRows (INTEGRATION.md §3j), set before the first insert: every later insert is one record as
+ * UnsafeRowSerializer writes it ([int32 big-endian size][row]) and its partition_id is ignored; commit() makes one
+ * b2s_partition_compress_rows_hash_packed call with these key columns, which computes Spark's reduce ids on the GPU.
+ * The files are byte-identical to the ones the writer makes when fed the same rows with those ids.  In this mode the
+ * writer never stores into the exchange cache, even when it is on: the cache's reads serve fixed-size records only. */
+int b2sh_serialized_writer_hash_rows(b2sh_serialized_writer* w, uint32_t n_keys, const uint32_t* key_type,
+                                     const uint32_t* key_off, const uint32_t* key_len, const int32_t* key_null_field);
 int b2sh_serialized_writer_insert(b2sh_serialized_writer* w, int32_t partition_id, const uint8_t* bytes, uint64_t len);
 int b2sh_serialized_writer_commit(b2sh_serialized_writer* w, int64_t* partition_lengths_out);
 int b2sh_serialized_writer_statistics(b2sh_serialized_writer* w, uint64_t* bytes, uint64_t* nanos, char* line,

@@ -7,6 +7,8 @@
  *   compressPacked                         shuffle/S3ShuffleMapOutputWriter.scala:91-118 (commitAllPartitions)
  *   partitionCompressPacked                the GPU serialized writer (INTEGRATION.md §3d): records + reduce ids of a
  *                                          map task in, .data arena + partitionLengths + checksums out
+ *   partitionCompressRowsHashPacked        the same for a HashPartitioning exchange (INTEGRATION.md §3j): rows and
+ *                                          their key columns in, the reduce ids computed on the GPU
  *   decompressPacked / decompressedSize    storage/S3ShuffleReader.scala:98-110 (the codec seam, batched drain of
  *                                          storage/S3BufferedPrefetchIterator.scala:196-212)
  *   checksumPacked                         shuffle/S3SingleSpillShuffleMapOutputWriter.scala:54-63,
@@ -131,15 +133,38 @@ JNIEXPORT jint JNICALL J(compressPacked)(JNIEnv* e, jclass c, jint codec, jint l
  *      meta: long[1] = {dst_total}.  The per-partition results are collected in native memory during the blocking
  *      call and copied out with Set<Type>ArrayRegion afterwards: no Java array is held in a critical region while the
  *      GPU works. ---- */
-/* cached (may be NULL): int[1], the cached store's flag; then (shuffleId, mapId) keys the exchange-cache entry */
-static jint partition_compress(JNIEnv* e, jint shuffleId, jlong mapId, jintArray cached, jint codec, jint level,
-                               jint blockSize, jint alg, jint numPartitions, jlong nRecords, jlong records,
-                               jlong recBytes, jlong recLen, jlong recPart, jlong dst, jlong dstCap, jlongArray dstOff,
-                               jlongArray dstLen, jlongArray meta, jlongArray checksums, jintArray status) {
+/* a composite key: int[n] key_type / key_off / key_len / key_null_field, as the C ABI's *_keys calls take them */
+typedef struct {
+  jint n; /* 1..16 columns */
+  jintArray type, off, len, nullField;
+} composite_key;
+static int bad_keys(JNIEnv* e, const composite_key* keys) {
+  return keys->n < 1 || keys->n > 16 || !keys->type || !keys->off || !keys->len || !keys->nullField ||
+         (*e)->GetArrayLength(e, keys->type) < keys->n || (*e)->GetArrayLength(e, keys->off) < keys->n ||
+         (*e)->GetArrayLength(e, keys->len) < keys->n || (*e)->GetArrayLength(e, keys->nullField) < keys->n;
+}
+
+/* cached (may be NULL): int[1], the cached store's flag; then (shuffleId, mapId) keys the exchange-cache entry.
+ * hash (may be NULL, then cached is NULL): the records are serialized rows whose reduce ids are Spark's
+ * HashPartitioning ids by these key columns (partitionCompressRowsHashPacked); recPart is not read */
+static jint partition_compress(JNIEnv* e, jint shuffleId, jlong mapId, jintArray cached, const composite_key* hash,
+                               jint codec, jint level, jint blockSize, jint alg, jint numPartitions, jlong nRecords,
+                               jlong records, jlong recBytes, jlong recLen, jlong recPart, jlong dst, jlong dstCap,
+                               jlongArray dstOff, jlongArray dstLen, jlongArray meta, jlongArray checksums,
+                               jintArray status) {
   if ((cached && (*e)->GetArrayLength(e, cached) < 1) || numPartitions < 1 || !dstOff || !dstLen || !meta || !status || (*e)->GetArrayLength(e, dstOff) < numPartitions ||
       (*e)->GetArrayLength(e, dstLen) < numPartitions || (*e)->GetArrayLength(e, status) < numPartitions ||
       (*e)->GetArrayLength(e, meta) < 1 || (checksums && (*e)->GetArrayLength(e, checksums) < numPartitions))
     return B2S_E_ARG;
+  if (hash && bad_keys(e, hash)) return B2S_E_ARG;
+  uint32_t kt[16], ko[16], kl[16];
+  int32_t knf[16];
+  if (hash) {
+    (*e)->GetIntArrayRegion(e, hash->type, 0, hash->n, (jint*)kt);
+    (*e)->GetIntArrayRegion(e, hash->off, 0, hash->n, (jint*)ko);
+    (*e)->GetIntArrayRegion(e, hash->len, 0, hash->n, (jint*)kl);
+    (*e)->GetIntArrayRegion(e, hash->nullField, 0, hash->n, (jint*)knf);
+  }
   const size_t R = (size_t)numPartitions;
   uint64_t* buf = (uint64_t*)malloc(R * 3 * sizeof(uint64_t));
   int32_t* st = (int32_t*)malloc(R * sizeof(int32_t));
@@ -151,7 +176,12 @@ static jint partition_compress(JNIEnv* e, jint shuffleId, jlong mapId, jintArray
   uint64_t total = 0;
   int32_t stored = 0;
   const int rc =
-      cached ? b2s_partition_compress_cached_packed(
+      hash ? b2s_partition_compress_rows_hash_packed(
+                 (uint32_t)codec, (int32_t)level, (uint32_t)blockSize, (uint32_t)alg, (uint32_t)numPartitions,
+                 (uint64_t)nRecords, PTR(const uint8_t, records), (uint64_t)recBytes, PTR(const uint32_t, recLen),
+                 (uint32_t)hash->n, kt, ko, kl, knf, PTR(uint8_t, dst), (uint64_t)dstCap, buf, buf + R, &total,
+                 buf + 2 * R, st)
+      : cached ? b2s_partition_compress_cached_packed(
                    (int32_t)shuffleId, (int64_t)mapId, (uint32_t)codec, (int32_t)level, (uint32_t)blockSize,
                    (uint32_t)alg, (uint32_t)numPartitions, (uint64_t)nRecords, PTR(const uint8_t, records),
                    (uint64_t)recBytes, PTR(const uint32_t, recLen), PTR(const uint32_t, recPart), PTR(uint8_t, dst),
@@ -180,8 +210,23 @@ JNIEXPORT jint JNICALL J(partitionCompressPacked)(JNIEnv* e, jclass c, jint code
                                                   jlongArray dstOff, jlongArray dstLen, jlongArray meta,
                                                   jlongArray checksums, jintArray status) {
   (void)c;
-  return partition_compress(e, 0, 0, 0, codec, level, blockSize, alg, numPartitions, nRecords, records, recBytes, recLen,
-                            recPart, dst, dstCap, dstOff, dstLen, meta, checksums, status);
+  return partition_compress(e, 0, 0, 0, 0, codec, level, blockSize, alg, numPartitions, nRecords, records, recBytes,
+                            recLen, recPart, dst, dstCap, dstOff, dstLen, meta, checksums, status);
+}
+/* HashPartitioning exchange of UnsafeRows (INTEGRATION.md §3j): records as UnsafeRowSerializer writes them, recLen
+ * (u32) per record, no reduce ids: the GPU computes Spark's pmod(Murmur3Hash(key columns, 42), numPartitions).  The key
+ * columns are int[nKeys] keyType / keyOff / keyLen / keyNullField; the rest as partitionCompressPacked */
+JNIEXPORT jint JNICALL J(partitionCompressRowsHashPacked)(JNIEnv* e, jclass c, jint codec, jint level, jint blockSize,
+                                                          jint alg, jint numPartitions, jlong nRecords, jlong records,
+                                                          jlong recBytes, jlong recLen, jint nKeys, jintArray keyType,
+                                                          jintArray keyOff, jintArray keyLen, jintArray keyNullField,
+                                                          jlong dst, jlong dstCap, jlongArray dstOff,
+                                                          jlongArray dstLen, jlongArray meta, jlongArray checksums,
+                                                          jintArray status) {
+  (void)c;
+  const composite_key keys = {nKeys, keyType, keyOff, keyLen, keyNullField};
+  return partition_compress(e, 0, 0, 0, &keys, codec, level, blockSize, alg, numPartitions, nRecords, records,
+                            recBytes, recLen, 0, dst, dstCap, dstOff, dstLen, meta, checksums, status);
 }
 /* the same, keeping the partitioned records in the exchange cache as (shuffleId, mapId); cached: int[1] = stored */
 JNIEXPORT jint JNICALL J(partitionCompressCachedPacked)(JNIEnv* e, jclass c, jint shuffleId, jlong mapId, jint codec,
@@ -192,8 +237,8 @@ JNIEXPORT jint JNICALL J(partitionCompressCachedPacked)(JNIEnv* e, jclass c, jin
                                                         jintArray status, jintArray cached) {
   (void)c;
   if (!cached) return B2S_E_ARG;
-  return partition_compress(e, shuffleId, mapId, cached, codec, level, blockSize, alg, numPartitions, nRecords, records,
-                            recBytes, recLen, recPart, dst, dstCap, dstOff, dstLen, meta, checksums, status);
+  return partition_compress(e, shuffleId, mapId, cached, 0, codec, level, blockSize, alg, numPartitions, nRecords,
+                            records, recBytes, recLen, recPart, dst, dstCap, dstOff, dstLen, meta, checksums, status);
 }
 
 /* ---- read side: n prefetched blocks; block i owns slices [sliceBase[i], sliceBase[i+1]) of sliceLen/sliceChecksum
@@ -241,10 +286,6 @@ JNIEXPORT jint JNICALL J(decompressPacked)(JNIEnv* e, jclass c, jint codec, jint
  * aggregation (decompressAggregateRowsPacked) with int[nAggs] aggOp / aggOff / aggNullField, and meta long[3] =
  * {dst_total, n_records, n_groups}.  keys (rows only; NULL: the one key keyType / keyOff / keyLen / nullField): a
  * composite key (decompressSortRowsKeysPacked / decompressAggregateRowsKeysPacked) */
-typedef struct {
-  jint n; /* 1..16 columns */
-  jintArray type, off, len, nullField;
-} composite_key;
 static jint sort_packed(JNIEnv* e, jint shuffleId, jint startReduce, jint endReduce, jlongArray mapIds,
                         jintArray cached, jint codec, jint alg, jint n, jlong src, jlongArray off, jlongArray len,
                         jintArray sliceBase, jlongArray sliceLen, jlongArray sliceChecksum, jint recordBytes,
@@ -253,10 +294,7 @@ static jint sort_packed(JNIEnv* e, jint shuffleId, jint startReduce, jint endRed
                         jlongArray meta, jintArray status, jintArray badSlice) {
   const jsize n_meta = aggOp ? 3 : 2;
   if (n < 0 || !meta || (*e)->GetArrayLength(e, meta) < n_meta) return B2S_E_ARG;
-  if (keys && (keys->n < 1 || keys->n > 16 || !keys->type || !keys->off || !keys->len || !keys->nullField ||
-               (*e)->GetArrayLength(e, keys->type) < keys->n || (*e)->GetArrayLength(e, keys->off) < keys->n ||
-               (*e)->GetArrayLength(e, keys->len) < keys->n || (*e)->GetArrayLength(e, keys->nullField) < keys->n))
-    return B2S_E_ARG;
+  if (keys && bad_keys(e, keys)) return B2S_E_ARG;
   if (aggOp && (nAggs < 0 || nAggs > 16 || !aggOff || !aggNullField || (*e)->GetArrayLength(e, aggOp) < nAggs ||
                 (*e)->GetArrayLength(e, aggOff) < nAggs || (*e)->GetArrayLength(e, aggNullField) < nAggs))
     return B2S_E_ARG;

@@ -68,6 +68,12 @@ PROTOTYPES = [
      [_u32, _i32, _u32, _u32, _u32, _u64, _u8p, _u64, _u32p, _u32p, _u8p, _u64, _u64p, _u64p, _u64p, _u64p, _i32p]),
     ("b2s_partition_compress_dev", C.c_int,
      [_u32, _u32, _i32, _u32, _u32, _u32, _u64, _vp, _u64, _u32p, _u32p, _vp, _u64, _u64p, _u64p, _u64p, _u64p, _i32p]),
+    ("b2s_partition_compress_rows_hash_packed", C.c_int,
+     [_u32, _i32, _u32, _u32, _u32, _u64, _u8p, _u64, _u32p, _u32, _u32p, _u32p, _u32p, _i32p, _u8p, _u64, _u64p,
+      _u64p, _u64p, _u64p, _i32p]),
+    ("b2s_partition_compress_rows_hash_dev", C.c_int,
+     [_u32, _u32, _i32, _u32, _u32, _u32, _u64, _vp, _u64, _u32p, _u32, _u32p, _u32p, _u32p, _i32p, _vp, _u64, _u64p,
+      _u64p, _u64p, _u64p, _i32p]),
     ("b2s_decompress_batch", C.c_int,
      [_u32, _u32, _u32, _vp, _u64p, _u32p, _vp, _vp, _vp, _u64p, _u64p, _i32p, _i32p]),
     ("b2s_decompress_packed", C.c_int,
@@ -597,6 +603,36 @@ def partition_compress_dev(codec, d_records, rec_bytes, d_rec_len, d_rec_part, n
                                              d_records, rec_bytes, d_rec_len, d_rec_part, d_dst, dst_cap,
                                              _ptr(dst_off), _ptr(dst_len), C.addressof(total), _ptr(cks), _ptr(st)),
            "b2s_partition_compress_dev")
+    return dict(dst_off=dst_off, dst_len=dst_len, total=total.value, checksums=cks, status=st)
+
+
+def partition_compress_rows_hash_packed(codec, records, rec_len, keys, num_partitions, dst, block_size=0,
+                                        checksum_alg=CHECKSUM_NONE, level=0):
+    """partition_compress_packed of serialized UnsafeRows ([int32 big-endian size][row] each), every record's reduce
+    id Spark's pmod(Murmur3Hash(key columns, 42), num_partitions); keys as in decompress_sort_rows_keys_packed.
+    -> dict(dst_off, dst_len, total, checksums, status)"""
+    records, dst = _as_u8(records), _as_u8(dst)
+    rec_len = np.ascontiguousarray(rec_len, dtype=np.uint32)
+    nk, kt, ko, kl, kn = _key_arrays(keys)
+    dst_off, dst_len, cks, st = _partition_out(num_partitions)
+    total = _u64(0)
+    _check(load().b2s_partition_compress_rows_hash_packed(
+        codec, level, block_size, checksum_alg, num_partitions, rec_len.size, _ptr(records), records.size,
+        _ptr(rec_len), nk, _ptr(kt), _ptr(ko), _ptr(kl), _ptr(kn), _ptr(dst), dst.size, _ptr(dst_off), _ptr(dst_len),
+        C.addressof(total), _ptr(cks), _ptr(st)), "b2s_partition_compress_rows_hash_packed")
+    return dict(dst_off=dst_off, dst_len=dst_len, total=total.value, checksums=cks, status=st)
+
+
+def partition_compress_rows_hash_dev(codec, d_records, rec_bytes, d_rec_len, n_records, keys, num_partitions, d_dst,
+                                     dst_cap, block_size=0, checksum_alg=CHECKSUM_NONE, level=0, dev=0):
+    """partition_compress_rows_hash_packed on device addresses (records, u32 lengths, destination arena)"""
+    nk, kt, ko, kl, kn = _key_arrays(keys)
+    dst_off, dst_len, cks, st = _partition_out(num_partitions)
+    total = _u64(0)
+    _check(load().b2s_partition_compress_rows_hash_dev(
+        dev, codec, level, block_size, checksum_alg, num_partitions, n_records, d_records, rec_bytes, d_rec_len, nk,
+        _ptr(kt), _ptr(ko), _ptr(kl), _ptr(kn), d_dst, dst_cap, _ptr(dst_off), _ptr(dst_len), C.addressof(total),
+        _ptr(cks), _ptr(st)), "b2s_partition_compress_rows_hash_dev")
     return dict(dst_off=dst_off, dst_len=dst_len, total=total.value, checksums=cks, status=st)
 
 

@@ -1697,23 +1697,35 @@ static uint64_t first_record_past(const uint64_t* d_off, const uint32_t* d_len, 
 // The partition step and the compression of the non-empty partitions, on device-resident records.  d_dst receives the
 // .data arena (dst_cap bytes); *arena_bytes the bytes it needs.  Returns B2S_E_DST_TOO_SMALL (status[] set for the
 // partitions that do not fit) when dst_cap is short.  part_start (optional) receives the R + 1 partition offsets of the
-// partitioned records, which are in d_dst (codec NONE) or S.parena.
+// partitioned records, which are in d_dst (codec NONE) or S.parena.  hash (d_part unused): the ids are Spark's
+// HashPartitioning ids of the rows by these key columns, computed between the offsets and the radix passes (S.ev_f[0]
+// and S.ev_f[1] bracket that step), and a bad record fails the call.
 static int partition_compress_run(Device* D, Slot& S, uint32_t codec, int32_t level, uint32_t bs, uint32_t alg,
                                   uint32_t R, uint64_t n, const uint8_t* d_rec, uint64_t rec_bytes,
                                   const uint32_t* d_len, const uint32_t* d_part, uint8_t* d_dst, uint64_t dst_cap,
                                   uint64_t* dst_off, uint64_t* dst_len, uint64_t* checksum_out, int32_t* status,
                                   uint64_t* arena_bytes, uint64_t* launches,
-                                  std::vector<uint64_t>* part_start = nullptr) {
+                                  std::vector<uint64_t>* part_start = nullptr, const KeySpec* hash = nullptr) {
   cudaStream_t st = S.st;
   std::vector<uint64_t> pstart(R), plen(R);
   CU(cudaEventRecord(S.ev_p0, st));
   CU(cudaEventRecord(S.ev_k0, st));
   PartitionPlan P;
   if (n) {
-    int rc = S.pws.ensure(partition_ws_bytes(n, R));
+    int rc = S.pws.ensure(partition_ws_bytes(n, R, hash != nullptr));
     if (rc) return rc;
-    launch_partition(d_len, d_part, n, R, (uint8_t*)S.pws.p, &P, st, launches);
-    // the one readback between the partition step and compression: [bad id, byte total, partition offsets]
+    uint8_t* ws = (uint8_t*)S.pws.p;
+    if (hash) {
+      launch_partition_offsets(d_len, nullptr, n, R, ws, &P, st, launches);
+      CU(cudaEventRecord(S.ev_f[0], st));
+      launch_rows_hash(d_rec, rec_bytes, P.src_off, d_len, n, *hash, R, P.ids, P.readback, st, launches);
+      CU(cudaEventRecord(S.ev_f[1], st));
+      launch_partition_order(d_len, P.ids, n, R, ws, &P, st, launches);
+    } else {
+      launch_partition(d_len, d_part, n, R, ws, &P, st, launches);
+    }
+    // the one readback between the partition step and compression: [bad id (hash: bad record), byte total, partition
+    // offsets]
     rc = S.hmeta.ensure(P.readback_bytes);
     if (rc) return rc;
     const uint64_t* rb = (const uint64_t*)S.hmeta.p;
@@ -1721,6 +1733,15 @@ static int partition_compress_run(Device* D, Slot& S, uint32_t codec, int32_t le
     CU(cudaStreamSynchronize(st));
     CU(cudaGetLastError());
     char msg[256];
+    if (hash && rb[0] != ~0ull) {
+      static const char* const why[] = {"", "rec_len is below 4", "its size prefix is not rec_len - 4",
+                                        "its row does not hold a key slot", "its row does not hold a key's null word",
+                                        "a string key runs past its row",
+                                        "a decimal key's size is not 1..16 or it runs past its row"};
+      snprintf(msg, sizeof msg, "record %llu is not a serialized row of the key columns: %s",
+               (unsigned long long)(rb[0] >> 3), why[rb[0] & 7]);
+      return fail(B2S_E_ARG, "%s", msg);
+    }
     if (rb[0] != ~0ull) {
       uint32_t id = 0;
       CU(cudaMemcpy(&id, d_part + rb[0], 4, cudaMemcpyDeviceToHost));
@@ -1831,37 +1852,45 @@ static int partition_compress_run(Device* D, Slot& S, uint32_t codec, int32_t le
   return 0;
 }
 
+// hash: the ids are hashed from the rows, so rec_part is not read
 static int partition_args(uint32_t codec, uint32_t bs, uint32_t alg, uint32_t R, uint64_t n, const void* rec_base,
                           uint64_t rec_bytes, const uint32_t* rec_len, const uint32_t* rec_part, const void* dst_base,
-                          const uint64_t* dst_off, const uint64_t* dst_len, const int32_t* status) {
+                          const uint64_t* dst_off, const uint64_t* dst_len, const int32_t* status,
+                          const KeySpec* hash) {
   if (alg > B2S_CHECKSUM_CRC32C) return fail(B2S_E_UNSUPPORTED, "Unsupported shuffle checksum algorithm%s");
   if (codec != B2S_CODEC_NONE)
     if (int rc = check_codec_block(codec, bs)) return rc;
   if (R < 1 || R > (1u << 24)) return fail(B2S_E_ARG, "num_partitions must be in [1, 2^24]%s");
   if (n > 0xffffffffull) return fail(B2S_E_ARG, "more than 2^32 - 1 records in one call%s");
-  if ((n && (!rec_len || !rec_part)) || (rec_bytes && !rec_base) || !dst_off || !dst_len || !status)
+  if ((n && (!rec_len || (!rec_part && !hash))) || (rec_bytes && !rec_base) || !dst_off || !dst_len || !status)
     return fail(B2S_E_ARG, "null argument%s");
   if (rec_bytes && !dst_base) return fail(B2S_E_ARG, "null argument%s");
   return 0;
 }
 
-// kernel_ms: partition step + compression; top_kernel_ms: the codec step, or the partition step for codec NONE
-static void partition_kernel_times(Slot& S, uint32_t codec) {
+// kernel_ms: partition step + compression; top_kernel_ms: the codec step, or the partition step for codec NONE.
+// hash: dominant_ms / dominant_launches = the hash step alone.
+static void partition_kernel_times(Slot& S, uint32_t codec, const KeySpec* hash, uint64_t n) {
   t_timing.kernel_ms = ms_between(S.ev_p0, S.ev_k1);
   if (codec == B2S_CODEC_NONE) t_timing.top_kernel_ms = ms_between(S.ev_p0, S.ev_p1);
+  if (hash) {
+    t_timing.dominant_ms = n ? ms_between(S.ev_f[0], S.ev_f[1]) : 0;
+    t_timing.dominant_launches = n ? 1 : 0;
+  }
 }
 
-int b2s_partition_compress_dev(uint32_t dev_index, uint32_t codec, int32_t level, uint32_t codec_block_size,
-                               uint32_t checksum_alg, uint32_t num_partitions, uint64_t n_records,
-                               const uint8_t* rec_base, uint64_t rec_bytes, const uint32_t* rec_len,
-                               const uint32_t* rec_part, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_off,
-                               uint64_t* dst_len, uint64_t* dst_total, uint64_t* checksum_out, int32_t* status) {
+static int partition_compress_dev(uint32_t dev_index, uint32_t codec, int32_t level, uint32_t codec_block_size,
+                                  uint32_t checksum_alg, uint32_t num_partitions, uint64_t n_records,
+                                  const uint8_t* rec_base, uint64_t rec_bytes, const uint32_t* rec_len,
+                                  const uint32_t* rec_part, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_off,
+                                  uint64_t* dst_len, uint64_t* dst_total, uint64_t* checksum_out, int32_t* status,
+                                  const KeySpec* hash) {
   WallTimer wt;
   t_timing = b2s_timing{};
   if (dst_total) *dst_total = 0;
   const uint32_t bs = block_size_or_default(codec_block_size);
   int rc = partition_args(codec, bs, checksum_alg, num_partitions, n_records, rec_base, rec_bytes, rec_len, rec_part,
-                          dst_base, dst_off, dst_len, status);
+                          dst_base, dst_off, dst_len, status, hash);
   if (rc) return rc;
   Device* D;
   rc = get_device(dev_index, &D);
@@ -1873,13 +1902,23 @@ int b2s_partition_compress_dev(uint32_t dev_index, uint32_t codec, int32_t level
   uint64_t launches = 0, arena = 0;
   rc = partition_compress_run(D, S, codec, level, bs, checksum_alg, num_partitions, n_records, rec_base, rec_bytes,
                               rec_len, rec_part, dst_base, dst_cap, dst_off, dst_len, cks.data(), status, &arena,
-                              &launches);
+                              &launches, nullptr, hash);
   if (rc && rc != B2S_E_DST_TOO_SMALL) return rc;
   if (checksum_out) memcpy(checksum_out, cks.data(), (size_t)num_partitions * 8);
   if (dst_total) *dst_total = arena;
   end_timing(wt, launches, CallBytes{rec_bytes, arena, 0, 0}, &S);
-  partition_kernel_times(S, codec);
+  partition_kernel_times(S, codec, hash, n_records);
   return rc;
+}
+
+int b2s_partition_compress_dev(uint32_t dev_index, uint32_t codec, int32_t level, uint32_t codec_block_size,
+                               uint32_t checksum_alg, uint32_t num_partitions, uint64_t n_records,
+                               const uint8_t* rec_base, uint64_t rec_bytes, const uint32_t* rec_len,
+                               const uint32_t* rec_part, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_off,
+                               uint64_t* dst_len, uint64_t* dst_total, uint64_t* checksum_out, int32_t* status) {
+  return partition_compress_dev(dev_index, codec, level, codec_block_size, checksum_alg, num_partitions, n_records,
+                                rec_base, rec_bytes, rec_len, rec_part, dst_base, dst_cap, dst_off, dst_len, dst_total,
+                                checksum_out, status, nullptr);
 }
 
 // what a cached store keeps: the exchange-cache key and where to report whether it was stored
@@ -1894,13 +1933,13 @@ static int partition_compress_packed(uint32_t codec, int32_t level, uint32_t cod
                                      uint64_t rec_bytes, const uint32_t* rec_len, const uint32_t* rec_part,
                                      uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_off, uint64_t* dst_len,
                                      uint64_t* dst_total, uint64_t* checksum_out, int32_t* status,
-                                     const ExStore* store) {
+                                     const ExStore* store, const KeySpec* hash = nullptr) {
   WallTimer wt;
   t_timing = b2s_timing{};
   if (dst_total) *dst_total = 0;
   const uint32_t bs = block_size_or_default(codec_block_size);
   int rc = partition_args(codec, bs, checksum_alg, num_partitions, n_records, rec_base, rec_bytes, rec_len, rec_part,
-                          dst_base, dst_off, dst_len, status);
+                          dst_base, dst_off, dst_len, status, hash);
   if (rc) return rc;
   Device* D;
   rc = get_device(t_device, &D);
@@ -1923,14 +1962,14 @@ static int partition_compress_packed(uint32_t codec, int32_t level, uint32_t cod
   if (rec_bytes) CU(cudaMemcpyAsync(d_rec, rec_base, rec_bytes, cudaMemcpyHostToDevice, st));
   if (n_records) {
     CU(cudaMemcpyAsync(d_len, rec_len, n_records * 4, cudaMemcpyHostToDevice, st));
-    CU(cudaMemcpyAsync(d_part, rec_part, n_records * 4, cudaMemcpyHostToDevice, st));
+    if (!hash) CU(cudaMemcpyAsync(d_part, rec_part, n_records * 4, cudaMemcpyHostToDevice, st));
   }
   CU(cudaEventRecord(S.ev_h1, st));
   std::vector<uint64_t> cks(num_partitions), part_start;
   uint64_t launches = 0, arena = 0;
   rc = partition_compress_run(D, S, codec, level, bs, checksum_alg, num_partitions, n_records, d_rec, rec_bytes, d_len,
                               d_part, (uint8_t*)S.dst.p, S.dst.cap, dst_off, dst_len, cks.data(), status, &arena,
-                              &launches, store ? &part_start : nullptr);
+                              &launches, store ? &part_start : nullptr, hash);
   if (rc) return rc;
   // the device arena is sized by the bound, so a short caller arena shows up here: copy what fits, flag the rest
   int result = 0;
@@ -1954,8 +1993,8 @@ static int partition_compress_packed(uint32_t codec, int32_t level, uint32_t cod
     const uint8_t* parts = (const uint8_t*)(codec == B2S_CODEC_NONE ? S.dst.p : S.parena.p);
     *store->cached = ex_store(D->ordinal, st, store->shuffle, store->map, parts, rec_bytes, std::move(part_start));
   }
-  end_timing(wt, launches, CallBytes{rec_bytes, arena, rec_bytes + n_records * 8, fit}, &S, kH2D | kD2H);
-  partition_kernel_times(S, codec);
+  end_timing(wt, launches, CallBytes{rec_bytes, arena, rec_bytes + n_records * (hash ? 4 : 8), fit}, &S, kH2D | kD2H);
+  partition_kernel_times(S, codec, hash, n_records);
   return result;
 }
 
@@ -2372,6 +2411,28 @@ static uint64_t agg_min_row(const RecordSpec& spec) {
   return m;
 }
 
+// the key columns of rows: n_keys, the arrays, and each column's type, flags, key_len and null field
+static int key_columns_args(const RecordSpec& spec) {
+  const KeySpec& ks = spec.keys;
+  if (spec.n_keys < 1 || spec.n_keys > kMaxKeys) return fail(B2S_E_ARG, "n_keys must be in [1, 16]%s");
+  if (!spec.key_arrays) return fail(B2S_E_ARG, "null argument%s");
+  for (uint32_t c = 0; c < ks.n; c++) {
+    const uint32_t type = ks.type[c] & kKeyTypeMask, flags = ks.type[c] & ~kKeyTypeMask, key_len = ks.len[c];
+    const bool composite_type = type == kStringKey || (type >= B2S_KEY_INT16 && type <= kDecimalKey);
+    if (type > B2S_KEY_INT64 && !(spec.composite && composite_type)) return fail(B2S_E_ARG, "unknown key_type%s");
+    if (flags && (!spec.composite || (flags & ~(B2S_KEY_DESCENDING | B2S_KEY_NULLS_LAST))))
+      return fail(B2S_E_ARG, "unknown key_type flag%s");
+    if (type == B2S_KEY_BYTES && (key_len < 1 || key_len > 16))
+      return fail(B2S_E_ARG, "key_len must be in [1, 16]%s");
+    // the fixed key_len of every other type: the value's bytes, or a string's or decimal's 8-byte slot
+    static const uint32_t fixed_len[] = {0, 4, 8, 8, 0, 2, 1, 4, 8, 8};
+    if (type != B2S_KEY_BYTES && key_len != fixed_len[type])
+      return fail(B2S_E_ARG, "key_len does not match the key_type (INT8 1, INT16 2, INT32 / FLOAT32 4, else 8)%s");
+    if (ks.null_field[c] < -1) return fail(B2S_E_ARG, "null_field must be -1 or a field ordinal%s");
+  }
+  return 0;
+}
+
 static int sort_args(uint32_t codec, uint32_t alg, uint32_t n, const uint64_t* src_off, const uint64_t* src_len,
                      const uint32_t* slice_base, const uint64_t* slice_len, const uint64_t* slice_checksum,
                      const RecordSpec& spec, const void* src_base, const void* dst_base, uint64_t dst_cap,
@@ -2380,22 +2441,7 @@ static int sort_args(uint32_t codec, uint32_t alg, uint32_t n, const uint64_t* s
   if (codec > B2S_CODEC_ZSTD) return fail(B2S_E_UNSUPPORTED, "codec %s not supported by this build", "");
   const KeySpec& ks = spec.keys;
   if (spec.rows()) {
-    if (spec.n_keys < 1 || spec.n_keys > kMaxKeys) return fail(B2S_E_ARG, "n_keys must be in [1, 16]%s");
-    if (!spec.key_arrays) return fail(B2S_E_ARG, "null argument%s");
-    for (uint32_t c = 0; c < ks.n; c++) {
-      const uint32_t type = ks.type[c] & kKeyTypeMask, flags = ks.type[c] & ~kKeyTypeMask, key_len = ks.len[c];
-      const bool composite_type = type == kStringKey || (type >= B2S_KEY_INT16 && type <= kDecimalKey);
-      if (type > B2S_KEY_INT64 && !(spec.composite && composite_type)) return fail(B2S_E_ARG, "unknown key_type%s");
-      if (flags && (!spec.composite || (flags & ~(B2S_KEY_DESCENDING | B2S_KEY_NULLS_LAST))))
-        return fail(B2S_E_ARG, "unknown key_type flag%s");
-      if (type == B2S_KEY_BYTES && (key_len < 1 || key_len > 16))
-        return fail(B2S_E_ARG, "key_len must be in [1, 16]%s");
-      // the fixed key_len of every other type: the value's bytes, or a string's or decimal's 8-byte slot
-      static const uint32_t fixed_len[] = {0, 4, 8, 8, 0, 2, 1, 4, 8, 8};
-      if (type != B2S_KEY_BYTES && key_len != fixed_len[type])
-        return fail(B2S_E_ARG, "key_len does not match the key_type (INT8 1, INT16 2, INT32 / FLOAT32 4, else 8)%s");
-      if (ks.null_field[c] < -1) return fail(B2S_E_ARG, "null_field must be -1 or a field ordinal%s");
-    }
+    if (int rc = key_columns_args(spec)) return rc;
     if (spec.aggregate)
       if (int rc = agg_args(spec)) return rc;
   } else {
@@ -2418,6 +2464,64 @@ static int sort_device(uint32_t dev_index, Device** out) {
   if (!g_ctx)
     if (int rc = no_device()) return rc;
   return get_device(dev_index, out);
+}
+
+// ------------------------------------------------------------------------------------------------------------
+// write side, hash-partitioned rows: Spark's HashPartitioning id of every row, then the partition + compress step
+// ------------------------------------------------------------------------------------------------------------
+// The composite calls' column rules, then what a hash takes: no order flags, B2S_KEY_BYTES only as a 1-byte boolean.
+// With the partition step's own checks first, so that without a usable device a well-formed call reports B2S_E_CUDA
+// (as the sort calls do) and an ill-formed one B2S_E_ARG.
+static int hash_args(uint32_t codec, uint32_t codec_block_size, uint32_t alg, uint32_t R, uint64_t n,
+                     const void* rec_base, uint64_t rec_bytes, const uint32_t* rec_len, const RecordSpec& spec,
+                     const void* dst_base, const uint64_t* dst_off, const uint64_t* dst_len, const int32_t* status) {
+  const uint32_t bs = block_size_or_default(codec_block_size);
+  if (int rc = partition_args(codec, bs, alg, R, n, rec_base, rec_bytes, rec_len, nullptr, dst_base, dst_off, dst_len,
+                              status, &spec.keys))
+    return rc;
+  if (int rc = key_columns_args(spec)) return rc;
+  for (uint32_t c = 0; c < spec.keys.n; c++) {
+    if (spec.keys.type[c] & ~kKeyTypeMask) return fail(B2S_E_ARG, "a hashed key column takes no order flag%s");
+    if (spec.keys.type[c] == B2S_KEY_BYTES && spec.keys.len[c] != 1)
+      return fail(B2S_E_ARG, "a hashed B2S_KEY_BYTES column is a boolean: key_len must be 1%s");
+  }
+  if (!g_ctx)
+    if (int rc = no_device()) return rc;
+  return 0;
+}
+
+int b2s_partition_compress_rows_hash_packed(uint32_t codec, int32_t level, uint32_t codec_block_size,
+                                            uint32_t checksum_alg, uint32_t num_partitions, uint64_t n_records,
+                                            const uint8_t* rec_base, uint64_t rec_bytes, const uint32_t* rec_len,
+                                            uint32_t n_keys, const uint32_t* key_type, const uint32_t* key_off,
+                                            const uint32_t* key_len, const int32_t* key_null_field, uint8_t* dst_base,
+                                            uint64_t dst_cap, uint64_t* dst_off, uint64_t* dst_len,
+                                            uint64_t* dst_total, uint64_t* checksum_out, int32_t* status) {
+  if (dst_total) *dst_total = 0;
+  const RecordSpec spec = keys_spec(n_keys, key_type, key_off, key_len, key_null_field);
+  if (int rc = hash_args(codec, codec_block_size, checksum_alg, num_partitions, n_records, rec_base, rec_bytes, rec_len,
+                         spec, dst_base, dst_off, dst_len, status))
+    return rc;
+  return partition_compress_packed(codec, level, codec_block_size, checksum_alg, num_partitions, n_records, rec_base,
+                                   rec_bytes, rec_len, nullptr, dst_base, dst_cap, dst_off, dst_len, dst_total,
+                                   checksum_out, status, nullptr, &spec.keys);
+}
+
+int b2s_partition_compress_rows_hash_dev(uint32_t dev_index, uint32_t codec, int32_t level, uint32_t codec_block_size,
+                                         uint32_t checksum_alg, uint32_t num_partitions, uint64_t n_records,
+                                         const uint8_t* rec_base, uint64_t rec_bytes, const uint32_t* rec_len,
+                                         uint32_t n_keys, const uint32_t* key_type, const uint32_t* key_off,
+                                         const uint32_t* key_len, const int32_t* key_null_field, uint8_t* dst_base,
+                                         uint64_t dst_cap, uint64_t* dst_off, uint64_t* dst_len, uint64_t* dst_total,
+                                         uint64_t* checksum_out, int32_t* status) {
+  if (dst_total) *dst_total = 0;
+  const RecordSpec spec = keys_spec(n_keys, key_type, key_off, key_len, key_null_field);
+  if (int rc = hash_args(codec, codec_block_size, checksum_alg, num_partitions, n_records, rec_base, rec_bytes, rec_len,
+                         spec, dst_base, dst_off, dst_len, status))
+    return rc;
+  return partition_compress_dev(dev_index, codec, level, codec_block_size, checksum_alg, num_partitions, n_records,
+                                rec_base, rec_bytes, rec_len, nullptr, dst_base, dst_cap, dst_off, dst_len, dst_total,
+                                checksum_out, status, &spec.keys);
 }
 
 // The whole-task buffers of a sort call (read-lane slot 0: compressed blocks, decoded arena, sorted copy, sort

@@ -158,12 +158,14 @@ void launch_zstd_stream_meta(const uint32_t* d_blk_base, uint32_t n_streams, uin
 // of partition p, in input order, belong at part_start[p] .. (the arena offsets of the records in sorted order are in
 // sdst; idx = sorted record indices, nullptr = identity).  readback = [first record with an id >= num_partitions
 // (~0 = none), sum of rec_len, part_start[num_partitions] (~0 = no records)], readback_bytes long.
+// ids: the id array of a workspace sized with hashed ids (partition_ws_bytes(n, R, true)), else nullptr.
 struct PartitionPlan {
   uint64_t* src_off = nullptr;
   uint64_t* sdst = nullptr;
   const uint32_t* idx = nullptr;
   uint64_t* readback = nullptr;
   size_t readback_bytes = 0;
+  uint32_t* ids = nullptr;
 };
 // One stable LSD radix pass over n (key, record index) pairs (n < 2^32), digit (key >> shift) & (nd - 1), nd a power of
 // two <= 256: a per-tile histogram, one scan over the digit-major histogram, a stable scatter.  idx_in == nullptr: the
@@ -174,7 +176,17 @@ void launch_radix_pass(const uint32_t* keys_in, const uint32_t* idx_in, uint32_t
                        uint64_t* hist, uint64_t* hist_total, uint64_t* scan_ws, uint32_t* keys_out, uint32_t* idx_out,
                        cudaStream_t st, uint64_t* launches);
 uint32_t partition_radix_passes(uint32_t num_partitions);
-size_t partition_ws_bytes(uint64_t n, uint32_t num_partitions);  // d_ws of launch_partition
+// d_ws of launch_partition; hashed_ids: with room for the id array (plan->ids) behind the rest
+size_t partition_ws_bytes(uint64_t n, uint32_t num_partitions, bool hashed_ids = false);
+// launch_partition = launch_partition_offsets, then launch_partition_order over the same d_ws and plan.  Between the
+// two, src_off holds the record offsets and the readback's first word is ~0, so ids can be computed there (rows_hash).
+// offsets: the readback reset, the offsets (rec_len scanned); d_rec_part == nullptr skips the id check.
+void launch_partition_offsets(const uint32_t* d_rec_len, const uint32_t* d_rec_part, uint64_t n,
+                              uint32_t num_partitions, uint8_t* d_ws, PartitionPlan* plan, cudaStream_t st,
+                              uint64_t* launches);
+// order: the radix passes over the ids, the sorted offsets and the partition bounds
+void launch_partition_order(const uint32_t* d_rec_len, const uint32_t* d_rec_part, uint64_t n, uint32_t num_partitions,
+                            uint8_t* d_ws, PartitionPlan* plan, cudaStream_t st, uint64_t* launches);
 void launch_partition(const uint32_t* d_rec_len, const uint32_t* d_rec_part, uint64_t n, uint32_t num_partitions,
                       uint8_t* d_ws, PartitionPlan* plan, cudaStream_t st,
                       uint64_t* launches);
@@ -314,6 +326,19 @@ const uint32_t* rows_refine_heads(uint8_t* d_rws, uint64_t n, uint32_t n_ranges)
 // the emitted records to d_dst in the order idx
 void launch_rows_gather(const uint8_t* arena, uint64_t n, uint32_t key_bytes, const uint32_t* idx, uint8_t* d_ws,
                         uint8_t* d_dst, cudaStream_t st, uint64_t* launches);
+
+// ---------------- rows_hash.cu (Spark's HashPartitioning ids of length-prefixed UnsafeRow records) ----------------
+// Record i: rec_len[i] bytes at rec + rec_off[i], [size: int32 big-endian][row].  ids[i] = pmod(Murmur3Hash(key
+// columns, 42), num_partitions), the columns (ks, no order flags; B2S_KEY_BYTES is a 1-byte boolean) folded left to
+// right, a null one skipped.  A bad record takes id 0 and lowers *bad (device, ~0 = none) to (i << 3) | its reason:
+// kHashBadShort rec_len < 4, kHashBadSize the size prefix is not rec_len - 4, kHashBadKey / kHashBadNull the row does
+// not hold a key slot / a key's null word, kHashBadString a non-null string runs past the row, kHashBadDecimal a
+// non-null decimal's size is not 1..16 or it runs past the row.  Records ending past rec_bytes are not read.
+constexpr uint64_t kHashBadShort = 1, kHashBadSize = 2, kHashBadKey = 3, kHashBadNull = 4, kHashBadString = 5,
+                   kHashBadDecimal = 6;
+void launch_rows_hash(const uint8_t* rec, uint64_t rec_bytes, const uint64_t* rec_off, const uint32_t* rec_len,
+                      uint64_t n, const KeySpec& ks, uint32_t num_partitions, uint32_t* ids, uint64_t* bad,
+                      cudaStream_t st, uint64_t* launches);
 
 // ---------------- aggregate.cu (group key-sorted rows and merge their aggregate buffers) ----------------
 // Aggregate a: op[a] (B2S_AGG_*) over the 8-byte slot at row offset off[a], null bit null_field[a] (-1: never null).

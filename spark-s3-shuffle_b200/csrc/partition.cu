@@ -29,13 +29,14 @@ __device__ __forceinline__ unsigned lanemask_lt() {
 }
 
 // off[i] = rec_len[i] (scanned in place afterwards); the first record with an id >= num_partitions goes to *bad
+// (rec_part == nullptr: no ids yet, nothing checked)
 __global__ void __launch_bounds__(kPartThreads) part_prep_kernel(const uint32_t* __restrict__ rec_len,
                                                                  const uint32_t* __restrict__ rec_part, uint64_t n,
                                                                  uint32_t num_partitions, uint64_t* __restrict__ off,
                                                                  unsigned long long* __restrict__ bad) {
   for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
     off[i] = rec_len[i];
-    if (rec_part[i] >= num_partitions) atomicMin(bad, (unsigned long long)i);
+    if (rec_part && rec_part[i] >= num_partitions) atomicMin(bad, (unsigned long long)i);
   }
 }
 
@@ -218,40 +219,71 @@ void launch_radix_pass(const uint32_t* keys_in, const uint32_t* idx_in, uint32_t
   if (launches) *launches += 2;
 }
 
-size_t partition_ws_bytes(uint64_t n, uint32_t num_partitions) {
+size_t partition_ws_bytes(uint64_t n, uint32_t num_partitions, bool hashed_ids) {
   const size_t hist = radix_hist_elems(n);
   auto a = [](size_t b) { return (b + 255) / 256 * 256; };
   return a((n + 1) * 8) * 2 + a(n * 4) * 4 + a(hist * 8) + a(scan_ws_elems(std::max<size_t>(hist, n + 1)) * 8) +
-         256 + a(((size_t)num_partitions + 2) * 8) + 1024;
+         256 + a(((size_t)num_partitions + 2) * 8) + 1024 + (hashed_ids ? a(n * 4) : 0);
+}
+
+namespace {
+
+// launch_partition's workspace: the plan's arrays, the radix buffers, the histogram and its scan workspace
+struct PartitionWs {
+  uint32_t *kA, *iA, *kB, *iB;
+  uint64_t *hist, *ws, *unused_total;
+};
+
+PartitionWs carve_partition_ws(uint8_t* d_ws, uint64_t n, uint32_t num_partitions, PartitionPlan* plan) {
+  auto a = [](size_t b) { return (b + 255) / 256 * 256; };
+  const size_t hist_elems = radix_hist_elems(n);
+  PartitionWs w;
+  uint8_t* p = d_ws;
+  plan->src_off = (uint64_t*)p;  p += a((n + 1) * 8);
+  plan->sdst = (uint64_t*)p;     p += a((n + 1) * 8);
+  w.kA = (uint32_t*)p;           p += a(n * 4);
+  w.iA = (uint32_t*)p;           p += a(n * 4);
+  w.kB = (uint32_t*)p;           p += a(n * 4);
+  w.iB = (uint32_t*)p;           p += a(n * 4);
+  w.hist = (uint64_t*)p;         p += a(hist_elems * 8);
+  w.ws = (uint64_t*)p;           p += a(scan_ws_elems(std::max<size_t>(hist_elems, n + 1)) * 8);
+  w.unused_total = (uint64_t*)p; p += 256;  // grand totals of the histogram scans and of the sorted-length scan
+  // readback block: [bad, total, part_start[num_partitions]]
+  plan->readback = (uint64_t*)p;
+  plan->readback_bytes = ((size_t)num_partitions + 2) * 8;
+  p += a(plan->readback_bytes) + 1024;
+  plan->ids = (uint32_t*)p;  // only inside a workspace sized with hashed ids
+  return w;
+}
+
+}  // namespace
+
+void launch_partition_offsets(const uint32_t* d_rec_len, const uint32_t* d_rec_part, uint64_t n,
+                              uint32_t num_partitions, uint8_t* d_ws, PartitionPlan* plan, cudaStream_t st,
+                              uint64_t* launches) {
+  const PartitionWs w = carve_partition_ws(d_ws, n, num_partitions, plan);
+  uint64_t* bad = plan->readback;
+  uint64_t* total = plan->readback + 1;
+  cudaMemsetAsync(plan->readback, 0xff, plan->readback_bytes, st);
+
+  part_prep_kernel<<<grid_for(n), kPartThreads, 0, st>>>(d_rec_len, d_rec_part, n, num_partitions, plan->src_off,
+                                                         (unsigned long long*)bad);
+  launch_exclusive_scan_u64(plan->src_off, n, total, w.ws, st, launches);
 }
 
 void launch_partition(const uint32_t* d_rec_len, const uint32_t* d_rec_part, uint64_t n, uint32_t num_partitions,
                       uint8_t* d_ws, PartitionPlan* plan, cudaStream_t st,
                       uint64_t* launches) {
-  auto a = [](size_t b) { return (b + 255) / 256 * 256; };
-  const size_t hist_elems = radix_hist_elems(n);
-  uint8_t* p = d_ws;
-  plan->src_off = (uint64_t*)p;  p += a((n + 1) * 8);
-  plan->sdst = (uint64_t*)p;     p += a((n + 1) * 8);
-  uint32_t* kA = (uint32_t*)p;   p += a(n * 4);
-  uint32_t* iA = (uint32_t*)p;   p += a(n * 4);
-  uint32_t* kB = (uint32_t*)p;   p += a(n * 4);
-  uint32_t* iB = (uint32_t*)p;   p += a(n * 4);
-  uint64_t* hist = (uint64_t*)p; p += a(hist_elems * 8);
-  uint64_t* ws = (uint64_t*)p;   p += a(scan_ws_elems(std::max<size_t>(hist_elems, n + 1)) * 8);
-  uint64_t* unused_total = (uint64_t*)p;  p += 256;  // grand totals of the histogram scans and of the sorted-length scan
-  // readback block: [bad, total, part_start[num_partitions]]
-  plan->readback = (uint64_t*)p;
-  plan->readback_bytes = ((size_t)num_partitions + 2) * 8;
-  uint64_t* bad = plan->readback;
-  uint64_t* total = plan->readback + 1;
+  launch_partition_offsets(d_rec_len, d_rec_part, n, num_partitions, d_ws, plan, st, launches);
+  launch_partition_order(d_rec_len, d_rec_part, n, num_partitions, d_ws, plan, st, launches);
+}
+
+void launch_partition_order(const uint32_t* d_rec_len, const uint32_t* d_rec_part, uint64_t n, uint32_t num_partitions,
+                            uint8_t* d_ws, PartitionPlan* plan, cudaStream_t st, uint64_t* launches) {
+  const PartitionWs w = carve_partition_ws(d_ws, n, num_partitions, plan);
+  uint32_t *kA = w.kA, *iA = w.iA, *kB = w.kB, *iB = w.iB;
+  uint64_t *hist = w.hist, *ws = w.ws, *unused_total = w.unused_total;
   uint64_t* part_start = plan->readback + 2;
-  cudaMemsetAsync(plan->readback, 0xff, plan->readback_bytes, st);
-
-  part_prep_kernel<<<grid_for(n), kPartThreads, 0, st>>>(d_rec_len, d_rec_part, n, num_partitions, plan->src_off,
-                                                         (unsigned long long*)bad);
-  launch_exclusive_scan_u64(plan->src_off, n, total, ws, st, launches);
-
   const uint32_t passes = partition_radix_passes(num_partitions);
   uint32_t bits = 0;
   while (bits < 32 && (1ull << bits) < num_partitions) bits++;

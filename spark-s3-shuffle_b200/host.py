@@ -77,6 +77,7 @@ PROTOTYPES = [
     ("b2sh_reader_remote_bytes_read", _u64, [_vp]),
     ("b2sh_reader_destroy", None, [_vp]),
     ("b2sh_serialized_writer_create", C.c_int, [_vp, _i32, _i64, _i32, C.POINTER(_vp)]),
+    ("b2sh_serialized_writer_hash_rows", C.c_int, [_vp, _u32, _vp, _vp, _vp, _vp]),
     ("b2sh_serialized_writer_insert", C.c_int, [_vp, _i32, _vp, _u64]),
     ("b2sh_serialized_writer_commit", C.c_int, [_vp, _vp]),
     ("b2sh_serialized_writer_statistics", C.c_int, [_vp, C.POINTER(_u64), C.POINTER(_u64), C.c_char_p, _u32]),
@@ -283,6 +284,13 @@ class S3SerializedShuffleWriter:
         self._h = _vp()
         self.numPartitions = numPartitions
         _check(load().b2sh_serialized_writer_create(dispatcher._h, shuffleId, mapId, numPartitions, C.byref(self._h)))
+
+    def hashRows(self, keys):
+        """HashPartitioning by keys = [(key_type, key_off, key_len, null_field), ...], before the first insert: each
+        later record is one serialized row, its partitionId ignored; commit() computes Spark's ids on the GPU"""
+        keys = list(keys)
+        arrs = [np.array([k[i] for k in keys] or [0], dtype=np.int32 if i == 3 else np.uint32) for i in range(4)]
+        _check(load().b2sh_serialized_writer_hash_rows(self._h, len(keys), *[a.ctypes.data for a in arrs]))
 
     def insertRecord(self, partitionId, record):
         a = np.frombuffer(record, dtype=np.uint8) if not isinstance(record, np.ndarray) else np.ascontiguousarray(record)

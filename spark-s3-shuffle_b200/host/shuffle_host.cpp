@@ -511,12 +511,24 @@ class S3SerializedShuffleWriter {
       throw RuntimeException("Precondition: numPartitions must be in [1, 2^24].");
     if (!d.gpuEnabled) throw UnsupportedOperationException("the serialized GPU writer needs spark.shuffle.s3.gpu.enabled");
   }
+  // HashPartitioning by these key columns (b2s_partition_compress_rows_hash_packed): every later insert is one
+  // serialized row whose partitionId is ignored, and commit() computes Spark's ids on the GPU
+  void hashRows(uint32_t nKeys, const uint32_t* type, const uint32_t* off, const uint32_t* len, const int32_t* nullField) {
+    if (!recLen_.empty()) throw RuntimeException("Precondition: hash_rows must come before the first insert.");
+    if (nKeys < 1 || nKeys > 16) throw RuntimeException("Precondition: n_keys must be in [1, 16].");
+    keyType_.assign(type, type + nKeys);
+    keyOff_.assign(off, off + nKeys);
+    keyLen_.assign(len, len + nKeys);
+    keyNull_.assign(nullField, nullField + nKeys);
+  }
   void insertRecord(int32_t partitionId, const uint8_t* b, uint64_t n) {
-    if (partitionId < 0 || partitionId >= numPartitions_) throw RuntimeException("Precondition: Invalid partition id.");
+    const bool hashed = !keyType_.empty();
+    if (!hashed && (partitionId < 0 || partitionId >= numPartitions_))
+      throw RuntimeException("Precondition: Invalid partition id.");
     if (n > 0xffffffffull) throw RuntimeException("Precondition: record longer than 4 GiB.");
     records_.append(b, n);
     recLen_.push_back((uint32_t)n);
-    recPart_.push_back((uint32_t)partitionId);
+    if (!hashed) recPart_.push_back((uint32_t)partitionId);
   }
   std::vector<int64_t> commit() {
     ensure_codec_runtime();
@@ -529,7 +541,14 @@ class S3SerializedShuffleWriter {
     std::vector<int32_t> status(R);
     uint64_t total = 0;
     int rc;
-    if (d_.gpuExchangeCacheBytes) {  // the same outputs, and the partitioned records stay in HBM for local reducers
+    const char* call = "b2s_partition_compress_packed";
+    if (!keyType_.empty()) {  // hashed rows: never cached (the exchange cache's reads serve fixed-size records only)
+      call = "b2s_partition_compress_rows_hash_packed";
+      rc = b2s_partition_compress_rows_hash_packed(
+          codec, d_.zstdLevel, d_.lz4BlockSize, alg, R, recLen_.size(), records_.data(), records_.size(),
+          recLen_.data(), (uint32_t)keyType_.size(), keyType_.data(), keyOff_.data(), keyLen_.data(), keyNull_.data(),
+          out_.data(), bound, doff.data(), dlen.data(), &total, cks.data(), status.data());
+    } else if (d_.gpuExchangeCacheBytes) {  // the same outputs, and the partitioned records stay in HBM for local reducers
       d_.applyExchangeBudget();
       int32_t cached = 0;
       rc = b2s_partition_compress_cached_packed(shuffleId_, mapId_, codec, d_.zstdLevel, d_.lz4BlockSize, alg, R,
@@ -541,8 +560,7 @@ class S3SerializedShuffleWriter {
                                          records_.size(), recLen_.data(), recPart_.data(), out_.data(), bound,
                                          doff.data(), dlen.data(), &total, cks.data(), status.data());
     }
-    if (rc != 0)
-      throw CodecException(std::string("b2s_partition_compress_packed: ") + b2s_strerror(rc) + ": " + b2s_last_error());
+    if (rc != 0) throw CodecException(std::string(call) + ": " + b2s_strerror(rc) + ": " + b2s_last_error());
     std::vector<int64_t> lengths(R), checksums(R);
     for (uint32_t p = 0; p < R; p++) {
       if (status[p] != 0) throw IOException(std::string("compress failed: ") + b2s_strerror(status[p]));
@@ -561,6 +579,8 @@ class S3SerializedShuffleWriter {
   int32_t numPartitions_;
   PinnedArena records_, out_;
   std::vector<uint32_t> recLen_, recPart_;
+  std::vector<uint32_t> keyType_, keyOff_, keyLen_;  // hashRows' key columns (empty: the caller's partition ids)
+  std::vector<int32_t> keyNull_;
   std::unique_ptr<S3MeasureOutputStream> measure_;
 };
 
@@ -1258,6 +1278,10 @@ int b2sh_serialized_writer_create(b2sh_dispatcher* d, int32_t shuffle_id, int64_
   return guarded([&] {
     *out = new b2sh_serialized_writer{std::make_unique<S3SerializedShuffleWriter>(*d->d, shuffle_id, map_id, num_partitions)};
   });
+}
+int b2sh_serialized_writer_hash_rows(b2sh_serialized_writer* w, uint32_t n_keys, const uint32_t* key_type,
+                                     const uint32_t* key_off, const uint32_t* key_len, const int32_t* key_null_field) {
+  return guarded([&] { w->w->hashRows(n_keys, key_type, key_off, key_len, key_null_field); });
 }
 int b2sh_serialized_writer_insert(b2sh_serialized_writer* w, int32_t partition_id, const uint8_t* bytes, uint64_t len) {
   return guarded([&] { w->w->insertRecord(partition_id, bytes, len); });
