@@ -35,6 +35,9 @@ namespace {
 
 thread_local std::string t_last_error;
 thread_local b2s_timing t_timing;
+// the timed call this thread is running (begin_call): marks and dominant pairs another call recorded are never read
+thread_local uint64_t t_call = 0;
+std::atomic<uint64_t> g_calls{0};
 thread_local uint32_t t_device = 0;  // device (index into the b2s_init selection) used by this thread's host-pointer calls
 
 int fail(int code, const char* fmt, const char* a = "") {
@@ -221,26 +224,41 @@ struct Carver {
   }
 };
 
+double ms_between(cudaEvent_t a, cudaEvent_t b) {
+  float ms = 0;
+  if (cudaEventElapsedTime(&ms, a, b) != cudaSuccess) {
+    (void)cudaGetLastError();  // unrecorded event: not an error of the call being timed
+    return 0;
+  }
+  return ms;
+}
+
+// The timed marks of a slot's main stream, which b2s_last_timing is read from (add_times): kernel region (K), codec
+// step (T), upload (H), download (D), partition or sort step (P), row framing: walk + count, emit (F0-F1, F2-F3; the
+// hash step of a hash partition: F0-F1), grouping + merge of an aggregation (G).  Stop: where a call that did not
+// record the end of a span it reads stopped.
+enum Mark { K0, K1, T0, T1, H0, H1, D0, D1, P0, P1, F0, F1, F2, F3, G0, G1, kStop, kMarks };
+
 struct Slot {
   cudaStream_t st = nullptr;
   cudaStream_t st2 = nullptr;                               // side stream: match kernels of chunk k+1 overlap parse/emit of chunk k
   cudaEvent_t ev_fork = nullptr, ev_match[2] = {nullptr, nullptr}, ev_free[2] = {nullptr, nullptr};
   cudaEvent_t ev_a = nullptr, ev_b = nullptr;              // readback milestones
-  cudaEvent_t ev_k0 = nullptr, ev_k1 = nullptr;            // kernel region
-  cudaEvent_t ev_t0 = nullptr, ev_t1 = nullptr;            // dominant kernel
-  cudaEvent_t ev_h0 = nullptr, ev_h1 = nullptr, ev_d0 = nullptr, ev_d1 = nullptr;  // copies
-  cudaEvent_t ev_p0 = nullptr, ev_p1 = nullptr;            // partition step (b2s_partition_compress_*)
-  cudaEvent_t ev_f[4] = {nullptr, nullptr, nullptr, nullptr};  // row framing: walk + count, emit (sort_rows)
-  cudaEvent_t ev_g[2] = {nullptr, nullptr};                    // grouping + merge (aggregate_rows)
+  cudaEvent_t ev_mark[kMarks] = {};
+  uint64_t mark_call[kMarks] = {};      // the call (t_call) that last recorded each mark
+  uint64_t mark_launches[kMarks] = {};  // the call's launch count at the mark, where the step passed it
   DevBuf meta, scratch, desc, src, dst, zmeta;
   DevBuf pws, parena;  // partition workspace (sort keys, offsets) and the partitioned arena in front of compression
   DevBuf xpieces;      // the copy pieces of an exchange-cache read (exchange.cu)
   DevBuf fws;          // row framing workspace: bitmap over the decoded arena, tile counts, verdicts (rows.cu)
   PinBuf hmeta;
-  // per-launch event pairs around the dominant kernel of a call (grow-only pool; `used` pairs are valid)
+  // per-launch event pairs around the dominant kernel of a call (grow-only pool; dom_used pairs of call dom_call)
   std::vector<cudaEvent_t> ev_dom;
   size_t dom_used = 0;
+  uint64_t dom_call = 0;
   int dom_pair(cudaEvent_t* a, cudaEvent_t* b) {
+    if (dom_call != t_call) dom_used = 0;  // what another call left is not this call's
+    dom_call = t_call;
     if (dom_used * 2 + 2 > ev_dom.size()) {
       cudaEvent_t x = nullptr, y = nullptr;
       if (cudaEventCreate(&x) != cudaSuccess || cudaEventCreate(&y) != cudaSuccess) return -1;
@@ -252,12 +270,38 @@ struct Slot {
     dom_used++;
     return 0;
   }
+  // adds this call's dominant pairs to b2s_last_timing and empties the pool
+  void take_pairs() {
+    const size_t n = dom_call == t_call ? dom_used : 0;
+    for (size_t k = 0; k < n; k++) t_timing.dominant_ms += ms_between(ev_dom[2 * k], ev_dom[2 * k + 1]);
+    t_timing.dominant_launches += n;
+    dom_used = 0;
+  }
+  cudaError_t mark(Mark m, cudaStream_t s, uint64_t launches = 0) {
+    mark_call[m] = t_call;
+    mark_launches[m] = launches;
+    return cudaEventRecord(ev_mark[m], s);
+  }
+  bool mine(Mark m) const { return mark_call[m] == t_call; }
+  // this call's ms from a to b: 0 when the call did not record a; up to where the call stopped when it did not record b
+  // (the stop mark, recorded and waited for once)
+  double span(Mark a, Mark b) {
+    if (!mine(a)) return 0;
+    if (!mine(b)) {
+      if (!mine(kStop) && (mark(kStop, st) != cudaSuccess || cudaEventSynchronize(ev_mark[kStop]) != cudaSuccess)) {
+        (void)cudaGetLastError();  // the call's work is done: an unreadable time is 0, not a failure
+        return 0;
+      }
+      b = kStop;
+    }
+    return ms_between(ev_mark[a], ev_mark[b]);
+  }
   // the fixed events, created by create() and destroyed by release(); the first kUntimed only order the two streams
   static constexpr int kUntimed = 5;
-  std::array<cudaEvent_t*, 23> events() {
-    return {&ev_fork, &ev_match[0], &ev_match[1], &ev_free[0], &ev_free[1], &ev_a,    &ev_b,    &ev_k0,
-            &ev_k1,   &ev_t0,       &ev_t1,       &ev_h0,      &ev_h1,      &ev_d0,   &ev_d1,   &ev_p0,
-            &ev_p1,   &ev_f[0],     &ev_f[1],     &ev_f[2],    &ev_f[3],    &ev_g[0], &ev_g[1]};
+  std::array<cudaEvent_t*, 7 + kMarks> events() {
+    std::array<cudaEvent_t*, 7 + kMarks> e{&ev_fork, &ev_match[0], &ev_match[1], &ev_free[0], &ev_free[1], &ev_a, &ev_b};
+    for (int m = 0; m < kMarks; m++) e[7 + m] = &ev_mark[m];
+    return e;
   }
   int create(int prio) {
     CU(cudaStreamCreateWithPriority(&st, cudaStreamNonBlocking, prio));
@@ -330,19 +374,17 @@ uint32_t pick_tile_shift(uint64_t total_bytes) {
   return s;
 }
 
-double ms_between(cudaEvent_t a, cudaEvent_t b) {
-  float ms = 0;
-  if (cudaEventElapsedTime(&ms, a, b) != cudaSuccess) {
-    (void)cudaGetLastError();  // unrecorded event: not an error of the call being timed
-    return 0;
-  }
-  return ms;
-}
-
 struct WallTimer {
   std::chrono::steady_clock::time_point t0 = std::chrono::steady_clock::now();
   double ms() const { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count(); }
 };
+
+// Starts a timed call: a new call id, an empty b2s_last_timing and the wall clock
+WallTimer begin_call() {
+  t_call = ++g_calls;
+  t_timing = b2s_timing{};
+  return WallTimer{};
+}
 
 // --------------------------------------------------------------------------------------------------------------
 // compress job: one chunk of n streams living in a device source arena
@@ -483,8 +525,8 @@ int compress_chunk(Slot& S, const ChecksumTables& tabs, uint32_t codec, int32_t 
   cudaStream_t st = S.st;
   CU(cudaMemcpyAsync(M.up, J.h.up, M.up_bytes, cudaMemcpyHostToDevice, st));
   CU(cudaMemsetAsync(M.down, 0, M.down_bytes, st));
-  CU(cudaEventRecord(S.ev_k0, st));
-  CU(cudaEventRecord(S.ev_t0, st));
+  CU(S.mark(K0, st));
+  CU(S.mark(T0, st));
   // Match kernels (issue bound, shared-memory limited) on the side stream, parse (latency bound), scan and emit on st.
   // The side stream forks BEFORE the per-block XXH32 pass (LZ4Block headers; only the emit kernel needs it), so that
   // pass runs beside the first group's match kernel instead of in front of it.
@@ -504,7 +546,7 @@ int compress_chunk(Slot& S, const ChecksumTables& tabs, uint32_t codec, int32_t 
     return 0;
   };
   if (int r = run_block_groups(S, nb, chunk, (uint8_t*)S.scratch.p, ws_bytes, match, parse_emit)) return r;
-  CU(cudaEventRecord(S.ev_t1, st));
+  CU(S.mark(T1, st));
   if (codec == B2S_CODEC_ZSTD)
     launch_zstd_stream_meta(M.blk_base, n, nb, M.sizes, M.total, d_dst, dst_cap, M.dst_off, M.dst_len, M.status, st,
                             launches);
@@ -518,7 +560,7 @@ int compress_chunk(Slot& S, const ChecksumTables& tabs, uint32_t codec, int32_t 
     uint32_t shift = pick_tile_shift(dst_cap < (uint64_t)nb * bs ? dst_cap : (uint64_t)nb * bs);
     launch_checksum(tabs, alg, d_dst, M.dst_off, M.dst_len, n, shift, M.work_base, M.ws, M.cks, st, launches);
   }
-  CU(cudaEventRecord(S.ev_k1, st));
+  CU(S.mark(K1, st));
   CU(cudaMemcpyAsync(J.h.down, M.down, M.down_bytes, cudaMemcpyDeviceToHost, st));
   CU(cudaEventRecord(S.ev_a, st));
   CU(cudaGetLastError());
@@ -639,7 +681,7 @@ int decompress_phase_a(Slot& S, const ChecksumTables& tabs, uint32_t codec, uint
   CU(cudaMemcpyAsync(M.up, H.up, M.up_bytes, cudaMemcpyHostToDevice, st));
   CU(cudaMemsetAsync(M.down, 0, M.down_bytes, st));
   CU(cudaMemsetAsync(M.bad, 0xff, (size_t)n * 4, st));
-  CU(cudaEventRecord(S.ev_k0, st));
+  CU(S.mark(K0, st));
   if (alg != B2S_CHECKSUM_NONE && s) {
     launch_checksum(tabs, alg, d_src, M.slice_off, M.slice_len, s, pick_tile_shift(src_bytes), M.work_base, M.ws,
                     M.cks_got, st, launches);
@@ -698,11 +740,11 @@ int decompress_enqueue_b(Slot& S, DecompressJob& J, const uint8_t* d_src, uint8_
   J.total_out = J.h.totals[1];
   if (J.codec == B2S_CODEC_ZSTD) {
     cudaStream_t zst = S.st;
-    CU(cudaEventRecord(S.ev_t0, zst));
+    CU(S.mark(T0, zst));
     launch_zstd_execute(d_src, S.desc.p, J.zcnt, J.zbase, J.n, (const uint8_t*)S.scratch.p, J.zlit, J.znseq, J.d.dst_len,
                         d_dst, J.d.dst_off, dst_cap, J.d.status, zst, launches);
-    CU(cudaEventRecord(S.ev_t1, zst));
-    CU(cudaEventRecord(S.ev_k1, zst));
+    CU(S.mark(T1, zst));
+    CU(S.mark(K1, zst));
     CU(cudaMemcpyAsync(J.h.down, J.d.down, J.d.down_bytes, cudaMemcpyDeviceToHost, zst));
     CU(cudaEventRecord(S.ev_b, zst));
     CU(cudaGetLastError());
@@ -720,7 +762,7 @@ int decompress_enqueue_b(Slot& S, DecompressJob& J, const uint8_t* d_src, uint8_
   else
     launch_lz4block_fill(d_src, J.d.src_off, J.d.src_len, J.n, J.d.nblk, J.d.dst_off, J.d.dst_len, dst_cap, J.d.status, desc, st,
                          launches);
-  CU(cudaEventRecord(S.ev_t0, st));
+  CU(S.mark(T0, st));
   if (J.nb && J.codec == B2S_CODEC_LZ4BLOCK) {
     // one launch over every codec block: warp per block, parse and copies together (lz4_decode.cu)
     cudaEvent_t e0 = nullptr, e1 = nullptr;
@@ -757,13 +799,13 @@ int decompress_enqueue_b(Slot& S, DecompressJob& J, const uint8_t* d_src, uint8_
     };
     if (int r = run_block_groups(S, nb, chunk, (uint8_t*)S.scratch.p + nrec_bytes, ws_bytes, tokens, copy)) return r;
   }
-  CU(cudaEventRecord(S.ev_t1, st));
+  CU(S.mark(T1, st));
   // One XXH32 pass over all decoded blocks after the last chunk.  Queueing it chunk by chunk on the side stream (beside
   // the next chunk's copy kernel) was measured slower: both kernels are
   // memory-latency bound and take each other's L2 / DRAM queue slots.
   if (J.codec == B2S_CODEC_LZ4BLOCK)
     launch_xxh32_verify(desc, (uint32_t)J.nb, d_dst, kXxhSeed, 0x0FFFFFFFu, J.d.status, st, launches);
-  CU(cudaEventRecord(S.ev_k1, st));
+  CU(S.mark(K1, st));
   CU(cudaMemcpyAsync(J.h.down, J.d.down, J.d.down_bytes, cudaMemcpyDeviceToHost, st));
   CU(cudaEventRecord(S.ev_b, st));
   CU(cudaGetLastError());
@@ -779,31 +821,61 @@ int get_device(uint32_t dev_index, Device** out) {
   return 0;
 }
 
-void add_timing(Slot& S, bool copies) {
-  t_timing.kernel_ms += ms_between(S.ev_k0, S.ev_k1);
-  t_timing.top_kernel_ms += ms_between(S.ev_t0, S.ev_t1);
-  for (size_t k = 0; k < S.dom_used; k++) {
-    t_timing.dominant_ms += ms_between(S.ev_dom[2 * k], S.ev_dom[2 * k + 1]);
-    t_timing.dominant_launches++;
+// the kinds of call whose steps add_times reads into b2s_last_timing, one rule each
+enum class Family { kCodec, kPartition, kPartitionNone, kSort, kSortRows, kAggregate };
+
+// Adds the times of this call's steps on S to b2s_last_timing: kernel_ms, top_kernel_ms, dominant_ms / _launches by
+// the rule of its family, and h2d_ms.  A step the call did not run reads 0; one it started but did not finish ends
+// where the call stopped (Slot::span).  d2h_ms is read once the payload copy has run (end_call, retire_slot).
+void add_times(Slot& S, Family f) {
+  b2s_timing& t = t_timing;
+  auto dominant = [&](Mark a, Mark b) {  // a dominant step and the launches in it (the step passed its launch count)
+    t.dominant_ms += S.span(a, b);
+    t.dominant_launches += S.mine(a) && S.mine(b) ? S.mark_launches[b] - S.mark_launches[a] : 0;
+  };
+  switch (f) {
+    case Family::kCodec:  // checksum, compress, decompress, exchange read, and each chunk of a pipelined call: the
+                          // kernel region; the codec step; the dominant pairs (match, LZ4 decode, Snappy copy)
+      t.kernel_ms += S.span(K0, K1);
+      t.top_kernel_ms += S.span(T0, T1);
+      S.take_pairs();
+      break;
+    case Family::kPartition:      // partition step + compression; the codec step; the match launches
+    case Family::kPartitionNone:  // partition step + checksum (without one, the gather); the partition step
+      t.kernel_ms += S.span(P0, f == Family::kPartitionNone && !S.mine(K1) ? P1 : K1);
+      t.top_kernel_ms += f == Family::kPartition ? S.span(T0, T1) : S.span(P0, P1);
+      if (S.mine(F0)) dominant(F0, F1);  // a hash partition: the hash step
+      else S.take_pairs();
+      break;
+    case Family::kSort:       // verification + decode + sort; the sort step; the decoder's dominant pairs
+    case Family::kSortRows:   // the same; framing + order + gather; the framing (walk + count, emit)
+    case Family::kAggregate:  // the same; framing through merge; grouping + merge
+      t.kernel_ms += S.span(K0, P1);
+      t.top_kernel_ms += S.span(P0, P1);
+      if (f == Family::kSort) S.take_pairs();
+      if (f == Family::kSortRows) {
+        dominant(F0, F1);
+        dominant(F2, F3);
+      }
+      if (f == Family::kAggregate) dominant(G0, G1);
+      break;
   }
-  S.dom_used = 0;
-  if (copies) t_timing.h2d_ms += ms_between(S.ev_h0, S.ev_h1);  // d2h is added once the payload copy has run
+  t.h2d_ms += S.span(H0, H1);
 }
 
 // what a call moved: bytes into and out of its kernels, and over PCIe
 struct CallBytes {
   uint64_t src = 0, dst = 0, h2d = 0, d2h = 0;
 };
-constexpr int kH2D = 1, kD2H = 2;
 
 // Ends a successful call's b2s_last_timing: its bytes, its launches (also counted for the process) and its wall time.
-// S: the one slot the call ran on, whose kernel events are read, and its copy events where the call recorded them
-// (copies: kH2D | kD2H); nullptr for a call pipelined over slots, whose chunks added their own times (add_timing).
-void end_timing(const WallTimer& wt, uint64_t launches, const CallBytes& b, Slot* S = nullptr, int copies = 0) {
+// S: the one slot the call ran on, whose steps give the times (add_times); nullptr for a call pipelined over slots,
+// whose chunks added their own times.
+void end_call(const WallTimer& wt, uint64_t launches, const CallBytes& b, Slot* S = nullptr,
+              Family f = Family::kCodec) {
   if (S) {
-    add_timing(*S, false);
-    if (copies & kH2D) t_timing.h2d_ms = ms_between(S->ev_h0, S->ev_h1);
-    if (copies & kD2H) t_timing.d2h_ms = ms_between(S->ev_d0, S->ev_d1);
+    add_times(*S, f);
+    t_timing.d2h_ms += S->span(D0, D1);
   }
   t_timing.src_bytes += b.src;
   t_timing.dst_bytes += b.dst;
@@ -817,7 +889,7 @@ void end_timing(const WallTimer& wt, uint64_t launches, const CallBytes& b, Slot
 // run_chunks' retire: the slot's stream has drained, the payload download of its last chunk included
 int retire_slot(Slot& S, bool used) {
   CU(cudaStreamSynchronize(S.st));
-  if (used) t_timing.d2h_ms += ms_between(S.ev_d0, S.ev_d1);
+  if (used) t_timing.d2h_ms += S.span(D0, D1);
   return 0;
 }
 
@@ -851,27 +923,27 @@ uint64_t plan_runs(uint32_t cnt, const uint8_t* const* ptr, const uint64_t* len,
 }
 
 // Stages the cnt sources of a chunk in S.src: dev_off[i] receives where source i sits, the return value the arena's
-// bytes (what the chunk uploads).  The copies run between ev_h0 and ev_h1.
+// bytes (what the chunk uploads).  The copies run between marks H0 and H1.
 int upload_chunk(Slot& S, uint32_t cnt, const uint8_t* const* ptr, const uint64_t* len, uint64_t* dev_off,
                  std::vector<Run>& runs, uint64_t* bytes) {
   *bytes = plan_runs(cnt, ptr, len, dev_off, runs);
   if (int rc = S.src.ensure(*bytes + 64)) return rc;
-  CU(cudaEventRecord(S.ev_h0, S.st));
+  CU(S.mark(H0, S.st));
   for (const Run& r : runs)
     CU(cudaMemcpyAsync((uint8_t*)S.src.p + r.dev_off, r.host, r.bytes, cudaMemcpyHostToDevice, S.st));
-  CU(cudaEventRecord(S.ev_h1, S.st));
+  CU(S.mark(H1, S.st));
   return 0;
 }
 
 // Copies a finished chunk of n streams (stream k: len[k] bytes at off[k] of S.dst, chunk_total bytes in all) to the
-// host between ev_d0 and ev_d1, and adds what it copied to d2h_bytes.  packed_dst: the whole chunk at run_off of that
+// host between marks D0 and D1, and adds what it copied to d2h_bytes.  packed_dst: the whole chunk at run_off of that
 // arena, as much of it as fits in packed_cap, and every stream still OK that does not fit entirely gets
 // B2S_E_DST_TOO_SMALL.  dst: stream k of an OK status to dst[k], or B2S_E_DST_TOO_SMALL when it exceeds dst_cap[k].
 // Neither: nothing is copied.
 int download_chunk(Slot& S, uint32_t n, const uint64_t* off, const uint64_t* len, uint64_t chunk_total,
                    uint8_t* packed_dst, uint64_t packed_cap, uint64_t run_off, uint8_t* const* dst,
                    const uint64_t* dst_cap, int32_t* status) {
-  CU(cudaEventRecord(S.ev_d0, S.st));
+  CU(S.mark(D0, S.st));
   if (packed_dst) {
     uint64_t fit = chunk_total;
     if (run_off + chunk_total > packed_cap) {
@@ -893,7 +965,7 @@ int download_chunk(Slot& S, uint32_t n, const uint64_t* off, const uint64_t* len
       t_timing.d2h_bytes += len[k];
     }
   }
-  CU(cudaEventRecord(S.ev_d1, S.st));
+  CU(S.mark(D1, S.st));
   return 0;
 }
 
@@ -1417,12 +1489,12 @@ static int checksum_chunk_dev(Device* D, Slot& S, uint32_t alg, uint32_t n, cons
   memcpy(h_len, len, (size_t)n * 8);
   cudaStream_t st = S.st;
   CU(cudaMemcpyAsync(d_off, h_off, up, cudaMemcpyHostToDevice, st));
-  CU(cudaEventRecord(S.ev_k0, st));
-  CU(cudaEventRecord(S.ev_t0, st));
+  CU(S.mark(K0, st));
+  CU(S.mark(T0, st));
   launch_checksum(D->tabs, alg, d_base, d_off, d_len, n, pick_tile_shift(total_bytes), d_work, d_ws, d_out, st,
                   launches);
-  CU(cudaEventRecord(S.ev_t1, st));
-  CU(cudaEventRecord(S.ev_k1, st));
+  CU(S.mark(T1, st));
+  CU(S.mark(K1, st));
   CU(cudaMemcpyAsync(h_out, d_out, (size_t)n * 8, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
   CU(cudaGetLastError());
@@ -1432,8 +1504,7 @@ static int checksum_chunk_dev(Device* D, Slot& S, uint32_t alg, uint32_t n, cons
 
 int b2s_checksum_dev(uint32_t dev_index, uint32_t alg, uint32_t n, const void* d_base, const uint64_t* off,
                      const uint64_t* len, uint64_t* out) {
-  WallTimer wt;
-  t_timing = b2s_timing{};
+  const WallTimer wt = begin_call();
   Device* D;
   int rc = get_device(dev_index, &D);
   if (rc) return rc;
@@ -1444,13 +1515,12 @@ int b2s_checksum_dev(uint32_t dev_index, uint32_t alg, uint32_t n, const void* d
   for (uint32_t i = 0; i < n; i++) total += len[i];
   rc = checksum_chunk_dev(D, Ln.slot[0], alg, n, (const uint8_t*)d_base, off, len, out, total, &launches);
   if (rc) return rc;
-  end_timing(wt, launches, CallBytes{total, 0, 0, 0}, &Ln.slot[0]);
+  end_call(wt, launches, CallBytes{total, 0, 0, 0}, &Ln.slot[0]);
   return 0;
 }
 
 static int checksum_host(uint32_t alg, uint32_t n, const uint8_t* const* ptr, const uint64_t* len, uint64_t* out) {
-  WallTimer wt;
-  t_timing = b2s_timing{};
+  const WallTimer wt = begin_call();
   Device* D;
   int rc = get_device(t_device, &D);
   if (rc) return rc;
@@ -1470,12 +1540,12 @@ static int checksum_host(uint32_t alg, uint32_t n, const uint8_t* const* ptr, co
     rc = checksum_chunk_dev(D, S, alg, cnt, (const uint8_t*)S.src.p, dev_off.data(), len + i0, out + i0, bytes,
                             &launches);
     if (rc) return rc;
-    add_timing(S, true);
+    add_times(S, Family::kCodec);
     t_timing.h2d_bytes += bytes;
     t_timing.d2h_bytes += (uint64_t)cnt * 8;
     t_timing.src_bytes += bytes;
   }
-  end_timing(wt, launches, CallBytes{});
+  end_call(wt, launches, CallBytes{});
   return 0;
 }
 
@@ -1512,8 +1582,7 @@ int b2s_compress_dev(uint32_t dev_index, uint32_t codec, int32_t level, uint32_t
                      uint32_t checksum_alg, uint32_t n, const void* d_src_base, const uint64_t* src_off,
                      const uint64_t* src_len, void* d_dst_base, uint64_t dst_cap, uint64_t* dst_off,
                      uint64_t* dst_len, uint64_t* dst_total, uint64_t* checksum_out, int32_t* status) {
-  WallTimer wt;
-  t_timing = b2s_timing{};
+  const WallTimer wt = begin_call();
   Device* D;
   int rc = get_device(dev_index, &D);
   if (rc) return rc;
@@ -1541,7 +1610,7 @@ int b2s_compress_dev(uint32_t dev_index, uint32_t codec, int32_t level, uint32_t
   uint64_t total = J.h.total[0] + stream_overhead(codec) * n, srcb = 0;
   for (uint32_t i = 0; i < n; i++) srcb += src_len[i];
   if (dst_total) *dst_total = total;
-  end_timing(wt, launches, CallBytes{srcb, total, 0, 0}, &S);
+  end_call(wt, launches, CallBytes{srcb, total, 0, 0}, &S);
   return 0;
 }
 
@@ -1550,8 +1619,7 @@ static int compress_host(uint32_t codec, int32_t level, uint32_t codec_block_siz
                          const uint8_t* const* src, const uint64_t* src_len, uint8_t* packed_dst, uint64_t packed_cap,
                          uint8_t* const* dst, const uint64_t* dst_cap, uint64_t* dst_off, uint64_t* dst_len,
                          uint64_t* dst_total, uint64_t* checksum_out, int32_t* status) {
-  WallTimer wt;
-  t_timing = b2s_timing{};
+  const WallTimer wt = begin_call();
   Device* D;
   int rc = get_device(t_device, &D);
   if (rc) return rc;
@@ -1582,7 +1650,7 @@ static int compress_host(uint32_t codec, int32_t level, uint32_t codec_block_siz
   auto finish = [&](Slot& S, size_t c, uint32_t i0, uint32_t cnt) -> int {
     const CompressLayout& H = jobs[c].h;
     CU(cudaEventSynchronize(S.ev_a));
-    add_timing(S, true);
+    add_times(S, Family::kCodec);
     const uint64_t chunk_total = H.total[0] + stream_overhead(codec) * cnt;
     for (uint32_t k = 0; k < cnt; k++) {
       status[i0 + k] = H.status[k];
@@ -1602,7 +1670,7 @@ static int compress_host(uint32_t codec, int32_t level, uint32_t codec_block_siz
     return r;
   CU(cudaGetLastError());
   if (dst_total) *dst_total = run_off;
-  end_timing(wt, launches, CallBytes{});
+  end_call(wt, launches, CallBytes{});
   return 0;
 }
 
@@ -1698,8 +1766,8 @@ static uint64_t first_record_past(const uint64_t* d_off, const uint32_t* d_len, 
 // .data arena (dst_cap bytes); *arena_bytes the bytes it needs.  Returns B2S_E_DST_TOO_SMALL (status[] set for the
 // partitions that do not fit) when dst_cap is short.  part_start (optional) receives the R + 1 partition offsets of the
 // partitioned records, which are in d_dst (codec NONE) or S.parena.  hash (d_part unused): the ids are Spark's
-// HashPartitioning ids of the rows by these key columns, computed between the offsets and the radix passes (S.ev_f[0]
-// and S.ev_f[1] bracket that step), and a bad record fails the call.
+// HashPartitioning ids of the rows by these key columns, computed between the offsets and the radix passes (marks F0
+// and F1 bracket that step), and a bad record fails the call.
 static int partition_compress_run(Device* D, Slot& S, uint32_t codec, int32_t level, uint32_t bs, uint32_t alg,
                                   uint32_t R, uint64_t n, const uint8_t* d_rec, uint64_t rec_bytes,
                                   const uint32_t* d_len, const uint32_t* d_part, uint8_t* d_dst, uint64_t dst_cap,
@@ -1708,8 +1776,7 @@ static int partition_compress_run(Device* D, Slot& S, uint32_t codec, int32_t le
                                   std::vector<uint64_t>* part_start = nullptr, const KeySpec* hash = nullptr) {
   cudaStream_t st = S.st;
   std::vector<uint64_t> pstart(R), plen(R);
-  CU(cudaEventRecord(S.ev_p0, st));
-  CU(cudaEventRecord(S.ev_k0, st));
+  CU(S.mark(P0, st));
   PartitionPlan P;
   if (n) {
     int rc = S.pws.ensure(partition_ws_bytes(n, R, hash != nullptr));
@@ -1717,9 +1784,9 @@ static int partition_compress_run(Device* D, Slot& S, uint32_t codec, int32_t le
     uint8_t* ws = (uint8_t*)S.pws.p;
     if (hash) {
       launch_partition_offsets(d_len, nullptr, n, R, ws, &P, st, launches);
-      CU(cudaEventRecord(S.ev_f[0], st));
+      CU(S.mark(F0, st, *launches));
       launch_rows_hash(d_rec, rec_bytes, P.src_off, d_len, n, *hash, R, P.ids, P.readback, st, launches);
-      CU(cudaEventRecord(S.ev_f[1], st));
+      CU(S.mark(F1, st, *launches));
       launch_partition_order(d_len, P.ids, n, R, ws, &P, st, launches);
     } else {
       launch_partition(d_len, d_part, n, R, ws, &P, st, launches);
@@ -1782,12 +1849,11 @@ static int partition_compress_run(Device* D, Slot& S, uint32_t codec, int32_t le
       return fail(B2S_E_DST_TOO_SMALL, "dst_cap is below the %s bytes of records", std::to_string(rec_bytes).c_str());
     }
     launch_partition_gather(d_rec, d_len, n, P, d_dst, st, launches);
-    CU(cudaEventRecord(S.ev_p1, st));
+    CU(S.mark(P1, st));
     if (alg && rec_bytes) {  // over every partition, empty ones included
       int rc = checksum_chunk_dev(D, S, alg, R, d_dst, pstart.data(), plen.data(), checksum_out, rec_bytes, launches);
       if (rc) return rc;
     } else {
-      CU(cudaEventRecord(S.ev_k1, st));
       CU(cudaStreamSynchronize(st));
       for (uint32_t p = 0; p < R; p++) checksum_out[p] = alg ? empty_checksum(alg) : 0;
     }
@@ -1812,20 +1878,13 @@ static int partition_compress_run(Device* D, Slot& S, uint32_t codec, int32_t le
     int rc = S.parena.ensure(rec_bytes + 64);
     if (rc) return rc;
     launch_partition_gather(d_rec, d_len, n, P, (uint8_t*)S.parena.p, st, launches);
-    CU(cudaEventRecord(S.ev_p1, st));
+    CU(S.mark(P1, st));
     rc = compress_chunk(S, D->tabs, codec, level, bs, alg, m, ne_off.data(), ne_len.data(),
                         (const uint8_t*)S.parena.p, d_dst, dst_cap, J, launches);
     if (rc) return rc;
     CU(cudaEventSynchronize(S.ev_a));
     CU(cudaGetLastError());
     total = J.h.total[0] + stream_overhead(codec) * m;
-  } else {
-    CU(cudaEventRecord(S.ev_p1, st));
-    CU(cudaEventRecord(S.ev_k0, st));
-    CU(cudaEventRecord(S.ev_t0, st));
-    CU(cudaEventRecord(S.ev_t1, st));
-    CU(cudaEventRecord(S.ev_k1, st));
-    CU(cudaStreamSynchronize(st));
   }
   *arena_bytes = total;
   bool short_dst = false;
@@ -1868,15 +1927,8 @@ static int partition_args(uint32_t codec, uint32_t bs, uint32_t alg, uint32_t R,
   return 0;
 }
 
-// kernel_ms: partition step + compression; top_kernel_ms: the codec step, or the partition step for codec NONE.
-// hash: dominant_ms / dominant_launches = the hash step alone.
-static void partition_kernel_times(Slot& S, uint32_t codec, const KeySpec* hash, uint64_t n) {
-  t_timing.kernel_ms = ms_between(S.ev_p0, S.ev_k1);
-  if (codec == B2S_CODEC_NONE) t_timing.top_kernel_ms = ms_between(S.ev_p0, S.ev_p1);
-  if (hash) {
-    t_timing.dominant_ms = n ? ms_between(S.ev_f[0], S.ev_f[1]) : 0;
-    t_timing.dominant_launches = n ? 1 : 0;
-  }
+static Family partition_family(uint32_t codec) {
+  return codec == B2S_CODEC_NONE ? Family::kPartitionNone : Family::kPartition;
 }
 
 static int partition_compress_dev(uint32_t dev_index, uint32_t codec, int32_t level, uint32_t codec_block_size,
@@ -1885,8 +1937,7 @@ static int partition_compress_dev(uint32_t dev_index, uint32_t codec, int32_t le
                                   const uint32_t* rec_part, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_off,
                                   uint64_t* dst_len, uint64_t* dst_total, uint64_t* checksum_out, int32_t* status,
                                   const KeySpec* hash) {
-  WallTimer wt;
-  t_timing = b2s_timing{};
+  const WallTimer wt = begin_call();
   if (dst_total) *dst_total = 0;
   const uint32_t bs = block_size_or_default(codec_block_size);
   int rc = partition_args(codec, bs, checksum_alg, num_partitions, n_records, rec_base, rec_bytes, rec_len, rec_part,
@@ -1906,8 +1957,7 @@ static int partition_compress_dev(uint32_t dev_index, uint32_t codec, int32_t le
   if (rc && rc != B2S_E_DST_TOO_SMALL) return rc;
   if (checksum_out) memcpy(checksum_out, cks.data(), (size_t)num_partitions * 8);
   if (dst_total) *dst_total = arena;
-  end_timing(wt, launches, CallBytes{rec_bytes, arena, 0, 0}, &S);
-  partition_kernel_times(S, codec, hash, n_records);
+  end_call(wt, launches, CallBytes{rec_bytes, arena, 0, 0}, &S, partition_family(codec));
   return rc;
 }
 
@@ -1934,8 +1984,7 @@ static int partition_compress_packed(uint32_t codec, int32_t level, uint32_t cod
                                      uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_off, uint64_t* dst_len,
                                      uint64_t* dst_total, uint64_t* checksum_out, int32_t* status,
                                      const ExStore* store, const KeySpec* hash = nullptr) {
-  WallTimer wt;
-  t_timing = b2s_timing{};
+  const WallTimer wt = begin_call();
   if (dst_total) *dst_total = 0;
   const uint32_t bs = block_size_or_default(codec_block_size);
   int rc = partition_args(codec, bs, checksum_alg, num_partitions, n_records, rec_base, rec_bytes, rec_len, rec_part,
@@ -1958,13 +2007,13 @@ static int partition_compress_packed(uint32_t codec, int32_t level, uint32_t cod
   uint32_t* d_len = (uint32_t*)(d_rec + rec_sz);
   uint32_t* d_part = (uint32_t*)(d_rec + rec_sz + len_sz);
   cudaStream_t st = S.st;
-  CU(cudaEventRecord(S.ev_h0, st));
+  CU(S.mark(H0, st));
   if (rec_bytes) CU(cudaMemcpyAsync(d_rec, rec_base, rec_bytes, cudaMemcpyHostToDevice, st));
   if (n_records) {
     CU(cudaMemcpyAsync(d_len, rec_len, n_records * 4, cudaMemcpyHostToDevice, st));
     if (!hash) CU(cudaMemcpyAsync(d_part, rec_part, n_records * 4, cudaMemcpyHostToDevice, st));
   }
-  CU(cudaEventRecord(S.ev_h1, st));
+  CU(S.mark(H1, st));
   std::vector<uint64_t> cks(num_partitions), part_start;
   uint64_t launches = 0, arena = 0;
   rc = partition_compress_run(D, S, codec, level, bs, checksum_alg, num_partitions, n_records, d_rec, rec_bytes, d_len,
@@ -1980,9 +2029,9 @@ static int partition_compress_packed(uint32_t codec, int32_t level, uint32_t cod
       if (dst_len[p] && dst_off[p] + dst_len[p] > dst_cap) status[p] = B2S_E_DST_TOO_SMALL;
     result = fail(B2S_E_DST_TOO_SMALL, "dst_cap is below the %s bytes of the .data arena", std::to_string(arena).c_str());
   }
-  CU(cudaEventRecord(S.ev_d0, st));
+  CU(S.mark(D0, st));
   if (fit) CU(cudaMemcpyAsync(dst_base, S.dst.p, fit, cudaMemcpyDeviceToHost, st));
-  CU(cudaEventRecord(S.ev_d1, st));
+  CU(S.mark(D1, st));
   CU(cudaStreamSynchronize(st));
   CU(cudaGetLastError());
   if (checksum_out) memcpy(checksum_out, cks.data(), (size_t)num_partitions * 8);
@@ -1993,8 +2042,8 @@ static int partition_compress_packed(uint32_t codec, int32_t level, uint32_t cod
     const uint8_t* parts = (const uint8_t*)(codec == B2S_CODEC_NONE ? S.dst.p : S.parena.p);
     *store->cached = ex_store(D->ordinal, st, store->shuffle, store->map, parts, rec_bytes, std::move(part_start));
   }
-  end_timing(wt, launches, CallBytes{rec_bytes, arena, rec_bytes + n_records * (hash ? 4 : 8), fit}, &S, kH2D | kD2H);
-  partition_kernel_times(S, codec, hash, n_records);
+  end_call(wt, launches, CallBytes{rec_bytes, arena, rec_bytes + n_records * (hash ? 4 : 8), fit}, &S,
+           partition_family(codec));
   return result;
 }
 
@@ -2042,8 +2091,7 @@ int b2s_decompress_dev(uint32_t dev_index, uint32_t codec, uint32_t checksum_alg
                        const uint64_t* slice_len, const uint64_t* slice_checksum, void* d_dst_base, uint64_t dst_cap,
                        uint64_t* dst_off, uint64_t* dst_len, uint64_t* dst_total, int32_t* status,
                        int32_t* bad_slice) {
-  WallTimer wt;
-  t_timing = b2s_timing{};
+  const WallTimer wt = begin_call();
   Device* D;
   int rc = get_device(dev_index, &D);
   if (rc) return rc;
@@ -2072,7 +2120,7 @@ int b2s_decompress_dev(uint32_t dev_index, uint32_t codec, uint32_t checksum_alg
   memcpy(status, J.h.status, (size_t)n * 4);
   if (bad_slice) memcpy(bad_slice, J.h.bad, (size_t)n * 4);
   if (dst_total) *dst_total = J.total_out;
-  end_timing(wt, launches, CallBytes{srcb, J.total_out, 0, 0}, &S);
+  end_call(wt, launches, CallBytes{srcb, J.total_out, 0, 0}, &S);
   return 0;
 }
 
@@ -2081,8 +2129,7 @@ static int decompress_host(uint32_t codec, uint32_t alg, uint32_t n, const uint8
                            const uint64_t* slice_sum, uint8_t* packed_dst, uint64_t packed_cap, uint8_t* const* dst,
                            const uint64_t* dst_cap, uint64_t* dst_off, uint64_t* dst_len, uint64_t* dst_total,
                            int32_t* status, int32_t* bad_slice, bool size_only) {
-  WallTimer wt;
-  t_timing = b2s_timing{};
+  const WallTimer wt = begin_call();
   Device* D;
   int rc = get_device(t_device, &D);
   if (rc) return rc;
@@ -2128,12 +2175,10 @@ static int decompress_host(uint32_t codec, uint32_t alg, uint32_t n, const uint8
         sb[k + 1] = (uint32_t)l.size();
       }
       uint64_t total = 0;
-      const b2s_timing keep = t_timing;
       rc = m ? decompress_host(codec, alg, m, sp.data(), sl.data(), sb.data(), l.data(), c.data(), packed_dst, packed_cap,
                                dst ? dp.data() : nullptr, dst_cap ? dc.data() : nullptr, doff.data(), dl.data(), &total,
                                st.data(), bd.data(), size_only)
              : 0;
-      if (!m) t_timing = keep;
       if (rc) return rc;
       uint32_t k = 0;
       uint64_t at = 0;
@@ -2194,7 +2239,7 @@ static int decompress_host(uint32_t codec, uint32_t alg, uint32_t n, const uint8
   auto stage_c = [&](Slot& S, size_t c, uint32_t i0, uint32_t) -> int {
     const DecompressJob& J = jobs[c];
     CU(cudaEventSynchronize(S.ev_b));
-    if (!size_only) add_timing(S, true);
+    if (!size_only) add_times(S, Family::kCodec);
     for (uint32_t k = 0; k < J.n; k++) {
       const uint32_t i = i0 + k;
       status[i] = J.h.status[k];
@@ -2217,7 +2262,7 @@ static int decompress_host(uint32_t codec, uint32_t alg, uint32_t n, const uint8
     return r;
   CU(cudaGetLastError());
   if (dst_total) *dst_total = run_off;
-  end_timing(wt, launches, CallBytes{});
+  end_call(wt, launches, CallBytes{});
   return 0;
 }
 
@@ -2317,6 +2362,7 @@ struct RecordSpec {
   const uint32_t* agg_off = nullptr;
   const int32_t* agg_null_field = nullptr;
   bool rows() const { return is_rows; }
+  Family family() const { return aggregate ? Family::kAggregate : is_rows ? Family::kSortRows : Family::kSort; }
 };
 static RecordSpec fixed_spec(uint32_t record_bytes, uint32_t key_off, uint32_t key_len) {
   RecordSpec r;
@@ -2549,7 +2595,7 @@ struct SortSource {
 
 // The end of an aggregation (b2s_decompress_aggregate_rows_*), from the sorted indices idx of the records: grouping,
 // one readback of the group count and output bytes (which checks out_cap), the heads' gather and the merge into
-// d_out.  *total = output bytes.  The dominant step is this one.
+// d_out.  *total = output bytes.  The dominant step is this one (marks G0, G1).
 static int aggregate_rows_tail(Slot& S, const RecordSpec& spec, const uint8_t* arena, uint64_t records,
                                const uint32_t* idx, const uint32_t* heads, uint8_t* ws, uint8_t* aws, uint8_t* d_out,
                                uint64_t out_cap, uint64_t* total, uint64_t* n_rec, uint64_t* n_groups,
@@ -2563,9 +2609,8 @@ static int aggregate_rows_tail(Slot& S, const RecordSpec& spec, const uint8_t* a
     agg.off[k] = spec.agg_off[k];
     agg.null_field[k] = spec.agg_null_field[k];
   }
-  const uint64_t agg_launches = *launches;
   uint64_t rb[2] = {0, 0};  // groups, output bytes
-  CU(cudaEventRecord(S.ev_g[0], st));
+  CU(S.mark(G0, st, *launches));
   if (records) {
     launch_rows_group(arena, records, idx, heads, key_bytes, agg, ws, aws, st, launches);
     CU(cudaMemcpyAsync(rb, rows_aggregate_readback(aws, records, agg.n), sizeof rb, cudaMemcpyDeviceToHost, st));
@@ -2576,13 +2621,10 @@ static int aggregate_rows_tail(Slot& S, const RecordSpec& spec, const uint8_t* a
   if (rb[1] > out_cap)
     return fail(B2S_E_DST_TOO_SMALL, "dst_cap is below the %s output bytes", std::to_string(rb[1]).c_str());
   launch_rows_aggregate(arena, records, rb[0], key_bytes, agg.n, ws, aws, d_out, st, launches);
-  CU(cudaEventRecord(S.ev_g[1], st));
-  CU(cudaEventRecord(S.ev_p1, st));
+  CU(S.mark(G1, st, *launches));
+  CU(S.mark(P1, st));
   CU(cudaStreamSynchronize(st));
   CU(cudaGetLastError());
-  S.dom_used = 0;
-  t_timing.dominant_ms = ms_between(S.ev_g[0], S.ev_g[1]);
-  t_timing.dominant_launches = *launches - agg_launches;
   *n_rec = records;
   if (n_groups) *n_groups = rb[0];
   return 0;
@@ -2619,7 +2661,7 @@ static int decompress_sort_run(Device* D, Slot& S, uint32_t codec, uint32_t alg,
     CU(cudaStreamSynchronize(st));
     CU(cudaGetLastError());
   } else {  // every source is cached
-    CU(cudaEventRecord(S.ev_k0, st));
+    CU(S.mark(K0, st));
   }
   const uint32_t n_src = mix ? (uint32_t)mix->size() : n;
   auto cached = [&](uint32_t i) { return mix && (*mix)[i].cached; };
@@ -2649,31 +2691,14 @@ static int decompress_sort_run(Device* D, Slot& S, uint32_t codec, uint32_t alg,
     at += len;
   }
   *total = mix ? at : J.h.totals[1];
-  auto report = [&]() {
+  auto report = [&]() {  // -> 0, the result of a call that ends because a source failed (nothing is sorted or written)
     for (uint32_t i = 0; i < n_src; i++) {
       status[i] = cached(i) ? cached_status[i] : J.h.status[block(i)];
       if (bad_slice) bad_slice[i] = cached(i) ? -1 : J.h.bad[block(i)];
     }
-  };
-  auto skip_events = [&](bool decode, bool sort) -> int {  // stand-ins for the steps a call does not run
-    if (decode) {
-      CU(cudaEventRecord(S.ev_t0, st));
-      CU(cudaEventRecord(S.ev_t1, st));
-      CU(cudaEventRecord(S.ev_k1, st));
-    }
-    if (sort) {
-      CU(cudaEventRecord(S.ev_p0, st));
-      CU(cudaEventRecord(S.ev_p1, st));
-    }
-    if (sort && spec.rows())
-      for (cudaEvent_t e : S.ev_f) CU(cudaEventRecord(e, st));
-    CU(cudaStreamSynchronize(st));
     return 0;
   };
-  if (failed) {
-    report();
-    return skip_events(true, true);
-  }
+  if (failed) return report();
   if (!spec.rows() && *total / spec.record_bytes > 0xffffffffull)
     return fail(B2S_E_ARG, "more than 2^32 - 1 records in one call (%s bytes)", std::to_string(*total).c_str());
   if (!spec.aggregate && *total > out_cap) {  // an aggregation's output is sized once the groups are known
@@ -2715,7 +2740,6 @@ static int decompress_sort_run(Device* D, Slot& S, uint32_t codec, uint32_t alg,
                              cudaMemcpyDeviceToDevice, st));
       arena = (const uint8_t*)S.dst.p;
     }
-    if ((rc = skip_events(true, false))) return rc;
   } else {
     if (!mix && (rc = S.dst.ensure(*total + 64))) return rc;
     rc = decompress_enqueue_b(S, J, d_src, (uint8_t*)S.dst.p, S.dst.cap, launches);
@@ -2723,10 +2747,7 @@ static int decompress_sort_run(Device* D, Slot& S, uint32_t codec, uint32_t alg,
     CU(cudaEventSynchronize(S.ev_b));
     CU(cudaGetLastError());
     for (uint32_t i = 0; i < n; i++) failed |= J.h.status[i] != B2S_OK;
-    if (failed) {
-      report();
-      return skip_events(false, true);
-    }
+    if (failed) return report();
     arena = (const uint8_t*)S.dst.p;
   }
   report();
@@ -2738,10 +2759,10 @@ static int decompress_sort_run(Device* D, Slot& S, uint32_t codec, uint32_t alg,
   if (!spec.rows()) {
     const uint64_t records = *total / spec.record_bytes;
     if (records && (rc = S.pws.ensure(key_sort_ws_bytes(records, spec.keys.len[0])))) return rc;
-    CU(cudaEventRecord(S.ev_p0, st));
+    CU(S.mark(P0, st));
     launch_key_sort(arena, records, spec.record_bytes, spec.keys.off[0], spec.keys.len[0], (uint8_t*)S.pws.p,
                     *d_sorted, st, launches);
-    CU(cudaEventRecord(S.ev_p1, st));
+    CU(S.mark(P1, st));
     CU(cudaStreamSynchronize(st));
     CU(cudaGetLastError());
     *n_rec = records;
@@ -2757,12 +2778,11 @@ static int decompress_sort_run(Device* D, Slot& S, uint32_t codec, uint32_t alg,
   }
   if ((rc = S.fws.ensure(rows_frame_ws_bytes(*total, n_src)))) return rc;
   uint8_t* fws = (uint8_t*)S.fws.p;
-  uint64_t frame_launches = *launches;
-  CU(cudaEventRecord(S.ev_p0, st));
-  CU(cudaEventRecord(S.ev_f[0], st));
+  CU(S.mark(P0, st));
+  CU(S.mark(F0, st, *launches));
   launch_rows_frame(arena, *total, place.data(), length.data(), n_src, min_key, min_null, agg_min_row(spec), fws, st,
                     launches);
-  CU(cudaEventRecord(S.ev_f[1], st));
+  CU(S.mark(F1, st, *launches));
   std::vector<uint64_t> rb(n_src + 1);
   CU(cudaMemcpyAsync(rb.data(), rows_frame_readback(fws, *total, n_src), rows_frame_readback_bytes(n_src),
                      cudaMemcpyDeviceToHost, st));
@@ -2788,16 +2808,8 @@ static int decompress_sort_run(Device* D, Slot& S, uint32_t codec, uint32_t alg,
       failed = true;
     }
   };
-  auto failed_rows = [&]() -> int {  // nothing is sorted or written
-    report();
-    CU(cudaEventRecord(S.ev_f[2], st));
-    CU(cudaEventRecord(S.ev_f[3], st));
-    CU(cudaEventRecord(S.ev_p1, st));
-    CU(cudaStreamSynchronize(st));
-    return 0;
-  };
   take_verdicts(rb.data() + 1);
-  if (failed) return failed_rows();
+  if (failed) return report();
   const uint64_t records = rb[0];
   if (records > 0xffffffffull)
     return fail(B2S_E_ARG, "more than 2^32 - 1 records in one call (%s records)", std::to_string(records).c_str());
@@ -2809,10 +2821,9 @@ static int decompress_sort_run(Device* D, Slot& S, uint32_t codec, uint32_t alg,
   if (records && (rc = S.pws.ensure(sort_ws + agg_ws + refine_ws))) return rc;
   uint8_t* ws = (uint8_t*)S.pws.p;
   uint8_t* rws = refine ? ws + sort_ws + agg_ws : nullptr;
-  CU(cudaEventRecord(S.ev_f[2], st));
+  CU(S.mark(F2, st, *launches));
   launch_rows_emit(arena, *total, n_src, fws, records, key_bytes, ws, st, launches);
-  CU(cudaEventRecord(S.ev_f[3], st));
-  frame_launches = *launches - frame_launches;
+  CU(S.mark(F3, st, *launches));
   const uint32_t* idx = launch_rows_order(arena, records, ks, rows_frame_ranges(fws, *total, n_src), n_src, ws, rws,
                                           st, launches);
   const uint32_t* heads = nullptr;
@@ -2827,7 +2838,7 @@ static int decompress_sort_run(Device* D, Slot& S, uint32_t codec, uint32_t alg,
       CU(cudaGetLastError());
       if (!round) {
         take_verdicts(rrb.data() + 1);
-        if (failed) return failed_rows();
+        if (failed) return report();
       }
       const uint64_t tied = rrb[0] & 0xffffffffull, runs = rrb[0] >> 32;
       if (!tied) break;
@@ -2839,21 +2850,11 @@ static int decompress_sort_run(Device* D, Slot& S, uint32_t codec, uint32_t alg,
   if (spec.aggregate) return aggregate_rows_tail(S, spec, arena, records, idx, heads, ws, ws + sort_ws, *d_sorted,
                                                  out_cap, total, n_rec, n_groups, launches);
   launch_rows_gather(arena, records, key_bytes, idx, ws, *d_sorted, st, launches);
-  CU(cudaEventRecord(S.ev_p1, st));
+  CU(S.mark(P1, st));
   CU(cudaStreamSynchronize(st));
   CU(cudaGetLastError());
-  // the dominant step of a row sort is the framing (walk + count, emit), not the decoder's kernel
-  S.dom_used = 0;
-  t_timing.dominant_ms = ms_between(S.ev_f[0], S.ev_f[1]) + ms_between(S.ev_f[2], S.ev_f[3]);
-  t_timing.dominant_launches = frame_launches;
   *n_rec = records;
   return 0;
-}
-
-// kernel_ms: verification + decode + sort; top_kernel_ms: the sort step (rows: framing + sort)
-static void sort_kernel_times(Slot& S) {
-  t_timing.kernel_ms = ms_between(S.ev_k0, S.ev_p1);
-  t_timing.top_kernel_ms = ms_between(S.ev_p0, S.ev_p1);
 }
 
 // decompress_sort on the read lane of D over device-resident blocks, sorted into dst_base (device memory)
@@ -2874,8 +2875,7 @@ static int sort_dev_run(Device* D, uint32_t codec, uint32_t alg, uint32_t n, con
                                slice_checksum, spec, &out, dst_cap, dst_total, n_records, n_groups, status,
                                bad_slice, &launches, mix);
   if (rc) return rc;
-  end_timing(wt, launches, CallBytes{srcb, *dst_total, 0, 0}, &S);
-  sort_kernel_times(S);
+  end_call(wt, launches, CallBytes{srcb, *dst_total, 0, 0}, &S, spec.family());
   return 0;
 }
 
@@ -2900,7 +2900,7 @@ static int sort_packed_run(Device* D, uint32_t codec, uint32_t alg, uint32_t n, 
   int rc;
   if ((rc = S.src.ensure(srcb + 64))) return rc;
   cudaStream_t st = S.st;
-  CU(cudaEventRecord(S.ev_h0, st));
+  CU(S.mark(H0, st));
   for (uint32_t i = 0; i < n;) {  // blocks adjacent in host memory go up in one copy
     uint32_t j = i + 1;
     while (j < n && src_off[j] == src_off[j - 1] + src_len[j - 1]) j++;
@@ -2908,7 +2908,7 @@ static int sort_packed_run(Device* D, uint32_t codec, uint32_t alg, uint32_t n, 
     if (bytes) CU(cudaMemcpyAsync((uint8_t*)S.src.p + dev_off[i], src_base + src_off[i], bytes, cudaMemcpyHostToDevice, st));
     i = j;
   }
-  CU(cudaEventRecord(S.ev_h1, st));
+  CU(S.mark(H1, st));
   uint64_t launches = 0;
   uint8_t* sorted = nullptr;
   rc = decompress_sort_run(D, S, codec, alg, n, (const uint8_t*)S.src.p, dev_off.data(), src_len, true, slice_base,
@@ -2916,13 +2916,12 @@ static int sort_packed_run(Device* D, uint32_t codec, uint32_t alg, uint32_t n, 
                            bad_slice, &launches, mix);
   if (rc) return rc;
   const uint64_t down = *n_records ? *dst_total : 0;
-  CU(cudaEventRecord(S.ev_d0, st));
+  CU(S.mark(D0, st));
   if (down) CU(cudaMemcpyAsync(dst_base, sorted, down, cudaMemcpyDeviceToHost, st));
-  CU(cudaEventRecord(S.ev_d1, st));
+  CU(S.mark(D1, st));
   CU(cudaStreamSynchronize(st));
   CU(cudaGetLastError());
-  end_timing(wt, launches, CallBytes{srcb, *dst_total, srcb, down}, &S, kH2D | kD2H);
-  sort_kernel_times(S);
+  end_call(wt, launches, CallBytes{srcb, *dst_total, srcb, down}, &S, spec.family());
   return 0;
 }
 
@@ -2993,8 +2992,7 @@ static int sort_call(uint32_t dev_index, bool packed, const ExchangeRead* x, uin
                      const uint32_t* slice_base, const uint64_t* slice_len, const uint64_t* slice_checksum,
                      const RecordSpec& spec, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_total,
                      uint64_t* n_records, int32_t* status, int32_t* bad_slice, uint64_t* n_groups = nullptr) {
-  WallTimer wt;
-  t_timing = b2s_timing{};
+  const WallTimer wt = begin_call();
   if (dst_total) *dst_total = 0;
   if (n_records) *n_records = 0;
   if (n_groups) *n_groups = 0;
@@ -3245,8 +3243,7 @@ int b2s_exchange_lookup(int32_t shuffle_id, int32_t start_reduce, int32_t end_re
 int b2s_exchange_read_packed(int32_t shuffle_id, int32_t start_reduce, int32_t end_reduce, uint32_t n_maps,
                              const int64_t* map_ids, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_off,
                              uint64_t* dst_len, uint64_t* dst_total, int32_t* status) {
-  WallTimer wt;
-  t_timing = b2s_timing{};
+  const WallTimer wt = begin_call();
   if (dst_total) *dst_total = 0;
   int rc = reduce_range_args(start_reduce, end_reduce);
   if (rc) return rc;
@@ -3280,21 +3277,21 @@ int b2s_exchange_read_packed(int32_t shuffle_id, int32_t start_reduce, int32_t e
   uint64_t launches = 0;
   if ((rc = S.dst.ensure(total + 64)) || (rc = S.xpieces.ensure(pieces.size() * sizeof(ExchangePiece) + 64)))
     return rc;
-  CU(cudaEventRecord(S.ev_k0, st));
-  CU(cudaEventRecord(S.ev_t0, st));
+  CU(S.mark(K0, st));
+  CU(S.mark(T0, st));
   if (!pieces.empty()) {
     CU(cudaMemcpyAsync(S.xpieces.p, pieces.data(), pieces.size() * sizeof(ExchangePiece), cudaMemcpyHostToDevice, st));
     launch_exchange_gather((const ExchangePiece*)S.xpieces.p, (uint32_t)pieces.size(), (uint8_t*)S.dst.p, st,
                            &launches);
   }
-  CU(cudaEventRecord(S.ev_t1, st));
-  CU(cudaEventRecord(S.ev_k1, st));
-  CU(cudaEventRecord(S.ev_d0, st));
+  CU(S.mark(T1, st));
+  CU(S.mark(K1, st));
+  CU(S.mark(D0, st));
   if (total) CU(cudaMemcpyAsync(dst_base, S.dst.p, total, cudaMemcpyDeviceToHost, st));
-  CU(cudaEventRecord(S.ev_d1, st));
+  CU(S.mark(D1, st));
   CU(cudaStreamSynchronize(st));
   CU(cudaGetLastError());
-  end_timing(wt, launches, CallBytes{total, total, 0, total}, &S, kD2H);
+  end_call(wt, launches, CallBytes{total, total, 0, total}, &S);
   return 0;
 }
 
