@@ -224,6 +224,49 @@ int b2s_partition_compress_rows_hash_dev(uint32_t dev_index, uint32_t codec, int
                                          uint64_t dst_cap, uint64_t* dst_off, uint64_t* dst_len, uint64_t* dst_total,
                                          uint64_t* checksum_out, int32_t* status);
 
+/* ---- write side, range-partitioned rows: Spark's RangePartitioner ids computed on the GPU ----
+ * b2s_partition_compress_* for a RangePartitioning exchange of UnsafeRows (a global ORDER BY's map side): the reduce id
+ * of every record is what Spark's RangePartitioner.getPartition returns for its sort key over the n_bounds range
+ * bounds, so the caller passes no rec_part, and num_partitions = n_bounds + 1 (dst_off / dst_len / checksum_out /
+ * status have that many entries).  The id is the number of bounds strictly below the record's key (with strictly
+ * increasing bounds both of getPartition's branches, the linear scan and the binary search, return it): a key equal
+ * to bound p goes to partition p.  Records are framed as for the hash call ([size: int32 big-endian][row], rec_len[i] =
+ * 4 + size).  The key columns are given as to the composite-key calls, order flags included (B2S_KEY_DESCENDING,
+ * B2S_KEY_NULLS_LAST), and compared in Spark SQL's order: -0.0 equals 0.0, NaN equals NaN and sorts above +inf,
+ * strings and binary as unsigned bytes, decimals by value, a null string is not an empty one.
+ * Bounds: n_bounds (0..2^24 - 1) rows framed the same way, back to back in bound_base (bound_bytes, bound_len[j] each),
+ * as Spark holds them: UnsafeProjection(sort order children) rows, so key column c is field c of a bound row (its slot
+ * at 8 * ceil(n_keys / 64) + 8 c, its null bit c when key_null_field[c] >= 0, else never null; type, flags and key_len
+ * those of the records' column c).  The bound arrays are host memory in both forms; they are uploaded once per call.
+ * n_bounds = 0 sends every record to partition 0; n_records = 0 is valid.
+ * Outputs: byte for byte what b2s_partition_compress_packed / _dev return for the same records and those ids.
+ * Errors, B2S_E_ARG, nothing reported as written, b2s_last_error() says why: what the hash call rejects, except that
+ * order flags and B2S_KEY_BYTES of key_len 1..16 are allowed; n_bounds above 2^24 - 1; a null bound array with n_bounds
+ * > 0; bound_len not summing to bound_bytes; a bad bound (bound_len < 4, a size prefix other than bound_len - 4, a row
+ * that does not hold a key slot or null word, a string past its row, a bad decimal) or a bound whose key is not above
+ * the one before it (equal ones included, such as -0.0 after 0.0, two NaNs or two nulls): the lowest such bound is named;
+ * a bad record, as for the hash call.  A bad bound is named before a bad record.  No usable device -> B2S_E_CUDA.
+ * b2s_last_timing as for the partition calls, plus dominant_ms / dominant_launches = the range step (the bound checks
+ * and the id kernel).  No exchange-cache form. */
+int b2s_partition_compress_rows_range_packed(uint32_t codec, int32_t level, uint32_t codec_block_size,
+                                             uint32_t checksum_alg, uint64_t n_records, const uint8_t* rec_base,
+                                             uint64_t rec_bytes, const uint32_t* rec_len, uint32_t n_keys,
+                                             const uint32_t* key_type, const uint32_t* key_off, const uint32_t* key_len,
+                                             const int32_t* key_null_field, uint32_t n_bounds,
+                                             const uint8_t* bound_base, uint64_t bound_bytes,
+                                             const uint32_t* bound_len, uint8_t* dst_base, uint64_t dst_cap,
+                                             uint64_t* dst_off, uint64_t* dst_len, uint64_t* dst_total,
+                                             uint64_t* checksum_out, int32_t* status);
+/* same, with rec_base / rec_len / dst_base in device memory of dev_index (the bound arrays stay in host memory) */
+int b2s_partition_compress_rows_range_dev(uint32_t dev_index, uint32_t codec, int32_t level, uint32_t codec_block_size,
+                                          uint32_t checksum_alg, uint64_t n_records, const uint8_t* rec_base,
+                                          uint64_t rec_bytes, const uint32_t* rec_len, uint32_t n_keys,
+                                          const uint32_t* key_type, const uint32_t* key_off, const uint32_t* key_len,
+                                          const int32_t* key_null_field, uint32_t n_bounds, const uint8_t* bound_base,
+                                          uint64_t bound_bytes, const uint32_t* bound_len, uint8_t* dst_base,
+                                          uint64_t dst_cap, uint64_t* dst_off, uint64_t* dst_len, uint64_t* dst_total,
+                                          uint64_t* checksum_out, int32_t* status);
+
 /* ---- read side ---- */
 /* n compressed blocks as produced by S3BufferedPrefetchIterator.next() (storage/S3BufferedPrefetchIterator.scala:196-212).
  * Block i covers n_slices[i] consecutive reduce partitions (1 for ShuffleBlockId, >1 for ShuffleBlockBatchId,

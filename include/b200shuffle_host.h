@@ -117,6 +117,16 @@ int b2sh_serialized_writer_create(b2sh_dispatcher* d, int32_t shuffle_id, int64_
  * writer never stores into the exchange cache, even when it is on: the cache's reads serve fixed-size records only. */
 int b2sh_serialized_writer_hash_rows(b2sh_serialized_writer* w, uint32_t n_keys, const uint32_t* key_type,
                                      const uint32_t* key_off, const uint32_t* key_len, const int32_t* key_null_field);
+/* RangePartitioning of UnsafeRows (INTEGRATION.md §3k), set before the first insert: every later insert is one record
+ * as UnsafeRowSerializer writes it and its partition_id is ignored; commit() makes one
+ * b2s_partition_compress_rows_range_packed call with these key columns and the n_bounds bound rows (framed the same
+ * way, back to back in bound_base, bound_len[j] each; copied), which computes Spark's RangePartitioner ids on the GPU.
+ * n_bounds + 1 must be the writer's num_partitions.  The files are byte-identical to the ones the writer makes when fed
+ * the same rows with those ids.  In this mode the writer never stores into the exchange cache, as for hash_rows. */
+int b2sh_serialized_writer_range_rows(b2sh_serialized_writer* w, uint32_t n_keys, const uint32_t* key_type,
+                                      const uint32_t* key_off, const uint32_t* key_len, const int32_t* key_null_field,
+                                      uint32_t n_bounds, const uint8_t* bound_base, uint64_t bound_bytes,
+                                      const uint32_t* bound_len);
 int b2sh_serialized_writer_insert(b2sh_serialized_writer* w, int32_t partition_id, const uint8_t* bytes, uint64_t len);
 int b2sh_serialized_writer_commit(b2sh_serialized_writer* w, int64_t* partition_lengths_out);
 int b2sh_serialized_writer_statistics(b2sh_serialized_writer* w, uint64_t* bytes, uint64_t* nanos, char* line,

@@ -9,6 +9,8 @@
  *                                          map task in, .data arena + partitionLengths + checksums out
  *   partitionCompressRowsHashPacked        the same for a HashPartitioning exchange (INTEGRATION.md §3j): rows and
  *                                          their key columns in, the reduce ids computed on the GPU
+ *   partitionCompressRowsRangePacked       the same for a RangePartitioning exchange (INTEGRATION.md §3k): rows,
+ *                                          their sort-key columns and the partitioner's bound rows in
  *   decompressPacked / decompressedSize    storage/S3ShuffleReader.scala:98-110 (the codec seam, batched drain of
  *                                          storage/S3BufferedPrefetchIterator.scala:196-212)
  *   checksumPacked                         shuffle/S3SingleSpillShuffleMapOutputWriter.scala:54-63,
@@ -144,19 +146,30 @@ static int bad_keys(JNIEnv* e, const composite_key* keys) {
          (*e)->GetArrayLength(e, keys->len) < keys->n || (*e)->GetArrayLength(e, keys->nullField) < keys->n;
 }
 
+/* a RangePartitioner's bounds: n rows framed as UnsafeRowSerializer writes them, back to back at the direct buffer
+ * address rows (bytes long), their lengths int[n] len */
+typedef struct {
+  jint n;
+  jlong rows, bytes;
+  jintArray len;
+} range_bounds;
+
 /* cached (may be NULL): int[1], the cached store's flag; then (shuffleId, mapId) keys the exchange-cache entry.
- * hash (may be NULL, then cached is NULL): the records are serialized rows whose reduce ids are Spark's
- * HashPartitioning ids by these key columns (partitionCompressRowsHashPacked); recPart is not read */
+ * hash (may be NULL, then cached is NULL): the records are serialized rows whose reduce ids are computed on the GPU
+ * from these key columns, recPart is not read: Spark's HashPartitioning ids (partitionCompressRowsHashPacked), or with
+ * range its RangePartitioner ids over those bounds (partitionCompressRowsRangePacked; numPartitions = range->n + 1) */
 static jint partition_compress(JNIEnv* e, jint shuffleId, jlong mapId, jintArray cached, const composite_key* hash,
-                               jint codec, jint level, jint blockSize, jint alg, jint numPartitions, jlong nRecords,
-                               jlong records, jlong recBytes, jlong recLen, jlong recPart, jlong dst, jlong dstCap,
-                               jlongArray dstOff, jlongArray dstLen, jlongArray meta, jlongArray checksums,
-                               jintArray status) {
+                               const range_bounds* range, jint codec, jint level, jint blockSize, jint alg,
+                               jint numPartitions, jlong nRecords, jlong records, jlong recBytes, jlong recLen,
+                               jlong recPart, jlong dst, jlong dstCap, jlongArray dstOff, jlongArray dstLen,
+                               jlongArray meta, jlongArray checksums, jintArray status) {
   if ((cached && (*e)->GetArrayLength(e, cached) < 1) || numPartitions < 1 || !dstOff || !dstLen || !meta || !status || (*e)->GetArrayLength(e, dstOff) < numPartitions ||
       (*e)->GetArrayLength(e, dstLen) < numPartitions || (*e)->GetArrayLength(e, status) < numPartitions ||
       (*e)->GetArrayLength(e, meta) < 1 || (checksums && (*e)->GetArrayLength(e, checksums) < numPartitions))
     return B2S_E_ARG;
   if (hash && bad_keys(e, hash)) return B2S_E_ARG;
+  if (range && (range->n < 0 || (range->n && (!range->len || (*e)->GetArrayLength(e, range->len) < range->n))))
+    return B2S_E_ARG;
   uint32_t kt[16], ko[16], kl[16];
   int32_t knf[16];
   if (hash) {
@@ -168,15 +181,24 @@ static jint partition_compress(JNIEnv* e, jint shuffleId, jlong mapId, jintArray
   const size_t R = (size_t)numPartitions;
   uint64_t* buf = (uint64_t*)malloc(R * 3 * sizeof(uint64_t));
   int32_t* st = (int32_t*)malloc(R * sizeof(int32_t));
-  if (!buf || !st) {
+  /* the bound lengths, copied out of the Java array so that none is held while the GPU works */
+  uint32_t* bl = range ? (uint32_t*)malloc(((size_t)range->n + 1) * sizeof(uint32_t)) : 0;
+  if (!buf || !st || (range && !bl)) {
     free(buf);
     free(st);
+    free(bl);
     return B2S_E_NOMEM;
   }
+  if (range && range->n) (*e)->GetIntArrayRegion(e, range->len, 0, range->n, (jint*)bl);
   uint64_t total = 0;
   int32_t stored = 0;
   const int rc =
-      hash ? b2s_partition_compress_rows_hash_packed(
+      range ? b2s_partition_compress_rows_range_packed(
+                  (uint32_t)codec, (int32_t)level, (uint32_t)blockSize, (uint32_t)alg, (uint64_t)nRecords,
+                  PTR(const uint8_t, records), (uint64_t)recBytes, PTR(const uint32_t, recLen), (uint32_t)hash->n, kt,
+                  ko, kl, knf, (uint32_t)range->n, PTR(const uint8_t, range->rows), (uint64_t)range->bytes, bl,
+                  PTR(uint8_t, dst), (uint64_t)dstCap, buf, buf + R, &total, buf + 2 * R, st)
+      : hash ? b2s_partition_compress_rows_hash_packed(
                  (uint32_t)codec, (int32_t)level, (uint32_t)blockSize, (uint32_t)alg, (uint32_t)numPartitions,
                  (uint64_t)nRecords, PTR(const uint8_t, records), (uint64_t)recBytes, PTR(const uint32_t, recLen),
                  (uint32_t)hash->n, kt, ko, kl, knf, PTR(uint8_t, dst), (uint64_t)dstCap, buf, buf + R, &total,
@@ -200,6 +222,7 @@ static jint partition_compress(JNIEnv* e, jint shuffleId, jlong mapId, jintArray
   }
   const jlong m = (jlong)total;
   (*e)->SetLongArrayRegion(e, meta, 0, 1, &m);
+  free(bl);
   free(st);
   free(buf);
   return rc;
@@ -210,8 +233,8 @@ JNIEXPORT jint JNICALL J(partitionCompressPacked)(JNIEnv* e, jclass c, jint code
                                                   jlongArray dstOff, jlongArray dstLen, jlongArray meta,
                                                   jlongArray checksums, jintArray status) {
   (void)c;
-  return partition_compress(e, 0, 0, 0, 0, codec, level, blockSize, alg, numPartitions, nRecords, records, recBytes,
-                            recLen, recPart, dst, dstCap, dstOff, dstLen, meta, checksums, status);
+  return partition_compress(e, 0, 0, 0, 0, 0, codec, level, blockSize, alg, numPartitions, nRecords, records,
+                            recBytes, recLen, recPart, dst, dstCap, dstOff, dstLen, meta, checksums, status);
 }
 /* HashPartitioning exchange of UnsafeRows (INTEGRATION.md §3j): records as UnsafeRowSerializer writes them, recLen
  * (u32) per record, no reduce ids: the GPU computes Spark's pmod(Murmur3Hash(key columns, 42), numPartitions).  The key
@@ -225,7 +248,29 @@ JNIEXPORT jint JNICALL J(partitionCompressRowsHashPacked)(JNIEnv* e, jclass c, j
                                                           jintArray status) {
   (void)c;
   const composite_key keys = {nKeys, keyType, keyOff, keyLen, keyNullField};
-  return partition_compress(e, 0, 0, 0, &keys, codec, level, blockSize, alg, numPartitions, nRecords, records,
+  return partition_compress(e, 0, 0, 0, &keys, 0, codec, level, blockSize, alg, numPartitions, nRecords, records,
+                            recBytes, recLen, 0, dst, dstCap, dstOff, dstLen, meta, checksums, status);
+}
+/* RangePartitioning exchange of UnsafeRows (INTEGRATION.md §3k): records and key columns as
+ * partitionCompressRowsHashPacked (order flags allowed), no numPartitions: the RangePartitioner's nBounds bound rows
+ * (UnsafeProjection(sort order children) rows, each with its int32 big-endian size prefix) lie back to back at the
+ * direct buffer address bounds, boundBytes long, their lengths in int[nBounds] boundLen; the GPU computes every
+ * record's RangePartitioner id, and dstOff / dstLen / checksums / status have nBounds + 1 entries.  The bounds are an
+ * address rather than a byte[]: the exchange serialises them once into a direct buffer its map tasks share, and no
+ * Java array is held while the GPU works (boundLen is copied out first) */
+JNIEXPORT jint JNICALL J(partitionCompressRowsRangePacked)(JNIEnv* e, jclass c, jint codec, jint level, jint blockSize,
+                                                           jint alg, jlong nRecords, jlong records, jlong recBytes,
+                                                           jlong recLen, jint nKeys, jintArray keyType,
+                                                           jintArray keyOff, jintArray keyLen, jintArray keyNullField,
+                                                           jint nBounds, jlong bounds, jlong boundBytes,
+                                                           jintArray boundLen, jlong dst, jlong dstCap,
+                                                           jlongArray dstOff, jlongArray dstLen, jlongArray meta,
+                                                           jlongArray checksums, jintArray status) {
+  (void)c;
+  if (nBounds < 0 || nBounds > (1 << 24) - 1) return B2S_E_ARG;
+  const composite_key keys = {nKeys, keyType, keyOff, keyLen, keyNullField};
+  const range_bounds range = {nBounds, bounds, boundBytes, boundLen};
+  return partition_compress(e, 0, 0, 0, &keys, &range, codec, level, blockSize, alg, nBounds + 1, nRecords, records,
                             recBytes, recLen, 0, dst, dstCap, dstOff, dstLen, meta, checksums, status);
 }
 /* the same, keeping the partitioned records in the exchange cache as (shuffleId, mapId); cached: int[1] = stored */
@@ -237,8 +282,9 @@ JNIEXPORT jint JNICALL J(partitionCompressCachedPacked)(JNIEnv* e, jclass c, jin
                                                         jintArray status, jintArray cached) {
   (void)c;
   if (!cached) return B2S_E_ARG;
-  return partition_compress(e, shuffleId, mapId, cached, 0, codec, level, blockSize, alg, numPartitions, nRecords,
-                            records, recBytes, recLen, recPart, dst, dstCap, dstOff, dstLen, meta, checksums, status);
+  return partition_compress(e, shuffleId, mapId, cached, 0, 0, codec, level, blockSize, alg, numPartitions,
+                            nRecords, records, recBytes, recLen, recPart, dst, dstCap, dstOff, dstLen, meta, checksums,
+                            status);
 }
 
 /* ---- read side: n prefetched blocks; block i owns slices [sliceBase[i], sliceBase[i+1]) of sliceLen/sliceChecksum

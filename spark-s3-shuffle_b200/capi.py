@@ -74,6 +74,12 @@ PROTOTYPES = [
     ("b2s_partition_compress_rows_hash_dev", C.c_int,
      [_u32, _u32, _i32, _u32, _u32, _u32, _u64, _vp, _u64, _u32p, _u32, _u32p, _u32p, _u32p, _i32p, _vp, _u64, _u64p,
       _u64p, _u64p, _u64p, _i32p]),
+    ("b2s_partition_compress_rows_range_packed", C.c_int,
+     [_u32, _i32, _u32, _u32, _u64, _u8p, _u64, _u32p, _u32, _u32p, _u32p, _u32p, _i32p, _u32, _u8p, _u64, _u32p,
+      _u8p, _u64, _u64p, _u64p, _u64p, _u64p, _i32p]),
+    ("b2s_partition_compress_rows_range_dev", C.c_int,
+     [_u32, _u32, _i32, _u32, _u32, _u64, _vp, _u64, _u32p, _u32, _u32p, _u32p, _u32p, _i32p, _u32, _u8p, _u64, _u32p,
+      _vp, _u64, _u64p, _u64p, _u64p, _u64p, _i32p]),
     ("b2s_decompress_batch", C.c_int,
      [_u32, _u32, _u32, _vp, _u64p, _u32p, _vp, _vp, _vp, _u64p, _u64p, _i32p, _i32p]),
     ("b2s_decompress_packed", C.c_int,
@@ -633,6 +639,48 @@ def partition_compress_rows_hash_dev(codec, d_records, rec_bytes, d_rec_len, n_r
         dev, codec, level, block_size, checksum_alg, num_partitions, n_records, d_records, rec_bytes, d_rec_len, nk,
         _ptr(kt), _ptr(ko), _ptr(kl), _ptr(kn), d_dst, dst_cap, _ptr(dst_off), _ptr(dst_len), C.addressof(total),
         _ptr(cks), _ptr(st)), "b2s_partition_compress_rows_hash_dev")
+    return dict(dst_off=dst_off, dst_len=dst_len, total=total.value, checksums=cks, status=st)
+
+
+def _bound_arrays(bounds):
+    """bounds = the RangePartitioner's bound rows, each framed as UnsafeRowSerializer writes it ([int32 big-endian
+    size][row]) -> (n, rows back to back, their lengths)"""
+    bounds = [bytes(b) for b in bounds]
+    base = np.frombuffer(b"".join(bounds) or b"\0", dtype=np.uint8).copy()
+    return len(bounds), base, sum(len(b) for b in bounds), np.array([len(b) for b in bounds] or [0], dtype=np.uint32)
+
+
+def partition_compress_rows_range_packed(codec, records, rec_len, keys, bounds, dst, block_size=0,
+                                         checksum_alg=CHECKSUM_NONE, level=0):
+    """partition_compress_packed of serialized UnsafeRows ([int32 big-endian size][row] each), every record's reduce
+    id Spark's RangePartitioner id of its key over the bounds (framed rows, _bound_arrays); len(bounds) + 1 partitions;
+    keys as in decompress_sort_rows_keys_packed, order flags included.  -> dict(dst_off, dst_len, total, checksums,
+    status)"""
+    records, dst = _as_u8(records), _as_u8(dst)
+    rec_len = np.ascontiguousarray(rec_len, dtype=np.uint32)
+    nk, kt, ko, kl, kn = _key_arrays(keys)
+    nb, bb, bbytes, bl = _bound_arrays(bounds)
+    dst_off, dst_len, cks, st = _partition_out(nb + 1)
+    total = _u64(0)
+    _check(load().b2s_partition_compress_rows_range_packed(
+        codec, level, block_size, checksum_alg, rec_len.size, _ptr(records), records.size, _ptr(rec_len), nk, _ptr(kt),
+        _ptr(ko), _ptr(kl), _ptr(kn), nb, _ptr(bb), bbytes, _ptr(bl), _ptr(dst), dst.size, _ptr(dst_off),
+        _ptr(dst_len), C.addressof(total), _ptr(cks), _ptr(st)), "b2s_partition_compress_rows_range_packed")
+    return dict(dst_off=dst_off, dst_len=dst_len, total=total.value, checksums=cks, status=st)
+
+
+def partition_compress_rows_range_dev(codec, d_records, rec_bytes, d_rec_len, n_records, keys, bounds, d_dst, dst_cap,
+                                      block_size=0, checksum_alg=CHECKSUM_NONE, level=0, dev=0):
+    """partition_compress_rows_range_packed on device addresses (records, u32 lengths, destination arena); the bounds
+    stay host memory"""
+    nk, kt, ko, kl, kn = _key_arrays(keys)
+    nb, bb, bbytes, bl = _bound_arrays(bounds)
+    dst_off, dst_len, cks, st = _partition_out(nb + 1)
+    total = _u64(0)
+    _check(load().b2s_partition_compress_rows_range_dev(
+        dev, codec, level, block_size, checksum_alg, n_records, d_records, rec_bytes, d_rec_len, nk, _ptr(kt), _ptr(ko),
+        _ptr(kl), _ptr(kn), nb, _ptr(bb), bbytes, _ptr(bl), d_dst, dst_cap, _ptr(dst_off), _ptr(dst_len),
+        C.addressof(total), _ptr(cks), _ptr(st)), "b2s_partition_compress_rows_range_dev")
     return dict(dst_off=dst_off, dst_len=dst_len, total=total.value, checksums=cks, status=st)
 
 

@@ -235,7 +235,7 @@ double ms_between(cudaEvent_t a, cudaEvent_t b) {
 
 // The timed marks of a slot's main stream, which b2s_last_timing is read from (add_times): kernel region (K), codec
 // step (T), upload (H), download (D), partition or sort step (P), row framing: walk + count, emit (F0-F1, F2-F3; the
-// hash step of a hash partition: F0-F1), grouping + merge of an aggregation (G).  Stop: where a call that did not
+// hash step of a hash partition, the range step of a range partition: F0-F1), grouping + merge of an aggregation (G).  Stop: where a call that did not
 // record the end of a span it reads stopped.
 enum Mark { K0, K1, T0, T1, H0, H1, D0, D1, P0, P1, F0, F1, F2, F3, G0, G1, kStop, kMarks };
 
@@ -844,7 +844,7 @@ void add_times(Slot& S, Family f) {
     case Family::kPartitionNone:  // partition step + checksum (without one, the gather); the partition step
       t.kernel_ms += S.span(P0, f == Family::kPartitionNone && !S.mine(K1) ? P1 : K1);
       t.top_kernel_ms += f == Family::kPartition ? S.span(T0, T1) : S.span(P0, P1);
-      if (S.mine(F0)) dominant(F0, F1);  // a hash partition: the hash step
+      if (S.mine(F0)) dominant(F0, F1);  // a hash or range partition: the hash or range step
       else S.take_pairs();
       break;
     case Family::kSort:       // verification + decode + sort; the sort step; the decoder's dominant pairs
@@ -1762,37 +1762,92 @@ static uint64_t first_record_past(const uint64_t* d_off, const uint32_t* d_len, 
   return lo;
 }
 
+// How a rows call computes its reduce ids on the device: Spark's HashPartitioning ids of the rows by these key columns,
+// or (range) its RangePartitioner ids over n_bounds bound rows of bound_bytes in host memory, bound_len[j] each
+struct RowIds {
+  KeySpec keys;
+  bool range = false;
+  uint32_t n_bounds = 0;
+  const uint8_t* bound_base = nullptr;
+  uint64_t bound_bytes = 0;
+  const uint32_t* bound_len = nullptr;
+};
+
+// The B2S_E_ARG of a rows call's verdict word (~0: none): a bad record (kHashBad*, launch_rows_hash), or for a range
+// call a bad bound or a bad record (launch_rows_range)
+static int row_ids_verdict(const RowIds& ids, uint64_t v) {
+  static const char* const why[] = {"", "bound_len is below 4", "its size prefix is not bound_len - 4",
+                                    "its row does not hold a key slot", "its row does not hold a key's null word",
+                                    "a string key runs past its row",
+                                    "a decimal key's size is not 1..16 or it runs past its row"};
+  static const char* const rec_why[] = {"", "rec_len is below 4", "its size prefix is not rec_len - 4"};
+  char msg[256];
+  if (ids.range && !(v & kRangeBadRecord)) {
+    if ((v & 7) == kRangeBadOrder)
+      snprintf(msg, sizeof msg, "bound %llu is not above the bound before it: the bounds must be strictly increasing",
+               (unsigned long long)(v >> 3));
+    else
+      snprintf(msg, sizeof msg, "bound %llu is not a serialized row of the key columns: %s",
+               (unsigned long long)(v >> 3), why[v & 7]);
+    return fail(B2S_E_ARG, "%s", msg);
+  }
+  v &= ~kRangeBadRecord;
+  snprintf(msg, sizeof msg, "record %llu is not a serialized row of the key columns: %s", (unsigned long long)(v >> 3),
+           (v & 7) < 3 ? rec_why[v & 7] : why[v & 7]);
+  return fail(B2S_E_ARG, "%s", msg);
+}
+
+// the range call's bounds into their workspace at d_ws: the rows and their offsets, one upload each
+static int upload_bounds(const RowIds& ids, uint8_t* d_ws, RangeWs* w, cudaStream_t st) {
+  *w = carve_rows_range_ws(d_ws, ids.n_bounds, ids.bound_bytes);
+  if (!ids.n_bounds) return 0;
+  std::vector<uint64_t> off(ids.n_bounds + 1, 0);
+  for (uint32_t j = 0; j < ids.n_bounds; j++) off[j + 1] = off[j] + ids.bound_len[j];
+  CU(cudaMemcpyAsync(w->off, off.data(), off.size() * 8, cudaMemcpyHostToDevice, st));
+  if (ids.bound_bytes) CU(cudaMemcpyAsync(w->rows, ids.bound_base, ids.bound_bytes, cudaMemcpyHostToDevice, st));
+  return 0;  // a copy from pageable memory has taken its source when it returns, so off may go
+}
+
 // The partition step and the compression of the non-empty partitions, on device-resident records.  d_dst receives the
 // .data arena (dst_cap bytes); *arena_bytes the bytes it needs.  Returns B2S_E_DST_TOO_SMALL (status[] set for the
 // partitions that do not fit) when dst_cap is short.  part_start (optional) receives the R + 1 partition offsets of the
-// partitioned records, which are in d_dst (codec NONE) or S.parena.  hash (d_part unused): the ids are Spark's
-// HashPartitioning ids of the rows by these key columns, computed between the offsets and the radix passes (marks F0
-// and F1 bracket that step), and a bad record fails the call.
+// partitioned records, which are in d_dst (codec NONE) or S.parena.  ids (d_part unused): the ids are computed from the
+// rows on the device (RowIds), between the offsets and the radix passes (marks F0 and F1 bracket that step: the hash
+// kernel, or the range call's bound checks and id kernel), and a bad record or bound fails the call.
 static int partition_compress_run(Device* D, Slot& S, uint32_t codec, int32_t level, uint32_t bs, uint32_t alg,
                                   uint32_t R, uint64_t n, const uint8_t* d_rec, uint64_t rec_bytes,
                                   const uint32_t* d_len, const uint32_t* d_part, uint8_t* d_dst, uint64_t dst_cap,
                                   uint64_t* dst_off, uint64_t* dst_len, uint64_t* checksum_out, int32_t* status,
                                   uint64_t* arena_bytes, uint64_t* launches,
-                                  std::vector<uint64_t>* part_start = nullptr, const KeySpec* hash = nullptr) {
+                                  std::vector<uint64_t>* part_start = nullptr, const RowIds* ids = nullptr) {
   cudaStream_t st = S.st;
   std::vector<uint64_t> pstart(R), plen(R);
+  const bool range = ids && ids->range;
   CU(S.mark(P0, st));
   PartitionPlan P;
   if (n) {
-    int rc = S.pws.ensure(partition_ws_bytes(n, R, hash != nullptr));
+    const size_t pws = partition_ws_bytes(n, R, ids != nullptr);
+    int rc = S.pws.ensure(pws + (range ? rows_range_ws_bytes(ids->n_bounds, ids->bound_bytes) : 0));
     if (rc) return rc;
     uint8_t* ws = (uint8_t*)S.pws.p;
-    if (hash) {
+    RangeWs rw;
+    if (range)
+      if (int rc = upload_bounds(*ids, ws + pws, &rw, st)) return rc;
+    if (ids) {
       launch_partition_offsets(d_len, nullptr, n, R, ws, &P, st, launches);
       CU(S.mark(F0, st, *launches));
-      launch_rows_hash(d_rec, rec_bytes, P.src_off, d_len, n, *hash, R, P.ids, P.readback, st, launches);
+      if (range)
+        launch_rows_range(d_rec, rec_bytes, P.src_off, d_len, n, ids->keys, rw, ids->n_bounds, P.ids, P.readback, st,
+                          launches);
+      else
+        launch_rows_hash(d_rec, rec_bytes, P.src_off, d_len, n, ids->keys, R, P.ids, P.readback, st, launches);
       CU(S.mark(F1, st, *launches));
       launch_partition_order(d_len, P.ids, n, R, ws, &P, st, launches);
     } else {
       launch_partition(d_len, d_part, n, R, ws, &P, st, launches);
     }
-    // the one readback between the partition step and compression: [bad id (hash: bad record), byte total, partition
-    // offsets]
+    // the one readback between the partition step and compression: [bad id (ids: bad record or bound), byte total,
+    // partition offsets]
     rc = S.hmeta.ensure(P.readback_bytes);
     if (rc) return rc;
     const uint64_t* rb = (const uint64_t*)S.hmeta.p;
@@ -1800,15 +1855,7 @@ static int partition_compress_run(Device* D, Slot& S, uint32_t codec, int32_t le
     CU(cudaStreamSynchronize(st));
     CU(cudaGetLastError());
     char msg[256];
-    if (hash && rb[0] != ~0ull) {
-      static const char* const why[] = {"", "rec_len is below 4", "its size prefix is not rec_len - 4",
-                                        "its row does not hold a key slot", "its row does not hold a key's null word",
-                                        "a string key runs past its row",
-                                        "a decimal key's size is not 1..16 or it runs past its row"};
-      snprintf(msg, sizeof msg, "record %llu is not a serialized row of the key columns: %s",
-               (unsigned long long)(rb[0] >> 3), why[rb[0] & 7]);
-      return fail(B2S_E_ARG, "%s", msg);
-    }
+    if (ids && rb[0] != ~0ull) return row_ids_verdict(*ids, rb[0]);
     if (rb[0] != ~0ull) {
       uint32_t id = 0;
       CU(cudaMemcpy(&id, d_part + rb[0], 4, cudaMemcpyDeviceToHost));
@@ -1834,6 +1881,23 @@ static int partition_compress_run(Device* D, Slot& S, uint32_t codec, int32_t le
     }
   } else if (rec_bytes) {
     return fail(B2S_E_ARG, "rec_len sums to 0 bytes, rec_bytes is %s", std::to_string(rec_bytes).c_str());
+  } else if (range && ids->n_bounds) {  // no records: the bounds are still checked, with a readback of their verdict
+    int rc = S.pws.ensure(rows_range_ws_bytes(ids->n_bounds, ids->bound_bytes));
+    if (rc) return rc;
+    RangeWs rw;
+    if (int rc = upload_bounds(*ids, (uint8_t*)S.pws.p, &rw, st)) return rc;
+    CU(cudaMemsetAsync(rw.verdict, 0xff, 8, st));
+    CU(S.mark(F0, st, *launches));
+    launch_rows_range(nullptr, 0, nullptr, nullptr, 0, ids->keys, rw, ids->n_bounds, nullptr, rw.verdict, st,
+                      launches);
+    CU(S.mark(F1, st, *launches));
+    rc = S.hmeta.ensure(8);
+    if (rc) return rc;
+    CU(cudaMemcpyAsync(S.hmeta.p, rw.verdict, 8, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    CU(cudaGetLastError());
+    const uint64_t v = *(const uint64_t*)S.hmeta.p;
+    if (v != ~0ull) return row_ids_verdict(*ids, v);
   }
   if (part_start) {
     part_start->assign(pstart.begin(), pstart.end());
@@ -1911,17 +1975,17 @@ static int partition_compress_run(Device* D, Slot& S, uint32_t codec, int32_t le
   return 0;
 }
 
-// hash: the ids are hashed from the rows, so rec_part is not read
+// ids: the ids are computed from the rows, so rec_part is not read
 static int partition_args(uint32_t codec, uint32_t bs, uint32_t alg, uint32_t R, uint64_t n, const void* rec_base,
                           uint64_t rec_bytes, const uint32_t* rec_len, const uint32_t* rec_part, const void* dst_base,
                           const uint64_t* dst_off, const uint64_t* dst_len, const int32_t* status,
-                          const KeySpec* hash) {
+                          const RowIds* ids) {
   if (alg > B2S_CHECKSUM_CRC32C) return fail(B2S_E_UNSUPPORTED, "Unsupported shuffle checksum algorithm%s");
   if (codec != B2S_CODEC_NONE)
     if (int rc = check_codec_block(codec, bs)) return rc;
   if (R < 1 || R > (1u << 24)) return fail(B2S_E_ARG, "num_partitions must be in [1, 2^24]%s");
   if (n > 0xffffffffull) return fail(B2S_E_ARG, "more than 2^32 - 1 records in one call%s");
-  if ((n && (!rec_len || (!rec_part && !hash))) || (rec_bytes && !rec_base) || !dst_off || !dst_len || !status)
+  if ((n && (!rec_len || (!rec_part && !ids))) || (rec_bytes && !rec_base) || !dst_off || !dst_len || !status)
     return fail(B2S_E_ARG, "null argument%s");
   if (rec_bytes && !dst_base) return fail(B2S_E_ARG, "null argument%s");
   return 0;
@@ -1936,12 +2000,12 @@ static int partition_compress_dev(uint32_t dev_index, uint32_t codec, int32_t le
                                   const uint8_t* rec_base, uint64_t rec_bytes, const uint32_t* rec_len,
                                   const uint32_t* rec_part, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_off,
                                   uint64_t* dst_len, uint64_t* dst_total, uint64_t* checksum_out, int32_t* status,
-                                  const KeySpec* hash) {
+                                  const RowIds* ids) {
   const WallTimer wt = begin_call();
   if (dst_total) *dst_total = 0;
   const uint32_t bs = block_size_or_default(codec_block_size);
   int rc = partition_args(codec, bs, checksum_alg, num_partitions, n_records, rec_base, rec_bytes, rec_len, rec_part,
-                          dst_base, dst_off, dst_len, status, hash);
+                          dst_base, dst_off, dst_len, status, ids);
   if (rc) return rc;
   Device* D;
   rc = get_device(dev_index, &D);
@@ -1953,7 +2017,7 @@ static int partition_compress_dev(uint32_t dev_index, uint32_t codec, int32_t le
   uint64_t launches = 0, arena = 0;
   rc = partition_compress_run(D, S, codec, level, bs, checksum_alg, num_partitions, n_records, rec_base, rec_bytes,
                               rec_len, rec_part, dst_base, dst_cap, dst_off, dst_len, cks.data(), status, &arena,
-                              &launches, nullptr, hash);
+                              &launches, nullptr, ids);
   if (rc && rc != B2S_E_DST_TOO_SMALL) return rc;
   if (checksum_out) memcpy(checksum_out, cks.data(), (size_t)num_partitions * 8);
   if (dst_total) *dst_total = arena;
@@ -1983,12 +2047,12 @@ static int partition_compress_packed(uint32_t codec, int32_t level, uint32_t cod
                                      uint64_t rec_bytes, const uint32_t* rec_len, const uint32_t* rec_part,
                                      uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_off, uint64_t* dst_len,
                                      uint64_t* dst_total, uint64_t* checksum_out, int32_t* status,
-                                     const ExStore* store, const KeySpec* hash = nullptr) {
+                                     const ExStore* store, const RowIds* ids = nullptr) {
   const WallTimer wt = begin_call();
   if (dst_total) *dst_total = 0;
   const uint32_t bs = block_size_or_default(codec_block_size);
   int rc = partition_args(codec, bs, checksum_alg, num_partitions, n_records, rec_base, rec_bytes, rec_len, rec_part,
-                          dst_base, dst_off, dst_len, status, hash);
+                          dst_base, dst_off, dst_len, status, ids);
   if (rc) return rc;
   Device* D;
   rc = get_device(t_device, &D);
@@ -2011,14 +2075,14 @@ static int partition_compress_packed(uint32_t codec, int32_t level, uint32_t cod
   if (rec_bytes) CU(cudaMemcpyAsync(d_rec, rec_base, rec_bytes, cudaMemcpyHostToDevice, st));
   if (n_records) {
     CU(cudaMemcpyAsync(d_len, rec_len, n_records * 4, cudaMemcpyHostToDevice, st));
-    if (!hash) CU(cudaMemcpyAsync(d_part, rec_part, n_records * 4, cudaMemcpyHostToDevice, st));
+    if (!ids) CU(cudaMemcpyAsync(d_part, rec_part, n_records * 4, cudaMemcpyHostToDevice, st));
   }
   CU(S.mark(H1, st));
   std::vector<uint64_t> cks(num_partitions), part_start;
   uint64_t launches = 0, arena = 0;
   rc = partition_compress_run(D, S, codec, level, bs, checksum_alg, num_partitions, n_records, d_rec, rec_bytes, d_len,
                               d_part, (uint8_t*)S.dst.p, S.dst.cap, dst_off, dst_len, cks.data(), status, &arena,
-                              &launches, store ? &part_start : nullptr, hash);
+                              &launches, store ? &part_start : nullptr, ids);
   if (rc) return rc;
   // the device arena is sized by the bound, so a short caller arena shows up here: copy what fits, flag the rest
   int result = 0;
@@ -2042,7 +2106,8 @@ static int partition_compress_packed(uint32_t codec, int32_t level, uint32_t cod
     const uint8_t* parts = (const uint8_t*)(codec == B2S_CODEC_NONE ? S.dst.p : S.parena.p);
     *store->cached = ex_store(D->ordinal, st, store->shuffle, store->map, parts, rec_bytes, std::move(part_start));
   }
-  end_call(wt, launches, CallBytes{rec_bytes, arena, rec_bytes + n_records * (hash ? 4 : 8), fit}, &S,
+  const uint64_t h2d = rec_bytes + n_records * (ids ? 4 : 8) + (ids && ids->range ? ids->bound_bytes : 0);
+  end_call(wt, launches, CallBytes{rec_bytes, arena, h2d, fit}, &S,
            partition_family(codec));
   return result;
 }
@@ -2522,8 +2587,9 @@ static int hash_args(uint32_t codec, uint32_t codec_block_size, uint32_t alg, ui
                      const void* rec_base, uint64_t rec_bytes, const uint32_t* rec_len, const RecordSpec& spec,
                      const void* dst_base, const uint64_t* dst_off, const uint64_t* dst_len, const int32_t* status) {
   const uint32_t bs = block_size_or_default(codec_block_size);
+  const RowIds ids{spec.keys};
   if (int rc = partition_args(codec, bs, alg, R, n, rec_base, rec_bytes, rec_len, nullptr, dst_base, dst_off, dst_len,
-                              status, &spec.keys))
+                              status, &ids))
     return rc;
   if (int rc = key_columns_args(spec)) return rc;
   for (uint32_t c = 0; c < spec.keys.n; c++) {
@@ -2545,12 +2611,13 @@ int b2s_partition_compress_rows_hash_packed(uint32_t codec, int32_t level, uint3
                                             uint64_t* dst_total, uint64_t* checksum_out, int32_t* status) {
   if (dst_total) *dst_total = 0;
   const RecordSpec spec = keys_spec(n_keys, key_type, key_off, key_len, key_null_field);
+  const RowIds ids{spec.keys};
   if (int rc = hash_args(codec, codec_block_size, checksum_alg, num_partitions, n_records, rec_base, rec_bytes, rec_len,
                          spec, dst_base, dst_off, dst_len, status))
     return rc;
   return partition_compress_packed(codec, level, codec_block_size, checksum_alg, num_partitions, n_records, rec_base,
                                    rec_bytes, rec_len, nullptr, dst_base, dst_cap, dst_off, dst_len, dst_total,
-                                   checksum_out, status, nullptr, &spec.keys);
+                                   checksum_out, status, nullptr, &ids);
 }
 
 int b2s_partition_compress_rows_hash_dev(uint32_t dev_index, uint32_t codec, int32_t level, uint32_t codec_block_size,
@@ -2562,12 +2629,92 @@ int b2s_partition_compress_rows_hash_dev(uint32_t dev_index, uint32_t codec, int
                                          uint64_t* checksum_out, int32_t* status) {
   if (dst_total) *dst_total = 0;
   const RecordSpec spec = keys_spec(n_keys, key_type, key_off, key_len, key_null_field);
+  const RowIds ids{spec.keys};
   if (int rc = hash_args(codec, codec_block_size, checksum_alg, num_partitions, n_records, rec_base, rec_bytes, rec_len,
                          spec, dst_base, dst_off, dst_len, status))
     return rc;
   return partition_compress_dev(dev_index, codec, level, codec_block_size, checksum_alg, num_partitions, n_records,
                                 rec_base, rec_bytes, rec_len, nullptr, dst_base, dst_cap, dst_off, dst_len, dst_total,
-                                checksum_out, status, &spec.keys);
+                                checksum_out, status, &ids);
+}
+
+// ------------------------------------------------------------------------------------------------------------
+// write side, range-partitioned rows: Spark's RangePartitioner id of every row, then the partition + compress step
+// ------------------------------------------------------------------------------------------------------------
+// The composite calls' column rules (order flags allowed), the partition step's checks with n_bounds + 1 partitions,
+// and the bound arrays'; a device is needed only after them, as for the hash call.
+static int range_args(uint32_t codec, uint32_t codec_block_size, uint32_t alg, uint64_t n, const void* rec_base,
+                      uint64_t rec_bytes, const uint32_t* rec_len, const RecordSpec& spec, const RowIds& ids,
+                      const void* dst_base, const uint64_t* dst_off, const uint64_t* dst_len, const int32_t* status) {
+  if (ids.n_bounds > (1u << 24) - 1) return fail(B2S_E_ARG, "n_bounds must be at most 2^24 - 1%s");
+  const uint32_t bs = block_size_or_default(codec_block_size);
+  if (int rc = partition_args(codec, bs, alg, ids.n_bounds + 1, n, rec_base, rec_bytes, rec_len, nullptr, dst_base,
+                              dst_off, dst_len, status, &ids))
+    return rc;
+  if (int rc = key_columns_args(spec)) return rc;
+  if (ids.n_bounds && (!ids.bound_base || !ids.bound_len)) return fail(B2S_E_ARG, "null argument%s");
+  uint64_t sum = 0;
+  for (uint32_t j = 0; j < ids.n_bounds; j++) sum += ids.bound_len[j];
+  if (sum != ids.bound_bytes) {
+    char msg[128];
+    snprintf(msg, sizeof msg, "bound_len sums to %llu bytes, bound_bytes is %llu", (unsigned long long)sum,
+             (unsigned long long)ids.bound_bytes);
+    return fail(B2S_E_ARG, "%s", msg);
+  }
+  if (!g_ctx)
+    if (int rc = no_device()) return rc;
+  return 0;
+}
+
+static RowIds range_ids(const RecordSpec& spec, uint32_t n_bounds, const uint8_t* bound_base, uint64_t bound_bytes,
+                        const uint32_t* bound_len) {
+  RowIds ids;
+  ids.keys = spec.keys;
+  ids.range = true;
+  ids.n_bounds = n_bounds;
+  ids.bound_base = bound_base;
+  ids.bound_bytes = bound_bytes;
+  ids.bound_len = bound_len;
+  return ids;
+}
+
+int b2s_partition_compress_rows_range_packed(uint32_t codec, int32_t level, uint32_t codec_block_size,
+                                             uint32_t checksum_alg, uint64_t n_records, const uint8_t* rec_base,
+                                             uint64_t rec_bytes, const uint32_t* rec_len, uint32_t n_keys,
+                                             const uint32_t* key_type, const uint32_t* key_off, const uint32_t* key_len,
+                                             const int32_t* key_null_field, uint32_t n_bounds,
+                                             const uint8_t* bound_base, uint64_t bound_bytes,
+                                             const uint32_t* bound_len, uint8_t* dst_base, uint64_t dst_cap,
+                                             uint64_t* dst_off, uint64_t* dst_len, uint64_t* dst_total,
+                                             uint64_t* checksum_out, int32_t* status) {
+  if (dst_total) *dst_total = 0;
+  const RecordSpec spec = keys_spec(n_keys, key_type, key_off, key_len, key_null_field);
+  const RowIds ids = range_ids(spec, n_bounds, bound_base, bound_bytes, bound_len);
+  if (int rc = range_args(codec, codec_block_size, checksum_alg, n_records, rec_base, rec_bytes, rec_len, spec, ids,
+                          dst_base, dst_off, dst_len, status))
+    return rc;
+  return partition_compress_packed(codec, level, codec_block_size, checksum_alg, n_bounds + 1, n_records, rec_base,
+                                   rec_bytes, rec_len, nullptr, dst_base, dst_cap, dst_off, dst_len, dst_total,
+                                   checksum_out, status, nullptr, &ids);
+}
+
+int b2s_partition_compress_rows_range_dev(uint32_t dev_index, uint32_t codec, int32_t level, uint32_t codec_block_size,
+                                          uint32_t checksum_alg, uint64_t n_records, const uint8_t* rec_base,
+                                          uint64_t rec_bytes, const uint32_t* rec_len, uint32_t n_keys,
+                                          const uint32_t* key_type, const uint32_t* key_off, const uint32_t* key_len,
+                                          const int32_t* key_null_field, uint32_t n_bounds, const uint8_t* bound_base,
+                                          uint64_t bound_bytes, const uint32_t* bound_len, uint8_t* dst_base,
+                                          uint64_t dst_cap, uint64_t* dst_off, uint64_t* dst_len, uint64_t* dst_total,
+                                          uint64_t* checksum_out, int32_t* status) {
+  if (dst_total) *dst_total = 0;
+  const RecordSpec spec = keys_spec(n_keys, key_type, key_off, key_len, key_null_field);
+  const RowIds ids = range_ids(spec, n_bounds, bound_base, bound_bytes, bound_len);
+  if (int rc = range_args(codec, codec_block_size, checksum_alg, n_records, rec_base, rec_bytes, rec_len, spec, ids,
+                          dst_base, dst_off, dst_len, status))
+    return rc;
+  return partition_compress_dev(dev_index, codec, level, codec_block_size, checksum_alg, n_bounds + 1, n_records,
+                                rec_base, rec_bytes, rec_len, nullptr, dst_base, dst_cap, dst_off, dst_len, dst_total,
+                                checksum_out, status, &ids);
 }
 
 // The whole-task buffers of a sort call (read-lane slot 0: compressed blocks, decoded arena, sorted copy, sort

@@ -340,6 +340,29 @@ void launch_rows_hash(const uint8_t* rec, uint64_t rec_bytes, const uint64_t* re
                       uint64_t n, const KeySpec& ks, uint32_t num_partitions, uint32_t* ids, uint64_t* bad,
                       cudaStream_t st, uint64_t* launches);
 
+// ---------------- rows_range.cu (Spark's RangePartitioner ids of length-prefixed UnsafeRow records) ----------------
+// n_bounds bound rows (< 2^24), framed as records ([size: int32 big-endian][row]) back to back: w.rows[w.off[j] ..
+// w.off[j + 1]), both uploaded by the caller into a workspace of rows_range_ws_bytes(n_bounds, bound_bytes) bytes.  Bound
+// j's key column c is its field c (the records' column's type, flags and key_len; slot 8 * ceil(n / 64) + 8 c, null bit
+// c when the records' column is nullable).  Records and key columns ks (order flags allowed) as launch_rows_hash's.
+// ids[i] = the number of bounds whose key is below record i's, by the key encoding (KeySpec): Spark's
+// RangePartitioner.getPartition over strictly increasing bounds.  Verdicts lower *bad (device, ~0 = none):
+//   a bad bound j: (j << 3) | its kHashBad* reason (as a record's), or kRangeBadOrder when its key is not above bound
+//   j - 1's; a bad record i: kRangeBadRecord | (i << 3) | its kHashBad* reason, so a bad bound always wins.
+// n == 0: only the bound step runs.
+constexpr uint64_t kRangeBadOrder = 7, kRangeBadRecord = 1ull << 63;
+struct RangeWs {
+  uint4* words;       // bound j: its first kKeyPrefixBytes encoded bytes (five big-endian words), its encoded length
+  uint64_t* off;      // n_bounds + 1 row offsets
+  uint8_t* rows;      // bound_bytes, with 16 bytes of slack
+  uint64_t* verdict;  // one word for a call without records
+};
+size_t rows_range_ws_bytes(uint32_t n_bounds, uint64_t bound_bytes);
+RangeWs carve_rows_range_ws(uint8_t* d_ws, uint32_t n_bounds, uint64_t bound_bytes);
+void launch_rows_range(const uint8_t* rec, uint64_t rec_bytes, const uint64_t* rec_off, const uint32_t* rec_len,
+                       uint64_t n, const KeySpec& ks, const RangeWs& w, uint32_t n_bounds, uint32_t* ids,
+                       uint64_t* bad, cudaStream_t st, uint64_t* launches);
+
 // ---------------- aggregate.cu (group key-sorted rows and merge their aggregate buffers) ----------------
 // Aggregate a: op[a] (B2S_AGG_*) over the 8-byte slot at row offset off[a], null bit null_field[a] (-1: never null).
 constexpr uint32_t kMaxAggs = 16;

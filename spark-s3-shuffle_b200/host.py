@@ -78,6 +78,7 @@ PROTOTYPES = [
     ("b2sh_reader_destroy", None, [_vp]),
     ("b2sh_serialized_writer_create", C.c_int, [_vp, _i32, _i64, _i32, C.POINTER(_vp)]),
     ("b2sh_serialized_writer_hash_rows", C.c_int, [_vp, _u32, _vp, _vp, _vp, _vp]),
+    ("b2sh_serialized_writer_range_rows", C.c_int, [_vp, _u32, _vp, _vp, _vp, _vp, _u32, _vp, _u64, _vp]),
     ("b2sh_serialized_writer_insert", C.c_int, [_vp, _i32, _vp, _u64]),
     ("b2sh_serialized_writer_commit", C.c_int, [_vp, _vp]),
     ("b2sh_serialized_writer_statistics", C.c_int, [_vp, C.POINTER(_u64), C.POINTER(_u64), C.c_char_p, _u32]),
@@ -291,6 +292,16 @@ class S3SerializedShuffleWriter:
         keys = list(keys)
         arrs = [np.array([k[i] for k in keys] or [0], dtype=np.int32 if i == 3 else np.uint32) for i in range(4)]
         _check(load().b2sh_serialized_writer_hash_rows(self._h, len(keys), *[a.ctypes.data for a in arrs]))
+
+    def rangeRows(self, keys, bounds):
+        """RangePartitioning by keys (as hashRows, order flags allowed) over bounds = the RangePartitioner's bound rows,
+        each framed as UnsafeRowSerializer writes it, before the first insert; len(bounds) + 1 must be numPartitions"""
+        keys, bounds = list(keys), [bytes(b) for b in bounds]
+        arrs = [np.array([k[i] for k in keys] or [0], dtype=np.int32 if i == 3 else np.uint32) for i in range(4)]
+        base = np.frombuffer(b"".join(bounds) or b"\0", dtype=np.uint8).copy()
+        bl = np.array([len(b) for b in bounds] or [0], dtype=np.uint32)
+        _check(load().b2sh_serialized_writer_range_rows(self._h, len(keys), *[a.ctypes.data for a in arrs], len(bounds),
+                                                        base.ctypes.data, sum(len(b) for b in bounds), bl.ctypes.data))
 
     def insertRecord(self, partitionId, record):
         a = np.frombuffer(record, dtype=np.uint8) if not isinstance(record, np.ndarray) else np.ascontiguousarray(record)

@@ -521,6 +521,18 @@ class S3SerializedShuffleWriter {
     keyLen_.assign(len, len + nKeys);
     keyNull_.assign(nullField, nullField + nKeys);
   }
+  // RangePartitioning by these key columns over these bounds (b2s_partition_compress_rows_range_packed): as hashRows,
+  // with Spark's RangePartitioner ids; the writer's numPartitions is the bounds' count + 1
+  void rangeRows(uint32_t nKeys, const uint32_t* type, const uint32_t* off, const uint32_t* len, const int32_t* nullField,
+                 uint32_t nBounds, const uint8_t* boundBase, uint64_t boundBytes, const uint32_t* boundLen) {
+    if ((uint64_t)nBounds + 1 != (uint64_t)numPartitions_)
+      throw RuntimeException("Precondition: range_rows needs n_bounds + 1 == numPartitions.");
+    if (nBounds && (!boundBase || !boundLen)) throw RuntimeException("Precondition: null bound arrays.");
+    hashRows(nKeys, type, off, len, nullField);
+    range_ = true;
+    boundRows_.assign(boundBase, boundBase + (nBounds ? boundBytes : 0));
+    boundLen_.assign(boundLen, boundLen + nBounds);
+  }
   void insertRecord(int32_t partitionId, const uint8_t* b, uint64_t n) {
     const bool hashed = !keyType_.empty();
     if (!hashed && (partitionId < 0 || partitionId >= numPartitions_))
@@ -542,7 +554,14 @@ class S3SerializedShuffleWriter {
     uint64_t total = 0;
     int rc;
     const char* call = "b2s_partition_compress_packed";
-    if (!keyType_.empty()) {  // hashed rows: never cached (the exchange cache's reads serve fixed-size records only)
+    if (range_) {  // range-partitioned rows: never cached, as hashed ones
+      call = "b2s_partition_compress_rows_range_packed";
+      rc = b2s_partition_compress_rows_range_packed(
+          codec, d_.zstdLevel, d_.lz4BlockSize, alg, recLen_.size(), records_.data(), records_.size(), recLen_.data(),
+          (uint32_t)keyType_.size(), keyType_.data(), keyOff_.data(), keyLen_.data(), keyNull_.data(),
+          (uint32_t)boundLen_.size(), boundRows_.data(), boundRows_.size(), boundLen_.data(), out_.data(), bound,
+          doff.data(), dlen.data(), &total, cks.data(), status.data());
+    } else if (!keyType_.empty()) {  // hashed rows: never cached (the exchange cache's reads serve fixed-size records only)
       call = "b2s_partition_compress_rows_hash_packed";
       rc = b2s_partition_compress_rows_hash_packed(
           codec, d_.zstdLevel, d_.lz4BlockSize, alg, R, recLen_.size(), records_.data(), records_.size(),
@@ -581,6 +600,9 @@ class S3SerializedShuffleWriter {
   std::vector<uint32_t> recLen_, recPart_;
   std::vector<uint32_t> keyType_, keyOff_, keyLen_;  // hashRows' key columns (empty: the caller's partition ids)
   std::vector<int32_t> keyNull_;
+  bool range_ = false;  // rangeRows: the ids are RangePartitioner ids over these bounds
+  std::vector<uint8_t> boundRows_;
+  std::vector<uint32_t> boundLen_;
   std::unique_ptr<S3MeasureOutputStream> measure_;
 };
 
@@ -1282,6 +1304,14 @@ int b2sh_serialized_writer_create(b2sh_dispatcher* d, int32_t shuffle_id, int64_
 int b2sh_serialized_writer_hash_rows(b2sh_serialized_writer* w, uint32_t n_keys, const uint32_t* key_type,
                                      const uint32_t* key_off, const uint32_t* key_len, const int32_t* key_null_field) {
   return guarded([&] { w->w->hashRows(n_keys, key_type, key_off, key_len, key_null_field); });
+}
+int b2sh_serialized_writer_range_rows(b2sh_serialized_writer* w, uint32_t n_keys, const uint32_t* key_type,
+                                      const uint32_t* key_off, const uint32_t* key_len, const int32_t* key_null_field,
+                                      uint32_t n_bounds, const uint8_t* bound_base, uint64_t bound_bytes,
+                                      const uint32_t* bound_len) {
+  return guarded([&] {
+    w->w->rangeRows(n_keys, key_type, key_off, key_len, key_null_field, n_bounds, bound_base, bound_bytes, bound_len);
+  });
 }
 int b2sh_serialized_writer_insert(b2sh_serialized_writer* w, int32_t partition_id, const uint8_t* bytes, uint64_t len) {
   return guarded([&] { w->w->insertRecord(partition_id, bytes, len); });
