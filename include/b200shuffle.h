@@ -79,6 +79,13 @@ extern "C" {
 #define B2S_AGG_MAX_INT64 5
 #define B2S_AGG_MIN_FLOAT64 6
 #define B2S_AGG_MAX_FLOAT64 7
+/* Decimal buffers (8 is unassigned).  SUM_DECIMAL carries the buffer's precision P (1..38) in bits 8..15:
+ * B2S_AGG_SUM_DECIMAL | (P << 8).  P <= 18: the slot holds the unscaled long; P > 18: the slot is (offset << 32) | size
+ * naming 1..16 big-endian two's-complement bytes, as B2S_DECIMAL_KEY reads them.  MIN / MAX_DECIMAL take a
+ * Decimal(p > 18) slot in that out-of-line form; a Decimal(p <= 18) min / max is MIN / MAX_INT64. */
+#define B2S_AGG_SUM_DECIMAL (9)  /* Sum(decimal)'s and Average(decimal)'s sum: exact, null on overflow of 10^P */
+#define B2S_AGG_MIN_DECIMAL (10) /* Min(decimal p > 18) */
+#define B2S_AGG_MAX_DECIMAL (11) /* Max(decimal p > 18) */
 
 /* per-block status / call errors.  The Scala shim maps them to the reference's exception types:            */
 #define B2S_OK 0
@@ -379,17 +386,42 @@ int b2s_decompress_sort_rows_dev(uint32_t dev_index, uint32_t codec, uint32_t ch
  *                             equal values the first in stable order is kept with its exact bits (Least / Greatest)
  * A group with no non-null input for aggregate a gets its null bit set and an all-zero slot (UnsafeRow.setNullAt);
  * otherwise the null bit is cleared and the slot holds the result.  n_aggs = 0 keeps the first row of every key.
+ * The Decimal ops:
+ *   B2S_AGG_SUM_DECIMAL | P << 8 : Spark's Sum / Average decimal merge into an UnsafeRow buffer (Sum.mergeExpressions
+ *       with DecimalAddNoOverflowCheck, Average's sum.left + sum.right, each result written by UnsafeRow.setDecimal(...,
+ *       P), whose changePrecision(P) turns an overflow into null).  Over the group's records in stable order, starting
+ *       from 0, the result is null when some input is null (a decimal sum buffer is null only after an overflow; its
+ *       initial value is 0) or some running sum S_k has |S_k| >= 10^P; the null sticks, later inputs do not clear it.
+ *       Otherwise it is the exact sum.  Unlike the other ops it propagates nulls, so it needs agg_null_field[a] >= 0.
+ *   B2S_AGG_MIN/MAX_DECIMAL : the signed minimum / maximum of the non-null inputs; null when there is none.
+ *   A result is written as UnsafeRow.setDecimal writes it.  P <= 18: the long, or an all-zero slot when null.  Out of
+ *   line (P > 18, and MIN / MAX_DECIMAL): the 16 bytes at the head row's offset are zeroed; a non-null result's minimal
+ *   two's-complement bytes (BigInteger.toByteArray: bitlen(x >= 0 ? x : ~x) / 8 + 1 of them, so 0 is 00, 128 is
+ *   00 80, -128 is 80) go there and the slot becomes (offset << 32) | length; a null result leaves the slot
+ *   offset << 32 ("keep the offset for future update") with the null bit set.
+ *   Spark's buffers map to them so (the final If(isEmpty, null, sum), overflow check or ANSI error stay on the CPU):
+ *     Sum(decimal) [sum, isEmpty]     : SUM_DECIMAL | P << 8 on sum, MIN_INT32 on isEmpty (a BooleanType slot is byte 0
+ *                                       with bytes 1..7 zero, so the minimum is the AND Spark merges with)
+ *     Average(decimal) [sum, count]   : SUM_DECIMAL | P << 8, SUM_INT64
+ *     Min / Max(decimal p > 18)       : MIN / MAX_DECIMAL
  * Output: one record per group, back to back, groups in the row sort's order (ascending, nulls first) — again a valid
  * UnsafeRowSerializer stream.  A group's record is its first record in stable order, byte for byte (size prefix and
  * variable-length region included) except each aggregate's slot and null bit.  *dst_total = output bytes, *n_records =
  * input records, *n_groups = output records.  The output is never longer than the decoded input, so a dst_cap of at
  * least the decoded bytes never gets B2S_E_DST_TOO_SMALL.
  * Per block, B2S_E_CORRUPT for every framing rule of b2s_decompress_sort_rows_packed and when a row is shorter than an
- * aggregate slot (agg_off[a] + 8) or an aggregate's null word.  Checksums, "nothing is written when a block fails"
+ * aggregate slot (agg_off[a] + 8) or an aggregate's null word.  With an out-of-line Decimal aggregate also, for the
+ * block of the first bad record: a non-null input whose size is not 1..16 or whose bytes run past its row; a record
+ * whose 16-byte region [offset, offset + 16) is not inside its row (any record can be a group's head), or starts
+ * before the end of a key or aggregate slot or a null word the call uses.  The region is not checked against a string
+ * or decimal key's out-of-line bytes or another decimal's region: Spark gives each its own bytes, and a row that
+ * shares them gets a merged decimal written over them.  Checksums, "nothing is written when a block fails"
  * (*n_records = *n_groups = 0, the call returns 0), B2S_E_NOMEM, codec NONE, the read lane and the 1 GiB buffer trim
  * are as in b2s_decompress_sort_*.  dst_cap below the output bytes -> B2S_E_DST_TOO_SMALL with *dst_total = the bytes
  * needed.
- * Errors -> B2S_E_ARG: those of b2s_decompress_sort_rows_packed; n_aggs > 16; an unknown op; agg_null_field[a] < -1;
+ * Errors -> B2S_E_ARG: those of b2s_decompress_sort_rows_packed; n_aggs > 16; an unknown op; precision bits on any op
+ * but SUM_DECIMAL, or a SUM_DECIMAL precision of 0 or above 38; SUM_DECIMAL with agg_null_field[a] = -1;
+ * agg_null_field[a] < -1;
  * NULL agg arrays with n_aggs > 0; an aggregate slot that overlaps another slot, the key bytes, or an 8-byte null word
  * that the key or an aggregate uses.
  * Timing (b2s_last_timing): kernel_ms = the whole call; top_kernel_ms = framing + keys + radix + aggregation;

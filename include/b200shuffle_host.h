@@ -175,8 +175,8 @@ int b2sh_reader_read_sorted_rows(b2sh_reader* r, uint32_t key_type, uint32_t key
 /* read_aggregated_rows(): read() for a Spark SQL exchange whose reducer merges partial aggregates by one typed key
  * (INTEGRATION.md §3h, spark.shuffle.s3.gpu.aggregateRows).  Fetches the task's non-empty blocks as read_sorted_rows()
  * does, then makes ONE b2s_decompress_aggregate_rows_packed call with the key and the n_aggs aggregates (agg_op /
- * agg_off / agg_null_field as there): *data / *len receive one UnsafeRowSerializer record per key, in the row sort's
- * order, *n_records the input records and *n_groups the output records.  The buffer stays valid until the reader's next
+ * agg_off / agg_null_field as there, the Decimal ops included): *data / *len receive one UnsafeRowSerializer record
+ * per key, in the row sort's order, *n_records the input records and *n_groups the output records.  The buffer stays valid until the reader's next
  * read or its destruction.  A checksum mismatch returns B2SH_E_SPARK with the reference's message, a malformed row
  * stream B2SH_E_IO.  The exchange cache is not consulted: every block is fetched. */
 int b2sh_reader_read_aggregated_rows(b2sh_reader* r, uint32_t key_type, uint32_t key_off, uint32_t key_len,

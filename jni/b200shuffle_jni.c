@@ -474,8 +474,8 @@ JNIEXPORT jint JNICALL J(decompressSortRowsPacked)(JNIEnv* e, jclass c, jint cod
 
 /* ---- read side, aggregated (a Spark SQL exchange read followed by a HashAggregateExec(Final), INTEGRATION.md §3h):
  *      verify, decode, group the task's UnsafeRow records by one typed key and merge nAggs aggregates (aggOp /
- *      aggOff / aggNullField: int[nAggs], B2S_AGG_* ops).  meta: long[3] = {dst_total, n_records, n_groups}; other
- *      arrays as decompressSortRowsPacked. ---- */
+ *      aggOff / aggNullField: int[nAggs], B2S_AGG_* ops, B2S_AGG_SUM_DECIMAL with its precision in bits 8..15).
+ *      meta: long[3] = {dst_total, n_records, n_groups}; other arrays as decompressSortRowsPacked. ---- */
 JNIEXPORT jint JNICALL J(decompressAggregateRowsPacked)(JNIEnv* e, jclass c, jint codec, jint alg, jint n, jlong src,
                                                         jlongArray off, jlongArray len, jintArray sliceBase,
                                                         jlongArray sliceLen, jlongArray sliceChecksum, jint keyType,

@@ -20,11 +20,19 @@ KEY_DESCENDING, KEY_NULLS_LAST = 1 << 8, 1 << 9
 # aggregate ops of the row aggregation (decompress_aggregate_rows_*)
 (AGG_SUM_INT64, AGG_SUM_FLOAT64, AGG_MIN_INT32, AGG_MAX_INT32, AGG_MIN_INT64, AGG_MAX_INT64, AGG_MIN_FLOAT64,
  AGG_MAX_FLOAT64) = range(8)
+# the Decimal ops (8 is unassigned); SUM_DECIMAL takes its buffer's precision P (1..38) as AGG_SUM_DECIMAL | P << 8
+AGG_SUM_DECIMAL, AGG_MIN_DECIMAL, AGG_MAX_DECIMAL = 9, 10, 11
 OK, E_CORRUPT, E_CHECKSUM, E_DST_TOO_SMALL, E_UNSUPPORTED, E_ARG, E_CUDA, E_NOT_INIT, E_NOMEM, E_NOT_CACHED = (
     0, -1, -2, -3, -4, -5, -6, -7, -8, -9)
 NOT_RESIDENT = 2**64 - 1  # b2s_exchange_lookup's length of a map output that is not resident
 CODEC_BY_NAME = {"lz4": CODEC_LZ4BLOCK, "snappy": CODEC_SNAPPY_XERIAL, "zstd": CODEC_ZSTD}
 CHECKSUM_BY_NAME = {"ADLER32": CHECKSUM_ADLER32, "CRC32": CHECKSUM_CRC32, "CRC32C": CHECKSUM_CRC32C}
+
+
+def agg_sum_decimal(precision):
+    """the op of a Decimal(precision) sum buffer"""
+    return AGG_SUM_DECIMAL | (precision << 8)
+
 
 _u8p, _u64p, _u32p, _i32p, _vp = C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p
 _u32, _u64, _i32 = C.c_uint32, C.c_uint64, C.c_int32

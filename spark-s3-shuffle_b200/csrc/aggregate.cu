@@ -15,9 +15,17 @@
 //             lane's value broadcast in turn), so it is bit for bit the sequential sum.  One thread writes an output
 //             row's slots and then its null words, one read-modify-write per aggregate, so aggregates (and the key)
 //             that share a null word never race.
+// The Decimal ops (B2S_AGG_*_DECIMAL) are merged by kernels of their own (the *_dec kernels, launched only when the spec
+// has one), so the kernels of the other ops keep their code and registers.  An out-of-line decimal is staged by the
+// heads step as 16 bytes (the value's low words in vals, its high words in vhi), which also checks every record's
+// 16-byte region.  The sum is exact and null once an input is null or a running sum leaves (-10^P, 10^P): a thread adds
+// with the 128-bit overflow of decimal128.h; a warp scans each round of 32 inputs in three 64-bit words (33 * 10^38 <
+// 2^133), adds the rounds before it and checks every lane's running sum with one vote.
 #include <algorithm>
 
+#include "decimal128.h"
 #include "kernels.h"
+#include "rows_key.cuh"
 
 namespace b2s {
 
@@ -34,8 +42,9 @@ inline unsigned grid_for(uint64_t n) {
   return (unsigned)(want < (uint64_t)kSMs * 16 ? (want ? want : 1) : (uint64_t)kSMs * 16);
 }
 
-// the aggregate workspace: heads (scanned in place), readback [groups, output bytes], per group the head's record
-// index, first position (+ n at the end) and record length, the dense null bits and values, the spec
+// the aggregate workspace: heads (scanned in place), readback [groups, output bytes, decimal verdict], per group the
+// head's record index, first position (+ n at the end) and record length, the dense null bits and values, the high
+// words of the out-of-line decimals, the spec
 struct AggWs {
   uint64_t* head;
   uint64_t* readback;
@@ -44,19 +53,21 @@ struct AggWs {
   uint32_t* glen;
   uint32_t* nulls;
   uint64_t* vals;
+  uint64_t* vhi;
   AggSpec* spec;
 };
 
-AggWs carve_agg_ws(uint8_t* d_aws, uint64_t n, uint32_t n_aggs) {
+AggWs carve_agg_ws(uint8_t* d_aws, uint64_t n, uint32_t n_aggs, uint32_t n_wide) {
   AggWs a;
   uint8_t* p = d_aws;
   a.head = (uint64_t*)p;     p += a256(n * 8);
-  a.readback = (uint64_t*)p; p += a256(16);
+  a.readback = (uint64_t*)p; p += a256(24);
   a.hidx = (uint32_t*)p;     p += a256(n * 4);
   a.gpos = (uint32_t*)p;     p += a256((n + 1) * 4);
   a.glen = (uint32_t*)p;     p += a256(n * 4);
   a.nulls = (uint32_t*)p;    p += a256(n * 4);
   a.vals = (uint64_t*)p;     p += a256(n * n_aggs * 8);
+  a.vhi = (uint64_t*)p;      p += a256(n * n_wide * 8);
   a.spec = (AggSpec*)p;
   return a;
 }
@@ -67,14 +78,19 @@ __device__ __forceinline__ bool bit_set(const uint8_t* row, int32_t field) {
   return (w >> (field & 63)) & 1;
 }
 
+// Dec (a spec with an out-of-line decimal): such an aggregate's value is staged as (vals, vhi) = its (lo, hi), 0 when
+// null, and a record whose value or 16-byte region is bad lowers *bad to its arena offset << 2 | kAggBad*
+template <bool Dec>
 __global__ void __launch_bounds__(kAggThreads) agg_heads_kernel(const uint8_t* __restrict__ arena,
                                                                 const uint64_t* __restrict__ rec_off,
+                                                                const uint32_t* __restrict__ rec_len,
                                                                 const uint32_t* __restrict__ idx, uint64_t n,
                                                                 const uint32_t* __restrict__ words, uint32_t W,
                                                                 const uint32_t* __restrict__ heads,
                                                                 const AggSpec* __restrict__ spec,
                                                                 uint64_t* __restrict__ head, uint32_t* __restrict__ nulls,
-                                                                uint64_t* __restrict__ vals) {
+                                                                uint64_t* __restrict__ vals, uint64_t* __restrict__ vhi,
+                                                                unsigned long long* __restrict__ bad) {
   const uint32_t n_aggs = spec->n;
   for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (uint64_t)gridDim.x * blockDim.x) {
     const uint32_t i = idx ? idx[j] : (uint32_t)j;
@@ -93,9 +109,26 @@ __global__ void __launch_bounds__(kAggThreads) agg_heads_kernel(const uint8_t* _
     for (uint32_t a = 0; a < n_aggs; a++) {
       uint64_t v, unused;
       ld_span16<true>(row + spec->off[a], 8, v, unused);
-      vals[(size_t)a * n + j] = v;
       const int32_t nf = spec->null_field[a];
-      if (nf >= 0 && bit_set(row, nf)) nm |= 1u << a;
+      const bool null = nf >= 0 && bit_set(row, nf);
+      if (null) nm |= 1u << a;
+      if (Dec && agg_decimal_wide(spec->op[a])) {
+        const uint32_t size = rec_len[i] - 4, so = (uint32_t)(v >> 32);
+        uint64_t hi = 0, lo = 0;
+        bool bad_value = false;
+        if (!null) {
+          decimal_bits(row, size, v, hi, lo, &bad_value);
+          hi ^= 1ull << 63;  // decimal_bits flips the sign bit for the sort
+        }
+        const uint64_t why = bad_value                      ? kAggBadDecimal
+                             : (uint64_t)so + 16 > size     ? kAggBadRegionEnd
+                             : so < spec->region_from       ? kAggBadRegionStart
+                                                            : 0;
+        if (why) atomicMin(bad, (unsigned long long)((rec_off[i] << 2) | why));
+        v = lo;
+        vhi[(size_t)spec->wide[a] * n + j] = hi;
+      }
+      vals[(size_t)a * n + j] = v;
     }
     nulls[j] = nm;
   }
@@ -328,20 +361,242 @@ __global__ void __launch_bounds__(kAggThreads) agg_merge_large_kernel(const uint
   }
 }
 
-}  // namespace
-
-size_t rows_aggregate_ws_bytes(uint64_t n, uint32_t n_aggs) {
-  return a256(n * 8) + a256(16) + 3 * a256(n * 4) + a256((n + 1) * 4) + a256(n * n_aggs * 8) + a256(sizeof(AggSpec));
+// ---- the Decimal ops ----
+// aggregate a (a Decimal op; wa: its index among the out-of-line ones) of the records at positions [s, e), by one
+// thread; returns false when the result is null
+__device__ __forceinline__ bool merge_thread_dec(uint32_t op, uint32_t a, uint32_t wa,
+                                                 const uint64_t* __restrict__ vals, const uint64_t* __restrict__ vhi,
+                                                 const uint32_t* __restrict__ nulls, uint64_t n, uint32_t s, uint32_t e,
+                                                 Dec128* out) {
+  const uint64_t* va = vals + (size_t)a * n;
+  const uint64_t* ha = vhi + (size_t)wa * n;
+  const bool wide = agg_decimal_wide(op);
+  if (agg_base_op(op) == B2S_AGG_SUM_DECIMAL) {  // stable order from 0: null at the first null input or overflow
+    const uint32_t P = agg_precision(op);
+    Dec128 acc{0, 0};
+    for (uint32_t j = s; j < e; j++) {
+      if ((__ldg(nulls + j) >> a) & 1) return false;
+      const Dec128 x = wide ? Dec128{__ldg(va + j), __ldg(ha + j)} : dec_of_long(__ldg(va + j));
+      bool ovf;
+      acc = dec_add(acc, x, &ovf);
+      if (ovf || !dec_fits(acc, P)) return false;
+    }
+    *out = acc;
+    return true;
+  }
+  const bool mx = agg_base_op(op) == B2S_AGG_MAX_DECIMAL;
+  bool has = false;
+  Dec128 best{0, 0};
+  for (uint32_t j = s; j < e; j++) {
+    if ((__ldg(nulls + j) >> a) & 1) continue;
+    const Dec128 x{__ldg(va + j), __ldg(ha + j)};
+    if (!has || (mx ? dec_less(best, x) : dec_less(x, best))) best = x;
+    has = true;
+  }
+  *out = best;
+  return has;
 }
 
-uint64_t* rows_aggregate_readback(uint8_t* d_aws, uint64_t n, uint32_t n_aggs) {
-  return carve_agg_ws(d_aws, n, n_aggs).readback;
+// (a2, a1, a0) += (b2, b1, b0): 192-bit two's complement
+__device__ __forceinline__ void add192(uint64_t& a0, uint64_t& a1, uint64_t& a2, uint64_t b0, uint64_t b1,
+                                       uint64_t b2) {
+  a0 += b0;
+  const uint64_t c0 = a0 < b0 ? 1 : 0;
+  uint64_t t = a1 + b1;
+  uint64_t c1 = t < b1 ? 1 : 0;
+  t += c0;
+  c1 += t < c0 ? 1 : 0;
+  a1 = t;
+  a2 += b2 + c1;
+}
+
+// merge_thread_dec by the whole warp (every lane returns the result).  The sum: per round of 32 records an inclusive
+// scan of the inputs in three 64-bit words plus the running sum of the rounds before; the result is null as soon as
+// any lane's input is null or any lane's running sum is out of range (one vote each, so the decision is warp-uniform),
+// and no further rounds are loaded.  Min / max: each lane over its records, then the lanes combined, the earliest
+// position kept among equal values.  Loads: four rounds of 32 in flight, as merge_warp.
+__device__ __forceinline__ bool merge_warp_dec(uint32_t op, uint32_t a, uint32_t wa, const uint64_t* __restrict__ vals,
+                                               const uint64_t* __restrict__ vhi, const uint32_t* __restrict__ nulls,
+                                               uint64_t n, uint32_t s, uint32_t e, uint32_t lane, Dec128* out) {
+  const uint64_t* va = vals + (size_t)a * n;
+  const uint64_t* ha = vhi + (size_t)wa * n;
+  const bool wide = agg_decimal_wide(op);
+  if (agg_base_op(op) == B2S_AGG_SUM_DECIMAL) {
+    const uint32_t P = agg_precision(op);
+    uint64_t c0 = 0, c1 = 0, c2 = 0;  // the running sum before the round
+    bool null = false;
+    for (uint32_t b = s; b < e && !null; b += 128) {
+      Dec128 x[4];
+      bool nl[4];
+#pragma unroll
+      for (int r = 0; r < 4; r++) {
+        const uint32_t j = b + 32 * r + lane;
+        nl[r] = j < e && ((__ldg(nulls + j) >> a) & 1);
+        const bool in = j < e && !nl[r];
+        const uint64_t lo = in ? __ldg(va + j) : 0;
+        x[r] = wide ? Dec128{lo, in ? __ldg(ha + j) : 0} : dec_of_long(lo);
+      }
+#pragma unroll
+      for (int r = 0; r < 4; r++) {
+        if (__any_sync(FULL, nl[r])) {
+          null = true;
+          break;
+        }
+        uint64_t p0 = x[r].lo, p1 = x[r].hi, p2 = (uint64_t)((int64_t)x[r].hi >> 63);
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+          const uint64_t q0 = __shfl_up_sync(FULL, p0, d), q1 = __shfl_up_sync(FULL, p1, d),
+                         q2 = __shfl_up_sync(FULL, p2, d);
+          if (lane >= (uint32_t)d) add192(p0, p1, p2, q0, q1, q2);
+        }
+        add192(p0, p1, p2, c0, c1, c2);
+        const bool ok = p2 == (uint64_t)((int64_t)p1 >> 63) && dec_fits(Dec128{p0, p1}, P);
+        if (__any_sync(FULL, !ok)) {
+          null = true;
+          break;
+        }
+        c0 = __shfl_sync(FULL, p0, 31);
+        c1 = __shfl_sync(FULL, p1, 31);
+        c2 = __shfl_sync(FULL, p2, 31);
+      }
+    }
+    *out = Dec128{c0, c1};
+    return !null;
+  }
+  const bool mx = agg_base_op(op) == B2S_AGG_MAX_DECIMAL;
+  bool has = false;
+  Dec128 best{0, 0};
+  uint32_t pbest = 0;
+  for (uint32_t b = s; b < e; b += 128) {
+    Dec128 x[4];
+    bool in[4];
+#pragma unroll
+    for (int r = 0; r < 4; r++) {
+      const uint32_t j = b + 32 * r + lane;
+      in[r] = j < e && !((__ldg(nulls + j) >> a) & 1);
+      x[r] = in[r] ? Dec128{__ldg(va + j), __ldg(ha + j)} : Dec128{0, 0};
+    }
+#pragma unroll
+    for (int r = 0; r < 4; r++) {
+      if (!in[r]) continue;
+      if (!has || (mx ? dec_less(best, x[r]) : dec_less(x[r], best))) {
+        best = x[r];
+        pbest = b + 32 * r + lane;
+      }
+      has = true;
+    }
+  }
+  const bool any = __any_sync(FULL, has);
+#pragma unroll
+  for (int d = 16; d; d >>= 1) {
+    const bool oh = __shfl_xor_sync(FULL, has, d);
+    const Dec128 o{__shfl_xor_sync(FULL, best.lo, d), __shfl_xor_sync(FULL, best.hi, d)};
+    const uint32_t op_ = __shfl_xor_sync(FULL, pbest, d);
+    const bool eq = o.lo == best.lo && o.hi == best.hi;
+    if (oh && (!has || (mx ? dec_less(best, o) : dec_less(o, best)) || (eq && op_ < pbest))) {
+      has = true;
+      best = o;
+      pbest = op_;
+    }
+  }
+  *out = best;
+  return any;
+}
+
+// a Decimal op's result into the output row.  A compact sum (P <= 18): as put.  Out of line: the 16 bytes at the row's
+// own offset zeroed, the minimal bytes written there and the slot (offset << 32) | length; null: the slot offset << 32
+// (UnsafeRow.setDecimal keeps the offset for a later update) and the null bit.
+__device__ __forceinline__ void put_decimal(uint8_t* row, uint32_t op, uint32_t off, uint32_t a, bool has, Dec128 x,
+                                            uint32_t* null_mask) {
+  if (!agg_decimal_wide(op)) {
+    put(row, op, off, a, has, x.lo, null_mask);
+    return;
+  }
+  uint64_t slot, unused;
+  ld_span16<false>(row + off, 8, slot, unused);
+  const uint32_t so = (uint32_t)(slot >> 32);
+  uint64_t m0 = 0, m1 = 0;
+  uint32_t len = 0;
+  if (has) {
+    len = dec_bytes(x);
+    dec_encode(x, len, &m0, &m1);
+  }
+  st_span16(row + so, 16, m0, m1);
+  st_span16(row + off, 8, ((uint64_t)so << 32) | len, 0);
+  if (!has) *null_mask |= 1u << a;
+}
+
+__device__ __forceinline__ bool is_decimal(uint32_t op) { return agg_base_op(op) >= B2S_AGG_SUM_DECIMAL; }
+
+// agg_merge_small_kernel for a spec with a Decimal op
+__global__ void __launch_bounds__(kAggThreads) agg_merge_small_dec_kernel(
+    const uint32_t* __restrict__ gpos, uint64_t G, uint64_t n, const uint64_t* __restrict__ vals,
+    const uint64_t* __restrict__ vhi, const uint32_t* __restrict__ nulls, const AggSpec* __restrict__ spec,
+    uint32_t n_aggs, const uint64_t* __restrict__ gdst, uint8_t* __restrict__ dst) {
+  for (uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; g < G; g += (uint64_t)gridDim.x * blockDim.x) {
+    const uint32_t s = gpos[g], e = gpos[g + 1];
+    if (e - s > kSmallGroup) continue;
+    uint8_t* row = dst + gdst[g] + 4;
+    uint32_t null_mask = 0;
+    for (uint32_t a = 0; a < n_aggs; a++) {
+      const uint32_t op = spec->op[a];
+      if (is_decimal(op)) {
+        Dec128 x;
+        const bool has = merge_thread_dec(op, a, spec->wide[a], vals, vhi, nulls, n, s, e, &x);
+        put_decimal(row, op, spec->off[a], a, has, x, &null_mask);
+      } else {
+        uint64_t v;
+        const bool has = merge_thread(op, a, vals, nulls, n, s, e, &v);
+        put(row, op, spec->off[a], a, has, v, &null_mask);
+      }
+    }
+    put_null_bits(row, spec, n_aggs, null_mask);
+  }
+}
+
+// agg_merge_large_kernel for a spec with a Decimal op
+__global__ void __launch_bounds__(kAggThreads) agg_merge_large_dec_kernel(
+    const uint32_t* __restrict__ gpos, uint64_t G, uint64_t n, const uint64_t* __restrict__ vals,
+    const uint64_t* __restrict__ vhi, const uint32_t* __restrict__ nulls, const AggSpec* __restrict__ spec,
+    uint32_t n_aggs, const uint64_t* __restrict__ gdst, uint8_t* __restrict__ dst) {
+  const uint32_t lane = threadIdx.x & 31;
+  const uint64_t warps = (uint64_t)gridDim.x * (kAggThreads / 32);
+  for (uint64_t g = (uint64_t)blockIdx.x * (kAggThreads / 32) + (threadIdx.x >> 5); g < G; g += warps) {
+    const uint32_t s = gpos[g], e = gpos[g + 1];
+    if (e - s <= kSmallGroup) continue;  // uniform over the warp
+    uint8_t* row = dst + gdst[g] + 4;
+    uint32_t null_mask = 0;
+    for (uint32_t a = 0; a < n_aggs; a++) {
+      const uint32_t op = spec->op[a];
+      if (is_decimal(op)) {
+        Dec128 x;
+        const bool has = merge_warp_dec(op, a, spec->wide[a], vals, vhi, nulls, n, s, e, lane, &x);
+        if (lane == 0) put_decimal(row, op, spec->off[a], a, has, x, &null_mask);
+      } else {
+        uint64_t v;
+        const bool has = merge_warp(op, a, vals, nulls, n, s, e, lane, &v);
+        if (lane == 0) put(row, op, spec->off[a], a, has, v, &null_mask);
+      }
+    }
+    if (lane == 0) put_null_bits(row, spec, n_aggs, null_mask);
+  }
+}
+
+}  // namespace
+
+size_t rows_aggregate_ws_bytes(uint64_t n, uint32_t n_aggs, uint32_t n_wide) {
+  return a256(n * 8) + a256(24) + 3 * a256(n * 4) + a256((n + 1) * 4) + a256(n * n_aggs * 8) + a256(n * n_wide * 8) +
+         a256(sizeof(AggSpec));
+}
+
+uint64_t* rows_aggregate_readback(uint8_t* d_aws, uint64_t n, uint32_t n_aggs, uint32_t n_wide) {
+  return carve_agg_ws(d_aws, n, n_aggs, n_wide).readback;
 }
 
 void launch_rows_group(const uint8_t* arena, uint64_t n, const uint32_t* idx, const uint32_t* heads,
                        uint32_t key_bytes, const AggSpec& spec, uint8_t* d_ws, uint8_t* d_aws, cudaStream_t st,
                        uint64_t* launches) {
-  const AggWs a = carve_agg_ws(d_aws, n, spec.n);
+  const AggWs a = carve_agg_ws(d_aws, n, spec.n, spec.n_wide);
   if (!n) {
     cudaMemsetAsync(a.readback, 0, 16, st);
     return;
@@ -349,8 +604,16 @@ void launch_rows_group(const uint8_t* arena, uint64_t n, const uint32_t* idx, co
   const KeySortWs w = carve_key_sort_ws(d_ws, n, key_bytes);
   uint64_t* scan_ws = (uint64_t*)(d_ws + key_sort_ws_bytes(n, key_bytes));
   cudaMemcpyAsync(a.spec, &spec, sizeof(AggSpec), cudaMemcpyHostToDevice, st);
-  agg_heads_kernel<<<grid_for(n), kAggThreads, 0, st>>>(arena, w.src_off, idx, n, w.words, (key_bytes + 3) / 4, heads,
-                                                        a.spec, a.head, a.nulls, a.vals);
+  if (spec.n_wide) {
+    cudaMemsetAsync(a.readback + 2, 0xff, 8, st);
+    agg_heads_kernel<true><<<grid_for(n), kAggThreads, 0, st>>>(
+        arena, w.src_off, w.len, idx, n, w.words, (key_bytes + 3) / 4, heads, a.spec, a.head, a.nulls, a.vals, a.vhi,
+        (unsigned long long*)(a.readback + 2));
+  } else {
+    agg_heads_kernel<false><<<grid_for(n), kAggThreads, 0, st>>>(arena, w.src_off, w.len, idx, n, w.words,
+                                                                 (key_bytes + 3) / 4, heads, a.spec, a.head, a.nulls,
+                                                                 a.vals, nullptr, nullptr);
+  }
   launch_exclusive_scan_u64(a.head, n, a.readback, scan_ws, st, launches);
   agg_compact_kernel<<<grid_for(n), kAggThreads, 0, st>>>(a.head, a.readback, idx, w.len, n, a.hidx, a.gpos, a.glen);
   // the group lengths are already in group order: no index
@@ -358,22 +621,31 @@ void launch_rows_group(const uint8_t* arena, uint64_t n, const uint32_t* idx, co
   if (launches) *launches += 2;
 }
 
-void launch_rows_aggregate(const uint8_t* arena, uint64_t n, uint64_t groups, uint32_t key_bytes, uint32_t n_aggs,
+void launch_rows_aggregate(const uint8_t* arena, uint64_t n, uint64_t groups, uint32_t key_bytes, const AggSpec& spec,
                            uint8_t* d_ws, uint8_t* d_aws, uint8_t* d_dst, cudaStream_t st, uint64_t* launches) {
   if (!groups) return;
+  const uint32_t n_aggs = spec.n;
   const KeySortWs w = carve_key_sort_ws(d_ws, n, key_bytes);
-  const AggWs a = carve_agg_ws(d_aws, n, n_aggs);
+  const AggWs a = carve_agg_ws(d_aws, n, n_aggs, spec.n_wide);
   PartitionPlan plan;
   plan.src_off = w.src_off;
   plan.sdst = w.sdst;
   plan.idx = a.hidx;
   launch_partition_gather(arena, w.len, groups, plan, d_dst, st, launches);
   if (!n_aggs) return;
-  agg_merge_small_kernel<<<grid_for(groups), kAggThreads, 0, st>>>(a.gpos, groups, n, a.vals, a.nulls, a.spec, n_aggs,
-                                                                    w.sdst, d_dst);
   const uint64_t ctas = (groups + kAggThreads / 32 - 1) / (kAggThreads / 32);
-  agg_merge_large_kernel<<<(unsigned)std::min<uint64_t>(ctas, (uint64_t)kSMs * 16), kAggThreads, 0, st>>>(
-      a.gpos, groups, n, a.vals, a.nulls, a.spec, n_aggs, w.sdst, d_dst);
+  const unsigned large_grid = (unsigned)std::min<uint64_t>(ctas, (uint64_t)kSMs * 16);
+  if (spec.decimal) {
+    agg_merge_small_dec_kernel<<<grid_for(groups), kAggThreads, 0, st>>>(a.gpos, groups, n, a.vals, a.vhi, a.nulls,
+                                                                          a.spec, n_aggs, w.sdst, d_dst);
+    agg_merge_large_dec_kernel<<<large_grid, kAggThreads, 0, st>>>(a.gpos, groups, n, a.vals, a.vhi, a.nulls, a.spec,
+                                                                   n_aggs, w.sdst, d_dst);
+  } else {
+    agg_merge_small_kernel<<<grid_for(groups), kAggThreads, 0, st>>>(a.gpos, groups, n, a.vals, a.nulls, a.spec,
+                                                                      n_aggs, w.sdst, d_dst);
+    agg_merge_large_kernel<<<large_grid, kAggThreads, 0, st>>>(a.gpos, groups, n, a.vals, a.nulls, a.spec, n_aggs,
+                                                               w.sdst, d_dst);
+  }
   if (launches) *launches += 2;
 }
 

@@ -2493,9 +2493,17 @@ static int agg_args(const RecordSpec& spec) {
   for (uint32_t c = 0; c < ks.n; c++)
     if (ks.null_field[c] >= 0) words.push_back({null_word(ks.null_field[c]), null_word(ks.null_field[c]) + 8});
   for (uint32_t k = 0; k < n; k++) {
-    if (spec.agg_op[k] > B2S_AGG_MAX_FLOAT64) return fail(B2S_E_ARG, "unknown aggregate op%s");
+    const uint32_t op = spec.agg_op[k], base = agg_base_op(op), precision = agg_precision(op);
+    if ((op >> 16) || (base > B2S_AGG_MAX_FLOAT64 && base < B2S_AGG_SUM_DECIMAL) || base > B2S_AGG_MAX_DECIMAL)
+      return fail(B2S_E_ARG, "unknown aggregate op%s");
+    if (base != B2S_AGG_SUM_DECIMAL && precision)
+      return fail(B2S_E_ARG, "only B2S_AGG_SUM_DECIMAL takes a precision%s");
+    if (base == B2S_AGG_SUM_DECIMAL && (precision < 1 || precision > 38))
+      return fail(B2S_E_ARG, "B2S_AGG_SUM_DECIMAL's precision must be in [1, 38]%s");
     const int32_t f = spec.agg_null_field[k];
     if (f < -1) return fail(B2S_E_ARG, "agg_null_field must be -1 or a field ordinal%s");
+    if (base == B2S_AGG_SUM_DECIMAL && f < 0)
+      return fail(B2S_E_ARG, "B2S_AGG_SUM_DECIMAL needs an agg_null_field: its result can be null%s");
     if (f >= 0) words.push_back({null_word(f), null_word(f) + 8});
   }
   for (uint32_t k = 0; k < n; k++) {
@@ -2510,6 +2518,31 @@ static int agg_args(const RecordSpec& spec) {
       if (overlaps(s0, s1, w.first, w.second)) return fail(B2S_E_ARG, "an aggregate slot overlaps a null word%s");
   }
   return 0;
+}
+
+// The device form of the aggregates: ops, slots and null bits; the index of every out-of-line decimal among them; where
+// their 16-byte regions may start (past every key and aggregate slot and every null word the call uses).
+static AggSpec agg_spec(const RecordSpec& spec) {
+  AggSpec agg;
+  agg.n = spec.n_aggs;
+  uint64_t from = 0;
+  const KeySpec& ks = spec.keys;
+  for (uint32_t c = 0; c < ks.n; c++) {
+    from = std::max<uint64_t>(from, (uint64_t)ks.off[c] + ks.len[c]);
+    if (ks.null_field[c] >= 0) from = std::max<uint64_t>(from, null_word(ks.null_field[c]) + 8);
+  }
+  for (uint32_t k = 0; k < agg.n; k++) {
+    const uint32_t op = spec.agg_op[k];
+    agg.op[k] = op;
+    agg.off[k] = spec.agg_off[k];
+    agg.null_field[k] = spec.agg_null_field[k];
+    if (agg_decimal_wide(op)) agg.wide[k] = agg.n_wide++;
+    agg.decimal |= agg_base_op(op) >= B2S_AGG_SUM_DECIMAL;
+    from = std::max<uint64_t>(from, (uint64_t)spec.agg_off[k] + 8);
+    if (spec.agg_null_field[k] >= 0) from = std::max<uint64_t>(from, null_word(spec.agg_null_field[k]) + 8);
+  }
+  agg.region_from = (uint32_t)std::min<uint64_t>(from, 0xffffffffull);
+  return agg;
 }
 
 // the bytes a row must hold for the aggregates: every slot and every aggregate null word (0 without aggregates)
@@ -2741,33 +2774,31 @@ struct SortSource {
 };
 
 // The end of an aggregation (b2s_decompress_aggregate_rows_*), from the sorted indices idx of the records: grouping,
-// one readback of the group count and output bytes (which checks out_cap), the heads' gather and the merge into
-// d_out.  *total = output bytes.  The dominant step is this one (marks G0, G1).
+// one readback of the group count, output bytes and decimal verdict (which checks out_cap), the heads' gather and the
+// merge into d_out.  *total = output bytes.  *bad: the verdict of the out-of-line decimals' checks (kernels.h,
+// kAggBad*); when it is not ~0 nothing is written.  The dominant step is this one (marks G0, G1).
 static int aggregate_rows_tail(Slot& S, const RecordSpec& spec, const uint8_t* arena, uint64_t records,
                                const uint32_t* idx, const uint32_t* heads, uint8_t* ws, uint8_t* aws, uint8_t* d_out,
-                               uint64_t out_cap, uint64_t* total, uint64_t* n_rec, uint64_t* n_groups,
+                               uint64_t out_cap, uint64_t* total, uint64_t* n_rec, uint64_t* n_groups, uint64_t* bad,
                                uint64_t* launches) {
   cudaStream_t st = S.st;
   const uint32_t key_bytes = rows_key_bytes(spec.keys);
-  AggSpec agg;
-  agg.n = spec.n_aggs;
-  for (uint32_t k = 0; k < agg.n; k++) {
-    agg.op[k] = spec.agg_op[k];
-    agg.off[k] = spec.agg_off[k];
-    agg.null_field[k] = spec.agg_null_field[k];
-  }
-  uint64_t rb[2] = {0, 0};  // groups, output bytes
+  const AggSpec agg = agg_spec(spec);
+  uint64_t rb[3] = {0, 0, ~0ull};  // groups, output bytes, decimal verdict
   CU(S.mark(G0, st, *launches));
   if (records) {
     launch_rows_group(arena, records, idx, heads, key_bytes, agg, ws, aws, st, launches);
-    CU(cudaMemcpyAsync(rb, rows_aggregate_readback(aws, records, agg.n), sizeof rb, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(rb, rows_aggregate_readback(aws, records, agg.n, agg.n_wide), (agg.n_wide ? 3 : 2) * 8,
+                       cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
     CU(cudaGetLastError());
   }
+  *bad = rb[2];
+  if (rb[2] != ~0ull) return 0;
   *total = rb[1];
   if (rb[1] > out_cap)
     return fail(B2S_E_DST_TOO_SMALL, "dst_cap is below the %s output bytes", std::to_string(rb[1]).c_str());
-  launch_rows_aggregate(arena, records, rb[0], key_bytes, agg.n, ws, aws, d_out, st, launches);
+  launch_rows_aggregate(arena, records, rb[0], key_bytes, agg, ws, aws, d_out, st, launches);
   CU(S.mark(G1, st, *launches));
   CU(S.mark(P1, st));
   CU(cudaStreamSynchronize(st));
@@ -2963,7 +2994,7 @@ static int decompress_sort_run(Device* D, Slot& S, uint32_t codec, uint32_t alg,
   const uint32_t key_bytes = rows_key_bytes(ks);
   const bool refine = rows_key_refines(ks);
   const size_t sort_ws = rows_sort_ws_bytes(records, key_bytes);
-  const size_t agg_ws = spec.aggregate ? rows_aggregate_ws_bytes(records, spec.n_aggs) : 0;
+  const size_t agg_ws = spec.aggregate ? rows_aggregate_ws_bytes(records, spec.n_aggs, agg_spec(spec).n_wide) : 0;
   const size_t refine_ws = refine ? rows_refine_ws_bytes(records, n_src) : 0;
   if (records && (rc = S.pws.ensure(sort_ws + agg_ws + refine_ws))) return rc;
   uint8_t* ws = (uint8_t*)S.pws.p;
@@ -2994,8 +3025,29 @@ static int decompress_sort_run(Device* D, Slot& S, uint32_t codec, uint32_t alg,
     idx = rows_refine_order(rws, records, n_src);
     heads = rows_refine_heads(rws, records, n_src);
   }
-  if (spec.aggregate) return aggregate_rows_tail(S, spec, arena, records, idx, heads, ws, ws + sort_ws, *d_sorted,
-                                                 out_cap, total, n_rec, n_groups, launches);
+  if (spec.aggregate) {
+    uint64_t bad = ~0ull;
+    if ((rc = aggregate_rows_tail(S, spec, arena, records, idx, heads, ws, ws + sort_ws, *d_sorted, out_cap, total,
+                                  n_rec, n_groups, &bad, launches)) ||
+        bad == ~0ull)
+      return rc;
+    // a bad decimal: the source holding the record (the last that starts at or before it) fails, as a framing verdict
+    const uint64_t at_byte = bad >> 2;
+    uint32_t i = 0;
+    for (uint32_t k = 0; k < n_src; k++)
+      if (place[k] <= at_byte && length[k]) i = k;
+    (cached(i) ? cached_status[i] : J.h.status[block(i)]) = B2S_E_CORRUPT;
+    static const char* const why[] = {"",
+                                      "a decimal aggregate's size is not in [1, 16] or its bytes run past the end of "
+                                      "its row",
+                                      "a decimal aggregate's 16-byte region runs past the end of its row",
+                                      "a decimal aggregate's 16-byte region starts before the end of a slot or null "
+                                      "word in use"};
+    snprintf(msg, sizeof msg, "%s %u: bad row record at byte %llu: %s", cached(i) ? "cached source" : "block", i,
+             (unsigned long long)(at_byte - place[i]), why[bad & 3]);
+    fail(B2S_E_CORRUPT, "%s", msg);
+    return report();
+  }
   launch_rows_gather(arena, records, key_bytes, idx, ws, *d_sorted, st, launches);
   CU(S.mark(P1, st));
   CU(cudaStreamSynchronize(st));

@@ -364,18 +364,35 @@ void launch_rows_range(const uint8_t* rec, uint64_t rec_bytes, const uint64_t* r
                        uint64_t* bad, cudaStream_t st, uint64_t* launches);
 
 // ---------------- aggregate.cu (group key-sorted rows and merge their aggregate buffers) ----------------
-// Aggregate a: op[a] (B2S_AGG_*) over the 8-byte slot at row offset off[a], null bit null_field[a] (-1: never null).
+// Aggregate a: op[a] (B2S_AGG_*, with SUM_DECIMAL's precision in bits 8..15) over the 8-byte slot at row offset off[a],
+// null bit null_field[a] (-1: never null).  An out-of-line decimal (agg_decimal_wide) is staged as 16 bytes: its high
+// words at index wide[a] of n_wide; its 16-byte region must start at or after region_from (the end of every slot and
+// null word the call uses).
 constexpr uint32_t kMaxAggs = 16;
 struct AggSpec {
   uint32_t n = 0;
   uint32_t op[kMaxAggs] = {};
   uint32_t off[kMaxAggs] = {};
   int32_t null_field[kMaxAggs] = {};
+  uint32_t wide[kMaxAggs] = {};
+  uint32_t n_wide = 0;
+  uint32_t region_from = 0;
+  bool decimal = false;  // some op is a Decimal op: the merge runs the kernels that know them
 };
-// d_aws: rows_aggregate_ws_bytes(n, n_aggs), beside the sort workspace d_ws of the same n records
-size_t rows_aggregate_ws_bytes(uint64_t n, uint32_t n_aggs);
-// after launch_rows_group: [group count, output bytes] (device)
-uint64_t* rows_aggregate_readback(uint8_t* d_aws, uint64_t n, uint32_t n_aggs);
+__host__ __device__ inline uint32_t agg_base_op(uint32_t op) { return op & 0xff; }
+__host__ __device__ inline uint32_t agg_precision(uint32_t op) { return (op >> 8) & 0xff; }
+// the op's value is out of line: 16 bytes at (offset << 32) | size
+__host__ __device__ inline bool agg_decimal_wide(uint32_t op) {
+  const uint32_t b = agg_base_op(op);
+  return b == B2S_AGG_MIN_DECIMAL || b == B2S_AGG_MAX_DECIMAL || (b == B2S_AGG_SUM_DECIMAL && agg_precision(op) > 18);
+}
+// the verdict of the decimal region checks (rows_aggregate_readback's third word): ~0, or the lowest bad record's arena
+// offset << 2 | one of these
+constexpr uint64_t kAggBadDecimal = 1, kAggBadRegionEnd = 2, kAggBadRegionStart = 3;
+// d_aws: rows_aggregate_ws_bytes(n, n_aggs, n_wide), beside the sort workspace d_ws of the same n records
+size_t rows_aggregate_ws_bytes(uint64_t n, uint32_t n_aggs, uint32_t n_wide);
+// after launch_rows_group: [group count, output bytes, decimal verdict (only with an out-of-line decimal)] (device)
+uint64_t* rows_aggregate_readback(uint8_t* d_aws, uint64_t n, uint32_t n_aggs, uint32_t n_wide);
 // the groups of the records in the order idx (launch_rows_order): heads, group starts, the heads' output offsets and
 // the readback.  Also stages every aggregate's inputs in sorted order.  heads (keys that refine: rows_refine_heads)
 // flags where a new key starts; nullptr: where the key words differ.
@@ -384,7 +401,7 @@ void launch_rows_group(const uint8_t* arena, uint64_t n, const uint32_t* idx, co
                        uint64_t* launches);
 // the groups (count read back) to d_dst: the first record of each, whole, with the aggregates' slots and null bits
 // replaced by the merged values
-void launch_rows_aggregate(const uint8_t* arena, uint64_t n, uint64_t groups, uint32_t key_bytes, uint32_t n_aggs,
+void launch_rows_aggregate(const uint8_t* arena, uint64_t n, uint64_t groups, uint32_t key_bytes, const AggSpec& spec,
                            uint8_t* d_ws, uint8_t* d_aws, uint8_t* d_dst, cudaStream_t st, uint64_t* launches);
 
 // ---------------- exchange.cu (exchange-cache reads: ranges of device memory gathered into one arena) ----------------

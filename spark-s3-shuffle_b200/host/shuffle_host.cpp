@@ -905,8 +905,8 @@ class S3ShuffleReader {
     const int32_t* nullField;
     bool composite;
   };
-  // The aggregates of readRows: aggregate k is op[k] (B2S_AGG_*) over the 8-byte slot at row offset off[k], null bit
-  // nullField[k] (-1 = never null).
+  // The aggregates of readRows: aggregate k is op[k] (B2S_AGG_*, B2S_AGG_SUM_DECIMAL with its precision in bits
+  // 8..15) over the 8-byte slot at row offset off[k], null bit nullField[k] (-1 = never null).
   struct RowAggregates {
     uint32_t n;
     const uint32_t* op;

@@ -26,7 +26,18 @@ count and min equal to a torch scatter reference exactly (the count mod 2^64), m
 reference's, and the double sum within 1e-12 of the sum of the absolute inputs of its key (torch adds in another order).
 The card's name and power limit are read in the same run.
 
+--buffers decimal swaps the four buffers for Spark's Decimal ones, the shape of sum(decimal(28,2)) and
+avg(decimal(28,2)) partials: [sum, isEmpty] and [sum, count], i.e. B2S_AGG_SUM_DECIMAL | 28 << 8 (out of line, never
+null: no partial overflowed), MIN_INT32 (isEmpty, 1 in ~2 % of rows), SUM_DECIMAL | 28 << 8 and SUM_INT64 (the count).
+A record is 84 bytes: the 52-byte layout's four slots, then each sum's 16 bytes (|v| < 10^15, written as all 16
+big-endian bytes).  Its algorithmic bytes add, per record, the two 16-byte values read and their high words staged
+(2 x 16 B), and per group the two 16-byte regions rewritten.  Validation: every key appears once, with both sums equal
+to the exact per-key sum (torch adds the high and low 32-bit halves in int64; Python joins them), the count exact,
+isEmpty the AND of the inputs and no null bit but the null key's.  Both buffer kinds report the largest reducer's
+aggregation step per row (one warp merges its one large group).
+
     python tools/aggregate_rows_bench.py [--gib 2] [--maps 400] [--partitions 200] [--codec snappy] [--hot 0.05]
+                                         [--buffers longs|decimal]
 
 Prints one JSON document.
 """
@@ -41,6 +52,8 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 REC = 52              # size prefix + null bitset + key + count + sum + min + max
+REC_DEC = 84          # size prefix + null bitset + key + sum, isEmpty, sum, count slots + two 16-byte decimals
+P_DEC = 28
 KEY_OFF = 8           # field 0 of the row: after the one-word null bitset
 HBM_PEAK = 3.35e12    # H100 SXM data sheet
 
@@ -78,7 +91,35 @@ def make_map(torch, gen, n, K, hot, R, dev):
         (cnt, fsum, fmin, fmax, nulls)
 
 
+def make_map_decimal(torch, gen, n, K, hot, R, dev):
+    """the --buffers decimal rows of one map task -> (records, rec_len u32, reduce ids u32, dense key index, fields)"""
+    key = torch.randint(0, K, (n,), generator=gen, device=dev, dtype=torch.int64)
+    if hot:
+        key[torch.rand(n, generator=gen, device=dev) < hot] = 0
+    knull = torch.rand(n, generator=gen, device=dev) < 0.05
+    s1 = torch.randint(-10**15, 10**15, (n,), generator=gen, device=dev, dtype=torch.int64)
+    s2 = torch.randint(-10**15, 10**15, (n,), generator=gen, device=dev, dtype=torch.int64)
+    empty = (torch.rand(n, generator=gen, device=dev) < 0.02).to(torch.int64)
+    cnt = torch.randint(1, 100, (n,), generator=gen, device=dev, dtype=torch.int64)
+    row = REC_DEC - 4
+    slot1 = torch.full((n,), (48 << 32) | 16, dtype=torch.int64, device=dev)
+    slot2 = torch.full((n,), (64 << 32) | 16, dtype=torch.int64, device=dev)
+    rec = torch.empty((n, REC_DEC), dtype=torch.uint8, device=dev)
+    rec[:, :4] = torch.tensor([0, 0, 0, row], dtype=torch.uint8, device=dev)
+    for k, col in enumerate([knull.to(torch.int64), key, slot1, empty, slot2, cnt]):
+        rec[:, 4 + 8 * k:12 + 8 * k] = col[:, None].view(torch.uint8).view(n, 8)
+    for k, v in enumerate([s1, s2]):  # 16 big-endian bytes: the sign, then the long
+        o = 4 + 48 + 16 * k
+        rec[:, o:o + 8] = torch.where(v < 0, 255, 0).to(torch.uint8)[:, None].expand(n, 8)
+        rec[:, o + 8:o + 16] = v[:, None].view(torch.uint8).view(n, 8).flip(1)
+    part = torch.where(knull, torch.zeros_like(key), (key * 2654435761) % R).to(torch.int32)
+    dense = torch.where(knull, torch.full_like(key, K), key)
+    return rec.flatten(), torch.full((n,), REC_DEC, dtype=torch.int32, device=dev), part, dense, (s1, s2, empty, cnt)
+
+
 def run_shape(torch, c, args, codec, K, hot, dev, gen):
+    if args.buffers == "decimal":
+        return run_shape_decimal(torch, c, args, codec, K, hot, dev, gen)
     M, R = args.maps, args.partitions
     n = int(args.gib * (1 << 30)) // REC
     per = [n // M] * (M - 1) + [n - n // M * (M - 1)]
@@ -217,10 +258,141 @@ def run_shape(torch, c, args, codec, K, hot, dev, gen):
                            "b_ms": round(tb[mid], 3), "c_ms": round(tc[mid], 3),
                            "aggregation_step_ms": round(tagg[mid], 3)},
         "largest_reducer": {"records": recs_per[big], "groups": groups_per[big], "c_ms": round(tc[big], 3),
-                            "aggregation_step_ms": round(tagg[big], 3)},
+                            "aggregation_step_ms": round(tagg[big], 3),
+                            "aggregation_ns_per_row": round(tagg[big] * 1e6 / max(recs_per[big], 1), 1)},
         "valid": bool(valid),
         "checks": {"calls_and_groups": bool(ok), "null_bits": ok_bits, "count": ok_cnt, "min": ok_min, "max": ok_max,
                    "sum_within_1e-12": ok_sum, "max_sum_rel_err": float(err.max()) if err.numel() else 0.0},
+    }
+
+
+def stage_maps(torch, c, args, codec, M, R, per, make, dev, on_map):
+    """every map's rows made by make(m) and partition-compressed into one device arena; on_map(fields, dense) feeds
+    the reference -> (per-map results, their arena offsets, the arena)"""
+    maps, map_base, bounds, compressed = [], [], [], None
+    for m in range(M):
+        rec, rec_len, part, dense, fields = make(m)
+        on_map(fields, dense)
+        bound = (c.partition_compress_bound(codec, 0, R, rec.numel()) + 255) // 256 * 256
+        if compressed is None:
+            compressed = torch.empty(bound * (M + 1), dtype=torch.uint8, device=dev)
+        at = sum(bounds)
+        assert at + bound <= compressed.numel()
+        torch.cuda.synchronize()
+        r = c.partition_compress_dev(codec, rec.data_ptr(), rec.numel(), rec_len.data_ptr(), part.data_ptr(), per[m],
+                                     R, compressed.data_ptr() + at, bound, checksum_alg=c.CHECKSUM_CRC32C)
+        assert not r["status"].any()
+        maps.append(r)
+        map_base.append(at)
+        bounds.append(bound)
+        del rec, rec_len, part, dense
+    torch.cuda.empty_cache()
+    return maps, map_base, compressed
+
+
+def run_shape_decimal(torch, c, args, codec, K, hot, dev, gen):
+    """run_shape with the Decimal buffers (module docstring, --buffers decimal)"""
+    M, R = args.maps, args.partitions
+    n = int(args.gib * (1 << 30)) // REC_DEC
+    per = [n // M] * (M - 1) + [n - n // M * (M - 1)]
+    G = K + 1
+    halves = torch.zeros((4, G), dtype=torch.int64, device=dev)  # s1 lo, s1 hi, s2 lo, s2 hi
+    ref_cnt = torch.zeros(G, dtype=torch.int64, device=dev)
+    ref_empty = torch.ones(G, dtype=torch.int64, device=dev)
+    ref_rows = torch.zeros(G, dtype=torch.int64, device=dev)
+
+    def on_map(fields, dense):
+        s1, s2, empty, cnt = fields
+        ref_rows.index_add_(0, dense, torch.ones_like(dense))
+        for k, v in enumerate((s1, s2)):
+            halves[2 * k].index_add_(0, dense, v & 0xFFFFFFFF)
+            halves[2 * k + 1].index_add_(0, dense, v >> 32)
+        ref_cnt.index_add_(0, dense, cnt)
+        ref_empty.scatter_reduce_(0, dense, empty, "amin")
+
+    maps, map_base, compressed = stage_maps(torch, c, args, codec, M, R, per,
+                                            lambda m: make_map_decimal(torch, gen, per[m], K, hot, R, dev), dev,
+                                            on_map)
+
+    def blocks(red):
+        off = [map_base[m] + int(maps[m]["dst_off"][red]) for m in range(M)]
+        ln = [int(maps[m]["dst_len"][red]) for m in range(M)]
+        ck = [int(maps[m]["checksums"][red]) for m in range(M)]
+        return off, ln, list(range(M + 1)), ln, ck
+
+    biggest = max(sum(int(maps[m]["dst_len"][red]) for m in range(M)) for red in range(R))
+    cap = (biggest * (1 if codec == c.CODEC_NONE else 4)) + (1 << 20)
+    out = torch.empty(cap + 64, dtype=torch.uint8, device=dev)
+    sum_op = c.agg_sum_decimal(P_DEC)
+    aggs = [(sum_op, 16, 2), (c.AGG_MIN_INT32, 24, -1), (sum_op, 32, 4), (c.AGG_SUM_INT64, 40, -1)]
+
+    def call_c(red):
+        off, ln, sb, sl, ck = blocks(red)
+        return c.decompress_aggregate_rows_dev(codec, compressed.data_ptr(), off, ln, out.data_ptr(), cap,
+                                               c.KEY_INT64, KEY_OFF, 8, 0, aggs, c.CHECKSUM_CRC32C, sb, sl, ck)
+
+    for _ in range(args.warmup):
+        call_c(0)
+    tc, tagg, agg_bytes, recs_per, groups_per = [], [], [], [], []
+    got = {}  # dense key -> (bits, s1, isEmpty, s2, count)
+    ok = True
+    for red in range(R):
+        c.mark(0)
+        rc = call_c(red)
+        c.mark(1)
+        tc.append(c.marks_elapsed_ms())
+        t = c.last_timing()
+        ok &= not rc["status"].any() and rc["total"] == rc["n_groups"] * REC_DEC
+        tagg.append(t["dominant_ms"])
+        nr, ng = rc["n_records"], rc["n_groups"]
+        recs_per.append(nr)
+        groups_per.append(ng)
+        agg_bytes.append(nr * (4 + 24 + 40 + 32 + 2 * 52 + 24) + ng * (2 * REC_DEC + 40 + 32))
+        o = out[: ng * REC_DEC].view(ng, REC_DEC)[:, 4:].cpu().numpy()
+        for row in o:
+            word = int.from_bytes(row[0:8].tobytes(), "little")
+            dk = K if word & 1 else int.from_bytes(row[8:16].tobytes(), "little", signed=True)
+            vals = []
+            for so in (16, 32):
+                slot = int.from_bytes(row[so:so + 8].tobytes(), "little")
+                p, ln = slot >> 32, slot & 0xFFFFFFFF
+                vals.append(int.from_bytes(row[p:p + ln].tobytes(), "big", signed=True))
+            ok &= dk not in got
+            got[dk] = (word, vals[0], int.from_bytes(row[24:32].tobytes(), "little"), vals[1],
+                       int.from_bytes(row[40:48].tobytes(), "little", signed=True))
+    h, cnt = halves.cpu().tolist(), ref_cnt.cpu().tolist()
+    emp, rows_ = ref_empty.cpu().tolist(), ref_rows.cpu().tolist()
+    present = [g for g in range(G) if rows_[g]]
+    ok_keys = sorted(got) == present
+    ok_sum = ok_cnt = ok_bits = True
+    for g in present:
+        if g not in got:
+            continue
+        word, v1, e, v2, k = got[g]
+        ok_sum &= v1 == h[1][g] * 2**32 + h[0][g] and v2 == h[3][g] * 2**32 + h[2][g]
+        ok_cnt &= k == cnt[g] and e == emp[g]
+        ok_bits &= (word & 0b10101) == (1 if g == K else 0)
+    valid = ok and ok_keys and ok_sum and ok_cnt and ok_bits
+    agg_s = sum(tagg) * 1e-3
+    mid = sorted(range(R), key=lambda i: recs_per[i])[R // 2]
+    big = max(range(R), key=lambda i: recs_per[i])
+    return {
+        "buffers": "decimal", "keys": K, "hot": hot, "records": n, "groups": len(present),
+        "largest_group": max(rows_), "compressed_bytes": sum(int(m["dst_len"].sum()) for m in maps),
+        "records_per_reducer": spread(recs_per), "groups_per_reducer": spread(groups_per),
+        "c_decompress_aggregate_rows_ms": spread(tc), "aggregation_step_ms": spread(tagg),
+        "sum_ms": {"c_decompress_aggregate_rows": round(sum(tc), 3), "aggregation_step": round(sum(tagg), 3)},
+        "aggregation_algorithmic_bytes": sum(agg_bytes),
+        "aggregation_GBps": round(sum(agg_bytes) / agg_s / 1e9, 1),
+        "aggregation_share_of_3.35TBps": round(sum(agg_bytes) / agg_s / HBM_PEAK, 3),
+        "median_reducer": {"records": recs_per[mid], "groups": groups_per[mid], "c_ms": round(tc[mid], 3),
+                           "aggregation_step_ms": round(tagg[mid], 3)},
+        "largest_reducer": {"records": recs_per[big], "groups": groups_per[big], "c_ms": round(tc[big], 3),
+                            "aggregation_step_ms": round(tagg[big], 3),
+                            "aggregation_ns_per_row": round(tagg[big] * 1e6 / max(recs_per[big], 1), 1)},
+        "valid": bool(valid),
+        "checks": {"calls_and_groups": bool(ok), "keys_once": ok_keys, "sums_exact": ok_sum,
+                   "count_and_isEmpty": ok_cnt, "null_bits": ok_bits},
     }
 
 
@@ -234,6 +406,8 @@ def main():
     ap.add_argument("--hot", type=float, default=0.05)
     ap.add_argument("--warmup", type=int, default=2)
     ap.add_argument("--seed", type=int, default=42)
+    ap.add_argument("--buffers", default="longs", choices=["longs", "decimal"],
+                    help="longs: count, double sum, long min, double max; decimal: Sum / Average decimal buffers")
     args = ap.parse_args()
 
     import torch
@@ -246,11 +420,13 @@ def main():
     dev = torch.device("cuda", 0)
     gen = torch.Generator(device=dev)
     gen.manual_seed(args.seed)
-    K = args.keys or max(1, int(args.gib * (1 << 30)) // REC // args.maps)
+    rec = REC if args.buffers == "longs" else REC_DEC
+    K = args.keys or max(1, int(args.gib * (1 << 30)) // rec // args.maps)
     shapes = {"many": run_shape(torch, c, args, codec, K, 0.0, dev, gen),
               "hot": run_shape(torch, c, args, codec, K, args.hot, dev, gen)}
-    result = {"card": card(), "codec": args.codec, "maps": args.maps, "partitions": args.partitions,
-              "gib": args.gib, "shapes": shapes, "valid": all(s["valid"] for s in shapes.values())}
+    result = {"card": card(), "buffers": args.buffers, "codec": args.codec, "maps": args.maps,
+              "partitions": args.partitions, "gib": args.gib, "shapes": shapes,
+              "valid": all(s["valid"] for s in shapes.values())}
     print(json.dumps(result, indent=1))
     c.shutdown()
 

@@ -8,6 +8,10 @@ one block: --codec, default snappy, + CRC32C), the reducer a hash of the key:
   q67  : partial-aggregate rows of a GROUP BY of eight columns, TPC-DS q67's shape: four strings of 5-50 bytes
          (i_category, i_class, i_brand, i_product_name: a few category / class prefixes shared by many values) and four
          ints, then a count and a sum buffer (longs).  --groups distinct keys, so a key has about rows / groups rows.
+         --q67-decimal adds q67's real buffers to the same rows: sum(ss_sales_price * ss_quantity)'s decimal(28,2)
+         [sum, isEmpty], the sum out of line (BigInteger.toByteArray of the long sum x 10^17, 1..9 bytes, in a 16-byte
+         region) and isEmpty false; the aggregation is then also timed with those two buffers
+         (B2S_AGG_SUM_DECIMAL | 28 << 8, MIN_INT32) and every merged sum checked against the long sum x 10^17.
   join : the build side of a sort-merge join on (string id, int): a 16-40 byte id with a shared 12-byte prefix, an int,
          and two longs (the second used for the two-INT64 comparison below).
   window: q67's window input, rank() over (partition by i_category order by sumsales desc): i_category (one of ten
@@ -19,6 +23,7 @@ Per reducer, after --warmup untimed calls, CUDA-event times (b2s_last_timing.ker
   keys     : the composite-key call; framing (its dominant_ms for the sort)
   first    : the same rows sorted by one INT32 column (resolved by the first pass: no refinement)
   agg      : q67 only, the composite-key aggregation; its aggregation step is dominant_ms
+  agg_dec  : q67 with --q67-decimal, the same with the decimal [sum, isEmpty] buffers instead of the longs
   i64x2    : join only, the two-INT64 composite beside the single-INT64 row sort on the same rows
   window   : window only, the sort by (i_category ASC NULLS FIRST, sumsales DESC NULLS LAST), as the WindowExec's
              SortExec asks; asc: the same columns ASC NULLS FIRST; i64: a one-INT64 row sort of the same rows.  Every
@@ -28,6 +33,7 @@ per round), which also validates every output byte against a Python sort (and th
 The card's name and power limit are read in the same run.
 
     python tools/sort_rows_keys_bench.py [--rows 1000000] [--maps 400] [--partitions 200] [--codec snappy]
+                                         [--q67-decimal]
 
 Prints one JSON document.
 """
@@ -77,8 +83,14 @@ def strings(rng, n, prefixes, lo, hi):
     return out, np.maximum(ln, plen)
 
 
-def make_rows(rng, shape, n, groups):
-    """-> (rows uint8 [n, L], key columns [(type, off, len, null field)], aggs, partition key)"""
+def to_byte_array(x):
+    """java.math.BigInteger.toByteArray"""
+    return x.to_bytes((x if x >= 0 else ~x).bit_length() // 8 + 1, "big", signed=True)
+
+
+def make_rows(rng, shape, n, groups, decimal=False):
+    """-> (rows uint8 [n, L], key columns [(type, off, len, null field)], aggs, partition key, decimal aggs (q67 with
+    decimal: [sum, isEmpty] after the long buffers, the sum's 16 bytes after the strings; else []))"""
     if shape == "q67":
         g = rng.integers(0, groups, n)  # the group of each row: its key values come from the group id
         grng = np.random.default_rng(7)
@@ -94,9 +106,10 @@ def make_rows(rng, shape, n, groups):
         s_vals = [strings(rng, n, [b"AAAAAAAABBBB"], 16, 40)]
         i_vals = np.stack([rng.integers(-100, 100, n), rng.integers(-2**62, 2**62, n), rng.integers(0, 8, n)], 1)
         n_str, n_int, n_agg = 1, 3, 0
-    fields = n_str + n_int + n_agg
+    n_dec = 2 if shape == "q67" and decimal else 0
+    fields = n_str + n_int + n_agg + n_dec
     fixed = 8 + 8 * fields
-    L = fixed + SLOT * n_str
+    L = fixed + SLOT * n_str + (16 if n_dec else 0)
     rows = np.zeros((n, L), np.uint8)
     keys = []
     for s in range(n_str):
@@ -119,9 +132,23 @@ def make_rows(rng, shape, n, groups):
         o = 8 + 8 * (n_str + n_int + a)
         rows[:, o:o + 8] = (np.ones(n, np.int64) if a == 0 else rng.integers(-1000, 1000, n)).view(np.uint8).reshape(n, 8)
         aggs.append((0, o, -1))
+    dec_aggs = []
+    if n_dec:  # the long sum x 10^17 as a decimal(28,2) sum: its minimal bytes, one table row per long value
+        lsum = rows[:, aggs[1][1]:aggs[1][1] + 8].copy().view(np.int64).ravel()
+        table = np.zeros((2001, 16), np.uint8)
+        size = np.zeros(2001, np.uint64)
+        for v in range(-1000, 1001):
+            b = to_byte_array(v * 10**17)
+            table[v + 1000, :len(b)] = np.frombuffer(b, np.uint8)
+            size[v + 1000] = len(b)
+        o, region = 8 + 8 * (n_str + n_int + n_agg), fixed + SLOT * n_str
+        rows[:, region:region + 16] = table[lsum + 1000]
+        slot = (np.uint64(region) << np.uint64(32)) | size[lsum + 1000]
+        rows[:, o:o + 8] = slot.view(np.uint8).reshape(n, 8)
+        dec_aggs = [(9 | 28 << 8, o, n_str + n_int + n_agg), (2, o + 8, -1)]  # SUM_DECIMAL(28), MIN_INT32 (isEmpty 0)
     if shape == "join":  # sort key (string id, int); the two longs for the INT64 comparison
         keys = [keys[0], keys[1]]
-    return rows, keys, aggs, g
+    return rows, keys, aggs, g, dec_aggs
 
 
 def window_rows(rng, n):
@@ -276,6 +303,7 @@ def main():
     ap.add_argument("--seed", type=int, default=42)
     ap.add_argument("--reducers", type=int, default=0, help="reducers timed (0: all)")
     ap.add_argument("--shapes", default="q67,join,window")
+    ap.add_argument("--q67-decimal", action="store_true", help="also aggregate q67 with its decimal [sum, isEmpty]")
     args = ap.parse_args()
     import spark_s3_shuffle_b200 as pkg
     c = pkg.capi
@@ -286,13 +314,14 @@ def main():
     rng = np.random.default_rng(args.seed)
     timed = functools.partial(timed_call, c, args.warmup)
     for shape in [x for x in args.shapes.split(",") if x in ("q67", "join")]:
-        rows, keys, aggs, g = make_rows(rng, shape, args.rows, args.groups)
+        rows, keys, aggs, g, dec_aggs = make_rows(rng, shape, args.rows, args.groups, args.q67_decimal)
         L = rows.shape[1]
         red = (g * 2654435761 % 2**32) % args.partitions
         mp = rng.integers(0, args.maps, args.rows)
         order = np.lexsort((mp, red))  # reducer, then map; stable within
         R = args.reducers or args.partitions
-        stats = {k: [] for k in ("decode", "keys", "framing", "first", "agg", "agg_step", "i64x2", "i64")}
+        stats = {k: [] for k in ("decode", "keys", "framing", "first", "agg", "agg_step", "agg_dec", "agg_dec_step",
+                                 "i64x2", "i64")}
         round_counts, ok = [], True
         prefix = L.to_bytes(4, "big")  # every record's size prefix
         ik = next(k for k in keys if k[0] == KEY_INT32)
@@ -333,6 +362,23 @@ def main():
                 outrows = got[:res["total"]].reshape(-1, 4 + L)[:, 4:]
                 cnt = outrows[:, aggs[0][1]:aggs[0][1] + 8].copy().view(np.int64).ravel()
                 ok &= int(cnt.sum()) == len(kv)
+                if dec_aggs:
+                    res, t = timed(c.decompress_aggregate_rows_keys_dev, *a, keys, dec_aggs, **sk)
+                    stats["agg_dec"].append(t["kernel_ms"])
+                    stats["agg_dec_step"].append(t["dominant_ms"])
+                    ok &= res["n_groups"] == ngroups
+                    if res["total"]:
+                        c.dev_memcpy(got.ctypes.data, d_dst, res["total"], 2)
+                    want_sum = {}
+                    lo = aggs[1][1]
+                    for k, row in zip(kv, blk):
+                        want_sum[k] = want_sum.get(k, 0) + int(row[lo:lo + 8].view(np.int64)[0])
+                    do = dec_aggs[0][1]
+                    for row in got[:res["total"]].reshape(-1, 4 + L)[:, 4:]:
+                        slot = int(row[do:do + 8].view(np.uint64)[0])
+                        p, ln = slot >> 32, slot & 0xFFFFFFFF
+                        v = int.from_bytes(row[p:p + ln].tobytes(), "big", signed=True)
+                        ok &= v == want_sum.get(tuple(col_value(bytes(row), k) for k in keys)) * 10**17
             else:
                 _, t = timed(c.decompress_sort_rows_dev, *a, KEY_INT64, keys[1][1] + 8, 8, -1, **sk)
                 stats["i64"].append(t["kernel_ms"])
