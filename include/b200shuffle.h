@@ -274,6 +274,39 @@ int b2s_partition_compress_rows_range_dev(uint32_t dev_index, uint32_t codec, in
                                           uint64_t dst_cap, uint64_t* dst_off, uint64_t* dst_len, uint64_t* dst_total,
                                           uint64_t* checksum_out, int32_t* status);
 
+/* ---- write side, round-robin-partitioned rows: Spark's repartition(n) order and ids computed on the GPU ----
+ * b2s_partition_compress_* for a RoundRobinPartitioning exchange of UnsafeRows (Dataset.repartition(n) without
+ * columns, the REPARTITION(n) hint): the caller passes no rec_part.  Records are framed as for the hash call ([size:
+ * int32 big-endian][row], rec_len[i] = 4 + size).  start_position is Spark's position before the task's first row,
+ * new XORShiftRandom(partitionId).nextInt(num_partitions), computed by the caller.  sort_rows (0 or 1) is
+ * spark.sql.execution.sortBeforeRepartition: with num_partitions > 1 the rows are first sorted as Spark's
+ * UnsafeExternalRowSorter does, by row.hashCode() (Murmur3 hashUnsafeWords of the row, seed 42) as a signed int, then
+ * by RecordBinaryComparator (the shorter row first, then unsigned bytes); rows tied on both are identical, so the order
+ * is unique.  With num_partitions == 1, or sort_rows == 0, the rows stay in input order.  The k-th row of that order
+ * (0-based) goes to partition (start_position + 1 + k) mod num_partitions.
+ * Outputs: byte for byte what b2s_partition_compress_packed / _dev return for the records in that order with those ids.
+ * Errors, B2S_E_ARG, nothing reported as written, b2s_last_error() says why: what b2s_partition_compress_* rejects;
+ * start_position outside [0, num_partitions); sort_rows above 1; start_position + n_records above 2^31 - 1 (Spark's
+ * position would wrap: keep such a task on the CPU path); a bad record (rec_len < 4, a size prefix other than rec_len -
+ * 4, a row size that is not a multiple of 8), the lowest one named, in both modes.  No usable device -> B2S_E_CUDA.
+ * b2s_last_timing as for the partition calls, plus dominant_ms / dominant_launches = the round-robin step (the checks
+ * and hash, the sort with its refinement rounds, the ids).  No exchange-cache form. */
+int b2s_partition_compress_rows_round_robin_packed(uint32_t codec, int32_t level, uint32_t codec_block_size,
+                                                   uint32_t checksum_alg, uint32_t num_partitions,
+                                                   int32_t start_position, uint32_t sort_rows, uint64_t n_records,
+                                                   const uint8_t* rec_base, uint64_t rec_bytes,
+                                                   const uint32_t* rec_len, uint8_t* dst_base, uint64_t dst_cap,
+                                                   uint64_t* dst_off, uint64_t* dst_len, uint64_t* dst_total,
+                                                   uint64_t* checksum_out, int32_t* status);
+/* same, with rec_base / rec_len / dst_base in device memory of dev_index */
+int b2s_partition_compress_rows_round_robin_dev(uint32_t dev_index, uint32_t codec, int32_t level,
+                                                uint32_t codec_block_size, uint32_t checksum_alg,
+                                                uint32_t num_partitions, int32_t start_position, uint32_t sort_rows,
+                                                uint64_t n_records, const uint8_t* rec_base, uint64_t rec_bytes,
+                                                const uint32_t* rec_len, uint8_t* dst_base, uint64_t dst_cap,
+                                                uint64_t* dst_off, uint64_t* dst_len, uint64_t* dst_total,
+                                                uint64_t* checksum_out, int32_t* status);
+
 /* ---- read side ---- */
 /* n compressed blocks as produced by S3BufferedPrefetchIterator.next() (storage/S3BufferedPrefetchIterator.scala:196-212).
  * Block i covers n_slices[i] consecutive reduce partitions (1 for ShuffleBlockId, >1 for ShuffleBlockBatchId,

@@ -127,6 +127,14 @@ int b2sh_serialized_writer_range_rows(b2sh_serialized_writer* w, uint32_t n_keys
                                       const uint32_t* key_off, const uint32_t* key_len, const int32_t* key_null_field,
                                       uint32_t n_bounds, const uint8_t* bound_base, uint64_t bound_bytes,
                                       const uint32_t* bound_len);
+/* RoundRobinPartitioning of UnsafeRows (INTEGRATION.md §3l), set before the first insert: every later insert is one
+ * record as UnsafeRowSerializer writes it and its partition_id is ignored; commit() makes one
+ * b2s_partition_compress_rows_round_robin_packed call with start_position (Spark's XORShiftRandom(partitionId)
+ * .nextInt(num_partitions)) and sort_rows (spark.sql.execution.sortBeforeRepartition).  num_partitions must be the
+ * writer's numPartitions.  The files are byte-identical to the ones the writer makes when fed the same rows in Spark's
+ * order with Spark's ids.  In this mode the writer never stores into the exchange cache, as for hash_rows. */
+int b2sh_serialized_writer_round_robin_rows(b2sh_serialized_writer* w, uint32_t num_partitions, int32_t start_position,
+                                            uint32_t sort_rows);
 int b2sh_serialized_writer_insert(b2sh_serialized_writer* w, int32_t partition_id, const uint8_t* bytes, uint64_t len);
 int b2sh_serialized_writer_commit(b2sh_serialized_writer* w, int64_t* partition_lengths_out);
 int b2sh_serialized_writer_statistics(b2sh_serialized_writer* w, uint64_t* bytes, uint64_t* nanos, char* line,

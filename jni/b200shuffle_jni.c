@@ -11,6 +11,8 @@
  *                                          their key columns in, the reduce ids computed on the GPU
  *   partitionCompressRowsRangePacked       the same for a RangePartitioning exchange (INTEGRATION.md §3k): rows,
  *                                          their sort-key columns and the partitioner's bound rows in
+ *   partitionCompressRowsRoundRobinPacked  the same for a RoundRobinPartitioning exchange (INTEGRATION.md §3l): rows,
+ *                                          the task's start position and sortBeforeRepartition in
  *   decompressPacked / decompressedSize    storage/S3ShuffleReader.scala:98-110 (the codec seam, batched drain of
  *                                          storage/S3BufferedPrefetchIterator.scala:196-212)
  *   checksumPacked                         shuffle/S3SingleSpillShuffleMapOutputWriter.scala:54-63,
@@ -157,10 +159,12 @@ typedef struct {
 /* cached (may be NULL): int[1], the cached store's flag; then (shuffleId, mapId) keys the exchange-cache entry.
  * hash (may be NULL, then cached is NULL): the records are serialized rows whose reduce ids are computed on the GPU
  * from these key columns, recPart is not read: Spark's HashPartitioning ids (partitionCompressRowsHashPacked), or with
- * range its RangePartitioner ids over those bounds (partitionCompressRowsRangePacked; numPartitions = range->n + 1) */
+ * range its RangePartitioner ids over those bounds (partitionCompressRowsRangePacked; numPartitions = range->n + 1).
+ * rr (may be NULL; then hash is NULL): {startPosition, sortRows}, the records are serialized rows dealt out in Spark's
+ * repartition(n) order (partitionCompressRowsRoundRobinPacked); recPart is not read */
 static jint partition_compress(JNIEnv* e, jint shuffleId, jlong mapId, jintArray cached, const composite_key* hash,
-                               const range_bounds* range, jint codec, jint level, jint blockSize, jint alg,
-                               jint numPartitions, jlong nRecords, jlong records, jlong recBytes, jlong recLen,
+                               const range_bounds* range, const jint* rr, jint codec, jint level, jint blockSize,
+                               jint alg, jint numPartitions, jlong nRecords, jlong records, jlong recBytes, jlong recLen,
                                jlong recPart, jlong dst, jlong dstCap, jlongArray dstOff, jlongArray dstLen,
                                jlongArray meta, jlongArray checksums, jintArray status) {
   if ((cached && (*e)->GetArrayLength(e, cached) < 1) || numPartitions < 1 || !dstOff || !dstLen || !meta || !status || (*e)->GetArrayLength(e, dstOff) < numPartitions ||
@@ -193,7 +197,11 @@ static jint partition_compress(JNIEnv* e, jint shuffleId, jlong mapId, jintArray
   uint64_t total = 0;
   int32_t stored = 0;
   const int rc =
-      range ? b2s_partition_compress_rows_range_packed(
+      rr ? b2s_partition_compress_rows_round_robin_packed(
+               (uint32_t)codec, (int32_t)level, (uint32_t)blockSize, (uint32_t)alg, (uint32_t)numPartitions, rr[0],
+               (uint32_t)rr[1], (uint64_t)nRecords, PTR(const uint8_t, records), (uint64_t)recBytes,
+               PTR(const uint32_t, recLen), PTR(uint8_t, dst), (uint64_t)dstCap, buf, buf + R, &total, buf + 2 * R, st)
+      : range ? b2s_partition_compress_rows_range_packed(
                   (uint32_t)codec, (int32_t)level, (uint32_t)blockSize, (uint32_t)alg, (uint64_t)nRecords,
                   PTR(const uint8_t, records), (uint64_t)recBytes, PTR(const uint32_t, recLen), (uint32_t)hash->n, kt,
                   ko, kl, knf, (uint32_t)range->n, PTR(const uint8_t, range->rows), (uint64_t)range->bytes, bl,
@@ -233,7 +241,7 @@ JNIEXPORT jint JNICALL J(partitionCompressPacked)(JNIEnv* e, jclass c, jint code
                                                   jlongArray dstOff, jlongArray dstLen, jlongArray meta,
                                                   jlongArray checksums, jintArray status) {
   (void)c;
-  return partition_compress(e, 0, 0, 0, 0, 0, codec, level, blockSize, alg, numPartitions, nRecords, records,
+  return partition_compress(e, 0, 0, 0, 0, 0, 0, codec, level, blockSize, alg, numPartitions, nRecords, records,
                             recBytes, recLen, recPart, dst, dstCap, dstOff, dstLen, meta, checksums, status);
 }
 /* HashPartitioning exchange of UnsafeRows (INTEGRATION.md §3j): records as UnsafeRowSerializer writes them, recLen
@@ -248,7 +256,7 @@ JNIEXPORT jint JNICALL J(partitionCompressRowsHashPacked)(JNIEnv* e, jclass c, j
                                                           jintArray status) {
   (void)c;
   const composite_key keys = {nKeys, keyType, keyOff, keyLen, keyNullField};
-  return partition_compress(e, 0, 0, 0, &keys, 0, codec, level, blockSize, alg, numPartitions, nRecords, records,
+  return partition_compress(e, 0, 0, 0, &keys, 0, 0, codec, level, blockSize, alg, numPartitions, nRecords, records,
                             recBytes, recLen, 0, dst, dstCap, dstOff, dstLen, meta, checksums, status);
 }
 /* RangePartitioning exchange of UnsafeRows (INTEGRATION.md §3k): records and key columns as
@@ -270,7 +278,23 @@ JNIEXPORT jint JNICALL J(partitionCompressRowsRangePacked)(JNIEnv* e, jclass c, 
   if (nBounds < 0 || nBounds > (1 << 24) - 1) return B2S_E_ARG;
   const composite_key keys = {nKeys, keyType, keyOff, keyLen, keyNullField};
   const range_bounds range = {nBounds, bounds, boundBytes, boundLen};
-  return partition_compress(e, 0, 0, 0, &keys, &range, codec, level, blockSize, alg, nBounds + 1, nRecords, records,
+  return partition_compress(e, 0, 0, 0, &keys, &range, 0, codec, level, blockSize, alg, nBounds + 1, nRecords, records,
+                            recBytes, recLen, 0, dst, dstCap, dstOff, dstLen, meta, checksums, status);
+}
+/* RoundRobinPartitioning exchange of UnsafeRows (INTEGRATION.md §3l): records as partitionCompressRowsHashPacked, no
+ * key columns: startPosition is new XORShiftRandom(partitionId).nextInt(numPartitions), sortRows (0 / 1) is
+ * spark.sql.execution.sortBeforeRepartition; the GPU sorts the rows as UnsafeExternalRowSorter would and deals the
+ * k-th to (startPosition + 1 + k) % numPartitions */
+JNIEXPORT jint JNICALL J(partitionCompressRowsRoundRobinPacked)(JNIEnv* e, jclass c, jint codec, jint level,
+                                                                jint blockSize, jint alg, jint numPartitions,
+                                                                jint startPosition, jint sortRows, jlong nRecords,
+                                                                jlong records, jlong recBytes, jlong recLen, jlong dst,
+                                                                jlong dstCap, jlongArray dstOff, jlongArray dstLen,
+                                                                jlongArray meta, jlongArray checksums,
+                                                                jintArray status) {
+  (void)c;
+  const jint rr[2] = {startPosition, sortRows};
+  return partition_compress(e, 0, 0, 0, 0, 0, rr, codec, level, blockSize, alg, numPartitions, nRecords, records,
                             recBytes, recLen, 0, dst, dstCap, dstOff, dstLen, meta, checksums, status);
 }
 /* the same, keeping the partitioned records in the exchange cache as (shuffleId, mapId); cached: int[1] = stored */
@@ -282,7 +306,7 @@ JNIEXPORT jint JNICALL J(partitionCompressCachedPacked)(JNIEnv* e, jclass c, jin
                                                         jintArray status, jintArray cached) {
   (void)c;
   if (!cached) return B2S_E_ARG;
-  return partition_compress(e, shuffleId, mapId, cached, 0, 0, codec, level, blockSize, alg, numPartitions,
+  return partition_compress(e, shuffleId, mapId, cached, 0, 0, 0, codec, level, blockSize, alg, numPartitions,
                             nRecords, records, recBytes, recLen, recPart, dst, dstCap, dstOff, dstLen, meta, checksums,
                             status);
 }

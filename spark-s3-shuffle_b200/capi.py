@@ -88,6 +88,12 @@ PROTOTYPES = [
     ("b2s_partition_compress_rows_range_dev", C.c_int,
      [_u32, _u32, _i32, _u32, _u32, _u64, _vp, _u64, _u32p, _u32, _u32p, _u32p, _u32p, _i32p, _u32, _u8p, _u64, _u32p,
       _vp, _u64, _u64p, _u64p, _u64p, _u64p, _i32p]),
+    ("b2s_partition_compress_rows_round_robin_packed", C.c_int,
+     [_u32, _i32, _u32, _u32, _u32, _i32, _u32, _u64, _u8p, _u64, _u32p, _u8p, _u64, _u64p, _u64p, _u64p, _u64p,
+      _i32p]),
+    ("b2s_partition_compress_rows_round_robin_dev", C.c_int,
+     [_u32, _u32, _i32, _u32, _u32, _u32, _i32, _u32, _u64, _vp, _u64, _u32p, _vp, _u64, _u64p, _u64p, _u64p, _u64p,
+      _i32p]),
     ("b2s_decompress_batch", C.c_int,
      [_u32, _u32, _u32, _vp, _u64p, _u32p, _vp, _vp, _vp, _u64p, _u64p, _i32p, _i32p]),
     ("b2s_decompress_packed", C.c_int,
@@ -689,6 +695,35 @@ def partition_compress_rows_range_dev(codec, d_records, rec_bytes, d_rec_len, n_
         dev, codec, level, block_size, checksum_alg, n_records, d_records, rec_bytes, d_rec_len, nk, _ptr(kt), _ptr(ko),
         _ptr(kl), _ptr(kn), nb, _ptr(bb), bbytes, _ptr(bl), d_dst, dst_cap, _ptr(dst_off), _ptr(dst_len),
         C.addressof(total), _ptr(cks), _ptr(st)), "b2s_partition_compress_rows_range_dev")
+    return dict(dst_off=dst_off, dst_len=dst_len, total=total.value, checksums=cks, status=st)
+
+
+def partition_compress_rows_round_robin_packed(codec, records, rec_len, num_partitions, start_position, sort_rows,
+                                               dst, block_size=0, checksum_alg=CHECKSUM_NONE, level=0):
+    """partition_compress_packed of serialized UnsafeRows ([int32 big-endian size][row] each) in Spark's repartition(n)
+    order and ids: sorted by (row hash, row bytes) when sort_rows and num_partitions > 1, then the k-th row to
+    (start_position + 1 + k) % num_partitions.  -> dict(dst_off, dst_len, total, checksums, status)"""
+    records, dst = _as_u8(records), _as_u8(dst)
+    rec_len = np.ascontiguousarray(rec_len, dtype=np.uint32)
+    dst_off, dst_len, cks, st = _partition_out(num_partitions)
+    total = _u64(0)
+    _check(load().b2s_partition_compress_rows_round_robin_packed(
+        codec, level, block_size, checksum_alg, num_partitions, start_position, sort_rows, rec_len.size, _ptr(records),
+        records.size, _ptr(rec_len), _ptr(dst), dst.size, _ptr(dst_off), _ptr(dst_len), C.addressof(total), _ptr(cks),
+        _ptr(st)), "b2s_partition_compress_rows_round_robin_packed")
+    return dict(dst_off=dst_off, dst_len=dst_len, total=total.value, checksums=cks, status=st)
+
+
+def partition_compress_rows_round_robin_dev(codec, d_records, rec_bytes, d_rec_len, n_records, num_partitions,
+                                            start_position, sort_rows, d_dst, dst_cap, block_size=0,
+                                            checksum_alg=CHECKSUM_NONE, level=0, dev=0):
+    """partition_compress_rows_round_robin_packed on device addresses (records, u32 lengths, destination arena)"""
+    dst_off, dst_len, cks, st = _partition_out(num_partitions)
+    total = _u64(0)
+    _check(load().b2s_partition_compress_rows_round_robin_dev(
+        dev, codec, level, block_size, checksum_alg, num_partitions, start_position, sort_rows, n_records, d_records,
+        rec_bytes, d_rec_len, d_dst, dst_cap, _ptr(dst_off), _ptr(dst_len), C.addressof(total), _ptr(cks), _ptr(st)),
+        "b2s_partition_compress_rows_round_robin_dev")
     return dict(dst_off=dst_off, dst_len=dst_len, total=total.value, checksums=cks, status=st)
 
 

@@ -235,8 +235,8 @@ double ms_between(cudaEvent_t a, cudaEvent_t b) {
 
 // The timed marks of a slot's main stream, which b2s_last_timing is read from (add_times): kernel region (K), codec
 // step (T), upload (H), download (D), partition or sort step (P), row framing: walk + count, emit (F0-F1, F2-F3; the
-// hash step of a hash partition, the range step of a range partition: F0-F1), grouping + merge of an aggregation (G).  Stop: where a call that did not
-// record the end of a span it reads stopped.
+// hash step of a hash partition, the range step of a range partition, the round-robin step: F0-F1), grouping + merge
+// of an aggregation (G).  Stop: where a call that did not record the end of a span it reads stopped.
 enum Mark { K0, K1, T0, T1, H0, H1, D0, D1, P0, P1, F0, F1, F2, F3, G0, G1, kStop, kMarks };
 
 struct Slot {
@@ -844,7 +844,7 @@ void add_times(Slot& S, Family f) {
     case Family::kPartitionNone:  // partition step + checksum (without one, the gather); the partition step
       t.kernel_ms += S.span(P0, f == Family::kPartitionNone && !S.mine(K1) ? P1 : K1);
       t.top_kernel_ms += f == Family::kPartition ? S.span(T0, T1) : S.span(P0, P1);
-      if (S.mine(F0)) dominant(F0, F1);  // a hash or range partition: the hash or range step
+      if (S.mine(F0)) dominant(F0, F1);  // a hash, range or round-robin partition: its id step
       else S.take_pairs();
       break;
     case Family::kSort:       // verification + decode + sort; the sort step; the decoder's dominant pairs
@@ -1763,7 +1763,8 @@ static uint64_t first_record_past(const uint64_t* d_off, const uint32_t* d_len, 
 }
 
 // How a rows call computes its reduce ids on the device: Spark's HashPartitioning ids of the rows by these key columns,
-// or (range) its RangePartitioner ids over n_bounds bound rows of bound_bytes in host memory, bound_len[j] each
+// or (range) its RangePartitioner ids over n_bounds bound rows of bound_bytes in host memory, bound_len[j] each, or
+// (round_robin) its RoundRobinPartitioning ids from position start, the rows sorted first when sort is set
 struct RowIds {
   KeySpec keys;
   bool range = false;
@@ -1771,10 +1772,14 @@ struct RowIds {
   const uint8_t* bound_base = nullptr;
   uint64_t bound_bytes = 0;
   const uint32_t* bound_len = nullptr;
+  bool round_robin = false;
+  uint32_t start = 0;
+  bool sort = false;
 };
 
 // The B2S_E_ARG of a rows call's verdict word (~0: none): a bad record (kHashBad*, launch_rows_hash), or for a range
-// call a bad bound or a bad record (launch_rows_range)
+// call a bad bound or a bad record (launch_rows_range), or for a round-robin call a bad record
+// (launch_rows_round_robin_hash)
 static int row_ids_verdict(const RowIds& ids, uint64_t v) {
   static const char* const why[] = {"", "bound_len is below 4", "its size prefix is not bound_len - 4",
                                     "its row does not hold a key slot", "its row does not hold a key's null word",
@@ -1782,6 +1787,11 @@ static int row_ids_verdict(const RowIds& ids, uint64_t v) {
                                     "a decimal key's size is not 1..16 or it runs past its row"};
   static const char* const rec_why[] = {"", "rec_len is below 4", "its size prefix is not rec_len - 4"};
   char msg[256];
+  if (ids.round_robin) {
+    snprintf(msg, sizeof msg, "record %llu is not a serialized UnsafeRow: %s", (unsigned long long)(v >> 3),
+             (v & 7) == kRowsBadWords ? "its row size is not a multiple of 8" : rec_why[v & 7]);
+    return fail(B2S_E_ARG, "%s", msg);
+  }
   if (ids.range && !(v & kRangeBadRecord)) {
     if ((v & 7) == kRangeBadOrder)
       snprintf(msg, sizeof msg, "bound %llu is not above the bound before it: the bounds must be strictly increasing",
@@ -1808,12 +1818,45 @@ static int upload_bounds(const RowIds& ids, uint8_t* d_ws, RangeWs* w, cudaStrea
   return 0;  // a copy from pageable memory has taken its source when it returns, so off may go
 }
 
+// The round-robin step's order: every record checked (lowering P's bad-record word) and, with the sort (sws / rws:
+// the whole-row sort's workspaces, else nullptr), hashed and sorted by its whole-row key.  *order = the record at each
+// sorted position (nullptr: input order).  One 8-byte readback per refinement round; the first also brings the
+// bad-record word and the byte total, so a bad record fails the call, and a record past rec_bytes ends the sort,
+// before any round reads it (the partition step's readback then names that record).
+static int round_robin_order(Slot& S, const RowIds& ids, uint64_t n, const uint8_t* d_rec, uint64_t rec_bytes,
+                             const uint32_t* d_len, const PartitionPlan& P, uint8_t* sws, uint8_t* rws,
+                             const uint32_t** order, uint64_t* launches) {
+  cudaStream_t st = S.st;
+  *order = nullptr;
+  launch_rows_round_robin_hash(d_rec, rec_bytes, P.src_off, d_len, n, rws ? rows_whole_words(sws, n) : nullptr,
+                               rws ? rows_refine_klen(rws, n) : nullptr, P.readback, st, launches);
+  if (!rws) return 0;
+  launch_rows_whole_order(n, sws, rws, st, launches);
+  if (int rc = S.hmeta.ensure(24)) return rc;
+  uint64_t* rb = (uint64_t*)S.hmeta.p;  // [tied records | runs << 32, bad record, byte total]
+  for (uint32_t d = 4, round = 0;; d += kKeyChunkBytes, round++) {
+    launch_rows_refine_mark(n, d, rws, 0, st, launches);
+    CU(cudaMemcpyAsync(rb, rows_refine_readback(rws, n, 0), 8, cudaMemcpyDeviceToHost, st));
+    if (!round) CU(cudaMemcpyAsync(rb + 1, P.readback, 16, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    CU(cudaGetLastError());
+    if (!round && rb[1] != ~0ull) return row_ids_verdict(ids, rb[1]);
+    if (!round && rb[2] != rec_bytes) return 0;
+    const uint64_t tied = rb[0] & 0xffffffffull, runs = rb[0] >> 32;
+    if (!tied) break;
+    launch_rows_whole_refine_round(d_rec, P.src_off, d_len, n, tied, runs, d, sws, rws, st, launches);
+  }
+  *order = rows_refine_order(rws, n, 0);
+  return 0;
+}
+
 // The partition step and the compression of the non-empty partitions, on device-resident records.  d_dst receives the
 // .data arena (dst_cap bytes); *arena_bytes the bytes it needs.  Returns B2S_E_DST_TOO_SMALL (status[] set for the
 // partitions that do not fit) when dst_cap is short.  part_start (optional) receives the R + 1 partition offsets of the
 // partitioned records, which are in d_dst (codec NONE) or S.parena.  ids (d_part unused): the ids are computed from the
 // rows on the device (RowIds), between the offsets and the radix passes (marks F0 and F1 bracket that step: the hash
-// kernel, or the range call's bound checks and id kernel), and a bad record or bound fails the call.
+// kernel, the range call's bound checks and id kernel, or the round-robin call's hash, sort and id kernel), and a bad
+// record or bound fails the call.
 static int partition_compress_run(Device* D, Slot& S, uint32_t codec, int32_t level, uint32_t bs, uint32_t alg,
                                   uint32_t R, uint64_t n, const uint8_t* d_rec, uint64_t rec_bytes,
                                   const uint32_t* d_len, const uint32_t* d_part, uint8_t* d_dst, uint64_t dst_cap,
@@ -1823,11 +1866,14 @@ static int partition_compress_run(Device* D, Slot& S, uint32_t codec, int32_t le
   cudaStream_t st = S.st;
   std::vector<uint64_t> pstart(R), plen(R);
   const bool range = ids && ids->range;
+  const bool rr = ids && ids->round_robin, rr_sort = rr && ids->sort && R > 1;  // R == 1: Spark does not sort
   CU(S.mark(P0, st));
   PartitionPlan P;
   if (n) {
     const size_t pws = partition_ws_bytes(n, R, ids != nullptr);
-    int rc = S.pws.ensure(pws + (range ? rows_range_ws_bytes(ids->n_bounds, ids->bound_bytes) : 0));
+    const size_t sws = rr_sort ? rows_sort_ws_bytes(n, kKeyPrefixBytes) : 0;
+    int rc = S.pws.ensure(pws + (range ? rows_range_ws_bytes(ids->n_bounds, ids->bound_bytes) : 0) +
+                          (rr_sort ? sws + rows_refine_ws_bytes(n, 0) : 0));
     if (rc) return rc;
     uint8_t* ws = (uint8_t*)S.pws.p;
     RangeWs rw;
@@ -1836,13 +1882,20 @@ static int partition_compress_run(Device* D, Slot& S, uint32_t codec, int32_t le
     if (ids) {
       launch_partition_offsets(d_len, nullptr, n, R, ws, &P, st, launches);
       CU(S.mark(F0, st, *launches));
-      if (range)
+      const uint32_t* order = nullptr;
+      if (rr) {
+        if (int rc = round_robin_order(S, *ids, n, d_rec, rec_bytes, d_len, P, rr_sort ? ws + pws : nullptr,
+                                       rr_sort ? ws + pws + sws : nullptr, &order, launches))
+          return rc;
+        launch_rows_round_robin_ids(n, ids->start, R, P.ids, st, launches);
+      } else if (range) {
         launch_rows_range(d_rec, rec_bytes, P.src_off, d_len, n, ids->keys, rw, ids->n_bounds, P.ids, P.readback, st,
                           launches);
-      else
+      } else {
         launch_rows_hash(d_rec, rec_bytes, P.src_off, d_len, n, ids->keys, R, P.ids, P.readback, st, launches);
+      }
       CU(S.mark(F1, st, *launches));
-      launch_partition_order(d_len, P.ids, n, R, ws, &P, st, launches);
+      launch_partition_order(d_len, P.ids, n, R, ws, &P, st, launches, order);
     } else {
       launch_partition(d_len, d_part, n, R, ws, &P, st, launches);
     }
@@ -2746,6 +2799,70 @@ int b2s_partition_compress_rows_range_dev(uint32_t dev_index, uint32_t codec, in
                           dst_base, dst_off, dst_len, status))
     return rc;
   return partition_compress_dev(dev_index, codec, level, codec_block_size, checksum_alg, n_bounds + 1, n_records,
+                                rec_base, rec_bytes, rec_len, nullptr, dst_base, dst_cap, dst_off, dst_len, dst_total,
+                                checksum_out, status, &ids);
+}
+
+// ------------------------------------------------------------------------------------------------------------
+// write side, round-robin-partitioned rows: Spark's repartition(n) order and ids, then the partition + compress step
+// ------------------------------------------------------------------------------------------------------------
+// The partition step's checks, then the position and sort flag; a device is needed only after them, as for the hash
+// call.  start + n past 2^31 - 1 is refused: Spark's Int position would wrap there.
+static int round_robin_args(uint32_t codec, uint32_t codec_block_size, uint32_t alg, uint32_t R, int32_t start,
+                            uint32_t sort, uint64_t n, const void* rec_base, uint64_t rec_bytes,
+                            const uint32_t* rec_len, const RowIds& ids, const void* dst_base, const uint64_t* dst_off,
+                            const uint64_t* dst_len, const int32_t* status) {
+  const uint32_t bs = block_size_or_default(codec_block_size);
+  if (int rc = partition_args(codec, bs, alg, R, n, rec_base, rec_bytes, rec_len, nullptr, dst_base, dst_off, dst_len,
+                              status, &ids))
+    return rc;
+  if (start < 0 || (uint32_t)start >= R) return fail(B2S_E_ARG, "start_position must be in [0, num_partitions)%s");
+  if (sort > 1) return fail(B2S_E_ARG, "sort_rows must be 0 or 1%s");
+  if ((uint64_t)start + n > 0x7fffffffull)
+    return fail(B2S_E_ARG, "start_position + n_records is past 2^31 - 1, where Spark's position wraps%s");
+  if (!g_ctx)
+    if (int rc = no_device()) return rc;
+  return 0;
+}
+
+static RowIds round_robin_ids(int32_t start, uint32_t sort) {
+  RowIds ids;
+  ids.round_robin = true;
+  ids.start = (uint32_t)start;
+  ids.sort = sort != 0;
+  return ids;
+}
+
+int b2s_partition_compress_rows_round_robin_packed(uint32_t codec, int32_t level, uint32_t codec_block_size,
+                                                   uint32_t checksum_alg, uint32_t num_partitions,
+                                                   int32_t start_position, uint32_t sort_rows, uint64_t n_records,
+                                                   const uint8_t* rec_base, uint64_t rec_bytes,
+                                                   const uint32_t* rec_len, uint8_t* dst_base, uint64_t dst_cap,
+                                                   uint64_t* dst_off, uint64_t* dst_len, uint64_t* dst_total,
+                                                   uint64_t* checksum_out, int32_t* status) {
+  if (dst_total) *dst_total = 0;
+  const RowIds ids = round_robin_ids(start_position, sort_rows);
+  if (int rc = round_robin_args(codec, codec_block_size, checksum_alg, num_partitions, start_position, sort_rows,
+                                n_records, rec_base, rec_bytes, rec_len, ids, dst_base, dst_off, dst_len, status))
+    return rc;
+  return partition_compress_packed(codec, level, codec_block_size, checksum_alg, num_partitions, n_records, rec_base,
+                                   rec_bytes, rec_len, nullptr, dst_base, dst_cap, dst_off, dst_len, dst_total,
+                                   checksum_out, status, nullptr, &ids);
+}
+
+int b2s_partition_compress_rows_round_robin_dev(uint32_t dev_index, uint32_t codec, int32_t level,
+                                                uint32_t codec_block_size, uint32_t checksum_alg,
+                                                uint32_t num_partitions, int32_t start_position, uint32_t sort_rows,
+                                                uint64_t n_records, const uint8_t* rec_base, uint64_t rec_bytes,
+                                                const uint32_t* rec_len, uint8_t* dst_base, uint64_t dst_cap,
+                                                uint64_t* dst_off, uint64_t* dst_len, uint64_t* dst_total,
+                                                uint64_t* checksum_out, int32_t* status) {
+  if (dst_total) *dst_total = 0;
+  const RowIds ids = round_robin_ids(start_position, sort_rows);
+  if (int rc = round_robin_args(codec, codec_block_size, checksum_alg, num_partitions, start_position, sort_rows,
+                                n_records, rec_base, rec_bytes, rec_len, ids, dst_base, dst_off, dst_len, status))
+    return rc;
+  return partition_compress_dev(dev_index, codec, level, codec_block_size, checksum_alg, num_partitions, n_records,
                                 rec_base, rec_bytes, rec_len, nullptr, dst_base, dst_cap, dst_off, dst_len, dst_total,
                                 checksum_out, status, &ids);
 }

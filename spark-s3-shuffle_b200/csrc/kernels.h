@@ -184,9 +184,11 @@ size_t partition_ws_bytes(uint64_t n, uint32_t num_partitions, bool hashed_ids =
 void launch_partition_offsets(const uint32_t* d_rec_len, const uint32_t* d_rec_part, uint64_t n,
                               uint32_t num_partitions, uint8_t* d_ws, PartitionPlan* plan, cudaStream_t st,
                               uint64_t* launches);
-// order: the radix passes over the ids, the sorted offsets and the partition bounds
+// order: the radix passes over the ids, the sorted offsets and the partition bounds.  idx_in (nullptr: the position):
+// the record index of position k, whose id is d_rec_part[k]; the passes are stable, so a partition keeps that order.
 void launch_partition_order(const uint32_t* d_rec_len, const uint32_t* d_rec_part, uint64_t n, uint32_t num_partitions,
-                            uint8_t* d_ws, PartitionPlan* plan, cudaStream_t st, uint64_t* launches);
+                            uint8_t* d_ws, PartitionPlan* plan, cudaStream_t st, uint64_t* launches,
+                            const uint32_t* idx_in = nullptr);
 void launch_partition(const uint32_t* d_rec_len, const uint32_t* d_rec_part, uint64_t n, uint32_t num_partitions,
                       uint8_t* d_ws, PartitionPlan* plan, cudaStream_t st,
                       uint64_t* launches);
@@ -323,6 +325,20 @@ void launch_rows_refine_round(const uint8_t* arena, uint64_t n, const KeySpec& k
 // after the last round (no tied record): the sorted record indices, and per position 1 where a new key starts
 const uint32_t* rows_refine_order(uint8_t* d_rws, uint64_t n, uint32_t n_ranges);
 const uint32_t* rows_refine_heads(uint8_t* d_rws, uint64_t n, uint32_t n_ranges);
+// Whole-row sort (a round-robin exchange's sortBeforeRepartition order): the key of record i (rec_len[i] bytes at
+// rec + rec_off[i], [size: int32 big-endian][row], size a multiple of 8) is [hash ^ 0x80000000: 4 B][size: 4 B][row]
+// (big-endian words), prefix-free: rows of different sizes differ within the first 8 bytes, rows of equal size end
+// together.  d_ws: rows_sort_ws_bytes(n, kKeyPrefixBytes); d_rws: rows_refine_ws_bytes(n, 0).  The caller stores each
+// key's first word at rows_whole_words(d_ws, n)[i] and its length at rows_refine_klen(d_rws, n)[i] (0: never read);
+// launch_rows_whole_order radix-sorts the first word only (4 passes) and sets up the order and head flags; the rounds
+// are launch_rows_refine_mark and launch_rows_whole_refine_round from d = 4, kKeyChunkBytes more each; the order ends
+// in rows_refine_order.
+uint32_t* rows_whole_words(uint8_t* d_ws, uint64_t n);
+uint32_t* rows_refine_klen(uint8_t* d_rws, uint64_t n);
+void launch_rows_whole_order(uint64_t n, uint8_t* d_ws, uint8_t* d_rws, cudaStream_t st, uint64_t* launches);
+void launch_rows_whole_refine_round(const uint8_t* rec, const uint64_t* rec_off, const uint32_t* rec_len, uint64_t n,
+                                    uint64_t m, uint64_t segs, uint32_t d, uint8_t* d_ws, uint8_t* d_rws,
+                                    cudaStream_t st, uint64_t* launches);
 // the emitted records to d_dst in the order idx
 void launch_rows_gather(const uint8_t* arena, uint64_t n, uint32_t key_bytes, const uint32_t* idx, uint8_t* d_ws,
                         uint8_t* d_dst, cudaStream_t st, uint64_t* launches);
@@ -362,6 +378,19 @@ RangeWs carve_rows_range_ws(uint8_t* d_ws, uint32_t n_bounds, uint64_t bound_byt
 void launch_rows_range(const uint8_t* rec, uint64_t rec_bytes, const uint64_t* rec_off, const uint32_t* rec_len,
                        uint64_t n, const KeySpec& ks, const RangeWs& w, uint32_t n_bounds, uint32_t* ids,
                        uint64_t* bad, cudaStream_t st, uint64_t* launches);
+
+// ---------------- rows_round_robin.cu (Spark's RoundRobinPartitioning of length-prefixed UnsafeRow records) ---------
+// Records as launch_rows_hash's.  A bad record lowers *bad (device, ~0 = none) to (i << 3) | its reason: kHashBadShort,
+// kHashBadSize, or kRowsBadWords (its row size is not a multiple of 8: not an UnsafeRow).  words / klen (nullptr: no
+// sort, only the checks): the whole-row sort's first key word, hashUnsafeWords(row, 42) ^ 0x80000000 (signed order as
+// unsigned), and key length 8 + size; a bad record, or one ending past rec_bytes, gets length 0: it is not read again.
+constexpr uint64_t kRowsBadWords = 7;
+void launch_rows_round_robin_hash(const uint8_t* rec, uint64_t rec_bytes, const uint64_t* rec_off,
+                                  const uint32_t* rec_len, uint64_t n, uint32_t* words, uint32_t* klen, uint64_t* bad,
+                                  cudaStream_t st, uint64_t* launches);
+// ids[k] = (start + 1 + k) mod num_partitions, k < n: the id of the k-th row the writer sees (start + n < 2^31)
+void launch_rows_round_robin_ids(uint64_t n, uint32_t start, uint32_t num_partitions, uint32_t* ids, cudaStream_t st,
+                                 uint64_t* launches);
 
 // ---------------- aggregate.cu (group key-sorted rows and merge their aggregate buffers) ----------------
 // Aggregate a: op[a] (B2S_AGG_*, with SUM_DECIMAL's precision in bits 8..15) over the 8-byte slot at row offset off[a],

@@ -279,7 +279,8 @@ void launch_partition(const uint32_t* d_rec_len, const uint32_t* d_rec_part, uin
 }
 
 void launch_partition_order(const uint32_t* d_rec_len, const uint32_t* d_rec_part, uint64_t n, uint32_t num_partitions,
-                            uint8_t* d_ws, PartitionPlan* plan, cudaStream_t st, uint64_t* launches) {
+                            uint8_t* d_ws, PartitionPlan* plan, cudaStream_t st, uint64_t* launches,
+                            const uint32_t* idx_in) {
   const PartitionWs w = carve_partition_ws(d_ws, n, num_partitions, plan);
   uint32_t *kA = w.kA, *iA = w.iA, *kB = w.kB, *iB = w.iB;
   uint64_t *hist = w.hist, *ws = w.ws, *unused_total = w.unused_total;
@@ -288,7 +289,7 @@ void launch_partition_order(const uint32_t* d_rec_len, const uint32_t* d_rec_par
   uint32_t bits = 0;
   while (bits < 32 && (1ull << bits) < num_partitions) bits++;
   const uint32_t* keys = nullptr;
-  const uint32_t* idx = nullptr;
+  const uint32_t* idx = idx_in;
   int shift = 0;
   for (uint32_t k = 0; k < passes; k++) {
     const uint32_t pb = (bits - (uint32_t)shift + (passes - k) - 1) / (passes - k);  // spread the bits evenly

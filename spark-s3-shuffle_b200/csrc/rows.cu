@@ -15,7 +15,8 @@
 //   radix  : the fixed-size sort's radix passes (launch_key_radix): the sorted record indices
 //   refine : only for keys longer than the first pass: rounds over the records still tied (runs of equal first bytes
 //            whose keys go on): compacted in order, their next kKeyChunkBytes bytes extracted behind their run number,
-//            radix-sorted stably and put back into their runs' positions, until no run is tied
+//            radix-sorted stably and put back into their runs' positions, until no run is tied.  A whole-row key (the
+//            round-robin exchange's sort, launch_rows_whole_*) refines the same way, its rows read where they lie
 //   gather : sorted lengths -> scan -> destination offsets (launch_sorted_offsets), the partition step's gather (a row
 //            sort; a grouped aggregation gathers only each group's first record, aggregate.cu)
 #include <algorithm>
@@ -296,6 +297,45 @@ __global__ void __launch_bounds__(kRowThreads) refine_extract_kernel(
   }
 }
 
+// Bytes [d, d + kKeyChunkBytes) of a whole-row key (kernels.h, launch_rows_whole_order) as four big-endian words, for
+// d = 4 + 16 r: the size word and row bytes [0, 12) when d == 4, else row bytes [d - 8, d + 8); zero past the row.
+// The row's size is a multiple of 8, so every word lies wholly inside or wholly past it.
+__device__ __forceinline__ uint4 row_key_window(const uint8_t* row, uint32_t size, uint32_t d) {
+  const uint32_t from = d == 4 ? 0 : d - 8, want = d == 4 ? 12 : 16;
+  const uint32_t take = from < size ? min(size - from, want) : 0;
+  uint64_t lo = 0, hi = 0;
+  if (take) {
+    ld_span16<true>(row + from, (int)take, lo, hi);
+    if (take < 8) lo &= (1ull << (8 * take)) - 1;
+    hi = take <= 8 ? 0 : take < 16 ? hi & ((1ull << (8 * (take - 8))) - 1) : hi;
+  }
+  const uint32_t a = __byte_perm((uint32_t)lo, 0, 0x0123), b = __byte_perm((uint32_t)(lo >> 32), 0, 0x0123);
+  const uint32_t c = __byte_perm((uint32_t)hi, 0, 0x0123), e = __byte_perm((uint32_t)(hi >> 32), 0, 0x0123);
+  return d == 4 ? make_uint4(size, a, b, c) : make_uint4(a, b, c, e);
+}
+
+// refine_extract_kernel for whole-row keys: the records are read where they lie (rec + rec_off[i], rec_len[i] bytes,
+// framed), only tied ones, whose key length (klen) says they are whole rows inside the records
+__global__ void __launch_bounds__(kRowThreads) refine_extract_row_kernel(
+    const uint8_t* __restrict__ rec, const uint64_t* __restrict__ rec_off, const uint32_t* __restrict__ rec_len,
+    uint64_t n, const uint32_t* __restrict__ ord, const uint32_t* __restrict__ head, const uint32_t* __restrict__ klen,
+    const uint64_t* __restrict__ scan, uint64_t m, uint32_t d, uint32_t* __restrict__ cpos, uint32_t* __restrict__ cidx,
+    uint32_t* __restrict__ words) {
+  for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (uint64_t)gridDim.x * blockDim.x) {
+    if (!tied(j, n, d, ord, head, klen)) continue;
+    const uint32_t k = (uint32_t)scan[j], s = (uint32_t)(scan[j] >> 32) + head[j] - 1;
+    const uint32_t i = ord[j];
+    cpos[k] = (uint32_t)j;
+    cidx[k] = i;
+    const uint4 w = row_key_window(rec + rec_off[i] + 4, rec_len[i] - 4, d);
+    words[k] = s;
+    words[m + k] = w.x;
+    words[2 * m + k] = w.y;
+    words[3 * m + k] = w.z;
+    words[4 * m + k] = w.w;
+  }
+}
+
 // the k-th of the sorted tied records (sidx) to the k-th tied position; a new key starts where (run, bytes) changes
 __global__ void __launch_bounds__(kRowThreads) refine_scatter_kernel(const uint32_t* __restrict__ sidx, uint64_t m,
                                                                      const uint32_t* __restrict__ words,
@@ -340,6 +380,15 @@ RefineWs carve_refine_ws(uint8_t* d_rws, uint64_t n) {
   r.scan_ws = (uint64_t*)p; p += a256(scan_ws_elems(n) * 8);
   r.readback = (uint64_t*)p;
   return r;
+}
+
+// a refinement round's end: the m extracted (run, bytes) keys sorted stably and put back into their runs' positions
+void refine_sort_scatter(const KeySortWs& w, const RefineWs& r, uint64_t m, uint64_t segs, cudaStream_t st,
+                         uint64_t* launches) {
+  // the run number takes as many passes as it has bytes (none for a single run)
+  const uint32_t lead = segs <= 1 ? 0 : segs <= 256 ? 1 : segs <= 65536 ? 2 : segs <= (1u << 24) ? 3 : 4;
+  const uint32_t* sidx = launch_key_radix(w, m, 4 + kKeyChunkBytes, st, launches, lead);
+  refine_scatter_kernel<<<grid_for(m), kRowThreads, 0, st>>>(sidx, m, w.words, r.cpos, r.cidx, r.ord, r.head);
 }
 
 // the framing workspace: bitmap (whole tiles), tile counts, their scan workspace, readback, ranges, work counter
@@ -472,10 +521,30 @@ void launch_rows_refine_round(const uint8_t* arena, uint64_t n, const KeySpec& k
   const RefineWs r = carve_refine_ws(d_rws, n);
   refine_extract_kernel<<<grid_for(n), kRowThreads, 0, st>>>(arena, w.src_off, w.len, n, ks, r.ord, r.head, r.klen,
                                                              r.scan, m, d, r.cpos, r.cidx, w.words);
-  // the run number takes as many passes as it has bytes (none for a single run)
-  const uint32_t lead = segs <= 1 ? 0 : segs <= 256 ? 1 : segs <= 65536 ? 2 : segs <= (1u << 24) ? 3 : 4;
-  const uint32_t* sidx = launch_key_radix(w, m, 4 + kKeyChunkBytes, st, launches, lead);
-  refine_scatter_kernel<<<grid_for(m), kRowThreads, 0, st>>>(sidx, m, w.words, r.cpos, r.cidx, r.ord, r.head);
+  refine_sort_scatter(w, r, m, segs, st, launches);
+  if (launches) *launches += 2;
+}
+
+uint32_t* rows_whole_words(uint8_t* d_ws, uint64_t n) { return carve_key_sort_ws(d_ws, n, kKeyPrefixBytes).words; }
+uint32_t* rows_refine_klen(uint8_t* d_rws, uint64_t n) { return carve_refine_ws(d_rws, n).klen; }
+
+void launch_rows_whole_order(uint64_t n, uint8_t* d_ws, uint8_t* d_rws, cudaStream_t st, uint64_t* launches) {
+  if (!n) return;
+  const KeySortWs w = carve_key_sort_ws(d_ws, n, kKeyPrefixBytes);
+  const RefineWs r = carve_refine_ws(d_rws, n);
+  const uint32_t* idx = launch_key_radix(w, n, 4, st, launches);
+  refine_init_kernel<<<grid_for(n), kRowThreads, 0, st>>>(idx, n, w.words, 1, r.ord, r.head);
+  if (launches) *launches += 1;
+}
+
+void launch_rows_whole_refine_round(const uint8_t* rec, const uint64_t* rec_off, const uint32_t* rec_len, uint64_t n,
+                                    uint64_t m, uint64_t segs, uint32_t d, uint8_t* d_ws, uint8_t* d_rws,
+                                    cudaStream_t st, uint64_t* launches) {
+  const KeySortWs w = carve_key_sort_ws(d_ws, n, kKeyPrefixBytes);
+  const RefineWs r = carve_refine_ws(d_rws, n);
+  refine_extract_row_kernel<<<grid_for(n), kRowThreads, 0, st>>>(rec, rec_off, rec_len, n, r.ord, r.head, r.klen,
+                                                                 r.scan, m, d, r.cpos, r.cidx, w.words);
+  refine_sort_scatter(w, r, m, segs, st, launches);
   if (launches) *launches += 2;
 }
 

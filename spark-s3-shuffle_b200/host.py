@@ -79,6 +79,7 @@ PROTOTYPES = [
     ("b2sh_serialized_writer_create", C.c_int, [_vp, _i32, _i64, _i32, C.POINTER(_vp)]),
     ("b2sh_serialized_writer_hash_rows", C.c_int, [_vp, _u32, _vp, _vp, _vp, _vp]),
     ("b2sh_serialized_writer_range_rows", C.c_int, [_vp, _u32, _vp, _vp, _vp, _vp, _u32, _vp, _u64, _vp]),
+    ("b2sh_serialized_writer_round_robin_rows", C.c_int, [_vp, _u32, _i32, _u32]),
     ("b2sh_serialized_writer_insert", C.c_int, [_vp, _i32, _vp, _u64]),
     ("b2sh_serialized_writer_commit", C.c_int, [_vp, _vp]),
     ("b2sh_serialized_writer_statistics", C.c_int, [_vp, C.POINTER(_u64), C.POINTER(_u64), C.c_char_p, _u32]),
@@ -302,6 +303,11 @@ class S3SerializedShuffleWriter:
         bl = np.array([len(b) for b in bounds] or [0], dtype=np.uint32)
         _check(load().b2sh_serialized_writer_range_rows(self._h, len(keys), *[a.ctypes.data for a in arrs], len(bounds),
                                                         base.ctypes.data, sum(len(b) for b in bounds), bl.ctypes.data))
+
+    def roundRobinRows(self, numPartitions, startPosition, sortRows):
+        """RoundRobinPartitioning (Spark's repartition(n)) from startPosition, the rows sorted first when sortRows,
+        before the first insert; numPartitions must be the writer's"""
+        _check(load().b2sh_serialized_writer_round_robin_rows(self._h, numPartitions, startPosition, int(sortRows)))
 
     def insertRecord(self, partitionId, record):
         a = np.frombuffer(record, dtype=np.uint8) if not isinstance(record, np.ndarray) else np.ascontiguousarray(record)

@@ -533,8 +533,18 @@ class S3SerializedShuffleWriter {
     boundRows_.assign(boundBase, boundBase + (nBounds ? boundBytes : 0));
     boundLen_.assign(boundLen, boundLen + nBounds);
   }
+  // RoundRobinPartitioning (b2s_partition_compress_rows_round_robin_packed): every later insert is one serialized row
+  // whose partitionId is ignored, and commit() sorts (sortRows) and deals the rows out on the GPU from startPosition
+  void roundRobinRows(uint32_t numPartitions, int32_t startPosition, uint32_t sortRows) {
+    if (!recLen_.empty()) throw RuntimeException("Precondition: round_robin_rows must come before the first insert.");
+    if ((uint64_t)numPartitions != (uint64_t)numPartitions_)
+      throw RuntimeException("Precondition: round_robin_rows needs num_partitions == numPartitions.");
+    roundRobin_ = true;
+    rrStart_ = startPosition;
+    rrSort_ = sortRows;
+  }
   void insertRecord(int32_t partitionId, const uint8_t* b, uint64_t n) {
-    const bool hashed = !keyType_.empty();
+    const bool hashed = !keyType_.empty() || roundRobin_;
     if (!hashed && (partitionId < 0 || partitionId >= numPartitions_))
       throw RuntimeException("Precondition: Invalid partition id.");
     if (n > 0xffffffffull) throw RuntimeException("Precondition: record longer than 4 GiB.");
@@ -554,7 +564,13 @@ class S3SerializedShuffleWriter {
     uint64_t total = 0;
     int rc;
     const char* call = "b2s_partition_compress_packed";
-    if (range_) {  // range-partitioned rows: never cached, as hashed ones
+    if (roundRobin_) {  // round-robin rows: never cached, as hashed ones
+      call = "b2s_partition_compress_rows_round_robin_packed";
+      rc = b2s_partition_compress_rows_round_robin_packed(
+          codec, d_.zstdLevel, d_.lz4BlockSize, alg, R, rrStart_, rrSort_, recLen_.size(), records_.data(),
+          records_.size(), recLen_.data(), out_.data(), bound, doff.data(), dlen.data(), &total, cks.data(),
+          status.data());
+    } else if (range_) {  // range-partitioned rows: never cached, as hashed ones
       call = "b2s_partition_compress_rows_range_packed";
       rc = b2s_partition_compress_rows_range_packed(
           codec, d_.zstdLevel, d_.lz4BlockSize, alg, recLen_.size(), records_.data(), records_.size(), recLen_.data(),
@@ -603,6 +619,9 @@ class S3SerializedShuffleWriter {
   bool range_ = false;  // rangeRows: the ids are RangePartitioner ids over these bounds
   std::vector<uint8_t> boundRows_;
   std::vector<uint32_t> boundLen_;
+  bool roundRobin_ = false;  // roundRobinRows: Spark's repartition(n) order and ids from rrStart_
+  int32_t rrStart_ = 0;
+  uint32_t rrSort_ = 0;
   std::unique_ptr<S3MeasureOutputStream> measure_;
 };
 
@@ -1312,6 +1331,10 @@ int b2sh_serialized_writer_range_rows(b2sh_serialized_writer* w, uint32_t n_keys
   return guarded([&] {
     w->w->rangeRows(n_keys, key_type, key_off, key_len, key_null_field, n_bounds, bound_base, bound_bytes, bound_len);
   });
+}
+int b2sh_serialized_writer_round_robin_rows(b2sh_serialized_writer* w, uint32_t num_partitions, int32_t start_position,
+                                            uint32_t sort_rows) {
+  return guarded([&] { w->w->roundRobinRows(num_partitions, start_position, sort_rows); });
 }
 int b2sh_serialized_writer_insert(b2sh_serialized_writer* w, int32_t partition_id, const uint8_t* bytes, uint64_t len) {
   return guarded([&] { w->w->insertRecord(partition_id, bytes, len); });
