@@ -214,7 +214,8 @@ int b2s_partition_compress_dev(uint32_t dev_index, uint32_t codec, int32_t level
  * b2s_last_error() names the lowest bad record and why: rec_len < 4, a size prefix other than rec_len - 4, a row that
  * does not hold a key slot or a key's null word, a non-null string past the row, a non-null decimal whose size is not
  * 1..16 or that runs past the row.  No usable device -> B2S_E_CUDA.  b2s_last_timing as for the partition calls, plus
- * dominant_ms / dominant_launches = the hash step alone.  No exchange-cache form. */
+ * dominant_ms / dominant_launches = the hash step alone.  Exchange-cache form: b2s_partition_compress_rows_hash_cached_packed
+ * (below, with the exchange cache). */
 int b2s_partition_compress_rows_hash_packed(uint32_t codec, int32_t level, uint32_t codec_block_size,
                                             uint32_t checksum_alg, uint32_t num_partitions, uint64_t n_records,
                                             const uint8_t* rec_base, uint64_t rec_bytes, const uint32_t* rec_len,
@@ -254,7 +255,7 @@ int b2s_partition_compress_rows_hash_dev(uint32_t dev_index, uint32_t codec, int
  * the one before it (equal ones included, such as -0.0 after 0.0, two NaNs or two nulls): the lowest such bound is named;
  * a bad record, as for the hash call.  A bad bound is named before a bad record.  No usable device -> B2S_E_CUDA.
  * b2s_last_timing as for the partition calls, plus dominant_ms / dominant_launches = the range step (the bound checks
- * and the id kernel).  No exchange-cache form. */
+ * and the id kernel).  Exchange-cache form: b2s_partition_compress_rows_range_cached_packed (below). */
 int b2s_partition_compress_rows_range_packed(uint32_t codec, int32_t level, uint32_t codec_block_size,
                                              uint32_t checksum_alg, uint64_t n_records, const uint8_t* rec_base,
                                              uint64_t rec_bytes, const uint32_t* rec_len, uint32_t n_keys,
@@ -290,7 +291,8 @@ int b2s_partition_compress_rows_range_dev(uint32_t dev_index, uint32_t codec, in
  * position would wrap: keep such a task on the CPU path); a bad record (rec_len < 4, a size prefix other than rec_len -
  * 4, a row size that is not a multiple of 8), the lowest one named, in both modes.  No usable device -> B2S_E_CUDA.
  * b2s_last_timing as for the partition calls, plus dominant_ms / dominant_launches = the round-robin step (the checks
- * and hash, the sort with its refinement rounds, the ids).  No exchange-cache form. */
+ * and hash, the sort with its refinement rounds, the ids).  Exchange-cache form:
+ * b2s_partition_compress_rows_round_robin_cached_packed (below). */
 int b2s_partition_compress_rows_round_robin_packed(uint32_t codec, int32_t level, uint32_t codec_block_size,
                                                    uint32_t checksum_alg, uint32_t num_partitions,
                                                    int32_t start_position, uint32_t sort_rows, uint64_t n_records,
@@ -560,7 +562,8 @@ int b2s_decompress_aggregate_rows_keys_dev(uint32_t dev_index, uint32_t codec, u
  * instead of fetching, verifying and decoding the .data ranges.  The object store stays the source of truth: an entry is
  * never the only copy, and a miss is served by the usual fetch.  An entry on another device of the process is a miss.
  *
- * Budget: per device, in bytes of cached records; 0 (the default) turns the cache off.  Stores evict least recently used
+ * Budget: per device, in bytes of cached records and of the row writers' record boundaries (8 per record); 0 (the
+ * default) turns the cache off.  Stores evict least recently used
  * entries that no read is using until the new entry fits; a read counts as a use.  Lowering a budget evicts down to it.
  * Device memory: when one of the library's own workspaces cannot grow, unreferenced entries of that device are evicted
  * and the allocation is retried once, so a generous budget does not make another call fail with B2S_E_NOMEM.
@@ -613,6 +616,91 @@ int b2s_exchange_read_sort_dev(uint32_t dev_index, int32_t shuffle_id, int32_t s
                                uint32_t record_bytes, uint32_t key_off, uint32_t key_len, uint8_t* dst_base,
                                uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records, int32_t* status,
                                int32_t* bad_slice);
+/* The row writers' cached forms: b2s_partition_compress_rows_{hash,range,round_robin}_packed, byte for byte (outputs,
+ * status and return value), that also keep the partitioned rows as the entry (shuffle_id, map_id), as
+ * b2s_partition_compress_cached_packed does, together with their record boundaries: every record's offset in the entry
+ * (device memory, 8 bytes per record, counted against the budget beside the records' bytes rounded up to 8) and each
+ * partition's first record index.  A read of such an entry marks its records from the boundaries, a thread per record,
+ * instead of walking the size chain (b2s_exchange_read_*_rows_keys_*).  b2s_exchange_lookup's len stays the bytes of records.  The entry
+ * is also served by b2s_exchange_read_packed.  cached NULL -> B2S_E_ARG; otherwise the argument errors of the uncached
+ * form, then the exchange cache's (B2S_E_CUDA without a usable device, B2S_E_NOT_INIT before b2s_init). */
+int b2s_partition_compress_rows_hash_cached_packed(int32_t shuffle_id, int64_t map_id, uint32_t codec, int32_t level,
+                                                   uint32_t codec_block_size, uint32_t checksum_alg,
+                                                   uint32_t num_partitions, uint64_t n_records,
+                                                   const uint8_t* rec_base, uint64_t rec_bytes,
+                                                   const uint32_t* rec_len, uint32_t n_keys, const uint32_t* key_type,
+                                                   const uint32_t* key_off, const uint32_t* key_len,
+                                                   const int32_t* key_null_field, uint8_t* dst_base, uint64_t dst_cap,
+                                                   uint64_t* dst_off, uint64_t* dst_len, uint64_t* dst_total,
+                                                   uint64_t* checksum_out, int32_t* status, int32_t* cached);
+int b2s_partition_compress_rows_range_cached_packed(int32_t shuffle_id, int64_t map_id, uint32_t codec, int32_t level,
+                                                    uint32_t codec_block_size, uint32_t checksum_alg,
+                                                    uint64_t n_records, const uint8_t* rec_base, uint64_t rec_bytes,
+                                                    const uint32_t* rec_len, uint32_t n_keys,
+                                                    const uint32_t* key_type, const uint32_t* key_off,
+                                                    const uint32_t* key_len, const int32_t* key_null_field,
+                                                    uint32_t n_bounds, const uint8_t* bound_base,
+                                                    uint64_t bound_bytes, const uint32_t* bound_len,
+                                                    uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_off,
+                                                    uint64_t* dst_len, uint64_t* dst_total, uint64_t* checksum_out,
+                                                    int32_t* status, int32_t* cached);
+int b2s_partition_compress_rows_round_robin_cached_packed(int32_t shuffle_id, int64_t map_id, uint32_t codec,
+                                                          int32_t level, uint32_t codec_block_size,
+                                                          uint32_t checksum_alg, uint32_t num_partitions,
+                                                          int32_t start_position, uint32_t sort_rows,
+                                                          uint64_t n_records, const uint8_t* rec_base,
+                                                          uint64_t rec_bytes, const uint32_t* rec_len,
+                                                          uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_off,
+                                                          uint64_t* dst_len, uint64_t* dst_total,
+                                                          uint64_t* checksum_out, int32_t* status, int32_t* cached);
+/* b2s_decompress_sort_rows_keys_* and b2s_decompress_aggregate_rows_keys_* over n sources of which some are served
+ * from the cache, with b2s_exchange_read_sort_packed's contract: source i is the cached range [start_reduce,
+ * end_reduce) of map_ids[i] when cached[i] != 0, fetched block i otherwise; source order is block order and the sort is
+ * stable; a cached source that is not resident sets status[i] = B2S_E_NOT_CACHED; cached sources are not
+ * checksum-verified; when any source fails nothing is sorted or written (*n_records = 0, and *n_groups = 0, the call
+ * returns 0).  Every row rule of the composite-key calls applies to cached sources too: a cached row too short for the
+ * read's key, null word or aggregate slot fails its source with B2S_E_CORRUPT, and b2s_last_error() names "cached source
+ * i" and the byte offset of its lowest bad record, as for a fetched block.  A cached range of a row writer's entry is
+ * framed from its stored record boundaries; one of an id-taking entry (b2s_partition_compress_cached_packed) is walked
+ * as a fetched block is.  With n_keys = 1 these serve the single-key calls' reads.  Errors -> B2S_E_ARG: those of the
+ * composite-key calls, and b2s_exchange_read_sort_packed's (NULL map_ids / cached / status, a bad reduce range). */
+int b2s_exchange_read_sort_rows_keys_packed(int32_t shuffle_id, int32_t start_reduce, int32_t end_reduce,
+                                            const int64_t* map_ids, const uint8_t* cached, uint32_t codec,
+                                            uint32_t checksum_alg, uint32_t n, const uint8_t* src_base,
+                                            const uint64_t* src_off, const uint64_t* src_len,
+                                            const uint32_t* slice_base, const uint64_t* slice_len,
+                                            const uint64_t* slice_checksum, uint32_t n_keys, const uint32_t* key_type,
+                                            const uint32_t* key_off, const uint32_t* key_len,
+                                            const int32_t* key_null_field, uint8_t* dst_base, uint64_t dst_cap,
+                                            uint64_t* dst_total, uint64_t* n_records, int32_t* status,
+                                            int32_t* bad_slice);
+/* same, with src_base / dst_base in device memory of dev_index (and the cache entries of that device) */
+int b2s_exchange_read_sort_rows_keys_dev(uint32_t dev_index, int32_t shuffle_id, int32_t start_reduce,
+                                         int32_t end_reduce, const int64_t* map_ids, const uint8_t* cached,
+                                         uint32_t codec, uint32_t checksum_alg, uint32_t n, const uint8_t* src_base,
+                                         const uint64_t* src_off, const uint64_t* src_len, const uint32_t* slice_base,
+                                         const uint64_t* slice_len, const uint64_t* slice_checksum, uint32_t n_keys,
+                                         const uint32_t* key_type, const uint32_t* key_off, const uint32_t* key_len,
+                                         const int32_t* key_null_field, uint8_t* dst_base, uint64_t dst_cap,
+                                         uint64_t* dst_total, uint64_t* n_records, int32_t* status,
+                                         int32_t* bad_slice);
+int b2s_exchange_read_aggregate_rows_keys_packed(
+    int32_t shuffle_id, int32_t start_reduce, int32_t end_reduce, const int64_t* map_ids, const uint8_t* cached,
+    uint32_t codec, uint32_t checksum_alg, uint32_t n, const uint8_t* src_base, const uint64_t* src_off,
+    const uint64_t* src_len, const uint32_t* slice_base, const uint64_t* slice_len, const uint64_t* slice_checksum,
+    uint32_t n_keys, const uint32_t* key_type, const uint32_t* key_off, const uint32_t* key_len,
+    const int32_t* key_null_field, uint32_t n_aggs, const uint32_t* agg_op, const uint32_t* agg_off,
+    const int32_t* agg_null_field, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records,
+    uint64_t* n_groups, int32_t* status, int32_t* bad_slice);
+/* same, with src_base / dst_base in device memory of dev_index (and the cache entries of that device) */
+int b2s_exchange_read_aggregate_rows_keys_dev(
+    uint32_t dev_index, int32_t shuffle_id, int32_t start_reduce, int32_t end_reduce, const int64_t* map_ids,
+    const uint8_t* cached, uint32_t codec, uint32_t checksum_alg, uint32_t n, const uint8_t* src_base,
+    const uint64_t* src_off, const uint64_t* src_len, const uint32_t* slice_base, const uint64_t* slice_len,
+    const uint64_t* slice_checksum, uint32_t n_keys, const uint32_t* key_type, const uint32_t* key_off,
+    const uint32_t* key_len, const int32_t* key_null_field, uint32_t n_aggs, const uint32_t* agg_op,
+    const uint32_t* agg_off, const int32_t* agg_null_field, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_total,
+    uint64_t* n_records, uint64_t* n_groups, int32_t* status, int32_t* bad_slice);
 /* removes the entry (shuffle_id, map_id) — map_id -1: every map output of the shuffle — on every device (the hook for
  * removeShuffle).  Returns the number of entries removed. */
 int b2s_exchange_remove(int32_t shuffle_id, int64_t map_id);

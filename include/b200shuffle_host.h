@@ -113,8 +113,9 @@ int b2sh_serialized_writer_create(b2sh_dispatcher* d, int32_t shuffle_id, int64_
 /* HashPartitioning of UnsafeRows (INTEGRATION.md §3j), set before the first insert: every later insert is one record as
  * UnsafeRowSerializer writes it ([int32 big-endian size][row]) and its partition_id is ignored; commit() makes one
  * b2s_partition_compress_rows_hash_packed call with these key columns, which computes Spark's reduce ids on the GPU.
- * The files are byte-identical to the ones the writer makes when fed the same rows with those ids.  In this mode the
- * writer never stores into the exchange cache, even when it is on: the cache's reads serve fixed-size records only. */
+ * The files are byte-identical to the ones the writer makes when fed the same rows with those ids.  With the exchange
+ * cache on, the call is b2s_partition_compress_rows_hash_cached_packed instead: the same files, and the partitioned rows
+ * stay in HBM with their record boundaries for the row reads below (INTEGRATION.md §3m). */
 int b2sh_serialized_writer_hash_rows(b2sh_serialized_writer* w, uint32_t n_keys, const uint32_t* key_type,
                                      const uint32_t* key_off, const uint32_t* key_len, const int32_t* key_null_field);
 /* RangePartitioning of UnsafeRows (INTEGRATION.md §3k), set before the first insert: every later insert is one record
@@ -122,7 +123,7 @@ int b2sh_serialized_writer_hash_rows(b2sh_serialized_writer* w, uint32_t n_keys,
  * b2s_partition_compress_rows_range_packed call with these key columns and the n_bounds bound rows (framed the same
  * way, back to back in bound_base, bound_len[j] each; copied), which computes Spark's RangePartitioner ids on the GPU.
  * n_bounds + 1 must be the writer's num_partitions.  The files are byte-identical to the ones the writer makes when fed
- * the same rows with those ids.  In this mode the writer never stores into the exchange cache, as for hash_rows. */
+ * the same rows with those ids.  With the exchange cache on, the call is its cached form, as for hash_rows. */
 int b2sh_serialized_writer_range_rows(b2sh_serialized_writer* w, uint32_t n_keys, const uint32_t* key_type,
                                       const uint32_t* key_off, const uint32_t* key_len, const int32_t* key_null_field,
                                       uint32_t n_bounds, const uint8_t* bound_base, uint64_t bound_bytes,
@@ -132,7 +133,7 @@ int b2sh_serialized_writer_range_rows(b2sh_serialized_writer* w, uint32_t n_keys
  * b2s_partition_compress_rows_round_robin_packed call with start_position (Spark's XORShiftRandom(partitionId)
  * .nextInt(num_partitions)) and sort_rows (spark.sql.execution.sortBeforeRepartition).  num_partitions must be the
  * writer's numPartitions.  The files are byte-identical to the ones the writer makes when fed the same rows in Spark's
- * order with Spark's ids.  In this mode the writer never stores into the exchange cache, as for hash_rows. */
+ * order with Spark's ids.  With the exchange cache on, the call is its cached form, as for hash_rows. */
 int b2sh_serialized_writer_round_robin_rows(b2sh_serialized_writer* w, uint32_t num_partitions, int32_t start_position,
                                             uint32_t sort_rows);
 int b2sh_serialized_writer_insert(b2sh_serialized_writer* w, int32_t partition_id, const uint8_t* bytes, uint64_t len);
@@ -176,8 +177,9 @@ int b2sh_reader_read_sorted(b2sh_reader* r, uint32_t record_bytes, uint32_t key_
  * ([int32 big-endian size][row]) sorted by the key key_type (B2S_KEY_*) at row offset key_off, nulls first (null_field:
  * the key's null bit, -1 = none), stable in map, then reduce-id order.  The buffer stays valid until the reader's next
  * read or its destruction.  A checksum mismatch returns B2SH_E_SPARK with the reference's message, a malformed row
- * stream B2SH_E_IO.  Codec "none" is verified and sorted only.  The exchange cache is not consulted: every block is
- * fetched. */
+ * stream B2SH_E_IO.  Codec "none" is verified and sorted only.  With the exchange cache on, the maps resident on this
+ * thread's device are cached sources as in read_sorted() (b2s_exchange_read_sort_rows_keys_packed with one key column;
+ * maps evicted after the lookup are fetched and the call repeated), and only the others are fetched. */
 int b2sh_reader_read_sorted_rows(b2sh_reader* r, uint32_t key_type, uint32_t key_off, uint32_t key_len,
                                  int32_t null_field, const uint8_t** data, uint64_t* len, uint64_t* n_records);
 /* read_aggregated_rows(): read() for a Spark SQL exchange whose reducer merges partial aggregates by one typed key
@@ -186,7 +188,8 @@ int b2sh_reader_read_sorted_rows(b2sh_reader* r, uint32_t key_type, uint32_t key
  * agg_off / agg_null_field as there, the Decimal ops included): *data / *len receive one UnsafeRowSerializer record
  * per key, in the row sort's order, *n_records the input records and *n_groups the output records.  The buffer stays valid until the reader's next
  * read or its destruction.  A checksum mismatch returns B2SH_E_SPARK with the reference's message, a malformed row
- * stream B2SH_E_IO.  The exchange cache is not consulted: every block is fetched. */
+ * stream B2SH_E_IO.  The exchange cache is consulted as in read_sorted_rows() (b2s_exchange_read_aggregate_rows_keys_packed
+ * with one key column). */
 int b2sh_reader_read_aggregated_rows(b2sh_reader* r, uint32_t key_type, uint32_t key_off, uint32_t key_len,
                                      int32_t null_field, uint32_t n_aggs, const uint32_t* agg_op,
                                      const uint32_t* agg_off, const int32_t* agg_null_field, const uint8_t** data,
@@ -194,7 +197,8 @@ int b2sh_reader_read_aggregated_rows(b2sh_reader* r, uint32_t key_type, uint32_t
 /* read_sorted_rows_keys() / read_aggregated_rows_keys(): read_sorted_rows() / read_aggregated_rows() by a composite
  * key of n_keys (1..16) columns, strings included (key_type / key_off / key_len / key_null_field as in
  * b2s_decompress_sort_rows_keys_packed): ONE b2s_decompress_sort_rows_keys_packed or
- * b2s_decompress_aggregate_rows_keys_packed call, with the same buffer lifetime and error mapping. */
+ * b2s_decompress_aggregate_rows_keys_packed call (their b2s_exchange_read_* forms when maps are resident in the exchange
+ * cache), with the same buffer lifetime and error mapping. */
 int b2sh_reader_read_sorted_rows_keys(b2sh_reader* r, uint32_t n_keys, const uint32_t* key_type,
                                       const uint32_t* key_off, const uint32_t* key_len, const int32_t* key_null_field,
                                       const uint8_t** data, uint64_t* len, uint64_t* n_records);

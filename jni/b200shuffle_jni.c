@@ -13,6 +13,8 @@
  *                                          their sort-key columns and the partitioner's bound rows in
  *   partitionCompressRowsRoundRobinPacked  the same for a RoundRobinPartitioning exchange (INTEGRATION.md §3l): rows,
  *                                          the task's start position and sortBeforeRepartition in
+ *   partitionCompressRows*CachedPacked     the three row writers keeping their map output in the exchange cache
+ *                                          (INTEGRATION.md §3m); exchangeRead{Sort,Aggregate}RowsKeysPacked read it
  *   decompressPacked / decompressedSize    storage/S3ShuffleReader.scala:98-110 (the codec seam, batched drain of
  *                                          storage/S3BufferedPrefetchIterator.scala:196-212)
  *   checksumPacked                         shuffle/S3SingleSpillShuffleMapOutputWriter.scala:54-63,
@@ -157,7 +159,7 @@ typedef struct {
 } range_bounds;
 
 /* cached (may be NULL): int[1], the cached store's flag; then (shuffleId, mapId) keys the exchange-cache entry.
- * hash (may be NULL, then cached is NULL): the records are serialized rows whose reduce ids are computed on the GPU
+ * hash (may be NULL): the records are serialized rows whose reduce ids are computed on the GPU
  * from these key columns, recPart is not read: Spark's HashPartitioning ids (partitionCompressRowsHashPacked), or with
  * range its RangePartitioner ids over those bounds (partitionCompressRowsRangePacked; numPartitions = range->n + 1).
  * rr (may be NULL; then hash is NULL): {startPosition, sortRows}, the records are serialized rows dealt out in Spark's
@@ -197,15 +199,31 @@ static jint partition_compress(JNIEnv* e, jint shuffleId, jlong mapId, jintArray
   uint64_t total = 0;
   int32_t stored = 0;
   const int rc =
-      rr ? b2s_partition_compress_rows_round_robin_packed(
+      rr && cached ? b2s_partition_compress_rows_round_robin_cached_packed(
+               (int32_t)shuffleId, (int64_t)mapId, (uint32_t)codec, (int32_t)level, (uint32_t)blockSize, (uint32_t)alg,
+               (uint32_t)numPartitions, rr[0], (uint32_t)rr[1], (uint64_t)nRecords, PTR(const uint8_t, records),
+               (uint64_t)recBytes, PTR(const uint32_t, recLen), PTR(uint8_t, dst), (uint64_t)dstCap, buf, buf + R,
+               &total, buf + 2 * R, st, &stored)
+      : rr ? b2s_partition_compress_rows_round_robin_packed(
                (uint32_t)codec, (int32_t)level, (uint32_t)blockSize, (uint32_t)alg, (uint32_t)numPartitions, rr[0],
                (uint32_t)rr[1], (uint64_t)nRecords, PTR(const uint8_t, records), (uint64_t)recBytes,
                PTR(const uint32_t, recLen), PTR(uint8_t, dst), (uint64_t)dstCap, buf, buf + R, &total, buf + 2 * R, st)
+      : range && cached ? b2s_partition_compress_rows_range_cached_packed(
+                  (int32_t)shuffleId, (int64_t)mapId, (uint32_t)codec, (int32_t)level, (uint32_t)blockSize,
+                  (uint32_t)alg, (uint64_t)nRecords, PTR(const uint8_t, records), (uint64_t)recBytes,
+                  PTR(const uint32_t, recLen), (uint32_t)hash->n, kt, ko, kl, knf, (uint32_t)range->n,
+                  PTR(const uint8_t, range->rows), (uint64_t)range->bytes, bl, PTR(uint8_t, dst), (uint64_t)dstCap,
+                  buf, buf + R, &total, buf + 2 * R, st, &stored)
       : range ? b2s_partition_compress_rows_range_packed(
                   (uint32_t)codec, (int32_t)level, (uint32_t)blockSize, (uint32_t)alg, (uint64_t)nRecords,
                   PTR(const uint8_t, records), (uint64_t)recBytes, PTR(const uint32_t, recLen), (uint32_t)hash->n, kt,
                   ko, kl, knf, (uint32_t)range->n, PTR(const uint8_t, range->rows), (uint64_t)range->bytes, bl,
                   PTR(uint8_t, dst), (uint64_t)dstCap, buf, buf + R, &total, buf + 2 * R, st)
+      : hash && cached ? b2s_partition_compress_rows_hash_cached_packed(
+                 (int32_t)shuffleId, (int64_t)mapId, (uint32_t)codec, (int32_t)level, (uint32_t)blockSize,
+                 (uint32_t)alg, (uint32_t)numPartitions, (uint64_t)nRecords, PTR(const uint8_t, records),
+                 (uint64_t)recBytes, PTR(const uint32_t, recLen), (uint32_t)hash->n, kt, ko, kl, knf, PTR(uint8_t, dst),
+                 (uint64_t)dstCap, buf, buf + R, &total, buf + 2 * R, st, &stored)
       : hash ? b2s_partition_compress_rows_hash_packed(
                  (uint32_t)codec, (int32_t)level, (uint32_t)blockSize, (uint32_t)alg, (uint32_t)numPartitions,
                  (uint64_t)nRecords, PTR(const uint8_t, records), (uint64_t)recBytes, PTR(const uint32_t, recLen),
@@ -297,6 +315,58 @@ JNIEXPORT jint JNICALL J(partitionCompressRowsRoundRobinPacked)(JNIEnv* e, jclas
   return partition_compress(e, 0, 0, 0, 0, 0, rr, codec, level, blockSize, alg, numPartitions, nRecords, records,
                             recBytes, recLen, 0, dst, dstCap, dstOff, dstLen, meta, checksums, status);
 }
+/* the row writers' cached forms (INTEGRATION.md §3m): their arguments behind (shuffleId, mapId), and cached: int[1] =
+ * stored; the entry keeps every record's offset, so a reducer's read marks its rows instead of walking them */
+JNIEXPORT jint JNICALL J(partitionCompressRowsHashCachedPacked)(JNIEnv* e, jclass c, jint shuffleId, jlong mapId,
+                                                                jint codec, jint level, jint blockSize, jint alg,
+                                                                jint numPartitions, jlong nRecords, jlong records,
+                                                                jlong recBytes, jlong recLen, jint nKeys,
+                                                                jintArray keyType, jintArray keyOff, jintArray keyLen,
+                                                                jintArray keyNullField, jlong dst, jlong dstCap,
+                                                                jlongArray dstOff, jlongArray dstLen, jlongArray meta,
+                                                                jlongArray checksums, jintArray status,
+                                                                jintArray cached) {
+  (void)c;
+  if (!cached) return B2S_E_ARG;
+  const composite_key keys = {nKeys, keyType, keyOff, keyLen, keyNullField};
+  return partition_compress(e, shuffleId, mapId, cached, &keys, 0, 0, codec, level, blockSize, alg, numPartitions,
+                            nRecords, records, recBytes, recLen, 0, dst, dstCap, dstOff, dstLen, meta, checksums,
+                            status);
+}
+JNIEXPORT jint JNICALL J(partitionCompressRowsRangeCachedPacked)(JNIEnv* e, jclass c, jint shuffleId, jlong mapId,
+                                                                 jint codec, jint level, jint blockSize, jint alg,
+                                                                 jlong nRecords, jlong records, jlong recBytes,
+                                                                 jlong recLen, jint nKeys, jintArray keyType,
+                                                                 jintArray keyOff, jintArray keyLen,
+                                                                 jintArray keyNullField, jint nBounds, jlong bounds,
+                                                                 jlong boundBytes, jintArray boundLen, jlong dst,
+                                                                 jlong dstCap, jlongArray dstOff, jlongArray dstLen,
+                                                                 jlongArray meta, jlongArray checksums,
+                                                                 jintArray status, jintArray cached) {
+  (void)c;
+  if (!cached || nBounds < 0 || nBounds > (1 << 24) - 1) return B2S_E_ARG;
+  const composite_key keys = {nKeys, keyType, keyOff, keyLen, keyNullField};
+  const range_bounds range = {nBounds, bounds, boundBytes, boundLen};
+  return partition_compress(e, shuffleId, mapId, cached, &keys, &range, 0, codec, level, blockSize, alg, nBounds + 1,
+                            nRecords, records, recBytes, recLen, 0, dst, dstCap, dstOff, dstLen, meta, checksums,
+                            status);
+}
+JNIEXPORT jint JNICALL J(partitionCompressRowsRoundRobinCachedPacked)(JNIEnv* e, jclass c, jint shuffleId,
+                                                                      jlong mapId, jint codec, jint level,
+                                                                      jint blockSize, jint alg, jint numPartitions,
+                                                                      jint startPosition, jint sortRows,
+                                                                      jlong nRecords, jlong records, jlong recBytes,
+                                                                      jlong recLen, jlong dst, jlong dstCap,
+                                                                      jlongArray dstOff, jlongArray dstLen,
+                                                                      jlongArray meta, jlongArray checksums,
+                                                                      jintArray status, jintArray cached) {
+  (void)c;
+  if (!cached) return B2S_E_ARG;
+  const jint rr[2] = {startPosition, sortRows};
+  return partition_compress(e, shuffleId, mapId, cached, 0, 0, rr, codec, level, blockSize, alg, numPartitions,
+                            nRecords, records, recBytes, recLen, 0, dst, dstCap, dstOff, dstLen, meta, checksums,
+                            status);
+}
 /* the same, keeping the partitioned records in the exchange cache as (shuffleId, mapId); cached: int[1] = stored */
 JNIEXPORT jint JNICALL J(partitionCompressCachedPacked)(JNIEnv* e, jclass c, jint shuffleId, jlong mapId, jint codec,
                                                         jint level, jint blockSize, jint alg, jint numPartitions,
@@ -351,7 +421,7 @@ JNIEXPORT jint JNICALL J(decompressPacked)(JNIEnv* e, jclass c, jint codec, jint
  *      meta: long[2] = {dst_total, n_records}; status, badSlice: int[n].  All arrays go through native copies, so no
  *      Java array is held in a critical region while the GPU works. ---- */
 /* mapIds (NULL: a plain decompressSortPacked): long[n] and cached: int[n] make it an exchange-cache read of the
- * partitions [startReduce, endReduce) of shuffleId.  rows: a row sort (decompressSortRowsPacked) of UnsafeRow records
+ * partitions [startReduce, endReduce) of shuffleId (with keys: exchangeRead{Sort,Aggregate}RowsKeysPacked).  rows: a row sort (decompressSortRowsPacked) of UnsafeRow records
  * by the key keyType at keyOff (recordBytes unused, mapIds NULL).  aggOp (rows only; NULL otherwise): a row
  * aggregation (decompressAggregateRowsPacked) with int[nAggs] aggOp / aggOff / aggNullField, and meta long[3] =
  * {dst_total, n_records, n_groups}.  keys (rows only; NULL: the one key keyType / keyOff / keyLen / nullField): a
@@ -424,7 +494,13 @@ static jint sort_packed(JNIEnv* e, jint shuffleId, jint startReduce, jint endRed
         (*e)->GetIntArrayRegion(e, aggOff, 0, nAggs, (jint*)aoff);
         (*e)->GetIntArrayRegion(e, aggNullField, 0, nAggs, (jint*)anf);
       }
-      if (keys)
+      if (keys && mapIds)
+        rc = b2s_exchange_read_aggregate_rows_keys_packed(
+            (int32_t)shuffleId, (int32_t)startReduce, (int32_t)endReduce, ids, hit, (uint32_t)codec, (uint32_t)alg,
+            (uint32_t)n, PTR(const uint8_t, src), blk, blk + N, with_slices ? sb : 0, with_slices ? sl : 0,
+            with_slices ? sl + ns : 0, (uint32_t)keys->n, kt, ko, kl, knf, (uint32_t)nAggs, aop, aoff, anf,
+            PTR(uint8_t, dst), (uint64_t)dstCap, &total, &nrec, &ngrp, st, st + N);
+      else if (keys)
         rc = b2s_decompress_aggregate_rows_keys_packed(
             (uint32_t)codec, (uint32_t)alg, (uint32_t)n, PTR(const uint8_t, src), blk, blk + N, with_slices ? sb : 0,
             with_slices ? sl : 0, with_slices ? sl + ns : 0, (uint32_t)keys->n, kt, ko, kl, knf, (uint32_t)nAggs, aop,
@@ -435,7 +511,13 @@ static jint sort_packed(JNIEnv* e, jint shuffleId, jint startReduce, jint endRed
             with_slices ? sl : 0, with_slices ? sl + ns : 0, (uint32_t)keyType, (uint32_t)keyOff, (uint32_t)keyLen,
             (int32_t)nullField, (uint32_t)nAggs, aop, aoff, anf, PTR(uint8_t, dst), (uint64_t)dstCap, &total, &nrec,
             &ngrp, st, st + N);
-    } else if (keys)
+    } else if (keys && mapIds)
+      rc = b2s_exchange_read_sort_rows_keys_packed(
+          (int32_t)shuffleId, (int32_t)startReduce, (int32_t)endReduce, ids, hit, (uint32_t)codec, (uint32_t)alg,
+          (uint32_t)n, PTR(const uint8_t, src), blk, blk + N, with_slices ? sb : 0, with_slices ? sl : 0,
+          with_slices ? sl + ns : 0, (uint32_t)keys->n, kt, ko, kl, knf, PTR(uint8_t, dst), (uint64_t)dstCap, &total,
+          &nrec, st, st + N);
+    else if (keys)
       rc = b2s_decompress_sort_rows_keys_packed((uint32_t)codec, (uint32_t)alg, (uint32_t)n, PTR(const uint8_t, src),
                                                 blk, blk + N, with_slices ? sb : 0, with_slices ? sl : 0,
                                                 with_slices ? sl + ns : 0, (uint32_t)keys->n, kt, ko, kl, knf,
@@ -618,6 +700,42 @@ JNIEXPORT jint JNICALL J(exchangeReadSortPacked)(JNIEnv* e, jclass c, jint shuff
   if (!mapIds) return B2S_E_ARG;
   return sort_packed(e, shuffleId, startReduce, endReduce, mapIds, cached, codec, alg, n, src, off, len, sliceBase,
                      sliceLen, sliceChecksum, recordBytes, 0, 0, keyOff, keyLen, -1, 0, 0, 0, 0, 0, dst, dstCap,
+                     meta, status, badSlice);
+}
+
+/* decompressSortRowsKeysPacked / decompressAggregateRowsKeysPacked over sources of which those with cached[i] != 0
+ * are the cached range of mapIds[i] (INTEGRATION.md §3m; mapIds: long[n], cached: int[n]) */
+JNIEXPORT jint JNICALL J(exchangeReadSortRowsKeysPacked)(JNIEnv* e, jclass c, jint shuffleId, jint startReduce,
+                                                         jint endReduce, jlongArray mapIds, jintArray cached,
+                                                         jint codec, jint alg, jint n, jlong src, jlongArray off,
+                                                         jlongArray len, jintArray sliceBase, jlongArray sliceLen,
+                                                         jlongArray sliceChecksum, jint nKeys, jintArray keyType,
+                                                         jintArray keyOff, jintArray keyLen, jintArray keyNullField,
+                                                         jlong dst, jlong dstCap, jlongArray meta, jintArray status,
+                                                         jintArray badSlice) {
+  (void)c;
+  if (!mapIds) return B2S_E_ARG;
+  const composite_key k = {nKeys, keyType, keyOff, keyLen, keyNullField};
+  return sort_packed(e, shuffleId, startReduce, endReduce, mapIds, cached, codec, alg, n, src, off, len, sliceBase,
+                     sliceLen, sliceChecksum, 0, 1, 0, 0, 0, -1, &k, 0, 0, 0, 0, dst, dstCap, meta, status,
+                     badSlice);
+}
+JNIEXPORT jint JNICALL J(exchangeReadAggregateRowsKeysPacked)(JNIEnv* e, jclass c, jint shuffleId,
+                                                              jint startReduce, jint endReduce, jlongArray mapIds,
+                                                              jintArray cached, jint codec, jint alg, jint n,
+                                                              jlong src, jlongArray off, jlongArray len,
+                                                              jintArray sliceBase, jlongArray sliceLen,
+                                                              jlongArray sliceChecksum, jint nKeys, jintArray keyType,
+                                                              jintArray keyOff, jintArray keyLen,
+                                                              jintArray keyNullField, jint nAggs, jintArray aggOp,
+                                                              jintArray aggOff, jintArray aggNullField, jlong dst,
+                                                              jlong dstCap, jlongArray meta, jintArray status,
+                                                              jintArray badSlice) {
+  (void)c;
+  if (!mapIds || !aggOp) return B2S_E_ARG;
+  const composite_key k = {nKeys, keyType, keyOff, keyLen, keyNullField};
+  return sort_packed(e, shuffleId, startReduce, endReduce, mapIds, cached, codec, alg, n, src, off, len, sliceBase,
+                     sliceLen, sliceChecksum, 0, 1, 0, 0, 0, -1, &k, nAggs, aggOp, aggOff, aggNullField, dst, dstCap,
                      meta, status, badSlice);
 }
 

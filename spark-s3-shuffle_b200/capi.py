@@ -140,6 +140,27 @@ PROTOTYPES = [
     ("b2s_exchange_read_sort_dev", C.c_int,
      [_u32, _i32, _i32, _i32, _vp, _vp, _u32, _u32, _u32, _vp, _u64p, _u64p, _u32p, _u64p, _u64p, _u32, _u32, _u32,
       _vp, _u64, _u64p, _u64p, _i32p, _i32p]),
+    ("b2s_partition_compress_rows_hash_cached_packed", C.c_int,
+     [_i32, C.c_int64, _u32, _i32, _u32, _u32, _u32, _u64, _u8p, _u64, _u32p, _u32, _u32p, _u32p, _u32p, _i32p, _u8p,
+      _u64, _u64p, _u64p, _u64p, _u64p, _i32p, _i32p]),
+    ("b2s_partition_compress_rows_range_cached_packed", C.c_int,
+     [_i32, C.c_int64, _u32, _i32, _u32, _u32, _u64, _u8p, _u64, _u32p, _u32, _u32p, _u32p, _u32p, _i32p, _u32, _u8p,
+      _u64, _u32p, _u8p, _u64, _u64p, _u64p, _u64p, _u64p, _i32p, _i32p]),
+    ("b2s_partition_compress_rows_round_robin_cached_packed", C.c_int,
+     [_i32, C.c_int64, _u32, _i32, _u32, _u32, _u32, _i32, _u32, _u64, _u8p, _u64, _u32p, _u8p, _u64, _u64p, _u64p,
+      _u64p, _u64p, _i32p, _i32p]),
+    ("b2s_exchange_read_sort_rows_keys_packed", C.c_int,
+     [_i32, _i32, _i32, _vp, _vp, _u32, _u32, _u32, _u8p, _u64p, _u64p, _u32p, _u64p, _u64p, _u32, _u32p, _u32p, _u32p,
+      _i32p, _u8p, _u64, _u64p, _u64p, _i32p, _i32p]),
+    ("b2s_exchange_read_sort_rows_keys_dev", C.c_int,
+     [_u32, _i32, _i32, _i32, _vp, _vp, _u32, _u32, _u32, _vp, _u64p, _u64p, _u32p, _u64p, _u64p, _u32, _u32p, _u32p,
+      _u32p, _i32p, _vp, _u64, _u64p, _u64p, _i32p, _i32p]),
+    ("b2s_exchange_read_aggregate_rows_keys_packed", C.c_int,
+     [_i32, _i32, _i32, _vp, _vp, _u32, _u32, _u32, _u8p, _u64p, _u64p, _u32p, _u64p, _u64p, _u32, _u32p, _u32p, _u32p,
+      _i32p, _u32, _u32p, _u32p, _i32p, _u8p, _u64, _u64p, _u64p, _u64p, _i32p, _i32p]),
+    ("b2s_exchange_read_aggregate_rows_keys_dev", C.c_int,
+     [_u32, _i32, _i32, _i32, _vp, _vp, _u32, _u32, _u32, _vp, _u64p, _u64p, _u32p, _u64p, _u64p, _u32, _u32p, _u32p,
+      _u32p, _i32p, _u32, _u32p, _u32p, _i32p, _vp, _u64, _u64p, _u64p, _u64p, _i32p, _i32p]),
     ("b2s_exchange_remove", C.c_int, [_i32, C.c_int64]),
     ("b2s_checksum_dev", C.c_int, [_u32, _u32, _u32, _vp, _u64p, _u64p, _u64p]),
     ("b2s_compress_dev", C.c_int,
@@ -731,7 +752,8 @@ def partition_compress_rows_round_robin_dev(codec, d_records, rec_bytes, d_rec_l
 # exchange cache: map outputs kept resident in HBM for reducers on the same device
 # ---------------------------------------------------------------------------------------------------------------
 def exchange_set_budget(nbytes, dev=0):
-    """per-device budget in bytes of cached records; 0 (the default) turns the cache off"""
+    """per-device budget in bytes of cached records and of the row entries' record boundaries (8 per record); 0 (the
+    default) turns the cache off"""
     _check(load().b2s_exchange_set_budget(dev, nbytes), "b2s_exchange_set_budget")
 
 
@@ -800,6 +822,96 @@ def exchange_read_sort_dev(shuffle_id, start_reduce, end_reduce, map_ids, cached
     return _sort_call("b2s_exchange_read_sort_dev", codec, d_src, off, length, d_dst, dst_cap,
                       (record_bytes, key_off, key_len), checksum_alg, (slice_base, slice_len, slice_checksum), dev,
                       lead=(shuffle_id, start_reduce, end_reduce, ids, cm), n=ids.size)
+
+
+def _rows_cached(symbol, shuffle_id, map_id, codec, level, block_size, checksum_alg, num_partitions, mid, records,
+                 rec_len, dst):
+    """One cached row store: symbol's arguments are shuffle_id, map_id, codec, level, block_size, checksum_alg, *mid
+    (the call's own, numpy arrays among them passed as pointers, with n_records, records and rec_len in their places
+    given as None), dst, dst_cap, the per-partition outputs, cached.
+    -> dict(dst_off, dst_len, total, checksums, status, cached)"""
+    records, dst = _as_u8(records), _as_u8(dst)
+    rec_len = np.ascontiguousarray(rec_len, dtype=np.uint32)
+    fill = iter((rec_len.size, records, records.size, rec_len))
+    mid = [next(fill) if a is None else a for a in mid]
+    dst_off, dst_len, cks, st = _partition_out(num_partitions)
+    total, cached = _u64(0), _i32(0)
+    _check(getattr(load(), symbol)(
+        shuffle_id, map_id, codec, level, block_size, checksum_alg, *map(_arg, mid), _ptr(dst), dst.size,
+        _ptr(dst_off), _ptr(dst_len), C.addressof(total), _ptr(cks), _ptr(st), C.addressof(cached)), symbol)
+    return dict(dst_off=dst_off, dst_len=dst_len, total=total.value, checksums=cks, status=st, cached=cached.value)
+
+
+def partition_compress_rows_hash_cached_packed(shuffle_id, map_id, codec, records, rec_len, keys, num_partitions, dst,
+                                               block_size=0, checksum_alg=CHECKSUM_NONE, level=0):
+    """partition_compress_rows_hash_packed that also keeps the partitioned rows and their record boundaries as the cache
+    entry (shuffle_id, map_id).  -> dict(dst_off, dst_len, total, checksums, status, cached)"""
+    return _rows_cached("b2s_partition_compress_rows_hash_cached_packed", shuffle_id, map_id, codec, level, block_size,
+                        checksum_alg, num_partitions,
+                        (num_partitions, None, None, None, None, *_key_arrays(keys)), records, rec_len, dst)
+
+
+def partition_compress_rows_range_cached_packed(shuffle_id, map_id, codec, records, rec_len, keys, bounds, dst,
+                                                block_size=0, checksum_alg=CHECKSUM_NONE, level=0):
+    """partition_compress_rows_range_packed that also keeps the partitioned rows and their record boundaries as the
+    cache entry (shuffle_id, map_id).  -> dict(dst_off, dst_len, total, checksums, status, cached)"""
+    nb, bb, bbytes, bl = _bound_arrays(bounds)
+    return _rows_cached("b2s_partition_compress_rows_range_cached_packed", shuffle_id, map_id, codec, level,
+                        block_size, checksum_alg, nb + 1,
+                        (None, None, None, None, *_key_arrays(keys), nb, bb, bbytes, bl), records, rec_len, dst)
+
+
+def partition_compress_rows_round_robin_cached_packed(shuffle_id, map_id, codec, records, rec_len, num_partitions,
+                                                      start_position, sort_rows, dst, block_size=0,
+                                                      checksum_alg=CHECKSUM_NONE, level=0):
+    """partition_compress_rows_round_robin_packed that also keeps the partitioned rows and their record boundaries as
+    the cache entry (shuffle_id, map_id).  -> dict(dst_off, dst_len, total, checksums, status, cached)"""
+    return _rows_cached("b2s_partition_compress_rows_round_robin_cached_packed", shuffle_id, map_id, codec, level,
+                        block_size, checksum_alg, num_partitions,
+                        (num_partitions, start_position, sort_rows, None, None, None, None), records, rec_len, dst)
+
+
+def exchange_read_sort_rows_keys_packed(shuffle_id, start_reduce, end_reduce, map_ids, cached, codec, src, off,
+                                        length, dst, keys, checksum_alg=CHECKSUM_NONE, slice_base=None,
+                                        slice_len=None, slice_checksum=None):
+    """decompress_sort_rows_keys_packed over sources of which those with cached[i] set are the cached range of
+    map_ids[i].  -> dict(total, n_records, status, bad_slice)"""
+    ids, cm = _exchange_sources(map_ids, cached)
+    return _sort_call("b2s_exchange_read_sort_rows_keys_packed", codec, src, off, length, dst, None, _key_arrays(keys),
+                      checksum_alg, (slice_base, slice_len, slice_checksum),
+                      lead=(shuffle_id, start_reduce, end_reduce, ids, cm), n=ids.size)
+
+
+def exchange_read_sort_rows_keys_dev(shuffle_id, start_reduce, end_reduce, map_ids, cached, codec, d_src, off, length,
+                                     d_dst, dst_cap, keys, checksum_alg=CHECKSUM_NONE, slice_base=None,
+                                     slice_len=None, slice_checksum=None, dev=0):
+    """exchange_read_sort_rows_keys_packed with the fetched blocks (d_src) and the output (d_dst) in device memory"""
+    ids, cm = _exchange_sources(map_ids, cached)
+    return _sort_call("b2s_exchange_read_sort_rows_keys_dev", codec, d_src, off, length, d_dst, dst_cap,
+                      _key_arrays(keys), checksum_alg, (slice_base, slice_len, slice_checksum), dev,
+                      lead=(shuffle_id, start_reduce, end_reduce, ids, cm), n=ids.size)
+
+
+def exchange_read_aggregate_rows_keys_packed(shuffle_id, start_reduce, end_reduce, map_ids, cached, codec, src, off,
+                                             length, dst, keys, aggs=(), checksum_alg=CHECKSUM_NONE, slice_base=None,
+                                             slice_len=None, slice_checksum=None):
+    """decompress_aggregate_rows_keys_packed over sources of which those with cached[i] set are the cached range of
+    map_ids[i].  -> dict(total, n_records, n_groups, status, bad_slice)"""
+    ids, cm = _exchange_sources(map_ids, cached)
+    return _sort_call("b2s_exchange_read_aggregate_rows_keys_packed", codec, src, off, length, dst, None,
+                      (*_key_arrays(keys), *_agg_arrays(aggs)), checksum_alg, (slice_base, slice_len, slice_checksum),
+                      lead=(shuffle_id, start_reduce, end_reduce, ids, cm), n=ids.size)
+
+
+def exchange_read_aggregate_rows_keys_dev(shuffle_id, start_reduce, end_reduce, map_ids, cached, codec, d_src, off,
+                                          length, d_dst, dst_cap, keys, aggs=(), checksum_alg=CHECKSUM_NONE,
+                                          slice_base=None, slice_len=None, slice_checksum=None, dev=0):
+    """exchange_read_aggregate_rows_keys_packed with the fetched blocks (d_src) and the output (d_dst) in device
+    memory"""
+    ids, cm = _exchange_sources(map_ids, cached)
+    return _sort_call("b2s_exchange_read_aggregate_rows_keys_dev", codec, d_src, off, length, d_dst, dst_cap,
+                      (*_key_arrays(keys), *_agg_arrays(aggs)), checksum_alg, (slice_base, slice_len, slice_checksum),
+                      dev, lead=(shuffle_id, start_reduce, end_reduce, ids, cm), n=ids.size)
 
 
 def exchange_remove(shuffle_id, map_id=-1):

@@ -1030,8 +1030,14 @@ struct ExEntry {
   int64_t map = 0;
   int ordinal = 0;  // CUDA device holding buf
   uint8_t* buf = nullptr;
-  uint64_t bytes = 0;
+  uint64_t bytes = 0;                // of records
   std::vector<uint64_t> part_start;  // R + 1 offsets of the partitions in buf
+  // Record boundaries (entries of the row writers; empty / nullptr for the id-taking store): every record's offset in
+  // buf, in order (device memory, in buf's allocation behind the records), and the R + 1 indices in rec_off of each
+  // partition's first record
+  const uint64_t* rec_off = nullptr;
+  std::vector<uint64_t> rec_start;
+  uint64_t charged = 0;  // what counts against the budget: the records' bytes (8-aligned with boundaries), 8 per boundary
   uint32_t refs = 0;
   uint64_t last_use = 0;
   bool linked = true;
@@ -1047,7 +1053,7 @@ ExCache g_ex;
 // unlinks e (caller holds g_ex.mtx); an unreferenced entry goes to `dead`, for the caller to free outside the lock
 void ex_unlink(ExEntry* e, std::vector<ExEntry*>& dead) {
   g_ex.by_key.erase({e->shuffle, e->map});
-  g_ex.used[e->ordinal] -= e->bytes;
+  g_ex.used[e->ordinal] -= e->charged;
   e->linked = false;
   if (!e->refs) dead.push_back(e);
 }
@@ -1074,7 +1080,7 @@ bool ex_make_room(int ordinal, uint64_t bytes, std::vector<ExEntry*>& dead, bool
   const uint64_t budget = g_ex.budget[ordinal];
   uint64_t idle = 0;
   for (auto& kv : g_ex.by_key)
-    if (kv.second->ordinal == ordinal && !kv.second->refs) idle += kv.second->bytes;
+    if (kv.second->ordinal == ordinal && !kv.second->refs) idle += kv.second->charged;
   const bool fits = bytes <= budget && g_ex.used[ordinal] - idle <= budget - bytes;
   if (!fits && !partial) return false;
   while (g_ex.used[ordinal] + bytes > budget) {
@@ -1141,20 +1147,44 @@ struct ExRefs {
     *len = e->part_start[(size_t)end] - e->part_start[(size_t)start];
     return e->buf + e->part_start[(size_t)start];
   }
+  // the record boundaries of partitions [start, end) of source i (false: its entry keeps none): *off = the first
+  // record's offset in rec_off's numbering (the entry's), *first = its offsets, *count = how many
+  bool bounds(uint32_t i, int32_t start, int32_t end, uint64_t* off, const uint64_t** first, uint64_t* count) const {
+    const ExEntry* e = entry[i];
+    if (e->rec_start.empty()) return false;
+    *off = e->part_start[(size_t)start];
+    *first = e->rec_off + e->rec_start[(size_t)start];
+    *count = e->rec_start[(size_t)end] - e->rec_start[(size_t)start];
+    return true;
+  }
+};
+
+// The record boundaries a row writer's store keeps (ex_store): its partition plan (launch_partition_order's, over n
+// records: sdst holds every record's offset in the partitioned arena, and the readback block, already read back, is
+// free to take rec_start), and pinned host memory for rec_start's readback (R + 1 u64)
+struct ExBounds {
+  const PartitionPlan* plan;
+  uint64_t n;
+  uint64_t* host;
+  uint64_t* launches;
 };
 
 // Keeps `bytes` of partitioned records at d_rec (device memory of the current device `ordinal`, stream st) as the
-// entry (shuffle, map): exact-size allocation, device-to-device copy.  Returns 1 when stored, 0 when it does not fit.
+// entry (shuffle, map): exact-size allocation, device-to-device copy.  rb (rows): the record boundaries too, their
+// offsets copied behind the records and rec_start computed from the sorted ids and read back, all before the one
+// synchronisation.  Returns 1 when stored, 0 when it does not fit.
 int ex_store(int ordinal, cudaStream_t st, int32_t shuffle, int64_t map, const uint8_t* d_rec, uint64_t bytes,
-             std::vector<uint64_t>&& part_start) {
+             std::vector<uint64_t>&& part_start, const ExBounds* rb = nullptr) {
+  // the charge is what the entry holds: the records, and for a row entry their 8-aligned size and the offsets
+  const uint64_t rec_sz = align_up(bytes, 8), n = rb ? rb->n : 0, charged = (n ? rec_sz : bytes) + 8 * n;
   std::vector<ExEntry*> dead;
   bool fits;
   {
     std::lock_guard<std::mutex> lk(g_ex.mtx);
     auto it = g_ex.by_key.find({shuffle, map});
     if (it != g_ex.by_key.end()) ex_unlink(it->second, dead);  // a stale output of this map is never served again
-    fits = g_ex.budget[ordinal] > 0 && ex_make_room(ordinal, bytes, dead);
-    if (fits) g_ex.used[ordinal] += bytes;  // reserved until the entry is linked
+    fits = g_ex.budget[ordinal] > 0 && ex_make_room(ordinal, charged, dead);
+    if (fits) g_ex.used[ordinal] += charged;  // reserved until the entry is linked
   }
   ex_free(dead);
   dead.clear();
@@ -1164,23 +1194,34 @@ int ex_store(int ordinal, cudaStream_t st, int32_t shuffle, int64_t map, const u
   e->map = map;
   e->ordinal = ordinal;
   e->bytes = bytes;
+  e->charged = charged;
+  const uint32_t R = (uint32_t)part_start.size() - 1;
   e->part_start = std::move(part_start);
+  if (rb) e->rec_start.assign((size_t)R + 1, 0);
   bool ok = true;
   if (bytes) {
-    ok = cudaMalloc(&e->buf, bytes) == cudaSuccess &&
-         cudaMemcpyAsync(e->buf, d_rec, bytes, cudaMemcpyDeviceToDevice, st) == cudaSuccess &&
-         cudaStreamSynchronize(st) == cudaSuccess;
+    ok = cudaMalloc(&e->buf, rec_sz + 8 * n) == cudaSuccess &&
+         cudaMemcpyAsync(e->buf, d_rec, bytes, cudaMemcpyDeviceToDevice, st) == cudaSuccess;
+    if (ok && n) {
+      e->rec_off = (const uint64_t*)(e->buf + rec_sz);
+      launch_partition_rec_start(*rb->plan, n, R, rb->plan->readback, st, rb->launches);
+      ok = cudaMemcpyAsync(e->buf + rec_sz, rb->plan->sdst, 8 * n, cudaMemcpyDeviceToDevice, st) == cudaSuccess &&
+           cudaMemcpyAsync(rb->host, rb->plan->readback, ((size_t)R + 1) * 8, cudaMemcpyDeviceToHost, st) ==
+               cudaSuccess;
+    }
+    ok = ok && cudaStreamSynchronize(st) == cudaSuccess && cudaGetLastError() == cudaSuccess;
     if (!ok) (void)cudaGetLastError();  // not stored; the call's own outputs are unaffected
+    if (ok && n) e->rec_start.assign(rb->host, rb->host + (size_t)R + 1);
   }
   {
     std::lock_guard<std::mutex> lk(g_ex.mtx);
-    g_ex.used[ordinal] -= bytes;
+    g_ex.used[ordinal] -= charged;
     if (!ok) {
       dead.push_back(e);
     } else {
       auto it = g_ex.by_key.find({shuffle, map});
       if (it != g_ex.by_key.end()) ex_unlink(it->second, dead);  // stored by another thread meanwhile
-      g_ex.used[ordinal] += bytes;
+      g_ex.used[ordinal] += charged;
       e->last_use = ++g_ex.tick;
       g_ex.by_key[{shuffle, map}] = e;
     }
@@ -1856,13 +1897,15 @@ static int round_robin_order(Slot& S, const RowIds& ids, uint64_t n, const uint8
 // partitioned records, which are in d_dst (codec NONE) or S.parena.  ids (d_part unused): the ids are computed from the
 // rows on the device (RowIds), between the offsets and the radix passes (marks F0 and F1 bracket that step: the hash
 // kernel, the range call's bound checks and id kernel, or the round-robin call's hash, sort and id kernel), and a bad
-// record or bound fails the call.
+// record or bound fails the call.  plan (optional, n > 0): receives the partition plan, whose arrays in S.pws outlive
+// the call until the slot's next use (compression does not touch them).
 static int partition_compress_run(Device* D, Slot& S, uint32_t codec, int32_t level, uint32_t bs, uint32_t alg,
                                   uint32_t R, uint64_t n, const uint8_t* d_rec, uint64_t rec_bytes,
                                   const uint32_t* d_len, const uint32_t* d_part, uint8_t* d_dst, uint64_t dst_cap,
                                   uint64_t* dst_off, uint64_t* dst_len, uint64_t* checksum_out, int32_t* status,
                                   uint64_t* arena_bytes, uint64_t* launches,
-                                  std::vector<uint64_t>* part_start = nullptr, const RowIds* ids = nullptr) {
+                                  std::vector<uint64_t>* part_start = nullptr, const RowIds* ids = nullptr,
+                                  PartitionPlan* plan = nullptr) {
   cudaStream_t st = S.st;
   std::vector<uint64_t> pstart(R), plen(R);
   const bool range = ids && ids->range;
@@ -1932,6 +1975,7 @@ static int partition_compress_run(Device* D, Slot& S, uint32_t codec, int32_t le
       plen[p] = next - pstart[p];
       next = pstart[p];
     }
+    if (plan) *plan = P;
   } else if (rec_bytes) {
     return fail(B2S_E_ARG, "rec_len sums to 0 bytes, rec_bytes is %s", std::to_string(rec_bytes).c_str());
   } else if (range && ids->n_bounds) {  // no records: the bounds are still checked, with a readback of their verdict
@@ -2133,9 +2177,10 @@ static int partition_compress_packed(uint32_t codec, int32_t level, uint32_t cod
   CU(S.mark(H1, st));
   std::vector<uint64_t> cks(num_partitions), part_start;
   uint64_t launches = 0, arena = 0;
+  PartitionPlan P;
   rc = partition_compress_run(D, S, codec, level, bs, checksum_alg, num_partitions, n_records, d_rec, rec_bytes, d_len,
                               d_part, (uint8_t*)S.dst.p, S.dst.cap, dst_off, dst_len, cks.data(), status, &arena,
-                              &launches, store ? &part_start : nullptr, ids);
+                              &launches, store ? &part_start : nullptr, ids, &P);
   if (rc) return rc;
   // the device arena is sized by the bound, so a short caller arena shows up here: copy what fits, flag the rest
   int result = 0;
@@ -2157,7 +2202,11 @@ static int partition_compress_packed(uint32_t codec, int32_t level, uint32_t cod
     // the partitioned records are still in this slot (the write lane is held): in front of compression, or the arena
     // itself for codec NONE
     const uint8_t* parts = (const uint8_t*)(codec == B2S_CODEC_NONE ? S.dst.p : S.parena.p);
-    *store->cached = ex_store(D->ordinal, st, store->shuffle, store->map, parts, rec_bytes, std::move(part_start));
+    // a row writer's entry keeps its record boundaries: the plan's offsets, also still in this slot (S.pws); S.hmeta
+    // (only grown) has held the partition step's readback of R + 2 words
+    ExBounds rb{&P, n_records, (uint64_t*)S.hmeta.p, &launches};
+    *store->cached = ex_store(D->ordinal, st, store->shuffle, store->map, parts, rec_bytes, std::move(part_start),
+                              ids ? &rb : nullptr);
   }
   const uint64_t h2d = rec_bytes + n_records * (ids ? 4 : 8) + (ids && ids->range ? ids->bound_bytes : 0);
   end_call(wt, launches, CallBytes{rec_bytes, arena, h2d, fit}, &S,
@@ -2688,6 +2737,44 @@ static int hash_args(uint32_t codec, uint32_t codec_block_size, uint32_t alg, ui
   return 0;
 }
 
+// A packed rows call's checks, then (store: a cached form) the exchange cache's, before its partition + compress step
+static int rows_packed(const ExStore* store, const RowIds& ids, int args_rc, uint32_t codec, int32_t level,
+                       uint32_t codec_block_size, uint32_t checksum_alg, uint32_t num_partitions, uint64_t n_records,
+                       const uint8_t* rec_base, uint64_t rec_bytes, const uint32_t* rec_len, uint8_t* dst_base,
+                       uint64_t dst_cap, uint64_t* dst_off, uint64_t* dst_len, uint64_t* dst_total,
+                       uint64_t* checksum_out, int32_t* status) {
+  if (args_rc) return args_rc;
+  if (store)
+    if (int rc = exchange_ready()) return rc;
+  return partition_compress_packed(codec, level, codec_block_size, checksum_alg, num_partitions, n_records, rec_base,
+                                   rec_bytes, rec_len, nullptr, dst_base, dst_cap, dst_off, dst_len, dst_total,
+                                   checksum_out, status, store, &ids);
+}
+
+// the outputs a cached store zeroes before its checks: *dst_total, and *cached (B2S_E_ARG when it is NULL)
+static int cached_args(uint64_t* dst_total, int32_t* cached) {
+  if (dst_total) *dst_total = 0;
+  if (!cached) return fail(B2S_E_ARG, "null argument%s");
+  *cached = 0;
+  return 0;
+}
+
+static int rows_hash_packed(const ExStore* store, uint32_t codec, int32_t level, uint32_t codec_block_size,
+                            uint32_t checksum_alg, uint32_t num_partitions, uint64_t n_records,
+                            const uint8_t* rec_base, uint64_t rec_bytes, const uint32_t* rec_len, uint32_t n_keys,
+                            const uint32_t* key_type, const uint32_t* key_off, const uint32_t* key_len,
+                            const int32_t* key_null_field, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_off,
+                            uint64_t* dst_len, uint64_t* dst_total, uint64_t* checksum_out, int32_t* status) {
+  if (dst_total) *dst_total = 0;
+  const RecordSpec spec = keys_spec(n_keys, key_type, key_off, key_len, key_null_field);
+  const RowIds ids{spec.keys};
+  return rows_packed(store, ids,
+                     hash_args(codec, codec_block_size, checksum_alg, num_partitions, n_records, rec_base, rec_bytes,
+                               rec_len, spec, dst_base, dst_off, dst_len, status),
+                     codec, level, codec_block_size, checksum_alg, num_partitions, n_records, rec_base, rec_bytes,
+                     rec_len, dst_base, dst_cap, dst_off, dst_len, dst_total, checksum_out, status);
+}
+
 int b2s_partition_compress_rows_hash_packed(uint32_t codec, int32_t level, uint32_t codec_block_size,
                                             uint32_t checksum_alg, uint32_t num_partitions, uint64_t n_records,
                                             const uint8_t* rec_base, uint64_t rec_bytes, const uint32_t* rec_len,
@@ -2695,15 +2782,25 @@ int b2s_partition_compress_rows_hash_packed(uint32_t codec, int32_t level, uint3
                                             const uint32_t* key_len, const int32_t* key_null_field, uint8_t* dst_base,
                                             uint64_t dst_cap, uint64_t* dst_off, uint64_t* dst_len,
                                             uint64_t* dst_total, uint64_t* checksum_out, int32_t* status) {
-  if (dst_total) *dst_total = 0;
-  const RecordSpec spec = keys_spec(n_keys, key_type, key_off, key_len, key_null_field);
-  const RowIds ids{spec.keys};
-  if (int rc = hash_args(codec, codec_block_size, checksum_alg, num_partitions, n_records, rec_base, rec_bytes, rec_len,
-                         spec, dst_base, dst_off, dst_len, status))
-    return rc;
-  return partition_compress_packed(codec, level, codec_block_size, checksum_alg, num_partitions, n_records, rec_base,
-                                   rec_bytes, rec_len, nullptr, dst_base, dst_cap, dst_off, dst_len, dst_total,
-                                   checksum_out, status, nullptr, &ids);
+  return rows_hash_packed(nullptr, codec, level, codec_block_size, checksum_alg, num_partitions, n_records, rec_base,
+                          rec_bytes, rec_len, n_keys, key_type, key_off, key_len, key_null_field, dst_base, dst_cap,
+                          dst_off, dst_len, dst_total, checksum_out, status);
+}
+
+int b2s_partition_compress_rows_hash_cached_packed(int32_t shuffle_id, int64_t map_id, uint32_t codec, int32_t level,
+                                                   uint32_t codec_block_size, uint32_t checksum_alg,
+                                                   uint32_t num_partitions, uint64_t n_records,
+                                                   const uint8_t* rec_base, uint64_t rec_bytes,
+                                                   const uint32_t* rec_len, uint32_t n_keys, const uint32_t* key_type,
+                                                   const uint32_t* key_off, const uint32_t* key_len,
+                                                   const int32_t* key_null_field, uint8_t* dst_base, uint64_t dst_cap,
+                                                   uint64_t* dst_off, uint64_t* dst_len, uint64_t* dst_total,
+                                                   uint64_t* checksum_out, int32_t* status, int32_t* cached) {
+  if (int rc = cached_args(dst_total, cached)) return rc;
+  const ExStore store{shuffle_id, map_id, cached};
+  return rows_hash_packed(&store, codec, level, codec_block_size, checksum_alg, num_partitions, n_records, rec_base,
+                          rec_bytes, rec_len, n_keys, key_type, key_off, key_len, key_null_field, dst_base, dst_cap,
+                          dst_off, dst_len, dst_total, checksum_out, status);
 }
 
 int b2s_partition_compress_rows_hash_dev(uint32_t dev_index, uint32_t codec, int32_t level, uint32_t codec_block_size,
@@ -2764,6 +2861,23 @@ static RowIds range_ids(const RecordSpec& spec, uint32_t n_bounds, const uint8_t
   return ids;
 }
 
+static int rows_range_packed(const ExStore* store, uint32_t codec, int32_t level, uint32_t codec_block_size,
+                             uint32_t checksum_alg, uint64_t n_records, const uint8_t* rec_base, uint64_t rec_bytes,
+                             const uint32_t* rec_len, uint32_t n_keys, const uint32_t* key_type,
+                             const uint32_t* key_off, const uint32_t* key_len, const int32_t* key_null_field,
+                             uint32_t n_bounds, const uint8_t* bound_base, uint64_t bound_bytes,
+                             const uint32_t* bound_len, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_off,
+                             uint64_t* dst_len, uint64_t* dst_total, uint64_t* checksum_out, int32_t* status) {
+  if (dst_total) *dst_total = 0;
+  const RecordSpec spec = keys_spec(n_keys, key_type, key_off, key_len, key_null_field);
+  const RowIds ids = range_ids(spec, n_bounds, bound_base, bound_bytes, bound_len);
+  return rows_packed(store, ids,
+                     range_args(codec, codec_block_size, checksum_alg, n_records, rec_base, rec_bytes, rec_len, spec,
+                                ids, dst_base, dst_off, dst_len, status),
+                     codec, level, codec_block_size, checksum_alg, n_bounds + 1, n_records, rec_base, rec_bytes,
+                     rec_len, dst_base, dst_cap, dst_off, dst_len, dst_total, checksum_out, status);
+}
+
 int b2s_partition_compress_rows_range_packed(uint32_t codec, int32_t level, uint32_t codec_block_size,
                                              uint32_t checksum_alg, uint64_t n_records, const uint8_t* rec_base,
                                              uint64_t rec_bytes, const uint32_t* rec_len, uint32_t n_keys,
@@ -2773,15 +2887,29 @@ int b2s_partition_compress_rows_range_packed(uint32_t codec, int32_t level, uint
                                              const uint32_t* bound_len, uint8_t* dst_base, uint64_t dst_cap,
                                              uint64_t* dst_off, uint64_t* dst_len, uint64_t* dst_total,
                                              uint64_t* checksum_out, int32_t* status) {
-  if (dst_total) *dst_total = 0;
-  const RecordSpec spec = keys_spec(n_keys, key_type, key_off, key_len, key_null_field);
-  const RowIds ids = range_ids(spec, n_bounds, bound_base, bound_bytes, bound_len);
-  if (int rc = range_args(codec, codec_block_size, checksum_alg, n_records, rec_base, rec_bytes, rec_len, spec, ids,
-                          dst_base, dst_off, dst_len, status))
-    return rc;
-  return partition_compress_packed(codec, level, codec_block_size, checksum_alg, n_bounds + 1, n_records, rec_base,
-                                   rec_bytes, rec_len, nullptr, dst_base, dst_cap, dst_off, dst_len, dst_total,
-                                   checksum_out, status, nullptr, &ids);
+  return rows_range_packed(nullptr, codec, level, codec_block_size, checksum_alg, n_records, rec_base, rec_bytes,
+                           rec_len, n_keys, key_type, key_off, key_len, key_null_field, n_bounds, bound_base,
+                           bound_bytes, bound_len, dst_base, dst_cap, dst_off, dst_len, dst_total, checksum_out,
+                           status);
+}
+
+int b2s_partition_compress_rows_range_cached_packed(int32_t shuffle_id, int64_t map_id, uint32_t codec, int32_t level,
+                                                    uint32_t codec_block_size, uint32_t checksum_alg,
+                                                    uint64_t n_records, const uint8_t* rec_base, uint64_t rec_bytes,
+                                                    const uint32_t* rec_len, uint32_t n_keys,
+                                                    const uint32_t* key_type, const uint32_t* key_off,
+                                                    const uint32_t* key_len, const int32_t* key_null_field,
+                                                    uint32_t n_bounds, const uint8_t* bound_base,
+                                                    uint64_t bound_bytes, const uint32_t* bound_len,
+                                                    uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_off,
+                                                    uint64_t* dst_len, uint64_t* dst_total, uint64_t* checksum_out,
+                                                    int32_t* status, int32_t* cached) {
+  if (int rc = cached_args(dst_total, cached)) return rc;
+  const ExStore store{shuffle_id, map_id, cached};
+  return rows_range_packed(&store, codec, level, codec_block_size, checksum_alg, n_records, rec_base, rec_bytes,
+                           rec_len, n_keys, key_type, key_off, key_len, key_null_field, n_bounds, bound_base,
+                           bound_bytes, bound_len, dst_base, dst_cap, dst_off, dst_len, dst_total, checksum_out,
+                           status);
 }
 
 int b2s_partition_compress_rows_range_dev(uint32_t dev_index, uint32_t codec, int32_t level, uint32_t codec_block_size,
@@ -2833,6 +2961,21 @@ static RowIds round_robin_ids(int32_t start, uint32_t sort) {
   return ids;
 }
 
+static int rows_round_robin_packed(const ExStore* store, uint32_t codec, int32_t level, uint32_t codec_block_size,
+                                   uint32_t checksum_alg, uint32_t num_partitions, int32_t start_position,
+                                   uint32_t sort_rows, uint64_t n_records, const uint8_t* rec_base, uint64_t rec_bytes,
+                                   const uint32_t* rec_len, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_off,
+                                   uint64_t* dst_len, uint64_t* dst_total, uint64_t* checksum_out, int32_t* status) {
+  if (dst_total) *dst_total = 0;
+  const RowIds ids = round_robin_ids(start_position, sort_rows);
+  return rows_packed(store, ids,
+                     round_robin_args(codec, codec_block_size, checksum_alg, num_partitions, start_position, sort_rows,
+                                      n_records, rec_base, rec_bytes, rec_len, ids, dst_base, dst_off, dst_len,
+                                      status),
+                     codec, level, codec_block_size, checksum_alg, num_partitions, n_records, rec_base, rec_bytes,
+                     rec_len, dst_base, dst_cap, dst_off, dst_len, dst_total, checksum_out, status);
+}
+
 int b2s_partition_compress_rows_round_robin_packed(uint32_t codec, int32_t level, uint32_t codec_block_size,
                                                    uint32_t checksum_alg, uint32_t num_partitions,
                                                    int32_t start_position, uint32_t sort_rows, uint64_t n_records,
@@ -2840,14 +2983,25 @@ int b2s_partition_compress_rows_round_robin_packed(uint32_t codec, int32_t level
                                                    const uint32_t* rec_len, uint8_t* dst_base, uint64_t dst_cap,
                                                    uint64_t* dst_off, uint64_t* dst_len, uint64_t* dst_total,
                                                    uint64_t* checksum_out, int32_t* status) {
-  if (dst_total) *dst_total = 0;
-  const RowIds ids = round_robin_ids(start_position, sort_rows);
-  if (int rc = round_robin_args(codec, codec_block_size, checksum_alg, num_partitions, start_position, sort_rows,
-                                n_records, rec_base, rec_bytes, rec_len, ids, dst_base, dst_off, dst_len, status))
-    return rc;
-  return partition_compress_packed(codec, level, codec_block_size, checksum_alg, num_partitions, n_records, rec_base,
-                                   rec_bytes, rec_len, nullptr, dst_base, dst_cap, dst_off, dst_len, dst_total,
-                                   checksum_out, status, nullptr, &ids);
+  return rows_round_robin_packed(nullptr, codec, level, codec_block_size, checksum_alg, num_partitions,
+                                 start_position, sort_rows, n_records, rec_base, rec_bytes, rec_len, dst_base, dst_cap,
+                                 dst_off, dst_len, dst_total, checksum_out, status);
+}
+
+int b2s_partition_compress_rows_round_robin_cached_packed(int32_t shuffle_id, int64_t map_id, uint32_t codec,
+                                                          int32_t level, uint32_t codec_block_size,
+                                                          uint32_t checksum_alg, uint32_t num_partitions,
+                                                          int32_t start_position, uint32_t sort_rows,
+                                                          uint64_t n_records, const uint8_t* rec_base,
+                                                          uint64_t rec_bytes, const uint32_t* rec_len,
+                                                          uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_off,
+                                                          uint64_t* dst_len, uint64_t* dst_total,
+                                                          uint64_t* checksum_out, int32_t* status, int32_t* cached) {
+  if (int rc = cached_args(dst_total, cached)) return rc;
+  const ExStore store{shuffle_id, map_id, cached};
+  return rows_round_robin_packed(&store, codec, level, codec_block_size, checksum_alg, num_partitions,
+                                 start_position, sort_rows, n_records, rec_base, rec_bytes, rec_len, dst_base, dst_cap,
+                                 dst_off, dst_len, dst_total, checksum_out, status);
 }
 
 int b2s_partition_compress_rows_round_robin_dev(uint32_t dev_index, uint32_t codec, int32_t level,
@@ -2881,13 +3035,18 @@ struct SortBufferTrim {
 };
 
 // A source of an exchange-cache sorted read (b2s_exchange_read_sort_*): a cached range (records on the device, held by
-// a reference for the call; status B2S_E_NOT_CACHED when it is not resident) or fetched block `block`.
+// a reference for the call; status B2S_E_NOT_CACHED when it is not resident) or fetched block `block`.  A cached range
+// of a row writer's entry has its record boundaries (marked): n_rec offsets at rec_off, numbered in the entry, whose
+// first record is at entry offset first_off.
 struct SortSource {
   bool cached = false;
   int32_t status = B2S_OK;
   const uint8_t* src = nullptr;
   uint64_t len = 0;
   uint32_t block = 0;
+  bool marked = false;
+  const uint64_t* rec_off = nullptr;
+  uint64_t first_off = 0, n_rec = 0;
 };
 
 // The end of an aggregation (b2s_decompress_aggregate_rows_*), from the sorted indices idx of the records: grouping,
@@ -3071,18 +3230,29 @@ static int decompress_sort_run(Device* D, Slot& S, uint32_t codec, uint32_t alg,
     min_key = std::max<uint64_t>(min_key, (uint64_t)ks.off[c] + ks.len[c]);
     if (ks.null_field[c] >= 0) min_null = std::max<uint64_t>(min_null, null_word(ks.null_field[c]) + 8);
   }
-  if ((rc = S.fws.ensure(rows_frame_ws_bytes(*total, n_src)))) return rc;
+  // a cached range with record boundaries is marked from them instead of walked (its walk is empty)
+  std::vector<uint64_t> walk(length);
+  std::vector<RowsMark> marks;
+  for (uint32_t i = 0; i < n_src; i++) {
+    if (!cached(i) || !(*mix)[i].marked) continue;
+    const SortSource& s = (*mix)[i];
+    walk[i] = 0;
+    marks.push_back(RowsMark{s.rec_off, place[i] - s.first_off, place[i],
+                             marks.empty() ? 0 : marks.back().first + marks.back().count, s.n_rec, i});
+  }
+  if ((rc = S.fws.ensure(rows_frame_ws_bytes(*total, n_src, (uint32_t)marks.size())))) return rc;
   uint8_t* fws = (uint8_t*)S.fws.p;
   CU(S.mark(P0, st));
   CU(S.mark(F0, st, *launches));
-  launch_rows_frame(arena, *total, place.data(), length.data(), n_src, min_key, min_null, agg_min_row(spec), fws, st,
-                    launches);
+  launch_rows_frame(arena, *total, place.data(), walk.data(), n_src, min_key, min_null, agg_min_row(spec), fws, st,
+                    launches, marks.data(), (uint32_t)marks.size());
   CU(S.mark(F1, st, *launches));
   std::vector<uint64_t> rb(n_src + 1);
   CU(cudaMemcpyAsync(rb.data(), rows_frame_readback(fws, *total, n_src), rows_frame_readback_bytes(n_src),
                      cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
   CU(cudaGetLastError());
+  for (const RowsMark& m : marks) rb[1 + m.range] = rows_mark_verdict(rb[1 + m.range]);
   // a source whose verdict (framing, or the key pass's string check) is not ~0 fails, the first one named
   auto take_verdicts = [&](const uint64_t* v) {
     for (uint32_t i = 0; i < n_src; i++) {
@@ -3286,8 +3456,12 @@ static int exchange_sort_sources(const ExRefs& refs, int32_t start_reduce, int32
   for (uint32_t i = 0; i < (uint32_t)M.src.size(); i++) {
     SortSource& s = M.src[i];
     if (!s.cached) continue;
-    if (refs.entry[i]) s.src = refs.range(i, start_reduce, end_reduce, &s.len);
-    else s.status = B2S_E_NOT_CACHED;
+    if (refs.entry[i]) {
+      s.src = refs.range(i, start_reduce, end_reduce, &s.len);
+      s.marked = refs.bounds(i, start_reduce, end_reduce, &s.first_off, &s.rec_off, &s.n_rec);
+    } else {
+      s.status = B2S_E_NOT_CACHED;
+    }
   }
   return 0;
 }
@@ -3389,18 +3563,20 @@ int b2s_decompress_sort_rows_packed(uint32_t codec, uint32_t checksum_alg, uint3
                    n_records, status, bad_slice);
 }
 
-// the row sort's call with the aggregates; *dst_total is 0 when a block failed (nothing is written)
+// the row sort's call with the aggregates; *dst_total is 0 when a block failed (nothing is written).  x: an exchange
+// read, as for sort_call
 static int aggregate_call(uint32_t dev_index, bool packed, uint32_t codec, uint32_t alg, uint32_t n,
                           const uint8_t* src_base, const uint64_t* src_off, const uint64_t* src_len,
                           const uint32_t* slice_base, const uint64_t* slice_len, const uint64_t* slice_checksum,
                           const RecordSpec& spec, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_total,
-                          uint64_t* n_records, uint64_t* n_groups, int32_t* status, int32_t* bad_slice) {
+                          uint64_t* n_records, uint64_t* n_groups, int32_t* status, int32_t* bad_slice,
+                          const ExchangeRead* x = nullptr) {
   if (!n_groups) {
     if (dst_total) *dst_total = 0;
     if (n_records) *n_records = 0;
     return fail(B2S_E_ARG, "null argument%s");
   }
-  const int rc = sort_call(dev_index, packed, nullptr, codec, alg, n, src_base, src_off, src_len, slice_base,
+  const int rc = sort_call(dev_index, packed, x, codec, alg, n, src_base, src_off, src_len, slice_base,
                            slice_len, slice_checksum, spec, dst_base, dst_cap, dst_total, n_records, status, bad_slice,
                            n_groups);
   if (!rc && !*n_records) *dst_total = 0;
@@ -3642,6 +3818,72 @@ int b2s_decompressed_size_batch(uint32_t codec, uint32_t n, const uint8_t* const
   if (n && (!src || !src_len || !out_len || !status)) return fail(B2S_E_ARG, "null argument%s");
   return decompress_host(codec, 0, n, src, src_len, nullptr, nullptr, nullptr, nullptr, 0, nullptr, nullptr, nullptr,
                          out_len, nullptr, status, nullptr, true);
+}
+
+// ------------------------------------------------------------------------------------------------------------
+// exchange cache, rows: the composite-key row sort and aggregation over cached and fetched sources
+// ------------------------------------------------------------------------------------------------------------
+int b2s_exchange_read_sort_rows_keys_packed(int32_t shuffle_id, int32_t start_reduce, int32_t end_reduce,
+                                            const int64_t* map_ids, const uint8_t* cached, uint32_t codec,
+                                            uint32_t checksum_alg, uint32_t n, const uint8_t* src_base,
+                                            const uint64_t* src_off, const uint64_t* src_len,
+                                            const uint32_t* slice_base, const uint64_t* slice_len,
+                                            const uint64_t* slice_checksum, uint32_t n_keys, const uint32_t* key_type,
+                                            const uint32_t* key_off, const uint32_t* key_len,
+                                            const int32_t* key_null_field, uint8_t* dst_base, uint64_t dst_cap,
+                                            uint64_t* dst_total, uint64_t* n_records, int32_t* status,
+                                            int32_t* bad_slice) {
+  const ExchangeRead x{shuffle_id, start_reduce, end_reduce, map_ids, cached};
+  return sort_call(t_device, true, &x, codec, checksum_alg, n, src_base, src_off, src_len, slice_base, slice_len,
+                   slice_checksum, keys_spec(n_keys, key_type, key_off, key_len, key_null_field), dst_base, dst_cap,
+                   dst_total, n_records, status, bad_slice);
+}
+
+int b2s_exchange_read_sort_rows_keys_dev(uint32_t dev_index, int32_t shuffle_id, int32_t start_reduce,
+                                         int32_t end_reduce, const int64_t* map_ids, const uint8_t* cached,
+                                         uint32_t codec, uint32_t checksum_alg, uint32_t n, const uint8_t* src_base,
+                                         const uint64_t* src_off, const uint64_t* src_len, const uint32_t* slice_base,
+                                         const uint64_t* slice_len, const uint64_t* slice_checksum, uint32_t n_keys,
+                                         const uint32_t* key_type, const uint32_t* key_off, const uint32_t* key_len,
+                                         const int32_t* key_null_field, uint8_t* dst_base, uint64_t dst_cap,
+                                         uint64_t* dst_total, uint64_t* n_records, int32_t* status,
+                                         int32_t* bad_slice) {
+  const ExchangeRead x{shuffle_id, start_reduce, end_reduce, map_ids, cached};
+  return sort_call(dev_index, false, &x, codec, checksum_alg, n, src_base, src_off, src_len, slice_base, slice_len,
+                   slice_checksum, keys_spec(n_keys, key_type, key_off, key_len, key_null_field), dst_base, dst_cap,
+                   dst_total, n_records, status, bad_slice);
+}
+
+int b2s_exchange_read_aggregate_rows_keys_packed(
+    int32_t shuffle_id, int32_t start_reduce, int32_t end_reduce, const int64_t* map_ids, const uint8_t* cached,
+    uint32_t codec, uint32_t checksum_alg, uint32_t n, const uint8_t* src_base, const uint64_t* src_off,
+    const uint64_t* src_len, const uint32_t* slice_base, const uint64_t* slice_len, const uint64_t* slice_checksum,
+    uint32_t n_keys, const uint32_t* key_type, const uint32_t* key_off, const uint32_t* key_len,
+    const int32_t* key_null_field, uint32_t n_aggs, const uint32_t* agg_op, const uint32_t* agg_off,
+    const int32_t* agg_null_field, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records,
+    uint64_t* n_groups, int32_t* status, int32_t* bad_slice) {
+  const ExchangeRead x{shuffle_id, start_reduce, end_reduce, map_ids, cached};
+  return aggregate_call(t_device, true, codec, checksum_alg, n, src_base, src_off, src_len, slice_base, slice_len,
+                        slice_checksum,
+                        with_aggregates(keys_spec(n_keys, key_type, key_off, key_len, key_null_field), n_aggs, agg_op,
+                                        agg_off, agg_null_field),
+                        dst_base, dst_cap, dst_total, n_records, n_groups, status, bad_slice, &x);
+}
+
+int b2s_exchange_read_aggregate_rows_keys_dev(
+    uint32_t dev_index, int32_t shuffle_id, int32_t start_reduce, int32_t end_reduce, const int64_t* map_ids,
+    const uint8_t* cached, uint32_t codec, uint32_t checksum_alg, uint32_t n, const uint8_t* src_base,
+    const uint64_t* src_off, const uint64_t* src_len, const uint32_t* slice_base, const uint64_t* slice_len,
+    const uint64_t* slice_checksum, uint32_t n_keys, const uint32_t* key_type, const uint32_t* key_off,
+    const uint32_t* key_len, const int32_t* key_null_field, uint32_t n_aggs, const uint32_t* agg_op,
+    const uint32_t* agg_off, const int32_t* agg_null_field, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_total,
+    uint64_t* n_records, uint64_t* n_groups, int32_t* status, int32_t* bad_slice) {
+  const ExchangeRead x{shuffle_id, start_reduce, end_reduce, map_ids, cached};
+  return aggregate_call(dev_index, false, codec, checksum_alg, n, src_base, src_off, src_len, slice_base, slice_len,
+                        slice_checksum,
+                        with_aggregates(keys_spec(n_keys, key_type, key_off, key_len, key_null_field), n_aggs, agg_op,
+                                        agg_off, agg_null_field),
+                        dst_base, dst_cap, dst_total, n_records, n_groups, status, bad_slice, &x);
 }
 
 }  // extern "C"

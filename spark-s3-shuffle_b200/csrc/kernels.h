@@ -166,6 +166,7 @@ struct PartitionPlan {
   uint64_t* readback = nullptr;
   size_t readback_bytes = 0;
   uint32_t* ids = nullptr;
+  const uint32_t* keys = nullptr;  // the sorted ids (nullptr: no radix pass, one partition)
 };
 // One stable LSD radix pass over n (key, record index) pairs (n < 2^32), digit (key >> shift) & (nd - 1), nd a power of
 // two <= 256: a per-tile histogram, one scan over the digit-major histogram, a stable scatter.  idx_in == nullptr: the
@@ -192,6 +193,10 @@ void launch_partition_order(const uint32_t* d_rec_len, const uint32_t* d_rec_par
 void launch_partition(const uint32_t* d_rec_len, const uint32_t* d_rec_part, uint64_t n, uint32_t num_partitions,
                       uint8_t* d_ws, PartitionPlan* plan, cudaStream_t st,
                       uint64_t* launches);
+// rec_start[p] (num_partitions + 1 u64, device memory) = the sorted index of partition p's first record, n past the
+// last record (an empty partition: the next non-empty one's first), from the sorted ids of launch_partition_order; n > 0
+void launch_partition_rec_start(const PartitionPlan& plan, uint64_t n, uint32_t num_partitions, uint64_t* rec_start,
+                                cudaStream_t st, uint64_t* launches);
 // copies the records into d_dst in sorted order (only once the readback has shown every id valid and the lengths sum
 // to the arena size)
 void launch_partition_gather(const uint8_t* rec_base, const uint32_t* d_rec_len, uint64_t n, const PartitionPlan& plan,
@@ -240,14 +245,30 @@ const uint32_t* launch_key_radix(const KeySortWs& w, uint64_t n, uint32_t key_by
 // decimal's slot does not name 1..16 bytes inside its row.
 constexpr uint64_t kRowsBadPrefix = 1, kRowsBadNegative = 2, kRowsBadPastEnd = 3, kRowsBadKey = 4, kRowsBadNull = 5,
                    kRowsBadAgg = 6, kRowsBadString = 7;
-size_t rows_frame_ws_bytes(uint64_t arena_bytes, uint32_t n_ranges);
+// Marked ranges (n_marks of them, h_marks in host memory): ranges whose record offsets are known, so they are not
+// walked (their h_len entries are 0) but marked, a thread per record.  Mark k covers count records: record j's start is
+// arena offset base + off[j] (mod 2^64); it is checked against min_key, min_null and min_agg only (its size prefix was
+// checked when the offsets were taken), and the verdict of its range (index `range`) is lowered to the lowest bad
+// record, offset-major: rows_mark_verdict turns it into the walk's form.  `first` numbers the marks' records in order
+// (a prefix sum of count).
+struct RowsMark {
+  const uint64_t* off;
+  uint64_t base;   // the range's arena offset minus the offset of its first record in off's numbering
+  uint64_t place;  // the range's arena offset
+  uint64_t first;
+  uint64_t count;
+  uint32_t range;
+};
+// a marked range's verdict as the readback brings it, re-packed into the walk's form (kRowsBad* << 61 | offset)
+inline uint64_t rows_mark_verdict(uint64_t v) { return v == ~0ull ? v : ((v & 7) << 61) | (v >> 3); }
+size_t rows_frame_ws_bytes(uint64_t arena_bytes, uint32_t n_ranges, uint32_t n_marks = 0);
 inline size_t rows_frame_readback_bytes(uint32_t n_ranges) { return ((size_t)n_ranges + 1) * 8; }
 uint64_t* rows_frame_readback(uint8_t* d_fws, uint64_t arena_bytes, uint32_t n_ranges);
 // the ranges' arena offsets on the device (ascending), as launch_rows_frame uploaded them
 const uint64_t* rows_frame_ranges(uint8_t* d_fws, uint64_t arena_bytes, uint32_t n_ranges);
 void launch_rows_frame(const uint8_t* arena, uint64_t arena_bytes, const uint64_t* h_off, const uint64_t* h_len,
                        uint32_t n_ranges, uint64_t min_key, uint64_t min_null, uint64_t min_agg, uint8_t* d_fws,
-                       cudaStream_t st, uint64_t* launches);
+                       cudaStream_t st, uint64_t* launches, const RowsMark* h_marks = nullptr, uint32_t n_marks = 0);
 // The sort key of a row: n columns compared left to right.  Column c: type[c] (low 8 bits: B2S_KEY_*, B2S_STRING_KEY or
 // B2S_DECIMAL_KEY; above them the order flags B2S_KEY_DESCENDING / B2S_KEY_NULLS_LAST) at row offset off[c], len[c]
 // bytes (a string or a decimal: its 8-byte slot, (offset << 32) | size), null bit null_field[c] (-1: never null).

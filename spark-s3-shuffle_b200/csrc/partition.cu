@@ -136,6 +136,21 @@ __global__ void __launch_bounds__(kPartThreads) part_bounds_kernel(const uint32_
   }
 }
 
+// rec_start[p] = sorted index of partition p's first record, or of the next non-empty partition's first (n past the
+// last one), p in [0, num_partitions]: the partition starting at sorted index j fills the entries from the previous
+// record's partition (exclusive) to its own.  keys == nullptr (no radix pass: one partition) reads every id as 0.
+__global__ void __launch_bounds__(kPartThreads) part_rec_start_kernel(const uint32_t* __restrict__ keys, uint64_t n,
+                                                                      uint32_t num_partitions,
+                                                                      uint64_t* __restrict__ rec_start) {
+  for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (uint64_t)gridDim.x * blockDim.x) {
+    const uint32_t p = keys ? keys[j] : 0;
+    const uint32_t from = j == 0 ? 0 : (keys ? keys[j - 1] : 0) + 1;
+    for (uint32_t q = from; q <= p; q++) rec_start[q] = j;
+    if (j == n - 1)
+      for (uint32_t q = p + 1; q <= num_partitions; q++) rec_start[q] = n;
+  }
+}
+
 // one lane copies n bytes: destination-aligned 16-byte stores, sources read as aligned 8-byte words (ld_span16)
 __device__ __forceinline__ void lane_copy(uint8_t* __restrict__ d, const uint8_t* __restrict__ s, uint32_t n) {
   uint64_t lo, hi;
@@ -303,6 +318,7 @@ void launch_partition_order(const uint32_t* d_rec_len, const uint32_t* d_rec_par
     shift += (int)pb;
   }
   plan->idx = idx;
+  plan->keys = keys;
   launch_sorted_offsets(idx, d_rec_len, n, plan->sdst, unused_total, ws, st, launches);
   part_bounds_kernel<<<grid_for(n), kPartThreads, 0, st>>>(keys, d_rec_part, n, num_partitions, plan->sdst, part_start);
   if (launches) *launches += 2;
@@ -312,6 +328,12 @@ void launch_sorted_offsets(const uint32_t* idx, const uint32_t* d_rec_len, uint6
                            uint64_t* scan_ws, cudaStream_t st, uint64_t* launches) {
   part_sorted_len_kernel<<<grid_for(n), kPartThreads, 0, st>>>(idx, d_rec_len, n, sdst);
   launch_exclusive_scan_u64(sdst, n, total, scan_ws, st, launches);
+  if (launches) *launches += 1;
+}
+
+void launch_partition_rec_start(const PartitionPlan& plan, uint64_t n, uint32_t num_partitions, uint64_t* rec_start,
+                                cudaStream_t st, uint64_t* launches) {
+  part_rec_start_kernel<<<grid_for(n), kPartThreads, 0, st>>>(plan.keys, n, num_partitions, rec_start);
   if (launches) *launches += 1;
 }
 

@@ -146,6 +146,31 @@ __global__ void __launch_bounds__(kFrameWarps * 32) rows_frame_kernel(
   }
 }
 
+// Marks the records of ranges whose offsets are known (kernels.h, RowsMark), a thread per record: t-th marked record ->
+// its mark by a binary search over the marks' first record numbers, its start from its stored offset, its size prefix
+// from the arena.  A record the read's checks reject lowers its range's verdict, offset-major ((offset << 3) | why, so
+// the lowest bad record wins; re-packed on the host); a good one sets its start bit.
+__global__ void __launch_bounds__(kRowThreads) rows_mark_kernel(const uint8_t* __restrict__ arena,
+                                                                const RowsMark* __restrict__ marks, uint32_t n_marks,
+                                                                uint64_t total, uint64_t min_key, uint64_t min_null,
+                                                                uint64_t min_agg, uint32_t* __restrict__ bitmap,
+                                                                uint64_t* __restrict__ verdict) {
+  for (uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (uint64_t)gridDim.x * blockDim.x) {
+    uint32_t lo = 0, hi = n_marks;
+    while (hi - lo > 1) {
+      const uint32_t mid = (lo + hi) / 2;
+      if (marks[mid].first <= t) lo = mid;
+      else hi = mid;
+    }
+    const RowsMark& m = marks[lo];
+    const uint64_t q = m.base + m.off[t - m.first];
+    const uint64_t s = __byte_perm(ld32u_ro(arena + q), 0, 0x0123);
+    const uint64_t why = s < min_key ? kRowsBadKey : s < min_null ? kRowsBadNull : s < min_agg ? kRowsBadAgg : 0;
+    if (why) atomicMin((unsigned long long*)(verdict + m.range), (unsigned long long)(((q - m.place) << 3) | why));
+    else atomicOr(bitmap + (q >> 5), 1u << (q & 31));
+  }
+}
+
 // exclusive scan of one u32 per thread over the CTA (kRowThreads threads)
 __device__ __forceinline__ uint32_t cta_exclusive_scan(uint32_t v) {
   __shared__ uint32_t warp_sums[kRowThreads / 32];
@@ -400,6 +425,7 @@ struct FrameWs {
   uint64_t* r_off;
   uint64_t* r_len;
   unsigned int* counter;
+  RowsMark* marks;
   uint64_t tiles;
 };
 
@@ -418,16 +444,18 @@ FrameWs carve_frame_ws(uint8_t* d_fws, uint64_t arena_bytes, uint32_t n_ranges) 
   f.readback = (uint64_t*)p; p += a256(rows_frame_readback_bytes(n_ranges));
   f.r_off = (uint64_t*)p;    p += a256((size_t)n_ranges * 8);
   f.r_len = (uint64_t*)p;    p += a256((size_t)n_ranges * 8);
-  f.counter = (unsigned int*)p;
+  f.counter = (unsigned int*)p; p += 256;
+  f.marks = (RowsMark*)p;
   return f;
 }
 
 }  // namespace
 
-size_t rows_frame_ws_bytes(uint64_t arena_bytes, uint32_t n_ranges) {
+size_t rows_frame_ws_bytes(uint64_t arena_bytes, uint32_t n_ranges, uint32_t n_marks) {
   const uint64_t tiles = frame_tiles(arena_bytes);
   return a256(tiles * kTileWords * 4) + a256(tiles * 8) + a256(scan_ws_elems(tiles) * 8) +
-         a256(rows_frame_readback_bytes(n_ranges)) + 2 * a256((size_t)n_ranges * 8) + 256;
+         a256(rows_frame_readback_bytes(n_ranges)) + 2 * a256((size_t)n_ranges * 8) + 256 +
+         a256((size_t)n_marks * sizeof(RowsMark));
 }
 
 uint64_t* rows_frame_readback(uint8_t* d_fws, uint64_t arena_bytes, uint32_t n_ranges) {
@@ -436,7 +464,7 @@ uint64_t* rows_frame_readback(uint8_t* d_fws, uint64_t arena_bytes, uint32_t n_r
 
 void launch_rows_frame(const uint8_t* arena, uint64_t arena_bytes, const uint64_t* h_off, const uint64_t* h_len,
                        uint32_t n_ranges, uint64_t min_key, uint64_t min_null, uint64_t min_agg, uint8_t* d_fws,
-                       cudaStream_t st, uint64_t* launches) {
+                       cudaStream_t st, uint64_t* launches, const RowsMark* h_marks, uint32_t n_marks) {
   const FrameWs f = carve_frame_ws(d_fws, arena_bytes, n_ranges);
   cudaMemsetAsync(f.bitmap, 0, f.tiles * kTileWords * 4, st);
   cudaMemsetAsync(f.readback, 0xff, rows_frame_readback_bytes(n_ranges), st);
@@ -452,6 +480,14 @@ void launch_rows_frame(const uint8_t* arena, uint64_t arena_bytes, const uint64_
     rows_frame_kernel<<<(unsigned)grid, kFrameWarps * 32, 0, st>>>(arena, f.r_off, f.r_len, n_ranges, min_key,
                                                                     min_null, min_agg, f.bitmap, f.readback + 1,
                                                                     f.counter);
+    if (launches) *launches += 1;
+  }
+  // after the walk, which writes every range's verdict (a marked range's walk is empty)
+  const uint64_t marked = n_marks ? h_marks[n_marks - 1].first + h_marks[n_marks - 1].count : 0;
+  if (marked) {
+    cudaMemcpyAsync(f.marks, h_marks, (size_t)n_marks * sizeof(RowsMark), cudaMemcpyHostToDevice, st);
+    rows_mark_kernel<<<grid_for(marked), kRowThreads, 0, st>>>(arena, f.marks, n_marks, marked, min_key, min_null,
+                                                               min_agg, f.bitmap, f.readback + 1);
     if (launches) *launches += 1;
   }
   rows_count_kernel<<<(unsigned)f.tiles, kRowThreads, 0, st>>>(f.bitmap, f.tile_cnt);

@@ -374,15 +374,15 @@ class S3ShuffleReader:
 
     def readSortedRows(self, keyType, keyOffset, keyLength, nullField=-1):
         """read() of a SQL exchange sorted by one typed key (spark.shuffle.s3.gpu.sortRows): every UnsafeRowSerializer
-        record of the task in ascending key order, nulls first, stable.  Fetched blocks only (no exchange cache).
-        -> (bytes, number of records)"""
+        record of the task in ascending key order, nulls first, stable.  With the exchange cache on, resident maps are
+        read from it.  -> (bytes, number of records)"""
         return _read_sorted(self._h, load().b2sh_reader_read_sorted_rows, keyType, keyOffset, keyLength, nullField)
 
     def readAggregatedRows(self, keyType, keyOffset, keyLength, nullField=-1, aggs=()):
         """read() of a SQL exchange whose partial aggregates are merged by one typed key
         (spark.shuffle.s3.gpu.aggregateRows): one UnsafeRowSerializer record per key, in the row sort's order, with
-        each aggregate (op, offset, null field) merged over the key's records.  Fetched blocks only (no exchange cache).
-        -> (bytes, number of input records, number of groups)"""
+        each aggregate (op, offset, null field) merged over the key's records.  With the exchange cache on, resident
+        maps are read from it.  -> (bytes, number of input records, number of groups)"""
         return _read_sorted(self._h, load().b2sh_reader_read_aggregated_rows, keyType, keyOffset, keyLength,
                             nullField, *_agg_arrays(aggs), groups=True)
 

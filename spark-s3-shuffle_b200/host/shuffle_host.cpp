@@ -564,28 +564,51 @@ class S3SerializedShuffleWriter {
     uint64_t total = 0;
     int rc;
     const char* call = "b2s_partition_compress_packed";
-    if (roundRobin_) {  // round-robin rows: never cached, as hashed ones
+    // With the exchange cache on, every form calls its cached one: the same outputs, and the partitioned records stay in
+    // HBM for local reducers (a row writer's with its record boundaries)
+    const bool cache = d_.gpuExchangeCacheBytes != 0;
+    if (cache) d_.applyExchangeBudget();
+    int32_t cached = 0;
+    if (roundRobin_ && cache) {
+      call = "b2s_partition_compress_rows_round_robin_cached_packed";
+      rc = b2s_partition_compress_rows_round_robin_cached_packed(
+          shuffleId_, mapId_, codec, d_.zstdLevel, d_.lz4BlockSize, alg, R, rrStart_, rrSort_, recLen_.size(),
+          records_.data(), records_.size(), recLen_.data(), out_.data(), bound, doff.data(), dlen.data(), &total,
+          cks.data(), status.data(), &cached);
+    } else if (roundRobin_) {
       call = "b2s_partition_compress_rows_round_robin_packed";
       rc = b2s_partition_compress_rows_round_robin_packed(
           codec, d_.zstdLevel, d_.lz4BlockSize, alg, R, rrStart_, rrSort_, recLen_.size(), records_.data(),
           records_.size(), recLen_.data(), out_.data(), bound, doff.data(), dlen.data(), &total, cks.data(),
           status.data());
-    } else if (range_) {  // range-partitioned rows: never cached, as hashed ones
+    } else if (range_ && cache) {
+      call = "b2s_partition_compress_rows_range_cached_packed";
+      rc = b2s_partition_compress_rows_range_cached_packed(
+          shuffleId_, mapId_, codec, d_.zstdLevel, d_.lz4BlockSize, alg, recLen_.size(), records_.data(),
+          records_.size(), recLen_.data(), (uint32_t)keyType_.size(), keyType_.data(), keyOff_.data(), keyLen_.data(),
+          keyNull_.data(), (uint32_t)boundLen_.size(), boundRows_.data(), boundRows_.size(), boundLen_.data(),
+          out_.data(), bound, doff.data(), dlen.data(), &total, cks.data(), status.data(), &cached);
+    } else if (range_) {
       call = "b2s_partition_compress_rows_range_packed";
       rc = b2s_partition_compress_rows_range_packed(
           codec, d_.zstdLevel, d_.lz4BlockSize, alg, recLen_.size(), records_.data(), records_.size(), recLen_.data(),
           (uint32_t)keyType_.size(), keyType_.data(), keyOff_.data(), keyLen_.data(), keyNull_.data(),
           (uint32_t)boundLen_.size(), boundRows_.data(), boundRows_.size(), boundLen_.data(), out_.data(), bound,
           doff.data(), dlen.data(), &total, cks.data(), status.data());
-    } else if (!keyType_.empty()) {  // hashed rows: never cached (the exchange cache's reads serve fixed-size records only)
+    } else if (!keyType_.empty() && cache) {
+      call = "b2s_partition_compress_rows_hash_cached_packed";
+      rc = b2s_partition_compress_rows_hash_cached_packed(
+          shuffleId_, mapId_, codec, d_.zstdLevel, d_.lz4BlockSize, alg, R, recLen_.size(), records_.data(),
+          records_.size(), recLen_.data(), (uint32_t)keyType_.size(), keyType_.data(), keyOff_.data(), keyLen_.data(),
+          keyNull_.data(), out_.data(), bound, doff.data(), dlen.data(), &total, cks.data(), status.data(), &cached);
+    } else if (!keyType_.empty()) {
       call = "b2s_partition_compress_rows_hash_packed";
       rc = b2s_partition_compress_rows_hash_packed(
           codec, d_.zstdLevel, d_.lz4BlockSize, alg, R, recLen_.size(), records_.data(), records_.size(),
           recLen_.data(), (uint32_t)keyType_.size(), keyType_.data(), keyOff_.data(), keyLen_.data(), keyNull_.data(),
           out_.data(), bound, doff.data(), dlen.data(), &total, cks.data(), status.data());
-    } else if (d_.gpuExchangeCacheBytes) {  // the same outputs, and the partitioned records stay in HBM for local reducers
-      d_.applyExchangeBudget();
-      int32_t cached = 0;
+    } else if (cache) {
+      call = "b2s_partition_compress_cached_packed";
       rc = b2s_partition_compress_cached_packed(shuffleId_, mapId_, codec, d_.zstdLevel, d_.lz4BlockSize, alg, R,
                                                 recLen_.size(), records_.data(), records_.size(), recLen_.data(),
                                                 recPart_.data(), out_.data(), bound, doff.data(), dlen.data(), &total,
@@ -830,14 +853,26 @@ class S3ShuffleReader {
 
   void open() { start(false); }
 
-  // read() for a shuffle with a key ordering whose records are recordBytes long and order by the unsigned bytes
-  // [keyOff, keyOff + keyLen) (INTEGRATION.md §3e): every non-empty block is fetched and staged, then ONE
-  // b2s_decompress_sort_packed call verifies, decodes and key-sorts all of the task's records.  The blocks go in
-  // computeShuffleBlocks order (map, then reduce id), so records with equal keys come out in that order whatever the
-  // order the fetches completed in.  Codec NONE (spark.shuffle.compress=false) is verified and sorted only.  With the
-  // exchange cache on, a map resident on this thread's device is one cached source in that order instead of its blocks
-  // (b2s_exchange_read_sort_packed); maps the cache no longer holds when the call runs are fetched and the call repeated.
-  void readSorted(uint32_t recordBytes, uint32_t keyOff, uint32_t keyLen) {
+  // One sorted-read call's sources, as readSources stages them for `call`
+  struct Sources {
+    uint32_t codec, alg, n;
+    const int64_t* ids;      // the map of each source
+    const uint8_t* cached;   // 1: the source is that map's cached range
+    bool anyCached;          // false: every source is a fetched block (the plain calls apply)
+    StagedBlocks& src;       // the fetched blocks, a cached source staged as no bytes
+    const uint32_t* sb;      // their checksum slices (nullptr without checksums)
+    const uint64_t* sl;
+    const uint64_t* sc;
+    int32_t* status;
+    int32_t* bad;
+  };
+  // The body of readSorted and readRows: the task's blocks are fetched and staged in computeShuffleBlocks order (map,
+  // then reduce id), except that with the exchange cache on a map resident on this thread's device is one cached source
+  // in its place; then call(sources, cap, &total, &records, &groups, &name) runs the one read into sorted_ (cap bytes;
+  // a call that finds cap too small ends with the bytes needed in total and is run once more with exactly that).  Maps
+  // the cache no longer holds when the call runs (status B2S_E_NOT_CACHED) are fetched and the call repeated.
+  template <typename Call>
+  void readSources(Call&& call) {
     std::vector<uint8_t> fetch = cacheMisses();
     start(true, &fetch);
     std::vector<FetchedBlock> fetched;
@@ -867,35 +902,28 @@ class S3ShuffleReader {
       }
       const uint32_t n = (uint32_t)ids.size();
       StagedBlocks src(info_, from);
+      const bool anyCached = std::find(cached.begin(), cached.end(), 1) != cached.end();
       uint64_t cachedBytes = 0;
-      if (std::find(cached.begin(), cached.end(), 1) != cached.end()) {
+      if (anyCached) {
         std::vector<uint64_t> hitLen(n);
         lookup(n, ids.data(), hitLen.data());
         for (uint32_t k = 0; k < n; k++)
           if (cached[k] && hitLen[k] != UINT64_MAX) cachedBytes += hitLen[k];
       }
-      const uint32_t* sb = verify ? src.sliceBase.data() : nullptr;
-      const uint64_t* sl = verify ? src.sliceLen.data() : nullptr;
-      const uint64_t* sc = verify ? src.sliceSum.data() : nullptr;
       std::vector<int32_t> status(n), bad(n);
-      uint64_t total = 0, records = 0;
+      const Sources x{codec, alg, n, ids.data(), cached.data(), anyCached, src,
+                      verify ? src.sliceBase.data() : nullptr, verify ? src.sliceLen.data() : nullptr,
+                      verify ? src.sliceSum.data() : nullptr, status.data(), bad.data()};
+      uint64_t total = 0, records = 0, groups = 0;
+      const char* name = "";
       // Output size: codec NONE decodes to the stored bytes.  For a codec, a first guess of 4x the compressed bytes (the
       // pages of the untouched tail are never faulted in); a call it is too small for ends after verification with the
       // bytes needed in `total`, and the one retry uses exactly that.
       const uint64_t guess = (codec == B2S_CODEC_NONE ? src.bytes : src.bytes * 4) + cachedBytes;
-      const int rc = callWithRetry(sorted_, guess, total, [&](uint64_t cap) {
-        if (fetch == std::vector<uint8_t>(M, 1))
-          return b2s_decompress_sort_packed(codec, alg, n, src.src.data(), src.off.data(), src.len.data(), sb, sl, sc,
-                                            recordBytes, keyOff, keyLen, sorted_.get(), cap, &total, &records,
-                                            status.data(), bad.data());
-        return b2s_exchange_read_sort_packed(shuffleId_, start_, end_, ids.data(), cached.data(), codec, alg, n,
-                                             src.src.data(), src.off.data(), src.len.data(), sb, sl, sc, recordBytes,
-                                             keyOff, keyLen, sorted_.get(), cap, &total, &records, status.data(),
-                                             bad.data());
-      });
-      if (rc != 0)
-        throw CodecException(std::string("b2s_decompress_sort_packed: ") + b2s_strerror(rc) + ": " + b2s_last_error());
-      std::vector<uint8_t> late(M, 0);  // maps evicted between the lookup and the call: fetch them, then sort again
+      const int rc = callWithRetry(sorted_, guess, total,
+                                   [&](uint64_t cap) { return call(x, cap, &total, &records, &groups, &name); });
+      if (rc != 0) throw CodecException(std::string(name) + ": " + b2s_strerror(rc) + ": " + b2s_last_error());
+      std::vector<uint8_t> late(M, 0);  // maps evicted between the lookup and the call: fetch them, then read again
       for (uint32_t k = 0; k < n; k++)
         if (status[k] == B2S_E_NOT_CACHED) late[mapOf[k]] = fetch[mapOf[k]] = 1;
       if (std::find(late.begin(), late.end(), 1) != late.end()) {
@@ -909,8 +937,30 @@ class S3ShuffleReader {
         throwBlockStatus(status[k], cached[k] ? cachedBlockId(ids[k]) : info_[from[k]->first].id);
       sortedLen_ = total;
       sortedRecords_ = records;
+      sortedGroups_ = groups;
       return;
     }
+  }
+
+  // read() for a shuffle with a key ordering whose records are recordBytes long and order by the unsigned bytes
+  // [keyOff, keyOff + keyLen) (INTEGRATION.md §3e): every non-empty block is fetched and staged, then ONE
+  // b2s_decompress_sort_packed call verifies, decodes and key-sorts all of the task's records.  The blocks go in
+  // computeShuffleBlocks order (map, then reduce id), so records with equal keys come out in that order whatever the
+  // order the fetches completed in.  Codec NONE (spark.shuffle.compress=false) is verified and sorted only.  With the
+  // exchange cache on, a map resident on this thread's device is one cached source in that order instead of its blocks
+  // (b2s_exchange_read_sort_packed); maps the cache no longer holds when the call runs are fetched and the call repeated.
+  void readSorted(uint32_t recordBytes, uint32_t keyOff, uint32_t keyLen) {
+    readSources([&](const Sources& x, uint64_t cap, uint64_t* total, uint64_t* records, uint64_t*, const char** call) {
+      *call = "b2s_decompress_sort_packed";
+      if (!x.anyCached)
+        return b2s_decompress_sort_packed(x.codec, x.alg, x.n, x.src.src.data(), x.src.off.data(), x.src.len.data(),
+                                          x.sb, x.sl, x.sc, recordBytes, keyOff, keyLen, sorted_.get(), cap, total,
+                                          records, x.status, x.bad);
+      return b2s_exchange_read_sort_packed(shuffleId_, start_, end_, x.ids, x.cached, x.codec, x.alg, x.n,
+                                           x.src.src.data(), x.src.off.data(), x.src.len.data(), x.sb, x.sl, x.sc,
+                                           recordBytes, keyOff, keyLen, sorted_.get(), cap, total, records, x.status,
+                                           x.bad);
+    });
   }
   // The key columns of readRows: column c is type[c] (B2S_KEY_*, B2S_STRING_KEY or B2S_DECIMAL_KEY, with the order
   // flags B2S_KEY_DESCENDING / B2S_KEY_NULLS_LAST) at row offset off[c], len[c] bytes, null bit nullField[c].
@@ -937,58 +987,54 @@ class S3ShuffleReader {
   // staged, then ONE b2s_decompress_{sort,aggregate}_rows[_keys]_packed call verifies, decodes and sorts the task's
   // UnsafeRowSerializer records ([int32 big-endian size][row]) by the key, nulls first, or groups them and merges each
   // group into one row per key in that order.  Blocks go in computeShuffleBlocks order, so equal keys come out in map,
-  // then reduce-id order.  Codec NONE is verified and sorted only.  It reads fetched blocks only: the exchange cache is
-  // not consulted.
+  // then reduce-id order.  Codec NONE is verified and sorted only.  With the exchange cache on, the maps resident on this
+  // thread's device are cached sources in that order, as in readSorted, through the composite-key exchange reads
+  // (b2s_exchange_read_{sort,aggregate}_rows_keys_packed; a one-key read is their n_keys = 1 case, INTEGRATION.md §3m).
   void readRows(const RowKeys& keys, const RowAggregates* aggs) {
-    start(true);
-    std::vector<FetchedBlock> fetched;
-    drainWhole(fetched);
-    std::sort(fetched.begin(), fetched.end(), [](const auto& a, const auto& b) { return a.first < b.first; });
-    const bool verify = d_.checksumEnabled;
-    const uint32_t alg = verify ? S3ShuffleHelper::createChecksumAlgorithm(d_.checksumAlgorithm) : 0;
-    ensure_codec_runtime();
-    const uint32_t codec = (uint32_t)d_.codecId();
-    const uint32_t n = (uint32_t)fetched.size();
-    std::vector<const FetchedBlock*> blocks;
-    for (const auto& f : fetched) blocks.push_back(&f);
-    StagedBlocks src(info_, blocks);
-    const uint32_t* sb = verify ? src.sliceBase.data() : nullptr;
-    const uint64_t* sl = verify ? src.sliceLen.data() : nullptr;
-    const uint64_t* sc = verify ? src.sliceSum.data() : nullptr;
-    std::vector<int32_t> status(n), bad(n);
-    uint64_t total = 0, records = 0, groups = 0;
-    // output size as in readSorted: a first guess, then one retry with the bytes needed
-    const uint64_t guess = codec == B2S_CODEC_NONE ? src.bytes : src.bytes * 4;
-    const int rc = callWithRetry(sorted_, guess, total, [&](uint64_t cap) {
-      if (aggs && keys.composite)
-        return b2s_decompress_aggregate_rows_keys_packed(codec, alg, n, src.src.data(), src.off.data(), src.len.data(),
-                                                         sb, sl, sc, keys.n, keys.type, keys.off, keys.len,
-                                                         keys.nullField, aggs->n, aggs->op, aggs->off, aggs->nullField,
-                                                         sorted_.get(), cap, &total, &records, &groups, status.data(),
-                                                         bad.data());
-      if (aggs)
-        return b2s_decompress_aggregate_rows_packed(codec, alg, n, src.src.data(), src.off.data(), src.len.data(), sb,
-                                                    sl, sc, keys.type[0], keys.off[0], keys.len[0], keys.nullField[0],
-                                                    aggs->n, aggs->op, aggs->off, aggs->nullField, sorted_.get(), cap,
-                                                    &total, &records, &groups, status.data(), bad.data());
-      if (keys.composite)
-        return b2s_decompress_sort_rows_keys_packed(codec, alg, n, src.src.data(), src.off.data(), src.len.data(), sb,
-                                                    sl, sc, keys.n, keys.type, keys.off, keys.len, keys.nullField,
-                                                    sorted_.get(), cap, &total, &records, status.data(), bad.data());
-      return b2s_decompress_sort_rows_packed(codec, alg, n, src.src.data(), src.off.data(), src.len.data(), sb, sl, sc,
-                                             keys.type[0], keys.off[0], keys.len[0], keys.nullField[0], sorted_.get(),
-                                             cap, &total, &records, status.data(), bad.data());
+    readSources([&](const Sources& x, uint64_t cap, uint64_t* total, uint64_t* records, uint64_t* groups,
+                    const char** call) {
+      const uint32_t codec = x.codec, alg = x.alg, n = x.n;
+      const uint8_t* src = x.src.src.data();
+      const uint64_t *off = x.src.off.data(), *len = x.src.len.data();
+      if (x.anyCached && aggs) {
+        *call = "b2s_exchange_read_aggregate_rows_keys_packed";
+        return b2s_exchange_read_aggregate_rows_keys_packed(
+            shuffleId_, start_, end_, x.ids, x.cached, codec, alg, n, src, off, len, x.sb, x.sl, x.sc, keys.n,
+            keys.type, keys.off, keys.len, keys.nullField, aggs->n, aggs->op, aggs->off, aggs->nullField,
+            sorted_.get(), cap, total, records, groups, x.status, x.bad);
+      }
+      if (x.anyCached) {
+        *call = "b2s_exchange_read_sort_rows_keys_packed";
+        return b2s_exchange_read_sort_rows_keys_packed(shuffleId_, start_, end_, x.ids, x.cached, codec, alg, n, src,
+                                                       off, len, x.sb, x.sl, x.sc, keys.n, keys.type, keys.off,
+                                                       keys.len, keys.nullField, sorted_.get(), cap, total, records,
+                                                       x.status, x.bad);
+      }
+      if (aggs && keys.composite) {
+        *call = "b2s_decompress_aggregate_rows_keys_packed";
+        return b2s_decompress_aggregate_rows_keys_packed(codec, alg, n, src, off, len, x.sb, x.sl, x.sc, keys.n,
+                                                         keys.type, keys.off, keys.len, keys.nullField, aggs->n,
+                                                         aggs->op, aggs->off, aggs->nullField, sorted_.get(), cap,
+                                                         total, records, groups, x.status, x.bad);
+      }
+      if (aggs) {
+        *call = "b2s_decompress_aggregate_rows_packed";
+        return b2s_decompress_aggregate_rows_packed(codec, alg, n, src, off, len, x.sb, x.sl, x.sc, keys.type[0],
+                                                    keys.off[0], keys.len[0], keys.nullField[0], aggs->n, aggs->op,
+                                                    aggs->off, aggs->nullField, sorted_.get(), cap, total, records,
+                                                    groups, x.status, x.bad);
+      }
+      if (keys.composite) {
+        *call = "b2s_decompress_sort_rows_keys_packed";
+        return b2s_decompress_sort_rows_keys_packed(codec, alg, n, src, off, len, x.sb, x.sl, x.sc, keys.n, keys.type,
+                                                    keys.off, keys.len, keys.nullField, sorted_.get(), cap, total,
+                                                    records, x.status, x.bad);
+      }
+      *call = "b2s_decompress_sort_rows_packed";
+      return b2s_decompress_sort_rows_packed(codec, alg, n, src, off, len, x.sb, x.sl, x.sc, keys.type[0], keys.off[0],
+                                             keys.len[0], keys.nullField[0], sorted_.get(), cap, total, records,
+                                             x.status, x.bad);
     });
-    if (rc != 0)
-      throw CodecException(std::string(aggs ? (keys.composite ? "b2s_decompress_aggregate_rows_keys_packed: "
-                                                              : "b2s_decompress_aggregate_rows_packed: ")
-                                            : (keys.composite ? "b2s_decompress_sort_rows_keys_packed: "
-                                                              : "b2s_decompress_sort_rows_packed: ")) +
-                           b2s_strerror(rc) + ": " + b2s_last_error());
-    for (uint32_t k = 0; k < n; k++) throwBlockStatus(status[k], info_[fetched[k].first].id);
-    sortedLen_ = total;
-    sortedRecords_ = records;
-    sortedGroups_ = groups;
   }
   const uint8_t* sortedData() const { return sorted_.get(); }
   uint64_t sortedLen() const { return sortedLen_; }
