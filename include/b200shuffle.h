@@ -555,6 +555,79 @@ int b2s_decompress_aggregate_rows_keys_dev(uint32_t dev_index, uint32_t codec, u
                                            uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records,
                                            uint64_t* n_groups, int32_t* status, int32_t* bad_slice);
 
+/* ---- read side, sort-merge join: a reducer's two shuffled UnsafeRow inputs joined in one call ----
+ * Spark SQL's SortMergeJoinExec on a reducer: both children's shuffle reads sorted by the join key and merged into
+ * joined rows (UnsafeRowJoiner), for an equi-join without a further condition.
+ * Sides.  Blocks [0, n_left) are the left (streamed) side's fetched blocks, blocks [n_left, n) the right (buffered)
+ * side's.  Both sides share one codec and one checksum algorithm.  Blocks, slices, checksums and framing as in
+ * b2s_decompress_sort_rows_packed: [size: int32 BE][row], no end marker.
+ * Keys.  Column c has one key_type[c] and key_len[c] for both sides (Spark coerces join keys to one type) and its own
+ * slot and null bit on each side: left_key_off[c] / left_key_null_field[c] and right_key_off[c] /
+ * right_key_null_field[c] (-1: never null on that side).  Every type of the composite-key calls is accepted; the order
+ * flags are not (the join orders ascending, nulls first).  Two keys are equal when every column is non-null on both
+ * sides and the values are equal by the composite-key aggregation's grouping rule (strings by length and bytes, 0.0
+ * equal to -0.0, every NaN equal to every other NaN: Spark's NormalizeFloatingNumbers).  A key with a null column
+ * matches nothing.
+ * Order.  Ls: the left records stably sorted by the key (ascending, nulls first, ties in block order, then in their
+ * order in the block); Rs: the right records sorted the same way.
+ *   B2S_JOIN_INNER: for each l of Ls, for each r of Rs whose key equals l's, in Rs order: join(l, r).
+ *   B2S_JOIN_LEFT_OUTER: the same; a left record without an equal right key (a null key included) gives join(l, null).
+ *   B2S_JOIN_LEFT_SEMI: l itself, byte for byte, once, when it has a match.
+ *   B2S_JOIN_LEFT_ANTI: l itself when it has no match, null keys included (NOT EXISTS; not the null-aware form).
+ * Joined row: UnsafeRowJoiner's, which is UnsafeProjection(left.output ++ right.output) when each input's
+ * variable-length data is laid out as UnsafeProjection writes it.  nL, nR: the sides' field counts (n_left_fields,
+ * n_right_fields); bL, bR, b: the null-bitset words of the left row, the right row and the output, ceil(nL / 64),
+ * ceil(nR / 64), ceil((nL + nR) / 64); varX = size(X) - 8 (bX + nX), side X's variable-length bytes.  The output is
+ * [b words of null bits][left's 8 nL bytes of slots][right's 8 nR][left's var bytes][right's var bytes].  Null bit i
+ * is left bit i for i < nL, right bit i - nL below nL + nR, zero past it.  Every VAR or DECIMAL_WIDE field whose slot
+ * is not zero has its offset (the high 32 bits) moved by 8 (b - bL + nR) on the left, by 8 (b - bR + nL) + varL on
+ * the right; a zero slot (a null string) stays zero, and a null wide decimal (offset << 32) is moved.
+ * The null right side (left outer): every right null bit set, every right slot zero, except that each DECIMAL_WIDE
+ * right field gets 16 zero bytes appended to the var bytes, in field order, and its slot is offset << 32 (what
+ * UnsafeRowWriter.write(i, (Decimal) null, p, s) writes).
+ * Outputs.  [size BE][row] records, an UnsafeRowSerializer stream, *n_out_records of them, *dst_total bytes; dst_cap
+ * below that -> B2S_E_DST_TOO_SMALL with *dst_total = the bytes needed.  *n_left_records / *n_right_records: the input
+ * record counts.  The field-kind arrays (B2S_FIELD_*, one per field) may be NULL for semi and anti joins.
+ * Errors -> B2S_E_ARG: an unknown join_type; n_left > n; a key column the composite-key calls reject, or any order
+ * flag; a key slot outside its side's slots [8 bX, 8 (bX + nX)) or a null bit not below its side's field count; a field
+ * count outside 1..65536; NULL or unknown field kinds for inner and left outer; more than 2^32 - 1 input records.
+ * Per block, B2S_E_CORRUPT for every framing rule of the composite-key calls with that block's side's key columns, and
+ * when a row is shorter than its side's fixed region 8 (bX + nX); b2s_last_error() names the block and the byte offset
+ * of the bad record.  A joined row longer than 2^31 - 1 bytes -> B2S_E_UNSUPPORTED.  Checksums and bad_slice as in the
+ * sorts.  When a block fails nothing is written, every count is 0 and the call returns 0.  The task or its output not
+ * fitting in device memory -> B2S_E_NOMEM (the caller keeps Spark's join).
+ * Runs on the read lane with the sorts' 1 GiB buffer trim.  b2s_last_timing: kernel_ms the whole call, top_kernel_ms
+ * framing, keys, sort and join, dominant_ms / dominant_launches the join step alone (from the sorted order to the
+ * written output). */
+#define B2S_JOIN_INNER 0
+#define B2S_JOIN_LEFT_OUTER 1
+#define B2S_JOIN_LEFT_SEMI 2
+#define B2S_JOIN_LEFT_ANTI 3
+/* field kinds of a side's schema (the joined row's offset fix-up and the null right side of a left outer join) */
+#define B2S_FIELD_FIXED 0        /* a fixed-width value in its 8-byte slot */
+#define B2S_FIELD_VAR 1          /* (offset << 32) | size: string, binary, array, map, struct */
+#define B2S_FIELD_DECIMAL_WIDE 2 /* Decimal(p > 18): (offset << 32) | size, 16 bytes reserved */
+int b2s_decompress_join_rows_keys_packed(
+    uint32_t join_type, uint32_t codec, uint32_t checksum_alg, uint32_t n_left, uint32_t n, const uint8_t* src_base,
+    const uint64_t* src_off, const uint64_t* src_len, const uint32_t* slice_base, const uint64_t* slice_len,
+    const uint64_t* slice_checksum, uint32_t n_keys, const uint32_t* key_type, const uint32_t* key_len,
+    const uint32_t* left_key_off, const int32_t* left_key_null_field, const uint32_t* right_key_off,
+    const int32_t* right_key_null_field, uint32_t n_left_fields, const uint8_t* left_field_kind,
+    uint32_t n_right_fields, const uint8_t* right_field_kind, uint8_t* dst_base, uint64_t dst_cap,
+    uint64_t* dst_total, uint64_t* n_left_records, uint64_t* n_right_records, uint64_t* n_out_records, int32_t* status,
+    int32_t* bad_slice);
+/* same, with src_base / dst_base in device memory of dev_index; the descriptor, key and field-kind arrays stay host
+ * arrays */
+int b2s_decompress_join_rows_keys_dev(
+    uint32_t dev_index, uint32_t join_type, uint32_t codec, uint32_t checksum_alg, uint32_t n_left, uint32_t n,
+    const uint8_t* src_base, const uint64_t* src_off, const uint64_t* src_len, const uint32_t* slice_base,
+    const uint64_t* slice_len, const uint64_t* slice_checksum, uint32_t n_keys, const uint32_t* key_type,
+    const uint32_t* key_len, const uint32_t* left_key_off, const int32_t* left_key_null_field,
+    const uint32_t* right_key_off, const int32_t* right_key_null_field, uint32_t n_left_fields,
+    const uint8_t* left_field_kind, uint32_t n_right_fields, const uint8_t* right_field_kind, uint8_t* dst_base,
+    uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_left_records, uint64_t* n_right_records,
+    uint64_t* n_out_records, int32_t* status, int32_t* bad_slice);
+
 /* ---- exchange cache: map outputs kept resident in HBM for reducers on the same device ----
  * (docs/f4_gpu_resident_exchange.md steps 2 and 3, local half.)  The serialized writer's partition step already leaves
  * a map task's records partitioned by reduce id in HBM; the cached store keeps that arena, keyed by (shuffle_id,

@@ -208,6 +208,19 @@ int b2sh_reader_read_aggregated_rows_keys(b2sh_reader* r, uint32_t n_keys, const
                                           const uint32_t* agg_off, const int32_t* agg_null_field,
                                           const uint8_t** data, uint64_t* len, uint64_t* n_records,
                                           uint64_t* n_groups);
+/* read_joined_rows(): Spark's SortMergeJoinExec on a reducer, left's reduce partitions joined with right's (the same
+ * partitions of another shuffle; INTEGRATION.md §3n).  Both readers' non-empty blocks are fetched, left's first, each
+ * in computeShuffleBlocks order, and ONE b2s_decompress_join_rows_keys_packed call (retried once with the exact size on
+ * B2S_E_DST_TOO_SMALL) verifies, decodes, sorts and joins them; the arguments are that call's.  The exchange cache is
+ * not consulted.  *data / *len: the joined rows (for semi and anti joins the left records), valid until left's next
+ * read; *n_out_records of them.  Errors as read_sorted_rows_keys(). */
+int b2sh_reader_read_joined_rows(b2sh_reader* left, b2sh_reader* right, uint32_t join_type, uint32_t n_keys,
+                                 const uint32_t* key_type, const uint32_t* key_len, const uint32_t* left_key_off,
+                                 const int32_t* left_key_null_field, const uint32_t* right_key_off,
+                                 const int32_t* right_key_null_field, uint32_t n_left_fields,
+                                 const uint8_t* left_field_kind, uint32_t n_right_fields,
+                                 const uint8_t* right_field_kind, const uint8_t** data, uint64_t* len,
+                                 uint64_t* n_left_records, uint64_t* n_right_records, uint64_t* n_out_records);
 int b2sh_reader_block(b2sh_reader* r, uint32_t k, int64_t* map_id, int32_t* start_reduce, int32_t* end_reduce,
                       const uint8_t** data, uint64_t* len);
 uint64_t b2sh_reader_remote_bytes_read(b2sh_reader* r); /* metric parity with storage/S3ShuffleReader.scala:94-95 */

@@ -703,6 +703,80 @@ JNIEXPORT jint JNICALL J(exchangeReadSortPacked)(JNIEnv* e, jclass c, jint shuff
                      meta, status, badSlice);
 }
 
+/* a native copy of the first n elements (elem bytes each: 1 byte, 4 int, 8 long) of a Java array; NULL for a NULL
+ * array.  *rc: B2S_E_ARG when the array is shorter than n, B2S_E_NOMEM when the copy cannot be had (nothing is done
+ * once *rc is set) */
+static void* region(JNIEnv* e, jarray a, jsize n, size_t elem, int* rc) {
+  if (!a || *rc) return 0;
+  if (n < 0 || (*e)->GetArrayLength(e, a) < n) {
+    *rc = B2S_E_ARG;
+    return 0;
+  }
+  void* p = malloc((size_t)n * elem + 1);
+  if (!p) {
+    *rc = B2S_E_NOMEM;
+    return 0;
+  }
+  if (elem == 1) (*e)->GetByteArrayRegion(e, (jbyteArray)a, 0, n, (jbyte*)p);
+  else if (elem == 4) (*e)->GetIntArrayRegion(e, (jintArray)a, 0, n, (jint*)p);
+  else (*e)->GetLongArrayRegion(e, (jlongArray)a, 0, n, (jlong*)p);
+  return p;
+}
+
+/* ---- read side, sort-merge join (INTEGRATION.md §3n): blocks [0, nLeft) are the left side's, the rest the right's.
+ *      keyType / keyLen: int[nKeys] for both sides; left/rightKeyOff and left/rightKeyNullField: int[nKeys] per side;
+ *      left/rightFieldKind: byte[nFields] of B2S_FIELD_* (null for semi and anti joins); meta: long[4] = {dst_total,
+ *      n_left_records, n_right_records, n_out_records}; other arrays as decompressSortRowsPacked.  Every array goes
+ *      through a native copy. ---- */
+JNIEXPORT jint JNICALL J(decompressJoinRowsKeysPacked)(JNIEnv* e, jclass c, jint joinType, jint codec, jint alg,
+                                                       jint nLeft, jint n, jlong src, jlongArray off, jlongArray len,
+                                                       jintArray sliceBase, jlongArray sliceLen,
+                                                       jlongArray sliceChecksum, jint nKeys, jintArray keyType,
+                                                       jintArray keyLen, jintArray leftKeyOff,
+                                                       jintArray leftKeyNullField, jintArray rightKeyOff,
+                                                       jintArray rightKeyNullField, jint nLeftFields,
+                                                       jbyteArray leftFieldKind, jint nRightFields,
+                                                       jbyteArray rightFieldKind, jlong dst, jlong dstCap,
+                                                       jlongArray meta, jintArray status, jintArray badSlice) {
+  (void)c;
+  if (n < 0 || !meta || (*e)->GetArrayLength(e, meta) < 4) return B2S_E_ARG;
+  if (n > 0 && (!status || (*e)->GetArrayLength(e, status) < n || (badSlice && (*e)->GetArrayLength(e, badSlice) < n)))
+    return B2S_E_ARG;
+  const int with_slices = alg != 0 && n > 0;
+  int rc = 0;
+  uint64_t* o = region(e, off, n, 8, &rc);
+  uint64_t* l = region(e, len, n, 8, &rc);
+  uint32_t* sb = with_slices ? region(e, sliceBase, n + 1, 4, &rc) : 0;
+  const jsize ns = sb && !rc ? (jsize)sb[n] : 0;
+  uint64_t* sl = with_slices ? region(e, sliceLen, ns, 8, &rc) : 0;
+  uint64_t* sc = with_slices ? region(e, sliceChecksum, ns, 8, &rc) : 0;
+  uint32_t* kt = region(e, keyType, nKeys, 4, &rc);
+  uint32_t* kl = region(e, keyLen, nKeys, 4, &rc);
+  uint32_t* lo = region(e, leftKeyOff, nKeys, 4, &rc);
+  int32_t* ln = region(e, leftKeyNullField, nKeys, 4, &rc);
+  uint32_t* ro = region(e, rightKeyOff, nKeys, 4, &rc);
+  int32_t* rn = region(e, rightKeyNullField, nKeys, 4, &rc);
+  uint8_t* lk = region(e, leftFieldKind, nLeftFields, 1, &rc);
+  uint8_t* rk = region(e, rightFieldKind, nRightFields, 1, &rc);
+  int32_t* st = (int32_t*)malloc((size_t)n * 2 * sizeof(int32_t) + 1);
+  if (!rc && !st) rc = B2S_E_NOMEM;
+  uint64_t m[4] = {0, 0, 0, 0};
+  if (!rc) {
+    rc = b2s_decompress_join_rows_keys_packed(
+        (uint32_t)joinType, (uint32_t)codec, (uint32_t)alg, (uint32_t)nLeft, (uint32_t)n, PTR(const uint8_t, src), o,
+        l, sb, sl, sc, (uint32_t)nKeys, kt, kl, lo, ln, ro, rn, (uint32_t)nLeftFields, lk, (uint32_t)nRightFields, rk,
+        PTR(uint8_t, dst), (uint64_t)dstCap, &m[0], &m[1], &m[2], &m[3], st, st + n);
+    (*e)->SetLongArrayRegion(e, meta, 0, 4, (const jlong*)m);
+    if (n > 0) {
+      (*e)->SetIntArrayRegion(e, status, 0, n, (const jint*)st);
+      if (badSlice) (*e)->SetIntArrayRegion(e, badSlice, 0, n, (const jint*)(st + n));
+    }
+  }
+  void* owned[] = {o, l, sb, sl, sc, kt, kl, lo, ln, ro, rn, lk, rk, st};
+  for (size_t i = 0; i < sizeof owned / sizeof owned[0]; i++) free(owned[i]);
+  return rc;
+}
+
 /* decompressSortRowsKeysPacked / decompressAggregateRowsKeysPacked over sources of which those with cached[i] != 0
  * are the cached range of mapIds[i] (INTEGRATION.md §3m; mapIds: long[n], cached: int[n]) */
 JNIEXPORT jint JNICALL J(exchangeReadSortRowsKeysPacked)(JNIEnv* e, jclass c, jint shuffleId, jint startReduce,

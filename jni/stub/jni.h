@@ -24,6 +24,7 @@ typedef jobject jstring;
 typedef jobject jarray;
 typedef jarray jlongArray;
 typedef jarray jintArray;
+typedef jarray jbyteArray;
 
 struct JNINativeInterface_;
 typedef const struct JNINativeInterface_* JNIEnv;
@@ -40,5 +41,6 @@ struct JNINativeInterface_ {
   void (*SetIntArrayRegion)(JNIEnv* env, jintArray array, jsize start, jsize len, const jint* buf);
   void (*GetLongArrayRegion)(JNIEnv* env, jlongArray array, jsize start, jsize len, jlong* buf);
   void (*GetIntArrayRegion)(JNIEnv* env, jintArray array, jsize start, jsize len, jint* buf);
+  void (*GetByteArrayRegion)(JNIEnv* env, jbyteArray array, jsize start, jsize len, jbyte* buf);
 };
 #endif

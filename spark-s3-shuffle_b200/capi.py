@@ -22,6 +22,9 @@ KEY_DESCENDING, KEY_NULLS_LAST = 1 << 8, 1 << 9
  AGG_MAX_FLOAT64) = range(8)
 # the Decimal ops (8 is unassigned); SUM_DECIMAL takes its buffer's precision P (1..38) as AGG_SUM_DECIMAL | P << 8
 AGG_SUM_DECIMAL, AGG_MIN_DECIMAL, AGG_MAX_DECIMAL = 9, 10, 11
+# join types of the row join (decompress_join_rows_keys_*) and the field kinds of its sides' schemas
+JOIN_INNER, JOIN_LEFT_OUTER, JOIN_LEFT_SEMI, JOIN_LEFT_ANTI = 0, 1, 2, 3
+FIELD_FIXED, FIELD_VAR, FIELD_DECIMAL_WIDE = 0, 1, 2
 OK, E_CORRUPT, E_CHECKSUM, E_DST_TOO_SMALL, E_UNSUPPORTED, E_ARG, E_CUDA, E_NOT_INIT, E_NOMEM, E_NOT_CACHED = (
     0, -1, -2, -3, -4, -5, -6, -7, -8, -9)
 NOT_RESIDENT = 2**64 - 1  # b2s_exchange_lookup's length of a map output that is not resident
@@ -128,6 +131,12 @@ PROTOTYPES = [
     ("b2s_decompress_aggregate_rows_keys_dev", C.c_int,
      [_u32, _u32, _u32, _u32, _vp, _u64p, _u64p, _u32p, _u64p, _u64p, _u32, _u32p, _u32p, _u32p, _i32p, _u32, _u32p,
       _u32p, _i32p, _vp, _u64, _u64p, _u64p, _u64p, _i32p, _i32p]),
+    ("b2s_decompress_join_rows_keys_packed", C.c_int,
+     [_u32, _u32, _u32, _u32, _u32, _u8p, _u64p, _u64p, _u32p, _u64p, _u64p, _u32, _u32p, _u32p, _u32p, _i32p, _u32p,
+      _i32p, _u32, _u8p, _u32, _u8p, _u8p, _u64, _u64p, _u64p, _u64p, _u64p, _i32p, _i32p]),
+    ("b2s_decompress_join_rows_keys_dev", C.c_int,
+     [_u32, _u32, _u32, _u32, _u32, _u32, _vp, _u64p, _u64p, _u32p, _u64p, _u64p, _u32, _u32p, _u32p, _u32p, _i32p,
+      _u32p, _i32p, _u32, _u8p, _u32, _u8p, _vp, _u64, _u64p, _u64p, _u64p, _u64p, _i32p, _i32p]),
     ("b2s_exchange_set_budget", C.c_int, [_u32, _u64]),
     ("b2s_partition_compress_cached_packed", C.c_int,
      [_i32, C.c_int64, _u32, _i32, _u32, _u32, _u32, _u64, _u8p, _u64, _u32p, _u32p, _u8p, _u64, _u64p, _u64p, _u64p,
@@ -459,12 +468,14 @@ def _arg(a):
     return _ptr(a) if isinstance(a, np.ndarray) else a
 
 
-def _sort_call(symbol, codec, src, off, length, dst, dst_cap, mid, checksum_alg, slices, dev=None, lead=(), n=None):
-    """One call of the sort family, whose arguments are [dev,] *lead, codec, checksum_alg, n, src, off, length, the
-    three slice arrays, *mid, dst, dst_cap, total, n_records, [n_groups,] status, bad_slice.  dev None: the packed form,
-    src and dst host arrays (dst_cap is dst's size); else src and dst are device addresses.  lead and mid are the
-    call's own arguments, numpy arrays among them passed as pointers; n defaults to the number of blocks in off.
-    -> dict(total, n_records, status, bad_slice), with n_groups after n_records for the aggregate calls"""
+def _sort_call(symbol, codec, src, off, length, dst, dst_cap, mid, checksum_alg, slices, dev=None, lead=(), n=None,
+               before_n=()):
+    """One call of the sort family, whose arguments are [dev,] *lead, codec, checksum_alg, *before_n, n, src, off,
+    length, the three slice arrays, *mid, dst, dst_cap, total, n_records, [n_groups,] status, bad_slice.  dev None: the
+    packed form, src and dst host arrays (dst_cap is dst's size); else src and dst are device addresses.  lead,
+    before_n and mid are the call's own arguments, numpy arrays among them passed as pointers; n defaults to the number
+    of blocks in off.  -> dict(total, n_records, status, bad_slice), with n_groups after n_records for the aggregate
+    calls; the join calls return n_left_records, n_right_records and n_out_records in n_records' place"""
     if dev is None:
         src, dst = _as_u8(src), _as_u8(dst)
         dst_cap = dst.size
@@ -474,12 +485,13 @@ def _sort_call(symbol, codec, src, off, length, dst, dst_cap, mid, checksum_alg,
     sb, sl, sc = _slice_arrays(checksum_alg, *slices)
     st = np.zeros(max(n, 1), dtype=np.int32)
     bad = np.zeros(max(n, 1), dtype=np.int32)
-    groups = "_aggregate_" in symbol
-    counts = [_u64(0) for _ in range(3 if groups else 2)]
-    args = ([] if dev is None else [dev]) + [*lead, codec, checksum_alg, n, src, off, length, sb, sl, sc, *mid, dst,
-                                             dst_cap]
+    names = (("total", "n_left_records", "n_right_records", "n_out_records") if "_join_" in symbol else
+             ("total", "n_records", "n_groups") if "_aggregate_" in symbol else ("total", "n_records"))
+    counts = [_u64(0) for _ in names]
+    args = ([] if dev is None else [dev]) + [*lead, codec, checksum_alg, *before_n, n, src, off, length, sb, sl, sc,
+                                             *mid, dst, dst_cap]
     _check(getattr(load(), symbol)(*map(_arg, args), *map(C.addressof, counts), _ptr(st), _ptr(bad)), symbol)
-    r = dict(zip(("total", "n_records", "n_groups"), (c.value for c in counts)))
+    r = dict(zip(names, (c.value for c in counts)))
     r.update(status=st[:n], bad_slice=bad[:n])
     return r
 
@@ -531,6 +543,32 @@ def decompress_aggregate_rows_keys_packed(codec, src, off, length, dst, keys, ag
     -> dict(total, n_records, n_groups, status, bad_slice)"""
     return _sort_call("b2s_decompress_aggregate_rows_keys_packed", codec, src, off, length, dst, None,
                       (*_key_arrays(keys), *_agg_arrays(aggs)), checksum_alg, (slice_base, slice_len, slice_checksum))
+
+
+def _join_arrays(left_keys, right_keys, left_kinds, right_kinds):
+    """the join's key and field-kind arguments: the columns' types and lengths are the left keys', each side's slots
+    and null fields its own; a kinds sequence of None is passed as NULL"""
+    n, kt, lo, kl, ln = _key_arrays(left_keys)
+    _, _, ro, _, rn = _key_arrays(right_keys)
+    kinds = [None if k is None else np.ascontiguousarray(k, dtype=np.uint8) for k in (left_kinds, right_kinds)]
+    return n, kt, kl, lo, ln, ro, rn, kinds[0], kinds[1]
+
+
+def decompress_join_rows_keys_packed(join_type, codec, src, off, length, n_left, dst, left_keys, right_keys,
+                                     n_left_fields, n_right_fields, left_kinds=None, right_kinds=None,
+                                     checksum_alg=CHECKSUM_NONE, slice_base=None, slice_len=None,
+                                     slice_checksum=None):
+    """Sort-merge joins a reducer's two shuffled sides of UnsafeRow records: blocks [0, n_left) are the left side's,
+    the rest the right's.  left_keys / right_keys: [(key type, row offset, length, null field or -1), ...] as in
+    decompress_sort_rows_keys_packed without order flags, one entry per join key column on each side (the types and
+    lengths are the left's).  The kinds (FIELD_*, one per field; None for semi and anti joins) say which slots hold an
+    offset.  dst receives Spark's joined rows ([int32 big-endian size][row]) for JOIN_INNER / JOIN_LEFT_OUTER, the left
+    records for JOIN_LEFT_SEMI / JOIN_LEFT_ANTI.
+    -> dict(total, n_left_records, n_right_records, n_out_records, status, bad_slice)"""
+    n, kt, kl, lo, ln, ro, rn, lk, rk = _join_arrays(left_keys, right_keys, left_kinds, right_kinds)
+    return _sort_call("b2s_decompress_join_rows_keys_packed", codec, src, off, length, dst, None,
+                      (n, kt, kl, lo, ln, ro, rn, n_left_fields, lk, n_right_fields, rk), checksum_alg,
+                      (slice_base, slice_len, slice_checksum), lead=(join_type,), before_n=(n_left,))
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -633,6 +671,17 @@ def decompress_aggregate_rows_keys_dev(codec, d_src, off, length, d_dst, dst_cap
     return _sort_call("b2s_decompress_aggregate_rows_keys_dev", codec, d_src, off, length, d_dst, dst_cap,
                       (*_key_arrays(keys), *_agg_arrays(aggs)), checksum_alg, (slice_base, slice_len, slice_checksum),
                       dev)
+
+
+def decompress_join_rows_keys_dev(join_type, codec, d_src, off, length, n_left, d_dst, dst_cap, left_keys, right_keys,
+                                  n_left_fields, n_right_fields, left_kinds=None, right_kinds=None,
+                                  checksum_alg=CHECKSUM_NONE, slice_base=None, slice_len=None, slice_checksum=None,
+                                  dev=0):
+    """decompress_join_rows_keys_packed on device-resident blocks (d_src) into a device arena (d_dst)"""
+    n, kt, kl, lo, ln, ro, rn, lk, rk = _join_arrays(left_keys, right_keys, left_kinds, right_kinds)
+    return _sort_call("b2s_decompress_join_rows_keys_dev", codec, d_src, off, length, d_dst, dst_cap,
+                      (n, kt, kl, lo, ln, ro, rn, n_left_fields, lk, n_right_fields, rk), checksum_alg,
+                      (slice_base, slice_len, slice_checksum), dev, lead=(join_type,), before_n=(n_left,))
 
 
 def partition_compress_dev(codec, d_records, rec_bytes, d_rec_len, d_rec_part, n_records, num_partitions, d_dst,

@@ -822,7 +822,7 @@ int get_device(uint32_t dev_index, Device** out) {
 }
 
 // the kinds of call whose steps add_times reads into b2s_last_timing, one rule each
-enum class Family { kCodec, kPartition, kPartitionNone, kSort, kSortRows, kAggregate };
+enum class Family { kCodec, kPartition, kPartitionNone, kSort, kSortRows, kAggregate, kJoin };
 
 // Adds the times of this call's steps on S to b2s_last_timing: kernel_ms, top_kernel_ms, dominant_ms / _launches by
 // the rule of its family, and h2d_ms.  A step the call did not run reads 0; one it started but did not finish ends
@@ -850,6 +850,7 @@ void add_times(Slot& S, Family f) {
     case Family::kSort:       // verification + decode + sort; the sort step; the decoder's dominant pairs
     case Family::kSortRows:   // the same; framing + order + gather; the framing (walk + count, emit)
     case Family::kAggregate:  // the same; framing through merge; grouping + merge
+    case Family::kJoin:       // the same; framing through join; the join step (grouping, counts, emit)
       t.kernel_ms += S.span(K0, P1);
       t.top_kernel_ms += S.span(P0, P1);
       if (f == Family::kSort) S.take_pairs();
@@ -857,7 +858,7 @@ void add_times(Slot& S, Family f) {
         dominant(F0, F1);
         dominant(F2, F3);
       }
-      if (f == Family::kAggregate) dominant(G0, G1);
+      if (f == Family::kAggregate || f == Family::kJoin) dominant(G0, G1);
       break;
   }
   t.h2d_ms += S.span(H0, H1);
@@ -2516,6 +2517,7 @@ int b2s_decompress_packed(uint32_t codec, uint32_t checksum_alg, uint32_t n, con
 // What the records of a sort call are: fixed-size (record_bytes long, an unsigned byte key) or length-prefixed UnsafeRow
 // records (rows: [size: int32 big-endian][row], key columns in the row, each with its null bit).  aggregate: rows
 // grouped by the key and merged (b2s_decompress_aggregate_rows_*: the caller's n_aggs aggregates), not sorted.
+struct JoinSpec;
 struct RecordSpec {
   bool is_rows = false;
   uint32_t record_bytes = 0;
@@ -2528,8 +2530,22 @@ struct RecordSpec {
   const uint32_t* agg_op = nullptr;
   const uint32_t* agg_off = nullptr;
   const int32_t* agg_null_field = nullptr;
+  const JoinSpec* join = nullptr;  // a join: keys are the left side's columns
   bool rows() const { return is_rows; }
-  Family family() const { return aggregate ? Family::kAggregate : is_rows ? Family::kSortRows : Family::kSort; }
+  Family family() const {
+    return join ? Family::kJoin : aggregate ? Family::kAggregate : is_rows ? Family::kSortRows : Family::kSort;
+  }
+};
+// A join's other arguments (b2s_decompress_join_rows_keys_*): its type, the left blocks, the right side's key columns,
+// both sides' field counts and kinds, and the per-side record counts it returns.  Side 0 is the left.
+struct JoinSpec {
+  uint32_t type = 0;
+  uint32_t n_left = 0;
+  KeySpec right;
+  bool right_arrays = true;  // the right side's key arrays are not NULL
+  uint32_t n_fields[2] = {};
+  const uint8_t* kind[2] = {};
+  uint64_t* n_side[2] = {};
 };
 static RecordSpec fixed_spec(uint32_t record_bytes, uint32_t key_off, uint32_t key_len) {
   RecordSpec r;
@@ -2679,6 +2695,43 @@ static int key_columns_args(const RecordSpec& spec) {
   return 0;
 }
 
+// the null-bitset words of n fields
+static uint32_t bitset_words(uint32_t n) { return (n + 63) / 64; }
+
+// a join's checks past the composite key's (the left columns): its type and blocks, the right columns, no order flag,
+// each side's fields, and every key slot and null bit inside its side's fixed region
+static int join_args(const RecordSpec& spec, uint32_t n) {
+  const JoinSpec& js = *spec.join;
+  if (js.type > B2S_JOIN_LEFT_ANTI) return fail(B2S_E_ARG, "unknown join_type%s");
+  if (js.n_left > n) return fail(B2S_E_ARG, "n_left must be at most n%s");
+  RecordSpec right = spec;
+  right.keys = js.right;
+  right.key_arrays = js.right_arrays;
+  if (int rc = key_columns_args(right)) return rc;
+  const KeySpec* side[2] = {&spec.keys, &js.right};
+  const bool kinds = js.type == B2S_JOIN_INNER || js.type == B2S_JOIN_LEFT_OUTER;
+  for (uint32_t s = 0; s < 2; s++) {
+    const uint32_t nf = js.n_fields[s];
+    if (nf < 1 || nf > 65536) return fail(B2S_E_ARG, "a side's field count must be in [1, 65536]%s");
+    const uint64_t lo = 8ull * bitset_words(nf), hi = lo + 8ull * nf;
+    for (uint32_t c = 0; c < side[s]->n; c++) {
+      if (side[s]->type[c] & ~kKeyTypeMask) return fail(B2S_E_ARG, "a join key column takes no order flag%s");
+      if (side[s]->off[c] < lo || (uint64_t)side[s]->off[c] + side[s]->len[c] > hi)
+        return fail(B2S_E_ARG, "a key slot lies outside its side's field slots%s");
+      if (side[s]->null_field[c] >= (int64_t)nf)
+        return fail(B2S_E_ARG, "a key null bit is not below its side's field count%s");
+    }
+    if (kinds) {
+      if (!js.kind[s]) return fail(B2S_E_ARG, "field kinds are required for inner and left outer joins%s");
+      for (uint32_t f = 0; f < nf; f++)
+        if (js.kind[s][f] > B2S_FIELD_DECIMAL_WIDE) return fail(B2S_E_ARG, "unknown field kind%s");
+    }
+  }
+  for (uint32_t s = 0; s < 2; s++)
+    if (!js.n_side[s]) return fail(B2S_E_ARG, "null argument%s");
+  return 0;
+}
+
 static int sort_args(uint32_t codec, uint32_t alg, uint32_t n, const uint64_t* src_off, const uint64_t* src_len,
                      const uint32_t* slice_base, const uint64_t* slice_len, const uint64_t* slice_checksum,
                      const RecordSpec& spec, const void* src_base, const void* dst_base, uint64_t dst_cap,
@@ -2690,6 +2743,8 @@ static int sort_args(uint32_t codec, uint32_t alg, uint32_t n, const uint64_t* s
     if (int rc = key_columns_args(spec)) return rc;
     if (spec.aggregate)
       if (int rc = agg_args(spec)) return rc;
+    if (spec.join)
+      if (int rc = join_args(spec, n)) return rc;
   } else {
     const uint32_t key_len = ks.len[0];
     if (spec.record_bytes == 0) return fail(B2S_E_ARG, "record_bytes must be at least 1%s");
@@ -3084,6 +3139,42 @@ static int aggregate_rows_tail(Slot& S, const RecordSpec& spec, const uint8_t* a
   return 0;
 }
 
+// A join's key columns per side (JoinKeys: a column nullable on one side only takes kNullByteOnly on the other, so
+// equal keys encode equal; split: the arena offset of the right side's first block) and its joined row's shape, whose
+// field lists (left VAR / DECIMAL_WIDE fields, right ones, right DECIMAL_WIDE ones) go to fields.
+static void join_layout(const RecordSpec& spec, uint64_t split, JoinKeys& jk, JoinShape& shape,
+                        std::vector<uint32_t>& fields) {
+  const JoinSpec& js = *spec.join;
+  jk.side[0] = spec.keys;
+  jk.side[1] = js.right;
+  for (uint32_t c = 0; c < spec.keys.n; c++) {
+    int32_t& l = jk.side[0].null_field[c];
+    int32_t& r = jk.side[1].null_field[c];
+    if (l >= 0 && r < 0) r = kNullByteOnly;
+    if (r >= 0 && l < 0) l = kNullByteOnly;
+  }
+  jk.split = split;
+  shape.type = js.type;
+  shape.split = split;
+  shape.left_keys = spec.keys;
+  for (uint32_t s = 0; s < 2; s++) {
+    shape.n[s] = js.n_fields[s];
+    shape.bw[s] = bitset_words(js.n_fields[s]);
+    jk.fixed[s] = 8 * (shape.bw[s] + shape.n[s]);
+  }
+  shape.out_bw = bitset_words(shape.n[0] + shape.n[1]);
+  fields.clear();
+  const bool rows = js.type == B2S_JOIN_INNER || js.type == B2S_JOIN_LEFT_OUTER;  // a semi or anti join: no kinds
+  for (uint32_t s = 0; s < 2; s++) {
+    for (uint32_t f = 0; rows && f < shape.n[s]; f++)
+      if (js.kind[s][f] != B2S_FIELD_FIXED) fields.push_back(f);
+    shape.n_var[s] = (uint32_t)fields.size() - (s ? shape.n_var[0] : 0);
+  }
+  for (uint32_t f = 0; rows && f < shape.n[1]; f++)
+    if (js.kind[1][f] == B2S_FIELD_DECIMAL_WIDE) fields.push_back(f);
+  shape.n_wide_right = (uint32_t)fields.size() - shape.n_var[0] - shape.n_var[1];
+}
+
 // The whole reduce task on the device: compressed blocks at d_src + src_dev_off[i] (src_contiguous: back to back from
 // d_src in block order, no gaps).  Phase A verifies the slices and sizes every block; a failed block, or (fixed-size
 // records) a decoded length that is not a multiple of record_bytes, ends the call with status[] set and *n_rec = 0
@@ -3155,7 +3246,7 @@ static int decompress_sort_run(Device* D, Slot& S, uint32_t codec, uint32_t alg,
   if (failed) return report();
   if (!spec.rows() && *total / spec.record_bytes > 0xffffffffull)
     return fail(B2S_E_ARG, "more than 2^32 - 1 records in one call (%s bytes)", std::to_string(*total).c_str());
-  if (!spec.aggregate && *total > out_cap) {  // an aggregation's output is sized once the groups are known
+  if (!spec.aggregate && !spec.join && *total > out_cap) {  // an aggregation's or join's output is sized later
     report();
     return fail(B2S_E_DST_TOO_SMALL, "dst_cap is below the %s decoded bytes", std::to_string(*total).c_str());
   }
@@ -3206,7 +3297,7 @@ static int decompress_sort_run(Device* D, Slot& S, uint32_t codec, uint32_t alg,
   }
   report();
 
-  if (!*d_sorted) {
+  if (!*d_sorted && !spec.join) {
     if ((rc = S.parena.ensure(*total + 64))) return rc;
     *d_sorted = (uint8_t*)S.parena.p;
   }
@@ -3226,7 +3317,7 @@ static int decompress_sort_run(Device* D, Slot& S, uint32_t codec, uint32_t alg,
   // rows: frame every source's range, then one readback of the record count and the verdicts
   const KeySpec& ks = spec.keys;
   uint64_t min_key = 0, min_null = 0;
-  for (uint32_t c = 0; c < ks.n; c++) {
+  for (uint32_t c = 0; c < ks.n && !spec.join; c++) {  // a join checks each side's rows in its key pass
     min_key = std::max<uint64_t>(min_key, (uint64_t)ks.off[c] + ks.len[c]);
     if (ks.null_field[c] >= 0) min_null = std::max<uint64_t>(min_null, null_word(ks.null_field[c]) + 8);
   }
@@ -3259,13 +3350,14 @@ static int decompress_sort_run(Device* D, Slot& S, uint32_t codec, uint32_t alg,
       if (v[i] == ~0ull) continue;
       (cached(i) ? cached_status[i] : J.h.status[block(i)]) = B2S_E_CORRUPT;
       if (!failed) {
-        static const char* const why[] = {"", "the block ends inside a size prefix", "the size is negative",
-                                          "the record runs past the block end",
-                                          "the row is shorter than key_off + key_len",
-                                          "the row does not hold the null-bit word",
-                                          "the row is shorter than an aggregate slot",
-                                          "a string key runs past the end of its row, or a decimal key's size "
-                                          "is not in [1, 16] or its bytes run past the end of its row"};
+        const char* const why[] = {"", "the block ends inside a size prefix", "the size is negative",
+                                   "the record runs past the block end",
+                                   spec.join ? "the row is shorter than its side's fixed region"
+                                             : "the row is shorter than key_off + key_len",
+                                   "the row does not hold the null-bit word",
+                                   "the row is shorter than an aggregate slot",
+                                   "a string key runs past the end of its row, or a decimal key's size "
+                                   "is not in [1, 16] or its bytes run past the end of its row"};
         snprintf(msg, sizeof msg, "%s %u: bad row record at byte %llu: %s", cached(i) ? "cached source" : "block", i,
                  (unsigned long long)(v[i] & ((1ull << 61) - 1)), why[v[i] >> 61]);
         fail(B2S_E_CORRUPT, "%s", msg);
@@ -3278,19 +3370,35 @@ static int decompress_sort_run(Device* D, Slot& S, uint32_t codec, uint32_t alg,
   const uint64_t records = rb[0];
   if (records > 0xffffffffull)
     return fail(B2S_E_ARG, "more than 2^32 - 1 records in one call (%s records)", std::to_string(records).c_str());
-  const uint32_t key_bytes = rows_key_bytes(ks);
-  const bool refine = rows_key_refines(ks);
+  // a join: its key columns per side as its kernels encode them (a column nullable on one side only takes a null byte
+  // on both), which set the key's width for every step, and its joined row's shape
+  std::vector<uint32_t> join_fields;
+  JoinKeys jk;
+  JoinShape shape{};
+  if (spec.join)
+    join_layout(spec, n_src > spec.join->n_left ? place[spec.join->n_left] : *total, jk, shape, join_fields);
+  const KeySpec& encoded = spec.join ? jk.side[0] : ks;
+  const uint32_t key_bytes = rows_key_bytes(encoded);
+  const bool refine = rows_key_refines(encoded);
   const size_t sort_ws = rows_sort_ws_bytes(records, key_bytes);
   const size_t agg_ws = spec.aggregate ? rows_aggregate_ws_bytes(records, spec.n_aggs, agg_spec(spec).n_wide) : 0;
   const size_t refine_ws = refine ? rows_refine_ws_bytes(records, n_src) : 0;
-  if (records && (rc = S.pws.ensure(sort_ws + agg_ws + refine_ws))) return rc;
+  // a join: the grouping's workspace (an aggregation without aggregates) and the join's
+  const size_t join_ws = spec.join ? rows_aggregate_ws_bytes(records, 0, 0) : 0;
+  const size_t join_own_ws = spec.join ? join_ws_bytes(records, n_src, (uint32_t)join_fields.size()) : 0;
+  if ((records || spec.join) && (rc = S.pws.ensure(sort_ws + agg_ws + refine_ws + join_ws + join_own_ws))) return rc;
   uint8_t* ws = (uint8_t*)S.pws.p;
   uint8_t* rws = refine ? ws + sort_ws + agg_ws : nullptr;
+  uint8_t* gws = ws + sort_ws + agg_ws + refine_ws;  // a join's grouping workspace, then its own
+  uint8_t* jws = gws + join_ws;
   CU(S.mark(F2, st, *launches));
   launch_rows_emit(arena, *total, n_src, fws, records, key_bytes, ws, st, launches);
   CU(S.mark(F3, st, *launches));
-  const uint32_t* idx = launch_rows_order(arena, records, ks, rows_frame_ranges(fws, *total, n_src), n_src, ws, rws,
-                                          st, launches);
+  const uint64_t* ranges = rows_frame_ranges(fws, *total, n_src);
+  const uint32_t* idx =
+      spec.join ? launch_rows_join_order(arena, records, jk, ranges, n_src, join_readback(jws, records, n_src) + 4, ws,
+                                         rws, st, launches)
+                : launch_rows_order(arena, records, ks, ranges, n_src, ws, rws, st, launches);
   const uint32_t* heads = nullptr;
   if (refine && records) {
     // one readback per round: the tied records and their runs (the first also brings the string verdicts)
@@ -3307,10 +3415,45 @@ static int decompress_sort_run(Device* D, Slot& S, uint32_t codec, uint32_t alg,
       }
       const uint64_t tied = rrb[0] & 0xffffffffull, runs = rrb[0] >> 32;
       if (!tied) break;
-      launch_rows_refine_round(arena, records, ks, tied, runs, d, ws, rws, n_src, st, launches);
+      if (spec.join) launch_rows_join_refine_round(arena, records, jk, tied, runs, d, ws, rws, st, launches);
+      else launch_rows_refine_round(arena, records, ks, tied, runs, d, ws, rws, n_src, st, launches);
     }
     idx = rows_refine_order(rws, records, n_src);
     heads = rows_refine_heads(rws, records, n_src);
+  }
+  if (spec.join) {  // the join step: grouping, counts (one readback with the key pass's verdicts), emit
+    std::vector<uint64_t> jb(4 + n_src, ~0ull);
+    jb[0] = jb[1] = jb[2] = jb[3] = 0;
+    CU(S.mark(G0, st, *launches));
+    if (records) {
+      launch_rows_group(arena, records, idx, heads, key_bytes, AggSpec{}, ws, gws, st, launches);
+      launch_join_count(arena, records, idx, shape, join_fields.data(), (uint32_t)join_fields.size(), key_bytes, ws,
+                        gws, jws, n_src, st, launches);
+      CU(cudaMemcpyAsync(jb.data(), join_readback(jws, records, n_src), join_readback_bytes(n_src),
+                         cudaMemcpyDeviceToHost, st));
+      CU(cudaStreamSynchronize(st));
+      CU(cudaGetLastError());
+    }
+    take_verdicts(jb.data() + 4);
+    if (failed) return report();
+    if (jb[3]) return fail(B2S_E_UNSUPPORTED, "a joined row is longer than 2^31 - 1 bytes%s");
+    *total = jb[1];
+    if (jb[1] > out_cap)
+      return fail(B2S_E_DST_TOO_SMALL, "dst_cap is below the %s output bytes", std::to_string(jb[1]).c_str());
+    if (!*d_sorted) {
+      if ((rc = S.parena.ensure(jb[1] + 64))) return rc;
+      *d_sorted = (uint8_t*)S.parena.p;
+    }
+    launch_join_emit(arena, records, idx, jb[0], key_bytes, spec.join->type >= B2S_JOIN_LEFT_SEMI, ws, jws, n_src,
+                     *d_sorted, st, launches);
+    CU(S.mark(G1, st, *launches));
+    CU(S.mark(P1, st));
+    CU(cudaStreamSynchronize(st));
+    CU(cudaGetLastError());
+    *n_rec = jb[0];
+    *spec.join->n_side[0] = jb[2];
+    *spec.join->n_side[1] = records - jb[2];
+    return 0;
   }
   if (spec.aggregate) {
     uint64_t bad = ~0ull;
@@ -3665,6 +3808,71 @@ int b2s_decompress_aggregate_rows_keys_dev(uint32_t dev_index, uint32_t codec, u
                         with_aggregates(keys_spec(n_keys, key_type, key_off, key_len, key_null_field), n_aggs, agg_op,
                                         agg_off, agg_null_field),
                         dst_base, dst_cap, dst_total, n_records, n_groups, status, bad_slice);
+}
+
+// The join calls: the composite-key row sort's call over both sides, with the join's outputs zeroed first; every
+// count and *dst_total are 0 when a block failed (nothing is written).
+static int join_call(uint32_t dev_index, bool packed, uint32_t join_type, uint32_t codec, uint32_t alg,
+                     uint32_t n_left, uint32_t n, const uint8_t* src_base, const uint64_t* src_off,
+                     const uint64_t* src_len, const uint32_t* slice_base, const uint64_t* slice_len,
+                     const uint64_t* slice_checksum, uint32_t n_keys, const uint32_t* key_type, const uint32_t* key_len,
+                     const uint32_t* left_key_off, const int32_t* left_key_null_field, const uint32_t* right_key_off,
+                     const int32_t* right_key_null_field, uint32_t n_left_fields, const uint8_t* left_field_kind,
+                     uint32_t n_right_fields, const uint8_t* right_field_kind, uint8_t* dst_base, uint64_t dst_cap,
+                     uint64_t* dst_total, uint64_t* n_left_records, uint64_t* n_right_records,
+                     uint64_t* n_out_records, int32_t* status, int32_t* bad_slice) {
+  if (n_left_records) *n_left_records = 0;
+  if (n_right_records) *n_right_records = 0;
+  JoinSpec js;
+  js.type = join_type;
+  js.n_left = n_left;
+  const RecordSpec right = keys_spec(n_keys, key_type, right_key_off, key_len, right_key_null_field);
+  js.right = right.keys;
+  js.right_arrays = right.key_arrays;
+  js.n_fields[0] = n_left_fields;
+  js.n_fields[1] = n_right_fields;
+  js.kind[0] = left_field_kind;
+  js.kind[1] = right_field_kind;
+  js.n_side[0] = n_left_records;
+  js.n_side[1] = n_right_records;
+  RecordSpec spec = keys_spec(n_keys, key_type, left_key_off, key_len, left_key_null_field);
+  spec.join = &js;
+  const int rc = sort_call(dev_index, packed, nullptr, codec, alg, n, src_base, src_off, src_len, slice_base, slice_len,
+                           slice_checksum, spec, dst_base, dst_cap, dst_total, n_out_records, status, bad_slice);
+  if (!rc && !*n_out_records) *dst_total = 0;
+  return rc;
+}
+
+int b2s_decompress_join_rows_keys_packed(
+    uint32_t join_type, uint32_t codec, uint32_t checksum_alg, uint32_t n_left, uint32_t n, const uint8_t* src_base,
+    const uint64_t* src_off, const uint64_t* src_len, const uint32_t* slice_base, const uint64_t* slice_len,
+    const uint64_t* slice_checksum, uint32_t n_keys, const uint32_t* key_type, const uint32_t* key_len,
+    const uint32_t* left_key_off, const int32_t* left_key_null_field, const uint32_t* right_key_off,
+    const int32_t* right_key_null_field, uint32_t n_left_fields, const uint8_t* left_field_kind,
+    uint32_t n_right_fields, const uint8_t* right_field_kind, uint8_t* dst_base, uint64_t dst_cap,
+    uint64_t* dst_total, uint64_t* n_left_records, uint64_t* n_right_records, uint64_t* n_out_records, int32_t* status,
+    int32_t* bad_slice) {
+  return join_call(t_device, true, join_type, codec, checksum_alg, n_left, n, src_base, src_off, src_len, slice_base,
+                   slice_len, slice_checksum, n_keys, key_type, key_len, left_key_off, left_key_null_field,
+                   right_key_off, right_key_null_field, n_left_fields, left_field_kind, n_right_fields,
+                   right_field_kind, dst_base, dst_cap, dst_total, n_left_records, n_right_records, n_out_records,
+                   status, bad_slice);
+}
+
+int b2s_decompress_join_rows_keys_dev(
+    uint32_t dev_index, uint32_t join_type, uint32_t codec, uint32_t checksum_alg, uint32_t n_left, uint32_t n,
+    const uint8_t* src_base, const uint64_t* src_off, const uint64_t* src_len, const uint32_t* slice_base,
+    const uint64_t* slice_len, const uint64_t* slice_checksum, uint32_t n_keys, const uint32_t* key_type,
+    const uint32_t* key_len, const uint32_t* left_key_off, const int32_t* left_key_null_field,
+    const uint32_t* right_key_off, const int32_t* right_key_null_field, uint32_t n_left_fields,
+    const uint8_t* left_field_kind, uint32_t n_right_fields, const uint8_t* right_field_kind, uint8_t* dst_base,
+    uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_left_records, uint64_t* n_right_records,
+    uint64_t* n_out_records, int32_t* status, int32_t* bad_slice) {
+  return join_call(dev_index, false, join_type, codec, checksum_alg, n_left, n, src_base, src_off, src_len, slice_base,
+                   slice_len, slice_checksum, n_keys, key_type, key_len, left_key_off, left_key_null_field,
+                   right_key_off, right_key_null_field, n_left_fields, left_field_kind, n_right_fields,
+                   right_field_kind, dst_base, dst_cap, dst_total, n_left_records, n_right_records, n_out_records,
+                   status, bad_slice);
 }
 
 // ------------------------------------------------------------------------------------------------------------

@@ -281,6 +281,9 @@ void launch_rows_frame(const uint8_t* arena, uint64_t arena_bytes, const uint64_
 // complements every value byte of the column (a string's markers included): the column's code stays prefix-free and
 // its order reverses.
 constexpr uint32_t kMaxKeys = 16;
+// a join's key column that is never null on its side but nullable on the other: it encodes the null byte of a non-null
+// value, so that equal keys of the two sides encode equal (rows_key.cuh, encode_key<true>)
+constexpr int32_t kNullByteOnly = -2;
 constexpr uint32_t kStringKey = B2S_STRING_KEY, kDecimalKey = B2S_DECIMAL_KEY;
 constexpr uint32_t kKeyTypeMask = 0xff;
 // the encoded value bytes of a fixed-width column of type ty (low 8 bits) and key_len len: a decimal's 16, else len
@@ -301,7 +304,7 @@ inline uint32_t rows_key_encoded_bytes(const KeySpec& ks) {
   for (uint32_t c = 0; c < ks.n; c++) {
     const uint32_t ty = ks.type[c] & kKeyTypeMask;
     if (ty == kStringKey) return ~0u;
-    b += key_value_bytes(ty, ks.len[c]) + (ks.null_field[c] >= 0 ? 1 : 0);
+    b += key_value_bytes(ty, ks.len[c]) + (ks.null_field[c] != -1 ? 1 : 0);
   }
   return b;
 }
@@ -360,9 +363,27 @@ void launch_rows_whole_order(uint64_t n, uint8_t* d_ws, uint8_t* d_rws, cudaStre
 void launch_rows_whole_refine_round(const uint8_t* rec, const uint64_t* rec_off, const uint32_t* rec_len, uint64_t n,
                                     uint64_t m, uint64_t segs, uint32_t d, uint8_t* d_ws, uint8_t* d_rws,
                                     cudaStream_t st, uint64_t* launches);
-// the emitted records to d_dst in the order idx
+// A join's key pass (two row layouts in one sort): record i is a left record when its arena offset is below split (the
+// left blocks come first, so the left records are a prefix), else a right one, and it is keyed with its side's columns
+// side[0] / side[1] (encoded to equal widths: a column nullable on one side only has kNullByteOnly on the other).  A
+// row shorter than its side's fixed region fixed[s] lowers its range's verdict (verdict[r], as rows_keys_kernel's) with
+// kRowsBadKey; a bad string or decimal with kRowsBadString.  Such a record gets key length 0 (never refined).
+struct JoinKeys {
+  KeySpec side[2];
+  uint64_t split;
+  uint32_t fixed[2];
+};
+// launch_rows_order for a join: the same workspaces and order, the key words from each record's side; verdict
+// (n_ranges words, device) is reset here
+const uint32_t* launch_rows_join_order(const uint8_t* arena, uint64_t n, const JoinKeys& jk, const uint64_t* ranges,
+                                       uint32_t n_ranges, uint64_t* verdict, uint8_t* d_ws, uint8_t* d_rws,
+                                       cudaStream_t st, uint64_t* launches);
+// launch_rows_refine_round for a join's keys
+void launch_rows_join_refine_round(const uint8_t* arena, uint64_t n, const JoinKeys& jk, uint64_t m, uint64_t segs,
+                                   uint32_t d, uint8_t* d_ws, uint8_t* d_rws, cudaStream_t st, uint64_t* launches);
+// the emitted records to d_dst in the order idx; count (below n): only the records idx[0 .. count), a subset
 void launch_rows_gather(const uint8_t* arena, uint64_t n, uint32_t key_bytes, const uint32_t* idx, uint8_t* d_ws,
-                        uint8_t* d_dst, cudaStream_t st, uint64_t* launches);
+                        uint8_t* d_dst, cudaStream_t st, uint64_t* launches, uint64_t count = ~0ull);
 
 // ---------------- rows_hash.cu (Spark's HashPartitioning ids of length-prefixed UnsafeRow records) ----------------
 // Record i: rec_len[i] bytes at rec + rec_off[i], [size: int32 big-endian][row].  ids[i] = pmod(Murmur3Hash(key
@@ -453,6 +474,46 @@ void launch_rows_group(const uint8_t* arena, uint64_t n, const uint32_t* idx, co
 // replaced by the merged values
 void launch_rows_aggregate(const uint8_t* arena, uint64_t n, uint64_t groups, uint32_t key_bytes, const AggSpec& spec,
                            uint8_t* d_ws, uint8_t* d_aws, uint8_t* d_dst, cudaStream_t st, uint64_t* launches);
+
+// after launch_rows_group: per sorted position the number of group heads before it (a head's group index), and per
+// group its first position (n after the last group)
+const uint64_t* rows_group_heads_before(uint8_t* d_aws, uint64_t n);
+const uint32_t* rows_group_starts(uint8_t* d_aws, uint64_t n);
+
+// ---------------- join.cu (sort-merge join of a reducer's two sorted sides into Spark's joined UnsafeRows) -----------
+// The records of both sides, stably sorted together by the join key (launch_rows_join_order) and grouped
+// (launch_rows_group): each group holds its key's left records, then its right ones.  The shape of the joined row:
+// field counts n[s], null-bitset words bw[s] and out_bw of the inputs and the output, and the non-fixed fields (VAR and
+// DECIMAL_WIDE: their slots' offsets move) of each side, and the right side's DECIMAL_WIDE fields (the null right
+// side's 16-byte regions), as device lists.
+constexpr uint32_t kJoinInner = B2S_JOIN_INNER, kJoinLeftOuter = B2S_JOIN_LEFT_OUTER,
+                   kJoinLeftSemi = B2S_JOIN_LEFT_SEMI, kJoinLeftAnti = B2S_JOIN_LEFT_ANTI;
+struct JoinShape {
+  uint32_t type;
+  uint64_t split;      // the arena offset of the first right record (JoinKeys::split)
+  uint32_t n[2], bw[2], out_bw;
+  uint32_t n_var[2], n_wide_right;
+  const uint32_t* var[2];
+  const uint32_t* wide_right;
+  KeySpec left_keys;   // the left side's key columns (a left record's null columns)
+};
+// d_jws: join_ws_bytes(n, n_ranges, n_fields) bytes; launch_join_count uploads the shape and its field lists (h_fields:
+// the left's non-fixed fields, the right's, the right's DECIMAL_WIDE ones)
+size_t join_ws_bytes(uint64_t n, uint32_t n_ranges, uint32_t n_fields);
+// the readback: [output records, output bytes, left records, a joined row is too long (0 / 1), verdict of range 0, 1,
+// ...] (the verdicts: launch_rows_join_order's)
+uint64_t* join_readback(uint8_t* d_jws, uint64_t n, uint32_t n_ranges);
+inline size_t join_readback_bytes(uint32_t n_ranges) { return (4 + (size_t)n_ranges) * 8; }
+// per left position its output records and bytes, scanned; the totals and the left record count into the readback
+// (its first four words).  idx: the sorted order (nullptr: arena order), heads as launch_rows_group's.
+void launch_join_count(const uint8_t* arena, uint64_t n, const uint32_t* idx, JoinShape shape,
+                       const uint32_t* h_fields, uint32_t n_fields, uint32_t key_bytes, uint8_t* d_ws,
+                       uint8_t* d_aws, uint8_t* d_jws, uint32_t n_ranges, cudaStream_t st, uint64_t* launches);
+// the out_rows joined records (read back) to d_dst, a warp per record; whole (semi and anti joins): the kept left
+// records, compacted and gathered by launch_rows_gather
+void launch_join_emit(const uint8_t* arena, uint64_t n, const uint32_t* idx, uint64_t out_rows, uint32_t key_bytes,
+                      bool whole, uint8_t* d_ws, uint8_t* d_jws, uint32_t n_ranges, uint8_t* d_dst, cudaStream_t st,
+                      uint64_t* launches);
 
 // ---------------- exchange.cu (exchange-cache reads: ranges of device memory gathered into one arena) ----------------
 // piece: len bytes at src (device pointer, any alignment) go to d_dst + dst

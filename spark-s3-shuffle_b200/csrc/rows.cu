@@ -264,6 +264,43 @@ __global__ void __launch_bounds__(kRowThreads, 8) rows_keys_kernel(
   }
 }
 
+// The join's key pass (kernels.h, JoinKeys): rows_keys_kernel with each record's side's columns and its fixed-region
+// check.  A kernel of its own, so that the single-spec sorts keep theirs.
+__global__ void __launch_bounds__(kRowThreads) rows_join_keys_kernel(
+    const uint8_t* __restrict__ arena, const uint64_t* __restrict__ rec_off, const uint32_t* __restrict__ rec_len,
+    uint64_t n, const __grid_constant__ JoinKeys jk, uint32_t key_bytes, uint32_t* __restrict__ words,
+    uint32_t* __restrict__ klen, const uint64_t* __restrict__ ranges, uint32_t n_ranges,
+    uint64_t* __restrict__ verdict) {
+  const uint32_t W = (key_bytes + 3) / 4;
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+    const uint64_t ro = rec_off[i];
+    const uint32_t s = ro >= jk.split, size = rec_len[i] - 4;
+    KeyWindow kw{0, 0, 0, 0, 0, 0, key_bytes};
+    bool bad = false;
+    uint32_t len = 0;
+    uint64_t why = 0;
+    if (size < jk.fixed[s]) {  // its key slots and null words are not all inside it: not read
+      why = kRowsBadKey;
+    } else {
+      len = encode_key<true>(arena + ro + 4, size, jk.side[s], kw, klen != nullptr, &bad);
+      if (bad) why = kRowsBadString;
+    }
+#pragma unroll
+    for (uint32_t k = 0; k < 5; k++)
+      if (k < W) words[(size_t)k * n + i] = kw.word(k);
+    if (klen) klen[i] = why ? 0 : len;
+    if (why) {  // the range holding the record: the last that starts at or before it
+      uint32_t lo = 0, hi = n_ranges;
+      while (hi - lo > 1) {
+        const uint32_t mid = (lo + hi) / 2;
+        if (ranges[mid] <= ro) lo = mid;
+        else hi = mid;
+      }
+      atomicMin((unsigned long long*)(verdict + lo), (unsigned long long)((why << 61) | (ro - ranges[lo])));
+    }
+  }
+}
+
 // ---- refinement (keys longer than the first pass: kernels.h, launch_rows_refine_*) ----
 // ord[j] = the record at position j of the current order, head[j] = 1 where a new key (so far) starts
 __global__ void __launch_bounds__(kRowThreads) refine_init_kernel(const uint32_t* __restrict__ idx, uint64_t n,
@@ -316,6 +353,29 @@ __global__ void __launch_bounds__(kRowThreads) refine_extract_kernel(
     KeyWindow kw{0, 0, 0, 0, 0, d, kKeyChunkBytes};
     bool bad = false;
     encode_key(arena + rec_off[i] + 4, rec_len[i] - 4, ks, kw, false, &bad);
+    words[k] = s;
+#pragma unroll
+    for (uint32_t q = 0; q < 4; q++) words[(size_t)(q + 1) * m + k] = kw.word(q);
+  }
+}
+
+// refine_extract_kernel for a join's keys: each record with its side's columns (a bad record has key length 0: never
+// tied, never read here)
+__global__ void __launch_bounds__(kRowThreads) refine_extract_join_kernel(
+    const uint8_t* __restrict__ arena, const uint64_t* __restrict__ rec_off, const uint32_t* __restrict__ rec_len,
+    uint64_t n, const __grid_constant__ JoinKeys jk, const uint32_t* __restrict__ ord,
+    const uint32_t* __restrict__ head, const uint32_t* __restrict__ klen, const uint64_t* __restrict__ scan, uint64_t m,
+    uint32_t d,
+    uint32_t* __restrict__ cpos, uint32_t* __restrict__ cidx, uint32_t* __restrict__ words) {
+  for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (uint64_t)gridDim.x * blockDim.x) {
+    if (!tied(j, n, d, ord, head, klen)) continue;
+    const uint32_t k = (uint32_t)scan[j], s = (uint32_t)(scan[j] >> 32) + head[j] - 1;
+    const uint32_t i = ord[j];
+    cpos[k] = (uint32_t)j;
+    cidx[k] = i;
+    KeyWindow kw{0, 0, 0, 0, 0, d, kKeyChunkBytes};
+    bool bad = false;
+    encode_key<true>(arena + rec_off[i] + 4, rec_len[i] - 4, jk.side[rec_off[i] >= jk.split], kw, false, &bad);
     words[k] = s;
 #pragma unroll
     for (uint32_t q = 0; q < 4; q++) words[(size_t)(q + 1) * m + k] = kw.word(q);
@@ -542,6 +602,39 @@ const uint32_t* launch_rows_order(const uint8_t* arena, uint64_t n, const KeySpe
   return idx;
 }
 
+const uint32_t* launch_rows_join_order(const uint8_t* arena, uint64_t n, const JoinKeys& jk, const uint64_t* ranges,
+                                       uint32_t n_ranges, uint64_t* verdict, uint8_t* d_ws, uint8_t* d_rws,
+                                       cudaStream_t st, uint64_t* launches) {
+  cudaMemsetAsync(verdict, 0xff, (size_t)n_ranges * 8, st);
+  if (!n) return nullptr;
+  const uint32_t key_bytes = rows_key_bytes(jk.side[0]);
+  const KeySortWs w = carve_key_sort_ws(d_ws, n, key_bytes);
+  RefineWs r{};
+  if (d_rws) {  // the verdicts are the join's: the refinement's first readback finds none
+    r = carve_refine_ws(d_rws, n);
+    cudaMemsetAsync(r.readback + 1, 0xff, (size_t)n_ranges * 8, st);
+  }
+  rows_join_keys_kernel<<<grid_for(n), kRowThreads, 0, st>>>(arena, w.src_off, w.len, n, jk, key_bytes, w.words, r.klen,
+                                                             ranges, n_ranges, verdict);
+  if (launches) *launches += 1;
+  const uint32_t* idx = launch_key_radix(w, n, key_bytes, st, launches);
+  if (d_rws) {
+    refine_init_kernel<<<grid_for(n), kRowThreads, 0, st>>>(idx, n, w.words, (key_bytes + 3) / 4, r.ord, r.head);
+    if (launches) *launches += 1;
+  }
+  return idx;
+}
+
+void launch_rows_join_refine_round(const uint8_t* arena, uint64_t n, const JoinKeys& jk, uint64_t m, uint64_t segs,
+                                   uint32_t d, uint8_t* d_ws, uint8_t* d_rws, cudaStream_t st, uint64_t* launches) {
+  const KeySortWs w = carve_key_sort_ws(d_ws, n, kKeyPrefixBytes);
+  const RefineWs r = carve_refine_ws(d_rws, n);
+  refine_extract_join_kernel<<<grid_for(n), kRowThreads, 0, st>>>(arena, w.src_off, w.len, n, jk, r.ord, r.head,
+                                                                  r.klen, r.scan, m, d, r.cpos, r.cidx, w.words);
+  refine_sort_scatter(w, r, m, segs, st, launches);
+  if (launches) *launches += 2;
+}
+
 void launch_rows_refine_mark(uint64_t n, uint32_t d, uint8_t* d_rws, uint32_t, cudaStream_t st, uint64_t* launches) {
   const RefineWs r = carve_refine_ws(d_rws, n);
   refine_mark_kernel<<<grid_for(n), kRowThreads, 0, st>>>(r.ord, r.head, r.klen, n, d, r.scan);
@@ -585,16 +678,17 @@ void launch_rows_whole_refine_round(const uint8_t* rec, const uint64_t* rec_off,
 }
 
 void launch_rows_gather(const uint8_t* arena, uint64_t n, uint32_t key_bytes, const uint32_t* idx, uint8_t* d_ws,
-                        uint8_t* d_dst, cudaStream_t st, uint64_t* launches) {
-  if (!n) return;
+                        uint8_t* d_dst, cudaStream_t st, uint64_t* launches, uint64_t count) {
+  const uint64_t m = count < n ? count : n;
+  if (!m) return;
   const KeySortWs w = carve_key_sort_ws(d_ws, n, key_bytes);
   uint64_t* offsets_scan_ws = (uint64_t*)(d_ws + key_sort_ws_bytes(n, key_bytes));
   PartitionPlan plan;
   plan.src_off = w.src_off;
   plan.sdst = w.sdst;
   plan.idx = idx;
-  launch_sorted_offsets(plan.idx, w.len, n, w.sdst, w.total, offsets_scan_ws, st, launches);
-  launch_partition_gather(arena, w.len, n, plan, d_dst, st, launches);
+  launch_sorted_offsets(plan.idx, w.len, m, w.sdst, w.total, offsets_scan_ws, st, launches);
+  launch_partition_gather(arena, w.len, m, plan, d_dst, st, launches);
 }
 
 }  // namespace b2s

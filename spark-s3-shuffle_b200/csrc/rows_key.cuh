@@ -76,7 +76,9 @@ __device__ __forceinline__ void decimal_bits(const uint8_t* row, uint32_t row_si
 // The window kw of the encoded key of a row of row_size bytes.  whole: every column is walked and the return value is
 // the key's encoded length (else the walk stops at the window's end); every non-null decimal slot is then checked.
 // *bad: a non-null string slot runs past the row, or a decimal slot is bad (decimal_bits); the bytes read are then
-// clamped to the row, so no load leaves it.
+// clamped to the row, so no load leaves it.  Join (the join's key pass): a column whose null_field is kNullByteOnly
+// takes the null byte of a non-null value without reading a null word (its other side's column is nullable).
+template <bool Join = false>
 __device__ __forceinline__ uint32_t encode_key(const uint8_t* row, uint32_t row_size, const KeySpec& ks, KeyWindow& kw,
                                                bool whole, bool* bad) {
   const uint32_t wend = kw.d + kw.nb;
@@ -92,6 +94,8 @@ __device__ __forceinline__ uint32_t encode_key(const uint8_t* row, uint32_t row_
       ld_span16<true>(row + 8 * (uint32_t)(nf >> 6), 8, nw, unused);
       is_null = (nw >> (nf & 63)) & 1;
       kw.put(p++, is_null == ((ks.type[c] & B2S_KEY_NULLS_LAST) != 0) ? 1 : 0);
+    } else if (Join && nf == kNullByteOnly) {
+      kw.put(p++, 1);
     }
     if (ty == kStringKey) {
       if (is_null) continue;

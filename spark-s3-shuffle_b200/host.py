@@ -7,7 +7,7 @@ import ctypes as C
 import numpy as np
 
 from . import _build
-from .capi import _agg_arrays, _arg, _key_arrays
+from .capi import _agg_arrays, _arg, _join_arrays, _key_arrays
 
 OK, E_RUNTIME, E_IO, E_SPARK, E_UNSUPPORTED, E_CODEC = 0, -101, -102, -103, -104, -105
 
@@ -72,6 +72,9 @@ PROTOTYPES = [
     ("b2sh_reader_read_aggregated_rows_keys", C.c_int,
      [_vp, _u32, _vp, _vp, _vp, _vp, _u32, _vp, _vp, _vp, C.POINTER(_vp), C.POINTER(_u64), C.POINTER(_u64),
       C.POINTER(_u64)]),
+    ("b2sh_reader_read_joined_rows", C.c_int,
+     [_vp, _vp, _u32, _u32, _vp, _vp, _vp, _vp, _vp, _vp, _u32, _vp, _u32, _vp, C.POINTER(_vp), C.POINTER(_u64),
+      C.POINTER(_u64), C.POINTER(_u64), C.POINTER(_u64)]),
     ("b2sh_reader_block", C.c_int,
      [_vp, _u32, C.POINTER(_i64), C.POINTER(_i32), C.POINTER(_i32), C.POINTER(_vp), C.POINTER(_u64)]),
     ("b2sh_reader_remote_bytes_read", _u64, [_vp]),
@@ -398,6 +401,19 @@ class S3ShuffleReader:
         -> (bytes, number of input records, number of groups)"""
         return _read_sorted(self._h, load().b2sh_reader_read_aggregated_rows_keys, *_key_arrays(keys),
                             *_agg_arrays(aggs), groups=True)
+
+    def readJoinedRows(self, right, joinType, leftKeys, rightKeys, nLeftFields, nRightFields, leftKinds=None,
+                       rightKinds=None):
+        """Spark's sort-merge join of this reader's partitions (the left side) with right's (the same partitions of
+        another shuffle): both readers' blocks through ONE capi.decompress_join_rows_keys_packed call, whose arguments
+        these are.  -> (joined rows, n_left_records, n_right_records, n_out_records)"""
+        n, kt, kl, lo, ln, ro, rn, lk, rk = _join_arrays(leftKeys, rightKeys, leftKinds, rightKinds)
+        p, size = _vp(), _u64()
+        counts = [_u64(), _u64(), _u64()]
+        _check(load().b2sh_reader_read_joined_rows(self._h, right._h, joinType, n, *map(_arg, (kt, kl, lo, ln, ro, rn)),
+                                                   nLeftFields, _arg(lk), nRightFields, _arg(rk), C.byref(p),
+                                                   C.byref(size), *map(C.byref, counts)))
+        return ((C.string_at(p.value, size.value) if size.value else b""),) + tuple(c.value for c in counts)
 
     def _blocks(self, n):
         out = []

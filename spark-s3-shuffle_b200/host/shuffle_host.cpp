@@ -777,21 +777,30 @@ using FetchedBlock = std::pair<uint64_t, std::vector<uint8_t>>;
 // source's offset and length there, and its checksum slices (source k's are [sliceBase[k], sliceBase[k + 1])).  A null
 // source, the place of a map the exchange cache serves, stages as no bytes and no slices.
 struct StagedBlocks {
-  StagedBlocks(const std::vector<ShuffleBlockInfo>& info, const std::vector<const FetchedBlock*>& sources) {
-    for (const FetchedBlock* f : sources) {
-      off.push_back(bytes);
-      len.push_back(f ? f->second.size() : 0);
-      bytes += len.back();
-      if (f) {
-        const ShuffleBlockInfo& bi = info[f->first];
-        sliceLen.insert(sliceLen.end(), bi.sliceLen.begin(), bi.sliceLen.end());
-        sliceSum.insert(sliceSum.end(), bi.sliceSum.begin(), bi.sliceSum.end());
+  using Side = std::pair<const std::vector<ShuffleBlockInfo>*, const std::vector<const FetchedBlock*>*>;
+  StagedBlocks(const std::vector<ShuffleBlockInfo>& info, const std::vector<const FetchedBlock*>& sources)
+      : StagedBlocks({Side{&info, &sources}}) {}
+  // the sources of several readers back to back, each with its reader's block info
+  explicit StagedBlocks(std::initializer_list<Side> sides) {
+    for (const Side& side : sides)
+      for (const FetchedBlock* f : *side.second) {
+        off.push_back(bytes);
+        len.push_back(f ? f->second.size() : 0);
+        bytes += len.back();
+        if (f) {
+          const ShuffleBlockInfo& bi = (*side.first)[f->first];
+          sliceLen.insert(sliceLen.end(), bi.sliceLen.begin(), bi.sliceLen.end());
+          sliceSum.insert(sliceSum.end(), bi.sliceSum.begin(), bi.sliceSum.end());
+        }
+        sliceBase.push_back((uint32_t)sliceLen.size());
       }
-      sliceBase.push_back((uint32_t)sliceLen.size());
-    }
     src.resize(bytes ? bytes : 1);
-    for (size_t k = 0; k < sources.size(); k++)
-      if (sources[k]) memcpy(src.data() + off[k], sources[k]->second.data(), (size_t)len[k]);
+    size_t k = 0;
+    for (const Side& side : sides)
+      for (const FetchedBlock* f : *side.second) {
+        if (f) memcpy(src.data() + off[k], f->second.data(), (size_t)len[k]);
+        k++;
+      }
   }
   PinnedArena src;
   uint64_t bytes = 0;
@@ -1035,6 +1044,62 @@ class S3ShuffleReader {
                                              keys.len[0], keys.nullField[0], sorted_.get(), cap, total, records,
                                              x.status, x.bad);
     });
+  }
+  // The join's arguments (b2s_decompress_join_rows_keys_packed): its type, the key columns' types and lengths, each
+  // side's key slots and null bits, field counts and field kinds.
+  struct JoinArgs {
+    uint32_t type, nKeys;
+    const uint32_t *keyType, *keyLen, *leftOff;
+    const int32_t* leftNull;
+    const uint32_t* rightOff;
+    const int32_t* rightNull;
+    uint32_t nLeftFields;
+    const uint8_t* leftKind;
+    uint32_t nRightFields;
+    const uint8_t* rightKind;
+  };
+  // read() for the left (streamed) side of a sort-merge join whose right (buffered) side `right` reads
+  // (INTEGRATION.md §3n): both readers' non-empty blocks are fetched (the exchange cache is not consulted), each in
+  // computeShuffleBlocks order, and staged left first; then ONE b2s_decompress_join_rows_keys_packed call verifies,
+  // decodes, sorts and joins them, retried once with the exact size when its first guess is too small.  The joined rows
+  // stay in this reader as a sorted read's records do; sortedRecords() is the number of output rows.
+  void readJoined(S3ShuffleReader& right, const JoinArgs& j, uint64_t* nLeft, uint64_t* nRight) {
+    std::vector<FetchedBlock> lf, rf;
+    fetchAll(lf);
+    right.fetchAll(rf);
+    std::vector<const FetchedBlock*> ls, rs;
+    for (const auto& f : lf)
+      if (!f.second.empty()) ls.push_back(&f);
+    for (const auto& f : rf)
+      if (!f.second.empty()) rs.push_back(&f);
+    const uint32_t alg = d_.checksumEnabled ? S3ShuffleHelper::createChecksumAlgorithm(d_.checksumAlgorithm) : 0;
+    ensure_codec_runtime();
+    const uint32_t codec = (uint32_t)d_.codecId();
+    StagedBlocks src({StagedBlocks::Side{&info_, &ls}, StagedBlocks::Side{&right.info_, &rs}});
+    const uint32_t nl = (uint32_t)ls.size(), n = nl + (uint32_t)rs.size();
+    std::vector<int32_t> status(n), bad(n);
+    uint64_t total = 0, out = 0;
+    const uint64_t guess = codec == B2S_CODEC_NONE ? src.bytes : src.bytes * 4;
+    const int rc = callWithRetry(sorted_, guess, total, [&](uint64_t cap) {
+      return b2s_decompress_join_rows_keys_packed(
+          j.type, codec, alg, nl, n, src.src.data(), src.off.data(), src.len.data(), alg ? src.sliceBase.data() : 0,
+          alg ? src.sliceLen.data() : 0, alg ? src.sliceSum.data() : 0, j.nKeys, j.keyType, j.keyLen, j.leftOff,
+          j.leftNull, j.rightOff, j.rightNull, j.nLeftFields, j.leftKind, j.nRightFields, j.rightKind, sorted_.get(),
+          cap, &total, nLeft, nRight, &out, status.data(), bad.data());
+    });
+    if (rc != 0)
+      throw CodecException(std::string("b2s_decompress_join_rows_keys_packed: ") + b2s_strerror(rc) + ": " +
+                           b2s_last_error());
+    for (uint32_t k = 0; k < n; k++)
+      throwBlockStatus(status[k], k < nl ? info_[ls[k]->first].id : right.info_[rs[k - nl]->first].id);
+    sortedLen_ = total;
+    sortedRecords_ = out;
+  }
+  // every block of the task, fetched whole, in computeShuffleBlocks order
+  void fetchAll(std::vector<FetchedBlock>& fetched) {
+    start(true);
+    drainWhole(fetched);
+    std::sort(fetched.begin(), fetched.end(), [](const auto& a, const auto& b) { return a.first < b.first; });
   }
   const uint8_t* sortedData() const { return sorted_.get(); }
   uint64_t sortedLen() const { return sortedLen_; }
@@ -1468,6 +1533,21 @@ int b2sh_reader_read_aggregated_rows_keys(b2sh_reader* r, uint32_t n_keys, const
     const S3ShuffleReader::RowAggregates aggs{n_aggs, agg_op, agg_off, agg_null_field};
     r->r->readRows(S3ShuffleReader::RowKeys{n_keys, key_type, key_off, key_len, key_null_field, true}, &aggs);
     sorted_result(*r->r, data, len, n_records, n_groups);
+  });
+}
+int b2sh_reader_read_joined_rows(b2sh_reader* left, b2sh_reader* right, uint32_t join_type, uint32_t n_keys,
+                                 const uint32_t* key_type, const uint32_t* key_len, const uint32_t* left_key_off,
+                                 const int32_t* left_key_null_field, const uint32_t* right_key_off,
+                                 const int32_t* right_key_null_field, uint32_t n_left_fields,
+                                 const uint8_t* left_field_kind, uint32_t n_right_fields,
+                                 const uint8_t* right_field_kind, const uint8_t** data, uint64_t* len,
+                                 uint64_t* n_left_records, uint64_t* n_right_records, uint64_t* n_out_records) {
+  return guarded([&] {
+    const S3ShuffleReader::JoinArgs j{join_type,     n_keys,         key_type,        key_len,
+                                      left_key_off,  left_key_null_field, right_key_off, right_key_null_field,
+                                      n_left_fields, left_field_kind, n_right_fields,  right_field_kind};
+    left->r->readJoined(*right->r, j, n_left_records, n_right_records);
+    sorted_result(*left->r, data, len, n_out_records);
   });
 }
 int b2sh_reader_block(b2sh_reader* r, uint32_t k, int64_t* map_id, int32_t* start_reduce, int32_t* end_reduce,
