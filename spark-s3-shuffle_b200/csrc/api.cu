@@ -3104,37 +3104,283 @@ struct SortSource {
   uint64_t first_off = 0, n_rec = 0;
 };
 
-// The end of an aggregation (b2s_decompress_aggregate_rows_*), from the sorted indices idx of the records: grouping,
-// one readback of the group count, output bytes and decimal verdict (which checks out_cap), the heads' gather and the
-// merge into d_out.  *total = output bytes.  *bad: the verdict of the out-of-line decimals' checks (kernels.h,
-// kAggBad*); when it is not ~0 nothing is written.  The dominant step is this one (marks G0, G1).
-static int aggregate_rows_tail(Slot& S, const RecordSpec& spec, const uint8_t* arena, uint64_t records,
-                               const uint32_t* idx, const uint32_t* heads, uint8_t* ws, uint8_t* aws, uint8_t* d_out,
-                               uint64_t out_cap, uint64_t* total, uint64_t* n_rec, uint64_t* n_groups, uint64_t* bad,
+// A reduce task's sources once decoded (decode_task): their records back to back in source order in arena (source i:
+// length[i] bytes at place[i]) and their statuses.  Only this struct tells a fetched block (its status is the decode
+// job's) from an exchange read's cached range (mix: its SortSource's).  report() writes status[] and bad_slice[].
+struct DecodedTask {
+  std::vector<SortSource>* mix;
+  int32_t *status_out, *bad_slice_out;  // bad_slice_out: nullptr when not wanted
+  uint32_t n_src;
+  std::vector<uint64_t> place, length;
+  DecompressJob J;
+  const uint8_t* arena = nullptr;
+  uint64_t total = 0;
+  bool failed = false;  // a source failed: the call ends with nothing sorted or written
+
+  DecodedTask(std::vector<SortSource>* mix, uint32_t n, int32_t* status, int32_t* bad_slice)
+      : mix(mix), status_out(status), bad_slice_out(bad_slice), n_src(mix ? (uint32_t)mix->size() : n), place(n_src),
+        length(n_src) {}
+  bool cached(uint32_t i) const { return mix && (*mix)[i].cached; }
+  uint32_t block(uint32_t i) const { return mix ? (*mix)[i].block : i; }
+  int32_t& status(uint32_t i) { return cached(i) ? (*mix)[i].status : J.h.status[block(i)]; }
+  const SortSource* marked(uint32_t i) const { return cached(i) && (*mix)[i].marked ? &(*mix)[i] : nullptr; }
+  // Source i fails with B2S_E_CORRUPT.  Only the call's first failed source is named in b2s_last_error ("block i" or
+  // "cached source i", then what); a later one only gets its status.
+  void fail_source(uint32_t i, const std::string& what) {
+    status(i) = B2S_E_CORRUPT;
+    if (!failed) fail(B2S_E_CORRUPT, cached(i) ? "cached source %s" : "block %s", (std::to_string(i) + what).c_str());
+    failed = true;
+  }
+  void bad_row(uint32_t i, uint64_t byte, const char* why) {
+    fail_source(i, ": bad row record at byte " + std::to_string(byte) + ": " + why);
+  }
+  int report() {  // -> 0, the result of a call that ends because a source failed (nothing is sorted or written)
+    for (uint32_t i = 0; i < n_src; i++) {
+      status_out[i] = status(i);
+      if (bad_slice_out) bad_slice_out[i] = cached(i) ? -1 : J.h.bad[block(i)];
+    }
+    return 0;
+  }
+};
+
+// Decodes the n blocks at d_src + src_dev_off[i] (src_contiguous: back to back) into T.  Phase A verifies and sizes
+// them; a failed block, or (fixed-size records) a length that is not a multiple of record_bytes, fails the call.  Phase
+// B decodes into S.dst (codec NONE: used in place, or copied there).  An exchange read (T.mix): the decoded offsets are
+// shifted past the cached bytes before each block, and one gather moves the cached ranges (NONE: and blocks) around.
+static int decode_task(Device* D, Slot& S, uint32_t codec, uint32_t alg, uint32_t n, const uint8_t* d_src,
+                       const uint64_t* src_dev_off, const uint64_t* src_len, bool src_contiguous,
+                       const uint32_t* slice_base, const uint64_t* slice_len, const uint64_t* slice_sum,
+                       uint64_t srcb, const RecordSpec& spec, uint64_t out_cap, DecodedTask& T,
+                       uint64_t* launches) {
+  cudaStream_t st = S.st;
+  DecompressJob& J = T.J;
+  int rc;
+  if (n) {
+    rc = decompress_phase_a(S, D->tabs, codec, alg, n, src_dev_off, src_len, alg ? slice_base[n] : 0, slice_base,
+                            slice_len, slice_sum, d_src, srcb, J, launches, true);
+    if (rc) return rc;
+    // the phase-A verdicts (checksums, stream headers) and decoded lengths, before anything is decoded
+    CU(cudaMemcpyAsync(J.h.down, J.d.down, J.d.down_bytes, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    CU(cudaGetLastError());
+  } else {  // every source is cached
+    CU(S.mark(K0, st));
+  }
+  uint64_t at = 0;
+  for (uint32_t i = 0; i < T.n_src; i++) {
+    const bool c = T.cached(i);
+    const uint64_t len = c ? (*T.mix)[i].len : J.h.dst_len[T.block(i)];
+    if (T.status(i) == B2S_OK && !spec.rows() && len % spec.record_bytes)
+      T.fail_source(i, std::string(c ? " holds " : " decodes to ") + std::to_string(len) +
+                           " bytes, not a multiple of record_bytes " + std::to_string(spec.record_bytes));
+    T.failed |= T.status(i) != B2S_OK;
+    T.place[i] = at;
+    T.length[i] = len;
+    at += len;
+  }
+  T.total = T.mix ? at : J.h.totals[1];
+  if (T.failed) return T.report();
+  if (!spec.rows() && T.total / spec.record_bytes > 0xffffffffull)
+    return fail(B2S_E_ARG, "more than 2^32 - 1 records in one call (%s bytes)", std::to_string(T.total).c_str());
+  if (!spec.aggregate && !spec.join && T.total > out_cap) {  // an aggregation's or join's output is sized later
+    T.report();
+    return fail(B2S_E_DST_TOO_SMALL, "dst_cap is below the %s decoded bytes", std::to_string(T.total).c_str());
+  }
+
+  // the decoded arena: every source's records back to back in order; in S.dst unless codec NONE left them so
+  T.arena = d_src;
+  if (T.mix || codec != B2S_CODEC_NONE || (!src_contiguous && T.total)) {
+    if ((rc = S.dst.ensure(T.total + 64))) return rc;
+    T.arena = (const uint8_t*)S.dst.p;
+  }
+  if (T.mix) {
+    std::vector<ExchangePiece> pieces;
+    for (uint32_t i = 0; i < T.n_src; i++) {
+      const SortSource& s = (*T.mix)[i];
+      if (s.cached)
+        exchange_add_pieces(pieces, s.src, T.place[i], s.len);
+      else if (codec == B2S_CODEC_NONE)
+        exchange_add_pieces(pieces, d_src + src_dev_off[s.block], T.place[i], src_len[s.block]);
+      else
+        J.h.dst_off[s.block] = T.place[i];
+    }
+    if (n && codec != B2S_CODEC_NONE)  // phase B decodes every block straight to its place among the cached ranges
+      CU(cudaMemcpyAsync(J.d.dst_off, J.h.dst_off, (size_t)n * 8, cudaMemcpyHostToDevice, st));
+    if (!pieces.empty()) {
+      if ((rc = S.xpieces.ensure(pieces.size() * sizeof(ExchangePiece)))) return rc;
+      CU(cudaMemcpyAsync(S.xpieces.p, pieces.data(), pieces.size() * sizeof(ExchangePiece), cudaMemcpyHostToDevice,
+                         st));
+      launch_exchange_gather((const ExchangePiece*)S.xpieces.p, (uint32_t)pieces.size(), (uint8_t*)S.dst.p, st,
+                             launches);
+    }
+  }
+  if (codec != B2S_CODEC_NONE && n) {
+    if ((rc = decompress_enqueue_b(S, J, d_src, (uint8_t*)S.dst.p, S.dst.cap, launches))) return rc;
+    CU(cudaEventSynchronize(S.ev_b));
+    CU(cudaGetLastError());
+    for (uint32_t i = 0; i < n; i++) T.failed |= J.h.status[i] != B2S_OK;
+  } else if (!T.mix && !src_contiguous) {
+    for (uint32_t i = 0; i < n; i++)
+      if (src_len[i])
+        CU(cudaMemcpyAsync((uint8_t*)S.dst.p + J.h.dst_off[i], d_src + src_dev_off[i], src_len[i],
+                           cudaMemcpyDeviceToDevice, st));
+  }
+  return T.report();
+}
+
+// a source whose row verdict v[i] (framing, or the key pass's string check) is not ~0 fails, the first one named
+static void take_verdicts(DecodedTask& T, const RecordSpec& spec, const uint64_t* v) {
+  const char* const why[] = {"", "the block ends inside a size prefix", "the size is negative",
+                             "the record runs past the block end",
+                             spec.join ? "the row is shorter than its side's fixed region"
+                                       : "the row is shorter than key_off + key_len",
+                             "the row does not hold the null-bit word", "the row is shorter than an aggregate slot",
+                             "a string key runs past the end of its row, or a decimal key's size "
+                             "is not in [1, 16] or its bytes run past the end of its row"};
+  for (uint32_t i = 0; i < T.n_src; i++)
+    if (v[i] != ~0ull) T.bad_row(i, v[i] & ((1ull << 61) - 1), why[v[i] >> 61]);
+}
+
+// A reduce task's rows in key order (order_rows): idx (nullptr: arena order), heads (nullptr: where key words differ),
+// and S.pws's parts in order: sort, aggregation, refinement (nullptr unless the key refines), join grouping, join.
+struct RowOrder {
+  uint64_t records = 0;
+  uint32_t key_bytes = 0;
+  const uint32_t *idx = nullptr, *heads = nullptr;
+  uint8_t *ws = nullptr, *aws = nullptr, *rws = nullptr, *gws = nullptr, *jws = nullptr;
+  void carve(uint8_t* base, const size_t (&bytes)[5]) {
+    uint8_t** part[] = {&ws, &aws, &rws, &gws, &jws};
+    for (int k = 0; k < 5; k++) {
+      *part[k] = base;
+      base += bytes[k];
+    }
+  }
+};
+
+// Orders T's rows by key into R: framing, one readback of the record count and the verdicts (a bad source fails the
+// call), which sizes the workspace with the tail's parts (a join's n_join_fields), then emit, the first-pass sort and
+// the refine rounds, one readback each.  jk: a join's keys per side as its kernels encode them; nullptr: spec.keys.
+static int order_rows(Slot& S, const RecordSpec& spec, DecodedTask& T, const JoinKeys* jk, uint32_t n_join_fields,
+                      RowOrder& R, uint64_t* launches) {
+  cudaStream_t st = S.st;
+  const KeySpec& ks = spec.keys;
+  const uint32_t n_src = T.n_src;
+  uint64_t min_key = 0, min_null = 0;
+  for (uint32_t c = 0; c < ks.n && !jk; c++) {  // a join checks each side's rows in its key pass
+    min_key = std::max<uint64_t>(min_key, (uint64_t)ks.off[c] + ks.len[c]);
+    if (ks.null_field[c] >= 0) min_null = std::max<uint64_t>(min_null, null_word(ks.null_field[c]) + 8);
+  }
+  // a cached range with record boundaries is marked from them instead of walked (its walk is empty)
+  std::vector<uint64_t> walk(T.length);
+  std::vector<RowsMark> marks;
+  for (uint32_t i = 0; i < n_src; i++) {
+    const SortSource* s = T.marked(i);
+    if (!s) continue;
+    walk[i] = 0;
+    marks.push_back(RowsMark{s->rec_off, T.place[i] - s->first_off, T.place[i],
+                             marks.empty() ? 0 : marks.back().first + marks.back().count, s->n_rec, i});
+  }
+  int rc;
+  if ((rc = S.fws.ensure(rows_frame_ws_bytes(T.total, n_src, (uint32_t)marks.size())))) return rc;
+  uint8_t* fws = (uint8_t*)S.fws.p;
+  CU(S.mark(P0, st));
+  CU(S.mark(F0, st, *launches));
+  launch_rows_frame(T.arena, T.total, T.place.data(), walk.data(), n_src, min_key, min_null, agg_min_row(spec), fws,
+                    st, launches, marks.data(), (uint32_t)marks.size());
+  CU(S.mark(F1, st, *launches));
+  std::vector<uint64_t> rb(n_src + 1);
+  CU(cudaMemcpyAsync(rb.data(), rows_frame_readback(fws, T.total, n_src), rows_frame_readback_bytes(n_src),
+                     cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  CU(cudaGetLastError());
+  for (const RowsMark& m : marks) rb[1 + m.range] = rows_mark_verdict(rb[1 + m.range]);
+  take_verdicts(T, spec, rb.data() + 1);
+  if (T.failed) return T.report();
+  const uint64_t records = R.records = rb[0];
+  if (records > 0xffffffffull)
+    return fail(B2S_E_ARG, "more than 2^32 - 1 records in one call (%s records)", std::to_string(records).c_str());
+  const KeySpec& encoded = jk ? jk->side[0] : ks;
+  R.key_bytes = rows_key_bytes(encoded);
+  const bool refine = rows_key_refines(encoded);
+  const size_t part[5] = {rows_sort_ws_bytes(records, R.key_bytes),
+                          spec.aggregate ? rows_aggregate_ws_bytes(records, spec.n_aggs, agg_spec(spec).n_wide) : 0,
+                          refine ? rows_refine_ws_bytes(records, n_src) : 0,
+                          jk ? rows_aggregate_ws_bytes(records, 0, 0) : 0,
+                          jk ? join_ws_bytes(records, n_src, n_join_fields) : 0};
+  if ((records || jk) && (rc = S.pws.ensure(part[0] + part[1] + part[2] + part[3] + part[4]))) return rc;
+  R.carve((uint8_t*)S.pws.p, part);
+  if (!refine) R.rws = nullptr;
+  CU(S.mark(F2, st, *launches));
+  launch_rows_emit(T.arena, T.total, n_src, fws, records, R.key_bytes, R.ws, st, launches);
+  CU(S.mark(F3, st, *launches));
+  const uint64_t* ranges = rows_frame_ranges(fws, T.total, n_src);
+  R.idx = jk ? launch_rows_join_order(T.arena, records, *jk, ranges, n_src, join_readback(R.jws, records, n_src) + 4,
+                                      R.ws, R.rws, st, launches)
+             : launch_rows_order(T.arena, records, ks, ranges, n_src, R.ws, R.rws, st, launches);
+  if (!refine || !records) return 0;
+  // one readback per round: the tied records and their runs (the first also brings the string verdicts)
+  std::vector<uint64_t> rrb(n_src + 1);
+  for (uint32_t d = kKeyPrefixBytes, round = 0;; d += kKeyChunkBytes, round++) {
+    launch_rows_refine_mark(records, d, R.rws, n_src, st, launches);
+    CU(cudaMemcpyAsync(rrb.data(), rows_refine_readback(R.rws, records, n_src), (round ? 1 : rrb.size()) * 8,
+                       cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    CU(cudaGetLastError());
+    if (!round) {
+      take_verdicts(T, spec, rrb.data() + 1);
+      if (T.failed) return T.report();
+    }
+    const uint64_t tied = rrb[0] & 0xffffffffull, runs = rrb[0] >> 32;
+    if (!tied) break;
+    if (jk) launch_rows_join_refine_round(T.arena, records, *jk, tied, runs, d, R.ws, R.rws, st, launches);
+    else launch_rows_refine_round(T.arena, records, ks, tied, runs, d, R.ws, R.rws, n_src, st, launches);
+  }
+  R.idx = rows_refine_order(R.rws, records, n_src);
+  R.heads = rows_refine_heads(R.rws, records, n_src);
+  return 0;
+}
+
+// The end of an aggregation: grouping, one readback of the group count, output bytes (*total, checked against out_cap)
+// and decimal verdict, the heads' gather and the merge into d_out.  A bad out-of-line decimal (kAggBad*) fails its
+// source and nothing is written.  The dominant step is this one (marks G0, G1).
+static int aggregate_rows_tail(Slot& S, const RecordSpec& spec, DecodedTask& T, const RowOrder& R, uint8_t* d_out,
+                               uint64_t out_cap, uint64_t* total, uint64_t* n_rec, uint64_t* n_groups,
                                uint64_t* launches) {
   cudaStream_t st = S.st;
-  const uint32_t key_bytes = rows_key_bytes(spec.keys);
   const AggSpec agg = agg_spec(spec);
   uint64_t rb[3] = {0, 0, ~0ull};  // groups, output bytes, decimal verdict
   CU(S.mark(G0, st, *launches));
-  if (records) {
-    launch_rows_group(arena, records, idx, heads, key_bytes, agg, ws, aws, st, launches);
-    CU(cudaMemcpyAsync(rb, rows_aggregate_readback(aws, records, agg.n, agg.n_wide), (agg.n_wide ? 3 : 2) * 8,
+  if (R.records) {
+    launch_rows_group(T.arena, R.records, R.idx, R.heads, R.key_bytes, agg, R.ws, R.aws, st, launches);
+    CU(cudaMemcpyAsync(rb, rows_aggregate_readback(R.aws, R.records, agg.n, agg.n_wide), (agg.n_wide ? 3 : 2) * 8,
                        cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
     CU(cudaGetLastError());
   }
-  *bad = rb[2];
-  if (rb[2] != ~0ull) return 0;
+  if (rb[2] != ~0ull) {
+    // a bad decimal: the source holding the record (the last that starts at or before it) fails, as a framing verdict
+    const uint64_t at_byte = rb[2] >> 2;
+    uint32_t i = 0;
+    for (uint32_t k = 0; k < T.n_src; k++)
+      if (T.place[k] <= at_byte && T.length[k]) i = k;
+    static const char* const why[] = {"",
+                                      "a decimal aggregate's size is not in [1, 16] or its bytes run past the end of "
+                                      "its row",
+                                      "a decimal aggregate's 16-byte region runs past the end of its row",
+                                      "a decimal aggregate's 16-byte region starts before the end of a slot or null "
+                                      "word in use"};
+    T.bad_row(i, at_byte - T.place[i], why[rb[2] & 3]);
+    return T.report();
+  }
   *total = rb[1];
   if (rb[1] > out_cap)
     return fail(B2S_E_DST_TOO_SMALL, "dst_cap is below the %s output bytes", std::to_string(rb[1]).c_str());
-  launch_rows_aggregate(arena, records, rb[0], key_bytes, agg, ws, aws, d_out, st, launches);
+  launch_rows_aggregate(T.arena, R.records, rb[0], R.key_bytes, agg, R.ws, R.aws, d_out, st, launches);
   CU(S.mark(G1, st, *launches));
   CU(S.mark(P1, st));
   CU(cudaStreamSynchronize(st));
   CU(cudaGetLastError());
-  *n_rec = records;
+  *n_rec = R.records;
   if (n_groups) *n_groups = rb[0];
   return 0;
 }
@@ -3175,387 +3421,141 @@ static void join_layout(const RecordSpec& spec, uint64_t split, JoinKeys& jk, Jo
   shape.n_wide_right = (uint32_t)fields.size() - shape.n_var[0] - shape.n_var[1];
 }
 
-// The whole reduce task on the device: compressed blocks at d_src + src_dev_off[i] (src_contiguous: back to back from
-// d_src in block order, no gaps).  Phase A verifies the slices and sizes every block; a failed block, or (fixed-size
-// records) a decoded length that is not a multiple of record_bytes, ends the call with status[] set and *n_rec = 0
-// (nothing decoded or sorted).  Then the blocks are decoded into S.dst (codec NONE: used in place, or copied there) and
-// their records sorted into *d_sorted (nullptr: into S.parena, returned there).  Rows are framed first, over each
-// source's range of the decoded arena; the record count and the per-source verdicts come back in one readback, which
-// sizes the sort workspace, and a source that is not whole records fails the call as above.
-// mix (exchange-cache reads): the call's sources in order, the n blocks being its fetched ones; status[] / bad_slice[]
-// are per source.  Every source's records land at their source-order place in S.dst: phase A's decoded offsets are
-// shifted past the cached bytes in front of each block before phase B decodes, and one gather moves the cached ranges
-// (codec NONE: and the fetched blocks) around them.
-static int decompress_sort_run(Device* D, Slot& S, uint32_t codec, uint32_t alg, uint32_t n, const uint8_t* d_src,
-                               const uint64_t* src_dev_off, const uint64_t* src_len, bool src_contiguous,
-                               const uint32_t* slice_base, const uint64_t* slice_len, const uint64_t* slice_sum,
-                               const RecordSpec& spec, uint8_t** d_sorted, uint64_t out_cap, uint64_t* total,
-                               uint64_t* n_rec, uint64_t* n_groups, int32_t* status, int32_t* bad_slice,
-                               uint64_t* launches, const std::vector<SortSource>* mix = nullptr) {
+// The end of a join: grouping, counts (one readback with the key pass's verdicts; *total = output bytes), the joined
+// rows into *d_out (nullptr: into S.parena, returned there) and the per-side counts.  The dominant step (G0, G1).
+static int join_rows_tail(Slot& S, const RecordSpec& spec, DecodedTask& T, const RowOrder& R, const JoinShape& shape,
+                          const std::vector<uint32_t>& fields, uint8_t** d_out, uint64_t out_cap, uint64_t* total,
+                          uint64_t* n_rec, uint64_t* launches) {
   cudaStream_t st = S.st;
-  DecompressJob J;
-  int rc;
-  if (n) {
-    uint64_t srcb = 0;
-    for (uint32_t i = 0; i < n; i++) srcb += src_len[i];
-    rc = decompress_phase_a(S, D->tabs, codec, alg, n, src_dev_off, src_len, alg ? slice_base[n] : 0, slice_base,
-                            slice_len, slice_sum, d_src, srcb, J, launches, true);
-    if (rc) return rc;
-    // the phase-A verdicts (checksums, stream headers) and decoded lengths, before anything is decoded
-    CU(cudaMemcpyAsync(J.h.down, J.d.down, J.d.down_bytes, cudaMemcpyDeviceToHost, st));
+  std::vector<uint64_t> jb(4 + T.n_src, ~0ull);
+  jb[0] = jb[1] = jb[2] = jb[3] = 0;
+  CU(S.mark(G0, st, *launches));
+  if (R.records) {
+    launch_rows_group(T.arena, R.records, R.idx, R.heads, R.key_bytes, AggSpec{}, R.ws, R.gws, st, launches);
+    launch_join_count(T.arena, R.records, R.idx, shape, fields.data(), (uint32_t)fields.size(), R.key_bytes, R.ws,
+                      R.gws, R.jws, T.n_src, st, launches);
+    CU(cudaMemcpyAsync(jb.data(), join_readback(R.jws, R.records, T.n_src), join_readback_bytes(T.n_src),
+                       cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
     CU(cudaGetLastError());
-  } else {  // every source is cached
-    CU(S.mark(K0, st));
   }
-  const uint32_t n_src = mix ? (uint32_t)mix->size() : n;
-  auto cached = [&](uint32_t i) { return mix && (*mix)[i].cached; };
-  auto block = [&](uint32_t i) { return mix ? (*mix)[i].block : i; };
-  std::vector<int32_t> cached_status(n_src, B2S_OK);
-  std::vector<uint64_t> place(n_src), length(n_src);  // each source's range of the decoded arena
-  uint64_t at = 0;
-  *n_rec = 0;
-  bool failed = false;
-  char msg[256];
-  for (uint32_t i = 0; i < n_src; i++) {
-    const bool c = cached(i);
-    int32_t& s = c ? cached_status[i] : J.h.status[block(i)];
-    const uint64_t len = c ? (*mix)[i].len : J.h.dst_len[block(i)];
-    if (c) s = (*mix)[i].status;
-    if (s == B2S_OK && !spec.rows() && len % spec.record_bytes) {
-      s = B2S_E_CORRUPT;
-      if (!failed) {
-        snprintf(msg, sizeof msg, "%s %u %s %llu bytes, not a multiple of record_bytes %u", c ? "cached source" : "block",
-                 i, c ? "holds" : "decodes to", (unsigned long long)len, spec.record_bytes);
-        fail(B2S_E_CORRUPT, "%s", msg);
-      }
-    }
-    failed |= s != B2S_OK;
-    place[i] = at;
-    length[i] = len;
-    at += len;
+  take_verdicts(T, spec, jb.data() + 4);
+  if (T.failed) return T.report();
+  if (jb[3]) return fail(B2S_E_UNSUPPORTED, "a joined row is longer than 2^31 - 1 bytes%s");
+  *total = jb[1];
+  if (jb[1] > out_cap)
+    return fail(B2S_E_DST_TOO_SMALL, "dst_cap is below the %s output bytes", std::to_string(jb[1]).c_str());
+  if (!*d_out) {
+    if (int rc = S.parena.ensure(jb[1] + 64)) return rc;
+    *d_out = (uint8_t*)S.parena.p;
   }
-  *total = mix ? at : J.h.totals[1];
-  auto report = [&]() {  // -> 0, the result of a call that ends because a source failed (nothing is sorted or written)
-    for (uint32_t i = 0; i < n_src; i++) {
-      status[i] = cached(i) ? cached_status[i] : J.h.status[block(i)];
-      if (bad_slice) bad_slice[i] = cached(i) ? -1 : J.h.bad[block(i)];
-    }
-    return 0;
-  };
-  if (failed) return report();
-  if (!spec.rows() && *total / spec.record_bytes > 0xffffffffull)
-    return fail(B2S_E_ARG, "more than 2^32 - 1 records in one call (%s bytes)", std::to_string(*total).c_str());
-  if (!spec.aggregate && !spec.join && *total > out_cap) {  // an aggregation's or join's output is sized later
-    report();
-    return fail(B2S_E_DST_TOO_SMALL, "dst_cap is below the %s decoded bytes", std::to_string(*total).c_str());
-  }
-
-  // the decoded arena: every block's records back to back in block order
-  const uint8_t* arena = d_src;
-  if (mix) {
-    if ((rc = S.dst.ensure(*total + 64))) return rc;
-    arena = (const uint8_t*)S.dst.p;
-    std::vector<ExchangePiece> pieces;
-    for (uint32_t i = 0; i < n_src; i++) {
-      const SortSource& s = (*mix)[i];
-      if (s.cached)
-        exchange_add_pieces(pieces, s.src, place[i], s.len);
-      else if (codec == B2S_CODEC_NONE)
-        exchange_add_pieces(pieces, d_src + src_dev_off[s.block], place[i], src_len[s.block]);
-      else
-        J.h.dst_off[s.block] = place[i];
-    }
-    if (n && codec != B2S_CODEC_NONE)  // phase B decodes every block straight to its place among the cached ranges
-      CU(cudaMemcpyAsync(J.d.dst_off, J.h.dst_off, (size_t)n * 8, cudaMemcpyHostToDevice, st));
-    if (!pieces.empty()) {
-      if ((rc = S.xpieces.ensure(pieces.size() * sizeof(ExchangePiece)))) return rc;
-      CU(cudaMemcpyAsync(S.xpieces.p, pieces.data(), pieces.size() * sizeof(ExchangePiece), cudaMemcpyHostToDevice,
-                         st));
-      launch_exchange_gather((const ExchangePiece*)S.xpieces.p, (uint32_t)pieces.size(), (uint8_t*)S.dst.p, st,
-                             launches);
-    }
-  }
-  if (codec == B2S_CODEC_NONE || !n) {
-    if (!mix && !src_contiguous && *total) {
-      if ((rc = S.dst.ensure(*total + 64))) return rc;
-      for (uint32_t i = 0; i < n; i++)
-        if (src_len[i])
-          CU(cudaMemcpyAsync((uint8_t*)S.dst.p + J.h.dst_off[i], d_src + src_dev_off[i], src_len[i],
-                             cudaMemcpyDeviceToDevice, st));
-      arena = (const uint8_t*)S.dst.p;
-    }
-  } else {
-    if (!mix && (rc = S.dst.ensure(*total + 64))) return rc;
-    rc = decompress_enqueue_b(S, J, d_src, (uint8_t*)S.dst.p, S.dst.cap, launches);
-    if (rc) return rc;
-    CU(cudaEventSynchronize(S.ev_b));
-    CU(cudaGetLastError());
-    for (uint32_t i = 0; i < n; i++) failed |= J.h.status[i] != B2S_OK;
-    if (failed) return report();
-    arena = (const uint8_t*)S.dst.p;
-  }
-  report();
-
-  if (!*d_sorted && !spec.join) {
-    if ((rc = S.parena.ensure(*total + 64))) return rc;
-    *d_sorted = (uint8_t*)S.parena.p;
-  }
-  if (!spec.rows()) {
-    const uint64_t records = *total / spec.record_bytes;
-    if (records && (rc = S.pws.ensure(key_sort_ws_bytes(records, spec.keys.len[0])))) return rc;
-    CU(S.mark(P0, st));
-    launch_key_sort(arena, records, spec.record_bytes, spec.keys.off[0], spec.keys.len[0], (uint8_t*)S.pws.p,
-                    *d_sorted, st, launches);
-    CU(S.mark(P1, st));
-    CU(cudaStreamSynchronize(st));
-    CU(cudaGetLastError());
-    *n_rec = records;
-    return 0;
-  }
-
-  // rows: frame every source's range, then one readback of the record count and the verdicts
-  const KeySpec& ks = spec.keys;
-  uint64_t min_key = 0, min_null = 0;
-  for (uint32_t c = 0; c < ks.n && !spec.join; c++) {  // a join checks each side's rows in its key pass
-    min_key = std::max<uint64_t>(min_key, (uint64_t)ks.off[c] + ks.len[c]);
-    if (ks.null_field[c] >= 0) min_null = std::max<uint64_t>(min_null, null_word(ks.null_field[c]) + 8);
-  }
-  // a cached range with record boundaries is marked from them instead of walked (its walk is empty)
-  std::vector<uint64_t> walk(length);
-  std::vector<RowsMark> marks;
-  for (uint32_t i = 0; i < n_src; i++) {
-    if (!cached(i) || !(*mix)[i].marked) continue;
-    const SortSource& s = (*mix)[i];
-    walk[i] = 0;
-    marks.push_back(RowsMark{s.rec_off, place[i] - s.first_off, place[i],
-                             marks.empty() ? 0 : marks.back().first + marks.back().count, s.n_rec, i});
-  }
-  if ((rc = S.fws.ensure(rows_frame_ws_bytes(*total, n_src, (uint32_t)marks.size())))) return rc;
-  uint8_t* fws = (uint8_t*)S.fws.p;
-  CU(S.mark(P0, st));
-  CU(S.mark(F0, st, *launches));
-  launch_rows_frame(arena, *total, place.data(), walk.data(), n_src, min_key, min_null, agg_min_row(spec), fws, st,
-                    launches, marks.data(), (uint32_t)marks.size());
-  CU(S.mark(F1, st, *launches));
-  std::vector<uint64_t> rb(n_src + 1);
-  CU(cudaMemcpyAsync(rb.data(), rows_frame_readback(fws, *total, n_src), rows_frame_readback_bytes(n_src),
-                     cudaMemcpyDeviceToHost, st));
-  CU(cudaStreamSynchronize(st));
-  CU(cudaGetLastError());
-  for (const RowsMark& m : marks) rb[1 + m.range] = rows_mark_verdict(rb[1 + m.range]);
-  // a source whose verdict (framing, or the key pass's string check) is not ~0 fails, the first one named
-  auto take_verdicts = [&](const uint64_t* v) {
-    for (uint32_t i = 0; i < n_src; i++) {
-      if (v[i] == ~0ull) continue;
-      (cached(i) ? cached_status[i] : J.h.status[block(i)]) = B2S_E_CORRUPT;
-      if (!failed) {
-        const char* const why[] = {"", "the block ends inside a size prefix", "the size is negative",
-                                   "the record runs past the block end",
-                                   spec.join ? "the row is shorter than its side's fixed region"
-                                             : "the row is shorter than key_off + key_len",
-                                   "the row does not hold the null-bit word",
-                                   "the row is shorter than an aggregate slot",
-                                   "a string key runs past the end of its row, or a decimal key's size "
-                                   "is not in [1, 16] or its bytes run past the end of its row"};
-        snprintf(msg, sizeof msg, "%s %u: bad row record at byte %llu: %s", cached(i) ? "cached source" : "block", i,
-                 (unsigned long long)(v[i] & ((1ull << 61) - 1)), why[v[i] >> 61]);
-        fail(B2S_E_CORRUPT, "%s", msg);
-      }
-      failed = true;
-    }
-  };
-  take_verdicts(rb.data() + 1);
-  if (failed) return report();
-  const uint64_t records = rb[0];
-  if (records > 0xffffffffull)
-    return fail(B2S_E_ARG, "more than 2^32 - 1 records in one call (%s records)", std::to_string(records).c_str());
-  // a join: its key columns per side as its kernels encode them (a column nullable on one side only takes a null byte
-  // on both), which set the key's width for every step, and its joined row's shape
-  std::vector<uint32_t> join_fields;
-  JoinKeys jk;
-  JoinShape shape{};
-  if (spec.join)
-    join_layout(spec, n_src > spec.join->n_left ? place[spec.join->n_left] : *total, jk, shape, join_fields);
-  const KeySpec& encoded = spec.join ? jk.side[0] : ks;
-  const uint32_t key_bytes = rows_key_bytes(encoded);
-  const bool refine = rows_key_refines(encoded);
-  const size_t sort_ws = rows_sort_ws_bytes(records, key_bytes);
-  const size_t agg_ws = spec.aggregate ? rows_aggregate_ws_bytes(records, spec.n_aggs, agg_spec(spec).n_wide) : 0;
-  const size_t refine_ws = refine ? rows_refine_ws_bytes(records, n_src) : 0;
-  // a join: the grouping's workspace (an aggregation without aggregates) and the join's
-  const size_t join_ws = spec.join ? rows_aggregate_ws_bytes(records, 0, 0) : 0;
-  const size_t join_own_ws = spec.join ? join_ws_bytes(records, n_src, (uint32_t)join_fields.size()) : 0;
-  if ((records || spec.join) && (rc = S.pws.ensure(sort_ws + agg_ws + refine_ws + join_ws + join_own_ws))) return rc;
-  uint8_t* ws = (uint8_t*)S.pws.p;
-  uint8_t* rws = refine ? ws + sort_ws + agg_ws : nullptr;
-  uint8_t* gws = ws + sort_ws + agg_ws + refine_ws;  // a join's grouping workspace, then its own
-  uint8_t* jws = gws + join_ws;
-  CU(S.mark(F2, st, *launches));
-  launch_rows_emit(arena, *total, n_src, fws, records, key_bytes, ws, st, launches);
-  CU(S.mark(F3, st, *launches));
-  const uint64_t* ranges = rows_frame_ranges(fws, *total, n_src);
-  const uint32_t* idx =
-      spec.join ? launch_rows_join_order(arena, records, jk, ranges, n_src, join_readback(jws, records, n_src) + 4, ws,
-                                         rws, st, launches)
-                : launch_rows_order(arena, records, ks, ranges, n_src, ws, rws, st, launches);
-  const uint32_t* heads = nullptr;
-  if (refine && records) {
-    // one readback per round: the tied records and their runs (the first also brings the string verdicts)
-    std::vector<uint64_t> rrb(n_src + 1);
-    for (uint32_t d = kKeyPrefixBytes, round = 0;; d += kKeyChunkBytes, round++) {
-      launch_rows_refine_mark(records, d, rws, n_src, st, launches);
-      CU(cudaMemcpyAsync(rrb.data(), rows_refine_readback(rws, records, n_src), (round ? 1 : rrb.size()) * 8,
-                         cudaMemcpyDeviceToHost, st));
-      CU(cudaStreamSynchronize(st));
-      CU(cudaGetLastError());
-      if (!round) {
-        take_verdicts(rrb.data() + 1);
-        if (failed) return report();
-      }
-      const uint64_t tied = rrb[0] & 0xffffffffull, runs = rrb[0] >> 32;
-      if (!tied) break;
-      if (spec.join) launch_rows_join_refine_round(arena, records, jk, tied, runs, d, ws, rws, st, launches);
-      else launch_rows_refine_round(arena, records, ks, tied, runs, d, ws, rws, n_src, st, launches);
-    }
-    idx = rows_refine_order(rws, records, n_src);
-    heads = rows_refine_heads(rws, records, n_src);
-  }
-  if (spec.join) {  // the join step: grouping, counts (one readback with the key pass's verdicts), emit
-    std::vector<uint64_t> jb(4 + n_src, ~0ull);
-    jb[0] = jb[1] = jb[2] = jb[3] = 0;
-    CU(S.mark(G0, st, *launches));
-    if (records) {
-      launch_rows_group(arena, records, idx, heads, key_bytes, AggSpec{}, ws, gws, st, launches);
-      launch_join_count(arena, records, idx, shape, join_fields.data(), (uint32_t)join_fields.size(), key_bytes, ws,
-                        gws, jws, n_src, st, launches);
-      CU(cudaMemcpyAsync(jb.data(), join_readback(jws, records, n_src), join_readback_bytes(n_src),
-                         cudaMemcpyDeviceToHost, st));
-      CU(cudaStreamSynchronize(st));
-      CU(cudaGetLastError());
-    }
-    take_verdicts(jb.data() + 4);
-    if (failed) return report();
-    if (jb[3]) return fail(B2S_E_UNSUPPORTED, "a joined row is longer than 2^31 - 1 bytes%s");
-    *total = jb[1];
-    if (jb[1] > out_cap)
-      return fail(B2S_E_DST_TOO_SMALL, "dst_cap is below the %s output bytes", std::to_string(jb[1]).c_str());
-    if (!*d_sorted) {
-      if ((rc = S.parena.ensure(jb[1] + 64))) return rc;
-      *d_sorted = (uint8_t*)S.parena.p;
-    }
-    launch_join_emit(arena, records, idx, jb[0], key_bytes, spec.join->type >= B2S_JOIN_LEFT_SEMI, ws, jws, n_src,
-                     *d_sorted, st, launches);
-    CU(S.mark(G1, st, *launches));
-    CU(S.mark(P1, st));
-    CU(cudaStreamSynchronize(st));
-    CU(cudaGetLastError());
-    *n_rec = jb[0];
-    *spec.join->n_side[0] = jb[2];
-    *spec.join->n_side[1] = records - jb[2];
-    return 0;
-  }
-  if (spec.aggregate) {
-    uint64_t bad = ~0ull;
-    if ((rc = aggregate_rows_tail(S, spec, arena, records, idx, heads, ws, ws + sort_ws, *d_sorted, out_cap, total,
-                                  n_rec, n_groups, &bad, launches)) ||
-        bad == ~0ull)
-      return rc;
-    // a bad decimal: the source holding the record (the last that starts at or before it) fails, as a framing verdict
-    const uint64_t at_byte = bad >> 2;
-    uint32_t i = 0;
-    for (uint32_t k = 0; k < n_src; k++)
-      if (place[k] <= at_byte && length[k]) i = k;
-    (cached(i) ? cached_status[i] : J.h.status[block(i)]) = B2S_E_CORRUPT;
-    static const char* const why[] = {"",
-                                      "a decimal aggregate's size is not in [1, 16] or its bytes run past the end of "
-                                      "its row",
-                                      "a decimal aggregate's 16-byte region runs past the end of its row",
-                                      "a decimal aggregate's 16-byte region starts before the end of a slot or null "
-                                      "word in use"};
-    snprintf(msg, sizeof msg, "%s %u: bad row record at byte %llu: %s", cached(i) ? "cached source" : "block", i,
-             (unsigned long long)(at_byte - place[i]), why[bad & 3]);
-    fail(B2S_E_CORRUPT, "%s", msg);
-    return report();
-  }
-  launch_rows_gather(arena, records, key_bytes, idx, ws, *d_sorted, st, launches);
+  launch_join_emit(T.arena, R.records, R.idx, jb[0], R.key_bytes, spec.join->type >= B2S_JOIN_LEFT_SEMI, R.ws,
+                   R.jws, T.n_src, *d_out, st, launches);
+  CU(S.mark(G1, st, *launches));
   CU(S.mark(P1, st));
   CU(cudaStreamSynchronize(st));
+  CU(cudaGetLastError());
+  *n_rec = jb[0];
+  *spec.join->n_side[0] = jb[2];
+  *spec.join->n_side[1] = R.records - jb[2];
+  return 0;
+}
+
+// After decode_task: the fixed-size records' key sort, or order_rows and the tail of the call's family (a row sort's:
+// the gather), into *d_sorted (nullptr: into S.parena, returned there).  A failed source: 0, status[] set, *n_rec 0.
+static int run_reduce_task(Slot& S, const RecordSpec& spec, DecodedTask& T, uint8_t** d_sorted, uint64_t out_cap,
+                           uint64_t* total, uint64_t* n_rec, uint64_t* n_groups, uint64_t* launches) {
+  int rc;
+  if (!*d_sorted && !spec.join) {
+    if ((rc = S.parena.ensure(T.total + 64))) return rc;
+    *d_sorted = (uint8_t*)S.parena.p;
+  }
+  uint64_t records;
+  if (!spec.rows()) {  // fixed-size records: their key sort
+    records = T.total / spec.record_bytes;
+    if (records && (rc = S.pws.ensure(key_sort_ws_bytes(records, spec.keys.len[0])))) return rc;
+    CU(S.mark(P0, S.st));
+    launch_key_sort(T.arena, records, spec.record_bytes, spec.keys.off[0], spec.keys.len[0], (uint8_t*)S.pws.p,
+                    *d_sorted, S.st, launches);
+  } else {
+    // a join: its key columns per side as its kernels encode them (a column nullable on one side only takes a null
+    // byte on both), which set the key's width for every step, and its joined row's shape
+    std::vector<uint32_t> join_fields;
+    JoinKeys jk;
+    JoinShape shape{};
+    if (spec.join)
+      join_layout(spec, T.n_src > spec.join->n_left ? T.place[spec.join->n_left] : T.total, jk, shape, join_fields);
+    RowOrder R;
+    rc = order_rows(S, spec, T, spec.join ? &jk : nullptr, (uint32_t)join_fields.size(), R, launches);
+    if (rc || T.failed) return rc;
+    if (spec.join) return join_rows_tail(S, spec, T, R, shape, join_fields, d_sorted, out_cap, total, n_rec, launches);
+    if (spec.aggregate) return aggregate_rows_tail(S, spec, T, R, *d_sorted, out_cap, total, n_rec, n_groups, launches);
+    records = R.records;
+    launch_rows_gather(T.arena, records, R.key_bytes, R.idx, R.ws, *d_sorted, S.st, launches);
+  }
+  CU(S.mark(P1, S.st));
+  CU(cudaStreamSynchronize(S.st));
   CU(cudaGetLastError());
   *n_rec = records;
   return 0;
 }
 
-// decompress_sort on the read lane of D over device-resident blocks, sorted into dst_base (device memory)
-static int sort_dev_run(Device* D, uint32_t codec, uint32_t alg, uint32_t n, const uint8_t* src_base,
-                        const uint64_t* src_off, const uint64_t* src_len, const uint32_t* slice_base,
-                        const uint64_t* slice_len, const uint64_t* slice_checksum, const RecordSpec& spec,
-                        uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records,
-                        uint64_t* n_groups, int32_t* status, int32_t* bad_slice, const WallTimer& wt,
-                        const std::vector<SortSource>* mix) {
+// A reduce task on the read lane of D (decode_task, run_reduce_task) over device blocks into device memory at dst_base,
+// or (packed) over host blocks, with one upload before and one download into dst_base (host memory) after.
+static int read_task_run(Device* D, bool packed, uint32_t codec, uint32_t alg, uint32_t n, const uint8_t* src_base,
+                         const uint64_t* src_off, const uint64_t* src_len, const uint32_t* slice_base,
+                         const uint64_t* slice_len, const uint64_t* slice_checksum, const RecordSpec& spec,
+                         uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records,
+                         uint64_t* n_groups, int32_t* status, int32_t* bad_slice, const WallTimer& wt,
+                         std::vector<SortSource>* mix) {
   Lane& Ln = D->lane[kLaneRead];
   std::lock_guard<std::mutex> lk(Ln.mtx);
   Slot& S = Ln.slot[0];
   SortBufferTrim trim{S};
-  uint64_t launches = 0, srcb = 0;
-  for (uint32_t i = 0; i < n; i++) srcb += src_len[i];
-  uint8_t* out = dst_base;
-  int rc = decompress_sort_run(D, S, codec, alg, n, src_base, src_off, src_len, false, slice_base, slice_len,
-                               slice_checksum, spec, &out, dst_cap, dst_total, n_records, n_groups, status,
-                               bad_slice, &launches, mix);
-  if (rc) return rc;
-  end_call(wt, launches, CallBytes{srcb, *dst_total, 0, 0}, &S, spec.family());
-  return 0;
-}
-
-// decompress_sort on the read lane of D over host blocks: one upload, the sort, one download into dst_base
-static int sort_packed_run(Device* D, uint32_t codec, uint32_t alg, uint32_t n, const uint8_t* src_base,
-                           const uint64_t* src_off, const uint64_t* src_len, const uint32_t* slice_base,
-                           const uint64_t* slice_len, const uint64_t* slice_checksum, const RecordSpec& spec,
-                           uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records,
-                           uint64_t* n_groups, int32_t* status, int32_t* bad_slice, const WallTimer& wt,
-                           const std::vector<SortSource>* mix) {
-  Lane& Ln = D->lane[kLaneRead];
-  std::lock_guard<std::mutex> lk(Ln.mtx);
-  Slot& S = Ln.slot[0];
-  SortBufferTrim trim{S};
-  // one upload of every block, back to back (the whole task is resident at once: no chunking)
-  std::vector<uint64_t> dev_off(n);
+  cudaStream_t st = S.st;
+  std::vector<uint64_t> dev_off;  // packed: each block's place in the upload, back to back
   uint64_t srcb = 0;
   for (uint32_t i = 0; i < n; i++) {
-    dev_off[i] = srcb;
+    if (packed) dev_off.push_back(srcb);
     srcb += src_len[i];
   }
   int rc;
-  if ((rc = S.src.ensure(srcb + 64))) return rc;
-  cudaStream_t st = S.st;
-  CU(S.mark(H0, st));
-  for (uint32_t i = 0; i < n;) {  // blocks adjacent in host memory go up in one copy
-    uint32_t j = i + 1;
-    while (j < n && src_off[j] == src_off[j - 1] + src_len[j - 1]) j++;
-    const uint64_t bytes = dev_off[j - 1] + src_len[j - 1] - dev_off[i];
-    if (bytes) CU(cudaMemcpyAsync((uint8_t*)S.src.p + dev_off[i], src_base + src_off[i], bytes, cudaMemcpyHostToDevice, st));
-    i = j;
+  uint8_t* out = packed ? nullptr : dst_base;
+  if (packed) {  // one upload of every block (the whole task is resident at once: no chunking)
+    if ((rc = S.src.ensure(srcb + 64))) return rc;
+    CU(S.mark(H0, st));
+    for (uint32_t i = 0; i < n;) {  // blocks adjacent in host memory go up in one copy
+      uint32_t j = i + 1;
+      while (j < n && src_off[j] == src_off[j - 1] + src_len[j - 1]) j++;
+      const uint64_t bytes = dev_off[j - 1] + src_len[j - 1] - dev_off[i];
+      if (bytes)
+        CU(cudaMemcpyAsync((uint8_t*)S.src.p + dev_off[i], src_base + src_off[i], bytes, cudaMemcpyHostToDevice, st));
+      i = j;
+    }
+    CU(S.mark(H1, st));
   }
-  CU(S.mark(H1, st));
   uint64_t launches = 0;
-  uint8_t* sorted = nullptr;
-  rc = decompress_sort_run(D, S, codec, alg, n, (const uint8_t*)S.src.p, dev_off.data(), src_len, true, slice_base,
-                           slice_len, slice_checksum, spec, &sorted, dst_cap, dst_total, n_records, n_groups, status,
-                           bad_slice, &launches, mix);
+  DecodedTask T(mix, n, status, bad_slice);
+  rc = decode_task(D, S, codec, alg, n, packed ? (const uint8_t*)S.src.p : src_base, packed ? dev_off.data() : src_off,
+                   src_len, packed, slice_base, slice_len, slice_checksum, srcb, spec, dst_cap, T, &launches);
+  *dst_total = T.total;
+  *n_records = 0;
+  if (!rc && !T.failed) rc = run_reduce_task(S, spec, T, &out, dst_cap, dst_total, n_records, n_groups, &launches);
   if (rc) return rc;
-  const uint64_t down = *n_records ? *dst_total : 0;
-  CU(S.mark(D0, st));
-  if (down) CU(cudaMemcpyAsync(dst_base, sorted, down, cudaMemcpyDeviceToHost, st));
-  CU(S.mark(D1, st));
-  CU(cudaStreamSynchronize(st));
-  CU(cudaGetLastError());
-  end_call(wt, launches, CallBytes{srcb, *dst_total, srcb, down}, &S, spec.family());
+  const uint64_t down = packed && *n_records ? *dst_total : 0;
+  if (packed) {
+    CU(S.mark(D0, st));
+    if (down) CU(cudaMemcpyAsync(dst_base, out, down, cudaMemcpyDeviceToHost, st));
+    CU(S.mark(D1, st));
+    CU(cudaStreamSynchronize(st));
+    CU(cudaGetLastError());
+  }
+  end_call(wt, launches, CallBytes{srcb, *dst_total, packed ? srcb : 0, down}, &S, spec.family());
   return 0;
 }
 
 // The sources of an exchange sorted read: the fetched ones compacted in source order with their slices (what
-// decompress_sort_run takes as its blocks), and every source in order.
+// read_task_run takes as its blocks), and every source in order.
 struct MixedSources {
   std::vector<SortSource> src;
   std::vector<uint64_t> off, len, slice_len, slice_sum;
@@ -3646,7 +3646,7 @@ static int sort_call(uint32_t dev_index, bool packed, const ExchangeRead* x, uin
   }
   if (rc || !n) return rc;
   std::optional<ExRefs> refs;
-  const std::vector<SortSource>* mix = nullptr;
+  std::vector<SortSource>* mix = nullptr;
   if (x) {
     refs.emplace(D->ordinal, x->shuffle, n, x->map_ids, x->cached);
     if ((rc = exchange_sort_sources(*refs, x->start_reduce, x->end_reduce, M))) return rc;
@@ -3658,9 +3658,8 @@ static int sort_call(uint32_t dev_index, bool packed, const ExchangeRead* x, uin
     slice_checksum = M.slice_sum.data();
     mix = &M.src;
   }
-  return (packed ? sort_packed_run : sort_dev_run)(D, codec, alg, n, src_base, src_off, src_len, slice_base, slice_len,
-                                                   slice_checksum, spec, dst_base, dst_cap, dst_total, n_records,
-                                                   n_groups, status, bad_slice, wt, mix);
+  return read_task_run(D, packed, codec, alg, n, src_base, src_off, src_len, slice_base, slice_len, slice_checksum,
+                       spec, dst_base, dst_cap, dst_total, n_records, n_groups, status, bad_slice, wt, mix);
 }
 
 int b2s_decompress_sort_dev(uint32_t dev_index, uint32_t codec, uint32_t checksum_alg, uint32_t n,
