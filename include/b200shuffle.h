@@ -574,6 +574,16 @@ int b2s_decompress_aggregate_rows_keys_dev(uint32_t dev_index, uint32_t codec, u
  *   B2S_JOIN_LEFT_OUTER: the same; a left record without an equal right key (a null key included) gives join(l, null).
  *   B2S_JOIN_LEFT_SEMI: l itself, byte for byte, once, when it has a match.
  *   B2S_JOIN_LEFT_ANTI: l itself when it has no match, null keys included (NOT EXISTS; not the null-aware form).
+ *   B2S_JOIN_RIGHT_OUTER: for each r of Rs, for each l of Ls whose key equals r's, in Ls order: join(l, r); a right
+ *     record without an equal left key (a null key included) gives join(null, r).  SortMergeJoinExec's RightOuter
+ *     order (the right side streamed, the left buffered), so its outputOrdering, the right keys, holds.
+ *   B2S_JOIN_FULL_OUTER: by runs.  A run is a maximal set of records of both sides whose keys are equal in the sort
+ *     order, nulls equal to nulls there; it matches when its key has no null column and it holds records of both sides
+ *     (its records all have the same null columns).  Runs are taken in ascending key order, nulls first; within a run,
+ *     first each left record l in Ls order: join(l, r) for each right record r of the run in Rs order if the run
+ *     matches, else join(l, null); then, if the run does not match, each right record r in Rs order: join(null, r).
+ *     Spark declares no outputOrdering for a full outer sort-merge join; this order makes the output deterministic,
+ *     and without null keys it is the order of Spark's full outer scanner.
  * Joined row: UnsafeRowJoiner's, which is UnsafeProjection(left.output ++ right.output) when each input's
  * variable-length data is laid out as UnsafeProjection writes it.  nL, nR: the sides' field counts (n_left_fields,
  * n_right_fields); bL, bR, b: the null-bitset words of the left row, the right row and the output, ceil(nL / 64),
@@ -582,15 +592,19 @@ int b2s_decompress_aggregate_rows_keys_dev(uint32_t dev_index, uint32_t codec, u
  * is left bit i for i < nL, right bit i - nL below nL + nR, zero past it.  Every VAR or DECIMAL_WIDE field whose slot
  * is not zero has its offset (the high 32 bits) moved by 8 (b - bL + nR) on the left, by 8 (b - bR + nL) + varL on
  * the right; a zero slot (a null string) stays zero, and a null wide decimal (offset << 32) is moved.
- * The null right side (left outer): every right null bit set, every right slot zero, except that each DECIMAL_WIDE
- * right field gets 16 zero bytes appended to the var bytes, in field order, and its slot is offset << 32 (what
- * UnsafeRowWriter.write(i, (Decimal) null, p, s) writes).
+ * The null right side (left and full outer): every right null bit set, every right slot zero, except that each
+ * DECIMAL_WIDE right field gets 16 zero bytes appended to the var bytes, in field order, and its slot is offset << 32
+ * (what UnsafeRowWriter.write(i, (Decimal) null, p, s) writes).  The null left side (right and full outer) mirrors it:
+ * every left null bit set, every left slot zero, and each DECIMAL_WIDE left field k (in field order) 16 zero bytes in
+ * the left var bytes, its slot (8 (b + nL + nR) + 16 k) << 32; so varL = 16 * (the left DECIMAL_WIDE fields) and the
+ * right side's offsets move by 8 (b - bR + nL) + varL as above.  A joined row never has both sides null.
  * Outputs.  [size BE][row] records, an UnsafeRowSerializer stream, *n_out_records of them, *dst_total bytes; dst_cap
  * below that -> B2S_E_DST_TOO_SMALL with *dst_total = the bytes needed.  *n_left_records / *n_right_records: the input
  * record counts.  The field-kind arrays (B2S_FIELD_*, one per field) may be NULL for semi and anti joins.
  * Errors -> B2S_E_ARG: an unknown join_type; n_left > n; a key column the composite-key calls reject, or any order
  * flag; a key slot outside its side's slots [8 bX, 8 (bX + nX)) or a null bit not below its side's field count; a field
- * count outside 1..65536; NULL or unknown field kinds for inner and left outer; more than 2^32 - 1 input records.
+ * count outside 1..65536; NULL or unknown field kinds for every type but semi and anti; more than 2^32 - 1 input
+ * records.
  * Per block, B2S_E_CORRUPT for every framing rule of the composite-key calls with that block's side's key columns, and
  * when a row is shorter than its side's fixed region 8 (bX + nX); b2s_last_error() names the block and the byte offset
  * of the bad record.  A joined row longer than 2^31 - 1 bytes -> B2S_E_UNSUPPORTED.  Checksums and bad_slice as in the
@@ -603,7 +617,10 @@ int b2s_decompress_aggregate_rows_keys_dev(uint32_t dev_index, uint32_t codec, u
 #define B2S_JOIN_LEFT_OUTER 1
 #define B2S_JOIN_LEFT_SEMI 2
 #define B2S_JOIN_LEFT_ANTI 3
-/* field kinds of a side's schema (the joined row's offset fix-up and the null right side of a left outer join) */
+/* 4 is not assigned */
+#define B2S_JOIN_RIGHT_OUTER 5
+#define B2S_JOIN_FULL_OUTER 6
+/* field kinds of a side's schema (the joined row's offset fix-up and an outer join's null side) */
 #define B2S_FIELD_FIXED 0        /* a fixed-width value in its 8-byte slot */
 #define B2S_FIELD_VAR 1          /* (offset << 32) | size: string, binary, array, map, struct */
 #define B2S_FIELD_DECIMAL_WIDE 2 /* Decimal(p > 18): (offset << 32) | size, 16 bytes reserved */

@@ -212,8 +212,9 @@ int b2sh_reader_read_aggregated_rows_keys(b2sh_reader* r, uint32_t n_keys, const
  * partitions of another shuffle; INTEGRATION.md §3n).  Both readers' non-empty blocks are fetched, left's first, each
  * in computeShuffleBlocks order, and ONE b2s_decompress_join_rows_keys_packed call (retried once with the exact size on
  * B2S_E_DST_TOO_SMALL) verifies, decodes, sorts and joins them; the arguments are that call's.  The exchange cache is
- * not consulted.  *data / *len: the joined rows (for semi and anti joins the left records), valid until left's next
- * read; *n_out_records of them.  Errors as read_sorted_rows_keys(). */
+ * not consulted.  join_type: every B2S_JOIN_* (right and full outer joins too; their null-side rows can make the
+ * output larger than the first size guess, which the retry covers).  *data / *len: the joined rows (for semi and anti
+ * joins the left records), valid until left's next read; *n_out_records of them.  Errors as read_sorted_rows_keys(). */
 int b2sh_reader_read_joined_rows(b2sh_reader* left, b2sh_reader* right, uint32_t join_type, uint32_t n_keys,
                                  const uint32_t* key_type, const uint32_t* key_len, const uint32_t* left_key_off,
                                  const int32_t* left_key_null_field, const uint32_t* right_key_off,

@@ -24,6 +24,7 @@ KEY_DESCENDING, KEY_NULLS_LAST = 1 << 8, 1 << 9
 AGG_SUM_DECIMAL, AGG_MIN_DECIMAL, AGG_MAX_DECIMAL = 9, 10, 11
 # join types of the row join (decompress_join_rows_keys_*) and the field kinds of its sides' schemas
 JOIN_INNER, JOIN_LEFT_OUTER, JOIN_LEFT_SEMI, JOIN_LEFT_ANTI = 0, 1, 2, 3
+JOIN_RIGHT_OUTER, JOIN_FULL_OUTER = 5, 6  # 4 is not assigned
 FIELD_FIXED, FIELD_VAR, FIELD_DECIMAL_WIDE = 0, 1, 2
 OK, E_CORRUPT, E_CHECKSUM, E_DST_TOO_SMALL, E_UNSUPPORTED, E_ARG, E_CUDA, E_NOT_INIT, E_NOMEM, E_NOT_CACHED = (
     0, -1, -2, -3, -4, -5, -6, -7, -8, -9)
@@ -562,8 +563,10 @@ def decompress_join_rows_keys_packed(join_type, codec, src, off, length, n_left,
     the rest the right's.  left_keys / right_keys: [(key type, row offset, length, null field or -1), ...] as in
     decompress_sort_rows_keys_packed without order flags, one entry per join key column on each side (the types and
     lengths are the left's).  The kinds (FIELD_*, one per field; None for semi and anti joins) say which slots hold an
-    offset.  dst receives Spark's joined rows ([int32 big-endian size][row]) for JOIN_INNER / JOIN_LEFT_OUTER, the left
-    records for JOIN_LEFT_SEMI / JOIN_LEFT_ANTI.
+    offset.  dst receives Spark's joined rows ([int32 big-endian size][row]) for JOIN_INNER / JOIN_LEFT_OUTER /
+    JOIN_RIGHT_OUTER / JOIN_FULL_OUTER (left.output ++ right.output; a right outer join in the right side's key order,
+    a full outer join run by run in key order, as the header states), the left records for JOIN_LEFT_SEMI /
+    JOIN_LEFT_ANTI.
     -> dict(total, n_left_records, n_right_records, n_out_records, status, bad_slice)"""
     n, kt, kl, lo, ln, ro, rn, lk, rk = _join_arrays(left_keys, right_keys, left_kinds, right_kinds)
     return _sort_call("b2s_decompress_join_rows_keys_packed", codec, src, off, length, dst, None,

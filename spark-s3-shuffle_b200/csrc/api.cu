@@ -2702,14 +2702,15 @@ static uint32_t bitset_words(uint32_t n) { return (n + 63) / 64; }
 // each side's fields, and every key slot and null bit inside its side's fixed region
 static int join_args(const RecordSpec& spec, uint32_t n) {
   const JoinSpec& js = *spec.join;
-  if (js.type > B2S_JOIN_LEFT_ANTI) return fail(B2S_E_ARG, "unknown join_type%s");
+  if (js.type > B2S_JOIN_FULL_OUTER || js.type == B2S_JOIN_LEFT_ANTI + 1)  // 4 is not assigned
+    return fail(B2S_E_ARG, "unknown join_type%s");
   if (js.n_left > n) return fail(B2S_E_ARG, "n_left must be at most n%s");
   RecordSpec right = spec;
   right.keys = js.right;
   right.key_arrays = js.right_arrays;
   if (int rc = key_columns_args(right)) return rc;
   const KeySpec* side[2] = {&spec.keys, &js.right};
-  const bool kinds = js.type == B2S_JOIN_INNER || js.type == B2S_JOIN_LEFT_OUTER;
+  const bool kinds = !join_keeps_whole(js.type);
   for (uint32_t s = 0; s < 2; s++) {
     const uint32_t nf = js.n_fields[s];
     if (nf < 1 || nf > 65536) return fail(B2S_E_ARG, "a side's field count must be in [1, 65536]%s");
@@ -2722,7 +2723,7 @@ static int join_args(const RecordSpec& spec, uint32_t n) {
         return fail(B2S_E_ARG, "a key null bit is not below its side's field count%s");
     }
     if (kinds) {
-      if (!js.kind[s]) return fail(B2S_E_ARG, "field kinds are required for inner and left outer joins%s");
+      if (!js.kind[s]) return fail(B2S_E_ARG, "field kinds are required for joins that build joined rows%s");
       for (uint32_t f = 0; f < nf; f++)
         if (js.kind[s][f] > B2S_FIELD_DECIMAL_WIDE) return fail(B2S_E_ARG, "unknown field kind%s");
     }
@@ -3387,7 +3388,8 @@ static int aggregate_rows_tail(Slot& S, const RecordSpec& spec, DecodedTask& T, 
 
 // A join's key columns per side (JoinKeys: a column nullable on one side only takes kNullByteOnly on the other, so
 // equal keys encode equal; split: the arena offset of the right side's first block) and its joined row's shape, whose
-// field lists (left VAR / DECIMAL_WIDE fields, right ones, right DECIMAL_WIDE ones) go to fields.
+// field lists (left VAR / DECIMAL_WIDE fields, right ones, right DECIMAL_WIDE ones, left DECIMAL_WIDE ones) go to
+// fields.
 static void join_layout(const RecordSpec& spec, uint64_t split, JoinKeys& jk, JoinShape& shape,
                         std::vector<uint32_t>& fields) {
   const JoinSpec& js = *spec.join;
@@ -3402,7 +3404,8 @@ static void join_layout(const RecordSpec& spec, uint64_t split, JoinKeys& jk, Jo
   jk.split = split;
   shape.type = js.type;
   shape.split = split;
-  shape.left_keys = spec.keys;
+  shape.keys[0] = spec.keys;
+  shape.keys[1] = js.right;
   for (uint32_t s = 0; s < 2; s++) {
     shape.n[s] = js.n_fields[s];
     shape.bw[s] = bitset_words(js.n_fields[s]);
@@ -3410,15 +3413,18 @@ static void join_layout(const RecordSpec& spec, uint64_t split, JoinKeys& jk, Jo
   }
   shape.out_bw = bitset_words(shape.n[0] + shape.n[1]);
   fields.clear();
-  const bool rows = js.type == B2S_JOIN_INNER || js.type == B2S_JOIN_LEFT_OUTER;  // a semi or anti join: no kinds
+  const bool rows = !join_keeps_whole(js.type);  // a semi or anti join: no kinds
   for (uint32_t s = 0; s < 2; s++) {
     for (uint32_t f = 0; rows && f < shape.n[s]; f++)
       if (js.kind[s][f] != B2S_FIELD_FIXED) fields.push_back(f);
     shape.n_var[s] = (uint32_t)fields.size() - (s ? shape.n_var[0] : 0);
   }
-  for (uint32_t f = 0; rows && f < shape.n[1]; f++)
-    if (js.kind[1][f] == B2S_FIELD_DECIMAL_WIDE) fields.push_back(f);
-  shape.n_wide_right = (uint32_t)fields.size() - shape.n_var[0] - shape.n_var[1];
+  for (uint32_t s : {1u, 0u}) {  // the null side's wide decimals: the right side's, then the left side's
+    const size_t before = fields.size();
+    for (uint32_t f = 0; rows && f < shape.n[s]; f++)
+      if (js.kind[s][f] == B2S_FIELD_DECIMAL_WIDE) fields.push_back(f);
+    shape.n_wide[s] = (uint32_t)(fields.size() - before);
+  }
 }
 
 // The end of a join: grouping, counts (one readback with the key pass's verdicts; *total = output bytes), the joined
@@ -3449,7 +3455,7 @@ static int join_rows_tail(Slot& S, const RecordSpec& spec, DecodedTask& T, const
     if (int rc = S.parena.ensure(jb[1] + 64)) return rc;
     *d_out = (uint8_t*)S.parena.p;
   }
-  launch_join_emit(T.arena, R.records, R.idx, jb[0], R.key_bytes, spec.join->type >= B2S_JOIN_LEFT_SEMI, R.ws,
+  launch_join_emit(T.arena, R.records, R.idx, jb[0], R.key_bytes, join_keeps_whole(spec.join->type), R.ws,
                    R.jws, T.n_src, *d_out, st, launches);
   CU(S.mark(G1, st, *launches));
   CU(S.mark(P1, st));

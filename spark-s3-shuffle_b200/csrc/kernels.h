@@ -484,28 +484,34 @@ const uint32_t* rows_group_starts(uint8_t* d_aws, uint64_t n);
 // The records of both sides, stably sorted together by the join key (launch_rows_join_order) and grouped
 // (launch_rows_group): each group holds its key's left records, then its right ones.  The shape of the joined row:
 // field counts n[s], null-bitset words bw[s] and out_bw of the inputs and the output, and the non-fixed fields (VAR and
-// DECIMAL_WIDE: their slots' offsets move) of each side, and the right side's DECIMAL_WIDE fields (the null right
-// side's 16-byte regions), as device lists.
+// DECIMAL_WIDE: their slots' offsets move) of each side, and each side's DECIMAL_WIDE fields (a null side's 16-byte
+// regions), as device lists.
 constexpr uint32_t kJoinInner = B2S_JOIN_INNER, kJoinLeftOuter = B2S_JOIN_LEFT_OUTER,
-                   kJoinLeftSemi = B2S_JOIN_LEFT_SEMI, kJoinLeftAnti = B2S_JOIN_LEFT_ANTI;
+                   kJoinLeftSemi = B2S_JOIN_LEFT_SEMI, kJoinLeftAnti = B2S_JOIN_LEFT_ANTI,
+                   kJoinRightOuter = B2S_JOIN_RIGHT_OUTER, kJoinFullOuter = B2S_JOIN_FULL_OUTER;
+// a semi or anti join: its output is the kept left records themselves, not joined rows
+__host__ __device__ inline bool join_keeps_whole(uint32_t type) {
+  return type == kJoinLeftSemi || type == kJoinLeftAnti;
+}
 struct JoinShape {
   uint32_t type;
   uint64_t split;      // the arena offset of the first right record (JoinKeys::split)
   uint32_t n[2], bw[2], out_bw;
-  uint32_t n_var[2], n_wide_right;
+  uint32_t n_var[2], n_wide[2];
   const uint32_t* var[2];
-  const uint32_t* wide_right;
-  KeySpec left_keys;   // the left side's key columns (a left record's null columns)
+  const uint32_t* wide[2];
+  KeySpec keys[2];     // each side's key columns (a record's null columns)
 };
 // d_jws: join_ws_bytes(n, n_ranges, n_fields) bytes; launch_join_count uploads the shape and its field lists (h_fields:
-// the left's non-fixed fields, the right's, the right's DECIMAL_WIDE ones)
+// the left's non-fixed fields, the right's, the right's DECIMAL_WIDE ones, the left's DECIMAL_WIDE ones)
 size_t join_ws_bytes(uint64_t n, uint32_t n_ranges, uint32_t n_fields);
 // the readback: [output records, output bytes, left records, a joined row is too long (0 / 1), verdict of range 0, 1,
 // ...] (the verdicts: launch_rows_join_order's)
 uint64_t* join_readback(uint8_t* d_jws, uint64_t n, uint32_t n_ranges);
 inline size_t join_readback_bytes(uint32_t n_ranges) { return (4 + (size_t)n_ranges) * 8; }
-// per left position its output records and bytes, scanned; the totals and the left record count into the readback
-// (its first four words).  idx: the sorted order (nullptr: arena order), heads as launch_rows_group's.
+// per sorted position (of either side) its output records and bytes, scanned; the totals and the left record count
+// into the readback (its first four words).  idx: the sorted order (nullptr: arena order), heads as
+// launch_rows_group's.
 void launch_join_count(const uint8_t* arena, uint64_t n, const uint32_t* idx, JoinShape shape,
                        const uint32_t* h_fields, uint32_t n_fields, uint32_t key_bytes, uint8_t* d_ws,
                        uint8_t* d_aws, uint8_t* d_jws, uint32_t n_ranges, cudaStream_t st, uint64_t* launches);

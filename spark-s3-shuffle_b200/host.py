@@ -406,7 +406,8 @@ class S3ShuffleReader:
                        rightKinds=None):
         """Spark's sort-merge join of this reader's partitions (the left side) with right's (the same partitions of
         another shuffle): both readers' blocks through ONE capi.decompress_join_rows_keys_packed call, whose arguments
-        these are.  -> (joined rows, n_left_records, n_right_records, n_out_records)"""
+        these are (joinType: any capi.JOIN_*, right and full outer included).
+        -> (joined rows, n_left_records, n_right_records, n_out_records)"""
         n, kt, kl, lo, ln, ro, rn, lk, rk = _join_arrays(leftKeys, rightKeys, leftKinds, rightKinds)
         p, size = _vp(), _u64()
         counts = [_u64(), _u64(), _u64()]

@@ -12,16 +12,22 @@ rows).  Workloads:
   b : the same with a (string, int) key: a 16-byte string made from the key and an int of key mod 7.
   c : a: plus a skewed key: 1 % of each reducer's left rows carry one hot key that 2000 right rows match (many to
       many: 2000 joined rows per hot left row).
-Every timed reducer's output is checked against the model (tests/join_model.py) before it is timed.  Per reducer,
-after one untimed call of each path, each path is timed once (b2s_last_timing: kernel_ms = the whole call on the
-device, dominant_ms = the join step); the sorts' kernel_ms are summed over the two calls.  The card's name and power
-limit are read in the same run.
+  d : a, with partners missing on both sides: no left row carries 25 % of the dimension's keys, and 10 % of the left
+      rows carry a key outside the dimension, so right and full outer joins emit null-side rows.
+--join-types (inner, left_outer, left_semi, left_anti, right_outer, full_outer; default inner) are joined on the same
+blocks.  Every timed reducer's output is checked against the model (tests/outer_join_model.py) before it is timed.  Per
+reducer, after one untimed call of each path, each path is timed once (b2s_last_timing: kernel_ms = the whole call on
+the device, dominant_ms = the join step); the sorts' kernel_ms are summed over the two calls.  The card's name and
+power limit are read in the same run.  --model-cache DIR keeps each checked output's length and SHA-256 there, so
+runs over the same blocks (two builds alternated) check against the model without recomputing it.
 
     python tools/join_rows_bench.py [--gib 2] [--maps 400] [--partitions 200] [--reducers 3] [--workloads a,b,c]
+                                    [--join-types inner]
 
 Prints one JSON document.
 """
 import argparse
+import hashlib
 import json
 import os
 import statistics
@@ -37,6 +43,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 SNAPPY, CRC32C = 2, 3
 INT64, INT32, STRING = 2, 1, 3
 FIXED, VAR = 0, 1
+JOIN_TYPES = {"inner": 0, "left_outer": 1, "left_semi": 2, "left_anti": 3, "right_outer": 5, "full_outer": 6}
 
 
 def card():
@@ -88,6 +95,9 @@ def reducer_sides(rng, workload, n_left, keys, partitions, red):
     share = np.arange(red, keys, partitions, dtype=np.int64)  # the dimension keys that hash here
     lk = rng.choice(share, n_left)
     rk = rng.permutation(share)
+    if workload == "d":  # the first quarter of rk has no left row; a tenth of the left rows no dimension row
+        lk = rng.choice(rk[rk.size // 4:], n_left)
+        lk[rng.random(n_left) < 0.1] += keys
     if workload == "c":
         hot = int(share[0])
         lk[rng.random(n_left) < 0.01] = hot
@@ -136,7 +146,7 @@ def blocks(capi, records, rec_len, maps, rng):
 
 
 def run(capi, args, workload, red, d_src, d_dst, cap):
-    from join_model import INNER, model_join
+    from outer_join_model import model_join
     rng = np.random.default_rng(1000 * red + ord(workload))
     n_left = int(args.gib * 2**30 / 84 / args.partitions)
     (lrec, llen, lkeys, lkind), (rrec, rlen, rkeys, rkind) = reducer_sides(rng, workload, n_left, args.keys,
@@ -150,11 +160,9 @@ def run(capi, args, workload, red, d_src, d_dst, cap):
     n = off.size
     sb, sl = np.arange(n + 1, dtype=np.uint32), ln.astype(np.uint64)
     capi.dev_memcpy(d_src, arena.ctypes.data, arena.size, 1)
-    want = model_join(INNER, lplain, rplain, lkeys, rkeys, 5, 3, lkind, rkind)
-    assert len(want[0]) <= cap, "--cap-gib is below the reducer's output"
 
-    def join():
-        r = capi.decompress_join_rows_keys_dev(INNER, SNAPPY, d_src, off, ln, args.maps, d_dst, cap, lkeys, rkeys, 5, 3,
+    def join(jt):
+        r = capi.decompress_join_rows_keys_dev(jt, SNAPPY, d_src, off, ln, args.maps, d_dst, cap, lkeys, rkeys, 5, 3,
                                                lkind, rkind, CRC32C, sb, sl, ck)
         return r, capi.last_timing()
 
@@ -166,15 +174,33 @@ def run(capi, args, workload, red, d_src, d_dst, cap):
             t.append(capi.last_timing()["kernel_ms"])
         return sum(t)
 
-    r, _ = join()
-    out = np.zeros(max(r["total"], 1), np.uint8)
-    capi.dev_memcpy(out.ctypes.data, d_dst, r["total"], 2)
-    assert out[:r["total"]].tobytes() == want[0] and r["n_out_records"] == want[3], "join output differs from the model"
+    res = {"in_bytes": int(llen.sum() + rlen.sum()), "left_rows": int(llen.size), "right_rows": int(rlen.size)}
+    for name in args.join_types.split(","):
+        jt = JOIN_TYPES[name]
+        cached = args.model_cache and os.path.join(args.model_cache, "%s-%s-%d-%s.json" % (
+            workload, name, red, hashlib.sha256(json.dumps([args.gib, args.maps, args.partitions, args.keys]).encode()).hexdigest()[:12]))
+        if cached and os.path.exists(cached):
+            want = json.load(open(cached))
+        else:
+            stream, _, _, rows = model_join(jt, lplain, rplain, lkeys, rkeys, 5, 3, lkind, rkind)
+            want = {"bytes": len(stream), "sha256": hashlib.sha256(stream).hexdigest(), "rows": rows}
+            if cached:
+                os.makedirs(args.model_cache, exist_ok=True)
+                json.dump(want, open(cached, "w"))
+        assert want["bytes"] <= cap, "--cap-gib is below the reducer's output"
+        r, _ = join(jt)
+        out = np.zeros(max(r["total"], 1), np.uint8)
+        capi.dev_memcpy(out.ctypes.data, d_dst, r["total"], 2)
+        got = hashlib.sha256(out[:r["total"]].tobytes()).hexdigest()
+        assert (got, r["n_out_records"]) == (want["sha256"], want["rows"]), "%s differs from the model" % name
+        _, t = join(jt)
+        res[name + "_kernel_ms"] = t["kernel_ms"]
+        res[name + "_step_ms"] = t["dominant_ms"]
+        res[name + "_out_rows"] = r["n_out_records"]
+        res[name + "_out_mb"] = r["total"] / 1e6
     sorts()
-    _, t = join()
-    return {"join_kernel_ms": t["kernel_ms"], "join_step_ms": t["dominant_ms"], "two_sorts_kernel_ms": sorts(),
-            "out_bytes": r["total"], "out_rows": r["n_out_records"], "left_rows": r["n_left_records"],
-            "right_rows": r["n_right_records"], "in_bytes": int(llen.sum() + rlen.sum())}
+    res["two_sorts_kernel_ms"] = sorts()
+    return res
 
 
 def main():
@@ -185,7 +211,9 @@ def main():
     ap.add_argument("--reducers", type=int, default=3)
     ap.add_argument("--keys", type=int, default=10**7)
     ap.add_argument("--workloads", default="a,b,c")
+    ap.add_argument("--join-types", default="inner", help="comma-separated: " + ", ".join(JOIN_TYPES))
     ap.add_argument("--cap-gib", type=float, default=1.0, help="device output buffer")
+    ap.add_argument("--model-cache", default=None, help="a directory for the model outputs' lengths and hashes")
     args = ap.parse_args()
     import spark_s3_shuffle_b200 as pkg
     capi = pkg.capi
