@@ -645,6 +645,86 @@ int b2s_decompress_join_rows_keys_dev(
     uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_left_records, uint64_t* n_right_records,
     uint64_t* n_out_records, int32_t* status, int32_t* bad_slice);
 
+/* ---- read side, window: Spark's WindowExec (ranking functions) on a reducer's shuffled UnsafeRows ----
+ * Spark SQL's Sort -> [WindowGroupLimit(Final) ->] Window over a shuffle read, for window expressions that are ranking
+ * functions with their default frame, in one call: the rows are sorted by the window's key, each record gets the
+ * values of the n_fns functions over its partition, and each output row is the input row joined with those values.
+ * Blocks, slices, checksums and framing as in b2s_decompress_sort_rows_packed: [size: int32 BE][row], no end marker.
+ * Keys.  The composite key of the *_keys calls: n_keys (at most 16) columns key_type[c] / key_off[c] / key_len[c] /
+ * key_null_field[c], every type of those calls.  Its first n_partition_keys columns (0..15) are the PARTITION BY
+ * columns and take no order flag (WindowExec.requiredChildOrdering sorts them ascending, nulls first); the remaining
+ * columns (at least one) are the ORDER BY columns, with any flags.  Records are stably sorted by the whole key, exactly
+ * as b2s_decompress_sort_rows_keys_* sorts them (ties in block order, then in their order in the block).
+ * Partitions and peers.  A partition is a maximal run of sorted records that are equal on the partition columns, by
+ * the composite-key aggregation's grouping rule: nulls equal nulls, strings are equal by length and bytes, 0.0 equals
+ * -0.0 and every NaN equals every other NaN (on input NormalizeFloatingNumbers has normalised, WindowExec's equality
+ * of the projected partition rows).  With n_partition_keys == 0 the whole reducer is one partition.  Peers are records
+ * of one partition that are equal on the order columns by the same rule (RankLike's EqualNullSafe).
+ * Functions.  fn[j] (j < n_fns, 1..16 of them, in any order, repeats allowed) is one of B2S_WINDOW_*.  With N the
+ * partition's size, i the record's 0-based position in it and [gs, ge) its peer group's positions in it:
+ *   ROW_NUMBER    int     i + 1
+ *   RANK          int     gs + 1
+ *   DENSE_RANK    int     the number of peer groups of the partition up to and including this one
+ *   PERCENT_RANK  double  N > 1 ? (double) gs / (N - 1) : 0.0
+ *   CUME_DIST     double  (double) ge / N
+ *   NTILE         int     NTile(k)'s bucket, k = fn_arg[j] (at least 1): the first N % k buckets hold N / k + 1 rows
+ *                         each, the rest N / k, numbered from 1 in sorted order
+ * fn_arg[j] must be 0 for every function but NTILE.
+ * Limit (WindowGroupLimitExec).  limit_fn is B2S_WINDOW_NO_LIMIT with limit 0 (every record is output), or one of
+ * ROW_NUMBER, RANK and DENSE_RANK with limit at least 1: then only the records whose value of limit_fn is at most limit
+ * are output, so rank ties at the boundary are all kept.  With a limit every fn[j] must be ROW_NUMBER, RANK or
+ * DENSE_RANK: the only case Spark's InferWindowGroupLimit plans, and the only one where the values of the kept rows do
+ * not depend on the dropped ones.
+ * Output row.  The input row joined with a row of the n_fns values, laid out as UnsafeRowJoiner joins them: the join's
+ * joined row (b2s_decompress_join_rows_keys_*) with a right side of n_fns non-null FIXED fields and no var bytes.  With
+ * nC = n_fields, bC = ceil(nC / 64) and b = ceil((nC + n_fns) / 64):
+ *   [b words: the input's nC null bits, zeros above][the input's 8 nC bytes of slots][8 bytes per function, in fn
+ *   order][the input's var bytes]
+ * An int value is written as UnsafeRowWriter writes it, the 8-byte slot zeroed and then 4 little-endian bytes; a double
+ * as its 8 bytes.  Every VAR or DECIMAL_WIDE field (field_kind, B2S_FIELD_* as for the join; required) whose slot is
+ * not zero has its offset (the high 32 bits) moved by 8 (b - bC + n_fns).
+ * Outputs.  The output rows in sorted order as [size BE][row] records, an UnsafeRowSerializer stream: *n_out_records of
+ * them, *dst_total bytes; dst_cap below that -> B2S_E_DST_TOO_SMALL with *dst_total = the bytes needed.  *n_records:
+ * the input record count.
+ * Errors -> B2S_E_ARG: a key column the composite-key calls reject; an order flag on a partition column; no order
+ * column (n_partition_keys >= n_keys, or above 15); a key slot outside the input's slots [8 bC, 8 (bC + nC)) or a key
+ * null bit not below nC; n_fields outside 1..65536; NULL or unknown field kinds; n_fns outside 1..16, NULL fn or fn_arg,
+ * an unknown fn, an NTILE bucket count below 1 or a non-zero fn_arg of another function; a limit_fn that is none of
+ * the four, B2S_WINDOW_NO_LIMIT with a non-zero limit, a limit below 1, or a limit with a function other than the
+ * three; a NULL count pointer; more than 2^32 - 1 input records.
+ * Per block, B2S_E_CORRUPT for every framing rule of the composite-key calls and when a row is shorter than the input's
+ * fixed region 8 (bC + nC); b2s_last_error() names the block and the byte offset of the bad record.  A partition of
+ * more than 2^31 - 1 records (Spark's int values would wrap) or an output row longer than 2^31 - 1 bytes ->
+ * B2S_E_UNSUPPORTED.  When a block fails nothing is written, every count is 0 and the call returns 0.  Checksums and
+ * bad_slice, codec NONE and B2S_E_NOMEM (the caller keeps Spark's window) are as in the sorts.
+ * Runs on the read lane with the sorts' 1 GiB buffer trim.  b2s_last_timing: kernel_ms the whole call, top_kernel_ms
+ * framing through emit, dominant_ms / dominant_launches the window step alone (from the sorted order to the written
+ * rows). */
+#define B2S_WINDOW_ROW_NUMBER 0
+#define B2S_WINDOW_RANK 1
+#define B2S_WINDOW_DENSE_RANK 2
+#define B2S_WINDOW_PERCENT_RANK 3
+#define B2S_WINDOW_CUME_DIST 4
+#define B2S_WINDOW_NTILE 5
+#define B2S_WINDOW_NO_LIMIT 0xffffffffu
+int b2s_decompress_window_rows_keys_packed(
+    uint32_t codec, uint32_t checksum_alg, uint32_t n, const uint8_t* src_base, const uint64_t* src_off,
+    const uint64_t* src_len, const uint32_t* slice_base, const uint64_t* slice_len, const uint64_t* slice_checksum,
+    uint32_t n_partition_keys, uint32_t n_keys, const uint32_t* key_type, const uint32_t* key_off,
+    const uint32_t* key_len, const int32_t* key_null_field, uint32_t n_fields, const uint8_t* field_kind,
+    uint32_t n_fns, const uint32_t* fn, const int32_t* fn_arg, uint32_t limit_fn, int32_t limit,
+    uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records, uint64_t* n_out_records,
+    int32_t* status, int32_t* bad_slice);
+/* same, with src_base / dst_base in device memory of dev_index; every array stays a host array */
+int b2s_decompress_window_rows_keys_dev(
+    uint32_t dev_index, uint32_t codec, uint32_t checksum_alg, uint32_t n, const uint8_t* src_base,
+    const uint64_t* src_off, const uint64_t* src_len, const uint32_t* slice_base, const uint64_t* slice_len,
+    const uint64_t* slice_checksum, uint32_t n_partition_keys, uint32_t n_keys, const uint32_t* key_type,
+    const uint32_t* key_off, const uint32_t* key_len, const int32_t* key_null_field, uint32_t n_fields,
+    const uint8_t* field_kind, uint32_t n_fns, const uint32_t* fn, const int32_t* fn_arg, uint32_t limit_fn,
+    int32_t limit, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records,
+    uint64_t* n_out_records, int32_t* status, int32_t* bad_slice);
+
 /* ---- exchange cache: map outputs kept resident in HBM for reducers on the same device ----
  * (docs/f4_gpu_resident_exchange.md steps 2 and 3, local half.)  The serialized writer's partition step already leaves
  * a map task's records partitioned by reduce id in HBM; the cached store keeps that arena, keyed by (shuffle_id,

@@ -222,6 +222,17 @@ int b2sh_reader_read_joined_rows(b2sh_reader* left, b2sh_reader* right, uint32_t
                                  const uint8_t* left_field_kind, uint32_t n_right_fields,
                                  const uint8_t* right_field_kind, const uint8_t** data, uint64_t* len,
                                  uint64_t* n_left_records, uint64_t* n_right_records, uint64_t* n_out_records);
+/* read_window_rows(): Spark's Sort [-> WindowGroupLimit(Final)] -> Window over this reader's reduce partitions for the
+ * ranking functions (INTEGRATION.md §3o).  Every non-empty block is fetched in computeShuffleBlocks order and ONE
+ * b2s_decompress_window_rows_keys_packed call (retried once with the exact size on B2S_E_DST_TOO_SMALL) verifies,
+ * decodes and sorts the rows and evaluates the functions; the arguments are that call's.  The exchange cache is not
+ * consulted.  *data / *len: the output rows, valid until the reader's next read; *n_out_records of them, out of
+ * *n_records input records.  Errors as read_sorted_rows_keys(). */
+int b2sh_reader_read_window_rows(b2sh_reader* r, uint32_t n_partition_keys, uint32_t n_keys, const uint32_t* key_type,
+                                 const uint32_t* key_off, const uint32_t* key_len, const int32_t* key_null_field,
+                                 uint32_t n_fields, const uint8_t* field_kind, uint32_t n_fns, const uint32_t* fn,
+                                 const int32_t* fn_arg, uint32_t limit_fn, int32_t limit, const uint8_t** data,
+                                 uint64_t* len, uint64_t* n_records, uint64_t* n_out_records);
 int b2sh_reader_block(b2sh_reader* r, uint32_t k, int64_t* map_id, int32_t* start_reduce, int32_t* end_reduce,
                       const uint8_t** data, uint64_t* len);
 uint64_t b2sh_reader_remote_bytes_read(b2sh_reader* r); /* metric parity with storage/S3ShuffleReader.scala:94-95 */

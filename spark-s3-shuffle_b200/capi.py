@@ -26,6 +26,9 @@ AGG_SUM_DECIMAL, AGG_MIN_DECIMAL, AGG_MAX_DECIMAL = 9, 10, 11
 JOIN_INNER, JOIN_LEFT_OUTER, JOIN_LEFT_SEMI, JOIN_LEFT_ANTI = 0, 1, 2, 3
 JOIN_RIGHT_OUTER, JOIN_FULL_OUTER = 5, 6  # 4 is not assigned
 FIELD_FIXED, FIELD_VAR, FIELD_DECIMAL_WIDE = 0, 1, 2
+# ranking functions of the row window (decompress_window_rows_keys_*), and its limit function meaning "no limit"
+WINDOW_ROW_NUMBER, WINDOW_RANK, WINDOW_DENSE_RANK, WINDOW_PERCENT_RANK, WINDOW_CUME_DIST, WINDOW_NTILE = range(6)
+WINDOW_NO_LIMIT = 0xFFFFFFFF
 OK, E_CORRUPT, E_CHECKSUM, E_DST_TOO_SMALL, E_UNSUPPORTED, E_ARG, E_CUDA, E_NOT_INIT, E_NOMEM, E_NOT_CACHED = (
     0, -1, -2, -3, -4, -5, -6, -7, -8, -9)
 NOT_RESIDENT = 2**64 - 1  # b2s_exchange_lookup's length of a map output that is not resident
@@ -138,6 +141,12 @@ PROTOTYPES = [
     ("b2s_decompress_join_rows_keys_dev", C.c_int,
      [_u32, _u32, _u32, _u32, _u32, _u32, _vp, _u64p, _u64p, _u32p, _u64p, _u64p, _u32, _u32p, _u32p, _u32p, _i32p,
       _u32p, _i32p, _u32, _u8p, _u32, _u8p, _vp, _u64, _u64p, _u64p, _u64p, _u64p, _i32p, _i32p]),
+    ("b2s_decompress_window_rows_keys_packed", C.c_int,
+     [_u32, _u32, _u32, _u8p, _u64p, _u64p, _u32p, _u64p, _u64p, _u32, _u32, _u32p, _u32p, _u32p, _i32p, _u32, _u8p,
+      _u32, _u32p, _i32p, _u32, _i32, _u8p, _u64, _u64p, _u64p, _u64p, _i32p, _i32p]),
+    ("b2s_decompress_window_rows_keys_dev", C.c_int,
+     [_u32, _u32, _u32, _u32, _vp, _u64p, _u64p, _u32p, _u64p, _u64p, _u32, _u32, _u32p, _u32p, _u32p, _i32p, _u32,
+      _u8p, _u32, _u32p, _i32p, _u32, _i32, _vp, _u64, _u64p, _u64p, _u64p, _i32p, _i32p]),
     ("b2s_exchange_set_budget", C.c_int, [_u32, _u64]),
     ("b2s_partition_compress_cached_packed", C.c_int,
      [_i32, C.c_int64, _u32, _i32, _u32, _u32, _u32, _u64, _u8p, _u64, _u32p, _u32p, _u8p, _u64, _u64p, _u64p, _u64p,
@@ -476,7 +485,8 @@ def _sort_call(symbol, codec, src, off, length, dst, dst_cap, mid, checksum_alg,
     packed form, src and dst host arrays (dst_cap is dst's size); else src and dst are device addresses.  lead,
     before_n and mid are the call's own arguments, numpy arrays among them passed as pointers; n defaults to the number
     of blocks in off.  -> dict(total, n_records, status, bad_slice), with n_groups after n_records for the aggregate
-    calls; the join calls return n_left_records, n_right_records and n_out_records in n_records' place"""
+    calls; the join calls return n_left_records, n_right_records and n_out_records in n_records' place, the window
+    calls n_records and n_out_records"""
     if dev is None:
         src, dst = _as_u8(src), _as_u8(dst)
         dst_cap = dst.size
@@ -487,6 +497,7 @@ def _sort_call(symbol, codec, src, off, length, dst, dst_cap, mid, checksum_alg,
     st = np.zeros(max(n, 1), dtype=np.int32)
     bad = np.zeros(max(n, 1), dtype=np.int32)
     names = (("total", "n_left_records", "n_right_records", "n_out_records") if "_join_" in symbol else
+             ("total", "n_records", "n_out_records") if "_window_" in symbol else
              ("total", "n_records", "n_groups") if "_aggregate_" in symbol else ("total", "n_records"))
     counts = [_u64(0) for _ in names]
     args = ([] if dev is None else [dev]) + [*lead, codec, checksum_alg, *before_n, n, src, off, length, sb, sl, sc,
@@ -572,6 +583,34 @@ def decompress_join_rows_keys_packed(join_type, codec, src, off, length, n_left,
     return _sort_call("b2s_decompress_join_rows_keys_packed", codec, src, off, length, dst, None,
                       (n, kt, kl, lo, ln, ro, rn, n_left_fields, lk, n_right_fields, rk), checksum_alg,
                       (slice_base, slice_len, slice_checksum), lead=(join_type,), before_n=(n_left,))
+
+
+def _window_arrays(keys, n_partition_keys, n_fields, kinds, fns, limit):
+    """the window's key, field-kind, function and limit arguments: fns = [fn or (WINDOW_NTILE, k), ...]; limit None
+    (no limit) or (limit_fn, limit)"""
+    n, kt, ko, kl, kn = _key_arrays(keys)
+    fns = [f if isinstance(f, tuple) else (f, 0) for f in fns]
+    fn = np.array([f[0] for f in fns] or [0], dtype=np.uint32)
+    arg = np.array([f[1] for f in fns] or [0], dtype=np.int32)
+    kinds = None if kinds is None else np.ascontiguousarray(kinds, dtype=np.uint8)
+    limit_fn, lim = (WINDOW_NO_LIMIT, 0) if limit is None else limit
+    return n_partition_keys, n, kt, ko, kl, kn, n_fields, kinds, len(fns), fn, arg, limit_fn, lim
+
+
+def decompress_window_rows_keys_packed(codec, src, off, length, dst, keys, n_partition_keys, n_fields, kinds, fns,
+                                       limit=None, checksum_alg=CHECKSUM_NONE, slice_base=None, slice_len=None,
+                                       slice_checksum=None):
+    """Spark's WindowExec with ranking functions over a reducer's UnsafeRow records: keys as in
+    decompress_sort_rows_keys_packed, the first n_partition_keys of them the PARTITION BY columns (no order flags), the
+    rest the ORDER BY columns; n_fields / kinds (FIELD_*, one per field) the input schema; fns the functions
+    (WINDOW_ROW_NUMBER, WINDOW_RANK, WINDOW_DENSE_RANK, WINDOW_PERCENT_RANK, WINDOW_CUME_DIST, or (WINDOW_NTILE, k)),
+    each appended to the row as one 8-byte field; limit None or (WINDOW_ROW_NUMBER / RANK / DENSE_RANK, n): only the
+    rows whose value of that function is at most n (WindowGroupLimitExec).  dst receives the output rows in sorted
+    order ([int32 big-endian size][row], the input row joined with the values as UnsafeRowJoiner joins them).
+    -> dict(total, n_records, n_out_records, status, bad_slice)"""
+    return _sort_call("b2s_decompress_window_rows_keys_packed", codec, src, off, length, dst, None,
+                      _window_arrays(keys, n_partition_keys, n_fields, kinds, fns, limit), checksum_alg,
+                      (slice_base, slice_len, slice_checksum))
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -685,6 +724,15 @@ def decompress_join_rows_keys_dev(join_type, codec, d_src, off, length, n_left, 
     return _sort_call("b2s_decompress_join_rows_keys_dev", codec, d_src, off, length, d_dst, dst_cap,
                       (n, kt, kl, lo, ln, ro, rn, n_left_fields, lk, n_right_fields, rk), checksum_alg,
                       (slice_base, slice_len, slice_checksum), dev, lead=(join_type,), before_n=(n_left,))
+
+
+def decompress_window_rows_keys_dev(codec, d_src, off, length, d_dst, dst_cap, keys, n_partition_keys, n_fields, kinds,
+                                    fns, limit=None, checksum_alg=CHECKSUM_NONE, slice_base=None, slice_len=None,
+                                    slice_checksum=None, dev=0):
+    """decompress_window_rows_keys_packed on device-resident blocks (d_src) into a device arena (d_dst)"""
+    return _sort_call("b2s_decompress_window_rows_keys_dev", codec, d_src, off, length, d_dst, dst_cap,
+                      _window_arrays(keys, n_partition_keys, n_fields, kinds, fns, limit), checksum_alg,
+                      (slice_base, slice_len, slice_checksum), dev)
 
 
 def partition_compress_dev(codec, d_records, rec_bytes, d_rec_len, d_rec_part, n_records, num_partitions, d_dst,

@@ -822,7 +822,7 @@ int get_device(uint32_t dev_index, Device** out) {
 }
 
 // the kinds of call whose steps add_times reads into b2s_last_timing, one rule each
-enum class Family { kCodec, kPartition, kPartitionNone, kSort, kSortRows, kAggregate, kJoin };
+enum class Family { kCodec, kPartition, kPartitionNone, kSort, kSortRows, kAggregate, kJoin, kWindow };
 
 // Adds the times of this call's steps on S to b2s_last_timing: kernel_ms, top_kernel_ms, dominant_ms / _launches by
 // the rule of its family, and h2d_ms.  A step the call did not run reads 0; one it started but did not finish ends
@@ -851,6 +851,7 @@ void add_times(Slot& S, Family f) {
     case Family::kSortRows:   // the same; framing + order + gather; the framing (walk + count, emit)
     case Family::kAggregate:  // the same; framing through merge; grouping + merge
     case Family::kJoin:       // the same; framing through join; the join step (grouping, counts, emit)
+    case Family::kWindow:     // the same; framing through emit; the window step (grouping, values, emit)
       t.kernel_ms += S.span(K0, P1);
       t.top_kernel_ms += S.span(P0, P1);
       if (f == Family::kSort) S.take_pairs();
@@ -858,7 +859,7 @@ void add_times(Slot& S, Family f) {
         dominant(F0, F1);
         dominant(F2, F3);
       }
-      if (f == Family::kAggregate || f == Family::kJoin) dominant(G0, G1);
+      if (f == Family::kAggregate || f == Family::kJoin || f == Family::kWindow) dominant(G0, G1);
       break;
   }
   t.h2d_ms += S.span(H0, H1);
@@ -2518,6 +2519,7 @@ int b2s_decompress_packed(uint32_t codec, uint32_t checksum_alg, uint32_t n, con
 // records (rows: [size: int32 big-endian][row], key columns in the row, each with its null bit).  aggregate: rows
 // grouped by the key and merged (b2s_decompress_aggregate_rows_*: the caller's n_aggs aggregates), not sorted.
 struct JoinSpec;
+struct WindowSpec;
 struct RecordSpec {
   bool is_rows = false;
   uint32_t record_bytes = 0;
@@ -2531,9 +2533,11 @@ struct RecordSpec {
   const uint32_t* agg_off = nullptr;
   const int32_t* agg_null_field = nullptr;
   const JoinSpec* join = nullptr;  // a join: keys are the left side's columns
+  const WindowSpec* window = nullptr;  // a window: keys are the partition columns, then the order columns
   bool rows() const { return is_rows; }
   Family family() const {
-    return join ? Family::kJoin : aggregate ? Family::kAggregate : is_rows ? Family::kSortRows : Family::kSort;
+    return join ? Family::kJoin : window ? Family::kWindow : aggregate ? Family::kAggregate
+           : is_rows ? Family::kSortRows : Family::kSort;
   }
 };
 // A join's other arguments (b2s_decompress_join_rows_keys_*): its type, the left blocks, the right side's key columns,
@@ -2546,6 +2550,19 @@ struct JoinSpec {
   uint32_t n_fields[2] = {};
   const uint8_t* kind[2] = {};
   uint64_t* n_side[2] = {};
+};
+// A window's other arguments (b2s_decompress_window_rows_keys_*): how many key columns partition, the input's fields
+// and kinds, the functions and their arguments, the limit, and the input record count it returns.
+struct WindowSpec {
+  uint32_t n_partition_keys = 0;
+  uint32_t n_fields = 0;
+  const uint8_t* kind = nullptr;
+  uint32_t n_fns = 0;
+  const uint32_t* fn = nullptr;
+  const int32_t* fn_arg = nullptr;
+  uint32_t limit_fn = B2S_WINDOW_NO_LIMIT;
+  int32_t limit = 0;
+  uint64_t* n_in = nullptr;
 };
 static RecordSpec fixed_spec(uint32_t record_bytes, uint32_t key_off, uint32_t key_len) {
   RecordSpec r;
@@ -2733,6 +2750,43 @@ static int join_args(const RecordSpec& spec, uint32_t n) {
   return 0;
 }
 
+// a window's checks past the composite key's: the partition columns (no flag, at least one order column after them),
+// the input's fields and every key slot and null bit inside them, the functions and the limit
+static int window_args(const RecordSpec& spec) {
+  const WindowSpec& ws = *spec.window;
+  const KeySpec& ks = spec.keys;
+  if (ws.n_partition_keys >= spec.n_keys || ws.n_partition_keys >= kMaxKeys)
+    return fail(B2S_E_ARG, "n_partition_keys must be in [0, 15] and leave at least one ORDER BY column%s");
+  for (uint32_t c = 0; c < ws.n_partition_keys; c++)
+    if (ks.type[c] & ~kKeyTypeMask) return fail(B2S_E_ARG, "a partition column takes no order flag%s");
+  const uint32_t nf = ws.n_fields;
+  if (nf < 1 || nf > 65536) return fail(B2S_E_ARG, "n_fields must be in [1, 65536]%s");
+  const uint64_t lo = 8ull * bitset_words(nf), hi = lo + 8ull * nf;
+  for (uint32_t c = 0; c < ks.n; c++) {
+    if (ks.off[c] < lo || (uint64_t)ks.off[c] + ks.len[c] > hi)
+      return fail(B2S_E_ARG, "a key slot lies outside the input's field slots%s");
+    if (ks.null_field[c] >= (int64_t)nf) return fail(B2S_E_ARG, "a key null bit is not below n_fields%s");
+  }
+  if (!ws.kind) return fail(B2S_E_ARG, "field kinds are required%s");
+  for (uint32_t f = 0; f < nf; f++)
+    if (ws.kind[f] > B2S_FIELD_DECIMAL_WIDE) return fail(B2S_E_ARG, "unknown field kind%s");
+  if (ws.n_fns < 1 || ws.n_fns > kMaxWindowFns) return fail(B2S_E_ARG, "n_fns must be in [1, 16]%s");
+  if (!ws.fn || !ws.fn_arg || !ws.n_in) return fail(B2S_E_ARG, "null argument%s");
+  const bool limited = ws.limit_fn != B2S_WINDOW_NO_LIMIT;
+  auto rank_like = [](uint32_t f) { return f <= B2S_WINDOW_DENSE_RANK; };
+  for (uint32_t j = 0; j < ws.n_fns; j++) {
+    if (ws.fn[j] > B2S_WINDOW_NTILE) return fail(B2S_E_ARG, "unknown window function%s");
+    if (ws.fn[j] == B2S_WINDOW_NTILE ? ws.fn_arg[j] < 1 : ws.fn_arg[j] != 0)
+      return fail(B2S_E_ARG, "fn_arg must be NTILE's bucket count (at least 1), and 0 for every other function%s");
+    if (limited && !rank_like(ws.fn[j]))
+      return fail(B2S_E_ARG, "with a limit every function must be ROW_NUMBER, RANK or DENSE_RANK%s");
+  }
+  if (limited ? !rank_like(ws.limit_fn) || ws.limit < 1 : ws.limit != 0)
+    return fail(B2S_E_ARG, "limit_fn must be B2S_WINDOW_NO_LIMIT with limit 0, or ROW_NUMBER, RANK or DENSE_RANK with "
+                           "a limit of at least 1%s");
+  return 0;
+}
+
 static int sort_args(uint32_t codec, uint32_t alg, uint32_t n, const uint64_t* src_off, const uint64_t* src_len,
                      const uint32_t* slice_base, const uint64_t* slice_len, const uint64_t* slice_checksum,
                      const RecordSpec& spec, const void* src_base, const void* dst_base, uint64_t dst_cap,
@@ -2746,6 +2800,8 @@ static int sort_args(uint32_t codec, uint32_t alg, uint32_t n, const uint64_t* s
       if (int rc = agg_args(spec)) return rc;
     if (spec.join)
       if (int rc = join_args(spec, n)) return rc;
+    if (spec.window)
+      if (int rc = window_args(spec)) return rc;
   } else {
     const uint32_t key_len = ks.len[0];
     if (spec.record_bytes == 0) return fail(B2S_E_ARG, "record_bytes must be at least 1%s");
@@ -3183,7 +3239,8 @@ static int decode_task(Device* D, Slot& S, uint32_t codec, uint32_t alg, uint32_
   if (T.failed) return T.report();
   if (!spec.rows() && T.total / spec.record_bytes > 0xffffffffull)
     return fail(B2S_E_ARG, "more than 2^32 - 1 records in one call (%s bytes)", std::to_string(T.total).c_str());
-  if (!spec.aggregate && !spec.join && T.total > out_cap) {  // an aggregation's or join's output is sized later
+  // an aggregation's, join's or window's output is sized later
+  if (!spec.aggregate && !spec.join && !spec.window && T.total > out_cap) {
     T.report();
     return fail(B2S_E_DST_TOO_SMALL, "dst_cap is below the %s decoded bytes", std::to_string(T.total).c_str());
   }
@@ -3233,8 +3290,9 @@ static int decode_task(Device* D, Slot& S, uint32_t codec, uint32_t alg, uint32_
 static void take_verdicts(DecodedTask& T, const RecordSpec& spec, const uint64_t* v) {
   const char* const why[] = {"", "the block ends inside a size prefix", "the size is negative",
                              "the record runs past the block end",
-                             spec.join ? "the row is shorter than its side's fixed region"
-                                       : "the row is shorter than key_off + key_len",
+                             spec.join     ? "the row is shorter than its side's fixed region"
+                             : spec.window ? "the row is shorter than its fixed region"
+                                           : "the row is shorter than key_off + key_len",
                              "the row does not hold the null-bit word", "the row is shorter than an aggregate slot",
                              "a string key runs past the end of its row, or a decimal key's size "
                              "is not in [1, 16] or its bytes run past the end of its row"};
@@ -3243,15 +3301,16 @@ static void take_verdicts(DecodedTask& T, const RecordSpec& spec, const uint64_t
 }
 
 // A reduce task's rows in key order (order_rows): idx (nullptr: arena order), heads (nullptr: where key words differ),
-// and S.pws's parts in order: sort, aggregation, refinement (nullptr unless the key refines), join grouping, join.
+// and S.pws's parts in order: sort, aggregation, refinement (nullptr unless the key refines), join or window grouping,
+// join, window.
 struct RowOrder {
   uint64_t records = 0;
   uint32_t key_bytes = 0;
   const uint32_t *idx = nullptr, *heads = nullptr;
-  uint8_t *ws = nullptr, *aws = nullptr, *rws = nullptr, *gws = nullptr, *jws = nullptr;
-  void carve(uint8_t* base, const size_t (&bytes)[5]) {
-    uint8_t** part[] = {&ws, &aws, &rws, &gws, &jws};
-    for (int k = 0; k < 5; k++) {
+  uint8_t *ws = nullptr, *aws = nullptr, *rws = nullptr, *gws = nullptr, *jws = nullptr, *wws = nullptr;
+  void carve(uint8_t* base, const size_t (&bytes)[6]) {
+    uint8_t** part[] = {&ws, &aws, &rws, &gws, &jws, &wws};
+    for (int k = 0; k < 6; k++) {
       *part[k] = base;
       base += bytes[k];
     }
@@ -3271,6 +3330,8 @@ static int order_rows(Slot& S, const RecordSpec& spec, DecodedTask& T, const Joi
     min_key = std::max<uint64_t>(min_key, (uint64_t)ks.off[c] + ks.len[c]);
     if (ks.null_field[c] >= 0) min_null = std::max<uint64_t>(min_null, null_word(ks.null_field[c]) + 8);
   }
+  const WindowSpec* win = spec.window;  // a window's rows hold its whole fixed region, which holds every key slot
+  if (win) min_key = 8ull * (bitset_words(win->n_fields) + win->n_fields);
   // a cached range with record boundaries is marked from them instead of walked (its walk is empty)
   std::vector<uint64_t> walk(T.length);
   std::vector<RowsMark> marks;
@@ -3303,12 +3364,13 @@ static int order_rows(Slot& S, const RecordSpec& spec, DecodedTask& T, const Joi
   const KeySpec& encoded = jk ? jk->side[0] : ks;
   R.key_bytes = rows_key_bytes(encoded);
   const bool refine = rows_key_refines(encoded);
-  const size_t part[5] = {rows_sort_ws_bytes(records, R.key_bytes),
+  const size_t part[6] = {rows_sort_ws_bytes(records, R.key_bytes),
                           spec.aggregate ? rows_aggregate_ws_bytes(records, spec.n_aggs, agg_spec(spec).n_wide) : 0,
                           refine ? rows_refine_ws_bytes(records, n_src) : 0,
-                          jk ? rows_aggregate_ws_bytes(records, 0, 0) : 0,
-                          jk ? join_ws_bytes(records, n_src, n_join_fields) : 0};
-  if ((records || jk) && (rc = S.pws.ensure(part[0] + part[1] + part[2] + part[3] + part[4]))) return rc;
+                          jk || win ? rows_aggregate_ws_bytes(records, 0, 0) : 0,
+                          jk ? join_ws_bytes(records, n_src, n_join_fields) : 0,
+                          win ? window_ws_bytes(records, win->n_fns, win->n_fields) : 0};
+  if ((records || jk) && (rc = S.pws.ensure(part[0] + part[1] + part[2] + part[3] + part[4] + part[5]))) return rc;
   R.carve((uint8_t*)S.pws.p, part);
   if (!refine) R.rws = nullptr;
   CU(S.mark(F2, st, *launches));
@@ -3467,12 +3529,72 @@ static int join_rows_tail(Slot& S, const RecordSpec& spec, DecodedTask& T, const
   return 0;
 }
 
+// The end of a window: grouping (the peer groups), then partitions, values and output bytes (one readback: *total =
+// output bytes), the output rows into *d_out (nullptr: into S.parena, returned there) and the input record count.  The
+// dominant step (G0, G1).
+static int window_rows_tail(Slot& S, const RecordSpec& spec, DecodedTask& T, const RowOrder& R, uint8_t** d_out,
+                            uint64_t out_cap, uint64_t* total, uint64_t* n_rec, uint64_t* launches) {
+  cudaStream_t st = S.st;
+  const WindowSpec& ws = *spec.window;
+  WindowShape shape{};
+  shape.n = ws.n_fields;
+  shape.bw = bitset_words(ws.n_fields);
+  shape.out_bw = bitset_words(ws.n_fields + ws.n_fns);
+  shape.n_fns = ws.n_fns;
+  for (uint32_t j = 0; j < ws.n_fns; j++) {
+    shape.fn[j] = ws.fn[j];
+    shape.arg[j] = (uint32_t)ws.fn_arg[j];
+  }
+  shape.limit_fn = ws.limit_fn;
+  shape.limit = ws.limit;
+  shape.part.n = ws.n_partition_keys;
+  for (uint32_t c = 0; c < ws.n_partition_keys; c++) {
+    shape.part.type[c] = spec.keys.type[c];
+    shape.part.off[c] = spec.keys.off[c];
+    shape.part.len[c] = spec.keys.len[c];
+    shape.part.null_field[c] = spec.keys.null_field[c];
+  }
+  std::vector<uint32_t> fields;  // the slots whose offsets move
+  for (uint32_t f = 0; f < ws.n_fields; f++)
+    if (ws.kind[f] != B2S_FIELD_FIXED) fields.push_back(f);
+  shape.n_var = (uint32_t)fields.size();
+  uint64_t wb[4] = {0, 0, 0, 0};  // output records, output bytes, a row too long, a partition too large
+  CU(S.mark(G0, st, *launches));
+  if (R.records) {
+    launch_rows_group(T.arena, R.records, R.idx, R.heads, R.key_bytes, AggSpec{}, R.ws, R.gws, st, launches);
+    launch_window_values(T.arena, R.records, R.idx, shape, fields.data(), R.key_bytes, R.ws, R.gws, R.wws, st,
+                         launches);
+    CU(cudaMemcpyAsync(wb, window_readback(R.wws, R.records, ws.n_fns), kWindowReadbackBytes, cudaMemcpyDeviceToHost,
+                       st));
+    CU(cudaStreamSynchronize(st));
+    CU(cudaGetLastError());
+  }
+  if (wb[3]) return fail(B2S_E_UNSUPPORTED, "a window partition holds more than 2^31 - 1 records%s");
+  if (wb[2]) return fail(B2S_E_UNSUPPORTED, "an output row is longer than 2^31 - 1 bytes%s");
+  *total = wb[1];
+  if (wb[1] > out_cap)
+    return fail(B2S_E_DST_TOO_SMALL, "dst_cap is below the %s output bytes", std::to_string(wb[1]).c_str());
+  if (!*d_out) {
+    if (int rc = S.parena.ensure(wb[1] + 64)) return rc;
+    *d_out = (uint8_t*)S.parena.p;
+  }
+  launch_window_emit(T.arena, R.records, R.idx, wb[0], R.key_bytes, ws.n_fns, ws.limit_fn != B2S_WINDOW_NO_LIMIT,
+                     R.ws, R.wws, *d_out, st, launches);
+  CU(S.mark(G1, st, *launches));
+  CU(S.mark(P1, st));
+  CU(cudaStreamSynchronize(st));
+  CU(cudaGetLastError());
+  *n_rec = wb[0];
+  *ws.n_in = R.records;
+  return 0;
+}
+
 // After decode_task: the fixed-size records' key sort, or order_rows and the tail of the call's family (a row sort's:
 // the gather), into *d_sorted (nullptr: into S.parena, returned there).  A failed source: 0, status[] set, *n_rec 0.
 static int run_reduce_task(Slot& S, const RecordSpec& spec, DecodedTask& T, uint8_t** d_sorted, uint64_t out_cap,
                            uint64_t* total, uint64_t* n_rec, uint64_t* n_groups, uint64_t* launches) {
   int rc;
-  if (!*d_sorted && !spec.join) {
+  if (!*d_sorted && !spec.join && !spec.window) {
     if ((rc = S.parena.ensure(T.total + 64))) return rc;
     *d_sorted = (uint8_t*)S.parena.p;
   }
@@ -3495,6 +3617,7 @@ static int run_reduce_task(Slot& S, const RecordSpec& spec, DecodedTask& T, uint
     rc = order_rows(S, spec, T, spec.join ? &jk : nullptr, (uint32_t)join_fields.size(), R, launches);
     if (rc || T.failed) return rc;
     if (spec.join) return join_rows_tail(S, spec, T, R, shape, join_fields, d_sorted, out_cap, total, n_rec, launches);
+    if (spec.window) return window_rows_tail(S, spec, T, R, d_sorted, out_cap, total, n_rec, launches);
     if (spec.aggregate) return aggregate_rows_tail(S, spec, T, R, *d_sorted, out_cap, total, n_rec, n_groups, launches);
     records = R.records;
     launch_rows_gather(T.arena, records, R.key_bytes, R.idx, R.ws, *d_sorted, S.st, launches);
@@ -3878,6 +4001,63 @@ int b2s_decompress_join_rows_keys_dev(
                    right_key_off, right_key_null_field, n_left_fields, left_field_kind, n_right_fields,
                    right_field_kind, dst_base, dst_cap, dst_total, n_left_records, n_right_records, n_out_records,
                    status, bad_slice);
+}
+
+// The window calls: the composite-key row sort's call with the window's arguments, its input count zeroed first;
+// every count and *dst_total are 0 when a block failed (nothing is written).
+static int window_call(uint32_t dev_index, bool packed, uint32_t codec, uint32_t alg, uint32_t n,
+                       const uint8_t* src_base, const uint64_t* src_off, const uint64_t* src_len,
+                       const uint32_t* slice_base, const uint64_t* slice_len, const uint64_t* slice_checksum,
+                       uint32_t n_partition_keys, uint32_t n_keys, const uint32_t* key_type, const uint32_t* key_off,
+                       const uint32_t* key_len, const int32_t* key_null_field, uint32_t n_fields,
+                       const uint8_t* field_kind, uint32_t n_fns, const uint32_t* fn, const int32_t* fn_arg,
+                       uint32_t limit_fn, int32_t limit, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_total,
+                       uint64_t* n_records, uint64_t* n_out_records, int32_t* status, int32_t* bad_slice) {
+  if (n_records) *n_records = 0;
+  WindowSpec ws;
+  ws.n_partition_keys = n_partition_keys;
+  ws.n_fields = n_fields;
+  ws.kind = field_kind;
+  ws.n_fns = n_fns;
+  ws.fn = fn;
+  ws.fn_arg = fn_arg;
+  ws.limit_fn = limit_fn;
+  ws.limit = limit;
+  ws.n_in = n_records;
+  RecordSpec spec = keys_spec(n_keys, key_type, key_off, key_len, key_null_field);
+  spec.window = &ws;
+  const int rc = sort_call(dev_index, packed, nullptr, codec, alg, n, src_base, src_off, src_len, slice_base, slice_len,
+                           slice_checksum, spec, dst_base, dst_cap, dst_total, n_out_records, status, bad_slice);
+  if (!rc && !*n_out_records) *dst_total = 0;
+  return rc;
+}
+
+int b2s_decompress_window_rows_keys_packed(
+    uint32_t codec, uint32_t checksum_alg, uint32_t n, const uint8_t* src_base, const uint64_t* src_off,
+    const uint64_t* src_len, const uint32_t* slice_base, const uint64_t* slice_len, const uint64_t* slice_checksum,
+    uint32_t n_partition_keys, uint32_t n_keys, const uint32_t* key_type, const uint32_t* key_off,
+    const uint32_t* key_len, const int32_t* key_null_field, uint32_t n_fields, const uint8_t* field_kind,
+    uint32_t n_fns, const uint32_t* fn, const int32_t* fn_arg, uint32_t limit_fn, int32_t limit,
+    uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records, uint64_t* n_out_records,
+    int32_t* status, int32_t* bad_slice) {
+  return window_call(t_device, true, codec, checksum_alg, n, src_base, src_off, src_len, slice_base, slice_len,
+                     slice_checksum, n_partition_keys, n_keys, key_type, key_off, key_len, key_null_field, n_fields,
+                     field_kind, n_fns, fn, fn_arg, limit_fn, limit, dst_base, dst_cap, dst_total, n_records,
+                     n_out_records, status, bad_slice);
+}
+
+int b2s_decompress_window_rows_keys_dev(
+    uint32_t dev_index, uint32_t codec, uint32_t checksum_alg, uint32_t n, const uint8_t* src_base,
+    const uint64_t* src_off, const uint64_t* src_len, const uint32_t* slice_base, const uint64_t* slice_len,
+    const uint64_t* slice_checksum, uint32_t n_partition_keys, uint32_t n_keys, const uint32_t* key_type,
+    const uint32_t* key_off, const uint32_t* key_len, const int32_t* key_null_field, uint32_t n_fields,
+    const uint8_t* field_kind, uint32_t n_fns, const uint32_t* fn, const int32_t* fn_arg, uint32_t limit_fn,
+    int32_t limit, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records,
+    uint64_t* n_out_records, int32_t* status, int32_t* bad_slice) {
+  return window_call(dev_index, false, codec, checksum_alg, n, src_base, src_off, src_len, slice_base, slice_len,
+                     slice_checksum, n_partition_keys, n_keys, key_type, key_off, key_len, key_null_field, n_fields,
+                     field_kind, n_fns, fn, fn_arg, limit_fn, limit, dst_base, dst_cap, dst_total, n_records,
+                     n_out_records, status, bad_slice);
 }
 
 // ------------------------------------------------------------------------------------------------------------

@@ -521,6 +521,43 @@ void launch_join_emit(const uint8_t* arena, uint64_t n, const uint32_t* idx, uin
                       bool whole, uint8_t* d_ws, uint8_t* d_jws, uint32_t n_ranges, uint8_t* d_dst, cudaStream_t st,
                       uint64_t* launches);
 
+// ---------------- window.cu (Spark's WindowExec ranking functions over a reducer's key-sorted rows) ----------------
+// The records, stably sorted by the window's key (partition columns, then order columns: launch_rows_order) and grouped
+// by the whole key (launch_rows_group: the peer groups).  The shape of the output row: the input's field count n,
+// null-bitset words bw, the output's out_bw = ceil((n + n_fns) / 64), the functions (B2S_WINDOW_*) and their
+// arguments, the limit (limit_fn B2S_WINDOW_NO_LIMIT: none), the partition columns (the key's first part.n columns),
+// and the input's VAR and DECIMAL_WIDE fields (their slots' offsets move), as a device list.
+constexpr uint32_t kMaxWindowFns = 16;
+struct WindowShape {
+  uint32_t n, bw, out_bw;
+  uint32_t n_fns;
+  uint32_t fn[kMaxWindowFns];
+  uint32_t arg[kMaxWindowFns];
+  uint32_t limit_fn;
+  int32_t limit;
+  uint32_t n_var;
+  const uint32_t* var;
+  KeySpec part;
+};
+// d_wws: window_ws_bytes(n, n_fns, n_fields) bytes
+size_t window_ws_bytes(uint64_t n, uint32_t n_fns, uint32_t n_fields);
+// the readback: [output records, output bytes, an output row is too long (0 / 1), a partition is too large (0 / 1)]
+uint64_t* window_readback(uint8_t* d_wws, uint64_t n, uint32_t n_fns);
+constexpr size_t kWindowReadbackBytes = 32;
+// Per sorted position: whether it starts a partition (only peer heads compare their partition columns with their
+// predecessor's, encoded 16 bytes at a time), scanned, and the partitions' starts compacted; then every function's
+// value, whether the limit keeps the record and its output bytes, the kept records and bytes scanned, the totals and
+// the verdicts into the readback.  Uploads the shape and its field list (h_fields: shape.n_var fields).  idx: the
+// sorted order (nullptr: arena order); d_aws: launch_rows_group's workspace.
+void launch_window_values(const uint8_t* arena, uint64_t n, const uint32_t* idx, WindowShape shape,
+                          const uint32_t* h_fields, uint32_t key_bytes, uint8_t* d_ws, uint8_t* d_aws, uint8_t* d_wws,
+                          cudaStream_t st, uint64_t* launches);
+// the out_rows output records (read back) to d_dst, a warp per record; with a limit the kept positions are compacted
+// first, so only they are read
+void launch_window_emit(const uint8_t* arena, uint64_t n, const uint32_t* idx, uint64_t out_rows, uint32_t key_bytes,
+                        uint32_t n_fns, bool limited, uint8_t* d_ws, uint8_t* d_wws, uint8_t* d_dst, cudaStream_t st,
+                        uint64_t* launches);
+
 // ---------------- exchange.cu (exchange-cache reads: ranges of device memory gathered into one arena) ----------------
 // piece: len bytes at src (device pointer, any alignment) go to d_dst + dst
 struct ExchangePiece {

@@ -1095,6 +1095,53 @@ class S3ShuffleReader {
     sortedLen_ = total;
     sortedRecords_ = out;
   }
+  // The window's arguments (b2s_decompress_window_rows_keys_packed): the key columns (the first nPartitionKeys of them
+  // partition), the input's field count and kinds, the functions and their arguments, and the limit.
+  struct WindowArgs {
+    uint32_t nPartitionKeys, nKeys;
+    const uint32_t *keyType, *keyOff, *keyLen;
+    const int32_t* keyNull;
+    uint32_t nFields;
+    const uint8_t* kind;
+    uint32_t nFns;
+    const uint32_t* fn;
+    const int32_t* fnArg;
+    uint32_t limitFn;
+    int32_t limit;
+  };
+  // read() for a Spark SQL window over this shuffle read (INTEGRATION.md §3o): every non-empty block is fetched (the
+  // exchange cache is not consulted) in computeShuffleBlocks order, then ONE b2s_decompress_window_rows_keys_packed
+  // call verifies, decodes and sorts the rows and evaluates the ranking functions, retried once with the exact size
+  // when its first guess is too small.  The output rows stay in this reader as a sorted read's records do;
+  // sortedRecords() is the number of output rows, *nRecords the input's.
+  void readWindowRows(const WindowArgs& w, uint64_t* nRecords) {
+    std::vector<FetchedBlock> fetched;
+    fetchAll(fetched);
+    std::vector<const FetchedBlock*> sources;
+    for (const auto& f : fetched)
+      if (!f.second.empty()) sources.push_back(&f);
+    const uint32_t alg = d_.checksumEnabled ? S3ShuffleHelper::createChecksumAlgorithm(d_.checksumAlgorithm) : 0;
+    ensure_codec_runtime();
+    const uint32_t codec = (uint32_t)d_.codecId();
+    StagedBlocks src(info_, sources);
+    const uint32_t n = (uint32_t)sources.size();
+    std::vector<int32_t> status(n), bad(n);
+    uint64_t total = 0, out = 0;
+    const uint64_t guess = codec == B2S_CODEC_NONE ? src.bytes * 2 : src.bytes * 4;
+    const int rc = callWithRetry(sorted_, guess, total, [&](uint64_t cap) {
+      return b2s_decompress_window_rows_keys_packed(
+          codec, alg, n, src.src.data(), src.off.data(), src.len.data(), alg ? src.sliceBase.data() : 0,
+          alg ? src.sliceLen.data() : 0, alg ? src.sliceSum.data() : 0, w.nPartitionKeys, w.nKeys, w.keyType,
+          w.keyOff, w.keyLen, w.keyNull, w.nFields, w.kind, w.nFns, w.fn, w.fnArg, w.limitFn, w.limit, sorted_.get(),
+          cap, &total, nRecords, &out, status.data(), bad.data());
+    });
+    if (rc != 0)
+      throw CodecException(std::string("b2s_decompress_window_rows_keys_packed: ") + b2s_strerror(rc) + ": " +
+                           b2s_last_error());
+    for (uint32_t k = 0; k < n; k++) throwBlockStatus(status[k], info_[sources[k]->first].id);
+    sortedLen_ = total;
+    sortedRecords_ = out;
+  }
   // every block of the task, fetched whole, in computeShuffleBlocks order
   void fetchAll(std::vector<FetchedBlock>& fetched) {
     start(true);
@@ -1548,6 +1595,19 @@ int b2sh_reader_read_joined_rows(b2sh_reader* left, b2sh_reader* right, uint32_t
                                       n_left_fields, left_field_kind, n_right_fields,  right_field_kind};
     left->r->readJoined(*right->r, j, n_left_records, n_right_records);
     sorted_result(*left->r, data, len, n_out_records);
+  });
+}
+int b2sh_reader_read_window_rows(b2sh_reader* r, uint32_t n_partition_keys, uint32_t n_keys, const uint32_t* key_type,
+                                 const uint32_t* key_off, const uint32_t* key_len, const int32_t* key_null_field,
+                                 uint32_t n_fields, const uint8_t* field_kind, uint32_t n_fns, const uint32_t* fn,
+                                 const int32_t* fn_arg, uint32_t limit_fn, int32_t limit, const uint8_t** data,
+                                 uint64_t* len, uint64_t* n_records, uint64_t* n_out_records) {
+  return guarded([&] {
+    const S3ShuffleReader::WindowArgs w{n_partition_keys, n_keys,     key_type, key_off, key_len,  key_null_field,
+                                        n_fields,         field_kind, n_fns,    fn,      fn_arg,   limit_fn,
+                                        limit};
+    r->r->readWindowRows(w, n_records);
+    sorted_result(*r->r, data, len, n_out_records);
   });
 }
 int b2sh_reader_block(b2sh_reader* r, uint32_t k, int64_t* map_id, int32_t* start_reduce, int32_t* end_reduce,
