@@ -725,6 +725,104 @@ int b2s_decompress_window_rows_keys_dev(
     int32_t limit, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records,
     uint64_t* n_out_records, int32_t* status, int32_t* bad_slice);
 
+/* ---- read side, window aggregates: Spark's WindowExec with aggregate functions on a reducer's shuffled UnsafeRows ----
+ * b2s_decompress_window_rows_keys_* without a limit, where fn[j] may also be an aggregate function over a frame.  Blocks,
+ * keys, partitions, peers, the ranking functions, the output stream, the counts and everything not stated here are that
+ * call's.  The semantics are Spark 3.5's AggregateProcessor running each DeclarativeAggregate's update and evaluate
+ * expressions with spark.sql.ansi.enabled off.
+ * Per function j: fn[j], fn_arg[j] (NTILE's bucket count, else 0), fn_frame[j], val_type[j], val_off[j] and
+ * val_null_field[j].  A ranking function takes frame 0 (its own) and B2S_WINDOW_VAL_NONE.  An aggregate function
+ * (B2S_WINDOW_SUM .. B2S_WINDOW_AVG) takes one of the frames, with i the record's 0-based position in its partition of N
+ * and [gs, ge) its peer group's positions:
+ *   B2S_WINDOW_FRAME_PARTITION      positions [0, N): no ORDER BY, or UNBOUNDED PRECEDING AND UNBOUNDED FOLLOWING with
+ *                                   either frame type
+ *   B2S_WINDOW_FRAME_ROWS_RUNNING   positions [0, i]: ROWS BETWEEN UNBOUNDED PRECEDING AND CURRENT ROW
+ *   B2S_WINDOW_FRAME_RANGE_RUNNING  positions [0, ge), through the last peer: RANGE BETWEEN UNBOUNDED PRECEDING AND
+ *                                   CURRENT ROW, the default with ORDER BY
+ * With every function on FRAME_PARTITION the key may have no ORDER BY column (n_partition_keys == n_keys).
+ * Input.  val_type[j] is B2S_WINDOW_VAL_INT8, _INT16, _INT32, _INT64, _FLOAT32 or _FLOAT64, read from the field whose
+ * 8-byte slot is at byte val_off[j] (8 (bC + f) for a field f < nC) as UnsafeRowWriter writes it; or
+ * B2S_WINDOW_VAL_DECIMAL | p << 8 | s << 16 for decimal(p, s), 1 <= p <= 38, s <= p: for p <= 18 the slot holds the
+ * unscaled long, for p > 18 the field is DECIMAL_WIDE and its slot (offset << 32) | size points at the unscaled value's
+ * big-endian two's-complement bytes.  The field's kind must be DECIMAL_WIDE exactly when p > 18 and FIXED otherwise.
+ * val_null_field[j] is the field's null bit, or -1 (never null).  B2S_WINDOW_VAL_NONE is count(*) (COUNT only; val_off
+ * and val_null_field are then ignored).
+ * Fold order.  Every frame is folded over its records in sorted order from the partition's first record.  The sort is
+ * stable, so this is the order Spark's UnboundedWindowFunctionFrame and UnboundedPrecedingWindowFunctionFrame fold in
+ * whenever Spark's sort keeps ties in read order.  Only the double sums and the first-of-equal choice of MIN / MAX
+ * depend on it.
+ *   SUM    integral input: the 64-bit wrapping sum of the non-null inputs, sign-extended, a long.  Float or double
+ *          input: ((0.0 + x1) + x2) + ... over the non-null inputs in double, each add rounded to nearest (no
+ *          reassociation, no FMA; a float widened exactly; a lone -0.0 gives +0.0), a double.  decimal(p, s) with
+ *          p <= 28: the exact sum, a decimal(p + 10, s); below 2^31 records |S| < 2^31 10^p < 10^(p + 10) < 2^127, so it
+ *          never overflows.  Null when the frame has no non-null input.
+ *   COUNT  the number of non-null inputs (every record for VAL_NONE), a long; never null.
+ *   MIN / MAX  the input's type.  Spark SQL's order: -0.0 equals 0.0 and NaN is above every other value and equal to
+ *          every NaN; decimals compare as signed unscaled values.  Among equal values the first in fold order is kept
+ *          with its exact bits (Least / Greatest, as B2S_AGG_MIN / MAX_FLOAT64).  Null when no input is non-null.
+ *   AVG    numeric input: the SUM fold in double (integral inputs converted to double rounded to nearest) divided by
+ *          (double) count, a double.  decimal(p, s) with p <= 24: the exact sum divided by the count and rounded
+ *          HALF_UP (ties away from zero) to scale s + 4, a decimal(p + 4, s + 4).  Null when the count is 0.
+ *          Spark first divides to at least 38 significant digits (Decimal./, rounding HALF_UP) and then rounds that
+ *          to scale s + 4; for p <= 24 and counts c < 2^31 the two roundings equal this one.  |S| < c 10^p, so the
+ *          quotient has at most p - s <= 24 - s digits before the point and the first rounding keeps at least 14 + s
+ *          after it: an error of at most 10^-(14+s) / 2, which is 10^-10 / 2 units of 10^-(s+4).  In those units the
+ *          exact quotient is k + m / c (0 <= m < c): on a half-point (2m = c) it has s + 5 digits after the point and
+ *          the first rounding is exact; elsewhere it is at least 1 / (2c) > 2^-32 > 10^-10 / 2 units from every
+ *          half-point, so the first rounding cannot carry it across one.
+ * Output row.  The input row joined with the row of the n_fns values as UnsafeRowJoiner joins them, as in the ranking
+ * call, except that a value can be null and carry bytes.  With b = ceil((nC + n_fns) / 64): value j's null bit is
+ * nC + j, set exactly when its result is null (its slot is then zero).  Ints, longs, floats and doubles are written as
+ * UnsafeRowWriter writes them: the slot zeroed, then the value's bytes.  A decimal result of precision <= 18 is its
+ * unscaled long; a wider one takes 16 bytes appended after the input's var bytes, in function order, at offset
+ * 8 (b + nC + n_fns) + varC + 16 k for the k-th such function (varC: the input's var bytes), its slot (offset << 32) | len
+ * and its bytes BigInteger.toByteArray's minimal len, zero-padded to 16.  A null one keeps its 16 zero bytes and the
+ * slot offset << 32 (the join's null-side rule).
+ * Errors -> B2S_E_ARG: everything the ranking call rejects (except no ORDER BY column as above); n_fns outside 1..16;
+ * NULL fn, fn_arg, fn_frame, val_type, val_off or val_null_field; an unknown function or frame, or a frame the function
+ * does not take; a val_type the function does not take (SUM and AVG: the numeric types and decimals up to p 28 and 24;
+ * MIN and MAX: numeric and decimal; COUNT: those and VAL_NONE; ranking: VAL_NONE); a decimal precision or scale out of
+ * range or a field kind that does not match; a value slot that is not one of the input's slots, or a value null bit
+ * below -1 or not below nC.  These are checked before the device.  Per block, B2S_E_CORRUPT for the ranking call's
+ * rules and when a non-null DECIMAL_WIDE input's size is not 1..16 or its bytes run past its row; nothing is written
+ * when a block fails.  A partition of more than 2^31 - 1 records or an output row longer than 2^31 - 1 bytes ->
+ * B2S_E_UNSUPPORTED.  B2S_E_DST_TOO_SMALL, B2S_E_NOMEM, the read lane, the buffer trim and b2s_last_timing as in the
+ * ranking call (dominant_ms the window step). */
+#define B2S_WINDOW_SUM 6
+#define B2S_WINDOW_COUNT 7
+#define B2S_WINDOW_MIN 8
+#define B2S_WINDOW_MAX 9
+#define B2S_WINDOW_AVG 10
+#define B2S_WINDOW_FRAME_PARTITION 1
+#define B2S_WINDOW_FRAME_ROWS_RUNNING 2
+#define B2S_WINDOW_FRAME_RANGE_RUNNING 3
+#define B2S_WINDOW_VAL_NONE 0
+#define B2S_WINDOW_VAL_INT8 1
+#define B2S_WINDOW_VAL_INT16 2
+#define B2S_WINDOW_VAL_INT32 3
+#define B2S_WINDOW_VAL_INT64 4
+#define B2S_WINDOW_VAL_FLOAT32 5
+#define B2S_WINDOW_VAL_FLOAT64 6
+#define B2S_WINDOW_VAL_DECIMAL 7
+int b2s_decompress_window_aggregate_rows_keys_packed(
+    uint32_t codec, uint32_t checksum_alg, uint32_t n, const uint8_t* src_base, const uint64_t* src_off,
+    const uint64_t* src_len, const uint32_t* slice_base, const uint64_t* slice_len, const uint64_t* slice_checksum,
+    uint32_t n_partition_keys, uint32_t n_keys, const uint32_t* key_type, const uint32_t* key_off,
+    const uint32_t* key_len, const int32_t* key_null_field, uint32_t n_fields, const uint8_t* field_kind,
+    uint32_t n_fns, const uint32_t* fn, const int32_t* fn_arg, const uint32_t* fn_frame, const uint32_t* val_type,
+    const uint32_t* val_off, const int32_t* val_null_field, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_total,
+    uint64_t* n_records, uint64_t* n_out_records, int32_t* status, int32_t* bad_slice);
+/* same, with src_base / dst_base in device memory of dev_index; every array stays a host array */
+int b2s_decompress_window_aggregate_rows_keys_dev(
+    uint32_t dev_index, uint32_t codec, uint32_t checksum_alg, uint32_t n, const uint8_t* src_base,
+    const uint64_t* src_off, const uint64_t* src_len, const uint32_t* slice_base, const uint64_t* slice_len,
+    const uint64_t* slice_checksum, uint32_t n_partition_keys, uint32_t n_keys, const uint32_t* key_type,
+    const uint32_t* key_off, const uint32_t* key_len, const int32_t* key_null_field, uint32_t n_fields,
+    const uint8_t* field_kind, uint32_t n_fns, const uint32_t* fn, const int32_t* fn_arg, const uint32_t* fn_frame,
+    const uint32_t* val_type, const uint32_t* val_off, const int32_t* val_null_field, uint8_t* dst_base,
+    uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records, uint64_t* n_out_records, int32_t* status,
+    int32_t* bad_slice);
+
 /* ---- exchange cache: map outputs kept resident in HBM for reducers on the same device ----
  * (docs/f4_gpu_resident_exchange.md steps 2 and 3, local half.)  The serialized writer's partition step already leaves
  * a map task's records partitioned by reduce id in HBM; the cached store keeps that arena, keyed by (shuffle_id,

@@ -29,6 +29,16 @@ FIELD_FIXED, FIELD_VAR, FIELD_DECIMAL_WIDE = 0, 1, 2
 # ranking functions of the row window (decompress_window_rows_keys_*), and its limit function meaning "no limit"
 WINDOW_ROW_NUMBER, WINDOW_RANK, WINDOW_DENSE_RANK, WINDOW_PERCENT_RANK, WINDOW_CUME_DIST, WINDOW_NTILE = range(6)
 WINDOW_NO_LIMIT = 0xFFFFFFFF
+# aggregate functions, frames and input types of the aggregate window (decompress_window_aggregate_rows_keys_*); a
+# decimal(p, s) input is WINDOW_VAL_DECIMAL | p << 8 | s << 16 (window_val_decimal)
+WINDOW_SUM, WINDOW_COUNT, WINDOW_MIN, WINDOW_MAX, WINDOW_AVG = range(6, 11)
+WINDOW_FRAME_PARTITION, WINDOW_FRAME_ROWS_RUNNING, WINDOW_FRAME_RANGE_RUNNING = 1, 2, 3
+(WINDOW_VAL_NONE, WINDOW_VAL_INT8, WINDOW_VAL_INT16, WINDOW_VAL_INT32, WINDOW_VAL_INT64, WINDOW_VAL_FLOAT32,
+ WINDOW_VAL_FLOAT64, WINDOW_VAL_DECIMAL) = range(8)
+
+
+def window_val_decimal(p, s):
+    return WINDOW_VAL_DECIMAL | p << 8 | s << 16
 OK, E_CORRUPT, E_CHECKSUM, E_DST_TOO_SMALL, E_UNSUPPORTED, E_ARG, E_CUDA, E_NOT_INIT, E_NOMEM, E_NOT_CACHED = (
     0, -1, -2, -3, -4, -5, -6, -7, -8, -9)
 NOT_RESIDENT = 2**64 - 1  # b2s_exchange_lookup's length of a map output that is not resident
@@ -147,6 +157,12 @@ PROTOTYPES = [
     ("b2s_decompress_window_rows_keys_dev", C.c_int,
      [_u32, _u32, _u32, _u32, _vp, _u64p, _u64p, _u32p, _u64p, _u64p, _u32, _u32, _u32p, _u32p, _u32p, _i32p, _u32,
       _u8p, _u32, _u32p, _i32p, _u32, _i32, _vp, _u64, _u64p, _u64p, _u64p, _i32p, _i32p]),
+    ("b2s_decompress_window_aggregate_rows_keys_packed", C.c_int,
+     [_u32, _u32, _u32, _u8p, _u64p, _u64p, _u32p, _u64p, _u64p, _u32, _u32, _u32p, _u32p, _u32p, _i32p, _u32, _u8p,
+      _u32, _u32p, _i32p, _u32p, _u32p, _u32p, _i32p, _u8p, _u64, _u64p, _u64p, _u64p, _i32p, _i32p]),
+    ("b2s_decompress_window_aggregate_rows_keys_dev", C.c_int,
+     [_u32, _u32, _u32, _u32, _vp, _u64p, _u64p, _u32p, _u64p, _u64p, _u32, _u32, _u32p, _u32p, _u32p, _i32p, _u32,
+      _u8p, _u32, _u32p, _i32p, _u32p, _u32p, _u32p, _i32p, _vp, _u64, _u64p, _u64p, _u64p, _i32p, _i32p]),
     ("b2s_exchange_set_budget", C.c_int, [_u32, _u64]),
     ("b2s_partition_compress_cached_packed", C.c_int,
      [_i32, C.c_int64, _u32, _i32, _u32, _u32, _u32, _u64, _u8p, _u64, _u32p, _u32p, _u8p, _u64, _u64p, _u64p, _u64p,
@@ -597,6 +613,39 @@ def _window_arrays(keys, n_partition_keys, n_fields, kinds, fns, limit):
     return n_partition_keys, n, kt, ko, kl, kn, n_fields, kinds, len(fns), fn, arg, limit_fn, lim
 
 
+def _window_aggregate_arrays(keys, n_partition_keys, n_fields, kinds, fns):
+    """the aggregate window's key, field-kind and function arguments: fns = [ranking fn, (WINDOW_NTILE, k), or an
+    aggregate (fn, frame, val_type, val_off, val_null_field)]"""
+    n, kt, ko, kl, kn = _key_arrays(keys)
+    full = []
+    for f in fns:
+        if isinstance(f, tuple) and len(f) == 5:
+            full.append((f[0], 0) + tuple(f[1:]))
+        else:
+            fn, arg = f if isinstance(f, tuple) else (f, 0)
+            full.append((fn, arg, 0, WINDOW_VAL_NONE, 0, -1))
+    cols = list(zip(*full)) if full else [[0]] * 6
+    fn, arg, frame, vt, vo = (np.array(c, dtype=t) for c, t in zip(cols[:5], (np.uint32, np.int32, np.uint32,
+                                                                             np.uint32, np.uint32)))
+    vn = np.array(cols[5], dtype=np.int32)
+    kinds = None if kinds is None else np.ascontiguousarray(kinds, dtype=np.uint8)
+    return n_partition_keys, n, kt, ko, kl, kn, n_fields, kinds, len(full), fn, arg, frame, vt, vo, vn
+
+
+def decompress_window_aggregate_rows_keys_packed(codec, src, off, length, dst, keys, n_partition_keys, n_fields,
+                                                 kinds, fns, checksum_alg=CHECKSUM_NONE, slice_base=None,
+                                                 slice_len=None, slice_checksum=None):
+    """Spark's WindowExec with aggregate (and ranking) functions over a reducer's UnsafeRow records: as
+    decompress_window_rows_keys_packed without a limit, fns mixing ranking functions (as there) and aggregates
+    (WINDOW_SUM / COUNT / MIN / MAX / AVG, WINDOW_FRAME_*, WINDOW_VAL_* or window_val_decimal(p, s), the input's slot
+    offset, its null bit or -1).  An aggregate's value is null when its frame has no input, and a decimal result above
+    precision 18 takes 16 bytes after the input's var bytes.  -> dict(total, n_records, n_out_records, status,
+    bad_slice)"""
+    return _sort_call("b2s_decompress_window_aggregate_rows_keys_packed", codec, src, off, length, dst, None,
+                      _window_aggregate_arrays(keys, n_partition_keys, n_fields, kinds, fns), checksum_alg,
+                      (slice_base, slice_len, slice_checksum))
+
+
 def decompress_window_rows_keys_packed(codec, src, off, length, dst, keys, n_partition_keys, n_fields, kinds, fns,
                                        limit=None, checksum_alg=CHECKSUM_NONE, slice_base=None, slice_len=None,
                                        slice_checksum=None):
@@ -732,6 +781,15 @@ def decompress_window_rows_keys_dev(codec, d_src, off, length, d_dst, dst_cap, k
     """decompress_window_rows_keys_packed on device-resident blocks (d_src) into a device arena (d_dst)"""
     return _sort_call("b2s_decompress_window_rows_keys_dev", codec, d_src, off, length, d_dst, dst_cap,
                       _window_arrays(keys, n_partition_keys, n_fields, kinds, fns, limit), checksum_alg,
+                      (slice_base, slice_len, slice_checksum), dev)
+
+
+def decompress_window_aggregate_rows_keys_dev(codec, d_src, off, length, d_dst, dst_cap, keys, n_partition_keys,
+                                              n_fields, kinds, fns, checksum_alg=CHECKSUM_NONE, slice_base=None,
+                                              slice_len=None, slice_checksum=None, dev=0):
+    """decompress_window_aggregate_rows_keys_packed on device-resident blocks (d_src) into a device arena (d_dst)"""
+    return _sort_call("b2s_decompress_window_aggregate_rows_keys_dev", codec, d_src, off, length, d_dst, dst_cap,
+                      _window_aggregate_arrays(keys, n_partition_keys, n_fields, kinds, fns), checksum_alg,
                       (slice_base, slice_len, slice_checksum), dev)
 
 

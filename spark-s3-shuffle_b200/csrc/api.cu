@@ -2552,7 +2552,8 @@ struct JoinSpec {
   uint64_t* n_side[2] = {};
 };
 // A window's other arguments (b2s_decompress_window_rows_keys_*): how many key columns partition, the input's fields
-// and kinds, the functions and their arguments, the limit, and the input record count it returns.
+// and kinds, the functions and their arguments, the limit, and the input record count it returns.  The aggregate call
+// (b2s_decompress_window_aggregate_rows_keys_*, agg) adds each function's frame and input column, and has no limit.
 struct WindowSpec {
   uint32_t n_partition_keys = 0;
   uint32_t n_fields = 0;
@@ -2563,6 +2564,11 @@ struct WindowSpec {
   uint32_t limit_fn = B2S_WINDOW_NO_LIMIT;
   int32_t limit = 0;
   uint64_t* n_in = nullptr;
+  bool agg = false;
+  const uint32_t* frame = nullptr;
+  const uint32_t* val_type = nullptr;
+  const uint32_t* val_off = nullptr;
+  const int32_t* val_null = nullptr;
 };
 static RecordSpec fixed_spec(uint32_t record_bytes, uint32_t key_off, uint32_t key_len) {
   RecordSpec r;
@@ -2755,7 +2761,12 @@ static int join_args(const RecordSpec& spec, uint32_t n) {
 static int window_args(const RecordSpec& spec) {
   const WindowSpec& ws = *spec.window;
   const KeySpec& ks = spec.keys;
-  if (ws.n_partition_keys >= spec.n_keys || ws.n_partition_keys >= kMaxKeys)
+  // the aggregate call has checked its functions (window_agg_fn_args); with every frame the whole partition it needs
+  // no ORDER BY column
+  bool whole = ws.agg;
+  for (uint32_t j = 0; whole && j < ws.n_fns; j++) whole = ws.frame[j] == B2S_WINDOW_FRAME_PARTITION;
+  if (whole ? ws.n_partition_keys > spec.n_keys
+            : ws.n_partition_keys >= spec.n_keys || ws.n_partition_keys >= kMaxKeys)
     return fail(B2S_E_ARG, "n_partition_keys must be in [0, 15] and leave at least one ORDER BY column%s");
   for (uint32_t c = 0; c < ws.n_partition_keys; c++)
     if (ks.type[c] & ~kKeyTypeMask) return fail(B2S_E_ARG, "a partition column takes no order flag%s");
@@ -2772,6 +2783,7 @@ static int window_args(const RecordSpec& spec) {
     if (ws.kind[f] > B2S_FIELD_DECIMAL_WIDE) return fail(B2S_E_ARG, "unknown field kind%s");
   if (ws.n_fns < 1 || ws.n_fns > kMaxWindowFns) return fail(B2S_E_ARG, "n_fns must be in [1, 16]%s");
   if (!ws.fn || !ws.fn_arg || !ws.n_in) return fail(B2S_E_ARG, "null argument%s");
+  if (ws.agg) return 0;
   const bool limited = ws.limit_fn != B2S_WINDOW_NO_LIMIT;
   auto rank_like = [](uint32_t f) { return f <= B2S_WINDOW_DENSE_RANK; };
   for (uint32_t j = 0; j < ws.n_fns; j++) {
@@ -2784,6 +2796,51 @@ static int window_args(const RecordSpec& spec) {
   if (limited ? !rank_like(ws.limit_fn) || ws.limit < 1 : ws.limit != 0)
     return fail(B2S_E_ARG, "limit_fn must be B2S_WINDOW_NO_LIMIT with limit 0, or ROW_NUMBER, RANK or DENSE_RANK with "
                            "a limit of at least 1%s");
+  return 0;
+}
+
+// The aggregate window call's checks of its functions, before the device: the input's fields and kinds, and per
+// function its argument, frame, input type, slot and null bit (b2s_decompress_window_aggregate_rows_keys_*)
+static int window_agg_fn_args(const WindowSpec& ws) {
+  const uint32_t nf = ws.n_fields;
+  if (nf < 1 || nf > 65536) return fail(B2S_E_ARG, "n_fields must be in [1, 65536]%s");
+  if (!ws.kind) return fail(B2S_E_ARG, "field kinds are required%s");
+  for (uint32_t f = 0; f < nf; f++)
+    if (ws.kind[f] > B2S_FIELD_DECIMAL_WIDE) return fail(B2S_E_ARG, "unknown field kind%s");
+  if (ws.n_fns < 1 || ws.n_fns > kMaxWindowFns) return fail(B2S_E_ARG, "n_fns must be in [1, 16]%s");
+  if (!ws.fn || !ws.fn_arg || !ws.frame || !ws.val_type || !ws.val_off || !ws.val_null || !ws.n_in)
+    return fail(B2S_E_ARG, "null argument%s");
+  const uint64_t lo = 8ull * bitset_words(nf);
+  for (uint32_t j = 0; j < ws.n_fns; j++) {
+    const uint32_t fn = ws.fn[j], frame = ws.frame[j], vt = ws.val_type[j], kind = vt & 0xff;
+    if (fn > B2S_WINDOW_AVG) return fail(B2S_E_ARG, "unknown window function%s");
+    if (fn == B2S_WINDOW_NTILE ? ws.fn_arg[j] < 1 : ws.fn_arg[j] != 0)
+      return fail(B2S_E_ARG, "fn_arg must be NTILE's bucket count (at least 1), and 0 for every other function%s");
+    const bool ranking = fn <= B2S_WINDOW_NTILE;
+    if (ranking ? frame != 0 : frame < B2S_WINDOW_FRAME_PARTITION || frame > B2S_WINDOW_FRAME_RANGE_RUNNING)
+      return fail(B2S_E_ARG, "fn_frame must be 0 for a ranking function and a B2S_WINDOW_FRAME_* for an aggregate%s");
+    if (kind > B2S_WINDOW_VAL_DECIMAL || (kind != B2S_WINDOW_VAL_DECIMAL && (vt >> 8)) || (vt >> 24))
+      return fail(B2S_E_ARG, "unknown val_type%s");
+    if (kind == B2S_WINDOW_VAL_NONE) {
+      if (fn != B2S_WINDOW_COUNT && !ranking) return fail(B2S_E_ARG, "only COUNT takes B2S_WINDOW_VAL_NONE%s");
+      continue;
+    }
+    if (ranking) return fail(B2S_E_ARG, "a ranking function takes B2S_WINDOW_VAL_NONE%s");
+    const uint32_t p = (vt >> 8) & 0xff, sc = vt >> 16;
+    if (kind == B2S_WINDOW_VAL_DECIMAL) {
+      const uint32_t max_p = fn == B2S_WINDOW_SUM ? 28 : fn == B2S_WINDOW_AVG ? 24 : 38;
+      if (p < 1 || p > max_p || sc > p)
+        return fail(B2S_E_ARG, "a decimal input needs 1 <= p <= 38 (SUM 28, AVG 24) and s <= p%s");
+    }
+    const uint32_t off = ws.val_off[j];
+    if (off < lo || (off - lo) % 8 || (off - lo) / 8 >= nf)
+      return fail(B2S_E_ARG, "val_off is not one of the input's field slots%s");
+    const uint8_t want = kind == B2S_WINDOW_VAL_DECIMAL && p > 18 ? B2S_FIELD_DECIMAL_WIDE : B2S_FIELD_FIXED;
+    if (ws.kind[(off - lo) / 8] != want)
+      return fail(B2S_E_ARG, "a value field's kind must be DECIMAL_WIDE for a decimal above p 18, else FIXED%s");
+    if (ws.val_null[j] < -1 || ws.val_null[j] >= (int64_t)nf)
+      return fail(B2S_E_ARG, "val_null_field must be -1 or a field ordinal below n_fields%s");
+  }
   return 0;
 }
 
@@ -3191,6 +3248,15 @@ struct DecodedTask {
   void bad_row(uint32_t i, uint64_t byte, const char* why) {
     fail_source(i, ": bad row record at byte " + std::to_string(byte) + ": " + why);
   }
+  // a value the device found bad in the record at arena byte at_byte: the source holding it (the last non-empty one
+  // that starts at or before it) fails as for a framing verdict -> report()
+  int fail_row_at(uint64_t at_byte, const char* why) {
+    uint32_t i = 0;
+    for (uint32_t k = 0; k < n_src; k++)
+      if (place[k] <= at_byte && length[k]) i = k;
+    bad_row(i, at_byte - place[i], why);
+    return report();
+  }
   int report() {  // -> 0, the result of a call that ends because a source failed (nothing is sorted or written)
     for (uint32_t i = 0; i < n_src; i++) {
       status_out[i] = status(i);
@@ -3300,6 +3366,39 @@ static void take_verdicts(DecodedTask& T, const RecordSpec& spec, const uint64_t
     if (v[i] != ~0ull) T.bad_row(i, v[i] & ((1ull << 61) - 1), why[v[i] >> 61]);
 }
 
+// A window's output-row shape from its arguments (launch_window_values; the field list is the tail's)
+static void window_shape(const RecordSpec& spec, WindowShape& shape) {
+  const WindowSpec& ws = *spec.window;
+  shape.n = ws.n_fields;
+  shape.bw = bitset_words(ws.n_fields);
+  shape.out_bw = bitset_words(ws.n_fields + ws.n_fns);
+  shape.n_fns = ws.n_fns;
+  for (uint32_t j = 0; j < ws.n_fns; j++) {
+    shape.fn[j] = ws.fn[j];
+    shape.arg[j] = (uint32_t)ws.fn_arg[j];
+    shape.wide[j] = -1;
+    if (ws.fn[j] < B2S_WINDOW_SUM) continue;
+    const uint32_t vt = ws.val_type[j], p = (vt >> 8) & 0xff;
+    shape.frame[j] = ws.frame[j];
+    shape.vtype[j] = vt;
+    shape.voff[j] = ws.val_off[j];
+    shape.vnull[j] = ws.val_null[j];
+    shape.agg[j] = shape.n_agg++;
+    const uint32_t rp = p + (ws.fn[j] == B2S_WINDOW_SUM ? 10 : ws.fn[j] == B2S_WINDOW_AVG ? 4 : 0);
+    if ((vt & 0xff) == B2S_WINDOW_VAL_DECIMAL && ws.fn[j] != B2S_WINDOW_COUNT && rp > 18)
+      shape.wide[j] = (int32_t)shape.n_wide++;
+  }
+  shape.limit_fn = ws.limit_fn;
+  shape.limit = ws.limit;
+  shape.part.n = ws.n_partition_keys;
+  for (uint32_t c = 0; c < ws.n_partition_keys; c++) {
+    shape.part.type[c] = spec.keys.type[c];
+    shape.part.off[c] = spec.keys.off[c];
+    shape.part.len[c] = spec.keys.len[c];
+    shape.part.null_field[c] = spec.keys.null_field[c];
+  }
+}
+
 // A reduce task's rows in key order (order_rows): idx (nullptr: arena order), heads (nullptr: where key words differ),
 // and S.pws's parts in order: sort, aggregation, refinement (nullptr unless the key refines), join or window grouping,
 // join, window.
@@ -3332,6 +3431,8 @@ static int order_rows(Slot& S, const RecordSpec& spec, DecodedTask& T, const Joi
   }
   const WindowSpec* win = spec.window;  // a window's rows hold its whole fixed region, which holds every key slot
   if (win) min_key = 8ull * (bitset_words(win->n_fields) + win->n_fields);
+  WindowShape wshape{};
+  if (win) window_shape(spec, wshape);
   // a cached range with record boundaries is marked from them instead of walked (its walk is empty)
   std::vector<uint64_t> walk(T.length);
   std::vector<RowsMark> marks;
@@ -3369,7 +3470,7 @@ static int order_rows(Slot& S, const RecordSpec& spec, DecodedTask& T, const Joi
                           refine ? rows_refine_ws_bytes(records, n_src) : 0,
                           jk || win ? rows_aggregate_ws_bytes(records, 0, 0) : 0,
                           jk ? join_ws_bytes(records, n_src, n_join_fields) : 0,
-                          win ? window_ws_bytes(records, win->n_fns, win->n_fields) : 0};
+                          win ? window_ws_bytes(records, wshape) : 0};
   if ((records || jk) && (rc = S.pws.ensure(part[0] + part[1] + part[2] + part[3] + part[4] + part[5]))) return rc;
   R.carve((uint8_t*)S.pws.p, part);
   if (!refine) R.rws = nullptr;
@@ -3421,19 +3522,13 @@ static int aggregate_rows_tail(Slot& S, const RecordSpec& spec, DecodedTask& T, 
     CU(cudaGetLastError());
   }
   if (rb[2] != ~0ull) {
-    // a bad decimal: the source holding the record (the last that starts at or before it) fails, as a framing verdict
-    const uint64_t at_byte = rb[2] >> 2;
-    uint32_t i = 0;
-    for (uint32_t k = 0; k < T.n_src; k++)
-      if (T.place[k] <= at_byte && T.length[k]) i = k;
     static const char* const why[] = {"",
                                       "a decimal aggregate's size is not in [1, 16] or its bytes run past the end of "
                                       "its row",
                                       "a decimal aggregate's 16-byte region runs past the end of its row",
                                       "a decimal aggregate's 16-byte region starts before the end of a slot or null "
                                       "word in use"};
-    T.bad_row(i, at_byte - T.place[i], why[rb[2] & 3]);
-    return T.report();
+    return T.fail_row_at(rb[2] >> 2, why[rb[2] & 3]);
   }
   *total = rb[1];
   if (rb[1] > out_cap)
@@ -3537,38 +3632,25 @@ static int window_rows_tail(Slot& S, const RecordSpec& spec, DecodedTask& T, con
   cudaStream_t st = S.st;
   const WindowSpec& ws = *spec.window;
   WindowShape shape{};
-  shape.n = ws.n_fields;
-  shape.bw = bitset_words(ws.n_fields);
-  shape.out_bw = bitset_words(ws.n_fields + ws.n_fns);
-  shape.n_fns = ws.n_fns;
-  for (uint32_t j = 0; j < ws.n_fns; j++) {
-    shape.fn[j] = ws.fn[j];
-    shape.arg[j] = (uint32_t)ws.fn_arg[j];
-  }
-  shape.limit_fn = ws.limit_fn;
-  shape.limit = ws.limit;
-  shape.part.n = ws.n_partition_keys;
-  for (uint32_t c = 0; c < ws.n_partition_keys; c++) {
-    shape.part.type[c] = spec.keys.type[c];
-    shape.part.off[c] = spec.keys.off[c];
-    shape.part.len[c] = spec.keys.len[c];
-    shape.part.null_field[c] = spec.keys.null_field[c];
-  }
+  window_shape(spec, shape);
   std::vector<uint32_t> fields;  // the slots whose offsets move
   for (uint32_t f = 0; f < ws.n_fields; f++)
     if (ws.kind[f] != B2S_FIELD_FIXED) fields.push_back(f);
   shape.n_var = (uint32_t)fields.size();
-  uint64_t wb[4] = {0, 0, 0, 0};  // output records, output bytes, a row too long, a partition too large
+  // output records, output bytes, a row too long, a partition too large, a bad decimal input
+  uint64_t wb[5] = {0, 0, 0, 0, ~0ull};
   CU(S.mark(G0, st, *launches));
   if (R.records) {
     launch_rows_group(T.arena, R.records, R.idx, R.heads, R.key_bytes, AggSpec{}, R.ws, R.gws, st, launches);
     launch_window_values(T.arena, R.records, R.idx, shape, fields.data(), R.key_bytes, R.ws, R.gws, R.wws, st,
                          launches);
-    CU(cudaMemcpyAsync(wb, window_readback(R.wws, R.records, ws.n_fns), kWindowReadbackBytes, cudaMemcpyDeviceToHost,
+    CU(cudaMemcpyAsync(wb, window_readback(R.wws, R.records, shape), kWindowReadbackBytes, cudaMemcpyDeviceToHost,
                        st));
     CU(cudaStreamSynchronize(st));
     CU(cudaGetLastError());
   }
+  if (wb[4] != ~0ull)
+    return T.fail_row_at(wb[4] >> 2, "a decimal input's size is not in [1, 16] or its bytes run past the end of its row");
   if (wb[3]) return fail(B2S_E_UNSUPPORTED, "a window partition holds more than 2^31 - 1 records%s");
   if (wb[2]) return fail(B2S_E_UNSUPPORTED, "an output row is longer than 2^31 - 1 bytes%s");
   *total = wb[1];
@@ -3578,7 +3660,7 @@ static int window_rows_tail(Slot& S, const RecordSpec& spec, DecodedTask& T, con
     if (int rc = S.parena.ensure(wb[1] + 64)) return rc;
     *d_out = (uint8_t*)S.parena.p;
   }
-  launch_window_emit(T.arena, R.records, R.idx, wb[0], R.key_bytes, ws.n_fns, ws.limit_fn != B2S_WINDOW_NO_LIMIT,
+  launch_window_emit(T.arena, R.records, R.idx, wb[0], R.key_bytes, shape, ws.limit_fn != B2S_WINDOW_NO_LIMIT,
                      R.ws, R.wws, *d_out, st, launches);
   CU(S.mark(G1, st, *launches));
   CU(S.mark(P1, st));
@@ -4003,17 +4085,35 @@ int b2s_decompress_join_rows_keys_dev(
                    status, bad_slice);
 }
 
-// The window calls: the composite-key row sort's call with the window's arguments, its input count zeroed first;
-// every count and *dst_total are 0 when a block failed (nothing is written).
+// The window calls: the composite-key row sort's call with the window's arguments ws (its n_in the input count, zeroed
+// first); every count and *dst_total are 0 when a block failed (nothing is written).  The aggregate call checks its
+// functions before the device.
 static int window_call(uint32_t dev_index, bool packed, uint32_t codec, uint32_t alg, uint32_t n,
                        const uint8_t* src_base, const uint64_t* src_off, const uint64_t* src_len,
                        const uint32_t* slice_base, const uint64_t* slice_len, const uint64_t* slice_checksum,
-                       uint32_t n_partition_keys, uint32_t n_keys, const uint32_t* key_type, const uint32_t* key_off,
-                       const uint32_t* key_len, const int32_t* key_null_field, uint32_t n_fields,
-                       const uint8_t* field_kind, uint32_t n_fns, const uint32_t* fn, const int32_t* fn_arg,
-                       uint32_t limit_fn, int32_t limit, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_total,
-                       uint64_t* n_records, uint64_t* n_out_records, int32_t* status, int32_t* bad_slice) {
-  if (n_records) *n_records = 0;
+                       uint32_t n_keys, const uint32_t* key_type, const uint32_t* key_off, const uint32_t* key_len,
+                       const int32_t* key_null_field, WindowSpec& ws, uint8_t* dst_base, uint64_t dst_cap,
+                       uint64_t* dst_total, uint64_t* n_out_records, int32_t* status, int32_t* bad_slice) {
+  if (ws.n_in) *ws.n_in = 0;
+  if (ws.agg) {
+    if (dst_total) *dst_total = 0;
+    if (n_out_records) *n_out_records = 0;
+    if (int rc = window_agg_fn_args(ws)) {
+      begin_call();  // a new call, with an empty b2s_last_timing
+      return rc;
+    }
+  }
+  RecordSpec spec = keys_spec(n_keys, key_type, key_off, key_len, key_null_field);
+  spec.window = &ws;
+  const int rc = sort_call(dev_index, packed, nullptr, codec, alg, n, src_base, src_off, src_len, slice_base, slice_len,
+                           slice_checksum, spec, dst_base, dst_cap, dst_total, n_out_records, status, bad_slice);
+  if (!rc && !*n_out_records) *dst_total = 0;
+  return rc;
+}
+
+static WindowSpec window_ranking_spec(uint32_t n_partition_keys, uint32_t n_fields, const uint8_t* field_kind,
+                                      uint32_t n_fns, const uint32_t* fn, const int32_t* fn_arg, uint32_t limit_fn,
+                                      int32_t limit, uint64_t* n_records) {
   WindowSpec ws;
   ws.n_partition_keys = n_partition_keys;
   ws.n_fields = n_fields;
@@ -4024,12 +4124,21 @@ static int window_call(uint32_t dev_index, bool packed, uint32_t codec, uint32_t
   ws.limit_fn = limit_fn;
   ws.limit = limit;
   ws.n_in = n_records;
-  RecordSpec spec = keys_spec(n_keys, key_type, key_off, key_len, key_null_field);
-  spec.window = &ws;
-  const int rc = sort_call(dev_index, packed, nullptr, codec, alg, n, src_base, src_off, src_len, slice_base, slice_len,
-                           slice_checksum, spec, dst_base, dst_cap, dst_total, n_out_records, status, bad_slice);
-  if (!rc && !*n_out_records) *dst_total = 0;
-  return rc;
+  return ws;
+}
+
+static WindowSpec window_aggregate_spec(uint32_t n_partition_keys, uint32_t n_fields, const uint8_t* field_kind,
+                                        uint32_t n_fns, const uint32_t* fn, const int32_t* fn_arg,
+                                        const uint32_t* fn_frame, const uint32_t* val_type, const uint32_t* val_off,
+                                        const int32_t* val_null_field, uint64_t* n_records) {
+  WindowSpec ws = window_ranking_spec(n_partition_keys, n_fields, field_kind, n_fns, fn, fn_arg, B2S_WINDOW_NO_LIMIT,
+                                      0, n_records);
+  ws.agg = true;
+  ws.frame = fn_frame;
+  ws.val_type = val_type;
+  ws.val_off = val_off;
+  ws.val_null = val_null_field;
+  return ws;
 }
 
 int b2s_decompress_window_rows_keys_packed(
@@ -4040,10 +4149,11 @@ int b2s_decompress_window_rows_keys_packed(
     uint32_t n_fns, const uint32_t* fn, const int32_t* fn_arg, uint32_t limit_fn, int32_t limit,
     uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records, uint64_t* n_out_records,
     int32_t* status, int32_t* bad_slice) {
+  WindowSpec ws =
+      window_ranking_spec(n_partition_keys, n_fields, field_kind, n_fns, fn, fn_arg, limit_fn, limit, n_records);
   return window_call(t_device, true, codec, checksum_alg, n, src_base, src_off, src_len, slice_base, slice_len,
-                     slice_checksum, n_partition_keys, n_keys, key_type, key_off, key_len, key_null_field, n_fields,
-                     field_kind, n_fns, fn, fn_arg, limit_fn, limit, dst_base, dst_cap, dst_total, n_records,
-                     n_out_records, status, bad_slice);
+                     slice_checksum, n_keys, key_type, key_off, key_len, key_null_field, ws, dst_base, dst_cap,
+                     dst_total, n_out_records, status, bad_slice);
 }
 
 int b2s_decompress_window_rows_keys_dev(
@@ -4054,10 +4164,42 @@ int b2s_decompress_window_rows_keys_dev(
     const uint8_t* field_kind, uint32_t n_fns, const uint32_t* fn, const int32_t* fn_arg, uint32_t limit_fn,
     int32_t limit, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records,
     uint64_t* n_out_records, int32_t* status, int32_t* bad_slice) {
+  WindowSpec ws =
+      window_ranking_spec(n_partition_keys, n_fields, field_kind, n_fns, fn, fn_arg, limit_fn, limit, n_records);
   return window_call(dev_index, false, codec, checksum_alg, n, src_base, src_off, src_len, slice_base, slice_len,
-                     slice_checksum, n_partition_keys, n_keys, key_type, key_off, key_len, key_null_field, n_fields,
-                     field_kind, n_fns, fn, fn_arg, limit_fn, limit, dst_base, dst_cap, dst_total, n_records,
-                     n_out_records, status, bad_slice);
+                     slice_checksum, n_keys, key_type, key_off, key_len, key_null_field, ws, dst_base, dst_cap,
+                     dst_total, n_out_records, status, bad_slice);
+}
+
+int b2s_decompress_window_aggregate_rows_keys_packed(
+    uint32_t codec, uint32_t checksum_alg, uint32_t n, const uint8_t* src_base, const uint64_t* src_off,
+    const uint64_t* src_len, const uint32_t* slice_base, const uint64_t* slice_len, const uint64_t* slice_checksum,
+    uint32_t n_partition_keys, uint32_t n_keys, const uint32_t* key_type, const uint32_t* key_off,
+    const uint32_t* key_len, const int32_t* key_null_field, uint32_t n_fields, const uint8_t* field_kind,
+    uint32_t n_fns, const uint32_t* fn, const int32_t* fn_arg, const uint32_t* fn_frame, const uint32_t* val_type,
+    const uint32_t* val_off, const int32_t* val_null_field, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_total,
+    uint64_t* n_records, uint64_t* n_out_records, int32_t* status, int32_t* bad_slice) {
+  WindowSpec ws = window_aggregate_spec(n_partition_keys, n_fields, field_kind, n_fns, fn, fn_arg, fn_frame,
+                                        val_type, val_off, val_null_field, n_records);
+  return window_call(t_device, true, codec, checksum_alg, n, src_base, src_off, src_len, slice_base, slice_len,
+                     slice_checksum, n_keys, key_type, key_off, key_len, key_null_field, ws, dst_base, dst_cap,
+                     dst_total, n_out_records, status, bad_slice);
+}
+
+int b2s_decompress_window_aggregate_rows_keys_dev(
+    uint32_t dev_index, uint32_t codec, uint32_t checksum_alg, uint32_t n, const uint8_t* src_base,
+    const uint64_t* src_off, const uint64_t* src_len, const uint32_t* slice_base, const uint64_t* slice_len,
+    const uint64_t* slice_checksum, uint32_t n_partition_keys, uint32_t n_keys, const uint32_t* key_type,
+    const uint32_t* key_off, const uint32_t* key_len, const int32_t* key_null_field, uint32_t n_fields,
+    const uint8_t* field_kind, uint32_t n_fns, const uint32_t* fn, const int32_t* fn_arg, const uint32_t* fn_frame,
+    const uint32_t* val_type, const uint32_t* val_off, const int32_t* val_null_field, uint8_t* dst_base,
+    uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records, uint64_t* n_out_records, int32_t* status,
+    int32_t* bad_slice) {
+  WindowSpec ws = window_aggregate_spec(n_partition_keys, n_fields, field_kind, n_fns, fn, fn_arg, fn_frame,
+                                        val_type, val_off, val_null_field, n_records);
+  return window_call(dev_index, false, codec, checksum_alg, n, src_base, src_off, src_len, slice_base, slice_len,
+                     slice_checksum, n_keys, key_type, key_off, key_len, key_null_field, ws, dst_base, dst_cap,
+                     dst_total, n_out_records, status, bad_slice);
 }
 
 // ------------------------------------------------------------------------------------------------------------

@@ -521,12 +521,15 @@ void launch_join_emit(const uint8_t* arena, uint64_t n, const uint32_t* idx, uin
                       bool whole, uint8_t* d_ws, uint8_t* d_jws, uint32_t n_ranges, uint8_t* d_dst, cudaStream_t st,
                       uint64_t* launches);
 
-// ---------------- window.cu (Spark's WindowExec ranking functions over a reducer's key-sorted rows) ----------------
+// ---------------- window.cu (Spark's WindowExec ranking and aggregate functions over a reducer's key-sorted rows) -------
 // The records, stably sorted by the window's key (partition columns, then order columns: launch_rows_order) and grouped
 // by the whole key (launch_rows_group: the peer groups).  The shape of the output row: the input's field count n,
 // null-bitset words bw, the output's out_bw = ceil((n + n_fns) / 64), the functions (B2S_WINDOW_*) and their
 // arguments, the limit (limit_fn B2S_WINDOW_NO_LIMIT: none), the partition columns (the key's first part.n columns),
-// and the input's VAR and DECIMAL_WIDE fields (their slots' offsets move), as a device list.
+// and the input's VAR and DECIMAL_WIDE fields (their slots' offsets move), as a device list.  An aggregate function f
+// (fn[f] >= B2S_WINDOW_SUM) has its frame, input type (B2S_WINDOW_VAL_*, a decimal's p and s above), slot and null bit
+// (-1: never null), its index agg[f] among the n_agg aggregate functions, and wide[f], its ordinal among the n_wide
+// functions with a DECIMAL_WIDE result (-1 for every other function).
 constexpr uint32_t kMaxWindowFns = 16;
 struct WindowShape {
   uint32_t n, bw, out_bw;
@@ -538,25 +541,34 @@ struct WindowShape {
   uint32_t n_var;
   const uint32_t* var;
   KeySpec part;
+  uint32_t frame[kMaxWindowFns];
+  uint32_t vtype[kMaxWindowFns];
+  uint32_t voff[kMaxWindowFns];
+  int32_t vnull[kMaxWindowFns];
+  uint32_t agg[kMaxWindowFns];
+  int32_t wide[kMaxWindowFns];
+  uint32_t n_agg, n_wide;
 };
-// d_wws: window_ws_bytes(n, n_fns, n_fields) bytes
-size_t window_ws_bytes(uint64_t n, uint32_t n_fns, uint32_t n_fields);
-// the readback: [output records, output bytes, an output row is too long (0 / 1), a partition is too large (0 / 1)]
-uint64_t* window_readback(uint8_t* d_wws, uint64_t n, uint32_t n_fns);
-constexpr size_t kWindowReadbackBytes = 32;
+// d_wws: window_ws_bytes(n, shape) bytes
+size_t window_ws_bytes(uint64_t n, const WindowShape& shape);
+// the readback: [output records, output bytes, an output row is too long (0 / 1), a partition is too large (0 / 1),
+// the first bad DECIMAL_WIDE input (its arena offset << 2 | kAggBadDecimal; ~0: none)]
+uint64_t* window_readback(uint8_t* d_wws, uint64_t n, const WindowShape& shape);
+constexpr size_t kWindowReadbackBytes = 40;
 // Per sorted position: whether it starts a partition (only peer heads compare their partition columns with their
-// predecessor's, encoded 16 bytes at a time), scanned, and the partitions' starts compacted; then every function's
-// value, whether the limit keeps the record and its output bytes, the kept records and bytes scanned, the totals and
-// the verdicts into the readback.  Uploads the shape and its field list (h_fields: shape.n_var fields).  idx: the
-// sorted order (nullptr: arena order); d_aws: launch_rows_group's workspace.
+// predecessor's, encoded 16 bytes at a time), scanned, and the partitions' starts compacted; with aggregate functions,
+// their inputs staged and folded from each partition's start; then every function's value, whether the limit keeps
+// the record and its output bytes, the kept records and bytes scanned, the totals and the verdicts into the readback.
+// Uploads the shape and its field list (h_fields: shape.n_var fields).  idx: the sorted order (nullptr: arena order);
+// d_aws: launch_rows_group's workspace.
 void launch_window_values(const uint8_t* arena, uint64_t n, const uint32_t* idx, WindowShape shape,
                           const uint32_t* h_fields, uint32_t key_bytes, uint8_t* d_ws, uint8_t* d_aws, uint8_t* d_wws,
                           cudaStream_t st, uint64_t* launches);
 // the out_rows output records (read back) to d_dst, a warp per record; with a limit the kept positions are compacted
 // first, so only they are read
 void launch_window_emit(const uint8_t* arena, uint64_t n, const uint32_t* idx, uint64_t out_rows, uint32_t key_bytes,
-                        uint32_t n_fns, bool limited, uint8_t* d_ws, uint8_t* d_wws, uint8_t* d_dst, cudaStream_t st,
-                        uint64_t* launches);
+                        const WindowShape& shape, bool limited, uint8_t* d_ws, uint8_t* d_wws, uint8_t* d_dst,
+                        cudaStream_t st, uint64_t* launches);
 
 // ---------------- exchange.cu (exchange-cache reads: ranges of device memory gathered into one arena) ----------------
 // piece: len bytes at src (device pointer, any alignment) go to d_dst + dst

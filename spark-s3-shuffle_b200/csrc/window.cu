@@ -1,20 +1,31 @@
 // window.cu — Spark's WindowExec on a reducer for the ranking functions (row_number, rank, dense_rank, percent_rank,
-// cume_dist, ntile), with WindowGroupLimitExec's limit, and the output rows built as UnsafeRowJoiner joins the input
-// row with the row of values.  The records have been framed, keyed by the whole window key (partition columns, then
+// cume_dist, ntile), with WindowGroupLimitExec's limit, and for the aggregate functions (sum, count, min, max, avg)
+// over whole-partition and running frames, and the output rows built as UnsafeRowJoiner joins the input row with the
+// row of values.  The records have been framed, keyed by the whole window key (partition columns, then
 // order columns), stably sorted by rows.cu and grouped by aggregate.cu's launch_rows_group, whose groups are the peer
 // groups.  All on the device:
 //   heads  : one thread per sorted position: a partition starts at a peer head whose partition columns differ from its
 //            predecessor's, compared by encode_key 16 encoded bytes at a time until they differ or both keys end (so
 //            the equality is the sort's: strings by length and bytes, -0.0 with 0.0, NaN with NaN, null with null);
 //            the flags scanned, and each partition's first position compacted
+//   stage  : (aggregate functions) one thread per sorted position: each aggregate's input, null flag and, for a
+//            DECIMAL_WIDE input, its 16 bytes checked, into dense sorted-order state arrays (lo, hi, count)
+//   fold   : each state becomes its fold over the partition's positions up to it.  Integer sums, counts, decimal sums
+//            and min / max are associative: a log-step segmented scan, one pass per power of two below n, each
+//            position combining with the one d before it while that is in its partition (min / max keep the earlier
+//            of equal values).  Double sums are serial by contract: a warp per partition, 32 positions a round loaded
+//            one round ahead, each lane's value broadcast in turn and added in order, each lane keeping its prefix
 //   values : one thread per sorted position: from its partition's bounds and its peer group's bounds and index, every
-//            function's value (into a per-function array in sorted order), whether the limit keeps it, and its output
-//            bytes; the kept records and the bytes scanned, and the totals and the too-long and too-large-partition
+//            function's value (into a per-function array in sorted order; an aggregate's read from the fold at its
+//            frame's last position, with its null flag and a wide decimal's high word), whether the limit keeps it,
+//            and its output bytes; the kept records and the bytes scanned, and the totals and the too-long and too-large-partition
 //            flags come back in one readback
-//   emit   : a warp per output row (with a limit, over the compacted kept positions only): its null words widened, its
-//            slots, the function slots and its var bytes, then the VAR and DECIMAL_WIDE slots' offsets moved
+//   emit   : a warp per output row (with a limit, over the compacted kept positions only): its null words widened (with
+//            the values' null bits), its slots, the function slots, its var bytes and the wide decimal results' 16
+//            bytes each, then the VAR and DECIMAL_WIDE slots' offsets moved
 #include <algorithm>
 
+#include "decimal128.h"
 #include "rows_key.cuh"
 
 namespace b2s {
@@ -33,7 +44,8 @@ inline unsigned grid_for(uint64_t n) {
 // the window workspace: per position the partition-head flags (scanned in place, the partition count at [n]), the
 // partitions' first positions (n after the last), every function's value (function f at [f n, f n + n)), the kept
 // records and the output bytes (scanned in place), the kept positions compacted; scan workspace, readback, the shape
-// and its field list
+// and its field list; then, with aggregate functions, two sets of fold state (aggregate a at [a n, a n + n) of each
+// array), the values' null bits per position and the wide decimal results' high words (wide ordinal k at [k n, k n + n))
 struct WindowWs {
   uint64_t* phead;
   uint32_t* pstart;
@@ -45,21 +57,34 @@ struct WindowWs {
   uint64_t* readback;
   WindowShape* shape;
   uint32_t* fields;
+  uint64_t* lo[2];
+  uint64_t* hi[2];
+  uint32_t* cnt[2];
+  uint32_t* vnul;
+  uint64_t* vhi;
 };
 
-WindowWs carve_window_ws(uint8_t* d_wws, uint64_t n, uint32_t n_fns) {
+WindowWs carve_window_ws(uint8_t* d_wws, uint64_t n, const WindowShape& sh) {
   WindowWs w;
   uint8_t* p = d_wws;
   w.phead = (uint64_t*)p;    p += a256((n + 1) * 8);
   w.pstart = (uint32_t*)p;   p += a256((n + 1) * 4);
-  w.vals = (uint64_t*)p;     p += a256((size_t)n_fns * n * 8);
+  w.vals = (uint64_t*)p;     p += a256((size_t)sh.n_fns * n * 8);
   w.rows = (uint64_t*)p;     p += a256(n * 8);
   w.bytes = (uint64_t*)p;    p += a256(n * 8);
   w.kept = (uint32_t*)p;     p += a256(n * 4);
   w.scan_ws = (uint64_t*)p;  p += a256(scan_ws_elems(n + 1) * 8);
   w.readback = (uint64_t*)p; p += a256(kWindowReadbackBytes);
   w.shape = (WindowShape*)p; p += a256(sizeof(WindowShape));
-  w.fields = (uint32_t*)p;
+  w.fields = (uint32_t*)p;   p += a256((size_t)sh.n * 4);
+  const size_t m = (size_t)sh.n_agg * n;
+  for (int b = 0; b < 2; b++) {
+    w.lo[b] = (uint64_t*)p;  p += a256(m * 8);
+    w.hi[b] = (uint64_t*)p;  p += a256(m * 8);
+    w.cnt[b] = (uint32_t*)p; p += a256(m * 4);
+  }
+  w.vnul = (uint32_t*)p;     p += a256(sh.n_agg ? n * 4 : 0);
+  w.vhi = (uint64_t*)p;      p += a256((size_t)sh.n_wide * n * 8);
   return w;
 }
 
@@ -127,33 +152,281 @@ __device__ __forceinline__ uint64_t ntile(uint64_t i, uint64_t N, uint64_t k) {
   return i < big ? i / (q + 1) + 1 : r + (i - big) / q + 1;
 }
 
+// ---- aggregate functions ----
+constexpr unsigned kFull = 0xffffffffu;
+
+__device__ __forceinline__ uint32_t val_kind(uint32_t vt) { return vt & 0xff; }
+__device__ __forceinline__ uint32_t dec_p(uint32_t vt) { return (vt >> 8) & 0xff; }
+
+// SUM of a float or double and AVG of anything but a decimal fold in double, serially; every other aggregate is a
+// group operation (or min / max) and scans
+__device__ __forceinline__ bool folds_double(uint32_t fn, uint32_t vt) {
+  const uint32_t k = val_kind(vt);
+  return (fn == B2S_WINDOW_SUM && (k == B2S_WINDOW_VAL_FLOAT32 || k == B2S_WINDOW_VAL_FLOAT64)) ||
+         (fn == B2S_WINDOW_AVG && k != B2S_WINDOW_VAL_DECIMAL);
+}
+
+// a decimal result's precision: SUM p + 10, AVG p + 4, MIN / MAX p
+__device__ __forceinline__ uint32_t result_p(uint32_t fn, uint32_t vt) {
+  return dec_p(vt) + (fn == B2S_WINDOW_SUM ? 10 : fn == B2S_WINDOW_AVG ? 4 : 0);
+}
+
+__device__ __forceinline__ bool null_bit(const uint8_t* row, int32_t field) {
+  return field >= 0 && (ld64(row + 8 * (uint32_t)(field >> 6)) >> (field & 63)) & 1;
+}
+
+// Stage: per aggregate a (function f) and position j, (lo, hi) = the input as a signed 128-bit integer (ints and
+// decimals), its float or double bits (MIN / MAX of floats), or its double bits (double folds); count = 1 when it is
+// present (always for VAL_NONE), else 0 with (lo, hi) = 0.  A bad non-null DECIMAL_WIDE input lowers *bad to its
+// record's arena offset << 2 | kAggBadDecimal.
+__global__ void __launch_bounds__(kWindowThreads) window_stage_kernel(
+    const uint8_t* __restrict__ arena, const uint64_t* __restrict__ rec_off, const uint32_t* __restrict__ rec_len,
+    const uint32_t* __restrict__ idx, uint64_t n, const WindowShape* __restrict__ sh, uint64_t* __restrict__ lo,
+    uint64_t* __restrict__ hi, uint32_t* __restrict__ cnt, unsigned long long* __restrict__ bad) {
+  const uint32_t n_fns = sh->n_fns;
+  for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (uint64_t)gridDim.x * blockDim.x) {
+    const uint32_t i = at(idx, j);
+    const uint8_t* row = arena + rec_off[i] + 4;
+    for (uint32_t f = 0; f < n_fns; f++) {
+      const uint32_t fn = sh->fn[f];
+      if (fn < B2S_WINDOW_SUM) continue;
+      const uint32_t vt = sh->vtype[f], k = val_kind(vt);
+      uint64_t l = 0, h = 0;
+      uint32_t c = 1;
+      if (k != B2S_WINDOW_VAL_NONE) {
+        c = !null_bit(row, sh->vnull[f]);
+        if (c) {
+          const uint64_t v = ld64(row + sh->voff[f]);
+          switch (k) {
+            case B2S_WINDOW_VAL_INT8: l = (uint64_t)(int64_t)(int8_t)v; break;
+            case B2S_WINDOW_VAL_INT16: l = (uint64_t)(int64_t)(int16_t)v; break;
+            case B2S_WINDOW_VAL_INT32: l = (uint64_t)(int64_t)(int32_t)v; break;
+            case B2S_WINDOW_VAL_FLOAT32: l = (uint32_t)v; break;
+            default: l = v; break;  // INT64, FLOAT64, a decimal's long
+          }
+          h = (uint64_t)((int64_t)l >> 63);
+          if (k == B2S_WINDOW_VAL_DECIMAL && dec_p(vt) > 18) {
+            bool b = false;
+            decimal_bits(row, rec_len[i] - 4, v, h, l, &b);
+            h ^= 1ull << 63;  // decimal_bits flips the sign bit for the sort
+            if (b) atomicMin(bad, (unsigned long long)((rec_off[i] << 2) | kAggBadDecimal));
+          }
+          if (folds_double(fn, vt))
+            l = k == B2S_WINDOW_VAL_FLOAT32   ? __double_as_longlong((double)__int_as_float((int)l))
+                : k == B2S_WINDOW_VAL_FLOAT64 ? l
+                                              : __double_as_longlong(__ll2double_rn((long long)l));
+        }
+      }
+      const size_t at_a = (size_t)sh->agg[f] * n + j;
+      lo[at_a] = l;
+      hi[at_a] = h;
+      cnt[at_a] = c;
+    }
+  }
+}
+
+// Spark SQL's a < b for floats (k FLOAT32: the low 32 bits) or doubles: -0.0 == 0.0, NaN above everything else
+__device__ __forceinline__ bool float_less(uint32_t k, uint64_t a, uint64_t b) {
+  const double x = k == B2S_WINDOW_VAL_FLOAT32 ? (double)__int_as_float((int)a) : __longlong_as_double(a);
+  const double y = k == B2S_WINDOW_VAL_FLOAT32 ? (double)__int_as_float((int)b) : __longlong_as_double(b);
+  if (isnan(y)) return !isnan(x);
+  return x < y;
+}
+
+// One pass of the segmented scan: position j takes the combination of j - d's state (earlier) and its own when j - d
+// is in its partition, else keeps its own.  Only the scanning aggregates are touched.
+__global__ void __launch_bounds__(kWindowThreads) window_scan_pass_kernel(
+    uint64_t n, const WindowShape* __restrict__ sh, const uint64_t* __restrict__ phead,
+    const uint32_t* __restrict__ pstart, uint64_t d, const uint64_t* __restrict__ lo_in,
+    const uint64_t* __restrict__ hi_in, const uint32_t* __restrict__ cnt_in, uint64_t* __restrict__ lo_out,
+    uint64_t* __restrict__ hi_out, uint32_t* __restrict__ cnt_out) {
+  const uint64_t P = phead[n];
+  const uint32_t n_fns = sh->n_fns;
+  for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (uint64_t)gridDim.x * blockDim.x) {
+    const bool take = j >= pstart[next_scanned(phead, j, n, P) - 1] + d;
+    for (uint32_t f = 0; f < n_fns; f++) {
+      const uint32_t fn = sh->fn[f], vt = sh->vtype[f];
+      if (fn < B2S_WINDOW_SUM || folds_double(fn, vt)) continue;
+      const size_t x = (size_t)sh->agg[f] * n + j;
+      uint64_t l = lo_in[x], h = hi_in[x];
+      uint32_t c = cnt_in[x];
+      if (take) {
+        const uint64_t l0 = lo_in[x - d], h0 = hi_in[x - d];
+        const uint32_t c0 = cnt_in[x - d];
+        if (fn == B2S_WINDOW_MIN || fn == B2S_WINDOW_MAX) {
+          const uint32_t k = val_kind(vt);
+          const bool fl = k == B2S_WINDOW_VAL_FLOAT32 || k == B2S_WINDOW_VAL_FLOAT64;
+          const bool later_wins = fn == B2S_WINDOW_MIN
+                                      ? (fl ? float_less(k, l, l0) : dec_less(Dec128{l, h}, Dec128{l0, h0}))
+                                      : (fl ? float_less(k, l0, l) : dec_less(Dec128{l0, h0}, Dec128{l, h}));
+          if (c0 && !(c && later_wins)) {
+            l = l0;
+            h = h0;
+          }
+        } else {  // sums and counts, modulo 2^128
+          bool unused;
+          const Dec128 s = dec_add(Dec128{l0, h0}, Dec128{l, h}, &unused);
+          l = s.lo;
+          h = s.hi;
+        }
+        c += c0;
+      }
+      lo_out[x] = l;
+      hi_out[x] = h;
+      cnt_out[x] = c;
+    }
+  }
+}
+
+// The double folds: a warp per partition, ((0.0 + x1) + x2) + ... over the present inputs in sorted order, the running
+// sum and count written at every position.  lo_in / cnt_in may be lo_out / cnt_out: a position is read a round before
+// it is written, by the lane that writes it.
+__global__ void __launch_bounds__(kWindowThreads) window_fold_kernel(
+    uint64_t n, const WindowShape* __restrict__ sh, const uint64_t* __restrict__ phead,
+    const uint32_t* __restrict__ pstart, const uint64_t* lo_in, const uint32_t* cnt_in, uint64_t* lo_out,
+    uint32_t* cnt_out) {
+  const uint32_t lane = threadIdx.x & 31;
+  const uint64_t warps = (uint64_t)gridDim.x * (blockDim.x / 32);
+  const uint64_t P = phead[n];
+  const uint32_t n_fns = sh->n_fns;
+  for (uint64_t p = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) / 32; p < P; p += warps) {
+    const uint64_t s = pstart[p], e = pstart[p + 1];
+    for (uint32_t f = 0; f < n_fns; f++) {
+      if (sh->fn[f] < B2S_WINDOW_SUM || !folds_double(sh->fn[f], sh->vtype[f])) continue;
+      const size_t base = (size_t)sh->agg[f] * n;
+      double acc = 0.0;
+      uint32_t seen = 0;
+      uint64_t j = s + lane;
+      double x = j < e ? __longlong_as_double(lo_in[base + j]) : 0.0;
+      uint32_t c = j < e ? cnt_in[base + j] : 0;
+      for (uint64_t r = s; r < e; r += 32) {
+        const uint64_t jn = r + 32 + lane;
+        const double xn = jn < e ? __longlong_as_double(lo_in[base + jn]) : 0.0;
+        const uint32_t cn = jn < e ? cnt_in[base + jn] : 0;
+        const unsigned present = __ballot_sync(kFull, c != 0);
+        double mine = acc;
+#pragma unroll
+        for (uint32_t k = 0; k < 32; k++) {
+          const double y = __shfl_sync(kFull, x, k);
+          if ((present >> k) & 1) acc = __dadd_rn(acc, y);
+          if (lane == k) mine = acc;
+        }
+        j = r + lane;
+        if (j < e) {
+          lo_out[base + j] = __double_as_longlong(mine);
+          cnt_out[base + j] = seen + __popc(present & (0xffffffffu >> (31 - lane)));
+        }
+        seen += __popc(present);
+        x = xn;
+        c = cn;
+      }
+    }
+  }
+}
+
+// the exact decimal average: S / c rounded HALF_UP to 4 more digits, as q0 10^4 + round(r0 10^4 / c) with
+// q0 = |S| / c and r0 = |S| % c (c < 2^32, so each 32-bit limb's step divides a 64-bit number)
+__device__ __forceinline__ Dec128 dec_avg(Dec128 x, uint32_t c) {
+  const bool neg = x.hi >> 63;
+  if (neg) {
+    x.lo = ~x.lo + 1;
+    x.hi = ~x.hi + (x.lo == 0);
+  }
+  const uint32_t limb[4] = {(uint32_t)(x.hi >> 32), (uint32_t)x.hi, (uint32_t)(x.lo >> 32), (uint32_t)x.lo};
+  uint64_t r = 0, q[4];
+#pragma unroll
+  for (int k = 0; k < 4; k++) {
+    const uint64_t cur = (r << 32) | limb[k];
+    q[k] = cur / c;
+    r = cur % c;
+  }
+  const uint64_t ql = (q[2] << 32) | q[3], qh = (q[0] << 32) | q[1];
+  const uint64_t frac = (r * 20000 + c) / (2ull * c);  // r 10^4 / c rounded half up, 0..10^4
+  Dec128 y;
+  y.lo = ql * 10000;
+  y.hi = qh * 10000 + __umul64hi(ql, 10000);
+  const uint64_t lo = y.lo + frac;
+  y.hi += lo < y.lo;
+  y.lo = lo;
+  if (neg) {
+    y.lo = ~y.lo + 1;
+    y.hi = ~y.hi + (y.lo == 0);
+  }
+  return y;
+}
+
+// The state arrays an aggregate's value is read from (the folds), and where the values kernel puts the values' null
+// bits (a mask per position) and wide decimal results' high words; all nullptr without aggregate functions
+struct WindowAggIo {
+  const uint64_t* lo;
+  const uint64_t* hi;
+  const uint32_t* cnt;
+  uint32_t* vnul;
+  uint64_t* vhi;
+};
+
+// aggregate f's value at position j from the fold at its frame's last position e; *null when it is null (slot 0)
+__device__ uint64_t agg_value(const WindowShape* __restrict__ sh, uint32_t f, const WindowAggIo& io, uint64_t n,
+                              uint64_t e, uint64_t j, bool* null) {
+  const uint32_t fn = sh->fn[f], vt = sh->vtype[f], k = val_kind(vt);
+  const size_t x = (size_t)sh->agg[f] * n + e;
+  const uint32_t c = io.cnt[x];
+  if (fn == B2S_WINDOW_COUNT) return c;
+  *null = c == 0;
+  if (!c) return 0;
+  uint64_t l = io.lo[x];
+  if (folds_double(fn, vt))
+    return fn == B2S_WINDOW_AVG ? __double_as_longlong(__ddiv_rn(__longlong_as_double(l), (double)c)) : l;
+  if (k != B2S_WINDOW_VAL_DECIMAL) {
+    if (fn == B2S_WINDOW_SUM) return l;
+    return k == B2S_WINDOW_VAL_INT8 ? l & 0xff : k == B2S_WINDOW_VAL_INT16 ? l & 0xffff
+           : k == B2S_WINDOW_VAL_INT32 || k == B2S_WINDOW_VAL_FLOAT32 ? l & 0xffffffffull : l;
+  }
+  Dec128 v{l, io.hi[x]};
+  if (fn == B2S_WINDOW_AVG) v = dec_avg(v, c);
+  if (result_p(fn, vt) > 18) io.vhi[(size_t)sh->wide[f] * n + j] = v.hi;
+  return v.lo;
+}
+
 __global__ void __launch_bounds__(kWindowThreads) window_values_kernel(
     const uint32_t* __restrict__ rec_len, const uint32_t* __restrict__ idx, uint64_t n,
     const WindowShape* __restrict__ sh, const uint64_t* __restrict__ heads_before, const uint32_t* __restrict__ gpos,
     const uint64_t* __restrict__ groups, const uint64_t* __restrict__ phead, const uint32_t* __restrict__ pstart,
     uint64_t* __restrict__ vals, uint64_t* __restrict__ rows, uint64_t* __restrict__ bytes,
-    uint64_t* __restrict__ readback) {
+    uint64_t* __restrict__ readback, WindowAggIo io) {
   const uint64_t G = *groups, P = phead[n];
   const uint32_t n_fns = sh->n_fns, limit_fn = sh->limit_fn;
-  const uint64_t grow = 8ull * (sh->out_bw - sh->bw + n_fns);  // what the output row adds to the input row
+  // what the output row adds to the input row
+  const uint64_t grow = 8ull * (sh->out_bw - sh->bw + n_fns) + 16ull * sh->n_wide;
   for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (uint64_t)gridDim.x * blockDim.x) {
     const uint64_t g = next_scanned(heads_before, j, n, G) - 1, p = next_scanned(phead, j, n, P) - 1;
     const uint64_t ps = pstart[p], N = pstart[p + 1] - ps;
     const uint64_t i = j - ps, gs = gpos[g] - ps, ge = gpos[g + 1] - ps;
     const uint64_t dense = g - heads_before[ps] + 1;  // ps is a peer head: heads_before[ps] is its group
     if (N > 0x7fffffffull) readback[3] = 1;
+    uint32_t nul = 0;
     for (uint32_t f = 0; f < n_fns; f++) {
       uint64_t v;
+      bool null = false;
       switch (sh->fn[f]) {
         case B2S_WINDOW_ROW_NUMBER: v = int_slot(i + 1); break;
         case B2S_WINDOW_RANK: v = int_slot(gs + 1); break;
         case B2S_WINDOW_DENSE_RANK: v = int_slot(dense); break;
         case B2S_WINDOW_PERCENT_RANK: v = __double_as_longlong(N > 1 ? (double)gs / (double)(N - 1) : 0.0); break;
         case B2S_WINDOW_CUME_DIST: v = __double_as_longlong((double)ge / (double)N); break;
-        default: v = int_slot(ntile(i, N, sh->arg[f])); break;
+        case B2S_WINDOW_NTILE: v = int_slot(ntile(i, N, sh->arg[f])); break;
+        default: {
+          const uint32_t fr = sh->frame[f];
+          const uint64_t e = fr == B2S_WINDOW_FRAME_ROWS_RUNNING ? j
+                             : fr == B2S_WINDOW_FRAME_RANGE_RUNNING ? ps + ge - 1 : ps + N - 1;
+          v = agg_value(sh, f, io, n, e, j, &null);
+          break;
+        }
       }
       vals[(size_t)f * n + j] = v;
+      nul |= (uint32_t)null << f;
     }
+    if (io.vnul) io.vnul[j] = nul;
     bool keep = true;
     if (limit_fn != B2S_WINDOW_NO_LIMIT) {
       const uint64_t lv = limit_fn == B2S_WINDOW_ROW_NUMBER ? i + 1 : limit_fn == B2S_WINDOW_RANK ? gs + 1 : dense;
@@ -179,10 +452,10 @@ __global__ void __launch_bounds__(kWindowThreads) window_emit_kernel(
     const uint8_t* __restrict__ arena, const uint64_t* __restrict__ rec_off, const uint32_t* __restrict__ rec_len,
     const uint32_t* __restrict__ idx, uint64_t n, uint64_t out_rows, const uint32_t* __restrict__ kept,
     const WindowShape* __restrict__ sh, const uint64_t* __restrict__ vals, const uint64_t* __restrict__ bytes,
-    uint8_t* __restrict__ dst) {
+    const uint32_t* __restrict__ vnul, const uint64_t* __restrict__ vhi, uint8_t* __restrict__ dst) {
   const uint32_t lane = threadIdx.x & 31;
   const uint64_t warps = (uint64_t)gridDim.x * (blockDim.x / 32);
-  const uint32_t nf = sh->n, bw = sh->bw, b = sh->out_bw, n_fns = sh->n_fns;
+  const uint32_t nf = sh->n, bw = sh->bw, b = sh->out_bw, n_fns = sh->n_fns, n_wide = sh->n_wide;
   const uint32_t fixed_in = 8 * (bw + nf);
   const uint64_t fixed_out = 8ull * (b + nf + n_fns);
   const uint64_t shift = 8ull * (b - bw + n_fns) << 32;
@@ -193,7 +466,8 @@ __global__ void __launch_bounds__(kWindowThreads) window_emit_kernel(
     const uint64_t var = rec_len[i] - 4 - fixed_in;
     uint8_t* d = dst + bytes[j];
     uint8_t* row = d + 4;
-    if (lane == 0) st_span16(d, 4, __byte_perm((uint32_t)(fixed_out + var), 0, 0x0123), 0);
+    if (lane == 0) st_span16(d, 4, __byte_perm((uint32_t)(fixed_out + var + 16 * n_wide), 0, 0x0123), 0);
+    const uint32_t nul = vnul ? vnul[j] : 0;
     for (uint32_t w = lane; w < b; w += 32) {
       uint64_t bits = 0;
       if (w < bw) {
@@ -201,10 +475,29 @@ __global__ void __launch_bounds__(kWindowThreads) window_emit_kernel(
         const uint64_t left = nf - 64ull * w;
         if (left < 64) bits &= (1ull << left) - 1;
       }
+      for (uint32_t f = 0; f < n_fns; f++)  // the values' null bits nf + f
+        if ((nul >> f) & 1 && (nf + f) >> 6 == w) bits |= 1ull << ((nf + f) & 63);
       st_span16(row + 8 * w, 8, bits, 0);
     }
     warp_copy(row + 8 * b, src + 8 * bw, 8ull * nf, lane);
-    for (uint32_t f = lane; f < n_fns; f += 32) st_span16(row + 8 * (b + nf + f), 8, vals[(size_t)f * n + j], 0);
+    for (uint32_t f = lane; f < n_fns; f += 32) {
+      uint64_t slot = vals[(size_t)f * n + j];
+      const int32_t k = sh->wide[f];
+      if (k >= 0) {  // 16 bytes after the var bytes: BigInteger.toByteArray's, or zeros when null
+        const uint64_t off = fixed_out + var + 16ull * (uint32_t)k;
+        uint64_t m0 = 0, m1 = 0;
+        if ((nul >> f) & 1) {
+          slot = off << 32;
+        } else {
+          const Dec128 x{slot, vhi[(size_t)k * n + j]};
+          const uint32_t len = dec_bytes(x);
+          dec_encode(x, len, &m0, &m1);
+          slot = off << 32 | len;
+        }
+        st_span16(row + off, 16, m0, m1);
+      }
+      st_span16(row + 8 * (b + nf + f), 8, slot, 0);
+    }
     warp_copy(row + fixed_out, src + fixed_in, var, lane);
     __syncwarp();
     // a zero slot (a null string) stays zero
@@ -219,44 +512,77 @@ __global__ void __launch_bounds__(kWindowThreads) window_emit_kernel(
 
 }  // namespace
 
-size_t window_ws_bytes(uint64_t n, uint32_t n_fns, uint32_t n_fields) {
-  return a256((n + 1) * 8) + a256((n + 1) * 4) + a256((size_t)n_fns * n * 8) + 2 * a256(n * 8) + a256(n * 4) +
-         a256(scan_ws_elems(n + 1) * 8) + a256(kWindowReadbackBytes) + a256(sizeof(WindowShape)) +
-         a256((size_t)n_fields * 4);
+size_t window_ws_bytes(uint64_t n, const WindowShape& shape) {
+  const WindowWs w = carve_window_ws(nullptr, n, shape);  // the parts' offsets from 0
+  return reinterpret_cast<uintptr_t>(w.vhi) + a256((size_t)shape.n_wide * n * 8);
 }
 
-uint64_t* window_readback(uint8_t* d_wws, uint64_t n, uint32_t n_fns) {
-  return carve_window_ws(d_wws, n, n_fns).readback;
+uint64_t* window_readback(uint8_t* d_wws, uint64_t n, const WindowShape& shape) {
+  return carve_window_ws(d_wws, n, shape).readback;
 }
 
 void launch_window_values(const uint8_t* arena, uint64_t n, const uint32_t* idx, WindowShape shape,
                           const uint32_t* h_fields, uint32_t key_bytes, uint8_t* d_ws, uint8_t* d_aws, uint8_t* d_wws,
                           cudaStream_t st, uint64_t* launches) {
-  const WindowWs w = carve_window_ws(d_wws, n, shape.n_fns);
+  const WindowWs w = carve_window_ws(d_wws, n, shape);
   const KeySortWs k = carve_key_sort_ws(d_ws, n, key_bytes);
   shape.var = w.fields;
   cudaMemcpyAsync(w.shape, &shape, sizeof(WindowShape), cudaMemcpyHostToDevice, st);
   if (shape.n_var) cudaMemcpyAsync(w.fields, h_fields, (size_t)shape.n_var * 4, cudaMemcpyHostToDevice, st);
   cudaMemsetAsync(w.readback, 0, kWindowReadbackBytes, st);
+  cudaMemsetAsync(w.readback + 4, 0xff, 8, st);
   const uint64_t* heads_before = rows_group_heads_before(d_aws, n);
   const uint64_t* groups = rows_aggregate_readback(d_aws, n, 0, 0);
   window_part_heads_kernel<<<grid_for(n), kWindowThreads, 0, st>>>(arena, k.src_off, k.len, idx, n, w.shape,
                                                                    heads_before, groups, w.phead);
   launch_exclusive_scan_u64(w.phead, n, w.phead + n, w.scan_ws, st, launches);
   window_part_starts_kernel<<<grid_for(n), kWindowThreads, 0, st>>>(w.phead, n, w.pstart);
+  if (launches) *launches += 2;
+  WindowAggIo io{};
+  if (shape.n_agg) {
+    bool scans = false, folds = false;
+    for (uint32_t f = 0; f < shape.n_fns; f++) {
+      if (shape.fn[f] < B2S_WINDOW_SUM) continue;
+      const uint32_t kind = shape.vtype[f] & 0xff;
+      const bool dbl = (shape.fn[f] == B2S_WINDOW_SUM &&
+                        (kind == B2S_WINDOW_VAL_FLOAT32 || kind == B2S_WINDOW_VAL_FLOAT64)) ||
+                       (shape.fn[f] == B2S_WINDOW_AVG && kind != B2S_WINDOW_VAL_DECIMAL);
+      (dbl ? folds : scans) = true;
+    }
+    window_stage_kernel<<<grid_for(n), kWindowThreads, 0, st>>>(arena, k.src_off, k.len, idx, n, w.shape, w.lo[0],
+                                                                w.hi[0], w.cnt[0],
+                                                                (unsigned long long*)(w.readback + 4));
+    int cur = 0;  // the set holding the scanned folds
+    for (uint64_t d = 1; scans && d < n; d *= 2, cur ^= 1)
+      window_scan_pass_kernel<<<grid_for(n), kWindowThreads, 0, st>>>(n, w.shape, w.phead, w.pstart, d, w.lo[cur],
+                                                                      w.hi[cur], w.cnt[cur], w.lo[cur ^ 1],
+                                                                      w.hi[cur ^ 1], w.cnt[cur ^ 1]);
+    if (folds) {
+      const uint64_t want = (n + kWindowThreads / 32 - 1) / (kWindowThreads / 32);  // at most a warp per partition
+      const unsigned grid = (unsigned)std::min<uint64_t>(want, (uint64_t)kSMs * 16);
+      window_fold_kernel<<<grid, kWindowThreads, 0, st>>>(n, w.shape, w.phead, w.pstart, w.lo[0], w.cnt[0],
+                                                          w.lo[cur], w.cnt[cur]);
+    }
+    io = WindowAggIo{w.lo[cur], w.hi[cur], w.cnt[cur], w.vnul, w.vhi};
+    if (launches) {
+      uint64_t passes = 0;
+      for (uint64_t d = 1; scans && d < n; d *= 2) passes++;
+      *launches += 1 + passes + folds;
+    }
+  }
   window_values_kernel<<<grid_for(n), kWindowThreads, 0, st>>>(k.len, idx, n, w.shape, heads_before,
                                                                rows_group_starts(d_aws, n), groups, w.phead, w.pstart,
-                                                               w.vals, w.rows, w.bytes, w.readback);
+                                                               w.vals, w.rows, w.bytes, w.readback, io);
   launch_exclusive_scan_u64(w.rows, n, w.readback, w.scan_ws, st, launches);
   launch_exclusive_scan_u64(w.bytes, n, w.readback + 1, w.scan_ws, st, launches);
-  if (launches) *launches += 3;
+  if (launches) *launches += 1;
 }
 
 void launch_window_emit(const uint8_t* arena, uint64_t n, const uint32_t* idx, uint64_t out_rows, uint32_t key_bytes,
-                        uint32_t n_fns, bool limited, uint8_t* d_ws, uint8_t* d_wws, uint8_t* d_dst, cudaStream_t st,
-                        uint64_t* launches) {
+                        const WindowShape& shape, bool limited, uint8_t* d_ws, uint8_t* d_wws, uint8_t* d_dst,
+                        cudaStream_t st, uint64_t* launches) {
   if (!out_rows) return;
-  const WindowWs w = carve_window_ws(d_wws, n, n_fns);
+  const WindowWs w = carve_window_ws(d_wws, n, shape);
   const KeySortWs k = carve_key_sort_ws(d_ws, n, key_bytes);
   if (limited) {
     window_compact_kernel<<<grid_for(n), kWindowThreads, 0, st>>>(n, w.rows, out_rows, w.kept);
@@ -265,7 +591,8 @@ void launch_window_emit(const uint8_t* arena, uint64_t n, const uint32_t* idx, u
   const uint64_t want = (out_rows + kWindowThreads / 32 - 1) / (kWindowThreads / 32);
   const unsigned grid = (unsigned)std::min<uint64_t>(want, (uint64_t)kSMs * 16);
   window_emit_kernel<<<grid, kWindowThreads, 0, st>>>(arena, k.src_off, k.len, idx, n, out_rows,
-                                                      limited ? w.kept : nullptr, w.shape, w.vals, w.bytes, d_dst);
+                                                      limited ? w.kept : nullptr, w.shape, w.vals, w.bytes,
+                                                      shape.n_agg ? w.vnul : nullptr, w.vhi, d_dst);
   if (launches) *launches += 1;
 }
 
