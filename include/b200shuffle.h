@@ -40,7 +40,9 @@ extern "C" {
 #define B2S_CODEC_NONE 0
 #define B2S_CODEC_LZ4BLOCK 1      /* "lz4"   : lz4-java LZ4Block stream, XXH32 seed 0x9747b28c & 0x0FFFFFFF */
 #define B2S_CODEC_SNAPPY_XERIAL 2 /* "snappy": xerial SnappyOutputStream framing over raw snappy */
-#define B2S_CODEC_ZSTD 3          /* "zstd"  : RFC 8878 frames, concatenation allowed */
+#define B2S_CODEC_ZSTD 3          /* "zstd"  : RFC 8878 frames, concatenation allowed; a frame's Content_Checksum
+                                   * is skipped, not verified (Spark's ZStdCompressionCodec never sets the flag), so
+                                   * a frame that libzstd rejects for a wrong content checksum alone decodes here */
 
 /* checksum algorithms — spark.shuffle.checksum.algorithm (helper/S3ShuffleHelper.scala:94-103) */
 #define B2S_CHECKSUM_NONE 0
@@ -342,8 +344,8 @@ int b2s_decompress_packed(uint32_t codec, uint32_t checksum_alg, uint32_t n, con
  * verifies and sorts only (spark.shuffle.compress=false).
  * Per block: a corrupt stream, or a decoded length that is not a multiple of record_bytes (b2s_last_error() names the
  * block), sets status[i] = B2S_E_CORRUPT; a checksum mismatch sets B2S_E_CHECKSUM and bad_slice[i] (may be NULL).  When
- * a block fails, nothing is sorted, *n_records = 0 and the call returns 0; blocks whose slices fail verification are
- * not decoded.
+ * a block fails, nothing is sorted, *n_records = *dst_total = 0 and the call returns 0; blocks whose slices fail
+ * verification are not decoded.
  * Errors: key_len outside [1, 16], key_off + key_len > record_bytes, record_bytes == 0 or more than 2^32 - 1 records ->
  * B2S_E_ARG; dst_cap below the decoded bytes -> B2S_E_DST_TOO_SMALL with *dst_total = the bytes needed; device memory
  * for the whole task (compressed blocks, decoded records, sorted copy, sort workspace) that cannot be had -> B2S_E_NOMEM,

@@ -682,6 +682,7 @@ int64_t orc_xerial_compress2(const uint8_t* src, uint64_t n, uint32_t block_size
   return xerial_compress_impl(src, n, block_size, dst, cap, compressor);
 }
 static int64_t xerial_walk(const uint8_t* src, uint64_t n, uint8_t* dst, uint64_t cap) {
+  if (n == 0) return 0; /* SnappyInputStream.readHeader: no bytes at all is an empty stream */
   if (n < 16 || memcmp(src, XERIAL_HEADER, 8)) return -1;
   uint64_t ip = 16, op = 0;
   while (ip < n) {

@@ -3293,6 +3293,7 @@ static int decode_task(Device* D, Slot& S, uint32_t codec, uint32_t alg, uint32_
   for (uint32_t i = 0; i < T.n_src; i++) {
     const bool c = T.cached(i);
     const uint64_t len = c ? (*T.mix)[i].len : J.h.dst_len[T.block(i)];
+    if (!c && T.status(i) == B2S_E_CORRUPT) T.fail_source(i, ": the compressed stream is corrupt");
     if (T.status(i) == B2S_OK && !spec.rows() && len % spec.record_bytes)
       T.fail_source(i, std::string(c ? " holds " : " decodes to ") + std::to_string(len) +
                            " bytes, not a multiple of record_bytes " + std::to_string(spec.record_bytes));
@@ -3342,7 +3343,8 @@ static int decode_task(Device* D, Slot& S, uint32_t codec, uint32_t alg, uint32_
     if ((rc = decompress_enqueue_b(S, J, d_src, (uint8_t*)S.dst.p, S.dst.cap, launches))) return rc;
     CU(cudaEventSynchronize(S.ev_b));
     CU(cudaGetLastError());
-    for (uint32_t i = 0; i < n; i++) T.failed |= J.h.status[i] != B2S_OK;
+    for (uint32_t i = 0; i < T.n_src; i++)
+      if (!T.cached(i) && T.status(i) != B2S_OK) T.fail_source(i, ": the compressed stream is corrupt");
   } else if (!T.mix && !src_contiguous) {
     for (uint32_t i = 0; i < n; i++)
       if (src_len[i])
@@ -3749,7 +3751,7 @@ static int read_task_run(Device* D, bool packed, uint32_t codec, uint32_t alg, u
   DecodedTask T(mix, n, status, bad_slice);
   rc = decode_task(D, S, codec, alg, n, packed ? (const uint8_t*)S.src.p : src_base, packed ? dev_off.data() : src_off,
                    src_len, packed, slice_base, slice_len, slice_checksum, srcb, spec, dst_cap, T, &launches);
-  *dst_total = T.total;
+  *dst_total = T.failed ? 0 : T.total;  // a failed source: nothing is written
   *n_records = 0;
   if (!rc && !T.failed) rc = run_reduce_task(S, spec, T, &out, dst_cap, dst_total, n_records, n_groups, &launches);
   if (rc) return rc;

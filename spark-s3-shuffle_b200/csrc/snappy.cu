@@ -238,8 +238,10 @@ __global__ void xerial_walk_kernel(const uint8_t* __restrict__ src_base, const u
   uint32_t max_olen = 0, max_clen = 0;
   bool bad = false, too_small = false;
   if (FILL) too_small = (dst_off[i] + olen_total[i] > dst_cap);
-  // stream header: magic 82 53 4E 41 50 50 59 00, then version / compatible version (not checked beyond presence)
-  if (len < 16 || ld_be32(p) != 0x82534E41u || ld_be32(p + 4) != 0x50505900u) bad = true;
+  // stream header: magic 82 53 4E 41 50 50 59 00, then version / compatible version (not checked beyond presence).
+  // No bytes at all is an empty stream, as SnappyInputStream.readHeader takes it (a partition the map side wrote
+  // nothing for, fetched alone).
+  if (len && (len < 16 || ld_be32(p) != 0x82534E41u || ld_be32(p + 4) != 0x50505900u)) bad = true;
   ip = 16;
   while (!bad && ip < len) {
     if (len - ip < 4) {
