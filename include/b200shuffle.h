@@ -825,6 +825,79 @@ int b2s_decompress_window_aggregate_rows_keys_dev(
     uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records, uint64_t* n_out_records, int32_t* status,
     int32_t* bad_slice);
 
+/* ---- read side, window offsets: Spark's WindowExec with offset functions on a reducer's shuffled UnsafeRows ----
+ * b2s_decompress_window_aggregate_rows_keys_*, where fn[j] may also be an offset function, with two more per-function
+ * arrays: fn_flags[j] and fn_default[j].  Everything not stated here is that call's, and one fn array mixes ranking,
+ * aggregate and offset functions as one WindowExec does.  The semantics are Spark 3.5's FrameLessOffsetWindowFunctionFrame
+ * (Lag, Lead), First, Last and NthValue.  With N the partition's size, i the record's 0-based position in it and e its
+ * frame's last position (N - 1 for FRAME_PARTITION, i for FRAME_ROWS_RUNNING, ge - 1 for FRAME_RANGE_RUNNING):
+ *   fn          fn_arg          fn_frame        value
+ *   LEAD        offset k >= 1   0 (its own)     the input at position i + k if that is inside the partition, else the
+ *                                               default.  IGNORE_NULLS: the k-th non-null input after i in the partition,
+ *                                               else the default
+ *   LAG         offset k >= 1   0               the same backwards: i - k, or the k-th non-null input before i
+ *   FIRST       0               one of the      the input at position 0.  IGNORE_NULLS: the first non-null input in
+ *                               three frames    [0, e], or null
+ *   LAST        0               the three       the input at e.  IGNORE_NULLS: the last non-null input in [0, e], or null
+ *   NTH_VALUE   n >= 1          the three       the input at n - 1 if n - 1 <= e, else null.  IGNORE_NULLS: the n-th
+ *                                               non-null input in [0, e], or null
+ * A null input at the chosen position gives null, not the default.  The default is null unless fn_flags[j] has
+ * B2S_WINDOW_HAS_DEFAULT; then fn_default[j] holds the literal's slot bits as UnsafeRowWriter writes the input type
+ * (the slot zeroed, then the type's width).  HAS_DEFAULT is allowed only for LAG and LEAD of a fixed-width type (not
+ * VAL_BYTES, not a decimal above p 18).  B2S_WINDOW_IGNORE_NULLS is Spark's ignoreNulls.  LAG and LEAD need an ORDER BY
+ * column, as Spark's analyzer requires; FIRST, LAST and NTH_VALUE with every frame FRAME_PARTITION may have none, as
+ * aggregates may.  The result type is the input's type.
+ * Input.  val_type[j] / val_off[j] / val_null_field[j] as for an aggregate: every B2S_WINDOW_VAL_INT8 .. _FLOAT64 (the
+ * planner maps boolean to INT8, date to INT32 and timestamp to INT64), decimals of every precision 1..38, or
+ * B2S_WINDOW_VAL_BYTES: a B2S_FIELD_VAR field (string or binary) whose slot is (offset << 32) | size.  VAL_NONE is not an
+ * offset function's type, and an aggregate function does not take VAL_BYTES.
+ * Output row.  The input row joined with the value row, as in the aggregate call.  A null value sets bit nC + j.  A
+ * fixed-width value is written as UnsafeRowWriter writes it (the slot zeroed, then the type's width; floats keep their
+ * exact bits).  Every var-valued function has a region after the input's var bytes, the regions in function order: a
+ * wide decimal value (an offset function's or an aggregate's result) 16 bytes, BigInteger.toByteArray's minimal bytes
+ * re-encoded from the value and zero-padded, its slot (offset << 32) | len, a null one 16 zero bytes and slot
+ * offset << 32; a VAL_BYTES value its bytes zero-padded to a multiple of 8 as UnsafeRowWriter pads them, its slot
+ * (offset << 32) | size, a null one no bytes and a zero slot.  Without offset functions this is the aggregate call's row.
+ * Errors -> B2S_E_ARG: everything the aggregate call rejects (an offset function and VAL_BYTES aside); NULL fn_flags or
+ * fn_default; an offset or n below 1; a non-zero fn_arg for FIRST and LAST; a frame an offset function does not take;
+ * VAL_NONE for an offset function or VAL_BYTES for any other; an unknown flag bit, or flags on a function that is not an
+ * offset function; HAS_DEFAULT where it is not allowed; a non-zero fn_default without it; default bits above the
+ * type's width; VAL_BYTES on a field whose kind is not VAR.  These are checked before the device.  Per block,
+ * B2S_E_CORRUPT for the aggregate call's rules and when a non-null VAL_BYTES input's bytes lie outside its row's var
+ * region [8 (bC + nC), size) or a non-null DECIMAL_WIDE input of an offset function is bad as the aggregate call defines
+ * it; every non-null input of an offset function is checked, whether or not an output row takes it, so the verdict does
+ * not depend on the offsets; b2s_last_error() names the block and the record's offset, and nothing is written.  A
+ * partition of more than 2^31 - 1 records or an output row longer than 2^31 - 1 bytes -> B2S_E_UNSUPPORTED.
+ * B2S_E_DST_TOO_SMALL (with the exact size), B2S_E_NOMEM, the read lane, the buffer trim and b2s_last_timing
+ * (dominant_ms the window step) as in the aggregate call. */
+#define B2S_WINDOW_LAG 11
+#define B2S_WINDOW_LEAD 12
+#define B2S_WINDOW_FIRST 13
+#define B2S_WINDOW_LAST 14
+#define B2S_WINDOW_NTH_VALUE 15
+#define B2S_WINDOW_VAL_BYTES 8
+#define B2S_WINDOW_IGNORE_NULLS 1
+#define B2S_WINDOW_HAS_DEFAULT 2
+int b2s_decompress_window_offset_rows_keys_packed(
+    uint32_t codec, uint32_t checksum_alg, uint32_t n, const uint8_t* src_base, const uint64_t* src_off,
+    const uint64_t* src_len, const uint32_t* slice_base, const uint64_t* slice_len, const uint64_t* slice_checksum,
+    uint32_t n_partition_keys, uint32_t n_keys, const uint32_t* key_type, const uint32_t* key_off,
+    const uint32_t* key_len, const int32_t* key_null_field, uint32_t n_fields, const uint8_t* field_kind,
+    uint32_t n_fns, const uint32_t* fn, const int32_t* fn_arg, const uint32_t* fn_frame, const uint32_t* val_type,
+    const uint32_t* val_off, const int32_t* val_null_field, const uint32_t* fn_flags, const uint64_t* fn_default,
+    uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records, uint64_t* n_out_records,
+    int32_t* status, int32_t* bad_slice);
+/* same, with src_base / dst_base in device memory of dev_index; every array stays a host array */
+int b2s_decompress_window_offset_rows_keys_dev(
+    uint32_t dev_index, uint32_t codec, uint32_t checksum_alg, uint32_t n, const uint8_t* src_base,
+    const uint64_t* src_off, const uint64_t* src_len, const uint32_t* slice_base, const uint64_t* slice_len,
+    const uint64_t* slice_checksum, uint32_t n_partition_keys, uint32_t n_keys, const uint32_t* key_type,
+    const uint32_t* key_off, const uint32_t* key_len, const int32_t* key_null_field, uint32_t n_fields,
+    const uint8_t* field_kind, uint32_t n_fns, const uint32_t* fn, const int32_t* fn_arg, const uint32_t* fn_frame,
+    const uint32_t* val_type, const uint32_t* val_off, const int32_t* val_null_field, const uint32_t* fn_flags,
+    const uint64_t* fn_default, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records,
+    uint64_t* n_out_records, int32_t* status, int32_t* bad_slice);
+
 /* ---- exchange cache: map outputs kept resident in HBM for reducers on the same device ----
  * (docs/f4_gpu_resident_exchange.md steps 2 and 3, local half.)  The serialized writer's partition step already leaves
  * a map task's records partitioned by reduce id in HBM; the cached store keeps that arena, keyed by (shuffle_id,

@@ -889,6 +889,67 @@ JNIEXPORT jint JNICALL J(decompressWindowAggregateRowsKeysPacked)(JNIEnv* e, jcl
   return rc;
 }
 
+/* ---- read side, window offsets (INTEGRATION.md §3o): decompressWindowAggregateRowsKeysPacked where fn may also hold
+ *      offset functions (B2S_WINDOW_LAG .. NTH_VALUE, fnArg their offset or n, valType B2S_WINDOW_VAL_BYTES too);
+ *      fnFlags: int[nFns] (B2S_WINDOW_IGNORE_NULLS | B2S_WINDOW_HAS_DEFAULT, 0 for every other function), fnDefault:
+ *      long[nFns] (the default's slot bits).  Every array goes through a native copy. ---- */
+JNIEXPORT jint JNICALL J(decompressWindowOffsetRowsKeysPacked)(JNIEnv* e, jclass c, jint codec, jint alg, jint n,
+                                                               jlong src, jlongArray off, jlongArray len,
+                                                               jintArray sliceBase, jlongArray sliceLen,
+                                                               jlongArray sliceChecksum, jint nPartitionKeys,
+                                                               jint nKeys, jintArray keyType, jintArray keyOff,
+                                                               jintArray keyLen, jintArray keyNullField,
+                                                               jint nFields, jbyteArray fieldKind, jint nFns,
+                                                               jintArray fn, jintArray fnArg, jintArray fnFrame,
+                                                               jintArray valType, jintArray valOff,
+                                                               jintArray valNullField, jintArray fnFlags,
+                                                               jlongArray fnDefault, jlong dst, jlong dstCap,
+                                                               jlongArray meta, jintArray status,
+                                                               jintArray badSlice) {
+  (void)c;
+  if (n < 0 || !meta || (*e)->GetArrayLength(e, meta) < 3) return B2S_E_ARG;
+  if (n > 0 && (!status || (*e)->GetArrayLength(e, status) < n || (badSlice && (*e)->GetArrayLength(e, badSlice) < n)))
+    return B2S_E_ARG;
+  const int with_slices = alg != 0 && n > 0;
+  int rc = 0;
+  uint64_t* o = region(e, off, n, 8, &rc);
+  uint64_t* l = region(e, len, n, 8, &rc);
+  uint32_t* sb = with_slices ? region(e, sliceBase, n + 1, 4, &rc) : 0;
+  const jsize ns = sb && !rc ? (jsize)sb[n] : 0;
+  uint64_t* sl = with_slices ? region(e, sliceLen, ns, 8, &rc) : 0;
+  uint64_t* sc = with_slices ? region(e, sliceChecksum, ns, 8, &rc) : 0;
+  uint32_t* kt = region(e, keyType, nKeys, 4, &rc);
+  uint32_t* ko = region(e, keyOff, nKeys, 4, &rc);
+  uint32_t* kl = region(e, keyLen, nKeys, 4, &rc);
+  int32_t* kn = region(e, keyNullField, nKeys, 4, &rc);
+  uint8_t* fk = region(e, fieldKind, nFields, 1, &rc);
+  uint32_t* fs = region(e, fn, nFns, 4, &rc);
+  int32_t* fa = region(e, fnArg, nFns, 4, &rc);
+  uint32_t* fr = region(e, fnFrame, nFns, 4, &rc);
+  uint32_t* vt = region(e, valType, nFns, 4, &rc);
+  uint32_t* vo = region(e, valOff, nFns, 4, &rc);
+  int32_t* vn = region(e, valNullField, nFns, 4, &rc);
+  uint32_t* ff = region(e, fnFlags, nFns, 4, &rc);
+  uint64_t* fd = region(e, fnDefault, nFns, 8, &rc);
+  int32_t* st = (int32_t*)malloc((size_t)n * 2 * sizeof(int32_t) + 1);
+  if (!rc && !st) rc = B2S_E_NOMEM;
+  uint64_t m[3] = {0, 0, 0};
+  if (!rc) {
+    rc = b2s_decompress_window_offset_rows_keys_packed(
+        (uint32_t)codec, (uint32_t)alg, (uint32_t)n, PTR(const uint8_t, src), o, l, sb, sl, sc,
+        (uint32_t)nPartitionKeys, (uint32_t)nKeys, kt, ko, kl, kn, (uint32_t)nFields, fk, (uint32_t)nFns, fs, fa, fr,
+        vt, vo, vn, ff, fd, PTR(uint8_t, dst), (uint64_t)dstCap, &m[0], &m[1], &m[2], st, st + n);
+    (*e)->SetLongArrayRegion(e, meta, 0, 3, (const jlong*)m);
+    if (n > 0) {
+      (*e)->SetIntArrayRegion(e, status, 0, n, (const jint*)st);
+      if (badSlice) (*e)->SetIntArrayRegion(e, badSlice, 0, n, (const jint*)(st + n));
+    }
+  }
+  void* owned[] = {o, l, sb, sl, sc, kt, ko, kl, kn, fk, fs, fa, fr, vt, vo, vn, ff, fd, st};
+  for (size_t i = 0; i < sizeof owned / sizeof owned[0]; i++) free(owned[i]);
+  return rc;
+}
+
 /* decompressSortRowsKeysPacked / decompressAggregateRowsKeysPacked over sources of which those with cached[i] != 0
  * are the cached range of mapIds[i] (INTEGRATION.md §3m; mapIds: long[n], cached: int[n]) */
 JNIEXPORT jint JNICALL J(exchangeReadSortRowsKeysPacked)(JNIEnv* e, jclass c, jint shuffleId, jint startReduce,

@@ -37,6 +37,13 @@ WINDOW_FRAME_PARTITION, WINDOW_FRAME_ROWS_RUNNING, WINDOW_FRAME_RANGE_RUNNING = 
  WINDOW_VAL_FLOAT64, WINDOW_VAL_DECIMAL) = range(8)
 
 
+# offset functions of the offset window (decompress_window_offset_rows_keys_*), its string / binary input type, and the
+# per-function flags
+WINDOW_LAG, WINDOW_LEAD, WINDOW_FIRST, WINDOW_LAST, WINDOW_NTH_VALUE = range(11, 16)
+WINDOW_VAL_BYTES = 8
+WINDOW_IGNORE_NULLS, WINDOW_HAS_DEFAULT = 1, 2
+
+
 def window_val_decimal(p, s):
     return WINDOW_VAL_DECIMAL | p << 8 | s << 16
 OK, E_CORRUPT, E_CHECKSUM, E_DST_TOO_SMALL, E_UNSUPPORTED, E_ARG, E_CUDA, E_NOT_INIT, E_NOMEM, E_NOT_CACHED = (
@@ -163,6 +170,13 @@ PROTOTYPES = [
     ("b2s_decompress_window_aggregate_rows_keys_dev", C.c_int,
      [_u32, _u32, _u32, _u32, _vp, _u64p, _u64p, _u32p, _u64p, _u64p, _u32, _u32, _u32p, _u32p, _u32p, _i32p, _u32,
       _u8p, _u32, _u32p, _i32p, _u32p, _u32p, _u32p, _i32p, _vp, _u64, _u64p, _u64p, _u64p, _i32p, _i32p]),
+    ("b2s_decompress_window_offset_rows_keys_packed", C.c_int,
+     [_u32, _u32, _u32, _u8p, _u64p, _u64p, _u32p, _u64p, _u64p, _u32, _u32, _u32p, _u32p, _u32p, _i32p, _u32, _u8p,
+      _u32, _u32p, _i32p, _u32p, _u32p, _u32p, _i32p, _u32p, _u64p, _u8p, _u64, _u64p, _u64p, _u64p, _i32p, _i32p]),
+    ("b2s_decompress_window_offset_rows_keys_dev", C.c_int,
+     [_u32, _u32, _u32, _u32, _vp, _u64p, _u64p, _u32p, _u64p, _u64p, _u32, _u32, _u32p, _u32p, _u32p, _i32p, _u32,
+      _u8p, _u32, _u32p, _i32p, _u32p, _u32p, _u32p, _i32p, _u32p, _u64p, _vp, _u64, _u64p, _u64p, _u64p, _i32p,
+      _i32p]),
     ("b2s_exchange_set_budget", C.c_int, [_u32, _u64]),
     ("b2s_partition_compress_cached_packed", C.c_int,
      [_i32, C.c_int64, _u32, _i32, _u32, _u32, _u32, _u64, _u8p, _u64, _u32p, _u32p, _u8p, _u64, _u64p, _u64p, _u64p,
@@ -613,23 +627,51 @@ def _window_arrays(keys, n_partition_keys, n_fields, kinds, fns, limit):
     return n_partition_keys, n, kt, ko, kl, kn, n_fields, kinds, len(fns), fn, arg, limit_fn, lim
 
 
-def _window_aggregate_arrays(keys, n_partition_keys, n_fields, kinds, fns):
-    """the aggregate window's key, field-kind and function arguments: fns = [ranking fn, (WINDOW_NTILE, k), or an
-    aggregate (fn, frame, val_type, val_off, val_null_field)]"""
-    n, kt, ko, kl, kn = _key_arrays(keys)
+def _window_fn_rows(fns):
+    """fns -> [(fn, arg, frame, val_type, val_off, val_null_field, flags, default)]: a ranking fn or (WINDOW_NTILE, k),
+    an aggregate (fn, frame, val_type, val_off, val_null_field), or an offset function in the full form"""
     full = []
     for f in fns:
-        if isinstance(f, tuple) and len(f) == 5:
-            full.append((f[0], 0) + tuple(f[1:]))
+        if isinstance(f, tuple) and len(f) == 8:
+            full.append(tuple(f))
+        elif isinstance(f, tuple) and len(f) == 5:
+            full.append((f[0], 0) + tuple(f[1:]) + (0, 0))
         else:
             fn, arg = f if isinstance(f, tuple) else (f, 0)
-            full.append((fn, arg, 0, WINDOW_VAL_NONE, 0, -1))
-    cols = list(zip(*full)) if full else [[0]] * 6
-    fn, arg, frame, vt, vo = (np.array(c, dtype=t) for c, t in zip(cols[:5], (np.uint32, np.int32, np.uint32,
-                                                                             np.uint32, np.uint32)))
-    vn = np.array(cols[5], dtype=np.int32)
+            full.append((fn, arg, 0, WINDOW_VAL_NONE, 0, -1, 0, 0))
+    return full
+
+
+def _window_aggregate_arrays(keys, n_partition_keys, n_fields, kinds, fns, offset=False):
+    """the aggregate window's key, field-kind and function arguments: fns = [ranking fn, (WINDOW_NTILE, k), or an
+    aggregate (fn, frame, val_type, val_off, val_null_field)]; offset: the offset window's, whose fns may also be
+    offset functions (fn, arg, frame, val_type, val_off, val_null_field, flags, default), with the flags and defaults"""
+    n, kt, ko, kl, kn = _key_arrays(keys)
+    full = _window_fn_rows(fns)
+    cols = list(zip(*full)) if full else [[0]] * 8
+    fn, arg, frame, vt, vo, vn, fl, dv = (np.array(c, dtype=t) for c, t in zip(cols, (
+        np.uint32, np.int32, np.uint32, np.uint32, np.uint32, np.int32, np.uint32, np.uint64)))
     kinds = None if kinds is None else np.ascontiguousarray(kinds, dtype=np.uint8)
-    return n_partition_keys, n, kt, ko, kl, kn, n_fields, kinds, len(full), fn, arg, frame, vt, vo, vn
+    a = (n_partition_keys, n, kt, ko, kl, kn, n_fields, kinds, len(full), fn, arg, frame, vt, vo, vn)
+    return a + (fl, dv) if offset else a
+
+
+def _window_offset_arrays(keys, n_partition_keys, n_fields, kinds, fns):
+    return _window_aggregate_arrays(keys, n_partition_keys, n_fields, kinds, fns, offset=True)
+
+
+def decompress_window_offset_rows_keys_packed(codec, src, off, length, dst, keys, n_partition_keys, n_fields, kinds,
+                                              fns, checksum_alg=CHECKSUM_NONE, slice_base=None, slice_len=None,
+                                              slice_checksum=None):
+    """Spark's WindowExec with offset (and ranking and aggregate) functions over a reducer's UnsafeRow records: as
+    decompress_window_aggregate_rows_keys_packed, fns also taking offset functions (WINDOW_LAG / LEAD / FIRST / LAST /
+    NTH_VALUE, its offset or n (0 for FIRST and LAST), its frame (0 for LAG and LEAD), WINDOW_VAL_* (WINDOW_VAL_BYTES for
+    a string or binary), window_val_decimal(p, s), the input's slot offset, its null bit or -1, WINDOW_IGNORE_NULLS |
+    WINDOW_HAS_DEFAULT, the default's slot bits).  A string value's bytes follow the input's var bytes, padded to 8.
+    -> dict(total, n_records, n_out_records, status, bad_slice)"""
+    return _sort_call("b2s_decompress_window_offset_rows_keys_packed", codec, src, off, length, dst, None,
+                      _window_offset_arrays(keys, n_partition_keys, n_fields, kinds, fns), checksum_alg,
+                      (slice_base, slice_len, slice_checksum))
 
 
 def decompress_window_aggregate_rows_keys_packed(codec, src, off, length, dst, keys, n_partition_keys, n_fields,
@@ -782,6 +824,15 @@ def decompress_window_rows_keys_dev(codec, d_src, off, length, d_dst, dst_cap, k
     return _sort_call("b2s_decompress_window_rows_keys_dev", codec, d_src, off, length, d_dst, dst_cap,
                       _window_arrays(keys, n_partition_keys, n_fields, kinds, fns, limit), checksum_alg,
                       (slice_base, slice_len, slice_checksum), dev)
+
+
+def decompress_window_offset_rows_keys_dev(codec, d_src, off, length, d_dst, dst_cap, keys, n_partition_keys, n_fields,
+                                           kinds, fns, checksum_alg=CHECKSUM_NONE, slice_base=None, slice_len=None,
+                                           slice_checksum=None, dev=0):
+    """decompress_window_offset_rows_keys_packed on device-resident blocks (d_src) into a device arena (d_dst)"""
+    return _sort_call("b2s_decompress_window_offset_rows_keys_dev", codec, d_src, off, length, d_dst, dst_cap,
+                      _window_offset_arrays(keys, n_partition_keys, n_fields, kinds, fns), checksum_alg,
+                      (slice_base, slice_len, slice_checksum), dev=dev)
 
 
 def decompress_window_aggregate_rows_keys_dev(codec, d_src, off, length, d_dst, dst_cap, keys, n_partition_keys,

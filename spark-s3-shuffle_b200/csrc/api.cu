@@ -2553,7 +2553,8 @@ struct JoinSpec {
 };
 // A window's other arguments (b2s_decompress_window_rows_keys_*): how many key columns partition, the input's fields
 // and kinds, the functions and their arguments, the limit, and the input record count it returns.  The aggregate call
-// (b2s_decompress_window_aggregate_rows_keys_*, agg) adds each function's frame and input column, and has no limit.
+// (b2s_decompress_window_aggregate_rows_keys_*, agg) adds each function's frame and input column, and has no limit; the
+// offset call (b2s_decompress_window_offset_rows_keys_*, agg and offset) adds each function's flags and default.
 struct WindowSpec {
   uint32_t n_partition_keys = 0;
   uint32_t n_fields = 0;
@@ -2569,6 +2570,9 @@ struct WindowSpec {
   const uint32_t* val_type = nullptr;
   const uint32_t* val_off = nullptr;
   const int32_t* val_null = nullptr;
+  bool offset = false;
+  const uint32_t* flags = nullptr;
+  const uint64_t* dflt = nullptr;
 };
 static RecordSpec fixed_spec(uint32_t record_bytes, uint32_t key_off, uint32_t key_len) {
   RecordSpec r;
@@ -2800,7 +2804,8 @@ static int window_args(const RecordSpec& spec) {
 }
 
 // The aggregate window call's checks of its functions, before the device: the input's fields and kinds, and per
-// function its argument, frame, input type, slot and null bit (b2s_decompress_window_aggregate_rows_keys_*)
+// function its argument, frame, input type, slot and null bit (b2s_decompress_window_aggregate_rows_keys_*).  With
+// ws.offset (the offset call) the offset functions and VAL_BYTES are accepted too.
 static int window_agg_fn_args(const WindowSpec& ws) {
   const uint32_t nf = ws.n_fields;
   if (nf < 1 || nf > 65536) return fail(B2S_E_ARG, "n_fields must be in [1, 65536]%s");
@@ -2813,14 +2818,25 @@ static int window_agg_fn_args(const WindowSpec& ws) {
   const uint64_t lo = 8ull * bitset_words(nf);
   for (uint32_t j = 0; j < ws.n_fns; j++) {
     const uint32_t fn = ws.fn[j], frame = ws.frame[j], vt = ws.val_type[j], kind = vt & 0xff;
-    if (fn > B2S_WINDOW_AVG) return fail(B2S_E_ARG, "unknown window function%s");
-    if (fn == B2S_WINDOW_NTILE ? ws.fn_arg[j] < 1 : ws.fn_arg[j] != 0)
-      return fail(B2S_E_ARG, "fn_arg must be NTILE's bucket count (at least 1), and 0 for every other function%s");
+    if (fn > (ws.offset ? B2S_WINDOW_NTH_VALUE : B2S_WINDOW_AVG)) return fail(B2S_E_ARG, "unknown window function%s");
+    const bool offset = fn >= B2S_WINDOW_LAG, lag_lead = fn == B2S_WINDOW_LAG || fn == B2S_WINDOW_LEAD;
+    const bool counted = fn == B2S_WINDOW_NTILE || lag_lead || fn == B2S_WINDOW_NTH_VALUE;
+    if (counted ? ws.fn_arg[j] < 1 : ws.fn_arg[j] != 0)
+      return fail(B2S_E_ARG, ws.offset ? "fn_arg must be NTILE's bucket count, LAG / LEAD's offset or NTH_VALUE's n "
+                                         "(at least 1), and 0 for every other function%s"
+                                       : "fn_arg must be NTILE's bucket count (at least 1), and 0 for every other "
+                                         "function%s");
     const bool ranking = fn <= B2S_WINDOW_NTILE;
-    if (ranking ? frame != 0 : frame < B2S_WINDOW_FRAME_PARTITION || frame > B2S_WINDOW_FRAME_RANGE_RUNNING)
-      return fail(B2S_E_ARG, "fn_frame must be 0 for a ranking function and a B2S_WINDOW_FRAME_* for an aggregate%s");
-    if (kind > B2S_WINDOW_VAL_DECIMAL || (kind != B2S_WINDOW_VAL_DECIMAL && (vt >> 8)) || (vt >> 24))
+    if (ranking || lag_lead ? frame != 0 : frame < B2S_WINDOW_FRAME_PARTITION || frame > B2S_WINDOW_FRAME_RANGE_RUNNING)
+      return fail(B2S_E_ARG, ws.offset ? "fn_frame must be 0 for a ranking function, LAG and LEAD, and a "
+                                         "B2S_WINDOW_FRAME_* for an aggregate, FIRST, LAST and NTH_VALUE%s"
+                                       : "fn_frame must be 0 for a ranking function and a B2S_WINDOW_FRAME_* for an "
+                                         "aggregate%s");
+    const uint32_t max_kind = ws.offset ? B2S_WINDOW_VAL_BYTES : B2S_WINDOW_VAL_DECIMAL;
+    if (kind > max_kind || (kind != B2S_WINDOW_VAL_DECIMAL && (vt >> 8)) || (vt >> 24))
       return fail(B2S_E_ARG, "unknown val_type%s");
+    if (kind == B2S_WINDOW_VAL_BYTES && !offset)
+      return fail(B2S_E_ARG, "only an offset function takes B2S_WINDOW_VAL_BYTES%s");
     if (kind == B2S_WINDOW_VAL_NONE) {
       if (fn != B2S_WINDOW_COUNT && !ranking) return fail(B2S_E_ARG, "only COUNT takes B2S_WINDOW_VAL_NONE%s");
       continue;
@@ -2828,18 +2844,48 @@ static int window_agg_fn_args(const WindowSpec& ws) {
     if (ranking) return fail(B2S_E_ARG, "a ranking function takes B2S_WINDOW_VAL_NONE%s");
     const uint32_t p = (vt >> 8) & 0xff, sc = vt >> 16;
     if (kind == B2S_WINDOW_VAL_DECIMAL) {
-      const uint32_t max_p = fn == B2S_WINDOW_SUM ? 28 : fn == B2S_WINDOW_AVG ? 24 : 38;
+      const uint32_t max_p = fn == B2S_WINDOW_SUM ? 28 : fn == B2S_WINDOW_AVG ? 24 : 38;  // offset functions: 38
       if (p < 1 || p > max_p || sc > p)
         return fail(B2S_E_ARG, "a decimal input needs 1 <= p <= 38 (SUM 28, AVG 24) and s <= p%s");
     }
     const uint32_t off = ws.val_off[j];
     if (off < lo || (off - lo) % 8 || (off - lo) / 8 >= nf)
       return fail(B2S_E_ARG, "val_off is not one of the input's field slots%s");
-    const uint8_t want = kind == B2S_WINDOW_VAL_DECIMAL && p > 18 ? B2S_FIELD_DECIMAL_WIDE : B2S_FIELD_FIXED;
+    const uint8_t want = kind == B2S_WINDOW_VAL_BYTES                   ? B2S_FIELD_VAR
+                         : kind == B2S_WINDOW_VAL_DECIMAL && p > 18 ? B2S_FIELD_DECIMAL_WIDE
+                                                                    : B2S_FIELD_FIXED;
     if (ws.kind[(off - lo) / 8] != want)
-      return fail(B2S_E_ARG, "a value field's kind must be DECIMAL_WIDE for a decimal above p 18, else FIXED%s");
+      return fail(B2S_E_ARG, ws.offset ? "a value field's kind must be VAR for VAL_BYTES, DECIMAL_WIDE for a decimal "
+                                         "above p 18, else FIXED%s"
+                                       : "a value field's kind must be DECIMAL_WIDE for a decimal above p 18, else "
+                                         "FIXED%s");
     if (ws.val_null[j] < -1 || ws.val_null[j] >= (int64_t)nf)
       return fail(B2S_E_ARG, "val_null_field must be -1 or a field ordinal below n_fields%s");
+  }
+  return 0;
+}
+
+// The offset window call's checks of its functions, before the device (b2s_decompress_window_offset_rows_keys_*): the
+// aggregate call's, with offset functions and VAL_BYTES, then each function's flags and default
+static int window_offset_fn_args(const WindowSpec& ws) {
+  if (int rc = window_agg_fn_args(ws)) return rc;
+  if (!ws.flags || !ws.dflt) return fail(B2S_E_ARG, "null argument%s");
+  for (uint32_t j = 0; j < ws.n_fns; j++) {
+    const uint32_t fn = ws.fn[j], fl = ws.flags[j], kind = ws.val_type[j] & 0xff, p = (ws.val_type[j] >> 8) & 0xff;
+    if (fl & ~(uint32_t)(B2S_WINDOW_IGNORE_NULLS | B2S_WINDOW_HAS_DEFAULT) || (fl && fn < B2S_WINDOW_LAG))
+      return fail(B2S_E_ARG, "fn_flags takes B2S_WINDOW_IGNORE_NULLS and B2S_WINDOW_HAS_DEFAULT, on offset functions "
+                             "only%s");
+    if (!(fl & B2S_WINDOW_HAS_DEFAULT)) {
+      if (ws.dflt[j]) return fail(B2S_E_ARG, "a non-zero fn_default needs B2S_WINDOW_HAS_DEFAULT%s");
+      continue;
+    }
+    if ((fn != B2S_WINDOW_LAG && fn != B2S_WINDOW_LEAD) || kind == B2S_WINDOW_VAL_BYTES ||
+        (kind == B2S_WINDOW_VAL_DECIMAL && p > 18))
+      return fail(B2S_E_ARG, "B2S_WINDOW_HAS_DEFAULT is for LAG and LEAD of a fixed-width type%s");
+    const uint32_t width = kind == B2S_WINDOW_VAL_INT8 ? 1 : kind == B2S_WINDOW_VAL_INT16 ? 2
+                           : kind == B2S_WINDOW_VAL_INT32 || kind == B2S_WINDOW_VAL_FLOAT32 ? 4 : 8;
+    if (width < 8 && ws.dflt[j] >> (8 * width))
+      return fail(B2S_E_ARG, "fn_default has bits above its type's width%s");
   }
   return 0;
 }
@@ -3379,12 +3425,21 @@ static void window_shape(const RecordSpec& spec, WindowShape& shape) {
     shape.fn[j] = ws.fn[j];
     shape.arg[j] = (uint32_t)ws.fn_arg[j];
     shape.wide[j] = -1;
+    shape.nn[j] = -1;
     if (ws.fn[j] < B2S_WINDOW_SUM) continue;
     const uint32_t vt = ws.val_type[j], p = (vt >> 8) & 0xff;
     shape.frame[j] = ws.frame[j];
     shape.vtype[j] = vt;
     shape.voff[j] = ws.val_off[j];
     shape.vnull[j] = ws.val_null[j];
+    if (ws.fn[j] >= B2S_WINDOW_LAG) {  // an offset function: a non-null index when it skips nulls that can occur
+      shape.flags[j] = ws.flags[j];
+      shape.dflt[j] = ws.dflt[j];
+      if ((ws.flags[j] & B2S_WINDOW_IGNORE_NULLS) && ws.val_null[j] >= 0) shape.nn[j] = (int32_t)shape.n_nn++;
+      shape.n_off++;
+      if ((vt & 0xff) == B2S_WINDOW_VAL_DECIMAL && p > 18) shape.n_wide_off++;
+      continue;
+    }
     shape.agg[j] = shape.n_agg++;
     const uint32_t rp = p + (ws.fn[j] == B2S_WINDOW_SUM ? 10 : ws.fn[j] == B2S_WINDOW_AVG ? 4 : 0);
     if ((vt & 0xff) == B2S_WINDOW_VAL_DECIMAL && ws.fn[j] != B2S_WINDOW_COUNT && rp > 18)
@@ -3652,7 +3707,10 @@ static int window_rows_tail(Slot& S, const RecordSpec& spec, DecodedTask& T, con
     CU(cudaGetLastError());
   }
   if (wb[4] != ~0ull)
-    return T.fail_row_at(wb[4] >> 2, "a decimal input's size is not in [1, 16] or its bytes run past the end of its row");
+    return T.fail_row_at(wb[4] >> 2, (wb[4] & 3) == kWindowBadBytes
+                                         ? "a string input's bytes lie outside its row's variable-length region"
+                                         : "a decimal input's size is not in [1, 16] or its bytes run past the end of "
+                                           "its row");
   if (wb[3]) return fail(B2S_E_UNSUPPORTED, "a window partition holds more than 2^31 - 1 records%s");
   if (wb[2]) return fail(B2S_E_UNSUPPORTED, "an output row is longer than 2^31 - 1 bytes%s");
   *total = wb[1];
@@ -4088,8 +4146,8 @@ int b2s_decompress_join_rows_keys_dev(
 }
 
 // The window calls: the composite-key row sort's call with the window's arguments ws (its n_in the input count, zeroed
-// first); every count and *dst_total are 0 when a block failed (nothing is written).  The aggregate call checks its
-// functions before the device.
+// first); every count and *dst_total are 0 when a block failed (nothing is written).  The aggregate and offset calls
+// check their functions before the device.
 static int window_call(uint32_t dev_index, bool packed, uint32_t codec, uint32_t alg, uint32_t n,
                        const uint8_t* src_base, const uint64_t* src_off, const uint64_t* src_len,
                        const uint32_t* slice_base, const uint64_t* slice_len, const uint64_t* slice_checksum,
@@ -4100,7 +4158,7 @@ static int window_call(uint32_t dev_index, bool packed, uint32_t codec, uint32_t
   if (ws.agg) {
     if (dst_total) *dst_total = 0;
     if (n_out_records) *n_out_records = 0;
-    if (int rc = window_agg_fn_args(ws)) {
+    if (int rc = ws.offset ? window_offset_fn_args(ws) : window_agg_fn_args(ws)) {
       begin_call();  // a new call, with an empty b2s_last_timing
       return rc;
     }
@@ -4140,6 +4198,18 @@ static WindowSpec window_aggregate_spec(uint32_t n_partition_keys, uint32_t n_fi
   ws.val_type = val_type;
   ws.val_off = val_off;
   ws.val_null = val_null_field;
+  return ws;
+}
+
+static WindowSpec window_offset_spec(uint32_t n_partition_keys, uint32_t n_fields, const uint8_t* field_kind,
+                                     uint32_t n_fns, const uint32_t* fn, const int32_t* fn_arg, const uint32_t* fn_frame,
+                                     const uint32_t* val_type, const uint32_t* val_off, const int32_t* val_null_field,
+                                     const uint32_t* fn_flags, const uint64_t* fn_default, uint64_t* n_records) {
+  WindowSpec ws = window_aggregate_spec(n_partition_keys, n_fields, field_kind, n_fns, fn, fn_arg, fn_frame, val_type,
+                                        val_off, val_null_field, n_records);
+  ws.offset = true;
+  ws.flags = fn_flags;
+  ws.dflt = fn_default;
   return ws;
 }
 
@@ -4199,6 +4269,38 @@ int b2s_decompress_window_aggregate_rows_keys_dev(
     int32_t* bad_slice) {
   WindowSpec ws = window_aggregate_spec(n_partition_keys, n_fields, field_kind, n_fns, fn, fn_arg, fn_frame,
                                         val_type, val_off, val_null_field, n_records);
+  return window_call(dev_index, false, codec, checksum_alg, n, src_base, src_off, src_len, slice_base, slice_len,
+                     slice_checksum, n_keys, key_type, key_off, key_len, key_null_field, ws, dst_base, dst_cap,
+                     dst_total, n_out_records, status, bad_slice);
+}
+
+int b2s_decompress_window_offset_rows_keys_packed(
+    uint32_t codec, uint32_t checksum_alg, uint32_t n, const uint8_t* src_base, const uint64_t* src_off,
+    const uint64_t* src_len, const uint32_t* slice_base, const uint64_t* slice_len, const uint64_t* slice_checksum,
+    uint32_t n_partition_keys, uint32_t n_keys, const uint32_t* key_type, const uint32_t* key_off,
+    const uint32_t* key_len, const int32_t* key_null_field, uint32_t n_fields, const uint8_t* field_kind,
+    uint32_t n_fns, const uint32_t* fn, const int32_t* fn_arg, const uint32_t* fn_frame, const uint32_t* val_type,
+    const uint32_t* val_off, const int32_t* val_null_field, const uint32_t* fn_flags, const uint64_t* fn_default,
+    uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records, uint64_t* n_out_records,
+    int32_t* status, int32_t* bad_slice) {
+  WindowSpec ws = window_offset_spec(n_partition_keys, n_fields, field_kind, n_fns, fn, fn_arg, fn_frame, val_type,
+                                     val_off, val_null_field, fn_flags, fn_default, n_records);
+  return window_call(t_device, true, codec, checksum_alg, n, src_base, src_off, src_len, slice_base, slice_len,
+                     slice_checksum, n_keys, key_type, key_off, key_len, key_null_field, ws, dst_base, dst_cap,
+                     dst_total, n_out_records, status, bad_slice);
+}
+
+int b2s_decompress_window_offset_rows_keys_dev(
+    uint32_t dev_index, uint32_t codec, uint32_t checksum_alg, uint32_t n, const uint8_t* src_base,
+    const uint64_t* src_off, const uint64_t* src_len, const uint32_t* slice_base, const uint64_t* slice_len,
+    const uint64_t* slice_checksum, uint32_t n_partition_keys, uint32_t n_keys, const uint32_t* key_type,
+    const uint32_t* key_off, const uint32_t* key_len, const int32_t* key_null_field, uint32_t n_fields,
+    const uint8_t* field_kind, uint32_t n_fns, const uint32_t* fn, const int32_t* fn_arg, const uint32_t* fn_frame,
+    const uint32_t* val_type, const uint32_t* val_off, const int32_t* val_null_field, const uint32_t* fn_flags,
+    const uint64_t* fn_default, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records,
+    uint64_t* n_out_records, int32_t* status, int32_t* bad_slice) {
+  WindowSpec ws = window_offset_spec(n_partition_keys, n_fields, field_kind, n_fns, fn, fn_arg, fn_frame, val_type,
+                                     val_off, val_null_field, fn_flags, fn_default, n_records);
   return window_call(dev_index, false, codec, checksum_alg, n, src_base, src_off, src_len, slice_base, slice_len,
                      slice_checksum, n_keys, key_type, key_off, key_len, key_null_field, ws, dst_base, dst_cap,
                      dst_total, n_out_records, status, bad_slice);

@@ -529,7 +529,10 @@ void launch_join_emit(const uint8_t* arena, uint64_t n, const uint32_t* idx, uin
 // and the input's VAR and DECIMAL_WIDE fields (their slots' offsets move), as a device list.  An aggregate function f
 // (fn[f] >= B2S_WINDOW_SUM) has its frame, input type (B2S_WINDOW_VAL_*, a decimal's p and s above), slot and null bit
 // (-1: never null), its index agg[f] among the n_agg aggregate functions, and wide[f], its ordinal among the n_wide
-// functions with a DECIMAL_WIDE result (-1 for every other function).
+// functions with a DECIMAL_WIDE result (-1 for every other function).  An offset function (fn[f] >= B2S_WINDOW_LAG)
+// has the same input fields (B2S_WINDOW_VAL_BYTES too), its flags and default slot bits, and nn[f], its index among the
+// n_nn non-null indexes (IGNORE_NULLS over a nullable input; -1 for every other function); n_off offset functions, of
+// which n_wide_off take a DECIMAL_WIDE input (their values take 16 bytes each, as wide aggregate results do).
 constexpr uint32_t kMaxWindowFns = 16;
 struct WindowShape {
   uint32_t n, bw, out_bw;
@@ -548,16 +551,22 @@ struct WindowShape {
   uint32_t agg[kMaxWindowFns];
   int32_t wide[kMaxWindowFns];
   uint32_t n_agg, n_wide;
+  uint32_t flags[kMaxWindowFns];
+  uint64_t dflt[kMaxWindowFns];
+  int32_t nn[kMaxWindowFns];
+  uint32_t n_off, n_nn, n_wide_off;
 };
 // d_wws: window_ws_bytes(n, shape) bytes
 size_t window_ws_bytes(uint64_t n, const WindowShape& shape);
 // the readback: [output records, output bytes, an output row is too long (0 / 1), a partition is too large (0 / 1),
-// the first bad DECIMAL_WIDE input (its arena offset << 2 | kAggBadDecimal; ~0: none)]
+// the first bad DECIMAL_WIDE or string input (its arena offset << 2 | kAggBadDecimal or kWindowBadBytes; ~0: none)]
 uint64_t* window_readback(uint8_t* d_wws, uint64_t n, const WindowShape& shape);
 constexpr size_t kWindowReadbackBytes = 40;
+constexpr uint64_t kWindowBadBytes = 2;  // an offset function's string input lies outside its row's var region
 // Per sorted position: whether it starts a partition (only peer heads compare their partition columns with their
 // predecessor's, encoded 16 bytes at a time), scanned, and the partitions' starts compacted; with aggregate functions,
-// their inputs staged and folded from each partition's start; then every function's value, whether the limit keeps
+// their inputs staged and folded from each partition's start; with offset functions that skip nulls, a non-null index
+// each (present flags scanned, present positions compacted); then every function's value, whether the limit keeps
 // the record and its output bytes, the kept records and bytes scanned, the totals and the verdicts into the readback.
 // Uploads the shape and its field list (h_fields: shape.n_var fields).  idx: the sorted order (nullptr: arena order);
 // d_aws: launch_rows_group's workspace.

@@ -1,13 +1,17 @@
 // window.cu — Spark's WindowExec on a reducer for the ranking functions (row_number, rank, dense_rank, percent_rank,
-// cume_dist, ntile), with WindowGroupLimitExec's limit, and for the aggregate functions (sum, count, min, max, avg)
-// over whole-partition and running frames, and the output rows built as UnsafeRowJoiner joins the input row with the
-// row of values.  The records have been framed, keyed by the whole window key (partition columns, then
-// order columns), stably sorted by rows.cu and grouped by aggregate.cu's launch_rows_group, whose groups are the peer
-// groups.  All on the device:
+// cume_dist, ntile), with WindowGroupLimitExec's limit, for the aggregate functions (sum, count, min, max, avg) over
+// whole-partition and running frames, and for the offset functions (lag, lead, first, last, nth_value), and the output
+// rows built as UnsafeRowJoiner joins the input row with the row of values.  The records have been framed, keyed by the
+// whole window key (partition columns, then order columns), stably sorted by rows.cu and grouped by aggregate.cu's
+// launch_rows_group, whose groups are the peer groups.  All on the device:
 //   heads  : one thread per sorted position: a partition starts at a peer head whose partition columns differ from its
 //            predecessor's, compared by encode_key 16 encoded bytes at a time until they differ or both keys end (so
 //            the equality is the sort's: strings by length and bytes, -0.0 with 0.0, NaN with NaN, null with null);
 //            the flags scanned, and each partition's first position compacted
+//   nonnull: (offset functions with IGNORE_NULLS over a nullable input) per function a present flag per sorted position,
+//            exclusive-scanned to r(j) (the total at r(n)), and the present positions compacted into pres[]; a
+//            partition [ps, pe)'s present positions are then pres[r(ps) .. r(pe)), so every skip-nulls lookup is index
+//            arithmetic bounded by the partition or the frame
 //   stage  : (aggregate functions) one thread per sorted position: each aggregate's input, null flag and, for a
 //            DECIMAL_WIDE input, its 16 bytes checked, into dense sorted-order state arrays (lo, hi, count)
 //   fold   : each state becomes its fold over the partition's positions up to it.  Integer sums, counts, decimal sums
@@ -17,12 +21,15 @@
 //            one round ahead, each lane's value broadcast in turn and added in order, each lane keeping its prefix
 //   values : one thread per sorted position: from its partition's bounds and its peer group's bounds and index, every
 //            function's value (into a per-function array in sorted order; an aggregate's read from the fold at its
-//            frame's last position, with its null flag and a wide decimal's high word), whether the limit keeps it,
-//            and its output bytes; the kept records and the bytes scanned, and the totals and the too-long and too-large-partition
-//            flags come back in one readback
+//            frame's last position, with its null flag and a wide decimal's high word; an offset function's source
+//            position, read for a fixed-width value), whether the limit keeps it, and its output bytes (a string
+//            value's bytes padded to 8 make them per row); each record's own string and wide decimal inputs of offset
+//            functions are checked; the kept records and the bytes scanned, and the totals, the too-long and
+//            too-large-partition flags and the first bad input come back in one readback
 //   emit   : a warp per output row (with a limit, over the compacted kept positions only): its null words widened (with
-//            the values' null bits), its slots, the function slots, its var bytes and the wide decimal results' 16
-//            bytes each, then the VAR and DECIMAL_WIDE slots' offsets moved
+//            the values' null bits), its slots, the function slots, its var bytes and the var-valued functions' bytes in
+//            function order (16 per wide decimal, a string's padded to 8; with offset functions each region's offset is
+//            a warp scan of the sizes before it), then the VAR and DECIMAL_WIDE slots' offsets moved
 #include <algorithm>
 
 #include "decimal128.h"
@@ -45,7 +52,9 @@ inline unsigned grid_for(uint64_t n) {
 // partitions' first positions (n after the last), every function's value (function f at [f n, f n + n)), the kept
 // records and the output bytes (scanned in place), the kept positions compacted; scan workspace, readback, the shape
 // and its field list; then, with aggregate functions, two sets of fold state (aggregate a at [a n, a n + n) of each
-// array), the values' null bits per position and the wide decimal results' high words (wide ordinal k at [k n, k n + n))
+// array), the values' null bits per position (with aggregate or offset functions) and the wide decimal results' high
+// words (wide ordinal k at [k n, k n + n)); then per non-null index x the scanned present flags (n + 1 at [x stride,
+// x stride + n]) and the present positions (at [x n, x n + n))
 struct WindowWs {
   uint64_t* phead;
   uint32_t* pstart;
@@ -62,6 +71,10 @@ struct WindowWs {
   uint32_t* cnt[2];
   uint32_t* vnul;
   uint64_t* vhi;
+  uint64_t* rnk;
+  uint32_t* pres;
+  uint64_t stride;
+  uint8_t* end;
 };
 
 WindowWs carve_window_ws(uint8_t* d_wws, uint64_t n, const WindowShape& sh) {
@@ -83,8 +96,12 @@ WindowWs carve_window_ws(uint8_t* d_wws, uint64_t n, const WindowShape& sh) {
     w.hi[b] = (uint64_t*)p;  p += a256(m * 8);
     w.cnt[b] = (uint32_t*)p; p += a256(m * 4);
   }
-  w.vnul = (uint32_t*)p;     p += a256(sh.n_agg ? n * 4 : 0);
+  w.vnul = (uint32_t*)p;     p += a256(sh.n_agg || sh.n_off ? n * 4 : 0);
   w.vhi = (uint64_t*)p;      p += a256((size_t)sh.n_wide * n * 8);
+  w.stride = a256((n + 1) * 8) / 8;
+  w.rnk = (uint64_t*)p;      p += (size_t)sh.n_nn * w.stride * 8;
+  w.pres = (uint32_t*)p;     p += a256((size_t)sh.n_nn * n * 4);
+  w.end = p;
   return w;
 }
 
@@ -158,6 +175,9 @@ constexpr unsigned kFull = 0xffffffffu;
 __device__ __forceinline__ uint32_t val_kind(uint32_t vt) { return vt & 0xff; }
 __device__ __forceinline__ uint32_t dec_p(uint32_t vt) { return (vt >> 8) & 0xff; }
 
+// an aggregate function (offset functions are numbered after them)
+__host__ __device__ __forceinline__ bool is_agg(uint32_t fn) { return fn >= B2S_WINDOW_SUM && fn <= B2S_WINDOW_AVG; }
+
 // SUM of a float or double and AVG of anything but a decimal fold in double, serially; every other aggregate is a
 // group operation (or min / max) and scans
 __device__ __forceinline__ bool folds_double(uint32_t fn, uint32_t vt) {
@@ -189,7 +209,7 @@ __global__ void __launch_bounds__(kWindowThreads) window_stage_kernel(
     const uint8_t* row = arena + rec_off[i] + 4;
     for (uint32_t f = 0; f < n_fns; f++) {
       const uint32_t fn = sh->fn[f];
-      if (fn < B2S_WINDOW_SUM) continue;
+      if (!is_agg(fn)) continue;
       const uint32_t vt = sh->vtype[f], k = val_kind(vt);
       uint64_t l = 0, h = 0;
       uint32_t c = 1;
@@ -246,7 +266,7 @@ __global__ void __launch_bounds__(kWindowThreads) window_scan_pass_kernel(
     const bool take = j >= pstart[next_scanned(phead, j, n, P) - 1] + d;
     for (uint32_t f = 0; f < n_fns; f++) {
       const uint32_t fn = sh->fn[f], vt = sh->vtype[f];
-      if (fn < B2S_WINDOW_SUM || folds_double(fn, vt)) continue;
+      if (!is_agg(fn) || folds_double(fn, vt)) continue;
       const size_t x = (size_t)sh->agg[f] * n + j;
       uint64_t l = lo_in[x], h = hi_in[x];
       uint32_t c = cnt_in[x];
@@ -292,7 +312,7 @@ __global__ void __launch_bounds__(kWindowThreads) window_fold_kernel(
   for (uint64_t p = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) / 32; p < P; p += warps) {
     const uint64_t s = pstart[p], e = pstart[p + 1];
     for (uint32_t f = 0; f < n_fns; f++) {
-      if (sh->fn[f] < B2S_WINDOW_SUM || !folds_double(sh->fn[f], sh->vtype[f])) continue;
+      if (!is_agg(sh->fn[f]) || !folds_double(sh->fn[f], sh->vtype[f])) continue;
       const size_t base = (size_t)sh->agg[f] * n;
       double acc = 0.0;
       uint32_t seen = 0;
@@ -356,7 +376,8 @@ __device__ __forceinline__ Dec128 dec_avg(Dec128 x, uint32_t c) {
 }
 
 // The state arrays an aggregate's value is read from (the folds), and where the values kernel puts the values' null
-// bits (a mask per position) and wide decimal results' high words; all nullptr without aggregate functions
+// bits (a mask per position) and wide decimal results' high words; all nullptr without aggregate functions, but for
+// the null bits with offset functions
 struct WindowAggIo {
   const uint64_t* lo;
   const uint64_t* hi;
@@ -388,16 +409,153 @@ __device__ uint64_t agg_value(const WindowShape* __restrict__ sh, uint32_t f, co
   return v.lo;
 }
 
+// ---- offset functions ----
+__device__ __forceinline__ bool is_offset(uint32_t fn) { return fn >= B2S_WINDOW_LAG; }
+__device__ __forceinline__ bool wide_input(uint32_t vt) {
+  return val_kind(vt) == B2S_WINDOW_VAL_DECIMAL && dec_p(vt) > 18;
+}
+// the slot bits UnsafeRowWriter writes for a fixed-width value of kind k: the slot zeroed, then the type's width
+__device__ __forceinline__ uint64_t width_mask(uint32_t k) {
+  return k == B2S_WINDOW_VAL_INT8 ? 0xffull : k == B2S_WINDOW_VAL_INT16 ? 0xffffull
+         : k == B2S_WINDOW_VAL_INT32 || k == B2S_WINDOW_VAL_FLOAT32 ? 0xffffffffull : ~0ull;
+}
+constexpr uint64_t kNoSource = ~0ull;
+
+// Non-null index, step 1: per sorted position j and non-null index x (function f, nn[f] = x), rnk[x stride + j] = 1
+// when f's input is present
+__global__ void __launch_bounds__(kWindowThreads) window_present_kernel(
+    const uint8_t* __restrict__ arena, const uint64_t* __restrict__ rec_off, const uint32_t* __restrict__ idx, uint64_t n,
+    const WindowShape* __restrict__ sh, uint64_t stride, uint64_t* __restrict__ rnk) {
+  const uint32_t n_fns = sh->n_fns;
+  for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (uint64_t)gridDim.x * blockDim.x) {
+    const uint8_t* row = arena + rec_off[at(idx, j)] + 4;
+    for (uint32_t f = 0; f < n_fns; f++)
+      if (sh->nn[f] >= 0) rnk[(size_t)sh->nn[f] * stride + j] = !null_bit(row, sh->vnull[f]);
+  }
+}
+
+// step 3, after each index's scan: pres[x n + r(j)] = j for each present position j
+__global__ void __launch_bounds__(kWindowThreads) window_pres_kernel(uint64_t n, uint32_t n_nn, uint64_t stride,
+                                                                     const uint64_t* __restrict__ rnk,
+                                                                     uint32_t* __restrict__ pres) {
+  for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (uint64_t)gridDim.x * blockDim.x)
+    for (uint32_t x = 0; x < n_nn; x++) {
+      const uint64_t* r = rnk + (size_t)x * stride;
+      if (r[j + 1] != r[j]) pres[(size_t)x * n + r[j]] = (uint32_t)j;
+    }
+}
+
+// What the values kernel reads for offset functions: the records, and the non-null indexes (nullptr without one)
+struct WindowOffIo {
+  const uint8_t* arena;
+  const uint64_t* rec_off;
+  const uint64_t* rnk;
+  const uint32_t* pres;
+  uint64_t stride;
+};
+
+// Offset function f's source sorted position for position j of partition [ps, pe) whose frame ends at e (FIRST, LAST
+// and NTH_VALUE), or kNoSource: outside the partition or the frame (LAG / LEAD's default, else null).  With a
+// non-null index the partition's present positions are pres[r(ps) .. r(pe)) and the frame's pres[r(ps) .. r(e + 1)).
+__device__ __forceinline__ uint64_t offset_source(const WindowShape* __restrict__ sh, uint32_t f,
+                                                  const WindowOffIo& io, uint64_t n, uint64_t j, uint64_t ps,
+                                                  uint64_t pe, uint64_t e) {
+  const uint32_t fn = sh->fn[f];
+  const uint64_t k = sh->arg[f];  // LAG / LEAD's offset, NTH_VALUE's n; 0 for FIRST and LAST
+  const int32_t x = sh->nn[f];
+  if (x < 0) {  // every position is present
+    switch (fn) {
+      case B2S_WINDOW_LEAD: return j + k < pe ? j + k : kNoSource;
+      case B2S_WINDOW_LAG: return j - ps >= k ? j - k : kNoSource;
+      case B2S_WINDOW_FIRST: return ps;
+      case B2S_WINDOW_LAST: return e;
+      default: return ps + k - 1 <= e ? ps + k - 1 : kNoSource;
+    }
+  }
+  const uint64_t* r = io.rnk + (size_t)x * io.stride;
+  const uint64_t lo = r[ps];
+  uint64_t q;
+  switch (fn) {
+    case B2S_WINDOW_LEAD:
+      q = r[j + 1] + k - 1;
+      if (q >= r[pe]) return kNoSource;
+      break;
+    case B2S_WINDOW_LAG:
+      q = r[j];
+      if (q < lo + k) return kNoSource;
+      q -= k;
+      break;
+    case B2S_WINDOW_FIRST:
+      q = lo;
+      if (q >= r[e + 1]) return kNoSource;
+      break;
+    case B2S_WINDOW_LAST:
+      q = r[e + 1];
+      if (q <= lo) return kNoSource;
+      q -= 1;
+      break;
+    default:
+      q = lo + k - 1;
+      if (q >= r[e + 1]) return kNoSource;
+      break;
+  }
+  return io.pres[(size_t)x * n + q];
+}
+
+// Offset function f's value at position j: a fixed-width value's slot bits, LAG / LEAD's default, or (strings and wide
+// decimals) the source's sorted position for the emit; *null when it is null.  *extra grows by a string's bytes padded
+// to 8.  Position j's own input is checked (so the verdict does not depend on the offsets): a bad one lowers *bad to its
+// record's arena offset << 2 | kAggBadDecimal or kWindowBadBytes.
+__device__ __forceinline__ uint64_t offset_value(const uint32_t* __restrict__ rec_len, const uint32_t* __restrict__ idx,
+                                                 const WindowShape* __restrict__ sh, uint32_t f, const WindowOffIo& io,
+                                                 uint64_t n, uint64_t j, uint64_t ps, uint64_t pe, uint64_t e,
+                                                 bool* null, uint64_t* extra, unsigned long long* bad) {
+  const uint32_t vt = sh->vtype[f], k = val_kind(vt), voff = sh->voff[f];
+  const int32_t vnull = sh->vnull[f];
+  if (k == B2S_WINDOW_VAL_BYTES || wide_input(vt)) {
+    const uint32_t i = at(idx, j);
+    const uint8_t* row = io.arena + io.rec_off[i] + 4;
+    if (!null_bit(row, vnull)) {
+      const uint64_t slot = ld64(row + voff);
+      const uint32_t size = rec_len[i] - 4;
+      bool b = false;
+      if (k == B2S_WINDOW_VAL_BYTES) {
+        b = (slot >> 32) < 8ull * (sh->bw + sh->n) || (slot >> 32) + (uint32_t)slot > size;
+      } else {
+        uint64_t h, l;
+        decimal_bits(row, size, slot, h, l, &b);
+      }
+      if (b)
+        atomicMin(bad, (unsigned long long)((io.rec_off[i] << 2) |
+                                            (k == B2S_WINDOW_VAL_BYTES ? kWindowBadBytes : kAggBadDecimal)));
+    }
+  }
+  const uint64_t s = offset_source(sh, f, io, n, j, ps, pe, e);
+  if (s == kNoSource) {
+    *null = !(sh->flags[f] & B2S_WINDOW_HAS_DEFAULT);
+    return *null ? 0 : sh->dflt[f];
+  }
+  const uint32_t i = at(idx, s);
+  const uint8_t* row = io.arena + io.rec_off[i] + 4;
+  *null = null_bit(row, vnull);
+  if (*null) return 0;
+  if (k == B2S_WINDOW_VAL_BYTES) {
+    *extra += ((uint64_t)(uint32_t)ld64(row + voff) + 7) & ~7ull;
+    return s;
+  }
+  return wide_input(vt) ? s : ld64(row + voff) & width_mask(k);
+}
+
 __global__ void __launch_bounds__(kWindowThreads) window_values_kernel(
     const uint32_t* __restrict__ rec_len, const uint32_t* __restrict__ idx, uint64_t n,
     const WindowShape* __restrict__ sh, const uint64_t* __restrict__ heads_before, const uint32_t* __restrict__ gpos,
     const uint64_t* __restrict__ groups, const uint64_t* __restrict__ phead, const uint32_t* __restrict__ pstart,
     uint64_t* __restrict__ vals, uint64_t* __restrict__ rows, uint64_t* __restrict__ bytes,
-    uint64_t* __restrict__ readback, WindowAggIo io) {
+    uint64_t* __restrict__ readback, WindowAggIo io, WindowOffIo oio) {
   const uint64_t G = *groups, P = phead[n];
   const uint32_t n_fns = sh->n_fns, limit_fn = sh->limit_fn;
-  // what the output row adds to the input row
-  const uint64_t grow = 8ull * (sh->out_bw - sh->bw + n_fns) + 16ull * sh->n_wide;
+  // what the output row adds to the input row, past the offset functions' strings
+  const uint64_t grow = 8ull * (sh->out_bw - sh->bw + n_fns) + 16ull * (sh->n_wide + sh->n_wide_off);
   for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (uint64_t)gridDim.x * blockDim.x) {
     const uint64_t g = next_scanned(heads_before, j, n, G) - 1, p = next_scanned(phead, j, n, P) - 1;
     const uint64_t ps = pstart[p], N = pstart[p + 1] - ps;
@@ -405,6 +563,7 @@ __global__ void __launch_bounds__(kWindowThreads) window_values_kernel(
     const uint64_t dense = g - heads_before[ps] + 1;  // ps is a peer head: heads_before[ps] is its group
     if (N > 0x7fffffffull) readback[3] = 1;
     uint32_t nul = 0;
+    uint64_t extra = 0;
     for (uint32_t f = 0; f < n_fns; f++) {
       uint64_t v;
       bool null = false;
@@ -419,7 +578,9 @@ __global__ void __launch_bounds__(kWindowThreads) window_values_kernel(
           const uint32_t fr = sh->frame[f];
           const uint64_t e = fr == B2S_WINDOW_FRAME_ROWS_RUNNING ? j
                              : fr == B2S_WINDOW_FRAME_RANGE_RUNNING ? ps + ge - 1 : ps + N - 1;
-          v = agg_value(sh, f, io, n, e, j, &null);
+          v = is_offset(sh->fn[f]) ? offset_value(rec_len, idx, sh, f, oio, n, j, ps, ps + N, e, &null, &extra,
+                                                  (unsigned long long*)(readback + 4))
+                                   : agg_value(sh, f, io, n, e, j, &null);
           break;
         }
       }
@@ -432,7 +593,7 @@ __global__ void __launch_bounds__(kWindowThreads) window_values_kernel(
       const uint64_t lv = limit_fn == B2S_WINDOW_ROW_NUMBER ? i + 1 : limit_fn == B2S_WINDOW_RANK ? gs + 1 : dense;
       keep = lv <= (uint64_t)sh->limit;
     }
-    const uint64_t size = rec_len[at(idx, j)] - 4;
+    const uint64_t size = rec_len[at(idx, j)] - 4 + extra;
     if (keep && size + grow > 0x7fffffffull) readback[2] = 1;
     rows[j] = keep;
     bytes[j] = keep ? 4 + size + grow : 0;
@@ -455,7 +616,7 @@ __global__ void __launch_bounds__(kWindowThreads) window_emit_kernel(
     const uint32_t* __restrict__ vnul, const uint64_t* __restrict__ vhi, uint8_t* __restrict__ dst) {
   const uint32_t lane = threadIdx.x & 31;
   const uint64_t warps = (uint64_t)gridDim.x * (blockDim.x / 32);
-  const uint32_t nf = sh->n, bw = sh->bw, b = sh->out_bw, n_fns = sh->n_fns, n_wide = sh->n_wide;
+  const uint32_t nf = sh->n, bw = sh->bw, b = sh->out_bw, n_fns = sh->n_fns, n_wide = sh->n_wide, n_off = sh->n_off;
   const uint32_t fixed_in = 8 * (bw + nf);
   const uint64_t fixed_out = 8ull * (b + nf + n_fns);
   const uint64_t shift = 8ull * (b - bw + n_fns) << 32;
@@ -466,8 +627,35 @@ __global__ void __launch_bounds__(kWindowThreads) window_emit_kernel(
     const uint64_t var = rec_len[i] - 4 - fixed_in;
     uint8_t* d = dst + bytes[j];
     uint8_t* row = d + 4;
-    if (lane == 0) st_span16(d, 4, __byte_perm((uint32_t)(fixed_out + var + 16 * n_wide), 0, 0x0123), 0);
     const uint32_t nul = vnul ? vnul[j] : 0;
+    // lane f's var region (function f's, past the input's var bytes) starts vpre bytes in; every region's bytes: vall.
+    // With offset functions the regions are sized per row: a lane per function, its source row (vrow) and an inclusive
+    // warp scan of the sizes (16 per wide decimal, a non-null string's bytes padded to 8)
+    uint64_t vpre = lane < n_fns && sh->wide[lane] >= 0 ? 16ull * (uint32_t)sh->wide[lane] : 0, vall = 16ull * n_wide;
+    const uint8_t* vrow = nullptr;
+    uint32_t vlen = 0;
+    if (n_off) {
+      uint64_t sz = 0;
+      if (lane < n_fns) {
+        const uint32_t vt = sh->vtype[lane];
+        if (is_offset(sh->fn[lane]) && !((nul >> lane) & 1) && (val_kind(vt) == B2S_WINDOW_VAL_BYTES || wide_input(vt))) {
+          const uint32_t s = at(idx, vals[(size_t)lane * n + j]);
+          vrow = arena + rec_off[s] + 4;
+          vlen = val_kind(vt) == B2S_WINDOW_VAL_BYTES ? (uint32_t)ld64(vrow + sh->voff[lane]) : rec_len[s] - 4;
+        }
+        sz = sh->wide[lane] >= 0 || (is_offset(sh->fn[lane]) && wide_input(vt)) ? 16
+             : vrow ? ((uint64_t)vlen + 7) & ~7ull : 0;
+      }
+      uint64_t incl = sz;
+#pragma unroll
+      for (uint32_t o = 1; o < 32; o *= 2) {
+        const uint64_t y = __shfl_up_sync(kFull, incl, o);
+        if (lane >= o) incl += y;
+      }
+      vpre = incl - sz;
+      vall = __shfl_sync(kFull, incl, 31);
+    }
+    if (lane == 0) st_span16(d, 4, __byte_perm((uint32_t)(fixed_out + var + vall), 0, 0x0123), 0);
     for (uint32_t w = lane; w < b; w += 32) {
       uint64_t bits = 0;
       if (w < bw) {
@@ -480,25 +668,45 @@ __global__ void __launch_bounds__(kWindowThreads) window_emit_kernel(
       st_span16(row + 8 * w, 8, bits, 0);
     }
     warp_copy(row + 8 * b, src + 8 * bw, 8ull * nf, lane);
-    for (uint32_t f = lane; f < n_fns; f += 32) {
+    if (lane < n_fns) {
+      const uint32_t f = lane;
       uint64_t slot = vals[(size_t)f * n + j];
       const int32_t k = sh->wide[f];
-      if (k >= 0) {  // 16 bytes after the var bytes: BigInteger.toByteArray's, or zeros when null
-        const uint64_t off = fixed_out + var + 16ull * (uint32_t)k;
+      const uint64_t off = fixed_out + var + vpre;
+      const bool wide_off = n_off && is_offset(sh->fn[f]) && wide_input(sh->vtype[f]);
+      if (k >= 0 || wide_off) {  // 16 bytes in its region: BigInteger.toByteArray's, or zeros when null
         uint64_t m0 = 0, m1 = 0;
         if ((nul >> f) & 1) {
           slot = off << 32;
         } else {
-          const Dec128 x{slot, vhi[(size_t)k * n + j]};
+          Dec128 x{slot, 0};
+          if (wide_off) {  // the source's bytes, re-encoded minimally
+            bool unused = false;
+            decimal_bits(vrow, vlen, ld64(vrow + sh->voff[f]), x.hi, x.lo, &unused);
+            x.hi ^= 1ull << 63;
+          } else {
+            x.hi = vhi[(size_t)k * n + j];
+          }
           const uint32_t len = dec_bytes(x);
           dec_encode(x, len, &m0, &m1);
           slot = off << 32 | len;
         }
         st_span16(row + off, 16, m0, m1);
+      } else if (vrow) {  // a string: its bytes follow below
+        slot = off << 32 | vlen;
       }
       st_span16(row + 8 * (b + nf + f), 8, slot, 0);
     }
     warp_copy(row + fixed_out, src + fixed_in, var, lane);
+    // the offset functions' strings, each by the whole warp, zero-padded to 8 bytes
+    for (uint32_t f = 0; n_off && f < n_fns; f++) {
+      const uint8_t* s = (const uint8_t*)__shfl_sync(kFull, (unsigned long long)vrow, f);
+      if (!s || val_kind(sh->vtype[f]) != B2S_WINDOW_VAL_BYTES) continue;
+      const uint32_t len = __shfl_sync(kFull, vlen, f);
+      const uint64_t off = fixed_out + var + __shfl_sync(kFull, vpre, f);
+      warp_copy(row + off, s + (uint32_t)(ld64(s + sh->voff[f]) >> 32), len, lane);
+      if (lane == 0 && (len & 7)) st_span16(row + off + len, 8 - (len & 7), 0, 0);
+    }
     __syncwarp();
     // a zero slot (a null string) stays zero
     for (uint32_t x = lane; x < sh->n_var; x += 32) {
@@ -513,8 +721,7 @@ __global__ void __launch_bounds__(kWindowThreads) window_emit_kernel(
 }  // namespace
 
 size_t window_ws_bytes(uint64_t n, const WindowShape& shape) {
-  const WindowWs w = carve_window_ws(nullptr, n, shape);  // the parts' offsets from 0
-  return reinterpret_cast<uintptr_t>(w.vhi) + a256((size_t)shape.n_wide * n * 8);
+  return reinterpret_cast<uintptr_t>(carve_window_ws(nullptr, n, shape).end);  // the parts' offsets from 0
 }
 
 uint64_t* window_readback(uint8_t* d_wws, uint64_t n, const WindowShape& shape) {
@@ -538,11 +745,24 @@ void launch_window_values(const uint8_t* arena, uint64_t n, const uint32_t* idx,
   launch_exclusive_scan_u64(w.phead, n, w.phead + n, w.scan_ws, st, launches);
   window_part_starts_kernel<<<grid_for(n), kWindowThreads, 0, st>>>(w.phead, n, w.pstart);
   if (launches) *launches += 2;
+  WindowOffIo oio{arena, k.src_off, nullptr, nullptr, w.stride};
+  if (shape.n_nn) {  // the non-null indexes: present flags, a scan each, the present positions compacted
+    window_present_kernel<<<grid_for(n), kWindowThreads, 0, st>>>(arena, k.src_off, idx, n, w.shape, w.stride, w.rnk);
+    for (uint32_t x = 0; x < shape.n_nn; x++) {
+      uint64_t* r = w.rnk + (size_t)x * w.stride;
+      launch_exclusive_scan_u64(r, n, r + n, w.scan_ws, st, launches);
+    }
+    window_pres_kernel<<<grid_for(n), kWindowThreads, 0, st>>>(n, shape.n_nn, w.stride, w.rnk, w.pres);
+    oio.rnk = w.rnk;
+    oio.pres = w.pres;
+    if (launches) *launches += 2;
+  }
   WindowAggIo io{};
+  io.vnul = shape.n_off ? w.vnul : nullptr;
   if (shape.n_agg) {
     bool scans = false, folds = false;
     for (uint32_t f = 0; f < shape.n_fns; f++) {
-      if (shape.fn[f] < B2S_WINDOW_SUM) continue;
+      if (!is_agg(shape.fn[f])) continue;
       const uint32_t kind = shape.vtype[f] & 0xff;
       const bool dbl = (shape.fn[f] == B2S_WINDOW_SUM &&
                         (kind == B2S_WINDOW_VAL_FLOAT32 || kind == B2S_WINDOW_VAL_FLOAT64)) ||
@@ -572,7 +792,7 @@ void launch_window_values(const uint8_t* arena, uint64_t n, const uint32_t* idx,
   }
   window_values_kernel<<<grid_for(n), kWindowThreads, 0, st>>>(k.len, idx, n, w.shape, heads_before,
                                                                rows_group_starts(d_aws, n), groups, w.phead, w.pstart,
-                                                               w.vals, w.rows, w.bytes, w.readback, io);
+                                                               w.vals, w.rows, w.bytes, w.readback, io, oio);
   launch_exclusive_scan_u64(w.rows, n, w.readback, w.scan_ws, st, launches);
   launch_exclusive_scan_u64(w.bytes, n, w.readback + 1, w.scan_ws, st, launches);
   if (launches) *launches += 1;
@@ -592,7 +812,7 @@ void launch_window_emit(const uint8_t* arena, uint64_t n, const uint32_t* idx, u
   const unsigned grid = (unsigned)std::min<uint64_t>(want, (uint64_t)kSMs * 16);
   window_emit_kernel<<<grid, kWindowThreads, 0, st>>>(arena, k.src_off, k.len, idx, n, out_rows,
                                                       limited ? w.kept : nullptr, w.shape, w.vals, w.bytes,
-                                                      shape.n_agg ? w.vnul : nullptr, w.vhi, d_dst);
+                                                      shape.n_agg || shape.n_off ? w.vnul : nullptr, w.vhi, d_dst);
   if (launches) *launches += 1;
 }
 

@@ -1097,7 +1097,8 @@ class S3ShuffleReader {
   }
   // The window's arguments (b2s_decompress_window_rows_keys_packed): the key columns (the first nPartitionKeys of them
   // partition), the input's field count and kinds, the functions and their arguments, and the limit; with aggregate,
-  // b2s_decompress_window_aggregate_rows_keys_packed's, whose functions also have frames and input columns (no limit).
+  // b2s_decompress_window_aggregate_rows_keys_packed's, whose functions also have frames and input columns (no limit);
+  // with offset, b2s_decompress_window_offset_rows_keys_packed's, whose functions also have flags and defaults.
   struct WindowArgs {
     uint32_t nPartitionKeys, nKeys;
     const uint32_t *keyType, *keyOff, *keyLen;
@@ -1114,6 +1115,9 @@ class S3ShuffleReader {
     const uint32_t* valOff = nullptr;
     const int32_t* valNull = nullptr;
     bool aggregate = false;
+    const uint32_t* flags = nullptr;
+    const uint64_t* dflt = nullptr;
+    bool offset = false;
   };
   // read() for a Spark SQL window over this shuffle read (INTEGRATION.md §3o): every non-empty block is fetched (the
   // exchange cache is not consulted) in computeShuffleBlocks order, then ONE b2s_decompress_window_rows_keys_packed
@@ -1136,6 +1140,12 @@ class S3ShuffleReader {
     uint64_t total = 0, out = 0;
     const uint64_t guess = codec == B2S_CODEC_NONE ? src.bytes * 2 : src.bytes * 4;
     const int rc = callWithRetry(sorted_, guess, total, [&](uint64_t cap) {
+      if (w.offset)
+        return b2s_decompress_window_offset_rows_keys_packed(
+            codec, alg, n, src.src.data(), src.off.data(), src.len.data(), alg ? src.sliceBase.data() : 0,
+            alg ? src.sliceLen.data() : 0, alg ? src.sliceSum.data() : 0, w.nPartitionKeys, w.nKeys, w.keyType,
+            w.keyOff, w.keyLen, w.keyNull, w.nFields, w.kind, w.nFns, w.fn, w.fnArg, w.frame, w.valType, w.valOff,
+            w.valNull, w.flags, w.dflt, sorted_.get(), cap, &total, nRecords, &out, status.data(), bad.data());
       if (w.aggregate)
         return b2s_decompress_window_aggregate_rows_keys_packed(
             codec, alg, n, src.src.data(), src.off.data(), src.len.data(), alg ? src.sliceBase.data() : 0,
@@ -1149,8 +1159,9 @@ class S3ShuffleReader {
           cap, &total, nRecords, &out, status.data(), bad.data());
     });
     if (rc != 0)
-      throw CodecException(std::string(w.aggregate ? "b2s_decompress_window_aggregate_rows_keys_packed: "
-                                               : "b2s_decompress_window_rows_keys_packed: ") +
+      throw CodecException(std::string(w.offset      ? "b2s_decompress_window_offset_rows_keys_packed: "
+                                       : w.aggregate ? "b2s_decompress_window_aggregate_rows_keys_packed: "
+                                                     : "b2s_decompress_window_rows_keys_packed: ") +
                            b2s_strerror(rc) + ": " + b2s_last_error());
     for (uint32_t k = 0; k < n; k++) throwBlockStatus(status[k], info_[sources[k]->first].id);
     sortedLen_ = total;
@@ -1637,6 +1648,26 @@ int b2sh_reader_read_window_aggregate_rows(b2sh_reader* r, uint32_t n_partition_
                                         key_null_field,   n_fields, field_kind,      n_fns,            fn,
                                         fn_arg,           B2S_WINDOW_NO_LIMIT, 0,    fn_frame,         val_type,
                                         val_off,          val_null_field,      true};
+    r->r->readWindowRows(w, n_records);
+    sorted_result(*r->r, data, len, n_out_records);
+  });
+}
+int b2sh_reader_read_window_offset_rows(b2sh_reader* r, uint32_t n_partition_keys, uint32_t n_keys,
+                                        const uint32_t* key_type, const uint32_t* key_off, const uint32_t* key_len,
+                                        const int32_t* key_null_field, uint32_t n_fields, const uint8_t* field_kind,
+                                        uint32_t n_fns, const uint32_t* fn, const int32_t* fn_arg,
+                                        const uint32_t* fn_frame, const uint32_t* val_type, const uint32_t* val_off,
+                                        const int32_t* val_null_field, const uint32_t* fn_flags,
+                                        const uint64_t* fn_default, const uint8_t** data, uint64_t* len,
+                                        uint64_t* n_records, uint64_t* n_out_records) {
+  return guarded([&] {
+    S3ShuffleReader::WindowArgs w{n_partition_keys, n_keys,   key_type,        key_off,          key_len,
+                                  key_null_field,   n_fields, field_kind,      n_fns,            fn,
+                                  fn_arg,           B2S_WINDOW_NO_LIMIT, 0,    fn_frame,         val_type,
+                                  val_off,          val_null_field,      true};
+    w.flags = fn_flags;
+    w.dflt = fn_default;
+    w.offset = true;
     r->r->readWindowRows(w, n_records);
     sorted_result(*r->r, data, len, n_out_records);
   });
