@@ -20,13 +20,17 @@
  *   checksumPacked                         shuffle/S3SingleSpillShuffleMapOutputWriter.scala:54-63,
  *                                          helper/S3ShuffleHelper.scala:94-103
  * Payload travels in pinned direct ByteBuffers (hostAlloc/wrap): the methods take raw addresses (jlong), so no
- * jbyteArray is ever pinned or copied; the small descriptor arrays (offsets, lengths, checksums, status) are Java
- * long[]/int[] accessed with Get/ReleasePrimitiveArrayCritical — every Get is paired with a Release on every path.
+ * jbyteArray is ever pinned or copied.  The small descriptor arrays (offsets, lengths, checksums, status) are Java
+ * long[]/int[]/byte[]: compressPacked, decompressPacked, decompressedSizePacked, checksumPacked and lastTiming hold
+ * them with Get/ReleasePrimitiveArrayCritical (every Get paired with a Release on every path); every other native
+ * copies them through Get/Set<Type>ArrayRegion, so no Java array is held while the GPU works.  Every native checks
+ * each array's length against the count that sizes it, and each required array against null, before the library
+ * sees a pointer: a bad argument is B2S_E_ARG, never a read or write past a Java array.
  *
  * Build (reference side):  cc -shared -fPIC -I$JAVA_HOME/include -I$JAVA_HOME/include/linux -Iinclude \
  *                              jni/b200shuffle_jni.c -L. -lb200shuffle -o libb200shuffle_jni.so
- * Here (no JDK): tests/test_jni_shim.py compiles this file against jni/stub/jni.h with -Wall -Werror, so signatures,
- * argument order against b200shuffle.h and the Get/Release pairing are at least compiler- and script-checked.
+ * Without a JDK: tests/test_jni_shim.py compiles this file against jni/stub/jni.h with -Wall -Wextra -Werror and runs
+ * every native through a stand-in JNIEnv (tests/native/jni_env_host.c) that checks each call as -Xcheck:jni would.
  */
 #include <jni.h>
 #include <stdint.h>
@@ -112,6 +116,12 @@ JNIEXPORT jint JNICALL J(compressPacked)(JNIEnv* e, jclass c, jint codec, jint l
                                          jlongArray dstOff, jlongArray dstLen, jlongArray meta, jlongArray checksums,
                                          jintArray status) {
   (void)c;
+  if (n < 0 || !meta || (*e)->GetArrayLength(e, meta) < 1) return B2S_E_ARG;
+  if (n > 0 && (!off || !len || !dstOff || !dstLen || !status || (*e)->GetArrayLength(e, off) < n ||
+                (*e)->GetArrayLength(e, len) < n || (*e)->GetArrayLength(e, dstOff) < n ||
+                (*e)->GetArrayLength(e, dstLen) < n || (*e)->GetArrayLength(e, status) < n ||
+                (checksums && (*e)->GetArrayLength(e, checksums) < n)))
+    return B2S_E_ARG;
   jlong* o = crit_get(e, off);
   jlong* l = crit_get(e, len);
   jlong* dO = crit_get(e, dstOff);
@@ -388,6 +398,19 @@ JNIEXPORT jint JNICALL J(decompressPacked)(JNIEnv* e, jclass c, jint codec, jint
                                            jlongArray sliceChecksum, jlong dst, jlong dstCap, jlongArray dstOff,
                                            jlongArray dstLen, jlongArray meta, jintArray status, jintArray badSlice) {
   (void)c;
+  if (n < 0 || !meta || (*e)->GetArrayLength(e, meta) < 1) return B2S_E_ARG;
+  if (n > 0 && (!off || !len || !dstOff || !dstLen || !status || (*e)->GetArrayLength(e, off) < n ||
+                (*e)->GetArrayLength(e, len) < n || (*e)->GetArrayLength(e, dstOff) < n ||
+                (*e)->GetArrayLength(e, dstLen) < n || (*e)->GetArrayLength(e, status) < n ||
+                (badSlice && (*e)->GetArrayLength(e, badSlice) < n)))
+    return B2S_E_ARG;
+  if (alg != 0 && n > 0) { /* block i's slices are [sliceBase[i], sliceBase[i+1]): sliceBase[n] sizes the slice arrays */
+    if (!sliceBase || !sliceLen || !sliceChecksum || (*e)->GetArrayLength(e, sliceBase) < n + 1) return B2S_E_ARG;
+    jint ns = 0;
+    (*e)->GetIntArrayRegion(e, sliceBase, n, 1, &ns);
+    if (ns < 0 || (*e)->GetArrayLength(e, sliceLen) < ns || (*e)->GetArrayLength(e, sliceChecksum) < ns)
+      return B2S_E_ARG;
+  }
   jlong* o = crit_get(e, off);
   jlong* l = crit_get(e, len);
   jint* sb = crit_get(e, sliceBase);
@@ -722,6 +745,11 @@ static void* region(JNIEnv* e, jarray a, jsize n, size_t elem, int* rc) {
   else (*e)->GetLongArrayRegion(e, (jlongArray)a, 0, n, (jlong*)p);
   return p;
 }
+/* region of an array the call requires: a NULL one is B2S_E_ARG too */
+static void* need(JNIEnv* e, jarray a, jsize n, size_t elem, int* rc) {
+  if (!a && !*rc) *rc = B2S_E_ARG;
+  return region(e, a, n, elem, rc);
+}
 
 /* ---- read side, sort-merge join (INTEGRATION.md §3n): blocks [0, nLeft) are the left side's, the rest the right's;
  *      joinType: B2S_JOIN_* (inner, left outer, left semi, left anti, right outer, full outer).
@@ -740,23 +768,23 @@ JNIEXPORT jint JNICALL J(decompressJoinRowsKeysPacked)(JNIEnv* e, jclass c, jint
                                                        jbyteArray rightFieldKind, jlong dst, jlong dstCap,
                                                        jlongArray meta, jintArray status, jintArray badSlice) {
   (void)c;
-  if (n < 0 || !meta || (*e)->GetArrayLength(e, meta) < 4) return B2S_E_ARG;
+  if (n < 0 || nKeys < 1 || nKeys > 16 || !meta || (*e)->GetArrayLength(e, meta) < 4) return B2S_E_ARG;
   if (n > 0 && (!status || (*e)->GetArrayLength(e, status) < n || (badSlice && (*e)->GetArrayLength(e, badSlice) < n)))
     return B2S_E_ARG;
   const int with_slices = alg != 0 && n > 0;
   int rc = 0;
-  uint64_t* o = region(e, off, n, 8, &rc);
-  uint64_t* l = region(e, len, n, 8, &rc);
-  uint32_t* sb = with_slices ? region(e, sliceBase, n + 1, 4, &rc) : 0;
+  uint64_t* o = n > 0 ? need(e, off, n, 8, &rc) : 0;
+  uint64_t* l = n > 0 ? need(e, len, n, 8, &rc) : 0;
+  uint32_t* sb = with_slices ? need(e, sliceBase, n + 1, 4, &rc) : 0;
   const jsize ns = sb && !rc ? (jsize)sb[n] : 0;
-  uint64_t* sl = with_slices ? region(e, sliceLen, ns, 8, &rc) : 0;
-  uint64_t* sc = with_slices ? region(e, sliceChecksum, ns, 8, &rc) : 0;
-  uint32_t* kt = region(e, keyType, nKeys, 4, &rc);
-  uint32_t* kl = region(e, keyLen, nKeys, 4, &rc);
-  uint32_t* lo = region(e, leftKeyOff, nKeys, 4, &rc);
-  int32_t* ln = region(e, leftKeyNullField, nKeys, 4, &rc);
-  uint32_t* ro = region(e, rightKeyOff, nKeys, 4, &rc);
-  int32_t* rn = region(e, rightKeyNullField, nKeys, 4, &rc);
+  uint64_t* sl = with_slices ? need(e, sliceLen, ns, 8, &rc) : 0;
+  uint64_t* sc = with_slices ? need(e, sliceChecksum, ns, 8, &rc) : 0;
+  uint32_t* kt = need(e, keyType, nKeys, 4, &rc);
+  uint32_t* kl = need(e, keyLen, nKeys, 4, &rc);
+  uint32_t* lo = need(e, leftKeyOff, nKeys, 4, &rc);
+  int32_t* ln = need(e, leftKeyNullField, nKeys, 4, &rc);
+  uint32_t* ro = need(e, rightKeyOff, nKeys, 4, &rc);
+  int32_t* rn = need(e, rightKeyNullField, nKeys, 4, &rc);
   uint8_t* lk = region(e, leftFieldKind, nLeftFields, 1, &rc);
   uint8_t* rk = region(e, rightFieldKind, nRightFields, 1, &rc);
   int32_t* st = (int32_t*)malloc((size_t)n * 2 * sizeof(int32_t) + 1);
@@ -768,7 +796,7 @@ JNIEXPORT jint JNICALL J(decompressJoinRowsKeysPacked)(JNIEnv* e, jclass c, jint
         l, sb, sl, sc, (uint32_t)nKeys, kt, kl, lo, ln, ro, rn, (uint32_t)nLeftFields, lk, (uint32_t)nRightFields, rk,
         PTR(uint8_t, dst), (uint64_t)dstCap, &m[0], &m[1], &m[2], &m[3], st, st + n);
     (*e)->SetLongArrayRegion(e, meta, 0, 4, (const jlong*)m);
-    if (n > 0) {
+    if ((rc == 0 || rc == B2S_E_DST_TOO_SMALL) && n > 0) { /* a failed call leaves st unwritten */
       (*e)->SetIntArrayRegion(e, status, 0, n, (const jint*)st);
       if (badSlice) (*e)->SetIntArrayRegion(e, badSlice, 0, n, (const jint*)(st + n));
     }
@@ -794,24 +822,25 @@ JNIEXPORT jint JNICALL J(decompressWindowRowsKeysPacked)(JNIEnv* e, jclass c, ji
                                                          jlong dstCap, jlongArray meta, jintArray status,
                                                          jintArray badSlice) {
   (void)c;
-  if (n < 0 || !meta || (*e)->GetArrayLength(e, meta) < 3) return B2S_E_ARG;
+  if (n < 0 || nKeys < 1 || nKeys > 16 || nFns < 1 || nFns > 16 || !meta || (*e)->GetArrayLength(e, meta) < 3)
+    return B2S_E_ARG;
   if (n > 0 && (!status || (*e)->GetArrayLength(e, status) < n || (badSlice && (*e)->GetArrayLength(e, badSlice) < n)))
     return B2S_E_ARG;
   const int with_slices = alg != 0 && n > 0;
   int rc = 0;
-  uint64_t* o = region(e, off, n, 8, &rc);
-  uint64_t* l = region(e, len, n, 8, &rc);
-  uint32_t* sb = with_slices ? region(e, sliceBase, n + 1, 4, &rc) : 0;
+  uint64_t* o = n > 0 ? need(e, off, n, 8, &rc) : 0;
+  uint64_t* l = n > 0 ? need(e, len, n, 8, &rc) : 0;
+  uint32_t* sb = with_slices ? need(e, sliceBase, n + 1, 4, &rc) : 0;
   const jsize ns = sb && !rc ? (jsize)sb[n] : 0;
-  uint64_t* sl = with_slices ? region(e, sliceLen, ns, 8, &rc) : 0;
-  uint64_t* sc = with_slices ? region(e, sliceChecksum, ns, 8, &rc) : 0;
-  uint32_t* kt = region(e, keyType, nKeys, 4, &rc);
-  uint32_t* ko = region(e, keyOff, nKeys, 4, &rc);
-  uint32_t* kl = region(e, keyLen, nKeys, 4, &rc);
-  int32_t* kn = region(e, keyNullField, nKeys, 4, &rc);
-  uint8_t* fk = region(e, fieldKind, nFields, 1, &rc);
-  uint32_t* fs = region(e, fn, nFns, 4, &rc);
-  int32_t* fa = region(e, fnArg, nFns, 4, &rc);
+  uint64_t* sl = with_slices ? need(e, sliceLen, ns, 8, &rc) : 0;
+  uint64_t* sc = with_slices ? need(e, sliceChecksum, ns, 8, &rc) : 0;
+  uint32_t* kt = need(e, keyType, nKeys, 4, &rc);
+  uint32_t* ko = need(e, keyOff, nKeys, 4, &rc);
+  uint32_t* kl = need(e, keyLen, nKeys, 4, &rc);
+  int32_t* kn = need(e, keyNullField, nKeys, 4, &rc);
+  uint8_t* fk = need(e, fieldKind, nFields, 1, &rc);
+  uint32_t* fs = need(e, fn, nFns, 4, &rc);
+  int32_t* fa = need(e, fnArg, nFns, 4, &rc);
   int32_t* st = (int32_t*)malloc((size_t)n * 2 * sizeof(int32_t) + 1);
   if (!rc && !st) rc = B2S_E_NOMEM;
   uint64_t m[3] = {0, 0, 0};
@@ -821,7 +850,7 @@ JNIEXPORT jint JNICALL J(decompressWindowRowsKeysPacked)(JNIEnv* e, jclass c, ji
         (uint32_t)nPartitionKeys, (uint32_t)nKeys, kt, ko, kl, kn, (uint32_t)nFields, fk, (uint32_t)nFns, fs, fa,
         (uint32_t)limitFn, (int32_t)limit, PTR(uint8_t, dst), (uint64_t)dstCap, &m[0], &m[1], &m[2], st, st + n);
     (*e)->SetLongArrayRegion(e, meta, 0, 3, (const jlong*)m);
-    if (n > 0) {
+    if ((rc == 0 || rc == B2S_E_DST_TOO_SMALL) && n > 0) { /* a failed call leaves st unwritten */
       (*e)->SetIntArrayRegion(e, status, 0, n, (const jint*)st);
       if (badSlice) (*e)->SetIntArrayRegion(e, badSlice, 0, n, (const jint*)(st + n));
     }
@@ -848,28 +877,29 @@ JNIEXPORT jint JNICALL J(decompressWindowAggregateRowsKeysPacked)(JNIEnv* e, jcl
                                                                   jlongArray meta, jintArray status,
                                                                   jintArray badSlice) {
   (void)c;
-  if (n < 0 || !meta || (*e)->GetArrayLength(e, meta) < 3) return B2S_E_ARG;
+  if (n < 0 || nKeys < 1 || nKeys > 16 || nFns < 1 || nFns > 16 || !meta || (*e)->GetArrayLength(e, meta) < 3)
+    return B2S_E_ARG;
   if (n > 0 && (!status || (*e)->GetArrayLength(e, status) < n || (badSlice && (*e)->GetArrayLength(e, badSlice) < n)))
     return B2S_E_ARG;
   const int with_slices = alg != 0 && n > 0;
   int rc = 0;
-  uint64_t* o = region(e, off, n, 8, &rc);
-  uint64_t* l = region(e, len, n, 8, &rc);
-  uint32_t* sb = with_slices ? region(e, sliceBase, n + 1, 4, &rc) : 0;
+  uint64_t* o = n > 0 ? need(e, off, n, 8, &rc) : 0;
+  uint64_t* l = n > 0 ? need(e, len, n, 8, &rc) : 0;
+  uint32_t* sb = with_slices ? need(e, sliceBase, n + 1, 4, &rc) : 0;
   const jsize ns = sb && !rc ? (jsize)sb[n] : 0;
-  uint64_t* sl = with_slices ? region(e, sliceLen, ns, 8, &rc) : 0;
-  uint64_t* sc = with_slices ? region(e, sliceChecksum, ns, 8, &rc) : 0;
-  uint32_t* kt = region(e, keyType, nKeys, 4, &rc);
-  uint32_t* ko = region(e, keyOff, nKeys, 4, &rc);
-  uint32_t* kl = region(e, keyLen, nKeys, 4, &rc);
-  int32_t* kn = region(e, keyNullField, nKeys, 4, &rc);
-  uint8_t* fk = region(e, fieldKind, nFields, 1, &rc);
-  uint32_t* fs = region(e, fn, nFns, 4, &rc);
-  int32_t* fa = region(e, fnArg, nFns, 4, &rc);
-  uint32_t* fr = region(e, fnFrame, nFns, 4, &rc);
-  uint32_t* vt = region(e, valType, nFns, 4, &rc);
-  uint32_t* vo = region(e, valOff, nFns, 4, &rc);
-  int32_t* vn = region(e, valNullField, nFns, 4, &rc);
+  uint64_t* sl = with_slices ? need(e, sliceLen, ns, 8, &rc) : 0;
+  uint64_t* sc = with_slices ? need(e, sliceChecksum, ns, 8, &rc) : 0;
+  uint32_t* kt = need(e, keyType, nKeys, 4, &rc);
+  uint32_t* ko = need(e, keyOff, nKeys, 4, &rc);
+  uint32_t* kl = need(e, keyLen, nKeys, 4, &rc);
+  int32_t* kn = need(e, keyNullField, nKeys, 4, &rc);
+  uint8_t* fk = need(e, fieldKind, nFields, 1, &rc);
+  uint32_t* fs = need(e, fn, nFns, 4, &rc);
+  int32_t* fa = need(e, fnArg, nFns, 4, &rc);
+  uint32_t* fr = need(e, fnFrame, nFns, 4, &rc);
+  uint32_t* vt = need(e, valType, nFns, 4, &rc);
+  uint32_t* vo = need(e, valOff, nFns, 4, &rc);
+  int32_t* vn = need(e, valNullField, nFns, 4, &rc);
   int32_t* st = (int32_t*)malloc((size_t)n * 2 * sizeof(int32_t) + 1);
   if (!rc && !st) rc = B2S_E_NOMEM;
   uint64_t m[3] = {0, 0, 0};
@@ -879,7 +909,7 @@ JNIEXPORT jint JNICALL J(decompressWindowAggregateRowsKeysPacked)(JNIEnv* e, jcl
         (uint32_t)nPartitionKeys, (uint32_t)nKeys, kt, ko, kl, kn, (uint32_t)nFields, fk, (uint32_t)nFns, fs, fa, fr,
         vt, vo, vn, PTR(uint8_t, dst), (uint64_t)dstCap, &m[0], &m[1], &m[2], st, st + n);
     (*e)->SetLongArrayRegion(e, meta, 0, 3, (const jlong*)m);
-    if (n > 0) {
+    if ((rc == 0 || rc == B2S_E_DST_TOO_SMALL) && n > 0) { /* a failed call leaves st unwritten */
       (*e)->SetIntArrayRegion(e, status, 0, n, (const jint*)st);
       if (badSlice) (*e)->SetIntArrayRegion(e, badSlice, 0, n, (const jint*)(st + n));
     }
@@ -907,30 +937,31 @@ JNIEXPORT jint JNICALL J(decompressWindowOffsetRowsKeysPacked)(JNIEnv* e, jclass
                                                                jlongArray meta, jintArray status,
                                                                jintArray badSlice) {
   (void)c;
-  if (n < 0 || !meta || (*e)->GetArrayLength(e, meta) < 3) return B2S_E_ARG;
+  if (n < 0 || nKeys < 1 || nKeys > 16 || nFns < 1 || nFns > 16 || !meta || (*e)->GetArrayLength(e, meta) < 3)
+    return B2S_E_ARG;
   if (n > 0 && (!status || (*e)->GetArrayLength(e, status) < n || (badSlice && (*e)->GetArrayLength(e, badSlice) < n)))
     return B2S_E_ARG;
   const int with_slices = alg != 0 && n > 0;
   int rc = 0;
-  uint64_t* o = region(e, off, n, 8, &rc);
-  uint64_t* l = region(e, len, n, 8, &rc);
-  uint32_t* sb = with_slices ? region(e, sliceBase, n + 1, 4, &rc) : 0;
+  uint64_t* o = n > 0 ? need(e, off, n, 8, &rc) : 0;
+  uint64_t* l = n > 0 ? need(e, len, n, 8, &rc) : 0;
+  uint32_t* sb = with_slices ? need(e, sliceBase, n + 1, 4, &rc) : 0;
   const jsize ns = sb && !rc ? (jsize)sb[n] : 0;
-  uint64_t* sl = with_slices ? region(e, sliceLen, ns, 8, &rc) : 0;
-  uint64_t* sc = with_slices ? region(e, sliceChecksum, ns, 8, &rc) : 0;
-  uint32_t* kt = region(e, keyType, nKeys, 4, &rc);
-  uint32_t* ko = region(e, keyOff, nKeys, 4, &rc);
-  uint32_t* kl = region(e, keyLen, nKeys, 4, &rc);
-  int32_t* kn = region(e, keyNullField, nKeys, 4, &rc);
-  uint8_t* fk = region(e, fieldKind, nFields, 1, &rc);
-  uint32_t* fs = region(e, fn, nFns, 4, &rc);
-  int32_t* fa = region(e, fnArg, nFns, 4, &rc);
-  uint32_t* fr = region(e, fnFrame, nFns, 4, &rc);
-  uint32_t* vt = region(e, valType, nFns, 4, &rc);
-  uint32_t* vo = region(e, valOff, nFns, 4, &rc);
-  int32_t* vn = region(e, valNullField, nFns, 4, &rc);
-  uint32_t* ff = region(e, fnFlags, nFns, 4, &rc);
-  uint64_t* fd = region(e, fnDefault, nFns, 8, &rc);
+  uint64_t* sl = with_slices ? need(e, sliceLen, ns, 8, &rc) : 0;
+  uint64_t* sc = with_slices ? need(e, sliceChecksum, ns, 8, &rc) : 0;
+  uint32_t* kt = need(e, keyType, nKeys, 4, &rc);
+  uint32_t* ko = need(e, keyOff, nKeys, 4, &rc);
+  uint32_t* kl = need(e, keyLen, nKeys, 4, &rc);
+  int32_t* kn = need(e, keyNullField, nKeys, 4, &rc);
+  uint8_t* fk = need(e, fieldKind, nFields, 1, &rc);
+  uint32_t* fs = need(e, fn, nFns, 4, &rc);
+  int32_t* fa = need(e, fnArg, nFns, 4, &rc);
+  uint32_t* fr = need(e, fnFrame, nFns, 4, &rc);
+  uint32_t* vt = need(e, valType, nFns, 4, &rc);
+  uint32_t* vo = need(e, valOff, nFns, 4, &rc);
+  int32_t* vn = need(e, valNullField, nFns, 4, &rc);
+  uint32_t* ff = need(e, fnFlags, nFns, 4, &rc);
+  uint64_t* fd = need(e, fnDefault, nFns, 8, &rc);
   int32_t* st = (int32_t*)malloc((size_t)n * 2 * sizeof(int32_t) + 1);
   if (!rc && !st) rc = B2S_E_NOMEM;
   uint64_t m[3] = {0, 0, 0};
@@ -940,7 +971,7 @@ JNIEXPORT jint JNICALL J(decompressWindowOffsetRowsKeysPacked)(JNIEnv* e, jclass
         (uint32_t)nPartitionKeys, (uint32_t)nKeys, kt, ko, kl, kn, (uint32_t)nFields, fk, (uint32_t)nFns, fs, fa, fr,
         vt, vo, vn, ff, fd, PTR(uint8_t, dst), (uint64_t)dstCap, &m[0], &m[1], &m[2], st, st + n);
     (*e)->SetLongArrayRegion(e, meta, 0, 3, (const jlong*)m);
-    if (n > 0) {
+    if ((rc == 0 || rc == B2S_E_DST_TOO_SMALL) && n > 0) { /* a failed call leaves st unwritten */
       (*e)->SetIntArrayRegion(e, status, 0, n, (const jint*)st);
       if (badSlice) (*e)->SetIntArrayRegion(e, badSlice, 0, n, (const jint*)(st + n));
     }
@@ -993,6 +1024,10 @@ JNIEXPORT jint JNICALL J(decompressedSizePacked)(JNIEnv* e, jclass c, jint codec
   enum { kStack = 256 };
   const uint8_t* ptrs_stack[kStack];
   const uint8_t** ptrs = ptrs_stack;
+  if (n < 0 || (n > 0 && (!off || !len || !outLen || !status || (*e)->GetArrayLength(e, off) < n ||
+                          (*e)->GetArrayLength(e, len) < n || (*e)->GetArrayLength(e, outLen) < n ||
+                          (*e)->GetArrayLength(e, status) < n)))
+    return B2S_E_ARG;
   jlong* o = crit_get(e, off);
   jlong* l = crit_get(e, len);
   jlong* out = crit_get(e, outLen);
@@ -1016,6 +1051,9 @@ JNIEXPORT jint JNICALL J(decompressedSizePacked)(JNIEnv* e, jclass c, jint codec
 JNIEXPORT jint JNICALL J(checksumPacked)(JNIEnv* e, jclass c, jint alg, jint n, jlong base, jlongArray off, jlongArray len,
                                          jlongArray out) {
   (void)c;
+  if (n < 0 || (n > 0 && (!off || !len || !out || (*e)->GetArrayLength(e, off) < n ||
+                          (*e)->GetArrayLength(e, len) < n || (*e)->GetArrayLength(e, out) < n)))
+    return B2S_E_ARG;
   jlong* o = crit_get(e, off);
   jlong* l = crit_get(e, len);
   jlong* r = crit_get(e, out);
@@ -1031,9 +1069,9 @@ JNIEXPORT jint JNICALL J(checksumPacked)(JNIEnv* e, jclass c, jint alg, jint n, 
  *      thread's last call, for the MiB/s log lines of shuffle/S3MeasureOutputStream.scala:55-63 ---- */
 JNIEXPORT jint JNICALL J(lastTiming)(JNIEnv* e, jclass c, jlongArray out8) {
   (void)c;
+  if (!out8 || (*e)->GetArrayLength(e, out8) < 8) return B2S_E_ARG;
   b2s_timing t;
   const int rc = b2s_last_timing(&t);
-  if ((*e)->GetArrayLength(e, out8) < 8) return B2S_E_ARG;
   jlong* o = crit_get(e, out8);
   if (o) {
     o[0] = (jlong)(t.total_ms * 1000.0);
