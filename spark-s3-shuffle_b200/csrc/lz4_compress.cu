@@ -86,12 +86,12 @@ __global__ void __launch_bounds__(kMatchMaxWarps * 32, 2) lz4_match_kernel(
     const uint8_t* __restrict__ src_base, const uint64_t* __restrict__ src_off, const uint64_t* __restrict__ src_len,
     const uint32_t* __restrict__ blk_base, uint32_t n_streams, uint32_t b0, uint32_t m, uint32_t block_size,
     uint32_t stride, uint32_t near_limit, uint16_t* __restrict__ offarr, uint16_t* __restrict__ mlarr,
-    unsigned int* __restrict__ work_counter, uint32_t stage_bytes) {
+    unsigned int* __restrict__ work_counter, uint32_t stage_bytes, bool ahead) {
   extern __shared__ __align__(16) uint8_t smem[];
   __shared__ __align__(8) uint64_t bar;  // completion of the bulk copy
   __shared__ const uint8_t* blk_src;     // source address of stage byte 0
   __shared__ uint32_t blk_id;
-  __shared__ int blk_n, blk_a, blk_bulk;
+  __shared__ int blk_n, blk_a;
   constexpr unsigned FULL = 0xffffffffu;
   const int W = blockDim.x >> 5, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const uint32_t* st32 = reinterpret_cast<const uint32_t*>(smem);
@@ -102,46 +102,61 @@ __global__ void __launch_bounds__(kMatchMaxWarps * 32, 2) lz4_match_kernel(
   // guarantees determinism almost never iterates.
   const int r_me = 31 - lane;
   const uint32_t bar_a = smem_addr(&bar);
+  // With `ahead`, the CTA's next block is claimed one ahead, while the block before it is being worked on, by the last
+  // warp (which has no pass-1 segment): the counter's round trip and the search for the block's stream stay off the
+  // path on which all warps wait, and the next block's interior is prefetched into L2 so that its bulk copy does not
+  // wait on HBM.  Without it, thread 0 claims each block at its start while the other threads wait.
+  const bool claimer = threadIdx.x == blockDim.x - 32;
+  auto claim_next = [&]() {
+    const uint32_t bl = atomicAdd(work_counter, 1u);
+    blk_id = bl;
+    if (bl < m) {
+      const BlockSpan B = block_span(src_base, src_off, src_len, blk_base, n_streams, b0 + bl, block_size);
+      const int a = (int)(reinterpret_cast<uintptr_t>(B.s) & 15u);
+      const int lo = (a + 15) & ~15, hi = (a + B.n) & ~15;
+      blk_src = B.s - a;
+      blk_n = B.n;
+      blk_a = a;
+      if (ahead && hi > lo)
+        asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(B.s - a + lo), "r"(hi - lo) : "memory");
+    }
+  };
   if (threadIdx.x == 0) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar_a) : "memory");
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
+  if (ahead && claimer) claim_next();
   uint32_t phase = 0;
 
   for (;;) {
     __syncthreads();  // the previous block's staged bytes and tables are no longer read
-    if (threadIdx.x == 0) {
-      const uint32_t bl = atomicAdd(work_counter, 1u);
-      blk_id = bl;
-      if (bl < m) {
-        const BlockSpan B = block_span(src_base, src_off, src_len, blk_base, n_streams, b0 + bl, block_size);
-        const int a = (int)(reinterpret_cast<uintptr_t>(B.s) & 15u);
-        const int lo = (a + 15) & ~15, hi = (a + B.n) & ~15;
-        blk_src = B.s - a;
-        blk_n = B.n;
-        blk_a = a;
-        blk_bulk = hi > lo;
-        if (hi > lo) {
-          // order the generic-proxy reads of the previous block before the async-proxy writes of this one
-          asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-          asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar_a), "r"(hi - lo) : "memory");
-          asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                       ::"r"(smem_addr(smem + lo)), "l"(B.s - a + lo), "r"(hi - lo), "r"(bar_a) : "memory");
-        }
-      }
+    if (!ahead) {
+      if (threadIdx.x == 0) claim_next();
+      __syncthreads();
     }
-    __syncthreads();
     const uint32_t bl = blk_id;
     if (bl >= m) break;
     const int n = blk_n, a = blk_a;
+    const int lo = (a + 15) & ~15, hi = (a + n) & ~15;
+    const bool bulk = hi > lo;
+    if (threadIdx.x == 0 && bulk) {
+      // order the generic-proxy reads of the previous block before the async-proxy writes of this one
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+      asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar_a), "r"(hi - lo) : "memory");
+      asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                   ::"r"(smem_addr(smem + lo)), "l"(blk_src + lo), "r"(hi - lo), "r"(bar_a) : "memory");
+    }
     {
       const uint8_t* g = blk_src;
-      const int lo = (a + 15) & ~15, hi = (a + n) & ~15;
       const int head_end = lo < a + n ? lo : a + n, tail_beg = hi > lo ? hi : lo;
       for (int i = a + threadIdx.x; i < head_end; i += blockDim.x) smem[i] = __ldg(g + i);
       for (int i = tail_beg + threadIdx.x; i < a + n; i += blockDim.x) smem[i] = __ldg(g + i);
     }
-    if (blk_bulk) {
+    if (warp < W - 1) {  // pass 1's table starts empty; cleared while the block arrives
+      uint4* t4 = reinterpret_cast<uint4*>(table);
+      for (int j = lane; j < (1 << HLOG) / 8; j += 32) t4[j] = make_uint4(0, 0, 0, 0);
+    }
+    if (bulk) {
       uint32_t done;
       do {
         asm volatile(
@@ -152,7 +167,8 @@ __global__ void __launch_bounds__(kMatchMaxWarps * 32, 2) lz4_match_kernel(
       } while (!done);
       phase ^= 1u;
     }
-    __syncthreads();  // head and tail bytes visible
+    __syncthreads();  // head and tail bytes visible; every thread has read blk_*
+    if (ahead && claimer) claim_next();
     if (n < kMFLimit + 1) continue;
     const int mflimit = n - kMFLimit;
     const int matchlimit = n - kLastLiterals;
@@ -163,9 +179,6 @@ __global__ void __launch_bounds__(kMatchMaxWarps * 32, 2) lz4_match_kernel(
 
     // pass 1: the table of the warp's own segment alone (the last segment's is never needed)
     if (warp < W - 1) {
-      uint4* t4 = reinterpret_cast<uint4*>(table);
-      for (int j = lane; j < (1 << HLOG) / 8; j += 32) t4[j] = make_uint4(0, 0, 0, 0);
-      __syncwarp();
       for (int k = wb; k < we; k++) {
         const int p = 32 * k + r_me;
         const bool valid = p <= mflimit;
@@ -825,9 +838,14 @@ static void launch_match_t(const uint8_t* src_base, const uint64_t* d_src_off, c
   if (per_sm < 1) per_sm = 1;
   uint64_t grid = (uint64_t)kSMs * per_sm;  // persistent: one wave, CTAs pull blocks from the counter
   if (grid > m) grid = m;
+  // Claiming blocks one ahead pays only with one CTA per SM (with two, each CTA hides the other's stage-in) and on a
+  // long launch.  The parse kernel of the previous group runs beside this launch; beside a short one (config 3's last
+  // group of 7,232 blocks) it was measured to take 9.6 instead of 4.3 ms with the claim-ahead, most of it after the
+  // match launch had ended, which cost that write pass 5 ms (DESIGN §5).  16,384 blocks is half a default group.
+  const bool ahead = per_sm == 1 && m >= 16384u;
   lz4_match_kernel<HLOG><<<(unsigned)grid, warps * 32, smem, st>>>(
       src_base, d_src_off, d_src_len, d_blk_base, n_streams, b0, m, block_size, stride, near_limit, d_off, d_ml,
-      d_counter, stage);
+      d_counter, stage, ahead);
 }
 
 static void launch_match_warp_13(const uint8_t* src_base, const uint64_t* d_src_off, const uint64_t* d_src_len,
