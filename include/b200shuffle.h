@@ -136,7 +136,8 @@ int b2s_host_unregister(void* p);
 /* ---- sizing ---- */
 /* worst-case compressed size of one stream of src_len bytes (codec_block_size 0 = Spark default 32 KiB) */
 uint64_t b2s_compress_bound(uint32_t codec, uint32_t codec_block_size, uint64_t src_len);
-/* decompressed size of each compressed stream (LZ4Block: sum of originalLen; Snappy: sum of chunk varints) */
+/* decompressed size of each compressed stream (LZ4Block: sum of originalLen; Snappy: sum of chunk varints).  A stream
+ * whose framing, or a Snappy chunk's claim, fails the rules of b2s_decompress_batch gets its status here, per stream. */
 int b2s_decompressed_size_batch(uint32_t codec, uint32_t n, const uint8_t* const* src, const uint64_t* src_len,
                                 uint64_t* out_len, int32_t* status);
 
@@ -319,7 +320,12 @@ int b2s_partition_compress_rows_round_robin_dev(uint32_t dev_index, uint32_t cod
  * before decoding; a mismatch yields status[i] = B2S_E_CHECKSUM and bad_slice[i] = k (may be NULL).
  * n_slices / slice_* may be NULL when checksum_alg == 0.
  * A block whose status is not B2S_OK leaves the bytes of its own output range unspecified (the decoder may have
- * written part of it before it met the corruption); the output ranges of the other blocks are never touched by it. */
+ * written part of it before it met the corruption); the output ranges of the other blocks are never touched by it.
+ * Verdicts are per block: B2S_E_CORRUPT for a stream that breaks its codec's format, and B2S_E_UNSUPPORTED for a
+ * well-formed stream this decoder does not take: a Zstandard frame with a Dictionary_ID, or a Snappy chunk of more
+ * than 65536 decoded bytes or of 65536 compressed bytes or more (snappy-java's blockSize above 64 KiB).  A Snappy
+ * chunk that claims more than 64 decoded bytes per 3 compressed bytes (more than any element sequence yields) is
+ * B2S_E_CORRUPT.  Neither claim counts towards any decoded length or size: the call, and the other blocks, go on. */
 int b2s_decompress_batch(uint32_t codec, uint32_t checksum_alg, uint32_t n, const uint8_t* const* src,
                          const uint64_t* src_len, const uint32_t* n_slices, const uint64_t* const* slice_len,
                          const uint64_t* const* slice_checksum, uint8_t* const* dst, const uint64_t* dst_cap,

@@ -771,9 +771,9 @@ int decompress_enqueue_b(Slot& S, DecompressJob& J, const uint8_t* d_src, uint8_
     launch_lz4_decode_warp(desc, (uint32_t)J.nb, d_src, d_dst, J.d.status, J.d.counter, st, launches);
     CU(cudaEventRecord(e1, st));
   } else if (J.nb && J.codec == B2S_CODEC_SNAPPY_XERIAL) {
-    const uint64_t max_olen = J.h.totals[2], max_clen = J.h.totals[3];
-    if (max_olen > 65536 || max_clen >= 65536)
-      return fail(B2S_E_UNSUPPORTED, "snappy chunks larger than 64 KiB are not supported%s");
+    // the walk has failed every stream with a chunk of more than 64 KiB (B2S_E_UNSUPPORTED for that stream alone), so
+    // the largest chunk left is under 64 KiB compressed: the records' 16-bit fields hold every count and position
+    const uint64_t max_clen = J.h.totals[3];
     // tokens (thread per block) + copy (lane per sequence), in chunks that bound the record workspace
     const uint32_t nb = (uint32_t)J.nb;
     const uint32_t rec_stride = snappy_decode_rec_stride((uint32_t)max_clen);

@@ -236,7 +236,7 @@ __global__ void xerial_walk_kernel(const uint8_t* __restrict__ src_base, const u
   const uint64_t len = src_len[i];
   uint64_t ip = 0, cnt = 0, total = 0;
   uint32_t max_olen = 0, max_clen = 0;
-  bool bad = false, too_small = false;
+  bool bad = false, unsupported = false, too_small = false;
   if (FILL) too_small = (dst_off[i] + olen_total[i] > dst_cap);
   // stream header: magic 82 53 4E 41 50 50 59 00, then version / compatible version (not checked beyond presence).
   // No bytes at all is an empty stream, as SnappyInputStream.readHeader takes it (a partition the map side wrote
@@ -268,6 +268,18 @@ __global__ void xerial_walk_kernel(const uint8_t* __restrict__ src_base, const u
       bad = true;
       break;
     }
+    // A chunk is judged on its claim before anything is sized from it.  No element yields more than 64 / 3 decoded
+    // bytes per compressed byte (copy-2: 3 bytes, up to 64; copy-4: 5 bytes, 64; copy-1: 2 bytes, 11; a literal: one
+    // less than its bytes), so a longer claim is corrupt whatever the elements hold.  A plausible chunk of more than
+    // 64 KiB decoded, or of 64 KiB or more compressed, is not decoded here: its stream alone is unsupported.
+    if ((uint64_t)ulen * 3 > (uint64_t)(clen - (uint32_t)vb) * 64) {
+      bad = true;
+      break;
+    }
+    if (ulen > 65536u || clen >= 65536u) {
+      unsupported = true;
+      break;
+    }
     if (FILL) {
       BlockDesc d;
       d.src = src_off[i] + ip + vb;  // elements start after the varint
@@ -286,8 +298,8 @@ __global__ void xerial_walk_kernel(const uint8_t* __restrict__ src_base, const u
     ip += clen;
   }
   if (!FILL) {
-    if (bad) {
-      status[i] = B2S_E_CORRUPT;
+    if (bad || unsupported) {
+      status[i] = bad ? B2S_E_CORRUPT : B2S_E_UNSUPPORTED;
       cnt = 0;
       total = 0;
     }
@@ -356,13 +368,14 @@ __global__ void __launch_bounds__(64) snappy_tokens_kernel(const BlockDesc* __re
           err = true;
           break;
         }
-        len = 0;
-        for (int k = 0; k < nbytes; k++) len |= (int)__ldg(in + ip + k) << (8 * k);
-        if (len < 0 || len >= (1 << 24)) {  // cannot fit a chunk that passed the size limits
+        uint32_t l = 0;
+        for (int k = 0; k < nbytes; k++) l |= (uint32_t)__ldg(in + ip + k) << (8 * k);
+        l += 1;  // 32-bit, as in the snappy library: 0xFFFFFFFF wraps to an empty literal, which it accepts
+        if (l >= (1u << 24)) {  // cannot fit a chunk that passed the size limits
           err = true;
           break;
         }
-        len += 1;
+        len = (int)l;
         ip += nbytes;
       }
       if (len > clen - ip || len > olen - op) {
