@@ -235,6 +235,89 @@ int b2s_partition_compress_rows_hash_dev(uint32_t dev_index, uint32_t codec, int
                                          uint64_t dst_cap, uint64_t* dst_off, uint64_t* dst_len, uint64_t* dst_total,
                                          uint64_t* checksum_out, int32_t* status);
 
+/* ---- write side, partial aggregation: Spark's HashAggregateExec(Partial) and its hash exchange on the GPU ----
+ * The map side of a grouped aggregation's shuffle (HashAggregateExec(Partial) -> Exchange hashpartitioning(keys)) in
+ * one call: the map task's rows are grouped by the key columns, Spark's aggregation buffers are folded over each group,
+ * one partial row is written per key, and the partial rows are hash-partitioned and compressed into the .data object.
+ * A reducer merges them with b2s_decompress_aggregate_rows_keys_* (the merge ops below).
+ * Records: as for b2s_partition_compress_rows_hash_*: [size: int32 big-endian][row], rec_len[i] = 4 + size.
+ * Key columns: exactly those of the hash call (n_keys 1..16, its types, no order flags; B2S_KEY_BYTES is a 1-byte
+ * boolean).  n_keys = 0, a global aggregate, is B2S_E_ARG: Spark does not hash-partition it.
+ * Grouping: a group is a maximal set of records whose every key column is equal by the composite-key aggregation's
+ * rule: nulls equal nulls, strings are equal when their lengths and bytes are, 0.0 equals -0.0, every NaN equals every
+ * NaN.
+ * Aggregates: agg_fn[a] (a < n_aggs, at most 16; 0 is DISTINCT) is B2S_WINDOW_SUM .. B2S_WINDOW_AVG, val_type[a] a
+ * B2S_WINDOW_VAL_* (a decimal(p, s): B2S_WINDOW_VAL_DECIMAL | p << 8 | s << 16), val_off[a] the input's 8-byte slot
+ * (for p > 18 the slot (offset << 32) | size names 1..16 big-endian two's-complement bytes), val_null_field[a] its
+ * null bit or -1, as in the window aggregate call.  The semantics are Spark 3.5's DeclarativeAggregate.updateExpressions
+ * with ANSI off, folded over the group's records in input order.  Each function writes its buffers (Spark's
+ * aggBufferAttributes order), in function order:
+ *   SUM int8/16/32/64        long: the wrapping sum of the non-null inputs, sign-extended; null if none.
+ *                            Merge: B2S_AGG_SUM_INT64
+ *   SUM float / double       double: ((0.0 + x1) + x2) + ... over the non-null inputs, floats widened exactly, each add
+ *                            rounded to nearest (a lone -0.0 gives +0.0); null if none.  Merge: B2S_AGG_SUM_FLOAT64
+ *   SUM decimal(p, s), p<=28 decimal(p + 10, s): the exact sum, 0 if no input is non-null (below 2^32 records it never
+ *                            overflows); boolean isEmpty: 1 iff no input is non-null.  Never null.
+ *                            Merge: B2S_AGG_SUM_DECIMAL | (p + 10) << 8, B2S_AGG_MIN_INT32
+ *   COUNT, any val_type,     long: the non-null inputs (every record for VAL_NONE, count(*)); never null.
+ *   VAL_NONE or VAL_BYTES    Merge: B2S_AGG_SUM_INT64
+ *   AVG int8 .. double       double sum ((0.0 + c1) + c2) + ..., c the input cast to double (a long rounded to nearest),
+ *                            0.0 when null; long count of the non-null inputs.  Never null.
+ *                            Merge: B2S_AGG_SUM_FLOAT64, B2S_AGG_SUM_INT64
+ *   AVG decimal(p, s), p<=27 decimal(p + 10, s) exact sum (0 if none), long count.  Merge: B2S_AGG_SUM_DECIMAL |
+ *                            (p + 10) << 8, B2S_AGG_SUM_INT64.  Spark's Average adds with Add, whose result type for
+ *                            (P, s) + (P, s) is decimal(P + 1, s), exact only while P + 1 <= 38; Sum adds with
+ *                            DecimalAddNoOverflowCheck into its buffer type, so it takes p 28.
+ *   MIN / MAX int / date     int; long / timestamp / decimal(p <= 18): long; double: double; decimal(p > 18): decimal.
+ *                            Spark's Least / Greatest in Spark SQL's order (-0.0 equals 0.0, NaN above every other value
+ *                            and equal to every NaN): among equal values the first is kept, with its exact bits.  Null
+ *                            if none.  Merge: B2S_AGG_MIN / MAX_INT32, _INT64, _FLOAT64, _DECIMAL
+ * Partial row: as UnsafeProjection(groupingAttributes ++ aggBufferAttributes) writes it, with nf = n_keys + buffers
+ * (at most 32, so one null word, b = 1): field c < n_keys is key column c, buffer k is field n_keys + k, whose null bit
+ * is set only for a null value.  Fixed values are written as UnsafeRowWriter writes them (the 8-byte slot zeroed, then
+ * the type's width; an isEmpty boolean one byte).  Key values come from the group's first record in input order; float
+ * and double keys are normalized as NormalizeNaNAndZero leaves them (-0.0 as 0.0, any NaN as the canonical NaN).  Var
+ * regions follow the fixed region 8 (b + nf), in field order: a string or binary key its bytes zero-padded to 8 (a null
+ * one: slot 0, no bytes); a decimal(p > 18) key or buffer 16 bytes holding BigInteger.toByteArray's minimal bytes,
+ * zero-padded, slot (offset << 32) | length (a null one: 16 zero bytes, slot offset << 32).
+ * Order and outputs: the partial rows are produced in the composite-key sort's order (ascending, nulls first) and then
+ * partitioned stably by pmod(Murmur3Hash(key columns, 42), num_partitions).  dst_off / dst_len / checksum_out / status,
+ * *dst_total and the return value are byte for byte what b2s_partition_compress_rows_hash_packed returns for those
+ * partial rows in that order, keyed by the key columns at their output slots (8 + 8 c, null bit c when key_null_field[c]
+ * >= 0).  *n_groups (required) = the partial rows.
+ * Sizing: dst_cap below the arena -> B2S_E_DST_TOO_SMALL with *dst_total = the bytes needed, as the partition calls.
+ * With W the decimal(p > 18) fields (keys and buffers) and S the string / binary key columns, an arena of
+ *   b2s_partition_compress_bound(codec, codec_block_size, num_partitions,
+ *                                n_records * (4 + 8 (1 + nf) + 16 W + 8 S) + S * rec_bytes)
+ * bytes always suffices: a partial row's string key holds at most its input row's bytes plus 7 of padding, so the bound
+ * holds even when several key columns name the same bytes.
+ * Errors, B2S_E_ARG, checked before the device: what the hash call rejects; n_records >= 2^32; n_aggs above 16 or a
+ * NULL aggregate array (n_aggs > 0) or n_groups; an unknown function or val_type; a decimal p outside 1..38 or s > p;
+ * VAL_NONE or VAL_BYTES with a function other than COUNT; MIN / MAX of byte, short, float or bytes (the reducer cannot
+ * merge them); decimal SUM with p > 28 or AVG with p > 27; more than 16 buffers in all (the reduce-side merge's limit);
+ * a val_off that is not a multiple of 8 of at least 8 (a field's slot), or a val_null_field outside -1..65535.  A bad
+ * record -> B2S_E_ARG, nothing reported as written, b2s_last_error() names the lowest bad record and why: the hash call's
+ * record checks, a row that does not hold a value slot or a value's null word, a non-null decimal(p > 18) value whose
+ * size is not 1..16 or that runs past its row.  Device memory that cannot be had -> B2S_E_NOMEM (the caller keeps
+ * Spark's partial aggregation).  No usable device -> B2S_E_CUDA.
+ * Runs on the write lane.  b2s_last_timing: kernel_ms the whole call's device work, dominant_ms / dominant_launches the
+ * aggregation step (from the input records to the written partial rows). */
+int b2s_aggregate_partition_compress_rows_hash_packed(
+    uint32_t codec, int32_t level, uint32_t codec_block_size, uint32_t checksum_alg, uint32_t num_partitions,
+    uint64_t n_records, const uint8_t* rec_base, uint64_t rec_bytes, const uint32_t* rec_len, uint32_t n_keys,
+    const uint32_t* key_type, const uint32_t* key_off, const uint32_t* key_len, const int32_t* key_null_field,
+    uint32_t n_aggs, const uint32_t* agg_fn, const uint32_t* val_type, const uint32_t* val_off,
+    const int32_t* val_null_field, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_off, uint64_t* dst_len,
+    uint64_t* dst_total, uint64_t* checksum_out, int32_t* status, uint64_t* n_groups);
+/* same, with rec_base / rec_len / dst_base in device memory of dev_index; the other arrays stay host arrays */
+int b2s_aggregate_partition_compress_rows_hash_dev(
+    uint32_t dev_index, uint32_t codec, int32_t level, uint32_t codec_block_size, uint32_t checksum_alg,
+    uint32_t num_partitions, uint64_t n_records, const uint8_t* rec_base, uint64_t rec_bytes, const uint32_t* rec_len,
+    uint32_t n_keys, const uint32_t* key_type, const uint32_t* key_off, const uint32_t* key_len,
+    const int32_t* key_null_field, uint32_t n_aggs, const uint32_t* agg_fn, const uint32_t* val_type,
+    const uint32_t* val_off, const int32_t* val_null_field, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_off,
+    uint64_t* dst_len, uint64_t* dst_total, uint64_t* checksum_out, int32_t* status, uint64_t* n_groups);
+
 /* ---- write side, range-partitioned rows: Spark's RangePartitioner ids computed on the GPU ----
  * b2s_partition_compress_* for a RangePartitioning exchange of UnsafeRows (a global ORDER BY's map side): the reduce id
  * of every record is what Spark's RangePartitioner.getPartition returns for its sort key over the n_bounds range

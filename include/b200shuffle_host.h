@@ -136,6 +136,14 @@ int b2sh_serialized_writer_range_rows(b2sh_serialized_writer* w, uint32_t n_keys
  * order with Spark's ids.  With the exchange cache on, the call is its cached form, as for hash_rows. */
 int b2sh_serialized_writer_round_robin_rows(b2sh_serialized_writer* w, uint32_t num_partitions, int32_t start_position,
                                             uint32_t sort_rows);
+/* The partial aggregation of a grouped aggregation's map side (INTEGRATION.md §3p), set after hash_rows and before the
+ * first insert: commit() makes one b2s_aggregate_partition_compress_rows_hash_packed call with hash_rows' key columns and
+ * these n_aggs functions (agg_fn, val_type, val_off, val_null_field as that call takes them; copied), which groups the
+ * rows, folds Spark's aggregation buffers and hash-partitions one partial row per key on the GPU.  The files hold those
+ * partial rows as hash_rows' files would.  The call has no exchange-cache form: with the cache on it is the same call. */
+int b2sh_serialized_writer_aggregate_rows(b2sh_serialized_writer* w, uint32_t n_aggs, const uint32_t* agg_fn,
+                                          const uint32_t* val_type, const uint32_t* val_off,
+                                          const int32_t* val_null_field);
 int b2sh_serialized_writer_insert(b2sh_serialized_writer* w, int32_t partition_id, const uint8_t* bytes, uint64_t len);
 int b2sh_serialized_writer_commit(b2sh_serialized_writer* w, int64_t* partition_lengths_out);
 int b2sh_serialized_writer_statistics(b2sh_serialized_writer* w, uint64_t* bytes, uint64_t* nanos, char* line,

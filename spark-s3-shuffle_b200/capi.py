@@ -106,6 +106,12 @@ PROTOTYPES = [
     ("b2s_partition_compress_rows_hash_dev", C.c_int,
      [_u32, _u32, _i32, _u32, _u32, _u32, _u64, _vp, _u64, _u32p, _u32, _u32p, _u32p, _u32p, _i32p, _vp, _u64, _u64p,
       _u64p, _u64p, _u64p, _i32p]),
+    ("b2s_aggregate_partition_compress_rows_hash_packed", C.c_int,
+     [_u32, _i32, _u32, _u32, _u32, _u64, _u8p, _u64, _u32p, _u32, _u32p, _u32p, _u32p, _i32p, _u32, _u32p, _u32p, _u32p,
+      _i32p, _u8p, _u64, _u64p, _u64p, _u64p, _u64p, _i32p, _u64p]),
+    ("b2s_aggregate_partition_compress_rows_hash_dev", C.c_int,
+     [_u32, _u32, _i32, _u32, _u32, _u32, _u64, _vp, _u64, _u32p, _u32, _u32p, _u32p, _u32p, _i32p, _u32, _u32p, _u32p,
+      _u32p, _i32p, _vp, _u64, _u64p, _u64p, _u64p, _u64p, _i32p, _u64p]),
     ("b2s_partition_compress_rows_range_packed", C.c_int,
      [_u32, _i32, _u32, _u32, _u64, _u8p, _u64, _u32p, _u32, _u32p, _u32p, _u32p, _i32p, _u32, _u8p, _u64, _u32p,
       _u8p, _u64, _u64p, _u64p, _u64p, _u64p, _i32p]),
@@ -884,6 +890,51 @@ def partition_compress_rows_hash_dev(codec, d_records, rec_bytes, d_rec_len, n_r
         _ptr(kt), _ptr(ko), _ptr(kl), _ptr(kn), d_dst, dst_cap, _ptr(dst_off), _ptr(dst_len), C.addressof(total),
         _ptr(cks), _ptr(st)), "b2s_partition_compress_rows_hash_dev")
     return dict(dst_off=dst_off, dst_len=dst_len, total=total.value, checksums=cks, status=st)
+
+
+def _partial_agg_arrays(aggs):
+    """aggs = [(fn, val_type, val_off, val_null_field), ...]: WINDOW_SUM / COUNT / MIN / MAX / AVG, WINDOW_VAL_* or
+    window_val_decimal(p, s) -> (n, fn, val_type, val_off, val_null_field) arrays"""
+    aggs = list(aggs)
+    cols = list(zip(*aggs)) if aggs else [[0]] * 4
+    fn, vt, vo, vn = (np.array(c, dtype=t) for c, t in zip(cols, (np.uint32, np.uint32, np.uint32, np.int32)))
+    return len(aggs), fn, vt, vo, vn
+
+
+def aggregate_partition_compress_rows_hash_packed(codec, records, rec_len, keys, aggs, num_partitions, dst,
+                                                  block_size=0, checksum_alg=CHECKSUM_NONE, level=0):
+    """Spark's HashAggregateExec(Partial) and its hash exchange: the serialized UnsafeRows grouped by the key columns
+    (as in partition_compress_rows_hash_packed), the aggregation buffers of aggs (_partial_agg_arrays) folded per key,
+    one partial row per key, hash-partitioned and compressed.  -> dict(dst_off, dst_len, total, checksums, status,
+    n_groups)"""
+    records, dst = _as_u8(records), _as_u8(dst)
+    rec_len = np.ascontiguousarray(rec_len, dtype=np.uint32)
+    nk, kt, ko, kl, kn = _key_arrays(keys)
+    na, fn, vt, vo, vn = _partial_agg_arrays(aggs)
+    dst_off, dst_len, cks, st = _partition_out(num_partitions)
+    total, groups = _u64(0), _u64(0)
+    _check(load().b2s_aggregate_partition_compress_rows_hash_packed(
+        codec, level, block_size, checksum_alg, num_partitions, rec_len.size, _ptr(records), records.size,
+        _ptr(rec_len), nk, _ptr(kt), _ptr(ko), _ptr(kl), _ptr(kn), na, _ptr(fn), _ptr(vt), _ptr(vo), _ptr(vn),
+        _ptr(dst), dst.size, _ptr(dst_off), _ptr(dst_len), C.addressof(total), _ptr(cks), _ptr(st),
+        C.addressof(groups)), "b2s_aggregate_partition_compress_rows_hash_packed")
+    return dict(dst_off=dst_off, dst_len=dst_len, total=total.value, checksums=cks, status=st, n_groups=groups.value)
+
+
+def aggregate_partition_compress_rows_hash_dev(codec, d_records, rec_bytes, d_rec_len, n_records, keys, aggs,
+                                               num_partitions, d_dst, dst_cap, block_size=0,
+                                               checksum_alg=CHECKSUM_NONE, level=0, dev=0):
+    """aggregate_partition_compress_rows_hash_packed on device addresses (records, u32 lengths, destination arena)"""
+    nk, kt, ko, kl, kn = _key_arrays(keys)
+    na, fn, vt, vo, vn = _partial_agg_arrays(aggs)
+    dst_off, dst_len, cks, st = _partition_out(num_partitions)
+    total, groups = _u64(0), _u64(0)
+    _check(load().b2s_aggregate_partition_compress_rows_hash_dev(
+        dev, codec, level, block_size, checksum_alg, num_partitions, n_records, d_records, rec_bytes, d_rec_len, nk,
+        _ptr(kt), _ptr(ko), _ptr(kl), _ptr(kn), na, _ptr(fn), _ptr(vt), _ptr(vo), _ptr(vn), d_dst, dst_cap,
+        _ptr(dst_off), _ptr(dst_len), C.addressof(total), _ptr(cks), _ptr(st), C.addressof(groups)),
+        "b2s_aggregate_partition_compress_rows_hash_dev")
+    return dict(dst_off=dst_off, dst_len=dst_len, total=total.value, checksums=cks, status=st, n_groups=groups.value)
 
 
 def _bound_arrays(bounds):

@@ -251,6 +251,7 @@ struct Slot {
   DevBuf pws, parena;  // partition workspace (sort keys, offsets) and the partitioned arena in front of compression
   DevBuf xpieces;      // the copy pieces of an exchange-cache read (exchange.cu)
   DevBuf fws;          // row framing workspace: bitmap over the decoded arena, tile counts, verdicts (rows.cu)
+  DevBuf aggrows;      // a partial aggregation's partial rows, in front of the partition step (partial_agg.cu)
   PinBuf hmeta;
   // per-launch event pairs around the dominant kernel of a call (grow-only pool; dom_used pairs of call dom_call)
   std::vector<cudaEvent_t> ev_dom;
@@ -313,7 +314,7 @@ struct Slot {
   }
   // frees whatever the slot holds (buffers, events, streams); a slot that was never created holds nothing
   void release() {
-    for (DevBuf* b : {&meta, &scratch, &desc, &src, &dst, &zmeta, &pws, &parena, &xpieces, &fws}) b->release();
+    for (DevBuf* b : {&meta, &scratch, &desc, &src, &dst, &zmeta, &pws, &parena, &xpieces, &fws, &aggrows}) b->release();
     hmeta.release();
     for (cudaEvent_t* e : events())
       if (*e) cudaEventDestroy(*e);
@@ -822,7 +823,7 @@ int get_device(uint32_t dev_index, Device** out) {
 }
 
 // the kinds of call whose steps add_times reads into b2s_last_timing, one rule each
-enum class Family { kCodec, kPartition, kPartitionNone, kSort, kSortRows, kAggregate, kJoin, kWindow };
+enum class Family { kCodec, kPartition, kPartitionNone, kSort, kSortRows, kAggregate, kJoin, kWindow, kPartialAggregate };
 
 // Adds the times of this call's steps on S to b2s_last_timing: kernel_ms, top_kernel_ms, dominant_ms / _launches by
 // the rule of its family, and h2d_ms.  A step the call did not run reads 0; one it started but did not finish ends
@@ -860,6 +861,12 @@ void add_times(Slot& S, Family f) {
         dominant(F2, F3);
       }
       if (f == Family::kAggregate || f == Family::kJoin || f == Family::kWindow) dominant(G0, G1);
+      break;
+    case Family::kPartialAggregate:  // aggregation + partition step + compression (or checksums); the codec step (or
+                                     // the partition step); the aggregation step
+      t.kernel_ms += S.span(G0, S.mine(K1) ? K1 : P1);
+      t.top_kernel_ms += S.mine(T0) ? S.span(T0, T1) : S.span(P0, P1);
+      dominant(G0, G1);
       break;
   }
   t.h2d_ms += S.span(H0, H1);
@@ -3037,6 +3044,306 @@ int b2s_partition_compress_rows_hash_dev(uint32_t dev_index, uint32_t codec, int
 }
 
 // ------------------------------------------------------------------------------------------------------------
+// write side, partial aggregation: a map task's rows grouped by key, Spark's buffers folded, one partial row per key,
+// then the hash call's partition + compress step over the partial rows
+// ------------------------------------------------------------------------------------------------------------
+// The buffers of the n_aggs functions (each function's in Spark's aggBufferAttributes order) as the device folds them,
+// checked before the device: the function, its input type, the buffer count, the value slot and null bit.
+static int partial_agg_args(uint32_t n_aggs, const uint32_t* fn, const uint32_t* val_type, const uint32_t* val_off,
+                            const int32_t* val_null, PartialAggSpec* out) {
+  PartialAggSpec& s = *out;
+  if (n_aggs > kMaxAggs) return fail(B2S_E_ARG, "n_aggs must be at most 16%s");
+  if (n_aggs && (!fn || !val_type || !val_off || !val_null)) return fail(B2S_E_ARG, "null argument%s");
+  auto add = [&](uint32_t op, uint32_t stage, uint32_t vt, uint32_t off, int32_t nf, bool to_double) {
+    if (s.n_bufs == kMaxAggs) return false;
+    const uint32_t k = s.n_bufs++;
+    s.op[k] = op;
+    s.stage[k] = stage;
+    s.to_double[k] = to_double;
+    s.vtype[k] = vt;
+    s.voff[k] = off;
+    s.vnull[k] = nf;
+    if (agg_base_op(op) >= B2S_AGG_SUM_DECIMAL) s.wide[k] = s.n_dec++;
+    s.dsum |= op == B2S_AGG_SUM_FLOAT64;
+    return true;
+  };
+  for (uint32_t a = 0; a < n_aggs; a++) {
+    const uint32_t f = fn[a], vt = val_type[a], kind = vt & 0xff, p = (vt >> 8) & 0xff, sc = vt >> 16;
+    if (f < B2S_WINDOW_SUM || f > B2S_WINDOW_AVG) return fail(B2S_E_ARG, "unknown aggregate function%s");
+    if (kind > B2S_WINDOW_VAL_BYTES || (kind != B2S_WINDOW_VAL_DECIMAL && (vt >> 8)) || (vt >> 24))
+      return fail(B2S_E_ARG, "unknown val_type%s");
+    if (kind == B2S_WINDOW_VAL_DECIMAL && (p < 1 || p > 38 || sc > p))
+      return fail(B2S_E_ARG, "a decimal input needs 1 <= p <= 38 and s <= p%s");
+    const bool none = kind == B2S_WINDOW_VAL_NONE, bytes = kind == B2S_WINDOW_VAL_BYTES;
+    const bool dec = kind == B2S_WINDOW_VAL_DECIMAL, fp = kind == B2S_WINDOW_VAL_FLOAT32 || kind == B2S_WINDOW_VAL_FLOAT64;
+    if ((none || bytes) && f != B2S_WINDOW_COUNT)
+      return fail(B2S_E_ARG, "only COUNT takes B2S_WINDOW_VAL_NONE or B2S_WINDOW_VAL_BYTES%s");
+    if (!none) {
+      if (val_off[a] < 8 || val_off[a] % 8)
+        return fail(B2S_E_ARG, "val_off must be a field's 8-byte slot (a multiple of 8, past the null words)%s");
+      if (val_null[a] < -1 || val_null[a] >= 65536)
+        return fail(B2S_E_ARG, "val_null_field must be -1 or a field ordinal below 65536%s");
+    }
+    const uint32_t off = none ? 0 : val_off[a];
+    const int32_t nf = none ? -1 : val_null[a];
+    bool ok = true;
+    switch (f) {
+      case B2S_WINDOW_SUM:
+        if (dec) {
+          if (p > 28) return fail(B2S_E_ARG, "a decimal SUM input needs p <= 28 (its buffer is decimal(p + 10))%s");
+          ok = add(B2S_AGG_SUM_DECIMAL | (p + 10) << 8, kStageZero, vt, off, nf, false) &&
+               add(B2S_AGG_MIN_INT32, kStageIsEmpty, vt, off, nf, false);
+        } else {
+          ok = add(fp ? B2S_AGG_SUM_FLOAT64 : B2S_AGG_SUM_INT64, kStageValue, vt, off, nf, false);
+        }
+        break;
+      case B2S_WINDOW_COUNT:
+        ok = add(B2S_AGG_SUM_INT64, kStageCount, vt, off, nf, false);
+        break;
+      case B2S_WINDOW_AVG:
+        if (dec) {
+          if (p > 27) return fail(B2S_E_ARG, "a decimal AVG input needs p <= 27 (Average adds with Add)%s");
+          ok = add(B2S_AGG_SUM_DECIMAL | (p + 10) << 8, kStageZero, vt, off, nf, false);
+        } else {
+          ok = add(B2S_AGG_SUM_FLOAT64, kStageZero, vt, off, nf, true);
+        }
+        ok = ok && add(B2S_AGG_SUM_INT64, kStageCount, vt, off, nf, false);
+        break;
+      default: {  // MIN, MAX
+        const bool mx = f == B2S_WINDOW_MAX;
+        uint32_t op;
+        if (kind == B2S_WINDOW_VAL_INT32) op = mx ? B2S_AGG_MAX_INT32 : B2S_AGG_MIN_INT32;
+        else if (kind == B2S_WINDOW_VAL_INT64 || (dec && p <= 18)) op = mx ? B2S_AGG_MAX_INT64 : B2S_AGG_MIN_INT64;
+        else if (kind == B2S_WINDOW_VAL_FLOAT64) op = mx ? B2S_AGG_MAX_FLOAT64 : B2S_AGG_MIN_FLOAT64;
+        else if (dec) op = mx ? B2S_AGG_MAX_DECIMAL : B2S_AGG_MIN_DECIMAL;
+        else
+          return fail(B2S_E_ARG, "MIN and MAX take an int, long, double or decimal input (the reduce side merges no "
+                                 "other)%s");
+        ok = add(op, kStageValue, vt, off, nf, false);
+      }
+    }
+    if (!ok) return fail(B2S_E_ARG, "more than 16 aggregation buffers (the reduce-side merge's limit)%s");
+  }
+  return 0;
+}
+
+// The key columns as the partial rows hold them: column c is field c (slot 8 + 8 c, one null word), null bit c when the
+// input's column is nullable
+static KeySpec partial_row_keys(const KeySpec& in) {
+  KeySpec k = in;
+  for (uint32_t c = 0; c < in.n; c++) {
+    k.off[c] = 8 + 8 * c;
+    k.null_field[c] = in.null_field[c] >= 0 ? (int32_t)c : -1;
+  }
+  return k;
+}
+
+// The aggregation step on S over n device-resident records (d_rec, rec_bytes; d_len): offsets, checks (one readback:
+// a bad record or a wrong byte total fails the call), the key sort and its refinement rounds, the grouping, the folds
+// (one readback: groups, partial-row bytes) and the partial rows into S.aggrows, their record lengths at *row_len (in
+// S.fws).  Marks G0, G1.
+static int partial_agg_rows(Slot& S, const PartialAggSpec& spec, uint64_t n, const uint8_t* d_rec, uint64_t rec_bytes,
+                            const uint32_t* d_len, uint64_t* groups, uint64_t* out_bytes, const uint32_t** row_len,
+                            uint64_t* launches) {
+  cudaStream_t st = S.st;
+  const KeySpec& ks = spec.keys;
+  const uint32_t key_bytes = rows_key_bytes(ks);
+  const bool refine = rows_key_refines(ks);
+  const size_t part[4] = {rows_sort_ws_bytes(n, key_bytes), refine ? rows_refine_ws_bytes(n, 1) : 0,
+                          rows_aggregate_ws_bytes(n, 0, 0), partial_agg_ws_bytes(n, spec)};
+  if (int rc = S.fws.ensure(part[0] + part[1] + part[2] + part[3])) return rc;
+  uint8_t* ws = (uint8_t*)S.fws.p;
+  uint8_t *rws = refine ? ws + part[0] : nullptr, *gws = ws + part[0] + part[1], *paws = gws + part[2];
+  uint64_t* hdr = partial_agg_header(paws);
+  *row_len = partial_agg_row_len(paws, n, spec);
+  if (int rc = S.hmeta.ensure(48)) return rc;
+  uint64_t* rb = (uint64_t*)S.hmeta.p;
+  CU(S.mark(G0, st, *launches));
+  launch_partial_agg_offsets(d_len, n, key_bytes, ws, paws, st, launches);
+  launch_partial_agg_check(d_rec, rec_bytes, n, key_bytes, spec, ws, paws,
+                           (uint32_t*)partial_agg_row_len(paws, n, spec), st, launches);
+  CU(cudaMemcpyAsync(rb, hdr, 24, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  CU(cudaGetLastError());
+  if (rb[0] != ~0ull) {
+    if ((rb[0] & 7) != kPaBadValue) return row_ids_verdict(RowIds{ks}, rb[0]);
+    static const char* const why[] = {"", "its row does not hold a value slot", "its row does not hold a value's null word",
+                                      "a decimal value's size is not 1..16 or it runs past its row"};
+    char msg[256];
+    snprintf(msg, sizeof msg, "record %llu is not a serialized row of the aggregated columns: %s",
+             (unsigned long long)(rb[0] >> 3), why[rb[2] & 3]);
+    return fail(B2S_E_ARG, "%s", msg);
+  }
+  if (rb[1] != rec_bytes) {
+    char msg[256];
+    const KeySortWs w = carve_key_sort_ws(ws, n, key_bytes);
+    if (rb[1] > rec_bytes)
+      snprintf(msg, sizeof msg, "rec_len sums to %llu bytes, rec_bytes is %llu: record %llu ends past rec_bytes",
+               (unsigned long long)rb[1], (unsigned long long)rec_bytes,
+               (unsigned long long)first_record_past(w.src_off, w.len, n, rec_bytes));
+    else
+      snprintf(msg, sizeof msg, "rec_len sums to %llu bytes, rec_bytes is %llu", (unsigned long long)rb[1],
+               (unsigned long long)rec_bytes);
+    return fail(B2S_E_ARG, "%s", msg);
+  }
+  *groups = *out_bytes = 0;
+  if (!n) {
+    CU(S.mark(G1, st, *launches));
+    return 0;
+  }
+  const uint32_t* idx = launch_rows_order(d_rec, n, ks, hdr + 3, 1, ws, rws, st, launches);
+  const uint32_t* heads = nullptr;
+  if (refine) {  // the key columns were checked, so no round finds a bad string or decimal
+    for (uint32_t d = kKeyPrefixBytes;; d += kKeyChunkBytes) {
+      launch_rows_refine_mark(n, d, rws, 1, st, launches);
+      CU(cudaMemcpyAsync(rb, rows_refine_readback(rws, n, 1), 8, cudaMemcpyDeviceToHost, st));
+      CU(cudaStreamSynchronize(st));
+      CU(cudaGetLastError());
+      const uint64_t tied = rb[0] & 0xffffffffull, runs = rb[0] >> 32;
+      if (!tied) break;
+      launch_rows_refine_round(d_rec, n, ks, tied, runs, d, ws, rws, 1, st, launches);
+    }
+    idx = rows_refine_order(rws, n, 1);
+    heads = rows_refine_heads(rws, n, 1);
+  }
+  launch_rows_group(d_rec, n, idx, heads, key_bytes, AggSpec{}, ws, gws, st, launches);
+  launch_partial_agg_fold(d_rec, n, idx, key_bytes, spec, ws, gws, paws, st, launches);
+  CU(cudaMemcpyAsync(rb, hdr + 4, 16, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  CU(cudaGetLastError());
+  *groups = rb[0];
+  *out_bytes = rb[1];
+  if (int rc = S.aggrows.ensure(rb[1] + 64)) return rc;
+  launch_partial_agg_emit(d_rec, n, rb[0], idx, key_bytes, spec, ws, gws, paws, (uint8_t*)S.aggrows.p, st, launches);
+  CU(S.mark(G1, st, *launches));
+  return 0;
+}
+
+// the largest whole-task buffer a call keeps for the next one (SortBufferTrim, PartialAggTrim)
+constexpr size_t kSortKeepBytes = 1ull << 30;
+
+// The aggregation step's buffers, sized by the call's records (staged and folded values, the partial rows), are given
+// back when the call ends if they are larger than the sorts keep, so one large map task does not hold them for the life
+// of the process
+struct PartialAggTrim {
+  Slot& S;
+  ~PartialAggTrim() {
+    for (DevBuf* b : {&S.fws, &S.aggrows})
+      if (b->cap > kSortKeepBytes) b->release();
+  }
+};
+
+// b2s_aggregate_partition_compress_rows_hash_*: the checks before the device, then on the write lane the aggregation
+// step and the partition + compress step over the partial rows, from host records (packed: one upload, one download)
+// or device ones
+static int aggregate_partition_call(bool packed, uint32_t dev_index, uint32_t codec, int32_t level,
+                                    uint32_t codec_block_size, uint32_t checksum_alg, uint32_t num_partitions,
+                                    uint64_t n_records, const uint8_t* rec_base, uint64_t rec_bytes,
+                                    const uint32_t* rec_len, uint32_t n_keys, const uint32_t* key_type,
+                                    const uint32_t* key_off, const uint32_t* key_len, const int32_t* key_null_field,
+                                    uint32_t n_aggs, const uint32_t* agg_fn, const uint32_t* val_type,
+                                    const uint32_t* val_off, const int32_t* val_null_field, uint8_t* dst_base,
+                                    uint64_t dst_cap, uint64_t* dst_off, uint64_t* dst_len, uint64_t* dst_total,
+                                    uint64_t* checksum_out, int32_t* status, uint64_t* n_groups) {
+  const WallTimer wt = begin_call();
+  if (dst_total) *dst_total = 0;
+  if (n_groups) *n_groups = 0;
+  const RecordSpec rspec = keys_spec(n_keys, key_type, key_off, key_len, key_null_field);
+  PartialAggSpec spec;
+  spec.keys = rspec.keys;
+  if (!n_groups) return fail(B2S_E_ARG, "null argument%s");
+  if (int rc = partial_agg_args(n_aggs, agg_fn, val_type, val_off, val_null_field, &spec)) return rc;
+  if (int rc = hash_args(codec, codec_block_size, checksum_alg, num_partitions, n_records, rec_base, rec_bytes, rec_len,
+                         rspec, dst_base, dst_off, dst_len, status))
+    return rc;
+  const uint32_t bs = block_size_or_default(codec_block_size);
+  if (!n_records && rec_bytes)
+    return fail(B2S_E_ARG, "rec_len sums to 0 bytes, rec_bytes is %s", std::to_string(rec_bytes).c_str());
+  Device* D;
+  if (int rc = get_device(packed ? t_device : dev_index, &D)) return rc;
+  Lane& Ln = D->lane[kLaneWrite];
+  std::lock_guard<std::mutex> lk(Ln.mtx);
+  Slot& S = Ln.slot[0];
+  const PartialAggTrim trim{S};
+  cudaStream_t st = S.st;
+  const uint8_t* d_rec = rec_base;
+  const uint32_t* d_len = rec_len;
+  if (packed) {  // one upload of [records | rec_len]
+    const size_t rec_sz = align_up(rec_bytes, 16), len_sz = align_up(n_records * 4, 16);
+    if (int rc = S.src.ensure(rec_sz + len_sz + 64)) return rc;
+    d_rec = (const uint8_t*)S.src.p;
+    d_len = (const uint32_t*)((uint8_t*)S.src.p + rec_sz);
+    CU(S.mark(H0, st));
+    if (rec_bytes) CU(cudaMemcpyAsync((uint8_t*)S.src.p, rec_base, rec_bytes, cudaMemcpyHostToDevice, st));
+    if (n_records) CU(cudaMemcpyAsync((uint8_t*)d_len, rec_len, n_records * 4, cudaMemcpyHostToDevice, st));
+    CU(S.mark(H1, st));
+  }
+  uint64_t launches = 0, groups = 0, rows_bytes = 0, arena = 0;
+  const uint32_t* d_row_len = nullptr;
+  int rc = partial_agg_rows(S, spec, n_records, d_rec, rec_bytes, d_len, &groups, &rows_bytes, &d_row_len, &launches);
+  if (rc) return rc;
+  const RowIds ids{partial_row_keys(spec.keys)};
+  uint8_t* d_dst = dst_base;
+  uint64_t cap = dst_cap;
+  if (packed) {  // sized by the bound: a short caller arena shows up after the run, as in the packed partition call
+    if ((rc = S.dst.ensure(b2s_partition_compress_bound(codec, bs, num_partitions, rows_bytes) + 64))) return rc;
+    d_dst = (uint8_t*)S.dst.p;
+    cap = S.dst.cap;
+  }
+  std::vector<uint64_t> cks(num_partitions);
+  rc = partition_compress_run(D, S, codec, level, bs, checksum_alg, num_partitions, groups,
+                              (const uint8_t*)S.aggrows.p, rows_bytes, d_row_len, nullptr, d_dst, cap, dst_off, dst_len,
+                              cks.data(), status, &arena, &launches, nullptr, &ids);
+  if (rc && rc != B2S_E_DST_TOO_SMALL) return rc;
+  uint64_t fit = 0;
+  if (packed) {
+    fit = std::min(arena, dst_cap);
+    if (arena > dst_cap) {
+      for (uint32_t p = 0; p < num_partitions; p++)
+        if (dst_len[p] && dst_off[p] + dst_len[p] > dst_cap) status[p] = B2S_E_DST_TOO_SMALL;
+      rc = fail(B2S_E_DST_TOO_SMALL, "dst_cap is below the %s bytes of the .data arena", std::to_string(arena).c_str());
+    }
+    CU(S.mark(D0, st));
+    if (fit) CU(cudaMemcpyAsync(dst_base, S.dst.p, fit, cudaMemcpyDeviceToHost, st));
+    CU(S.mark(D1, st));
+    CU(cudaStreamSynchronize(st));
+    CU(cudaGetLastError());
+  }
+  if (checksum_out) memcpy(checksum_out, cks.data(), (size_t)num_partitions * 8);
+  if (dst_total) *dst_total = arena;
+  *n_groups = groups;
+  end_call(wt, launches, CallBytes{rec_bytes, arena, packed ? rec_bytes + n_records * 4 : 0, fit}, &S,
+           Family::kPartialAggregate);
+  return rc;
+}
+
+int b2s_aggregate_partition_compress_rows_hash_packed(
+    uint32_t codec, int32_t level, uint32_t codec_block_size, uint32_t checksum_alg, uint32_t num_partitions,
+    uint64_t n_records, const uint8_t* rec_base, uint64_t rec_bytes, const uint32_t* rec_len, uint32_t n_keys,
+    const uint32_t* key_type, const uint32_t* key_off, const uint32_t* key_len, const int32_t* key_null_field,
+    uint32_t n_aggs, const uint32_t* agg_fn, const uint32_t* val_type, const uint32_t* val_off,
+    const int32_t* val_null_field, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_off, uint64_t* dst_len,
+    uint64_t* dst_total, uint64_t* checksum_out, int32_t* status, uint64_t* n_groups) {
+  return aggregate_partition_call(true, 0, codec, level, codec_block_size, checksum_alg, num_partitions, n_records,
+                                  rec_base, rec_bytes, rec_len, n_keys, key_type, key_off, key_len, key_null_field,
+                                  n_aggs, agg_fn, val_type, val_off, val_null_field, dst_base, dst_cap, dst_off,
+                                  dst_len, dst_total, checksum_out, status, n_groups);
+}
+
+int b2s_aggregate_partition_compress_rows_hash_dev(
+    uint32_t dev_index, uint32_t codec, int32_t level, uint32_t codec_block_size, uint32_t checksum_alg,
+    uint32_t num_partitions, uint64_t n_records, const uint8_t* rec_base, uint64_t rec_bytes, const uint32_t* rec_len,
+    uint32_t n_keys, const uint32_t* key_type, const uint32_t* key_off, const uint32_t* key_len,
+    const int32_t* key_null_field, uint32_t n_aggs, const uint32_t* agg_fn, const uint32_t* val_type,
+    const uint32_t* val_off, const int32_t* val_null_field, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_off,
+    uint64_t* dst_len, uint64_t* dst_total, uint64_t* checksum_out, int32_t* status, uint64_t* n_groups) {
+  return aggregate_partition_call(false, dev_index, codec, level, codec_block_size, checksum_alg, num_partitions,
+                                  n_records, rec_base, rec_bytes, rec_len, n_keys, key_type, key_off, key_len,
+                                  key_null_field, n_aggs, agg_fn, val_type, val_off, val_null_field, dst_base, dst_cap,
+                                  dst_off, dst_len, dst_total, checksum_out, status, n_groups);
+}
+
+// ------------------------------------------------------------------------------------------------------------
 // write side, range-partitioned rows: Spark's RangePartitioner id of every row, then the partition + compress step
 // ------------------------------------------------------------------------------------------------------------
 // The composite calls' column rules (order flags allowed), the partition step's checks with n_bounds + 1 partitions,
@@ -3240,7 +3547,6 @@ int b2s_partition_compress_rows_round_robin_dev(uint32_t dev_index, uint32_t cod
 // workspace) only grow while they are in use.  When a call ends — whatever its result — every one of them above
 // kSortKeepBytes is freed, so one oversized task does not keep several times its size of device memory for the rest
 // of the process; buffers up to that size stay for the next call (a TeraSort reducer of 200 over 10 GiB needs ~55 MB).
-constexpr size_t kSortKeepBytes = 1ull << 30;
 struct SortBufferTrim {
   Slot& S;
   ~SortBufferTrim() {

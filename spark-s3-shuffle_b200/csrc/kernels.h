@@ -480,6 +480,55 @@ void launch_rows_aggregate(const uint8_t* arena, uint64_t n, uint64_t groups, ui
 const uint64_t* rows_group_heads_before(uint8_t* d_aws, uint64_t n);
 const uint32_t* rows_group_starts(uint8_t* d_aws, uint64_t n);
 
+// ---------------- partial_agg.cu (a map task's partial aggregation: one partial row per key) ----------------
+// The caller's records ([size: int32 big-endian][row], rec_len each, back to back), sorted by the key columns keys
+// (launch_rows_order) and grouped (launch_rows_group, an AggSpec of no aggregates, in d_gws).  Buffer k < n_bufs:
+// merge op op[k] (B2S_AGG_*; SUM_DECIMAL | P << 8), staged from its input (B2S_WINDOW_VAL_* vtype[k], a decimal's p in
+// bits 8..15; slot voff[k], null bit vnull[k] or -1) by stage[k]: kStageValue the value (a null is skipped),
+// kStageZero the value or 0 when null (to_double[k]: an integer cast to double, rounded to nearest), kStageCount 1 per
+// non-null input (every input for VAL_NONE), kStageIsEmpty 1 per null input.  A decimal buffer (op >= SUM_DECIMAL) is
+// staged in 128 bits: wide[k] is its index among the n_dec of them.  dsum: some buffer is a double sum.
+constexpr uint32_t kStageValue = 0, kStageZero = 1, kStageCount = 2, kStageIsEmpty = 3;
+struct PartialAggSpec {
+  KeySpec keys;
+  uint32_t n_bufs = 0;
+  uint32_t op[kMaxAggs] = {};
+  uint32_t stage[kMaxAggs] = {};
+  uint32_t to_double[kMaxAggs] = {};
+  uint32_t vtype[kMaxAggs] = {};
+  uint32_t voff[kMaxAggs] = {};
+  int32_t vnull[kMaxAggs] = {};
+  uint32_t wide[kMaxAggs] = {};
+  uint32_t n_dec = 0;
+  bool dsum = false;
+};
+// the check verdict (header word 0) of a record whose value is bad: (i << 3) | kPaBadValue, beside launch_rows_hash's
+// kHashBad* reasons; header word 2 then holds (i << 2) | kPaBadSlot, kPaBadNull or kPaBadDecimal
+constexpr uint64_t kPaBadValue = 7, kPaBadSlot = 1, kPaBadNull = 2, kPaBadDecimal = 3;
+size_t partial_agg_ws_bytes(uint64_t n, const PartialAggSpec& spec);
+// the workspace's header (device): [check verdict (~0: none), record bytes, check detail (~0: none), 0 (the one range's
+// offset), groups, partial-row bytes]
+uint64_t* partial_agg_header(uint8_t* d_paws);
+// the record offsets: rec_len scanned into the sort workspace d_ws (key_bytes: its key width), as launch_rows_emit
+// leaves them; their total into header word 1.  Resets the header.
+void launch_partial_agg_offsets(const uint32_t* rec_len, uint64_t n, uint32_t key_bytes, uint8_t* d_ws,
+                                uint8_t* d_paws, cudaStream_t st, uint64_t* launches);
+// every record checked (its framing and key columns by launch_rows_hash, into ids, n u32 of scratch; its values here):
+// the lowest bad record into header words 0 and 2
+void launch_partial_agg_check(const uint8_t* rec, uint64_t rec_bytes, uint64_t n, uint32_t key_bytes,
+                              const PartialAggSpec& spec, uint8_t* d_ws, uint8_t* d_paws, uint32_t* ids,
+                              cudaStream_t st, uint64_t* launches);
+// after launch_rows_group: staging, the folds, the partial rows' lengths and offsets; header words 4, 5
+void launch_partial_agg_fold(const uint8_t* rec, uint64_t n, const uint32_t* idx, uint32_t key_bytes,
+                             const PartialAggSpec& spec, uint8_t* d_ws, uint8_t* d_gws, uint8_t* d_paws,
+                             cudaStream_t st, uint64_t* launches);
+// per partial row its record length (4 + row), after launch_partial_agg_fold
+const uint32_t* partial_agg_row_len(uint8_t* d_paws, uint64_t n, const PartialAggSpec& spec);
+// the groups (count read back) as partial rows, [size: int32 big-endian][row] back to back, to d_dst
+void launch_partial_agg_emit(const uint8_t* rec, uint64_t n, uint64_t groups, const uint32_t* idx, uint32_t key_bytes,
+                             const PartialAggSpec& spec, uint8_t* d_ws, uint8_t* d_gws, uint8_t* d_paws,
+                             uint8_t* d_dst, cudaStream_t st, uint64_t* launches);
+
 // ---------------- join.cu (sort-merge join of a reducer's two sorted sides into Spark's joined UnsafeRows) -----------
 // The records of both sides, stably sorted together by the join key (launch_rows_join_order) and grouped
 // (launch_rows_group): each group holds its key's left records, then its right ones.  The shape of the joined row:

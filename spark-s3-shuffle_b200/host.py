@@ -93,6 +93,7 @@ PROTOTYPES = [
     ("b2sh_serialized_writer_hash_rows", C.c_int, [_vp, _u32, _vp, _vp, _vp, _vp]),
     ("b2sh_serialized_writer_range_rows", C.c_int, [_vp, _u32, _vp, _vp, _vp, _vp, _u32, _vp, _u64, _vp]),
     ("b2sh_serialized_writer_round_robin_rows", C.c_int, [_vp, _u32, _i32, _u32]),
+    ("b2sh_serialized_writer_aggregate_rows", C.c_int, [_vp, _u32, _vp, _vp, _vp, _vp]),
     ("b2sh_serialized_writer_insert", C.c_int, [_vp, _i32, _vp, _u64]),
     ("b2sh_serialized_writer_commit", C.c_int, [_vp, _vp]),
     ("b2sh_serialized_writer_statistics", C.c_int, [_vp, C.POINTER(_u64), C.POINTER(_u64), C.c_char_p, _u32]),
@@ -321,6 +322,14 @@ class S3SerializedShuffleWriter:
         """RoundRobinPartitioning (Spark's repartition(n)) from startPosition, the rows sorted first when sortRows,
         before the first insert; numPartitions must be the writer's"""
         _check(load().b2sh_serialized_writer_round_robin_rows(self._h, numPartitions, startPosition, int(sortRows)))
+
+    def aggregateRows(self, aggs):
+        """the map side's partial aggregation, after hashRows and before the first insert: aggs = [(fn, val_type,
+        val_off, val_null_field), ...] as capi.aggregate_partition_compress_rows_hash_packed takes them; commit() writes
+        one partial row per key of hashRows' key columns, hash-partitioned"""
+        aggs = list(aggs)
+        arrs = [np.array([a[i] for a in aggs] or [0], dtype=np.int32 if i == 3 else np.uint32) for i in range(4)]
+        _check(load().b2sh_serialized_writer_aggregate_rows(self._h, len(aggs), *[a.ctypes.data for a in arrs]))
 
     def insertRecord(self, partitionId, record):
         a = np.frombuffer(record, dtype=np.uint8) if not isinstance(record, np.ndarray) else np.ascontiguousarray(record)

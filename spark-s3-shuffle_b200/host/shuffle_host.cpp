@@ -543,6 +543,23 @@ class S3SerializedShuffleWriter {
     rrStart_ = startPosition;
     rrSort_ = sortRows;
   }
+  // The partial aggregation of a grouped aggregation's map side (b2s_aggregate_partition_compress_rows_hash_packed):
+  // after hashRows and before the first insert; commit() groups the rows by hashRows' key columns, folds these
+  // functions' buffers and hash-partitions the partial rows on the GPU.  No cached form exists, so the call is the same
+  // with the exchange cache on.
+  void aggregateRows(uint32_t nAggs, const uint32_t* fn, const uint32_t* valType, const uint32_t* valOff,
+                     const int32_t* valNull) {
+    if (!recLen_.empty()) throw RuntimeException("Precondition: aggregate_rows must come before the first insert.");
+    if (keyType_.empty() || range_ || roundRobin_)
+      throw RuntimeException("Precondition: aggregate_rows needs hash_rows first.");
+    if (nAggs > 16) throw RuntimeException("Precondition: n_aggs must be at most 16.");
+    if (nAggs && (!fn || !valType || !valOff || !valNull)) throw RuntimeException("Precondition: null aggregate arrays.");
+    aggregate_ = true;
+    aggFn_.assign(fn, fn + nAggs);
+    aggType_.assign(valType, valType + nAggs);
+    aggOff_.assign(valOff, valOff + nAggs);
+    aggNull_.assign(valNull, valNull + nAggs);
+  }
   void insertRecord(int32_t partitionId, const uint8_t* b, uint64_t n) {
     const bool hashed = !keyType_.empty() || roundRobin_;
     if (!hashed && (partitionId < 0 || partitionId >= numPartitions_))
@@ -569,7 +586,21 @@ class S3SerializedShuffleWriter {
     const bool cache = d_.gpuExchangeCacheBytes != 0;
     if (cache) d_.applyExchangeBudget();
     int32_t cached = 0;
-    if (roundRobin_ && cache) {
+    if (aggregate_) {
+      // the partial rows' arena is not known before the call: the bound of the input's bytes first, then the exact
+      // size the call reports when that is short
+      call = "b2s_aggregate_partition_compress_rows_hash_packed";
+      uint64_t groups = 0;
+      for (int attempt = 0;; attempt++) {
+        rc = b2s_aggregate_partition_compress_rows_hash_packed(
+            codec, d_.zstdLevel, d_.lz4BlockSize, alg, R, recLen_.size(), records_.data(), records_.size(),
+            recLen_.data(), (uint32_t)keyType_.size(), keyType_.data(), keyOff_.data(), keyLen_.data(),
+            keyNull_.data(), (uint32_t)aggFn_.size(), aggFn_.data(), aggType_.data(), aggOff_.data(), aggNull_.data(),
+            out_.data(), out_.size(), doff.data(), dlen.data(), &total, cks.data(), status.data(), &groups);
+        if (rc != B2S_E_DST_TOO_SMALL || attempt) break;
+        out_.resize(total);
+      }
+    } else if (roundRobin_ && cache) {
       call = "b2s_partition_compress_rows_round_robin_cached_packed";
       rc = b2s_partition_compress_rows_round_robin_cached_packed(
           shuffleId_, mapId_, codec, d_.zstdLevel, d_.lz4BlockSize, alg, R, rrStart_, rrSort_, recLen_.size(),
@@ -642,6 +673,9 @@ class S3SerializedShuffleWriter {
   bool range_ = false;  // rangeRows: the ids are RangePartitioner ids over these bounds
   std::vector<uint8_t> boundRows_;
   std::vector<uint32_t> boundLen_;
+  bool aggregate_ = false;  // aggregateRows: the rows are aggregated by hashRows' key columns first
+  std::vector<uint32_t> aggFn_, aggType_, aggOff_;
+  std::vector<int32_t> aggNull_;
   bool roundRobin_ = false;  // roundRobinRows: Spark's repartition(n) order and ids from rrStart_
   int32_t rrStart_ = 0;
   uint32_t rrSort_ = 0;
@@ -1518,6 +1552,11 @@ int b2sh_serialized_writer_range_rows(b2sh_serialized_writer* w, uint32_t n_keys
 int b2sh_serialized_writer_round_robin_rows(b2sh_serialized_writer* w, uint32_t num_partitions, int32_t start_position,
                                             uint32_t sort_rows) {
   return guarded([&] { w->w->roundRobinRows(num_partitions, start_position, sort_rows); });
+}
+int b2sh_serialized_writer_aggregate_rows(b2sh_serialized_writer* w, uint32_t n_aggs, const uint32_t* agg_fn,
+                                          const uint32_t* val_type, const uint32_t* val_off,
+                                          const int32_t* val_null_field) {
+  return guarded([&] { w->w->aggregateRows(n_aggs, agg_fn, val_type, val_off, val_null_field); });
 }
 int b2sh_serialized_writer_insert(b2sh_serialized_writer* w, int32_t partition_id, const uint8_t* bytes, uint64_t len) {
   return guarded([&] { w->w->insertRecord(partition_id, bytes, len); });
