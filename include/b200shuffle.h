@@ -318,6 +318,61 @@ int b2s_aggregate_partition_compress_rows_hash_dev(
     const uint32_t* val_off, const int32_t* val_null_field, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_off,
     uint64_t* dst_len, uint64_t* dst_total, uint64_t* checksum_out, int32_t* status, uint64_t* n_groups);
 
+/* ---- write side, grouping sets: Spark's Expand and HashAggregateExec(Partial) and its hash exchange on the GPU ----
+ * The map side of a ROLLUP, CUBE or GROUPING SETS aggregation's shuffle (Expand -> HashAggregateExec(Partial) ->
+ * Exchange hashpartitioning(grouping columns, spark_grouping_id)) in one call.  The arguments are those of
+ * b2s_aggregate_partition_compress_rows_hash_* in the same order, with n_sets / set_mask after the aggregate arrays:
+ * bit c of set_mask[k] is set when key column c belongs to grouping set k.  The semantics are Spark 3.5's Expand
+ * followed by HashAggregateExec(Partial), ANSI off, spark.sql.legacy.integerGroupingId off:
+ * Input records: as for b2s_aggregate_partition_compress_rows_hash_*.  Record r stands for the n_sets projected records
+ * (r, k), in row-major order (0, 0), (0, 1), .., (1, 0), ..: ExpandExec's output order.  Every record of a group comes
+ * from one set, so each group's fold order is the input order.
+ * Projected record (r, k): key column c takes record r's value if bit c of set_mask[k] is set, and null otherwise; one
+ * more key column follows them: gid, a never-null long, the sum of 1 << (n_keys - 1 - c) over the columns c outside the
+ * set (Spark's spark_grouping_id: ROLLUP(a, b, c)'s sets give 0, 1, 3, 7; CUBE(a, b)'s 0, 1, 2, 3).  Aggregate inputs
+ * are read from record r unmasked: Spark's aggregate functions reference the child's attribute, not the nulled
+ * grouping alias.
+ * Partial rows: n_keys grouping columns, every one nullable, then gid (INT64, slot 8 + 8 n_keys), then the buffers, as
+ * UnsafeProjection(groupingAttributes ++ aggBufferAttributes) writes them; nf = n_keys + 1 + buffers <= 32.  They come
+ * in the composite-key order of (grouping columns ascending, nulls first; gid) and are partitioned by
+ * pmod(Murmur3Hash(grouping columns, gid; 42), num_partitions).
+ * Defining contract: dst_off / dst_len / checksum_out / status, *dst_total, *n_groups and the return value are byte for
+ * byte what b2s_aggregate_partition_compress_rows_hash_packed returns for the materialized Expand output in row-major
+ * order, keyed by the n_keys grouping columns (each with a real null bit) and gid (B2S_KEY_INT64, null bit -1), with the
+ * same aggregates at their projected slots.
+ * Errors, B2S_E_ARG, checked before the device: what b2s_aggregate_partition_compress_rows_hash_* rejects; n_keys outside
+ * 1..15 (gid takes the 16th key column); n_sets == 0 or a NULL set_mask; a mask bit at or above n_keys; two equal masks
+ * (Spark adds a _gen_grouping_pos column for duplicate sets); n_records * n_sets >= 2^32.  (n_keys + 1 + buffers is then
+ * at most 32.)  The empty set (mask 0, the grand total) and a single full set are allowed.  A bad record -> B2S_E_ARG
+ * naming its input index, for the reasons b2s_aggregate_partition_compress_rows_hash_* gives.  A record whose row,
+ * projected for a set (its in-set strings, 16 bytes per decimal(p > 18) key or input, 8 (2 + nf') bytes of fixed region),
+ * would pass 2^31 - 1 bytes -> B2S_E_UNSUPPORTED.  Device memory that cannot be had -> B2S_E_NOMEM (the caller keeps
+ * Spark's Expand and partial aggregation).  No usable device -> B2S_E_CUDA.
+ * Sizing: dst_cap below the arena -> B2S_E_DST_TOO_SMALL with *dst_total = the bytes needed.  The bound of
+ * b2s_aggregate_partition_compress_rows_hash_* with n_records and rec_bytes multiplied by n_sets and nf as above,
+ *   b2s_partition_compress_bound(codec, codec_block_size, num_partitions,
+ *                                n_sets * (n_records * (4 + 8 (1 + nf) + 16 W + 8 S) + S * rec_bytes))
+ * always suffices.
+ * Runs on the write lane.  b2s_last_timing: kernel_ms the whole call's device work, dominant_ms / dominant_launches the
+ * aggregation step, the expansion included. */
+int b2s_aggregate_grouping_sets_partition_compress_rows_hash_packed(
+    uint32_t codec, int32_t level, uint32_t codec_block_size, uint32_t checksum_alg, uint32_t num_partitions,
+    uint64_t n_records, const uint8_t* rec_base, uint64_t rec_bytes, const uint32_t* rec_len, uint32_t n_keys,
+    const uint32_t* key_type, const uint32_t* key_off, const uint32_t* key_len, const int32_t* key_null_field,
+    uint32_t n_aggs, const uint32_t* agg_fn, const uint32_t* val_type, const uint32_t* val_off,
+    const int32_t* val_null_field, uint32_t n_sets, const uint32_t* set_mask, uint8_t* dst_base, uint64_t dst_cap,
+    uint64_t* dst_off, uint64_t* dst_len, uint64_t* dst_total, uint64_t* checksum_out, int32_t* status,
+    uint64_t* n_groups);
+/* same, with rec_base / rec_len / dst_base in device memory of dev_index; the other arrays stay host arrays */
+int b2s_aggregate_grouping_sets_partition_compress_rows_hash_dev(
+    uint32_t dev_index, uint32_t codec, int32_t level, uint32_t codec_block_size, uint32_t checksum_alg,
+    uint32_t num_partitions, uint64_t n_records, const uint8_t* rec_base, uint64_t rec_bytes, const uint32_t* rec_len,
+    uint32_t n_keys, const uint32_t* key_type, const uint32_t* key_off, const uint32_t* key_len,
+    const int32_t* key_null_field, uint32_t n_aggs, const uint32_t* agg_fn, const uint32_t* val_type,
+    const uint32_t* val_off, const int32_t* val_null_field, uint32_t n_sets, const uint32_t* set_mask,
+    uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_off, uint64_t* dst_len, uint64_t* dst_total,
+    uint64_t* checksum_out, int32_t* status, uint64_t* n_groups);
+
 /* ---- write side, range-partitioned rows: Spark's RangePartitioner ids computed on the GPU ----
  * b2s_partition_compress_* for a RangePartitioning exchange of UnsafeRows (a global ORDER BY's map side): the reduce id
  * of every record is what Spark's RangePartitioner.getPartition returns for its sort key over the n_bounds range

@@ -144,6 +144,12 @@ int b2sh_serialized_writer_round_robin_rows(b2sh_serialized_writer* w, uint32_t 
 int b2sh_serialized_writer_aggregate_rows(b2sh_serialized_writer* w, uint32_t n_aggs, const uint32_t* agg_fn,
                                           const uint32_t* val_type, const uint32_t* val_off,
                                           const int32_t* val_null_field);
+/* The grouping sets of a ROLLUP, CUBE or GROUPING SETS aggregation's map side (INTEGRATION.md §3q), set after
+ * aggregate_rows and before the first insert: commit() makes one b2s_aggregate_grouping_sets_partition_compress_rows_hash_packed
+ * call with these n_sets masks (bit c of set_mask[k]: hash_rows' key column c is in set k; copied), which expands every
+ * row once per set and writes the partial rows keyed by the grouping columns and spark_grouping_id.  When the partial
+ * rows outgrow the input's bound, commit() retries with the exact size the call reports. */
+int b2sh_serialized_writer_grouping_sets(b2sh_serialized_writer* w, uint32_t n_sets, const uint32_t* set_mask);
 int b2sh_serialized_writer_insert(b2sh_serialized_writer* w, int32_t partition_id, const uint8_t* bytes, uint64_t len);
 int b2sh_serialized_writer_commit(b2sh_serialized_writer* w, int64_t* partition_lengths_out);
 int b2sh_serialized_writer_statistics(b2sh_serialized_writer* w, uint64_t* bytes, uint64_t* nanos, char* line,

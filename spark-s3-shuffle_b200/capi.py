@@ -112,6 +112,12 @@ PROTOTYPES = [
     ("b2s_aggregate_partition_compress_rows_hash_dev", C.c_int,
      [_u32, _u32, _i32, _u32, _u32, _u32, _u64, _vp, _u64, _u32p, _u32, _u32p, _u32p, _u32p, _i32p, _u32, _u32p, _u32p,
       _u32p, _i32p, _vp, _u64, _u64p, _u64p, _u64p, _u64p, _i32p, _u64p]),
+    ("b2s_aggregate_grouping_sets_partition_compress_rows_hash_packed", C.c_int,
+     [_u32, _i32, _u32, _u32, _u32, _u64, _u8p, _u64, _u32p, _u32, _u32p, _u32p, _u32p, _i32p, _u32, _u32p, _u32p, _u32p,
+      _i32p, _u32, _u32p, _u8p, _u64, _u64p, _u64p, _u64p, _u64p, _i32p, _u64p]),
+    ("b2s_aggregate_grouping_sets_partition_compress_rows_hash_dev", C.c_int,
+     [_u32, _u32, _i32, _u32, _u32, _u32, _u64, _vp, _u64, _u32p, _u32, _u32p, _u32p, _u32p, _i32p, _u32, _u32p, _u32p,
+      _u32p, _i32p, _u32, _u32p, _vp, _u64, _u64p, _u64p, _u64p, _u64p, _i32p, _u64p]),
     ("b2s_partition_compress_rows_range_packed", C.c_int,
      [_u32, _i32, _u32, _u32, _u64, _u8p, _u64, _u32p, _u32, _u32p, _u32p, _u32p, _i32p, _u32, _u8p, _u64, _u32p,
       _u8p, _u64, _u64p, _u64p, _u64p, _u64p, _i32p]),
@@ -934,6 +940,46 @@ def aggregate_partition_compress_rows_hash_dev(codec, d_records, rec_bytes, d_re
         _ptr(kt), _ptr(ko), _ptr(kl), _ptr(kn), na, _ptr(fn), _ptr(vt), _ptr(vo), _ptr(vn), d_dst, dst_cap,
         _ptr(dst_off), _ptr(dst_len), C.addressof(total), _ptr(cks), _ptr(st), C.addressof(groups)),
         "b2s_aggregate_partition_compress_rows_hash_dev")
+    return dict(dst_off=dst_off, dst_len=dst_len, total=total.value, checksums=cks, status=st, n_groups=groups.value)
+
+
+def aggregate_grouping_sets_partition_compress_rows_hash_packed(codec, records, rec_len, keys, aggs, sets,
+                                                                num_partitions, dst, block_size=0,
+                                                                checksum_alg=CHECKSUM_NONE, level=0):
+    """Spark's Expand over grouping sets, then HashAggregateExec(Partial) and its hash exchange: as
+    aggregate_partition_compress_rows_hash_packed, each record once per grouping set (sets: one mask per set, bit c for
+    key column c), the partial rows keyed by the grouping columns and spark_grouping_id.  -> dict(dst_off, dst_len,
+    total, checksums, status, n_groups)"""
+    records, dst = _as_u8(records), _as_u8(dst)
+    rec_len = np.ascontiguousarray(rec_len, dtype=np.uint32)
+    nk, kt, ko, kl, kn = _key_arrays(keys)
+    na, fn, vt, vo, vn = _partial_agg_arrays(aggs)
+    masks = np.ascontiguousarray(list(sets) or [0], dtype=np.uint32)
+    dst_off, dst_len, cks, st = _partition_out(num_partitions)
+    total, groups = _u64(0), _u64(0)
+    _check(load().b2s_aggregate_grouping_sets_partition_compress_rows_hash_packed(
+        codec, level, block_size, checksum_alg, num_partitions, rec_len.size, _ptr(records), records.size,
+        _ptr(rec_len), nk, _ptr(kt), _ptr(ko), _ptr(kl), _ptr(kn), na, _ptr(fn), _ptr(vt), _ptr(vo), _ptr(vn),
+        len(sets), _ptr(masks), _ptr(dst), dst.size, _ptr(dst_off), _ptr(dst_len), C.addressof(total), _ptr(cks),
+        _ptr(st), C.addressof(groups)), "b2s_aggregate_grouping_sets_partition_compress_rows_hash_packed")
+    return dict(dst_off=dst_off, dst_len=dst_len, total=total.value, checksums=cks, status=st, n_groups=groups.value)
+
+
+def aggregate_grouping_sets_partition_compress_rows_hash_dev(codec, d_records, rec_bytes, d_rec_len, n_records, keys,
+                                                             aggs, sets, num_partitions, d_dst, dst_cap, block_size=0,
+                                                             checksum_alg=CHECKSUM_NONE, level=0, dev=0):
+    """aggregate_grouping_sets_partition_compress_rows_hash_packed on device addresses (records, u32 lengths,
+    destination arena)"""
+    nk, kt, ko, kl, kn = _key_arrays(keys)
+    na, fn, vt, vo, vn = _partial_agg_arrays(aggs)
+    masks = np.ascontiguousarray(list(sets) or [0], dtype=np.uint32)
+    dst_off, dst_len, cks, st = _partition_out(num_partitions)
+    total, groups = _u64(0), _u64(0)
+    _check(load().b2s_aggregate_grouping_sets_partition_compress_rows_hash_dev(
+        dev, codec, level, block_size, checksum_alg, num_partitions, n_records, d_records, rec_bytes, d_rec_len, nk,
+        _ptr(kt), _ptr(ko), _ptr(kl), _ptr(kn), na, _ptr(fn), _ptr(vt), _ptr(vo), _ptr(vn), len(sets), _ptr(masks),
+        d_dst, dst_cap, _ptr(dst_off), _ptr(dst_len), C.addressof(total), _ptr(cks), _ptr(st), C.addressof(groups)),
+        "b2s_aggregate_grouping_sets_partition_compress_rows_hash_dev")
     return dict(dst_off=dst_off, dst_len=dst_len, total=total.value, checksums=cks, status=st, n_groups=groups.value)
 
 

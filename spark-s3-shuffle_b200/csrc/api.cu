@@ -252,6 +252,7 @@ struct Slot {
   DevBuf xpieces;      // the copy pieces of an exchange-cache read (exchange.cu)
   DevBuf fws;          // row framing workspace: bitmap over the decoded arena, tile counts, verdicts (rows.cu)
   DevBuf aggrows;      // a partial aggregation's partial rows, in front of the partition step (partial_agg.cu)
+  DevBuf xrows;        // grouping sets: the projected records' lengths, then the records (rows_expand.cu)
   PinBuf hmeta;
   // per-launch event pairs around the dominant kernel of a call (grow-only pool; dom_used pairs of call dom_call)
   std::vector<cudaEvent_t> ev_dom;
@@ -314,7 +315,7 @@ struct Slot {
   }
   // frees whatever the slot holds (buffers, events, streams); a slot that was never created holds nothing
   void release() {
-    for (DevBuf* b : {&meta, &scratch, &desc, &src, &dst, &zmeta, &pws, &parena, &xpieces, &fws, &aggrows}) b->release();
+    for (DevBuf* b : {&meta, &scratch, &desc, &src, &dst, &zmeta, &pws, &parena, &xpieces, &fws, &aggrows, &xrows}) b->release();
     hmeta.release();
     for (cudaEvent_t* e : events())
       if (*e) cudaEventDestroy(*e);
@@ -3138,30 +3139,17 @@ static KeySpec partial_row_keys(const KeySpec& in) {
   return k;
 }
 
-// The aggregation step on S over n device-resident records (d_rec, rec_bytes; d_len): offsets, checks (one readback:
-// a bad record or a wrong byte total fails the call), the key sort and its refinement rounds, the grouping, the folds
-// (one readback: groups, partial-row bytes) and the partial rows into S.aggrows, their record lengths at *row_len (in
-// S.fws).  Marks G0, G1.
-static int partial_agg_rows(Slot& S, const PartialAggSpec& spec, uint64_t n, const uint8_t* d_rec, uint64_t rec_bytes,
-                            const uint32_t* d_len, uint64_t* groups, uint64_t* out_bytes, const uint32_t** row_len,
-                            uint64_t* launches) {
+// The records' offsets (into the sort workspace ws, with key_bytes of key) and their checks (the verdict in paws' header,
+// ids n u32 of scratch), one readback: a bad record or a wrong byte total fails the call with the record it names
+static int partial_agg_checked(Slot& S, const PartialAggSpec& spec, uint64_t n, const uint8_t* d_rec,
+                               uint64_t rec_bytes, const uint32_t* d_len, uint32_t key_bytes, uint8_t* ws,
+                               uint8_t* paws, uint32_t* ids, uint64_t* launches) {
   cudaStream_t st = S.st;
   const KeySpec& ks = spec.keys;
-  const uint32_t key_bytes = rows_key_bytes(ks);
-  const bool refine = rows_key_refines(ks);
-  const size_t part[4] = {rows_sort_ws_bytes(n, key_bytes), refine ? rows_refine_ws_bytes(n, 1) : 0,
-                          rows_aggregate_ws_bytes(n, 0, 0), partial_agg_ws_bytes(n, spec)};
-  if (int rc = S.fws.ensure(part[0] + part[1] + part[2] + part[3])) return rc;
-  uint8_t* ws = (uint8_t*)S.fws.p;
-  uint8_t *rws = refine ? ws + part[0] : nullptr, *gws = ws + part[0] + part[1], *paws = gws + part[2];
   uint64_t* hdr = partial_agg_header(paws);
-  *row_len = partial_agg_row_len(paws, n, spec);
-  if (int rc = S.hmeta.ensure(48)) return rc;
   uint64_t* rb = (uint64_t*)S.hmeta.p;
-  CU(S.mark(G0, st, *launches));
   launch_partial_agg_offsets(d_len, n, key_bytes, ws, paws, st, launches);
-  launch_partial_agg_check(d_rec, rec_bytes, n, key_bytes, spec, ws, paws,
-                           (uint32_t*)partial_agg_row_len(paws, n, spec), st, launches);
+  launch_partial_agg_check(d_rec, rec_bytes, n, key_bytes, spec, ws, paws, ids, st, launches);
   CU(cudaMemcpyAsync(rb, hdr, 24, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
   CU(cudaGetLastError());
@@ -3186,6 +3174,40 @@ static int partial_agg_rows(Slot& S, const PartialAggSpec& spec, uint64_t n, con
                (unsigned long long)rec_bytes);
     return fail(B2S_E_ARG, "%s", msg);
   }
+  return 0;
+}
+
+// the aggregation step's workspace in S.fws: the key sort's, the refinement rounds', the grouping's and its own
+static size_t partial_agg_fws_bytes(uint64_t n, const PartialAggSpec& spec) {
+  const uint32_t key_bytes = rows_key_bytes(spec.keys);
+  return rows_sort_ws_bytes(n, key_bytes) + (rows_key_refines(spec.keys) ? rows_refine_ws_bytes(n, 1) : 0) +
+         rows_aggregate_ws_bytes(n, 0, 0) + partial_agg_ws_bytes(n, spec);
+}
+
+// The aggregation step on S over n device-resident records (d_rec, rec_bytes; d_len): offsets, checks
+// (partial_agg_checked), the key sort and its refinement rounds, the grouping, the folds (one readback: groups,
+// partial-row bytes) and the partial rows into S.aggrows, their record lengths at *row_len (in S.fws).  Marks G1, and G0
+// unless the caller marked it before a step of its own.
+static int partial_agg_rows(Slot& S, const PartialAggSpec& spec, uint64_t n, const uint8_t* d_rec, uint64_t rec_bytes,
+                            const uint32_t* d_len, uint64_t* groups, uint64_t* out_bytes, const uint32_t** row_len,
+                            uint64_t* launches, bool mark_g0 = true) {
+  cudaStream_t st = S.st;
+  const KeySpec& ks = spec.keys;
+  const uint32_t key_bytes = rows_key_bytes(ks);
+  const bool refine = rows_key_refines(ks);
+  const size_t part[4] = {rows_sort_ws_bytes(n, key_bytes), refine ? rows_refine_ws_bytes(n, 1) : 0,
+                          rows_aggregate_ws_bytes(n, 0, 0), partial_agg_ws_bytes(n, spec)};
+  if (int rc = S.fws.ensure(partial_agg_fws_bytes(n, spec))) return rc;
+  uint8_t* ws = (uint8_t*)S.fws.p;
+  uint8_t *rws = refine ? ws + part[0] : nullptr, *gws = ws + part[0] + part[1], *paws = gws + part[2];
+  uint64_t* hdr = partial_agg_header(paws);
+  *row_len = partial_agg_row_len(paws, n, spec);
+  if (int rc = S.hmeta.ensure(48)) return rc;
+  uint64_t* rb = (uint64_t*)S.hmeta.p;
+  if (mark_g0) CU(S.mark(G0, st, *launches));
+  if (int rc = partial_agg_checked(S, spec, n, d_rec, rec_bytes, d_len, key_bytes, ws, paws,
+                                   (uint32_t*)partial_agg_row_len(paws, n, spec), launches))
+    return rc;
   *groups = *out_bytes = 0;
   if (!n) {
     CU(S.mark(G1, st, *launches));
@@ -3228,14 +3250,117 @@ constexpr size_t kSortKeepBytes = 1ull << 30;
 struct PartialAggTrim {
   Slot& S;
   ~PartialAggTrim() {
-    for (DevBuf* b : {&S.fws, &S.aggrows})
+    for (DevBuf* b : {&S.fws, &S.aggrows, &S.xrows})
       if (b->cap > kSortKeepBytes) b->release();
   }
 };
 
-// b2s_aggregate_partition_compress_rows_hash_*: the checks before the device, then on the write lane the aggregation
-// step and the partition + compress step over the partial rows, from host records (packed: one upload, one download)
-// or device ones
+// b2s_aggregate_grouping_sets_partition_compress_rows_hash_*'s grouping sets: n_sets masks of key columns
+struct GroupingSets {
+  uint32_t n_sets;
+  const uint32_t* mask;
+};
+
+// The grouping sets' rules, before the device: gid takes the 16th key column; every mask names key columns only, once
+// (n_keys + 1 + buffers <= 15 + 1 + 16 = 32 partial-row fields follows: one null word, as the partial rows need)
+static int grouping_sets_args(uint32_t n_keys, uint64_t n, const GroupingSets& g) {
+  if (n_keys < 1 || n_keys >= kMaxKeys)
+    return fail(B2S_E_ARG, "n_keys must be in [1, 15] with grouping sets (gid is the 16th key column)%s");
+  if (!g.n_sets || !g.mask) return fail(B2S_E_ARG, "grouping sets need n_sets >= 1 and a set_mask array%s");
+  if (n >= ((1ull << 32) + g.n_sets - 1) / g.n_sets)
+    return fail(B2S_E_ARG, "n_records * n_sets must be below 2^32 (the projected records)%s");
+  std::vector<uint8_t> seen(1u << n_keys);
+  for (uint32_t k = 0; k < g.n_sets; k++) {
+    const uint32_t m = g.mask[k];
+    if (m >> n_keys) return fail(B2S_E_ARG, "a grouping set's mask names a column at or above n_keys%s");
+    if (seen[m]++) return fail(B2S_E_ARG, "two grouping sets are equal (Spark adds _gen_grouping_pos for them)%s");
+  }
+  return 0;
+}
+
+// The aggregation over the projected records (rows_expand.cu): key columns c at slot 8 + 8 c with null bit c, gid an
+// INT64 at slot 8 + 8 n_keys that is never null, aggregate input i at slot 8 + 8 (n_keys + 1 + i) with null bit
+// n_keys + 1 + i when the caller's input has one; and the expansion's own spec
+static int grouping_sets_spec(const KeySpec& ks, uint32_t n_aggs, const uint32_t* fn, const uint32_t* val_type,
+                              const uint32_t* val_off, const int32_t* val_null, uint32_t n_sets, ExpandSpec* xs,
+                              PartialAggSpec* out) {
+  const uint32_t nk = ks.n;
+  xs->keys = ks;
+  xs->n_sets = n_sets;
+  uint32_t ty[kMaxKeys], off[kMaxKeys], len[kMaxKeys];
+  int32_t nul[kMaxKeys];
+  for (uint32_t c = 0; c < nk; c++) {
+    ty[c] = ks.type[c];
+    off[c] = 8 + 8 * c;
+    len[c] = ks.len[c];
+    nul[c] = (int32_t)c;
+  }
+  ty[nk] = B2S_KEY_INT64;
+  off[nk] = 8 + 8 * nk;
+  len[nk] = 8;
+  nul[nk] = -1;
+  uint32_t poff[kMaxAggs] = {};
+  int32_t pnull[kMaxAggs];
+  for (uint32_t a = 0; a < n_aggs; a++) {
+    pnull[a] = -1;
+    if ((val_type[a] & 0xff) == B2S_WINDOW_VAL_NONE) continue;
+    const uint32_t i = xs->n_in++, f = nk + 1 + i;
+    xs->vtype[i] = val_type[a];
+    xs->voff[i] = val_off[a];
+    xs->vnull[i] = val_null[a];
+    xs->reads[i] = fn[a] != B2S_WINDOW_COUNT;
+    poff[a] = 8 + 8 * f;
+    pnull[a] = val_null[a] >= 0 ? (int32_t)f : -1;
+  }
+  out->keys = keys_spec(nk + 1, ty, off, len, nul).keys;
+  return partial_agg_args(n_aggs, fn, val_type, poff, pnull, out);
+}
+
+// Expand on S: the caller's n records checked once (partial_agg_checked: a bad record is named by its input index),
+// then each projected once per grouping set into S.xrows (rows_expand.cu; one readback: the projected bytes) ->
+// *x_rec, *x_bytes, *x_len, the aggregation step's records.  S.fws is sized once for this and for the aggregation step
+// over the projected records (xagg).  After G0, which the caller marks.
+static int expand_rows(Slot& S, const PartialAggSpec& spec, const PartialAggSpec& xagg, const ExpandSpec& xs,
+                       const uint32_t* set_mask, uint64_t n, const uint8_t* d_rec, uint64_t rec_bytes,
+                       const uint32_t* d_len, const uint8_t** x_rec, uint64_t* x_bytes, const uint32_t** x_len,
+                       uint64_t* launches) {
+  cudaStream_t st = S.st;
+  const uint32_t key_bytes = rows_key_bytes(spec.keys);
+  const size_t part[3] = {rows_sort_ws_bytes(n, key_bytes), 256 + align_up(n * 4, 256), expand_ws_bytes(n, xs.n_sets)};
+  if (int rc = S.fws.ensure(std::max(part[0] + part[1] + part[2], partial_agg_fws_bytes(n * xs.n_sets, xagg))))
+    return rc;
+  if (int rc = S.hmeta.ensure(48)) return rc;
+  uint8_t* ws = (uint8_t*)S.fws.p;
+  uint8_t *paws = ws + part[0], *xws = paws + part[1];
+  uint64_t* rb = (uint64_t*)S.hmeta.p;
+  if (int rc = partial_agg_checked(S, spec, n, d_rec, rec_bytes, d_len, key_bytes, ws, paws, (uint32_t*)(paws + 256),
+                                   launches))
+    return rc;
+  const uint64_t* rec_off = carve_key_sort_ws(ws, n, key_bytes).src_off;
+  CU(cudaMemcpyAsync(expand_masks(xws, n, xs.n_sets), set_mask, (size_t)xs.n_sets * 4, cudaMemcpyHostToDevice, st));
+  launch_expand_size(d_rec, rec_off, n, xs, xws, st, launches);
+  CU(cudaMemcpyAsync(rb, expand_header(xws), 16, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  CU(cudaGetLastError());
+  if (rb[1] != ~0ull) {
+    char msg[256];
+    snprintf(msg, sizeof msg, "record %llu: its row projected for a grouping set passes UnsafeRow's 2^31 - 1 bytes",
+             (unsigned long long)rb[1]);
+    return fail(B2S_E_UNSUPPORTED, "%s", msg);
+  }
+  const uint64_t N = n * xs.n_sets, len_sz = align_up(N * 4, 256);
+  *x_bytes = rb[0];
+  if (int rc = S.xrows.ensure(len_sz + rb[0] + 64)) return rc;
+  *x_len = (const uint32_t*)S.xrows.p;
+  *x_rec = (const uint8_t*)S.xrows.p + len_sz;
+  launch_expand_write(d_rec, rec_off, n, xs, xws, (uint32_t*)S.xrows.p, (uint8_t*)S.xrows.p + len_sz, st, launches);
+  return 0;
+}
+
+// b2s_aggregate_partition_compress_rows_hash_* (gs null) and b2s_aggregate_grouping_sets_partition_compress_rows_hash_*:
+// the checks before the device, then on the write lane (with grouping sets, the expansion first) the aggregation step
+// and the partition + compress step over the partial rows, from host records (packed: one upload, one download) or
+// device ones
 static int aggregate_partition_call(bool packed, uint32_t dev_index, uint32_t codec, int32_t level,
                                     uint32_t codec_block_size, uint32_t checksum_alg, uint32_t num_partitions,
                                     uint64_t n_records, const uint8_t* rec_base, uint64_t rec_bytes,
@@ -3244,7 +3369,8 @@ static int aggregate_partition_call(bool packed, uint32_t dev_index, uint32_t co
                                     uint32_t n_aggs, const uint32_t* agg_fn, const uint32_t* val_type,
                                     const uint32_t* val_off, const int32_t* val_null_field, uint8_t* dst_base,
                                     uint64_t dst_cap, uint64_t* dst_off, uint64_t* dst_len, uint64_t* dst_total,
-                                    uint64_t* checksum_out, int32_t* status, uint64_t* n_groups) {
+                                    uint64_t* checksum_out, int32_t* status, uint64_t* n_groups,
+                                    const GroupingSets* gs = nullptr) {
   const WallTimer wt = begin_call();
   if (dst_total) *dst_total = 0;
   if (n_groups) *n_groups = 0;
@@ -3253,9 +3379,18 @@ static int aggregate_partition_call(bool packed, uint32_t dev_index, uint32_t co
   spec.keys = rspec.keys;
   if (!n_groups) return fail(B2S_E_ARG, "null argument%s");
   if (int rc = partial_agg_args(n_aggs, agg_fn, val_type, val_off, val_null_field, &spec)) return rc;
+  if (gs)
+    if (int rc = grouping_sets_args(n_keys, n_records, *gs)) return rc;
   if (int rc = hash_args(codec, codec_block_size, checksum_alg, num_partitions, n_records, rec_base, rec_bytes, rec_len,
                          rspec, dst_base, dst_off, dst_len, status))
     return rc;
+  PartialAggSpec xagg;  // with grouping sets, the aggregation over the projected records
+  ExpandSpec xs;
+  if (gs)
+    if (int rc = grouping_sets_spec(spec.keys, n_aggs, agg_fn, val_type, val_off, val_null_field, gs->n_sets, &xs,
+                                    &xagg))
+      return rc;
+  const PartialAggSpec& step = gs ? xagg : spec;
   const uint32_t bs = block_size_or_default(codec_block_size);
   if (!n_records && rec_bytes)
     return fail(B2S_E_ARG, "rec_len sums to 0 bytes, rec_bytes is %s", std::to_string(rec_bytes).c_str());
@@ -3280,9 +3415,22 @@ static int aggregate_partition_call(bool packed, uint32_t dev_index, uint32_t co
   }
   uint64_t launches = 0, groups = 0, rows_bytes = 0, arena = 0;
   const uint32_t* d_row_len = nullptr;
-  int rc = partial_agg_rows(S, spec, n_records, d_rec, rec_bytes, d_len, &groups, &rows_bytes, &d_row_len, &launches);
+  int rc;
+  if (gs) {  // the aggregation step over the projected records; its span (G0, G1) takes in the expansion
+    const uint8_t* x_rec = nullptr;
+    const uint32_t* x_len = nullptr;
+    uint64_t x_bytes = 0;
+    CU(S.mark(G0, st, launches));
+    if ((rc = expand_rows(S, spec, xagg, xs, gs->mask, n_records, d_rec, rec_bytes, d_len, &x_rec, &x_bytes, &x_len,
+                          &launches)))
+      return rc;
+    rc = partial_agg_rows(S, step, n_records * gs->n_sets, x_rec, x_bytes, x_len, &groups, &rows_bytes, &d_row_len,
+                          &launches, false);
+  } else {
+    rc = partial_agg_rows(S, spec, n_records, d_rec, rec_bytes, d_len, &groups, &rows_bytes, &d_row_len, &launches);
+  }
   if (rc) return rc;
-  const RowIds ids{partial_row_keys(spec.keys)};
+  const RowIds ids{partial_row_keys(step.keys)};
   uint8_t* d_dst = dst_base;
   uint64_t cap = dst_cap;
   if (packed) {  // sized by the bound: a short caller arena shows up after the run, as in the packed partition call
@@ -3341,6 +3489,36 @@ int b2s_aggregate_partition_compress_rows_hash_dev(
                                   n_records, rec_base, rec_bytes, rec_len, n_keys, key_type, key_off, key_len,
                                   key_null_field, n_aggs, agg_fn, val_type, val_off, val_null_field, dst_base, dst_cap,
                                   dst_off, dst_len, dst_total, checksum_out, status, n_groups);
+}
+
+int b2s_aggregate_grouping_sets_partition_compress_rows_hash_packed(
+    uint32_t codec, int32_t level, uint32_t codec_block_size, uint32_t checksum_alg, uint32_t num_partitions,
+    uint64_t n_records, const uint8_t* rec_base, uint64_t rec_bytes, const uint32_t* rec_len, uint32_t n_keys,
+    const uint32_t* key_type, const uint32_t* key_off, const uint32_t* key_len, const int32_t* key_null_field,
+    uint32_t n_aggs, const uint32_t* agg_fn, const uint32_t* val_type, const uint32_t* val_off,
+    const int32_t* val_null_field, uint32_t n_sets, const uint32_t* set_mask, uint8_t* dst_base, uint64_t dst_cap,
+    uint64_t* dst_off, uint64_t* dst_len, uint64_t* dst_total, uint64_t* checksum_out, int32_t* status,
+    uint64_t* n_groups) {
+  const GroupingSets gs{n_sets, set_mask};
+  return aggregate_partition_call(true, 0, codec, level, codec_block_size, checksum_alg, num_partitions, n_records,
+                                  rec_base, rec_bytes, rec_len, n_keys, key_type, key_off, key_len, key_null_field,
+                                  n_aggs, agg_fn, val_type, val_off, val_null_field, dst_base, dst_cap, dst_off,
+                                  dst_len, dst_total, checksum_out, status, n_groups, &gs);
+}
+
+int b2s_aggregate_grouping_sets_partition_compress_rows_hash_dev(
+    uint32_t dev_index, uint32_t codec, int32_t level, uint32_t codec_block_size, uint32_t checksum_alg,
+    uint32_t num_partitions, uint64_t n_records, const uint8_t* rec_base, uint64_t rec_bytes, const uint32_t* rec_len,
+    uint32_t n_keys, const uint32_t* key_type, const uint32_t* key_off, const uint32_t* key_len,
+    const int32_t* key_null_field, uint32_t n_aggs, const uint32_t* agg_fn, const uint32_t* val_type,
+    const uint32_t* val_off, const int32_t* val_null_field, uint32_t n_sets, const uint32_t* set_mask,
+    uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_off, uint64_t* dst_len, uint64_t* dst_total,
+    uint64_t* checksum_out, int32_t* status, uint64_t* n_groups) {
+  const GroupingSets gs{n_sets, set_mask};
+  return aggregate_partition_call(false, dev_index, codec, level, codec_block_size, checksum_alg, num_partitions,
+                                  n_records, rec_base, rec_bytes, rec_len, n_keys, key_type, key_off, key_len,
+                                  key_null_field, n_aggs, agg_fn, val_type, val_off, val_null_field, dst_base, dst_cap,
+                                  dst_off, dst_len, dst_total, checksum_out, status, n_groups, &gs);
 }
 
 // ------------------------------------------------------------------------------------------------------------

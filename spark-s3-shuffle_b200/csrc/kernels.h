@@ -529,6 +529,34 @@ void launch_partial_agg_emit(const uint8_t* rec, uint64_t n, uint64_t groups, co
                              const PartialAggSpec& spec, uint8_t* d_ws, uint8_t* d_gws, uint8_t* d_paws,
                              uint8_t* d_dst, cudaStream_t st, uint64_t* launches);
 
+// ---------------- rows_expand.cu (Spark's Expand for grouping sets, in front of the partial aggregation) ----------------
+// The caller's records (checked by launch_partial_agg_check; offsets rec_off as launch_partial_agg_offsets leaves them),
+// each projected once per grouping set into a compact UnsafeRow: key column c (nullable; null outside the set), gid
+// (Spark's spark_grouping_id, a long), then input i < n_in of the aggregates that read one (type vtype[i], slot voff[i],
+// null bit vnull[i] or -1; reads[i]: its value is read, not only its null bit).  Set k's mask is device word k of
+// expand_masks; projected record r * n_sets + k is record r under set k.
+struct ExpandSpec {
+  KeySpec keys;
+  uint32_t n_in = 0;
+  uint32_t vtype[kMaxAggs] = {};
+  uint32_t voff[kMaxAggs] = {};
+  int32_t vnull[kMaxAggs] = {};
+  uint32_t reads[kMaxAggs] = {};
+  uint32_t n_sets = 0;
+};
+size_t expand_ws_bytes(uint64_t n, uint32_t n_sets);
+// the workspace's header (device): [projected bytes, the lowest record whose projected row passes 2^31 - 1 bytes
+// (~0: none)]
+uint64_t* expand_header(uint8_t* d_xws);
+// the n_sets set masks (device), for the caller to fill
+uint32_t* expand_masks(uint8_t* d_xws, uint64_t n, uint32_t n_sets);
+// the projected records' lengths and 64-bit offsets; header words 0 and 1.  Resets the header.
+void launch_expand_size(const uint8_t* rec, const uint64_t* rec_off, uint64_t n, const ExpandSpec& spec,
+                        uint8_t* d_xws, cudaStream_t st, uint64_t* launches);
+// the projected records ([size: int32 big-endian][row], header word 0 bytes) to d_out, their lengths to d_out_len
+void launch_expand_write(const uint8_t* rec, const uint64_t* rec_off, uint64_t n, const ExpandSpec& spec,
+                         uint8_t* d_xws, uint32_t* d_out_len, uint8_t* d_out, cudaStream_t st, uint64_t* launches);
+
 // ---------------- join.cu (sort-merge join of a reducer's two sorted sides into Spark's joined UnsafeRows) -----------
 // The records of both sides, stably sorted together by the join key (launch_rows_join_order) and grouped
 // (launch_rows_group): each group holds its key's left records, then its right ones.  The shape of the joined row:

@@ -94,6 +94,7 @@ PROTOTYPES = [
     ("b2sh_serialized_writer_range_rows", C.c_int, [_vp, _u32, _vp, _vp, _vp, _vp, _u32, _vp, _u64, _vp]),
     ("b2sh_serialized_writer_round_robin_rows", C.c_int, [_vp, _u32, _i32, _u32]),
     ("b2sh_serialized_writer_aggregate_rows", C.c_int, [_vp, _u32, _vp, _vp, _vp, _vp]),
+    ("b2sh_serialized_writer_grouping_sets", C.c_int, [_vp, _u32, _vp]),
     ("b2sh_serialized_writer_insert", C.c_int, [_vp, _i32, _vp, _u64]),
     ("b2sh_serialized_writer_commit", C.c_int, [_vp, _vp]),
     ("b2sh_serialized_writer_statistics", C.c_int, [_vp, C.POINTER(_u64), C.POINTER(_u64), C.c_char_p, _u32]),
@@ -330,6 +331,13 @@ class S3SerializedShuffleWriter:
         aggs = list(aggs)
         arrs = [np.array([a[i] for a in aggs] or [0], dtype=np.int32 if i == 3 else np.uint32) for i in range(4)]
         _check(load().b2sh_serialized_writer_aggregate_rows(self._h, len(aggs), *[a.ctypes.data for a in arrs]))
+
+    def groupingSets(self, masks):
+        """the grouping sets of a ROLLUP, CUBE or GROUPING SETS aggregation, after aggregateRows and before the first
+        insert: masks = [bit c set when hashRows' key column c is in the set, ...]; commit() writes the partial rows
+        keyed by the grouping columns and spark_grouping_id"""
+        m = np.array(list(masks) or [0], dtype=np.uint32)
+        _check(load().b2sh_serialized_writer_grouping_sets(self._h, len(masks), m.ctypes.data))
 
     def insertRecord(self, partitionId, record):
         a = np.frombuffer(record, dtype=np.uint8) if not isinstance(record, np.ndarray) else np.ascontiguousarray(record)

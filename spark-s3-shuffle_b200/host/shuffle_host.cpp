@@ -560,6 +560,16 @@ class S3SerializedShuffleWriter {
     aggOff_.assign(valOff, valOff + nAggs);
     aggNull_.assign(valNull, valNull + nAggs);
   }
+  // The grouping sets of a ROLLUP, CUBE or GROUPING SETS aggregation's map side
+  // (b2s_aggregate_grouping_sets_partition_compress_rows_hash_packed): after aggregateRows and before the first insert;
+  // commit() expands every row once per set (bit c of a mask: key column c is in the set), then aggregates and
+  // hash-partitions the partial rows keyed by the grouping columns and spark_grouping_id on the GPU.
+  void groupingSets(uint32_t nSets, const uint32_t* mask) {
+    if (!recLen_.empty()) throw RuntimeException("Precondition: grouping_sets must come before the first insert.");
+    if (!aggregate_) throw RuntimeException("Precondition: grouping_sets needs aggregate_rows first.");
+    if (!nSets || !mask) throw RuntimeException("Precondition: grouping_sets needs at least one set.");
+    setMask_.assign(mask, mask + nSets);
+  }
   void insertRecord(int32_t partitionId, const uint8_t* b, uint64_t n) {
     const bool hashed = !keyType_.empty() || roundRobin_;
     if (!hashed && (partitionId < 0 || partitionId >= numPartitions_))
@@ -589,14 +599,25 @@ class S3SerializedShuffleWriter {
     if (aggregate_) {
       // the partial rows' arena is not known before the call: the bound of the input's bytes first, then the exact
       // size the call reports when that is short
-      call = "b2s_aggregate_partition_compress_rows_hash_packed";
+      const bool sets = !setMask_.empty();
+      call = sets ? "b2s_aggregate_grouping_sets_partition_compress_rows_hash_packed"
+                  : "b2s_aggregate_partition_compress_rows_hash_packed";
       uint64_t groups = 0;
       for (int attempt = 0;; attempt++) {
-        rc = b2s_aggregate_partition_compress_rows_hash_packed(
-            codec, d_.zstdLevel, d_.lz4BlockSize, alg, R, recLen_.size(), records_.data(), records_.size(),
-            recLen_.data(), (uint32_t)keyType_.size(), keyType_.data(), keyOff_.data(), keyLen_.data(),
-            keyNull_.data(), (uint32_t)aggFn_.size(), aggFn_.data(), aggType_.data(), aggOff_.data(), aggNull_.data(),
-            out_.data(), out_.size(), doff.data(), dlen.data(), &total, cks.data(), status.data(), &groups);
+        if (sets)
+          rc = b2s_aggregate_grouping_sets_partition_compress_rows_hash_packed(
+              codec, d_.zstdLevel, d_.lz4BlockSize, alg, R, recLen_.size(), records_.data(), records_.size(),
+              recLen_.data(), (uint32_t)keyType_.size(), keyType_.data(), keyOff_.data(), keyLen_.data(),
+              keyNull_.data(), (uint32_t)aggFn_.size(), aggFn_.data(), aggType_.data(), aggOff_.data(),
+              aggNull_.data(), (uint32_t)setMask_.size(), setMask_.data(), out_.data(), out_.size(), doff.data(),
+              dlen.data(), &total, cks.data(), status.data(), &groups);
+        else
+          rc = b2s_aggregate_partition_compress_rows_hash_packed(
+              codec, d_.zstdLevel, d_.lz4BlockSize, alg, R, recLen_.size(), records_.data(), records_.size(),
+              recLen_.data(), (uint32_t)keyType_.size(), keyType_.data(), keyOff_.data(), keyLen_.data(),
+              keyNull_.data(), (uint32_t)aggFn_.size(), aggFn_.data(), aggType_.data(), aggOff_.data(),
+              aggNull_.data(), out_.data(), out_.size(), doff.data(), dlen.data(), &total, cks.data(), status.data(),
+              &groups);
         if (rc != B2S_E_DST_TOO_SMALL || attempt) break;
         out_.resize(total);
       }
@@ -676,6 +697,7 @@ class S3SerializedShuffleWriter {
   bool aggregate_ = false;  // aggregateRows: the rows are aggregated by hashRows' key columns first
   std::vector<uint32_t> aggFn_, aggType_, aggOff_;
   std::vector<int32_t> aggNull_;
+  std::vector<uint32_t> setMask_;  // groupingSets: the rows are expanded once per set before the aggregation
   bool roundRobin_ = false;  // roundRobinRows: Spark's repartition(n) order and ids from rrStart_
   int32_t rrStart_ = 0;
   uint32_t rrSort_ = 0;
@@ -1557,6 +1579,9 @@ int b2sh_serialized_writer_aggregate_rows(b2sh_serialized_writer* w, uint32_t n_
                                           const uint32_t* val_type, const uint32_t* val_off,
                                           const int32_t* val_null_field) {
   return guarded([&] { w->w->aggregateRows(n_aggs, agg_fn, val_type, val_off, val_null_field); });
+}
+int b2sh_serialized_writer_grouping_sets(b2sh_serialized_writer* w, uint32_t n_sets, const uint32_t* set_mask) {
+  return guarded([&] { w->w->groupingSets(n_sets, set_mask); });
 }
 int b2sh_serialized_writer_insert(b2sh_serialized_writer* w, int32_t partition_id, const uint8_t* bytes, uint64_t len) {
   return guarded([&] { w->w->insertRecord(partition_id, bytes, len); });

@@ -1,0 +1,139 @@
+"""The grouping-sets write calls (b2s_aggregate_grouping_sets_partition_compress_rows_hash_*) without a GPU: a
+well-formed call fails loudly with B2S_E_CUDA and reports nothing as written; every ill-formed call, the partial
+aggregation call's rejections included, is B2S_E_ARG with b2s_last_error set before any device is needed.  Also: the
+prototypes match the headers."""
+import ctypes as C
+import os
+import re
+
+import numpy as np
+import pytest
+
+import spark_s3_shuffle_b200 as pkg
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+NAMES = ["b2s_aggregate_grouping_sets_partition_compress_rows_hash_packed",
+         "b2s_aggregate_grouping_sets_partition_compress_rows_hash_dev"]
+SUM, COUNT, MIN, MAX, AVG = 6, 7, 8, 9, 10
+NONE, I8, I16, I32, I64, F32, F64, DEC, BYTES = range(9)
+
+
+def dec(p, s=0):
+    return DEC | p << 8 | s << 16
+
+
+def _has_gpu():
+    try:
+        import torch
+        return torch.cuda.is_available()
+    except Exception:
+        return os.path.exists("/dev/nvidia0")
+
+
+AGGS = [(SUM, I64, 16, 1), (COUNT, NONE, 0, -1), (AVG, dec(10, 2), 24, 2), (MIN, F64, 32, -1)]
+KEYS = ((1, 8, 4, 0), (2, 16, 8, -1))
+ROLLUP2 = (0b11, 0b01, 0)
+
+
+def _call(L, c, dev=False, R=4, n=2, keys=KEYS, aggs=AGGS, sets=ROLLUP2, rec_len=(44, 44), records=True, groups=True,
+          agg_arrays=True, mask_array=True, n_sets=None):
+    rec = np.zeros(128, np.uint8)
+    rl = np.array(rec_len, np.uint32)
+    kt = np.array([k[0] for k in keys] or [0], np.uint32)
+    ko = np.array([k[1] for k in keys] or [0], np.uint32)
+    kl = np.array([k[2] for k in keys] or [0], np.uint32)
+    kn = np.array([k[3] for k in keys] or [0], np.int32)
+    fn = np.array([a[0] for a in aggs] or [0], np.uint32)
+    vt = np.array([a[1] for a in aggs] or [0], np.uint32)
+    vo = np.array([a[2] for a in aggs] or [0], np.uint32)
+    vn = np.array([a[3] for a in aggs] or [0], np.int32)
+    masks = np.array(list(sets) or [0], np.uint32)
+    doff, dlen, cks = np.zeros(R, np.uint64), np.zeros(R, np.uint64), np.zeros(R, np.uint64)
+    st = np.zeros(R, np.int32)
+    out = np.zeros(512, np.uint8)
+    total, ng = C.c_uint64(7), C.c_uint64(9)
+    a = (lambda x: x.ctypes.data) if agg_arrays else (lambda x: None)
+    args = (c.CODEC_LZ4BLOCK, 0, 0, c.CHECKSUM_CRC32C, R, n, rec.ctypes.data if records else None, int(rl.sum()),
+            rl.ctypes.data, len(keys), kt.ctypes.data, ko.ctypes.data, kl.ctypes.data, kn.ctypes.data, len(aggs),
+            a(fn), a(vt), a(vo), a(vn), len(sets) if n_sets is None else n_sets,
+            masks.ctypes.data if mask_array else None, out.ctypes.data, out.size, doff.ctypes.data, dlen.ctypes.data,
+            C.byref(total), cks.ctypes.data, st.ctypes.data, C.byref(ng) if groups else None)
+    rc = L.b2s_aggregate_grouping_sets_partition_compress_rows_hash_dev(0, *args) if dev else \
+        L.b2s_aggregate_grouping_sets_partition_compress_rows_hash_packed(*args)
+    return rc, total.value, ng.value, L.b2s_last_error()
+
+
+@pytest.mark.skipif(_has_gpu(), reason="GPU present")
+def test_calls_return_cuda_error_without_a_device():
+    c = pkg.capi
+    L = c.load()
+    assert L.b2s_init(0, 0, 0) == c.E_CUDA
+    for dev in (False, True):
+        for aggs in (AGGS, ()):
+            for sets in (ROLLUP2, (0,), (0b11,), (0b11, 0b10, 0b01, 0)):
+                rc, total, ng, err = _call(L, c, dev, aggs=aggs, sets=sets)
+                assert rc == c.E_CUDA and total == 0 and ng == 0 and err
+    with pytest.raises(c.B2SError) as e:
+        c.aggregate_grouping_sets_partition_compress_rows_hash_packed(
+            c.CODEC_LZ4BLOCK, np.zeros(28, np.uint8), [28], [(c.KEY_INT64, 8, 8, -1)], [], [1, 0], 200,
+            np.zeros(64, np.uint8))
+    assert e.value.code == c.E_CUDA
+
+
+@pytest.mark.skipif(_has_gpu(), reason="GPU present: the zero-filled records would be bad records")
+def test_fifteen_keys_and_sixteen_buffers_are_well_formed_without_a_device():
+    """15 grouping columns, gid and 16 buffers make the 32 fields of one null word"""
+    c = pkg.capi
+    L = c.load()
+    keys = tuple((1, 8 + 8 * k, 4, k) for k in range(15))
+    rc, _, _, _ = _call(L, c, keys=keys, aggs=[(AVG, I64, 16, 1)] * 8, sets=(0x7FFF, 0x3FFF, 1, 0))
+    assert rc == c.E_CUDA
+
+
+@pytest.mark.parametrize("kw", [
+    # the grouping sets'
+    dict(keys=((1, 8, 4, 0),) * 16), dict(keys=()), dict(sets=()), dict(n_sets=0), dict(mask_array=False),
+    dict(sets=(0b100,)), dict(sets=(0b11, 1 << 31)), dict(sets=(0b01, 0, 0b01)), dict(sets=(0, 0)),
+    dict(n=2**31, sets=(0b11, 0)), dict(n=2**30, sets=(3, 2, 1, 0)),
+    # the partial aggregation call's, passed through: the hash call's ...
+    dict(R=0), dict(keys=((4, 8, 8, -1),)), dict(keys=((0, 8, 2, -1),)), dict(keys=((1 | (1 << 8), 8, 4, -1),)),
+    dict(keys=((1, 8, 4, -2),)), dict(records=False), dict(n=2**32, rec_len=(44, 44)),
+    # ... and the aggregates'
+    dict(aggs=[(SUM, I64, 16, 1)] * 17), dict(agg_arrays=False), dict(groups=False), dict(aggs=[(5, I64, 16, 1)]),
+    dict(aggs=[(SUM, 9, 16, 1)]), dict(aggs=[(SUM, dec(39), 16, 1)]), dict(aggs=[(SUM, NONE, 0, -1)]),
+    dict(aggs=[(MIN, I8, 16, 1)]), dict(aggs=[(MAX, BYTES, 16, 1)]), dict(aggs=[(SUM, dec(29), 16, 1)]),
+    dict(aggs=[(AVG, dec(28), 16, 1)]), dict(aggs=[(AVG, I64, 16, 1)] * 9), dict(aggs=[(SUM, I64, 12, 1)]),
+    dict(aggs=[(SUM, I64, 16, 65536)])])
+def test_ill_formed_calls_are_argument_errors_before_the_device(kw):
+    c = pkg.capi
+    L = c.load()
+    for dev in (False, True):
+        rc, total, ng, err = _call(L, c, dev, **kw)
+        assert rc == c.E_ARG and total == 0 and err, kw
+        assert ng == (0 if kw.get("groups", True) else 9), kw  # *n_groups is zeroed when there is one
+
+
+def test_grouping_set_rejections_name_their_rule():
+    c = pkg.capi
+    L = c.load()
+    for kw, words in ((dict(keys=((1, 8, 4, 0),) * 16), b"[1, 15]"), (dict(n_sets=0), b"n_sets"),
+                      (dict(sets=(0b100,)), b"n_keys"), (dict(sets=(1, 1)), b"equal"),
+                      (dict(n=2**31, sets=(0b11, 0)), b"2^32")):
+        rc, _, _, err = _call(L, c, **kw)
+        assert rc == c.E_ARG and words in err, (kw, err)
+
+
+def test_prototypes_match_the_headers():
+    protos = dict((p[0], p[2]) for p in pkg.capi.PROTOTYPES)
+    assert [len(protos[n]) for n in NAMES] == [29, 30]
+    assert set(NAMES) <= set(pkg.capi.SYMBOLS)
+    hdr = open(os.path.join(ROOT, "include", "b200shuffle.h")).read()
+    for name in NAMES:
+        decl = re.search(name + r"\(([^;]*)\);", hdr).group(1)
+        assert decl.count(",") + 1 == len(protos[name])
+        assert "uint32_t n_sets, const uint32_t* set_mask" in " ".join(decl.split())
+    hp = dict((p[0], p[2]) for p in pkg.host.PROTOTYPES)
+    assert "b2sh_serialized_writer_grouping_sets" in pkg.host.SYMBOLS
+    host = open(os.path.join(ROOT, "include", "b200shuffle_host.h")).read()
+    decl = re.search(r"b2sh_serialized_writer_grouping_sets\(([^;]*)\);", host).group(1)
+    assert decl.count(",") + 1 == len(hp["b2sh_serialized_writer_grouping_sets"]) == 3
