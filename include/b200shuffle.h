@@ -1042,6 +1042,66 @@ int b2s_decompress_window_offset_rows_keys_dev(
     const uint64_t* fn_default, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records,
     uint64_t* n_out_records, int32_t* status, int32_t* bad_slice);
 
+/* ---- read side, window frames: Spark's WindowExec over sliding ROWS and RANGE frames on a reducer's UnsafeRows ----
+ * b2s_decompress_window_offset_rows_keys_*, with two more per-function arrays after fn_default: frame_lower[j] and
+ * frame_upper[j].  Everything not stated here is that call's, and one fn array mixes ranking functions, LAG / LEAD, the
+ * older frames and the new ones.  fn_frame[j] may also be B2S_WINDOW_FRAME_ROWS or B2S_WINDOW_FRAME_RANGE, for SUM,
+ * COUNT, MIN, MAX, AVG, FIRST, LAST and NTH_VALUE (not ranking functions, LAG or LEAD); then frame_lower[j] /
+ * frame_upper[j] are the frame's bounds: B2S_WINDOW_UNBOUNDED_PRECEDING (lower only), B2S_WINDOW_UNBOUNDED_FOLLOWING
+ * (upper only), 0 CURRENT ROW, -k k PRECEDING, +k k FOLLOWING.  Frames 0..3 keep their meaning with both bounds 0.
+ * Frames.  With [ps, pe) the partition's sorted positions and i a record's, its frame is the span [s, e] (possibly
+ * empty) that Spark 3.5's frame classes produce for these bounds: UnboundedPreceding (lower unbounded: the running
+ * fold, read at e), UnboundedFollowing (upper unbounded: a fresh fold from s to the partition's end), Unbounded (both:
+ * the partition) and Sliding (any other: a fresh fold of the buffered rows from s).
+ *   ROWS   [max(ps, i + lower), min(pe - 1, i + upper)]: RowBoundOrdering's j - (i + k).  Offsets fit in an int.
+ *   RANGE  the positions whose order value lies between the bounds in the column's sort order (RangeBoundOrdering):
+ *          CURRENT ROW is the peer group's edge and takes any order key; an offset bound is v + k ascending and
+ *          v + (-k) descending in the column type's arithmetic, null when v is null (a null bound equals the null
+ *          inputs and sorts before or after every value by the null order, so a null-keyed row's frame is its null
+ *          peers).  An offset needs exactly one ORDER BY column (n_keys - n_partition_keys == 1) of type B2S_KEY_INT8,
+ *          _INT16, _INT32 (int or date) or _INT64, any direction and null order; it must fit the column's type and,
+ *          descending, not be the type's minimum.  Float, double, decimal and interval offsets are not taken.
+ * Values, folded over [s, e] in sorted order from s: SUM of an integral the wrapping 64-bit sum, of a decimal exact;
+ * COUNT the non-null inputs (0 on an empty frame, never null); MIN / MAX the first of equal values with its bits; SUM of
+ * a float or double and AVG of a non-decimal ((0.0 + x_s) + x_{s+1}) + ... in double (for an unbounded lower end the
+ * running fold at e); AVG of a decimal the exact sum rounded HALF_UP as in the aggregate call; FIRST / LAST /
+ * NTH_VALUE the input at s, at e, or at s + n - 1 if that is <= e (IGNORE_NULLS: the first, last or n-th non-null
+ * input in [s, e]).  An empty frame gives null for everything but COUNT.
+ * Errors -> B2S_E_ARG, before the device: everything the offset call rejects (with frames 4 and 5 accepted as above);
+ * NULL frame_lower or frame_upper; non-zero bounds on frames 0..3; UNBOUNDED FOLLOWING as a lower or UNBOUNDED
+ * PRECEDING as an upper bound; lower above upper; a ROWS offset outside the int range; a RANGE offset without exactly
+ * one ORDER BY column of the four integral key types, or that does not fit the column (descending: or is its minimum).
+ * B2S_E_UNSUPPORTED (the caller keeps Spark's window; nothing is written), where Spark's int compare or bound arithmetic
+ * would wrap and its buffer loop no longer matches these frames: a partition of N records with N - 1 + |k| > 2^31 - 1
+ * for a finite ROWS offset k, or a non-null order value v whose exact v +- k leaves the column's type.  Everything else
+ * (the output row, B2S_E_CORRUPT, B2S_E_DST_TOO_SMALL, B2S_E_NOMEM, the lane, the trim, b2s_last_timing) is the offset
+ * call's.  b2s_decompress_window_aggregate_rows_keys_* and b2s_decompress_window_offset_rows_keys_* keep rejecting
+ * frames 4 and 5. */
+#define B2S_WINDOW_FRAME_ROWS 4
+#define B2S_WINDOW_FRAME_RANGE 5
+#define B2S_WINDOW_UNBOUNDED_PRECEDING INT64_MIN
+#define B2S_WINDOW_UNBOUNDED_FOLLOWING INT64_MAX
+int b2s_decompress_window_frame_rows_keys_packed(
+    uint32_t codec, uint32_t checksum_alg, uint32_t n, const uint8_t* src_base, const uint64_t* src_off,
+    const uint64_t* src_len, const uint32_t* slice_base, const uint64_t* slice_len, const uint64_t* slice_checksum,
+    uint32_t n_partition_keys, uint32_t n_keys, const uint32_t* key_type, const uint32_t* key_off,
+    const uint32_t* key_len, const int32_t* key_null_field, uint32_t n_fields, const uint8_t* field_kind,
+    uint32_t n_fns, const uint32_t* fn, const int32_t* fn_arg, const uint32_t* fn_frame, const uint32_t* val_type,
+    const uint32_t* val_off, const int32_t* val_null_field, const uint32_t* fn_flags, const uint64_t* fn_default,
+    const int64_t* frame_lower, const int64_t* frame_upper, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_total,
+    uint64_t* n_records, uint64_t* n_out_records, int32_t* status, int32_t* bad_slice);
+/* same, with src_base / dst_base in device memory of dev_index; every array stays a host array */
+int b2s_decompress_window_frame_rows_keys_dev(
+    uint32_t dev_index, uint32_t codec, uint32_t checksum_alg, uint32_t n, const uint8_t* src_base,
+    const uint64_t* src_off, const uint64_t* src_len, const uint32_t* slice_base, const uint64_t* slice_len,
+    const uint64_t* slice_checksum, uint32_t n_partition_keys, uint32_t n_keys, const uint32_t* key_type,
+    const uint32_t* key_off, const uint32_t* key_len, const int32_t* key_null_field, uint32_t n_fields,
+    const uint8_t* field_kind, uint32_t n_fns, const uint32_t* fn, const int32_t* fn_arg, const uint32_t* fn_frame,
+    const uint32_t* val_type, const uint32_t* val_off, const int32_t* val_null_field, const uint32_t* fn_flags,
+    const uint64_t* fn_default, const int64_t* frame_lower, const int64_t* frame_upper, uint8_t* dst_base,
+    uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records, uint64_t* n_out_records, int32_t* status,
+    int32_t* bad_slice);
+
 /* ---- exchange cache: map outputs kept resident in HBM for reducers on the same device ----
  * (docs/f4_gpu_resident_exchange.md steps 2 and 3, local half.)  The serialized writer's partition step already leaves
  * a map task's records partitioned by reduce id in HBM; the cached store keeps that arena, keyed by (shuffle_id,

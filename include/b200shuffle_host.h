@@ -267,6 +267,17 @@ int b2sh_reader_read_window_offset_rows(b2sh_reader* r, uint32_t n_partition_key
                                         const int32_t* val_null_field, const uint32_t* fn_flags,
                                         const uint64_t* fn_default, const uint8_t** data, uint64_t* len,
                                         uint64_t* n_records, uint64_t* n_out_records);
+/* read_window_frame_rows(): read_window_offset_rows() with sliding ROWS and RANGE frames (INTEGRATION.md §3o): ONE
+ * b2s_decompress_window_frame_rows_keys_packed call instead, whose arguments these are.  Fetched blocks only. */
+int b2sh_reader_read_window_frame_rows(b2sh_reader* r, uint32_t n_partition_keys, uint32_t n_keys,
+                                       const uint32_t* key_type, const uint32_t* key_off, const uint32_t* key_len,
+                                       const int32_t* key_null_field, uint32_t n_fields, const uint8_t* field_kind,
+                                       uint32_t n_fns, const uint32_t* fn, const int32_t* fn_arg,
+                                       const uint32_t* fn_frame, const uint32_t* val_type, const uint32_t* val_off,
+                                       const int32_t* val_null_field, const uint32_t* fn_flags,
+                                       const uint64_t* fn_default, const int64_t* frame_lower,
+                                       const int64_t* frame_upper, const uint8_t** data, uint64_t* len,
+                                       uint64_t* n_records, uint64_t* n_out_records);
 int b2sh_reader_block(b2sh_reader* r, uint32_t k, int64_t* map_id, int32_t* start_reduce, int32_t* end_reduce,
                       const uint8_t** data, uint64_t* len);
 uint64_t b2sh_reader_remote_bytes_read(b2sh_reader* r); /* metric parity with storage/S3ShuffleReader.scala:94-95 */

@@ -42,6 +42,10 @@ WINDOW_FRAME_PARTITION, WINDOW_FRAME_ROWS_RUNNING, WINDOW_FRAME_RANGE_RUNNING = 
 WINDOW_LAG, WINDOW_LEAD, WINDOW_FIRST, WINDOW_LAST, WINDOW_NTH_VALUE = range(11, 16)
 WINDOW_VAL_BYTES = 8
 WINDOW_IGNORE_NULLS, WINDOW_HAS_DEFAULT = 1, 2
+# the sliding frames of the frame window (decompress_window_frame_rows_keys_*) and their unbounded ends; a bound is
+# otherwise 0 (CURRENT ROW), -k (k PRECEDING) or +k (k FOLLOWING)
+WINDOW_FRAME_ROWS, WINDOW_FRAME_RANGE = 4, 5
+WINDOW_UNBOUNDED_PRECEDING, WINDOW_UNBOUNDED_FOLLOWING = -2**63, 2**63 - 1
 
 
 def window_val_decimal(p, s):
@@ -189,6 +193,14 @@ PROTOTYPES = [
      [_u32, _u32, _u32, _u32, _vp, _u64p, _u64p, _u32p, _u64p, _u64p, _u32, _u32, _u32p, _u32p, _u32p, _i32p, _u32,
       _u8p, _u32, _u32p, _i32p, _u32p, _u32p, _u32p, _i32p, _u32p, _u64p, _vp, _u64, _u64p, _u64p, _u64p, _i32p,
       _i32p]),
+    ("b2s_decompress_window_frame_rows_keys_packed", C.c_int,
+     [_u32, _u32, _u32, _u8p, _u64p, _u64p, _u32p, _u64p, _u64p, _u32, _u32, _u32p, _u32p, _u32p, _i32p, _u32, _u8p,
+      _u32, _u32p, _i32p, _u32p, _u32p, _u32p, _i32p, _u32p, _u64p, _vp, _vp, _u8p, _u64, _u64p, _u64p, _u64p, _i32p,
+      _i32p]),
+    ("b2s_decompress_window_frame_rows_keys_dev", C.c_int,
+     [_u32, _u32, _u32, _u32, _vp, _u64p, _u64p, _u32p, _u64p, _u64p, _u32, _u32, _u32p, _u32p, _u32p, _i32p, _u32,
+      _u8p, _u32, _u32p, _i32p, _u32p, _u32p, _u32p, _i32p, _u32p, _u64p, _vp, _vp, _vp, _u64, _u64p, _u64p, _u64p,
+      _i32p, _i32p]),
     ("b2s_exchange_set_budget", C.c_int, [_u32, _u64]),
     ("b2s_partition_compress_cached_packed", C.c_int,
      [_i32, C.c_int64, _u32, _i32, _u32, _u32, _u32, _u64, _u8p, _u64, _u32p, _u32p, _u8p, _u64, _u64p, _u64p, _u64p,
@@ -672,6 +684,28 @@ def _window_offset_arrays(keys, n_partition_keys, n_fields, kinds, fns):
     return _window_aggregate_arrays(keys, n_partition_keys, n_fields, kinds, fns, offset=True)
 
 
+def _window_frame_arrays(keys, n_partition_keys, n_fields, kinds, fns):
+    """the frame window's arguments: the offset window's, fns also taking (fn, arg, frame, val_type, val_off,
+    val_null_field, flags, default, lower, upper) (every other form has bounds 0), with the bounds appended"""
+    bounds = [tuple(f[8:]) if isinstance(f, tuple) and len(f) == 10 else (0, 0) for f in fns]
+    rows = [tuple(f[:8]) if isinstance(f, tuple) and len(f) == 10 else f for f in fns]
+    lo, hi = (np.array([b[u] for b in bounds] or [0], dtype=np.int64) for u in (0, 1))
+    return _window_aggregate_arrays(keys, n_partition_keys, n_fields, kinds, rows, offset=True) + (lo, hi)
+
+
+def decompress_window_frame_rows_keys_packed(codec, src, off, length, dst, keys, n_partition_keys, n_fields, kinds, fns,
+                                             checksum_alg=CHECKSUM_NONE, slice_base=None, slice_len=None,
+                                             slice_checksum=None):
+    """Spark's WindowExec over sliding ROWS and RANGE frames (with ranking, offset and aggregate functions) over a
+    reducer's UnsafeRow records: as decompress_window_offset_rows_keys_packed, fns also taking (fn, arg, frame,
+    val_type, val_off, val_null_field, flags, default, lower, upper) with frame WINDOW_FRAME_ROWS or WINDOW_FRAME_RANGE
+    and the bounds WINDOW_UNBOUNDED_PRECEDING / WINDOW_UNBOUNDED_FOLLOWING, 0 (CURRENT ROW), -k or +k.
+    -> dict(total, n_records, n_out_records, status, bad_slice)"""
+    return _sort_call("b2s_decompress_window_frame_rows_keys_packed", codec, src, off, length, dst, None,
+                      _window_frame_arrays(keys, n_partition_keys, n_fields, kinds, fns), checksum_alg,
+                      (slice_base, slice_len, slice_checksum))
+
+
 def decompress_window_offset_rows_keys_packed(codec, src, off, length, dst, keys, n_partition_keys, n_fields, kinds,
                                               fns, checksum_alg=CHECKSUM_NONE, slice_base=None, slice_len=None,
                                               slice_checksum=None):
@@ -836,6 +870,15 @@ def decompress_window_rows_keys_dev(codec, d_src, off, length, d_dst, dst_cap, k
     return _sort_call("b2s_decompress_window_rows_keys_dev", codec, d_src, off, length, d_dst, dst_cap,
                       _window_arrays(keys, n_partition_keys, n_fields, kinds, fns, limit), checksum_alg,
                       (slice_base, slice_len, slice_checksum), dev)
+
+
+def decompress_window_frame_rows_keys_dev(codec, d_src, off, length, d_dst, dst_cap, keys, n_partition_keys, n_fields,
+                                          kinds, fns, checksum_alg=CHECKSUM_NONE, slice_base=None, slice_len=None,
+                                          slice_checksum=None, dev=0):
+    """decompress_window_frame_rows_keys_packed on device-resident blocks (d_src) into a device arena (d_dst)"""
+    return _sort_call("b2s_decompress_window_frame_rows_keys_dev", codec, d_src, off, length, d_dst, dst_cap,
+                      _window_frame_arrays(keys, n_partition_keys, n_fields, kinds, fns), checksum_alg,
+                      (slice_base, slice_len, slice_checksum), dev=dev)
 
 
 def decompress_window_offset_rows_keys_dev(codec, d_src, off, length, d_dst, dst_cap, keys, n_partition_keys, n_fields,

@@ -2581,6 +2581,9 @@ struct WindowSpec {
   bool offset = false;
   const uint32_t* flags = nullptr;
   const uint64_t* dflt = nullptr;
+  bool frames = false;  // the frame call (b2s_decompress_window_frame_rows_keys_*, agg and offset): sliding bounds
+  const int64_t* lower = nullptr;
+  const int64_t* upper = nullptr;
 };
 static RecordSpec fixed_spec(uint32_t record_bytes, uint32_t key_off, uint32_t key_len) {
   RecordSpec r;
@@ -2835,7 +2838,8 @@ static int window_agg_fn_args(const WindowSpec& ws) {
                                        : "fn_arg must be NTILE's bucket count (at least 1), and 0 for every other "
                                          "function%s");
     const bool ranking = fn <= B2S_WINDOW_NTILE;
-    if (ranking || lag_lead ? frame != 0 : frame < B2S_WINDOW_FRAME_PARTITION || frame > B2S_WINDOW_FRAME_RANGE_RUNNING)
+    const uint32_t max_frame = ws.frames ? B2S_WINDOW_FRAME_RANGE : B2S_WINDOW_FRAME_RANGE_RUNNING;
+    if (ranking || lag_lead ? frame != 0 : frame < B2S_WINDOW_FRAME_PARTITION || frame > max_frame)
       return fail(B2S_E_ARG, ws.offset ? "fn_frame must be 0 for a ranking function, LAG and LEAD, and a "
                                          "B2S_WINDOW_FRAME_* for an aggregate, FIRST, LAST and NTH_VALUE%s"
                                        : "fn_frame must be 0 for a ranking function and a B2S_WINDOW_FRAME_* for an "
@@ -2894,6 +2898,47 @@ static int window_offset_fn_args(const WindowSpec& ws) {
                            : kind == B2S_WINDOW_VAL_INT32 || kind == B2S_WINDOW_VAL_FLOAT32 ? 4 : 8;
     if (width < 8 && ws.dflt[j] >> (8 * width))
       return fail(B2S_E_ARG, "fn_default has bits above its type's width%s");
+  }
+  return 0;
+}
+
+// The frame window call's checks of its functions, before the device (b2s_decompress_window_frame_rows_keys_*): the
+// offset call's, with frames 4 and 5 for the functions that take a frame, then each function's bounds, and a RANGE
+// offset's order column (n_keys, key_type: the caller's key; the key itself is checked with the sort's)
+static int window_frame_fn_args(const WindowSpec& ws, uint32_t n_keys, const uint32_t* key_type) {
+  if (int rc = window_offset_fn_args(ws)) return rc;
+  if (!ws.lower || !ws.upper) return fail(B2S_E_ARG, "null argument%s");
+  for (uint32_t j = 0; j < ws.n_fns; j++) {
+    const int64_t lo = ws.lower[j], hi = ws.upper[j];
+    const uint32_t frame = ws.frame[j];
+    if (frame != B2S_WINDOW_FRAME_ROWS && frame != B2S_WINDOW_FRAME_RANGE) {
+      if (lo || hi) return fail(B2S_E_ARG, "frame_lower and frame_upper must be 0 unless fn_frame is "
+                                           "B2S_WINDOW_FRAME_ROWS or B2S_WINDOW_FRAME_RANGE%s");
+      continue;
+    }
+    if (lo == B2S_WINDOW_UNBOUNDED_FOLLOWING || hi == B2S_WINDOW_UNBOUNDED_PRECEDING)
+      return fail(B2S_E_ARG, "UNBOUNDED FOLLOWING is an upper bound and UNBOUNDED PRECEDING a lower one%s");
+    if (lo > hi) return fail(B2S_E_ARG, "a frame's lower bound must not exceed its upper bound%s");
+    if (frame == B2S_WINDOW_FRAME_ROWS)
+      for (const int64_t k : {lo, hi})
+        if (k != B2S_WINDOW_UNBOUNDED_PRECEDING && k != B2S_WINDOW_UNBOUNDED_FOLLOWING &&
+            (k < INT32_MIN || k > INT32_MAX))
+          return fail(B2S_E_ARG, "a ROWS frame's offset must fit in an int%s");
+    if (frame != B2S_WINDOW_FRAME_RANGE) continue;
+    for (const int64_t k : {lo, hi}) {  // an offset: one integral ORDER BY column whose type the offset fits
+      if (k == 0 || k == B2S_WINDOW_UNBOUNDED_PRECEDING || k == B2S_WINDOW_UNBOUNDED_FOLLOWING) continue;
+      if (n_keys != ws.n_partition_keys + 1 || n_keys > kMaxKeys || !key_type)
+        return fail(B2S_E_ARG, "a RANGE frame with an offset needs exactly one ORDER BY column%s");
+      const uint32_t ty = key_type[ws.n_partition_keys], base = ty & kKeyTypeMask;
+      const int bits = base == B2S_KEY_INT8 ? 8 : base == B2S_KEY_INT16 ? 16 : base == B2S_KEY_INT32 ? 32
+                       : base == B2S_KEY_INT64 ? 64 : 0;
+      if (!bits)
+        return fail(B2S_E_ARG, "a RANGE frame's offset needs a byte, short, int, date or long ORDER BY column%s");
+      const int64_t tmax = bits == 64 ? INT64_MAX : (int64_t)((1ull << (bits - 1)) - 1), tmin = -tmax - 1;
+      if (k < tmin || k > tmax || ((ty & B2S_KEY_DESCENDING) && k == tmin))
+        return fail(B2S_E_ARG, "a RANGE frame's offset must fit its ORDER BY column's type (and not be its minimum "
+                               "when descending)%s");
+    }
   }
   return 0;
 }
@@ -3929,6 +3974,41 @@ static void window_shape(const RecordSpec& spec, WindowShape& shape) {
     if ((vt & 0xff) == B2S_WINDOW_VAL_DECIMAL && ws.fn[j] != B2S_WINDOW_COUNT && rp > 18)
       shape.wide[j] = (int32_t)shape.n_wide++;
   }
+  for (uint32_t j = 0; j < ws.n_fns; j++) {  // sliding frames: bounds sets, result states, the staged order column
+    shape.bnd[j] = shape.res[j] = -1;
+    if (!ws.frames || (ws.frame[j] != B2S_WINDOW_FRAME_ROWS && ws.frame[j] != B2S_WINDOW_FRAME_RANGE)) continue;
+    const int64_t lo = ws.lower[j], hi = ws.upper[j];
+    uint32_t b = 0;
+    while (b < shape.n_bnd && !(shape.bkind[b] == ws.frame[j] && shape.blo[b] == lo && shape.bhi[b] == hi)) b++;
+    if (b == shape.n_bnd) {
+      shape.bkind[b] = ws.frame[j];
+      shape.blo[b] = lo;
+      shape.bhi[b] = hi;
+      shape.n_bnd++;
+    }
+    shape.bnd[j] = (int32_t)b;
+    const bool finite = [](int64_t k) {
+      return k != 0 && k != B2S_WINDOW_UNBOUNDED_PRECEDING && k != B2S_WINDOW_UNBOUNDED_FOLLOWING;
+    }(lo) || (hi != 0 && hi != B2S_WINDOW_UNBOUNDED_PRECEDING && hi != B2S_WINDOW_UNBOUNDED_FOLLOWING);
+    if (ws.frame[j] == B2S_WINDOW_FRAME_RANGE && finite) {
+      const uint32_t c = ws.n_partition_keys;
+      shape.ord_staged = true;
+      shape.ord_type = spec.keys.type[c];
+      shape.ord_off = spec.keys.off[c];
+      shape.ord_len = spec.keys.len[c];
+      shape.ord_null = spec.keys.null_field[c];
+    }
+    const uint32_t fn = ws.fn[j], kind = ws.val_type[j] & 0xff;
+    if (lo == B2S_WINDOW_UNBOUNDED_PRECEDING || fn < B2S_WINDOW_SUM || fn > B2S_WINDOW_AVG) continue;
+    const bool dbl = (fn == B2S_WINDOW_SUM && (kind == B2S_WINDOW_VAL_FLOAT32 || kind == B2S_WINDOW_VAL_FLOAT64)) ||
+                     (fn == B2S_WINDOW_AVG && kind != B2S_WINDOW_VAL_DECIMAL);
+    if (!dbl && fn != B2S_WINDOW_MIN && fn != B2S_WINDOW_MAX) continue;  // sums and counts: prefix differences
+    shape.res[j] = (int32_t)shape.n_res++;
+    if (dbl) continue;
+    const bool rows = ws.frame[j] == B2S_WINDOW_FRAME_ROWS && hi != B2S_WINDOW_UNBOUNDED_FOLLOWING;
+    const uint64_t width = rows ? (uint64_t)(hi - lo + 1) : ~0ull;
+    shape.rmq_width = std::max(shape.rmq_width, width);
+  }
   shape.limit_fn = ws.limit_fn;
   shape.limit = ws.limit;
   shape.part.n = ws.n_partition_keys;
@@ -4178,8 +4258,8 @@ static int window_rows_tail(Slot& S, const RecordSpec& spec, DecodedTask& T, con
   for (uint32_t f = 0; f < ws.n_fields; f++)
     if (ws.kind[f] != B2S_FIELD_FIXED) fields.push_back(f);
   shape.n_var = (uint32_t)fields.size();
-  // output records, output bytes, a row too long, a partition too large, a bad decimal input
-  uint64_t wb[5] = {0, 0, 0, 0, ~0ull};
+  // output records, output bytes, a row too long, a partition too large, a bad decimal input, a frame bound wraps
+  uint64_t wb[6] = {0, 0, 0, 0, ~0ull, 0};
   CU(S.mark(G0, st, *launches));
   if (R.records) {
     launch_rows_group(T.arena, R.records, R.idx, R.heads, R.key_bytes, AggSpec{}, R.ws, R.gws, st, launches);
@@ -4196,6 +4276,9 @@ static int window_rows_tail(Slot& S, const RecordSpec& spec, DecodedTask& T, con
                                          : "a decimal input's size is not in [1, 16] or its bytes run past the end of "
                                            "its row");
   if (wb[3]) return fail(B2S_E_UNSUPPORTED, "a window partition holds more than 2^31 - 1 records%s");
+  if (wb[5])
+    return fail(B2S_E_UNSUPPORTED, "a sliding frame's bound wraps in Spark's int arithmetic (a partition's size plus "
+                                   "a ROWS offset past 2^31 - 1, or a RANGE bound outside its column's type)%s");
   if (wb[2]) return fail(B2S_E_UNSUPPORTED, "an output row is longer than 2^31 - 1 bytes%s");
   *total = wb[1];
   if (wb[1] > out_cap)
@@ -4642,7 +4725,9 @@ static int window_call(uint32_t dev_index, bool packed, uint32_t codec, uint32_t
   if (ws.agg) {
     if (dst_total) *dst_total = 0;
     if (n_out_records) *n_out_records = 0;
-    if (int rc = ws.offset ? window_offset_fn_args(ws) : window_agg_fn_args(ws)) {
+    if (int rc = ws.frames   ? window_frame_fn_args(ws, n_keys, key_type)
+                 : ws.offset ? window_offset_fn_args(ws)
+                             : window_agg_fn_args(ws)) {
       begin_call();  // a new call, with an empty b2s_last_timing
       return rc;
     }
@@ -4785,6 +4870,52 @@ int b2s_decompress_window_offset_rows_keys_dev(
     uint64_t* n_out_records, int32_t* status, int32_t* bad_slice) {
   WindowSpec ws = window_offset_spec(n_partition_keys, n_fields, field_kind, n_fns, fn, fn_arg, fn_frame, val_type,
                                      val_off, val_null_field, fn_flags, fn_default, n_records);
+  return window_call(dev_index, false, codec, checksum_alg, n, src_base, src_off, src_len, slice_base, slice_len,
+                     slice_checksum, n_keys, key_type, key_off, key_len, key_null_field, ws, dst_base, dst_cap,
+                     dst_total, n_out_records, status, bad_slice);
+}
+
+static WindowSpec window_frame_spec(uint32_t n_partition_keys, uint32_t n_fields, const uint8_t* field_kind,
+                                    uint32_t n_fns, const uint32_t* fn, const int32_t* fn_arg, const uint32_t* fn_frame,
+                                    const uint32_t* val_type, const uint32_t* val_off, const int32_t* val_null_field,
+                                    const uint32_t* fn_flags, const uint64_t* fn_default, const int64_t* frame_lower,
+                                    const int64_t* frame_upper, uint64_t* n_records) {
+  WindowSpec ws = window_offset_spec(n_partition_keys, n_fields, field_kind, n_fns, fn, fn_arg, fn_frame, val_type,
+                                     val_off, val_null_field, fn_flags, fn_default, n_records);
+  ws.frames = true;
+  ws.lower = frame_lower;
+  ws.upper = frame_upper;
+  return ws;
+}
+
+int b2s_decompress_window_frame_rows_keys_packed(
+    uint32_t codec, uint32_t checksum_alg, uint32_t n, const uint8_t* src_base, const uint64_t* src_off,
+    const uint64_t* src_len, const uint32_t* slice_base, const uint64_t* slice_len, const uint64_t* slice_checksum,
+    uint32_t n_partition_keys, uint32_t n_keys, const uint32_t* key_type, const uint32_t* key_off,
+    const uint32_t* key_len, const int32_t* key_null_field, uint32_t n_fields, const uint8_t* field_kind,
+    uint32_t n_fns, const uint32_t* fn, const int32_t* fn_arg, const uint32_t* fn_frame, const uint32_t* val_type,
+    const uint32_t* val_off, const int32_t* val_null_field, const uint32_t* fn_flags, const uint64_t* fn_default,
+    const int64_t* frame_lower, const int64_t* frame_upper, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_total,
+    uint64_t* n_records, uint64_t* n_out_records, int32_t* status, int32_t* bad_slice) {
+  WindowSpec ws = window_frame_spec(n_partition_keys, n_fields, field_kind, n_fns, fn, fn_arg, fn_frame, val_type,
+                                    val_off, val_null_field, fn_flags, fn_default, frame_lower, frame_upper, n_records);
+  return window_call(t_device, true, codec, checksum_alg, n, src_base, src_off, src_len, slice_base, slice_len,
+                     slice_checksum, n_keys, key_type, key_off, key_len, key_null_field, ws, dst_base, dst_cap,
+                     dst_total, n_out_records, status, bad_slice);
+}
+
+int b2s_decompress_window_frame_rows_keys_dev(
+    uint32_t dev_index, uint32_t codec, uint32_t checksum_alg, uint32_t n, const uint8_t* src_base,
+    const uint64_t* src_off, const uint64_t* src_len, const uint32_t* slice_base, const uint64_t* slice_len,
+    const uint64_t* slice_checksum, uint32_t n_partition_keys, uint32_t n_keys, const uint32_t* key_type,
+    const uint32_t* key_off, const uint32_t* key_len, const int32_t* key_null_field, uint32_t n_fields,
+    const uint8_t* field_kind, uint32_t n_fns, const uint32_t* fn, const int32_t* fn_arg, const uint32_t* fn_frame,
+    const uint32_t* val_type, const uint32_t* val_off, const int32_t* val_null_field, const uint32_t* fn_flags,
+    const uint64_t* fn_default, const int64_t* frame_lower, const int64_t* frame_upper, uint8_t* dst_base,
+    uint64_t dst_cap, uint64_t* dst_total, uint64_t* n_records, uint64_t* n_out_records, int32_t* status,
+    int32_t* bad_slice) {
+  WindowSpec ws = window_frame_spec(n_partition_keys, n_fields, field_kind, n_fns, fn, fn_arg, fn_frame, val_type,
+                                    val_off, val_null_field, fn_flags, fn_default, frame_lower, frame_upper, n_records);
   return window_call(dev_index, false, codec, checksum_alg, n, src_base, src_off, src_len, slice_base, slice_len,
                      slice_checksum, n_keys, key_type, key_off, key_len, key_null_field, ws, dst_base, dst_cap,
                      dst_total, n_out_records, status, bad_slice);

@@ -632,13 +632,31 @@ struct WindowShape {
   uint64_t dflt[kMaxWindowFns];
   int32_t nn[kMaxWindowFns];
   uint32_t n_off, n_nn, n_wide_off;
+  // Sliding frames (fn_frame B2S_WINDOW_FRAME_ROWS / _RANGE): function f's frame is bounds set bnd[f] (-1: an older
+  // frame), one per distinct (frame, lower, upper): its frame code bkind, and its bounds blo / bhi (INT64_MIN /
+  // INT64_MAX unbounded, 0 CURRENT ROW, else the signed offset).  An aggregate whose frame value is not read from the
+  // prefix folds has its own result state at index res[f] among n_res (-1 otherwise): a MIN / MAX with a bounded lower
+  // end (range-minimum passes over frames of at most rmq_width positions; 0: none, ~0: unbounded) or a double fold with
+// one (a fold per row).  The
+  // order column of a RANGE offset (ord_type with its flags, slot, width and null bit) is staged when ord_staged.
+  int32_t bnd[kMaxWindowFns];
+  uint32_t n_bnd;
+  uint32_t bkind[kMaxWindowFns];
+  int64_t blo[kMaxWindowFns], bhi[kMaxWindowFns];
+  int32_t res[kMaxWindowFns];
+  uint32_t n_res;
+  uint64_t rmq_width;
+  bool ord_staged;
+  uint32_t ord_type, ord_off, ord_len;
+  int32_t ord_null;
 };
 // d_wws: window_ws_bytes(n, shape) bytes
 size_t window_ws_bytes(uint64_t n, const WindowShape& shape);
 // the readback: [output records, output bytes, an output row is too long (0 / 1), a partition is too large (0 / 1),
-// the first bad DECIMAL_WIDE or string input (its arena offset << 2 | kAggBadDecimal or kWindowBadBytes; ~0: none)]
+// the first bad DECIMAL_WIDE or string input (its arena offset << 2 | kAggBadDecimal or kWindowBadBytes; ~0: none),
+// a sliding frame's bound would wrap in Spark's arithmetic (0 / 1)]
 uint64_t* window_readback(uint8_t* d_wws, uint64_t n, const WindowShape& shape);
-constexpr size_t kWindowReadbackBytes = 40;
+constexpr size_t kWindowReadbackBytes = 48;
 constexpr uint64_t kWindowBadBytes = 2;  // an offset function's string input lies outside its row's var region
 // Per sorted position: whether it starts a partition (only peer heads compare their partition columns with their
 // predecessor's, encoded 16 bytes at a time), scanned, and the partitions' starts compacted; with aggregate functions,

@@ -19,6 +19,10 @@
 //            position combining with the one d before it while that is in its partition (min / max keep the earlier
 //            of equal values).  Double sums are serial by contract: a warp per partition, 32 positions a round loaded
 //            one round ahead, each lane's value broadcast in turn and added in order, each lane keeping its prefix
+//   frames : (sliding ROWS / RANGE frames) one thread per sorted position: each distinct bounds set's frame [fs, ft),
+//            by arithmetic, the peer group, or a binary search over the staged RANGE column; then, from the staged
+//            inputs, range-minimum passes for MIN / MAX and a fresh double fold per row for double sums whose frame's
+//            lower end is bounded (every other aggregate reads the prefix folds at both ends of its frame)
 //   values : one thread per sorted position: from its partition's bounds and its peer group's bounds and index, every
 //            function's value (into a per-function array in sorted order; an aggregate's read from the fold at its
 //            frame's last position, with its null flag and a wide decimal's high word; an offset function's source
@@ -74,6 +78,13 @@ struct WindowWs {
   uint64_t* rnk;
   uint32_t* pres;
   uint64_t stride;
+  uint32_t* fs;
+  uint32_t* ft;
+  uint64_t* ov;
+  uint8_t* onull;
+  uint64_t* rlo[3];
+  uint64_t* rhi[3];
+  uint32_t* rcnt[3];
   uint8_t* end;
 };
 
@@ -101,6 +112,18 @@ WindowWs carve_window_ws(uint8_t* d_wws, uint64_t n, const WindowShape& sh) {
   w.stride = a256((n + 1) * 8) / 8;
   w.rnk = (uint64_t*)p;      p += (size_t)sh.n_nn * w.stride * 8;
   w.pres = (uint32_t*)p;     p += a256((size_t)sh.n_nn * n * 4);
+  // sliding frames: per bounds set b each position's frame [fs, ft) (at [b n, b n + n)), the staged order column, and
+  // per result state r (at [r n, r n + n)) its value, then with range-minimum passes two sets of level state
+  w.fs = (uint32_t*)p;       p += a256((size_t)sh.n_bnd * n * 4);
+  w.ft = (uint32_t*)p;       p += a256((size_t)sh.n_bnd * n * 4);
+  w.ov = (uint64_t*)p;       p += a256(sh.ord_staged ? n * 8 : 0);
+  w.onull = p;               p += a256(sh.ord_staged ? n : 0);
+  for (int b = 0; b < 3; b++) {
+    const size_t r = b == 0 || sh.rmq_width > 1 ? (size_t)sh.n_res * n : 0;
+    w.rlo[b] = (uint64_t*)p;  p += a256(r * 8);
+    w.rhi[b] = (uint64_t*)p;  p += a256(r * 8);
+    w.rcnt[b] = (uint32_t*)p; p += a256(r * 4);
+  }
   w.end = p;
   return w;
 }
@@ -253,6 +276,20 @@ __device__ __forceinline__ bool float_less(uint32_t k, uint64_t a, uint64_t b) {
   return x < y;
 }
 
+// MIN / MAX of an earlier state (l0, h0, c0) and a later one (l, h, c), into (l, h): the later value is kept only when
+// it is present and strictly better (or the earlier is absent), so the first of equal values keeps its exact bits
+__device__ __forceinline__ void minmax_keep(uint32_t fn, uint32_t vt, uint64_t l0, uint64_t h0, uint32_t c0,
+                                            uint64_t& l, uint64_t& h, uint32_t c) {
+  const uint32_t k = val_kind(vt);
+  const bool fl = k == B2S_WINDOW_VAL_FLOAT32 || k == B2S_WINDOW_VAL_FLOAT64;
+  const bool later_wins = fn == B2S_WINDOW_MIN ? (fl ? float_less(k, l, l0) : dec_less(Dec128{l, h}, Dec128{l0, h0}))
+                                               : (fl ? float_less(k, l0, l) : dec_less(Dec128{l0, h0}, Dec128{l, h}));
+  if (c0 && !(c && later_wins)) {
+    l = l0;
+    h = h0;
+  }
+}
+
 // One pass of the segmented scan: position j takes the combination of j - d's state (earlier) and its own when j - d
 // is in its partition, else keeps its own.  Only the scanning aggregates are touched.
 __global__ void __launch_bounds__(kWindowThreads) window_scan_pass_kernel(
@@ -274,15 +311,7 @@ __global__ void __launch_bounds__(kWindowThreads) window_scan_pass_kernel(
         const uint64_t l0 = lo_in[x - d], h0 = hi_in[x - d];
         const uint32_t c0 = cnt_in[x - d];
         if (fn == B2S_WINDOW_MIN || fn == B2S_WINDOW_MAX) {
-          const uint32_t k = val_kind(vt);
-          const bool fl = k == B2S_WINDOW_VAL_FLOAT32 || k == B2S_WINDOW_VAL_FLOAT64;
-          const bool later_wins = fn == B2S_WINDOW_MIN
-                                      ? (fl ? float_less(k, l, l0) : dec_less(Dec128{l, h}, Dec128{l0, h0}))
-                                      : (fl ? float_less(k, l0, l) : dec_less(Dec128{l0, h0}, Dec128{l, h}));
-          if (c0 && !(c && later_wins)) {
-            l = l0;
-            h = h0;
-          }
+          minmax_keep(fn, vt, l0, h0, c0, l, h, c);
         } else {  // sums and counts, modulo 2^128
           bool unused;
           const Dec128 s = dec_add(Dec128{l0, h0}, Dec128{l, h}, &unused);
@@ -344,6 +373,184 @@ __global__ void __launch_bounds__(kWindowThreads) window_fold_kernel(
   }
 }
 
+// ---- sliding frames ----
+__host__ __device__ __forceinline__ bool is_sliding(uint32_t frame) { return frame >= B2S_WINDOW_FRAME_ROWS; }
+constexpr int64_t kUnboundedPreceding = INT64_MIN, kUnboundedFollowing = INT64_MAX;
+
+// Stage the RANGE order column: per sorted position its value sign-extended from the column's width, and its null flag
+__global__ void __launch_bounds__(kWindowThreads) window_order_stage_kernel(
+    const uint8_t* __restrict__ arena, const uint64_t* __restrict__ rec_off, const uint32_t* __restrict__ idx, uint64_t n,
+    const WindowShape* __restrict__ sh, uint64_t* __restrict__ ov, uint8_t* __restrict__ onull) {
+  const uint32_t len = sh->ord_len, off = sh->ord_off;
+  const int32_t nf = sh->ord_null;
+  for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (uint64_t)gridDim.x * blockDim.x) {
+    const uint8_t* row = arena + rec_off[at(idx, j)] + 4;
+    uint64_t v, unused;
+    ld_span16<true>(row + off, (int)len, v, unused);
+    const int sh_bits = 64 - 8 * (int)len;
+    ov[j] = (uint64_t)(((int64_t)(v << sh_bits)) >> sh_bits);
+    onull[j] = null_bit(row, nf);
+  }
+}
+
+// The first position p in [a, b) whose staged order value is not before (upper: is after) the bound B in the column's
+// sort order; b when there is none.  Both predicates are monotone over a partition's sorted positions.
+__device__ __forceinline__ uint64_t range_search(const uint64_t* __restrict__ ov, const uint8_t* __restrict__ onull,
+                                                 uint64_t a, uint64_t b, int64_t B, bool desc, bool nulls_first,
+                                                 bool upper) {
+  while (a < b) {
+    const uint64_t m = a + (b - a) / 2;
+    bool hit;
+    if (onull[m]) {
+      hit = !nulls_first;  // B is not null: a null sorts before it with NULLS FIRST, after it with NULLS LAST
+    } else {
+      const int64_t v = (int64_t)ov[m];
+      hit = upper ? (desc ? v < B : v > B) : (desc ? v <= B : v >= B);
+    }
+    if (hit) b = m;
+    else a = m + 1;
+  }
+  return a;
+}
+
+// Per sorted position j and bounds set b, the frame [fs, ft) of j's partition [ps, pe) (ft == fs: empty).  ROWS: j + lo
+// .. j + hi clipped; RANGE: CURRENT ROW the peer group's edge, an offset the binary search for v + k (v - k
+// descending) over the partition's staged order values, a null-keyed row's the null peers.  A partition whose ROWS
+// offset k has N - 1 + |k| > 2^31 - 1, or a non-null v +- k outside the column's type, sets readback[5].
+__global__ void __launch_bounds__(kWindowThreads) window_bounds_kernel(
+    uint64_t n, const WindowShape* __restrict__ sh, const uint64_t* __restrict__ heads_before,
+    const uint32_t* __restrict__ gpos, const uint64_t* __restrict__ groups, const uint64_t* __restrict__ phead,
+    const uint32_t* __restrict__ pstart, const uint64_t* __restrict__ ov, const uint8_t* __restrict__ onull,
+    uint32_t* __restrict__ fs, uint32_t* __restrict__ ft, uint64_t* __restrict__ readback) {
+  const uint64_t G = *groups, P = phead[n];
+  const uint32_t n_bnd = sh->n_bnd;
+  const bool desc = sh->ord_type & B2S_KEY_DESCENDING, nulls_first = !(sh->ord_type & B2S_KEY_NULLS_LAST);
+  const int64_t tmax = sh->ord_len >= 8 ? INT64_MAX : (int64_t)((1ull << (8 * sh->ord_len - 1)) - 1);
+  const int64_t tmin = -tmax - 1;
+  for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (uint64_t)gridDim.x * blockDim.x) {
+    const uint64_t g = next_scanned(heads_before, j, n, G) - 1, p = next_scanned(phead, j, n, P) - 1;
+    const uint64_t ps = pstart[p], pe = pstart[p + 1], gs = gpos[g], ge = gpos[g + 1];
+    bool wraps = false;
+    for (uint32_t b = 0; b < n_bnd; b++) {
+      const int64_t lo = sh->blo[b], hi = sh->bhi[b];
+      int64_t s, t;  // the frame's first position and one past its last, before clipping to the partition
+      if (sh->bkind[b] == B2S_WINDOW_FRAME_ROWS) {
+        s = lo == kUnboundedPreceding ? (int64_t)ps : (int64_t)j + lo;
+        t = hi == kUnboundedFollowing ? (int64_t)pe : (int64_t)j + hi + 1;
+        const uint64_t N1 = pe - ps - 1;
+        if (j == ps && ((lo != kUnboundedPreceding && N1 + (uint64_t)(lo < 0 ? -lo : lo) > 0x7fffffffull) ||
+                        (hi != kUnboundedFollowing && N1 + (uint64_t)(hi < 0 ? -hi : hi) > 0x7fffffffull)))
+          wraps = true;
+      } else {
+        const bool null = ov && onull[j];
+        const int64_t v = ov ? (int64_t)ov[j] : 0;
+        int64_t e[2];
+        for (int u = 0; u < 2; u++) {
+          const int64_t k = u ? hi : lo;
+          if (k == kUnboundedPreceding) e[u] = (int64_t)ps;
+          else if (k == kUnboundedFollowing) e[u] = (int64_t)pe;
+          else if (k == 0 || null) e[u] = (int64_t)(u ? ge : gs);  // the peer group: with an offset, the null peers
+          else {
+            const int64_t d = desc ? -k : k;  // the column's checks keep -k in range
+            const bool ovf = d > 0 ? v > tmax - d : v < tmin - d;
+            if (ovf) {
+              wraps = true;
+              e[u] = (int64_t)j;
+            } else {
+              e[u] = (int64_t)range_search(ov, onull, ps, pe, v + d, desc, nulls_first, u);
+            }
+          }
+        }
+        s = e[0];
+        t = e[1];
+      }
+      s = s < (int64_t)ps ? (int64_t)ps : s > (int64_t)pe ? (int64_t)pe : s;
+      t = t < s ? s : t > (int64_t)pe ? (int64_t)pe : t;
+      fs[(size_t)b * n + j] = (uint32_t)s;
+      ft[(size_t)b * n + j] = (uint32_t)t;
+    }
+    if (wraps) readback[5] = 1;
+  }
+}
+
+// A MIN / MAX whose frame's lower end is bounded (res[f] >= 0, not a double fold): level k of the range-minimum passes
+// holds per position j the state of [j, j + 2^k) (clipped to n); level 0 is the staged input.  Pass k writes the result
+// of every position whose frame width w has floor(log2 w) == k, as the earlier of level k at fs and at ft - 2^k (the
+// earlier wins ties, so the first of equal values is kept), then (build) level k + 1.  An empty frame's state is zero.
+__global__ void __launch_bounds__(kWindowThreads) window_rmq_pass_kernel(
+    uint64_t n, const WindowShape* __restrict__ sh, const uint32_t* __restrict__ fs, const uint32_t* __restrict__ ft,
+    uint32_t k, bool staged, bool build, const uint64_t* __restrict__ lo_in, const uint64_t* __restrict__ hi_in,
+    const uint32_t* __restrict__ cnt_in, uint64_t* __restrict__ lo_out, uint64_t* __restrict__ hi_out,
+    uint32_t* __restrict__ cnt_out, uint64_t* __restrict__ rlo, uint64_t* __restrict__ rhi,
+    uint32_t* __restrict__ rcnt) {
+  const uint32_t n_fns = sh->n_fns;
+  const uint64_t d = 1ull << k;
+  for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (uint64_t)gridDim.x * blockDim.x) {
+    for (uint32_t f = 0; f < n_fns; f++) {
+      const uint32_t fn = sh->fn[f], vt = sh->vtype[f];
+      if (sh->res[f] < 0 || (fn != B2S_WINDOW_MIN && fn != B2S_WINDOW_MAX)) continue;
+      const size_t in = (size_t)(staged ? sh->agg[f] : (uint32_t)sh->res[f]) * n, r = (size_t)sh->res[f] * n;
+      const size_t bx = (size_t)sh->bnd[f] * n + j;
+      const uint64_t s = fs[bx], t = ft[bx];
+      if (t > s && 63 - __clzll(t - s) == (int)k) {
+        uint64_t l = lo_in[in + t - d], h = hi_in[in + t - d];
+        const uint32_t c = cnt_in[in + t - d], c0 = cnt_in[in + s];
+        minmax_keep(fn, vt, lo_in[in + s], hi_in[in + s], c0, l, h, c);
+        rlo[r + j] = l;
+        rhi[r + j] = h;
+        rcnt[r + j] = c0 + c;
+      } else if (k == 0 && t <= s) {
+        rlo[r + j] = rhi[r + j] = 0;
+        rcnt[r + j] = 0;
+      }
+      if (build) {
+        uint64_t l = lo_in[in + j], h = hi_in[in + j];
+        uint32_t c = cnt_in[in + j];
+        if (j + d < n) {
+          const uint64_t l1 = lo_in[in + j + d], h1 = hi_in[in + j + d];
+          const uint32_t c1 = cnt_in[in + j + d];
+          uint64_t a = l1, b = h1;
+          minmax_keep(fn, vt, l, h, c, a, b, c1);
+          l = a;
+          h = b;
+          c += c1;
+        }
+        lo_out[r + j] = l;
+        hi_out[r + j] = h;
+        cnt_out[r + j] = c;
+      }
+    }
+  }
+}
+
+// A double fold whose frame's lower end is bounded (Spark's sliding and shrinking frames re-fold the frame from its
+// first row): per position, ((0.0 + x_s) + x_{s+1}) + ... over the frame's present staged inputs, with their count.
+// One thread per position, so the cost is the sum of the frame widths, as Spark's own.
+__global__ void __launch_bounds__(kWindowThreads) window_frame_fold_kernel(
+    uint64_t n, const WindowShape* __restrict__ sh, const uint32_t* __restrict__ fs, const uint32_t* __restrict__ ft,
+    const uint64_t* __restrict__ lo_in, const uint32_t* __restrict__ cnt_in, uint64_t* __restrict__ rlo,
+    uint32_t* __restrict__ rcnt) {
+  const uint32_t n_fns = sh->n_fns;
+  for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (uint64_t)gridDim.x * blockDim.x) {
+    for (uint32_t f = 0; f < n_fns; f++) {
+      if (sh->res[f] < 0 || !folds_double(sh->fn[f], sh->vtype[f])) continue;
+      const size_t in = (size_t)sh->agg[f] * n, bx = (size_t)sh->bnd[f] * n + j;
+      const uint64_t s = fs[bx], t = ft[bx];
+      double acc = 0.0;
+      uint32_t c = 0;
+      for (uint64_t p = s; p < t; p++) {
+        if (!cnt_in[in + p]) continue;
+        // a NaN sum keeps its own payload, as Java's (x86's) acc + x does when both are NaN; the add alone may return
+        // x's
+        if (!isnan(acc)) acc = __dadd_rn(acc, __longlong_as_double(lo_in[in + p]));
+        c++;
+      }
+      rlo[(size_t)sh->res[f] * n + j] = __double_as_longlong(acc);
+      rcnt[(size_t)sh->res[f] * n + j] = c;
+    }
+  }
+}
+
 // the exact decimal average: S / c rounded HALF_UP to 4 more digits, as q0 10^4 + round(r0 10^4 / c) with
 // q0 = |S| / c and r0 = |S| % c (c < 2^32, so each 32-bit limb's step divides a 64-bit number)
 __device__ __forceinline__ Dec128 dec_avg(Dec128 x, uint32_t c) {
@@ -386,16 +593,13 @@ struct WindowAggIo {
   uint64_t* vhi;
 };
 
-// aggregate f's value at position j from the fold at its frame's last position e; *null when it is null (slot 0)
-__device__ uint64_t agg_value(const WindowShape* __restrict__ sh, uint32_t f, const WindowAggIo& io, uint64_t n,
-                              uint64_t e, uint64_t j, bool* null) {
+// aggregate f's value at position j from its frame's state (l, h, c); *null when it is null (slot 0)
+__device__ uint64_t agg_finish(const WindowShape* __restrict__ sh, uint32_t f, const WindowAggIo& io, uint64_t n,
+                               uint64_t j, uint64_t l, uint64_t h, uint32_t c, bool* null) {
   const uint32_t fn = sh->fn[f], vt = sh->vtype[f], k = val_kind(vt);
-  const size_t x = (size_t)sh->agg[f] * n + e;
-  const uint32_t c = io.cnt[x];
   if (fn == B2S_WINDOW_COUNT) return c;
   *null = c == 0;
   if (!c) return 0;
-  uint64_t l = io.lo[x];
   if (folds_double(fn, vt))
     return fn == B2S_WINDOW_AVG ? __double_as_longlong(__ddiv_rn(__longlong_as_double(l), (double)c)) : l;
   if (k != B2S_WINDOW_VAL_DECIMAL) {
@@ -403,10 +607,52 @@ __device__ uint64_t agg_value(const WindowShape* __restrict__ sh, uint32_t f, co
     return k == B2S_WINDOW_VAL_INT8 ? l & 0xff : k == B2S_WINDOW_VAL_INT16 ? l & 0xffff
            : k == B2S_WINDOW_VAL_INT32 || k == B2S_WINDOW_VAL_FLOAT32 ? l & 0xffffffffull : l;
   }
-  Dec128 v{l, io.hi[x]};
+  Dec128 v{l, h};
   if (fn == B2S_WINDOW_AVG) v = dec_avg(v, c);
   if (result_p(fn, vt) > 18) io.vhi[(size_t)sh->wide[f] * n + j] = v.hi;
   return v.lo;
+}
+
+// aggregate f's value at position j from the fold at its frame's last position e
+__device__ uint64_t agg_value(const WindowShape* __restrict__ sh, uint32_t f, const WindowAggIo& io, uint64_t n,
+                              uint64_t e, uint64_t j, bool* null) {
+  const size_t x = (size_t)sh->agg[f] * n + e;
+  return agg_finish(sh, f, io, n, j, io.lo[x], io.hi[x], io.cnt[x], null);
+}
+
+// What the values kernel reads for sliding frames: each bounds set's frames, and the result states
+struct WindowFrameIo {
+  const uint32_t* fs;
+  const uint32_t* ft;
+  const uint64_t* rlo;
+  const uint64_t* rhi;
+  const uint32_t* rcnt;
+};
+
+// aggregate f's value at position j of partition [ps, pe) over the sliding frame [s, t): its own result state, or the
+// prefix folds' state at t - 1, less (sums and counts, exact modulo 2^128 and 2^32) the state at s - 1 when s > ps.  A
+// frame whose lower end is unbounded (s == ps) reads the running fold as the older frames do.
+__device__ uint64_t frame_agg_value(const WindowShape* __restrict__ sh, uint32_t f, const WindowAggIo& io,
+                                    const WindowFrameIo& fio, uint64_t n, uint64_t ps, uint64_t s, uint64_t t,
+                                    uint64_t j, bool* null) {
+  if (sh->res[f] >= 0) {
+    const size_t x = (size_t)sh->res[f] * n + j;
+    return agg_finish(sh, f, io, n, j, fio.rlo[x], fio.rhi[x], fio.rcnt[x], null);
+  }
+  if (t <= s) return agg_finish(sh, f, io, n, j, 0, 0, 0, null);
+  const size_t base = (size_t)sh->agg[f] * n;
+  uint64_t l = io.lo[base + t - 1], h = io.hi[base + t - 1];
+  uint32_t c = io.cnt[base + t - 1];
+  if (s > ps) {
+    const size_t x = base + s - 1;
+    const uint64_t nl = ~io.lo[x] + 1, nh = ~io.hi[x] + (io.lo[x] == 0);  // -state(s - 1)
+    bool unused;
+    const Dec128 d = dec_add(Dec128{l, h}, Dec128{nl, nh}, &unused);
+    l = d.lo;
+    h = d.hi;
+    c -= io.cnt[x];
+  }
+  return agg_finish(sh, f, io, n, j, l, h, c, null);
 }
 
 // ---- offset functions ----
@@ -454,12 +700,13 @@ struct WindowOffIo {
   uint64_t stride;
 };
 
-// Offset function f's source sorted position for position j of partition [ps, pe) whose frame ends at e (FIRST, LAST
-// and NTH_VALUE), or kNoSource: outside the partition or the frame (LAG / LEAD's default, else null).  With a
-// non-null index the partition's present positions are pres[r(ps) .. r(pe)) and the frame's pres[r(ps) .. r(e + 1)).
+// Offset function f's source sorted position for position j of partition [ps, pe) whose frame is [s, e] (FIRST, LAST
+// and NTH_VALUE; e + 1 == s: empty), or kNoSource: outside the partition or the frame (LAG / LEAD's default, else
+// null).  With a non-null index the partition's present positions are pres[r(ps) .. r(pe)) and the frame's
+// pres[r(s) .. r(e + 1)).
 __device__ __forceinline__ uint64_t offset_source(const WindowShape* __restrict__ sh, uint32_t f,
                                                   const WindowOffIo& io, uint64_t n, uint64_t j, uint64_t ps,
-                                                  uint64_t pe, uint64_t e) {
+                                                  uint64_t pe, uint64_t s, uint64_t e) {
   const uint32_t fn = sh->fn[f];
   const uint64_t k = sh->arg[f];  // LAG / LEAD's offset, NTH_VALUE's n; 0 for FIRST and LAST
   const int32_t x = sh->nn[f];
@@ -467,13 +714,13 @@ __device__ __forceinline__ uint64_t offset_source(const WindowShape* __restrict_
     switch (fn) {
       case B2S_WINDOW_LEAD: return j + k < pe ? j + k : kNoSource;
       case B2S_WINDOW_LAG: return j - ps >= k ? j - k : kNoSource;
-      case B2S_WINDOW_FIRST: return ps;
-      case B2S_WINDOW_LAST: return e;
-      default: return ps + k - 1 <= e ? ps + k - 1 : kNoSource;
+      case B2S_WINDOW_FIRST: return s < e + 1 ? s : kNoSource;
+      case B2S_WINDOW_LAST: return s < e + 1 ? e : kNoSource;
+      default: return s + k - 1 < e + 1 ? s + k - 1 : kNoSource;
     }
   }
   const uint64_t* r = io.rnk + (size_t)x * io.stride;
-  const uint64_t lo = r[ps];
+  const uint64_t lo = r[s];
   uint64_t q;
   switch (fn) {
     case B2S_WINDOW_LEAD:
@@ -482,7 +729,7 @@ __device__ __forceinline__ uint64_t offset_source(const WindowShape* __restrict_
       break;
     case B2S_WINDOW_LAG:
       q = r[j];
-      if (q < lo + k) return kNoSource;
+      if (q < r[ps] + k) return kNoSource;
       q -= k;
       break;
     case B2S_WINDOW_FIRST:
@@ -508,8 +755,8 @@ __device__ __forceinline__ uint64_t offset_source(const WindowShape* __restrict_
 // record's arena offset << 2 | kAggBadDecimal or kWindowBadBytes.
 __device__ __forceinline__ uint64_t offset_value(const uint32_t* __restrict__ rec_len, const uint32_t* __restrict__ idx,
                                                  const WindowShape* __restrict__ sh, uint32_t f, const WindowOffIo& io,
-                                                 uint64_t n, uint64_t j, uint64_t ps, uint64_t pe, uint64_t e,
-                                                 bool* null, uint64_t* extra, unsigned long long* bad) {
+                                                 uint64_t n, uint64_t j, uint64_t ps, uint64_t pe, uint64_t s,
+                                                 uint64_t e, bool* null, uint64_t* extra, unsigned long long* bad) {
   const uint32_t vt = sh->vtype[f], k = val_kind(vt), voff = sh->voff[f];
   const int32_t vnull = sh->vnull[f];
   if (k == B2S_WINDOW_VAL_BYTES || wide_input(vt)) {
@@ -530,20 +777,20 @@ __device__ __forceinline__ uint64_t offset_value(const uint32_t* __restrict__ re
                                             (k == B2S_WINDOW_VAL_BYTES ? kWindowBadBytes : kAggBadDecimal)));
     }
   }
-  const uint64_t s = offset_source(sh, f, io, n, j, ps, pe, e);
-  if (s == kNoSource) {
+  const uint64_t src = offset_source(sh, f, io, n, j, ps, pe, s, e);
+  if (src == kNoSource) {
     *null = !(sh->flags[f] & B2S_WINDOW_HAS_DEFAULT);
     return *null ? 0 : sh->dflt[f];
   }
-  const uint32_t i = at(idx, s);
+  const uint32_t i = at(idx, src);
   const uint8_t* row = io.arena + io.rec_off[i] + 4;
   *null = null_bit(row, vnull);
   if (*null) return 0;
   if (k == B2S_WINDOW_VAL_BYTES) {
     *extra += ((uint64_t)(uint32_t)ld64(row + voff) + 7) & ~7ull;
-    return s;
+    return src;
   }
-  return wide_input(vt) ? s : ld64(row + voff) & width_mask(k);
+  return wide_input(vt) ? src : ld64(row + voff) & width_mask(k);
 }
 
 __global__ void __launch_bounds__(kWindowThreads) window_values_kernel(
@@ -551,7 +798,7 @@ __global__ void __launch_bounds__(kWindowThreads) window_values_kernel(
     const WindowShape* __restrict__ sh, const uint64_t* __restrict__ heads_before, const uint32_t* __restrict__ gpos,
     const uint64_t* __restrict__ groups, const uint64_t* __restrict__ phead, const uint32_t* __restrict__ pstart,
     uint64_t* __restrict__ vals, uint64_t* __restrict__ rows, uint64_t* __restrict__ bytes,
-    uint64_t* __restrict__ readback, WindowAggIo io, WindowOffIo oio) {
+    uint64_t* __restrict__ readback, WindowAggIo io, WindowOffIo oio, WindowFrameIo fio) {
   const uint64_t G = *groups, P = phead[n];
   const uint32_t n_fns = sh->n_fns, limit_fn = sh->limit_fn;
   // what the output row adds to the input row, past the offset functions' strings
@@ -576,10 +823,16 @@ __global__ void __launch_bounds__(kWindowThreads) window_values_kernel(
         case B2S_WINDOW_NTILE: v = int_slot(ntile(i, N, sh->arg[f])); break;
         default: {
           const uint32_t fr = sh->frame[f];
-          const uint64_t e = fr == B2S_WINDOW_FRAME_ROWS_RUNNING ? j
-                             : fr == B2S_WINDOW_FRAME_RANGE_RUNNING ? ps + ge - 1 : ps + N - 1;
-          v = is_offset(sh->fn[f]) ? offset_value(rec_len, idx, sh, f, oio, n, j, ps, ps + N, e, &null, &extra,
+          uint64_t s = ps, e = fr == B2S_WINDOW_FRAME_ROWS_RUNNING ? j
+                               : fr == B2S_WINDOW_FRAME_RANGE_RUNNING ? ps + ge - 1 : ps + N - 1;
+          if (is_sliding(fr)) {  // [s, e]: empty when e + 1 == s
+            const size_t bx = (size_t)sh->bnd[f] * n + j;
+            s = fio.fs[bx];
+            e = (uint64_t)fio.ft[bx] - 1;
+          }
+          v = is_offset(sh->fn[f]) ? offset_value(rec_len, idx, sh, f, oio, n, j, ps, ps + N, s, e, &null, &extra,
                                                   (unsigned long long*)(readback + 4))
+              : is_sliding(fr)     ? frame_agg_value(sh, f, io, fio, n, ps, s, e + 1, j, &null)
                                    : agg_value(sh, f, io, n, e, j, &null);
           break;
         }
@@ -745,6 +998,16 @@ void launch_window_values(const uint8_t* arena, uint64_t n, const uint32_t* idx,
   launch_exclusive_scan_u64(w.phead, n, w.phead + n, w.scan_ws, st, launches);
   window_part_starts_kernel<<<grid_for(n), kWindowThreads, 0, st>>>(w.phead, n, w.pstart);
   if (launches) *launches += 2;
+  const WindowFrameIo fio{w.fs, w.ft, w.rlo[0], w.rhi[0], w.rcnt[0]};
+  if (shape.n_bnd) {  // sliding frames: the order column staged for a RANGE offset, then every bounds set's frames
+    if (shape.ord_staged)
+      window_order_stage_kernel<<<grid_for(n), kWindowThreads, 0, st>>>(arena, k.src_off, idx, n, w.shape, w.ov,
+                                                                         w.onull);
+    window_bounds_kernel<<<grid_for(n), kWindowThreads, 0, st>>>(
+        n, w.shape, heads_before, rows_group_starts(d_aws, n), groups, w.phead, w.pstart,
+        shape.ord_staged ? w.ov : nullptr, w.onull, w.fs, w.ft, w.readback);
+    if (launches) *launches += 1 + shape.ord_staged;
+  }
   WindowOffIo oio{arena, k.src_off, nullptr, nullptr, w.stride};
   if (shape.n_nn) {  // the non-null indexes: present flags, a scan each, the present positions compacted
     window_present_kernel<<<grid_for(n), kWindowThreads, 0, st>>>(arena, k.src_off, idx, n, w.shape, w.stride, w.rnk);
@@ -760,18 +1023,35 @@ void launch_window_values(const uint8_t* arena, uint64_t n, const uint32_t* idx,
   WindowAggIo io{};
   io.vnul = shape.n_off ? w.vnul : nullptr;
   if (shape.n_agg) {
-    bool scans = false, folds = false;
+    bool scans = false, folds = false, rmq = false, frame_folds = false;
     for (uint32_t f = 0; f < shape.n_fns; f++) {
       if (!is_agg(shape.fn[f])) continue;
       const uint32_t kind = shape.vtype[f] & 0xff;
       const bool dbl = (shape.fn[f] == B2S_WINDOW_SUM &&
                         (kind == B2S_WINDOW_VAL_FLOAT32 || kind == B2S_WINDOW_VAL_FLOAT64)) ||
                        (shape.fn[f] == B2S_WINDOW_AVG && kind != B2S_WINDOW_VAL_DECIMAL);
-      (dbl ? folds : scans) = true;
+      // a sliding frame's own result state replaces the prefix folds
+      if (shape.res[f] >= 0) (dbl ? frame_folds : rmq) = true;
+      else (dbl ? folds : scans) = true;
     }
     window_stage_kernel<<<grid_for(n), kWindowThreads, 0, st>>>(arena, k.src_off, k.len, idx, n, w.shape, w.lo[0],
                                                                 w.hi[0], w.cnt[0],
                                                                 (unsigned long long*)(w.readback + 4));
+    // the sliding frames read the staged inputs (set 0) before the scans and the running fold overwrite them; the
+    // range-minimum passes read levels 0 .. floor(log2(the widest frame))
+    uint32_t levels = 0;
+    for (uint64_t wmax = std::min<uint64_t>(shape.rmq_width, n); rmq && wmax; wmax >>= 1) levels++;
+    for (uint32_t lv = 0; lv < levels; lv++) {
+      const int in = lv & 1 ? 1 : 2, out = lv & 1 ? 2 : 1;  // level lv in rlo[in] (level 0: the staged set)
+      window_rmq_pass_kernel<<<grid_for(n), kWindowThreads, 0, st>>>(
+          n, w.shape, w.fs, w.ft, lv, lv == 0, lv + 1 < levels, lv ? w.rlo[in] : w.lo[0],
+          lv ? w.rhi[in] : w.hi[0], lv ? w.rcnt[in] : w.cnt[0], w.rlo[out], w.rhi[out], w.rcnt[out], w.rlo[0],
+          w.rhi[0], w.rcnt[0]);
+    }
+    if (frame_folds)
+      window_frame_fold_kernel<<<grid_for(n), kWindowThreads, 0, st>>>(n, w.shape, w.fs, w.ft, w.lo[0], w.cnt[0],
+                                                                       w.rlo[0], w.rcnt[0]);
+    if (launches) *launches += levels + frame_folds;
     int cur = 0;  // the set holding the scanned folds
     for (uint64_t d = 1; scans && d < n; d *= 2, cur ^= 1)
       window_scan_pass_kernel<<<grid_for(n), kWindowThreads, 0, st>>>(n, w.shape, w.phead, w.pstart, d, w.lo[cur],
@@ -792,7 +1072,7 @@ void launch_window_values(const uint8_t* arena, uint64_t n, const uint32_t* idx,
   }
   window_values_kernel<<<grid_for(n), kWindowThreads, 0, st>>>(k.len, idx, n, w.shape, heads_before,
                                                                rows_group_starts(d_aws, n), groups, w.phead, w.pstart,
-                                                               w.vals, w.rows, w.bytes, w.readback, io, oio);
+                                                               w.vals, w.rows, w.bytes, w.readback, io, oio, fio);
   launch_exclusive_scan_u64(w.rows, n, w.readback, w.scan_ws, st, launches);
   launch_exclusive_scan_u64(w.bytes, n, w.readback + 1, w.scan_ws, st, launches);
   if (launches) *launches += 1;

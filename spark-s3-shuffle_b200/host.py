@@ -8,7 +8,7 @@ import numpy as np
 
 from . import _build
 from .capi import (_agg_arrays, _arg, _join_arrays, _key_arrays, _window_aggregate_arrays, _window_arrays,
-                   _window_offset_arrays)
+                   _window_offset_arrays, _window_frame_arrays)
 
 OK, E_RUNTIME, E_IO, E_SPARK, E_UNSUPPORTED, E_CODEC = 0, -101, -102, -103, -104, -105
 
@@ -85,6 +85,9 @@ PROTOTYPES = [
     ("b2sh_reader_read_window_offset_rows", C.c_int,
      [_vp, _u32, _u32, _vp, _vp, _vp, _vp, _u32, _vp, _u32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, C.POINTER(_vp),
       C.POINTER(_u64), C.POINTER(_u64), C.POINTER(_u64)]),
+    ("b2sh_reader_read_window_frame_rows", C.c_int,
+     [_vp, _u32, _u32, _vp, _vp, _vp, _vp, _u32, _vp, _u32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+      C.POINTER(_vp), C.POINTER(_u64), C.POINTER(_u64), C.POINTER(_u64)]),
     ("b2sh_reader_block", C.c_int,
      [_vp, _u32, C.POINTER(_i64), C.POINTER(_i32), C.POINTER(_i32), C.POINTER(_vp), C.POINTER(_u64)]),
     ("b2sh_reader_remote_bytes_read", _u64, [_vp]),
@@ -477,6 +480,18 @@ class S3ShuffleReader:
         counts = [_u64(), _u64()]
         _check(load().b2sh_reader_read_window_offset_rows(self._h, *map(_arg, a), C.byref(p), C.byref(size),
                                                           *map(C.byref, counts)))
+        return ((C.string_at(p.value, size.value) if size.value else b""),) + tuple(c.value for c in counts)
+
+    def readWindowFrameRows(self, keys, nPartitionKeys, nFields, kinds, fns):
+        """Spark's window over sliding ROWS and RANGE frames (with ranking, aggregate and offset functions) over this
+        reader's partitions: its blocks through ONE capi.decompress_window_frame_rows_keys_packed call, whose arguments
+        these are (fns: as in readWindowOffsetRows, or (fn, arg, frame, val_type, val_off, val_null_field, flags,
+        default, lower, upper)).  -> (output rows, n_records, n_out_records)"""
+        a = _window_frame_arrays(keys, nPartitionKeys, nFields, kinds, fns)
+        p, size = _vp(), _u64()
+        counts = [_u64(), _u64()]
+        _check(load().b2sh_reader_read_window_frame_rows(self._h, *map(_arg, a), C.byref(p), C.byref(size),
+                                                         *map(C.byref, counts)))
         return ((C.string_at(p.value, size.value) if size.value else b""),) + tuple(c.value for c in counts)
 
     def _blocks(self, n):

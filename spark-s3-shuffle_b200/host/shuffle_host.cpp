@@ -1174,6 +1174,9 @@ class S3ShuffleReader {
     const uint32_t* flags = nullptr;
     const uint64_t* dflt = nullptr;
     bool offset = false;
+    const int64_t* lower = nullptr;  // with frames, b2s_decompress_window_frame_rows_keys_packed's bounds
+    const int64_t* upper = nullptr;
+    bool frames = false;
   };
   // read() for a Spark SQL window over this shuffle read (INTEGRATION.md §3o): every non-empty block is fetched (the
   // exchange cache is not consulted) in computeShuffleBlocks order, then ONE b2s_decompress_window_rows_keys_packed
@@ -1196,6 +1199,13 @@ class S3ShuffleReader {
     uint64_t total = 0, out = 0;
     const uint64_t guess = codec == B2S_CODEC_NONE ? src.bytes * 2 : src.bytes * 4;
     const int rc = callWithRetry(sorted_, guess, total, [&](uint64_t cap) {
+      if (w.frames)
+        return b2s_decompress_window_frame_rows_keys_packed(
+            codec, alg, n, src.src.data(), src.off.data(), src.len.data(), alg ? src.sliceBase.data() : 0,
+            alg ? src.sliceLen.data() : 0, alg ? src.sliceSum.data() : 0, w.nPartitionKeys, w.nKeys, w.keyType,
+            w.keyOff, w.keyLen, w.keyNull, w.nFields, w.kind, w.nFns, w.fn, w.fnArg, w.frame, w.valType, w.valOff,
+            w.valNull, w.flags, w.dflt, w.lower, w.upper, sorted_.get(), cap, &total, nRecords, &out, status.data(),
+            bad.data());
       if (w.offset)
         return b2s_decompress_window_offset_rows_keys_packed(
             codec, alg, n, src.src.data(), src.off.data(), src.len.data(), alg ? src.sliceBase.data() : 0,
@@ -1215,7 +1225,8 @@ class S3ShuffleReader {
           cap, &total, nRecords, &out, status.data(), bad.data());
     });
     if (rc != 0)
-      throw CodecException(std::string(w.offset      ? "b2s_decompress_window_offset_rows_keys_packed: "
+      throw CodecException(std::string(w.frames      ? "b2s_decompress_window_frame_rows_keys_packed: "
+                                       : w.offset    ? "b2s_decompress_window_offset_rows_keys_packed: "
                                        : w.aggregate ? "b2s_decompress_window_aggregate_rows_keys_packed: "
                                                      : "b2s_decompress_window_rows_keys_packed: ") +
                            b2s_strerror(rc) + ": " + b2s_last_error());
@@ -1732,6 +1743,30 @@ int b2sh_reader_read_window_offset_rows(b2sh_reader* r, uint32_t n_partition_key
     w.flags = fn_flags;
     w.dflt = fn_default;
     w.offset = true;
+    r->r->readWindowRows(w, n_records);
+    sorted_result(*r->r, data, len, n_out_records);
+  });
+}
+int b2sh_reader_read_window_frame_rows(b2sh_reader* r, uint32_t n_partition_keys, uint32_t n_keys,
+                                       const uint32_t* key_type, const uint32_t* key_off, const uint32_t* key_len,
+                                       const int32_t* key_null_field, uint32_t n_fields, const uint8_t* field_kind,
+                                       uint32_t n_fns, const uint32_t* fn, const int32_t* fn_arg,
+                                       const uint32_t* fn_frame, const uint32_t* val_type, const uint32_t* val_off,
+                                       const int32_t* val_null_field, const uint32_t* fn_flags,
+                                       const uint64_t* fn_default, const int64_t* frame_lower,
+                                       const int64_t* frame_upper, const uint8_t** data, uint64_t* len,
+                                       uint64_t* n_records, uint64_t* n_out_records) {
+  return guarded([&] {
+    S3ShuffleReader::WindowArgs w{n_partition_keys, n_keys,   key_type,        key_off,          key_len,
+                                  key_null_field,   n_fields, field_kind,      n_fns,            fn,
+                                  fn_arg,           B2S_WINDOW_NO_LIMIT, 0,    fn_frame,         val_type,
+                                  val_off,          val_null_field,      true};
+    w.flags = fn_flags;
+    w.dflt = fn_default;
+    w.offset = true;
+    w.lower = frame_lower;
+    w.upper = frame_upper;
+    w.frames = true;
     r->r->readWindowRows(w, n_records);
     sorted_result(*r->r, data, len, n_out_records);
   });
