@@ -140,8 +140,9 @@ void launch_lz4block_fill(const uint8_t* src_base, const uint64_t* d_src_off, co
 
 // ---- lz4_decode_warp_kernel: WARP per LZ4 codec block, token parse and copies in one pass, no per-sequence records.
 //
-// Each step loads the 128 compressed bytes from the cursor ip into shared memory (aligned words that hold block bytes
-// only).  Lane l owns window positions 4l..4l+3 and computes the header a token at each of them would have — ll with
+// Each step puts the 128 compressed bytes from the cursor ip into shared memory (aligned words that hold block bytes
+// only); their loads are issued as soon as the step before has found its cursor, so they fly while that step's bytes
+// are copied.  Lane l owns window positions 4l..4l+3 and computes the header a token at each of them would have — ll with
 // at most one extension byte, the offset, ml with at most one extension byte — and next(p), the position of the token
 // after it.  A header that needs a byte at or past the window's end (or the block's), or a second extension byte, is
 // "unresolved".  Pointer doubling over next (four rounds of shuffles on four byte-packed tables J_k = next^(2^k)) then
@@ -243,21 +244,28 @@ __global__ void __launch_bounds__(kWarpDecWarps * 32, 4)
       continue;
     }
     const int clen = (int)d.clen, olen = (int)d.olen;
+    // the window at p: bytes p .. p + min(clen - p, kWin) - 1 of the block, from the aligned words that contain them
+    // (lane l: word l; lane 31 also word 32), so nothing at or past clen is read
+    auto window_words = [&](int p, uint32_t& w, uint32_t& w32) {
+      const int lim = min(clen - p, kWin);
+      const uintptr_t wa = reinterpret_cast<uintptr_t>(in) + (uintptr_t)p;
+      const uint32_t* wp = reinterpret_cast<const uint32_t*>(wa & ~uintptr_t(3));
+      const int a = (int)(wa & 3u);
+      w = 4 * lane < a + lim ? __ldg(wp + lane) : 0u;
+      w32 = (lane == 31 && kWin < a + lim) ? __ldg(wp + 32) : 0u;
+    };
     int ip = 0, base_op = 0;
     bool err = false;
+    uint32_t w = 0, w32 = 0;  // the window at ip, loaded while the batch before it was copied
+    if (clen > 0) window_words(0, w, w32);
     for (;;) {
       if (ip >= clen) {  // a token must start here
         err = true;
         break;
       }
-      // ---- window: bytes ip .. ip + lim - 1 of the block, from the aligned words that contain them
+      // ---- window: bytes ip .. ip + lim - 1 of the block
       const int lim = min(clen - ip, kWin);
-      const uintptr_t wa = reinterpret_cast<uintptr_t>(in) + (uintptr_t)ip;
-      const uint32_t* wp = reinterpret_cast<const uint32_t*>(wa & ~uintptr_t(3));
-      const int a = (int)(wa & 3u);
-      const unsigned wsh = 8u * (unsigned)a;
-      const uint32_t w = 4 * lane < a + lim ? __ldg(wp + lane) : 0u;
-      const uint32_t w32 = (lane == 31 && kWin < a + lim) ? __ldg(wp + 32) : 0u;
+      const unsigned wsh = 8u * (unsigned)((reinterpret_cast<uintptr_t>(in) + (uintptr_t)ip) & 3u);
       uint32_t wn = __shfl_down_sync(FULL, w, 1);
       if (lane == 31) wn = w32;
       const uint32_t mine = __funnelshift_r(w, wn, wsh);  // window bytes 4*lane .. 4*lane + 3
@@ -337,6 +345,7 @@ __global__ void __launch_bounds__(kWarpDecWarps * 32, 4)
       }
       const int nbatch = nres + (serial ? 1 : 0);
       if (serial) nip = __shfl_sync(FULL, nip, nres);
+      if (nip < clen) window_words(nip, w, w32);  // the next window's loads fly while this batch is copied
       const int op = base_op + inc - (ll + ml);
       if (resolved) {  // the serial lane has checked itself; a resolved token is never the final one
         const int opl = op + ll;
