@@ -373,6 +373,57 @@ int b2s_aggregate_grouping_sets_partition_compress_rows_hash_dev(
     uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_off, uint64_t* dst_len, uint64_t* dst_total,
     uint64_t* checksum_out, int32_t* status, uint64_t* n_groups);
 
+/* ---- write side, window group limit: Spark's Sort and WindowGroupLimitExec(Partial) and its exchange on the GPU ----
+ * The map side of a top-N-per-group window's shuffle (Sort(pk ++ ord, global = false) -> WindowGroupLimitExec(pk, ord,
+ * rank_fn, limit, Partial) -> Exchange hashpartitioning(pk) | SinglePartition) in one call.  A reducer finishes it with
+ * b2s_decompress_window_rows_keys_* and the same limit (WindowGroupLimitExec(Final) and the window).
+ * Records: as for b2s_partition_compress_rows_hash_*: [size: int32 big-endian][row], rec_len[i] = 4 + size.
+ * Key columns: as for b2s_decompress_window_rows_keys_*: n_keys (1..16) composite-key columns, the first
+ * n_partition_keys (0..15) the PARTITION BY columns, with the hash call's types (B2S_KEY_BYTES only as a 1-byte boolean)
+ * and no order flag; the rest, at least one, the ORDER BY columns, of any composite-key type and any order flags.
+ * Sort: the records are sorted stably by the whole key exactly as b2s_decompress_sort_rows_keys_* sorts them, ties in
+ * input order (the local SortExec in front of the Partial limit).
+ * Limit: partitions and peers follow the window call's rules (nulls equal nulls, 0.0 equals -0.0, NaN equals NaN).
+ * limit_fn is B2S_WINDOW_ROW_NUMBER, B2S_WINDOW_RANK or B2S_WINDOW_DENSE_RANK and limit at least 1; a record is kept
+ * when its limit_fn value within its partition is at most limit, so every rank tie at the boundary is kept and
+ * ROW_NUMBER cuts ties in input order.
+ * Outputs: the kept records, unchanged and in sorted order, partitioned stably by pmod(Murmur3Hash(partition columns,
+ * 42), num_partitions) and compressed.  n_partition_keys == 0 is Spark's SinglePartition exchange: num_partitions must
+ * be 1 and every kept record goes to partition 0.  *n_out_records (required) = the kept records.
+ * Defining contract: dst_off / dst_len / checksum_out / status, *dst_total and the return value are byte for byte what
+ * b2s_partition_compress_rows_hash_packed returns for the kept records in sorted order, keyed by the partition columns
+ * at their input slots and null bits; without partition columns, what b2s_partition_compress_packed returns for them
+ * with num_partitions 1 and every id 0.
+ * Sizing: the kept records never outgrow the input, so an arena of
+ *   b2s_partition_compress_bound(codec, codec_block_size, num_partitions, rec_bytes)
+ * always suffices; dst_cap below the arena -> B2S_E_DST_TOO_SMALL with *dst_total = the bytes needed, as the partition
+ * calls.
+ * Errors, B2S_E_ARG, checked before the device: what the hash call rejects for the partition columns; what the window
+ * call rejects for the key (n_keys outside 1..16, a type not listed, a key_len that does not match its type, an order
+ * flag on a partition column, n_partition_keys above 15 or leaving no ORDER BY column); limit_fn not one of the three or
+ * limit < 1; n_partition_keys == 0 with num_partitions != 1; n_records >= 2^32; a NULL n_out_records.  A bad record ->
+ * B2S_E_ARG, nothing reported as written, b2s_last_error() names the lowest bad record and why, by the hash call's
+ * record checks applied to every key column.  A partition of more than 2^31 - 1 records -> B2S_E_UNSUPPORTED, as in the
+ * window call.  Device memory that cannot be had -> B2S_E_NOMEM (the caller keeps Spark's Sort and partial limit).  No
+ * usable device -> B2S_E_CUDA.
+ * Runs on the write lane.  b2s_last_timing: kernel_ms the whole call's device work, dominant_ms / dominant_launches the
+ * limit step (from the input records to the gathered kept records, the sort included).  No exchange-cache form. */
+int b2s_window_limit_partition_compress_rows_hash_packed(
+    uint32_t codec, int32_t level, uint32_t codec_block_size, uint32_t checksum_alg, uint32_t num_partitions,
+    uint64_t n_records, const uint8_t* rec_base, uint64_t rec_bytes, const uint32_t* rec_len,
+    uint32_t n_partition_keys, uint32_t n_keys, const uint32_t* key_type, const uint32_t* key_off,
+    const uint32_t* key_len, const int32_t* key_null_field, uint32_t limit_fn, int32_t limit, uint8_t* dst_base,
+    uint64_t dst_cap, uint64_t* dst_off, uint64_t* dst_len, uint64_t* dst_total, uint64_t* checksum_out,
+    int32_t* status, uint64_t* n_out_records);
+/* same, with rec_base / rec_len / dst_base in device memory of dev_index; the other arrays stay host arrays */
+int b2s_window_limit_partition_compress_rows_hash_dev(
+    uint32_t dev_index, uint32_t codec, int32_t level, uint32_t codec_block_size, uint32_t checksum_alg,
+    uint32_t num_partitions, uint64_t n_records, const uint8_t* rec_base, uint64_t rec_bytes, const uint32_t* rec_len,
+    uint32_t n_partition_keys, uint32_t n_keys, const uint32_t* key_type, const uint32_t* key_off,
+    const uint32_t* key_len, const int32_t* key_null_field, uint32_t limit_fn, int32_t limit, uint8_t* dst_base,
+    uint64_t dst_cap, uint64_t* dst_off, uint64_t* dst_len, uint64_t* dst_total, uint64_t* checksum_out,
+    int32_t* status, uint64_t* n_out_records);
+
 /* ---- write side, range-partitioned rows: Spark's RangePartitioner ids computed on the GPU ----
  * b2s_partition_compress_* for a RangePartitioning exchange of UnsafeRows (a global ORDER BY's map side): the reduce id
  * of every record is what Spark's RangePartitioner.getPartition returns for its sort key over the n_bounds range

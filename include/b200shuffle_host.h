@@ -150,6 +150,14 @@ int b2sh_serialized_writer_aggregate_rows(b2sh_serialized_writer* w, uint32_t n_
  * row once per set and writes the partial rows keyed by the grouping columns and spark_grouping_id.  When the partial
  * rows outgrow the input's bound, commit() retries with the exact size the call reports. */
 int b2sh_serialized_writer_grouping_sets(b2sh_serialized_writer* w, uint32_t n_sets, const uint32_t* set_mask);
+/* The partial limit of a top-N-per-group window's map side (INTEGRATION.md §3r), in place of hash_rows and before the
+ * first insert: commit() makes one b2s_window_limit_partition_compress_rows_hash_packed call with these n_keys window
+ * key columns (the first n_partition_keys the PARTITION BY columns, hashed; the rest the ORDER BY columns; copied),
+ * limit_fn and limit, which sorts the rows, keeps each partition's first rows and hash-partitions them (no partition
+ * columns: SinglePartition, a writer of one partition). */
+int b2sh_serialized_writer_window_limit(b2sh_serialized_writer* w, uint32_t n_partition_keys, uint32_t n_keys,
+                                        const uint32_t* key_type, const uint32_t* key_off, const uint32_t* key_len,
+                                        const int32_t* key_null_field, uint32_t limit_fn, int32_t limit);
 int b2sh_serialized_writer_insert(b2sh_serialized_writer* w, int32_t partition_id, const uint8_t* bytes, uint64_t len);
 int b2sh_serialized_writer_commit(b2sh_serialized_writer* w, int64_t* partition_lengths_out);
 int b2sh_serialized_writer_statistics(b2sh_serialized_writer* w, uint64_t* bytes, uint64_t* nanos, char* line,

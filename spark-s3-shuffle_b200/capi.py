@@ -122,6 +122,12 @@ PROTOTYPES = [
     ("b2s_aggregate_grouping_sets_partition_compress_rows_hash_dev", C.c_int,
      [_u32, _u32, _i32, _u32, _u32, _u32, _u64, _vp, _u64, _u32p, _u32, _u32p, _u32p, _u32p, _i32p, _u32, _u32p, _u32p,
       _u32p, _i32p, _u32, _u32p, _vp, _u64, _u64p, _u64p, _u64p, _u64p, _i32p, _u64p]),
+    ("b2s_window_limit_partition_compress_rows_hash_packed", C.c_int,
+     [_u32, _i32, _u32, _u32, _u32, _u64, _u8p, _u64, _u32p, _u32, _u32, _u32p, _u32p, _u32p, _i32p, _u32, _i32, _u8p,
+      _u64, _u64p, _u64p, _u64p, _u64p, _i32p, _u64p]),
+    ("b2s_window_limit_partition_compress_rows_hash_dev", C.c_int,
+     [_u32, _u32, _i32, _u32, _u32, _u32, _u64, _vp, _u64, _u32p, _u32, _u32, _u32p, _u32p, _u32p, _i32p, _u32, _i32,
+      _vp, _u64, _u64p, _u64p, _u64p, _u64p, _i32p, _u64p]),
     ("b2s_partition_compress_rows_range_packed", C.c_int,
      [_u32, _i32, _u32, _u32, _u64, _u8p, _u64, _u32p, _u32, _u32p, _u32p, _u32p, _i32p, _u32, _u8p, _u64, _u32p,
       _u8p, _u64, _u64p, _u64p, _u64p, _u64p, _i32p]),
@@ -1024,6 +1030,42 @@ def aggregate_grouping_sets_partition_compress_rows_hash_dev(codec, d_records, r
         d_dst, dst_cap, _ptr(dst_off), _ptr(dst_len), C.addressof(total), _ptr(cks), _ptr(st), C.addressof(groups)),
         "b2s_aggregate_grouping_sets_partition_compress_rows_hash_dev")
     return dict(dst_off=dst_off, dst_len=dst_len, total=total.value, checksums=cks, status=st, n_groups=groups.value)
+
+
+def window_limit_partition_compress_rows_hash_packed(codec, records, rec_len, keys, n_partition_keys, limit_fn, limit,
+                                                     num_partitions, dst, block_size=0, checksum_alg=CHECKSUM_NONE,
+                                                     level=0):
+    """Spark's Sort and WindowGroupLimitExec(Partial), then its exchange: the records sorted by keys (the first
+    n_partition_keys the PARTITION BY columns, the rest the ORDER BY columns), those whose limit_fn (WINDOW_ROW_NUMBER,
+    WINDOW_RANK or WINDOW_DENSE_RANK) value in their partition is at most limit kept and hash-partitioned by the partition
+    columns (none: SinglePartition, num_partitions 1).  -> dict(dst_off, dst_len, total, checksums, status,
+    n_out_records)"""
+    records, dst = _as_u8(records), _as_u8(dst)
+    rec_len = np.ascontiguousarray(rec_len, dtype=np.uint32)
+    nk, kt, ko, kl, kn = _key_arrays(keys)
+    dst_off, dst_len, cks, st = _partition_out(num_partitions)
+    total, kept = _u64(0), _u64(0)
+    _check(load().b2s_window_limit_partition_compress_rows_hash_packed(
+        codec, level, block_size, checksum_alg, num_partitions, rec_len.size, _ptr(records), records.size,
+        _ptr(rec_len), n_partition_keys, nk, _ptr(kt), _ptr(ko), _ptr(kl), _ptr(kn), limit_fn, limit, _ptr(dst),
+        dst.size, _ptr(dst_off), _ptr(dst_len), C.addressof(total), _ptr(cks), _ptr(st), C.addressof(kept)),
+        "b2s_window_limit_partition_compress_rows_hash_packed")
+    return dict(dst_off=dst_off, dst_len=dst_len, total=total.value, checksums=cks, status=st, n_out_records=kept.value)
+
+
+def window_limit_partition_compress_rows_hash_dev(codec, d_records, rec_bytes, d_rec_len, n_records, keys,
+                                                  n_partition_keys, limit_fn, limit, num_partitions, d_dst, dst_cap,
+                                                  block_size=0, checksum_alg=CHECKSUM_NONE, level=0, dev=0):
+    """window_limit_partition_compress_rows_hash_packed on device addresses (records, u32 lengths, destination arena)"""
+    nk, kt, ko, kl, kn = _key_arrays(keys)
+    dst_off, dst_len, cks, st = _partition_out(num_partitions)
+    total, kept = _u64(0), _u64(0)
+    _check(load().b2s_window_limit_partition_compress_rows_hash_dev(
+        dev, codec, level, block_size, checksum_alg, num_partitions, n_records, d_records, rec_bytes, d_rec_len,
+        n_partition_keys, nk, _ptr(kt), _ptr(ko), _ptr(kl), _ptr(kn), limit_fn, limit, d_dst, dst_cap, _ptr(dst_off),
+        _ptr(dst_len), C.addressof(total), _ptr(cks), _ptr(st), C.addressof(kept)),
+        "b2s_window_limit_partition_compress_rows_hash_dev")
+    return dict(dst_off=dst_off, dst_len=dst_len, total=total.value, checksums=cks, status=st, n_out_records=kept.value)
 
 
 def _bound_arrays(bounds):

@@ -251,7 +251,8 @@ struct Slot {
   DevBuf pws, parena;  // partition workspace (sort keys, offsets) and the partitioned arena in front of compression
   DevBuf xpieces;      // the copy pieces of an exchange-cache read (exchange.cu)
   DevBuf fws;          // row framing workspace: bitmap over the decoded arena, tile counts, verdicts (rows.cu)
-  DevBuf aggrows;      // a partial aggregation's partial rows, in front of the partition step (partial_agg.cu)
+  DevBuf aggrows;      // a partial aggregation's partial rows (partial_agg.cu) or a window limit's kept rows and their
+                       // lengths (window.cu), in front of the partition step
   DevBuf xrows;        // grouping sets: the projected records' lengths, then the records (rows_expand.cu)
   PinBuf hmeta;
   // per-launch event pairs around the dominant kernel of a call (grow-only pool; dom_used pairs of call dom_call)
@@ -3229,6 +3230,31 @@ static size_t partial_agg_fws_bytes(uint64_t n, const PartialAggSpec& spec) {
          rows_aggregate_ws_bytes(n, 0, 0) + partial_agg_ws_bytes(n, spec);
 }
 
+// The key sort of n checked records (ranges: their one range's offset) and, for a key that refines (rws), its rounds,
+// one readback each: the sorted record indices *idx and the head flags *heads (nullptr: where the key words differ)
+static int sort_checked_rows(Slot& S, const KeySpec& ks, uint64_t n, const uint8_t* d_rec, const uint64_t* ranges,
+                             uint8_t* ws, uint8_t* rws, const uint32_t** idx, const uint32_t** heads,
+                             uint64_t* launches) {
+  cudaStream_t st = S.st;
+  uint64_t* rb = (uint64_t*)S.hmeta.p;
+  *idx = launch_rows_order(d_rec, n, ks, ranges, 1, ws, rws, st, launches);
+  *heads = nullptr;
+  if (!rws) return 0;
+  // the key columns were checked, so no round finds a bad string or decimal
+  for (uint32_t d = kKeyPrefixBytes;; d += kKeyChunkBytes) {
+    launch_rows_refine_mark(n, d, rws, 1, st, launches);
+    CU(cudaMemcpyAsync(rb, rows_refine_readback(rws, n, 1), 8, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    CU(cudaGetLastError());
+    const uint64_t tied = rb[0] & 0xffffffffull, runs = rb[0] >> 32;
+    if (!tied) break;
+    launch_rows_refine_round(d_rec, n, ks, tied, runs, d, ws, rws, 1, st, launches);
+  }
+  *idx = rows_refine_order(rws, n, 1);
+  *heads = rows_refine_heads(rws, n, 1);
+  return 0;
+}
+
 // The aggregation step on S over n device-resident records (d_rec, rec_bytes; d_len): offsets, checks
 // (partial_agg_checked), the key sort and its refinement rounds, the grouping, the folds (one readback: groups,
 // partial-row bytes) and the partial rows into S.aggrows, their record lengths at *row_len (in S.fws).  Marks G1, and G0
@@ -3258,21 +3284,8 @@ static int partial_agg_rows(Slot& S, const PartialAggSpec& spec, uint64_t n, con
     CU(S.mark(G1, st, *launches));
     return 0;
   }
-  const uint32_t* idx = launch_rows_order(d_rec, n, ks, hdr + 3, 1, ws, rws, st, launches);
-  const uint32_t* heads = nullptr;
-  if (refine) {  // the key columns were checked, so no round finds a bad string or decimal
-    for (uint32_t d = kKeyPrefixBytes;; d += kKeyChunkBytes) {
-      launch_rows_refine_mark(n, d, rws, 1, st, launches);
-      CU(cudaMemcpyAsync(rb, rows_refine_readback(rws, n, 1), 8, cudaMemcpyDeviceToHost, st));
-      CU(cudaStreamSynchronize(st));
-      CU(cudaGetLastError());
-      const uint64_t tied = rb[0] & 0xffffffffull, runs = rb[0] >> 32;
-      if (!tied) break;
-      launch_rows_refine_round(d_rec, n, ks, tied, runs, d, ws, rws, 1, st, launches);
-    }
-    idx = rows_refine_order(rws, n, 1);
-    heads = rows_refine_heads(rws, n, 1);
-  }
+  const uint32_t *idx, *heads;
+  if (int rc = sort_checked_rows(S, ks, n, d_rec, hdr + 3, ws, rws, &idx, &heads, launches)) return rc;
   launch_rows_group(d_rec, n, idx, heads, key_bytes, AggSpec{}, ws, gws, st, launches);
   launch_partial_agg_fold(d_rec, n, idx, key_bytes, spec, ws, gws, paws, st, launches);
   CU(cudaMemcpyAsync(rb, hdr + 4, 16, cudaMemcpyDeviceToHost, st));
@@ -3402,6 +3415,45 @@ static int expand_rows(Slot& S, const PartialAggSpec& spec, const PartialAggSpec
   return 0;
 }
 
+// The partition + compress step of a map-side call over the n rows its own step left on S (d_rows, rows_bytes;
+// d_row_len), with the ids of ids, into the caller's arena (packed: into S.dst, sized by the bound, then one download
+// of what fits, *fit bytes; a short caller arena shows up after the run, as in the packed partition call).  Sets
+// dst_off / dst_len / checksum_out / status and *arena; B2S_E_DST_TOO_SMALL leaves them set.
+static int map_rows_partition(Device* D, Slot& S, bool packed, uint32_t codec, int32_t level, uint32_t bs,
+                              uint32_t checksum_alg, uint32_t num_partitions, uint64_t n, const uint8_t* d_rows,
+                              uint64_t rows_bytes, const uint32_t* d_row_len, const RowIds& ids, uint8_t* dst_base,
+                              uint64_t dst_cap, uint64_t* dst_off, uint64_t* dst_len, uint64_t* checksum_out,
+                              int32_t* status, uint64_t* arena, uint64_t* fit, uint64_t* launches) {
+  cudaStream_t st = S.st;
+  uint8_t* d_dst = dst_base;
+  uint64_t cap = dst_cap;
+  int rc;
+  if (packed) {
+    if ((rc = S.dst.ensure(b2s_partition_compress_bound(codec, bs, num_partitions, rows_bytes) + 64))) return rc;
+    d_dst = (uint8_t*)S.dst.p;
+    cap = S.dst.cap;
+  }
+  std::vector<uint64_t> cks(num_partitions);
+  rc = partition_compress_run(D, S, codec, level, bs, checksum_alg, num_partitions, n, d_rows, rows_bytes, d_row_len,
+                              nullptr, d_dst, cap, dst_off, dst_len, cks.data(), status, arena, launches, nullptr, &ids);
+  if (rc && rc != B2S_E_DST_TOO_SMALL) return rc;
+  if (packed) {
+    *fit = std::min(*arena, dst_cap);
+    if (*arena > dst_cap) {
+      for (uint32_t p = 0; p < num_partitions; p++)
+        if (dst_len[p] && dst_off[p] + dst_len[p] > dst_cap) status[p] = B2S_E_DST_TOO_SMALL;
+      rc = fail(B2S_E_DST_TOO_SMALL, "dst_cap is below the %s bytes of the .data arena", std::to_string(*arena).c_str());
+    }
+    CU(S.mark(D0, st));
+    if (*fit) CU(cudaMemcpyAsync(dst_base, S.dst.p, *fit, cudaMemcpyDeviceToHost, st));
+    CU(S.mark(D1, st));
+    CU(cudaStreamSynchronize(st));
+    CU(cudaGetLastError());
+  }
+  if (checksum_out) memcpy(checksum_out, cks.data(), (size_t)num_partitions * 8);
+  return rc;
+}
+
 // b2s_aggregate_partition_compress_rows_hash_* (gs null) and b2s_aggregate_grouping_sets_partition_compress_rows_hash_*:
 // the checks before the device, then on the write lane (with grouping sets, the expansion first) the aggregation step
 // and the partition + compress step over the partial rows, from host records (packed: one upload, one download) or
@@ -3475,34 +3527,11 @@ static int aggregate_partition_call(bool packed, uint32_t dev_index, uint32_t co
     rc = partial_agg_rows(S, spec, n_records, d_rec, rec_bytes, d_len, &groups, &rows_bytes, &d_row_len, &launches);
   }
   if (rc) return rc;
-  const RowIds ids{partial_row_keys(step.keys)};
-  uint8_t* d_dst = dst_base;
-  uint64_t cap = dst_cap;
-  if (packed) {  // sized by the bound: a short caller arena shows up after the run, as in the packed partition call
-    if ((rc = S.dst.ensure(b2s_partition_compress_bound(codec, bs, num_partitions, rows_bytes) + 64))) return rc;
-    d_dst = (uint8_t*)S.dst.p;
-    cap = S.dst.cap;
-  }
-  std::vector<uint64_t> cks(num_partitions);
-  rc = partition_compress_run(D, S, codec, level, bs, checksum_alg, num_partitions, groups,
-                              (const uint8_t*)S.aggrows.p, rows_bytes, d_row_len, nullptr, d_dst, cap, dst_off, dst_len,
-                              cks.data(), status, &arena, &launches, nullptr, &ids);
-  if (rc && rc != B2S_E_DST_TOO_SMALL) return rc;
   uint64_t fit = 0;
-  if (packed) {
-    fit = std::min(arena, dst_cap);
-    if (arena > dst_cap) {
-      for (uint32_t p = 0; p < num_partitions; p++)
-        if (dst_len[p] && dst_off[p] + dst_len[p] > dst_cap) status[p] = B2S_E_DST_TOO_SMALL;
-      rc = fail(B2S_E_DST_TOO_SMALL, "dst_cap is below the %s bytes of the .data arena", std::to_string(arena).c_str());
-    }
-    CU(S.mark(D0, st));
-    if (fit) CU(cudaMemcpyAsync(dst_base, S.dst.p, fit, cudaMemcpyDeviceToHost, st));
-    CU(S.mark(D1, st));
-    CU(cudaStreamSynchronize(st));
-    CU(cudaGetLastError());
-  }
-  if (checksum_out) memcpy(checksum_out, cks.data(), (size_t)num_partitions * 8);
+  rc = map_rows_partition(D, S, packed, codec, level, bs, checksum_alg, num_partitions, groups,
+                          (const uint8_t*)S.aggrows.p, rows_bytes, d_row_len, RowIds{partial_row_keys(step.keys)},
+                          dst_base, dst_cap, dst_off, dst_len, checksum_out, status, &arena, &fit, &launches);
+  if (rc && rc != B2S_E_DST_TOO_SMALL) return rc;
   if (dst_total) *dst_total = arena;
   *n_groups = groups;
   end_call(wt, launches, CallBytes{rec_bytes, arena, packed ? rec_bytes + n_records * 4 : 0, fit}, &S,
@@ -3564,6 +3593,180 @@ int b2s_aggregate_grouping_sets_partition_compress_rows_hash_dev(
                                   n_records, rec_base, rec_bytes, rec_len, n_keys, key_type, key_off, key_len,
                                   key_null_field, n_aggs, agg_fn, val_type, val_off, val_null_field, dst_base, dst_cap,
                                   dst_off, dst_len, dst_total, checksum_out, status, n_groups, &gs);
+}
+
+// ------------------------------------------------------------------------------------------------------------
+// write side, window group limit: a map task's rows sorted by the window key and cut to each partition's first rows
+// by WindowGroupLimitExec(Partial)'s rule, then the hash call's partition + compress step over the kept rows
+// ------------------------------------------------------------------------------------------------------------
+// The limit's own rules, before the device: *n_out, the whole key as a composite key, the partition columns (no order
+// flag, at least one order column after them), the limit, and SinglePartition (num_partitions 1) without partition
+// columns
+static int window_limit_args(const RecordSpec& spec, uint32_t n_partition_keys, uint32_t limit_fn, int32_t limit,
+                             uint32_t num_partitions, const uint64_t* n_out) {
+  if (!n_out) return fail(B2S_E_ARG, "null argument%s");
+  if (int rc = key_columns_args(spec)) return rc;
+  if (n_partition_keys >= spec.n_keys || n_partition_keys >= kMaxKeys)
+    return fail(B2S_E_ARG, "n_partition_keys must be in [0, 15] and leave at least one ORDER BY column%s");
+  for (uint32_t c = 0; c < n_partition_keys; c++)
+    if (spec.keys.type[c] & ~kKeyTypeMask) return fail(B2S_E_ARG, "a partition column takes no order flag%s");
+  if (limit_fn > B2S_WINDOW_DENSE_RANK || limit < 1)
+    return fail(B2S_E_ARG, "limit_fn must be ROW_NUMBER, RANK or DENSE_RANK, with a limit of at least 1%s");
+  if (!n_partition_keys && num_partitions != 1)
+    return fail(B2S_E_ARG, "without partition columns the exchange is SinglePartition: num_partitions must be 1%s");
+  return 0;
+}
+
+// The limit step on S over n device-resident records (d_rec, rec_bytes; d_len): offsets and checks (partial_agg_checked,
+// every key column by the hash call's record checks), the key sort and its refinement rounds, the peer groups, the
+// partitions and limit values (one readback: kept records, their bytes, a partition too large), then the kept records
+// gathered in sorted order into S.aggrows: their lengths, then the records -> *kept, *kept_bytes, *kept_len,
+// *kept_rec.  Marks G0, G1.
+static int window_limit_rows(Slot& S, const KeySpec& ks, const WindowShape& shape, uint64_t n, const uint8_t* d_rec,
+                             uint64_t rec_bytes, const uint32_t* d_len, uint64_t* kept, uint64_t* kept_bytes,
+                             const uint32_t** kept_len, const uint8_t** kept_rec, uint64_t* launches) {
+  cudaStream_t st = S.st;
+  PartialAggSpec checks;  // no buffers; the key columns without their order flags, as the hash kernel reads them
+  checks.keys = ks;
+  for (uint32_t c = 0; c < ks.n; c++) checks.keys.type[c] &= kKeyTypeMask;
+  const uint32_t key_bytes = rows_key_bytes(ks);
+  const bool refine = rows_key_refines(ks);
+  const size_t part[5] = {rows_sort_ws_bytes(n, key_bytes), refine ? rows_refine_ws_bytes(n, 1) : 0,
+                          rows_aggregate_ws_bytes(n, 0, 0), partial_agg_ws_bytes(n, checks), window_ws_bytes(n, shape)};
+  if (int rc = S.fws.ensure(part[0] + part[1] + part[2] + part[3] + part[4])) return rc;
+  uint8_t* ws = (uint8_t*)S.fws.p;
+  uint8_t *rws = refine ? ws + part[0] : nullptr, *gws = ws + part[0] + part[1], *paws = gws + part[2];
+  uint8_t* wws = paws + part[3];
+  if (int rc = S.hmeta.ensure(kWindowReadbackBytes)) return rc;
+  uint64_t* rb = (uint64_t*)S.hmeta.p;
+  CU(S.mark(G0, st, *launches));
+  if (int rc = partial_agg_checked(S, checks, n, d_rec, rec_bytes, d_len, key_bytes, ws, paws,
+                                   (uint32_t*)partial_agg_row_len(paws, n, checks), launches))
+    return rc;
+  *kept = *kept_bytes = 0;
+  if (!n) {
+    CU(S.mark(G1, st, *launches));
+    return 0;
+  }
+  const uint32_t *idx, *heads;
+  if (int rc = sort_checked_rows(S, ks, n, d_rec, partial_agg_header(paws) + 3, ws, rws, &idx, &heads, launches))
+    return rc;
+  launch_rows_group(d_rec, n, idx, heads, key_bytes, AggSpec{}, ws, gws, st, launches);
+  launch_window_limit(d_rec, n, idx, shape, key_bytes, ws, gws, wws, st, launches);
+  CU(cudaMemcpyAsync(rb, window_readback(wws, n, shape), kWindowReadbackBytes, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  CU(cudaGetLastError());
+  if (rb[3]) return fail(B2S_E_UNSUPPORTED, "a window partition holds more than 2^31 - 1 records%s");
+  *kept = rb[0];
+  *kept_bytes = rb[1];
+  const uint64_t len_sz = align_up(rb[0] * 4, 256);
+  if (int rc = S.aggrows.ensure(len_sz + rb[1] + 64)) return rc;
+  *kept_len = (const uint32_t*)S.aggrows.p;
+  *kept_rec = (const uint8_t*)S.aggrows.p + len_sz;
+  launch_window_limit_gather(d_rec, n, idx, rb[0], key_bytes, shape, ws, wws, (uint32_t*)S.aggrows.p,
+                             (uint8_t*)S.aggrows.p + len_sz, st, launches);
+  CU(S.mark(G1, st, *launches));
+  return 0;
+}
+
+// b2s_window_limit_partition_compress_rows_hash_*: the checks before the device, then on the write lane the limit step
+// and the partition + compress step over the kept rows, hashed by the partition columns (none: every id 0, the range
+// ids of no bounds), from host records (packed: one upload, one download) or device ones
+static int window_limit_partition_call(bool packed, uint32_t dev_index, uint32_t codec, int32_t level,
+                                       uint32_t codec_block_size, uint32_t checksum_alg, uint32_t num_partitions,
+                                       uint64_t n_records, const uint8_t* rec_base, uint64_t rec_bytes,
+                                       const uint32_t* rec_len, uint32_t n_partition_keys, uint32_t n_keys,
+                                       const uint32_t* key_type, const uint32_t* key_off, const uint32_t* key_len,
+                                       const int32_t* key_null_field, uint32_t limit_fn, int32_t limit,
+                                       uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_off, uint64_t* dst_len,
+                                       uint64_t* dst_total, uint64_t* checksum_out, int32_t* status,
+                                       uint64_t* n_out_records) {
+  const WallTimer wt = begin_call();
+  if (dst_total) *dst_total = 0;
+  if (n_out_records) *n_out_records = 0;
+  const RecordSpec spec = keys_spec(n_keys, key_type, key_off, key_len, key_null_field);
+  if (int rc = window_limit_args(spec, n_partition_keys, limit_fn, limit, num_partitions, n_out_records)) return rc;
+  const RecordSpec pspec = keys_spec(n_partition_keys, key_type, key_off, key_len, key_null_field);
+  RowIds ids{pspec.keys};
+  const uint32_t bs = block_size_or_default(codec_block_size);
+  int rc;
+  if (n_partition_keys) {
+    rc = hash_args(codec, codec_block_size, checksum_alg, num_partitions, n_records, rec_base, rec_bytes, rec_len,
+                   pspec, dst_base, dst_off, dst_len, status);
+  } else {
+    ids.keys = spec.keys;
+    ids.range = true;
+    rc = partition_args(codec, bs, checksum_alg, num_partitions, n_records, rec_base, rec_bytes, rec_len, nullptr,
+                        dst_base, dst_off, dst_len, status, &ids);
+    if (!rc && !g_ctx) rc = no_device();
+  }
+  if (rc) return rc;
+  if (!n_records && rec_bytes)
+    return fail(B2S_E_ARG, "rec_len sums to 0 bytes, rec_bytes is %s", std::to_string(rec_bytes).c_str());
+  WindowShape shape{};  // no functions: the limit and the partition columns only
+  shape.limit_fn = limit_fn;
+  shape.limit = limit;
+  shape.part = pspec.keys;
+  Device* D;
+  if ((rc = get_device(packed ? t_device : dev_index, &D))) return rc;
+  Lane& Ln = D->lane[kLaneWrite];
+  std::lock_guard<std::mutex> lk(Ln.mtx);
+  Slot& S = Ln.slot[0];
+  const PartialAggTrim trim{S};
+  cudaStream_t st = S.st;
+  const uint8_t* d_rec = rec_base;
+  const uint32_t* d_len = rec_len;
+  if (packed) {  // one upload of [records | rec_len]
+    const size_t rec_sz = align_up(rec_bytes, 16), len_sz = align_up(n_records * 4, 16);
+    if ((rc = S.src.ensure(rec_sz + len_sz + 64))) return rc;
+    d_rec = (const uint8_t*)S.src.p;
+    d_len = (const uint32_t*)((uint8_t*)S.src.p + rec_sz);
+    CU(S.mark(H0, st));
+    if (rec_bytes) CU(cudaMemcpyAsync((uint8_t*)S.src.p, rec_base, rec_bytes, cudaMemcpyHostToDevice, st));
+    if (n_records) CU(cudaMemcpyAsync((uint8_t*)d_len, rec_len, n_records * 4, cudaMemcpyHostToDevice, st));
+    CU(S.mark(H1, st));
+  }
+  uint64_t launches = 0, kept = 0, kept_bytes = 0, arena = 0, fit = 0;
+  const uint32_t* d_kept_len = nullptr;
+  const uint8_t* d_kept = nullptr;
+  if ((rc = window_limit_rows(S, spec.keys, shape, n_records, d_rec, rec_bytes, d_len, &kept, &kept_bytes, &d_kept_len,
+                              &d_kept, &launches)))
+    return rc;
+  rc = map_rows_partition(D, S, packed, codec, level, bs, checksum_alg, num_partitions, kept, d_kept, kept_bytes,
+                          d_kept_len, ids, dst_base, dst_cap, dst_off, dst_len, checksum_out, status, &arena, &fit,
+                          &launches);
+  if (rc && rc != B2S_E_DST_TOO_SMALL) return rc;
+  if (dst_total) *dst_total = arena;
+  *n_out_records = kept;
+  end_call(wt, launches, CallBytes{rec_bytes, arena, packed ? rec_bytes + n_records * 4 : 0, fit}, &S,
+           Family::kPartialAggregate);
+  return rc;
+}
+
+int b2s_window_limit_partition_compress_rows_hash_packed(
+    uint32_t codec, int32_t level, uint32_t codec_block_size, uint32_t checksum_alg, uint32_t num_partitions,
+    uint64_t n_records, const uint8_t* rec_base, uint64_t rec_bytes, const uint32_t* rec_len,
+    uint32_t n_partition_keys, uint32_t n_keys, const uint32_t* key_type, const uint32_t* key_off,
+    const uint32_t* key_len, const int32_t* key_null_field, uint32_t limit_fn, int32_t limit, uint8_t* dst_base,
+    uint64_t dst_cap, uint64_t* dst_off, uint64_t* dst_len, uint64_t* dst_total, uint64_t* checksum_out,
+    int32_t* status, uint64_t* n_out_records) {
+  return window_limit_partition_call(true, 0, codec, level, codec_block_size, checksum_alg, num_partitions, n_records,
+                                     rec_base, rec_bytes, rec_len, n_partition_keys, n_keys, key_type, key_off,
+                                     key_len, key_null_field, limit_fn, limit, dst_base, dst_cap, dst_off, dst_len,
+                                     dst_total, checksum_out, status, n_out_records);
+}
+
+int b2s_window_limit_partition_compress_rows_hash_dev(
+    uint32_t dev_index, uint32_t codec, int32_t level, uint32_t codec_block_size, uint32_t checksum_alg,
+    uint32_t num_partitions, uint64_t n_records, const uint8_t* rec_base, uint64_t rec_bytes, const uint32_t* rec_len,
+    uint32_t n_partition_keys, uint32_t n_keys, const uint32_t* key_type, const uint32_t* key_off,
+    const uint32_t* key_len, const int32_t* key_null_field, uint32_t limit_fn, int32_t limit, uint8_t* dst_base,
+    uint64_t dst_cap, uint64_t* dst_off, uint64_t* dst_len, uint64_t* dst_total, uint64_t* checksum_out,
+    int32_t* status, uint64_t* n_out_records) {
+  return window_limit_partition_call(false, dev_index, codec, level, codec_block_size, checksum_alg, num_partitions,
+                                     n_records, rec_base, rec_bytes, rec_len, n_partition_keys, n_keys, key_type,
+                                     key_off, key_len, key_null_field, limit_fn, limit, dst_base, dst_cap, dst_off,
+                                     dst_len, dst_total, checksum_out, status, n_out_records);
 }
 
 // ------------------------------------------------------------------------------------------------------------

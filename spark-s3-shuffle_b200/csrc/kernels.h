@@ -673,6 +673,18 @@ void launch_window_values(const uint8_t* arena, uint64_t n, const uint32_t* idx,
 void launch_window_emit(const uint8_t* arena, uint64_t n, const uint32_t* idx, uint64_t out_rows, uint32_t key_bytes,
                         const WindowShape& shape, bool limited, uint8_t* d_ws, uint8_t* d_wws, uint8_t* d_dst,
                         cudaStream_t st, uint64_t* launches);
+// The map side's partial limit (WindowGroupLimitExec(Partial)) with a shape of no functions: the partition columns
+// (part), limit_fn and limit.  Per sorted position: whether it starts a partition (as launch_window_values finds it),
+// its limit_fn value, whether the limit keeps it and its record length when kept; the kept records and bytes scanned,
+// and readback words 0, 1 and 3 (the kept records, their bytes, a partition too large).  Uploads the shape.
+void launch_window_limit(const uint8_t* arena, uint64_t n, const uint32_t* idx, const WindowShape& shape,
+                         uint32_t key_bytes, uint8_t* d_ws, uint8_t* d_aws, uint8_t* d_wws, cudaStream_t st,
+                         uint64_t* launches);
+// the out_rows kept records (read back), unchanged and in sorted order, to d_out back to back, a warp per record, and
+// their lengths to d_out_len; the kept positions are compacted first
+void launch_window_limit_gather(const uint8_t* arena, uint64_t n, const uint32_t* idx, uint64_t out_rows,
+                                uint32_t key_bytes, const WindowShape& shape, uint8_t* d_ws, uint8_t* d_wws,
+                                uint32_t* d_out_len, uint8_t* d_out, cudaStream_t st, uint64_t* launches);
 
 // ---------------- exchange.cu (exchange-cache reads: ranges of device memory gathered into one arena) ----------------
 // piece: len bytes at src (device pointer, any alignment) go to d_dst + dst

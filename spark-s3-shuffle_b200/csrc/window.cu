@@ -34,6 +34,9 @@
 //            the values' null bits), its slots, the function slots, its var bytes and the var-valued functions' bytes in
 //            function order (16 per wide decimal, a string's padded to 8; with offset functions each region's offset is
 //            a warp scan of the sizes before it), then the VAR and DECIMAL_WIDE slots' offsets moved
+// A map task's partial limit (WindowGroupLimitExec(Partial), in front of the shuffle) takes the same heads, then a
+// thread per sorted position for its limit value, keep flag and kept length (scanned), and a warp per kept record that
+// copies it unchanged: the partition + compress step's input.
 #include <algorithm>
 
 #include "decimal128.h"
@@ -860,6 +863,44 @@ __global__ void __launch_bounds__(kWindowThreads) window_compact_kernel(uint64_t
     if (next_scanned(rows, j, n, out_rows) != rows[j]) kept[rows[j]] = (uint32_t)j;
 }
 
+// The map side's partial limit, a thread per sorted position j: its limit_fn value within its partition (row number,
+// rank or dense rank, as window_values_kernel derives them), rows[j] = whether it is at most limit, bytes[j] = the
+// kept record's length (else 0), and readback[3] = 1 for a partition of more than 2^31 - 1 records
+__global__ void __launch_bounds__(kWindowThreads) window_limit_kernel(
+    const uint32_t* __restrict__ rec_len, const uint32_t* __restrict__ idx, uint64_t n, uint32_t limit_fn,
+    uint64_t limit, const uint64_t* __restrict__ heads_before, const uint32_t* __restrict__ gpos,
+    const uint64_t* __restrict__ groups, const uint64_t* __restrict__ phead, const uint32_t* __restrict__ pstart,
+    uint64_t* __restrict__ rows, uint64_t* __restrict__ bytes, uint64_t* __restrict__ readback) {
+  const uint64_t G = *groups, P = phead[n];
+  for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (uint64_t)gridDim.x * blockDim.x) {
+    const uint64_t g = next_scanned(heads_before, j, n, G) - 1, p = next_scanned(phead, j, n, P) - 1;
+    const uint64_t ps = pstart[p];
+    if (pstart[p + 1] - ps > 0x7fffffffull) readback[3] = 1;
+    const uint64_t lv = limit_fn == B2S_WINDOW_ROW_NUMBER ? j - ps + 1
+                        : limit_fn == B2S_WINDOW_RANK     ? gpos[g] - ps + 1
+                                                          : g - heads_before[ps] + 1;  // ps is a peer head
+    const bool keep = lv <= limit;
+    rows[j] = keep;
+    bytes[j] = keep ? rec_len[at(idx, j)] : 0;
+  }
+}
+
+// Kept record t, by a warp: the record of the sorted position kept[t], unchanged, to dst + bytes[kept[t]] (the scanned
+// kept lengths), its length to out_len[t]
+__global__ void __launch_bounds__(kWindowThreads) window_limit_gather_kernel(
+    const uint8_t* __restrict__ arena, const uint64_t* __restrict__ rec_off, const uint32_t* __restrict__ rec_len,
+    const uint32_t* __restrict__ idx, uint64_t out_rows, const uint32_t* __restrict__ kept,
+    const uint64_t* __restrict__ bytes, uint32_t* __restrict__ out_len, uint8_t* __restrict__ dst) {
+  const uint32_t lane = threadIdx.x & 31;
+  const uint64_t warps = (uint64_t)gridDim.x * (blockDim.x / 32);
+  for (uint64_t t = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) / 32; t < out_rows; t += warps) {
+    const uint64_t j = kept[t];
+    const uint32_t i = at(idx, j), len = rec_len[i];
+    warp_copy(dst + bytes[j], arena + rec_off[i], len, lane);
+    if (lane == 0) out_len[t] = len;
+  }
+}
+
 // Output row t, by a warp: the sorted position j = kept[t] (no limit: t) and its record; the output row is
 // [out_bw null words: the input's n bits][the input's slots][the function slots][the input's var bytes]
 __global__ void __launch_bounds__(kWindowThreads) window_emit_kernel(
@@ -981,6 +1022,18 @@ uint64_t* window_readback(uint8_t* d_wws, uint64_t n, const WindowShape& shape) 
   return carve_window_ws(d_wws, n, shape).readback;
 }
 
+// the partitions of the peer groups in d_aws (the shape uploaded to w.shape): head flags scanned into w.phead (the count
+// at [n]), the partitions' first positions into w.pstart
+static void launch_window_partitions(const uint8_t* arena, uint64_t n, const uint32_t* idx, const KeySortWs& k,
+                                     const WindowWs& w, uint8_t* d_aws, cudaStream_t st, uint64_t* launches) {
+  window_part_heads_kernel<<<grid_for(n), kWindowThreads, 0, st>>>(arena, k.src_off, k.len, idx, n, w.shape,
+                                                                   rows_group_heads_before(d_aws, n),
+                                                                   rows_aggregate_readback(d_aws, n, 0, 0), w.phead);
+  launch_exclusive_scan_u64(w.phead, n, w.phead + n, w.scan_ws, st, launches);
+  window_part_starts_kernel<<<grid_for(n), kWindowThreads, 0, st>>>(w.phead, n, w.pstart);
+  if (launches) *launches += 2;
+}
+
 void launch_window_values(const uint8_t* arena, uint64_t n, const uint32_t* idx, WindowShape shape,
                           const uint32_t* h_fields, uint32_t key_bytes, uint8_t* d_ws, uint8_t* d_aws, uint8_t* d_wws,
                           cudaStream_t st, uint64_t* launches) {
@@ -993,11 +1046,7 @@ void launch_window_values(const uint8_t* arena, uint64_t n, const uint32_t* idx,
   cudaMemsetAsync(w.readback + 4, 0xff, 8, st);
   const uint64_t* heads_before = rows_group_heads_before(d_aws, n);
   const uint64_t* groups = rows_aggregate_readback(d_aws, n, 0, 0);
-  window_part_heads_kernel<<<grid_for(n), kWindowThreads, 0, st>>>(arena, k.src_off, k.len, idx, n, w.shape,
-                                                                   heads_before, groups, w.phead);
-  launch_exclusive_scan_u64(w.phead, n, w.phead + n, w.scan_ws, st, launches);
-  window_part_starts_kernel<<<grid_for(n), kWindowThreads, 0, st>>>(w.phead, n, w.pstart);
-  if (launches) *launches += 2;
+  launch_window_partitions(arena, n, idx, k, w, d_aws, st, launches);
   const WindowFrameIo fio{w.fs, w.ft, w.rlo[0], w.rhi[0], w.rcnt[0]};
   if (shape.n_bnd) {  // sliding frames: the order column staged for a RANGE offset, then every bounds set's frames
     if (shape.ord_staged)
@@ -1094,6 +1143,37 @@ void launch_window_emit(const uint8_t* arena, uint64_t n, const uint32_t* idx, u
                                                       limited ? w.kept : nullptr, w.shape, w.vals, w.bytes,
                                                       shape.n_agg || shape.n_off ? w.vnul : nullptr, w.vhi, d_dst);
   if (launches) *launches += 1;
+}
+
+void launch_window_limit(const uint8_t* arena, uint64_t n, const uint32_t* idx, const WindowShape& shape,
+                         uint32_t key_bytes, uint8_t* d_ws, uint8_t* d_aws, uint8_t* d_wws, cudaStream_t st,
+                         uint64_t* launches) {
+  const WindowWs w = carve_window_ws(d_wws, n, shape);
+  const KeySortWs k = carve_key_sort_ws(d_ws, n, key_bytes);
+  cudaMemcpyAsync(w.shape, &shape, sizeof(WindowShape), cudaMemcpyHostToDevice, st);
+  cudaMemsetAsync(w.readback, 0, kWindowReadbackBytes, st);
+  launch_window_partitions(arena, n, idx, k, w, d_aws, st, launches);
+  window_limit_kernel<<<grid_for(n), kWindowThreads, 0, st>>>(
+      k.len, idx, n, shape.limit_fn, (uint64_t)shape.limit, rows_group_heads_before(d_aws, n),
+      rows_group_starts(d_aws, n), rows_aggregate_readback(d_aws, n, 0, 0), w.phead, w.pstart, w.rows, w.bytes,
+      w.readback);
+  launch_exclusive_scan_u64(w.rows, n, w.readback, w.scan_ws, st, launches);
+  launch_exclusive_scan_u64(w.bytes, n, w.readback + 1, w.scan_ws, st, launches);
+  if (launches) *launches += 1;
+}
+
+void launch_window_limit_gather(const uint8_t* arena, uint64_t n, const uint32_t* idx, uint64_t out_rows,
+                                uint32_t key_bytes, const WindowShape& shape, uint8_t* d_ws, uint8_t* d_wws,
+                                uint32_t* d_out_len, uint8_t* d_out, cudaStream_t st, uint64_t* launches) {
+  if (!out_rows) return;
+  const WindowWs w = carve_window_ws(d_wws, n, shape);
+  const KeySortWs k = carve_key_sort_ws(d_ws, n, key_bytes);
+  window_compact_kernel<<<grid_for(n), kWindowThreads, 0, st>>>(n, w.rows, out_rows, w.kept);
+  const uint64_t want = (out_rows + kWindowThreads / 32 - 1) / (kWindowThreads / 32);
+  const unsigned grid = (unsigned)std::min<uint64_t>(want, (uint64_t)kSMs * 16);
+  window_limit_gather_kernel<<<grid, kWindowThreads, 0, st>>>(arena, k.src_off, k.len, idx, out_rows, w.kept, w.bytes,
+                                                              d_out_len, d_out);
+  if (launches) *launches += 2;
 }
 
 }  // namespace b2s

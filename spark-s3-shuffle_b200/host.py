@@ -98,6 +98,7 @@ PROTOTYPES = [
     ("b2sh_serialized_writer_round_robin_rows", C.c_int, [_vp, _u32, _i32, _u32]),
     ("b2sh_serialized_writer_aggregate_rows", C.c_int, [_vp, _u32, _vp, _vp, _vp, _vp]),
     ("b2sh_serialized_writer_grouping_sets", C.c_int, [_vp, _u32, _vp]),
+    ("b2sh_serialized_writer_window_limit", C.c_int, [_vp, _u32, _u32, _vp, _vp, _vp, _vp, _u32, _i32]),
     ("b2sh_serialized_writer_insert", C.c_int, [_vp, _i32, _vp, _u64]),
     ("b2sh_serialized_writer_commit", C.c_int, [_vp, _vp]),
     ("b2sh_serialized_writer_statistics", C.c_int, [_vp, C.POINTER(_u64), C.POINTER(_u64), C.c_char_p, _u32]),
@@ -341,6 +342,16 @@ class S3SerializedShuffleWriter:
         keyed by the grouping columns and spark_grouping_id"""
         m = np.array(list(masks) or [0], dtype=np.uint32)
         _check(load().b2sh_serialized_writer_grouping_sets(self._h, len(masks), m.ctypes.data))
+
+    def windowLimitRows(self, keys, nPartitionKeys, limitFn, limit):
+        """the partial limit of a top-N-per-group window, in place of hashRows and before the first insert: keys = the
+        window key as hashRows takes it (the first nPartitionKeys the PARTITION BY columns, then the ORDER BY columns,
+        order flags allowed); commit() sorts the rows, keeps those whose limitFn value in their partition is at most
+        limit and hash-partitions them by the partition columns"""
+        keys = list(keys)
+        arrs = [np.array([k[i] for k in keys] or [0], dtype=np.int32 if i == 3 else np.uint32) for i in range(4)]
+        _check(load().b2sh_serialized_writer_window_limit(self._h, nPartitionKeys, len(keys),
+                                                          *[a.ctypes.data for a in arrs], limitFn, limit))
 
     def insertRecord(self, partitionId, record):
         a = np.frombuffer(record, dtype=np.uint8) if not isinstance(record, np.ndarray) else np.ascontiguousarray(record)

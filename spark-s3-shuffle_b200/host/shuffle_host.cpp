@@ -550,7 +550,7 @@ class S3SerializedShuffleWriter {
   void aggregateRows(uint32_t nAggs, const uint32_t* fn, const uint32_t* valType, const uint32_t* valOff,
                      const int32_t* valNull) {
     if (!recLen_.empty()) throw RuntimeException("Precondition: aggregate_rows must come before the first insert.");
-    if (keyType_.empty() || range_ || roundRobin_)
+    if (keyType_.empty() || range_ || roundRobin_ || windowLimit_)
       throw RuntimeException("Precondition: aggregate_rows needs hash_rows first.");
     if (nAggs > 16) throw RuntimeException("Precondition: n_aggs must be at most 16.");
     if (nAggs && (!fn || !valType || !valOff || !valNull)) throw RuntimeException("Precondition: null aggregate arrays.");
@@ -569,6 +569,22 @@ class S3SerializedShuffleWriter {
     if (!aggregate_) throw RuntimeException("Precondition: grouping_sets needs aggregate_rows first.");
     if (!nSets || !mask) throw RuntimeException("Precondition: grouping_sets needs at least one set.");
     setMask_.assign(mask, mask + nSets);
+  }
+  // The partial limit of a top-N-per-group window's map side (b2s_window_limit_partition_compress_rows_hash_packed), in
+  // place of hashRows and before the first insert: commit() sorts the rows by these key columns (the first nPartKeys the
+  // PARTITION BY columns, then the ORDER BY columns), keeps those whose limitFn value in their partition is at most
+  // limit, and hash-partitions them by the partition columns on the GPU (none: SinglePartition).  No cached form exists,
+  // so the call is the same with the exchange cache on.
+  void windowLimit(uint32_t nPartKeys, uint32_t nKeys, const uint32_t* type, const uint32_t* off, const uint32_t* len,
+                   const int32_t* nullField, uint32_t limitFn, int32_t limit) {
+    if (!keyType_.empty() || roundRobin_)
+      throw RuntimeException("Precondition: window_limit takes the place of hash_rows, range_rows and round_robin_rows.");
+    if (nPartKeys >= nKeys) throw RuntimeException("Precondition: window_limit needs an ORDER BY column.");
+    hashRows(nKeys, type, off, len, nullField);
+    windowLimit_ = true;
+    limitPartKeys_ = nPartKeys;
+    limitFn_ = limitFn;
+    limit_ = limit;
   }
   void insertRecord(int32_t partitionId, const uint8_t* b, uint64_t n) {
     const bool hashed = !keyType_.empty() || roundRobin_;
@@ -621,6 +637,14 @@ class S3SerializedShuffleWriter {
         if (rc != B2S_E_DST_TOO_SMALL || attempt) break;
         out_.resize(total);
       }
+    } else if (windowLimit_) {
+      call = "b2s_window_limit_partition_compress_rows_hash_packed";
+      uint64_t kept = 0;
+      rc = b2s_window_limit_partition_compress_rows_hash_packed(
+          codec, d_.zstdLevel, d_.lz4BlockSize, alg, R, recLen_.size(), records_.data(), records_.size(),
+          recLen_.data(), limitPartKeys_, (uint32_t)keyType_.size(), keyType_.data(), keyOff_.data(), keyLen_.data(),
+          keyNull_.data(), limitFn_, limit_, out_.data(), bound, doff.data(), dlen.data(), &total, cks.data(),
+          status.data(), &kept);
     } else if (roundRobin_ && cache) {
       call = "b2s_partition_compress_rows_round_robin_cached_packed";
       rc = b2s_partition_compress_rows_round_robin_cached_packed(
@@ -698,6 +722,9 @@ class S3SerializedShuffleWriter {
   std::vector<uint32_t> aggFn_, aggType_, aggOff_;
   std::vector<int32_t> aggNull_;
   std::vector<uint32_t> setMask_;  // groupingSets: the rows are expanded once per set before the aggregation
+  bool windowLimit_ = false;  // windowLimit: hashRows' key columns are the window key, the first limitPartKeys_ hashed
+  uint32_t limitPartKeys_ = 0, limitFn_ = 0;
+  int32_t limit_ = 0;
   bool roundRobin_ = false;  // roundRobinRows: Spark's repartition(n) order and ids from rrStart_
   int32_t rrStart_ = 0;
   uint32_t rrSort_ = 0;
@@ -1593,6 +1620,13 @@ int b2sh_serialized_writer_aggregate_rows(b2sh_serialized_writer* w, uint32_t n_
 }
 int b2sh_serialized_writer_grouping_sets(b2sh_serialized_writer* w, uint32_t n_sets, const uint32_t* set_mask) {
   return guarded([&] { w->w->groupingSets(n_sets, set_mask); });
+}
+int b2sh_serialized_writer_window_limit(b2sh_serialized_writer* w, uint32_t n_partition_keys, uint32_t n_keys,
+                                        const uint32_t* key_type, const uint32_t* key_off, const uint32_t* key_len,
+                                        const int32_t* key_null_field, uint32_t limit_fn, int32_t limit) {
+  return guarded([&] {
+    w->w->windowLimit(n_partition_keys, n_keys, key_type, key_off, key_len, key_null_field, limit_fn, limit);
+  });
 }
 int b2sh_serialized_writer_insert(b2sh_serialized_writer* w, int32_t partition_id, const uint8_t* bytes, uint64_t len) {
   return guarded([&] { w->w->insertRecord(partition_id, bytes, len); });
