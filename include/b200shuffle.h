@@ -88,6 +88,13 @@ extern "C" {
 #define B2S_AGG_SUM_DECIMAL (9)  /* Sum(decimal)'s and Average(decimal)'s sum: exact, null on overflow of 10^P */
 #define B2S_AGG_MIN_DECIMAL (10) /* Min(decimal p > 18) */
 #define B2S_AGG_MAX_DECIMAL (11) /* Max(decimal p > 18) */
+/* Spark's CentralMomentAgg buffers of order 2 (stddev_*, var_*): one entry over three consecutive 8-byte double slots,
+ * n at agg_off, avg at agg_off + 8, m2 at agg_off + 16; never null (agg_null_field -1), no precision bits.  The group's
+ * buffer starts at (0.0, 0.0, 0.0) and merges each record's (n2, avg2, m2b) in stable order by mergeExpressions:
+ *   newN = n1 + n2; delta = avg2 - avg1; deltaN = newN == 0.0 ? 0.0 : delta / newN;
+ *   avg' = avg1 + deltaN * n2; m2' = (m2a + m2b) + ((delta * deltaN) * n1) * n2; n' = newN
+ * every operation one IEEE double operation rounded to nearest, left to right, no FMA. */
+#define B2S_AGG_VARIANCE (B2S_AGG_MAX_DECIMAL + 1)
 
 /* per-block status / call errors.  The Scala shim maps them to the reference's exception types:            */
 #define B2S_OK 0
@@ -246,7 +253,8 @@ int b2s_partition_compress_rows_hash_dev(uint32_t dev_index, uint32_t codec, int
  * Grouping: a group is a maximal set of records whose every key column is equal by the composite-key aggregation's
  * rule: nulls equal nulls, strings are equal when their lengths and bytes are, 0.0 equals -0.0, every NaN equals every
  * NaN.
- * Aggregates: agg_fn[a] (a < n_aggs, at most 16; 0 is DISTINCT) is B2S_WINDOW_SUM .. B2S_WINDOW_AVG, val_type[a] a
+ * Aggregates: agg_fn[a] (a < n_aggs, at most 16; 0 is DISTINCT) is B2S_WINDOW_SUM .. B2S_WINDOW_AVG or
+ * B2S_WINDOW_VARIANCE, val_type[a] a
  * B2S_WINDOW_VAL_* (a decimal(p, s): B2S_WINDOW_VAL_DECIMAL | p << 8 | s << 16), val_off[a] the input's 8-byte slot
  * (for p > 18 the slot (offset << 32) | size names 1..16 big-endian two's-complement bytes), val_null_field[a] its
  * null bit or -1, as in the window aggregate call.  The semantics are Spark 3.5's DeclarativeAggregate.updateExpressions
@@ -272,9 +280,15 @@ int b2s_partition_compress_rows_hash_dev(uint32_t dev_index, uint32_t codec, int
  *                            Spark's Least / Greatest in Spark SQL's order (-0.0 equals 0.0, NaN above every other value
  *                            and equal to every NaN): among equal values the first is kept, with its exact bits.  Null
  *                            if none.  Merge: B2S_AGG_MIN / MAX_INT32, _INT64, _FLOAT64, _DECIMAL
- * Partial row: as UnsafeProjection(groupingAttributes ++ aggBufferAttributes) writes it, with nf = n_keys + buffers
- * (at most 32, so one null word, b = 1): field c < n_keys is key column c, buffer k is field n_keys + k, whose null bit
- * is set only for a null value.  Fixed values are written as UnsafeRowWriter writes them (the 8-byte slot zeroed, then
+ *   VARIANCE (16) int8 ..    stddev / stddev_samp / stddev_pop / variance / var_samp / var_pop (CentralMomentAgg, order
+ *   int64, float, double     2): three doubles n, avg, m2, from (0, 0, 0), each non-null input x = Cast(child, Double) (a
+ *                            long rounded to nearest, a float widened) in input order by updateExpressions: newN = n +
+ *                            1.0; delta = x - avg; deltaN = delta / newN; avg' = avg + deltaN; m2' = m2 + delta * (delta
+ *                            - deltaN); every operation one IEEE double operation rounded to nearest, no FMA.  Never
+ *                            null.  One buffer, three fields.  Merge: B2S_AGG_VARIANCE at n's slot (null field -1)
+ * Partial row: as UnsafeProjection(groupingAttributes ++ aggBufferAttributes) writes it, with nf = n_keys + fields,
+ * the fields being 1 per buffer and 3 per VARIANCE (at most 32, so one null word, b = 1): field c < n_keys is key column
+ * c, then the buffers' fields in order, whose null bit is set only for a null value.  Fixed values are written as UnsafeRowWriter writes them (the 8-byte slot zeroed, then
  * the type's width; an isEmpty boolean one byte).  Key values come from the group's first record in input order; float
  * and double keys are normalized as NormalizeNaNAndZero leaves them (-0.0 as 0.0, any NaN as the canonical NaN).  Var
  * regions follow the fixed region 8 (b + nf), in field order: a string or binary key its bytes zero-padded to 8 (a null
@@ -294,7 +308,8 @@ int b2s_partition_compress_rows_hash_dev(uint32_t dev_index, uint32_t codec, int
  * Errors, B2S_E_ARG, checked before the device: what the hash call rejects; n_records >= 2^32; n_aggs above 16 or a
  * NULL aggregate array (n_aggs > 0) or n_groups; an unknown function or val_type; a decimal p outside 1..38 or s > p;
  * VAL_NONE or VAL_BYTES with a function other than COUNT; MIN / MAX of byte, short, float or bytes (the reducer cannot
- * merge them); decimal SUM with p > 28 or AVG with p > 27; more than 16 buffers in all (the reduce-side merge's limit);
+ * merge them); decimal SUM with p > 28 or AVG with p > 27; VARIANCE of a decimal, VAL_NONE or VAL_BYTES; more than 16
+ * buffers in all (the reduce-side merge's limit; a VARIANCE is one); n_keys + fields above 32;
  * a val_off that is not a multiple of 8 of at least 8 (a field's slot), or a val_null_field outside -1..65535.  A bad
  * record -> B2S_E_ARG, nothing reported as written, b2s_last_error() names the lowest bad record and why: the hash call's
  * record checks, a row that does not hold a value slot or a value's null word, a non-null decimal(p > 18) value whose
@@ -333,7 +348,8 @@ int b2s_aggregate_partition_compress_rows_hash_dev(
  * are read from record r unmasked: Spark's aggregate functions reference the child's attribute, not the nulled
  * grouping alias.
  * Partial rows: n_keys grouping columns, every one nullable, then gid (INT64, slot 8 + 8 n_keys), then the buffers, as
- * UnsafeProjection(groupingAttributes ++ aggBufferAttributes) writes them; nf = n_keys + 1 + buffers <= 32.  They come
+ * UnsafeProjection(groupingAttributes ++ aggBufferAttributes) writes them; nf = n_keys + 1 + fields <= 32 (3 fields
+ * per VARIANCE, 1 per other buffer).  They come
  * in the composite-key order of (grouping columns ascending, nulls first; gid) and are partitioned by
  * pmod(Murmur3Hash(grouping columns, gid; 42), num_partitions).
  * Defining contract: dst_off / dst_len / checksum_out / status, *dst_total, *n_groups and the return value are byte for
@@ -342,8 +358,8 @@ int b2s_aggregate_partition_compress_rows_hash_dev(
  * same aggregates at their projected slots.
  * Errors, B2S_E_ARG, checked before the device: what b2s_aggregate_partition_compress_rows_hash_* rejects; n_keys outside
  * 1..15 (gid takes the 16th key column); n_sets == 0 or a NULL set_mask; a mask bit at or above n_keys; two equal masks
- * (Spark adds a _gen_grouping_pos column for duplicate sets); n_records * n_sets >= 2^32.  (n_keys + 1 + buffers is then
- * at most 32.)  The empty set (mask 0, the grand total) and a single full set are allowed.  A bad record -> B2S_E_ARG
+ * (Spark adds a _gen_grouping_pos column for duplicate sets); n_records * n_sets >= 2^32; n_keys + 1 + fields above 32
+ * (only VARIANCE buffers can pass it).  The empty set (mask 0, the grand total) and a single full set are allowed.  A bad record -> B2S_E_ARG
  * naming its input index, for the reasons b2s_aggregate_partition_compress_rows_hash_* gives.  A record whose row,
  * projected for a set (its in-set strings, 16 bytes per decimal(p > 18) key or input, 8 (2 + nf') bytes of fixed region),
  * would pass 2^31 - 1 bytes -> B2S_E_UNSUPPORTED.  Device memory that cannot be had -> B2S_E_NOMEM (the caller keeps
@@ -636,6 +652,10 @@ int b2s_decompress_sort_rows_dev(uint32_t dev_index, uint32_t codec, uint32_t ch
  *                                       with bytes 1..7 zero, so the minimum is the AND Spark merges with)
  *     Average(decimal) [sum, count]   : SUM_DECIMAL | P << 8, SUM_INT64
  *     Min / Max(decimal p > 18)       : MIN / MAX_DECIMAL
+ *     CentralMomentAgg [n, avg, m2]   : B2S_AGG_VARIANCE at n's slot, agg_null_field -1 (stddev_* / var_*)
+ *   B2S_AGG_VARIANCE : one entry over three consecutive double slots (agg_off, + 8, + 16), merged by mergeExpressions
+ *       from (0, 0, 0) over every record of the group in stable order (see its define); never null, so no null bit
+ *       is written.  Its 24 bytes count in every overlap check and in the row length a record must have.
  * Output: one record per group, back to back, groups in the row sort's order (ascending, nulls first) — again a valid
  * UnsafeRowSerializer stream.  A group's record is its first record in stable order, byte for byte (size prefix and
  * variable-length region included) except each aggregate's slot and null bit.  *dst_total = output bytes, *n_records =
@@ -652,7 +672,8 @@ int b2s_decompress_sort_rows_dev(uint32_t dev_index, uint32_t codec, uint32_t ch
  * are as in b2s_decompress_sort_*.  dst_cap below the output bytes -> B2S_E_DST_TOO_SMALL with *dst_total = the bytes
  * needed.
  * Errors -> B2S_E_ARG: those of b2s_decompress_sort_rows_packed; n_aggs > 16; an unknown op; precision bits on any op
- * but SUM_DECIMAL, or a SUM_DECIMAL precision of 0 or above 38; SUM_DECIMAL with agg_null_field[a] = -1;
+ * but SUM_DECIMAL, or a SUM_DECIMAL precision of 0 or above 38; SUM_DECIMAL with agg_null_field[a] = -1; VARIANCE with
+ * agg_null_field[a] >= 0;
  * agg_null_field[a] < -1;
  * NULL agg arrays with n_aggs > 0; an aggregate slot that overlaps another slot, the key bytes, or an 8-byte null word
  * that the key or an aggregate uses.
@@ -1070,6 +1091,9 @@ int b2s_decompress_window_aggregate_rows_keys_dev(
 #define B2S_WINDOW_FIRST 13
 #define B2S_WINDOW_LAST 14
 #define B2S_WINDOW_NTH_VALUE 15
+/* the partial aggregation's central-moment function (stddev / variance, b2s_aggregate_*partition_compress_rows_hash_*
+ * only; every window call rejects it) */
+#define B2S_WINDOW_VARIANCE 16
 #define B2S_WINDOW_VAL_BYTES 8
 #define B2S_WINDOW_IGNORE_NULLS 1
 #define B2S_WINDOW_HAS_DEFAULT 2

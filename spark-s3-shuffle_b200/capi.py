@@ -22,6 +22,9 @@ KEY_DESCENDING, KEY_NULLS_LAST = 1 << 8, 1 << 9
  AGG_MAX_FLOAT64) = range(8)
 # the Decimal ops (8 is unassigned); SUM_DECIMAL takes its buffer's precision P (1..38) as AGG_SUM_DECIMAL | P << 8
 AGG_SUM_DECIMAL, AGG_MIN_DECIMAL, AGG_MAX_DECIMAL = 9, 10, 11
+# Spark's CentralMomentAgg buffers [n, avg, m2] (stddev_*, var_*): one entry over three 8-byte doubles at off, off + 8,
+# off + 16; never null (null field -1)
+AGG_VARIANCE = 12
 # join types of the row join (decompress_join_rows_keys_*) and the field kinds of its sides' schemas
 JOIN_INNER, JOIN_LEFT_OUTER, JOIN_LEFT_SEMI, JOIN_LEFT_ANTI = 0, 1, 2, 3
 JOIN_RIGHT_OUTER, JOIN_FULL_OUTER = 5, 6  # 4 is not assigned
@@ -41,6 +44,9 @@ WINDOW_FRAME_PARTITION, WINDOW_FRAME_ROWS_RUNNING, WINDOW_FRAME_RANGE_RUNNING = 
 # per-function flags
 WINDOW_LAG, WINDOW_LEAD, WINDOW_FIRST, WINDOW_LAST, WINDOW_NTH_VALUE = range(11, 16)
 WINDOW_VAL_BYTES = 8
+# the partial aggregation's central-moment function (aggregate_*partition_compress_rows_hash_*; its buffers n, avg and
+# m2 are three partial-row fields, merged by AGG_VARIANCE); the window calls reject it
+WINDOW_VARIANCE = 16
 WINDOW_IGNORE_NULLS, WINDOW_HAS_DEFAULT = 1, 2
 # the sliding frames of the frame window (decompress_window_frame_rows_keys_*) and their unbounded ends; a bound is
 # otherwise 0 (CURRENT ROW), -k (k PRECEDING) or +k (k FOLLOWING)
@@ -948,7 +954,7 @@ def partition_compress_rows_hash_dev(codec, d_records, rec_bytes, d_rec_len, n_r
 
 
 def _partial_agg_arrays(aggs):
-    """aggs = [(fn, val_type, val_off, val_null_field), ...]: WINDOW_SUM / COUNT / MIN / MAX / AVG, WINDOW_VAL_* or
+    """aggs = [(fn, val_type, val_off, val_null_field), ...]: WINDOW_SUM / COUNT / MIN / MAX / AVG / VARIANCE, WINDOW_VAL_* or
     window_val_decimal(p, s) -> (n, fn, val_type, val_off, val_null_field) arrays"""
     aggs = list(aggs)
     cols = list(zip(*aggs)) if aggs else [[0]] * 4

@@ -21,6 +21,10 @@
 // 16-byte region.  The sum is exact and null once an input is null or a running sum leaves (-10^P, 10^P): a thread adds
 // with the 128-bit overflow of decimal128.h; a warp scans each round of 32 inputs in three 64-bit words (33 * 10^38 <
 // 2^133), adds the rounds before it and checks every lane's running sum with one vote.
+// B2S_AGG_VARIANCE (Spark's CentralMomentAgg [n, avg, m2]) is merged by kernels of its own too (the *_var kernels,
+// which also know the Decimal ops): the heads step stages n with the other slots and avg, m2 in arrays of their own; a
+// thread per small group, or a warp per large one (loads in parallel, each lane's triple broadcast in turn), runs
+// mergeExpressions in stable order from (0, 0, 0), one rounded double operation at a time.
 #include <algorithm>
 
 #include "decimal128.h"
@@ -44,7 +48,7 @@ inline unsigned grid_for(uint64_t n) {
 
 // the aggregate workspace: heads (scanned in place), readback [groups, output bytes, decimal verdict], per group the
 // head's record index, first position (+ n at the end) and record length, the dense null bits and values, the high
-// words of the out-of-line decimals, the spec
+// words of the out-of-line decimals, the spec, the variance entries' avg and m2 words
 struct AggWs {
   uint64_t* head;
   uint64_t* readback;
@@ -55,9 +59,10 @@ struct AggWs {
   uint64_t* vals;
   uint64_t* vhi;
   AggSpec* spec;
+  uint64_t* vmom;
 };
 
-AggWs carve_agg_ws(uint8_t* d_aws, uint64_t n, uint32_t n_aggs, uint32_t n_wide) {
+AggWs carve_agg_ws(uint8_t* d_aws, uint64_t n, uint32_t n_aggs, uint32_t n_wide, uint32_t n_var = 0) {
   AggWs a;
   uint8_t* p = d_aws;
   a.head = (uint64_t*)p;     p += a256(n * 8);
@@ -68,7 +73,8 @@ AggWs carve_agg_ws(uint8_t* d_aws, uint64_t n, uint32_t n_aggs, uint32_t n_wide)
   a.nulls = (uint32_t*)p;    p += a256(n * 4);
   a.vals = (uint64_t*)p;     p += a256(n * n_aggs * 8);
   a.vhi = (uint64_t*)p;      p += a256(n * n_wide * 8);
-  a.spec = (AggSpec*)p;
+  a.spec = (AggSpec*)p;      p += a256(sizeof(AggSpec));
+  a.vmom = n_var ? (uint64_t*)p : nullptr;
   return a;
 }
 
@@ -79,18 +85,16 @@ __device__ __forceinline__ bool bit_set(const uint8_t* row, int32_t field) {
 }
 
 // Dec (a spec with an out-of-line decimal): such an aggregate's value is staged as (vals, vhi) = its (lo, hi), 0 when
-// null, and a record whose value or 16-byte region is bad lowers *bad to its arena offset << 2 | kAggBad*
-template <bool Dec>
-__global__ void __launch_bounds__(kAggThreads) agg_heads_kernel(const uint8_t* __restrict__ arena,
-                                                                const uint64_t* __restrict__ rec_off,
-                                                                const uint32_t* __restrict__ rec_len,
-                                                                const uint32_t* __restrict__ idx, uint64_t n,
-                                                                const uint32_t* __restrict__ words, uint32_t W,
-                                                                const uint32_t* __restrict__ heads,
-                                                                const AggSpec* __restrict__ spec,
-                                                                uint64_t* __restrict__ head, uint32_t* __restrict__ nulls,
-                                                                uint64_t* __restrict__ vals, uint64_t* __restrict__ vhi,
-                                                                unsigned long long* __restrict__ bad) {
+// null, and a record whose value or 16-byte region is bad lowers *bad to its arena offset << 2 | kAggBad*.  Var (a spec
+// with a variance entry): its avg and m2 words (slots off + 8, off + 16) into vmom.
+template <bool Dec, bool Var>
+__device__ __forceinline__ void agg_heads(const uint8_t* __restrict__ arena, const uint64_t* __restrict__ rec_off,
+                                          const uint32_t* __restrict__ rec_len, const uint32_t* __restrict__ idx,
+                                          uint64_t n, const uint32_t* __restrict__ words, uint32_t W,
+                                          const uint32_t* __restrict__ heads, const AggSpec* __restrict__ spec,
+                                          uint64_t* __restrict__ head, uint32_t* __restrict__ nulls,
+                                          uint64_t* __restrict__ vals, uint64_t* __restrict__ vhi,
+                                          uint64_t* __restrict__ vmom, unsigned long long* __restrict__ bad) {
   const uint32_t n_aggs = spec->n;
   for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (uint64_t)gridDim.x * blockDim.x) {
     const uint32_t i = idx ? idx[j] : (uint32_t)j;
@@ -128,10 +132,41 @@ __global__ void __launch_bounds__(kAggThreads) agg_heads_kernel(const uint8_t* _
         v = lo;
         vhi[(size_t)spec->wide[a] * n + j] = hi;
       }
+      if (Var && spec->op[a] == B2S_AGG_VARIANCE) {
+        uint64_t avg, m2;
+        ld_span16<true>(row + spec->off[a] + 8, 16, avg, m2);
+        vmom[(size_t)(2 * spec->var[a]) * n + j] = avg;
+        vmom[(size_t)(2 * spec->var[a] + 1) * n + j] = m2;
+      }
       vals[(size_t)a * n + j] = v;
     }
     nulls[j] = nm;
   }
+}
+
+template <bool Dec>
+__global__ void __launch_bounds__(kAggThreads) agg_heads_kernel(const uint8_t* __restrict__ arena,
+                                                                const uint64_t* __restrict__ rec_off,
+                                                                const uint32_t* __restrict__ rec_len,
+                                                                const uint32_t* __restrict__ idx, uint64_t n,
+                                                                const uint32_t* __restrict__ words, uint32_t W,
+                                                                const uint32_t* __restrict__ heads,
+                                                                const AggSpec* __restrict__ spec,
+                                                                uint64_t* __restrict__ head, uint32_t* __restrict__ nulls,
+                                                                uint64_t* __restrict__ vals, uint64_t* __restrict__ vhi,
+                                                                unsigned long long* __restrict__ bad) {
+  agg_heads<Dec, false>(arena, rec_off, rec_len, idx, n, words, W, heads, spec, head, nulls, vals, vhi, nullptr, bad);
+}
+
+// agg_heads_kernel for a spec with a variance entry
+template <bool Dec>
+__global__ void __launch_bounds__(kAggThreads) agg_heads_var_kernel(
+    const uint8_t* __restrict__ arena, const uint64_t* __restrict__ rec_off, const uint32_t* __restrict__ rec_len,
+    const uint32_t* __restrict__ idx, uint64_t n, const uint32_t* __restrict__ words, uint32_t W,
+    const uint32_t* __restrict__ heads, const AggSpec* __restrict__ spec, uint64_t* __restrict__ head,
+    uint32_t* __restrict__ nulls, uint64_t* __restrict__ vals, uint64_t* __restrict__ vhi, uint64_t* __restrict__ vmom,
+    unsigned long long* __restrict__ bad) {
+  agg_heads<Dec, true>(arena, rec_off, rec_len, idx, n, words, W, heads, spec, head, nulls, vals, vhi, vmom, bad);
 }
 
 // head holds the exclusive scan of the flags, *groups their total
@@ -582,11 +617,138 @@ __global__ void __launch_bounds__(kAggThreads) agg_merge_large_dec_kernel(
   }
 }
 
+// ---- the variance ----
+// one mergeExpressions step of CentralMomentAgg (order 2): (n1, avg1, m2a) merged with (n2, avg2, m2b), every operation
+// one double operation rounded to nearest, in Spark's order
+__device__ __forceinline__ void var_merge(double& n1, double& avg1, double& m2a, double n2, double avg2, double m2b) {
+  const double newN = __dadd_rn(n1, n2);
+  const double delta = __dsub_rn(avg2, avg1);
+  const double deltaN = newN == 0.0 ? 0.0 : __ddiv_rn(delta, newN);
+  avg1 = __dadd_rn(avg1, __dmul_rn(deltaN, n2));
+  m2a = __dadd_rn(__dadd_rn(m2a, m2b), __dmul_rn(__dmul_rn(__dmul_rn(delta, deltaN), n1), n2));
+  n1 = newN;
+}
+
+__device__ __forceinline__ double dbl(uint64_t b) { return __longlong_as_double((long long)b); }
+__device__ __forceinline__ uint64_t bits(double x) { return (uint64_t)__double_as_longlong(x); }
+
+// variance entry a (v: its index among them) of the records at positions [s, e), by one thread, from (0, 0, 0)
+__device__ __forceinline__ void merge_thread_var(uint32_t a, uint32_t v, const uint64_t* __restrict__ vals,
+                                                 const uint64_t* __restrict__ vmom, uint64_t n, uint32_t s,
+                                                 uint32_t e, double r[3]) {
+  const uint64_t *vn = vals + (size_t)a * n, *va = vmom + (size_t)(2 * v) * n, *vm = va + n;
+  double n1 = 0.0, avg = 0.0, m2 = 0.0;
+  for (uint32_t j = s; j < e; j++) var_merge(n1, avg, m2, dbl(__ldg(vn + j)), dbl(__ldg(va + j)), dbl(__ldg(vm + j)));
+  r[0] = n1;
+  r[1] = avg;
+  r[2] = m2;
+}
+
+// merge_thread_var by the whole warp (every lane returns the result): four rounds of 32 triples loaded in parallel,
+// then each lane's triple broadcast in record order into the one chain
+__device__ __forceinline__ void merge_warp_var(uint32_t a, uint32_t v, const uint64_t* __restrict__ vals,
+                                               const uint64_t* __restrict__ vmom, uint64_t n, uint32_t s, uint32_t e,
+                                               uint32_t lane, double r[3]) {
+  const uint64_t *vn = vals + (size_t)a * n, *va = vmom + (size_t)(2 * v) * n, *vm = va + n;
+  double n1 = 0.0, avg = 0.0, m2 = 0.0;
+  for (uint32_t b = s; b < e; b += 128) {
+    uint64_t x[4][3];
+#pragma unroll
+    for (int q = 0; q < 4; q++) {
+      const uint32_t j = b + 32 * q + lane;
+      const bool in = j < e;
+      x[q][0] = in ? __ldg(vn + j) : 0;
+      x[q][1] = in ? __ldg(va + j) : 0;
+      x[q][2] = in ? __ldg(vm + j) : 0;
+    }
+#pragma unroll
+    for (int q = 0; q < 4; q++) {
+      const uint32_t m = min(32u, e - min(e, b + 32 * q));
+      for (uint32_t l = 0; l < m; l++) {
+        const double n2 = dbl(__shfl_sync(FULL, x[q][0], l)), a2 = dbl(__shfl_sync(FULL, x[q][1], l)),
+                     m2b = dbl(__shfl_sync(FULL, x[q][2], l));
+        var_merge(n1, avg, m2, n2, a2, m2b);
+      }
+    }
+  }
+  r[0] = n1;
+  r[1] = avg;
+  r[2] = m2;
+}
+
+// a variance entry's three slots (never null)
+__device__ __forceinline__ void put_var(uint8_t* row, uint32_t off, const double r[3]) {
+  st_span16(row + off, 16, bits(r[0]), bits(r[1]));
+  st_span16(row + off + 16, 8, bits(r[2]), 0);
+}
+
+// agg_merge_small_kernel for a spec with a variance entry (and any other op)
+__global__ void __launch_bounds__(kAggThreads) agg_merge_small_var_kernel(
+    const uint32_t* __restrict__ gpos, uint64_t G, uint64_t n, const uint64_t* __restrict__ vals,
+    const uint64_t* __restrict__ vhi, const uint64_t* __restrict__ vmom, const uint32_t* __restrict__ nulls,
+    const AggSpec* __restrict__ spec, uint32_t n_aggs, const uint64_t* __restrict__ gdst, uint8_t* __restrict__ dst) {
+  for (uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; g < G; g += (uint64_t)gridDim.x * blockDim.x) {
+    const uint32_t s = gpos[g], e = gpos[g + 1];
+    if (e - s > kSmallGroup) continue;
+    uint8_t* row = dst + gdst[g] + 4;
+    uint32_t null_mask = 0;
+    for (uint32_t a = 0; a < n_aggs; a++) {
+      const uint32_t op = spec->op[a];
+      if (op == B2S_AGG_VARIANCE) {
+        double r[3];
+        merge_thread_var(a, spec->var[a], vals, vmom, n, s, e, r);
+        put_var(row, spec->off[a], r);
+      } else if (agg_decimal_op(op)) {
+        Dec128 x;
+        const bool has = merge_thread_dec(op, a, spec->wide[a], vals, vhi, nulls, n, s, e, &x);
+        put_decimal(row, op, spec->off[a], a, has, x, &null_mask);
+      } else {
+        uint64_t v;
+        const bool has = merge_thread(op, a, vals, nulls, n, s, e, &v);
+        put(row, op, spec->off[a], a, has, v, &null_mask);
+      }
+    }
+    put_null_bits(row, spec, n_aggs, null_mask);
+  }
+}
+
+// agg_merge_large_kernel for a spec with a variance entry (and any other op)
+__global__ void __launch_bounds__(kAggThreads) agg_merge_large_var_kernel(
+    const uint32_t* __restrict__ gpos, uint64_t G, uint64_t n, const uint64_t* __restrict__ vals,
+    const uint64_t* __restrict__ vhi, const uint64_t* __restrict__ vmom, const uint32_t* __restrict__ nulls,
+    const AggSpec* __restrict__ spec, uint32_t n_aggs, const uint64_t* __restrict__ gdst, uint8_t* __restrict__ dst) {
+  const uint32_t lane = threadIdx.x & 31;
+  const uint64_t warps = (uint64_t)gridDim.x * (kAggThreads / 32);
+  for (uint64_t g = (uint64_t)blockIdx.x * (kAggThreads / 32) + (threadIdx.x >> 5); g < G; g += warps) {
+    const uint32_t s = gpos[g], e = gpos[g + 1];
+    if (e - s <= kSmallGroup) continue;  // uniform over the warp
+    uint8_t* row = dst + gdst[g] + 4;
+    uint32_t null_mask = 0;
+    for (uint32_t a = 0; a < n_aggs; a++) {
+      const uint32_t op = spec->op[a];
+      if (op == B2S_AGG_VARIANCE) {
+        double r[3];
+        merge_warp_var(a, spec->var[a], vals, vmom, n, s, e, lane, r);
+        if (lane == 0) put_var(row, spec->off[a], r);
+      } else if (agg_decimal_op(op)) {
+        Dec128 x;
+        const bool has = merge_warp_dec(op, a, spec->wide[a], vals, vhi, nulls, n, s, e, lane, &x);
+        if (lane == 0) put_decimal(row, op, spec->off[a], a, has, x, &null_mask);
+      } else {
+        uint64_t v;
+        const bool has = merge_warp(op, a, vals, nulls, n, s, e, lane, &v);
+        if (lane == 0) put(row, op, spec->off[a], a, has, v, &null_mask);
+      }
+    }
+    if (lane == 0) put_null_bits(row, spec, n_aggs, null_mask);
+  }
+}
+
 }  // namespace
 
-size_t rows_aggregate_ws_bytes(uint64_t n, uint32_t n_aggs, uint32_t n_wide) {
+size_t rows_aggregate_ws_bytes(uint64_t n, uint32_t n_aggs, uint32_t n_wide, uint32_t n_var) {
   return a256(n * 8) + a256(24) + 3 * a256(n * 4) + a256((n + 1) * 4) + a256(n * n_aggs * 8) + a256(n * n_wide * 8) +
-         a256(sizeof(AggSpec));
+         a256(sizeof(AggSpec)) + a256(n * n_var * 16);
 }
 
 uint64_t* rows_aggregate_readback(uint8_t* d_aws, uint64_t n, uint32_t n_aggs, uint32_t n_wide) {
@@ -599,7 +761,7 @@ const uint32_t* rows_group_starts(uint8_t* d_aws, uint64_t n) { return carve_agg
 void launch_rows_group(const uint8_t* arena, uint64_t n, const uint32_t* idx, const uint32_t* heads,
                        uint32_t key_bytes, const AggSpec& spec, uint8_t* d_ws, uint8_t* d_aws, cudaStream_t st,
                        uint64_t* launches) {
-  const AggWs a = carve_agg_ws(d_aws, n, spec.n, spec.n_wide);
+  const AggWs a = carve_agg_ws(d_aws, n, spec.n, spec.n_wide, spec.n_var);
   if (!n) {
     cudaMemsetAsync(a.readback, 0, 16, st);
     return;
@@ -607,7 +769,13 @@ void launch_rows_group(const uint8_t* arena, uint64_t n, const uint32_t* idx, co
   const KeySortWs w = carve_key_sort_ws(d_ws, n, key_bytes);
   uint64_t* scan_ws = (uint64_t*)(d_ws + key_sort_ws_bytes(n, key_bytes));
   cudaMemcpyAsync(a.spec, &spec, sizeof(AggSpec), cudaMemcpyHostToDevice, st);
-  if (spec.n_wide) {
+  if (spec.n_var) {
+    if (spec.n_wide) cudaMemsetAsync(a.readback + 2, 0xff, 8, st);
+    auto heads_var = spec.n_wide ? agg_heads_var_kernel<true> : agg_heads_var_kernel<false>;
+    heads_var<<<grid_for(n), kAggThreads, 0, st>>>(arena, w.src_off, w.len, idx, n, w.words, (key_bytes + 3) / 4, heads,
+                                                   a.spec, a.head, a.nulls, a.vals, a.vhi, a.vmom,
+                                                   (unsigned long long*)(a.readback + 2));
+  } else if (spec.n_wide) {
     cudaMemsetAsync(a.readback + 2, 0xff, 8, st);
     agg_heads_kernel<true><<<grid_for(n), kAggThreads, 0, st>>>(
         arena, w.src_off, w.len, idx, n, w.words, (key_bytes + 3) / 4, heads, a.spec, a.head, a.nulls, a.vals, a.vhi,
@@ -629,7 +797,7 @@ void launch_rows_aggregate(const uint8_t* arena, uint64_t n, uint64_t groups, ui
   if (!groups) return;
   const uint32_t n_aggs = spec.n;
   const KeySortWs w = carve_key_sort_ws(d_ws, n, key_bytes);
-  const AggWs a = carve_agg_ws(d_aws, n, n_aggs, spec.n_wide);
+  const AggWs a = carve_agg_ws(d_aws, n, n_aggs, spec.n_wide, spec.n_var);
   PartitionPlan plan;
   plan.src_off = w.src_off;
   plan.sdst = w.sdst;
@@ -638,7 +806,12 @@ void launch_rows_aggregate(const uint8_t* arena, uint64_t n, uint64_t groups, ui
   if (!n_aggs) return;
   const uint64_t ctas = (groups + kAggThreads / 32 - 1) / (kAggThreads / 32);
   const unsigned large_grid = (unsigned)std::min<uint64_t>(ctas, (uint64_t)kSMs * 16);
-  if (spec.decimal) {
+  if (spec.n_var) {
+    agg_merge_small_var_kernel<<<grid_for(groups), kAggThreads, 0, st>>>(a.gpos, groups, n, a.vals, a.vhi, a.vmom,
+                                                                          a.nulls, a.spec, n_aggs, w.sdst, d_dst);
+    agg_merge_large_var_kernel<<<large_grid, kAggThreads, 0, st>>>(a.gpos, groups, n, a.vals, a.vhi, a.vmom, a.nulls,
+                                                                   a.spec, n_aggs, w.sdst, d_dst);
+  } else if (spec.decimal) {
     agg_merge_small_dec_kernel<<<grid_for(groups), kAggThreads, 0, st>>>(a.gpos, groups, n, a.vals, a.vhi, a.nulls,
                                                                           a.spec, n_aggs, w.sdst, d_dst);
     agg_merge_large_dec_kernel<<<large_grid, kAggThreads, 0, st>>>(a.gpos, groups, n, a.vals, a.vhi, a.nulls, a.spec,

@@ -2623,6 +2623,8 @@ static RecordSpec keys_spec(uint32_t n_keys, const uint32_t* type, const uint32_
 }
 
 static bool overlaps(uint64_t a0, uint64_t a1, uint64_t b0, uint64_t b1) { return a0 < b1 && b0 < a1; }
+// the bytes an aggregate's slots take from agg_off: a variance entry's three doubles, every other op's one slot
+static uint64_t agg_width(uint32_t op) { return agg_base_op(op) == B2S_AGG_VARIANCE ? 24 : 8; }
 // the row offset of field f's 8-byte null word
 static uint64_t null_word(int32_t f) { return 8ull * (uint32_t)(f >> 6); }
 
@@ -2640,7 +2642,8 @@ static RecordSpec aggregate_spec(uint32_t key_type, uint32_t key_off, uint32_t k
   return with_aggregates(rows_spec(key_type, key_off, key_len, null_field), n_aggs, op, off, agg_null);
 }
 
-// each aggregate is a known op on 8 bytes that touch no other slot, a key column, or a null word in use
+// each aggregate is a known op on 8 bytes (a variance entry: 24) that touch no other slot, a key column, or a null word
+// in use
 static int agg_args(const RecordSpec& spec) {
   const uint32_t n = spec.n_aggs;
   const KeySpec& ks = spec.keys;
@@ -2651,7 +2654,7 @@ static int agg_args(const RecordSpec& spec) {
     if (ks.null_field[c] >= 0) words.push_back({null_word(ks.null_field[c]), null_word(ks.null_field[c]) + 8});
   for (uint32_t k = 0; k < n; k++) {
     const uint32_t op = spec.agg_op[k], base = agg_base_op(op), precision = agg_precision(op);
-    if ((op >> 16) || (base > B2S_AGG_MAX_FLOAT64 && base < B2S_AGG_SUM_DECIMAL) || base > B2S_AGG_MAX_DECIMAL)
+    if ((op >> 16) || (base > B2S_AGG_MAX_FLOAT64 && base < B2S_AGG_SUM_DECIMAL) || base > B2S_AGG_VARIANCE)
       return fail(B2S_E_ARG, "unknown aggregate op%s");
     if (base != B2S_AGG_SUM_DECIMAL && precision)
       return fail(B2S_E_ARG, "only B2S_AGG_SUM_DECIMAL takes a precision%s");
@@ -2661,15 +2664,17 @@ static int agg_args(const RecordSpec& spec) {
     if (f < -1) return fail(B2S_E_ARG, "agg_null_field must be -1 or a field ordinal%s");
     if (base == B2S_AGG_SUM_DECIMAL && f < 0)
       return fail(B2S_E_ARG, "B2S_AGG_SUM_DECIMAL needs an agg_null_field: its result can be null%s");
+    if (base == B2S_AGG_VARIANCE && f >= 0)
+      return fail(B2S_E_ARG, "B2S_AGG_VARIANCE takes agg_null_field -1: its buffers are never null%s");
     if (f >= 0) words.push_back({null_word(f), null_word(f) + 8});
   }
   for (uint32_t k = 0; k < n; k++) {
-    const uint64_t s0 = spec.agg_off[k], s1 = s0 + 8;
+    const uint64_t s0 = spec.agg_off[k], s1 = s0 + agg_width(spec.agg_op[k]);
     for (uint32_t c = 0; c < ks.n; c++)
       if (overlaps(s0, s1, ks.off[c], (uint64_t)ks.off[c] + ks.len[c]))
         return fail(B2S_E_ARG, "an aggregate slot overlaps the key%s");
     for (uint32_t m = 0; m < k; m++)
-      if (overlaps(s0, s1, spec.agg_off[m], (uint64_t)spec.agg_off[m] + 8))
+      if (overlaps(s0, s1, spec.agg_off[m], (uint64_t)spec.agg_off[m] + agg_width(spec.agg_op[m])))
         return fail(B2S_E_ARG, "aggregate slots overlap%s");
     for (const auto& w : words)
       if (overlaps(s0, s1, w.first, w.second)) return fail(B2S_E_ARG, "an aggregate slot overlaps a null word%s");
@@ -2678,7 +2683,8 @@ static int agg_args(const RecordSpec& spec) {
 }
 
 // The device form of the aggregates: ops, slots and null bits; the index of every out-of-line decimal among them; where
-// their 16-byte regions may start (past every key and aggregate slot and every null word the call uses).
+// their 16-byte regions may start (past every key and aggregate slot and every null word the call uses); the index of
+// every variance entry among them.
 static AggSpec agg_spec(const RecordSpec& spec) {
   AggSpec agg;
   agg.n = spec.n_aggs;
@@ -2694,8 +2700,9 @@ static AggSpec agg_spec(const RecordSpec& spec) {
     agg.off[k] = spec.agg_off[k];
     agg.null_field[k] = spec.agg_null_field[k];
     if (agg_decimal_wide(op)) agg.wide[k] = agg.n_wide++;
-    agg.decimal |= agg_base_op(op) >= B2S_AGG_SUM_DECIMAL;
-    from = std::max<uint64_t>(from, (uint64_t)spec.agg_off[k] + 8);
+    if (op == B2S_AGG_VARIANCE) agg.var[k] = agg.n_var++;
+    agg.decimal |= agg_decimal_op(op);
+    from = std::max<uint64_t>(from, (uint64_t)spec.agg_off[k] + agg_width(op));
     if (spec.agg_null_field[k] >= 0) from = std::max<uint64_t>(from, null_word(spec.agg_null_field[k]) + 8);
   }
   agg.region_from = (uint32_t)std::min<uint64_t>(from, 0xffffffffull);
@@ -2706,7 +2713,7 @@ static AggSpec agg_spec(const RecordSpec& spec) {
 static uint64_t agg_min_row(const RecordSpec& spec) {
   uint64_t m = 0;
   for (uint32_t k = 0; k < spec.n_aggs; k++) {
-    m = std::max<uint64_t>(m, (uint64_t)spec.agg_off[k] + 8);
+    m = std::max<uint64_t>(m, (uint64_t)spec.agg_off[k] + agg_width(spec.agg_op[k]));
     if (spec.agg_null_field[k] >= 0) m = std::max<uint64_t>(m, null_word(spec.agg_null_field[k]) + 8);
   }
   return m;
@@ -3095,7 +3102,8 @@ int b2s_partition_compress_rows_hash_dev(uint32_t dev_index, uint32_t codec, int
 // then the hash call's partition + compress step over the partial rows
 // ------------------------------------------------------------------------------------------------------------
 // The buffers of the n_aggs functions (each function's in Spark's aggBufferAttributes order) as the device folds them,
-// checked before the device: the function, its input type, the buffer count, the value slot and null bit.
+// checked before the device: the function, its input type, the buffer count, the value slot and null bit.  A variance
+// is one buffer (one merge entry) of three partial-row fields.
 static int partial_agg_args(uint32_t n_aggs, const uint32_t* fn, const uint32_t* val_type, const uint32_t* val_off,
                             const int32_t* val_null, PartialAggSpec* out) {
   PartialAggSpec& s = *out;
@@ -3110,13 +3118,16 @@ static int partial_agg_args(uint32_t n_aggs, const uint32_t* fn, const uint32_t*
     s.vtype[k] = vt;
     s.voff[k] = off;
     s.vnull[k] = nf;
-    if (agg_base_op(op) >= B2S_AGG_SUM_DECIMAL) s.wide[k] = s.n_dec++;
+    if (agg_decimal_op(op)) s.wide[k] = s.n_dec++;
+    if (op == B2S_AGG_VARIANCE) s.var[k] = s.n_var++;
+    s.n_fields += op == B2S_AGG_VARIANCE ? 3 : 1;
     s.dsum |= op == B2S_AGG_SUM_FLOAT64;
     return true;
   };
   for (uint32_t a = 0; a < n_aggs; a++) {
     const uint32_t f = fn[a], vt = val_type[a], kind = vt & 0xff, p = (vt >> 8) & 0xff, sc = vt >> 16;
-    if (f < B2S_WINDOW_SUM || f > B2S_WINDOW_AVG) return fail(B2S_E_ARG, "unknown aggregate function%s");
+    if ((f < B2S_WINDOW_SUM || f > B2S_WINDOW_AVG) && f != B2S_WINDOW_VARIANCE)
+      return fail(B2S_E_ARG, "unknown aggregate function%s");
     if (kind > B2S_WINDOW_VAL_BYTES || (kind != B2S_WINDOW_VAL_DECIMAL && (vt >> 8)) || (vt >> 24))
       return fail(B2S_E_ARG, "unknown val_type%s");
     if (kind == B2S_WINDOW_VAL_DECIMAL && (p < 1 || p > 38 || sc > p))
@@ -3155,6 +3166,12 @@ static int partial_agg_args(uint32_t n_aggs, const uint32_t* fn, const uint32_t*
           ok = add(B2S_AGG_SUM_FLOAT64, kStageZero, vt, off, nf, true);
         }
         ok = ok && add(B2S_AGG_SUM_INT64, kStageCount, vt, off, nf, false);
+        break;
+      case B2S_WINDOW_VARIANCE:  // [n, avg, m2] over Cast(child, DoubleType)
+        if (dec)
+          return fail(B2S_E_ARG, "VARIANCE takes an int8 .. int64, float or double input (a decimal's cast to double "
+                                 "is Decimal.toDouble)%s");
+        ok = add(B2S_AGG_VARIANCE, kStageValue, vt, off, nf, true);
         break;
       default: {  // MIN, MAX
         const bool mx = f == B2S_WINDOW_MAX;
@@ -3320,7 +3337,7 @@ struct GroupingSets {
 };
 
 // The grouping sets' rules, before the device: gid takes the 16th key column; every mask names key columns only, once
-// (n_keys + 1 + buffers <= 15 + 1 + 16 = 32 partial-row fields follows: one null word, as the partial rows need)
+// (aggregate_partition_call checks that n_keys + 1 + the buffers' fields stay within one null word's 32)
 static int grouping_sets_args(uint32_t n_keys, uint64_t n, const GroupingSets& g) {
   if (n_keys < 1 || n_keys >= kMaxKeys)
     return fail(B2S_E_ARG, "n_keys must be in [1, 15] with grouping sets (gid is the 16th key column)%s");
@@ -3476,6 +3493,9 @@ static int aggregate_partition_call(bool packed, uint32_t dev_index, uint32_t co
   spec.keys = rspec.keys;
   if (!n_groups) return fail(B2S_E_ARG, "null argument%s");
   if (int rc = partial_agg_args(n_aggs, agg_fn, val_type, val_off, val_null_field, &spec)) return rc;
+  if (spec.keys.n + (gs ? 1 : 0) + spec.n_fields > 32)
+    return fail(B2S_E_ARG, gs ? "n_keys + 1 + the buffers' fields (3 per VARIANCE) must be at most 32 (one null word)%s"
+                              : "n_keys + the buffers' fields (3 per VARIANCE) must be at most 32 (one null word)%s");
   if (gs)
     if (int rc = grouping_sets_args(n_keys, n_records, *gs)) return rc;
   if (int rc = hash_args(codec, codec_block_size, checksum_alg, num_partitions, n_records, rec_base, rec_bytes, rec_len,
@@ -4289,8 +4309,9 @@ static int order_rows(Slot& S, const RecordSpec& spec, DecodedTask& T, const Joi
   const KeySpec& encoded = jk ? jk->side[0] : ks;
   R.key_bytes = rows_key_bytes(encoded);
   const bool refine = rows_key_refines(encoded);
+  const AggSpec agg = spec.aggregate ? agg_spec(spec) : AggSpec{};
   const size_t part[6] = {rows_sort_ws_bytes(records, R.key_bytes),
-                          spec.aggregate ? rows_aggregate_ws_bytes(records, spec.n_aggs, agg_spec(spec).n_wide) : 0,
+                          spec.aggregate ? rows_aggregate_ws_bytes(records, spec.n_aggs, agg.n_wide, agg.n_var) : 0,
                           refine ? rows_refine_ws_bytes(records, n_src) : 0,
                           jk || win ? rows_aggregate_ws_bytes(records, 0, 0) : 0,
                           jk ? join_ws_bytes(records, n_src, n_join_fields) : 0,

@@ -449,9 +449,17 @@ struct AggSpec {
   uint32_t n_wide = 0;
   uint32_t region_from = 0;
   bool decimal = false;  // some op is a Decimal op: the merge runs the kernels that know them
+  // B2S_AGG_VARIANCE entries: n staged as the other slots, avg and m2 as words 2 var[a] and 2 var[a] + 1 of 2 n_var;
+  // with one, the merge runs the kernels that know them (which know the Decimal ops too)
+  uint32_t var[kMaxAggs] = {};
+  uint32_t n_var = 0;
 };
 __host__ __device__ inline uint32_t agg_base_op(uint32_t op) { return op & 0xff; }
 __host__ __device__ inline uint32_t agg_precision(uint32_t op) { return (op >> 8) & 0xff; }
+// a Decimal op (SUM / MIN / MAX_DECIMAL): its value is staged in 128 bits
+__host__ __device__ inline bool agg_decimal_op(uint32_t op) {
+  return agg_base_op(op) >= B2S_AGG_SUM_DECIMAL && agg_base_op(op) <= B2S_AGG_MAX_DECIMAL;
+}
 // the op's value is out of line: 16 bytes at (offset << 32) | size
 __host__ __device__ inline bool agg_decimal_wide(uint32_t op) {
   const uint32_t b = agg_base_op(op);
@@ -460,8 +468,8 @@ __host__ __device__ inline bool agg_decimal_wide(uint32_t op) {
 // the verdict of the decimal region checks (rows_aggregate_readback's third word): ~0, or the lowest bad record's arena
 // offset << 2 | one of these
 constexpr uint64_t kAggBadDecimal = 1, kAggBadRegionEnd = 2, kAggBadRegionStart = 3;
-// d_aws: rows_aggregate_ws_bytes(n, n_aggs, n_wide), beside the sort workspace d_ws of the same n records
-size_t rows_aggregate_ws_bytes(uint64_t n, uint32_t n_aggs, uint32_t n_wide);
+// d_aws: rows_aggregate_ws_bytes(n, n_aggs, n_wide, n_var), beside the sort workspace d_ws of the same n records
+size_t rows_aggregate_ws_bytes(uint64_t n, uint32_t n_aggs, uint32_t n_wide, uint32_t n_var = 0);
 // after launch_rows_group: [group count, output bytes, decimal verdict (only with an out-of-line decimal)] (device)
 uint64_t* rows_aggregate_readback(uint8_t* d_aws, uint64_t n, uint32_t n_aggs, uint32_t n_wide);
 // the groups of the records in the order idx (launch_rows_order): heads, group starts, the heads' output offsets and
@@ -487,7 +495,9 @@ const uint32_t* rows_group_starts(uint8_t* d_aws, uint64_t n);
 // bits 8..15; slot voff[k], null bit vnull[k] or -1) by stage[k]: kStageValue the value (a null is skipped),
 // kStageZero the value or 0 when null (to_double[k]: an integer cast to double, rounded to nearest), kStageCount 1 per
 // non-null input (every input for VAL_NONE), kStageIsEmpty 1 per null input.  A decimal buffer (op >= SUM_DECIMAL) is
-// staged in 128 bits: wide[k] is its index among the n_dec of them.  dsum: some buffer is a double sum.
+// staged in 128 bits: wide[k] is its index among the n_dec of them.  dsum: some buffer is a double sum.  A variance
+// buffer (op B2S_AGG_VARIANCE, kStageValue with to_double: the input cast to double, a null skipped) folds into three
+// fields (n, avg, m2); var[k] is its index among the n_var of them.  n_fields: the partial row's buffer fields.
 constexpr uint32_t kStageValue = 0, kStageZero = 1, kStageCount = 2, kStageIsEmpty = 3;
 struct PartialAggSpec {
   KeySpec keys;
@@ -501,6 +511,9 @@ struct PartialAggSpec {
   uint32_t wide[kMaxAggs] = {};
   uint32_t n_dec = 0;
   bool dsum = false;
+  uint32_t var[kMaxAggs] = {};
+  uint32_t n_var = 0;
+  uint32_t n_fields = 0;
 };
 // the check verdict (header word 0) of a record whose value is bad: (i << 3) | kPaBadValue, beside launch_rows_hash's
 // kHashBad* reasons; header word 2 then holds (i << 2) | kPaBadSlot, kPaBadNull or kPaBadDecimal

@@ -15,10 +15,13 @@
 //             a partial, and a warp per large group combines its chunks' partials.  Sums of integers and decimals are
 //             exact and so in any order; min / max keep the earliest position among equal values, so they too.  A
 //             double sum is one add chain per group in position order: a warp stages 256 values in shared memory and
-//             its lane 0 adds them, the next tile's loads in flight meanwhile.
+//             its lane 0 adds them, the next tile's loads in flight meanwhile.  A variance (CentralMomentAgg's
+//             [n, avg, m2]) is one update chain per group in position order the same way; it is not associative, so
+//             the warp, chunk and combine folds skip it, as they skip the double sums.
 //   size    : a thread per group: its partial row's length, scanned into the output offsets (the last scan total is the
 //             output bytes, read back with the group count)
-//   emit    : a warp per partial row, lane f writing field f (n_keys + buffers <= 32, so one null word)
+//   emit    : a warp per partial row, lane f writing field f (n_keys + fields <= 32, so one null word; a variance
+//             buffer is three fields)
 #include <algorithm>
 
 #include "decimal128.h"
@@ -54,8 +57,8 @@ struct PAcc {
 };
 
 // the workspace (partial_agg_ws_bytes): header [check verdict, record bytes, check detail, range 0 (= 0), groups,
-// output bytes], staged values, decimal high words, null bits, the folded buffers (per group), the chunk partials, the
-// partial rows' lengths and offsets and the offsets' scan workspace
+// output bytes], staged values, decimal high words, null bits, the folded buffers (per group; a variance's avg and m2
+// in rmom), the chunk partials, the partial rows' lengths and offsets and the offsets' scan workspace
 struct PaWs {
   uint64_t* hdr;
   uint64_t* vals;
@@ -64,6 +67,7 @@ struct PaWs {
   uint64_t* rlo;
   uint64_t* rhi;
   uint32_t* rnull;
+  uint64_t* rmom;
   PAcc* part;
   uint32_t* rowlen;
   uint64_t* rowoff;
@@ -82,6 +86,7 @@ PaWs carve_pa_ws(uint8_t* d, uint64_t n, const PartialAggSpec& s) {
   w.rlo = (uint64_t*)p;    p += a256(n * s.n_bufs * 8);
   w.rhi = (uint64_t*)p;    p += a256(n * s.n_dec * 8);
   w.rnull = (uint32_t*)p;  p += a256(n * 4);
+  w.rmom = (uint64_t*)p;   p += a256(n * s.n_var * 16);
   w.part = (PAcc*)p;       p += a256(n_chunks(n) * 2 * s.n_bufs * sizeof(PAcc));
   w.rowlen = (uint32_t*)p; p += a256(n * 4);
   w.rowoff = (uint64_t*)p; p += a256(n * 8);
@@ -218,7 +223,7 @@ __global__ void __launch_bounds__(kPaThreads) pa_stage_kernel(const uint8_t* __r
       uint64_t lo, hi;
       if (stage_one(row, size, s, k, lo, hi)) nm |= 1u << k;
       vals[(size_t)k * n + j] = lo;
-      if (agg_base_op(s.op[k]) >= B2S_AGG_SUM_DECIMAL) vhi[(size_t)s.wide[k] * n + j] = hi;
+      if (agg_decimal_op(s.op[k])) vhi[(size_t)s.wide[k] * n + j] = hi;
     }
     nulls[j] = nm;
   }
@@ -281,7 +286,7 @@ __device__ __forceinline__ PAcc load_acc(const PartialAggSpec& s, uint32_t k, co
   PAcc x;
   x.has = !((__ldg(nulls + j) >> k) & 1);
   x.lo = x.has ? __ldg(vals + (size_t)k * n + j) : 0;
-  x.hi = x.has && agg_base_op(s.op[k]) >= B2S_AGG_SUM_DECIMAL ? __ldg(vhi + (size_t)s.wide[k] * n + j) : 0;
+  x.hi = x.has && agg_decimal_op(s.op[k]) ? __ldg(vhi + (size_t)s.wide[k] * n + j) : 0;
   x.pos = j;
   return x;
 }
@@ -321,11 +326,36 @@ __device__ __forceinline__ PAcc fold_warp(const PartialAggSpec& s, uint32_t k, c
 }
 
 __device__ __forceinline__ bool dsum_op(uint32_t op) { return op == B2S_AGG_SUM_FLOAT64; }
+// a buffer folded by one chain in position order (pa_chain_kernel's), not by the associative folds
+__device__ __forceinline__ bool chain_op(uint32_t op) { return op == B2S_AGG_SUM_FLOAT64 || op == B2S_AGG_VARIANCE; }
+
+__device__ __forceinline__ double dbl(uint64_t b) { return __longlong_as_double((long long)b); }
+__device__ __forceinline__ uint64_t bits(double x) { return (uint64_t)__double_as_longlong(x); }
+
+// one updateExpressions step of CentralMomentAgg (order 2) with the non-null input x, every operation one double
+// operation rounded to nearest, in Spark's order
+__device__ __forceinline__ void var_update(double& cn, double& avg, double& m2, double x) {
+  const double newN = __dadd_rn(cn, 1.0);
+  const double delta = __dsub_rn(x, avg);
+  const double deltaN = __ddiv_rn(delta, newN);
+  avg = __dadd_rn(avg, deltaN);
+  m2 = __dadd_rn(m2, __dmul_rn(delta, __dsub_rn(delta, deltaN)));
+  cn = newN;
+}
+
+// a variance buffer's fold of group g: n into rlo, avg and m2 into rmom
+__device__ __forceinline__ void put_var(const PartialAggSpec& s, uint32_t k, uint64_t g, uint64_t n, double cn,
+                                        double avg, double m2, uint64_t* __restrict__ rlo,
+                                        uint64_t* __restrict__ rmom) {
+  rlo[(size_t)k * n + g] = bits(cn);
+  rmom[(size_t)(2 * s.var[k]) * n + g] = bits(avg);
+  rmom[(size_t)(2 * s.var[k] + 1) * n + g] = bits(m2);
+}
 
 __device__ __forceinline__ void put_result(const PartialAggSpec& s, uint32_t k, uint64_t g, uint64_t n, PAcc r,
                                            uint64_t* __restrict__ rlo, uint64_t* __restrict__ rhi) {
   rlo[(size_t)k * n + g] = r.lo;
-  if (agg_base_op(s.op[k]) >= B2S_AGG_SUM_DECIMAL) rhi[(size_t)s.wide[k] * n + g] = r.hi;
+  if (agg_decimal_op(s.op[k])) rhi[(size_t)s.wide[k] * n + g] = r.hi;
 }
 
 // the group of sorted position j, from the heads-before scan of launch_rows_group
@@ -333,7 +363,7 @@ __device__ __forceinline__ uint64_t group_of(const uint64_t* __restrict__ hb, ui
   return (j + 1 < n ? hb[j + 1] : G) - 1;
 }
 
-// groups of up to kSmallGroup records: a thread each, every buffer in position order (the double sums included)
+// groups of up to kSmallGroup records: a thread each, every buffer in position order (the chains included)
 __global__ void __launch_bounds__(kPaThreads) pa_fold_small_kernel(const uint32_t* __restrict__ gpos,
                                                                    const uint64_t* __restrict__ groups, uint64_t n,
                                                                    const __grid_constant__ PartialAggSpec s,
@@ -341,7 +371,8 @@ __global__ void __launch_bounds__(kPaThreads) pa_fold_small_kernel(const uint32_
                                                                    const uint64_t* __restrict__ vhi,
                                                                    const uint32_t* __restrict__ nulls,
                                                                    uint64_t* __restrict__ rlo, uint64_t* __restrict__ rhi,
-                                                                   uint32_t* __restrict__ rnull) {
+                                                                   uint32_t* __restrict__ rnull,
+                                                                   uint64_t* __restrict__ rmom) {
   const uint64_t G = *groups;
   for (uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; g < G; g += (uint64_t)gridDim.x * blockDim.x) {
     const uint32_t s0 = gpos[g], e0 = gpos[g + 1];
@@ -350,6 +381,13 @@ __global__ void __launch_bounds__(kPaThreads) pa_fold_small_kernel(const uint32_
     for (uint32_t k = 0; k < s.n_bufs; k++) {
       const uint32_t op = s.op[k];
       PAcc acc{0, 0, 0, 0};
+      if (op == B2S_AGG_VARIANCE) {  // never null
+        double cn = 0.0, avg = 0.0, m2 = 0.0;
+        for (uint32_t j = s0; j < e0; j++)
+          if (!((__ldg(nulls + j) >> k) & 1)) var_update(cn, avg, m2, dbl(__ldg(vals + (size_t)k * n + j)));
+        put_var(s, k, g, n, cn, avg, m2, rlo, rmom);
+        continue;
+      }
       if (dsum_op(op)) {
         double fs = 0.0;
         for (uint32_t j = s0; j < e0; j++) {
@@ -367,7 +405,7 @@ __global__ void __launch_bounds__(kPaThreads) pa_fold_small_kernel(const uint32_
   }
 }
 
-// groups of kSmallGroup + 1 .. kChunk records: a warp each (not the double sums: pa_dsum_kernel)
+// groups of kSmallGroup + 1 .. kChunk records: a warp each (not the chains: pa_chain_kernel)
 __global__ void __launch_bounds__(kPaThreads) pa_fold_warp_kernel(const uint32_t* __restrict__ gpos,
                                                                   const uint64_t* __restrict__ groups, uint64_t n,
                                                                   const __grid_constant__ PartialAggSpec s,
@@ -383,12 +421,12 @@ __global__ void __launch_bounds__(kPaThreads) pa_fold_warp_kernel(const uint32_t
     if (e0 - s0 <= kSmallGroup || e0 - s0 > kChunk) continue;  // uniform over the warp
     uint32_t nm = 0;
     for (uint32_t k = 0; k < s.n_bufs; k++) {
-      if (dsum_op(s.op[k])) continue;
+      if (chain_op(s.op[k])) continue;
       const PAcc r = fold_warp(s, k, vals, vhi, nulls, n, s0, e0, lane);
       if (!r.has) nm |= 1u << k;
       if (lane == 0) put_result(s, k, g, n, r, rlo, rhi);
     }
-    if (lane == 0) rnull[g] = nm;  // a double sum's bit: pa_dsum_kernel's atomicOr
+    if (lane == 0) rnull[g] = nm;  // a double sum's bit: pa_chain_kernel's atomicOr
   }
 }
 
@@ -414,7 +452,7 @@ __global__ void __launch_bounds__(kPaThreads) pa_fold_chunk_kernel(const uint32_
       if (e0 - s0 <= kChunk) continue;
       const uint32_t a = (uint32_t)std::max<uint64_t>(s0, p0), b = (uint32_t)std::min<uint64_t>(e0, p1);
       for (uint32_t k = 0; k < s.n_bufs; k++) {
-        if (dsum_op(s.op[k])) continue;
+        if (chain_op(s.op[k])) continue;
         const PAcc r = fold_warp(s, k, vals, vhi, nulls, n, a, b, lane);
         if (lane == 0) part[(c * 2 + slot) * s.n_bufs + k] = r;
       }
@@ -439,7 +477,7 @@ __global__ void __launch_bounds__(kPaThreads) pa_fold_combine_kernel(const uint3
     uint32_t nm = 0;
     for (uint32_t k = 0; k < s.n_bufs; k++) {
       const uint32_t op = s.op[k];
-      if (dsum_op(op)) continue;
+      if (chain_op(op)) continue;
       PAcc acc{0, 0, 0, 0};
       for (uint64_t c = c0 + lane; c <= c1; c += 32) {
         const uint32_t slot = (uint64_t)s0 <= c * kChunk ? 0 : 1;
@@ -453,16 +491,21 @@ __global__ void __launch_bounds__(kPaThreads) pa_fold_combine_kernel(const uint3
   }
 }
 
-// the double sums of the groups over kSmallGroup records: a warp each, one add chain in position order.  The warp loads
-// a tile of kTile values (coalesced) into shared memory and lane 0 adds them; the next tile's loads are issued before
-// the chain, so they are in flight while it runs.  Runs after the other folds, which wrote rnull[g] without these bits.
-__global__ void __launch_bounds__(kPaThreads) pa_dsum_kernel(const uint32_t* __restrict__ gpos,
-                                                             const uint64_t* __restrict__ groups, uint64_t n,
-                                                             const __grid_constant__ PartialAggSpec s,
-                                                             const uint64_t* __restrict__ vals,
-                                                             const uint32_t* __restrict__ nulls,
-                                                             uint64_t* __restrict__ rlo, uint32_t* __restrict__ rnull) {
+// The chains of the groups over kSmallGroup records, a warp each, one chain per buffer in position order: the double
+// sums (Var false: the adds, a null staged as +0.0) or the variances (Var true: var_update over the non-null inputs).
+// The warp loads a tile of kTile values (coalesced) into shared memory, with a variance's null bits, and lane 0 runs
+// the chain over them; the next tile's loads are issued before the chain, so they are in flight while it runs.  Runs
+// after the other folds, which wrote rnull[g] without a double sum's bit (a variance is never null).
+template <bool Var>
+__global__ void __launch_bounds__(kPaThreads) pa_chain_kernel(const uint32_t* __restrict__ gpos,
+                                                              const uint64_t* __restrict__ groups, uint64_t n,
+                                                              const __grid_constant__ PartialAggSpec s,
+                                                              const uint64_t* __restrict__ vals,
+                                                              const uint32_t* __restrict__ nulls,
+                                                              uint64_t* __restrict__ rlo, uint32_t* __restrict__ rnull,
+                                                              uint64_t* __restrict__ rmom) {
   __shared__ double tile[kPaThreads / 32][kTile];
+  __shared__ uint32_t tnull[kPaThreads / 32][Var ? kTile / 32 : 1];
   const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   const uint64_t G = *groups, warps = (uint64_t)gridDim.x * (kPaThreads / 32);
   constexpr uint32_t kPer = kTile / 32;
@@ -471,28 +514,40 @@ __global__ void __launch_bounds__(kPaThreads) pa_dsum_kernel(const uint32_t* __r
     if (e0 - s0 <= kSmallGroup) continue;
     uint32_t nm = 0;
     for (uint32_t k = 0; k < s.n_bufs; k++) {
-      if (!dsum_op(s.op[k])) continue;
+      if (s.op[k] != (Var ? B2S_AGG_VARIANCE : B2S_AGG_SUM_FLOAT64)) continue;
       const uint64_t* va = vals + (size_t)k * n;
       double next[kPer];
+      uint32_t next_null[kPer];
       bool any = false;
       auto load = [&](uint32_t b) {
 #pragma unroll
         for (uint32_t r = 0; r < kPer; r++) {
           const uint32_t j = b + r * 32 + lane;
           next[r] = j < e0 ? __longlong_as_double((long long)__ldg(va + j)) : 0.0;
-          any |= j < e0 && !((__ldg(nulls + j) >> k) & 1);
+          if (Var) {
+            next_null[r] = __ballot_sync(FULL, j < e0 && ((__ldg(nulls + j) >> k) & 1));
+          } else {
+            any |= j < e0 && !((__ldg(nulls + j) >> k) & 1);
+          }
         }
       };
       load(s0);
-      double fs = 0.0;
+      double fs = 0.0, cn = 0.0, avg = 0.0, m2 = 0.0;
       for (uint32_t b = s0; b < e0; b += kTile) {
 #pragma unroll
         for (uint32_t r = 0; r < kPer; r++) tile[wid][r * 32 + lane] = next[r];
+        if (Var && lane == 0) {
+#pragma unroll
+          for (uint32_t r = 0; r < kPer; r++) tnull[wid][r] = next_null[r];
+        }
         __syncwarp();
         if (b + kTile < e0) load(b + kTile);
         if (lane == 0) {
           const uint32_t m = min(kTile, e0 - b);
-          if (m == kTile) {
+          if (Var) {
+            for (uint32_t t = 0; t < m; t++)
+              if (!((tnull[wid][t >> 5] >> (t & 31)) & 1)) var_update(cn, avg, m2, tile[wid][t]);
+          } else if (m == kTile) {
 #pragma unroll 16
             for (uint32_t t = 0; t < kTile; t++) fs = __dadd_rn(fs, tile[wid][t]);
           } else {
@@ -501,8 +556,12 @@ __global__ void __launch_bounds__(kPaThreads) pa_dsum_kernel(const uint32_t* __r
         }
         __syncwarp();
       }
-      if (!__any_sync(FULL, any)) nm |= 1u << k;
-      if (lane == 0) rlo[(size_t)k * n + g] = (uint64_t)__double_as_longlong(fs);
+      if (Var) {
+        if (lane == 0) put_var(s, k, g, n, cn, avg, m2, rlo, rmom);
+      } else {
+        if (!__any_sync(FULL, any)) nm |= 1u << k;
+        if (lane == 0) rlo[(size_t)k * n + g] = (uint64_t)__double_as_longlong(fs);
+      }
     }
     if (lane == 0 && nm) atomicOr(rnull + g, nm);
   }
@@ -537,7 +596,7 @@ __global__ void __launch_bounds__(kPaThreads) pa_size_kernel(const uint8_t* __re
                                                              uint32_t* __restrict__ rowlen,
                                                              uint64_t* __restrict__ rowoff) {
   const uint64_t G = *groups;
-  const uint32_t nf = s.keys.n + s.n_bufs, fixed = 8 * (1 + nf);
+  const uint32_t nf = s.keys.n + s.n_fields, fixed = 8 * (1 + nf);
   for (uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; g < n; g += (uint64_t)gridDim.x * blockDim.x) {
     uint32_t len = 0;
     if (g < G) {
@@ -564,11 +623,12 @@ __global__ void __launch_bounds__(kPaThreads) pa_emit_kernel(const uint8_t* __re
                                                              const uint64_t* __restrict__ rlo,
                                                              const uint64_t* __restrict__ rhi,
                                                              const uint32_t* __restrict__ rnull,
+                                                             const uint64_t* __restrict__ rmom,
                                                              const uint32_t* __restrict__ rowlen,
                                                              const uint64_t* __restrict__ rowoff,
                                                              uint8_t* __restrict__ dst) {
   const uint32_t lane = threadIdx.x & 31;
-  const uint32_t nk = s.keys.n, nf = nk + s.n_bufs, fixed = 8 * (1 + nf);
+  const uint32_t nk = s.keys.n, nf = nk + s.n_fields, fixed = 8 * (1 + nf);
   const uint64_t warps = (uint64_t)gridDim.x * (kPaThreads / 32);
   for (uint64_t g = (uint64_t)blockIdx.x * (kPaThreads / 32) + (threadIdx.x >> 5); g < G; g += warps) {
     const uint32_t j = gpos[g], i = idx ? idx[j] : j;
@@ -613,9 +673,16 @@ __global__ void __launch_bounds__(kPaThreads) pa_emit_kernel(const uint8_t* __re
         dec = true;  // 16 zero bytes, slot offset << 32
       }
     } else if (lane < nf) {
-      const uint32_t k = lane - nk, op = s.op[k];
+      // the lane's buffer k and, for a variance, which of its three fields (n, avg, m2)
+      uint32_t k = 0, part = lane - nk;
+      for (; k + 1 < s.n_bufs; k++) {
+        const uint32_t w = s.op[k] == B2S_AGG_VARIANCE ? 3 : 1;
+        if (part < w) break;
+        part -= w;
+      }
+      const uint32_t op = s.op[k];
       null = (rnull[g] >> k) & 1;
-      const uint64_t lo = rlo[(size_t)k * n + g];
+      const uint64_t lo = part ? rmom[(size_t)(2 * s.var[k] + part - 1) * n + g] : rlo[(size_t)k * n + g];
       if (wide_buffer(op)) {
         var = 16;
         dec = true;
@@ -656,7 +723,7 @@ __global__ void __launch_bounds__(kPaThreads) pa_emit_kernel(const uint8_t* __re
 }  // namespace
 
 size_t partial_agg_ws_bytes(uint64_t n, const PartialAggSpec& s) {
-  return 256 + 2 * a256(n * s.n_bufs * 8) + 2 * a256(n * s.n_dec * 8) + 2 * a256(n * 4) +
+  return 256 + 2 * a256(n * s.n_bufs * 8) + 2 * a256(n * s.n_dec * 8) + 2 * a256(n * 4) + a256(n * s.n_var * 16) +
          a256(n_chunks(n) * 2 * s.n_bufs * sizeof(PAcc)) + a256(n * 4) + a256(n * 8) + a256(scan_ws_elems(n) * 8);
 }
 
@@ -701,7 +768,7 @@ void launch_partial_agg_fold(const uint8_t* rec, uint64_t n, const uint32_t* idx
   if (spec.n_bufs) {
     pa_stage_kernel<<<grid_for(n), kPaThreads, 0, st>>>(rec, w.src_off, w.len, idx, n, spec, a.vals, a.vhi, a.nulls);
     pa_fold_small_kernel<<<grid_for(n), kPaThreads, 0, st>>>(gpos, groups, n, spec, a.vals, a.vhi, a.nulls, a.rlo,
-                                                              a.rhi, a.rnull);
+                                                              a.rhi, a.rnull, a.rmom);
     const unsigned wg = warp_grid_for(n / kSmallGroup + 1);
     pa_fold_warp_kernel<<<wg, kPaThreads, 0, st>>>(gpos, groups, n, spec, a.vals, a.vhi, a.nulls, a.rlo, a.rhi,
                                                    a.rnull);
@@ -714,7 +781,11 @@ void launch_partial_agg_fold(const uint8_t* rec, uint64_t n, const uint32_t* idx
       launched += 2;
     }
     if (spec.dsum) {
-      pa_dsum_kernel<<<wg, kPaThreads, 0, st>>>(gpos, groups, n, spec, a.vals, a.nulls, a.rlo, a.rnull);
+      pa_chain_kernel<false><<<wg, kPaThreads, 0, st>>>(gpos, groups, n, spec, a.vals, a.nulls, a.rlo, a.rnull, a.rmom);
+      launched++;
+    }
+    if (spec.n_var) {
+      pa_chain_kernel<true><<<wg, kPaThreads, 0, st>>>(gpos, groups, n, spec, a.vals, a.nulls, a.rlo, a.rnull, a.rmom);
       launched++;
     }
     if (launches) *launches += launched;
@@ -735,8 +806,8 @@ void launch_partial_agg_emit(const uint8_t* rec, uint64_t n, uint64_t groups, co
   const KeySortWs w = carve_key_sort_ws(d_ws, n, key_bytes);
   const PaWs a = carve_pa_ws(d_paws, n, spec);
   pa_emit_kernel<<<warp_grid_for(groups), kPaThreads, 0, st>>>(rec, w.src_off, w.len, idx, rows_group_starts(d_gws, n),
-                                                              groups, n, spec, a.rlo, a.rhi, a.rnull, a.rowlen,
-                                                              a.rowoff, d_dst);
+                                                              groups, n, spec, a.rlo, a.rhi, a.rnull, a.rmom,
+                                                              a.rowlen, a.rowoff, d_dst);
   if (launches) *launches += 1;
 }
 
