@@ -389,6 +389,81 @@ int b2s_aggregate_grouping_sets_partition_compress_rows_hash_dev(
     uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_off, uint64_t* dst_len, uint64_t* dst_total,
     uint64_t* checksum_out, int32_t* status, uint64_t* n_groups);
 
+/* ---- read + write, one DISTINCT group: Spark's PartialMerge and Partial aggregates between two exchanges on the GPU ----
+ * The middle stage of an aggregate with one DISTINCT group (AggUtils.planAggregateWithOneDistinct, Spark 3.5): on the
+ * reducer of the exchange by G ++ X, HashAggregate(G ++ X, F: PartialMerge) then HashAggregate(G, F: PartialMerge, D:
+ * Partial), then the exchange by G, in one call per reduce task.  G are the grouping columns, X the distinct columns, F
+ * the non-distinct functions and D the distinct ones.  The map side is b2s_aggregate_partition_compress_rows_hash_*
+ * with key columns G ++ X and functions F; the final merge of this call's output is b2s_decompress_aggregate_rows_keys_*
+ * keyed by G with the merge ops of F's and D's buffers.
+ * Read side: codec, checksum_alg, the n fetched blocks (src_off / src_len, slices and checksums) and the per-block
+ * status[n] / bad_slice[n] exactly as b2s_decompress_aggregate_rows_keys_*.
+ * Input rows: the map side's partial rows for key columns G ++ X and functions F: one null word (n_keys + F's fields
+ * <= 32), key column c at slot 8 + 8 c with null bit c, then F's buffer fields in function order (1 per buffer, 3 per
+ * VARIANCE).  n_keys (1..16) key columns, the first n_group_keys (0..15) G and at least one X; key_type[c] / key_len[c]
+ * as the composite-key calls take them, no order flags (a G column of B2S_KEY_BYTES is a 1-byte boolean).  F:
+ * (agg_fn[a], val_type[a]), a < n_aggs, exactly as the map side took them (its rules apply); the call derives every
+ * buffer's slot, merge and initial value from them.
+ * D: (distinct_fn[a], distinct_val_type[a], distinct_column[a]), a < n_distinct (1..16): COUNT, SUM, AVG or VARIANCE
+ * with the map side's val_type rules (decimal SUM p <= 28, AVG p <= 27, VARIANCE not decimal), over distinct column
+ * distinct_column[a] (in [n_group_keys, n_keys)), whose key type must agree with val_type: INT8 .. INT64 with
+ * VAL_INT8 .. VAL_INT64, INT64 also with VAL_DECIMAL p <= 18, FLOAT32 / FLOAT64 with VAL_FLOAT32 / VAL_FLOAT64,
+ * B2S_DECIMAL_KEY with VAL_DECIMAL p > 18, string, binary and boolean with COUNT and VAL_BYTES only.  Or
+ * distinct_column[a] = B2S_DISTINCT_ALL_COLUMNS with COUNT and VAL_NONE: count(DISTINCT every distinct column), which
+ * counts the (G, X) groups in which no distinct column is null (Spark's Count of several children).  One DISTINCT
+ * group means every distinct function's children are all of X, so with several distinct columns only
+ * B2S_DISTINCT_ALL_COLUMNS is accepted (a function over one of them would fold a value once per (G, X) row, not once
+ * per distinct value).  MIN / MAX are B2S_E_ARG: Spark's optimizer removes their DISTINCT.
+ * Semantics (Spark 3.5, ANSI off), in the order this contract fixes (Spark's own is its hash maps' iteration order):
+ *   stage 2: the rows are sorted and grouped by G ++ X, and F's buffers merged per (G, X) group in stable (block)
+ *            order, byte for byte as b2s_decompress_aggregate_rows_keys_* merges them;
+ *   stage 3: the merged (G, X) rows in that order; for each G group, in ascending X order, F's buffers merged by
+ *            mergeExpressions from their initial values (a decimal sum is null once an input sum is null, which is an
+ *            overflow, or the running sum reaches 10^P; isEmpty is the AND; a variance is merged by CentralMomentAgg's
+ *            mergeExpressions) and D's buffers updated by updateExpressions over the column's value in each (G, X) row.
+ *            Double chains are one rounded add, or one rounded central-moment step, at a time, no FMA.
+ * Output rows: what b2s_aggregate_partition_compress_rows_hash_* writes for key columns G and functions F ++ D
+ * (UnsafeProjection(G ++ F's buffers ++ D's buffers)), key values from the G group's first row, in the composite-key
+ * order of G, partitioned stably by pmod(Murmur3Hash(G, 42), num_partitions) and compressed with codec, level,
+ * codec_block_size and checksum_alg.  n_group_keys == 0 is SinglePartition: num_partitions must be 1, and the call
+ * writes exactly one row, the initial buffers (Sum null, Count 0, Avg 0 and 0, decimal Sum 0 and isEmpty true, Variance
+ * (0, 0, 0)) when the task has no rows (HashAggregateExec's outputForEmptyGroupingKeyWithoutInput).
+ * Defining contract: dst_off / dst_len / checksum_out (may be NULL) / part_status (per output partition), *dst_total and
+ * the return value are byte for byte what b2s_partition_compress_rows_hash_packed returns for those rows in that order,
+ * keyed by G at its output slots (8 + 8 c, null bit c); without G, what b2s_partition_compress_packed returns with one
+ * partition and every id 0.  counts[3] (required): the input rows, the (G, X) groups, the rows written.
+ * A corrupt or mis-framed block: as in the aggregated read, its status is set, nothing is written, every partition's
+ * outputs are 0 and the call returns 0.  dst_cap below the arena -> B2S_E_DST_TOO_SMALL with *dst_total = the bytes
+ * needed (the caller cannot bound the output before decoding: retry once with that).
+ * Errors, B2S_E_ARG, checked before the device: every rule above (a single-column distinct function with more than
+ * one distinct column included); n_keys + F's fields above 32; more than 16 buffers in
+ * the input (F) or the output (F ++ D; a VARIANCE is one); n_group_keys + the output's fields above 32; n_distinct 0;
+ * the aggregated read's checks on the blocks and slices; the partition call's on codec, codec_block_size,
+ * num_partitions and the output arrays.  Device memory that cannot be had -> B2S_E_NOMEM; no usable device ->
+ * B2S_E_CUDA.
+ * Runs on the read lane's slot 0, as the aggregated read does (one lock, one stream).  b2s_last_timing: kernel_ms the
+ * whole call's device work, dominant_ms / dominant_launches stage 3 (from the merged (G, X) rows to the written rows). */
+#define B2S_DISTINCT_ALL_COLUMNS (-1)
+int b2s_decompress_aggregate_distinct_partition_compress_rows_hash_packed(
+    uint32_t codec, int32_t level, uint32_t codec_block_size, uint32_t checksum_alg, uint32_t n,
+    const uint8_t* src_base, const uint64_t* src_off, const uint64_t* src_len, const uint32_t* slice_base,
+    const uint64_t* slice_len, const uint64_t* slice_checksum, uint32_t n_group_keys, uint32_t n_keys,
+    const uint32_t* key_type, const uint32_t* key_len, uint32_t n_aggs, const uint32_t* agg_fn,
+    const uint32_t* val_type, uint32_t n_distinct, const uint32_t* distinct_fn, const uint32_t* distinct_val_type,
+    const int32_t* distinct_column, uint32_t num_partitions, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_off,
+    uint64_t* dst_len, uint64_t* dst_total, uint64_t* checksum_out, int32_t* part_status, uint64_t* counts,
+    int32_t* status, int32_t* bad_slice);
+/* same, with src_base and dst_base in device memory of dev_index; the other arrays stay host arrays */
+int b2s_decompress_aggregate_distinct_partition_compress_rows_hash_dev(
+    uint32_t dev_index, uint32_t codec, int32_t level, uint32_t codec_block_size, uint32_t checksum_alg, uint32_t n,
+    const uint8_t* src_base, const uint64_t* src_off, const uint64_t* src_len, const uint32_t* slice_base,
+    const uint64_t* slice_len, const uint64_t* slice_checksum, uint32_t n_group_keys, uint32_t n_keys,
+    const uint32_t* key_type, const uint32_t* key_len, uint32_t n_aggs, const uint32_t* agg_fn,
+    const uint32_t* val_type, uint32_t n_distinct, const uint32_t* distinct_fn, const uint32_t* distinct_val_type,
+    const int32_t* distinct_column, uint32_t num_partitions, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_off,
+    uint64_t* dst_len, uint64_t* dst_total, uint64_t* checksum_out, int32_t* part_status, uint64_t* counts,
+    int32_t* status, int32_t* bad_slice);
+
 /* ---- write side, window group limit: Spark's Sort and WindowGroupLimitExec(Partial) and its exchange on the GPU ----
  * The map side of a top-N-per-group window's shuffle (Sort(pk ++ ord, global = false) -> WindowGroupLimitExec(pk, ord,
  * rank_fn, limit, Partial) -> Exchange hashpartitioning(pk) | SinglePartition) in one call.  A reducer finishes it with

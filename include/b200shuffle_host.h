@@ -286,6 +286,21 @@ int b2sh_reader_read_window_frame_rows(b2sh_reader* r, uint32_t n_partition_keys
                                        const uint64_t* fn_default, const int64_t* frame_lower,
                                        const int64_t* frame_upper, const uint8_t** data, uint64_t* len,
                                        uint64_t* n_records, uint64_t* n_out_records);
+/* aggregate_distinct_rows(): one DISTINCT group's middle stage (INTEGRATION.md §3s).  r reads a reduce task of the
+ * exchange by G ++ X (its non-empty blocks fetched in computeShuffleBlocks order; the exchange cache is not consulted);
+ * w is a serialized writer of the exchange by G, created for map id = this reduce task and the second exchange's
+ * numPartitions (1 without G), with no partitioning set and no insert.  ONE
+ * b2s_decompress_aggregate_distinct_partition_compress_rows_hash_packed call (the arguments after w are that call's;
+ * retried once with the exact size on B2S_E_DST_TOO_SMALL) merges and folds the rows and partitions them into w's
+ * arena, and w writes .data / .index / .checksum exactly as its commit() lays them out.  partition_lengths_out:
+ * w's numPartitions values; counts[3]: the input rows, the (G, X) groups, the rows written.  A checksum mismatch
+ * returns B2SH_E_SPARK with the reference's message and a malformed stream B2SH_E_IO, and then no file is written. */
+int b2sh_reader_aggregate_distinct_rows(b2sh_reader* r, b2sh_serialized_writer* w, uint32_t n_group_keys,
+                                        uint32_t n_keys, const uint32_t* key_type, const uint32_t* key_len,
+                                        uint32_t n_aggs, const uint32_t* agg_fn, const uint32_t* val_type,
+                                        uint32_t n_distinct, const uint32_t* distinct_fn,
+                                        const uint32_t* distinct_val_type, const int32_t* distinct_column,
+                                        int64_t* partition_lengths_out, uint64_t* counts);
 int b2sh_reader_block(b2sh_reader* r, uint32_t k, int64_t* map_id, int32_t* start_reduce, int32_t* end_reduce,
                       const uint8_t** data, uint64_t* len);
 uint64_t b2sh_reader_remote_bytes_read(b2sh_reader* r); /* metric parity with storage/S3ShuffleReader.scala:94-95 */

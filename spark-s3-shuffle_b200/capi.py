@@ -128,6 +128,13 @@ PROTOTYPES = [
     ("b2s_aggregate_grouping_sets_partition_compress_rows_hash_dev", C.c_int,
      [_u32, _u32, _i32, _u32, _u32, _u32, _u64, _vp, _u64, _u32p, _u32, _u32p, _u32p, _u32p, _i32p, _u32, _u32p, _u32p,
       _u32p, _i32p, _u32, _u32p, _vp, _u64, _u64p, _u64p, _u64p, _u64p, _i32p, _u64p]),
+    ("b2s_decompress_aggregate_distinct_partition_compress_rows_hash_packed", C.c_int,
+     [_u32, _i32, _u32, _u32, _u32, _u8p, _u64p, _u64p, _u32p, _u64p, _u64p, _u32, _u32, _u32p, _u32p, _u32, _u32p,
+      _u32p, _u32, _u32p, _u32p, _i32p, _u32, _u8p, _u64, _u64p, _u64p, _u64p, _u64p, _i32p, _u64p, _i32p, _i32p]),
+    ("b2s_decompress_aggregate_distinct_partition_compress_rows_hash_dev", C.c_int,
+     [_u32, _u32, _i32, _u32, _u32, _u32, _vp, _u64p, _u64p, _u32p, _u64p, _u64p, _u32, _u32, _u32p, _u32p, _u32,
+      _u32p, _u32p, _u32, _u32p, _u32p, _i32p, _u32, _vp, _u64, _u64p, _u64p, _u64p, _u64p, _i32p, _u64p, _i32p,
+      _i32p]),
     ("b2s_window_limit_partition_compress_rows_hash_packed", C.c_int,
      [_u32, _i32, _u32, _u32, _u32, _u64, _u8p, _u64, _u32p, _u32, _u32, _u32p, _u32p, _u32p, _i32p, _u32, _i32, _u8p,
       _u64, _u64p, _u64p, _u64p, _u64p, _i32p, _u64p]),
@@ -996,6 +1003,49 @@ def aggregate_partition_compress_rows_hash_dev(codec, d_records, rec_bytes, d_re
         _ptr(dst_off), _ptr(dst_len), C.addressof(total), _ptr(cks), _ptr(st), C.addressof(groups)),
         "b2s_aggregate_partition_compress_rows_hash_dev")
     return dict(dst_off=dst_off, dst_len=dst_len, total=total.value, checksums=cks, status=st, n_groups=groups.value)
+
+
+DISTINCT_ALL_COLUMNS = -1  # B2S_DISTINCT_ALL_COLUMNS: count(DISTINCT every distinct column)
+
+
+def aggregate_distinct_partition_compress_rows_hash(codec, src, off, length, dst, n_group_keys, keys, aggs, distinct,
+                                                    num_partitions, checksum_alg=CHECKSUM_NONE, slice_base=None,
+                                                    slice_len=None, slice_checksum=None, block_size=0, level=0,
+                                                    dev=None, dst_cap=None):
+    """One DISTINCT group's middle stage on a reducer of the exchange by G ++ X: its blocks of the map side's partial
+    rows (keys G ++ X, functions aggs) merged per (G, X), folded per G (aggs' buffers merged, distinct's updated over
+    their columns), hash-partitioned by G and compressed into dst.  keys = [(key_type, key_len), ...], the first
+    n_group_keys G; aggs = [(fn, val_type), ...]; distinct = [(fn, val_type, column or DISTINCT_ALL_COLUMNS), ...].
+    dev None: src and dst host arrays; else device addresses (dst_cap required).  -> dict(dst_off, dst_len, total,
+    checksums, part_status, counts (input rows, (G, X) groups, rows written), status, bad_slice)"""
+    if dev is None:
+        src, dst = _as_u8(src), _as_u8(dst)
+        dst_cap = dst.size
+    off = np.ascontiguousarray(off, dtype=np.uint64)
+    length = np.ascontiguousarray(length, dtype=np.uint64)
+    n = off.size
+    sb, sl, sc = _slice_arrays(checksum_alg, slice_base, slice_len, slice_checksum)
+    kt = np.array([k[0] for k in keys] or [0], dtype=np.uint32)
+    kl = np.array([k[1] for k in keys] or [0], dtype=np.uint32)
+    fn = np.array([a[0] for a in aggs] or [0], dtype=np.uint32)
+    vt = np.array([a[1] for a in aggs] or [0], dtype=np.uint32)
+    dfn = np.array([a[0] for a in distinct] or [0], dtype=np.uint32)
+    dvt = np.array([a[1] for a in distinct] or [0], dtype=np.uint32)
+    dcol = np.array([a[2] for a in distinct] or [0], dtype=np.int32)
+    dst_off, dst_len, cks, pst = _partition_out(num_partitions)
+    total = _u64(0)
+    counts = np.zeros(3, dtype=np.uint64)
+    st = np.zeros(max(n, 1), dtype=np.int32)
+    bad = np.zeros(max(n, 1), dtype=np.int32)
+    symbol = "b2s_decompress_aggregate_distinct_partition_compress_rows_hash_" + ("packed" if dev is None else "dev")
+    lead = [] if dev is None else [dev]
+    _check(getattr(load(), symbol)(
+        *lead, codec, level, block_size, checksum_alg, n, _arg(src), _ptr(off), _ptr(length), _arg(sb), _arg(sl),
+        _arg(sc), n_group_keys, len(keys), _ptr(kt), _ptr(kl), len(aggs), _ptr(fn), _ptr(vt), len(distinct), _ptr(dfn),
+        _ptr(dvt), _ptr(dcol), num_partitions, _arg(dst), dst_cap, _ptr(dst_off), _ptr(dst_len), C.addressof(total),
+        _ptr(cks), _ptr(pst), _ptr(counts), _ptr(st), _ptr(bad)), symbol)
+    return dict(dst_off=dst_off, dst_len=dst_len, total=total.value, checksums=cks, part_status=pst,
+                counts=[int(c) for c in counts], status=st[:n], bad_slice=bad[:n])
 
 
 def aggregate_grouping_sets_partition_compress_rows_hash_packed(codec, records, rec_len, keys, aggs, sets,

@@ -757,6 +757,7 @@ uint64_t* rows_aggregate_readback(uint8_t* d_aws, uint64_t n, uint32_t n_aggs, u
 
 const uint64_t* rows_group_heads_before(uint8_t* d_aws, uint64_t n) { return carve_agg_ws(d_aws, n, 0, 0).head; }
 const uint32_t* rows_group_starts(uint8_t* d_aws, uint64_t n) { return carve_agg_ws(d_aws, n, 0, 0).gpos; }
+const uint32_t* rows_group_lengths(uint8_t* d_aws, uint64_t n) { return carve_agg_ws(d_aws, n, 0, 0).glen; }
 
 void launch_rows_group(const uint8_t* arena, uint64_t n, const uint32_t* idx, const uint32_t* heads,
                        uint32_t key_bytes, const AggSpec& spec, uint8_t* d_ws, uint8_t* d_aws, cudaStream_t st,

@@ -825,7 +825,9 @@ int get_device(uint32_t dev_index, Device** out) {
 }
 
 // the kinds of call whose steps add_times reads into b2s_last_timing, one rule each
-enum class Family { kCodec, kPartition, kPartitionNone, kSort, kSortRows, kAggregate, kJoin, kWindow, kPartialAggregate };
+enum class Family {
+  kCodec, kPartition, kPartitionNone, kSort, kSortRows, kAggregate, kJoin, kWindow, kPartialAggregate, kDistinctAggregate
+};
 
 // Adds the times of this call's steps on S to b2s_last_timing: kernel_ms, top_kernel_ms, dominant_ms / _launches by
 // the rule of its family, and h2d_ms.  A step the call did not run reads 0; one it started but did not finish ends
@@ -866,6 +868,12 @@ void add_times(Slot& S, Family f) {
       break;
     case Family::kPartialAggregate:  // aggregation + partition step + compression (or checksums); the codec step (or
                                      // the partition step); the aggregation step
+      t.kernel_ms += S.span(G0, S.mine(K1) ? K1 : P1);
+      t.top_kernel_ms += S.mine(T0) ? S.span(T0, T1) : S.span(P0, P1);
+      dominant(G0, G1);
+      break;
+    case Family::kDistinctAggregate:  // read + stage 2 (the call adds their span) + stage 3 + partition step +
+                                      // compression; the codec step (or the partition step); stage 3
       t.kernel_ms += S.span(G0, S.mine(K1) ? K1 : P1);
       t.top_kernel_ms += S.mine(T0) ? S.span(T0, T1) : S.span(P0, P1);
       dominant(G0, G1);
@@ -4873,6 +4881,411 @@ int b2s_decompress_aggregate_rows_keys_dev(uint32_t dev_index, uint32_t codec, u
 
 // The join calls: the composite-key row sort's call over both sides, with the join's outputs zeroed first; every
 // count and *dst_total are 0 when a block failed (nothing is written).
+// ------------------------------------------------------------------------------------------------------------
+// read + write, one DISTINCT group's middle stage: a reducer's (G ++ X, F) partial rows merged per (G, X) group as the
+// aggregated read merges them (Spark's PartialMerge), then folded per G group (F's buffers merged, D's updated over the
+// distinct column: HashAggregate(G, F: PartialMerge, D: Partial)), then hash-partitioned by G and compressed
+// ------------------------------------------------------------------------------------------------------------
+// The call's functions: the key columns (the first n_group_keys are G, the rest X), F as (fn, val_type) and D as
+// (fn, val_type, column)
+struct DistinctFns {
+  uint32_t n_group_keys, n_keys;
+  const uint32_t *key_type, *key_len;
+  uint32_t n_aggs;
+  const uint32_t *agg_fn, *val_type;
+  uint32_t n_distinct;
+  const uint32_t *distinct_fn, *distinct_val_type;
+  const int32_t* distinct_column;
+};
+
+// What the arguments make of a call: the aggregated read's spec over the input rows (its arrays held here), the step's
+// spec over the merged rows, and each output field's initial value (a global aggregate's row without input)
+struct DistinctPlan {
+  uint32_t key_off[kMaxKeys];
+  int32_t key_nf[kMaxKeys];
+  uint32_t op[kMaxAggs], off[kMaxAggs];
+  int32_t nf[kMaxAggs];
+  RecordSpec read;
+  PartialAggSpec step;
+  std::vector<int> init;  // per step buffer: 0 the value 0, 1 the value 1 (isEmpty), -1 null
+};
+
+// a key column's type agrees with a distinct function's val_type (the value the buffer reads from the column's slot)
+static bool distinct_type_ok(uint32_t kt, uint32_t fn, uint32_t vt) {
+  const uint32_t kind = vt & 0xff, p = (vt >> 8) & 0xff;
+  switch (kt) {
+    case B2S_KEY_INT8: return kind == B2S_WINDOW_VAL_INT8;
+    case B2S_KEY_INT16: return kind == B2S_WINDOW_VAL_INT16;
+    case B2S_KEY_INT32: return kind == B2S_WINDOW_VAL_INT32;
+    case B2S_KEY_INT64: return kind == B2S_WINDOW_VAL_INT64 || (kind == B2S_WINDOW_VAL_DECIMAL && p <= 18);
+    case B2S_KEY_FLOAT32: return kind == B2S_WINDOW_VAL_FLOAT32;
+    case B2S_KEY_FLOAT64: return kind == B2S_WINDOW_VAL_FLOAT64;
+    case kDecimalKey: return kind == B2S_WINDOW_VAL_DECIMAL && p > 18;
+    default: return fn == B2S_WINDOW_COUNT && kind == B2S_WINDOW_VAL_BYTES;  // string, binary, boolean
+  }
+}
+
+// the initial values of one function's buffers, in its buffers' order (Spark's initialValues)
+static void distinct_inits(uint32_t fn, uint32_t vt, std::vector<int>& init) {
+  const bool dec = (vt & 0xff) == B2S_WINDOW_VAL_DECIMAL;
+  if (fn == B2S_WINDOW_SUM) {
+    if (dec) init.insert(init.end(), {0, 1});
+    else init.push_back(-1);
+  } else if (fn == B2S_WINDOW_AVG) {
+    init.insert(init.end(), {0, 0});
+  } else if (fn == B2S_WINDOW_COUNT || fn == B2S_WINDOW_VARIANCE) {
+    init.push_back(0);
+  } else {
+    init.push_back(-1);
+  }
+}
+
+// Every rule of the call before the device (B2S_E_ARG): the key columns, F and D, the layouts' limits, and the merge
+// entries over the input's buffers: each of F's buffers at its field (n_keys + its field ordinal)
+static int distinct_plan(const DistinctFns& d, uint32_t num_partitions, DistinctPlan& P) {
+  if (d.n_keys < 1 || d.n_keys > kMaxKeys || d.n_group_keys >= d.n_keys)
+    return fail(B2S_E_ARG, "n_keys must be in [1, 16] and n_group_keys below it (at least one distinct column)%s");
+  if (!d.key_type || !d.key_len) return fail(B2S_E_ARG, "null argument%s");
+  if (d.n_aggs > kMaxAggs || d.n_distinct > kMaxAggs) return fail(B2S_E_ARG, "n_aggs and n_distinct must be at most 16%s");
+  if ((d.n_aggs && (!d.agg_fn || !d.val_type)) ||
+      (d.n_distinct && (!d.distinct_fn || !d.distinct_val_type || !d.distinct_column)))
+    return fail(B2S_E_ARG, "null argument%s");
+  if (!d.n_distinct) return fail(B2S_E_ARG, "n_distinct must be at least 1 (no DISTINCT function: use the "
+                                            "aggregated read)%s");
+  const uint32_t nk = d.n_keys;
+  for (uint32_t c = 0; c < nk; c++) {
+    P.key_off[c] = 8 + 8 * c;
+    P.key_nf[c] = (int32_t)c;
+  }
+  P.read = keys_spec(nk, d.key_type, P.key_off, d.key_len, P.key_nf);
+  if (int rc = key_columns_args(P.read)) return rc;
+  for (uint32_t c = 0; c < nk; c++) {
+    if (d.key_type[c] & ~kKeyTypeMask) return fail(B2S_E_ARG, "the key columns take no order flag%s");
+    if (c < d.n_group_keys && d.key_type[c] == B2S_KEY_BYTES && d.key_len[c] != 1)
+      return fail(B2S_E_ARG, "a hashed B2S_KEY_BYTES column is a boolean: key_len must be 1%s");
+  }
+  if (!d.n_group_keys && num_partitions != 1)
+    return fail(B2S_E_ARG, "without grouping columns the exchange is SinglePartition: num_partitions must be 1%s");
+  // F: its buffers as the map side lays them out, then a merge entry for each
+  PartialAggSpec& st = P.step;
+  st.merge = true;
+  uint32_t field = nk, n_read = 0;
+  for (uint32_t a = 0; a < d.n_aggs; a++) {
+    PartialAggSpec f;
+    const uint32_t off = 8, one_off[1] = {off};
+    const int32_t one_nf[1] = {-1};
+    if (int rc = partial_agg_args(1, d.agg_fn + a, d.val_type + a, one_off, one_nf, &f)) return rc;
+    distinct_inits(d.agg_fn[a], d.val_type[a], P.init);
+    for (uint32_t b = 0; b < f.n_bufs; b++) {
+      if (st.n_bufs == kMaxAggs || n_read == kMaxAggs)
+        return fail(B2S_E_ARG, "more than 16 aggregation buffers (the reduce-side merge's limit)%s");
+      const uint32_t op = f.op[b], k = st.n_bufs++, slot = 8 + 8 * field;
+      const bool var = op == B2S_AGG_VARIANCE;
+      uint32_t vt = f.vtype[b];
+      if (op == B2S_AGG_SUM_INT64) vt = B2S_WINDOW_VAL_INT64;
+      else if (op == B2S_AGG_SUM_FLOAT64 || var) vt = B2S_WINDOW_VAL_FLOAT64;
+      else if (op == B2S_AGG_MIN_INT32 && f.stage[b] == kStageIsEmpty) vt = B2S_WINDOW_VAL_INT32;
+      else if (agg_base_op(op) == B2S_AGG_SUM_DECIMAL) vt = B2S_WINDOW_VAL_DECIMAL | agg_precision(op) << 8;
+      st.op[k] = op;
+      st.vtype[k] = vt;
+      st.voff[k] = slot;
+      st.vnull[k] = var ? -1 : (int32_t)field;
+      st.stage[k] = var || agg_base_op(op) == B2S_AGG_SUM_DECIMAL ? kStageMerge : kStageValue;
+      if (st.stage[k] == kStageMerge) (var ? st.n_merge_var : st.n_merge_dec)++;
+      if (agg_decimal_op(op)) st.wide[k] = st.n_dec++;
+      if (var) {
+        st.wide[k] = st.n_dec;  // avg and m2 staged as two high words
+        st.n_dec += 2;
+        st.var[k] = st.n_var++;
+      }
+      st.dsum |= op == B2S_AGG_SUM_FLOAT64;
+      st.n_fields += var ? 3 : 1;
+      P.op[n_read] = op;
+      P.off[n_read] = slot;
+      P.nf[n_read] = var ? -1 : (int32_t)field;
+      n_read++;
+      field += var ? 3 : 1;
+    }
+  }
+  if (field > 32) return fail(B2S_E_ARG, "n_keys + F's buffer fields (3 per VARIANCE) must be at most 32 (the input's "
+                                         "one null word)%s");
+  P.read = with_aggregates(P.read, n_read, P.op, P.off, P.nf);
+  // D: each function's update over its distinct column, or count(DISTINCT every distinct column)
+  uint32_t all_mask = 0;
+  for (uint32_t c = d.n_group_keys; c < nk; c++) all_mask |= 1u << c;
+  for (uint32_t a = 0; a < d.n_distinct; a++) {
+    const uint32_t fn = d.distinct_fn[a], vt = d.distinct_val_type[a];
+    const int32_t col = d.distinct_column[a];
+    if (fn == B2S_WINDOW_MIN || fn == B2S_WINDOW_MAX)
+      return fail(B2S_E_ARG, "MIN and MAX take no DISTINCT (Spark's optimizer drops it)%s");
+    if (fn != B2S_WINDOW_SUM && fn != B2S_WINDOW_COUNT && fn != B2S_WINDOW_AVG && fn != B2S_WINDOW_VARIANCE)
+      return fail(B2S_E_ARG, "a distinct function must be COUNT, SUM, AVG or VARIANCE%s");
+    if (col == B2S_DISTINCT_ALL_COLUMNS) {
+      if (fn != B2S_WINDOW_COUNT || vt != B2S_WINDOW_VAL_NONE)
+        return fail(B2S_E_ARG, "B2S_DISTINCT_ALL_COLUMNS is count(DISTINCT every distinct column): COUNT with "
+                               "B2S_WINDOW_VAL_NONE%s");
+      if (st.n_bufs == kMaxAggs) return fail(B2S_E_ARG, "more than 16 aggregation buffers in the output%s");
+      const uint32_t k = st.n_bufs++;
+      st.op[k] = B2S_AGG_SUM_INT64;
+      st.stage[k] = kStageCountAll;
+      st.vtype[k] = B2S_WINDOW_VAL_NONE;
+      st.voff[k] = all_mask;
+      st.vnull[k] = -1;
+      st.n_fields++;
+      P.init.push_back(0);
+      continue;
+    }
+    if (col < (int32_t)d.n_group_keys || col >= (int32_t)nk)
+      return fail(B2S_E_ARG, "a distinct function's column must be a distinct column (in [n_group_keys, n_keys)) or "
+                             "B2S_DISTINCT_ALL_COLUMNS%s");
+    // one DISTINCT group: every distinct function's children are all of X, so with several X columns the only one is
+    // count(DISTINCT x1, .., xn); over one of them a (G, X) row is not a distinct value of that column
+    if (nk - d.n_group_keys > 1)
+      return fail(B2S_E_ARG, "with several distinct columns a distinct function must take them all "
+                             "(B2S_DISTINCT_ALL_COLUMNS)%s");
+    if (!distinct_type_ok(d.key_type[col], fn, vt))
+      return fail(B2S_E_ARG, "a distinct function's val_type does not agree with its column's key type%s");
+    PartialAggSpec f;
+    const uint32_t off[1] = {8 + 8 * (uint32_t)col};
+    const int32_t nf[1] = {col};
+    if (int rc = partial_agg_args(1, &fn, &vt, off, nf, &f)) return rc;
+    distinct_inits(fn, vt, P.init);
+    for (uint32_t b = 0; b < f.n_bufs; b++) {
+      if (st.n_bufs == kMaxAggs) return fail(B2S_E_ARG, "more than 16 aggregation buffers in the output%s");
+      const uint32_t k = st.n_bufs++, op = f.op[b];
+      st.op[k] = op;
+      st.stage[k] = f.stage[b];
+      st.to_double[k] = f.to_double[b];
+      st.vtype[k] = f.vtype[b];
+      st.voff[k] = f.voff[b];
+      st.vnull[k] = f.vnull[b];
+      if (agg_decimal_op(op)) st.wide[k] = st.n_dec++;
+      if (op == B2S_AGG_VARIANCE) st.var[k] = st.n_var++;
+      st.dsum |= op == B2S_AGG_SUM_FLOAT64;
+    }
+    st.n_fields += f.n_fields;
+  }
+  if (d.n_group_keys + st.n_fields > 32)
+    return fail(B2S_E_ARG, "n_group_keys + the output's buffer fields (3 per VARIANCE) must be at most 32 (one null "
+                           "word)%s");
+  st.keys = keys_spec(d.n_group_keys ? d.n_group_keys : 1, d.key_type, P.key_off, d.key_len, P.key_nf).keys;
+  st.keys.n = d.n_group_keys;
+  return 0;
+}
+
+// A global aggregate's one output row without input: HashAggregateExec's outputForEmptyGroupingKeyWithoutInput, the
+// initial buffers as UnsafeProjection writes them ([size: int32 big-endian][row])
+static std::vector<uint8_t> initial_row(const DistinctPlan& P) {
+  const PartialAggSpec& st = P.step;
+  const uint32_t nf = st.n_fields, fixed = 8 * (1 + nf);
+  uint32_t wide = 0;
+  for (uint32_t k = 0; k < st.n_bufs; k++) wide += agg_decimal_wide(st.op[k]) ? 1 : 0;
+  std::vector<uint8_t> rec(4 + fixed + 16 * wide, 0);
+  uint8_t* row = rec.data() + 4;
+  uint64_t nulls = 0;
+  uint32_t f = 0, var_at = fixed;
+  for (uint32_t k = 0; k < st.n_bufs; k++) {
+    const uint32_t op = st.op[k];
+    uint64_t slot = P.init[k] > 0 ? 1 : 0;
+    if (agg_decimal_wide(op)) {  // 16 bytes; 0 is BigInteger.toByteArray's one byte 00
+      slot = ((uint64_t)var_at << 32) | (P.init[k] < 0 ? 0 : 1);
+      var_at += 16;
+    }
+    if (P.init[k] < 0) nulls |= 1ull << f;
+    memcpy(row + 8 + 8 * f, &slot, 8);
+    f += op == B2S_AGG_VARIANCE ? 3 : 1;  // a variance's (0.0, 0.0, 0.0)
+  }
+  memcpy(row, &nulls, 8);
+  const uint32_t size = (uint32_t)rec.size() - 4;
+  for (int b = 0; b < 4; b++) rec[b] = (uint8_t)(size >> (24 - 8 * b));
+  return rec;
+}
+
+// The whole call on the read lane's slot 0: decode, the aggregated read's order and merge by G ++ X (the merged rows
+// into S.parena, their lengths in S.pws), the step over them in S.fws (no sort: heads where G's encoding changes) into
+// S.aggrows, and the partition + compress step.  No step ensures a buffer that holds its own input: the partition step
+// ensures S.pws, S.parena and (packed) S.dst, which hold only stage 2's inputs and outputs by then.
+static int distinct_task_run(Device* D, bool packed, uint32_t codec, int32_t level, uint32_t bs, uint32_t alg,
+                             uint32_t n, const uint8_t* src_base, const uint64_t* src_off, const uint64_t* src_len,
+                             const uint32_t* slice_base, const uint64_t* slice_len, const uint64_t* slice_checksum,
+                             const DistinctPlan& P, uint32_t num_partitions, uint8_t* dst_base, uint64_t dst_cap,
+                             uint64_t* dst_off, uint64_t* dst_len, uint64_t* dst_total, uint64_t* checksum_out,
+                             int32_t* part_status, uint64_t* counts, int32_t* status, int32_t* bad_slice,
+                             const WallTimer& wt) {
+  Lane& Ln = D->lane[kLaneRead];
+  std::lock_guard<std::mutex> lk(Ln.mtx);
+  Slot& S = Ln.slot[0];
+  const SortBufferTrim trim{S};
+  const PartialAggTrim trim_step{S};
+  cudaStream_t st = S.st;
+  std::vector<uint64_t> dev_off;
+  uint64_t srcb = 0;
+  for (uint32_t i = 0; i < n; i++) {
+    if (packed) dev_off.push_back(srcb);
+    srcb += src_len[i];
+  }
+  int rc;
+  if (packed) {
+    if ((rc = S.src.ensure(srcb + 64))) return rc;
+    CU(S.mark(H0, st));
+    for (uint32_t i = 0; i < n;) {
+      uint32_t j = i + 1;
+      while (j < n && src_off[j] == src_off[j - 1] + src_len[j - 1]) j++;
+      const uint64_t bytes = dev_off[j - 1] + src_len[j - 1] - dev_off[i];
+      if (bytes)
+        CU(cudaMemcpyAsync((uint8_t*)S.src.p + dev_off[i], src_base + src_off[i], bytes, cudaMemcpyHostToDevice, st));
+      i = j;
+    }
+    CU(S.mark(H1, st));
+  }
+  uint64_t launches = 0;
+  const RecordSpec& spec = P.read;
+  const PartialAggSpec& step = P.step;
+  DecodedTask T(nullptr, n, status, bad_slice);
+  RowOrder R;
+  if (n) {  // no blocks: an empty reducer, straight to the step
+    rc = decode_task(D, S, codec, alg, n, packed ? (const uint8_t*)S.src.p : src_base,
+                     packed ? dev_off.data() : src_off, src_len, packed, slice_base, slice_len, slice_checksum, srcb,
+                     spec, ~0ull, T, &launches);
+    if (rc) return rc;
+    if (!T.failed) rc = order_rows(S, spec, T, nullptr, 0, R, &launches);
+    if (rc) return rc;
+  }
+  // stage 2: the (G, X) groups merged into S.parena
+  uint64_t merged_bytes = 0, n_in = 0, n_gx = 0;
+  if (n && !T.failed) {
+    if ((rc = S.parena.ensure(T.total + 64))) return rc;
+    rc = aggregate_rows_tail(S, spec, T, R, (uint8_t*)S.parena.p, T.total, &merged_bytes, &n_in, &n_gx, &launches);
+    if (rc) return rc;
+  }
+  if (T.failed) {  // nothing is written
+    for (uint32_t p = 0; p < num_partitions; p++) {
+      dst_off[p] = dst_len[p] = 0;
+      if (checksum_out) checksum_out[p] = 0;
+      part_status[p] = B2S_OK;
+    }
+    return 0;
+  }
+  const double read_ms = S.span(K0, G1);
+  // stage 3 over the n_gx merged rows: offsets, G's heads, grouping, folds (one readback: rows, bytes), emit
+  const uint8_t* merged = (const uint8_t*)S.parena.p;
+  const uint32_t key_bytes = rows_key_bytes(step.keys);
+  const size_t part[4] = {rows_sort_ws_bytes(n_gx, key_bytes), 256 + align_up(n_gx * 4, 256),
+                          rows_aggregate_ws_bytes(n_gx, 0, 0), partial_agg_ws_bytes(n_gx, step)};
+  if ((rc = S.fws.ensure(part[0] + part[1] + part[2] + part[3]))) return rc;
+  uint8_t* ws = (uint8_t*)S.fws.p;
+  uint32_t* heads = (uint32_t*)(ws + part[0] + 256);
+  uint8_t *gws = ws + part[0] + part[1], *paws = gws + part[2];
+  if ((rc = S.hmeta.ensure(48))) return rc;
+  uint64_t* rb = (uint64_t*)S.hmeta.p;
+  CU(S.mark(G0, st, launches));
+  launch_partial_agg_offsets(rows_group_lengths(R.aws, R.records), n_gx, key_bytes, ws, paws, st, &launches);
+  uint64_t rows = 0, rows_bytes = 0;
+  const uint32_t* d_row_len = partial_agg_row_len(paws, n_gx, step);
+  if (n_gx) {
+    launch_partial_agg_heads(merged, n_gx, key_bytes, step.keys, ws, heads, st, &launches);
+    launch_rows_group(merged, n_gx, nullptr, heads, key_bytes, AggSpec{}, ws, gws, st, &launches);
+    launch_partial_agg_fold(merged, n_gx, nullptr, key_bytes, step, ws, gws, paws, st, &launches);
+    CU(cudaMemcpyAsync(rb, partial_agg_header(paws) + 4, 16, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    CU(cudaGetLastError());
+    rows = rb[0];
+    rows_bytes = rb[1];
+    if ((rc = S.aggrows.ensure(rows_bytes + 64))) return rc;
+    launch_partial_agg_emit(merged, n_gx, rows, nullptr, key_bytes, step, ws, gws, paws, (uint8_t*)S.aggrows.p, st,
+                            &launches);
+  } else if (!step.keys.n) {  // a global aggregate without input: its initial row
+    const std::vector<uint8_t> row = initial_row(P);
+    const uint32_t len = (uint32_t)row.size();
+    rows = 1;
+    rows_bytes = len;
+    if ((rc = S.aggrows.ensure(256 + len + 64))) return rc;
+    CU(cudaMemcpyAsync((uint8_t*)S.aggrows.p + 256, row.data(), len, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(S.aggrows.p, &len, 4, cudaMemcpyHostToDevice, st));
+    CU(cudaStreamSynchronize(st));
+    d_row_len = (const uint32_t*)S.aggrows.p;
+  }
+  CU(S.mark(G1, st, launches));
+  const uint8_t* d_rows = (const uint8_t*)S.aggrows.p + (n_gx || !rows ? 0 : 256);
+  RowIds ids{partial_row_keys(step.keys)};
+  if (!step.keys.n) ids.range = true;  // SinglePartition: the range ids of no bounds, every id 0
+  uint64_t arena = 0, fit = 0;
+  rc = map_rows_partition(D, S, packed, codec, level, bs, alg, num_partitions, rows, d_rows, rows_bytes, d_row_len, ids,
+                          dst_base, dst_cap, dst_off, dst_len, checksum_out, part_status, &arena, &fit, &launches);
+  if (rc && rc != B2S_E_DST_TOO_SMALL) return rc;
+  *dst_total = arena;
+  counts[0] = n_in;
+  counts[1] = n_gx;
+  counts[2] = rows;
+  t_timing.kernel_ms += read_ms;
+  end_call(wt, launches, CallBytes{srcb, arena, packed ? srcb : 0, fit}, &S, Family::kDistinctAggregate);
+  return rc;
+}
+
+// b2s_decompress_aggregate_distinct_partition_compress_rows_hash_*: zero the outputs, every check before the device,
+// then the device (B2S_E_CUDA without one) and the run
+static int distinct_call(bool packed, uint32_t dev_index, uint32_t codec, int32_t level, uint32_t codec_block_size,
+                         uint32_t alg, uint32_t n, const uint8_t* src_base, const uint64_t* src_off,
+                         const uint64_t* src_len, const uint32_t* slice_base, const uint64_t* slice_len,
+                         const uint64_t* slice_checksum, const DistinctFns& fns, uint32_t num_partitions,
+                         uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_off, uint64_t* dst_len,
+                         uint64_t* dst_total, uint64_t* checksum_out, int32_t* part_status, uint64_t* counts,
+                         int32_t* status, int32_t* bad_slice) {
+  const WallTimer wt = begin_call();
+  if (dst_total) *dst_total = 0;
+  if (counts) counts[0] = counts[1] = counts[2] = 0;
+  if (!counts || !dst_total) return fail(B2S_E_ARG, "null argument%s");
+  DistinctPlan P;
+  if (int rc = distinct_plan(fns, num_partitions, P)) return rc;
+  uint64_t unused_total = 0, unused_records = 0;
+  if (int rc = sort_args(codec, alg, n, src_off, src_len, slice_base, slice_len, slice_checksum, P.read, src_base,
+                         nullptr, 0, &unused_total, &unused_records, status))
+    return rc;
+  const uint32_t bs = block_size_or_default(codec_block_size);
+  const RowIds ids{P.step.keys};
+  if (int rc = partition_args(codec, bs, alg, num_partitions, 0, nullptr, 0, nullptr, nullptr, dst_base, dst_off,
+                              dst_len, part_status, &ids))
+    return rc;
+  if (dst_cap && !dst_base) return fail(B2S_E_ARG, "null argument%s");
+  Device* D;
+  if (int rc = sort_device(packed ? t_device : dev_index, &D)) return rc;
+  return distinct_task_run(D, packed, codec, level, bs, alg, n, src_base, src_off, src_len, slice_base, slice_len,
+                           slice_checksum, P, num_partitions, dst_base, dst_cap, dst_off, dst_len, dst_total,
+                           checksum_out, part_status, counts, status, bad_slice, wt);
+}
+
+int b2s_decompress_aggregate_distinct_partition_compress_rows_hash_packed(
+    uint32_t codec, int32_t level, uint32_t codec_block_size, uint32_t checksum_alg, uint32_t n,
+    const uint8_t* src_base, const uint64_t* src_off, const uint64_t* src_len, const uint32_t* slice_base,
+    const uint64_t* slice_len, const uint64_t* slice_checksum, uint32_t n_group_keys, uint32_t n_keys,
+    const uint32_t* key_type, const uint32_t* key_len, uint32_t n_aggs, const uint32_t* agg_fn,
+    const uint32_t* val_type, uint32_t n_distinct, const uint32_t* distinct_fn, const uint32_t* distinct_val_type,
+    const int32_t* distinct_column, uint32_t num_partitions, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_off,
+    uint64_t* dst_len, uint64_t* dst_total, uint64_t* checksum_out, int32_t* part_status, uint64_t* counts,
+    int32_t* status, int32_t* bad_slice) {
+  const DistinctFns fns{n_group_keys, n_keys, key_type, key_len, n_aggs, agg_fn, val_type,
+                        n_distinct, distinct_fn, distinct_val_type, distinct_column};
+  return distinct_call(true, 0, codec, level, codec_block_size, checksum_alg, n, src_base, src_off, src_len,
+                       slice_base, slice_len, slice_checksum, fns, num_partitions, dst_base, dst_cap, dst_off,
+                       dst_len, dst_total, checksum_out, part_status, counts, status, bad_slice);
+}
+
+int b2s_decompress_aggregate_distinct_partition_compress_rows_hash_dev(
+    uint32_t dev_index, uint32_t codec, int32_t level, uint32_t codec_block_size, uint32_t checksum_alg, uint32_t n,
+    const uint8_t* src_base, const uint64_t* src_off, const uint64_t* src_len, const uint32_t* slice_base,
+    const uint64_t* slice_len, const uint64_t* slice_checksum, uint32_t n_group_keys, uint32_t n_keys,
+    const uint32_t* key_type, const uint32_t* key_len, uint32_t n_aggs, const uint32_t* agg_fn,
+    const uint32_t* val_type, uint32_t n_distinct, const uint32_t* distinct_fn, const uint32_t* distinct_val_type,
+    const int32_t* distinct_column, uint32_t num_partitions, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_off,
+    uint64_t* dst_len, uint64_t* dst_total, uint64_t* checksum_out, int32_t* part_status, uint64_t* counts,
+    int32_t* status, int32_t* bad_slice) {
+  const DistinctFns fns{n_group_keys, n_keys, key_type, key_len, n_aggs, agg_fn, val_type,
+                        n_distinct, distinct_fn, distinct_val_type, distinct_column};
+  return distinct_call(false, dev_index, codec, level, codec_block_size, checksum_alg, n, src_base, src_off, src_len,
+                       slice_base, slice_len, slice_checksum, fns, num_partitions, dst_base, dst_cap, dst_off,
+                       dst_len, dst_total, checksum_out, part_status, counts, status, bad_slice);
+}
+
 static int join_call(uint32_t dev_index, bool packed, uint32_t join_type, uint32_t codec, uint32_t alg,
                      uint32_t n_left, uint32_t n, const uint8_t* src_base, const uint64_t* src_off,
                      const uint64_t* src_len, const uint32_t* slice_base, const uint64_t* slice_len,

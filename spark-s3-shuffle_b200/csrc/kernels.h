@@ -487,6 +487,8 @@ void launch_rows_aggregate(const uint8_t* arena, uint64_t n, uint64_t groups, ui
 // group its first position (n after the last group)
 const uint64_t* rows_group_heads_before(uint8_t* d_aws, uint64_t n);
 const uint32_t* rows_group_starts(uint8_t* d_aws, uint64_t n);
+// per group its head's record length, after launch_rows_group: the merged records' lengths, in output order
+const uint32_t* rows_group_lengths(uint8_t* d_aws, uint64_t n);
 
 // ---------------- partial_agg.cu (a map task's partial aggregation: one partial row per key) ----------------
 // The caller's records ([size: int32 big-endian][row], rec_len each, back to back), sorted by the key columns keys
@@ -498,7 +500,13 @@ const uint32_t* rows_group_starts(uint8_t* d_aws, uint64_t n);
 // staged in 128 bits: wide[k] is its index among the n_dec of them.  dsum: some buffer is a double sum.  A variance
 // buffer (op B2S_AGG_VARIANCE, kStageValue with to_double: the input cast to double, a null skipped) folds into three
 // fields (n, avg, m2); var[k] is its index among the n_var of them.  n_fields: the partial row's buffer fields.
-constexpr uint32_t kStageValue = 0, kStageZero = 1, kStageCount = 2, kStageIsEmpty = 3;
+// Merge entries (merge: some buffer has one; the distinct aggregation's step over merged rows): kStageCountAll stages 1
+// per row with no null bit of the mask voff[k] set (SUM_INT64: count(DISTINCT a, b, ..)); kStageMerge folds a buffer by
+// its mergeExpressions in position order: a SUM_DECIMAL | P << 8 buffer (vtype its decimal(P)) is null once an input is
+// null or the sum reaches 10^P; a VARIANCE buffer reads [n, avg, m2] at voff (staged in vhi words wide[k], wide[k] + 1
+// of n_dec).
+constexpr uint32_t kStageValue = 0, kStageZero = 1, kStageCount = 2, kStageIsEmpty = 3, kStageCountAll = 4,
+                   kStageMerge = 5;
 struct PartialAggSpec {
   KeySpec keys;
   uint32_t n_bufs = 0;
@@ -514,6 +522,8 @@ struct PartialAggSpec {
   uint32_t var[kMaxAggs] = {};
   uint32_t n_var = 0;
   uint32_t n_fields = 0;
+  bool merge = false;
+  uint32_t n_merge_dec = 0, n_merge_var = 0;  // the kStageMerge entries of each kind (pa_merge_chain_kernel's)
 };
 // the check verdict (header word 0) of a record whose value is bad: (i << 3) | kPaBadValue, beside launch_rows_hash's
 // kHashBad* reasons; header word 2 then holds (i << 2) | kPaBadSlot, kPaBadNull or kPaBadDecimal
@@ -537,6 +547,11 @@ void launch_partial_agg_fold(const uint8_t* rec, uint64_t n, const uint32_t* idx
                              cudaStream_t st, uint64_t* launches);
 // per partial row its record length (4 + row), after launch_partial_agg_fold
 const uint32_t* partial_agg_row_len(uint8_t* d_paws, uint64_t n, const PartialAggSpec& spec);
+// per position j < n of records already in the order of a key whose first columns are ks (offsets and lengths in the
+// sort workspace d_ws, as launch_partial_agg_offsets leaves them): heads[j] = 1 where ks's value differs from j - 1's
+// (and at 0), for launch_rows_group
+void launch_partial_agg_heads(const uint8_t* rec, uint64_t n, uint32_t key_bytes, const KeySpec& ks, uint8_t* d_ws,
+                              uint32_t* heads, cudaStream_t st, uint64_t* launches);
 // the groups (count read back) as partial rows, [size: int32 big-endian][row] back to back, to d_dst
 void launch_partial_agg_emit(const uint8_t* rec, uint64_t n, uint64_t groups, const uint32_t* idx, uint32_t key_bytes,
                              const PartialAggSpec& spec, uint8_t* d_ws, uint8_t* d_gws, uint8_t* d_paws,

@@ -22,6 +22,12 @@
 //             output bytes, read back with the group count)
 //   emit    : a warp per partial row, lane f writing field f (n_keys + fields <= 32, so one null word; a variance
 //             buffer is three fields)
+// The distinct aggregation's step (a spec with merge entries, the kernels' Merge instantiations) runs the same steps
+// over a reducer's merged rows, already in the key's order: no sort, the group heads where the key's encoding changes
+// (pa_heads_kernel).  Its merge entries (a decimal sum's or a variance's mergeExpressions) are chains in position
+// order, as the double sums are: a thread per small group, else pa_var_merge_kernel (a chain over shared-memory tiles)
+// or pa_dec_merge_kernel (a CTA's warps scan segments and check every prefix sum); the other merges are the update folds over the
+// buffer, which give the same bits.
 #include <algorithm>
 
 #include "decimal128.h"
@@ -169,8 +175,8 @@ __global__ void __launch_bounds__(kPaThreads) pa_check_kernel(const uint8_t* __r
 
 // buffer k's staged input from a checked row: (lo, hi) and whether it is null (then (0, 0))
 __device__ __forceinline__ bool stage_one(const uint8_t* row, uint32_t size, const PartialAggSpec& s, uint32_t k,
-                                          uint64_t& lo, uint64_t& hi) {
-  const uint32_t vt = s.vtype[k], st = s.stage[k], kind = vkind(vt);
+                                          uint32_t st, uint64_t& lo, uint64_t& hi) {
+  const uint32_t vt = s.vtype[k], kind = vkind(vt);
   const bool null = kind != B2S_WINDOW_VAL_NONE && s.vnull[k] >= 0 && bit_at(row, s.vnull[k]);
   lo = hi = 0;
   if (st == kStageCount) {
@@ -207,6 +213,10 @@ __device__ __forceinline__ bool stage_one(const uint8_t* row, uint32_t size, con
   return false;
 }
 
+// Merge (a spec with merge entries: the distinct aggregation's step over merged rows): kStageCountAll stages 1 when no
+// bit of the mask voff[k] is set in the row's null word; kStageMerge stages a decimal sum buffer as kStageValue does, and
+// a variance buffer's n into vals and its avg and m2 into vhi words wide[k] and wide[k] + 1
+template <bool Merge>
 __global__ void __launch_bounds__(kPaThreads) pa_stage_kernel(const uint8_t* __restrict__ rec,
                                                               const uint64_t* __restrict__ rec_off,
                                                               const uint32_t* __restrict__ rec_len,
@@ -221,7 +231,23 @@ __global__ void __launch_bounds__(kPaThreads) pa_stage_kernel(const uint8_t* __r
     uint32_t nm = 0;
     for (uint32_t k = 0; k < s.n_bufs; k++) {
       uint64_t lo, hi;
-      if (stage_one(row, size, s, k, lo, hi)) nm |= 1u << k;
+      const uint32_t st = s.stage[k];
+      if (Merge && st == kStageCountAll) {
+        uint64_t w, unused;
+        ld_span16<true>(row, 8, w, unused);
+        vals[(size_t)k * n + j] = (w & s.voff[k]) ? 0 : 1;
+        continue;
+      }
+      if (Merge && st == kStageMerge && s.op[k] == B2S_AGG_VARIANCE) {
+        uint64_t cn, avg, m2, unused;
+        ld_span16<true>(row + s.voff[k], 8, cn, unused);
+        ld_span16<true>(row + s.voff[k] + 8, 16, avg, m2);
+        vals[(size_t)k * n + j] = cn;
+        vhi[(size_t)s.wide[k] * n + j] = avg;
+        vhi[(size_t)(s.wide[k] + 1) * n + j] = m2;
+        continue;
+      }
+      if (stage_one(row, size, s, k, Merge && st == kStageMerge ? kStageValue : st, lo, hi)) nm |= 1u << k;
       vals[(size_t)k * n + j] = lo;
       if (agg_decimal_op(s.op[k])) vhi[(size_t)s.wide[k] * n + j] = hi;
     }
@@ -329,6 +355,12 @@ __device__ __forceinline__ bool dsum_op(uint32_t op) { return op == B2S_AGG_SUM_
 // a buffer folded by one chain in position order (pa_chain_kernel's), not by the associative folds
 __device__ __forceinline__ bool chain_op(uint32_t op) { return op == B2S_AGG_SUM_FLOAT64 || op == B2S_AGG_VARIANCE; }
 
+// a buffer the associative folds and the update chains skip: a chain's, or (Merge) a merge entry (pa_var_merge_kernel, pa_dec_merge_kernel)
+template <bool Merge>
+__device__ __forceinline__ bool skips(const PartialAggSpec& s, uint32_t k) {
+  return chain_op(s.op[k]) || (Merge && s.stage[k] == kStageMerge);
+}
+
 __device__ __forceinline__ double dbl(uint64_t b) { return __longlong_as_double((long long)b); }
 __device__ __forceinline__ uint64_t bits(double x) { return (uint64_t)__double_as_longlong(x); }
 
@@ -341,6 +373,27 @@ __device__ __forceinline__ void var_update(double& cn, double& avg, double& m2, 
   avg = __dadd_rn(avg, deltaN);
   m2 = __dadd_rn(m2, __dmul_rn(delta, __dsub_rn(delta, deltaN)));
   cn = newN;
+}
+
+// one mergeExpressions step of CentralMomentAgg (order 2): the group's buffer (cn, avg, m2) merged with (n2, avg2, m2b),
+// every operation one double operation rounded to nearest, in Spark's order
+__device__ __forceinline__ void var_merge(double& cn, double& avg, double& m2, double n2, double avg2, double m2b) {
+  const double newN = __dadd_rn(cn, n2);
+  const double delta = __dsub_rn(avg2, avg);
+  const double deltaN = newN == 0.0 ? 0.0 : __ddiv_rn(delta, newN);
+  const double n1 = cn;
+  avg = __dadd_rn(avg, __dmul_rn(deltaN, n2));
+  m2 = __dadd_rn(__dadd_rn(m2, m2b), __dmul_rn(__dmul_rn(__dmul_rn(delta, deltaN), n1), n2));
+  cn = newN;
+}
+
+// one step of a decimal sum's merge (Sum / Average mergeExpressions into a decimal(P) buffer): a null input, or a sum
+// reaching 10^P, makes the result null for good (*gone)
+__device__ __forceinline__ void dec_merge(Dec128& acc, bool& gone, bool null, Dec128 v, uint32_t P) {
+  if (gone) return;
+  bool ovf = false;
+  acc = dec_add(acc, v, &ovf);
+  gone = null || ovf || !dec_fits(acc, P);
 }
 
 // a variance buffer's fold of group g: n into rlo, avg and m2 into rmom
@@ -363,7 +416,9 @@ __device__ __forceinline__ uint64_t group_of(const uint64_t* __restrict__ hb, ui
   return (j + 1 < n ? hb[j + 1] : G) - 1;
 }
 
-// groups of up to kSmallGroup records: a thread each, every buffer in position order (the chains included)
+// groups of up to kSmallGroup records: a thread each, every buffer in position order (the chains included; Merge:
+// the merge entries' chains too)
+template <bool Merge>
 __global__ void __launch_bounds__(kPaThreads) pa_fold_small_kernel(const uint32_t* __restrict__ gpos,
                                                                    const uint64_t* __restrict__ groups, uint64_t n,
                                                                    const __grid_constant__ PartialAggSpec s,
@@ -381,6 +436,25 @@ __global__ void __launch_bounds__(kPaThreads) pa_fold_small_kernel(const uint32_
     for (uint32_t k = 0; k < s.n_bufs; k++) {
       const uint32_t op = s.op[k];
       PAcc acc{0, 0, 0, 0};
+      if (Merge && s.stage[k] == kStageMerge) {
+        if (op == B2S_AGG_VARIANCE) {
+          double cn = 0.0, avg = 0.0, m2 = 0.0;
+          for (uint32_t j = s0; j < e0; j++)
+            var_merge(cn, avg, m2, dbl(__ldg(vals + (size_t)k * n + j)), dbl(__ldg(vhi + (size_t)s.wide[k] * n + j)),
+                      dbl(__ldg(vhi + (size_t)(s.wide[k] + 1) * n + j)));
+          put_var(s, k, g, n, cn, avg, m2, rlo, rmom);
+        } else {
+          Dec128 sum{0, 0};
+          bool gone = false;
+          for (uint32_t j = s0; j < e0; j++)
+            dec_merge(sum, gone, (__ldg(nulls + j) >> k) & 1,
+                      Dec128{__ldg(vals + (size_t)k * n + j), __ldg(vhi + (size_t)s.wide[k] * n + j)},
+                      agg_precision(op));
+          if (gone) nm |= 1u << k;
+          put_result(s, k, g, n, PAcc{sum.lo, sum.hi, 0, 1}, rlo, rhi);
+        }
+        continue;
+      }
       if (op == B2S_AGG_VARIANCE) {  // never null
         double cn = 0.0, avg = 0.0, m2 = 0.0;
         for (uint32_t j = s0; j < e0; j++)
@@ -406,6 +480,7 @@ __global__ void __launch_bounds__(kPaThreads) pa_fold_small_kernel(const uint32_
 }
 
 // groups of kSmallGroup + 1 .. kChunk records: a warp each (not the chains: pa_chain_kernel)
+template <bool Merge>
 __global__ void __launch_bounds__(kPaThreads) pa_fold_warp_kernel(const uint32_t* __restrict__ gpos,
                                                                   const uint64_t* __restrict__ groups, uint64_t n,
                                                                   const __grid_constant__ PartialAggSpec s,
@@ -421,7 +496,7 @@ __global__ void __launch_bounds__(kPaThreads) pa_fold_warp_kernel(const uint32_t
     if (e0 - s0 <= kSmallGroup || e0 - s0 > kChunk) continue;  // uniform over the warp
     uint32_t nm = 0;
     for (uint32_t k = 0; k < s.n_bufs; k++) {
-      if (chain_op(s.op[k])) continue;
+      if (skips<Merge>(s, k)) continue;
       const PAcc r = fold_warp(s, k, vals, vhi, nulls, n, s0, e0, lane);
       if (!r.has) nm |= 1u << k;
       if (lane == 0) put_result(s, k, g, n, r, rlo, rhi);
@@ -432,6 +507,7 @@ __global__ void __launch_bounds__(kPaThreads) pa_fold_warp_kernel(const uint32_t
 
 // a warp per aligned chunk c of kChunk positions: the large groups (over kChunk records) it meets, at most two: the one
 // holding its first position (partial slot 0) and, if another, the one holding its last (slot 1)
+template <bool Merge>
 __global__ void __launch_bounds__(kPaThreads) pa_fold_chunk_kernel(const uint32_t* __restrict__ gpos,
                                                                    const uint64_t* __restrict__ hb,
                                                                    const uint64_t* __restrict__ groups, uint64_t n,
@@ -452,7 +528,7 @@ __global__ void __launch_bounds__(kPaThreads) pa_fold_chunk_kernel(const uint32_
       if (e0 - s0 <= kChunk) continue;
       const uint32_t a = (uint32_t)std::max<uint64_t>(s0, p0), b = (uint32_t)std::min<uint64_t>(e0, p1);
       for (uint32_t k = 0; k < s.n_bufs; k++) {
-        if (chain_op(s.op[k])) continue;
+        if (skips<Merge>(s, k)) continue;
         const PAcc r = fold_warp(s, k, vals, vhi, nulls, n, a, b, lane);
         if (lane == 0) part[(c * 2 + slot) * s.n_bufs + k] = r;
       }
@@ -461,6 +537,7 @@ __global__ void __launch_bounds__(kPaThreads) pa_fold_chunk_kernel(const uint32_
 }
 
 // a warp per large group: its chunks' partials combined (chunk c holds it in slot 0 when it holds c's first position)
+template <bool Merge>
 __global__ void __launch_bounds__(kPaThreads) pa_fold_combine_kernel(const uint32_t* __restrict__ gpos,
                                                                      const uint64_t* __restrict__ groups, uint64_t n,
                                                                      const __grid_constant__ PartialAggSpec s,
@@ -477,7 +554,7 @@ __global__ void __launch_bounds__(kPaThreads) pa_fold_combine_kernel(const uint3
     uint32_t nm = 0;
     for (uint32_t k = 0; k < s.n_bufs; k++) {
       const uint32_t op = s.op[k];
-      if (chain_op(op)) continue;
+      if (chain_op(op) || (Merge && s.stage[k] == kStageMerge)) continue;
       PAcc acc{0, 0, 0, 0};
       for (uint64_t c = c0 + lane; c <= c1; c += 32) {
         const uint32_t slot = (uint64_t)s0 <= c * kChunk ? 0 : 1;
@@ -495,8 +572,9 @@ __global__ void __launch_bounds__(kPaThreads) pa_fold_combine_kernel(const uint3
 // sums (Var false: the adds, a null staged as +0.0) or the variances (Var true: var_update over the non-null inputs).
 // The warp loads a tile of kTile values (coalesced) into shared memory, with a variance's null bits, and lane 0 runs
 // the chain over them; the next tile's loads are issued before the chain, so they are in flight while it runs.  Runs
-// after the other folds, which wrote rnull[g] without a double sum's bit (a variance is never null).
-template <bool Var>
+// after the other folds, which wrote rnull[g] without a double sum's bit (a variance is never null).  Merge: the merge
+// entries are pa_var_merge_kernel's and pa_dec_merge_kernel's.
+template <bool Var, bool Merge>
 __global__ void __launch_bounds__(kPaThreads) pa_chain_kernel(const uint32_t* __restrict__ gpos,
                                                               const uint64_t* __restrict__ groups, uint64_t n,
                                                               const __grid_constant__ PartialAggSpec s,
@@ -514,7 +592,7 @@ __global__ void __launch_bounds__(kPaThreads) pa_chain_kernel(const uint32_t* __
     if (e0 - s0 <= kSmallGroup) continue;
     uint32_t nm = 0;
     for (uint32_t k = 0; k < s.n_bufs; k++) {
-      if (s.op[k] != (Var ? B2S_AGG_VARIANCE : B2S_AGG_SUM_FLOAT64)) continue;
+      if (s.op[k] != (Var ? B2S_AGG_VARIANCE : B2S_AGG_SUM_FLOAT64) || (Merge && s.stage[k] == kStageMerge)) continue;
       const uint64_t* va = vals + (size_t)k * n;
       double next[kPer];
       uint32_t next_null[kPer];
@@ -564,6 +642,158 @@ __global__ void __launch_bounds__(kPaThreads) pa_chain_kernel(const uint32_t* __
       }
     }
     if (lane == 0 && nm) atomicOr(rnull + g, nm);
+  }
+}
+
+// The variance merge entries (Merge) of the groups over kSmallGroup records, a warp each, as pa_chain_kernel runs the
+// update chains: the warp loads a tile of kMergeTile [n, avg, m2] triples (vals, vhi words wide[k] and wide[k] + 1;
+// coalesced) into shared memory and lane 0 runs CentralMomentAgg's mergeExpressions over them in position order from
+// (0, 0, 0), the next tile's loads in flight meanwhile.
+constexpr uint32_t kMergeTile = 64;
+__global__ void __launch_bounds__(kPaThreads) pa_var_merge_kernel(const uint32_t* __restrict__ gpos,
+                                                                  const uint64_t* __restrict__ groups, uint64_t n,
+                                                                  const __grid_constant__ PartialAggSpec s,
+                                                                  const uint64_t* __restrict__ vals,
+                                                                  const uint64_t* __restrict__ vhi,
+                                                                  uint64_t* __restrict__ rlo,
+                                                                  uint64_t* __restrict__ rmom) {
+  constexpr uint32_t kPer = kMergeTile / 32;
+  __shared__ uint64_t tile[kPaThreads / 32][3][kMergeTile];
+  const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  const uint64_t G = *groups, warps = (uint64_t)gridDim.x * (kPaThreads / 32);
+  for (uint64_t g = (uint64_t)blockIdx.x * (kPaThreads / 32) + wid; g < G; g += warps) {
+    const uint32_t s0 = gpos[g], e0 = gpos[g + 1];
+    if (e0 - s0 <= kSmallGroup) continue;
+    for (uint32_t k = 0; k < s.n_bufs; k++) {
+      if (s.stage[k] != kStageMerge || s.op[k] != B2S_AGG_VARIANCE) continue;
+      const uint64_t *v0 = vals + (size_t)k * n, *v1 = vhi + (size_t)s.wide[k] * n, *v2 = v1 + n;
+      uint64_t next[3][kPer];
+      auto load = [&](uint32_t b) {
+#pragma unroll
+        for (uint32_t r = 0; r < kPer; r++) {
+          const uint32_t j = b + r * 32 + lane;
+          next[0][r] = j < e0 ? __ldg(v0 + j) : 0;
+          next[1][r] = j < e0 ? __ldg(v1 + j) : 0;
+          next[2][r] = j < e0 ? __ldg(v2 + j) : 0;
+        }
+      };
+      load(s0);
+      double cn = 0.0, avg = 0.0, m2 = 0.0;
+      for (uint32_t b = s0; b < e0; b += kMergeTile) {
+#pragma unroll
+        for (uint32_t r = 0; r < kPer; r++)
+#pragma unroll
+          for (uint32_t w = 0; w < 3; w++) tile[wid][w][r * 32 + lane] = next[w][r];
+        __syncwarp();
+        if (b + kMergeTile < e0) load(b + kMergeTile);
+        if (lane == 0) {
+          const uint32_t m = min(kMergeTile, e0 - b);
+          for (uint32_t t = 0; t < m; t++)
+            var_merge(cn, avg, m2, dbl(tile[wid][0][t]), dbl(tile[wid][1][t]), dbl(tile[wid][2][t]));
+        }
+        __syncwarp();
+      }
+      if (lane == 0) put_var(s, k, g, n, cn, avg, m2, rlo, rmom);
+    }
+  }
+}
+
+// a + b of 128-bit two's-complement words (mod 2^128)
+__device__ __forceinline__ Dec128 add128(Dec128 a, Dec128 b) {
+  Dec128 r;
+  r.lo = a.lo + b.lo;
+  r.hi = a.hi + b.hi + (r.lo < a.lo ? 1 : 0);
+  return r;
+}
+
+// The decimal sum merge entries (Merge) of the groups over kSmallGroup records, a CTA each.  The sequential merge
+// (dec_merge: null once an input is null or a running sum reaches 10^P) is null exactly when some input is null or some
+// prefix sum is out of range, so the prefixes are checked in parallel: each warp sums its segment of the group, the
+// segment sums give each warp the sum before its segment, and each warp then scans its segment 32 positions a round
+// (an inclusive 128-bit warp scan on top of the sum so far) and checks every prefix.  Prefixes are taken mod 2^128:
+// every input is below 10^P in magnitude (the read's merge nulls larger sums) and so is every prefix before the first
+// bad one, so that one is below 2 * 10^38 and still at least 10^38 in magnitude once wrapped, and it is found; with no
+// bad prefix every wrapped prefix is the true one.  Its null bit is ORed in.
+__global__ void __launch_bounds__(kPaThreads) pa_dec_merge_kernel(const uint32_t* __restrict__ gpos,
+                                                                  const uint64_t* __restrict__ groups, uint64_t n,
+                                                                  const __grid_constant__ PartialAggSpec s,
+                                                                  const uint64_t* __restrict__ vals,
+                                                                  const uint64_t* __restrict__ vhi,
+                                                                  const uint32_t* __restrict__ nulls,
+                                                                  uint64_t* __restrict__ rlo, uint64_t* __restrict__ rhi,
+                                                                  uint32_t* __restrict__ rnull) {
+  constexpr uint32_t kWarps = kPaThreads / 32;
+  __shared__ uint64_t seg_lo[kWarps], seg_hi[kWarps];
+  __shared__ uint32_t bad[kWarps];
+  const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  const uint64_t G = *groups;
+  for (uint64_t g = blockIdx.x; g < G; g += gridDim.x) {
+    const uint32_t s0 = gpos[g], e0 = gpos[g + 1];
+    if (e0 - s0 <= kSmallGroup) continue;  // uniform over the CTA
+    const uint32_t L = ((e0 - s0 + kWarps - 1) / kWarps + 31) / 32 * 32;
+    const uint32_t a = min(e0, s0 + wid * L), b = min(e0, a + L);
+    uint32_t nm = 0;
+    for (uint32_t k = 0; k < s.n_bufs; k++) {
+      if (s.stage[k] != kStageMerge || agg_base_op(s.op[k]) != B2S_AGG_SUM_DECIMAL) continue;
+      const uint64_t *v0 = vals + (size_t)k * n, *v1 = vhi + (size_t)s.wide[k] * n;
+      const uint32_t P = agg_precision(s.op[k]);
+      // pass 1: the segment's sum
+      Dec128 part{0, 0};
+      for (uint32_t j = a + lane; j < b; j += 32) part = add128(part, Dec128{__ldg(v0 + j), __ldg(v1 + j)});
+#pragma unroll
+      for (int d = 16; d; d >>= 1)
+        part = add128(part, Dec128{__shfl_xor_sync(FULL, part.lo, d), __shfl_xor_sync(FULL, part.hi, d)});
+      if (lane == 0) {
+        seg_lo[wid] = part.lo;
+        seg_hi[wid] = part.hi;
+      }
+      __syncthreads();
+      Dec128 sum{0, 0}, total{0, 0};
+      for (uint32_t w = 0; w < kWarps; w++) {
+        if (w == wid) sum = total;
+        total = add128(total, Dec128{seg_lo[w], seg_hi[w]});
+      }
+      // pass 2: every prefix of the segment, on top of the sum before it
+      bool gone = false;
+      for (uint32_t c = a; c < b && !gone; c += 32) {
+        const uint32_t j = c + lane;
+        const bool in = j < b;
+        const bool null = in && ((__ldg(nulls + j) >> k) & 1);
+        Dec128 x{in && !null ? __ldg(v0 + j) : 0, in && !null ? __ldg(v1 + j) : 0};
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+          const Dec128 y{__shfl_up_sync(FULL, x.lo, d), __shfl_up_sync(FULL, x.hi, d)};
+          if (lane >= (uint32_t)d) x = add128(x, y);
+        }
+        x = add128(sum, x);
+        gone = __any_sync(FULL, in && (null || !dec_fits(x, P)));
+        sum = Dec128{__shfl_sync(FULL, x.lo, 31), __shfl_sync(FULL, x.hi, 31)};
+      }
+      if (lane == 0) bad[wid] = gone;
+      __syncthreads();
+      bool any = false;
+      for (uint32_t w = 0; w < kWarps; w++) any |= bad[w] != 0;
+      if (any) nm |= 1u << k;
+      if (threadIdx.x == 0) put_result(s, k, g, n, PAcc{total.lo, total.hi, 0, 1}, rlo, rhi);
+      __syncthreads();  // the shared words are reused by the next entry
+    }
+    if (threadIdx.x == 0 && nm) atomicOr(rnull + g, nm);
+  }
+}
+
+// Position j of the merged rows (in their key order) starts a group of the key columns ks (a prefix of the order's
+// columns): j == 0, or its encoded key differs from j - 1's (encoded_keys_equal, as the window's partition heads
+// compare theirs; the read's key pass has checked every string and decimal).  No key columns: only position 0.
+__global__ void __launch_bounds__(kPaThreads) pa_heads_kernel(const uint8_t* __restrict__ rec,
+                                                              const uint64_t* __restrict__ rec_off,
+                                                              const uint32_t* __restrict__ rec_len, uint64_t n,
+                                                              const __grid_constant__ KeySpec ks,
+                                                              uint32_t* __restrict__ heads) {
+  for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (uint64_t)gridDim.x * blockDim.x) {
+    uint32_t h = j == 0;
+    if (j && ks.n)
+      h = !encoded_keys_equal(rec + rec_off[j] + 4, rec_len[j] - 4, rec + rec_off[j - 1] + 4, rec_len[j - 1] - 4, ks);
+    heads[j] = h;
   }
 }
 
@@ -720,6 +950,48 @@ __global__ void __launch_bounds__(kPaThreads) pa_emit_kernel(const uint8_t* __re
   }
 }
 
+// the staging, the folds and the chains of launch_partial_agg_fold (Merge: a spec with merge entries)
+template <bool Merge>
+void launch_fold(const uint8_t* rec, uint64_t n, const uint32_t* idx, const KeySortWs& w, const PaWs& a,
+                 const uint32_t* gpos, const uint64_t* hb, const uint64_t* groups, const PartialAggSpec& spec,
+                 cudaStream_t st, uint64_t* launches) {
+  pa_stage_kernel<Merge><<<grid_for(n), kPaThreads, 0, st>>>(rec, w.src_off, w.len, idx, n, spec, a.vals, a.vhi,
+                                                             a.nulls);
+  pa_fold_small_kernel<Merge><<<grid_for(n), kPaThreads, 0, st>>>(gpos, groups, n, spec, a.vals, a.vhi, a.nulls, a.rlo,
+                                                                  a.rhi, a.rnull, a.rmom);
+  const unsigned wg = warp_grid_for(n / kSmallGroup + 1);
+  pa_fold_warp_kernel<Merge><<<wg, kPaThreads, 0, st>>>(gpos, groups, n, spec, a.vals, a.vhi, a.nulls, a.rlo, a.rhi,
+                                                        a.rnull);
+  uint32_t launched = 3;
+  if (n > kChunk) {
+    pa_fold_chunk_kernel<Merge><<<warp_grid_for(n_chunks(n)), kPaThreads, 0, st>>>(gpos, hb, groups, n, spec, a.vals,
+                                                                                   a.vhi, a.nulls, a.part);
+    pa_fold_combine_kernel<Merge><<<warp_grid_for(n / kChunk + 1), kPaThreads, 0, st>>>(gpos, groups, n, spec, a.part,
+                                                                                        a.rlo, a.rhi, a.rnull);
+    launched += 2;
+  }
+  if (spec.dsum) {
+    pa_chain_kernel<false, Merge><<<wg, kPaThreads, 0, st>>>(gpos, groups, n, spec, a.vals, a.nulls, a.rlo, a.rnull,
+                                                             a.rmom);
+    launched++;
+  }
+  if (spec.n_var) {
+    pa_chain_kernel<true, Merge><<<wg, kPaThreads, 0, st>>>(gpos, groups, n, spec, a.vals, a.nulls, a.rlo, a.rnull,
+                                                            a.rmom);
+    launched++;
+  }
+  if (Merge && spec.n_merge_var) {
+    pa_var_merge_kernel<<<wg, kPaThreads, 0, st>>>(gpos, groups, n, spec, a.vals, a.vhi, a.rlo, a.rmom);
+    launched++;
+  }
+  if (Merge && spec.n_merge_dec) {
+    pa_dec_merge_kernel<<<grid_for(n), kPaThreads, 0, st>>>(gpos, groups, n, spec, a.vals, a.vhi, a.nulls, a.rlo,
+                                                            a.rhi, a.rnull);
+    launched++;
+  }
+  if (launches) *launches += launched;
+}
+
 }  // namespace
 
 size_t partial_agg_ws_bytes(uint64_t n, const PartialAggSpec& s) {
@@ -766,29 +1038,8 @@ void launch_partial_agg_fold(const uint8_t* rec, uint64_t n, const uint32_t* idx
   const uint64_t* hb = rows_group_heads_before(d_gws, n);
   cudaMemcpyAsync(a.hdr + 4, groups, 8, cudaMemcpyDeviceToDevice, st);
   if (spec.n_bufs) {
-    pa_stage_kernel<<<grid_for(n), kPaThreads, 0, st>>>(rec, w.src_off, w.len, idx, n, spec, a.vals, a.vhi, a.nulls);
-    pa_fold_small_kernel<<<grid_for(n), kPaThreads, 0, st>>>(gpos, groups, n, spec, a.vals, a.vhi, a.nulls, a.rlo,
-                                                              a.rhi, a.rnull, a.rmom);
-    const unsigned wg = warp_grid_for(n / kSmallGroup + 1);
-    pa_fold_warp_kernel<<<wg, kPaThreads, 0, st>>>(gpos, groups, n, spec, a.vals, a.vhi, a.nulls, a.rlo, a.rhi,
-                                                   a.rnull);
-    uint32_t launched = 3;
-    if (n > kChunk) {
-      pa_fold_chunk_kernel<<<warp_grid_for(n_chunks(n)), kPaThreads, 0, st>>>(gpos, hb, groups, n, spec, a.vals,
-                                                                              a.vhi, a.nulls, a.part);
-      pa_fold_combine_kernel<<<warp_grid_for(n / kChunk + 1), kPaThreads, 0, st>>>(gpos, groups, n, spec, a.part,
-                                                                                   a.rlo, a.rhi, a.rnull);
-      launched += 2;
-    }
-    if (spec.dsum) {
-      pa_chain_kernel<false><<<wg, kPaThreads, 0, st>>>(gpos, groups, n, spec, a.vals, a.nulls, a.rlo, a.rnull, a.rmom);
-      launched++;
-    }
-    if (spec.n_var) {
-      pa_chain_kernel<true><<<wg, kPaThreads, 0, st>>>(gpos, groups, n, spec, a.vals, a.nulls, a.rlo, a.rnull, a.rmom);
-      launched++;
-    }
-    if (launches) *launches += launched;
+    if (spec.merge) launch_fold<true>(rec, n, idx, w, a, gpos, hb, groups, spec, st, launches);
+    else launch_fold<false>(rec, n, idx, w, a, gpos, hb, groups, spec, st, launches);
   }
   pa_size_kernel<<<grid_for(n), kPaThreads, 0, st>>>(rec, w.src_off, idx, gpos, groups, n, spec, a.rowlen, a.rowoff);
   launch_exclusive_scan_u64(a.rowoff, n, a.hdr + 5, a.scan_ws, st, launches);
@@ -808,6 +1059,14 @@ void launch_partial_agg_emit(const uint8_t* rec, uint64_t n, uint64_t groups, co
   pa_emit_kernel<<<warp_grid_for(groups), kPaThreads, 0, st>>>(rec, w.src_off, w.len, idx, rows_group_starts(d_gws, n),
                                                               groups, n, spec, a.rlo, a.rhi, a.rnull, a.rmom,
                                                               a.rowlen, a.rowoff, d_dst);
+  if (launches) *launches += 1;
+}
+
+void launch_partial_agg_heads(const uint8_t* rec, uint64_t n, uint32_t key_bytes, const KeySpec& ks, uint8_t* d_ws,
+                              uint32_t* heads, cudaStream_t st, uint64_t* launches) {
+  if (!n) return;
+  const KeySortWs w = carve_key_sort_ws(d_ws, n, key_bytes);
+  pa_heads_kernel<<<grid_for(n), kPaThreads, 0, st>>>(rec, w.src_off, w.len, n, ks, heads);
   if (launches) *launches += 1;
 }
 

@@ -139,4 +139,18 @@ __device__ __forceinline__ uint32_t encode_key(const uint8_t* row, uint32_t row_
   return p;
 }
 
+// Two rows' keys ks are equal: their encodings compared kKeyChunkBytes at a time.  Equal so far and one key ended inside
+// the window: the encoding is prefix-free, so both did.  For keys whose strings and decimals have been checked.
+__device__ __forceinline__ bool encoded_keys_equal(const uint8_t* ra, uint32_t sa, const uint8_t* rb, uint32_t sb,
+                                                   const KeySpec& ks) {
+  bool bad = false;
+  for (uint32_t d = 0;; d += kKeyChunkBytes) {
+    KeyWindow wa{0, 0, 0, 0, 0, d, kKeyChunkBytes}, wb{0, 0, 0, 0, 0, d, kKeyChunkBytes};
+    const uint32_t la = encode_key(ra, sa, ks, wa, false, &bad);
+    const uint32_t lb = encode_key(rb, sb, ks, wb, false, &bad);
+    if (wa.w0 != wb.w0 || wa.w1 != wb.w1 || wa.w2 != wb.w2 || wa.w3 != wb.w3) return false;
+    if (min(la, lb) < d + kKeyChunkBytes) return true;
+  }
+}
+
 }  // namespace b2s

@@ -157,20 +157,8 @@ __global__ void __launch_bounds__(kWindowThreads) window_part_heads_kernel(
     uint64_t h = j == 0;
     if (j && ks.n && next_scanned(heads_before, j, n, G) != heads_before[j]) {
       const uint32_t a = at(idx, j), b = at(idx, j - 1);
-      const uint8_t *ra = arena + rec_off[a] + 4, *rb = arena + rec_off[b] + 4;
-      const uint32_t sa = rec_len[a] - 4, sb = rec_len[b] - 4;
-      bool bad = false;  // the sort's key pass has checked every string and decimal
-      for (uint32_t d = 0;; d += kKeyChunkBytes) {
-        KeyWindow wa{0, 0, 0, 0, 0, d, kKeyChunkBytes}, wb{0, 0, 0, 0, 0, d, kKeyChunkBytes};
-        const uint32_t la = encode_key(ra, sa, ks, wa, false, &bad);
-        const uint32_t lb = encode_key(rb, sb, ks, wb, false, &bad);
-        if (wa.w0 != wb.w0 || wa.w1 != wb.w1 || wa.w2 != wb.w2 || wa.w3 != wb.w3) {
-          h = 1;
-          break;
-        }
-        // equal so far and one key ended inside the window: the encoding is prefix-free, so both did
-        if (min(la, lb) < d + kKeyChunkBytes) break;
-      }
+      // the sort's key pass has checked every string and decimal
+      h = !encoded_keys_equal(arena + rec_off[a] + 4, rec_len[a] - 4, arena + rec_off[b] + 4, rec_len[b] - 4, ks);
     }
     phead[j] = h;
   }

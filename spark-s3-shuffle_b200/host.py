@@ -76,6 +76,8 @@ PROTOTYPES = [
     ("b2sh_reader_read_joined_rows", C.c_int,
      [_vp, _vp, _u32, _u32, _vp, _vp, _vp, _vp, _vp, _vp, _u32, _vp, _u32, _vp, C.POINTER(_vp), C.POINTER(_u64),
       C.POINTER(_u64), C.POINTER(_u64), C.POINTER(_u64)]),
+    ("b2sh_reader_aggregate_distinct_rows", C.c_int,
+     [_vp, _vp, _u32, _u32, _vp, _vp, _u32, _vp, _vp, _u32, _vp, _vp, _vp, _vp, _vp]),
     ("b2sh_reader_read_window_rows", C.c_int,
      [_vp, _u32, _u32, _vp, _vp, _vp, _vp, _u32, _vp, _u32, _vp, _vp, _u32, _i32, C.POINTER(_vp), C.POINTER(_u64),
       C.POINTER(_u64), C.POINTER(_u64)]),
@@ -456,6 +458,26 @@ class S3ShuffleReader:
                                                    nLeftFields, _arg(lk), nRightFields, _arg(rk), C.byref(p),
                                                    C.byref(size), *map(C.byref, counts)))
         return ((C.string_at(p.value, size.value) if size.value else b""),) + tuple(c.value for c in counts)
+
+    def aggregateDistinctRows(self, writer, nGroupKeys, keys, aggs, distinctAggs):
+        """One DISTINCT group's middle stage: this reader's blocks of the exchange by G ++ X (keys = [(key_type,
+        key_len), ...], the first nGroupKeys G; the map side's partial rows for functions aggs = [(fn, val_type), ...])
+        merged per (G, X), folded per G (aggs merged, distinctAggs = [(fn, val_type, column or
+        capi.DISTINCT_ALL_COLUMNS), ...] updated) and partitioned by G into writer, a S3SerializedShuffleWriter of the
+        exchange by G with no partitioning and no records, which commits its files.
+        -> (partitionLengths, [input rows, (G, X) groups, rows written])"""
+        arr = lambda vals, t: np.array(list(vals) or [0], dtype=t)  # noqa: E731
+        kt, kl = arr((k[0] for k in keys), np.uint32), arr((k[1] for k in keys), np.uint32)
+        fn, vt = arr((a[0] for a in aggs), np.uint32), arr((a[1] for a in aggs), np.uint32)
+        dfn, dvt = arr((a[0] for a in distinctAggs), np.uint32), arr((a[1] for a in distinctAggs), np.uint32)
+        dcol = arr((a[2] for a in distinctAggs), np.int32)
+        lengths = np.zeros(writer.numPartitions, dtype=np.int64)
+        counts = np.zeros(3, dtype=np.uint64)
+        _check(load().b2sh_reader_aggregate_distinct_rows(
+            self._h, writer._h, nGroupKeys, len(keys), kt.ctypes.data, kl.ctypes.data, len(aggs), fn.ctypes.data,
+            vt.ctypes.data, len(distinctAggs), dfn.ctypes.data, dvt.ctypes.data, dcol.ctypes.data, lengths.ctypes.data,
+            counts.ctypes.data))
+        return lengths, [int(c) for c in counts]
 
     def readWindowRows(self, keys, nPartitionKeys, nFields, kinds, fns, limit=None):
         """Spark's ranking window over this reader's partitions: its blocks through ONE

@@ -705,6 +705,35 @@ class S3SerializedShuffleWriter {
     return lengths;
   }
   const S3MeasureOutputStream* measure() const { return measure_.get(); }
+  int32_t numPartitions() const { return numPartitions_; }
+  // Commits a .data arena that another call writes in this writer's place (a reduce task that ends in this map
+  // output, S3ShuffleReader::aggregateDistinctRows): partition(dst, cap, dst_off, dst_len, &total, checksums, status)
+  // fills it like b2s_partition_compress_packed, retried once with the exact size on B2S_E_DST_TOO_SMALL; check() runs
+  // after the call and throws to leave no files; then .data / .index / .checksum are written as commit() writes them.
+  template <class Partition, class Check>
+  std::vector<int64_t> commitFrom(const char* call, uint64_t guess, Partition&& partition, Check&& check) {
+    if (!recLen_.empty() || !keyType_.empty() || roundRobin_)
+      throw RuntimeException("Precondition: a writer committed by a reader takes no rows and no partitioning.");
+    const uint32_t R = (uint32_t)numPartitions_;
+    std::vector<uint64_t> doff(R), dlen(R), cks(R);
+    std::vector<int32_t> status(R);
+    uint64_t total = 0;
+    int rc = B2S_E_DST_TOO_SMALL;
+    for (int attempt = 0; attempt < 2 && rc == B2S_E_DST_TOO_SMALL; attempt++) {
+      out_.resize(attempt ? (total ? total : 1) : (guess ? guess : 1));
+      rc = partition(out_.data(), (uint64_t)out_.size(), doff.data(), dlen.data(), &total, cks.data(), status.data());
+    }
+    if (rc != 0) throw CodecException(std::string(call) + ": " + b2s_strerror(rc) + ": " + b2s_last_error());
+    check();
+    std::vector<int64_t> lengths(R), checksums(R);
+    for (uint32_t p = 0; p < R; p++) {
+      if (status[p] != 0) throw IOException(std::string("compress failed: ") + b2s_strerror(status[p]));
+      lengths[p] = (int64_t)dlen[p];
+      checksums[p] = (int64_t)cks[p];
+    }
+    writeMapOutput(d_, shuffleId_, mapId_, true, {{out_.data(), total}}, total, lengths, checksums, measure_);
+    return lengths;
+  }
 
  private:
   S3ShuffleDispatcher& d_;
@@ -1261,6 +1290,50 @@ class S3ShuffleReader {
     sortedLen_ = total;
     sortedRecords_ = out;
   }
+  // One DISTINCT group's middle stage (b2s_decompress_aggregate_distinct_partition_compress_rows_hash_packed): the key
+  // columns G ++ X (the first nGroupKeys G), F as (fn, valType), D as (fn, valType, column).
+  struct DistinctArgs {
+    uint32_t nGroupKeys, nKeys;
+    const uint32_t *keyType, *keyLen;
+    uint32_t nAggs;
+    const uint32_t *aggFn, *valType;
+    uint32_t nDistinct;
+    const uint32_t *distinctFn, *distinctValType;
+    const int32_t* distinctColumn;
+  };
+  // A reduce task of the exchange by G ++ X that ends in the map output of the exchange by G (INTEGRATION.md §3s):
+  // every non-empty block is fetched (the exchange cache is not consulted) in computeShuffleBlocks order, then ONE call
+  // merges, folds and hash-partitions the rows into `out`'s arena, whose map id is this reduce task and whose
+  // numPartitions the second exchange's; `out` then commits its .data / .index / .checksum as its own commit() lays
+  // them out.  A corrupt block throws as the other reads do, and no file is written.  counts: the call's three.
+  std::vector<int64_t> aggregateDistinctRows(S3SerializedShuffleWriter& out, const DistinctArgs& a, uint64_t* counts) {
+    std::vector<FetchedBlock> fetched;
+    fetchAll(fetched);
+    std::vector<const FetchedBlock*> sources;
+    for (const auto& f : fetched)
+      if (!f.second.empty()) sources.push_back(&f);
+    const uint32_t alg = d_.checksumEnabled ? S3ShuffleHelper::createChecksumAlgorithm(d_.checksumAlgorithm) : 0;
+    ensure_codec_runtime();
+    const uint32_t codec = (uint32_t)d_.codecId();
+    StagedBlocks src(info_, sources);
+    const uint32_t n = (uint32_t)sources.size(), R = (uint32_t)out.numPartitions();
+    std::vector<int32_t> status(n ? n : 1), bad(n ? n : 1);
+    // the output rows are at most the input's size plus a partial row per group; the exact size is reported if not
+    const uint64_t guess = b2s_partition_compress_bound(codec, d_.lz4BlockSize, R, (src.bytes + 4096) * 4);
+    return out.commitFrom(
+        "b2s_decompress_aggregate_distinct_partition_compress_rows_hash_packed", guess,
+        [&](uint8_t* dst, uint64_t cap, uint64_t* doff, uint64_t* dlen, uint64_t* total, uint64_t* cks, int32_t* st) {
+          return b2s_decompress_aggregate_distinct_partition_compress_rows_hash_packed(
+              codec, d_.zstdLevel, d_.lz4BlockSize, alg, n, n ? src.src.data() : nullptr, src.off.data(),
+              src.len.data(), alg ? src.sliceBase.data() : 0, alg ? src.sliceLen.data() : 0,
+              alg ? src.sliceSum.data() : 0, a.nGroupKeys, a.nKeys, a.keyType, a.keyLen, a.nAggs, a.aggFn, a.valType,
+              a.nDistinct, a.distinctFn, a.distinctValType, a.distinctColumn, R, dst, cap, doff, dlen, total, cks, st,
+              counts, status.data(), bad.data());
+        },
+        [&] {
+          for (uint32_t k = 0; k < n; k++) throwBlockStatus(status[k], info_[sources[k]->first].id);
+        });
+  }
   // every block of the task, fetched whole, in computeShuffleBlocks order
   void fetchAll(std::vector<FetchedBlock>& fetched) {
     start(true);
@@ -1803,6 +1876,20 @@ int b2sh_reader_read_window_frame_rows(b2sh_reader* r, uint32_t n_partition_keys
     w.frames = true;
     r->r->readWindowRows(w, n_records);
     sorted_result(*r->r, data, len, n_out_records);
+  });
+}
+int b2sh_reader_aggregate_distinct_rows(b2sh_reader* r, b2sh_serialized_writer* w, uint32_t n_group_keys,
+                                        uint32_t n_keys, const uint32_t* key_type, const uint32_t* key_len,
+                                        uint32_t n_aggs, const uint32_t* agg_fn, const uint32_t* val_type,
+                                        uint32_t n_distinct, const uint32_t* distinct_fn,
+                                        const uint32_t* distinct_val_type, const int32_t* distinct_column,
+                                        int64_t* partition_lengths_out, uint64_t* counts) {
+  return guarded([&] {
+    if (!w || !partition_lengths_out || !counts) throw RuntimeException("Precondition: null argument.");
+    const S3ShuffleReader::DistinctArgs a{n_group_keys, n_keys, key_type, key_len, n_aggs, agg_fn, val_type,
+                                          n_distinct, distinct_fn, distinct_val_type, distinct_column};
+    const std::vector<int64_t> lengths = r->r->aggregateDistinctRows(*w->w, a, counts);
+    std::copy(lengths.begin(), lengths.end(), partition_lengths_out);
   });
 }
 int b2sh_reader_block(b2sh_reader* r, uint32_t k, int64_t* map_id, int32_t* start_reduce, int32_t* end_reduce,
