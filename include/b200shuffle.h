@@ -71,6 +71,13 @@ extern "C" {
  * accepted and changes nothing) */
 #define B2S_KEY_DESCENDING (1u << 8)
 #define B2S_KEY_NULLS_LAST (1u << 9)
+/* a null-safe (<=>) key column, OR-ed into key_type: Spark's ExtractEquiJoinKeys expands l <=> r into the key pairs
+ * (Coalesce(l, Literal.default(t)), Coalesce(r, ...)) and (IsNull(l), IsNull(r)), so the column is the pair
+ * (coalesce(v, default), isnull(v)): default 0 for numbers, dates and timestamps, 0 for decimals (a wide one as
+ * BigInteger.ZERO.toByteArray(), the one byte 0x00), empty for strings and binary, false for booleans.  Accepted only by
+ * the join calls (b2s_decompress_join_rows_keys_*) and the hash calls (b2s_partition_compress_rows_hash_*, their cached
+ * form included); every other call that takes key types returns B2S_E_ARG for it. */
+#define B2S_KEY_NULL_SAFE (1u << 10)
 
 /* aggregate ops of the row aggregation (b2s_decompress_aggregate_rows_*), each over an 8-byte slot of the row */
 #define B2S_AGG_SUM_INT64 0   /* wrapping two's-complement sum: Sum(long), Count, Average's count */
@@ -211,6 +218,9 @@ int b2s_partition_compress_dev(uint32_t dev_index, uint32_t codec, int32_t level
  * The key columns are given as to the composite-key calls (b2s_decompress_*_rows_keys_*, below): n_keys (1..16),
  * key_type[c] at row offset key_off[c], key_len[c] bytes, null bit key_null_field[c] (-1: never null).  Starting from
  * h = 42, each column left to right sets h = its hash with seed h; a null column leaves h as it is (all null: 42).
+ * A B2S_KEY_NULL_SAFE column takes two steps, as HashPartitioning over its expanded key pair does: h = the hash of its
+ * value by its type's rule below, of the type's default when the column is null (so a null changes h), then
+ * h = hashInt(isnull ? 1 : 0).  A column without a null bit (-1) is never null: its second step is hashInt(0).
  *   B2S_KEY_BYTES, key_len 1 (BooleanType): hashInt(byte != 0 ? 1 : 0)
  *   B2S_KEY_INT8 / B2S_KEY_INT16 / B2S_KEY_INT32 (ByteType, ShortType, IntegerType, DateType): hashInt of the value
  *   B2S_KEY_INT64 (LongType, TimestampType, Decimal(p <= 18)): hashLong
@@ -220,7 +230,8 @@ int b2s_partition_compress_dev(uint32_t dev_index, uint32_t codec, int32_t level
  *     slot's bytes, with Spark's tail (every byte after the last whole 4-byte word mixed on its own, sign-extended)
  * Outputs: byte for byte what b2s_partition_compress_packed / _dev return for the same records and those ids.
  * Errors, B2S_E_ARG: what b2s_partition_compress_* rejects; n_keys outside 1..16, a type not listed, a key_len that does
- * not match its type, an order flag, key_null_field < -1.  A bad record -> B2S_E_ARG, nothing reported as written, and
+ * not match its type, an order flag (B2S_KEY_NULL_SAFE is not one), key_null_field < -1.  A bad record -> B2S_E_ARG,
+ * nothing reported as written, and
  * b2s_last_error() names the lowest bad record and why: rec_len < 4, a size prefix other than rec_len - 4, a row that
  * does not hold a key slot or a key's null word, a non-null string past the row, a non-null decimal whose size is not
  * 1..16 or that runs past the row.  No usable device -> B2S_E_CUDA.  b2s_last_timing as for the partition calls, plus
@@ -861,6 +872,10 @@ int b2s_decompress_aggregate_rows_keys_dev(uint32_t dev_index, uint32_t codec, u
  * sides and the values are equal by the composite-key aggregation's grouping rule (strings by length and bytes, 0.0
  * equal to -0.0, every NaN equal to every other NaN: Spark's NormalizeFloatingNumbers).  A key with a null column
  * matches nothing.
+ * Null-safe columns.  A column whose key_type has B2S_KEY_NULL_SAFE (l <=> r) compares and orders as the pair
+ * (coalesce(v, default), isnull(v)), both ascending: a null equals a null and sorts directly after the non-null default
+ * value, and it does not make the key unmatchable; only a null in a plain column does.  A side whose null field is -1
+ * has isnull false.  Either side's pair form (Spark folds a non-nullable side's pair to (col, false)) is this one.
  * Order.  Ls: the left records stably sorted by the key (ascending, nulls first, ties in block order, then in their
  * order in the block); Rs: the right records sorted the same way.
  *   B2S_JOIN_INNER: for each l of Ls, for each r of Rs whose key equals l's, in Rs order: join(l, r).
@@ -876,7 +891,13 @@ int b2s_decompress_aggregate_rows_keys_dev(uint32_t dev_index, uint32_t codec, u
  *     first each left record l in Ls order: join(l, r) for each right record r of the run in Rs order if the run
  *     matches, else join(l, null); then, if the run does not match, each right record r in Rs order: join(null, r).
  *     Spark declares no outputOrdering for a full outer sort-merge join; this order makes the output deterministic,
- *     and without null keys it is the order of Spark's full outer scanner.
+ *     and without null keys it is the order of Spark's full outer scanner.  A run matches when its key has no null in a
+ *     plain column and it holds records of both sides.
+ *   B2S_JOIN_EXISTENCE: for each l of Ls, once: l joined with one non-null boolean field, 1 when l has a match, else 0
+ *     (SortMergeJoinExec(ExistenceJoin(exists)), whose output is left.output :+ exists).  The row is the window call's
+ *     output row with one value: b = ceil((nL + 1) / 64) null words holding the left's bits and zeros above them, the
+ *     left slots, the boolean slot (8 bytes, 0 or 1), the left var bytes; every VAR or DECIMAL_WIDE slot that is not
+ *     zero has its offset moved by 8 (b - bL + 1).  *n_out_records = the left record count.
  * Joined row: UnsafeRowJoiner's, which is UnsafeProjection(left.output ++ right.output) when each input's
  * variable-length data is laid out as UnsafeProjection writes it.  nL, nR: the sides' field counts (n_left_fields,
  * n_right_fields); bL, bR, b: the null-bitset words of the left row, the right row and the output, ceil(nL / 64),
@@ -893,11 +914,12 @@ int b2s_decompress_aggregate_rows_keys_dev(uint32_t dev_index, uint32_t codec, u
  * right side's offsets move by 8 (b - bR + nL) + varL as above.  A joined row never has both sides null.
  * Outputs.  [size BE][row] records, an UnsafeRowSerializer stream, *n_out_records of them, *dst_total bytes; dst_cap
  * below that -> B2S_E_DST_TOO_SMALL with *dst_total = the bytes needed.  *n_left_records / *n_right_records: the input
- * record counts.  The field-kind arrays (B2S_FIELD_*, one per field) may be NULL for semi and anti joins.
- * Errors -> B2S_E_ARG: an unknown join_type; n_left > n; a key column the composite-key calls reject, or any order
- * flag; a key slot outside its side's slots [8 bX, 8 (bX + nX)) or a null bit not below its side's field count; a field
- * count outside 1..65536; NULL or unknown field kinds for every type but semi and anti; more than 2^32 - 1 input
- * records.
+ * record counts.  The field-kind arrays (B2S_FIELD_*, one per field) may be NULL for semi and anti joins, and the right
+ * one for the existence join.
+ * Errors -> B2S_E_ARG: an unknown join_type; n_left > n; a key column the composite-key calls reject (B2S_KEY_NULL_SAFE
+ * aside), or any order flag; a key slot outside its side's slots [8 bX, 8 (bX + nX)) or a null bit not below its side's field count; a field
+ * count outside 1..65536; NULL or unknown field kinds for every type but semi and anti (the existence join: the left
+ * side's); more than 2^32 - 1 input records.
  * Per block, B2S_E_CORRUPT for every framing rule of the composite-key calls with that block's side's key columns, and
  * when a row is shorter than its side's fixed region 8 (bX + nX); b2s_last_error() names the block and the byte offset
  * of the bad record.  A joined row longer than 2^31 - 1 bytes -> B2S_E_UNSUPPORTED.  Checksums and bad_slice as in the
@@ -913,6 +935,8 @@ int b2s_decompress_aggregate_rows_keys_dev(uint32_t dev_index, uint32_t codec, u
 /* 4 is not assigned */
 #define B2S_JOIN_RIGHT_OUTER 5
 #define B2S_JOIN_FULL_OUTER 6
+/* 7 is not assigned */
+#define B2S_JOIN_EXISTENCE 8
 /* field kinds of a side's schema (the joined row's offset fix-up and an outer join's null side) */
 #define B2S_FIELD_FIXED 0        /* a fixed-width value in its 8-byte slot */
 #define B2S_FIELD_VAR 1          /* (offset << 32) | size: string, binary, array, map, struct */

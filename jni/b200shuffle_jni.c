@@ -752,9 +752,10 @@ static void* need(JNIEnv* e, jarray a, jsize n, size_t elem, int* rc) {
 }
 
 /* ---- read side, sort-merge join (INTEGRATION.md §3n): blocks [0, nLeft) are the left side's, the rest the right's;
- *      joinType: B2S_JOIN_* (inner, left outer, left semi, left anti, right outer, full outer).
- *      keyType / keyLen: int[nKeys] for both sides; left/rightKeyOff and left/rightKeyNullField: int[nKeys] per side;
- *      left/rightFieldKind: byte[nFields] of B2S_FIELD_* (null for semi and anti joins); meta: long[4] = {dst_total,
+ *      joinType: B2S_JOIN_* (inner, left outer, left semi, left anti, right outer, full outer, existence).
+ *      keyType / keyLen: int[nKeys] for both sides, a type OR-ed with B2S_KEY_NULL_SAFE for a <=> column;
+ *      left/rightKeyOff and left/rightKeyNullField: int[nKeys] per side; left/rightFieldKind: byte[nFields] of
+ *      B2S_FIELD_* (null for semi and anti joins; rightFieldKind null for existence joins); meta: long[4] = {dst_total,
  *      n_left_records, n_right_records, n_out_records}; other arrays as decompressSortRowsPacked.  Every array goes
  *      through a native copy. ---- */
 JNIEXPORT jint JNICALL J(decompressJoinRowsKeysPacked)(JNIEnv* e, jclass c, jint joinType, jint codec, jint alg,

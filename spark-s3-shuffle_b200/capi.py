@@ -17,6 +17,8 @@ STRING_KEY = 3  # the composite-key calls' variable-length key column (decompres
 # the composite-key calls' other column types (BooleanType is KEY_BYTES with length 1) and order flags
 KEY_INT16, KEY_INT8, KEY_FLOAT32, KEY_FLOAT64, DECIMAL_KEY = 5, 6, 7, 8, 9
 KEY_DESCENDING, KEY_NULLS_LAST = 1 << 8, 1 << 9
+# a null-safe (<=>) column, the pair (coalesce(v, default), isnull(v)): the join and hash calls only
+KEY_NULL_SAFE = 1 << 10
 # aggregate ops of the row aggregation (decompress_aggregate_rows_*)
 (AGG_SUM_INT64, AGG_SUM_FLOAT64, AGG_MIN_INT32, AGG_MAX_INT32, AGG_MIN_INT64, AGG_MAX_INT64, AGG_MIN_FLOAT64,
  AGG_MAX_FLOAT64) = range(8)
@@ -28,6 +30,7 @@ AGG_VARIANCE = 12
 # join types of the row join (decompress_join_rows_keys_*) and the field kinds of its sides' schemas
 JOIN_INNER, JOIN_LEFT_OUTER, JOIN_LEFT_SEMI, JOIN_LEFT_ANTI = 0, 1, 2, 3
 JOIN_RIGHT_OUTER, JOIN_FULL_OUTER = 5, 6  # 4 is not assigned
+JOIN_EXISTENCE = 8  # 7 is not assigned
 FIELD_FIXED, FIELD_VAR, FIELD_DECIMAL_WIDE = 0, 1, 2
 # ranking functions of the row window (decompress_window_rows_keys_*), and its limit function meaning "no limit"
 WINDOW_ROW_NUMBER, WINDOW_RANK, WINDOW_DENSE_RANK, WINDOW_PERCENT_RANK, WINDOW_CUME_DIST, WINDOW_NTILE = range(6)
@@ -646,11 +649,13 @@ def decompress_join_rows_keys_packed(join_type, codec, src, off, length, n_left,
     """Sort-merge joins a reducer's two shuffled sides of UnsafeRow records: blocks [0, n_left) are the left side's,
     the rest the right's.  left_keys / right_keys: [(key type, row offset, length, null field or -1), ...] as in
     decompress_sort_rows_keys_packed without order flags, one entry per join key column on each side (the types and
-    lengths are the left's).  The kinds (FIELD_*, one per field; None for semi and anti joins) say which slots hold an
-    offset.  dst receives Spark's joined rows ([int32 big-endian size][row]) for JOIN_INNER / JOIN_LEFT_OUTER /
+    lengths are the left's); a type OR-ed with KEY_NULL_SAFE is a null-safe (<=>) column, equal to a null when null.
+    The kinds (FIELD_*, one per field; None for semi and anti joins, and the right's for JOIN_EXISTENCE) say which slots
+    hold an offset.  dst receives Spark's joined rows ([int32 big-endian size][row]) for JOIN_INNER / JOIN_LEFT_OUTER /
     JOIN_RIGHT_OUTER / JOIN_FULL_OUTER (left.output ++ right.output; a right outer join in the right side's key order,
     a full outer join run by run in key order, as the header states), the left records for JOIN_LEFT_SEMI /
-    JOIN_LEFT_ANTI.
+    JOIN_LEFT_ANTI, and for JOIN_EXISTENCE every left record with one boolean field, whether it has a match
+    (left.output :+ exists).
     -> dict(total, n_left_records, n_right_records, n_out_records, status, bad_slice)"""
     n, kt, kl, lo, ln, ro, rn, lk, rk = _join_arrays(left_keys, right_keys, left_kinds, right_kinds)
     return _sort_call("b2s_decompress_join_rows_keys_packed", codec, src, off, length, dst, None,
@@ -933,7 +938,8 @@ def partition_compress_dev(codec, d_records, rec_bytes, d_rec_len, d_rec_part, n
 def partition_compress_rows_hash_packed(codec, records, rec_len, keys, num_partitions, dst, block_size=0,
                                         checksum_alg=CHECKSUM_NONE, level=0):
     """partition_compress_packed of serialized UnsafeRows ([int32 big-endian size][row] each), every record's reduce
-    id Spark's pmod(Murmur3Hash(key columns, 42), num_partitions); keys as in decompress_sort_rows_keys_packed.
+    id Spark's pmod(Murmur3Hash(key columns, 42), num_partitions); keys as in decompress_sort_rows_keys_packed, no
+    order flags; a type OR-ed with KEY_NULL_SAFE hashes as its (coalesce(v, default), isnull(v)) key pair.
     -> dict(dst_off, dst_len, total, checksums, status)"""
     records, dst = _as_u8(records), _as_u8(dst)
     rec_len = np.ascontiguousarray(rec_len, dtype=np.uint32)

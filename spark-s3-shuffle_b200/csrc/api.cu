@@ -2544,6 +2544,7 @@ struct RecordSpec {
   uint32_t n_keys = 1;      // as the caller passed it; keys holds the columns when it is in [1, 16]
   bool key_arrays = true;   // the caller's key arrays are not NULL
   bool composite = false;   // the *_keys calls: string, decimal, 16 / 8-bit and float columns and order flags accepted
+  bool null_safe = false;   // the join and hash calls: B2S_KEY_NULL_SAFE accepted too
   bool aggregate = false;
   uint32_t n_aggs = 0;
   const uint32_t* agg_op = nullptr;
@@ -2736,8 +2737,8 @@ static int key_columns_args(const RecordSpec& spec) {
     const uint32_t type = ks.type[c] & kKeyTypeMask, flags = ks.type[c] & ~kKeyTypeMask, key_len = ks.len[c];
     const bool composite_type = type == kStringKey || (type >= B2S_KEY_INT16 && type <= kDecimalKey);
     if (type > B2S_KEY_INT64 && !(spec.composite && composite_type)) return fail(B2S_E_ARG, "unknown key_type%s");
-    if (flags && (!spec.composite || (flags & ~(B2S_KEY_DESCENDING | B2S_KEY_NULLS_LAST))))
-      return fail(B2S_E_ARG, "unknown key_type flag%s");
+    const uint32_t known = B2S_KEY_DESCENDING | B2S_KEY_NULLS_LAST | (spec.null_safe ? B2S_KEY_NULL_SAFE : 0);
+    if (flags && (!spec.composite || (flags & ~known))) return fail(B2S_E_ARG, "unknown key_type flag%s");
     if (type == B2S_KEY_BYTES && (key_len < 1 || key_len > 16))
       return fail(B2S_E_ARG, "key_len must be in [1, 16]%s");
     // the fixed key_len of every other type: the value's bytes, or a string's or decimal's 8-byte slot
@@ -2756,8 +2757,8 @@ static uint32_t bitset_words(uint32_t n) { return (n + 63) / 64; }
 // each side's fields, and every key slot and null bit inside its side's fixed region
 static int join_args(const RecordSpec& spec, uint32_t n) {
   const JoinSpec& js = *spec.join;
-  if (js.type > B2S_JOIN_FULL_OUTER || js.type == B2S_JOIN_LEFT_ANTI + 1)  // 4 is not assigned
-    return fail(B2S_E_ARG, "unknown join_type%s");
+  if ((js.type > B2S_JOIN_FULL_OUTER && js.type != B2S_JOIN_EXISTENCE) || js.type == B2S_JOIN_LEFT_ANTI + 1)
+    return fail(B2S_E_ARG, "unknown join_type%s");  // 4 and 7 are not assigned
   if (js.n_left > n) return fail(B2S_E_ARG, "n_left must be at most n%s");
   RecordSpec right = spec;
   right.keys = js.right;
@@ -2770,13 +2771,14 @@ static int join_args(const RecordSpec& spec, uint32_t n) {
     if (nf < 1 || nf > 65536) return fail(B2S_E_ARG, "a side's field count must be in [1, 65536]%s");
     const uint64_t lo = 8ull * bitset_words(nf), hi = lo + 8ull * nf;
     for (uint32_t c = 0; c < side[s]->n; c++) {
-      if (side[s]->type[c] & ~kKeyTypeMask) return fail(B2S_E_ARG, "a join key column takes no order flag%s");
+      if (side[s]->type[c] & ~kKeyTypeMask & ~B2S_KEY_NULL_SAFE)
+        return fail(B2S_E_ARG, "a join key column takes no order flag%s");
       if (side[s]->off[c] < lo || (uint64_t)side[s]->off[c] + side[s]->len[c] > hi)
         return fail(B2S_E_ARG, "a key slot lies outside its side's field slots%s");
       if (side[s]->null_field[c] >= (int64_t)nf)
         return fail(B2S_E_ARG, "a key null bit is not below its side's field count%s");
     }
-    if (kinds) {
+    if (kinds && (s == 0 || js.type != B2S_JOIN_EXISTENCE)) {  // an existence join's row holds no right field
       if (!js.kind[s]) return fail(B2S_E_ARG, "field kinds are required for joins that build joined rows%s");
       for (uint32_t f = 0; f < nf; f++)
         if (js.kind[s][f] > B2S_FIELD_DECIMAL_WIDE) return fail(B2S_E_ARG, "unknown field kind%s");
@@ -3012,8 +3014,10 @@ static int hash_args(uint32_t codec, uint32_t codec_block_size, uint32_t alg, ui
     return rc;
   if (int rc = key_columns_args(spec)) return rc;
   for (uint32_t c = 0; c < spec.keys.n; c++) {
-    if (spec.keys.type[c] & ~kKeyTypeMask) return fail(B2S_E_ARG, "a hashed key column takes no order flag%s");
-    if (spec.keys.type[c] == B2S_KEY_BYTES && spec.keys.len[c] != 1)
+    const uint32_t flags = spec.keys.type[c] & ~kKeyTypeMask;
+    if (flags & ~(spec.null_safe ? B2S_KEY_NULL_SAFE : 0))
+      return fail(B2S_E_ARG, "a hashed key column takes no order flag%s");
+    if ((spec.keys.type[c] & kKeyTypeMask) == B2S_KEY_BYTES && spec.keys.len[c] != 1)
       return fail(B2S_E_ARG, "a hashed B2S_KEY_BYTES column is a boolean: key_len must be 1%s");
   }
   if (!g_ctx)
@@ -3050,7 +3054,8 @@ static int rows_hash_packed(const ExStore* store, uint32_t codec, int32_t level,
                             const int32_t* key_null_field, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_off,
                             uint64_t* dst_len, uint64_t* dst_total, uint64_t* checksum_out, int32_t* status) {
   if (dst_total) *dst_total = 0;
-  const RecordSpec spec = keys_spec(n_keys, key_type, key_off, key_len, key_null_field);
+  RecordSpec spec = keys_spec(n_keys, key_type, key_off, key_len, key_null_field);
+  spec.null_safe = true;
   const RowIds ids{spec.keys};
   return rows_packed(store, ids,
                      hash_args(codec, codec_block_size, checksum_alg, num_partitions, n_records, rec_base, rec_bytes,
@@ -3095,7 +3100,8 @@ int b2s_partition_compress_rows_hash_dev(uint32_t dev_index, uint32_t codec, int
                                          uint64_t dst_cap, uint64_t* dst_off, uint64_t* dst_len, uint64_t* dst_total,
                                          uint64_t* checksum_out, int32_t* status) {
   if (dst_total) *dst_total = 0;
-  const RecordSpec spec = keys_spec(n_keys, key_type, key_off, key_len, key_null_field);
+  RecordSpec spec = keys_spec(n_keys, key_type, key_off, key_len, key_null_field);
+  spec.null_safe = true;
   const RowIds ids{spec.keys};
   if (int rc = hash_args(codec, codec_block_size, checksum_alg, num_partitions, n_records, rec_base, rec_bytes, rec_len,
                          spec, dst_base, dst_off, dst_len, status))
@@ -4396,16 +4402,24 @@ static int aggregate_rows_tail(Slot& S, const RecordSpec& spec, DecodedTask& T, 
   return 0;
 }
 
-// A join's key columns per side (JoinKeys: a column nullable on one side only takes kNullByteOnly on the other, so
-// equal keys encode equal; split: the arena offset of the right side's first block) and its joined row's shape, whose
-// field lists (left VAR / DECIMAL_WIDE fields, right ones, right DECIMAL_WIDE ones, left DECIMAL_WIDE ones) go to
-// fields.
+// A join's key columns per side (JoinKeys: a plain column nullable on one side only takes kNullByteOnly on the other,
+// so equal keys encode equal; a null-safe column encodes its trailing isnull byte on both sides whatever their null
+// fields; split: the arena offset of the right side's first block) and its joined row's shape, whose key columns are
+// those a null makes unmatchable (a null-safe column's null field is -1 there) and whose field lists (left VAR /
+// DECIMAL_WIDE fields, right ones, right DECIMAL_WIDE ones, left DECIMAL_WIDE ones) go to fields.  An existence join's
+// row is the left row and one boolean field: no right field list.
 static void join_layout(const RecordSpec& spec, uint64_t split, JoinKeys& jk, JoinShape& shape,
                         std::vector<uint32_t>& fields) {
   const JoinSpec& js = *spec.join;
   jk.side[0] = spec.keys;
   jk.side[1] = js.right;
+  shape.keys[0] = spec.keys;
+  shape.keys[1] = js.right;
   for (uint32_t c = 0; c < spec.keys.n; c++) {
+    if (spec.keys.type[c] & B2S_KEY_NULL_SAFE) {
+      shape.keys[0].null_field[c] = shape.keys[1].null_field[c] = -1;
+      continue;
+    }
     int32_t& l = jk.side[0].null_field[c];
     int32_t& r = jk.side[1].null_field[c];
     if (l >= 0 && r < 0) r = kNullByteOnly;
@@ -4414,24 +4428,23 @@ static void join_layout(const RecordSpec& spec, uint64_t split, JoinKeys& jk, Jo
   jk.split = split;
   shape.type = js.type;
   shape.split = split;
-  shape.keys[0] = spec.keys;
-  shape.keys[1] = js.right;
   for (uint32_t s = 0; s < 2; s++) {
     shape.n[s] = js.n_fields[s];
     shape.bw[s] = bitset_words(js.n_fields[s]);
     jk.fixed[s] = 8 * (shape.bw[s] + shape.n[s]);
   }
-  shape.out_bw = bitset_words(shape.n[0] + shape.n[1]);
+  const bool exists = js.type == B2S_JOIN_EXISTENCE;
+  shape.out_bw = bitset_words(shape.n[0] + (exists ? 1 : shape.n[1]));
   fields.clear();
   const bool rows = !join_keeps_whole(js.type);  // a semi or anti join: no kinds
   for (uint32_t s = 0; s < 2; s++) {
-    for (uint32_t f = 0; rows && f < shape.n[s]; f++)
+    for (uint32_t f = 0; rows && !(exists && s) && f < shape.n[s]; f++)
       if (js.kind[s][f] != B2S_FIELD_FIXED) fields.push_back(f);
     shape.n_var[s] = (uint32_t)fields.size() - (s ? shape.n_var[0] : 0);
   }
   for (uint32_t s : {1u, 0u}) {  // the null side's wide decimals: the right side's, then the left side's
     const size_t before = fields.size();
-    for (uint32_t f = 0; rows && f < shape.n[s]; f++)
+    for (uint32_t f = 0; rows && !exists && f < shape.n[s]; f++)
       if (js.kind[s][f] == B2S_FIELD_DECIMAL_WIDE) fields.push_back(f);
     shape.n_wide[s] = (uint32_t)(fields.size() - before);
   }
@@ -4465,8 +4478,8 @@ static int join_rows_tail(Slot& S, const RecordSpec& spec, DecodedTask& T, const
     if (int rc = S.parena.ensure(jb[1] + 64)) return rc;
     *d_out = (uint8_t*)S.parena.p;
   }
-  launch_join_emit(T.arena, R.records, R.idx, jb[0], R.key_bytes, join_keeps_whole(spec.join->type), R.ws,
-                   R.jws, T.n_src, *d_out, st, launches);
+  launch_join_emit(T.arena, R.records, R.idx, jb[0], R.key_bytes, spec.join->type, R.ws, R.jws, T.n_src, *d_out, st,
+                   launches);
   CU(S.mark(G1, st, *launches));
   CU(S.mark(P1, st));
   CU(cudaStreamSynchronize(st));
@@ -5310,6 +5323,7 @@ static int join_call(uint32_t dev_index, bool packed, uint32_t join_type, uint32
   js.n_side[0] = n_left_records;
   js.n_side[1] = n_right_records;
   RecordSpec spec = keys_spec(n_keys, key_type, left_key_off, key_len, left_key_null_field);
+  spec.null_safe = true;
   spec.join = &js;
   const int rc = sort_call(dev_index, packed, nullptr, codec, alg, n, src_base, src_off, src_len, slice_base, slice_len,
                            slice_checksum, spec, dst_base, dst_cap, dst_total, n_out_records, status, bad_slice);

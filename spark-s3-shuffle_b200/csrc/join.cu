@@ -12,7 +12,7 @@
 //           records and bytes the record drives: a left record its rows with the group's right records (inner, left
 //           and full outer), a right record its rows with the group's left records (right outer), either one row with
 //           a null other side when its group does not match (left, right and full outer: a full outer join's right
-//           records only then); both are scanned, and the totals, the left record count and the too-long flag come
+//           records only then), or (existence) a left record its own row with the exists field; both are scanned, and the totals, the left record count and the too-long flag come
 //           back in one readback
 //   emit  : a warp per output record, whose driving position is found by a search in the scanned output record counts,
 //           so a hot key's many joined rows spread over the whole GPU; its partner is the k-th record of the other
@@ -20,7 +20,8 @@
 //           var][right var]: the four spans are copied 16 bytes per lane, the null words built from both sides' bits,
 //           and the slots of VAR and DECIMAL_WIDE fields moved by their side's shift; a null side has its bits set, its
 //           slots zero and 16 zero bytes for each DECIMAL_WIDE field.  A semi or anti join compacts its kept left
-//           positions and gathers those records with the row sort's gather.
+//           positions and gathers those records with the row sort's gather.  An existence join's rows are emitted by a
+//           warp per left position: the record with one more fixed field, as the window emit builds its rows.
 #include <algorithm>
 
 #include "kernels.h"
@@ -133,7 +134,7 @@ __global__ void __launch_bounds__(kJoinThreads) join_count_kernel(
     uint64_t r = 0, b = 0;
     uint32_t partner = kNoMatch;
     // a row shorter than its fixed region fails the call (the key pass's verdict): not read, no output
-    if (size >= fixed && !(right && join_keeps_whole(type))) {
+    if (size >= fixed && !(right && (join_keeps_whole(type) || type == kJoinExistence))) {
       const uint64_t g = group_of(heads_before, j, n, G), s = gpos[g], e = gpos[g + 1];
       uint64_t lo = right ? s : j + 1, hi = right ? j : e;  // the group's first right position: left records come first
       while (lo < hi) {
@@ -156,6 +157,11 @@ __global__ void __launch_bounds__(kJoinThreads) join_count_kernel(
       if (join_keeps_whole(type)) {
         r = matched == (type == kJoinLeftSemi);
         b = r ? 4 + (uint64_t)size : 0;
+      } else if (type == kJoinExistence) {  // its row grows by the null words it adds and the exists slot
+        r = 1;
+        b = 4 + (uint64_t)size + 8ull * (sh->out_bw - sh->bw[0] + 1);
+        if (b - 4 > 0x7fffffffull) readback[3] = 1;
+        partner = matched;
       } else if (drives && matched) {  // one row with each record of the other side's part of the group
         r = right ? L : R;
         b = r * (4 + fixed_out + var_own) + (right ? var[lo] - var[s] : var[e] - var[lo]);
@@ -270,6 +276,44 @@ __global__ void __launch_bounds__(kJoinThreads) join_emit_kernel(
   }
 }
 
+// An existence join's row of left position j (right positions have none), by a warp: [out_bw null words: the left's
+// bits][the left's slots][the exists slot: rpos[j]][the left's var bytes], its var slots moved past the added words
+__global__ void __launch_bounds__(kJoinThreads) join_exists_emit_kernel(
+    const uint8_t* __restrict__ arena, const uint64_t* __restrict__ rec_off, const uint32_t* __restrict__ rec_len,
+    const uint32_t* __restrict__ idx, uint64_t n, const JoinShape* __restrict__ sh, const uint64_t* __restrict__ bytes,
+    const uint32_t* __restrict__ rpos, uint8_t* __restrict__ dst) {
+  const uint32_t lane = threadIdx.x & 31;
+  const uint64_t warps = (uint64_t)gridDim.x * (blockDim.x / 32);
+  const uint64_t split = sh->split;
+  const uint32_t nl = sh->n[0], bl = sh->bw[0], b = sh->out_bw;
+  const uint32_t fixed_in = 8 * (bl + nl);
+  const uint64_t fixed_out = 8ull * (b + nl + 1);
+  const uint64_t shift = 8ull * (b - bl + 1) << 32;
+  for (uint64_t j = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) / 32; j < n; j += warps) {
+    const uint32_t i = at(idx, j);
+    if (rec_off[i] >= split) continue;
+    const uint8_t* src = arena + rec_off[i] + 4;
+    const uint64_t var = rec_len[i] - 4 - fixed_in;
+    uint8_t* d = dst + bytes[j];
+    uint8_t* row = d + 4;
+    if (lane == 0) {
+      st_span16(d, 4, __byte_perm((uint32_t)(fixed_out + var), 0, 0x0123), 0);
+      st_span16(row + 8 * (b + nl), 8, rpos[j], 0);
+    }
+    for (uint32_t w = lane; w < b; w += 32) st_span16(row + 8 * w, 8, bits_word(src, nl, w, false), 0);
+    warp_copy(row + 8 * b, src + 8 * bl, 8ull * nl, lane);
+    warp_copy(row + fixed_out, src + fixed_in, var, lane);
+    __syncwarp();
+    // a zero slot (a null string) stays zero
+    for (uint32_t x = lane; x < sh->n_var[0]; x += 32) {
+      const uint32_t f = sh->var[0][x];
+      const uint64_t slot = ld64(src + 8 * (bl + f));
+      if (slot) st_span16(row + 8 * (b + f), 8, slot + shift, 0);
+    }
+    __syncwarp();
+  }
+}
+
 }  // namespace
 
 size_t join_ws_bytes(uint64_t n, uint32_t n_ranges, uint32_t n_fields) {
@@ -308,17 +352,24 @@ void launch_join_count(const uint8_t* arena, uint64_t n, const uint32_t* idx, Jo
 }
 
 void launch_join_emit(const uint8_t* arena, uint64_t n, const uint32_t* idx, uint64_t out_rows, uint32_t key_bytes,
-                      bool whole, uint8_t* d_ws, uint8_t* d_jws, uint32_t n_ranges, uint8_t* d_dst, cudaStream_t st,
+                      uint32_t type, uint8_t* d_ws, uint8_t* d_jws, uint32_t n_ranges, uint8_t* d_dst, cudaStream_t st,
                       uint64_t* launches) {
   if (!out_rows) return;
   const JoinWs j = carve_join_ws(d_jws, n, n_ranges);
-  if (whole) {  // the kept left records' indices (in rpos, which these joins do not use), then the row sort's gather
+  if (join_keeps_whole(type)) {  // the kept left records' indices (in rpos, which these joins do not use), then the row sort's gather
     join_compact_kernel<<<grid_for(n), kJoinThreads, 0, st>>>(idx, n, j.rows, out_rows, j.rpos);
     if (launches) *launches += 1;
     launch_rows_gather(arena, n, key_bytes, j.rpos, d_ws, d_dst, st, launches, out_rows);
     return;
   }
   const KeySortWs w = carve_key_sort_ws(d_ws, n, key_bytes);
+  if (type == kJoinExistence) {  // a warp per sorted position
+    const uint64_t want = (n + kJoinThreads / 32 - 1) / (kJoinThreads / 32);
+    join_exists_emit_kernel<<<(unsigned)std::min<uint64_t>(want, (uint64_t)kSMs * 16), kJoinThreads, 0, st>>>(
+        arena, w.src_off, w.len, idx, n, j.shape, j.bytes, j.rpos, d_dst);
+    if (launches) *launches += 1;
+    return;
+  }
   const uint64_t want = (out_rows + kJoinThreads / 32 - 1) / (kJoinThreads / 32);
   const unsigned grid = (unsigned)std::min<uint64_t>(want, (uint64_t)kSMs * 16);
   join_emit_kernel<<<grid, kJoinThreads, 0, st>>>(arena, w.src_off, w.len, idx, n, out_rows, j.shape, j.rows, j.bytes,

@@ -304,7 +304,8 @@ inline uint32_t rows_key_encoded_bytes(const KeySpec& ks) {
   for (uint32_t c = 0; c < ks.n; c++) {
     const uint32_t ty = ks.type[c] & kKeyTypeMask;
     if (ty == kStringKey) return ~0u;
-    b += key_value_bytes(ty, ks.len[c]) + (ks.null_field[c] != -1 ? 1 : 0);
+    // a null byte (leading), or a null-safe column's isnull byte (trailing, with or without a null field)
+    b += key_value_bytes(ty, ks.len[c]) + (ks.null_field[c] != -1 || (ks.type[c] & B2S_KEY_NULL_SAFE) ? 1 : 0);
   }
   return b;
 }
@@ -365,7 +366,8 @@ void launch_rows_whole_refine_round(const uint8_t* rec, const uint64_t* rec_off,
                                     cudaStream_t st, uint64_t* launches);
 // A join's key pass (two row layouts in one sort): record i is a left record when its arena offset is below split (the
 // left blocks come first, so the left records are a prefix), else a right one, and it is keyed with its side's columns
-// side[0] / side[1] (encoded to equal widths: a column nullable on one side only has kNullByteOnly on the other).  A
+// side[0] / side[1] (encoded to equal widths: a plain column nullable on one side only has kNullByteOnly on the other;
+// a B2S_KEY_NULL_SAFE column encodes its trailing isnull byte on both sides, whatever their null fields).  A
 // row shorter than its side's fixed region fixed[s] lowers its range's verdict (verdict[r], as rows_keys_kernel's) with
 // kRowsBadKey; a bad string or decimal with kRowsBadString.  Such a record gets key length 0 (never refined).
 struct JoinKeys {
@@ -593,7 +595,8 @@ void launch_expand_write(const uint8_t* rec, const uint64_t* rec_off, uint64_t n
 // regions), as device lists.
 constexpr uint32_t kJoinInner = B2S_JOIN_INNER, kJoinLeftOuter = B2S_JOIN_LEFT_OUTER,
                    kJoinLeftSemi = B2S_JOIN_LEFT_SEMI, kJoinLeftAnti = B2S_JOIN_LEFT_ANTI,
-                   kJoinRightOuter = B2S_JOIN_RIGHT_OUTER, kJoinFullOuter = B2S_JOIN_FULL_OUTER;
+                   kJoinRightOuter = B2S_JOIN_RIGHT_OUTER, kJoinFullOuter = B2S_JOIN_FULL_OUTER,
+                   kJoinExistence = B2S_JOIN_EXISTENCE;
 // a semi or anti join: its output is the kept left records themselves, not joined rows
 __host__ __device__ inline bool join_keeps_whole(uint32_t type) {
   return type == kJoinLeftSemi || type == kJoinLeftAnti;
@@ -605,7 +608,7 @@ struct JoinShape {
   uint32_t n_var[2], n_wide[2];
   const uint32_t* var[2];
   const uint32_t* wide[2];
-  KeySpec keys[2];     // each side's key columns (a record's null columns)
+  KeySpec keys[2];     // each side's key columns whose null makes a key unmatchable (a null-safe column's is -1)
 };
 // d_jws: join_ws_bytes(n, n_ranges, n_fields) bytes; launch_join_count uploads the shape and its field lists (h_fields:
 // the left's non-fixed fields, the right's, the right's DECIMAL_WIDE ones, the left's DECIMAL_WIDE ones)
@@ -620,10 +623,11 @@ inline size_t join_readback_bytes(uint32_t n_ranges) { return (4 + (size_t)n_ran
 void launch_join_count(const uint8_t* arena, uint64_t n, const uint32_t* idx, JoinShape shape,
                        const uint32_t* h_fields, uint32_t n_fields, uint32_t key_bytes, uint8_t* d_ws,
                        uint8_t* d_aws, uint8_t* d_jws, uint32_t n_ranges, cudaStream_t st, uint64_t* launches);
-// the out_rows joined records (read back) to d_dst, a warp per record; whole (semi and anti joins): the kept left
-// records, compacted and gathered by launch_rows_gather
+// the out_rows joined records (read back) to d_dst, a warp per record; semi and anti joins (join_keeps_whole): the
+// kept left records, compacted and gathered by launch_rows_gather; the existence join: a warp per left record, the
+// record with its exists field
 void launch_join_emit(const uint8_t* arena, uint64_t n, const uint32_t* idx, uint64_t out_rows, uint32_t key_bytes,
-                      bool whole, uint8_t* d_ws, uint8_t* d_jws, uint32_t n_ranges, uint8_t* d_dst, cudaStream_t st,
+                      uint32_t type, uint8_t* d_ws, uint8_t* d_jws, uint32_t n_ranges, uint8_t* d_dst, cudaStream_t st,
                       uint64_t* launches);
 
 // ---------------- window.cu (Spark's WindowExec ranking and aggregate functions over a reducer's key-sorted rows) -------

@@ -265,7 +265,9 @@ __global__ void __launch_bounds__(kRowThreads, 8) rows_keys_kernel(
 }
 
 // The join's key pass (kernels.h, JoinKeys): rows_keys_kernel with each record's side's columns and its fixed-region
-// check.  A kernel of its own, so that the single-spec sorts keep theirs.
+// check.  A kernel of its own, so that the single-spec sorts keep theirs; NullSafe: a key with a B2S_KEY_NULL_SAFE
+// column (encode_key), its own instantiation so that plain keys keep theirs.
+template <bool NullSafe>
 __global__ void __launch_bounds__(kRowThreads) rows_join_keys_kernel(
     const uint8_t* __restrict__ arena, const uint64_t* __restrict__ rec_off, const uint32_t* __restrict__ rec_len,
     uint64_t n, const __grid_constant__ JoinKeys jk, uint32_t key_bytes, uint32_t* __restrict__ words,
@@ -282,7 +284,7 @@ __global__ void __launch_bounds__(kRowThreads) rows_join_keys_kernel(
     if (size < jk.fixed[s]) {  // its key slots and null words are not all inside it: not read
       why = kRowsBadKey;
     } else {
-      len = encode_key<true>(arena + ro + 4, size, jk.side[s], kw, klen != nullptr, &bad);
+      len = encode_key<true, NullSafe>(arena + ro + 4, size, jk.side[s], kw, klen != nullptr, &bad);
       if (bad) why = kRowsBadString;
     }
 #pragma unroll
@@ -361,6 +363,7 @@ __global__ void __launch_bounds__(kRowThreads) refine_extract_kernel(
 
 // refine_extract_kernel for a join's keys: each record with its side's columns (a bad record has key length 0: never
 // tied, never read here)
+template <bool NullSafe>
 __global__ void __launch_bounds__(kRowThreads) refine_extract_join_kernel(
     const uint8_t* __restrict__ arena, const uint64_t* __restrict__ rec_off, const uint32_t* __restrict__ rec_len,
     uint64_t n, const __grid_constant__ JoinKeys jk, const uint32_t* __restrict__ ord,
@@ -375,7 +378,7 @@ __global__ void __launch_bounds__(kRowThreads) refine_extract_join_kernel(
     cidx[k] = i;
     KeyWindow kw{0, 0, 0, 0, 0, d, kKeyChunkBytes};
     bool bad = false;
-    encode_key<true>(arena + rec_off[i] + 4, rec_len[i] - 4, jk.side[rec_off[i] >= jk.split], kw, false, &bad);
+    encode_key<true, NullSafe>(arena + rec_off[i] + 4, rec_len[i] - 4, jk.side[rec_off[i] >= jk.split], kw, false, &bad);
     words[k] = s;
 #pragma unroll
     for (uint32_t q = 0; q < 4; q++) words[(size_t)(q + 1) * m + k] = kw.word(q);
@@ -602,6 +605,13 @@ const uint32_t* launch_rows_order(const uint8_t* arena, uint64_t n, const KeySpe
   return idx;
 }
 
+// a join key with a B2S_KEY_NULL_SAFE column (both sides have the same types)
+static bool join_null_safe(const JoinKeys& jk) {
+  for (uint32_t c = 0; c < jk.side[0].n; c++)
+    if (jk.side[0].type[c] & B2S_KEY_NULL_SAFE) return true;
+  return false;
+}
+
 const uint32_t* launch_rows_join_order(const uint8_t* arena, uint64_t n, const JoinKeys& jk, const uint64_t* ranges,
                                        uint32_t n_ranges, uint64_t* verdict, uint8_t* d_ws, uint8_t* d_rws,
                                        cudaStream_t st, uint64_t* launches) {
@@ -614,8 +624,9 @@ const uint32_t* launch_rows_join_order(const uint8_t* arena, uint64_t n, const J
     r = carve_refine_ws(d_rws, n);
     cudaMemsetAsync(r.readback + 1, 0xff, (size_t)n_ranges * 8, st);
   }
-  rows_join_keys_kernel<<<grid_for(n), kRowThreads, 0, st>>>(arena, w.src_off, w.len, n, jk, key_bytes, w.words, r.klen,
-                                                             ranges, n_ranges, verdict);
+  auto keys = join_null_safe(jk) ? rows_join_keys_kernel<true> : rows_join_keys_kernel<false>;
+  keys<<<grid_for(n), kRowThreads, 0, st>>>(arena, w.src_off, w.len, n, jk, key_bytes, w.words, r.klen, ranges, n_ranges,
+                                            verdict);
   if (launches) *launches += 1;
   const uint32_t* idx = launch_key_radix(w, n, key_bytes, st, launches);
   if (d_rws) {
@@ -629,8 +640,9 @@ void launch_rows_join_refine_round(const uint8_t* arena, uint64_t n, const JoinK
                                    uint32_t d, uint8_t* d_ws, uint8_t* d_rws, cudaStream_t st, uint64_t* launches) {
   const KeySortWs w = carve_key_sort_ws(d_ws, n, kKeyPrefixBytes);
   const RefineWs r = carve_refine_ws(d_rws, n);
-  refine_extract_join_kernel<<<grid_for(n), kRowThreads, 0, st>>>(arena, w.src_off, w.len, n, jk, r.ord, r.head,
-                                                                  r.klen, r.scan, m, d, r.cpos, r.cidx, w.words);
+  auto extract = join_null_safe(jk) ? refine_extract_join_kernel<true> : refine_extract_join_kernel<false>;
+  extract<<<grid_for(n), kRowThreads, 0, st>>>(arena, w.src_off, w.len, n, jk, r.ord, r.head, r.klen, r.scan, m, d,
+                                               r.cpos, r.cidx, w.words);
   refine_sort_scatter(w, r, m, segs, st, launches);
   if (launches) *launches += 2;
 }

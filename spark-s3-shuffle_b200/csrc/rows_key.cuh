@@ -77,8 +77,10 @@ __device__ __forceinline__ void decimal_bits(const uint8_t* row, uint32_t row_si
 // the key's encoded length (else the walk stops at the window's end); every non-null decimal slot is then checked.
 // *bad: a non-null string slot runs past the row, or a decimal slot is bad (decimal_bits); the bytes read are then
 // clamped to the row, so no load leaves it.  Join (the join's key pass): a column whose null_field is kNullByteOnly
-// takes the null byte of a non-null value without reading a null word (its other side's column is nullable).
-template <bool Join = false>
+// takes the null byte of a non-null value without reading a null word (its other side's column is nullable).  NullSafe
+// (a join key with a B2S_KEY_NULL_SAFE column): such a column is (coalesce(v, default), isnull(v)): no leading null
+// byte, its value's bytes or the type's default's when null (a null's slot is not read), then a trailing 0 / 1 byte.
+template <bool Join = false, bool NullSafe = false>
 __device__ __forceinline__ uint32_t encode_key(const uint8_t* row, uint32_t row_size, const KeySpec& ks, KeyWindow& kw,
                                                bool whole, bool* bad) {
   const uint32_t wend = kw.d + kw.nb;
@@ -88,19 +90,21 @@ __device__ __forceinline__ uint32_t encode_key(const uint8_t* row, uint32_t row_
     const uint32_t ty = ks.type[c] & kKeyTypeMask, off = ks.off[c], len = ks.len[c];
     const uint32_t flip = ks.type[c] & B2S_KEY_DESCENDING ? 0xff : 0;  // DESC: every value byte complemented
     const int32_t nf = ks.null_field[c];
+    const bool safe = Join && NullSafe && (ks.type[c] & B2S_KEY_NULL_SAFE);
     bool is_null = false;
     if (nf >= 0) {
       uint64_t nw, unused;
       ld_span16<true>(row + 8 * (uint32_t)(nf >> 6), 8, nw, unused);
       is_null = (nw >> (nf & 63)) & 1;
-      kw.put(p++, is_null == ((ks.type[c] & B2S_KEY_NULLS_LAST) != 0) ? 1 : 0);
+      if (!safe) kw.put(p++, is_null == ((ks.type[c] & B2S_KEY_NULLS_LAST) != 0) ? 1 : 0);
     } else if (Join && nf == kNullByteOnly) {
       kw.put(p++, 1);
     }
     if (ty == kStringKey) {
-      if (is_null) continue;
+      if (is_null && !safe) continue;
       uint64_t slot, unused;
-      ld_span16<true>(row + off, 8, slot, unused);
+      if (safe && is_null) slot = 0;  // a null-safe null: the empty string
+      else ld_span16<true>(row + off, 8, slot, unused);
       uint32_t so = (uint32_t)(slot >> 32), sz = (uint32_t)slot;
       if ((uint64_t)so + sz > row_size) {
         *bad = true;
@@ -132,9 +136,17 @@ __device__ __forceinline__ uint32_t encode_key(const uint8_t* row, uint32_t row_
           const uint32_t s = ty == B2S_KEY_BYTES ? b : w - 1 - b;
           kw.put(p + b, ((uint32_t)(s < 8 ? lo >> (8 * s) : hi >> (8 * (s - 8))) & 0xff) ^ flip);
         }
+      } else if (safe && is_null && in_window) {  // the default, 0 (false; BYTES all zero), encoded as a value
+        const uint64_t lo = ty == B2S_KEY_BYTES || ty == kDecimalKey ? 0 : ordered_bits(ty, len, 0);
+        const uint64_t hi = ty == kDecimalKey ? 1ull << 63 : 0;
+        for (uint32_t b = 0; b < w; b++) {
+          const uint32_t s = ty == B2S_KEY_BYTES ? b : w - 1 - b;
+          kw.put(p + b, (uint32_t)(s < 8 ? lo >> (8 * s) : hi >> (8 * (s - 8))) & 0xff);
+        }
       }
       p += w;
     }
+    if (safe) kw.put(p++, is_null ? 1 : 0);
   }
   return p;
 }

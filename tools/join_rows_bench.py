@@ -14,8 +14,12 @@ rows).  Workloads:
       many: 2000 joined rows per hot left row).
   d : a, with partners missing on both sides: no left row carries 25 % of the dimension's keys, and 10 % of the left
       rows carry a key outside the dimension, so right and full outer joins emit null-side rows.
---join-types (inner, left_outer, left_semi, left_anti, right_outer, full_outer; default inner) are joined on the same
-blocks.  Every timed reducer's output is checked against the model (tests/outer_join_model.py) before it is timed.  Per
+  e : b with both key columns null-safe (<=>, the keys of an INTERSECT or EXCEPT) and each of them null in 5 % of the
+      rows on both sides, so about 10 % of the keys hold a null; run it as left_semi and left_anti.  Its two sorts
+      take the same columns as plain ones (the sort calls take no null-safe flag).
+--join-types (inner, left_outer, left_semi, left_anti, right_outer, full_outer, existence; default inner) are joined on
+the same blocks.  Every timed reducer's output is checked against the model (tests/outer_join_model.py, and
+tests/null_safe_join_model.py for workload e and the existence join) before it is timed.  Per
 reducer, after one untimed call of each path, each path is timed once (b2s_last_timing: kernel_ms = the whole call on
 the device, dominant_ms = the join step); the sorts' kernel_ms are summed over the two calls.  The card's name and
 power limit are read in the same run.  --model-cache DIR keeps each checked output's length and SHA-256 there, so
@@ -43,7 +47,9 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 SNAPPY, CRC32C = 2, 3
 INT64, INT32, STRING = 2, 1, 3
 FIXED, VAR = 0, 1
-JOIN_TYPES = {"inner": 0, "left_outer": 1, "left_semi": 2, "left_anti": 3, "right_outer": 5, "full_outer": 6}
+JOIN_TYPES = {"inner": 0, "left_outer": 1, "left_semi": 2, "left_anti": 3, "right_outer": 5, "full_outer": 6,
+              "existence": 8}
+NULL_SAFE = 1 << 10
 
 
 def card():
@@ -84,6 +90,15 @@ def rows_of(slots, var, rng):
     return out, (4 + size).astype(np.uint32)
 
 
+def set_nulls(records, rec_len, fields, rate, rng):
+    """sets each of fields' null bits (all in the first null word) in a share rate of the framed rows"""
+    starts = np.concatenate([[0], np.cumsum(rec_len.astype(np.int64))[:-1]])
+    bits = np.zeros(rec_len.size, np.uint8)
+    for f in fields:
+        bits |= ((rng.random(rec_len.size) < rate) << f).astype(np.uint8)
+    records[starts + 4] |= bits
+
+
 def key_string(keys):
     """16 bytes: "cust" and the key's 12 decimal digits"""
     digits = (keys[:, None] // 10 ** np.arange(11, -1, -1, dtype=np.int64)) % 10 + 48
@@ -112,7 +127,7 @@ def reducer_sides(rng, workload, n_left, keys, partitions, red):
     r_slots[:, 1] = rng.integers(0, 1 << 62, n_r).astype(np.uint64)
     l_var = {4: 8 * rng.integers(0, 9, n_left)}
     r_var = {2: 8 * rng.integers(1, 4, n_r)}
-    if workload == "b":
+    if workload in "be":
         l_var[0] = key_string(lk)
         r_var[0] = key_string(rk)
         l_slots[:, 2] = (lk % 7).astype(np.uint64)
@@ -124,7 +139,13 @@ def reducer_sides(rng, workload, n_left, keys, partitions, red):
         lkeys, rkeys = [(INT64, 8, 8, -1)], [(INT64, 8, 8, -1)]
     lkind = [VAR if f in l_var else FIXED for f in range(5)]
     rkind = [VAR if f in r_var else FIXED for f in range(3)]
-    return ((*rows_of(l_slots, l_var, rng), lkeys, lkind), (*rows_of(r_slots, r_var, rng), rkeys, rkind))
+    left, right = rows_of(l_slots, l_var, rng), rows_of(r_slots, r_var, rng)
+    if workload == "e":  # the key columns are fields 0 and 2 on the left, 0 and 1 on the right
+        set_nulls(*left, (0, 2), 0.05, rng)
+        set_nulls(*right, (0, 1), 0.05, rng)
+        lkeys = [(STRING | NULL_SAFE, 8, 8, 0), (INT32 | NULL_SAFE, 24, 4, 2)]
+        rkeys = [(STRING | NULL_SAFE, 8, 8, 0), (INT32 | NULL_SAFE, 16, 4, 1)]
+    return ((*left, lkeys, lkind), (*right, rkeys, rkind))
 
 
 def blocks(capi, records, rec_len, maps, rng):
@@ -146,7 +167,8 @@ def blocks(capi, records, rec_len, maps, rng):
 
 
 def run(capi, args, workload, red, d_src, d_dst, cap):
-    from outer_join_model import model_join
+    import null_safe_join_model
+    import outer_join_model
     rng = np.random.default_rng(1000 * red + ord(workload))
     n_left = int(args.gib * 2**30 / 84 / args.partitions)
     (lrec, llen, lkeys, lkind), (rrec, rlen, rkeys, rkind) = reducer_sides(rng, workload, n_left, args.keys,
@@ -169,6 +191,7 @@ def run(capi, args, workload, red, d_src, d_dst, cap):
     def sorts():
         t = []
         for lo_, hi_, keys in ((0, args.maps, lkeys), (args.maps, n, rkeys)):
+            keys = [(t & ~NULL_SAFE, o, ln_, nf) for t, o, ln_, nf in keys]  # the sort takes plain columns
             capi.decompress_sort_rows_keys_dev(SNAPPY, d_src, off[lo_:hi_], ln[lo_:hi_], d_dst, cap, keys, CRC32C,
                                                np.arange(hi_ - lo_ + 1, dtype=np.uint32), sl[lo_:hi_], ck[lo_:hi_])
             t.append(capi.last_timing()["kernel_ms"])
@@ -182,7 +205,8 @@ def run(capi, args, workload, red, d_src, d_dst, cap):
         if cached and os.path.exists(cached):
             want = json.load(open(cached))
         else:
-            stream, _, _, rows = model_join(jt, lplain, rplain, lkeys, rkeys, 5, 3, lkind, rkind)
+            model = (null_safe_join_model if workload == "e" or name == "existence" else outer_join_model).model_join
+            stream, _, _, rows = model(jt, lplain, rplain, lkeys, rkeys, 5, 3, lkind, rkind)
             want = {"bytes": len(stream), "sha256": hashlib.sha256(stream).hexdigest(), "rows": rows}
             if cached:
                 os.makedirs(args.model_cache, exist_ok=True)
