@@ -446,20 +446,41 @@ def _partition_out(num_partitions):
             np.zeros(num_partitions, dtype=np.uint64), np.zeros(num_partitions, dtype=np.int32))
 
 
+def _records(records, rec_len):
+    """a packed call's records (back to back) and their lengths -> its arguments n_records, rec_base, rec_bytes,
+    rec_len"""
+    records, rec_len = _as_u8(records), np.ascontiguousarray(rec_len, dtype=np.uint32)
+    return rec_len.size, records, records.size, rec_len
+
+
+def _partition_call(symbol, codec, level, block_size, checksum_alg, num_partitions, mid, dst, dst_cap=None, dev=None,
+                    lead=(), counts=()):
+    """One map-side partition call, whose arguments are [dev,] *lead, codec, level, block_size, checksum_alg, *mid, dst,
+    dst_cap, dst_off, dst_len, total, checksums, status, *counts.  dev None: the packed form, dst a host array (dst_cap
+    is its size); else dst is a device address.  lead and mid are the call's own arguments, numpy arrays among them
+    passed as pointers (_records gives a packed call's records); counts names the outputs after status (n_groups,
+    n_out_records or cached).  -> dict(dst_off, dst_len, total, checksums, status, *counts)"""
+    if dev is None:
+        dst = _as_u8(dst)
+        dst_cap = dst.size
+    dst_off, dst_len, cks, st = _partition_out(num_partitions)
+    total = _u64(0)
+    outs = [_i32(0) if name == "cached" else _u64(0) for name in counts]
+    args = ([] if dev is None else [dev]) + [*lead, codec, level, block_size, checksum_alg, *mid, dst, dst_cap]
+    _check(getattr(load(), symbol)(*map(_arg, args), _ptr(dst_off), _ptr(dst_len), C.addressof(total), _ptr(cks),
+                                   _ptr(st), *map(C.addressof, outs)), symbol)
+    r = dict(dst_off=dst_off, dst_len=dst_len, total=total.value, checksums=cks, status=st)
+    r.update(zip(counts, (o.value for o in outs)))
+    return r
+
+
 def partition_compress_packed(codec, records, rec_len, rec_part, num_partitions, dst, block_size=0,
                               checksum_alg=CHECKSUM_NONE, level=0):
     """records: the serialized records back to back (uint8 array, ideally HostBuffer.array); rec_len / rec_part: one
     length and one reduce id per record.  -> dict(dst_off, dst_len, total, checksums, status), one entry per partition"""
-    records, dst = _as_u8(records), _as_u8(dst)
-    rec_len = np.ascontiguousarray(rec_len, dtype=np.uint32)
-    rec_part = np.ascontiguousarray(rec_part, dtype=np.uint32)
-    dst_off, dst_len, cks, st = _partition_out(num_partitions)
-    total = _u64(0)
-    _check(load().b2s_partition_compress_packed(codec, level, block_size, checksum_alg, num_partitions, rec_len.size,
-                                                _ptr(records), records.size, _ptr(rec_len), _ptr(rec_part), _ptr(dst),
-                                                dst.size, _ptr(dst_off), _ptr(dst_len), C.addressof(total), _ptr(cks),
-                                                _ptr(st)), "b2s_partition_compress_packed")
-    return dict(dst_off=dst_off, dst_len=dst_len, total=total.value, checksums=cks, status=st)
+    return _partition_call("b2s_partition_compress_packed", codec, level, block_size, checksum_alg, num_partitions,
+                           (num_partitions, *_records(records, rec_len), np.ascontiguousarray(rec_part, np.uint32)),
+                           dst)
 
 
 def decompressed_size_batch(codec, blocks):
@@ -926,13 +947,9 @@ def decompress_window_aggregate_rows_keys_dev(codec, d_src, off, length, d_dst, 
 def partition_compress_dev(codec, d_records, rec_bytes, d_rec_len, d_rec_part, n_records, num_partitions, d_dst,
                            dst_cap, block_size=0, checksum_alg=CHECKSUM_NONE, level=0, dev=0):
     """d_*: device addresses (records, u32 lengths, u32 reduce ids, destination arena)"""
-    dst_off, dst_len, cks, st = _partition_out(num_partitions)
-    total = _u64(0)
-    _check(load().b2s_partition_compress_dev(dev, codec, level, block_size, checksum_alg, num_partitions, n_records,
-                                             d_records, rec_bytes, d_rec_len, d_rec_part, d_dst, dst_cap,
-                                             _ptr(dst_off), _ptr(dst_len), C.addressof(total), _ptr(cks), _ptr(st)),
-           "b2s_partition_compress_dev")
-    return dict(dst_off=dst_off, dst_len=dst_len, total=total.value, checksums=cks, status=st)
+    return _partition_call("b2s_partition_compress_dev", codec, level, block_size, checksum_alg, num_partitions,
+                           (num_partitions, n_records, d_records, rec_bytes, d_rec_len, d_rec_part), d_dst, dst_cap,
+                           dev)
 
 
 def partition_compress_rows_hash_packed(codec, records, rec_len, keys, num_partitions, dst, block_size=0,
@@ -941,29 +958,17 @@ def partition_compress_rows_hash_packed(codec, records, rec_len, keys, num_parti
     id Spark's pmod(Murmur3Hash(key columns, 42), num_partitions); keys as in decompress_sort_rows_keys_packed, no
     order flags; a type OR-ed with KEY_NULL_SAFE hashes as its (coalesce(v, default), isnull(v)) key pair.
     -> dict(dst_off, dst_len, total, checksums, status)"""
-    records, dst = _as_u8(records), _as_u8(dst)
-    rec_len = np.ascontiguousarray(rec_len, dtype=np.uint32)
-    nk, kt, ko, kl, kn = _key_arrays(keys)
-    dst_off, dst_len, cks, st = _partition_out(num_partitions)
-    total = _u64(0)
-    _check(load().b2s_partition_compress_rows_hash_packed(
-        codec, level, block_size, checksum_alg, num_partitions, rec_len.size, _ptr(records), records.size,
-        _ptr(rec_len), nk, _ptr(kt), _ptr(ko), _ptr(kl), _ptr(kn), _ptr(dst), dst.size, _ptr(dst_off), _ptr(dst_len),
-        C.addressof(total), _ptr(cks), _ptr(st)), "b2s_partition_compress_rows_hash_packed")
-    return dict(dst_off=dst_off, dst_len=dst_len, total=total.value, checksums=cks, status=st)
+    return _partition_call("b2s_partition_compress_rows_hash_packed", codec, level, block_size, checksum_alg,
+                           num_partitions, (num_partitions, *_records(records, rec_len), *_key_arrays(keys)), dst)
 
 
 def partition_compress_rows_hash_dev(codec, d_records, rec_bytes, d_rec_len, n_records, keys, num_partitions, d_dst,
                                      dst_cap, block_size=0, checksum_alg=CHECKSUM_NONE, level=0, dev=0):
     """partition_compress_rows_hash_packed on device addresses (records, u32 lengths, destination arena)"""
-    nk, kt, ko, kl, kn = _key_arrays(keys)
-    dst_off, dst_len, cks, st = _partition_out(num_partitions)
-    total = _u64(0)
-    _check(load().b2s_partition_compress_rows_hash_dev(
-        dev, codec, level, block_size, checksum_alg, num_partitions, n_records, d_records, rec_bytes, d_rec_len, nk,
-        _ptr(kt), _ptr(ko), _ptr(kl), _ptr(kn), d_dst, dst_cap, _ptr(dst_off), _ptr(dst_len), C.addressof(total),
-        _ptr(cks), _ptr(st)), "b2s_partition_compress_rows_hash_dev")
-    return dict(dst_off=dst_off, dst_len=dst_len, total=total.value, checksums=cks, status=st)
+    return _partition_call("b2s_partition_compress_rows_hash_dev", codec, level, block_size, checksum_alg,
+                           num_partitions,
+                           (num_partitions, n_records, d_records, rec_bytes, d_rec_len, *_key_arrays(keys)), d_dst,
+                           dst_cap, dev)
 
 
 def _partial_agg_arrays(aggs):
@@ -975,40 +980,32 @@ def _partial_agg_arrays(aggs):
     return len(aggs), fn, vt, vo, vn
 
 
+def _set_arrays(sets):
+    """sets = grouping-set masks -> (n_sets, set_mask array)"""
+    sets = list(sets)
+    return len(sets), np.ascontiguousarray(sets or [0], dtype=np.uint32)
+
+
 def aggregate_partition_compress_rows_hash_packed(codec, records, rec_len, keys, aggs, num_partitions, dst,
                                                   block_size=0, checksum_alg=CHECKSUM_NONE, level=0):
     """Spark's HashAggregateExec(Partial) and its hash exchange: the serialized UnsafeRows grouped by the key columns
     (as in partition_compress_rows_hash_packed), the aggregation buffers of aggs (_partial_agg_arrays) folded per key,
     one partial row per key, hash-partitioned and compressed.  -> dict(dst_off, dst_len, total, checksums, status,
     n_groups)"""
-    records, dst = _as_u8(records), _as_u8(dst)
-    rec_len = np.ascontiguousarray(rec_len, dtype=np.uint32)
-    nk, kt, ko, kl, kn = _key_arrays(keys)
-    na, fn, vt, vo, vn = _partial_agg_arrays(aggs)
-    dst_off, dst_len, cks, st = _partition_out(num_partitions)
-    total, groups = _u64(0), _u64(0)
-    _check(load().b2s_aggregate_partition_compress_rows_hash_packed(
-        codec, level, block_size, checksum_alg, num_partitions, rec_len.size, _ptr(records), records.size,
-        _ptr(rec_len), nk, _ptr(kt), _ptr(ko), _ptr(kl), _ptr(kn), na, _ptr(fn), _ptr(vt), _ptr(vo), _ptr(vn),
-        _ptr(dst), dst.size, _ptr(dst_off), _ptr(dst_len), C.addressof(total), _ptr(cks), _ptr(st),
-        C.addressof(groups)), "b2s_aggregate_partition_compress_rows_hash_packed")
-    return dict(dst_off=dst_off, dst_len=dst_len, total=total.value, checksums=cks, status=st, n_groups=groups.value)
+    return _partition_call("b2s_aggregate_partition_compress_rows_hash_packed", codec, level, block_size,
+                           checksum_alg, num_partitions,
+                           (num_partitions, *_records(records, rec_len), *_key_arrays(keys),
+                            *_partial_agg_arrays(aggs)), dst, counts=("n_groups",))
 
 
 def aggregate_partition_compress_rows_hash_dev(codec, d_records, rec_bytes, d_rec_len, n_records, keys, aggs,
                                                num_partitions, d_dst, dst_cap, block_size=0,
                                                checksum_alg=CHECKSUM_NONE, level=0, dev=0):
     """aggregate_partition_compress_rows_hash_packed on device addresses (records, u32 lengths, destination arena)"""
-    nk, kt, ko, kl, kn = _key_arrays(keys)
-    na, fn, vt, vo, vn = _partial_agg_arrays(aggs)
-    dst_off, dst_len, cks, st = _partition_out(num_partitions)
-    total, groups = _u64(0), _u64(0)
-    _check(load().b2s_aggregate_partition_compress_rows_hash_dev(
-        dev, codec, level, block_size, checksum_alg, num_partitions, n_records, d_records, rec_bytes, d_rec_len, nk,
-        _ptr(kt), _ptr(ko), _ptr(kl), _ptr(kn), na, _ptr(fn), _ptr(vt), _ptr(vo), _ptr(vn), d_dst, dst_cap,
-        _ptr(dst_off), _ptr(dst_len), C.addressof(total), _ptr(cks), _ptr(st), C.addressof(groups)),
-        "b2s_aggregate_partition_compress_rows_hash_dev")
-    return dict(dst_off=dst_off, dst_len=dst_len, total=total.value, checksums=cks, status=st, n_groups=groups.value)
+    return _partition_call("b2s_aggregate_partition_compress_rows_hash_dev", codec, level, block_size, checksum_alg,
+                           num_partitions,
+                           (num_partitions, n_records, d_records, rec_bytes, d_rec_len, *_key_arrays(keys),
+                            *_partial_agg_arrays(aggs)), d_dst, dst_cap, dev, counts=("n_groups",))
 
 
 DISTINCT_ALL_COLUMNS = -1  # B2S_DISTINCT_ALL_COLUMNS: count(DISTINCT every distinct column)
@@ -1061,19 +1058,10 @@ def aggregate_grouping_sets_partition_compress_rows_hash_packed(codec, records, 
     aggregate_partition_compress_rows_hash_packed, each record once per grouping set (sets: one mask per set, bit c for
     key column c), the partial rows keyed by the grouping columns and spark_grouping_id.  -> dict(dst_off, dst_len,
     total, checksums, status, n_groups)"""
-    records, dst = _as_u8(records), _as_u8(dst)
-    rec_len = np.ascontiguousarray(rec_len, dtype=np.uint32)
-    nk, kt, ko, kl, kn = _key_arrays(keys)
-    na, fn, vt, vo, vn = _partial_agg_arrays(aggs)
-    masks = np.ascontiguousarray(list(sets) or [0], dtype=np.uint32)
-    dst_off, dst_len, cks, st = _partition_out(num_partitions)
-    total, groups = _u64(0), _u64(0)
-    _check(load().b2s_aggregate_grouping_sets_partition_compress_rows_hash_packed(
-        codec, level, block_size, checksum_alg, num_partitions, rec_len.size, _ptr(records), records.size,
-        _ptr(rec_len), nk, _ptr(kt), _ptr(ko), _ptr(kl), _ptr(kn), na, _ptr(fn), _ptr(vt), _ptr(vo), _ptr(vn),
-        len(sets), _ptr(masks), _ptr(dst), dst.size, _ptr(dst_off), _ptr(dst_len), C.addressof(total), _ptr(cks),
-        _ptr(st), C.addressof(groups)), "b2s_aggregate_grouping_sets_partition_compress_rows_hash_packed")
-    return dict(dst_off=dst_off, dst_len=dst_len, total=total.value, checksums=cks, status=st, n_groups=groups.value)
+    return _partition_call("b2s_aggregate_grouping_sets_partition_compress_rows_hash_packed", codec, level,
+                           block_size, checksum_alg, num_partitions,
+                           (num_partitions, *_records(records, rec_len), *_key_arrays(keys),
+                            *_partial_agg_arrays(aggs), *_set_arrays(sets)), dst, counts=("n_groups",))
 
 
 def aggregate_grouping_sets_partition_compress_rows_hash_dev(codec, d_records, rec_bytes, d_rec_len, n_records, keys,
@@ -1081,17 +1069,10 @@ def aggregate_grouping_sets_partition_compress_rows_hash_dev(codec, d_records, r
                                                              checksum_alg=CHECKSUM_NONE, level=0, dev=0):
     """aggregate_grouping_sets_partition_compress_rows_hash_packed on device addresses (records, u32 lengths,
     destination arena)"""
-    nk, kt, ko, kl, kn = _key_arrays(keys)
-    na, fn, vt, vo, vn = _partial_agg_arrays(aggs)
-    masks = np.ascontiguousarray(list(sets) or [0], dtype=np.uint32)
-    dst_off, dst_len, cks, st = _partition_out(num_partitions)
-    total, groups = _u64(0), _u64(0)
-    _check(load().b2s_aggregate_grouping_sets_partition_compress_rows_hash_dev(
-        dev, codec, level, block_size, checksum_alg, num_partitions, n_records, d_records, rec_bytes, d_rec_len, nk,
-        _ptr(kt), _ptr(ko), _ptr(kl), _ptr(kn), na, _ptr(fn), _ptr(vt), _ptr(vo), _ptr(vn), len(sets), _ptr(masks),
-        d_dst, dst_cap, _ptr(dst_off), _ptr(dst_len), C.addressof(total), _ptr(cks), _ptr(st), C.addressof(groups)),
-        "b2s_aggregate_grouping_sets_partition_compress_rows_hash_dev")
-    return dict(dst_off=dst_off, dst_len=dst_len, total=total.value, checksums=cks, status=st, n_groups=groups.value)
+    return _partition_call("b2s_aggregate_grouping_sets_partition_compress_rows_hash_dev", codec, level, block_size,
+                           checksum_alg, num_partitions,
+                           (num_partitions, n_records, d_records, rec_bytes, d_rec_len, *_key_arrays(keys),
+                            *_partial_agg_arrays(aggs), *_set_arrays(sets)), d_dst, dst_cap, dev, counts=("n_groups",))
 
 
 def window_limit_partition_compress_rows_hash_packed(codec, records, rec_len, keys, n_partition_keys, limit_fn, limit,
@@ -1102,32 +1083,20 @@ def window_limit_partition_compress_rows_hash_packed(codec, records, rec_len, ke
     WINDOW_RANK or WINDOW_DENSE_RANK) value in their partition is at most limit kept and hash-partitioned by the partition
     columns (none: SinglePartition, num_partitions 1).  -> dict(dst_off, dst_len, total, checksums, status,
     n_out_records)"""
-    records, dst = _as_u8(records), _as_u8(dst)
-    rec_len = np.ascontiguousarray(rec_len, dtype=np.uint32)
-    nk, kt, ko, kl, kn = _key_arrays(keys)
-    dst_off, dst_len, cks, st = _partition_out(num_partitions)
-    total, kept = _u64(0), _u64(0)
-    _check(load().b2s_window_limit_partition_compress_rows_hash_packed(
-        codec, level, block_size, checksum_alg, num_partitions, rec_len.size, _ptr(records), records.size,
-        _ptr(rec_len), n_partition_keys, nk, _ptr(kt), _ptr(ko), _ptr(kl), _ptr(kn), limit_fn, limit, _ptr(dst),
-        dst.size, _ptr(dst_off), _ptr(dst_len), C.addressof(total), _ptr(cks), _ptr(st), C.addressof(kept)),
-        "b2s_window_limit_partition_compress_rows_hash_packed")
-    return dict(dst_off=dst_off, dst_len=dst_len, total=total.value, checksums=cks, status=st, n_out_records=kept.value)
+    return _partition_call("b2s_window_limit_partition_compress_rows_hash_packed", codec, level, block_size,
+                           checksum_alg, num_partitions,
+                           (num_partitions, *_records(records, rec_len), n_partition_keys, *_key_arrays(keys),
+                            limit_fn, limit), dst, counts=("n_out_records",))
 
 
 def window_limit_partition_compress_rows_hash_dev(codec, d_records, rec_bytes, d_rec_len, n_records, keys,
                                                   n_partition_keys, limit_fn, limit, num_partitions, d_dst, dst_cap,
                                                   block_size=0, checksum_alg=CHECKSUM_NONE, level=0, dev=0):
     """window_limit_partition_compress_rows_hash_packed on device addresses (records, u32 lengths, destination arena)"""
-    nk, kt, ko, kl, kn = _key_arrays(keys)
-    dst_off, dst_len, cks, st = _partition_out(num_partitions)
-    total, kept = _u64(0), _u64(0)
-    _check(load().b2s_window_limit_partition_compress_rows_hash_dev(
-        dev, codec, level, block_size, checksum_alg, num_partitions, n_records, d_records, rec_bytes, d_rec_len,
-        n_partition_keys, nk, _ptr(kt), _ptr(ko), _ptr(kl), _ptr(kn), limit_fn, limit, d_dst, dst_cap, _ptr(dst_off),
-        _ptr(dst_len), C.addressof(total), _ptr(cks), _ptr(st), C.addressof(kept)),
-        "b2s_window_limit_partition_compress_rows_hash_dev")
-    return dict(dst_off=dst_off, dst_len=dst_len, total=total.value, checksums=cks, status=st, n_out_records=kept.value)
+    return _partition_call("b2s_window_limit_partition_compress_rows_hash_dev", codec, level, block_size, checksum_alg,
+                           num_partitions,
+                           (num_partitions, n_records, d_records, rec_bytes, d_rec_len, n_partition_keys,
+                            *_key_arrays(keys), limit_fn, limit), d_dst, dst_cap, dev, counts=("n_out_records",))
 
 
 def _bound_arrays(bounds):
@@ -1144,32 +1113,20 @@ def partition_compress_rows_range_packed(codec, records, rec_len, keys, bounds, 
     id Spark's RangePartitioner id of its key over the bounds (framed rows, _bound_arrays); len(bounds) + 1 partitions;
     keys as in decompress_sort_rows_keys_packed, order flags included.  -> dict(dst_off, dst_len, total, checksums,
     status)"""
-    records, dst = _as_u8(records), _as_u8(dst)
-    rec_len = np.ascontiguousarray(rec_len, dtype=np.uint32)
-    nk, kt, ko, kl, kn = _key_arrays(keys)
-    nb, bb, bbytes, bl = _bound_arrays(bounds)
-    dst_off, dst_len, cks, st = _partition_out(nb + 1)
-    total = _u64(0)
-    _check(load().b2s_partition_compress_rows_range_packed(
-        codec, level, block_size, checksum_alg, rec_len.size, _ptr(records), records.size, _ptr(rec_len), nk, _ptr(kt),
-        _ptr(ko), _ptr(kl), _ptr(kn), nb, _ptr(bb), bbytes, _ptr(bl), _ptr(dst), dst.size, _ptr(dst_off),
-        _ptr(dst_len), C.addressof(total), _ptr(cks), _ptr(st)), "b2s_partition_compress_rows_range_packed")
-    return dict(dst_off=dst_off, dst_len=dst_len, total=total.value, checksums=cks, status=st)
+    bounds = _bound_arrays(bounds)
+    return _partition_call("b2s_partition_compress_rows_range_packed", codec, level, block_size, checksum_alg,
+                           bounds[0] + 1, (*_records(records, rec_len), *_key_arrays(keys), *bounds), dst)
 
 
 def partition_compress_rows_range_dev(codec, d_records, rec_bytes, d_rec_len, n_records, keys, bounds, d_dst, dst_cap,
                                       block_size=0, checksum_alg=CHECKSUM_NONE, level=0, dev=0):
     """partition_compress_rows_range_packed on device addresses (records, u32 lengths, destination arena); the bounds
     stay host memory"""
-    nk, kt, ko, kl, kn = _key_arrays(keys)
-    nb, bb, bbytes, bl = _bound_arrays(bounds)
-    dst_off, dst_len, cks, st = _partition_out(nb + 1)
-    total = _u64(0)
-    _check(load().b2s_partition_compress_rows_range_dev(
-        dev, codec, level, block_size, checksum_alg, n_records, d_records, rec_bytes, d_rec_len, nk, _ptr(kt), _ptr(ko),
-        _ptr(kl), _ptr(kn), nb, _ptr(bb), bbytes, _ptr(bl), d_dst, dst_cap, _ptr(dst_off), _ptr(dst_len),
-        C.addressof(total), _ptr(cks), _ptr(st)), "b2s_partition_compress_rows_range_dev")
-    return dict(dst_off=dst_off, dst_len=dst_len, total=total.value, checksums=cks, status=st)
+    bounds = _bound_arrays(bounds)
+    return _partition_call("b2s_partition_compress_rows_range_dev", codec, level, block_size, checksum_alg,
+                           bounds[0] + 1,
+                           (n_records, d_records, rec_bytes, d_rec_len, *_key_arrays(keys), *bounds), d_dst,
+                           dst_cap, dev)
 
 
 def partition_compress_rows_round_robin_packed(codec, records, rec_len, num_partitions, start_position, sort_rows,
@@ -1177,28 +1134,19 @@ def partition_compress_rows_round_robin_packed(codec, records, rec_len, num_part
     """partition_compress_packed of serialized UnsafeRows ([int32 big-endian size][row] each) in Spark's repartition(n)
     order and ids: sorted by (row hash, row bytes) when sort_rows and num_partitions > 1, then the k-th row to
     (start_position + 1 + k) % num_partitions.  -> dict(dst_off, dst_len, total, checksums, status)"""
-    records, dst = _as_u8(records), _as_u8(dst)
-    rec_len = np.ascontiguousarray(rec_len, dtype=np.uint32)
-    dst_off, dst_len, cks, st = _partition_out(num_partitions)
-    total = _u64(0)
-    _check(load().b2s_partition_compress_rows_round_robin_packed(
-        codec, level, block_size, checksum_alg, num_partitions, start_position, sort_rows, rec_len.size, _ptr(records),
-        records.size, _ptr(rec_len), _ptr(dst), dst.size, _ptr(dst_off), _ptr(dst_len), C.addressof(total), _ptr(cks),
-        _ptr(st)), "b2s_partition_compress_rows_round_robin_packed")
-    return dict(dst_off=dst_off, dst_len=dst_len, total=total.value, checksums=cks, status=st)
+    return _partition_call("b2s_partition_compress_rows_round_robin_packed", codec, level, block_size, checksum_alg,
+                           num_partitions,
+                           (num_partitions, start_position, sort_rows, *_records(records, rec_len)), dst)
 
 
 def partition_compress_rows_round_robin_dev(codec, d_records, rec_bytes, d_rec_len, n_records, num_partitions,
                                             start_position, sort_rows, d_dst, dst_cap, block_size=0,
                                             checksum_alg=CHECKSUM_NONE, level=0, dev=0):
     """partition_compress_rows_round_robin_packed on device addresses (records, u32 lengths, destination arena)"""
-    dst_off, dst_len, cks, st = _partition_out(num_partitions)
-    total = _u64(0)
-    _check(load().b2s_partition_compress_rows_round_robin_dev(
-        dev, codec, level, block_size, checksum_alg, num_partitions, start_position, sort_rows, n_records, d_records,
-        rec_bytes, d_rec_len, d_dst, dst_cap, _ptr(dst_off), _ptr(dst_len), C.addressof(total), _ptr(cks), _ptr(st)),
-        "b2s_partition_compress_rows_round_robin_dev")
-    return dict(dst_off=dst_off, dst_len=dst_len, total=total.value, checksums=cks, status=st)
+    return _partition_call("b2s_partition_compress_rows_round_robin_dev", codec, level, block_size, checksum_alg,
+                           num_partitions,
+                           (num_partitions, start_position, sort_rows, n_records, d_records, rec_bytes, d_rec_len),
+                           d_dst, dst_cap, dev)
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -1214,16 +1162,10 @@ def partition_compress_cached_packed(shuffle_id, map_id, codec, records, rec_len
                                      block_size=0, checksum_alg=CHECKSUM_NONE, level=0):
     """partition_compress_packed that also keeps the partitioned records as the cache entry (shuffle_id, map_id).
     -> dict(dst_off, dst_len, total, checksums, status, cached)"""
-    records, dst = _as_u8(records), _as_u8(dst)
-    rec_len = np.ascontiguousarray(rec_len, dtype=np.uint32)
-    rec_part = np.ascontiguousarray(rec_part, dtype=np.uint32)
-    dst_off, dst_len, cks, st = _partition_out(num_partitions)
-    total, cached = _u64(0), _i32(0)
-    _check(load().b2s_partition_compress_cached_packed(
-        shuffle_id, map_id, codec, level, block_size, checksum_alg, num_partitions, rec_len.size, _ptr(records),
-        records.size, _ptr(rec_len), _ptr(rec_part), _ptr(dst), dst.size, _ptr(dst_off), _ptr(dst_len),
-        C.addressof(total), _ptr(cks), _ptr(st), C.addressof(cached)), "b2s_partition_compress_cached_packed")
-    return dict(dst_off=dst_off, dst_len=dst_len, total=total.value, checksums=cks, status=st, cached=cached.value)
+    return _partition_call("b2s_partition_compress_cached_packed", codec, level, block_size, checksum_alg,
+                           num_partitions,
+                           (num_partitions, *_records(records, rec_len), np.ascontiguousarray(rec_part, np.uint32)),
+                           dst, lead=(shuffle_id, map_id), counts=("cached",))
 
 
 def exchange_lookup(shuffle_id, start_reduce, end_reduce, map_ids):
@@ -1277,41 +1219,23 @@ def exchange_read_sort_dev(shuffle_id, start_reduce, end_reduce, map_ids, cached
                       lead=(shuffle_id, start_reduce, end_reduce, ids, cm), n=ids.size)
 
 
-def _rows_cached(symbol, shuffle_id, map_id, codec, level, block_size, checksum_alg, num_partitions, mid, records,
-                 rec_len, dst):
-    """One cached row store: symbol's arguments are shuffle_id, map_id, codec, level, block_size, checksum_alg, *mid
-    (the call's own, numpy arrays among them passed as pointers, with n_records, records and rec_len in their places
-    given as None), dst, dst_cap, the per-partition outputs, cached.
-    -> dict(dst_off, dst_len, total, checksums, status, cached)"""
-    records, dst = _as_u8(records), _as_u8(dst)
-    rec_len = np.ascontiguousarray(rec_len, dtype=np.uint32)
-    fill = iter((rec_len.size, records, records.size, rec_len))
-    mid = [next(fill) if a is None else a for a in mid]
-    dst_off, dst_len, cks, st = _partition_out(num_partitions)
-    total, cached = _u64(0), _i32(0)
-    _check(getattr(load(), symbol)(
-        shuffle_id, map_id, codec, level, block_size, checksum_alg, *map(_arg, mid), _ptr(dst), dst.size,
-        _ptr(dst_off), _ptr(dst_len), C.addressof(total), _ptr(cks), _ptr(st), C.addressof(cached)), symbol)
-    return dict(dst_off=dst_off, dst_len=dst_len, total=total.value, checksums=cks, status=st, cached=cached.value)
-
-
 def partition_compress_rows_hash_cached_packed(shuffle_id, map_id, codec, records, rec_len, keys, num_partitions, dst,
                                                block_size=0, checksum_alg=CHECKSUM_NONE, level=0):
     """partition_compress_rows_hash_packed that also keeps the partitioned rows and their record boundaries as the cache
     entry (shuffle_id, map_id).  -> dict(dst_off, dst_len, total, checksums, status, cached)"""
-    return _rows_cached("b2s_partition_compress_rows_hash_cached_packed", shuffle_id, map_id, codec, level, block_size,
-                        checksum_alg, num_partitions,
-                        (num_partitions, None, None, None, None, *_key_arrays(keys)), records, rec_len, dst)
+    return _partition_call("b2s_partition_compress_rows_hash_cached_packed", codec, level, block_size, checksum_alg,
+                           num_partitions, (num_partitions, *_records(records, rec_len), *_key_arrays(keys)), dst,
+                           lead=(shuffle_id, map_id), counts=("cached",))
 
 
 def partition_compress_rows_range_cached_packed(shuffle_id, map_id, codec, records, rec_len, keys, bounds, dst,
                                                 block_size=0, checksum_alg=CHECKSUM_NONE, level=0):
     """partition_compress_rows_range_packed that also keeps the partitioned rows and their record boundaries as the
     cache entry (shuffle_id, map_id).  -> dict(dst_off, dst_len, total, checksums, status, cached)"""
-    nb, bb, bbytes, bl = _bound_arrays(bounds)
-    return _rows_cached("b2s_partition_compress_rows_range_cached_packed", shuffle_id, map_id, codec, level,
-                        block_size, checksum_alg, nb + 1,
-                        (None, None, None, None, *_key_arrays(keys), nb, bb, bbytes, bl), records, rec_len, dst)
+    bounds = _bound_arrays(bounds)
+    return _partition_call("b2s_partition_compress_rows_range_cached_packed", codec, level, block_size, checksum_alg,
+                           bounds[0] + 1, (*_records(records, rec_len), *_key_arrays(keys), *bounds), dst,
+                           lead=(shuffle_id, map_id), counts=("cached",))
 
 
 def partition_compress_rows_round_robin_cached_packed(shuffle_id, map_id, codec, records, rec_len, num_partitions,
@@ -1319,9 +1243,10 @@ def partition_compress_rows_round_robin_cached_packed(shuffle_id, map_id, codec,
                                                       checksum_alg=CHECKSUM_NONE, level=0):
     """partition_compress_rows_round_robin_packed that also keeps the partitioned rows and their record boundaries as
     the cache entry (shuffle_id, map_id).  -> dict(dst_off, dst_len, total, checksums, status, cached)"""
-    return _rows_cached("b2s_partition_compress_rows_round_robin_cached_packed", shuffle_id, map_id, codec, level,
-                        block_size, checksum_alg, num_partitions,
-                        (num_partitions, start_position, sort_rows, None, None, None, None), records, rec_len, dst)
+    return _partition_call("b2s_partition_compress_rows_round_robin_cached_packed", codec, level, block_size,
+                           checksum_alg, num_partitions,
+                           (num_partitions, start_position, sort_rows, *_records(records, rec_len)), dst,
+                           lead=(shuffle_id, map_id), counts=("cached",))
 
 
 def exchange_read_sort_rows_keys_packed(shuffle_id, start_reduce, end_reduce, map_ids, cached, codec, src, off,

@@ -15,6 +15,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <map>
 #include <mutex>
 #include <optional>
@@ -826,7 +827,7 @@ int get_device(uint32_t dev_index, Device** out) {
 
 // the kinds of call whose steps add_times reads into b2s_last_timing, one rule each
 enum class Family {
-  kCodec, kPartition, kPartitionNone, kSort, kSortRows, kAggregate, kJoin, kWindow, kPartialAggregate, kDistinctAggregate
+  kCodec, kPartition, kPartitionNone, kSort, kSortRows, kAggregate, kJoin, kWindow, kPartialAggregate
 };
 
 // Adds the times of this call's steps on S to b2s_last_timing: kernel_ms, top_kernel_ms, dominant_ms / _launches by
@@ -866,14 +867,9 @@ void add_times(Slot& S, Family f) {
       }
       if (f == Family::kAggregate || f == Family::kJoin || f == Family::kWindow) dominant(G0, G1);
       break;
-    case Family::kPartialAggregate:  // aggregation + partition step + compression (or checksums); the codec step (or
-                                     // the partition step); the aggregation step
-      t.kernel_ms += S.span(G0, S.mine(K1) ? K1 : P1);
-      t.top_kernel_ms += S.mine(T0) ? S.span(T0, T1) : S.span(P0, P1);
-      dominant(G0, G1);
-      break;
-    case Family::kDistinctAggregate:  // read + stage 2 (the call adds their span) + stage 3 + partition step +
-                                      // compression; the codec step (or the partition step); stage 3
+    case Family::kPartialAggregate:  // a map-side step (aggregation, window limit, or the DISTINCT call's stage 3, whose
+                                     // read and stage 2 the call adds) + partition step + compression (or checksums);
+                                     // the codec step (or the partition step); the map-side step
       t.kernel_ms += S.span(G0, S.mine(K1) ? K1 : P1);
       t.top_kernel_ms += S.mine(T0) ? S.span(T0, T1) : S.span(P0, P1);
       dominant(G0, G1);
@@ -1822,19 +1818,46 @@ static uint64_t first_record_past(const uint64_t* d_off, const uint32_t* d_len, 
   return lo;
 }
 
-// How a rows call computes its reduce ids on the device: Spark's HashPartitioning ids of the rows by these key columns,
-// or (range) its RangePartitioner ids over n_bounds bound rows of bound_bytes in host memory, bound_len[j] each, or
-// (round_robin) its RoundRobinPartitioning ids from position start, the rows sorted first when sort is set
+// Where a partition call's reduce ids come from: the caller's (kGiven, one per record), or computed from the rows on
+// the device: Spark's HashPartitioning ids by the key columns (kHash), its RangePartitioner ids over n_bounds bound rows
+// of bound_bytes in host memory, bound_len[j] each (kRange), or its RoundRobinPartitioning ids from position start, the
+// rows sorted first when sort is set (kRoundRobin)
 struct RowIds {
+  enum Kind { kGiven, kHash, kRange, kRoundRobin } kind = kGiven;
   KeySpec keys;
-  bool range = false;
   uint32_t n_bounds = 0;
   const uint8_t* bound_base = nullptr;
   uint64_t bound_bytes = 0;
   const uint32_t* bound_len = nullptr;
-  bool round_robin = false;
   uint32_t start = 0;
   bool sort = false;
+
+  static RowIds hash(const KeySpec& keys) {
+    RowIds ids;
+    ids.kind = kHash;
+    ids.keys = keys;
+    return ids;
+  }
+  static RowIds range(const KeySpec& keys, uint32_t n_bounds, const uint8_t* bound_base, uint64_t bound_bytes,
+                      const uint32_t* bound_len) {
+    RowIds ids;
+    ids.kind = kRange;
+    ids.keys = keys;
+    ids.n_bounds = n_bounds;
+    ids.bound_base = bound_base;
+    ids.bound_bytes = bound_bytes;
+    ids.bound_len = bound_len;
+    return ids;
+  }
+  // SinglePartition: the range ids of no bounds, every id 0, with every record still checked by the range kernel
+  static RowIds single_partition(const KeySpec& keys) { return range(keys, 0, nullptr, 0, nullptr); }
+  static RowIds round_robin(int32_t start, uint32_t sort) {
+    RowIds ids;
+    ids.kind = kRoundRobin;
+    ids.start = (uint32_t)start;
+    ids.sort = sort != 0;
+    return ids;
+  }
 };
 
 // The B2S_E_ARG of a rows call's verdict word (~0: none): a bad record (kHashBad*, launch_rows_hash), or for a range
@@ -1847,12 +1870,12 @@ static int row_ids_verdict(const RowIds& ids, uint64_t v) {
                                     "a decimal key's size is not 1..16 or it runs past its row"};
   static const char* const rec_why[] = {"", "rec_len is below 4", "its size prefix is not rec_len - 4"};
   char msg[256];
-  if (ids.round_robin) {
+  if (ids.kind == RowIds::kRoundRobin) {
     snprintf(msg, sizeof msg, "record %llu is not a serialized UnsafeRow: %s", (unsigned long long)(v >> 3),
              (v & 7) == kRowsBadWords ? "its row size is not a multiple of 8" : rec_why[v & 7]);
     return fail(B2S_E_ARG, "%s", msg);
   }
-  if (ids.range && !(v & kRangeBadRecord)) {
+  if (ids.kind == RowIds::kRange && !(v & kRangeBadRecord)) {
     if ((v & 7) == kRangeBadOrder)
       snprintf(msg, sizeof msg, "bound %llu is not above the bound before it: the bounds must be strictly increasing",
                (unsigned long long)(v >> 3));
@@ -1913,53 +1936,55 @@ static int round_robin_order(Slot& S, const RowIds& ids, uint64_t n, const uint8
 // The partition step and the compression of the non-empty partitions, on device-resident records.  d_dst receives the
 // .data arena (dst_cap bytes); *arena_bytes the bytes it needs.  Returns B2S_E_DST_TOO_SMALL (status[] set for the
 // partitions that do not fit) when dst_cap is short.  part_start (optional) receives the R + 1 partition offsets of the
-// partitioned records, which are in d_dst (codec NONE) or S.parena.  ids (d_part unused): the ids are computed from the
-// rows on the device (RowIds), between the offsets and the radix passes (marks F0 and F1 bracket that step: the hash
-// kernel, the range call's bound checks and id kernel, or the round-robin call's hash, sort and id kernel), and a bad
-// record or bound fails the call.  plan (optional, n > 0): receives the partition plan, whose arrays in S.pws outlive
-// the call until the slot's next use (compression does not touch them).
+// partitioned records, which are in d_dst (codec NONE) or S.parena.  ids: given (d_part), or computed from the rows on
+// the device between the offsets and the radix passes (marks F0 and F1 bracket that step: the hash kernel, the range
+// call's bound checks and id kernel, or the round-robin call's hash, sort and id kernel), where a bad record or bound
+// fails the call.  plan (optional, n > 0): receives the partition plan, whose arrays in S.pws outlive the call until
+// the slot's next use (compression does not touch them).
 static int partition_compress_run(Device* D, Slot& S, uint32_t codec, int32_t level, uint32_t bs, uint32_t alg,
                                   uint32_t R, uint64_t n, const uint8_t* d_rec, uint64_t rec_bytes,
                                   const uint32_t* d_len, const uint32_t* d_part, uint8_t* d_dst, uint64_t dst_cap,
                                   uint64_t* dst_off, uint64_t* dst_len, uint64_t* checksum_out, int32_t* status,
-                                  uint64_t* arena_bytes, uint64_t* launches,
-                                  std::vector<uint64_t>* part_start = nullptr, const RowIds* ids = nullptr,
-                                  PartitionPlan* plan = nullptr) {
+                                  uint64_t* arena_bytes, uint64_t* launches, std::vector<uint64_t>* part_start,
+                                  const RowIds& ids, PartitionPlan* plan) {
   cudaStream_t st = S.st;
   std::vector<uint64_t> pstart(R), plen(R);
-  const bool range = ids && ids->range;
-  const bool rr = ids && ids->round_robin, rr_sort = rr && ids->sort && R > 1;  // R == 1: Spark does not sort
+  const bool given = ids.kind == RowIds::kGiven, range = ids.kind == RowIds::kRange;
+  const bool rr_sort = ids.kind == RowIds::kRoundRobin && ids.sort && R > 1;  // R == 1: Spark does not sort
   CU(S.mark(P0, st));
   PartitionPlan P;
   if (n) {
-    const size_t pws = partition_ws_bytes(n, R, ids != nullptr);
+    const size_t pws = partition_ws_bytes(n, R, !given);
     const size_t sws = rr_sort ? rows_sort_ws_bytes(n, kKeyPrefixBytes) : 0;
-    int rc = S.pws.ensure(pws + (range ? rows_range_ws_bytes(ids->n_bounds, ids->bound_bytes) : 0) +
+    int rc = S.pws.ensure(pws + (range ? rows_range_ws_bytes(ids.n_bounds, ids.bound_bytes) : 0) +
                           (rr_sort ? sws + rows_refine_ws_bytes(n, 0) : 0));
     if (rc) return rc;
     uint8_t* ws = (uint8_t*)S.pws.p;
     RangeWs rw;
     if (range)
-      if (int rc = upload_bounds(*ids, ws + pws, &rw, st)) return rc;
-    if (ids) {
+      if (int rc = upload_bounds(ids, ws + pws, &rw, st)) return rc;
+    if (given) {
+      launch_partition(d_len, d_part, n, R, ws, &P, st, launches);
+    } else {
       launch_partition_offsets(d_len, nullptr, n, R, ws, &P, st, launches);
       CU(S.mark(F0, st, *launches));
       const uint32_t* order = nullptr;
-      if (rr) {
-        if (int rc = round_robin_order(S, *ids, n, d_rec, rec_bytes, d_len, P, rr_sort ? ws + pws : nullptr,
-                                       rr_sort ? ws + pws + sws : nullptr, &order, launches))
-          return rc;
-        launch_rows_round_robin_ids(n, ids->start, R, P.ids, st, launches);
-      } else if (range) {
-        launch_rows_range(d_rec, rec_bytes, P.src_off, d_len, n, ids->keys, rw, ids->n_bounds, P.ids, P.readback, st,
-                          launches);
-      } else {
-        launch_rows_hash(d_rec, rec_bytes, P.src_off, d_len, n, ids->keys, R, P.ids, P.readback, st, launches);
+      switch (ids.kind) {
+        case RowIds::kRoundRobin:
+          if (int rc = round_robin_order(S, ids, n, d_rec, rec_bytes, d_len, P, rr_sort ? ws + pws : nullptr,
+                                         rr_sort ? ws + pws + sws : nullptr, &order, launches))
+            return rc;
+          launch_rows_round_robin_ids(n, ids.start, R, P.ids, st, launches);
+          break;
+        case RowIds::kRange:
+          launch_rows_range(d_rec, rec_bytes, P.src_off, d_len, n, ids.keys, rw, ids.n_bounds, P.ids, P.readback, st,
+                            launches);
+          break;
+        default:
+          launch_rows_hash(d_rec, rec_bytes, P.src_off, d_len, n, ids.keys, R, P.ids, P.readback, st, launches);
       }
       CU(S.mark(F1, st, *launches));
       launch_partition_order(d_len, P.ids, n, R, ws, &P, st, launches, order);
-    } else {
-      launch_partition(d_len, d_part, n, R, ws, &P, st, launches);
     }
     // the one readback between the partition step and compression: [bad id (ids: bad record or bound), byte total,
     // partition offsets]
@@ -1970,7 +1995,7 @@ static int partition_compress_run(Device* D, Slot& S, uint32_t codec, int32_t le
     CU(cudaStreamSynchronize(st));
     CU(cudaGetLastError());
     char msg[256];
-    if (ids && rb[0] != ~0ull) return row_ids_verdict(*ids, rb[0]);
+    if (!given && rb[0] != ~0ull) return row_ids_verdict(ids, rb[0]);
     if (rb[0] != ~0ull) {
       uint32_t id = 0;
       CU(cudaMemcpy(&id, d_part + rb[0], 4, cudaMemcpyDeviceToHost));
@@ -1997,14 +2022,14 @@ static int partition_compress_run(Device* D, Slot& S, uint32_t codec, int32_t le
     if (plan) *plan = P;
   } else if (rec_bytes) {
     return fail(B2S_E_ARG, "rec_len sums to 0 bytes, rec_bytes is %s", std::to_string(rec_bytes).c_str());
-  } else if (range && ids->n_bounds) {  // no records: the bounds are still checked, with a readback of their verdict
-    int rc = S.pws.ensure(rows_range_ws_bytes(ids->n_bounds, ids->bound_bytes));
+  } else if (range && ids.n_bounds) {  // no records: the bounds are still checked, with a readback of their verdict
+    int rc = S.pws.ensure(rows_range_ws_bytes(ids.n_bounds, ids.bound_bytes));
     if (rc) return rc;
     RangeWs rw;
-    if (int rc = upload_bounds(*ids, (uint8_t*)S.pws.p, &rw, st)) return rc;
+    if (int rc = upload_bounds(ids, (uint8_t*)S.pws.p, &rw, st)) return rc;
     CU(cudaMemsetAsync(rw.verdict, 0xff, 8, st));
     CU(S.mark(F0, st, *launches));
-    launch_rows_range(nullptr, 0, nullptr, nullptr, 0, ids->keys, rw, ids->n_bounds, nullptr, rw.verdict, st,
+    launch_rows_range(nullptr, 0, nullptr, nullptr, 0, ids.keys, rw, ids.n_bounds, nullptr, rw.verdict, st,
                       launches);
     CU(S.mark(F1, st, *launches));
     rc = S.hmeta.ensure(8);
@@ -2013,7 +2038,7 @@ static int partition_compress_run(Device* D, Slot& S, uint32_t codec, int32_t le
     CU(cudaStreamSynchronize(st));
     CU(cudaGetLastError());
     const uint64_t v = *(const uint64_t*)S.hmeta.p;
-    if (v != ~0ull) return row_ids_verdict(*ids, v);
+    if (v != ~0ull) return row_ids_verdict(ids, v);
   }
   if (part_start) {
     part_start->assign(pstart.begin(), pstart.end());
@@ -2091,64 +2116,50 @@ static int partition_compress_run(Device* D, Slot& S, uint32_t codec, int32_t le
   return 0;
 }
 
-// ids: the ids are computed from the rows, so rec_part is not read
-static int partition_args(uint32_t codec, uint32_t bs, uint32_t alg, uint32_t R, uint64_t n, const void* rec_base,
-                          uint64_t rec_bytes, const uint32_t* rec_len, const uint32_t* rec_part, const void* dst_base,
-                          const uint64_t* dst_off, const uint64_t* dst_len, const int32_t* status,
-                          const RowIds* ids) {
-  if (alg > B2S_CHECKSUM_CRC32C) return fail(B2S_E_UNSUPPORTED, "Unsupported shuffle checksum algorithm%s");
-  if (codec != B2S_CODEC_NONE)
-    if (int rc = check_codec_block(codec, bs)) return rc;
-  if (R < 1 || R > (1u << 24)) return fail(B2S_E_ARG, "num_partitions must be in [1, 2^24]%s");
-  if (n > 0xffffffffull) return fail(B2S_E_ARG, "more than 2^32 - 1 records in one call%s");
-  if ((n && (!rec_len || (!rec_part && !ids))) || (rec_bytes && !rec_base) || !dst_off || !dst_len || !status)
+// What every map-side partition call takes besides its records: the device (packed: the thread's), the codec step's
+// settings, num_partitions, and the caller's .data arena with its per-partition outputs
+struct MapCall {
+  bool packed;
+  uint32_t dev_index;
+  uint32_t codec;
+  int32_t level;
+  uint32_t bs;  // block_size_or_default's
+  uint32_t alg;
+  uint32_t R;
+  uint8_t* dst_base;
+  uint64_t dst_cap;
+  uint64_t* dst_off;
+  uint64_t* dst_len;
+  uint64_t* dst_total;
+  uint64_t* checksum_out;
+  int32_t* status;
+};
+
+// n records of bytes at rec, their lengths at len: a call's input (host memory when packed), or the rows its own step
+// left on the slot
+struct MapRows {
+  uint64_t n;
+  const uint8_t* rec;
+  uint64_t bytes;
+  const uint32_t* len;
+};
+
+// rec_part is read only for given ids
+static int partition_args(const MapCall& c, const MapRows& in, const uint32_t* rec_part, const RowIds& ids) {
+  if (c.alg > B2S_CHECKSUM_CRC32C) return fail(B2S_E_UNSUPPORTED, "Unsupported shuffle checksum algorithm%s");
+  if (c.codec != B2S_CODEC_NONE)
+    if (int rc = check_codec_block(c.codec, c.bs)) return rc;
+  if (c.R < 1 || c.R > (1u << 24)) return fail(B2S_E_ARG, "num_partitions must be in [1, 2^24]%s");
+  if (in.n > 0xffffffffull) return fail(B2S_E_ARG, "more than 2^32 - 1 records in one call%s");
+  if ((in.n && (!in.len || (!rec_part && ids.kind == RowIds::kGiven))) || (in.bytes && !in.rec) || !c.dst_off ||
+      !c.dst_len || !c.status)
     return fail(B2S_E_ARG, "null argument%s");
-  if (rec_bytes && !dst_base) return fail(B2S_E_ARG, "null argument%s");
+  if (in.bytes && !c.dst_base) return fail(B2S_E_ARG, "null argument%s");
   return 0;
 }
 
 static Family partition_family(uint32_t codec) {
   return codec == B2S_CODEC_NONE ? Family::kPartitionNone : Family::kPartition;
-}
-
-static int partition_compress_dev(uint32_t dev_index, uint32_t codec, int32_t level, uint32_t codec_block_size,
-                                  uint32_t checksum_alg, uint32_t num_partitions, uint64_t n_records,
-                                  const uint8_t* rec_base, uint64_t rec_bytes, const uint32_t* rec_len,
-                                  const uint32_t* rec_part, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_off,
-                                  uint64_t* dst_len, uint64_t* dst_total, uint64_t* checksum_out, int32_t* status,
-                                  const RowIds* ids) {
-  const WallTimer wt = begin_call();
-  if (dst_total) *dst_total = 0;
-  const uint32_t bs = block_size_or_default(codec_block_size);
-  int rc = partition_args(codec, bs, checksum_alg, num_partitions, n_records, rec_base, rec_bytes, rec_len, rec_part,
-                          dst_base, dst_off, dst_len, status, ids);
-  if (rc) return rc;
-  Device* D;
-  rc = get_device(dev_index, &D);
-  if (rc) return rc;
-  Lane& Ln = D->lane[kLaneWrite];
-  std::lock_guard<std::mutex> lk(Ln.mtx);
-  Slot& S = Ln.slot[0];
-  std::vector<uint64_t> cks(num_partitions);
-  uint64_t launches = 0, arena = 0;
-  rc = partition_compress_run(D, S, codec, level, bs, checksum_alg, num_partitions, n_records, rec_base, rec_bytes,
-                              rec_len, rec_part, dst_base, dst_cap, dst_off, dst_len, cks.data(), status, &arena,
-                              &launches, nullptr, ids);
-  if (rc && rc != B2S_E_DST_TOO_SMALL) return rc;
-  if (checksum_out) memcpy(checksum_out, cks.data(), (size_t)num_partitions * 8);
-  if (dst_total) *dst_total = arena;
-  end_call(wt, launches, CallBytes{rec_bytes, arena, 0, 0}, &S, partition_family(codec));
-  return rc;
-}
-
-int b2s_partition_compress_dev(uint32_t dev_index, uint32_t codec, int32_t level, uint32_t codec_block_size,
-                               uint32_t checksum_alg, uint32_t num_partitions, uint64_t n_records,
-                               const uint8_t* rec_base, uint64_t rec_bytes, const uint32_t* rec_len,
-                               const uint32_t* rec_part, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_off,
-                               uint64_t* dst_len, uint64_t* dst_total, uint64_t* checksum_out, int32_t* status) {
-  return partition_compress_dev(dev_index, codec, level, codec_block_size, checksum_alg, num_partitions, n_records,
-                                rec_base, rec_bytes, rec_len, rec_part, dst_base, dst_cap, dst_off, dst_len, dst_total,
-                                checksum_out, status, nullptr);
 }
 
 // what a cached store keeps: the exchange-cache key and where to report whether it was stored
@@ -2158,79 +2169,138 @@ struct ExStore {
   int32_t* cached;
 };
 
-static int partition_compress_packed(uint32_t codec, int32_t level, uint32_t codec_block_size, uint32_t checksum_alg,
-                                     uint32_t num_partitions, uint64_t n_records, const uint8_t* rec_base,
-                                     uint64_t rec_bytes, const uint32_t* rec_len, const uint32_t* rec_part,
-                                     uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_off, uint64_t* dst_len,
-                                     uint64_t* dst_total, uint64_t* checksum_out, int32_t* status,
-                                     const ExStore* store, const RowIds* ids = nullptr) {
-  const WallTimer wt = begin_call();
-  if (dst_total) *dst_total = 0;
-  const uint32_t bs = block_size_or_default(codec_block_size);
-  int rc = partition_args(codec, bs, checksum_alg, num_partitions, n_records, rec_base, rec_bytes, rec_len, rec_part,
-                          dst_base, dst_off, dst_len, status, ids);
-  if (rc) return rc;
+// the largest whole-task buffer a call keeps for the next one (SortBufferTrim, PartialAggTrim)
+constexpr size_t kSortKeepBytes = 1ull << 30;
+
+// The aggregation step's buffers, sized by the call's records (staged and folded values, the partial rows), are given
+// back when the call ends if they are larger than the sorts keep, so one large map task does not hold them for the life
+// of the process
+struct PartialAggTrim {
+  Slot& S;
+  ~PartialAggTrim() {
+    for (DevBuf* b : {&S.fws, &S.aggrows, &S.xrows})
+      if (b->cap > kSortKeepBytes) b->release();
+  }
+};
+
+// The partition + compress step of a map-side call over the rows on S (its own step's, or its records), with the ids
+// of ids (given: d_part), into the caller's arena, or (packed) into S.dst, sized by the bound, then one download of what
+// fits (*fit bytes), a short caller arena flagged after the run.  Sets the per-partition outputs and *dst_total to the
+// *arena bytes the arena needs; B2S_E_DST_TOO_SMALL leaves them set.  store (packed): the partitioned records, with a
+// rows call's record boundaries, kept as an exchange-cache entry when the call succeeds.
+static int partition_tail(Device* D, Slot& S, const MapCall& c, const MapRows& rows, const uint32_t* d_part,
+                          const RowIds& ids, const ExStore* store, uint64_t* arena, uint64_t* fit,
+                          uint64_t* launches) {
+  cudaStream_t st = S.st;
+  uint8_t* d_dst = c.dst_base;
+  uint64_t cap = c.dst_cap;
+  if (c.packed) {
+    if (int rc = S.dst.ensure(b2s_partition_compress_bound(c.codec, c.bs, c.R, rows.bytes) + 64)) return rc;
+    d_dst = (uint8_t*)S.dst.p;
+    cap = S.dst.cap;
+  }
+  std::vector<uint64_t> cks(c.R), part_start;
+  PartitionPlan P;
+  int rc = partition_compress_run(D, S, c.codec, c.level, c.bs, c.alg, c.R, rows.n, rows.rec, rows.bytes, rows.len,
+                                  d_part, d_dst, cap, c.dst_off, c.dst_len, cks.data(), c.status, arena, launches,
+                                  store ? &part_start : nullptr, ids, &P);
+  if (rc && rc != B2S_E_DST_TOO_SMALL) return rc;
+  *fit = 0;
+  if (c.packed) {
+    *fit = std::min(*arena, c.dst_cap);
+    if (*arena > c.dst_cap) {
+      for (uint32_t p = 0; p < c.R; p++)
+        if (c.dst_len[p] && c.dst_off[p] + c.dst_len[p] > c.dst_cap) c.status[p] = B2S_E_DST_TOO_SMALL;
+      rc = fail(B2S_E_DST_TOO_SMALL, "dst_cap is below the %s bytes of the .data arena", std::to_string(*arena).c_str());
+    }
+    CU(S.mark(D0, st));
+    if (*fit) CU(cudaMemcpyAsync(c.dst_base, S.dst.p, *fit, cudaMemcpyDeviceToHost, st));
+    CU(S.mark(D1, st));
+    CU(cudaStreamSynchronize(st));
+    CU(cudaGetLastError());
+  }
+  if (c.checksum_out) memcpy(c.checksum_out, cks.data(), (size_t)c.R * 8);
+  if (c.dst_total) *c.dst_total = *arena;
+  if (store && !rc) {
+    // the partitioned records are still in this slot (its lane is held): in front of compression, or the arena itself
+    // for codec NONE
+    const uint8_t* parts = (const uint8_t*)(c.codec == B2S_CODEC_NONE ? S.dst.p : S.parena.p);
+    // a rows call's entry keeps its record boundaries: the plan's offsets, also still in this slot (S.pws); S.hmeta
+    // (only grown) has held the partition step's readback of R + 2 words
+    ExBounds rb{&P, rows.n, (uint64_t*)S.hmeta.p, launches};
+    *store->cached = ex_store(D->ordinal, st, store->shuffle, store->map, parts, rows.bytes, std::move(part_start),
+                              ids.kind == RowIds::kGiven ? nullptr : &rb);
+  }
+  return rc;
+}
+
+// A map-side call's own step on S: from its records on the device to the rows it partitions (launches: its count)
+using MapStep = std::function<int(Slot& S, const MapRows& records, MapRows* rows, uint64_t* launches)>;
+
+// the step of a call that partitions its records as they are
+static int pass_through(Slot&, const MapRows& in, MapRows* rows, uint64_t*) {
+  *rows = in;
+  return 0;
+}
+
+// A map-side call on the write lane's slot 0, after its checks.  Without a usable device a rows call reports B2S_E_CUDA
+// (as the sort calls do) and a call with given ids B2S_E_NOT_INIT.  Then (packed) one upload of [records | rec_len |
+// rec_part, for given ids] between marks H0 and H1 (the whole map output is partitioned at once: no chunking), the
+// call's step to the rows it partitions (*n_out: how many), and the partition + compress step over them.
+static int write_lane_run(const WallTimer& wt, const MapCall& c, const MapRows& in, const uint32_t* rec_part,
+                          const RowIds& ids, const ExStore* store, Family f, uint64_t* n_out, const MapStep& step) {
+  const bool given = ids.kind == RowIds::kGiven;
+  if (!given && !g_ctx)
+    if (int rc = no_device()) return rc;
   Device* D;
-  rc = get_device(t_device, &D);
-  if (rc) return rc;
+  if (int rc = get_device(c.packed ? t_device : c.dev_index, &D)) return rc;
   Lane& Ln = D->lane[kLaneWrite];
   std::lock_guard<std::mutex> lk(Ln.mtx);
   Slot& S = Ln.slot[0];
-  // one upload of [records | rec_len | rec_part]; the whole map output is partitioned at once, so there is no chunking
-  const size_t rec_sz = align_up(rec_bytes, 16), len_sz = align_up(n_records * 4, 16);
-  rc = S.src.ensure(rec_sz + 2 * len_sz + 64);
-  if (rc) return rc;
-  const uint64_t bound = b2s_partition_compress_bound(codec, bs, num_partitions, rec_bytes);
-  rc = S.dst.ensure(bound + 64);
-  if (rc) return rc;
-  uint8_t* d_rec = (uint8_t*)S.src.p;
-  uint32_t* d_len = (uint32_t*)(d_rec + rec_sz);
-  uint32_t* d_part = (uint32_t*)(d_rec + rec_sz + len_sz);
+  const PartialAggTrim trim{S};
   cudaStream_t st = S.st;
-  CU(S.mark(H0, st));
-  if (rec_bytes) CU(cudaMemcpyAsync(d_rec, rec_base, rec_bytes, cudaMemcpyHostToDevice, st));
-  if (n_records) {
-    CU(cudaMemcpyAsync(d_len, rec_len, n_records * 4, cudaMemcpyHostToDevice, st));
-    if (!ids) CU(cudaMemcpyAsync(d_part, rec_part, n_records * 4, cudaMemcpyHostToDevice, st));
+  MapRows d_in = in;
+  const uint32_t* d_part = rec_part;
+  if (c.packed) {
+    const size_t rec_sz = align_up(in.bytes, 16), len_sz = align_up(in.n * 4, 16);
+    if (int rc = S.src.ensure(rec_sz + (given ? 2 : 1) * len_sz + 64)) return rc;
+    uint8_t* d = (uint8_t*)S.src.p;
+    d_in.rec = d;
+    d_in.len = (const uint32_t*)(d + rec_sz);
+    d_part = (const uint32_t*)(d + rec_sz + len_sz);
+    CU(S.mark(H0, st));
+    if (in.bytes) CU(cudaMemcpyAsync(d, in.rec, in.bytes, cudaMemcpyHostToDevice, st));
+    if (in.n) {
+      CU(cudaMemcpyAsync(d + rec_sz, in.len, in.n * 4, cudaMemcpyHostToDevice, st));
+      if (given) CU(cudaMemcpyAsync(d + rec_sz + len_sz, rec_part, in.n * 4, cudaMemcpyHostToDevice, st));
+    }
+    CU(S.mark(H1, st));
   }
-  CU(S.mark(H1, st));
-  std::vector<uint64_t> cks(num_partitions), part_start;
-  uint64_t launches = 0, arena = 0;
-  PartitionPlan P;
-  rc = partition_compress_run(D, S, codec, level, bs, checksum_alg, num_partitions, n_records, d_rec, rec_bytes, d_len,
-                              d_part, (uint8_t*)S.dst.p, S.dst.cap, dst_off, dst_len, cks.data(), status, &arena,
-                              &launches, store ? &part_start : nullptr, ids, &P);
-  if (rc) return rc;
-  // the device arena is sized by the bound, so a short caller arena shows up here: copy what fits, flag the rest
-  int result = 0;
-  uint64_t fit = arena;
-  if (arena > dst_cap) {
-    fit = dst_cap;
-    for (uint32_t p = 0; p < num_partitions; p++)
-      if (dst_len[p] && dst_off[p] + dst_len[p] > dst_cap) status[p] = B2S_E_DST_TOO_SMALL;
-    result = fail(B2S_E_DST_TOO_SMALL, "dst_cap is below the %s bytes of the .data arena", std::to_string(arena).c_str());
-  }
-  CU(S.mark(D0, st));
-  if (fit) CU(cudaMemcpyAsync(dst_base, S.dst.p, fit, cudaMemcpyDeviceToHost, st));
-  CU(S.mark(D1, st));
-  CU(cudaStreamSynchronize(st));
-  CU(cudaGetLastError());
-  if (checksum_out) memcpy(checksum_out, cks.data(), (size_t)num_partitions * 8);
-  if (dst_total) *dst_total = arena;
-  if (store && !result) {
-    // the partitioned records are still in this slot (the write lane is held): in front of compression, or the arena
-    // itself for codec NONE
-    const uint8_t* parts = (const uint8_t*)(codec == B2S_CODEC_NONE ? S.dst.p : S.parena.p);
-    // a row writer's entry keeps its record boundaries: the plan's offsets, also still in this slot (S.pws); S.hmeta
-    // (only grown) has held the partition step's readback of R + 2 words
-    ExBounds rb{&P, n_records, (uint64_t*)S.hmeta.p, &launches};
-    *store->cached = ex_store(D->ordinal, st, store->shuffle, store->map, parts, rec_bytes, std::move(part_start),
-                              ids ? &rb : nullptr);
-  }
-  const uint64_t h2d = rec_bytes + n_records * (ids ? 4 : 8) + (ids && ids->range ? ids->bound_bytes : 0);
-  end_call(wt, launches, CallBytes{rec_bytes, arena, h2d, fit}, &S,
-           partition_family(codec));
-  return result;
+  uint64_t launches = 0, arena = 0, fit = 0;
+  MapRows rows{};
+  if (int rc = step(S, d_in, &rows, &launches)) return rc;
+  const int rc = partition_tail(D, S, c, rows, d_part, ids, store, &arena, &fit, &launches);
+  if (rc && rc != B2S_E_DST_TOO_SMALL) return rc;
+  if (n_out) *n_out = rows.n;
+  const uint64_t h2d =
+      c.packed ? in.bytes + in.n * (given ? 8 : 4) + (ids.kind == RowIds::kRange ? ids.bound_bytes : 0) : 0;
+  end_call(wt, launches, CallBytes{in.bytes, arena, h2d, fit}, &S, f);
+  return rc;
+}
+
+int b2s_partition_compress_dev(uint32_t dev_index, uint32_t codec, int32_t level, uint32_t codec_block_size,
+                               uint32_t checksum_alg, uint32_t num_partitions, uint64_t n_records,
+                               const uint8_t* rec_base, uint64_t rec_bytes, const uint32_t* rec_len,
+                               const uint32_t* rec_part, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_off,
+                               uint64_t* dst_len, uint64_t* dst_total, uint64_t* checksum_out, int32_t* status) {
+  const WallTimer wt = begin_call();
+  if (dst_total) *dst_total = 0;
+  const MapCall c{false, dev_index, codec, level, block_size_or_default(codec_block_size), checksum_alg,
+                  num_partitions, dst_base, dst_cap, dst_off, dst_len, dst_total, checksum_out, status};
+  const MapRows in{n_records, rec_base, rec_bytes, rec_len};
+  const RowIds ids;
+  if (int rc = partition_args(c, in, rec_part, ids)) return rc;
+  return write_lane_run(wt, c, in, rec_part, ids, nullptr, partition_family(codec), nullptr, pass_through);
 }
 
 int b2s_partition_compress_packed(uint32_t codec, int32_t level, uint32_t codec_block_size, uint32_t checksum_alg,
@@ -2238,9 +2308,14 @@ int b2s_partition_compress_packed(uint32_t codec, int32_t level, uint32_t codec_
                                   uint64_t rec_bytes, const uint32_t* rec_len, const uint32_t* rec_part,
                                   uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_off, uint64_t* dst_len,
                                   uint64_t* dst_total, uint64_t* checksum_out, int32_t* status) {
-  return partition_compress_packed(codec, level, codec_block_size, checksum_alg, num_partitions, n_records, rec_base,
-                                   rec_bytes, rec_len, rec_part, dst_base, dst_cap, dst_off, dst_len, dst_total,
-                                   checksum_out, status, nullptr);
+  const WallTimer wt = begin_call();
+  if (dst_total) *dst_total = 0;
+  const MapCall c{true, 0, codec, level, block_size_or_default(codec_block_size), checksum_alg,
+                  num_partitions, dst_base, dst_cap, dst_off, dst_len, dst_total, checksum_out, status};
+  const MapRows in{n_records, rec_base, rec_bytes, rec_len};
+  const RowIds ids;
+  if (int rc = partition_args(c, in, rec_part, ids)) return rc;
+  return write_lane_run(wt, c, in, rec_part, ids, nullptr, partition_family(codec), nullptr, pass_through);
 }
 
 int b2s_partition_compress_cached_packed(int32_t shuffle_id, int64_t map_id, uint32_t codec, int32_t level,
@@ -2252,10 +2327,15 @@ int b2s_partition_compress_cached_packed(int32_t shuffle_id, int64_t map_id, uin
   if (!cached) return fail(B2S_E_ARG, "null argument%s");
   *cached = 0;
   if (int rc = exchange_ready()) return rc;
+  const WallTimer wt = begin_call();
+  if (dst_total) *dst_total = 0;
+  const MapCall c{true, 0, codec, level, block_size_or_default(codec_block_size), checksum_alg,
+                  num_partitions, dst_base, dst_cap, dst_off, dst_len, dst_total, checksum_out, status};
+  const MapRows in{n_records, rec_base, rec_bytes, rec_len};
+  const RowIds ids;
+  if (int rc = partition_args(c, in, rec_part, ids)) return rc;
   const ExStore store{shuffle_id, map_id, cached};
-  return partition_compress_packed(codec, level, codec_block_size, checksum_alg, num_partitions, n_records, rec_base,
-                                   rec_bytes, rec_len, rec_part, dst_base, dst_cap, dst_off, dst_len, dst_total,
-                                   checksum_out, status, &store);
+  return write_lane_run(wt, c, in, rec_part, ids, &store, partition_family(codec), nullptr, pass_through);
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -3002,41 +3082,19 @@ static int sort_device(uint32_t dev_index, Device** out) {
 // write side, hash-partitioned rows: Spark's HashPartitioning id of every row, then the partition + compress step
 // ------------------------------------------------------------------------------------------------------------
 // The composite calls' column rules, then what a hash takes: no order flags, B2S_KEY_BYTES only as a 1-byte boolean.
-// With the partition step's own checks first, so that without a usable device a well-formed call reports B2S_E_CUDA
-// (as the sort calls do) and an ill-formed one B2S_E_ARG.
-static int hash_args(uint32_t codec, uint32_t codec_block_size, uint32_t alg, uint32_t R, uint64_t n,
-                     const void* rec_base, uint64_t rec_bytes, const uint32_t* rec_len, const RecordSpec& spec,
-                     const void* dst_base, const uint64_t* dst_off, const uint64_t* dst_len, const int32_t* status) {
-  const uint32_t bs = block_size_or_default(codec_block_size);
-  const RowIds ids{spec.keys};
-  if (int rc = partition_args(codec, bs, alg, R, n, rec_base, rec_bytes, rec_len, nullptr, dst_base, dst_off, dst_len,
-                              status, &ids))
-    return rc;
+// With the partition step's own checks first.  Like every rows call's checks, these come before the device, so that
+// without a usable device a well-formed call reports B2S_E_CUDA (as the sort calls do) and an ill-formed one B2S_E_ARG.
+static int hash_args(const MapCall& c, const MapRows& in, const RecordSpec& spec) {
+  if (int rc = partition_args(c, in, nullptr, RowIds::hash(spec.keys))) return rc;
   if (int rc = key_columns_args(spec)) return rc;
-  for (uint32_t c = 0; c < spec.keys.n; c++) {
-    const uint32_t flags = spec.keys.type[c] & ~kKeyTypeMask;
+  for (uint32_t k = 0; k < spec.keys.n; k++) {
+    const uint32_t flags = spec.keys.type[k] & ~kKeyTypeMask;
     if (flags & ~(spec.null_safe ? B2S_KEY_NULL_SAFE : 0))
       return fail(B2S_E_ARG, "a hashed key column takes no order flag%s");
-    if ((spec.keys.type[c] & kKeyTypeMask) == B2S_KEY_BYTES && spec.keys.len[c] != 1)
+    if ((spec.keys.type[k] & kKeyTypeMask) == B2S_KEY_BYTES && spec.keys.len[k] != 1)
       return fail(B2S_E_ARG, "a hashed B2S_KEY_BYTES column is a boolean: key_len must be 1%s");
   }
-  if (!g_ctx)
-    if (int rc = no_device()) return rc;
   return 0;
-}
-
-// A packed rows call's checks, then (store: a cached form) the exchange cache's, before its partition + compress step
-static int rows_packed(const ExStore* store, const RowIds& ids, int args_rc, uint32_t codec, int32_t level,
-                       uint32_t codec_block_size, uint32_t checksum_alg, uint32_t num_partitions, uint64_t n_records,
-                       const uint8_t* rec_base, uint64_t rec_bytes, const uint32_t* rec_len, uint8_t* dst_base,
-                       uint64_t dst_cap, uint64_t* dst_off, uint64_t* dst_len, uint64_t* dst_total,
-                       uint64_t* checksum_out, int32_t* status) {
-  if (args_rc) return args_rc;
-  if (store)
-    if (int rc = exchange_ready()) return rc;
-  return partition_compress_packed(codec, level, codec_block_size, checksum_alg, num_partitions, n_records, rec_base,
-                                   rec_bytes, rec_len, nullptr, dst_base, dst_cap, dst_off, dst_len, dst_total,
-                                   checksum_out, status, store, &ids);
 }
 
 // the outputs a cached store zeroes before its checks: *dst_total, and *cached (B2S_E_ARG when it is NULL)
@@ -3047,21 +3105,12 @@ static int cached_args(uint64_t* dst_total, int32_t* cached) {
   return 0;
 }
 
-static int rows_hash_packed(const ExStore* store, uint32_t codec, int32_t level, uint32_t codec_block_size,
-                            uint32_t checksum_alg, uint32_t num_partitions, uint64_t n_records,
-                            const uint8_t* rec_base, uint64_t rec_bytes, const uint32_t* rec_len, uint32_t n_keys,
-                            const uint32_t* key_type, const uint32_t* key_off, const uint32_t* key_len,
-                            const int32_t* key_null_field, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_off,
-                            uint64_t* dst_len, uint64_t* dst_total, uint64_t* checksum_out, int32_t* status) {
-  if (dst_total) *dst_total = 0;
+// the hash call's key columns: null-safe ones allowed
+static RecordSpec hash_spec(uint32_t n_keys, const uint32_t* key_type, const uint32_t* key_off, const uint32_t* key_len,
+                            const int32_t* key_null_field) {
   RecordSpec spec = keys_spec(n_keys, key_type, key_off, key_len, key_null_field);
   spec.null_safe = true;
-  const RowIds ids{spec.keys};
-  return rows_packed(store, ids,
-                     hash_args(codec, codec_block_size, checksum_alg, num_partitions, n_records, rec_base, rec_bytes,
-                               rec_len, spec, dst_base, dst_off, dst_len, status),
-                     codec, level, codec_block_size, checksum_alg, num_partitions, n_records, rec_base, rec_bytes,
-                     rec_len, dst_base, dst_cap, dst_off, dst_len, dst_total, checksum_out, status);
+  return spec;
 }
 
 int b2s_partition_compress_rows_hash_packed(uint32_t codec, int32_t level, uint32_t codec_block_size,
@@ -3071,9 +3120,15 @@ int b2s_partition_compress_rows_hash_packed(uint32_t codec, int32_t level, uint3
                                             const uint32_t* key_len, const int32_t* key_null_field, uint8_t* dst_base,
                                             uint64_t dst_cap, uint64_t* dst_off, uint64_t* dst_len,
                                             uint64_t* dst_total, uint64_t* checksum_out, int32_t* status) {
-  return rows_hash_packed(nullptr, codec, level, codec_block_size, checksum_alg, num_partitions, n_records, rec_base,
-                          rec_bytes, rec_len, n_keys, key_type, key_off, key_len, key_null_field, dst_base, dst_cap,
-                          dst_off, dst_len, dst_total, checksum_out, status);
+  const WallTimer wt = begin_call();
+  if (dst_total) *dst_total = 0;
+  const MapCall c{true, 0, codec, level, block_size_or_default(codec_block_size), checksum_alg,
+                  num_partitions, dst_base, dst_cap, dst_off, dst_len, dst_total, checksum_out, status};
+  const MapRows in{n_records, rec_base, rec_bytes, rec_len};
+  const RecordSpec spec = hash_spec(n_keys, key_type, key_off, key_len, key_null_field);
+  if (int rc = hash_args(c, in, spec)) return rc;
+  return write_lane_run(wt, c, in, nullptr, RowIds::hash(spec.keys), nullptr, partition_family(codec), nullptr,
+                        pass_through);
 }
 
 int b2s_partition_compress_rows_hash_cached_packed(int32_t shuffle_id, int64_t map_id, uint32_t codec, int32_t level,
@@ -3085,11 +3140,17 @@ int b2s_partition_compress_rows_hash_cached_packed(int32_t shuffle_id, int64_t m
                                                    const int32_t* key_null_field, uint8_t* dst_base, uint64_t dst_cap,
                                                    uint64_t* dst_off, uint64_t* dst_len, uint64_t* dst_total,
                                                    uint64_t* checksum_out, int32_t* status, int32_t* cached) {
+  const WallTimer wt = begin_call();
   if (int rc = cached_args(dst_total, cached)) return rc;
+  const MapCall c{true, 0, codec, level, block_size_or_default(codec_block_size), checksum_alg,
+                  num_partitions, dst_base, dst_cap, dst_off, dst_len, dst_total, checksum_out, status};
+  const MapRows in{n_records, rec_base, rec_bytes, rec_len};
+  const RecordSpec spec = hash_spec(n_keys, key_type, key_off, key_len, key_null_field);
+  if (int rc = hash_args(c, in, spec)) return rc;
+  if (int rc = exchange_ready()) return rc;
   const ExStore store{shuffle_id, map_id, cached};
-  return rows_hash_packed(&store, codec, level, codec_block_size, checksum_alg, num_partitions, n_records, rec_base,
-                          rec_bytes, rec_len, n_keys, key_type, key_off, key_len, key_null_field, dst_base, dst_cap,
-                          dst_off, dst_len, dst_total, checksum_out, status);
+  return write_lane_run(wt, c, in, nullptr, RowIds::hash(spec.keys), &store, partition_family(codec), nullptr,
+                        pass_through);
 }
 
 int b2s_partition_compress_rows_hash_dev(uint32_t dev_index, uint32_t codec, int32_t level, uint32_t codec_block_size,
@@ -3099,16 +3160,15 @@ int b2s_partition_compress_rows_hash_dev(uint32_t dev_index, uint32_t codec, int
                                          const uint32_t* key_len, const int32_t* key_null_field, uint8_t* dst_base,
                                          uint64_t dst_cap, uint64_t* dst_off, uint64_t* dst_len, uint64_t* dst_total,
                                          uint64_t* checksum_out, int32_t* status) {
+  const WallTimer wt = begin_call();
   if (dst_total) *dst_total = 0;
-  RecordSpec spec = keys_spec(n_keys, key_type, key_off, key_len, key_null_field);
-  spec.null_safe = true;
-  const RowIds ids{spec.keys};
-  if (int rc = hash_args(codec, codec_block_size, checksum_alg, num_partitions, n_records, rec_base, rec_bytes, rec_len,
-                         spec, dst_base, dst_off, dst_len, status))
-    return rc;
-  return partition_compress_dev(dev_index, codec, level, codec_block_size, checksum_alg, num_partitions, n_records,
-                                rec_base, rec_bytes, rec_len, nullptr, dst_base, dst_cap, dst_off, dst_len, dst_total,
-                                checksum_out, status, &ids);
+  const MapCall c{false, dev_index, codec, level, block_size_or_default(codec_block_size), checksum_alg,
+                  num_partitions, dst_base, dst_cap, dst_off, dst_len, dst_total, checksum_out, status};
+  const MapRows in{n_records, rec_base, rec_bytes, rec_len};
+  const RecordSpec spec = hash_spec(n_keys, key_type, key_off, key_len, key_null_field);
+  if (int rc = hash_args(c, in, spec)) return rc;
+  return write_lane_run(wt, c, in, nullptr, RowIds::hash(spec.keys), nullptr, partition_family(codec), nullptr,
+                        pass_through);
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -3231,7 +3291,7 @@ static int partial_agg_checked(Slot& S, const PartialAggSpec& spec, uint64_t n, 
   CU(cudaStreamSynchronize(st));
   CU(cudaGetLastError());
   if (rb[0] != ~0ull) {
-    if ((rb[0] & 7) != kPaBadValue) return row_ids_verdict(RowIds{ks}, rb[0]);
+    if ((rb[0] & 7) != kPaBadValue) return row_ids_verdict(RowIds::hash(ks), rb[0]);
     static const char* const why[] = {"", "its row does not hold a value slot", "its row does not hold a value's null word",
                                       "a decimal value's size is not 1..16 or it runs past its row"};
     char msg[256];
@@ -3329,20 +3389,6 @@ static int partial_agg_rows(Slot& S, const PartialAggSpec& spec, uint64_t n, con
   CU(S.mark(G1, st, *launches));
   return 0;
 }
-
-// the largest whole-task buffer a call keeps for the next one (SortBufferTrim, PartialAggTrim)
-constexpr size_t kSortKeepBytes = 1ull << 30;
-
-// The aggregation step's buffers, sized by the call's records (staged and folded values, the partial rows), are given
-// back when the call ends if they are larger than the sorts keep, so one large map task does not hold them for the life
-// of the process
-struct PartialAggTrim {
-  Slot& S;
-  ~PartialAggTrim() {
-    for (DevBuf* b : {&S.fws, &S.aggrows, &S.xrows})
-      if (b->cap > kSortKeepBytes) b->release();
-  }
-};
 
 // b2s_aggregate_grouping_sets_partition_compress_rows_hash_*'s grouping sets: n_sets masks of key columns
 struct GroupingSets {
@@ -3446,49 +3492,9 @@ static int expand_rows(Slot& S, const PartialAggSpec& spec, const PartialAggSpec
   return 0;
 }
 
-// The partition + compress step of a map-side call over the n rows its own step left on S (d_rows, rows_bytes;
-// d_row_len), with the ids of ids, into the caller's arena (packed: into S.dst, sized by the bound, then one download
-// of what fits, *fit bytes; a short caller arena shows up after the run, as in the packed partition call).  Sets
-// dst_off / dst_len / checksum_out / status and *arena; B2S_E_DST_TOO_SMALL leaves them set.
-static int map_rows_partition(Device* D, Slot& S, bool packed, uint32_t codec, int32_t level, uint32_t bs,
-                              uint32_t checksum_alg, uint32_t num_partitions, uint64_t n, const uint8_t* d_rows,
-                              uint64_t rows_bytes, const uint32_t* d_row_len, const RowIds& ids, uint8_t* dst_base,
-                              uint64_t dst_cap, uint64_t* dst_off, uint64_t* dst_len, uint64_t* checksum_out,
-                              int32_t* status, uint64_t* arena, uint64_t* fit, uint64_t* launches) {
-  cudaStream_t st = S.st;
-  uint8_t* d_dst = dst_base;
-  uint64_t cap = dst_cap;
-  int rc;
-  if (packed) {
-    if ((rc = S.dst.ensure(b2s_partition_compress_bound(codec, bs, num_partitions, rows_bytes) + 64))) return rc;
-    d_dst = (uint8_t*)S.dst.p;
-    cap = S.dst.cap;
-  }
-  std::vector<uint64_t> cks(num_partitions);
-  rc = partition_compress_run(D, S, codec, level, bs, checksum_alg, num_partitions, n, d_rows, rows_bytes, d_row_len,
-                              nullptr, d_dst, cap, dst_off, dst_len, cks.data(), status, arena, launches, nullptr, &ids);
-  if (rc && rc != B2S_E_DST_TOO_SMALL) return rc;
-  if (packed) {
-    *fit = std::min(*arena, dst_cap);
-    if (*arena > dst_cap) {
-      for (uint32_t p = 0; p < num_partitions; p++)
-        if (dst_len[p] && dst_off[p] + dst_len[p] > dst_cap) status[p] = B2S_E_DST_TOO_SMALL;
-      rc = fail(B2S_E_DST_TOO_SMALL, "dst_cap is below the %s bytes of the .data arena", std::to_string(*arena).c_str());
-    }
-    CU(S.mark(D0, st));
-    if (*fit) CU(cudaMemcpyAsync(dst_base, S.dst.p, *fit, cudaMemcpyDeviceToHost, st));
-    CU(S.mark(D1, st));
-    CU(cudaStreamSynchronize(st));
-    CU(cudaGetLastError());
-  }
-  if (checksum_out) memcpy(checksum_out, cks.data(), (size_t)num_partitions * 8);
-  return rc;
-}
-
 // b2s_aggregate_partition_compress_rows_hash_* (gs null) and b2s_aggregate_grouping_sets_partition_compress_rows_hash_*:
 // the checks before the device, then on the write lane (with grouping sets, the expansion first) the aggregation step
-// and the partition + compress step over the partial rows, from host records (packed: one upload, one download) or
-// device ones
+// and the partition + compress step over the partial rows
 static int aggregate_partition_call(bool packed, uint32_t dev_index, uint32_t codec, int32_t level,
                                     uint32_t codec_block_size, uint32_t checksum_alg, uint32_t num_partitions,
                                     uint64_t n_records, const uint8_t* rec_base, uint64_t rec_bytes,
@@ -3502,6 +3508,9 @@ static int aggregate_partition_call(bool packed, uint32_t dev_index, uint32_t co
   const WallTimer wt = begin_call();
   if (dst_total) *dst_total = 0;
   if (n_groups) *n_groups = 0;
+  const MapCall c{packed, dev_index, codec, level, block_size_or_default(codec_block_size), checksum_alg,
+                  num_partitions, dst_base, dst_cap, dst_off, dst_len, dst_total, checksum_out, status};
+  const MapRows in{n_records, rec_base, rec_bytes, rec_len};
   const RecordSpec rspec = keys_spec(n_keys, key_type, key_off, key_len, key_null_field);
   PartialAggSpec spec;
   spec.keys = rspec.keys;
@@ -3512,9 +3521,7 @@ static int aggregate_partition_call(bool packed, uint32_t dev_index, uint32_t co
                               : "n_keys + the buffers' fields (3 per VARIANCE) must be at most 32 (one null word)%s");
   if (gs)
     if (int rc = grouping_sets_args(n_keys, n_records, *gs)) return rc;
-  if (int rc = hash_args(codec, codec_block_size, checksum_alg, num_partitions, n_records, rec_base, rec_bytes, rec_len,
-                         rspec, dst_base, dst_off, dst_len, status))
-    return rc;
+  if (int rc = hash_args(c, in, rspec)) return rc;
   PartialAggSpec xagg;  // with grouping sets, the aggregation over the projected records
   ExpandSpec xs;
   if (gs)
@@ -3522,55 +3529,29 @@ static int aggregate_partition_call(bool packed, uint32_t dev_index, uint32_t co
                                     &xagg))
       return rc;
   const PartialAggSpec& step = gs ? xagg : spec;
-  const uint32_t bs = block_size_or_default(codec_block_size);
   if (!n_records && rec_bytes)
     return fail(B2S_E_ARG, "rec_len sums to 0 bytes, rec_bytes is %s", std::to_string(rec_bytes).c_str());
-  Device* D;
-  if (int rc = get_device(packed ? t_device : dev_index, &D)) return rc;
-  Lane& Ln = D->lane[kLaneWrite];
-  std::lock_guard<std::mutex> lk(Ln.mtx);
-  Slot& S = Ln.slot[0];
-  const PartialAggTrim trim{S};
-  cudaStream_t st = S.st;
-  const uint8_t* d_rec = rec_base;
-  const uint32_t* d_len = rec_len;
-  if (packed) {  // one upload of [records | rec_len]
-    const size_t rec_sz = align_up(rec_bytes, 16), len_sz = align_up(n_records * 4, 16);
-    if (int rc = S.src.ensure(rec_sz + len_sz + 64)) return rc;
-    d_rec = (const uint8_t*)S.src.p;
-    d_len = (const uint32_t*)((uint8_t*)S.src.p + rec_sz);
-    CU(S.mark(H0, st));
-    if (rec_bytes) CU(cudaMemcpyAsync((uint8_t*)S.src.p, rec_base, rec_bytes, cudaMemcpyHostToDevice, st));
-    if (n_records) CU(cudaMemcpyAsync((uint8_t*)d_len, rec_len, n_records * 4, cudaMemcpyHostToDevice, st));
-    CU(S.mark(H1, st));
-  }
-  uint64_t launches = 0, groups = 0, rows_bytes = 0, arena = 0;
-  const uint32_t* d_row_len = nullptr;
-  int rc;
-  if (gs) {  // the aggregation step over the projected records; its span (G0, G1) takes in the expansion
-    const uint8_t* x_rec = nullptr;
-    const uint32_t* x_len = nullptr;
-    uint64_t x_bytes = 0;
-    CU(S.mark(G0, st, launches));
-    if ((rc = expand_rows(S, spec, xagg, xs, gs->mask, n_records, d_rec, rec_bytes, d_len, &x_rec, &x_bytes, &x_len,
-                          &launches)))
-      return rc;
-    rc = partial_agg_rows(S, step, n_records * gs->n_sets, x_rec, x_bytes, x_len, &groups, &rows_bytes, &d_row_len,
-                          &launches, false);
-  } else {
-    rc = partial_agg_rows(S, spec, n_records, d_rec, rec_bytes, d_len, &groups, &rows_bytes, &d_row_len, &launches);
-  }
-  if (rc) return rc;
-  uint64_t fit = 0;
-  rc = map_rows_partition(D, S, packed, codec, level, bs, checksum_alg, num_partitions, groups,
-                          (const uint8_t*)S.aggrows.p, rows_bytes, d_row_len, RowIds{partial_row_keys(step.keys)},
-                          dst_base, dst_cap, dst_off, dst_len, checksum_out, status, &arena, &fit, &launches);
-  if (rc && rc != B2S_E_DST_TOO_SMALL) return rc;
-  if (dst_total) *dst_total = arena;
-  *n_groups = groups;
-  end_call(wt, launches, CallBytes{rec_bytes, arena, packed ? rec_bytes + n_records * 4 : 0, fit}, &S,
-           Family::kPartialAggregate);
-  return rc;
+  auto aggregate = [&](Slot& S, const MapRows& d_in, MapRows* rows, uint64_t* launches) -> int {
+    int rc;
+    if (gs) {  // the aggregation step over the projected records; its span (G0, G1) takes in the expansion
+      const uint8_t* x_rec = nullptr;
+      const uint32_t* x_len = nullptr;
+      uint64_t x_bytes = 0;
+      CU(S.mark(G0, S.st, *launches));
+      if ((rc = expand_rows(S, spec, xagg, xs, gs->mask, d_in.n, d_in.rec, d_in.bytes, d_in.len, &x_rec, &x_bytes,
+                            &x_len, launches)))
+        return rc;
+      rc = partial_agg_rows(S, step, d_in.n * gs->n_sets, x_rec, x_bytes, x_len, &rows->n, &rows->bytes, &rows->len,
+                            launches, false);
+    } else {
+      rc = partial_agg_rows(S, spec, d_in.n, d_in.rec, d_in.bytes, d_in.len, &rows->n, &rows->bytes, &rows->len,
+                            launches);
+    }
+    rows->rec = (const uint8_t*)S.aggrows.p;
+    return rc;
+  };
+  return write_lane_run(wt, c, in, nullptr, RowIds::hash(partial_row_keys(step.keys)), nullptr,
+                        Family::kPartialAggregate, n_groups, aggregate);
 }
 
 int b2s_aggregate_partition_compress_rows_hash_packed(
@@ -3704,8 +3685,7 @@ static int window_limit_rows(Slot& S, const KeySpec& ks, const WindowShape& shap
 }
 
 // b2s_window_limit_partition_compress_rows_hash_*: the checks before the device, then on the write lane the limit step
-// and the partition + compress step over the kept rows, hashed by the partition columns (none: every id 0, the range
-// ids of no bounds), from host records (packed: one upload, one download) or device ones
+// and the partition + compress step over the kept rows, hashed by the partition columns (none: SinglePartition)
 static int window_limit_partition_call(bool packed, uint32_t dev_index, uint32_t codec, int32_t level,
                                        uint32_t codec_block_size, uint32_t checksum_alg, uint32_t num_partitions,
                                        uint64_t n_records, const uint8_t* rec_base, uint64_t rec_bytes,
@@ -3718,63 +3698,25 @@ static int window_limit_partition_call(bool packed, uint32_t dev_index, uint32_t
   const WallTimer wt = begin_call();
   if (dst_total) *dst_total = 0;
   if (n_out_records) *n_out_records = 0;
+  const MapCall c{packed, dev_index, codec, level, block_size_or_default(codec_block_size), checksum_alg,
+                  num_partitions, dst_base, dst_cap, dst_off, dst_len, dst_total, checksum_out, status};
+  const MapRows in{n_records, rec_base, rec_bytes, rec_len};
   const RecordSpec spec = keys_spec(n_keys, key_type, key_off, key_len, key_null_field);
   if (int rc = window_limit_args(spec, n_partition_keys, limit_fn, limit, num_partitions, n_out_records)) return rc;
   const RecordSpec pspec = keys_spec(n_partition_keys, key_type, key_off, key_len, key_null_field);
-  RowIds ids{pspec.keys};
-  const uint32_t bs = block_size_or_default(codec_block_size);
-  int rc;
-  if (n_partition_keys) {
-    rc = hash_args(codec, codec_block_size, checksum_alg, num_partitions, n_records, rec_base, rec_bytes, rec_len,
-                   pspec, dst_base, dst_off, dst_len, status);
-  } else {
-    ids.keys = spec.keys;
-    ids.range = true;
-    rc = partition_args(codec, bs, checksum_alg, num_partitions, n_records, rec_base, rec_bytes, rec_len, nullptr,
-                        dst_base, dst_off, dst_len, status, &ids);
-    if (!rc && !g_ctx) rc = no_device();
-  }
-  if (rc) return rc;
+  const RowIds ids = n_partition_keys ? RowIds::hash(pspec.keys) : RowIds::single_partition(spec.keys);
+  if (int rc = n_partition_keys ? hash_args(c, in, pspec) : partition_args(c, in, nullptr, ids)) return rc;
   if (!n_records && rec_bytes)
     return fail(B2S_E_ARG, "rec_len sums to 0 bytes, rec_bytes is %s", std::to_string(rec_bytes).c_str());
   WindowShape shape{};  // no functions: the limit and the partition columns only
   shape.limit_fn = limit_fn;
   shape.limit = limit;
   shape.part = pspec.keys;
-  Device* D;
-  if ((rc = get_device(packed ? t_device : dev_index, &D))) return rc;
-  Lane& Ln = D->lane[kLaneWrite];
-  std::lock_guard<std::mutex> lk(Ln.mtx);
-  Slot& S = Ln.slot[0];
-  const PartialAggTrim trim{S};
-  cudaStream_t st = S.st;
-  const uint8_t* d_rec = rec_base;
-  const uint32_t* d_len = rec_len;
-  if (packed) {  // one upload of [records | rec_len]
-    const size_t rec_sz = align_up(rec_bytes, 16), len_sz = align_up(n_records * 4, 16);
-    if ((rc = S.src.ensure(rec_sz + len_sz + 64))) return rc;
-    d_rec = (const uint8_t*)S.src.p;
-    d_len = (const uint32_t*)((uint8_t*)S.src.p + rec_sz);
-    CU(S.mark(H0, st));
-    if (rec_bytes) CU(cudaMemcpyAsync((uint8_t*)S.src.p, rec_base, rec_bytes, cudaMemcpyHostToDevice, st));
-    if (n_records) CU(cudaMemcpyAsync((uint8_t*)d_len, rec_len, n_records * 4, cudaMemcpyHostToDevice, st));
-    CU(S.mark(H1, st));
-  }
-  uint64_t launches = 0, kept = 0, kept_bytes = 0, arena = 0, fit = 0;
-  const uint32_t* d_kept_len = nullptr;
-  const uint8_t* d_kept = nullptr;
-  if ((rc = window_limit_rows(S, spec.keys, shape, n_records, d_rec, rec_bytes, d_len, &kept, &kept_bytes, &d_kept_len,
-                              &d_kept, &launches)))
-    return rc;
-  rc = map_rows_partition(D, S, packed, codec, level, bs, checksum_alg, num_partitions, kept, d_kept, kept_bytes,
-                          d_kept_len, ids, dst_base, dst_cap, dst_off, dst_len, checksum_out, status, &arena, &fit,
-                          &launches);
-  if (rc && rc != B2S_E_DST_TOO_SMALL) return rc;
-  if (dst_total) *dst_total = arena;
-  *n_out_records = kept;
-  end_call(wt, launches, CallBytes{rec_bytes, arena, packed ? rec_bytes + n_records * 4 : 0, fit}, &S,
-           Family::kPartialAggregate);
-  return rc;
+  auto limit_step = [&](Slot& S, const MapRows& d_in, MapRows* rows, uint64_t* launches) {
+    return window_limit_rows(S, spec.keys, shape, d_in.n, d_in.rec, d_in.bytes, d_in.len, &rows->n, &rows->bytes,
+                             &rows->len, &rows->rec, launches);
+  };
+  return write_lane_run(wt, c, in, nullptr, ids, nullptr, Family::kPartialAggregate, n_out_records, limit_step);
 }
 
 int b2s_window_limit_partition_compress_rows_hash_packed(
@@ -3808,14 +3750,9 @@ int b2s_window_limit_partition_compress_rows_hash_dev(
 // ------------------------------------------------------------------------------------------------------------
 // The composite calls' column rules (order flags allowed), the partition step's checks with n_bounds + 1 partitions,
 // and the bound arrays'; a device is needed only after them, as for the hash call.
-static int range_args(uint32_t codec, uint32_t codec_block_size, uint32_t alg, uint64_t n, const void* rec_base,
-                      uint64_t rec_bytes, const uint32_t* rec_len, const RecordSpec& spec, const RowIds& ids,
-                      const void* dst_base, const uint64_t* dst_off, const uint64_t* dst_len, const int32_t* status) {
+static int range_args(const MapCall& c, const MapRows& in, const RecordSpec& spec, const RowIds& ids) {
   if (ids.n_bounds > (1u << 24) - 1) return fail(B2S_E_ARG, "n_bounds must be at most 2^24 - 1%s");
-  const uint32_t bs = block_size_or_default(codec_block_size);
-  if (int rc = partition_args(codec, bs, alg, ids.n_bounds + 1, n, rec_base, rec_bytes, rec_len, nullptr, dst_base,
-                              dst_off, dst_len, status, &ids))
-    return rc;
+  if (int rc = partition_args(c, in, nullptr, ids)) return rc;
   if (int rc = key_columns_args(spec)) return rc;
   if (ids.n_bounds && (!ids.bound_base || !ids.bound_len)) return fail(B2S_E_ARG, "null argument%s");
   uint64_t sum = 0;
@@ -3826,38 +3763,7 @@ static int range_args(uint32_t codec, uint32_t codec_block_size, uint32_t alg, u
              (unsigned long long)ids.bound_bytes);
     return fail(B2S_E_ARG, "%s", msg);
   }
-  if (!g_ctx)
-    if (int rc = no_device()) return rc;
   return 0;
-}
-
-static RowIds range_ids(const RecordSpec& spec, uint32_t n_bounds, const uint8_t* bound_base, uint64_t bound_bytes,
-                        const uint32_t* bound_len) {
-  RowIds ids;
-  ids.keys = spec.keys;
-  ids.range = true;
-  ids.n_bounds = n_bounds;
-  ids.bound_base = bound_base;
-  ids.bound_bytes = bound_bytes;
-  ids.bound_len = bound_len;
-  return ids;
-}
-
-static int rows_range_packed(const ExStore* store, uint32_t codec, int32_t level, uint32_t codec_block_size,
-                             uint32_t checksum_alg, uint64_t n_records, const uint8_t* rec_base, uint64_t rec_bytes,
-                             const uint32_t* rec_len, uint32_t n_keys, const uint32_t* key_type,
-                             const uint32_t* key_off, const uint32_t* key_len, const int32_t* key_null_field,
-                             uint32_t n_bounds, const uint8_t* bound_base, uint64_t bound_bytes,
-                             const uint32_t* bound_len, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_off,
-                             uint64_t* dst_len, uint64_t* dst_total, uint64_t* checksum_out, int32_t* status) {
-  if (dst_total) *dst_total = 0;
-  const RecordSpec spec = keys_spec(n_keys, key_type, key_off, key_len, key_null_field);
-  const RowIds ids = range_ids(spec, n_bounds, bound_base, bound_bytes, bound_len);
-  return rows_packed(store, ids,
-                     range_args(codec, codec_block_size, checksum_alg, n_records, rec_base, rec_bytes, rec_len, spec,
-                                ids, dst_base, dst_off, dst_len, status),
-                     codec, level, codec_block_size, checksum_alg, n_bounds + 1, n_records, rec_base, rec_bytes,
-                     rec_len, dst_base, dst_cap, dst_off, dst_len, dst_total, checksum_out, status);
 }
 
 int b2s_partition_compress_rows_range_packed(uint32_t codec, int32_t level, uint32_t codec_block_size,
@@ -3869,10 +3775,15 @@ int b2s_partition_compress_rows_range_packed(uint32_t codec, int32_t level, uint
                                              const uint32_t* bound_len, uint8_t* dst_base, uint64_t dst_cap,
                                              uint64_t* dst_off, uint64_t* dst_len, uint64_t* dst_total,
                                              uint64_t* checksum_out, int32_t* status) {
-  return rows_range_packed(nullptr, codec, level, codec_block_size, checksum_alg, n_records, rec_base, rec_bytes,
-                           rec_len, n_keys, key_type, key_off, key_len, key_null_field, n_bounds, bound_base,
-                           bound_bytes, bound_len, dst_base, dst_cap, dst_off, dst_len, dst_total, checksum_out,
-                           status);
+  const WallTimer wt = begin_call();
+  if (dst_total) *dst_total = 0;
+  const MapCall c{true, 0, codec, level, block_size_or_default(codec_block_size), checksum_alg,
+                  n_bounds + 1, dst_base, dst_cap, dst_off, dst_len, dst_total, checksum_out, status};
+  const MapRows in{n_records, rec_base, rec_bytes, rec_len};
+  const RecordSpec spec = keys_spec(n_keys, key_type, key_off, key_len, key_null_field);
+  const RowIds ids = RowIds::range(spec.keys, n_bounds, bound_base, bound_bytes, bound_len);
+  if (int rc = range_args(c, in, spec, ids)) return rc;
+  return write_lane_run(wt, c, in, nullptr, ids, nullptr, partition_family(codec), nullptr, pass_through);
 }
 
 int b2s_partition_compress_rows_range_cached_packed(int32_t shuffle_id, int64_t map_id, uint32_t codec, int32_t level,
@@ -3886,12 +3797,17 @@ int b2s_partition_compress_rows_range_cached_packed(int32_t shuffle_id, int64_t 
                                                     uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_off,
                                                     uint64_t* dst_len, uint64_t* dst_total, uint64_t* checksum_out,
                                                     int32_t* status, int32_t* cached) {
+  const WallTimer wt = begin_call();
   if (int rc = cached_args(dst_total, cached)) return rc;
+  const MapCall c{true, 0, codec, level, block_size_or_default(codec_block_size), checksum_alg,
+                  n_bounds + 1, dst_base, dst_cap, dst_off, dst_len, dst_total, checksum_out, status};
+  const MapRows in{n_records, rec_base, rec_bytes, rec_len};
+  const RecordSpec spec = keys_spec(n_keys, key_type, key_off, key_len, key_null_field);
+  const RowIds ids = RowIds::range(spec.keys, n_bounds, bound_base, bound_bytes, bound_len);
+  if (int rc = range_args(c, in, spec, ids)) return rc;
+  if (int rc = exchange_ready()) return rc;
   const ExStore store{shuffle_id, map_id, cached};
-  return rows_range_packed(&store, codec, level, codec_block_size, checksum_alg, n_records, rec_base, rec_bytes,
-                           rec_len, n_keys, key_type, key_off, key_len, key_null_field, n_bounds, bound_base,
-                           bound_bytes, bound_len, dst_base, dst_cap, dst_off, dst_len, dst_total, checksum_out,
-                           status);
+  return write_lane_run(wt, c, in, nullptr, ids, &store, partition_family(codec), nullptr, pass_through);
 }
 
 int b2s_partition_compress_rows_range_dev(uint32_t dev_index, uint32_t codec, int32_t level, uint32_t codec_block_size,
@@ -3902,15 +3818,15 @@ int b2s_partition_compress_rows_range_dev(uint32_t dev_index, uint32_t codec, in
                                           uint64_t bound_bytes, const uint32_t* bound_len, uint8_t* dst_base,
                                           uint64_t dst_cap, uint64_t* dst_off, uint64_t* dst_len, uint64_t* dst_total,
                                           uint64_t* checksum_out, int32_t* status) {
+  const WallTimer wt = begin_call();
   if (dst_total) *dst_total = 0;
+  const MapCall c{false, dev_index, codec, level, block_size_or_default(codec_block_size), checksum_alg,
+                  n_bounds + 1, dst_base, dst_cap, dst_off, dst_len, dst_total, checksum_out, status};
+  const MapRows in{n_records, rec_base, rec_bytes, rec_len};
   const RecordSpec spec = keys_spec(n_keys, key_type, key_off, key_len, key_null_field);
-  const RowIds ids = range_ids(spec, n_bounds, bound_base, bound_bytes, bound_len);
-  if (int rc = range_args(codec, codec_block_size, checksum_alg, n_records, rec_base, rec_bytes, rec_len, spec, ids,
-                          dst_base, dst_off, dst_len, status))
-    return rc;
-  return partition_compress_dev(dev_index, codec, level, codec_block_size, checksum_alg, n_bounds + 1, n_records,
-                                rec_base, rec_bytes, rec_len, nullptr, dst_base, dst_cap, dst_off, dst_len, dst_total,
-                                checksum_out, status, &ids);
+  const RowIds ids = RowIds::range(spec.keys, n_bounds, bound_base, bound_bytes, bound_len);
+  if (int rc = range_args(c, in, spec, ids)) return rc;
+  return write_lane_run(wt, c, in, nullptr, ids, nullptr, partition_family(codec), nullptr, pass_through);
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -3918,44 +3834,13 @@ int b2s_partition_compress_rows_range_dev(uint32_t dev_index, uint32_t codec, in
 // ------------------------------------------------------------------------------------------------------------
 // The partition step's checks, then the position and sort flag; a device is needed only after them, as for the hash
 // call.  start + n past 2^31 - 1 is refused: Spark's Int position would wrap there.
-static int round_robin_args(uint32_t codec, uint32_t codec_block_size, uint32_t alg, uint32_t R, int32_t start,
-                            uint32_t sort, uint64_t n, const void* rec_base, uint64_t rec_bytes,
-                            const uint32_t* rec_len, const RowIds& ids, const void* dst_base, const uint64_t* dst_off,
-                            const uint64_t* dst_len, const int32_t* status) {
-  const uint32_t bs = block_size_or_default(codec_block_size);
-  if (int rc = partition_args(codec, bs, alg, R, n, rec_base, rec_bytes, rec_len, nullptr, dst_base, dst_off, dst_len,
-                              status, &ids))
-    return rc;
-  if (start < 0 || (uint32_t)start >= R) return fail(B2S_E_ARG, "start_position must be in [0, num_partitions)%s");
+static int round_robin_args(const MapCall& c, const MapRows& in, int32_t start, uint32_t sort) {
+  if (int rc = partition_args(c, in, nullptr, RowIds::round_robin(start, sort))) return rc;
+  if (start < 0 || (uint32_t)start >= c.R) return fail(B2S_E_ARG, "start_position must be in [0, num_partitions)%s");
   if (sort > 1) return fail(B2S_E_ARG, "sort_rows must be 0 or 1%s");
-  if ((uint64_t)start + n > 0x7fffffffull)
+  if ((uint64_t)start + in.n > 0x7fffffffull)
     return fail(B2S_E_ARG, "start_position + n_records is past 2^31 - 1, where Spark's position wraps%s");
-  if (!g_ctx)
-    if (int rc = no_device()) return rc;
   return 0;
-}
-
-static RowIds round_robin_ids(int32_t start, uint32_t sort) {
-  RowIds ids;
-  ids.round_robin = true;
-  ids.start = (uint32_t)start;
-  ids.sort = sort != 0;
-  return ids;
-}
-
-static int rows_round_robin_packed(const ExStore* store, uint32_t codec, int32_t level, uint32_t codec_block_size,
-                                   uint32_t checksum_alg, uint32_t num_partitions, int32_t start_position,
-                                   uint32_t sort_rows, uint64_t n_records, const uint8_t* rec_base, uint64_t rec_bytes,
-                                   const uint32_t* rec_len, uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_off,
-                                   uint64_t* dst_len, uint64_t* dst_total, uint64_t* checksum_out, int32_t* status) {
-  if (dst_total) *dst_total = 0;
-  const RowIds ids = round_robin_ids(start_position, sort_rows);
-  return rows_packed(store, ids,
-                     round_robin_args(codec, codec_block_size, checksum_alg, num_partitions, start_position, sort_rows,
-                                      n_records, rec_base, rec_bytes, rec_len, ids, dst_base, dst_off, dst_len,
-                                      status),
-                     codec, level, codec_block_size, checksum_alg, num_partitions, n_records, rec_base, rec_bytes,
-                     rec_len, dst_base, dst_cap, dst_off, dst_len, dst_total, checksum_out, status);
 }
 
 int b2s_partition_compress_rows_round_robin_packed(uint32_t codec, int32_t level, uint32_t codec_block_size,
@@ -3965,9 +3850,14 @@ int b2s_partition_compress_rows_round_robin_packed(uint32_t codec, int32_t level
                                                    const uint32_t* rec_len, uint8_t* dst_base, uint64_t dst_cap,
                                                    uint64_t* dst_off, uint64_t* dst_len, uint64_t* dst_total,
                                                    uint64_t* checksum_out, int32_t* status) {
-  return rows_round_robin_packed(nullptr, codec, level, codec_block_size, checksum_alg, num_partitions,
-                                 start_position, sort_rows, n_records, rec_base, rec_bytes, rec_len, dst_base, dst_cap,
-                                 dst_off, dst_len, dst_total, checksum_out, status);
+  const WallTimer wt = begin_call();
+  if (dst_total) *dst_total = 0;
+  const MapCall c{true, 0, codec, level, block_size_or_default(codec_block_size), checksum_alg,
+                  num_partitions, dst_base, dst_cap, dst_off, dst_len, dst_total, checksum_out, status};
+  const MapRows in{n_records, rec_base, rec_bytes, rec_len};
+  if (int rc = round_robin_args(c, in, start_position, sort_rows)) return rc;
+  return write_lane_run(wt, c, in, nullptr, RowIds::round_robin(start_position, sort_rows), nullptr,
+                        partition_family(codec), nullptr, pass_through);
 }
 
 int b2s_partition_compress_rows_round_robin_cached_packed(int32_t shuffle_id, int64_t map_id, uint32_t codec,
@@ -3979,11 +3869,16 @@ int b2s_partition_compress_rows_round_robin_cached_packed(int32_t shuffle_id, in
                                                           uint8_t* dst_base, uint64_t dst_cap, uint64_t* dst_off,
                                                           uint64_t* dst_len, uint64_t* dst_total,
                                                           uint64_t* checksum_out, int32_t* status, int32_t* cached) {
+  const WallTimer wt = begin_call();
   if (int rc = cached_args(dst_total, cached)) return rc;
+  const MapCall c{true, 0, codec, level, block_size_or_default(codec_block_size), checksum_alg,
+                  num_partitions, dst_base, dst_cap, dst_off, dst_len, dst_total, checksum_out, status};
+  const MapRows in{n_records, rec_base, rec_bytes, rec_len};
+  if (int rc = round_robin_args(c, in, start_position, sort_rows)) return rc;
+  if (int rc = exchange_ready()) return rc;
   const ExStore store{shuffle_id, map_id, cached};
-  return rows_round_robin_packed(&store, codec, level, codec_block_size, checksum_alg, num_partitions,
-                                 start_position, sort_rows, n_records, rec_base, rec_bytes, rec_len, dst_base, dst_cap,
-                                 dst_off, dst_len, dst_total, checksum_out, status);
+  return write_lane_run(wt, c, in, nullptr, RowIds::round_robin(start_position, sort_rows), &store,
+                        partition_family(codec), nullptr, pass_through);
 }
 
 int b2s_partition_compress_rows_round_robin_dev(uint32_t dev_index, uint32_t codec, int32_t level,
@@ -3993,14 +3888,14 @@ int b2s_partition_compress_rows_round_robin_dev(uint32_t dev_index, uint32_t cod
                                                 const uint32_t* rec_len, uint8_t* dst_base, uint64_t dst_cap,
                                                 uint64_t* dst_off, uint64_t* dst_len, uint64_t* dst_total,
                                                 uint64_t* checksum_out, int32_t* status) {
+  const WallTimer wt = begin_call();
   if (dst_total) *dst_total = 0;
-  const RowIds ids = round_robin_ids(start_position, sort_rows);
-  if (int rc = round_robin_args(codec, codec_block_size, checksum_alg, num_partitions, start_position, sort_rows,
-                                n_records, rec_base, rec_bytes, rec_len, ids, dst_base, dst_off, dst_len, status))
-    return rc;
-  return partition_compress_dev(dev_index, codec, level, codec_block_size, checksum_alg, num_partitions, n_records,
-                                rec_base, rec_bytes, rec_len, nullptr, dst_base, dst_cap, dst_off, dst_len, dst_total,
-                                checksum_out, status, &ids);
+  const MapCall c{false, dev_index, codec, level, block_size_or_default(codec_block_size), checksum_alg,
+                  num_partitions, dst_base, dst_cap, dst_off, dst_len, dst_total, checksum_out, status};
+  const MapRows in{n_records, rec_base, rec_bytes, rec_len};
+  if (int rc = round_robin_args(c, in, start_position, sort_rows)) return rc;
+  return write_lane_run(wt, c, in, nullptr, RowIds::round_robin(start_position, sort_rows), nullptr,
+                        partition_family(codec), nullptr, pass_through);
 }
 
 // The whole-task buffers of a sort call (read-lane slot 0: compressed blocks, decoded arena, sorted copy, sort
@@ -4583,6 +4478,37 @@ static int run_reduce_task(Slot& S, const RecordSpec& spec, DecodedTask& T, uint
   return 0;
 }
 
+// A reduce task's n blocks at src_base + src_off[i], src_len[i] bytes each (*srcb in all), where its decode reads them:
+// device blocks where they are, or (packed) host blocks in one upload back to back into S.src between marks H0 and H1
+// (the whole task is resident at once: no chunking), blocks adjacent in host memory in one copy.  -> *base, *off.
+static int task_blocks(Slot& S, bool packed, uint32_t n, const uint8_t* src_base, const uint64_t* src_off,
+                       const uint64_t* src_len, std::vector<uint64_t>& dev_off, const uint8_t** base,
+                       const uint64_t** off, uint64_t* srcb) {
+  cudaStream_t st = S.st;
+  *srcb = 0;
+  for (uint32_t i = 0; i < n; i++) {
+    if (packed) dev_off.push_back(*srcb);
+    *srcb += src_len[i];
+  }
+  *base = src_base;
+  *off = src_off;
+  if (!packed) return 0;
+  if (int rc = S.src.ensure(*srcb + 64)) return rc;
+  CU(S.mark(H0, st));
+  for (uint32_t i = 0; i < n;) {
+    uint32_t j = i + 1;
+    while (j < n && src_off[j] == src_off[j - 1] + src_len[j - 1]) j++;
+    const uint64_t bytes = dev_off[j - 1] + src_len[j - 1] - dev_off[i];
+    if (bytes)
+      CU(cudaMemcpyAsync((uint8_t*)S.src.p + dev_off[i], src_base + src_off[i], bytes, cudaMemcpyHostToDevice, st));
+    i = j;
+  }
+  CU(S.mark(H1, st));
+  *base = (const uint8_t*)S.src.p;
+  *off = dev_off.data();
+  return 0;
+}
+
 // A reduce task on the read lane of D (decode_task, run_reduce_task) over device blocks into device memory at dst_base,
 // or (packed) over host blocks, with one upload before and one download into dst_base (host memory) after.
 static int read_task_run(Device* D, bool packed, uint32_t codec, uint32_t alg, uint32_t n, const uint8_t* src_base,
@@ -4596,31 +4522,17 @@ static int read_task_run(Device* D, bool packed, uint32_t codec, uint32_t alg, u
   Slot& S = Ln.slot[0];
   SortBufferTrim trim{S};
   cudaStream_t st = S.st;
-  std::vector<uint64_t> dev_off;  // packed: each block's place in the upload, back to back
-  uint64_t srcb = 0;
-  for (uint32_t i = 0; i < n; i++) {
-    if (packed) dev_off.push_back(srcb);
-    srcb += src_len[i];
-  }
-  int rc;
+  std::vector<uint64_t> dev_off;
+  const uint8_t* blocks;
+  const uint64_t* block_off;
+  uint64_t srcb;
+  int rc = task_blocks(S, packed, n, src_base, src_off, src_len, dev_off, &blocks, &block_off, &srcb);
+  if (rc) return rc;
   uint8_t* out = packed ? nullptr : dst_base;
-  if (packed) {  // one upload of every block (the whole task is resident at once: no chunking)
-    if ((rc = S.src.ensure(srcb + 64))) return rc;
-    CU(S.mark(H0, st));
-    for (uint32_t i = 0; i < n;) {  // blocks adjacent in host memory go up in one copy
-      uint32_t j = i + 1;
-      while (j < n && src_off[j] == src_off[j - 1] + src_len[j - 1]) j++;
-      const uint64_t bytes = dev_off[j - 1] + src_len[j - 1] - dev_off[i];
-      if (bytes)
-        CU(cudaMemcpyAsync((uint8_t*)S.src.p + dev_off[i], src_base + src_off[i], bytes, cudaMemcpyHostToDevice, st));
-      i = j;
-    }
-    CU(S.mark(H1, st));
-  }
   uint64_t launches = 0;
   DecodedTask T(mix, n, status, bad_slice);
-  rc = decode_task(D, S, codec, alg, n, packed ? (const uint8_t*)S.src.p : src_base, packed ? dev_off.data() : src_off,
-                   src_len, packed, slice_base, slice_len, slice_checksum, srcb, spec, dst_cap, T, &launches);
+  rc = decode_task(D, S, codec, alg, n, blocks, block_off, src_len, packed, slice_base, slice_len, slice_checksum, srcb,
+                   spec, dst_cap, T, &launches);
   *dst_total = T.failed ? 0 : T.total;  // a failed source: nothing is written
   *n_records = 0;
   if (!rc && !T.failed) rc = run_reduce_task(S, spec, T, &out, dst_cap, dst_total, n_records, n_groups, &launches);
@@ -5118,13 +5030,10 @@ static std::vector<uint8_t> initial_row(const DistinctPlan& P) {
 // into S.parena, their lengths in S.pws), the step over them in S.fws (no sort: heads where G's encoding changes) into
 // S.aggrows, and the partition + compress step.  No step ensures a buffer that holds its own input: the partition step
 // ensures S.pws, S.parena and (packed) S.dst, which hold only stage 2's inputs and outputs by then.
-static int distinct_task_run(Device* D, bool packed, uint32_t codec, int32_t level, uint32_t bs, uint32_t alg,
-                             uint32_t n, const uint8_t* src_base, const uint64_t* src_off, const uint64_t* src_len,
-                             const uint32_t* slice_base, const uint64_t* slice_len, const uint64_t* slice_checksum,
-                             const DistinctPlan& P, uint32_t num_partitions, uint8_t* dst_base, uint64_t dst_cap,
-                             uint64_t* dst_off, uint64_t* dst_len, uint64_t* dst_total, uint64_t* checksum_out,
-                             int32_t* part_status, uint64_t* counts, int32_t* status, int32_t* bad_slice,
-                             const WallTimer& wt) {
+static int distinct_task_run(Device* D, const MapCall& c, uint32_t n, const uint8_t* src_base, const uint64_t* src_off,
+                             const uint64_t* src_len, const uint32_t* slice_base, const uint64_t* slice_len,
+                             const uint64_t* slice_checksum, const DistinctPlan& P, uint64_t* counts, int32_t* status,
+                             int32_t* bad_slice, const WallTimer& wt) {
   Lane& Ln = D->lane[kLaneRead];
   std::lock_guard<std::mutex> lk(Ln.mtx);
   Slot& S = Ln.slot[0];
@@ -5132,34 +5041,19 @@ static int distinct_task_run(Device* D, bool packed, uint32_t codec, int32_t lev
   const PartialAggTrim trim_step{S};
   cudaStream_t st = S.st;
   std::vector<uint64_t> dev_off;
-  uint64_t srcb = 0;
-  for (uint32_t i = 0; i < n; i++) {
-    if (packed) dev_off.push_back(srcb);
-    srcb += src_len[i];
-  }
-  int rc;
-  if (packed) {
-    if ((rc = S.src.ensure(srcb + 64))) return rc;
-    CU(S.mark(H0, st));
-    for (uint32_t i = 0; i < n;) {
-      uint32_t j = i + 1;
-      while (j < n && src_off[j] == src_off[j - 1] + src_len[j - 1]) j++;
-      const uint64_t bytes = dev_off[j - 1] + src_len[j - 1] - dev_off[i];
-      if (bytes)
-        CU(cudaMemcpyAsync((uint8_t*)S.src.p + dev_off[i], src_base + src_off[i], bytes, cudaMemcpyHostToDevice, st));
-      i = j;
-    }
-    CU(S.mark(H1, st));
-  }
+  const uint8_t* blocks;
+  const uint64_t* block_off;
+  uint64_t srcb;
+  int rc = task_blocks(S, c.packed, n, src_base, src_off, src_len, dev_off, &blocks, &block_off, &srcb);
+  if (rc) return rc;
   uint64_t launches = 0;
   const RecordSpec& spec = P.read;
   const PartialAggSpec& step = P.step;
   DecodedTask T(nullptr, n, status, bad_slice);
   RowOrder R;
   if (n) {  // no blocks: an empty reducer, straight to the step
-    rc = decode_task(D, S, codec, alg, n, packed ? (const uint8_t*)S.src.p : src_base,
-                     packed ? dev_off.data() : src_off, src_len, packed, slice_base, slice_len, slice_checksum, srcb,
-                     spec, ~0ull, T, &launches);
+    rc = decode_task(D, S, c.codec, c.alg, n, blocks, block_off, src_len, c.packed, slice_base, slice_len,
+                     slice_checksum, srcb, spec, ~0ull, T, &launches);
     if (rc) return rc;
     if (!T.failed) rc = order_rows(S, spec, T, nullptr, 0, R, &launches);
     if (rc) return rc;
@@ -5172,10 +5066,10 @@ static int distinct_task_run(Device* D, bool packed, uint32_t codec, int32_t lev
     if (rc) return rc;
   }
   if (T.failed) {  // nothing is written
-    for (uint32_t p = 0; p < num_partitions; p++) {
-      dst_off[p] = dst_len[p] = 0;
-      if (checksum_out) checksum_out[p] = 0;
-      part_status[p] = B2S_OK;
+    for (uint32_t p = 0; p < c.R; p++) {
+      c.dst_off[p] = c.dst_len[p] = 0;
+      if (c.checksum_out) c.checksum_out[p] = 0;
+      c.status[p] = B2S_OK;
     }
     return 0;
   }
@@ -5220,18 +5114,17 @@ static int distinct_task_run(Device* D, bool packed, uint32_t codec, int32_t lev
   }
   CU(S.mark(G1, st, launches));
   const uint8_t* d_rows = (const uint8_t*)S.aggrows.p + (n_gx || !rows ? 0 : 256);
-  RowIds ids{partial_row_keys(step.keys)};
-  if (!step.keys.n) ids.range = true;  // SinglePartition: the range ids of no bounds, every id 0
+  const KeySpec keys = partial_row_keys(step.keys);
+  const RowIds ids = step.keys.n ? RowIds::hash(keys) : RowIds::single_partition(keys);
   uint64_t arena = 0, fit = 0;
-  rc = map_rows_partition(D, S, packed, codec, level, bs, alg, num_partitions, rows, d_rows, rows_bytes, d_row_len, ids,
-                          dst_base, dst_cap, dst_off, dst_len, checksum_out, part_status, &arena, &fit, &launches);
+  rc = partition_tail(D, S, c, MapRows{rows, d_rows, rows_bytes, d_row_len}, nullptr, ids, nullptr, &arena, &fit,
+                      &launches);
   if (rc && rc != B2S_E_DST_TOO_SMALL) return rc;
-  *dst_total = arena;
   counts[0] = n_in;
   counts[1] = n_gx;
   counts[2] = rows;
   t_timing.kernel_ms += read_ms;
-  end_call(wt, launches, CallBytes{srcb, arena, packed ? srcb : 0, fit}, &S, Family::kDistinctAggregate);
+  end_call(wt, launches, CallBytes{srcb, arena, c.packed ? srcb : 0, fit}, &S, Family::kPartialAggregate);
   return rc;
 }
 
@@ -5254,17 +5147,14 @@ static int distinct_call(bool packed, uint32_t dev_index, uint32_t codec, int32_
   if (int rc = sort_args(codec, alg, n, src_off, src_len, slice_base, slice_len, slice_checksum, P.read, src_base,
                          nullptr, 0, &unused_total, &unused_records, status))
     return rc;
-  const uint32_t bs = block_size_or_default(codec_block_size);
-  const RowIds ids{P.step.keys};
-  if (int rc = partition_args(codec, bs, alg, num_partitions, 0, nullptr, 0, nullptr, nullptr, dst_base, dst_off,
-                              dst_len, part_status, &ids))
-    return rc;
+  const MapCall c{packed, dev_index, codec, level, block_size_or_default(codec_block_size), alg, num_partitions,
+                  dst_base, dst_cap, dst_off, dst_len, dst_total, checksum_out, part_status};
+  if (int rc = partition_args(c, MapRows{}, nullptr, RowIds::hash(P.step.keys))) return rc;
   if (dst_cap && !dst_base) return fail(B2S_E_ARG, "null argument%s");
   Device* D;
   if (int rc = sort_device(packed ? t_device : dev_index, &D)) return rc;
-  return distinct_task_run(D, packed, codec, level, bs, alg, n, src_base, src_off, src_len, slice_base, slice_len,
-                           slice_checksum, P, num_partitions, dst_base, dst_cap, dst_off, dst_len, dst_total,
-                           checksum_out, part_status, counts, status, bad_slice, wt);
+  return distinct_task_run(D, c, n, src_base, src_off, src_len, slice_base, slice_len, slice_checksum, P, counts,
+                           status, bad_slice, wt);
 }
 
 int b2s_decompress_aggregate_distinct_partition_compress_rows_hash_packed(

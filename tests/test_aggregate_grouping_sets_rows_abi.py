@@ -36,9 +36,10 @@ ROLLUP2 = (0b11, 0b01, 0)
 
 
 def _call(L, c, dev=False, R=4, n=2, keys=KEYS, aggs=AGGS, sets=ROLLUP2, rec_len=(44, 44), records=True, groups=True,
-          agg_arrays=True, mask_array=True, n_sets=None):
+          agg_arrays=True, mask_array=True, n_sets=None, rec_bytes=None):
     rec = np.zeros(128, np.uint8)
     rl = np.array(rec_len, np.uint32)
+    nbytes = int(rl.sum()) if rec_bytes is None else rec_bytes
     kt = np.array([k[0] for k in keys] or [0], np.uint32)
     ko = np.array([k[1] for k in keys] or [0], np.uint32)
     kl = np.array([k[2] for k in keys] or [0], np.uint32)
@@ -53,7 +54,7 @@ def _call(L, c, dev=False, R=4, n=2, keys=KEYS, aggs=AGGS, sets=ROLLUP2, rec_len
     out = np.zeros(512, np.uint8)
     total, ng = C.c_uint64(7), C.c_uint64(9)
     a = (lambda x: x.ctypes.data) if agg_arrays else (lambda x: None)
-    args = (c.CODEC_LZ4BLOCK, 0, 0, c.CHECKSUM_CRC32C, R, n, rec.ctypes.data if records else None, int(rl.sum()),
+    args = (c.CODEC_LZ4BLOCK, 0, 0, c.CHECKSUM_CRC32C, R, n, rec.ctypes.data if records else None, nbytes,
             rl.ctypes.data, len(keys), kt.ctypes.data, ko.ctypes.data, kl.ctypes.data, kn.ctypes.data, len(aggs),
             a(fn), a(vt), a(vo), a(vn), len(sets) if n_sets is None else n_sets,
             masks.ctypes.data if mask_array else None, out.ctypes.data, out.size, doff.ctypes.data, dlen.ctypes.data,
@@ -103,7 +104,9 @@ def test_fifteen_keys_and_sixteen_buffers_are_well_formed_without_a_device():
     dict(aggs=[(SUM, 9, 16, 1)]), dict(aggs=[(SUM, dec(39), 16, 1)]), dict(aggs=[(SUM, NONE, 0, -1)]),
     dict(aggs=[(MIN, I8, 16, 1)]), dict(aggs=[(MAX, BYTES, 16, 1)]), dict(aggs=[(SUM, dec(29), 16, 1)]),
     dict(aggs=[(AVG, dec(28), 16, 1)]), dict(aggs=[(AVG, I64, 16, 1)] * 9), dict(aggs=[(SUM, I64, 12, 1)]),
-    dict(aggs=[(SUM, I64, 16, 65536)])])
+    dict(aggs=[(SUM, I64, 16, 65536)]),
+    # records the lengths do not cover
+    dict(n=0, rec_bytes=44), dict(n=0, rec_bytes=44, sets=(0,))])
 def test_ill_formed_calls_are_argument_errors_before_the_device(kw):
     c = pkg.capi
     L = c.load()

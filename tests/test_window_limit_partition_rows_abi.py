@@ -30,9 +30,10 @@ KEYS = ((STRING, 8, 8, 0), (DECIMAL | DESC | NULLS_LAST, 16, 8, 1))
 
 
 def _call(L, c, dev=False, R=4, n=2, npk=1, keys=KEYS, fn=RANK, limit=100, rec_len=(44, 44), records=True,
-          out_count=True, key_arrays=True):
+          out_count=True, key_arrays=True, rec_bytes=None):
     rec = np.zeros(128, np.uint8)
     rl = np.array(rec_len, np.uint32)
+    nbytes = int(rl.sum()) if rec_bytes is None else rec_bytes
     kt = np.array([k[0] for k in keys] or [0], np.uint32)
     ko = np.array([k[1] for k in keys] or [0], np.uint32)
     kl = np.array([k[2] for k in keys] or [0], np.uint32)
@@ -42,7 +43,7 @@ def _call(L, c, dev=False, R=4, n=2, npk=1, keys=KEYS, fn=RANK, limit=100, rec_l
     out = np.zeros(512, np.uint8)
     total, kept = C.c_uint64(7), C.c_uint64(9)
     a = (lambda x: x.ctypes.data) if key_arrays else (lambda x: None)
-    args = (c.CODEC_LZ4BLOCK, 0, 0, c.CHECKSUM_CRC32C, R, n, rec.ctypes.data if records else None, int(rl.sum()),
+    args = (c.CODEC_LZ4BLOCK, 0, 0, c.CHECKSUM_CRC32C, R, n, rec.ctypes.data if records else None, nbytes,
             rl.ctypes.data, npk, len(keys), a(kt), a(ko), a(kl), a(kn), fn, limit, out.ctypes.data, out.size,
             doff.ctypes.data, dlen.ctypes.data, C.byref(total), cks.ctypes.data, st.ctypes.data,
             C.byref(kept) if out_count else None)
@@ -82,7 +83,9 @@ def test_calls_return_cuda_error_without_a_device():
     dict(records=False), dict(n=2**32, rec_len=(44, 44)),
     # the limit's
     dict(fn=PERCENT_RANK), dict(fn=6), dict(fn=0xFFFFFFFF), dict(limit=0), dict(limit=-5), dict(npk=0, R=2),
-    dict(npk=0, R=200), dict(out_count=False)])
+    dict(npk=0, R=200), dict(out_count=False),
+    # records the lengths do not cover, with and without partition columns
+    dict(n=0, rec_bytes=44), dict(n=0, rec_bytes=44, npk=0, R=1)])
 def test_ill_formed_calls_are_argument_errors_before_the_device(kw):
     c = pkg.capi
     L = c.load()
